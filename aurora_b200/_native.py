@@ -17,7 +17,8 @@ AUR_OK = 0
 AUR_ERR_INVALID, AUR_ERR_CUDA, AUR_ERR_NOMEM, AUR_ERR_UNSUPPORTED, AUR_ERR_NO_DEVICE = -1, -2, -3, -4, -5
 AUR_BF16, AUR_F32 = 0, 1
 KERNEL_AUTO, KERNEL_SIMT, KERNEL_TC1, KERNEL_TC2 = 0, 1, 2, 3
-KERNEL_NAMES = {0: "auto", 1: "simt", 2: "tcgen05-cta1", 3: "tcgen05-cta2"}
+KERNEL_NAMES = {0: "auto", 1: "simt", 2: "wgmma-cta1", 3: "wgmma-cluster2"}
+TC_QUERY_ROWS = 64   # queries per CTA of the tensor-core kernel (kTcQRows, csrc/internal.h): the debug-score row count
 
 # every symbol include/aurora_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
@@ -76,7 +77,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryMissing(
-            f"{LIB_PATH} not found. Build it with `python -m aurora_b200.build` (needs nvcc, targets sm_100a). "
+            f"{LIB_PATH} not found. Build it with `python -m aurora_b200.build` (needs nvcc, targets sm_90a). "
             "aurora_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     vp, i32, i64 = C.c_void_p, C.c_int32, C.c_int64

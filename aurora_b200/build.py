@@ -1,7 +1,7 @@
-"""In-tree build of libaurora_b200.so (sm_100a only; nvcc cross-compiles without a GPU).
+"""In-tree build of libaurora_b200.so (sm_90a only; nvcc cross-compiles without a GPU).
 
 ``python -m aurora_b200.build`` or ``aurora_b200.build.build_native()``.  The .so lands
-next to this file so it travels with the repo snapshot to the GPU box.
+next to this file, so the package imports straight from the source tree.
 """
 
 from __future__ import annotations
@@ -14,14 +14,14 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libaurora_b200.so")
-SOURCES = ["capi.cu", "kernels_simt.cu", "simtopk_tc.cu", "encoder.cu", "encoder_simt.cu", "gemm_tc.cu", "attn_tc.cu", "attn_tc2.cu", "tokenizer.cpp", "host_merge.cpp"]
+SOURCES = ["capi.cu", "kernels_simt.cu", "simtopk_tc.cu", "encoder.cu", "encoder_simt.cu", "gemm_tc.cu", "attn_tc.cu", "tokenizer.cpp", "host_merge.cpp"]
 HEADERS = ["internal.h", "ptx.cuh", "unicode_tables.inc", os.path.join("..", "..", "include", "aurora_b200.h")]
 
-PROFILE = bool(int(os.environ.get("AUR_TC_PROFILE", "0")))   # bring-up timers in the tcgen05 kernel
-EXTRA_DEFS = os.environ.get("AUR_EXTRA_DEFS", "").split()     # e.g. -DAUR_ATTN_POLY_EVERY=0 for an A/B build
+PROFILE = bool(int(os.environ.get("AUR_TC_PROFILE", "0")))   # bring-up timers in the tensor-core similarity kernel
+EXTRA_DEFS = os.environ.get("AUR_EXTRA_DEFS", "").split()     # extra -D flags for an A/B build
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O2,-Wall,-Wno-unused-function",
     "--expt-relaxed-constexpr",
@@ -32,7 +32,7 @@ def _nvcc() -> str:
     for cand in (shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.exists(cand):
             return cand
-    raise RuntimeError("nvcc not found: aurora_b200 needs the CUDA toolkit to build its sm_100a library")
+    raise RuntimeError("nvcc not found: aurora_b200 needs the CUDA toolkit to build its sm_90a library")
 
 
 def _stale() -> bool:
@@ -59,7 +59,7 @@ def build_native(force: bool = False, verbose: bool = False, out: str = "", tag:
             print(" ".join(cmd), flush=True)
         subprocess.run(cmd, check=True)
         objs.append(obj)
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", *objs, "-o", lib, "-cudart", "static"]
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", *objs, "-o", lib, "-cudart", "static"]
     if verbose:
         print(" ".join(cmd), flush=True)
     subprocess.run(cmd, check=True)

@@ -1,22 +1,15 @@
-// Encoder self-attention on tcgen05, packed variable-length sequences, head dim 64, <= 512 keys.
+// Encoder self-attention on wgmma: packed variable-length sequences (<= 512 tokens), head dim 64.
 //
-// Work item = (sequence, 128-query block, head).  Because a whole score row (<= 512 keys) fits the
-// 512 TMEM columns, the softmax is an exact two-pass one (row max, then exp) with no online rescale:
-//   S_j = Q . K_j^T        SS-MMA  M128 N128 K16 x4, block j of 128 keys -> TMEM cols [128j, 128j+128)
-//   P_j = exp2(S_j*c - m*c) softmax threads (thread = query row) write bf16 P_j back over the first
-//                          64 columns of S_j (two keys per 32-bit column: the TS-MMA A layout)
-//   O  += P_j . V_j        TS-MMA  M128 N64 K16 x8, A from TMEM, B = V_j in shared memory read
-//                          MN-major (V rows are [key][64 dims], dims contiguous), O in TMEM cols
-//                          [64, 128) -- the half of S_0 that is dead once P_0 exists
-//   ctx = O / rowsum       bf16, one 128-byte store per query row and head
-// Warps: 0 TMA producer (Q, K_j, V_j tiles straight out of the packed [tokens, 3H] projection buffer),
-// 1 MMA issuer, 2..9 softmax (two per TMEM lane quarter).  Persistent: items round-robin over the CTAs; the producer runs ahead
-// into the next item as soon as the tensor core has released K (after the S MMAs) and V (after O).
-//
-// Keys past the end of a sequence are masked to -inf before the max, so P is exactly 0 there; the V
-// rows under them belong to the next sequence (finite), never to uninitialised memory (the host
-// zero-fills the activation buffers once).  Restates eager_attention_forward + softmax of
-// transformers' modeling_bert.py:115-140 (see oracle/bert_encoder.py).
+// One CTA per (work item, head); a work item is 128 queries of one sequence.  Thread 0 issues every TMA load of the
+// CTA at once -- the Q tile and, per 128-key block of the sequence, its K and V tiles, each block on its own
+// mbarrier -- so the first block's MMAs start while the later blocks are still in flight.  Two warpgroups, 64 query
+// rows each, walk the key blocks with an online softmax:
+//   S = Q K^T          wgmma m64n128k16 x 4, both operands K-major from shared memory
+//   P = exp2(S - m)    in registers (keys past the end of the sequence are masked to -inf, P = 0)
+//   O += P V           wgmma m64n64k16 x 8, P straight from registers (the accumulator layout of S is the A-operand
+//                      layout), V from shared memory read MN-major
+// and store O / rowsum as bf16.  The max is exact (rescale every block); P is rounded to bf16 for the PV MMA.
+// Restates eager_attention_forward + softmax of transformers' modeling_bert.py:115-140 (oracle/bert_encoder.py).
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -25,40 +18,16 @@
 #include "internal.h"
 #include "ptx.cuh"
 
-#include <stdio.h>
-#ifdef AUR_TC_PROFILE
-#define PROF_DECL(...) long long __VA_ARGS__
-#define PROF_T0() const long long t0_ = clock64()
-#define PROF_ADD(x) x += clock64() - t0_
-#else
-#define PROF_DECL(...)
-#define PROF_T0()
-#define PROF_ADD(x)
-#endif
-
 namespace aur {
 namespace {
 
 using namespace ptx;
 
-constexpr int kQB = 128, kKB = 128, kDh = 64, kMaxKBlocks = 4;
-constexpr int kTileBytes = 128 * kDh * 2;     // 16 KB: 128 rows x 128 B
-constexpr int kSoftmaxWarps = 8;
-constexpr int kAttnThreads = (2 + kSoftmaxWarps) * 32;
-constexpr int kOCol = 64;                     // O accumulator columns [64, 128)
-constexpr size_t kAttnSmem = 1024 + static_cast<size_t>(1 + 2 * kMaxKBlocks) * kTileBytes + 512 + 512 * 4;
+constexpr int kKB = 128, kDh = 64, kMaxKeyBlocks = 4;
+constexpr int kTile = 128 * kDh * 2;          // 16 KB: 128 rows x 128 B
+constexpr int kThreads = 256;
+constexpr size_t kSmemBytes = 1024 + static_cast<size_t>(1 + 2 * kMaxKeyBlocks) * kTile + 128;
 
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
 __device__ __forceinline__ float ex2_approx(float x) {
   float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y;
 }
@@ -67,266 +36,121 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
   return d;
 }
-__device__ __forceinline__ float max32(const uint32_t (&v)[32]) {
-  float m = fmaxf(__uint_as_float(v[0]), __uint_as_float(v[1]));
-#pragma unroll
-  for (int e = 2; e < 32; e += 2) m = fmaxf(m, fmaxf(__uint_as_float(v[e]), __uint_as_float(v[e + 1])));
-  return m;
-}
-// p_e = 2^(v_e * sc - mc) for 32 scores; packs them as bf16 pairs (the TS-MMA A layout) and returns their sum.
-__device__ __forceinline__ float exp_pack32(const uint32_t (&v)[32], float sc, float mc, uint32_t (&o)[16]) {
-  float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-  for (int e = 0; e < 32; e += 2) {
-    const float p0 = ex2_approx(fmaf(__uint_as_float(v[e]), sc, -mc));
-    const float p1 = ex2_approx(fmaf(__uint_as_float(v[e + 1]), sc, -mc));
-    s0 += p0; s1 += p1;
-    o[e >> 1] = pack_bf16x2(p0, p1);
-  }
-  return s0 + s1;
-}
-// Named barrier shared by the two softmax warps of one TMEM lane quarter (ids 1..4; 0 is __syncthreads).
-__device__ __forceinline__ void pair_sync(int quarter) {
-  asm volatile("bar.sync %0, 64;" ::"r"(quarter + 1) : "memory");
-}
-// kind::f16 instruction descriptor with B read MN-major (bit 16): D=f32, A=B=bf16.
-__host__ __device__ constexpr uint32_t idesc_bf16_f32_bmn(int m, int n) {
-  return idesc_bf16_f32(m, n) | (1u << 16);
-}
 
-__global__ void __launch_bounds__(kAttnThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + ((1024u - (base & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sQ = smem;
-  uint8_t* sK = smem + kTileBytes;
-  uint8_t* sV = sK + kMaxKBlocks * kTileBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kMaxKBlocks * kTileBytes);
-  uint64_t* bar_q = bars;                 // Q tile landed
-  uint64_t* bar_k = bars + 1;             // [4] K_j landed
-  uint64_t* bar_v = bars + 5;             // [4] V_j landed
-  uint64_t* bar_s = bars + 9;             // [4] S_j complete in TMEM
-  uint64_t* bar_p = bars + 13;            // [4] P_j written by all softmax warps
-  uint64_t* bar_qkfree = bars + 17;       // all S MMAs retired: Q / K smem reusable
-  uint64_t* bar_o = bars + 18;            // all PV MMAs retired: O complete, V smem reusable
-  uint64_t* bar_done = bars + 19;         // softmax warps finished reading O: TMEM reusable
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 20);
-  float* xch = reinterpret_cast<float*>(bars + 64);   // [2][2][128] partial row max / row sum of the warp pairs
+  uint8_t* sK = smem + kTile;                          // [kMaxKeyBlocks] tiles
+  uint8_t* sV = smem + (1 + kMaxKeyBlocks) * kTile;    // [kMaxKeyBlocks] tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (1 + 2 * kMaxKeyBlocks) * kTile);   // q_full, kv_full[4]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int total = p.n_items * p.heads;
+  const AttnItem item = p.items[blockIdx.x / p.heads];
+  const int head = blockIdx.x % p.heads;
+  const int n_kb = (item.len + kKB - 1) / kKB;
 
-  if (warp == 0 && lane == 0) {
+  grid_dep_launch();
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_qkv);
-    mbar_init(bar_q, 1);
-    for (int j = 0; j < kMaxKBlocks; ++j) {
-      mbar_init(&bar_k[j], 1); mbar_init(&bar_v[j], 1); mbar_init(&bar_s[j], 1); mbar_init(&bar_p[j], kSoftmaxWarps);
-    }
-    mbar_init(bar_qkfree, 1); mbar_init(bar_o, 1); mbar_init(bar_done, kSoftmaxWarps);
+    for (int i = 0; i < 1 + kMaxKeyBlocks; ++i) mbar_init(&bars[i], 1);
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc<1>(tmem_slot, 512); tmem_relinquish<1>(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  grid_dep_launch();
-  grid_dep_wait();     // the qkv projections come from the previous kernel
-
-  uint32_t blk_phase = 0;   // bit j: parity of the next completion of the per-block barriers j
-  int it = 0;
-#ifdef AUR_TC_PROFILE
-  long long pt[4] = {0, 0, 0, 0};
-  const long long pt_begin = clock64();
-#endif
-  AttnItem next_item = blockIdx.x < total ? p.items[blockIdx.x / p.heads] : AttnItem{0, 1, 0, 0};
-  for (int w = blockIdx.x; w < total; w += gridDim.x, ++it) {
-    const AttnItem item = next_item;      // fetched one iteration ahead: the L2 round trip is off the critical path
-    if (w + static_cast<int>(gridDim.x) < total) next_item = p.items[(w + gridDim.x) / p.heads];
-    const int head = w % p.heads;
-    const int nkb = (item.len + kKB - 1) / kKB;
-    const uint32_t par = it & 1, prev = par ^ 1;
-
-    if (warp == 0) {
-      // ---------------------------------------------------------- TMA producer
-      if (it > 0) mbar_wait(bar_qkfree, prev);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(bar_q, kTileBytes);
-        tma_load_2d(sQ, &tmap_qkv, bar_q, head * kDh, item.tok0 + item.q0, kEvictNormal);
-        for (int j = 0; j < nkb; ++j) {
-          mbar_arrive_expect_tx(&bar_k[j], kTileBytes);
-          tma_load_2d(sK + j * kTileBytes, &tmap_qkv, &bar_k[j], p.hidden + head * kDh, item.tok0 + j * kKB, kEvictNormal);
-        }
-      }
-      __syncwarp();
-      if (it > 0) mbar_wait(bar_o, prev);
-      if (elect_one()) {
-        for (int j = 0; j < nkb; ++j) {
-          mbar_arrive_expect_tx(&bar_v[j], kTileBytes);
-          tma_load_2d(sV + j * kTileBytes, &tmap_qkv, &bar_v[j], 2 * p.hidden + head * kDh, item.tok0 + j * kKB, kEvictNormal);
-        }
-      }
-      __syncwarp();
-    } else if (warp == 1) {
-      // ---------------------------------------------------------- MMA issuer
-      constexpr uint32_t idesc_s = idesc_bf16_f32(kQB, kKB);
-      constexpr uint32_t idesc_o = idesc_bf16_f32_bmn(kQB, kDh);
-      if (it > 0) { PROF_T0(); mbar_wait(bar_done, prev); PROF_ADD(pt[0]); }
-      { PROF_T0(); mbar_wait(bar_q, par); PROF_ADD(pt[1]); }
-      tc_fence_after();
-      const uint64_t q_desc = smem_desc_sw128(smem_u32(sQ));
-      for (int j = 0; j < nkb; ++j) {
-        { PROF_T0(); mbar_wait(&bar_k[j], (blk_phase >> j) & 1); PROF_ADD(pt[1]); }
-        tc_fence_after();
-        const uint64_t k_desc = smem_desc_sw128(smem_u32(sK + j * kTileBytes));
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < kDh / 16; ++ks)
-            mma_ss_bf16<1>(tmem_base + j * kKB, q_desc + 2 * ks, k_desc + 2 * ks, idesc_s, ks != 0);
-          mma_commit<1>(&bar_s[j]);
-          if (j == nkb - 1) mma_commit<1>(bar_qkfree);
-        }
-        __syncwarp();
-      }
-      for (int j = 0; j < nkb; ++j) {
-        { PROF_T0(); mbar_wait(&bar_p[j], (blk_phase >> j) & 1); PROF_ADD(pt[2]); }
-        { PROF_T0(); mbar_wait(&bar_v[j], (blk_phase >> j) & 1); PROF_ADD(pt[3]); }
-        tc_fence_after();
-        const uint64_t v_desc = smem_desc_sw128(smem_u32(sV + j * kTileBytes));
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < kKB / 16; ++ks)   // 16 keys = two 8-row swizzle groups = 2048 B of V
-            mma_ts_bf16<1>(tmem_base + kOCol, tmem_base + j * kKB + ks * 8, v_desc + (2048 >> 4) * ks, idesc_o,
-                           (j | ks) != 0);
-          if (j == nkb - 1) mma_commit<1>(bar_o);
-        }
-        __syncwarp();
-      }
-    } else {
-      // ---------------------------------------------------------- softmax
-      // Thread = query row; the two warps that share a TMEM lane quarter split every key block's
-      // columns ([0,64) / [64,128)) so each SM sub-partition has two warps to issue from, and
-      // exchange their partial row max / row sum through shared memory.
-      const int quarter = warp & 3, half = (warp - 2) >> 2;
-      const int row = quarter * 32 + lane;
-      const uint32_t trow = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-      const int c0 = half * 64;                    // this warp's first column inside a key block
-      float m = -INFINITY;
-      for (int j = 0; j < nkb; ++j) {
-        { PROF_T0(); mbar_wait(&bar_s[j], (blk_phase >> j) & 1); PROF_ADD(pt[0]); }
-        tc_fence_after();
-        const int nv = min(kKB, item.len - j * kKB) - c0;     // valid columns among this warp's 64
-        if (nv <= 0) continue;
-        uint32_t va[32], vb[32];
-        tmem_ld_x32(trow + j * kKB + c0, va);
-        tmem_ld_x32(trow + j * kKB + c0 + 32, vb);
-        tmem_wait_ld();
-        if (nv >= 64) {
-          m = fmaxf(m, fmaxf(max32(va), max32(vb)));
-        } else {
-#pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            if (e < nv) m = fmaxf(m, __uint_as_float(va[e]));
-            if (32 + e < nv) m = fmaxf(m, __uint_as_float(vb[e]));
-          }
-        }
-      }
-      xch[half * 128 + row] = m;
-      { PROF_T0(); pair_sync(quarter); PROF_ADD(pt[1]); }
-      m = fmaxf(m, xch[(half ^ 1) * 128 + row]);   // >= one valid key per sequence: finite
-      const float sc = p.scale_log2e, mc = m * sc;
-      float sum = 0.f;
-      for (int j = 0; j < nkb; ++j) {
-        const int nv = min(kKB, item.len - j * kKB) - c0;
-        const uint32_t tblk = trow + j * kKB;
-        uint32_t va[32], vb[32], oa[16], ob[16];
-        if (nv > 0) {
-          tmem_ld_x32(tblk + c0, va);
-          tmem_ld_x32(tblk + c0 + 32, vb);
-          tmem_wait_ld();
-        }
-        // P_j lands on columns [0,64) of S_j, i.e. on scores the other warp of the pair reads: both
-        // must hold their scores in registers before either writes
-        { PROF_T0(); pair_sync(quarter); PROF_ADD(pt[1]); }
-        PROF_T0();
-        if (nv >= 64) {
-          sum += exp_pack32(va, sc, mc, oa) + exp_pack32(vb, sc, mc, ob);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 32; e += 2) {
-            float p0 = 0.f, p1 = 0.f, p2 = 0.f, p3 = 0.f;
-            if (e < nv) p0 = ex2_approx(fmaf(__uint_as_float(va[e]), sc, -mc));
-            if (e + 1 < nv) p1 = ex2_approx(fmaf(__uint_as_float(va[e + 1]), sc, -mc));
-            if (32 + e < nv) p2 = ex2_approx(fmaf(__uint_as_float(vb[e]), sc, -mc));
-            if (33 + e < nv) p3 = ex2_approx(fmaf(__uint_as_float(vb[e + 1]), sc, -mc));
-            sum += (p0 + p1) + (p2 + p3);
-            oa[e >> 1] = pack_bf16x2(p0, p1); ob[e >> 1] = pack_bf16x2(p2, p3);
-          }
-        }
-        tmem_st_x16(tblk + (c0 >> 1), oa);
-        tmem_st_x16(tblk + (c0 >> 1) + 16, ob);
-        tmem_wait_st();
-        PROF_ADD(pt[2]);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_p[j]);
-      }
-      xch[256 + half * 128 + row] = sum;
-      pair_sync(quarter);
-      sum += xch[256 + (half ^ 1) * 128 + row];
-      { PROF_T0(); mbar_wait(bar_o, par); PROF_ADD(pt[3]); }
-      tc_fence_after();
-      const float inv = 1.0f / sum;
-      const bool live = item.q0 + row < item.len;
-      __nv_bfloat16* dst = p.ctx + static_cast<size_t>(item.tok0 + item.q0 + row) * p.ld_ctx + head * kDh + half * 32;
-      {
-        uint32_t v[32];
-        tmem_ld_x32(trow + kOCol + half * 32, v);
-        tmem_wait_ld();
-        // O is in registers: hand TMEM to the next item's S MMAs before the global stores
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_done);
-        if (live) {
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            uint4 q4;
-            q4.x = pack_bf16x2(__uint_as_float(v[8 * e + 0]) * inv, __uint_as_float(v[8 * e + 1]) * inv);
-            q4.y = pack_bf16x2(__uint_as_float(v[8 * e + 2]) * inv, __uint_as_float(v[8 * e + 3]) * inv);
-            q4.z = pack_bf16x2(__uint_as_float(v[8 * e + 4]) * inv, __uint_as_float(v[8 * e + 5]) * inv);
-            q4.w = pack_bf16x2(__uint_as_float(v[8 * e + 6]) * inv, __uint_as_float(v[8 * e + 7]) * inv);
-            reinterpret_cast<uint4*>(dst)[e] = q4;
-          }
-        }
-      }
+  if (threadIdx.x == 0) {
+    grid_dep_wait();     // the qkv projections come from the previous kernel
+    mbar_arrive_expect_tx(&bars[0], kTile);
+    tma_load_2d(sQ, &tmap_qkv, &bars[0], head * kDh, item.tok0 + item.q0, kEvictNormal);
+    for (int j = 0; j < n_kb; ++j) {
+      mbar_arrive_expect_tx(&bars[1 + j], 2 * kTile);
+      tma_load_2d(sK + j * kTile, &tmap_qkv, &bars[1 + j], p.hidden + head * kDh, item.tok0 + j * kKB, kEvictNormal);
+      tma_load_2d(sV + j * kTile, &tmap_qkv, &bars[1 + j], 2 * p.hidden + head * kDh, item.tok0 + j * kKB, kEvictNormal);
     }
-    blk_phase ^= (1u << nkb) - 1u;
   }
-#ifdef AUR_TC_PROFILE
-  if (blockIdx.x == 0 && lane == 0 && (warp == 1 || warp == 2 || warp == 6))
-    printf("attn prof warp %d items %d total %lld : %lld %lld %lld %lld  (mma: done,qk,p,v | softmax: wait_s,pair_sync,pass2,wait_o)\n",
-           warp, it, clock64() - pt_begin, pt[0], pt[1], pt[2], pt[3]);
-#endif
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc<1>(tmem_base, 512); }
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  // accumulator layout (m64nN): register 4 j + {0, 1} = row 16 w + l / 4, columns 8 j + 2 (l % 4) + {0, 1};
+  // 4 j + {2, 3} = the same columns of row + 8
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const float sc = p.scale_log2e;
+  const uint64_t q_desc = wgmma_desc_sw128(smem_u32(sQ + wg * 64 * 128));
+  mbar_wait(&bars[0], 0);
+  for (int j = 0; j < n_kb; ++j) {
+    mbar_wait(&bars[1 + j], 0);
+    float s[64];
+    const uint64_t k_desc = wgmma_desc_sw128(smem_u32(sK + j * kTile));
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kDh / 16; ++ks) wgmma_m64n128_ss(s, q_desc + 2 * ks, k_desc + 2 * ks, ks > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    // mask, scale to log2 units, running max per row (a row lives in the 4 lanes of a quad)
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const int key = j * kKB + 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+      const float v = key < item.len ? s[i] * sc : -INFINITY;
+      s[i] = v;
+      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], v);
+    }
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float m_new = fmaxf(m_run[h], mx[h]);
+      alpha[h] = ex2_approx(m_run[h] - m_new);
+      m_run[h] = m_new;
+      l_run[h] *= alpha[h];
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] *= alpha[(i >> 1) & 1];
+    uint32_t pa[8][4];   // P as the A operand of 8 K=16 steps
+#pragma unroll
+    for (int i = 0; i < 64; i += 2) {
+      const int h = (i >> 1) & 1;
+      const float p0 = ex2_approx(s[i] - m_run[h]), p1 = ex2_approx(s[i + 1] - m_run[h]);
+      l_run[h] += p0 + p1;
+      pa[i >> 3][(i >> 1) & 3] = pack_bf16x2(p0, p1);
+    }
+    const uint64_t v_desc = wgmma_desc_sw128(smem_u32(sV + j * kTile));
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < kKB / 16; ++ks) wgmma_m64n64_rs_tb(o, pa[ks], v_desc + (2048 >> 4) * ks);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+  }
+  // normalise and store this thread's two rows
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+    l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+    const int qrow = item.q0 + wg * 64 + 16 * w + (l >> 2) + 8 * h;
+    if (qrow >= item.len) continue;
+    const float inv = 1.f / l_run[h];
+    __nv_bfloat16* dst = p.ctx + static_cast<size_t>(item.tok0 + qrow) * p.ld_ctx + head * kDh + 2 * (l & 3);
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+      *reinterpret_cast<uint32_t*>(dst + 8 * jj) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+  }
 }
 
 }  // namespace
 
-cudaError_t attn_tc_launch(int sm_count, const void* tmap_qkv, const AttnParams& p, cudaStream_t s) {
-  const int total = p.n_items * p.heads;
-  if (total <= 0) return cudaSuccess;
+cudaError_t attn_tc_launch(const void* tmap_qkv, const AttnParams& p, cudaStream_t s) {
+  if (p.n_items <= 0) return cudaSuccess;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(kAttnSmem));
+    cudaError_t e = cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmemBytes));
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  const int grid = total < sm_count ? total : sm_count;
-  return launch_pdl(attn_tc_kernel, dim3(grid), dim3(kAttnThreads), kAttnSmem, s, 1,
+  return launch_pdl(attn_tc_kernel, dim3(static_cast<unsigned>(p.n_items * p.heads)), dim3(kThreads), kSmemBytes, s, 1,
                     *reinterpret_cast<const CUtensorMap*>(tmap_qkv), p);
 }
 

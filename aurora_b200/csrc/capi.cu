@@ -120,9 +120,9 @@ struct SearchCtx {
   int64_t snapshot_rows = 0;
   uint32_t epoch = 0;
   DevBuf<uint64_t> cand_a, cand_b;
-  DevBuf<uint64_t> pub;          // tcgen05 kernel's cross-CTA threshold exchange
+  DevBuf<uint64_t> pub;          // tensor-core kernel's cross-CTA threshold exchange
   DevBuf<uint32_t> cand_count;   // compacted candidates per query (self-resetting)
-  DevBuf<uint32_t> d_epoch;      // the tcgen05 kernel's launch counter, device resident (CUDA-graph replays advance it)
+  DevBuf<uint32_t> d_epoch;      // the tensor-core kernel's launch counter, device resident (CUDA-graph replays advance it)
   DevBuf<float> score_chunk;
   DevBuf<float> masked_inv;      // inverse norms with the invisible rows turned into NaN (tenant scope / id subset)
   DevBuf<int32_t> allow_rows;    // subset search: rows that stay visible
@@ -196,9 +196,9 @@ int build_tmaps(aur_index* ix) {
 
 bool tc_shape_ok(const aur_index* ix, int k, bool filtered) {
   if (!ix->tmap_ok || filtered || k > kMaxK) return false;
-  // candidate lists (k + slack per query) and, past 768 dims, part of the queries share the SM's
-  // shared memory with the TMA ring: large k at large dim leaves no room for a pipeline
-  return tc_pick_stages(2, 1, k + kSlack, ix->dim, ix->smem_optin) >= 2;
+  // candidate lists (k + slack per query) and the query block share the SM's shared memory with
+  // the TMA ring: large k at large dim leaves no room for a pipeline
+  return tc_pick_stages(1, k + kSlack, ix->dim, ix->smem_optin) >= 2;
 }
 
 int ctx_init(aur_index* ix, SearchCtx* c) {
@@ -235,19 +235,15 @@ void release_ctx(aur_index* ix, SearchCtx* c) {
   if (!c->bound) ix->free_ctxs.push_back(c);
 }
 
-// Runs one block of <= 256 queries through the tcgen05 kernel over the first n_rows rows.  Leaves candidate keys
+// Runs one block of queries (<= 128 single CTAs, <= 512 pairs) through the tensor-core kernel over the first n_rows rows.  Leaves candidate keys
 // in c->cand_a as [nqb_pad, n_lists, ksel]; returns n_lists.
 int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, int nqb, int ksel, int64_t n_rows, float* dbg,
                  int* n_lists_out, cudaStream_t s, const float* inv_norm = nullptr, const uint32_t* row_mask = nullptr,
                  const int32_t* q_scope = nullptr) {
   int n_qblocks = (nqb > kTcQRows) ? 2 : 1;
-  if (cta_group == 2 && n_qblocks != 2) {
-    // a pair works on 256 query rows.  A short tail block normally runs as single CTAs; when their larger
-    // TMA stages do not fit next to the lists (large k at dim > 768) it runs as a pair with a padding block
-    if (tc_pick_stages(1, 1, ksel, ix->dim, ix->smem_optin) >= 2) cta_group = 1; else n_qblocks = 2;
-  }
+  if (cta_group == 2 && nqb <= kTcQRows) cta_group = 1;   // a pair works on 128 query rows: a short tail runs as single CTAs
   const int pairs = ix->sm_count / 2;
-  int n_super = 1;   // query super-blocks of 256 (CTA pairs that walk the same tiles side by side, sharing them through L2)
+  int n_super = 1;   // query super-blocks of 128 (CTA pairs that walk the same tiles side by side, sharing them through L2)
   if (cta_group == 2) {
     n_super = (nqb + 2 * kTcQRows - 1) / (2 * kTcQRows);
     // the threshold exchange needs ceil(ksel / tile sets) <= 4 rows vouched for per CTA
@@ -259,10 +255,10 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   const int n_tsets = (cta_group == 2) ? pairs / n_super : grid / n_qblocks;
   // epilogue groups: 1 by default; 2 (alternating tiles) stays selectable for experiments
   int epi_groups = ix->opt_epi_groups;
-  if (epi_groups == 0) epi_groups = 1;   // measured: one group + a deeper TMA ring (11 stages) beats two groups + 8
-  const int stages = tc_pick_stages(cta_group, epi_groups, ksel, ix->dim, ix->smem_optin);
-  if (stages < 2) return fail(AUR_ERR_UNSUPPORTED, "k too large for the tcgen05 path's shared memory");
-  const size_t smem = tc_smem_bytes(cta_group, epi_groups, stages, ksel, ix->dim);
+  if (epi_groups == 0) epi_groups = 1;   // one group leaves the most shared memory to the TMA ring
+  const int stages = tc_pick_stages(epi_groups, ksel, ix->dim, ix->smem_optin);
+  if (stages < 2) return fail(AUR_ERR_UNSUPPORTED, "k too large for the tensor-core path's shared memory");
+  const size_t smem = tc_smem_bytes(epi_groups, stages, ksel, ix->dim);
   const int n_lists = n_tsets * epi_groups;   // candidate lists per query
   const size_t ncand = static_cast<size_t>(n_qblocks) * kTcQRows * n_lists * ksel;
   CU_TRY(c->cand_a.reserve(ncand));
@@ -331,7 +327,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
   int kernel = ix->opt_kernel;
   if (kernel == AUR_KERNEL_AUTO) kernel = tc_shape_ok(ix, k, filtered) ? AUR_KERNEL_TC2 : AUR_KERNEL_SIMT;
   if (kernel != AUR_KERNEL_SIMT && !tc_shape_ok(ix, k, filtered))
-    return fail(AUR_ERR_UNSUPPORTED, "tcgen05 path needs bf16, dim %% 64 == 0, dim <= %d, no per-query tenant filter, and k small "
+    return fail(AUR_ERR_UNSUPPORTED, "tensor-core path needs bf16, dim %% 64 == 0, dim <= %d, no per-query tenant filter, and k small "
                 "enough for its shared-memory lists at this dim", kTcMaxDim);
   c->last_kernel = kernel;
   c->last_launches = 0;
@@ -356,7 +352,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
     inv = c->masked_inv.p;
   }
 
-  // queries per launch: the generic kernel takes 1024; the tcgen05 kernel 256 per CTA pair and up to four pairs side by
+  // queries per launch: the generic kernel takes 1024; the tensor-core kernel 128 per CTA pair and up to four pairs side by
   // side on the same corpus tiles (fewer when k + slack is too large for the threshold exchange of that geometry)
   int qstep = 1024;
   if (kernel == AUR_KERNEL_TC1) qstep = 2 * kTcQRows;
@@ -406,7 +402,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
       cur = c->cand_a.p;
     }
     // dense candidate lists (SIMT path): fold until one sort of <= 4096 keys finishes the
-    // job.  The tcgen05 kernel already compacted its survivors per query.
+    // job.  The tensor-core kernel already compacted its survivors per query.
     const bool compact = kernel != AUR_KERNEL_SIMT;
     bool in_a = true;
     while (!compact && static_cast<int64_t>(n_lists) * ksel > 4096) {
@@ -538,7 +534,7 @@ int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, 
       sc.q_org = c->stage_qorg.p;
     }
     // the reference asks one tenant's question at a time (weaviate_client.py:244-249): when every query of the
-    // batch carries the same (user, org) scope the filter folds into the row scale and the tcgen05 kernel serves it
+    // batch carries the same (user, org) scope the filter folds into the row scale and the tensor-core kernel serves it
     bool uniform = true;
     scope[0] = q_user[0]; scope[1] = q_org ? q_org[0] : -1;
     for (int i = 1; i < nq && uniform; ++i) uniform = q_user[i] == scope[0] && (q_org ? q_org[i] : -1) == scope[1];
@@ -622,7 +618,7 @@ int aur_open(const aur_config* cfg, aur_index** out) {
   CU_TRY(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CU_TRY(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major < 10) return fail(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9) return fail(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
   aur_index* ix = new aur_index();
   ix->device = cfg->device; ix->dim = cfg->dim; ix->dtype = cfg->dtype; ix->capacity = cfg->capacity;
   ix->elt = cfg->dtype == AUR_BF16 ? 2 : 4;
@@ -1089,8 +1085,8 @@ int aur_debug_tc_scores(aur_index* ix, const void* queries_dev, int32_t nq, int3
   if (!ix || !queries_dev || !out_dev) return fail(AUR_ERR_INVALID, "null argument");
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   CU_TRY(cudaSetDevice(ix->device));
-  if (!ix->tmap_ok) return fail(AUR_ERR_UNSUPPORTED, "index shape has no tcgen05 path");
-  if (nq <= 0 || nq > 2 * kTcQRows) return fail(AUR_ERR_INVALID, "1..256 queries");
+  if (!ix->tmap_ok) return fail(AUR_ERR_UNSUPPORTED, "index shape has no tensor-core path");
+  if (nq <= 0 || nq > 2 * kTcQRows) return fail(AUR_ERR_INVALID, "1..%d queries", 2 * kTcQRows);
   int n_lists = 0;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
   SearchCtx* c = nullptr;

@@ -61,7 +61,6 @@ struct aur_encoder {
   std::vector<std::string> missing;   // parameter names not loaded yet
   __nv_bfloat16 *x = nullptr, *y = nullptr, *qkv = nullptr, *ctx = nullptr, *inter = nullptr;
   CUtensorMap tm_x, tm_ctx, tm_inter, tm_qkv;       // loads: box {64, 128}
-  CUtensorMap tmo_qkv, tmo_y, tmo_inter;            // GEMM outputs (TMA store): box {64, 32}
   int32_t *d_tok = nullptr, *d_pos = nullptr, *d_cu = nullptr;
   AttnItem* d_items = nullptr;
   int max_items = 0;
@@ -139,13 +138,13 @@ bool find_param(aur_encoder* e, const std::string& name, ParamSlot* out) {
   return false;
 }
 
-int gemm(aur_encoder* e, const CUtensorMap* tm_a, const CUtensorMap* tm_w, const CUtensorMap* tm_out, int m_rows, int n,
+int gemm(aur_encoder* e, const CUtensorMap* tm_a, const CUtensorMap* tm_w, __nv_bfloat16* out, int m_rows, int n,
          int k, int epi, const float* bias, const __nv_bfloat16* resid, int ldr) {
   GemmParams p{};
-  p.bias = bias; p.resid = resid; p.ldr = ldr;
+  p.bias = bias; p.resid = resid; p.ldr = ldr; p.out = out; p.ldo = n;
   const int tile_m = 128 * e->cta_group;
   p.m_tiles = (m_rows + tile_m - 1) / tile_m; p.n_tiles = n / e->bn; p.k_blocks = k / 64;
-  ENC_TRY(gemm_tc_launch(e->cta_group, e->bn, epi, e->sm_count, tm_a, tm_w, tm_out, p, e->stream));
+  ENC_TRY(gemm_tc_launch(e->cta_group, e->bn, epi, e->sm_count, tm_a, tm_w, p, e->stream));
   return AUR_OK;
 }
 
@@ -170,12 +169,12 @@ int forward_locked(aur_encoder* e, const int32_t* cu_host, int n_seq, int n_item
   for (int l = 0; l < c.layers; ++l) {
     Layer& L = e->layers[l];
     int rc;
-    if ((rc = gemm(e, &e->tm_x, &L.tm_wqkv, &e->tmo_qkv, T, 3 * HP, H, kEpiBias, L.bqkv, nullptr, 0))) return rc;
-    ENC_TRY(attn_launch(e->sm_count, &e->tm_qkv, ap, s));
-    if ((rc = gemm(e, &e->tm_ctx, &L.tm_wo, &e->tmo_y, T, H, HP, kEpiBiasResid, L.bo, e->x, H))) return rc;
+    if ((rc = gemm(e, &e->tm_x, &L.tm_wqkv, e->qkv, T, 3 * HP, H, kEpiBias, L.bqkv, nullptr, 0))) return rc;
+    ENC_TRY(attn_tc_launch(&e->tm_qkv, ap, s));
+    if ((rc = gemm(e, &e->tm_ctx, &L.tm_wo, e->y, T, H, HP, kEpiBiasResid, L.bo, e->x, H))) return rc;
     ENC_TRY(launch_layernorm(e->y, L.ln1_g, L.ln1_b, c.ln_eps, T, H, e->x, s));
-    if ((rc = gemm(e, &e->tm_x, &L.tm_wi, &e->tmo_inter, T, I, H, kEpiBiasGelu, L.bi, nullptr, 0))) return rc;
-    if ((rc = gemm(e, &e->tm_inter, &L.tm_wo2, &e->tmo_y, T, H, I, kEpiBiasResid, L.bo2, e->x, H))) return rc;
+    if ((rc = gemm(e, &e->tm_x, &L.tm_wi, e->inter, T, I, H, kEpiBiasGelu, L.bi, nullptr, 0))) return rc;
+    if ((rc = gemm(e, &e->tm_inter, &L.tm_wo2, e->y, T, H, I, kEpiBiasResid, L.bo2, e->x, H))) return rc;
     ENC_TRY(launch_layernorm(e->y, L.ln2_g, L.ln2_b, c.ln_eps, T, H, e->x, s));
     launches += 7;
   }
@@ -235,7 +234,7 @@ int aur_encoder_open(const aur_encoder_config* cfg, aur_encoder** out) {
   ENC_TRY(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   ENC_TRY(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) return report_error(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9) return report_error(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
   aur_encoder* e = new aur_encoder();
   e->cfg = *cfg;
   e->sm_count = prop.multiProcessorCount;
@@ -275,9 +274,7 @@ int aur_encoder_open(const aur_encoder_config* cfg, aur_encoder** out) {
   const int Ri = static_cast<int>(R);
   const int HP = e->hp;
   if ((rc = make_tmap(&e->tm_x, e->x, H, Ri, 128)) || (rc = make_tmap(&e->tm_ctx, e->ctx, HP, Ri, 128)) ||
-      (rc = make_tmap(&e->tm_inter, e->inter, I, Ri, 128)) || (rc = make_tmap(&e->tm_qkv, e->qkv, 3 * HP, Ri, 128)) ||
-      (rc = make_tmap(&e->tmo_qkv, e->qkv, 3 * HP, Ri, 32)) || (rc = make_tmap(&e->tmo_y, e->y, H, Ri, 32)) ||
-      (rc = make_tmap(&e->tmo_inter, e->inter, I, Ri, 32)))
+      (rc = make_tmap(&e->tm_inter, e->inter, I, Ri, 128)) || (rc = make_tmap(&e->tm_qkv, e->qkv, 3 * HP, Ri, 128)))
     return fail_open(rc);
   for (Layer& l : e->layers) {
     if ((rc = make_tmap(&l.tm_wqkv, l.wqkv, H, 3 * HP, e->bn / e->cta_group)) ||
@@ -424,19 +421,18 @@ int aur_debug_gemm(int32_t device, const uint16_t* a, const uint16_t* w, const f
   cudaMemcpy(dw, w, static_cast<size_t>(n) * k * 2, cudaMemcpyHostToDevice);
   cudaMemcpy(db, bias, sizeof(float) * n, cudaMemcpyHostToDevice);
   if (resid) cudaMemcpy(dr, resid, static_cast<size_t>(m) * n * 2, cudaMemcpyHostToDevice);
-  CUtensorMap tm_a, tm_w, tm_o;
-  if ((rc = make_tmap(&tm_a, da, k, m_pad, 128)) || (rc = make_tmap(&tm_w, dw, k, n, bn / cta_group)) ||
-      (rc = make_tmap(&tm_o, dout, n, m_pad, 32)))
+  CUtensorMap tm_a, tm_w;
+  if ((rc = make_tmap(&tm_a, da, k, m_pad, 128)) || (rc = make_tmap(&tm_w, dw, k, n, bn / cta_group)))
     return cleanup(rc);
   GemmParams p{};
-  p.bias = db; p.resid = dr; p.ldr = n;
+  p.bias = db; p.resid = dr; p.ldr = n; p.out = dout; p.ldo = n;
   p.m_tiles = m_pad / (128 * cta_group); p.n_tiles = n / bn; p.k_blocks = k / 64;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
   cudaError_t ce = cudaSuccess;
   for (int rep = 0; rep < 3 && ce == cudaSuccess; ++rep) {   // last repetition is the timed one
     cudaEventRecord(e0, nullptr);
-    ce = gemm_tc_launch(cta_group, bn, epi, prop.multiProcessorCount, &tm_a, &tm_w, &tm_o, p, nullptr);
+    ce = gemm_tc_launch(cta_group, bn, epi, prop.multiProcessorCount, &tm_a, &tm_w, p, nullptr);
     cudaEventRecord(e1, nullptr);
   }
   if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
@@ -464,8 +460,6 @@ int aur_debug_attention(int32_t device, const uint16_t* qkv, const int32_t* cu, 
     if (len < 1 || len > 512) return report_error(AUR_ERR_INVALID, "sequence length %d", len);
     for (int q0 = 0; q0 < len; q0 += 128) items.push_back(AttnItem{cu[i], len, q0, 0});
   }
-  if (getenv("AUR_ATTN_SORT"))        // A/B timing only: longest-first order measured 3 % SLOWER than sequence order (profiles/attn_ab_r2.txt)
-    std::stable_sort(items.begin(), items.end(), [](const AttnItem& a, const AttnItem& b) { return a.len > b.len; });
   __nv_bfloat16 *dq = nullptr, *dc = nullptr; AttnItem* di = nullptr;
   int rc = AUR_OK;
   auto A = [&](auto** p, size_t cnt) { if (rc == AUR_OK) rc = dev_alloc(p, cnt); };
@@ -484,7 +478,7 @@ int aur_debug_attention(int32_t device, const uint16_t* qkv, const int32_t* cu, 
   cudaError_t ce = cudaSuccess;
   for (int rep = 0; rep < 3 && ce == cudaSuccess; ++rep) {
     cudaEventRecord(e0, nullptr);
-    ce = attn_launch(prop.multiProcessorCount, &tm, ap, nullptr);
+    ce = attn_tc_launch(&tm, ap, nullptr);
     cudaEventRecord(e1, nullptr);
   }
   if (ce == cudaSuccess) ce = cudaDeviceSynchronize();

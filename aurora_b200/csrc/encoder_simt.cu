@@ -1,4 +1,4 @@
-// CUDA-core kernels of the encoder forward: the HBM-bound row operations around the tcgen05 GEMMs
+// CUDA-core kernels of the encoder forward: the HBM-bound row operations around the wgmma GEMMs
 // and attention.  One warp owns one token row (hidden <= 1024 lives in registers: hidden/8 16-byte
 // chunks striped over the lanes), LayerNorm statistics by warp shuffle in fp32 with the two-pass
 // variance torch.nn.LayerNorm uses (oracle/bert_encoder.py:layer_norm).

@@ -1,19 +1,14 @@
-// Encoder GEMM on tcgen05:  out[M, N] = act( A[M, K] . W[N, K]^T + bias ) (+ residual), bf16 in,
-// fp32 accumulate in TMEM, bf16 out.  Both operands are K-major (activations [tokens, K] and
+// Encoder GEMM on wgmma:  out[M, N] = act( A[M, K] . W[N, K]^T + bias ) (+ residual), bf16 in,
+// fp32 accumulate in registers, bf16 out.  Both operands are K-major (activations [tokens, K] and
 // torch-Linear weights [N, K]), so one {64 x rows} SWIZZLE_128B TMA box feeds either side.
 //
-// L2 -> shared-memory bandwidth (about 43 B/clk/SM chip-wide) bounds this kernel before the tensor
-// pipe does: a lone CTA streaming a 128 x 256 tile needs 96 B/clk.  So CTAs work in pairs
-// (cta_group::2): one 256 x BN tile per pair, each CTA loads its own 128 rows of A and HALF of the
-// weight tile (64 B/clk/SM), the leader issues M=256 MMAs that read both CTAs' shared memory, and each
-// CTA drains its own 128 accumulator rows.
-//
 // Persistent kernel, one CTA per SM, (128*kCtaGroup) x BN output tiles handed out round-robin:
-//   warp 0      TMA producer   (A 16 KB + W BN*128 B per 64-wide k-block, kStages ring)
-//   warp 1      MMA issuer     (4 x tcgen05.mma M128 N=BN K16 per k-block; two TMEM accumulators
-//                               so the epilogue of tile i overlaps the MMAs of tile i+1)
-//   warps 2..9  epilogue       (thread = output row; two warps per TMEM lane quarter split the
-//                               BN columns; bias / GELU / residual fused, 64-byte row stores)
+//   warpgroup 0   TMA producer (one thread; A 16 KB + W BN*128 B per 64-wide k-block, kStages ring)
+//   warpgroups 1-2 consumers: each owns 64 rows of the 128-row tile, wgmma m64 x BN x k16 (4 per k-block) into
+//                 registers, then bias / GELU / residual fused and bf16 pairs stored straight to the output
+//                 while the producer already streams the next tile's k-blocks
+// Two-CTA clusters (cta_group 2): one 256 x BN tile per pair, each CTA loads its own 128 rows of A and HALF of
+// the weight tile, multicast to both CTAs -- the weight tile crosses L2 -> SM once per pair.
 // SURVEY.md section 8 a11 (BERT-family encoder forward); structural oracle: oracle/bert_encoder.py.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -28,23 +23,8 @@ namespace {
 
 using namespace ptx;
 
-constexpr int kBM = 128, kBK = 64, kEpiWarps = 8, kGemmThreads = (2 + kEpiWarps) * 32;
+constexpr int kBM = 128, kBK = 64, kGemmThreads = 3 * 128;
 
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
-
-// GELU, exact-erf form (HF "gelu").  erf by Abramowitz-Stegun 7.1.26 (|err| < 1.5e-7 with exact
-// rcp / exp; the approx MUFU ops add ~1e-6, far below the bf16 rounding of the result); one
-// MUFU.RCP + one MUFU.EX2 per element, no slow paths.
 __device__ __forceinline__ float rcp_approx(float x) {
   float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y;
 }
@@ -69,227 +49,148 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
   return d;
 }
-__device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
-__device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xFFFF0000u); }
 
-template <int BN, int G>
+template <int BN>
 struct GemmSmem {
   static constexpr int kABytes = kBM * kBK * 2;          // 16 KB: this CTA's 128 rows of A
-  static constexpr int kBBytes = (BN / G) * kBK * 2;     // this CTA's share of the weight tile
+  static constexpr int kBBytes = BN * kBK * 2;           // the whole weight tile (half of it from the peer when paired)
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kOutBytes = kEpiWarps * 2 * 4096;  // per epilogue warp: two 32-row x 128-byte staging slabs
-  static constexpr int kStages = (160 * 1024) / kStageBytes > 8 ? 8 : (160 * 1024) / kStageBytes;
+  static constexpr int kStages = (192 * 1024) / kStageBytes > 8 ? 8 : (192 * 1024) / kStageBytes;
   static constexpr int kBarBytes = 256;
-  static constexpr size_t kTotal = 1024 + static_cast<size_t>(kStages) * kStageBytes + kOutBytes + kBarBytes;
+  static constexpr size_t kTotal = 1024 + static_cast<size_t>(kStages) * kStageBytes + kBarBytes;
+};
+
+template <int BN> struct Acc;
+template <> struct Acc<128> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128_ss(d, a, b, acc); }
+};
+template <> struct Acc<256> {
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n256_ss(d, a, b, acc); }
 };
 
 template <int BN, int EPI, int G>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               const __grid_constant__ CUtensorMap tmap_out, const GemmParams p) {
-  using S = GemmSmem<BN, G>;
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmParams p) {
+  using S = GemmSmem<BN>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (base & 1023u)) & 1023u);
   uint8_t* stage0 = smem;
-  uint8_t* out_stage = smem + S::kStages * S::kStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(out_stage + S::kOutBytes);
-  uint64_t* full = bars;                       // [kStages]  (the leader's copy is the live one)
-  uint64_t* empty = bars + S::kStages;         // [kStages]  per CTA: the commit multicasts to both
-  uint64_t* acc_full = bars + 2 * S::kStages;  // [2]        per CTA
-  uint64_t* acc_empty = acc_full + 2;          // [2]        leader's copy
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::kStages * S::kStageBytes);
+  uint64_t* full = bars;                       // [kStages]
+  uint64_t* empty = bars + S::kStages;         // [kStages]  both consumer warpgroups of every CTA the stage reaches
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const uint32_t rank = G == 2 ? cluster_ctarank() : 0u;
   const int group = blockIdx.x / G, n_groups = gridDim.x / G;
   const int n_tiles_total = p.m_tiles * p.n_tiles;   // tiles of (128*G) x BN
 
-  if constexpr (G == 2) cluster_sync_all();   // both CTAs resident before the paired TMEM allocation
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmap_a); prefetch_tmap(&tmap_b); prefetch_tmap(&tmap_out);
-    for (int s = 0; s < S::kStages; ++s) { mbar_init(&full[s], G); mbar_init(&empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&acc_full[a], 1); mbar_init(&acc_empty[a], kEpiWarps * G); }
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmap_a); prefetch_tmap(&tmap_b);
+    for (int s = 0; s < S::kStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2 * G); }
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc<G>(tmem_slot, 2 * BN); tmem_relinquish<G>(); }
-  tc_fence_before();
   if constexpr (G == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   grid_dep_launch();   // the next kernel may take over SMs as this grid's CTAs retire
   grid_dep_wait();     // everything above overlapped the previous kernel's tail; its output is needed from here on
 
-  if (warp == 0) {
-    // ------------------------------------------------------------ TMA producer (every CTA)
-    int stage = 0; uint32_t phase = 0;
-    for (int tile = group; tile < n_tiles_total; tile += n_groups) {
-      const int m_blk = tile / p.n_tiles, n_blk = tile % p.n_tiles;
-      const int a_row = (m_blk * G + static_cast<int>(rank)) * kBM;
-      const int b_row = n_blk * BN + static_cast<int>(rank) * (BN / G);
-      for (int kb = 0; kb < p.k_blocks; ++kb) {
-        mbar_wait(&empty[stage], phase ^ 1);
-        if (elect_one()) {
-          uint8_t* sa = stage0 + stage * S::kStageBytes;
-          if constexpr (G == 1) {
-            mbar_arrive_expect_tx(&full[stage], S::kStageBytes);
-            tma_load_2d(sa, &tmap_a, &full[stage], kb * kBK, a_row, kEvictNormal);
-            tma_load_2d(sa + S::kABytes, &tmap_b, &full[stage], kb * kBK, b_row, kEvictLast);
-          } else {
-            tma_load_2d_pair(sa, &tmap_a, &full[stage], kb * kBK, a_row, kEvictNormal);
-            tma_load_2d_pair(sa + S::kABytes, &tmap_b, &full[stage], kb * kBK, b_row, kEvictLast);
-            if (rank == 0) mbar_arrive_expect_tx(&full[stage], 2u * S::kStageBytes);
-            else mbar_arrive_cluster(&full[stage], 0);
-          }
-        }
-        __syncwarp();
-        if (++stage == S::kStages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (leader CTA)
-    if (rank == 0) {
-      constexpr uint32_t idesc = idesc_bf16_f32(kBM * G, BN);
-      int stage = 0; uint32_t phase = 0; int it = 0;
-      for (int tile = group; tile < n_tiles_total; tile += n_groups, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&acc_empty[acc], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BN;
+  if (wg == 0) {
+    // ------------------------------------------------------------ TMA producer
+    if (threadIdx.x == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int tile = group; tile < n_tiles_total; tile += n_groups) {
+        const int m_blk = tile / p.n_tiles, n_blk = tile % p.n_tiles;
+        const int a_row = (m_blk * G + static_cast<int>(rank)) * kBM;
+        const int b_row = n_blk * BN + static_cast<int>(rank) * (BN / G);
         for (int kb = 0; kb < p.k_blocks; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(stage0 + stage * S::kStageBytes);
-          const uint64_t a_desc = smem_desc_sw128(sa), b_desc = smem_desc_sw128(sa + S::kABytes);
-          if (elect_one()) {
-#pragma unroll
-            for (int ks = 0; ks < kBK / 16; ++ks)
-              mma_ss_bf16<G>(d_tmem, a_desc + 2 * ks, b_desc + 2 * ks, idesc, (kb | ks) != 0);
-            mma_commit<G>(&empty[stage]);
-            if (kb == p.k_blocks - 1) mma_commit<G>(&acc_full[acc]);
-          }
-          __syncwarp();
+          mbar_wait(&empty[stage], phase ^ 1);
+          uint8_t* sa = stage0 + stage * S::kStageBytes;
+          mbar_arrive_expect_tx(&full[stage], S::kStageBytes);
+          tma_load_2d(sa, &tmap_a, &full[stage], kb * kBK, a_row, kEvictNormal);
+          if constexpr (G == 1)
+            tma_load_2d(sa + S::kABytes, &tmap_b, &full[stage], kb * kBK, b_row, kEvictLast);
+          else
+            tma_load_2d_mc(sa + S::kABytes + rank * (S::kBBytes / 2), &tmap_b, &full[stage], kb * kBK, b_row, 0x3, kEvictLast);
           if (++stage == S::kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
   } else {
-    // ------------------------------------------------------------ epilogue (every CTA: its own 128 rows)
-    // Each warp turns [32 rows x 64 columns] of the accumulator into one 128-byte-swizzled slab in
-    // shared memory and hands it to a TMA store: full 128-byte lines leave the SM instead of 32
-    // scattered 16-byte pieces per store instruction.
-    const int ew = warp - 2, quarter = warp & 3, half = ew >> 2;
-    constexpr int kColsPerWarp = BN / 2;
-    uint8_t* my_stage = out_stage + ew * 8192;
-    const uint32_t sw = static_cast<uint32_t>(lane & 7);
-    int it = 0, slab = 0;
-    for (int tile = group; tile < n_tiles_total; tile += n_groups, ++it) {
+    // ------------------------------------------------------------ consumers: 64 rows each
+    const int t = threadIdx.x - 128 * wg, w = t >> 5, l = t & 31;
+    const int half = wg - 1;
+    int stage = 0; uint32_t phase = 0;
+    for (int tile = group; tile < n_tiles_total; tile += n_groups) {
       const int m_blk = tile / p.n_tiles, n_blk = tile % p.n_tiles;
-      const int acc = it & 1;
-      const int row0 = (m_blk * G + static_cast<int>(rank)) * kBM + quarter * 32;
-      const int col0 = n_blk * BN + half * kColsPerWarp;
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + half * kColsPerWarp;
-      const __nv_bfloat16* rrow = EPI == kEpiBiasResid ? p.resid + static_cast<size_t>(row0 + lane) * p.ldr + col0 : nullptr;
-      // Residual: every lane reads 64 bytes of ITS row per 32-column unit -- 32 different lines per load instruction,
-      // ~1 us from L2.  The loads do not depend on the accumulator, so the first two units are requested BEFORE the
-      // wait for the MMAs of this tile and each later unit two units ahead of its use; with K = 768 (out-proj) a tile's
-      // MMAs last only ~6k cycles and the exposed latency used to make this epilogue the slower side of the pipeline.
-      constexpr int kUnits = kColsPerWarp / 32;
-      uint4 res_q[2][4];
-      auto load_res = [&](int u, uint4 (&r)[4]) {
-        if constexpr (EPI == kEpiBiasResid) {
+      float d[BN / 2];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) r[j] = (u < kUnits) ? __ldg(reinterpret_cast<const uint4*>(rrow + 32 * u) + j) : make_uint4(0, 0, 0, 0);
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      for (int kb = 0; kb < p.k_blocks; ++kb) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(stage0 + stage * S::kStageBytes);
+        const uint64_t a_desc = wgmma_desc_sw128(sa + half * 64 * 128), b_desc = wgmma_desc_sw128(sa + S::kABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kBK / 16; ++ks) Acc<BN>::mma(d, a_desc + 2 * ks, b_desc + 2 * ks, 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(d);
+        if (t == 0) {
+          mbar_arrive(&empty[stage]);
+          if constexpr (G == 2) mbar_arrive_cluster(&empty[stage], rank ^ 1u);
         }
-      };
-      load_res(0, res_q[0]);
-      load_res(1, res_q[1]);
-      mbar_wait(&acc_full[acc], (it >> 1) & 1);
-      tc_fence_after();
+        if (++stage == S::kStages) { stage = 0; phase ^= 1; }
+      }
+      // epilogue: register i of the accumulator = row 16 w + l / 4 (+ 8 for i & 2), column 8 (i / 4) + 2 (l % 4) (+ 1)
+      const int row_lo = (m_blk * G + static_cast<int>(rank)) * kBM + half * 64 + 16 * w + (l >> 2);
+      const int col_base = n_blk * BN + 2 * (l & 3);
 #pragma unroll
-      for (int cu = 0; cu < kColsPerWarp / 64; ++cu, slab ^= 1) {
-        const int c = cu * 64;
-        uint8_t* buf = my_stage + slab * 4096;
-        // the TMA store that last read this slab (two slabs ago) must have drained it
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        __syncwarp();
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = col_base + 8 * j;
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
-          uint32_t v[32];
-          tmem_ld_x32(taddr + c + 32 * hh, v);
-          uint4 res[4];
+          const int row = row_lo + 8 * hh;
+          float x0 = d[4 * j + 2 * hh] + b.x, x1 = d[4 * j + 2 * hh + 1] + b.y;
+          if constexpr (EPI == kEpiBiasGelu) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
           if constexpr (EPI == kEpiBiasResid) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) res[j] = res_q[hh][j];
-            load_res(2 * cu + hh + 2, res_q[hh]);          // two units ahead
+            const __nv_bfloat162 r = *reinterpret_cast<const __nv_bfloat162*>(p.resid + static_cast<size_t>(row) * p.ldr + col);
+            x0 += __bfloat162float(r.x); x1 += __bfloat162float(r.y);
           }
-          tmem_wait_ld();
-          uint32_t o[16];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + c + 32 * hh) + j);
-            float x0 = __uint_as_float(v[4 * j + 0]) + b.x, x1 = __uint_as_float(v[4 * j + 1]) + b.y;
-            float x2 = __uint_as_float(v[4 * j + 2]) + b.z, x3 = __uint_as_float(v[4 * j + 3]) + b.w;
-            if constexpr (EPI == kEpiBiasGelu) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); x2 = gelu_erf(x2); x3 = gelu_erf(x3); }
-            if constexpr (EPI == kEpiBiasResid) {
-              const uint32_t* rw = reinterpret_cast<const uint32_t*>(res);
-              x0 += bf16_lo(rw[2 * j]); x1 += bf16_hi(rw[2 * j]); x2 += bf16_lo(rw[2 * j + 1]); x3 += bf16_hi(rw[2 * j + 1]);
-            }
-            o[2 * j] = pack_bf16x2(x0, x1); o[2 * j + 1] = pack_bf16x2(x2, x3);
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {   // 16-byte chunk (4*hh + j) of this lane's 128-byte row, XOR-swizzled
-            const uint32_t chunk = static_cast<uint32_t>(4 * hh + j) ^ sw;
-            *reinterpret_cast<uint4*>(buf + lane * 128 + chunk * 16) = make_uint4(o[4 * j], o[4 * j + 1], o[4 * j + 2], o[4 * j + 3]);
-          }
+          *reinterpret_cast<uint32_t*>(p.out + static_cast<size_t>(row) * p.ldo + col) = pack_bf16x2(x0, x1);
         }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::
-                           "l"(reinterpret_cast<uint64_t>(&tmap_out)), "r"(smem_u32(buf)), "r"(col0 + c), "r"(row0) : "memory");
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (G == 2) mbar_arrive_cluster(&acc_empty[acc], 0); else mbar_arrive(&acc_empty[acc]);
       }
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // stores complete before exit
   }
-  tc_fence_before();
-  if constexpr (G == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc<G>(tmem_base, 2 * BN); }
+  // no CTA of a pair exits while its peer may still multicast into it or arrive on its barriers
+  if constexpr (G == 2) cluster_sync_all();
 }
 
 template <int BN, int EPI, int G>
-cudaError_t launch_one(int sm_count, const void* tmap_a, const void* tmap_b, const void* tmap_out, const GemmParams& p,
-                       cudaStream_t s) {
+cudaError_t launch_one(int sm_count, const void* tmap_a, const void* tmap_b, const GemmParams& p, cudaStream_t s) {
   auto kern = gemm_tc_kernel<BN, EPI, G>;
   static bool attr_set = false;   // per instantiation
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(GemmSmem<BN, G>::kTotal));
+                                         static_cast<int>(GemmSmem<BN>::kTotal));
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
   const int tiles = p.m_tiles * p.n_tiles, groups = sm_count / G;
   return launch_pdl(kern, dim3(static_cast<unsigned>((tiles < groups ? tiles : groups) * G)), dim3(kGemmThreads),
-                    GemmSmem<BN, G>::kTotal, s, G, *reinterpret_cast<const CUtensorMap*>(tmap_a),
-                    *reinterpret_cast<const CUtensorMap*>(tmap_b), *reinterpret_cast<const CUtensorMap*>(tmap_out), p);
+                    GemmSmem<BN>::kTotal, s, G, *reinterpret_cast<const CUtensorMap*>(tmap_a),
+                    *reinterpret_cast<const CUtensorMap*>(tmap_b), p);
 }
 
 }  // namespace
 
 // cta_group: 1 = one CTA per 128 x bn tile, 2 = CTA pair per 256 x bn tile (p.m_tiles counts those).
-// tmap_b must have a {64, bn / cta_group} box, tmap_out (over the output matrix) a {64, 32} box.
+// tmap_b must have a {64, bn / cta_group} box.
 cudaError_t gemm_tc_launch(int cta_group, int bn, int epi, int sm_count, const void* tmap_a, const void* tmap_b,
-                           const void* tmap_out, const GemmParams& p, cudaStream_t s) {
+                           const GemmParams& p, cudaStream_t s) {
   if (p.m_tiles * p.n_tiles <= 0) return cudaSuccess;
 #define AUR_GEMM_CASE(BN, EPI, G) \
-  if (bn == BN && epi == EPI && cta_group == G) return launch_one<BN, EPI, G>(sm_count, tmap_a, tmap_b, tmap_out, p, s)
+  if (bn == BN && epi == EPI && cta_group == G) return launch_one<BN, EPI, G>(sm_count, tmap_a, tmap_b, p, s)
   AUR_GEMM_CASE(256, kEpiBias, 2); AUR_GEMM_CASE(256, kEpiBiasGelu, 2); AUR_GEMM_CASE(256, kEpiBiasResid, 2);
   AUR_GEMM_CASE(128, kEpiBias, 2); AUR_GEMM_CASE(128, kEpiBiasGelu, 2); AUR_GEMM_CASE(128, kEpiBiasResid, 2);
   AUR_GEMM_CASE(256, kEpiBias, 1); AUR_GEMM_CASE(256, kEpiBiasGelu, 1); AUR_GEMM_CASE(256, kEpiBiasResid, 1);

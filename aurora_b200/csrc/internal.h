@@ -34,34 +34,31 @@ __host__ __device__ __forceinline__ uint64_t make_key(float score, int32_t row) 
 __host__ __device__ __forceinline__ int32_t key_row(uint64_t k) { return static_cast<int32_t>(~static_cast<uint32_t>(k)); }
 __host__ __device__ __forceinline__ float key_score(uint64_t k) { return ord_to_f32(static_cast<uint32_t>(k >> 32)); }
 
-// ---------------------------------------------------------------- tcgen05 similarity kernel
+// ---------------------------------------------------------------- wgmma similarity kernel
 constexpr int kTcTileN = 64;       // corpus rows per tile  (MMA N)
-constexpr int kTcKBlock = 64;      // bf16 per 128-byte swizzled smem row
-constexpr int kTcKbPerStage = 4;   // k-blocks per pipeline stage
-constexpr int kTcQRows = 128;      // queries per CTA (TMEM lanes)
+constexpr int kTcKBlock = 64;      // bf16 per 128-byte swizzled smem row (one pipeline stage)
+constexpr int kTcQRows = 64;       // queries per CTA (MMA M of one warpgroup)
 constexpr int kTcChunk = 16;       // scores examined per threshold test
 constexpr int kTcListMin = 64;     // list slots per query: max(ksel, this) so a whole first tile appends
 constexpr int kTcMaxStages = 12;
-constexpr int kTcTmemDim = 768;    // query dims resident in TMEM (384 columns); dims beyond live in shared memory
-constexpr int kTcMaxDim = 1024;    // largest dim served by the tcgen05 path
-constexpr int kTcAccCol0 = 384;    // accumulator buffers at TMEM columns 384 / 448
+constexpr int kTcMaxDim = 1024;    // largest dim served by the tensor-core path (the query block stays in shared memory)
 constexpr int kTcFifoRecs = 16;    // parked 4-score groups per thread before the deferred slow path runs
 constexpr int kTcFifoMaxKsel = 64; // (the FIFO shares shared memory with the candidate lists)
 constexpr int kSlack = 8;          // extra candidates kept for the exact re-rank
 constexpr int kMaxK = 128;
 
 struct TcParams {
-  const __nv_bfloat16* q;   // [nq, dim] queries of this launch (<= 128 * n_qblocks)
+  const __nv_bfloat16* q;   // [nq, dim] queries of this launch (<= 64 * n_qblocks)
   const float* inv_norm;    // [n_rows]   1/|c_j|, 0 for zero rows, NaN for tombstones
   const uint32_t* row_mask; // nullable [n_rows]: bit s = tenant scope s of this batch may see the row (per-query scopes)
   const int32_t* q_scope;   // with row_mask: [nq] scope index (0..31) of every query
-  uint64_t* cand;           // [128 * n_qblocks, n_lists * ksel] candidate keys, compacted per
+  uint64_t* cand;           // [64 * n_qblocks, n_lists * ksel] candidate keys, compacted per
                             // query: only keys that pass the final threshold are appended
-  uint32_t* cand_count;     // [128 * n_qblocks] appended keys per query (zero on entry)
-  float* dbg_scores;        // optional [grid, 128, 64]: first tile's scores of every CTA
+  uint32_t* cand_count;     // [64 * n_qblocks] appended keys per query (zero on entry)
+  float* dbg_scores;        // optional [grid, 64, 64]: first tile's scores of every CTA
   uint64_t* pub;            // cross-CTA threshold exchange, entries (epoch << 32 | score bits):
-                            // [n_qblocks, 128, n_lists (even)] each CTA's m-th best per query,
-                            // then [n_qblocks, 128] the served thresholds
+                            // [n_qblocks, 64, n_lists (even)] each CTA's m-th best per query,
+                            // then [n_qblocks, 64] the served thresholds
   int64_t n_rows;
   uint32_t epoch;           // launch counter: pub entries of older launches are ignored
   const uint32_t* epoch_ptr;// when set, the counter lives in device memory (bumped by the finalize kernel)
@@ -73,12 +70,12 @@ struct TcParams {
 };
 constexpr int kTcPubMax = 74;      // published values a thread folds into its threshold
 
-// epi_groups: 1 = four epilogue warps take every tile; 2 = two sets of four alternate tiles
-// (each set owns one TMEM accumulator buffer and its own candidate lists).
-size_t tc_smem_bytes(int cta_group, int epi_groups, int num_stages, int ksel, int dim);
-int tc_pick_stages(int cta_group, int epi_groups, int ksel, int dim, size_t smem_limit);
-// Launches the fused similarity + top-k kernel.  tmap: CUtensorMap over the corpus with a
-// {64, 64 / cta_group} box and 128-byte swizzle.
+// epi_groups: 1 = two epilogue warps take every tile; 2 = two pairs of warps alternate tiles
+// (each pair owns one score buffer and its own candidate lists).
+size_t tc_smem_bytes(int epi_groups, int num_stages, int ksel, int dim);
+int tc_pick_stages(int epi_groups, int ksel, int dim, size_t smem_limit);
+// Launches the fused similarity + top-k kernel; cta_group 2 = two-CTA clusters sharing every corpus tile by TMA
+// multicast.  tmap: CUtensorMap over the corpus with a {64, 64 / cta_group} box and 128-byte swizzle.
 cudaError_t tc_launch(int cta_group, int epi_groups, int grid, const void* tmap, const TcParams& p, size_t smem,
                       cudaStream_t s);
 
@@ -107,7 +104,7 @@ struct FinalizeArgs {
   const uint64_t* cand; int n_lists; int ksel;
   uint32_t* counts;  // nullable: per-query number of valid keys at the front of its cand row
                      // (reset to 0 by the kernel); null = all n_lists * ksel slots are keys
-  uint32_t* epoch_bump;  // nullable: the tcgen05 kernel's device-resident launch counter, advanced here (never 0)
+  uint32_t* epoch_bump;  // nullable: the tensor-core kernel's device-resident launch counter, advanced here (never 0)
   const void* q; const void* rows; int dtype; int dim; int nq; int k;
   const int64_t* ids;
   float* out_scores; int64_t* out_ids; double* out_scores64;   // (out_scores / out_ids nullable in exchange mode)
@@ -147,7 +144,7 @@ cudaError_t launch_fill_f32(float* p, float v, int64_t n, cudaStream_t s);
 // out[i] = OR over the batch's distinct tenant scopes s < n_scopes of (visible(row i, scope s) << s); scopes = {user, org} pairs
 cudaError_t launch_row_scope_mask(const int32_t* row_user, const int32_t* row_org, const int32_t* scopes, int n_scopes, int64_t n,
                                   uint32_t* out, cudaStream_t s);
-// out[i] = visible(user u, org o) ? inv[i] : NaN  -- lets the tcgen05 kernel serve a batch whose queries all
+// out[i] = visible(user u, org o) ? inv[i] : NaN  -- lets the tensor-core kernel serve a batch whose queries all
 // carry the same tenant scope
 cudaError_t launch_mask_inv_norm(const float* inv, const int32_t* row_user, const int32_t* row_org, int32_t u, int32_t o,
                                  int64_t n, float* out, cudaStream_t s);
@@ -160,16 +157,18 @@ cudaError_t launch_gather_rows(const void* rows, const float* inv, const int64_t
                                int32_t* o_user, int32_t* o_org, cudaStream_t s);
 
 // ---------------------------------------------------------------- encoder (BERT-family forward)
-// out = epi(A . W^T + bias): A [m_tiles*128, K] bf16 (TMA box {64,128}), W [N, K] bf16 (TMA box {64,BN}).
+// out = epi(A . W^T + bias): A [m_tiles*128, K] bf16 (TMA box {64,128}), W [N, K] bf16 (TMA box {64,BN/cta_group}).
 enum { kEpiBias = 0, kEpiBiasGelu = 1, kEpiBiasResid = 2 };
 struct GemmParams {
   const float* bias;            // [N]
   const __nv_bfloat16* resid;   // [rows, ldr] (kEpiBiasResid only)
-  int ldr;                      // (the output goes through tmap_out: TMA store)
+  int ldr;
+  __nv_bfloat16* out;           // [m_tiles * 128 * cta_group, ldo]
+  int ldo;
   int m_tiles, n_tiles, k_blocks;   // (128 * cta_group)-row tiles, BN-column tiles, 64-wide k-blocks
 };
 cudaError_t gemm_tc_launch(int cta_group, int bn, int epi, int sm_count, const void* tmap_a, const void* tmap_b,
-                           const void* tmap_out, const GemmParams& p, cudaStream_t s);
+                           const GemmParams& p, cudaStream_t s);
 
 // Self-attention over packed variable-length sequences (<= 512 tokens each), head dim 64.
 // One work item = (sequence, 128-query block); every item runs for all heads.
@@ -180,14 +179,7 @@ struct AttnParams {
   float scale_log2e;                  // log2(e) / sqrt(head_dim)
 };
 // tmap_qkv: CUtensorMap over the packed [tokens, 3*hidden] projections, box {64, 128}, SWIZZLE_128B.
-cudaError_t attn_tc_launch(int sm_count, const void* tmap_qkv, const AttnParams& p, cudaStream_t s);
-// Version 2 (attn_tc2.cu): two work items in flight per CTA, one key block at a time, online softmax.  Same arguments.
-cudaError_t attn_tc2_launch(int sm_count, const void* tmap_qkv, const AttnParams& p, cudaStream_t s);
-// The attention kernel the encoder uses: version 2 unless AUR_ATTN_V1=1 is set in the environment (A/B runs).
-inline cudaError_t attn_launch(int sm_count, const void* tmap_qkv, const AttnParams& p, cudaStream_t s) {
-  static const bool v1 = [] { const char* e = getenv("AUR_ATTN_V1"); return e && e[0] == '1'; }();
-  return v1 ? attn_tc_launch(sm_count, tmap_qkv, p, s) : attn_tc2_launch(sm_count, tmap_qkv, p, s);
-}
+cudaError_t attn_tc_launch(const void* tmap_qkv, const AttnParams& p, cudaStream_t s);
 
 cudaError_t launch_embed_ln(const int32_t* tok, const int32_t* pos, int n_tok, int n_rows_pad,
                             const __nv_bfloat16* word, const __nv_bfloat16* pos_emb, const __nv_bfloat16* type_emb,

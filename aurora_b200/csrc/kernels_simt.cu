@@ -625,7 +625,7 @@ cudaError_t launch_cosine_pairs(const float* a, const float* b, int64_t n, int d
 }
 
 // Tenant scope folded into the row scale: rows the (user, org) pair may not see get NaN, which the
-// tcgen05 kernel treats exactly like a tombstone (never admitted, never published).  Same predicate
+// tensor-core kernel treats exactly like a tombstone (never admitted, never published).  Same predicate
 // as simt_scores_kernel: row_user == u OR (o >= 0 AND row_org == o)  (weaviate_client.py:244-249).
 __global__ void mask_inv_norm_kernel(const float* __restrict__ inv, const int32_t* __restrict__ row_user,
                                      const int32_t* __restrict__ row_org, int32_t u, int32_t o, int64_t n,

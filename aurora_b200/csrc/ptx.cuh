@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for the sm_100a features the similarity kernel uses:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / st / fences),
-// cluster barriers.  One wrapper = one instruction; no abstractions on top.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use: mbarrier, TMA
+// (cp.async.bulk.tensor, with cluster multicast), wgmma, cluster barriers.  One wrapper = one
+// instruction; no abstractions on top.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -120,132 +120,89 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, ui
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
       : "memory");
 }
-// CTA-pair variant: data lands in this CTA's smem, bytes are credited to the barrier at
-// the same offset in the pair's even (leader) CTA.
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0,
-                                                 int32_t c1, uint64_t hint) {
+// Cluster multicast: the box lands at the same smem offset in every CTA of cta_mask, and each
+// destination's barrier at the offset of `bar` is credited with the bytes it received.
+__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0, int32_t c1,
+                                               uint16_t cta_mask, uint64_t hint) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "l"(hint)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask), "l"(hint)
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols) : "memory");
-  else
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "r"(ncols) : "memory");
-}
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_relinquish() {
-  if constexpr (kCtaGroup == 1) asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  else asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  else
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[tmem] * B[smem]^T, bf16 inputs, fp32 accumulate.  One thread issues.
-template <int kCtaGroup>
-__device__ __forceinline__ void mma_ts_bf16(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T (used by the encoder GEMMs and the SS probe).
-template <int kCtaGroup>
-__device__ __forceinline__ void mma_ss_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// Make `bar` (same offset in every CTA of the MMA's group) complete a phase once all
-// previously issued MMAs of this thread have finished.  Implies fence::before_thread_sync.
-template <int kCtaGroup>
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  if constexpr (kCtaGroup == 1)
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-  else
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(static_cast<uint16_t>(3)) : "memory");
-}
-
-// smem matrix descriptor: K-major tile, 128-byte swizzle, rows 128 B apart, 8-row groups
-// 1024 B apart (the layout a {64 x rows} bf16 TMA box with SWIZZLE_128B produces).
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t smem_addr) {
+// ---------------------------------------------------------------- wgmma (sm_90a)
+// Shared-memory matrix descriptor, 128-byte swizzle (the layout a {64 x rows} bf16 TMA box with SWIZZLE_128B
+// produces): 8-row groups 1024 B apart.  K-major operand: advancing K by 16 elements = +32 B on the address.
+// MN-major operand (V of the attention): 64 elements of MN per 128-byte row, one row per K index, so a K step of 16
+// is +2048 B.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);          // start address   [0,14)
-  d |= static_cast<uint64_t>(0) << 16;                               // LBO (unused)    [16,30)
+  d |= static_cast<uint64_t>(1) << 16;                               // LBO (unused)    [16,30)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;                       // SBO             [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                               // version = 1     [46,48)
-  d |= static_cast<uint64_t>(2) << 61;                               // SWIZZLE_128B    [61,64)
+  d |= static_cast<uint64_t>(1) << 62;                               // SWIZZLE_128B    [62,64)
   return d;
 }
-__device__ __forceinline__ uint64_t pack_u64(uint32_t lo, uint32_t hi) {
-  uint64_t d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi));
-  return d;
-}
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major.
-__host__ __device__ constexpr uint32_t idesc_bf16_f32(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accumulator reads / writes across an in-flight wgmma.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 32-bit, N consecutive columns per thread: thread t <-> TMEM lane 32*(warp%4)+t.
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
+#define AUR_R8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64 x 64] (+)= A[smem, K-major] . B[smem, K-major]^T, bf16 in, fp32 accumulate; one K=16 step.
+__device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31},"
+      " %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : AUR_R8(0), AUR_R8(8), AUR_R8(16), AUR_R8(24)
+      : "l"(a), "l"(b), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_st_x16(uint32_t taddr, const uint32_t (&r)[16]) {
+// Same, N = 128.
+__device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t a, uint64_t b, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::
-          "r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63},"
+      " %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : AUR_R8(0), AUR_R8(8), AUR_R8(16), AUR_R8(24), AUR_R8(32), AUR_R8(40), AUR_R8(48), AUR_R8(56)
+      : "l"(a), "l"(b), "r"(accumulate));
 }
+// Same, N = 256.
+__device__ __forceinline__ void wgmma_m64n256_ss(float (&d)[128], uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+      "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+      "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127},"
+      " %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : AUR_R8(0), AUR_R8(8), AUR_R8(16), AUR_R8(24), AUR_R8(32), AUR_R8(40), AUR_R8(48), AUR_R8(56),
+        AUR_R8(64), AUR_R8(72), AUR_R8(80), AUR_R8(88), AUR_R8(96), AUR_R8(104), AUR_R8(112), AUR_R8(120)
+      : "l"(a), "l"(b), "r"(accumulate));
+}
+// D[64 x 64] += A[registers: four bf16x2 per thread, the accumulator layout of a 64 x 16 block] . B[smem, MN-major]
+__device__ __forceinline__ void wgmma_m64n64_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31},"
+      " {%32,%33,%34,%35}, %36, p, 1, 1, 1;\n\t}"
+      : AUR_R8(0), AUR_R8(8), AUR_R8(16), AUR_R8(24)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+}
+#undef AUR_R8
 
-// Packed fp32x2 multiply (FMUL2 on sm_100): both halves rounded like a scalar mul.rn.
-__device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
 __device__ __forceinline__ void unpack_u64(uint64_t v, uint32_t& lo, uint32_t& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v));
 }

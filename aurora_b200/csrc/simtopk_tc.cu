@@ -1,45 +1,40 @@
-// Fused similarity + top-k for sm_100a: S = Q . C^T on tcgen05 tensor cores with the
-// query block resident in TMEM, the corpus streamed once from HBM by TMA, and a per-query
+// Fused similarity + top-k for sm_90a: S = Q . C^T on wgmma tensor cores with the query
+// block resident in shared memory, the corpus streamed once from HBM by TMA, and a per-query
 // candidate list kept in shared memory by the epilogue warps.
 //
 // Replaces the dense leg of collection.query.hybrid(...) / near_text(...) that the
 // reference sends to Weaviate (server/routes/knowledge_base/weaviate_client.py:252-259,
 // server/routes/incident_feedback/weaviate_client.py:286-291).
 //
-// One CTA, persistent, 1 CTA / SM (G = 1 or 2 epilogue groups; 32 * (4G + 3) threads):
-//   warps 1..4G epilogue  : thread r of a group owns query r (TMEM lane r): tcgen05.ld its 64 scores of
-//                           a tile, scale by the rows' inverse norms (FMUL2), keep one max
-//                           per 16 scores and compare it with the query's threshold; a
-//                           four-score group that reaches it is parked in a per-thread FIFO
-//                           in shared memory and examined later, out of line and rarely
-//                           (drain_fifo); large k without room for the FIFO pushes at once
-//                           (push_group4).
-//   warp 0     threshold   : serves the certified global threshold of the one or two queries
-//                           assigned to this CTA (see "Threshold exchange").
-//                           With two groups, group g takes tiles g, g+2, ... (TMEM buffer g):
-//                           two MMA tile-times per tile, so the MMA rarely waits on them.
-//   warp 4G+1  TMA producer: corpus tiles [64 rows x 256 k] -> smem ring (SWIZZLE_128B)
-//   warp 4G+2  MMA issuer  : tcgen05.mma kind::f16, A = queries from TMEM (128 lanes = 128
-//                           queries, dim/2 columns; dims past 768 from a swizzled tile in
-//                           shared memory instead), B = corpus tile from smem, D = [128
-//                           queries x 64 rows] fp32 in one of two TMEM buffers.
-// (The scheduler favours the highest warp id of a sub-partition: the two latency-critical
-// single-thread roles get the top ids, the background threshold warp the bottom one.)
-// cta_group::2: a CTA pair shares every corpus tile -- each CTA TMA-loads 32 of the 64
-// rows, the leader issues M=256 MMAs, each CTA's TMEM holds its own 128 queries.
-// cta_group::1: M=128; when nq > 128 two CTAs take the same tiles for the two query halves.
+// One CTA, persistent, 1 CTA / SM (G = 1 or 2 epilogue groups):
+//   warps 1..2G  epilogue  : thread r of a group owns query r (score-buffer row r): reads its 64 scores of a
+//                            tile, scales them by the rows' inverse norms, keeps one max per 16 scores and
+//                            compares it with the query's threshold; a four-score group that reaches it is
+//                            parked in a per-thread FIFO in shared memory and examined later, out of line and
+//                            rarely (drain_fifo); large k without room for the FIFO pushes at once (push_group4).
+//   warp 0      threshold  : serves the certified global threshold of the queries assigned to this CTA (see
+//                            "Threshold exchange").
+//   warp 2G+1   TMA producer: corpus tiles [64 rows x 64 k] -> smem ring (SWIZZLE_128B)
+//   warpgroup   MMA        : wgmma m64n64k16, A = the CTA's 64 queries (K-major tiles in shared memory), B =
+//                            corpus tile from the ring; the [64 queries x 64 rows] fp32 accumulator lives in
+//                            registers for the whole tile and is then stored to a padded score buffer that the
+//                            epilogue group of that tile reads row-wise (one buffer per group).  The MMA of the
+//                            next tile runs while the epilogue works on the buffer it just released.
+// Two-CTA clusters (AUR_KERNEL_TC2): the pair shares every corpus tile -- each CTA TMA-loads 32 of the 64 rows and
+// multicasts them to both, so a tile crosses L2 -> SM once per pair; each CTA scores its own 64 queries.
+// Single CTAs: when nq > 64 several CTAs take the same tiles for different query blocks (sharing through L2).
 //
-// Threshold exchange.  A CTA sees only 1/74 of the corpus, so its own k-th best is a loose
+// Threshold exchange.  A CTA sees only a slice of the corpus, so its own k-th best is a loose
 // filter.  Every epilogue thread therefore publishes its best (or 2nd best) score so far
-// into a [query][CTA] table.  Query q is served by CTA q mod 74: its threshold warp reads
-// the row of q every couple of microseconds, takes the R-th largest entry (R * m >= k +
+// into a [query][CTA] table.  Query q is served by one CTA of its query block: its threshold
+// warp reads the row of q every couple of microseconds, takes the R-th largest entry (R * m >= k +
 // slack) and publishes it: at least k + slack rows with a score >= that value exist
 // somewhere, so nothing below it can reach the final top-k.  Every epilogue thread reads its
 // query's current threshold once per tile.  A query then admits only a handful of rows per
 // CTA over a 1M-row scan.
 //
 // Bootstrap.  On its first tile a thread only publishes the tile's best score and waits for
-// the first certified threshold (all CTAs do this at the same time, ~5 us once), then
+// the first certified threshold (all CTAs do this at the same time, once), then
 // examines the tile against it: no arbitrary rows ever enter a list.
 //
 // Candidate list.  Append-only, ksel slots per query.  If it fills up it is compacted:
@@ -64,31 +59,36 @@ using namespace ptx;
 namespace {
 
 constexpr int kThrWarps = 1;
-constexpr int kQStageBufs = 2;   // ring stages (the last ones) the query load borrows as its transpose buffer
+// warps: threshold, 2G epilogue, producer, then the MMA warpgroup at the next multiple of four.  G = 1: 8 warps, two per
+// SM sub-partition, up to 255 registers a thread (no spills).  G = 2 (selectable for experiments) needs 10 live warps,
+// three on some sub-partition, which caps a thread at 168 registers whatever the order of the roles: a spill of a few
+// bytes in that variant.
+__host__ __device__ constexpr int tc_mma_warp0(int epi_groups) { return (kThrWarps + 2 * epi_groups + 1 + 3) / 4 * 4; }
 constexpr uint32_t kSlot = kTcQRows * 8u;   // byte stride between list slots of one query
+constexpr uint32_t kStageBytes = kTcTileN * 128u;   // one 64-dim k-block of a 64-row corpus tile
+constexpr uint32_t kQTileBytes = kTcQRows * 128u;   // one 64-dim k-block of the query block
+constexpr int kScStride = kTcTileN + 4;             // floats per score-buffer row (padding spreads the banks)
+constexpr uint32_t kScBytes = kTcQRows * kScStride * 4u;
 
 struct SmemLayout {
-  uint32_t stage_bytes, box_bytes, lcap, fifo_recs, qs_kb;
-  uint32_t off_qs, off_list, off_norm, off_mask, off_fifo, off_tau, off_bar, total;
+  uint32_t lcap, fifo_recs;
+  uint32_t off_qs, off_sc, off_list, off_norm, off_mask, off_fifo, off_tau, off_bar, total;
 };
-__host__ __device__ inline SmemLayout make_layout(int cta_group, int epi_groups, int num_stages, int ksel, int dim) {
+__host__ __device__ inline SmemLayout make_layout(int epi_groups, int num_stages, int ksel, int dim) {
   SmemLayout L;
-  L.box_bytes = (kTcTileN / cta_group) * 128u;
-  L.stage_bytes = L.box_bytes * kTcKbPerStage;
   L.lcap = static_cast<uint32_t>(ksel);
-  uint32_t o = L.stage_bytes * num_stages;
-  // query dims beyond the 768 that fit TMEM: [128 queries x 64] bf16 K-major SWIZZLE_128B tiles, one per
-  // 64-dim k-block (the SS-MMA A operand); 1024-byte aligned because the stages are
-  L.qs_kb = dim > kTcTmemDim ? static_cast<uint32_t>((dim - kTcTmemDim) / kTcKBlock) : 0u;
-  L.off_qs = o;     o += L.qs_kb * (kTcQRows * 128u);
+  uint32_t o = kStageBytes * num_stages;
+  // the query block: [64 queries x 64] bf16 K-major SWIZZLE_128B tiles, one per k-block (the wgmma A operand)
+  L.off_qs = o;     o += static_cast<uint32_t>(dim / kTcKBlock) * kQTileBytes;
+  L.off_sc = o;     o += static_cast<uint32_t>(epi_groups) * kScBytes;
   L.off_list = o;   o += static_cast<uint32_t>(epi_groups) * L.lcap * kSlot;
-  L.off_norm = o;   o += static_cast<uint32_t>(epi_groups) * 4u * 2u * kTcTileN * 4u;
-  L.off_mask = o;   o += static_cast<uint32_t>(epi_groups) * 4u * 2u * kTcTileN * 4u;   // per-row tenant-scope bit masks (kMask launches)
+  L.off_norm = o;   o += static_cast<uint32_t>(epi_groups) * 2u * 2u * kTcTileN * 4u;
+  L.off_mask = o;   o += static_cast<uint32_t>(epi_groups) * 2u * 2u * kTcTileN * 4u;   // per-row tenant-scope bit masks (kMask launches)
   // deferred-candidate FIFO: per thread kTcFifoRecs records of four adjacent scores (16 B) + a row tag
   L.fifo_recs = (epi_groups == 1 && ksel <= kTcFifoMaxKsel) ? kTcFifoRecs : 0u;
   L.off_fifo = o;   o += L.fifo_recs * kTcQRows * (16u + 4u);
-  L.off_tau = o;    o += kTcQRows * 4u;   // certified thresholds of this CTA's 128 queries, refreshed by the threshold warp
-  L.off_bar = o;    o += (2u * kTcMaxStages + 2u + 2u + 2u) * 8u + 16u;
+  L.off_tau = o;    o += kTcQRows * 4u;   // certified thresholds of this CTA's queries, refreshed by the threshold warp
+  L.off_bar = o;    o += (2u * kTcMaxStages + 2u + 2u + 1u) * 8u + 16u;
   L.total = o;
   return L;
 }
@@ -246,7 +246,6 @@ __device__ __forceinline__ float read_threshold(const unsigned long long* tq, ui
   return (static_cast<uint32_t>(e >> 32) == epoch) ? __uint_as_float(static_cast<uint32_t>(e)) : -INFINITY;
 }
 
-constexpr uint32_t kDescHi = 0x40004040u;  // SBO = 1024 B, descriptor version 1, SWIZZLE_128B
 constexpr uint32_t kNaNBits = 0x7FC00000u;
 
 // kMask: the queries of the batch carry different tenant scopes (user_id == u OR org_id == o,
@@ -255,30 +254,29 @@ constexpr uint32_t kNaNBits = 0x7FC00000u;
 // else looks at them, exactly like tombstones.  (One scope for the whole batch needs none of this: it folds into the
 // inverse norms.)
 template <int kCtaGroup, int kEpiGroups, bool kMask>
-__global__ void __launch_bounds__(32 * (4 * kEpiGroups + 3), 1)
+__global__ void __launch_bounds__(32 * (tc_mma_warp0(kEpiGroups) + 4), 1)
 simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
-  constexpr int kEpiWarps = 4 * kEpiGroups;
+  constexpr int kEpiWarps = 2 * kEpiGroups;
   constexpr int kProducerWarp = kEpiWarps + kThrWarps;
-  constexpr int kMmaWarp = kProducerWarp + 1;
+  constexpr int kMmaWarp0 = tc_mma_warp0(kEpiGroups);   // first warp of the MMA warpgroup (warpgroup-aligned)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment; the runtime only guarantees 16.  Offsetting
   // the declared array (rather than round-tripping through an integer) keeps the compiler's
   // shared-address-space inference, i.e. LDS/STS instead of generic loads.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
 
-  const SmemLayout L = make_layout(kCtaGroup, kEpiGroups, p.num_stages, p.ksel, p.dim);
-  float* normbuf = reinterpret_cast<float*>(smem + L.off_norm);      // [4 warps][2][64]
-  uint32_t* maskbuf = reinterpret_cast<uint32_t*>(smem + L.off_mask);  // [4 warps][2][64]
-  volatile float* tau_s = reinterpret_cast<volatile float*>(smem + L.off_tau);   // [128]
+  const SmemLayout L = make_layout(kEpiGroups, p.num_stages, p.ksel, p.dim);
+  float* normbuf = reinterpret_cast<float*>(smem + L.off_norm);      // [2G warps][2][64]
+  uint32_t* maskbuf = reinterpret_cast<uint32_t*>(smem + L.off_mask);  // [2G warps][2][64]
+  float* scbuf = reinterpret_cast<float*>(smem + L.off_sc);          // [G][64 queries][kScStride]
+  volatile float* tau_s = reinterpret_cast<volatile float*>(smem + L.off_tau);   // [64]
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bar);
   uint64_t* full_bar = bars;                              // [kTcMaxStages]
   uint64_t* empty_bar = bars + kTcMaxStages;              // [kTcMaxStages]
-  uint64_t* tmem_full = bars + 2 * kTcMaxStages;          // [2]
-  uint64_t* tmem_empty = bars + 2 * kTcMaxStages + 2;     // [2]
-  uint64_t* q_ready = bars + 2 * kTcMaxStages + 4;        // [1]
-  uint64_t* q_staged = bars + 2 * kTcMaxStages + 5;       // [1] local: the query load no longer uses ring stages as scratch
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * kTcMaxStages + 6);
-  volatile int* epi_done = reinterpret_cast<volatile int*>(tmem_ptr_smem + 1);
+  uint64_t* acc_full = bars + 2 * kTcMaxStages;           // [2] score buffer g written
+  uint64_t* acc_empty = bars + 2 * kTcMaxStages + 2;      // [2] score buffer g read into registers
+  uint64_t* q_ready = bars + 2 * kTcMaxStages + 4;        // [1] the query block is in shared memory
+  volatile int* epi_done = reinterpret_cast<volatile int*>(bars + 2 * kTcMaxStages + 5);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -287,10 +285,10 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   // bumps it) so that a captured CUDA graph advances by itself when replayed
   const uint32_t epoch = p.epoch_ptr ? *p.epoch_ptr : p.epoch;
 
-  // Work split.  tset = which set of corpus tiles this CTA (pair) walks; qblock = which 128 queries.
-  // With more than 256 queries in a launch, S = n_qblocks / 2 CTA pairs ("query super-blocks") walk the SAME tile set
-  // side by side, each with its own 256 queries in TMEM: the first pair to ask for a tile pulls it from HBM, its
-  // siblings hit L2, so the corpus crosses the HBM interface once per 256 * S queries instead of once per 256.
+  // Work split.  tset = which set of corpus tiles this CTA (pair) walks; qblock = which 64 queries.
+  // With more than 128 queries in a launch, S = n_qblocks / 2 CTA pairs ("query super-blocks") walk the SAME tile set
+  // side by side, each with its own 128 queries: the first pair to ask for a tile pulls it from HBM, its
+  // siblings hit L2, so the corpus crosses the HBM interface once per 128 * S queries instead of once per 128.
   int qblock, tset, n_tsets;
   if constexpr (kCtaGroup == 2) {
     const int n_super = p.n_qblocks >> 1, pair = blockIdx.x >> 1;
@@ -313,32 +311,24 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   // (only CTAs that own at least one tile ever publish)
   const bool xchg = (p.pub != nullptr) && xm <= 4 && (xR <= min(nuse, p.n_tiles));
 
-  if constexpr (kCtaGroup == 2) cluster_sync_all();  // both CTAs resident before the paired TMEM alloc
-
-  if (warp == kMmaWarp && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&tmap);
     for (int i = 0; i < p.num_stages; ++i) {
-      mbar_init(&full_bar[i], kCtaGroup);  // leader's expect_tx arrive (+ the peer producer's arrive)
-      mbar_init(&empty_bar[i], 1);         // one tcgen05.commit
+      mbar_init(&full_bar[i], 1);          // this CTA's expect_tx arrive (the bytes may come from both CTAs)
+      mbar_init(&empty_bar[i], kCtaGroup); // the MMA warpgroup of every CTA the stage is multicast to
     }
     for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);                       // one tcgen05.commit
-      mbar_init(&tmem_empty[i], 4 * kCtaGroup);          // the four warps (per CTA) that drain this buffer
+      mbar_init(&acc_full[i], 128);        // every thread of the MMA warpgroup stores its part
+      mbar_init(&acc_empty[i], 2);         // the two warps of the epilogue group that reads this buffer
     }
-    mbar_init(q_ready, kEpiWarps * kCtaGroup);
-    mbar_init(q_staged, kEpiWarps);
+    mbar_init(q_ready, kEpiWarps);
     *epi_done = 0;
     fence_mbar_init();
-  } else if (warp == kProducerWarp) {
-    tmem_alloc<kCtaGroup>(tmem_ptr_smem, 512);
-    tmem_relinquish<kCtaGroup>();
   } else if (warp < kThrWarps) {
     for (int i = lane; i < kTcQRows; i += 32) tau_s[i] = -INFINITY;
   }
-  tc_fence_before();
+  // both CTAs' barriers initialised before any multicast or remote arrive
   if constexpr (kCtaGroup == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   grid_dep_launch();   // the exact re-rank kernel behind this one may start its prologue as CTAs here retire
 
   if (warp == kProducerWarp) {
@@ -347,7 +337,6 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       // read once -> evict first; shared with sibling CTAs (two single CTAs or several query super-blocks) -> keep in L2
       const uint64_t hint = ((kCtaGroup == 2 && p.n_qblocks == 2) || p.n_qblocks == 1) ? kEvictFirst : kEvictNormal;
       int stage = 0; uint32_t phase = 0;
-      bool q_done = p.num_stages < 2 * kQStageBufs;   // too few stages: the query load does not borrow any
       long long tp_wait = 0;
       const long long tp_begin = TCLK();
 #ifdef AUR_TC_PROFILE
@@ -356,25 +345,18 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       for (int it = 0; it < my_tiles; ++it) {
         const int tile = tset + it * n_tsets;
         const int row0 = tile * kTcTileN + static_cast<int>(rank) * (kTcTileN / kCtaGroup);
-        for (int kb0 = 0; kb0 < kbs; kb0 += kTcKbPerStage) {
-          const int nkb = min(kTcKbPerStage, kbs - kb0);
-          if (!q_done && stage >= p.num_stages - kQStageBufs) { mbar_wait(q_staged, 0); q_done = true; }   // (see the query load)
+        for (int kb = 0; kb < kbs; ++kb) {
           {
             const long long t0 = TCLK();
             mbar_wait(&empty_bar[stage], phase ^ 1u);
             tp_wait += TCLK() - t0;
           }
-          uint8_t* dst = smem + static_cast<uint32_t>(stage) * L.stage_bytes;
-          if constexpr (kCtaGroup == 1) {
-            mbar_arrive_expect_tx(&full_bar[stage], static_cast<uint32_t>(nkb) * L.box_bytes);
-            for (int j = 0; j < nkb; ++j)
-              tma_load_2d(dst + j * L.box_bytes, &tmap, &full_bar[stage], (kb0 + j) * kTcKBlock, row0, hint);
-          } else {
-            for (int j = 0; j < nkb; ++j)
-              tma_load_2d_pair(dst + j * L.box_bytes, &tmap, &full_bar[stage], (kb0 + j) * kTcKBlock, row0, hint);
-            if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2u * static_cast<uint32_t>(nkb) * L.box_bytes);
-            else mbar_arrive_cluster(&full_bar[stage], 0);
-          }
+          uint8_t* dst = smem + static_cast<uint32_t>(stage) * kStageBytes;
+          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);   // the whole tile lands here, half of it from the peer
+          if constexpr (kCtaGroup == 1)
+            tma_load_2d(dst, &tmap, &full_bar[stage], kb * kTcKBlock, row0, hint);
+          else
+            tma_load_2d_mc(dst + rank * (kStageBytes / 2), &tmap, &full_bar[stage], kb * kTcKBlock, row0, 0x3, hint);
           if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
         }
       }
@@ -387,79 +369,71 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       }
 #endif
     }
-  } else if (warp == kMmaWarp) {
-    // ============================== MMA issuer ==============================
-    // The whole warp walks the pipeline (so every operand stays warp-uniform and lives in
-    // uniform registers); one elected lane issues the MMAs and their commits.
-    if (rank == 0) {
-      mbar_wait(q_ready, 0);  // queries of (both) CTAs are in TMEM
-      tc_fence_after();
-      constexpr uint32_t idesc = idesc_bf16_f32(128 * kCtaGroup, kTcTileN);
-      constexpr uint32_t kBox16 = ((kTcTileN / kCtaGroup) * 128u) >> 4;  // box stride in descriptor units
-      int stage = 0; uint32_t phase = 0;
-      long long tm_empty = 0, tm_full = 0;
-      const long long tm_begin = TCLK();
-      for (int it = 0; it < my_tiles; ++it) {
-        const int b = it & 1;
+  } else if (warp >= kMmaWarp0) {
+    // ============================== MMA warpgroup ==============================
+    // wgmma accumulator layout (m64n64): thread t = 32 w + l holds rows 16 w + l / 4 (+ 8) and columns
+    // 8 j + 2 (l % 4) (+ 1), j = 0..7 -- stored into the score buffer as [query][corpus row].
+    const int wt = threadIdx.x - kMmaWarp0 * 32;
+    const int w4 = wt >> 5, l4 = wt & 31;
+    mbar_wait(q_ready, 0);   // the query block is in shared memory (and visible to the async proxy)
+    const uint32_t qs_a = smem_u32(smem + L.off_qs);
+    const uint32_t ring_a = smem_u32(smem);
+    int stage = 0; uint32_t phase = 0;
+    long long tm_empty = 0, tm_full = 0;
+    const long long tm_begin = TCLK();
+    for (int it = 0; it < my_tiles; ++it) {
+      const int b = (kEpiGroups == 2) ? (it & 1) : 0;
+      float d[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) d[i] = 0.f;
+      for (int kb = 0; kb < kbs; ++kb) {
         {
           const long long t0 = TCLK();
-          mbar_wait(&tmem_empty[b], ((static_cast<uint32_t>(it) >> 1) & 1u) ^ 1u);
-          tm_empty += TCLK() - t0;
+          mbar_wait(&full_bar[stage], phase);
+          tm_full += TCLK() - t0;
         }
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + kTcAccCol0 + b * kTcTileN;
-        for (int kb0 = 0; kb0 < kbs; kb0 += kTcKbPerStage) {
-          const int nkb = min(kTcKbPerStage, kbs - kb0);
-          {
-            const long long t0 = TCLK();
-            mbar_wait(&full_bar[stage], phase);
-            tm_full += TCLK() - t0;
-          }
-          tc_fence_after();
-          const uint32_t base_lo = (smem_u32(smem + static_cast<uint32_t>(stage) * L.stage_bytes) & 0x3FFFFu) >> 4;
-          const uint32_t a_col = tmem_base + static_cast<uint32_t>(kb0) * 32u;
-          if (elect_one()) {
+        if (!(p.dbg_flags & 2)) {
+          wgmma_fence();
+          const uint64_t da = wgmma_desc_sw128(qs_a + static_cast<uint32_t>(kb) * kQTileBytes);
+          const uint64_t db = wgmma_desc_sw128(ring_a + static_cast<uint32_t>(stage) * kStageBytes);
 #pragma unroll
-            for (int j = 0; j < kTcKbPerStage; ++j) {
-              if (j < nkb && !(p.dbg_flags & 2)) {
-                const int kb = kb0 + j;
-                if (kb < kTcTmemDim / kTcKBlock) {
-#pragma unroll
-                  for (int k = 0; k < 4; ++k) {  // 4 x K=16 per 128-byte k-block, queries from TMEM
-                    const uint32_t acc = (j | k) != 0 ? 1u : (kb0 != 0 ? 1u : 0u);
-                    mma_ts_bf16<kCtaGroup>(d_tmem, a_col + j * 32 + k * 8, pack_u64(base_lo + j * kBox16 + k * 2, kDescHi),
-                                           idesc, acc);
-                  }
-                } else {                         // dims past 768: queries from shared memory (SS)
-                  const uint32_t qs_lo = ((smem_u32(smem + L.off_qs) & 0x3FFFFu) >> 4) +
-                                         static_cast<uint32_t>(kb - kTcTmemDim / kTcKBlock) * ((kTcQRows * 128u) >> 4);
-#pragma unroll
-                  for (int k = 0; k < 4; ++k)
-                    mma_ss_bf16<kCtaGroup>(d_tmem, pack_u64(qs_lo + k * 2, kDescHi), pack_u64(base_lo + j * kBox16 + k * 2, kDescHi),
-                                           idesc, 1u);
-                }
-              }
-            }
-            mma_commit<kCtaGroup>(&empty_bar[stage]);  // smem slot free once these MMAs retire
-            if (kb0 + kTcKbPerStage >= kbs) mma_commit<kCtaGroup>(&tmem_full[b]);  // accumulator complete
-          }
-          __syncwarp();
-          if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
+          for (int k = 0; k < 4; ++k) wgmma_m64n64_ss(d, da + 2 * k, db + 2 * k, 1u);   // 4 x K=16 per 128-byte k-block
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_fence_regs(d);
         }
+        if (wt == 0) {   // this CTA's tensor core is done with the stage; so may be the peer's producer
+          mbar_arrive(&empty_bar[stage]);
+          if constexpr (kCtaGroup == 2) mbar_arrive_cluster(&empty_bar[stage], rank ^ 1u);
+        }
+        if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
       }
-      if ((p.dbg_flags & 64) && p.dbg_scores != nullptr && lane == 0) {
-        float* d = p.dbg_scores + static_cast<size_t>(blockIdx.x) * kTcQRows * kTcTileN + 32;
-        d[0] = static_cast<float>(tm_empty); d[1] = static_cast<float>(tm_full);
-        d[2] = static_cast<float>(TCLK() - tm_begin);
+      {
+        const long long t0 = TCLK();
+        mbar_wait(&acc_empty[b], ((static_cast<uint32_t>(it / kEpiGroups)) & 1u) ^ 1u);
+        tm_empty += TCLK() - t0;
       }
+      float* sc = scbuf + b * (kScBytes / 4);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int row = 16 * w4 + (l4 >> 2), col = 8 * j + 2 * (l4 & 3);
+        *reinterpret_cast<float2*>(sc + row * kScStride + col) = make_float2(d[4 * j + 0], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(sc + (row + 8) * kScStride + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+      }
+      mbar_arrive(&acc_full[b]);
     }
-  } else {
-    // ================= threshold warp (0) and epilogue warps (1-4) =================
-    const int quarter = warp & 3;              // TMEM lane quarter this warp may touch
-    const int r = quarter * 32 + lane;         // TMEM lane == query row inside the CTA
+    if ((p.dbg_flags & 64) && p.dbg_scores != nullptr && wt == 0) {
+      float* dd = p.dbg_scores + static_cast<size_t>(blockIdx.x) * kTcQRows * kTcTileN + 32;
+      dd[0] = static_cast<float>(tm_empty); dd[1] = static_cast<float>(tm_full);
+      dd[2] = static_cast<float>(TCLK() - tm_begin);
+    }
+  } else if (warp < kProducerWarp) {
+    // ================= threshold warp (0) and epilogue warps (1-2G) =================
+    const int ew = warp - kThrWarps;           // epilogue warp 0 .. 2G-1 (the threshold warp: -1)
+    const int quarter = ew & 1;                // which 32 queries of the block this warp owns
+    const int r = (warp < kThrWarps) ? lane : quarter * 32 + lane;   // query row inside the CTA
     const int qglob = qblock * kTcQRows + r;   // query index inside this launch
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16);
-    // exchange table: [qblock][query][CTA] -> a query's row is contiguous (592 B for 74 CTAs);
+    // exchange table: [qblock][query][CTA] -> a query's row is contiguous;
     // behind it, one published threshold per query
     const int pub_stride = (n_tsets + 1) & ~1;
     unsigned long long* pub_base =
@@ -513,21 +487,12 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       }
     } else {
       // ============================== epilogue warps ==============================
-      const int grp = (warp - kThrWarps) >> 2;   // epilogue group: takes tiles grp, grp + groups, ...
+      const int grp = ew >> 1;   // epilogue group: takes tiles grp, grp + groups, ...
       const long long t_kernel0 = TCLK();
-      // ---- park this thread's query row in TMEM (bf16 pairs, K ascending along columns);
-      //      with two groups each loads every other k-block
+      // ---- the query block into shared memory: [64 queries x 128 B] K-major tiles with the 128-byte swizzle TMA
+      //      would produce (16-byte chunk c of row r at c ^ (r & 7)); with two groups each loads every other k-block.
+      //      A warp reads its 32 rows coalesced (lane l takes 16-byte piece l of 4 consecutive rows per instruction).
       {
-        // A thread needs ITS row (TMEM lane = query), but 32 lanes reading 32 different rows cost 32 L1 wavefronts per
-        // load instruction -- 14k cycles for the block.  So a warp reads its 32 rows coalesced (lane l takes 16-byte
-        // piece l of 4 consecutive rows per instruction), transposes through shared memory -- borrowed from the last
-        // ring stages, which the TMA producer leaves alone until q_staged completes -- and every lane reads its own
-        // row back.  Staging layout = the 128-byte-swizzled K-major tile TMA would produce, so dims past 768 (which
-        // stay in shared memory as the SS-MMA operand) are written straight to their final place.
-        const bool staged = p.num_stages >= 2 * kQStageBufs;
-        const int ew = warp - kThrWarps;                      // epilogue warp 0 .. 4G-1
-        constexpr int kBufs = (kEpiGroups == 1) ? 2 : 1;      // 4 KB transpose buffers per warp
-        uint8_t* stg = smem + static_cast<uint32_t>(p.num_stages - kQStageBufs) * L.stage_bytes + ew * (kBufs * 4096);
         const uint8_t* qbase = reinterpret_cast<const uint8_t*>(p.q);
         const size_t row_bytes = static_cast<size_t>(p.dim) * 2;
         const int wrow0 = qblock * kTcQRows + quarter * 32;   // first query of this warp
@@ -539,85 +504,46 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
             if (kb < kbs && wrow0 + row < p.nq) x[i] = ldg_nc_v4(qbase + static_cast<size_t>(wrow0 + row) * row_bytes + kb * 128 + c * 16);
           }
         };
-        auto scatter_kb = [&](uint8_t* tile, const uint4 (&x)[8]) {   // tile: this warp's [32 rows x 128 B], swizzled
+        // every CTA of a query block reads the same block at the same moment: start each at a different
+        // k-block (rotation by tile set) so they do not all queue on the same L2 lines
+        const int n_j = (kbs - grp + kEpiGroups - 1) / kEpiGroups;      // k-blocks this group loads
+        const int rot = n_j > 0 ? tset % n_j : 0;
+        auto kb_of = [&](int j) { return (j < n_j) ? grp + ((j + rot) % n_j) * kEpiGroups : kbs; };
+        // four k-blocks of loads (32 x 16 B per lane) are issued before the first is consumed
+        constexpr int kDepth = 4;
+        uint4 x[kDepth][8];
+        for (int j0 = 0; j0 < n_j; j0 += kDepth) {
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int id = i * 32 + lane, row = id >> 3, c = id & 7;
-            *reinterpret_cast<uint4*>(tile + row * 128 + ((c ^ (row & 7)) << 4)) = x[i];
-          }
-        };
-        if (staged) {
-          // every CTA pair reads the same 256 x dim block at the same moment: start each pair at a different
-          // k-block (rotation by tile set) so they do not all queue on the same L2 lines
-          const int n_j = (kbs - grp + kEpiGroups - 1) / kEpiGroups;      // k-blocks this group loads
-          const int rot = n_j > 0 ? tset % n_j : 0;
-          auto kb_of = [&](int j) { return (j < n_j) ? grp + ((j + rot) % n_j) * kEpiGroups : kbs; };
-          // four k-blocks of loads (32 x 16 B per lane) are issued before the first is consumed: the block is read
-          // in three L2 round trips instead of twelve
-          constexpr int kDepth = 4;
-          uint4 x[kDepth][8];
-          for (int j0 = 0; j0 < n_j; j0 += kDepth) {
+          for (int u = 0; u < kDepth; ++u) load_kb(kb_of(j0 + u), x[u]);
 #pragma unroll
-            for (int u = 0; u < kDepth; ++u) load_kb(kb_of(j0 + u), x[u]);
-#pragma unroll
-            for (int u = 0; u < kDepth; ++u) {
-              const int j = j0 + u;
-              if (j >= n_j) break;
-              const int kb = kb_of(j);
-              if (kb < kTcTmemDim / kTcKBlock) {
-                uint8_t* buf = stg + (j % kBufs) * 4096;
-                if (kBufs == 1) __syncwarp();
-                scatter_kb(buf, x[u]);
-                __syncwarp();
-                uint32_t v[2][16];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                  const uint4 t = *reinterpret_cast<const uint4*>(buf + lane * 128 + ((c ^ (lane & 7)) << 4));
-                  v[c >> 2][(c & 3) * 4 + 0] = t.x; v[c >> 2][(c & 3) * 4 + 1] = t.y;
-                  v[c >> 2][(c & 3) * 4 + 2] = t.z; v[c >> 2][(c & 3) * 4 + 3] = t.w;
-                }
-                tmem_st_x16(lane_addr + kb * 32, v[0]);
-                tmem_st_x16(lane_addr + kb * 32 + 16, v[1]);
-              } else {
-                scatter_kb(smem + L.off_qs + static_cast<uint32_t>(kb - kTcTmemDim / kTcKBlock) * (kTcQRows * 128u) + quarter * 32 * 128, x[u]);
-              }
-            }
-          }
-        } else {   // hardly any ring (large k at dim > 768): every thread fetches its own row
-          const uint4* src = reinterpret_cast<const uint4*>(p.q + static_cast<size_t>(qglob) * p.dim);
-          for (int kb = grp; kb < kbs; kb += kEpiGroups) {
-            uint32_t v[2][16];
+          for (int u = 0; u < kDepth; ++u) {
+            const int j = j0 + u;
+            if (j >= n_j) break;
+            uint8_t* tile = smem + L.off_qs + static_cast<uint32_t>(kb_of(j)) * kQTileBytes + quarter * 32 * 128;
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-              uint4 x = make_uint4(0, 0, 0, 0);
-              if (qglob < p.nq) x = ldg_nc_v4(src + kb * 8 + i);
-              v[i >> 2][(i & 3) * 4 + 0] = x.x; v[i >> 2][(i & 3) * 4 + 1] = x.y;
-              v[i >> 2][(i & 3) * 4 + 2] = x.z; v[i >> 2][(i & 3) * 4 + 3] = x.w;
-            }
-            if (kb < kTcTmemDim / kTcKBlock) {
-              tmem_st_x16(lane_addr + kb * 32, v[0]);
-              tmem_st_x16(lane_addr + kb * 32 + 16, v[1]);
-            } else {   // K-major tile with the 128-byte swizzle TMA would have produced: 16-byte chunk c of row r at c ^ (r & 7)
-              uint8_t* qrow = smem + L.off_qs + static_cast<uint32_t>(kb - kTcTmemDim / kTcKBlock) * (kTcQRows * 128u) + r * 128u;
-#pragma unroll
-              for (int c = 0; c < 8; ++c)
-                *reinterpret_cast<uint4*>(qrow + ((c ^ (r & 7)) << 4)) =
-                    make_uint4(v[c >> 2][(c & 3) * 4 + 0], v[c >> 2][(c & 3) * 4 + 1], v[c >> 2][(c & 3) * 4 + 2], v[c >> 2][(c & 3) * 4 + 3]);
+              const int id = i * 32 + lane, row = id >> 3, c = id & 7;
+              *reinterpret_cast<uint4*>(tile + row * 128 + ((c ^ (row & 7)) << 4)) = x[u][i];
             }
           }
         }
-        tmem_wait_st();
-        fence_proxy_async_smem();   // (shared-memory part of the queries -> visible to the tensor core; the borrowed
-                                    //  ring stages -> safe for TMA to overwrite)
-        tc_fence_before();
+        fence_proxy_async_smem();   // the generic-proxy stores -> visible to the tensor core
         __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(q_staged);
-          if constexpr (kCtaGroup == 2) mbar_arrive_cluster(q_ready, 0); else mbar_arrive(q_ready);
-        }
+        if (lane == 0) mbar_arrive(q_ready);
       }
-      float* mynorm = normbuf + (warp - kThrWarps) * 2 * kTcTileN;
-      uint32_t* mymask = maskbuf + (warp - kThrWarps) * 2 * kTcTileN;
+      const float* myrow = scbuf + grp * (kScBytes / 4) + r * kScStride;   // this query's row of the group's score buffer
+      auto load_scores = [&](uint32_t (&acc)[4][16]) {
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+#pragma unroll
+          for (int j4 = 0; j4 < 4; ++j4) {
+            const float4 v = *reinterpret_cast<const float4*>(myrow + c * 16 + j4 * 4);
+            acc[c][j4 * 4 + 0] = __float_as_uint(v.x); acc[c][j4 * 4 + 1] = __float_as_uint(v.y);
+            acc[c][j4 * 4 + 2] = __float_as_uint(v.z); acc[c][j4 * 4 + 3] = __float_as_uint(v.w);
+          }
+      };
+      float* mynorm = normbuf + ew * 2 * kTcTileN;
+      uint32_t* mymask = maskbuf + ew * 2 * kTcTileN;
       uint32_t mybit = 0u;                                       // this query's tenant-scope bit
       if constexpr (kMask) { if (qglob < p.nq) mybit = 1u << (p.q_scope[qglob] & 31); }
       const uint32_t list_a = smem_u32(smem + L.off_list) + (static_cast<uint32_t>(grp) * L.lcap * kTcQRows + r) * 8u;
@@ -664,15 +590,18 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       // through the list would be all waste.  Read the tile once just for its best score(s),
       // publish them, wait until enough CTAs have done the same (~5 us, once), and let the
       // main loop examine the tile against the first certified threshold.  The accumulator
-      // is not released here, so the MMA cannot overwrite it before the loop reads it again.
+      // buffer is not released here, so the MMA cannot overwrite it before the loop reads it again.
       if (xchg && grp < my_tiles) {
-        mbar_wait(&tmem_full[grp & 1], 0);
-        tc_fence_after();
+        mbar_wait(&acc_full[grp], 0);
 #pragma unroll 1
         for (int c = 0; c < 4; ++c) {
           uint32_t a16[16];
-          tmem_ld_x16(lane_addr + kTcAccCol0 + (grp & 1) * kTcTileN + c * 16, a16);
-          tmem_wait_ld();
+#pragma unroll
+          for (int j4 = 0; j4 < 4; ++j4) {
+            const float4 v = *reinterpret_cast<const float4*>(myrow + c * 16 + j4 * 4);
+            a16[j4 * 4 + 0] = __float_as_uint(v.x); a16[j4 * 4 + 1] = __float_as_uint(v.y);
+            a16[j4 * 4 + 2] = __float_as_uint(v.z); a16[j4 * 4 + 3] = __float_as_uint(v.w);
+          }
           float m = -INFINITY;
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
@@ -702,7 +631,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       for (int it = grp; it < my_tiles; it += kEpiGroups, ++li) {
         const int tile = tset + it * n_tsets;
         const int row0 = tile * kTcTileN;
-        const int b = it & 1;
+        const int b = grp;
         const float* nb = mynorm + (li & 1) * kTcTileN;
         const long long t_top0 = TCLK();
         const float thr_now = (xchg && !(p.dbg_flags & 16)) ? tau_s[r] : -INFINITY;   // shared-memory copy kept by the threshold warp
@@ -719,27 +648,19 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
 
         {
           const long long t0 = TCLK();
-          mbar_wait(&tmem_full[b], (static_cast<uint32_t>(it) >> 1) & 1u);
+          mbar_wait(&acc_full[b], (static_cast<uint32_t>(li)) & 1u);
           t_wait += TCLK() - t0;
         }
-        tc_fence_after();
         const long long t_ld0 = TCLK();
         uint32_t acc[4][16];
-        if (!(p.dbg_flags & 1)) {
-#pragma unroll
-          for (int c = 0; c < 4; ++c) tmem_ld_x16(lane_addr + kTcAccCol0 + b * kTcTileN + c * 16, acc[c]);
-          tmem_wait_ld();
-        }
-        tc_fence_before();
+        if (!(p.dbg_flags & 1)) load_scores(acc);
         __syncwarp();
-        if (lane == 0) {  // accumulator drained into registers: hand the buffer back to the MMA warp
-          if constexpr (kCtaGroup == 2) mbar_arrive_cluster(&tmem_empty[b], 0); else mbar_arrive(&tmem_empty[b]);
-        }
+        if (lane == 0) mbar_arrive(&acc_empty[b]);   // scores in registers: hand the buffer back to the MMA warpgroup
         t_ld += TCLK() - t_ld0;
         if (p.dbg_flags & (1 | 4)) continue;
         const long long t_fast0 = TCLK();
 
-        // Fast path: scale by 1/|c_j| in place (packed FMUL2) and keep one running max per 16
+        // Fast path: scale by 1/|c_j| in place and keep one running max per 16
         // scores.  (NaN norm = tombstone / out of range: fmaxf drops it, `>=` rejects it.)
         if constexpr (kMask) {   // rows this query's tenant scope may not see: NaN, like tombstones
           const uint32_t* mb = mymask + (li & 1) * kTcTileN;
@@ -760,11 +681,11 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
           float m = -INFINITY;
 #pragma unroll
           for (int j4 = 0; j4 < 4; ++j4) {
-            const ulonglong2 nv = *reinterpret_cast<const ulonglong2*>(nb + c * 16 + j4 * 4);
-            const uint64_t p0 = mul_f32x2(pack_u64(acc[c][j4 * 4 + 0], acc[c][j4 * 4 + 1]), nv.x);
-            const uint64_t p1 = mul_f32x2(pack_u64(acc[c][j4 * 4 + 2], acc[c][j4 * 4 + 3]), nv.y);
-            unpack_u64(p0, acc[c][j4 * 4 + 0], acc[c][j4 * 4 + 1]);
-            unpack_u64(p1, acc[c][j4 * 4 + 2], acc[c][j4 * 4 + 3]);
+            const float4 nv = *reinterpret_cast<const float4*>(nb + c * 16 + j4 * 4);
+            acc[c][j4 * 4 + 0] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 0]), nv.x));
+            acc[c][j4 * 4 + 1] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 1]), nv.y));
+            acc[c][j4 * 4 + 2] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 2]), nv.z));
+            acc[c][j4 * 4 + 3] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 3]), nv.w));
             m = fmaxf(fmaxf(m, fmaxf(__uint_as_float(acc[c][j4 * 4 + 0]), __uint_as_float(acc[c][j4 * 4 + 1]))),
                       fmaxf(__uint_as_float(acc[c][j4 * 4 + 2]), __uint_as_float(acc[c][j4 * 4 + 3])));
           }
@@ -882,10 +803,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
 
   // ============================== teardown ==============================
   __syncwarp();
-  tc_fence_before();
-  if constexpr (kCtaGroup == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  if (warp == kProducerWarp) tmem_dealloc<kCtaGroup>(tmem_base, 512);
+  // no CTA of a pair exits while its peer may still multicast into it or arrive on its barriers
+  if constexpr (kCtaGroup == 2) cluster_sync_all();
 }
 
 template <int kCtaGroup, int kEpiGroups, bool kMask>
@@ -898,13 +817,13 @@ cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm,
 
 }  // namespace
 
-size_t tc_smem_bytes(int cta_group, int epi_groups, int num_stages, int ksel, int dim) {
-  return make_layout(cta_group, epi_groups, num_stages, ksel, dim).total + 1024;  // + alignment slack
+size_t tc_smem_bytes(int epi_groups, int num_stages, int ksel, int dim) {
+  return make_layout(epi_groups, num_stages, ksel, dim).total + 1024;  // + alignment slack
 }
 
-int tc_pick_stages(int cta_group, int epi_groups, int ksel, int dim, size_t smem_limit) {
+int tc_pick_stages(int epi_groups, int ksel, int dim, size_t smem_limit) {
   for (int s = kTcMaxStages; s >= 2; --s)
-    if (tc_smem_bytes(cta_group, epi_groups, s, ksel, dim) <= smem_limit) return s;
+    if (tc_smem_bytes(epi_groups, s, ksel, dim) <= smem_limit) return s;
   return 0;
 }
 
@@ -912,7 +831,7 @@ cudaError_t tc_launch(int cta_group, int epi_groups, int grid, const void* tmap,
                       cudaStream_t s) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(32 * (4 * epi_groups + 3));
+  cfg.blockDim = dim3(32 * (tc_mma_warp0(epi_groups) + 4));
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
   cudaLaunchAttribute attr[1];

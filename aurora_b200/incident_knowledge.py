@@ -1,4 +1,4 @@
-"""Drop-in for ``server/routes/incident_feedback/weaviate_client.py`` ("Aurora Learn") on the B200 engine.
+"""Drop-in for ``server/routes/incident_feedback/weaviate_client.py`` ("Aurora Learn") on the H100 engine.
 
 Same four public functions, keyword arguments, return shapes and error conventions as the reference
 (file:line cited on each).  This is the consumer whose score IS the engine's cosine: the reference runs

@@ -1,4 +1,4 @@
-"""Drop-in for ``server/routes/knowledge_base/weaviate_client.py`` backed by the B200 engine.
+"""Drop-in for ``server/routes/knowledge_base/weaviate_client.py`` backed by the H100 engine.
 
 Same public names, keyword arguments, return shapes and error conventions as the
 reference module (file:line cited on every function), so its callers keep working

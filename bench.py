@@ -22,7 +22,7 @@ N > 1 (torchrun): the corpus is row-sharded over the ranks (strong scaling at cf
 every rank's peer-mapped buffer over NVLink and the merge kernel waits on delivery flags (no collective call);
 --exchange nccl: one NCCL all-gather of the packed (fp64 score, id) planes + device merge.
 
-Other arms (run by hand, results under profiles/): --config cfg4 (1024 q x 10M x 1024, top-100), cfg5 (12.5M x 768 rows
+Other arms (run by hand): --config cfg4 (1024 q x 10M x 1024, top-100), cfg5 (12.5M x 768 rows
 per GPU, batch-512 queries with a concurrent encoder-ingest stream), cfg3 (bge-base encoder ingest, chunks/s).
 
 --impl reference: the reference's CPU path for the same config, timed on the host cores (the Weaviate / t2v
@@ -67,7 +67,7 @@ def _peaks():
             p = json.load(f)
         return float(p["hbm_gbs"]), float(p["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, 989.0, "fallback (H100 SXM data sheet: HBM3 bandwidth, dense BF16 at 700 W)"
 
 
 class ClockSampler:
@@ -339,9 +339,12 @@ def run_search(args, name: str):
         _barrier(torch, dist, world)
         e0.record()
         for _ in range(args.steps):
-            step_timed()
+            last = step_timed()
         e1.record()
         _barrier(torch, dist, world)
+        if args.dump_outputs and rank == 0:     # what the last timed step handed its caller
+            d_ids, d_sc = (g_ids, g_sc) if use_graph else last
+            dump_outputs(args.dump_outputs, ids=d_ids.cpu().numpy().astype(np.float64), scores=d_sc.cpu().numpy().astype(np.float32))
         # keep the sampler running a little so short runs still get a few samples under load
         # (local search only: a time-bounded loop must not contain collectives or exchanges)
         t_end = time.time() + 1.0
@@ -425,14 +428,15 @@ def run_search(args, name: str):
         return
 
     hbm_peak, tf_peak, peak_src = _peaks()
-    # queries per kernel launch: 256 per CTA pair, up to four pairs side by side on the same tiles ("query super-blocks"),
+    # queries per kernel launch: 128 per CTA pair, up to four pairs side by side on the same tiles ("query super-blocks"),
     # fewer when ceil((k + 8) / tile sets) would exceed 4 (same rule as csrc/capi.cu search_enqueue)
+    pairs = torch.cuda.get_device_properties(dev).multi_processor_count // 2
     n_super = 4
-    while n_super > 1 and -(-(k + 8) // (74 // n_super)) > 4:
+    while n_super > 1 and -(-(k + 8) // (pairs // n_super)) > 4:
         n_super -= 1
-    nq_pass = min(nq, 256 * n_super)
+    nq_pass = min(nq, 128 * n_super)
     passes = -(-nq // nq_pass)
-    shard_bytes = n_local * dim * 2 + nq_pass * dim * 2 + nq_pass * k * 8            # per kernel launch (one 256-query pass)
+    shard_bytes = n_local * dim * 2 + nq_pass * dim * 2 + nq_pass * k * 8            # per kernel launch (one query pass)
     flops_pass = 2.0 * nq_pass * n_local * dim
     if name == "cfg2":
         achieved = shard_bytes / (kernel_ms * 1e-3) / 1e9
@@ -441,15 +445,7 @@ def run_search(args, name: str):
         achieved = flops_pass / (kernel_ms * 1e-3) / 1e12
         roof = {"bound": "tensor", "achieved": achieved, "peak": tf_peak, "unit": "TFLOP/s", "frac": achieved / tf_peak,
                 "hbm_gbs_per_launch": shard_bytes / (kernel_ms * 1e-3) / 1e9, "queries_per_launch": nq_pass}
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "dram_traffic.json")
-    if os.path.exists(tpath) and world == 1 and name == "cfg2":
-        try:
-            traffic = json.load(open(tpath))["dram_bytes_per_launch"]
-        except Exception:
-            traffic = None
-    roof.update({"traffic": traffic, "traffic_source": "profiles/dram_traffic.json (ncu --set full capture of this kernel at this shape)" if traffic else None,
-                 "kernel": "simtopk_tc_kernel", "kernel_ms": kernel_ms, "launches_per_step": passes,
+    roof.update({"kernel": "simtopk_tc_kernel", "kernel_ms": kernel_ms, "launches_per_step": passes,
                  "algorithmic_bytes": shard_bytes, "algorithmic_flops": flops_pass, "peak_source": peak_src})
     exch = None if world == 1 else (
         "fused: finalize kernel stores (fp64 score, id) rows into every rank's IPC-mapped buffer over NVLink; merge kernel waits on delivery flags"
@@ -460,7 +456,7 @@ def run_search(args, name: str):
         "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": {"workload": cfg["workload"], "nq": nq, "rows": n_total, "rows_per_gpu": n_local, "dim": dim, "k": k,
                    "parallelism": f"row-shard x{world}",
-                   "l2": f"shard ({n_local * dim * 2 / 1e6:.0f} MB) vs L2 (126 MB): " + ("larger, no flush needed" if n_local * dim * 2 > 2.5e8 else "NOT much larger than L2 at this N"),
+                   "l2": f"shard ({n_local * dim * 2 / 1e6:.0f} MB) vs L2 (50 MB): " + ("larger, no flush needed" if n_local * dim * 2 > 1e8 else "NOT much larger than L2 at this N"),
                    "kernel": kernel_name, "exchange": exch,
                    "launch": "one CUDA graph per step (search + exact re-rank + exchange/merge captured once)" if use_graph else "stream launches"},
         "e2e": {"value": e2e, "unit": "queries/s", "ms_per_step": e2e_ms,
@@ -477,7 +473,7 @@ def run_search(args, name: str):
         if name == "cfg2" and not args.no_encoder:
             ix.close()
             torch.cuda.empty_cache()
-            out["encoder"] = encoder_leg(local)
+            out["encoder"] = encoder_leg(local, args.dump_outputs)
     print(json.dumps(out), flush=True)
     if world > 1:
         dist.barrier()
@@ -838,11 +834,12 @@ def text_ingest_leg(torch, dist, world, rank, dev, enc, ix, cfg, n_seq, lens, nx
             "text_bytes_per_batch": int(sum(len(t) for t in texts))}
 
 
-def encoder_leg(device: int) -> dict:
+def encoder_leg(device: int, dump_dir: str | None = None) -> dict:
     """Second hot-path row (SURVEY.md 8 a6/a11, BASELINE.json configs[2] shape): bge-base-en
     dimensions, random-init bf16 weights, cfg3 chunk lengths ~N(384, 96) clipped to [16, 512].
     Device time of the forward (CUDA events inside the library), the same call end to end with
-    host token ids in / host vectors out, and transformers' BertModel on the host cores beside it."""
+    host token ids in / host vectors out, and transformers' BertModel on the host cores beside it.
+    dump_dir: the pooled vectors of the last timed forward go there as encoder_embeddings.npy."""
     from aurora_b200.encoder import Encoder, EncoderConfig
 
     cfg = EncoderConfig()
@@ -856,10 +853,12 @@ def encoder_leg(device: int) -> dict:
         dev_ms, e2e_ms = [], []
         for _ in range(10):
             t0 = time.perf_counter()
-            enc.encode_packed(tok, cu)
+            emb = enc.encode_packed(tok, cu)
             e2e_ms.append((time.perf_counter() - t0) * 1e3)
             dev_ms.append(enc.stats()["total_ms"])
         st = enc.stats()
+    if dump_dir:
+        dump_outputs(dump_dir, encoder_embeddings=np.asarray(emb, dtype=np.float32))
     ms, ems = float(np.median(dev_ms)), float(np.median(e2e_ms))
     flops = st["gemm_flops"] + st["attn_flops"]
     _, peak_tf, peak_src = _peaks()
@@ -899,6 +898,15 @@ def encoder_leg(device: int) -> dict:
     return out
 
 
+def dump_outputs(out_dir: str, **arrays) -> None:
+    """--dump-outputs: each array as out_dir/<name>.npy (float32 / float64), so two builds can be compared output for
+    output on the same seeded inputs."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        assert a.dtype in (np.float32, np.float64) and a.nbytes <= 64 << 20, (name, a.dtype, a.nbytes)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -912,7 +920,16 @@ def main():
     ap.add_argument("--no-graph", dest="graph", action="store_false", help="time plain stream launches instead")
     ap.add_argument("--no-encoder", action="store_true", help="skip the encoder leg of the N=1 cfg2 run")
     ap.add_argument("--no-parity", action="store_true", help="skip the in-run oracle check (timing experiments only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed paths computed in their last step to DIR: the search's top-k (ids.npy as float64, "
+                         "scores.npy as float32) and, when the N=1 cfg2 run times its encoder leg, the pooled vectors "
+                         "(encoder_embeddings.npy, float32). cfg2 / cfg4; inputs are seeded, so runs with the same arguments "
+                         "are comparable")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.impl != "ours" or args.config not in ("cfg2", "cfg4")):
+        ap.error("--dump-outputs covers the search configs (cfg2, cfg4) of --impl ours")
     if args.impl == "reference":
         run_reference(args)
     elif args.config in ("cfg2", "cfg4"):

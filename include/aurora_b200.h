@@ -1,5 +1,5 @@
 /*
- * aurora_b200.h -- C ABI of the B200-native retrieval engine behind Aurora's
+ * aurora_b200.h -- C ABI of the H100-native retrieval engine behind Aurora's
  * knowledge-base RAG path.
  *
  * The reference (Arvo-AI/aurora) has no FFI for this path: its boundary is the Python
@@ -55,10 +55,10 @@ typedef enum aur_dtype { AUR_BF16 = 0, AUR_F32 = 1 } aur_dtype;
 
 /* Which similarity kernel serves a search (aur_set_option "kernel"). */
 typedef enum aur_kernel {
-  AUR_KERNEL_AUTO = 0,   /* tcgen05 path when the shape allows it, else SIMT      */
+  AUR_KERNEL_AUTO = 0,   /* tensor-core path when the shape allows it, else SIMT      */
   AUR_KERNEL_SIMT = 1,   /* generic CUDA-core path (any dim / dtype / filter)     */
-  AUR_KERNEL_TC1 = 2,    /* tcgen05, one CTA per MMA  (cta_group::1)              */
-  AUR_KERNEL_TC2 = 3     /* tcgen05, CTA pairs        (cta_group::2)              */
+  AUR_KERNEL_TC1 = 2,    /* wgmma, single CTAs                                    */
+  AUR_KERNEL_TC2 = 3     /* wgmma, two-CTA clusters sharing tiles by TMA multicast */
 } aur_kernel;
 
 typedef struct aur_index aur_index; /* opaque: one corpus shard resident on one GPU */
@@ -251,7 +251,7 @@ typedef struct aur_encoder_stats {
   int64_t tokens, seqs;      /* of the last call                                          */
   int32_t launches;          /* kernels launched by the last call                         */
   float   total_ms;          /* device time of the last forward (embeddings .. pooling)   */
-  float   gemm_ms, attn_ms;  /* thereof: tcgen05 GEMMs, attention                          */
+  float   gemm_ms, attn_ms;  /* thereof: wgmma GEMMs, attention                          */
   double  gemm_flops;        /* 2*M*N*K summed over the GEMMs, M = real (unpadded) tokens  */
   double  attn_flops;        /* 4 * len^2 * hidden per sequence and layer                  */
 } aur_encoder_stats;
@@ -298,7 +298,7 @@ int aur_encode_text_append(aur_encoder* enc, aur_tokenizer* tok, aur_index* ix, 
                            const int32_t* org_codes, int32_t n_threads);
 
 /* Bring-up / test hooks (not part of the drop-in surface). */
-/* out[M,N] = epi(A[M,K] . W[N,K]^T + bias) through the encoder's tcgen05 GEMM; host buffers,
+/* out[M,N] = epi(A[M,K] . W[N,K]^T + bias) through the encoder's wgmma GEMM; host buffers,
  * bf16 bits; epi 0 = bias, 1 = bias + GELU, 2 = bias + resid[M,N]; cta_group 1 or 2 (CTAs per tile). */
 int aur_debug_gemm(int32_t device, const uint16_t* a, const uint16_t* w, const float* bias,
                    const uint16_t* resid, int32_t m, int32_t n, int32_t k, int32_t epi,
@@ -310,7 +310,7 @@ int aur_debug_attention(int32_t device, const uint16_t* qkv, const int32_t* cu_s
 /* Final hidden states [tokens, hidden] (bf16 bits) of the last aur_encode call. */
 int aur_debug_encoder_hidden(aur_encoder* enc, uint16_t* out, int64_t count);
 int aur_debug_tc_scores(aur_index* ix, const void* queries_dev, int32_t nq,
-                        int32_t cta_group, float* out_dev /* [n_ctas,128,64] */,
+                        int32_t cta_group, float* out_dev /* [n_ctas,64,64] */,
                         int32_t* n_ctas_out, void* stream);
 
 #ifdef __cplusplus

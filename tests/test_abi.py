@@ -18,7 +18,7 @@ HEADER = os.path.join(ROOT, "include", "aurora_b200.h")
 def lib():
     from aurora_b200.build import build_native
 
-    build_native()          # nvcc cross-compiles for sm_100a without a GPU
+    build_native()          # nvcc cross-compiles for sm_90a without a GPU
     return N.load()
 
 

@@ -1,7 +1,7 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle on the same
 seeded inputs -- ids bit-exact, scores within 1e-3 (BASELINE.json north_star tolerance; in
 practice they agree to fp32 rounding because the final ranking is an fp64 re-score).
-Run on the B200 box:  python -m pytest tests -m gpu"""
+Run on an H100:  python -m pytest tests -m gpu"""
 
 import json
 import os
@@ -135,12 +135,12 @@ def test_uniform_tenant_scope_is_served_by_the_tcgen05_kernel(with_org):
         assert (none[0] == -1).all()
 
 
-# ------------------------------------------------------------------ tcgen05 path
+# ------------------------------------------------------------------ tensor-core path
 @pytest.mark.parametrize("kernel", [N.KERNEL_TC1, N.KERNEL_TC2])
 @pytest.mark.parametrize("n,d,nq,k", [
     (30000, 768, 256, 32), (9000, 384, 100, 10), (50001, 512, 200, 100), (20000, 768, 300, 5),
     (777, 64, 1, 1), (12345, 256, 129, 128), (64, 768, 256, 32), (5000, 768, 128, 64),
-    # dims past 768: the first 768 dims of the queries sit in TMEM, the rest in shared memory (SS MMAs)
+    # dims up to 1024: the whole query block stays in shared memory beside the TMA ring
     (20000, 1024, 256, 32), (9000, 1024, 300, 64), (7000, 896, 130, 10), (4000, 832, 64, 5),
 ])
 def test_tcgen05_parity(kernel, n, d, nq, k):
@@ -198,7 +198,7 @@ def test_one_strong_row_per_tile_large_k(kernel, tiles_per_pair):
 def test_large_k_at_dim_1024_falls_back_in_auto_mode():
     """dim 1024 with k = 128: the lists (k + slack per query) plus the shared-memory part of
     the queries leave no room for a TMA ring, so AUTO serves it with the generic kernel and an explicit
-    tcgen05 request is refused."""
+    tensor-core request is refused."""
     n, d, nq, k = 6000, 1024, 70, 128
     C, Q = _data(n, d, nq, seed=5)
     with Index(d, n) as ix:
@@ -344,7 +344,7 @@ def test_cosine_pairs_matches_reference_golden():
 
 # ------------------------------------------------------------------ BASELINE config 2 at full size: properties
 def test_cfg2_full_size_properties():
-    """1M x 768 bf16, 256 queries, top-32: planted neighbours are found, the tcgen05
+    """1M x 768 bf16, 256 queries, top-32: planted neighbours are found, the tensor-core
     variants agree with each other bit for bit, a repeated search is identical, and a
     subsample of queries matches the oracle."""
     n, d, nq, k, P = 1_000_000, 768, 256, 32, 8
@@ -493,7 +493,7 @@ def test_concurrent_ingest_and_search_threads():
 
 def test_search_subset_is_a_pre_filter():
     """aur_search_subset: a resolved metadata filter (ids) restricts the scan itself -- the allowed rows are found even
-    when thousands of better-scoring rows exist outside the list.  tcgen05 and generic kernels, with tombstones."""
+    when thousands of better-scoring rows exist outside the list.  tensor-core and generic kernels, with tombstones."""
     n, d, nq, k = 40000, 768, 5, 10
     C, Q = _data(n, d, nq, seed=21)
     rng = np.random.default_rng(3)

@@ -23,7 +23,11 @@ sys.path.insert(0, ROOT)
 
 from aurora_b200 import _native as N  # noqa: E402
 from aurora_b200.engine import DeviceBuffer, Index, to_bf16_bits  # noqa: E402
+
 from oracle import cosine_topk as O  # noqa: E402
+
+QROWS = N.TC_QUERY_ROWS
+MAX_CTAS = 1024      # debug-score buffers are sized for more CTAs than any GPU has SMs; the call returns the real count
 
 
 def _data(n, d, nq, seed=0, planted=True):
@@ -93,15 +97,17 @@ def stage_simt_filter_delete():
 
 
 def _tc_scores(cta_group):
-    n, d, nq = 148 * 64 + 37, 768, 256
+    # the debug entry takes one query block per CTA of a pair: 2 x QROWS queries; every CTA returns the first tile
+    # of its tile set, [QROWS queries x 64 rows]
+    n, d, nq = 200 * 64 + 37, 768, 2 * QROWS
     Cm, Qm = _data(n, d, nq, seed=11, planted=False)
     with Index(d, n) as ix:
         ix.add(Cm, np.arange(n, dtype=np.int64))
         dq = DeviceBuffer(nq * d * 2).upload(to_bf16_bits(Qm))
-        nctas = 148
-        dout = DeviceBuffer(nctas * 128 * 64 * 4).upload(np.full(nctas * 128 * 64, -7.0, dtype=np.float32))
+        cap = MAX_CTAS * QROWS * 64
+        dout = DeviceBuffer(cap * 4).upload(np.full(cap, -7.0, dtype=np.float32))
         got_ctas = ix.debug_tc_scores(dq.ptr, nq, cta_group, dout.ptr)
-        out = dout.download(np.empty((nctas, 128, 64), dtype=np.float32))
+        out = dout.download(np.empty((MAX_CTAS, QROWS, 64), dtype=np.float32))[:got_ctas]
     print(f"   kernel returned, n_ctas={got_ctas}")
     S = O.cosine_matrix(Qm, Cm) * np.linalg.norm(Qm.astype(np.float64), axis=1)[:, None]  # dot * inv|c|
     worst = 0.0
@@ -114,7 +120,7 @@ def _tc_scores(cta_group):
         row0 = lst * 64
         rows = np.arange(row0, row0 + 64)
         valid = rows < n
-        want = S[qblock * 128:(qblock + 1) * 128][:, rows[valid]]
+        want = S[qblock * QROWS:(qblock + 1) * QROWS][:, rows[valid]]
         got = out[cta][:, valid]
         err = np.abs(got - want)
         e = float(np.nanmax(err)) if err.size else 0.0
@@ -160,7 +166,7 @@ def stage_tc2_search():
 
 
 def stage_tc_big():
-    """1M x 768: tcgen05 paths against each other and the SIMT path (no CPU oracle at this size)."""
+    """1M x 768: tensor-core paths against each other and the SIMT path (no CPU oracle at this size)."""
     n, d, nq, k = 1_000_000, 768, 256, 32
     rng = np.random.default_rng(1002)
     bits = np.empty((n, d), dtype=np.uint16)

@@ -1,4 +1,4 @@
-"""GPU bring-up of the encoder kernels against numpy / the oracle (run on the B200 box).
+"""GPU bring-up of the encoder kernels against numpy / the oracle (run on an H100).
 
     python tools/bringup_encoder.py [--stage gemm|attn|tiny|bge|perf]
 """

@@ -109,7 +109,7 @@ def main():
             print(label, res[label], flush=True)
     res["speedup_vs_single_caller"] = res["64_callers_coalesced"]["requests_per_s"] / res["single_caller"]["requests_per_s"]
     res["note"] = ("every request = JSON over a Unix socket -> tokenise -> encoder forward (bge-base dims) -> tenant-scoped hybrid search "
-                   "(dense leg on the tcgen05 kernel + BM25 + ranked fusion) -> result dicts; Python daemon threads")
+                   "(dense leg on the tensor-core kernel + BM25 + ranked fusion) -> result dicts; Python daemon threads")
     os.makedirs(os.path.dirname(out) or ".", exist_ok=True)
     json.dump(res, open(out, "w"), indent=1)
     print(json.dumps(res))

@@ -1,5 +1,5 @@
 """Small end-to-end run for `compute-sanitizer --tool memcheck` (seconds under the tool):
-tcgen05 + generic search with partial query blocks, deletes, repeated launches; a tiny encoder forward
+tensor-core + generic search with partial query blocks, deletes, repeated launches; a tiny encoder forward
 with fused ingest.  Exits non-zero on a parity mismatch."""
 import os
 import sys

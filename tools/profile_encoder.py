@@ -1,4 +1,4 @@
-"""One bge-base forward over a synthetic cfg3 batch, for ncu / timing (run on the B200 box).
+"""One bge-base forward over a synthetic cfg3 batch, for ncu / timing (run on an H100).
 
     python tools/profile_encoder.py [n_seq] [reps]
 """
