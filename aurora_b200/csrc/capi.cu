@@ -281,6 +281,7 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   p.q = static_cast<const __nv_bfloat16*>(q_dev);
   p.inv_norm = inv_norm ? inv_norm : ix->d_inv_norm;
   p.row_mask = row_mask; p.q_scope = q_scope;
+  p.ids = ix->d_ids;
   p.cand = c->cand_a.p;
   p.cand_count = c->cand_count.p;
   p.dbg_scores = dbg;
@@ -384,7 +385,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
           const int64_t nr = (n_rows - r0 < chunk) ? n_rows - r0 : chunk;
           CU_TRY(launch_simt_scores(qb, ix->d_rows, ix->dtype, ix->dim, nqb, r0, nr, n_rows, inv ? inv : ix->d_inv_norm, f,
                                     c->score_chunk.p, s));
-          CU_TRY(launch_simt_select(c->score_chunk.p, nqb, r0, nr, ksel, c->cand_a.p, n_lists,
+          CU_TRY(launch_simt_select(c->score_chunk.p, nqb, r0, nr, ksel, ix->d_ids, c->cand_a.p, n_lists,
                                     static_cast<int>(r0 / kSimtSeg), s));
           c->last_launches += 2;
         }
@@ -411,7 +412,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
       DevBuf<uint64_t>& dst = in_a ? c->cand_b : c->cand_a;
       // rows of cand are indexed by the query position inside the block (TC pads to 128/256)
       CU_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
-      CU_TRY(launch_reduce_lists(cur, nqb, n_lists, ksel, group, dst.p, s));
+      CU_TRY(launch_reduce_lists(cur, nqb, n_lists, ksel, group, ix->d_ids, dst.p, s));
       c->last_launches += 1;
       cur = dst.p; n_lists = n_groups; in_a = !in_a;
     }

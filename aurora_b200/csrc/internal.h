@@ -33,6 +33,19 @@ __host__ __device__ __forceinline__ uint64_t make_key(float score, int32_t row) 
 }
 __host__ __device__ __forceinline__ int32_t key_row(uint64_t k) { return static_cast<int32_t>(~static_cast<uint32_t>(k)); }
 __host__ __device__ __forceinline__ float key_score(uint64_t k) { return ord_to_f32(static_cast<uint32_t>(k >> 32)); }
+#ifdef __CUDACC__
+// Candidate order wherever keys are compared, kept or evicted: (approximate score desc, id asc) -- the order of the
+// final ranking and of the cross-shard merge, so a group of tied rows cut anywhere keeps its lowest ids.  The key
+// carries the row (needed to fetch the vector); equal scores load ids[row], so only ties pay.  Keys without a row
+// (empty slots, sort padding) and equal ids fall back to the raw key: a strict total order on distinct keys.
+__device__ __forceinline__ bool key_before(uint64_t a, uint64_t b, const int64_t* __restrict__ ids) {
+  if ((a ^ b) >> 32) return a > b;
+  const int32_t ra = key_row(a), rb = key_row(b);
+  if ((ra | rb) < 0 || ra == rb) return a > b;
+  const int64_t ia = __ldg(ids + ra), ib = __ldg(ids + rb);
+  return ia != ib ? ia < ib : a > b;
+}
+#endif
 
 // ---------------------------------------------------------------- wgmma similarity kernel
 constexpr int kTcTileN = 64;       // corpus rows per tile  (MMA N)
@@ -52,7 +65,8 @@ struct TcParams {
   const float* inv_norm;    // [n_rows]   1/|c_j|, 0 for zero rows, NaN for tombstones
   const uint32_t* row_mask; // nullable [n_rows]: bit s = tenant scope s of this batch may see the row (per-query scopes)
   const int32_t* q_scope;   // with row_mask: [nq] scope index (0..31) of every query
-  uint64_t* cand;           // [64 * n_qblocks, n_lists * ksel] candidate keys, compacted per
+  const int64_t* ids;       // [n_rows] external ids: break ties between candidate keys (key_before)
+  uint64_t* cand;          // [64 * n_qblocks, n_lists * ksel] candidate keys, compacted per
                             // query: only keys that pass the final threshold are appended
   uint32_t* cand_count;     // [64 * n_qblocks] appended keys per query (zero on entry)
   float* dbg_scores;        // optional [grid, 64, 64]: first tile's scores of every CTA
@@ -94,10 +108,10 @@ cudaError_t launch_simt_scores(const void* q, const void* rows, int dtype, int d
                                int64_t nrows_chunk, int64_t n_rows, const float* inv_norm, FilterArgs f,
                                float* scores /* [nq, nrows_chunk] */, cudaStream_t s);
 cudaError_t launch_simt_select(const float* scores, int nq, int64_t row0, int64_t nrows_chunk, int ksel,
-                               uint64_t* cand, int n_lists, int list0, cudaStream_t s);
+                               const int64_t* ids, uint64_t* cand, int n_lists, int list0, cudaStream_t s);
 // [nq, n_lists, ksel] -> [nq, ceil(n_lists/group), ksel]; group*ksel <= 4096
-cudaError_t launch_reduce_lists(const uint64_t* in, int nq, int n_lists, int ksel, int group, uint64_t* out,
-                                cudaStream_t s);
+cudaError_t launch_reduce_lists(const uint64_t* in, int nq, int n_lists, int ksel, int group, const int64_t* ids,
+                                uint64_t* out, cudaStream_t s);
 // Final stage: best ksel of n_lists*ksel (<= 4096) keys, exact fp64 cosine re-rank,
 // (score desc, id asc) order, top-k out.
 struct FinalizeArgs {

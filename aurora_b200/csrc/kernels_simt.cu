@@ -120,8 +120,9 @@ __device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int m) {
   const uint32_t hi = __shfl_xor_sync(0xffffffffu, static_cast<uint32_t>(v >> 32), m);
   return (static_cast<uint64_t>(hi) << 32) | lo;
 }
+// Keys are ordered by key_before (score desc, id asc); ids = the rows' external ids.
 // Steps j = j_hi, j_hi / 2, ..., 1 of level k on every 64-key block (j_hi <= 32); with all_levels, levels 2 .. 64 in full.
-__device__ void bitonic_local64(uint64_t* s, int n, int k, bool all_levels) {
+__device__ void bitonic_local64(uint64_t* s, int n, int k, bool all_levels, const int64_t* ids) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   for (int base = warp * 64; base < n; base += nwarps * 64) {
     const int i0 = base + lane, i1 = i0 + 32;
@@ -129,13 +130,14 @@ __device__ void bitonic_local64(uint64_t* s, int n, int k, bool all_levels) {
     auto step = [&](int kk, int j) {
       if (j == 32) {
         const bool desc = (i0 & kk) == 0;
-        if ((e0 < e1) == desc) { const uint64_t t = e0; e0 = e1; e1 = t; }
+        if (desc ? key_before(e1, e0, ids) : key_before(e0, e1, ids)) { const uint64_t t = e0; e0 = e1; e1 = t; }
       } else {
         const uint64_t o0 = shfl_xor_u64(e0, j), o1 = shfl_xor_u64(e1, j);
         const bool lower = (lane & j) == 0;
         const bool want_max0 = ((i0 & kk) == 0) == lower, want_max1 = ((i1 & kk) == 0) == lower;
-        e0 = want_max0 ? (e0 > o0 ? e0 : o0) : (e0 < o0 ? e0 : o0);
-        e1 = want_max1 ? (e1 > o1 ? e1 : o1) : (e1 < o1 ? e1 : o1);
+        const bool b0 = key_before(e0, o0, ids), b1 = key_before(e1, o1, ids);
+        e0 = want_max0 == b0 ? e0 : o0;
+        e1 = want_max1 == b1 ? e1 : o1;
       }
     };
     if (all_levels) {
@@ -148,8 +150,8 @@ __device__ void bitonic_local64(uint64_t* s, int n, int k, bool all_levels) {
   }
   __syncthreads();
 }
-__device__ void bitonic_desc(uint64_t* s, int n) {
-  bitonic_local64(s, n, 0, true);
+__device__ void bitonic_desc(uint64_t* s, int n, const int64_t* ids) {
+  bitonic_local64(s, n, 0, true, ids);
   for (int k = 128; k <= n; k <<= 1) {
     for (int j = k >> 1; j >= 64; j >>= 1) {
       for (int i = threadIdx.x; i < n; i += blockDim.x) {
@@ -157,19 +159,19 @@ __device__ void bitonic_desc(uint64_t* s, int n) {
         if (l > i) {
           const uint64_t a = s[i], b = s[l];
           const bool desc = (i & k) == 0;
-          if ((a < b) == desc) { s[i] = b; s[l] = a; }
+          if (desc ? key_before(b, a, ids) : key_before(a, b, ids)) { s[i] = b; s[l] = a; }
         }
       }
       __syncthreads();
     }
-    bitonic_local64(s, n, k, false);
+    bitonic_local64(s, n, k, false, ids);
   }
 }
 
 // One block per (segment of kSimtSeg scores, query): keep the best ksel as keys.
 __global__ void __launch_bounds__(256)
 simt_select_kernel(const float* __restrict__ scores, int64_t row0, int64_t nrows_chunk, int ksel,
-                   uint64_t* __restrict__ cand, int n_lists, int list0) {
+                   const int64_t* __restrict__ ids, uint64_t* __restrict__ cand, int n_lists, int list0) {
   __shared__ uint64_t keys[kSimtSeg];
   const int seg = blockIdx.x, qi = blockIdx.y;
   const int64_t base = static_cast<int64_t>(seg) * kSimtSeg;
@@ -183,7 +185,7 @@ simt_select_kernel(const float* __restrict__ scores, int64_t row0, int64_t nrows
     keys[i] = key;
   }
   __syncthreads();
-  bitonic_desc(keys, kSimtSeg);
+  bitonic_desc(keys, kSimtSeg, ids);
   uint64_t* out = cand + (static_cast<size_t>(qi) * n_lists + list0 + seg) * ksel;
   for (int t = threadIdx.x; t < ksel; t += blockDim.x) out[t] = keys[t] == 0 ? kKeyEmpty : keys[t];
 }
@@ -192,8 +194,8 @@ constexpr int kSortCap = 4096;
 
 // [nq, n_lists, ksel] -> [nq, n_groups, ksel]
 __global__ void __launch_bounds__(512)
-reduce_lists_kernel(const uint64_t* __restrict__ in, int n_lists, int ksel, int group, uint64_t* __restrict__ out,
-                    int n_groups) {
+reduce_lists_kernel(const uint64_t* __restrict__ in, int n_lists, int ksel, int group, const int64_t* __restrict__ ids,
+                    uint64_t* __restrict__ out, int n_groups) {
   extern __shared__ uint64_t skeys[];
   const int g = blockIdx.x, qi = blockIdx.y;
   const int l0 = g * group, l1 = min(n_lists, l0 + group);
@@ -202,7 +204,7 @@ reduce_lists_kernel(const uint64_t* __restrict__ in, int n_lists, int ksel, int 
   const uint64_t* src = in + (static_cast<size_t>(qi) * n_lists + l0) * ksel;
   for (int i = threadIdx.x; i < P; i += blockDim.x) skeys[i] = i < n ? src[i] : 0ull;
   __syncthreads();
-  bitonic_desc(skeys, P);
+  bitonic_desc(skeys, P, ids);
   uint64_t* dst = out + (static_cast<size_t>(qi) * n_groups + g) * ksel;
   for (int t = threadIdx.x; t < ksel; t += blockDim.x) dst[t] = (t < P && skeys[t] != 0) ? skeys[t] : kKeyEmpty;
 }
@@ -267,7 +269,7 @@ finalize_kernel(FinalizeArgs a) {
         for (int i = carried + threadIdx.x; i < P; i += blockDim.x) skeys[i] = (i < m) ? src[done + i - carried] : 0ull;
       }
       __syncthreads();
-      bitonic_desc(skeys, P);
+      bitonic_desc(skeys, P, a.ids);
       done += take;
       carried = min(a.ksel, m);
     } while (done < n);
@@ -564,19 +566,19 @@ cudaError_t launch_simt_scores(const void* q, const void* rows, int dtype, int d
   return cudaGetLastError();
 }
 
-cudaError_t launch_simt_select(const float* scores, int nq, int64_t row0, int64_t nrows_chunk, int ksel, uint64_t* cand,
-                               int n_lists, int list0, cudaStream_t s) {
+cudaError_t launch_simt_select(const float* scores, int nq, int64_t row0, int64_t nrows_chunk, int ksel, const int64_t* ids,
+                               uint64_t* cand, int n_lists, int list0, cudaStream_t s) {
   dim3 grid(static_cast<unsigned>((nrows_chunk + kSimtSeg - 1) / kSimtSeg), static_cast<unsigned>(nq));
-  simt_select_kernel<<<grid, 256, 0, s>>>(scores, row0, nrows_chunk, ksel, cand, n_lists, list0);
+  simt_select_kernel<<<grid, 256, 0, s>>>(scores, row0, nrows_chunk, ksel, ids, cand, n_lists, list0);
   return cudaGetLastError();
 }
 
-cudaError_t launch_reduce_lists(const uint64_t* in, int nq, int n_lists, int ksel, int group, uint64_t* out,
-                                cudaStream_t s) {
+cudaError_t launch_reduce_lists(const uint64_t* in, int nq, int n_lists, int ksel, int group, const int64_t* ids,
+                                uint64_t* out, cudaStream_t s) {
   const int n_groups = (n_lists + group - 1) / group;
   int P = 64; while (P < group * ksel) P <<= 1;
   dim3 grid(static_cast<unsigned>(n_groups), static_cast<unsigned>(nq));
-  reduce_lists_kernel<<<grid, 512, static_cast<size_t>(P) * 8, s>>>(in, n_lists, ksel, group, out, n_groups);
+  reduce_lists_kernel<<<grid, 512, static_cast<size_t>(P) * 8, s>>>(in, n_lists, ksel, group, ids, out, n_groups);
   return cudaGetLastError();
 }
 

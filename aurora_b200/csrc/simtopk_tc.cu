@@ -102,17 +102,18 @@ struct TopkState {
   int minpos, nfill;
 };
 
-__device__ __forceinline__ void scan_min(uint32_t list_a, int n, uint64_t& m, int& mp) {
+// The last key of a list in candidate order (key_before): the one to evict.
+__device__ __forceinline__ void scan_min(uint32_t list_a, int n, const int64_t* ids, uint64_t& m, int& mp) {
   m = lds_u64(list_a); mp = 0;
 #pragma unroll 8
   for (int t = 1; t < n; ++t) {
     const uint64_t v = lds_u64(list_a + t * kSlot);
-    if (v < m) { m = v; mp = t; }
+    if (key_before(m, v, ids)) { m = v; mp = t; }
   }
 }
 
 // Drop what the threshold has made useless, then cut down to ksel entries.
-__device__ __noinline__ TopkState compact_list(TopkState st, uint32_t list_a, int ksel) {
+__device__ __noinline__ TopkState compact_list(TopkState st, uint32_t list_a, int ksel, const int64_t* ids) {
   const uint32_t thr = f32_to_ord(st.tau);
   int w = 0;
   for (int t = 0; t < st.nfill; ++t) {
@@ -122,12 +123,12 @@ __device__ __noinline__ TopkState compact_list(TopkState st, uint32_t list_a, in
   st.nfill = w;
   while (st.nfill > ksel) {  // rare: this CTA owns more than ksel of the current global best
     uint64_t m; int mp;
-    scan_min(list_a, st.nfill, m, mp);
+    scan_min(list_a, st.nfill, ids, m, mp);
     --st.nfill;
     sts_u64(list_a + mp * kSlot, lds_u64(list_a + st.nfill * kSlot));
   }
   if (st.nfill == ksel) {
-    scan_min(list_a, ksel, st.min_key, st.minpos);
+    scan_min(list_a, ksel, ids, st.min_key, st.minpos);
     st.tau_local = key_score(st.min_key);
     st.tau = fmaxf(st.tau, st.tau_local);
   }
@@ -135,15 +136,16 @@ __device__ __noinline__ TopkState compact_list(TopkState st, uint32_t list_a, in
 }
 
 // Admit one score into a query's list.
-__device__ __forceinline__ TopkState push_one(TopkState st, float s, int row, uint32_t list_a, int ksel, int lcap) {
+__device__ __forceinline__ TopkState push_one(TopkState st, float s, int row, uint32_t list_a, int ksel, int lcap,
+                                              const int64_t* ids) {
   const uint64_t key = make_key(s, row);
-  if (st.nfill == lcap) st = compact_list(st, list_a, ksel);
+  if (st.nfill == lcap) st = compact_list(st, list_a, ksel, ids);
   if (st.nfill < lcap) {
     sts_u64(list_a + st.nfill * kSlot, key);
     ++st.nfill;
-  } else if (key > st.min_key) {  // lcap == ksel and the list is full of live candidates
+  } else if (key_before(key, st.min_key, ids)) {  // lcap == ksel and the list is full of live candidates
     sts_u64(list_a + st.minpos * kSlot, key);
-    scan_min(list_a, ksel, st.min_key, st.minpos);
+    scan_min(list_a, ksel, ids, st.min_key, st.minpos);
     st.tau_local = key_score(st.min_key);
     st.tau = fmaxf(st.tau, st.tau_local);
   }
@@ -154,11 +156,11 @@ __device__ __forceinline__ TopkState push_one(TopkState st, float s, int row, ui
 // line and small: at warp level some lane needs this about twice per tile, so it has to be
 // cheap and its code has to stay resident next to the hot loop.
 __device__ __noinline__ TopkState push_group4(TopkState st, float s0, float s1, float s2, float s3, int row,
-                                              uint32_t list_a, int ksel) {
-  if (s0 >= st.tau) st = push_one(st, s0, row + 0, list_a, ksel, ksel);   // `>=` also rejects NaN
-  if (s1 >= st.tau) st = push_one(st, s1, row + 1, list_a, ksel, ksel);
-  if (s2 >= st.tau) st = push_one(st, s2, row + 2, list_a, ksel, ksel);
-  if (s3 >= st.tau) st = push_one(st, s3, row + 3, list_a, ksel, ksel);
+                                              uint32_t list_a, int ksel, const int64_t* ids) {
+  if (s0 >= st.tau) st = push_one(st, s0, row + 0, list_a, ksel, ksel, ids);   // `>=` also rejects NaN
+  if (s1 >= st.tau) st = push_one(st, s1, row + 1, list_a, ksel, ksel, ids);
+  if (s2 >= st.tau) st = push_one(st, s2, row + 2, list_a, ksel, ksel, ids);
+  if (s3 >= st.tau) st = push_one(st, s3, row + 3, list_a, ksel, ksel, ids);
   return st;
 }
 
@@ -183,7 +185,7 @@ __device__ __forceinline__ float top4_get(const float (&t)[4], int m) {   // t[m
 // much tighter) and admits the survivors.  The cold code is entered a handful of times per kernel
 // instead of ~100x per warp, and fewer scores pass.
 __device__ __noinline__ TopkState drain_fifo(TopkState st, uint32_t fifo_a, uint32_t ftag_a, int fcnt, uint32_t list_a,
-                                             int ksel) {
+                                             int ksel, const int64_t* ids) {
 #pragma unroll 1
   for (int rec = 0; rec < fcnt; ++rec) {
     int row;
@@ -191,10 +193,10 @@ __device__ __noinline__ TopkState drain_fifo(TopkState st, uint32_t fifo_a, uint
     asm volatile("ld.shared.b32 %0, [%1];" : "=r"(row) : "r"(ftag_a + rec * (kTcQRows * 4u)));
     asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(s0), "=f"(s1), "=f"(s2), "=f"(s3)
                  : "r"(fifo_a + rec * (kTcQRows * 16u)));
-    if (s0 >= st.tau) st = push_one(st, s0, row + 0, list_a, ksel, ksel);   // `>=` also rejects NaN
-    if (s1 >= st.tau) st = push_one(st, s1, row + 1, list_a, ksel, ksel);
-    if (s2 >= st.tau) st = push_one(st, s2, row + 2, list_a, ksel, ksel);
-    if (s3 >= st.tau) st = push_one(st, s3, row + 3, list_a, ksel, ksel);
+    if (s0 >= st.tau) st = push_one(st, s0, row + 0, list_a, ksel, ksel, ids);   // `>=` also rejects NaN
+    if (s1 >= st.tau) st = push_one(st, s1, row + 1, list_a, ksel, ksel, ids);
+    if (s2 >= st.tau) st = push_one(st, s2, row + 2, list_a, ksel, ksel, ids);
+    if (s3 >= st.tau) st = push_one(st, s3, row + 3, list_a, ksel, ksel, ids);
   }
   return st;
 }
@@ -716,7 +718,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
             if (cmax[c] >= st.tau) {
               if (fcnt > static_cast<int>(L.fifo_recs) - 4) {   // no room for four more groups: make room (rare)
                 const long long t0 = TCLK();
-                st = drain_fifo(st, fifo_a, ftag_a, fcnt, list_a, ksel);
+                st = drain_fifo(st, fifo_a, ftag_a, fcnt, list_a, ksel, p.ids);
                 fcnt = 0;
                 ++nslow;
                 t_slow += TCLK() - t0;
@@ -745,7 +747,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
               const float s0 = __uint_as_float(acc[c][4 * g]), s1 = __uint_as_float(acc[c][4 * g + 1]);
               const float s2 = __uint_as_float(acc[c][4 * g + 2]), s3 = __uint_as_float(acc[c][4 * g + 3]);
               if (fmaxf(fmaxf(s0, s1), fmaxf(s2, s3)) >= st.tau)
-                st = push_group4(st, s0, s1, s2, s3, row0 + c * 16 + 4 * g, list_a, ksel);
+                st = push_group4(st, s0, s1, s2, s3, row0 + c * 16 + 4 * g, list_a, ksel, p.ids);
             }
             ++nslow;
             t_slow += TCLK() - t0;
@@ -771,13 +773,13 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       if (xchg && my_tiles > 0) tau_end = read_threshold(thr_q, epoch);
       st.tau = fmaxf(st.tau, tau_end);
       if (use_fifo) {   // whatever is still parked meets the final threshold
-        if (__any_sync(0xffffffffu, fcnt > 0)) st = drain_fifo(st, fifo_a, ftag_a, fcnt, list_a, ksel);
+        if (__any_sync(0xffffffffu, fcnt > 0)) st = drain_fifo(st, fifo_a, ftag_a, fcnt, list_a, ksel, p.ids);
         fcnt = 0;
       }
 
       // ---- append the survivors (score >= the certified threshold, at most ksel of them)
       //      to this query's compact candidate row
-      st = compact_list(st, list_a, ksel);
+      st = compact_list(st, list_a, ksel, p.ids);
       {
         const size_t cap = static_cast<size_t>(n_tsets) * kEpiGroups * ksel;
         uint64_t* out = p.cand + static_cast<size_t>(qglob) * cap;

@@ -17,10 +17,12 @@ restated in ``oracle/ref_cosine.py``; this module is the same arithmetic vectori
 Tenant scope follows weaviate_client.py:244-249: a row is visible to a query iff
 ``row.user == q.user OR (q.org is set AND row.org == q.org)``.
 
-Exactness: candidates are selected with an fp64 BLAS product (k + slack kept) and
-then re-scored with extended precision (``np.longdouble``) accumulation, so the
-fp64 score of a row does not depend on its position in the matrix (bit-identical
-duplicate rows tie exactly and fall back to ``id asc``).
+Exactness: candidates are selected with an fp64 BLAS product (k + slack kept, widened
+to every row within ``TIE_MARGIN`` of the k-th when the kept set ends inside a tie
+group) and then re-scored with extended precision (``np.longdouble``) accumulation,
+so the fp64 score of a row does not depend on its position in the matrix
+(bit-identical duplicate rows tie exactly and fall back to ``id asc``, however many
+there are).
 
 Pinned by tests/test_oracle_golden.py: element-wise against golden vectors made by
 the real reference function, and cfg1's top-5 against the pure-Python flat scan.
@@ -96,6 +98,29 @@ def visible_mask(row_user, row_org, q_user: int, q_org: int) -> np.ndarray:
     return m
 
 
+# The fp64 selection keeps k + slack rows per query.  When its last kept score is within this margin of the k-th, a
+# group of (near-)tied rows may have been cut at an arbitrary point, so the candidates are widened to every row scoring
+# within the margin of the k-th before the exact re-rank orders them by id.  The margin only has to be far above the
+# error of an fp64 cosine (~1e-15), so that rows tied in exact arithmetic are never split by it.  A larger margin only
+# adds candidates, which the exact re-rank then orders: correctness does not depend on how many rows it pulls in.
+TIE_MARGIN = 1e-9
+
+
+def _chunk_scores(Q64, qn, C, lo, hi, qsel, live, row_user, row_org, q_user, q_org):
+    """fp64 cosine of the queries ``qsel`` against rows [lo, hi); invisible rows -inf."""
+    Cc = C[lo:hi].astype(np.float64)
+    denom = qn[qsel][:, None] * _norms64(Cc)[None, :]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        s = np.where(denom > 0, (Q64[qsel] @ Cc.T) / denom, 0.0)
+    if live is not None:
+        s[:, ~np.asarray(live[lo:hi], dtype=bool)] = -np.inf
+    if q_user is not None:
+        for j, i in enumerate(qsel):
+            qo = None if q_org is None else int(q_org[i])
+            s[j, ~visible_mask(row_user[lo:hi], row_org[lo:hi], int(q_user[i]), qo)] = -np.inf
+    return s
+
+
 def cosine_topk(Q, C, k: int, ids=None, live=None, row_user=None, row_org=None,
                 q_user=None, q_org=None, clamp: bool = False, slack: int = 16,
                 chunk: int = 131072):
@@ -121,20 +146,10 @@ def cosine_topk(Q, C, k: int, ids=None, live=None, row_user=None, row_org=None,
     keep = min(N, k + slack)
     cand_rows = np.zeros((nq, 0), dtype=np.int64)
     cand_sc = np.zeros((nq, 0), dtype=np.float64)
+    allq = np.arange(nq)
     for lo in range(0, N, chunk):
         hi = min(N, lo + chunk)
-        Cc = C[lo:hi].astype(np.float64)
-        cn = _norms64(Cc)
-        denom = qn[:, None] * cn[None, :]
-        with np.errstate(divide="ignore", invalid="ignore"):
-            s = np.where(denom > 0, (Q64 @ Cc.T) / denom, 0.0)
-        if live is not None:
-            s[:, ~np.asarray(live[lo:hi], dtype=bool)] = -np.inf
-        if q_user is not None:
-            for i in range(nq):
-                qo = None if q_org is None else int(q_org[i])
-                vm = visible_mask(row_user[lo:hi], row_org[lo:hi], int(q_user[i]), qo)
-                s[i, ~vm] = -np.inf
+        s = _chunk_scores(Q64, qn, C, lo, hi, allq, live, row_user, row_org, q_user, q_org)
         rows = np.broadcast_to(np.arange(lo, hi, dtype=np.int64), s.shape)
         cand_sc = np.concatenate([cand_sc, s], axis=1)
         cand_rows = np.concatenate([cand_rows, rows], axis=1)
@@ -143,11 +158,28 @@ def cosine_topk(Q, C, k: int, ids=None, live=None, row_user=None, row_org=None,
             cand_sc = np.take_along_axis(cand_sc, part, axis=1)
             cand_rows = np.take_along_axis(cand_rows, part, axis=1)
 
+    # queries whose kept set ends inside a tie group with the k-th: collect the whole group
+    fin = np.isfinite(cand_sc)
+    kth = -np.sort(-np.where(fin, cand_sc, -np.inf), axis=1)[:, min(k, keep) - 1]
+    smin = np.where(fin, cand_sc, np.inf).min(axis=1)
+    cut = np.nonzero((fin.sum(axis=1) == keep) & (keep < N) & (smin >= kth - TIE_MARGIN))[0]
+    extra = {}
+    for lo in range(0, N, chunk):
+        if cut.size == 0:
+            break
+        hi = min(N, lo + chunk)
+        s = _chunk_scores(Q64, qn, C, lo, hi, cut, live, row_user, row_org, q_user, q_org)
+        for j, i in enumerate(cut):
+            near = np.nonzero(s[j] >= kth[i] - TIE_MARGIN)[0] + lo
+            extra[i] = np.union1d(extra.get(i, near[:0]), near)
+
     for i in range(nq):
         valid = np.isfinite(cand_sc[i])
         rows = cand_rows[i][valid]
         if rows.size == 0:
             continue
+        if i in extra:
+            rows = np.union1d(rows, extra[i])
         ex = exact_cosine(Q[i], C[rows])
         if clamp:
             ex = np.clip(ex, 0.0, 1.0)

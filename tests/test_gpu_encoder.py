@@ -5,12 +5,11 @@ the HF-BertModel golden vectors, and the fused encode -> append -> search ingest
 Tolerance (floating point, stated here as the tier asks): the GPU keeps activations in bf16
 between kernels (fp32 accumulation inside them) while the oracle runs fp64 on the same
 bf16-rounded weights.  A pooled, L2-normalised vector must have cosine >= 0.9995 with the oracle's
-and every component within 1e-2; single kernels must be within one bf16 ulp of the output range
-(2^-8 relative) plus 1e-3."""
+and every component within 1e-2; single kernels must keep every output element within its own error bound, derived
+from the arithmetic the kernel does (tests/bounds.py)."""
 
 import ctypes as C
 import json
-import math
 import os
 
 import numpy as np
@@ -22,7 +21,9 @@ from aurora_b200 import _native as N
 from aurora_b200.encoder import EmbeddingClient, Encoder, EncoderConfig
 from aurora_b200.engine import Index, to_bf16_bits
 from oracle import bert_encoder as B
-from oracle.cosine_topk import bf16_bits_to_f32, round_to_bf16
+from oracle.cosine_topk import bf16_bits_to_f32
+from tests import bounds as BD
+from tests.test_oracle_bert import constant_row_weights
 
 # Floating-point tolerance of the encoder path (bf16 activations between kernels, fp32 accumulation) against the fp64
 # oracle on the same bf16-rounded weights: pooled unit vectors must agree to cosine >= 0.9999 and 4e-3 per component
@@ -43,54 +44,65 @@ def _mirror(cfg_o: B.BertConfig) -> EncoderConfig:
 SMALL = B.BertConfig(hidden=128, layers=2, heads=2, inter=256, vocab=120, max_pos=512, pool="cls")
 
 
+GEMM_SHAPES = [(128, 256, 64, 0), (130, 128, 192, 0), (1000, 768, 768, 2), (777, 3072, 768, 1), (640, 768, 3072, 2),
+               (500, 384, 384, 1), (1, 256, 64, 0),
+               # the pair-tile boundary (256 rows), single-CTA tile boundary (128), bge-large wo2 (K 4096), N = 384 (BN 128,
+               # three tiles) and 2304 (qkv of bge-base)
+               (255, 768, 768, 0), (256, 768, 768, 2), (257, 768, 768, 1), (127, 384, 256, 0), (129, 384, 256, 2),
+               (257, 1024, 4096, 2), (300, 2304, 768, 0)]
+
+
 @pytest.mark.parametrize("cta_group", [1, 2])
-@pytest.mark.parametrize("m,n,k,epi", [(128, 256, 64, 0), (130, 128, 192, 0), (1000, 768, 768, 2), (777, 3072, 768, 1),
-                                       (640, 768, 3072, 2), (500, 384, 384, 1), (1, 256, 64, 0)])
+@pytest.mark.parametrize("m,n,k,epi", GEMM_SHAPES)
 def test_gemm_matches_numpy(m, n, k, epi, cta_group):
+    _gemm_case(m, n, k, epi, cta_group)
+
+
+@pytest.mark.parametrize("cta_group", [1, 2])
+@pytest.mark.parametrize("case", ["gelu_spread", "resid_large"])
+def test_gemm_epilogue_edges(case, cta_group):
+    """GELU inputs over [-6, 6] (both tails of the erf approximation) and a residual 2^10 times the product (catches
+    a residual added after the bf16 rounding of the product)."""
+    if case == "gelu_spread":
+        _gemm_case(257, 384, 64, 1, cta_group, spread=True)
+    else:
+        _gemm_case(129, 768, 192, 2, cta_group, big_resid=True)
+
+
+def _gemm_case(m, n, k, epi, cta_group, spread=False, big_resid=False):
     lib = N.load()
-    rng = np.random.default_rng(m * 7 + n + k + epi)
-    a = round_to_bf16(rng.standard_normal((m, k)).astype(np.float32))
-    w = round_to_bf16((rng.standard_normal((n, k)) / math.sqrt(k)).astype(np.float32))
-    bias = rng.standard_normal(n).astype(np.float32)
-    resid = round_to_bf16(rng.standard_normal((m, n)).astype(np.float32))
+    a, w, bias, resid = BD.gemm_inputs(m, n, k, seed=m * 7 + n + k + epi, spread=spread, big_resid=big_resid)
     out = np.zeros((m, n), dtype=np.uint16)
     N.check(lib.aur_debug_gemm(0, _ptr(to_bf16_bits(a)), _ptr(to_bf16_bits(w)), _ptr(bias), _ptr(to_bf16_bits(resid)),
                                m, n, k, epi, cta_group, _ptr(out), None))
-    ref = a.astype(np.float64) @ w.astype(np.float64).T + bias
-    if epi == 1:
-        ref = B.gelu(ref)
-    if epi == 2:
-        ref = ref + resid
-    got = bf16_bits_to_f32(out).astype(np.float64)
-    assert np.abs(got - ref).max() <= np.abs(ref).max() * 2 ** -8 + 1e-3
+    ref, bound = BD.gemm_reference(a, w, bias, resid, epi)
+    BD.assert_within(f"gemm m={m} n={n} k={k} epi={epi} cta_group={cta_group}", bf16_bits_to_f32(out), ref, bound)
 
 
-def _attn_ref(qkv, cu, heads, hidden):
-    out = np.zeros((qkv.shape[0], hidden))
-    for s in range(len(cu) - 1):
-        x = qkv[cu[s]:cu[s + 1]].astype(np.float64)
-        for h in range(heads):
-            q, k, v = (x[:, i * hidden + h * 64: i * hidden + (h + 1) * 64] for i in range(3))
-            a = q @ k.T / 8.0
-            a = np.exp(a - a.max(axis=1, keepdims=True))
-            out[cu[s]:cu[s + 1], h * 64:(h + 1) * 64] = (a / a.sum(axis=1, keepdims=True)) @ v
-    return out
+def _attention(heads, lens, kind="random", seed=None):
+    lib = N.load()
+    hidden = heads * 64
+    qkv, cu = BD.attention_inputs(heads, lens, seed=sum(lens) + heads if seed is None else seed, kind=kind)
+    out = np.zeros((int(cu[-1]), hidden), dtype=np.uint16)
+    N.check(lib.aur_debug_attention(0, _ptr(to_bf16_bits(qkv)), _ptr(cu), len(lens), heads, hidden, _ptr(out), None))
+    ref, bound = BD.attention_reference(qkv, cu, heads, hidden)
+    BD.assert_within(f"attention heads={heads} kind={kind} lens={list(lens)[:8]}", bf16_bits_to_f32(out), ref, bound)
 
 
 @pytest.mark.parametrize("heads,lens", [(2, [1]), (2, [5]), (2, [128]), (2, [129, 1, 64]), (12, [300, 17, 512, 384, 200]),
-                                        (4, [512, 512, 511]), (1, [127, 256, 257])])
+                                        (4, [512, 512, 511]), (1, [127, 256, 257]),
+                                        # every key-block count and query-block boundary
+                                        (2, [1, 2, 127, 128, 129, 255, 256, 257, 383, 384, 385, 511, 512])])
 def test_attention_matches_numpy(heads, lens):
-    lib = N.load()
-    hidden = heads * 64
-    rng = np.random.default_rng(sum(lens) + heads)
-    cu = np.zeros(len(lens) + 1, dtype=np.int32)
-    cu[1:] = np.cumsum(lens)
-    qkv = round_to_bf16((rng.standard_normal((int(cu[-1]), 3 * hidden)) * 1.5).astype(np.float32))
-    out = np.zeros((int(cu[-1]), hidden), dtype=np.uint16)
-    N.check(lib.aur_debug_attention(0, _ptr(to_bf16_bits(qkv)), _ptr(cu), len(lens), heads, hidden, _ptr(out), None))
-    got = bf16_bits_to_f32(out).astype(np.float64)
-    ref = _attn_ref(qkv, cu, heads, hidden)
-    assert np.abs(got - ref).max() <= np.abs(ref).max() * 2 ** -7 + 1e-3   # P is rounded to bf16 before P.V
+    _attention(heads, lens)
+
+
+@pytest.mark.parametrize("kind,lens", [("onehot", [129, 385, 512]), ("lastmax", [1, 2, 128, 129, 257, 511]),
+                                       ("leak", [129, 300, 128, 40, 512, 257])])
+def test_attention_edges(kind, lens):
+    """Nearly one-hot rows (exp underflows), every query's largest logit on the last valid key (a key dropped by the
+    mask shows), and neighbours in the packed batch whose keys are 8x larger (a key leaking across the mask shows)."""
+    _attention(4, lens, kind)
 
 
 def test_attention_large_batch():
@@ -106,12 +118,94 @@ def test_attention_large_batch():
     qkv_bits = to_bf16_bits((rng.standard_normal((T, 3 * hidden), dtype=np.float32) * 1.5))
     out = np.zeros((T, hidden), dtype=np.uint16)
     N.check(lib.aur_debug_attention(0, _ptr(qkv_bits), _ptr(cu), n_seq, heads, hidden, _ptr(out), None))
+    worst = 0.0
     for s in list(range(0, 6)) + list(range(990, 1000)) + list(range(n_seq - 6, n_seq)):
         a, b = int(cu[s]), int(cu[s + 1])
-        qkv = bf16_bits_to_f32(qkv_bits[a:b])
-        ref = _attn_ref(qkv, np.array([0, b - a]), heads, hidden)
-        got = bf16_bits_to_f32(out[a:b]).astype(np.float64)
-        assert np.abs(got - ref).max() <= np.abs(ref).max() * 2 ** -7 + 1e-3, s
+        ref, bound = BD.attention_reference(bf16_bits_to_f32(qkv_bits[a:b]), np.array([0, b - a]), heads, hidden)
+        r = BD.ratio(bf16_bits_to_f32(out[a:b]), ref, bound)
+        assert r <= 1.0, (s, r)
+        worst = max(worst, r)
+    print(f"attention large batch: max(err / bound) = {worst:.4f}")
+
+
+# ------------------------------------------------------------------ per-token hidden states and pooling
+MINILM_SHAPE = B.BertConfig(hidden=384, layers=1, heads=12, inter=1536, vocab=120, max_pos=512, pool="mean")
+
+
+@pytest.mark.parametrize("layers", [1, 2])
+@pytest.mark.parametrize("shape", ["small", "minilm"])
+def test_hidden_states_match_the_bf16_store_oracle(shape, layers):
+    """Encoder.hidden_states() token by token against the oracle that rounds to bf16 exactly where the GPU stores bf16
+    (embedding LayerNorm, LayerNorm, attention with the zero-padded head dim 32 of the MiniLM shape included).
+
+    Every element is within 8 bf16 ulps of max(|ref|, RMS of its token's row) (measured on an H100: at most 5).  A LayerNorm output inherits the error
+    of its input's bf16 stores, whose ulps are set by the row's magnitude, not by the element's: one store that
+    rounds the other way (fp32 accumulation sits on the other side of a rounding boundary than fp64) moves small
+    elements of an O(1) row by many of their own ulps.  Counted in ulps of max(|ref|, 1/16) the head-dim-64 shape
+    stays within 2 ulps for 99.9 % of the elements and 8 for all; the MiniLM shape (H 384, I 1536) does not, and
+    the figures are printed."""
+    base = SMALL if shape == "small" else MINILM_SHAPE
+    cfg_o = B.BertConfig(**{**base.__dict__, "layers": layers})
+    w = B.init_weights(cfg_o, seed=7, bf16=True)
+    tok, cu = B.synth_batch(cfg_o, 7, 17 + layers, mean_len=150, std_len=140, min_len=1, max_len=400)
+    with Encoder(_mirror(cfg_o), max_tokens=4096, max_seqs=16) as enc:
+        enc.load_weights(w)
+        enc.encode_packed(tok, cu)
+        got = bf16_bits_to_f32(enc.hidden_states()).astype(np.float64)
+    ref = B.encode_tokens(cfg_o, w, tok, cu, bf16_stores=True)
+
+    def ulps(floor):
+        return np.abs(got - ref) / 2.0 ** (np.floor(np.log2(np.maximum(np.abs(ref), floor))) - 7)
+
+    e = ulps(1.0 / 16)
+    within2, worst = float((e <= 2).mean()), float(e.max())
+    e_row = ulps(np.sqrt((ref * ref).mean(axis=1, keepdims=True)))
+    print(f"hidden states {shape} layers={layers}: {100 * within2:.3f} % within 2 ulps of max(|ref|, 1/16), "
+          f"{100 * float((e == 0).mean()):.2f} % exact, max {worst:.1f} ulps; max {float(e_row.max()):.2f} ulps of "
+          f"max(|ref|, row RMS); {e.size} elements")
+    assert float(e_row.max()) <= 8
+    if shape == "small":
+        assert within2 >= 0.999 and worst <= 8
+
+
+@pytest.mark.parametrize("pool,normalize", [("cls", False), ("cls", True), ("mean", False), ("mean", True)])
+def test_pool_kernel_against_fp64_pool_of_its_own_hidden_states(pool, normalize):
+    """The pool kernel alone: the GPU's fp32 pooled vectors against an fp64 pool of the GPU's own hidden states.  A
+    mean of n bf16 values summed in fp32 is within (n + 4) u max|x| per component; normalising divides that by |v|
+    and adds the error of |v| (an H-term fp32 sum of squares, a square root and a division)."""
+    cfg_o = B.BertConfig(**{**SMALL.__dict__, "layers": 1, "pool": pool, "normalize": normalize})
+    w = B.init_weights(cfg_o, seed=7, bf16=True)
+    tok, cu = B.synth_batch(cfg_o, 9, 5, mean_len=150, std_len=140, min_len=1, max_len=512)
+    with Encoder(_mirror(cfg_o), max_tokens=8192, max_seqs=16) as enc:
+        enc.load_weights(w)
+        got = enc.encode_packed(tok, cu).astype(np.float64)
+        hs = bf16_bits_to_f32(enc.hidden_states()).astype(np.float64)
+    H = cfg_o.hidden
+    for s in range(len(cu) - 1):
+        x = hs[cu[s]:cu[s + 1]] if pool == "mean" else hs[cu[s]:cu[s] + 1]
+        n = x.shape[0]
+        v = x.mean(axis=0)
+        bound = (n + 4) * BD.U * np.abs(x).max(axis=0)
+        ref = v
+        if normalize:
+            nv = np.linalg.norm(v)
+            ref = v / nv
+            bound = bound / nv * (1 + np.sqrt(H) * np.abs(ref)) + (H + 4) * BD.U * np.abs(ref)
+        BD.assert_within(f"pool {pool} normalize={normalize} seq {s} (n={n})", got[s], ref, bound)
+
+
+def test_constant_row_layernorm_is_exact_on_gpu():
+    """A token whose embedding-LayerNorm input is a constant row (pos / type rows zero, constant word row, eps 1e-12)
+    and whose later LayerNorm inputs are constant too (zero layer weights, constant LN biases) comes out as exactly
+    bf16(ln2_b): each LayerNorm must return exactly its bias for a zero-variance row, with no NaN."""
+    cfg_o = B.BertConfig(**{**SMALL.__dict__, "layers": 1})
+    w = constant_row_weights(cfg_o)
+    tok, cu = np.array([1, 5, 5, 9, 5, 2], np.int32), np.array([0, 6], np.int32)
+    with Encoder(_mirror(cfg_o), max_tokens=256, max_seqs=2) as enc:
+        enc.load_weights(w)
+        enc.encode_packed(tok, cu)
+        got = bf16_bits_to_f32(enc.hidden_states())
+    assert np.array_equal(got[tok == 5], np.broadcast_to(w["l0.ln2_b"], (3, cfg_o.hidden)))
 
 
 def _check_pooled(got, ref):

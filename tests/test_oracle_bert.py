@@ -52,3 +52,43 @@ def test_pooling_modes_and_empty_sequence():
 def test_gelu_is_erf_form():
     x = np.array([-3.0, -1.0, 0.0, 0.5, 2.0])
     np.testing.assert_allclose(B.gelu(x), [-0.00404969409489031, -0.15865525393145702, 0.0, 0.34573123063700656, 1.9544997361036416], atol=1e-12)  # torch.nn.functional.gelu (float64)
+
+
+def test_bf16_store_mode_rounds_where_the_gpu_stores():
+    """encode_tokens(bf16_stores=True): every hidden state is a bf16 value, it stays close to the unrounded forward
+    (the roundings are small, but real), and under constant_row_weights a token with a constant embedding row comes
+    out as exactly bf16(ln2_b)."""
+    from oracle.cosine_topk import round_to_bf16
+
+    cfg = B.BertConfig(hidden=128, layers=2, heads=2, inter=256, vocab=120, max_pos=512, pool="cls")
+    w = B.init_weights(cfg, seed=7, bf16=True)
+    tok, cu = B.synth_batch(cfg, 4, 3, mean_len=40, std_len=30, min_len=1, max_len=128)
+    exact = B.encode_tokens(cfg, w, tok, cu)
+    stored = B.encode_tokens(cfg, w, tok, cu, bf16_stores=True)
+    assert np.array_equal(stored, round_to_bf16(stored.astype(np.float32)))
+    assert not np.array_equal(stored, round_to_bf16(exact.astype(np.float32)))
+    assert np.abs(stored - exact).max() <= 0.1
+    cos = (stored * exact).sum(1) / np.linalg.norm(stored, axis=1) / np.linalg.norm(exact, axis=1)
+    assert cos.min() >= 0.999
+
+    cfg1 = B.BertConfig(**{**cfg.__dict__, "layers": 1})
+    w1 = constant_row_weights(cfg1)
+    out = B.encode_tokens(cfg1, w1, np.array([1, 5, 5, 7], np.int32), np.array([0, 4], np.int32), bf16_stores=True)
+    assert np.array_equal(out[1:3], np.broadcast_to(w1["l0.ln2_b"], (2, cfg.hidden)))
+
+
+def constant_row_weights(cfg):
+    """Weights under which token 5's embedding-LayerNorm input is a constant row (pos / type rows zero, word row 5
+    constant) and every later LayerNorm input of that token is constant too: all layer matrices and biases zero, LN
+    biases constant vectors.  Its final hidden state is then exactly bf16(ln2_b), with eps 1e-12."""
+    w = B.init_weights(cfg, seed=3, bf16=True)
+    w["pos_emb"][:] = 0.0
+    w["type_emb"][:] = 0.0
+    w["word_emb"][5] = 0.3984375                               # a bf16 value
+    w["emb_ln_b"][:] = 0.5
+    for l in range(cfg.layers):
+        for n in ("wqkv", "bqkv", "wo", "bo", "wi", "bi", "wo2", "bo2"):
+            w[f"l{l}.{n}"][:] = 0.0
+        w[f"l{l}.ln1_b"][:] = -0.25
+        w[f"l{l}.ln2_b"][:] = 0.75
+    return w
