@@ -12,7 +12,7 @@ import os
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("AURORA_B200_LIB") or os.path.join(HERE, "libaurora_b200.so")   # override: A/B kernel builds
 
-ABI_VERSION = 2          # must equal AUR_ABI_VERSION of the library that gets loaded (struct layouts below)
+ABI_VERSION = 3         # must equal AUR_ABI_VERSION of the library that gets loaded (struct layouts below)
 AUR_OK = 0
 AUR_ERR_INVALID, AUR_ERR_CUDA, AUR_ERR_NOMEM, AUR_ERR_UNSUPPORTED, AUR_ERR_NO_DEVICE = -1, -2, -3, -4, -5
 AUR_BF16, AUR_F32 = 0, 1
@@ -42,7 +42,8 @@ class AurStats(C.Structure):
     _fields_ = [("rows", C.c_int64), ("live", C.c_int64), ("capacity", C.c_int64), ("dim", C.c_int32),
                 ("dtype", C.c_int32), ("last_kernel", C.c_int32), ("last_launches", C.c_int32),
                 ("last_kernel_ms", C.c_float), ("last_total_ms", C.c_float), ("last_finalize_ms", C.c_float),
-                ("last_merge_ms", C.c_float)]
+                ("last_merge_ms", C.c_float), ("last_candidates", C.c_int64), ("last_candidates_max", C.c_int32),
+                ("reserved", C.c_int32)]
 
 
 class AurEncoderConfig(C.Structure):

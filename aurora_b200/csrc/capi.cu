@@ -116,13 +116,14 @@ struct SearchCtx {
   cudaStream_t bound = nullptr;   // caller stream this context serves (nullptr = pool context)
   cudaEvent_t ev_begin = nullptr, ev_k0 = nullptr, ev_k1 = nullptr, ev_fin = nullptr, ev_end = nullptr;
   bool have_timing = false;
-  int last_kernel = 0, last_launches = 0;
+  int last_kernel = 0, last_launches = 0, last_nq = 0;
   int64_t snapshot_rows = 0;
   uint32_t epoch = 0;
   DevBuf<uint64_t> cand_a, cand_b;
   DevBuf<uint64_t> pub;          // tensor-core kernel's cross-CTA threshold exchange
   DevBuf<uint32_t> cand_count;   // compacted candidates per query (self-resetting)
   DevBuf<uint32_t> d_epoch;      // the tensor-core kernel's launch counter, device resident (CUDA-graph replays advance it)
+  DevBuf<uint32_t> cand_read;    // per query of the last search: candidate keys its exact re-rank read
   DevBuf<float> score_chunk;
   DevBuf<float> masked_inv;      // inverse norms with the invisible rows turned into NaN (tenant scope / id subset)
   DevBuf<int32_t> allow_rows;    // subset search: rows that stay visible
@@ -133,7 +134,7 @@ struct SearchCtx {
   DevBuf<float> stage_scores;
   DevBuf<int64_t> stage_ids;
   void release() {
-    cand_a.release(); cand_b.release(); pub.release(); cand_count.release(); d_epoch.release(); score_chunk.release(); masked_inv.release();
+    cand_a.release(); cand_b.release(); pub.release(); cand_count.release(); d_epoch.release(); cand_read.release(); score_chunk.release(); masked_inv.release();
     allow_rows.release(); row_mask.release(); scope_tab.release(); q_scope.release(); stage_q.release(); stage_quser.release(); stage_qorg.release(); stage_scores.release();
     stage_ids.release();
     if (ev_begin) cudaEventDestroy(ev_begin);
@@ -168,6 +169,7 @@ struct aur_index {
   int opt_kernel = AUR_KERNEL_AUTO;
   int opt_dbg_flags = 0;
   int opt_epi_groups = 0;        // 0 = auto
+  std::atomic<uint32_t> opt_dbg_epoch{0};   // bring-up: start value of the contexts' launch counters (0 = 1)
   std::vector<std::unique_ptr<SearchCtx>> ctxs;
   std::vector<SearchCtx*> free_ctxs;   // idle pool contexts
   SearchCtx* last_ctx = nullptr;       // context of the most recently enqueued search (aur_get_stats)
@@ -272,9 +274,9 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
     CU_TRY(cudaMemsetAsync(c->cand_count.p, 0, 8 * kTcQRows * 4, s));
   }
   if (c->d_epoch.n == 0) {
-    static const uint32_t one = 1;
+    const uint32_t e0 = ix->opt_dbg_epoch.load() ? ix->opt_dbg_epoch.load() : 1u;
     CU_TRY(c->d_epoch.reserve(1));
-    CU_TRY(cudaMemcpyAsync(c->d_epoch.p, &one, 4, cudaMemcpyHostToDevice, s));
+    CU_TRY(cudaMemcpyAsync(c->d_epoch.p, &e0, 4, cudaMemcpyHostToDevice, s));   // pageable source: staged before return
   }
   ++c->epoch;
   TcParams p;
@@ -286,9 +288,9 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   p.cand_count = c->cand_count.p;
   p.dbg_scores = dbg;
   p.pub = c->pub.p;
-  // searches: device-resident counter, advanced by the finalize kernel that follows; the bring-up entry point (no
-  // finalize behind it) tags its entries from a disjoint range on the host
-  p.epoch = 0x80000000u | c->epoch;
+  // searches: device-resident counter (1 .. kSearchEpochMax), advanced by the finalize kernel that follows; the bring-up
+  // entry point (no finalize behind it) tags its entries from the disjoint upper half on the host
+  p.epoch = (kSearchEpochMax + 1u) | c->epoch;
   p.epoch_ptr = dbg ? nullptr : c->d_epoch.p;
   p.n_rows = n_rows;
   p.nq = nqb; p.dim = ix->dim; p.ksel = ksel; p.n_lists = n_lists; p.n_qblocks = n_qblocks;
@@ -332,6 +334,8 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
                 "enough for its shared-memory lists at this dim", kTcMaxDim);
   c->last_kernel = kernel;
   c->last_launches = 0;
+  c->last_nq = nq;
+  CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
   c->snapshot_rows = n_rows;
   CU_TRY(cudaEventRecord(c->ev_begin, s));
   bool k_timed = false;
@@ -420,6 +424,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
     fa.cand = cur; fa.n_lists = n_lists; fa.ksel = ksel;
     fa.counts = compact ? c->cand_count.p : nullptr;
     fa.epoch_bump = compact ? c->d_epoch.p : nullptr;
+    fa.cand_read = c->cand_read.p + q0;
     fa.q = qb; fa.rows = ix->d_rows; fa.dtype = ix->dtype; fa.dim = ix->dim; fa.nq = nqb; fa.k = k;
     fa.ids = ix->d_ids;
     fa.out_scores = scores ? scores + static_cast<size_t>(q0) * k : nullptr;
@@ -679,6 +684,12 @@ int aur_get_stats(aur_index* ix, aur_stats* out) {
       CU_TRY(cudaEventElapsedTime(&out->last_total_ms, c->ev_begin, c->ev_end));
       CU_TRY(cudaEventElapsedTime(&out->last_finalize_ms, c->ev_k1, c->ev_fin));
       CU_TRY(cudaEventElapsedTime(&out->last_merge_ms, c->ev_fin, c->ev_end));
+      std::vector<uint32_t> n(std::min(static_cast<size_t>(c->last_nq), c->cand_read.n));
+      CU_TRY(cudaMemcpy(n.data(), c->cand_read.p, n.size() * 4, cudaMemcpyDeviceToHost));
+      for (uint32_t v : n) {
+        out->last_candidates += v;
+        out->last_candidates_max = std::max(out->last_candidates_max, static_cast<int32_t>(v));
+      }
     }
   }
   return AUR_OK;
@@ -779,6 +790,24 @@ int aur_compact(aur_index* ix, int64_t* reclaimed) {
 
 int aur_set_option(aur_index* ix, const char* key, int64_t value) {
   if (!ix || !key) return fail(AUR_ERR_INVALID, "null argument");
+  if (strcmp(key, "dbg_epoch") == 0) {   // bring-up: move every context's launch counter, e.g. to just before it wraps
+    if (value < 1 || value > kSearchEpochMax) return fail(AUR_ERR_INVALID, "dbg_epoch must be in 1 .. %u", kSearchEpochMax);
+    std::vector<SearchCtx*> cs;
+    {
+      std::lock_guard<std::mutex> lk(ix->mu);
+      ix->opt_dbg_epoch.store(static_cast<uint32_t>(value));   // contexts that start their counter later
+      for (auto& c : ix->ctxs) cs.push_back(c.get());
+    }
+    CU_TRY(cudaSetDevice(ix->device));
+    const uint32_t e = static_cast<uint32_t>(value);
+    for (SearchCtx* c : cs) {
+      std::lock_guard<std::mutex> cl(c->mu);
+      if (c->d_epoch.n == 0) continue;
+      CU_TRY(cudaDeviceSynchronize());   // searches already enqueued on the context finish with their own counter
+      CU_TRY(cudaMemcpy(c->d_epoch.p, &e, 4, cudaMemcpyHostToDevice));
+    }
+    return AUR_OK;
+  }
   std::lock_guard<std::mutex> lk(ix->mu);
   if (strcmp(key, "kernel") == 0) {
     if (value < AUR_KERNEL_AUTO || value > AUR_KERNEL_TC2) return fail(AUR_ERR_INVALID, "unknown kernel %lld", (long long)value);

@@ -74,7 +74,7 @@ struct TcParams {
                             // [n_qblocks, 64, n_lists (even)] each CTA's m-th best per query,
                             // then [n_qblocks, 64] the served thresholds
   int64_t n_rows;
-  uint32_t epoch;           // launch counter: pub entries of older launches are ignored
+  uint32_t epoch;           // launch counter: pub entries of other launches are ignored (kSearchEpochMax)
   const uint32_t* epoch_ptr;// when set, the counter lives in device memory (bumped by the finalize kernel)
   int nq, dim, ksel, n_lists, n_qblocks, num_stages, n_tiles;
   int dbg_flags;            // bring-up only (timing decomposition; results are wrong with 1..32): 1 = epilogue neither
@@ -83,6 +83,10 @@ struct TcParams {
                             // 32 = no inverse-norm prefetch, 64 = per-thread counters into dbg_scores
 };
 constexpr int kTcPubMax = 74;      // published values a thread folds into its threshold
+// Searches tag their exchange entries with the device-resident counter, which runs 1 .. kSearchEpochMax and wraps back
+// to 1; the bring-up entry point (aur_debug_tc_scores) tags from the disjoint upper half, so neither ever reads the
+// other's entries as its own.  0 is never a tag: it marks a zeroed table.
+constexpr uint32_t kSearchEpochMax = 0x7FFFFFFFu;
 
 // epi_groups: 1 = two epilogue warps take every tile; 2 = two pairs of warps alternate tiles
 // (each pair owns one score buffer and its own candidate lists).
@@ -119,6 +123,7 @@ struct FinalizeArgs {
   uint32_t* counts;  // nullable: per-query number of valid keys at the front of its cand row
                      // (reset to 0 by the kernel); null = all n_lists * ksel slots are keys
   uint32_t* epoch_bump;  // nullable: the tensor-core kernel's device-resident launch counter, advanced here (never 0)
+  uint32_t* cand_read;   // nullable: per query, the number of candidate keys the re-rank read (aur_stats.last_candidates)
   const void* q; const void* rows; int dtype; int dim; int nq; int k;
   const int64_t* ids;
   float* out_scores; int64_t* out_ids; double* out_scores64;   // (out_scores / out_ids nullable in exchange mode)

@@ -237,8 +237,8 @@ finalize_kernel(FinalizeArgs a) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");     // the candidate lists come from the previous kernel
   if (a.epoch_bump && blockIdx.x == 0 && threadIdx.x == 0) {   // that kernel is complete: next launch, next epoch
-    uint32_t e = *a.epoch_bump + 1;
-    *a.epoch_bump = e ? e : 1u;
+    const uint32_t e = *a.epoch_bump;
+    *a.epoch_bump = e >= kSearchEpochMax ? 1u : e + 1u;
   }
 
   const int cap = a.n_lists * a.ksel;                       // row stride of cand
@@ -252,6 +252,7 @@ finalize_kernel(FinalizeArgs a) {
     spec[u] = (a.counts && i < cap) ? src[i] : 0ull;
   }
   const int n = a.counts ? min(static_cast<int>(a.counts[qi]), cap) : cap;
+  if (a.cand_read && threadIdx.x == 0) a.cand_read[qi] = static_cast<uint32_t>(n);
   // Sort in rounds of at most sort_cap keys; the best ksel of earlier rounds ride along
   // at the front.  (One round unless a compacted row overflows the sort buffer.)
   int P = 1;

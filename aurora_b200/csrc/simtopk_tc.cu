@@ -248,6 +248,18 @@ __device__ __forceinline__ float read_threshold(const unsigned long long* tq, ui
   return (static_cast<uint32_t>(e >> 32) == epoch) ? __uint_as_float(static_cast<uint32_t>(e)) : -INFINITY;
 }
 
+// Publishes value v of this launch into a CTA's exchange slot.  The slot's first publish of a launch REPLACES the entry
+// (atomicExch), later ones keep the max.  A plain atomicMax would never get past an entry that another launch left with
+// a numerically larger tag -- a bring-up launch (upper half of the tags) or any search before the counter wrapped --
+// and the exchange would stay without a valid value for that slot until the table is reallocated.  With two epilogue
+// groups both groups' first publishes replace: the slot may drop to the smaller of their values for a moment, which is
+// still a value the CTA vouches for, so every threshold derived from it stays certified.
+__device__ __forceinline__ void publish_value(unsigned long long* slot, uint32_t epoch, float v, bool first) {
+  const unsigned long long e = (static_cast<unsigned long long>(epoch) << 32) | f32_to_ord(v);
+  if (first) atomicExch(slot, e);
+  else atomicMax(slot, e);
+}
+
 constexpr uint32_t kNaNBits = 0x7FC00000u;
 
 // kMask: the queries of the batch carry different tenant scopes (user_id == u OR org_id == o,
@@ -615,8 +627,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
         }
         const float pv0 = top4_get(st.top, xm);
         if (pv0 > -INFINITY) {
+          publish_value(pubrow + tset, epoch, pv0, true);
           published = pv0;
-          atomicMax(pubrow + tset, (static_cast<unsigned long long>(epoch) << 32) | f32_to_ord(pv0));
         }
         booted = true;
         const long long tb = clock64();
@@ -760,8 +772,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
         // publish this CTA's m-th best for the exchange (monotone, so stale reads stay valid)
         const float pv = top4_get(st.top, xm);
         if (xchg && pv > published) {
+          publish_value(pubrow + tset, epoch, pv, published == -INFINITY);
           published = pv;
-          atomicMax(pubrow + tset, (static_cast<unsigned long long>(epoch) << 32) | f32_to_ord(pv));
         }
         t_pub += TCLK() - t_pub0;
       }

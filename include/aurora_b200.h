@@ -40,7 +40,7 @@
 extern "C" {
 #endif
 
-#define AUR_ABI_VERSION 2
+#define AUR_ABI_VERSION 3
 
 typedef enum aur_status {
   AUR_OK = 0,
@@ -83,6 +83,9 @@ typedef struct aur_stats {
   float   last_finalize_ms; /* from the end of the (first) similarity kernel to the end of the last exact
                                re-rank kernel (for nq > 256 this spans the later query blocks too)         */
   float   last_merge_ms; /* aur_search_exchange_dev: delivery wait + cross-shard merge; else ~0           */
+  int64_t last_candidates;     /* candidate keys the last search's exact re-rank read, summed over its queries */
+  int32_t last_candidates_max; /* the most any one query of the last search carried into the re-rank          */
+  int32_t reserved;
 } aur_stats;
 
 int aur_abi_version(void);
@@ -94,6 +97,8 @@ int aur_device_count(void);
 int aur_open(const aur_config* cfg, aur_index** out);
 int aur_close(aur_index* ix);
 int aur_get_stats(aur_index* ix, aur_stats* out);
+/* Options: "kernel" (aur_kernel), "epi_groups"; bring-up only: "dbg_flags", and "dbg_epoch" (1 .. 2^31 - 1), which
+ * sets the tensor-core kernel's launch counter of every search context of the index, e.g. just before it wraps. */
 int aur_set_option(aur_index* ix, const char* key, int64_t value);
 int aur_sync(aur_index* ix);
 

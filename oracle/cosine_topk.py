@@ -123,7 +123,7 @@ def _chunk_scores(Q64, qn, C, lo, hi, qsel, live, row_user, row_org, q_user, q_o
 
 def cosine_topk(Q, C, k: int, ids=None, live=None, row_user=None, row_org=None,
                 q_user=None, q_org=None, clamp: bool = False, slack: int = 16,
-                chunk: int = 131072):
+                chunk: int = 131072, return_f64: bool = False):
     """Brute-force cosine top-k.
 
     Q [nq, D], C [N, D] (any float dtype; pass bf16-rounded fp32 to model a bf16
@@ -131,6 +131,8 @@ def cosine_topk(Q, C, k: int, ids=None, live=None, row_user=None, row_org=None,
     tombstone mask; ``row_user/row_org/q_user/q_org`` int codes for the tenant scope
     (all None = unfiltered).  Returns ``(ids [nq,k] int64, scores [nq,k] float32)``
     best-first, padded with (PAD_ID, PAD_SCORE) when fewer than k rows are visible.
+    ``return_f64``: also return the fp64 scores [nq,k] the float32 ones were rounded
+    from (same padding), as a third element.
     """
     Q = np.asarray(Q)
     C = np.asarray(C)
@@ -138,8 +140,9 @@ def cosine_topk(Q, C, k: int, ids=None, live=None, row_user=None, row_org=None,
     ids = np.arange(N, dtype=np.int64) if ids is None else np.asarray(ids, dtype=np.int64)
     out_ids = np.full((nq, k), PAD_ID, dtype=np.int64)
     out_sc = np.full((nq, k), PAD_SCORE, dtype=np.float32)
+    out64 = np.full((nq, k), PAD_SCORE, dtype=np.float64)
     if N == 0 or nq == 0 or k == 0:
-        return out_ids, out_sc
+        return (out_ids, out_sc, out64) if return_f64 else (out_ids, out_sc)
 
     Q64 = Q.astype(np.float64)
     qn = _norms64(Q64)
@@ -187,7 +190,8 @@ def cosine_topk(Q, C, k: int, ids=None, live=None, row_user=None, row_org=None,
         order = np.lexsort((rid, -ex))[:k]
         out_ids[i, : order.size] = rid[order]
         out_sc[i, : order.size] = ex[order].astype(np.float32)
-    return out_ids, out_sc
+        out64[i, : order.size] = ex[order]
+    return (out_ids, out_sc, out64) if return_f64 else (out_ids, out_sc)
 
 
 # --------------------------------------------------------- timed CPU baseline ("port")

@@ -37,9 +37,40 @@ def test_header_symbols_are_exported(lib):
         assert hasattr(raw, name), f"{name} declared in the header but not exported by the .so"
 
 
-def test_abi_version_and_error_string(lib):
-    assert lib.aur_abi_version() == N.ABI_VERSION == 2
+def test_abi_version_3_and_error_string(lib):
+    """Version 3: aur_stats grew by last_candidates / last_candidates_max, so a caller built against version 2 passes a
+    struct the library would write past.  The library, the header and the ctypes binding must agree on it."""
+    declared = int(re.search(r"#define AUR_ABI_VERSION (\d+)", open(HEADER).read()).group(1))
+    assert lib.aur_abi_version() == N.ABI_VERSION == declared == 3
     assert isinstance(lib.aur_last_error(), bytes)
+
+
+def _header_struct_fields(name):
+    src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
+    body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (name, name), src, flags=re.S).group(1)
+    ctypes_of = {"int64_t": C.c_int64, "int32_t": C.c_int32, "float": C.c_float, "double": C.c_double}
+    fields = []
+    for decl in body.split(";"):
+        decl = decl.strip()
+        if decl:
+            ctype, names = decl.split(None, 1)
+            fields += [(nm.strip(), ctypes_of[ctype]) for nm in names.split(",")]
+    return fields
+
+
+def test_stats_struct_matches_the_header():
+    """aur_stats as the header declares it, field by field (ABI 3 added last_candidates / last_candidates_max): the
+    ctypes mirror must agree in names, types and therefore offsets, or every stats read is garbage."""
+    assert N.AurStats._fields_ == _header_struct_fields("aur_stats")
+    assert N.AurStats.last_candidates.offset == 56 and N.AurStats.last_candidates_max.offset == 64
+    assert C.sizeof(N.AurStats) == 72
+
+
+def test_stats_without_a_search_report_no_candidates(lib):
+    """aur_get_stats rejects a null index; the new fields exist and start at zero in a zeroed struct."""
+    st = N.AurStats()
+    assert lib.aur_get_stats(None, C.byref(st)) == N.AUR_ERR_INVALID
+    assert st.last_candidates == 0 and st.last_candidates_max == 0
 
 
 def test_header_cites_reference_interfaces():

@@ -12,6 +12,7 @@ import pytest
 from aurora_b200 import _native as N
 from aurora_b200.engine import DeviceBuffer, Index, MultiIndex, cosine_pairs, merge_topk_dev, merge_topk_packed_dev, to_bf16_bits
 from oracle import cosine_topk as O
+from tests.gpu_exact import check_exact, dev_search
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -60,15 +61,18 @@ def test_cfg1_fp32_matches_reference_golden():
 @pytest.mark.parametrize("n,d,nq,k,dtype", [
     (1000, 384, 1, 5, "f32"), (5000, 768, 33, 32, "bf16"), (700, 100, 7, 10, "f32"), (3, 64, 2, 5, "bf16"),
     (4097, 200, 65, 128, "bf16"), (2048, 8, 3, 1, "bf16"),
+    (3, 5, 2, 5, "f32"), (2049, 1536, 4, 16, "bf16"),      # fewer rows than k; the re-rank's scalar gather
 ])
 def test_simt_parity(n, d, nq, k, dtype):
     C, Q = _data(n, d, nq, seed=n + d, bf16=(dtype == "bf16"))
     ext = np.arange(n, dtype=np.int64) * 3 + 7
+    want = O.cosine_topk(Q, C, k, ids=ext, return_f64=True)
     with Index(d, max(n, 64), dtype=dtype) as ix:
         ix.set_kernel(N.KERNEL_SIMT)
         ix.add(C, ext)
         ids, sc = ix.search(Q, k)
-    _check(ids, sc, *O.cosine_topk(Q, C, k, ids=ext))
+        check_exact(dev_search(ix, Q, k), Q, C, k, want=want)
+    _check(ids, sc, *want[:2])
 
 
 def test_simt_tenant_filter_and_tombstones():
@@ -142,15 +146,19 @@ def test_uniform_tenant_scope_is_served_by_the_tcgen05_kernel(with_org):
     (777, 64, 1, 1), (12345, 256, 129, 128), (64, 768, 256, 32), (5000, 768, 128, 64),
     # dims up to 1024: the whole query block stays in shared memory beside the TMA ring
     (20000, 1024, 256, 32), (9000, 1024, 300, 64), (7000, 896, 130, 10), (4000, 832, 64, 5),
+    # corpora shorter than one tile (fewer rows than k: padding)
+    (1, 256, 3, 5), (63, 128, 70, 32),
 ])
 def test_tcgen05_parity(kernel, n, d, nq, k):
     C, Q = _data(n, d, nq, seed=n % 1000 + nq + d)
+    want = O.cosine_topk(Q, C, k, return_f64=True)
     with Index(d, n) as ix:
         ix.add(C, np.arange(n, dtype=np.int64))
         ix.set_kernel(kernel)
         ids, sc = ix.search(Q, k)
         assert ix.stats()["last_kernel"] == kernel
-    _check(ids, sc, *O.cosine_topk(Q, C, k))
+        check_exact(dev_search(ix, Q, k), Q, C, k, want=want)
+    _check(ids, sc, *want[:2])
 
 
 @pytest.mark.parametrize("n,d,nq,k", [
