@@ -27,6 +27,7 @@ EXPORTS = [
     "aur_merge_topk_dev", "aur_merge_topk_packed_dev", "aur_merge_topk_host", "aur_exchange_create", "aur_exchange_connect", "aur_exchange_close",
     "aur_exchange_status", "aur_search_exchange_dev", "aur_cosine_pairs", "aur_dev_malloc", "aur_dev_free", "aur_memcpy_h2d", "aur_memcpy_d2h",
     "aur_debug_tc_scores",
+    "aur_kw_open", "aur_kw_close", "aur_kw_add", "aur_kw_remove", "aur_kw_compact", "aur_kw_get_stats", "aur_kw_search",
     "aur_encoder_open", "aur_encoder_close", "aur_encoder_load", "aur_encode", "aur_encode_append",
     "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
     "aur_tokenize", "aur_encode_text_append", "aur_debug_gemm", "aur_debug_attention", "aur_debug_encoder_hidden",
@@ -44,6 +45,12 @@ class AurStats(C.Structure):
                 ("last_kernel_ms", C.c_float), ("last_total_ms", C.c_float), ("last_finalize_ms", C.c_float),
                 ("last_merge_ms", C.c_float), ("last_candidates", C.c_int64), ("last_candidates_max", C.c_int32),
                 ("reserved", C.c_int32)]
+
+
+class AurKwStats(C.Structure):
+    _fields_ = [("docs", C.c_int64), ("live", C.c_int64), ("capacity", C.c_int64), ("postings_used", C.c_int64),
+                ("postings_allocated", C.c_int64), ("total_len", C.c_int64), ("last_launches", C.c_int32),
+                ("last_ms", C.c_float), ("last_terms", C.c_int32), ("last_spilled", C.c_int32)]
 
 
 class AurEncoderConfig(C.Structure):
@@ -115,6 +122,13 @@ def load():
         "aur_memcpy_h2d": (C.c_int, [i32, vp, vp, C.c_uint64]),
         "aur_memcpy_d2h": (C.c_int, [i32, vp, vp, C.c_uint64]),
         "aur_debug_tc_scores": (C.c_int, [vp, vp, i32, i32, vp, C.POINTER(i32), vp]),
+        "aur_kw_open": (C.c_int, [i32, i64, i64, C.POINTER(vp)]),
+        "aur_kw_close": (C.c_int, [vp]),
+        "aur_kw_add": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64]),
+        "aur_kw_remove": (C.c_int, [vp, vp, i64, C.POINTER(i64)]),
+        "aur_kw_compact": (C.c_int, [vp, C.POINTER(i64)]),
+        "aur_kw_get_stats": (C.c_int, [vp, C.POINTER(AurKwStats)]),
+        "aur_kw_search": (C.c_int, [vp, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, C.POINTER(i64)]),
         "aur_encoder_open": (C.c_int, [C.POINTER(AurEncoderConfig), C.POINTER(vp)]),
         "aur_encoder_close": (C.c_int, [vp]),
         "aur_encoder_load": (C.c_int, [vp, C.c_char_p, vp, i64]),

@@ -7,8 +7,9 @@ vector leg and ``1 - alpha`` for the keyword leg.  Both live inside the Weaviate
 not in /root/reference -- so this restates Weaviate 1.27's documented behaviour: BM25 with k1 = 1.2,
 b = 0.75, "word" tokenisation (lower-case, split on non-alphanumerics), idf = ln(1 + (N - n + 0.5) /
 (n + 0.5)); rankedFusion with the constant 60 and 0-based ranks.  Unpinned: the reference has no test
-at this boundary (SURVEY.md section 8c).  Like in the reference this leg is host (CPU) work over text;
-only the dense leg touches vectors and it runs on the GPU.
+at this boundary (SURVEY.md section 8c).  ``BM25Index`` is the host index (the path of the test doubles and
+the definition the device is held to); ``DeviceBM25`` keeps the vocabulary and tokenisation on the host and the
+postings, scoring and top-k in the GPU keyword store (csrc/keyword.cu, DESIGN.md section 10).
 """
 
 from __future__ import annotations
@@ -144,6 +145,128 @@ class BM25Index:
         if allow is not None:
             scores = {d: v for d, v in scores.items() if allow(d)}
         return sorted(scores.items(), key=lambda kv: (-kv[1], kv[0]))[:limit]
+
+
+def build_csr(vocab: Dict[str, int], texts: Iterable[str]):
+    """Documents -> (term ids int32, tf int32, offsets int64 [n + 1]) with term ids ascending inside each document.
+    New words get the next free id in ``vocab`` (grow-only)."""
+    import numpy as np
+
+    terms: List[int] = []
+    tfs: List[int] = []
+    offsets = [0]
+    for text in texts:
+        counts = Counter(tokenize(text))
+        row = []
+        for t, tf in counts.items():
+            tid = vocab.get(t)
+            if tid is None:
+                tid = vocab[t] = len(vocab)
+            row.append((tid, tf))
+        row.sort()
+        terms.extend(t for t, _ in row)
+        tfs.extend(f for _, f in row)
+        offsets.append(len(terms))
+    return np.asarray(terms, dtype=np.int32), np.asarray(tfs, dtype=np.int32), np.asarray(offsets, dtype=np.int64)
+
+
+def query_csr(vocab: Dict[str, int], queries: Iterable[str]):
+    """Queries -> (term ids int32, offsets int64 [nq + 1]): each query's ``sorted(set(tokenize(q)))`` -- the loop
+    path's summation order -- with words the vocabulary never saw dropped (they have no posting)."""
+    import numpy as np
+
+    terms: List[int] = []
+    offsets = [0]
+    for q in queries:
+        terms.extend(vocab[t] for t in sorted(set(tokenize(q))) if t in vocab)
+        offsets.append(len(terms))
+    return np.asarray(terms, dtype=np.int32), np.asarray(offsets, dtype=np.int64)
+
+
+class DeviceBM25:
+    """The keyword leg on the GPU (``engine.KeywordIndex``), with ``BM25Index``'s surface plus ``search_batch``.
+
+    Scores and order are those of ``BM25Index.search`` on its loop path, bit for bit (DESIGN.md section 10).  Holds the
+    vocabulary (word -> int32 term id, grow-only; a reloaded knowledge base rebuilds it from the texts) and tenant codes
+    per document, so a tenant scope is applied on the device like the dense leg's."""
+
+    def __init__(self, capacity: int = 1 << 20, device: int = 0, postings_capacity: int = 0, store=None):
+        if store is None:
+            from .engine import KeywordIndex
+
+            store = KeywordIndex(capacity, postings_capacity=postings_capacity, device=device)
+        self.store = store
+        self.vocab: Dict[str, int] = {}
+        self._docs: set = set()
+
+    def __len__(self) -> int:
+        return len(self._docs)
+
+    def add(self, doc_id: int, text: str, user_code: int = 0, org_code: int = -1) -> None:
+        self.add_many([doc_id], [text], [user_code], [org_code])
+
+    def add_many(self, doc_ids, texts, user_codes=None, org_codes=None) -> None:
+        """Upsert documents in one call (one device append)."""
+        import numpy as np
+
+        doc_ids = np.asarray(doc_ids, dtype=np.int64)
+        if len(doc_ids) == 0:
+            return
+        terms, tfs, offsets = build_csr(self.vocab, texts)
+        self.store.add(doc_ids, terms, tfs, offsets, user_codes, org_codes)
+        self._docs.update(int(d) for d in doc_ids)
+
+    def remove(self, doc_id: int) -> bool:
+        return self.remove_many([doc_id]) > 0
+
+    def remove_many(self, doc_ids) -> int:
+        import numpy as np
+
+        ids = [int(d) for d in doc_ids]
+        if not ids:
+            return 0
+        self._docs.difference_update(ids)
+        return self.store.remove(np.asarray(ids, dtype=np.int64))
+
+    def compact(self) -> int:
+        return self.store.compact()
+
+    def stats(self) -> dict:
+        return self.store.stats()
+
+    def search(self, query: str, limit: int, allow: Optional[Callable[[int], bool]] = None,
+               allowed: Optional[set] = None, allowed_sorted=None) -> List[Tuple[int, float]]:
+        """``BM25Index.search``: top-``limit`` (doc id, score), best first, ties by ascending id; ``allowed`` (a set of
+        ids) or ``allow`` (a predicate, resolved over the stored ids) pre-filter the documents."""
+        if limit <= 0 or not self._docs:
+            return []
+        allow_ids = None
+        if allowed_sorted is not None:
+            allow_ids = allowed_sorted
+        elif allowed is not None:
+            allow_ids = list(allowed)
+        if allow is not None:
+            base = self._docs if allow_ids is None else set(int(d) for d in allow_ids)
+            allow_ids = [d for d in base if allow(d)]
+        return self._run([query], limit, None, None, allow_ids)[0]
+
+    def search_batch(self, queries: List[str], limit: int, q_user=None, q_org=None) -> List[List[Tuple[int, float]]]:
+        """All queries in one device search; ``q_user`` / ``q_org``: per-query tenant codes (row_user == u or, for
+        org >= 0, row_org == o), None = unscoped."""
+        if not queries:
+            return []
+        if limit <= 0 or not self._docs:
+            return [[] for _ in queries]
+        return self._run(queries, limit, q_user, q_org, None)
+
+    def _run(self, queries, limit, q_user, q_org, allow_ids):
+        q_terms, q_off = query_csr(self.vocab, queries)
+        ids, scores, _ = self.store.search(q_terms, q_off, int(limit), q_user, q_org, allow_ids)
+        out = []
+        for row_i, row_s in zip(ids, scores):
+            n = int((row_i >= 0).sum())
+            out.append([(int(d), float(s)) for d, s in zip(row_i[:n], row_s[:n])])
+        return out
 
 
 def ranked_fusion(legs: Iterable[Tuple[float, List[int]]], limit: int) -> List[Tuple[int, float]]:

@@ -182,6 +182,13 @@ class SnapshotPolicy:
                     dead = kb.index.compact()
             except Exception:
                 pass
+            try:       # the GPU keyword store by the same rule (the host BM25Index keeps no tombstones)
+                if hasattr(kb.sparse, "compact"):
+                    ks = kb.sparse.stats()
+                    if ks["docs"] > 1024 and (ks["docs"] - ks["live"]) * 4 > ks["docs"]:
+                        kb.sparse.compact()
+            except Exception:
+                pass
             kb.save(self.dir)
             self.saves += 1
             return {"saved": True, "directory": self.dir, "seconds": round(time.perf_counter() - t0, 3), "compacted_rows": dead}

@@ -314,6 +314,80 @@ class MultiIndex:
         self.close()
 
 
+class KeywordIndex:
+    """BM25 keyword store resident on one GPU (aur_kw_*): documents as (term id, tf) postings, keyed by the same ids and
+    tenant codes as ``Index``.  The vocabulary (text -> term ids) lives in ``bm25.DeviceBM25``."""
+
+    def __init__(self, capacity: int, postings_capacity: int = 0, device: int = 0):
+        self._lib = N.load()
+        self.capacity, self.device = int(capacity), int(device)
+        self._h = C.c_void_p()
+        N.check(self._lib.aur_kw_open(self.device, self.capacity, int(postings_capacity), C.byref(self._h)))
+
+    def close(self) -> None:
+        if getattr(self, "_h", None) is not None and self._h.value:
+            self._lib.aur_kw_close(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def add(self, ids, term_ids, tfs, offsets, user_codes=None, org_codes=None) -> None:
+        """Upsert len(ids) documents: document i has postings [offsets[i], offsets[i+1]) of term_ids / tfs (term ids
+        strictly increasing within a document)."""
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+        if offsets.shape != (ids.shape[0] + 1,):
+            raise ValueError("offsets must be [n + 1]")
+        t = np.ascontiguousarray(term_ids, dtype=np.int32)
+        f = np.ascontiguousarray(tfs, dtype=np.int32)
+        u = None if user_codes is None else np.ascontiguousarray(user_codes, dtype=np.int32)
+        o = None if org_codes is None else np.ascontiguousarray(org_codes, dtype=np.int32)
+        N.check(self._lib.aur_kw_add(self._h, _ptr(ids), _ptr(u), _ptr(o), _ptr(t), _ptr(f), _ptr(offsets), ids.shape[0]))
+
+    def remove(self, ids) -> int:
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        removed = C.c_int64(0)
+        N.check(self._lib.aur_kw_remove(self._h, _ptr(ids), ids.shape[0], C.byref(removed)))
+        return int(removed.value)
+
+    def compact(self) -> int:
+        freed = C.c_int64(0)
+        N.check(self._lib.aur_kw_compact(self._h, C.byref(freed)))
+        return int(freed.value)
+
+    def stats(self) -> dict:
+        st = N.AurKwStats()
+        N.check(self._lib.aur_kw_get_stats(self._h, C.byref(st)))
+        return {f: getattr(st, f) for f, _ in N.AurKwStats._fields_}
+
+    def search(self, q_terms, q_offsets, k: int, q_user=None, q_org=None, allow_ids=None):
+        """(ids [nq,k] int64, scores [nq,k] float64, snapshot rows).  Query q's term ids are
+        q_terms[q_offsets[q]:q_offsets[q+1]] in summation order.  ``allow_ids``: None = every document."""
+        q_off = np.ascontiguousarray(q_offsets, dtype=np.int64)
+        nq = q_off.shape[0] - 1
+        qt = np.ascontiguousarray(q_terms, dtype=np.int32)
+        if qt.size == 0:
+            qt = np.zeros(1, dtype=np.int32)
+        scores = np.empty((nq, k), dtype=np.float64)
+        ids = np.empty((nq, k), dtype=np.int64)
+        u = None if q_user is None else np.ascontiguousarray(q_user, dtype=np.int32)
+        o = None if q_org is None else np.ascontiguousarray(q_org, dtype=np.int32)
+        allow, n_allow = None, 0
+        if allow_ids is not None:
+            allow = np.ascontiguousarray(allow_ids, dtype=np.int64)
+            n_allow = allow.shape[0]
+            if n_allow == 0:
+                allow = np.zeros(1, dtype=np.int64)     # a real pointer: "nothing is allowed"
+        snap = C.c_int64(-1)
+        N.check(self._lib.aur_kw_search(self._h, _ptr(qt), _ptr(q_off), int(nq), int(k), _ptr(u), _ptr(o), _ptr(allow),
+                                        int(n_allow), _ptr(scores), _ptr(ids), C.byref(snap)))
+        return ids, scores, int(snap.value)
+
+
 def merge_topk_packed_dev(device: int, packed_ptr: int, n_shards: int, nq: int, k: int, out_scores_ptr: int,
                           out_ids_ptr: int, out_scores64_ptr: int = 0, stream: int = 0) -> None:
     """packed: [n_shards][2][nq][k] 8-byte words (plane 0 fp64 scores, plane 1 int64 ids)."""

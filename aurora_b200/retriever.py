@@ -34,6 +34,7 @@ from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import numpy as np
 
+from .bm25 import BM25Index
 from .filters import Filter, HybridFusion  # noqa: F401  (re-exported for call sites)
 
 logger = logging.getLogger(__name__)
@@ -73,9 +74,9 @@ class KnowledgeBase:
             def index_factory(dim, cap):
                 return Index(dim, cap, dtype="bf16", device=device)
         self.index = index_factory(self.dim, int(capacity))
-        from .bm25 import BM25Index
-
-        self.sparse = BM25Index()       # keyword leg of the hybrid query (host text work, like in Weaviate)
+        # keyword leg of the hybrid query: on the GPU beside a CUDA vector index, else the host index
+        self.sparse = self._keyword_store(int(capacity))
+        self._kw_device = not isinstance(self.sparse, BM25Index)
         self._lock = threading.RLock()  # the reference's module globals are unlocked (weaviate_client.py:31-32)
         self._props: Dict[int, Dict[str, Any]] = {}   # id -> properties
         self._key2id: Dict[str, int] = {}             # uuid5 -> id
@@ -92,6 +93,25 @@ class KnowledgeBase:
         self._wal_sync = True
         self._replaying = False
         self._scope_cache: Dict[Tuple[Optional[str], Optional[str]], tuple] = {}   # tenant -> (mutations, id set, sorted ids)
+
+    def _keyword_store(self, capacity: int):
+        """``DeviceBM25`` on the vector index's GPU when that index is an ``engine.Index`` or a ``MultiIndex`` of them
+        (on its first shard's device), else ``BM25Index``.  Both score the same (DESIGN.md section 10)."""
+        from .bm25 import DeviceBM25
+        from .engine import Index, MultiIndex
+
+        ix = self.index
+        if isinstance(ix, Index):
+            return DeviceBM25(capacity, device=ix.device)
+        if isinstance(ix, MultiIndex) and ix.shards and all(isinstance(sh, Index) for sh in ix.shards):
+            return DeviceBM25(capacity, device=ix.shards[0].device)
+        return BM25Index()
+
+    def _scope_codes(self, user_id: Optional[str], org_id: Optional[str]) -> Tuple[int, int]:
+        """Tenant scope as the kernels take it: (user code, org code); -2 matches no row, org -1 = no org."""
+        cu = self._code(self._user_code, user_id, False) if user_id else -2
+        co = self._code(self._org_code, org_id, False) if org_id else -1
+        return cu, (-1 if co == -2 else co)
 
     # ------------------------------------------------------------------ tenant codes
     def _code(self, table: Dict[str, int], key: Optional[str], create: bool) -> int:
@@ -212,7 +232,10 @@ class KnowledgeBase:
                 self._by_user.setdefault(props.get("user_id"), set()).add(rid)
                 if props.get("org_id"):
                     self._by_org.setdefault(props["org_id"], set()).add(rid)
-                self.sparse.add(rid, text)
+                if not self._kw_device:
+                    self.sparse.add(rid, text)
+            if self._kw_device:
+                self.sparse.add_many(ids, texts, ucode, ocode)
             self.mutations += len(objs)
             self._log({"op": "put", "gen": gen, "user": user_id, "org": org_id, "objs": [list(o) for o in objs]})
         return len(objs)
@@ -242,7 +265,8 @@ class KnowledgeBase:
     # ------------------------------------------------------------------ search
     def query(self, query: str, limit: int, filters=None, user_id: Optional[str] = None,
               org_id: Optional[str] = None, alpha: Optional[float] = None, scoped: bool = False,
-              _dense: Optional[List[Tuple[int, float]]] = None) -> List[SimpleNamespace]:
+              _dense: Optional[List[Tuple[int, float]]] = None,
+              _sparse: Optional[List[Tuple[int, float]]] = None) -> List[SimpleNamespace]:
         """Top-``limit`` objects.  ``alpha`` None or >= 1: pure vector search, ``score`` = cosine
         (near_text, incident_feedback/weaviate_client.py:286-297).  ``alpha`` < 1: hybrid with ranked
         fusion (weaviate_client.py:252-259): dense and BM25 lists fused as alpha/(rank+60) +
@@ -310,14 +334,27 @@ class KnowledgeBase:
                 picked = [(rid, sc, sc) for rid, sc in dense[:limit]]
             else:
                 # keyword leg under the same pre-filter: the resolved filter's ids, else the tenant's own inverted lists
-                allowed_arr = None
-                if allowed is not None:
-                    allowed_set = set(allowed)
-                elif tenant:
-                    allowed_set, allowed_arr = self._tenant_scope(user_id, org_id)
+                if _sparse is not None:     # keyword leg already computed by query_batch (same scope, same fetch);
+                    # objects deleted since then drop out, as for the dense leg
+                    sparse = [(rid, sc) for rid, sc in _sparse if rid in self._props]
+                elif self._kw_device:       # the device applies the tenant scope itself, as the dense leg does
+                    if allowed is not None:
+                        sparse = self.sparse.search(query, _MAX_FETCH, allowed=allowed)
+                    elif tenant:
+                        cu, co = self._scope_codes(user_id, org_id)
+                        sparse = self.sparse.search_batch([query], _MAX_FETCH, np.array([cu], np.int32),
+                                                          np.array([co], np.int32))[0]
+                    else:
+                        sparse = self.sparse.search(query, _MAX_FETCH)
                 else:
-                    allowed_set = None
-                sparse = self.sparse.search(query, _MAX_FETCH, allowed=allowed_set, allowed_sorted=allowed_arr)
+                    allowed_arr = None
+                    if allowed is not None:
+                        allowed_set = set(allowed)
+                    elif tenant:
+                        allowed_set, allowed_arr = self._tenant_scope(user_id, org_id)
+                    else:
+                        allowed_set = None
+                    sparse = self.sparse.search(query, _MAX_FETCH, allowed=allowed_set, allowed_sorted=allowed_arr)
                 from .bm25 import ranked_fusion
 
                 cos = dict(dense)
@@ -332,11 +369,21 @@ class KnowledgeBase:
     def query_batch(self, reqs: List[Tuple[Optional[str], str, int, Optional[float], Optional[str]]]) -> List[List[SimpleNamespace]]:
         """Several tenant-scoped searches at once: ``(user_id, query, limit, alpha, org_id)`` each.  All query texts go
         through ONE encoder batch; the dense leg is ONE kernel launch per result size (the tenant scopes of the batch ride
-        along as per-row bit masks on the tensor-core kernel); fusion / shaping per request as in ``query``."""
+        along as per-row bit masks on the tensor-core kernel); on a GPU keyword store the keyword leg of every hybrid request
+        (alpha < 1) is ONE device search with per-request tenant codes; fusion / shaping per request as in ``query``."""
         need = [i for i, (u, q, lim, a, o) in enumerate(reqs) if lim > 0 and (u or o) and (a is None or a > 0.0)]
+        kw_need = [i for i, (u, q, lim, a, o) in enumerate(reqs)
+                   if lim > 0 and (u or o) and a is not None and a < 1.0] if self._kw_device else []
         vecs = self.encoder.encode([reqs[i][1] for i in need]) if need else None
         dense: Dict[int, List[Tuple[int, float]]] = {}
+        sparse: Dict[int, List[Tuple[int, float]]] = {}
         with self._lock:
+            if kw_need:
+                codes = [self._scope_codes(reqs[i][0], reqs[i][4]) for i in kw_need]
+                lists = self.sparse.search_batch([reqs[i][1] for i in kw_need], _MAX_FETCH,
+                                                 np.array([c[0] for c in codes], np.int32),
+                                                 np.array([c[1] for c in codes], np.int32))
+                sparse = dict(zip(kw_need, lists))
             groups: Dict[int, List[Tuple[int, int, int]]] = {}      # fetch size -> [(position, user code, org code)]
             for pos, i in enumerate(need):
                 u, _, lim, a, o = reqs[i]
@@ -355,7 +402,8 @@ class KnowledgeBase:
                     dense[need[p_]] = [(int(r), float(s_)) for r, s_ in zip(ids[row], scores[row]) if r >= 0]
         out = []
         for i, (u, q, lim, a, o) in enumerate(reqs):
-            out.append(self.query(q, lim, user_id=u, org_id=o, alpha=a, scoped=True, _dense=dense.get(i)))
+            out.append(self.query(q, lim, user_id=u, org_id=o, alpha=a, scoped=True, _dense=dense.get(i),
+                                  _sparse=sparse.get(i)))
         return out
 
     # ------------------------------------------------------------------ persistence
@@ -427,7 +475,13 @@ class KnowledgeBase:
             kb._by_user.setdefault(p.get("user_id"), set()).add(rid)
             if p.get("org_id"):
                 kb._by_org.setdefault(p["org_id"], set()).add(rid)
-            kb.sparse.add(rid, text_of(p))
+            if not kb._kw_device:
+                kb.sparse.add(rid, text_of(p))
+        if kb._kw_device and kb._props:     # one device append for the whole store
+            rids = list(kb._props)
+            kb.sparse.add_many(rids, [text_of(kb._props[r]) for r in rids],
+                               np.array([kb._code(kb._user_code, kb._props[r].get("user_id"), False) for r in rids], np.int32),
+                               np.array([kb._code(kb._org_code, kb._props[r].get("org_id"), False) for r in rids], np.int32))
         return kb
 
     # ------------------------------------------------------------------ deletes / counts
@@ -444,10 +498,13 @@ class KnowledgeBase:
                 gen = self.mutations
                 keys = [self._id2key.get(rid) for rid in ids]
                 self.index.remove(np.array(ids, dtype=np.int64))
+                if self._kw_device:
+                    self.sparse.remove_many(ids)
                 for rid in ids:
                     p = self._props.pop(rid)
                     self._unindex(rid, p)
-                    self.sparse.remove(rid)
+                    if not self._kw_device:
+                        self.sparse.remove(rid)
                     self._key2id.pop(self._id2key.pop(rid, None), None)
                 self.mutations += len(ids)
                 self._log({"op": "del", "gen": gen, "keys": [k for k in keys if k]})

@@ -227,6 +227,56 @@ int aur_dev_free(int32_t device, void* p);
 int aur_memcpy_h2d(int32_t device, void* dst_dev, const void* src_host, uint64_t bytes);
 int aur_memcpy_d2h(int32_t device, void* dst_host, const void* src_dev, uint64_t bytes);
 
+/* ------------------------------------------------------------------ BM25 keyword store
+ * Replaces the BM25 leg of collection.query.hybrid (weaviate_client.py:252-259), which Weaviate runs on its own host
+ * cores next to the vector leg.  A standalone store on one GPU, keyed by the same caller ids and tenant codes as an
+ * aur_index: a forward index of (term id, tf) postings per document, term ids chosen by the caller (aurora_b200.bm25
+ * keeps the vocabulary).  Scores are bm25.BM25Index.search's loop path bit for bit: k1 = 1.2, b = 0.75,
+ * idf = log(1 + (N - df + 0.5) / (df + 0.5)), avgdl = total_len / N (1 when total_len is 0), N / df / total_len over
+ * every live document of the store, a document's score summed in the order its query lists the terms, fp64.  Results are
+ * ordered (score desc, id asc), only documents with a matching term appear, padding is id -1 / score -INFINITY.
+ * Append-only with a published prefix like aur_index; a search scores exactly the prefix whose statistics it took
+ * (*snapshot_rows_out).  Upserts of existing ids, removes, posting growth and compaction wait for searches in flight. */
+typedef struct aur_kw aur_kw;
+
+typedef struct aur_kw_stats {
+  int64_t docs;               /* rows ever appended (including tombstones)          */
+  int64_t live;               /* documents visible to search (N)                    */
+  int64_t capacity;           /* document rows reserved at open                     */
+  int64_t postings_used;      /* postings of the appended rows                      */
+  int64_t postings_allocated; /* posting slots in HBM (grows on demand)             */
+  int64_t total_len;          /* tokens over the live documents                     */
+  int32_t last_launches;      /* kernels launched by the last search                */
+  float   last_ms;            /* device time of the last search (uploads included)  */
+  int32_t last_terms;         /* most distinct live terms one launch of it scored   */
+  int32_t last_spilled;       /* its launches whose per-warp term table did not fit shared
+                                 memory and lived in global memory instead          */
+} aur_kw_stats;
+
+/* Lifecycle; the keyword half of _ensure_collection (weaviate_client.py:35-133).  postings_capacity 0 = 2^20 to start
+ * with.  Without a device: AUR_ERR_NO_DEVICE. */
+int aur_kw_open(int32_t device, int64_t doc_capacity, int64_t postings_capacity, aur_kw** out);
+int aur_kw_close(aur_kw* kw);
+/* Upsert n documents (the text side of add_object, weaviate_client.py:167-186): document i has postings
+ * [offsets[i], offsets[i + 1]) of term_ids / tfs, term ids strictly increasing (0 .. 2^28 - 1), tf >= 1; an existing id
+ * loses its old row (weaviate_client.py:172).  user_codes / org_codes as for aur_add (NULL: user 0, org -1). */
+int aur_kw_add(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes,
+               const int32_t* term_ids, const int32_t* tfs, const int64_t* offsets, int64_t n);
+/* Deletes (collection.data.delete_many, weaviate_client.py:309): *removed (nullable) = ids that were live. */
+int aur_kw_remove(aur_kw* kw, const int64_t* ids, int64_t n, int64_t* removed);
+/* Stable compaction of the tombstones, as aur_compact; *reclaimed (nullable) = rows freed. */
+int aur_kw_compact(aur_kw* kw, int64_t* reclaimed);
+int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out);
+/* The BM25 leg of collection.query.hybrid (weaviate_client.py:252-259), batched: query q's term ids are
+ * q_terms[q_offsets[q] .. q_offsets[q + 1]) in summation order (repeats and unknown ids are ignored); top-k each,
+ * 1 <= k <= 128 (larger: AUR_ERR_UNSUPPORTED).  q_user / q_org: per-query tenant scope as in aur_search
+ * (weaviate_client.py:244-249; NULL q_user = unscoped).  allow_ids (n_allow of them) restrict every query of the batch to
+ * those documents, as aur_search_subset; NULL = no restriction, n_allow = 0 with a non-NULL pointer = nothing.
+ * scores_out / ids_out [nq * k]; *snapshot_rows_out (nullable) = appended rows the search saw. */
+int aur_kw_search(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k,
+                  const int32_t* q_user, const int32_t* q_org, const int64_t* allow_ids, int64_t n_allow,
+                  double* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out);
+
 /* ------------------------------------------------------------------ text encoder
  * Replaces the text2vec-transformers sidecar: EmbeddingClient.embed / embed_batch
  * (server/services/correlation/embedding_client.py:39-78, POST {base}/vectors) and the
