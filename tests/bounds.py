@@ -87,6 +87,31 @@ def gemm_reference(A, W, bias, resid=None, epi: int = 0):
     return ref, bound + 2.0 ** -8 * np.abs(ref)
 
 
+def gemm_schedule(m: int, n: int, k: int, cta_group: int, sm_count: int):
+    """gemm_tc.cu's persistent schedule for an aur_debug_gemm call: (bn, stages, tiles, groups, k_blocks).  The N tile
+    is 256 when it divides n, else 128 (aur_debug_gemm); the TMA ring has GemmSmem::kStages slots of one 64-wide
+    k-block each; tiles are (128 cta_group) x bn; launch_one starts min(tiles, sm_count / cta_group) groups of
+    cta_group CTAs, and group g takes tiles g, g + groups, ..."""
+    bn = 256 if n % 256 == 0 else 128
+    stages = min(8, (192 * 1024) // (128 * 64 * 2 + bn * 64 * 2))
+    tiles = -(-m // (128 * cta_group)) * (n // bn)
+    return bn, stages, tiles, min(tiles, sm_count // cta_group), k // 64
+
+
+# ------------------------------------------------------------------------------------------ encoder hidden states
+HIDDEN_ULPS = 8          # per-token hidden states, one layer against the bf16-store oracle
+
+
+def bf16_ulps(got, ref, floor=None):
+    """|got - ref| in bf16 ulps (2^(floor(log2 s) - 7)) of s = max(|ref|, floor); floor defaults to the RMS of the
+    element's token row.  A LayerNorm output inherits the error of its input's bf16 stores, whose ulps are set by
+    the row's magnitude, not by the element's, so small elements of an O(1) row are measured against the row."""
+    got, ref = _f64(got), _f64(ref)
+    if floor is None:
+        floor = np.sqrt((ref * ref).mean(axis=1, keepdims=True))
+    return np.abs(got - ref) / 2.0 ** (np.floor(np.log2(np.maximum(np.abs(ref), floor))) - 7)
+
+
 # -------------------------------------------------------------------------------------------------- attention
 def attention_reference(qkv, cu, heads: int, hidden: int, head_dim: int = 64):
     """Softmax(q k^T / sqrt(head_dim)) v per packed sequence and head, fp64.  Returns (ref, bound) [tokens, hidden].
@@ -116,14 +141,16 @@ def attention_reference(qkv, cu, heads: int, hidden: int, head_dim: int = 64):
 
 
 # ---------------------------------------------------------------------------------- inputs shared by CPU and GPU
-def gemm_inputs(m: int, n: int, k: int, seed: int, spread: bool = False, big_resid: bool = False):
-    """bf16-valued A [m, k], W [n, k], resid [m, n] and fp32 bias.  spread: a small product and a bias spanning
-    [-6, 6], so GELU inputs reach both tails of the erf approximation; big_resid: a residual 2^10 times the product."""
+def gemm_inputs(m: int, n: int, k: int, seed: int, spread: bool = False, big_resid: bool = False,
+                with_resid: bool = True):
+    """bf16-valued A [m, k], W [n, k], resid [m, n] (None unless with_resid) and fp32 bias.  spread: a small product
+    and a bias spanning [-6, 6], so GELU inputs reach both tails of the erf approximation; big_resid: a residual 2^10
+    times the product."""
     rng = np.random.default_rng(seed)
     a = _bf16(rng.standard_normal((m, k)))
     w = _bf16(rng.standard_normal((n, k)) / np.sqrt(k) * (0.05 if spread else 1.0))
     bias = (rng.uniform(-6, 6, n) if spread else rng.standard_normal(n)).astype(np.float32)
-    resid = _bf16(rng.standard_normal((m, n)) * (1024.0 if big_resid else 1.0))
+    resid = _bf16(rng.standard_normal((m, n)) * (1024.0 if big_resid else 1.0)) if with_resid else None
     return a, w, bias, resid
 
 

@@ -5,6 +5,7 @@ deliberately broken emulation -- a bug of the kind a kernel rewrite introduces -
 import numpy as np
 import pytest
 
+from oracle import bert_encoder as B
 from oracle.cosine_topk import bf16_bits_to_f32, f32_to_bf16_bits, round_to_bf16
 from tests import bounds as BD
 
@@ -36,11 +37,42 @@ def _gelu_tanh_f32(x):
     return F32(0.5) * x * (F32(1) + np.tanh(F32(0.7978845608) * (x + F32(0.044715) * x * x * x)))
 
 
-def emulate_gemm(a, w, bias, resid, epi, mutant=None):
+def _scheduled_product(a, w, groups, bm, bn, stages, mutant=None):
+    """a . w^T as gemm_tc_kernel's persistent schedule computes it: (bm x bn) tiles in row-major tile order, group g
+    takes tiles g, g + groups, ... and accumulates each in fp32 over the 64-wide k-blocks it streams through a ring of
+    ``stages`` slots.  Mutants: acc_carry (the accumulator is not zeroed between a group's tiles); stale_kblock (one
+    k-block of group 0's second tile reads its slot one ring lap stale: the block loaded ``stages`` loads earlier)."""
+    m, k = a.shape
+    a = np.concatenate([a, np.zeros((-m % bm, k), F32)])          # the zero rows a partial last row of tiles covers
+    m_tiles, n_tiles, kb = a.shape[0] // bm, w.shape[0] // bn, k // 64
+    out = np.empty((a.shape[0], w.shape[0]), F32)
+    for g in range(groups):
+        loads, d = [], None                                        # (rows, cols, k-block) of each load, in ring order
+        for i, t in enumerate(range(g, m_tiles * n_tiles, groups)):
+            r = slice(t // n_tiles * bm, t // n_tiles * bm + bm)
+            c = slice(t % n_tiles * bn, t % n_tiles * bn + bn)
+            blocks = [(r, c, j) for j in range(kb)]
+            read = list(blocks)
+            if mutant == "stale_kblock" and g == 0 and i == 1:
+                j = max(0, stages - kb)
+                assert j < kb, "the ring never wraps inside the second tile"
+                read[j] = (loads + blocks)[len(loads) + j - stages]
+            acc = d if (mutant == "acc_carry" and d is not None) else np.zeros((bm, bn), F32)
+            for rr, cc, j in read:
+                acc = acc + a[rr, 64 * j:64 * j + 64] @ w[cc, 64 * j:64 * j + 64].T
+            out[r, c] = d = acc
+            loads += blocks
+    return out[:m]
+
+
+def emulate_gemm(a, w, bias, resid, epi, mutant=None, groups=None, bm=256, bn=256, stages=4):
+    """gemm_tc.cu in numpy; groups: run its persistent tile schedule (``_scheduled_product``) over that many groups
+    of (bm x bn) tiles with a ``stages``-slot ring, instead of one product."""
     a, w = a.astype(F32), w.astype(F32)
     if mutant == "drop_last_k16":
         a, w = a[:, :-16], w[:, :-16]
-    x = (a @ w.T) + (np.roll(bias, -1) if mutant == "bias_shift" else bias).astype(F32)
+    prod = a @ w.T if groups is None else _scheduled_product(a, w, groups, bm, bn, stages, mutant)
+    x = prod + (np.roll(bias, -1) if mutant == "bias_shift" else bias).astype(F32)
     if epi == 1:
         x = _gelu_tanh_f32(x) if mutant == "tanh_gelu" else _gelu_erf_f32(x)
     if epi == 2:
@@ -74,6 +106,33 @@ def test_gemm_emulation_within_bound(case):
                                          ("rtz_store", "bias"), ("rtz_store", "resid_large")])
 def test_gemm_mutant_fails_bound(mutant, case):
     assert _gemm(case, mutant) > 1.0
+
+
+SCHEDULE_CASES = {   # name: (m, n, k, epi, cta_group, sm_count); every group takes 3 tiles plus a partial last round
+    "pair_bn256": (1263, 512, 320, 0, 2, 6),      # 10 tiles over 3 groups, 5 k-blocks in a 4-slot ring
+    "single_bn128": (1115, 384, 448, 1, 1, 8),    # 27 tiles over 8 groups, 7 k-blocks in a 6-slot ring
+    "pair_resid": (1436, 768, 1088, 2, 2, 10),    # 18 tiles over 5 groups, 17 k-blocks in a 4-slot ring
+}
+
+
+def _scheduled_gemm(case, mutant=None):
+    m, n, k, epi, g, sm = SCHEDULE_CASES[case]
+    bn, stages, tiles, groups, kb = BD.gemm_schedule(m, n, k, g, sm)
+    assert tiles // groups >= 3 and 0 < tiles % groups and kb % stages
+    a, w, bias, resid = BD.gemm_inputs(m, n, k, seed=m + n + k)
+    ref, bound = BD.gemm_reference(a, w, bias, resid, epi)
+    return BD.ratio(emulate_gemm(a, w, bias, resid, epi, mutant, groups, 128 * g, bn, stages), ref, bound)
+
+
+@pytest.mark.parametrize("case", sorted(SCHEDULE_CASES))
+def test_scheduled_gemm_emulation_within_bound(case):
+    assert _scheduled_gemm(case) <= 1.0
+
+
+@pytest.mark.parametrize("mutant", ["acc_carry", "stale_kblock"])
+@pytest.mark.parametrize("case", sorted(SCHEDULE_CASES))
+def test_scheduled_gemm_mutant_fails_bound(mutant, case):
+    assert _scheduled_gemm(case, mutant) > 1.0
 
 
 # -------------------------------------------------------------------------------------------------- attention
@@ -178,6 +237,61 @@ def test_sim_emulation_within_bound(dim):
 @pytest.mark.parametrize("dim", SIM_DIMS)
 def test_sim_mutant_fails_bound(mutant, dim):
     assert _sim(dim, mutant) > 1.0
+
+
+# ------------------------------------------------------------------------------------- encoder, one layer at a time
+TF_CFG = B.BertConfig(hidden=128, layers=4, heads=2, inter=256, vocab=120, max_pos=512, pool="cls")
+MUTANT_LAYER = 2
+
+
+def _mutated_gelu(mutant):
+    """B.gelu with one defect in the first sequence of at least 129 tokens: ``tile`` copies the 128 x 128 block of
+    GELU outputs at (0, 0) from its neighbour at (0, 128); ``row`` gives the middle token the GELU row of the token
+    before it."""
+    gelu, done = B.gelu, []
+
+    def g(x):
+        y = gelu(x)
+        if not done and len(y) > 128:
+            if mutant == "tile":
+                y[:128, :128] = y[:128, 128:256]
+            else:
+                y[len(y) // 2] = y[len(y) // 2 - 1]
+            done.append(True)
+        return y
+    return g
+
+
+def _teacher_forced_worst(monkeypatch=None, mutant=None):
+    """Worst bf16 ulps (BD.bf16_ulps) per layer of the fp32 bf16-store emulation of the encoder, each layer checked
+    against the fp64 bf16-store oracle of that layer run on the emulation's own output of the layer before (the
+    first layer on the oracle's own embedding)."""
+    w = B.init_weights(TF_CFG, seed=7, bf16=True)
+    tok, cu = B.synth_batch(TF_CFG, 6, 29, mean_len=200, std_len=120, min_len=1, max_len=512)
+    x32 = B.embed_tokens(TF_CFG, w, tok, cu, F32, bf16_stores=True)
+    x_in = B.embed_tokens(TF_CFG, w, tok, cu, bf16_stores=True)
+    worst = []
+    for l in range(TF_CFG.layers):
+        ref = B.encoder_layer(TF_CFG, w, l, x_in, cu, bf16_stores=True)
+        if mutant and l == MUTANT_LAYER:
+            monkeypatch.setattr(B, "gelu", _mutated_gelu(mutant))
+        x32 = B.encoder_layer(TF_CFG, w, l, x32, cu, F32, bf16_stores=True)
+        if mutant and l == MUTANT_LAYER:
+            monkeypatch.undo()
+        worst.append(float(BD.bf16_ulps(x32, ref).max()))
+        x_in = x32
+    print(f"teacher-forced emulation, mutant {mutant}: worst ulps per layer {[round(e, 2) for e in worst]}")
+    return worst
+
+
+def test_teacher_forced_emulation_within_hidden_ulps():
+    assert max(_teacher_forced_worst()) <= BD.HIDDEN_ULPS
+
+
+@pytest.mark.parametrize("mutant", ["tile", "row"])
+def test_teacher_forced_mutant_fails_hidden_ulps(mutant, monkeypatch):
+    worst = _teacher_forced_worst(monkeypatch, mutant)
+    assert worst[MUTANT_LAYER] > BD.HIDDEN_ULPS
 
 
 def test_bf16_helpers_round_to_nearest_and_toward_zero():
