@@ -24,10 +24,11 @@ TC_QUERY_ROWS = 64   # queries per CTA of the tensor-core kernel (kTcQRows, csrc
 EXPORTS = [
     "aur_abi_version", "aur_last_error", "aur_device_count", "aur_open", "aur_close", "aur_get_stats",
     "aur_set_option", "aur_sync", "aur_add", "aur_add_dev", "aur_export", "aur_read_rows", "aur_compact", "aur_remove", "aur_search", "aur_search_ex", "aur_search_subset", "aur_search_dev",
-    "aur_merge_topk_dev", "aur_merge_topk_packed_dev", "aur_merge_topk_host", "aur_exchange_create", "aur_exchange_connect", "aur_exchange_close",
+    "aur_merge_topk_dev", "aur_merge_topk_packed_dev", "aur_merge_topk_host", "aur_merge_topk_host_f64", "aur_exchange_create", "aur_exchange_connect", "aur_exchange_close",
     "aur_exchange_status", "aur_search_exchange_dev", "aur_cosine_pairs", "aur_dev_malloc", "aur_dev_free", "aur_memcpy_h2d", "aur_memcpy_d2h",
     "aur_debug_tc_scores",
     "aur_kw_open", "aur_kw_close", "aur_kw_add", "aur_kw_remove", "aur_kw_compact", "aur_kw_get_stats", "aur_kw_search",
+    "aur_kw_search_multi",
     "aur_encoder_open", "aur_encoder_close", "aur_encoder_load", "aur_encode", "aur_encode_append",
     "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
     "aur_tokenize", "aur_encode_text_append", "aur_debug_gemm", "aur_debug_attention", "aur_debug_encoder_hidden",
@@ -110,6 +111,7 @@ def load():
         "aur_search_dev": (C.c_int, [vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]),
         "aur_merge_topk_dev": (C.c_int, [i32, vp, vp, i32, i32, i32, vp, vp, vp, vp]),
         "aur_merge_topk_host": (C.c_int, [vp, vp, i32, i32, i32, i32, vp, vp]),
+        "aur_merge_topk_host_f64": (C.c_int, [vp, vp, i32, i32, i32, i32, vp, vp]),
         "aur_merge_topk_packed_dev": (C.c_int, [i32, vp, i32, i32, i32, vp, vp, vp, vp]),
         "aur_exchange_create": (C.c_int, [i32, i32, i32, i32, i32, C.POINTER(vp), vp]),
         "aur_exchange_connect": (C.c_int, [vp, vp]),
@@ -129,6 +131,7 @@ def load():
         "aur_kw_compact": (C.c_int, [vp, C.POINTER(i64)]),
         "aur_kw_get_stats": (C.c_int, [vp, C.POINTER(AurKwStats)]),
         "aur_kw_search": (C.c_int, [vp, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, C.POINTER(i64)]),
+        "aur_kw_search_multi": (C.c_int, [vp, i32, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, vp]),
         "aur_encoder_open": (C.c_int, [C.POINTER(AurEncoderConfig), C.POINTER(vp)]),
         "aur_encoder_close": (C.c_int, [vp]),
         "aur_encoder_load": (C.c_int, [vp, C.c_char_p, vp, i64]),

@@ -19,6 +19,9 @@
 // term up in the launch's term table and parks the row's contribution per unique term; then every lane sums its
 // queries' terms in their order.  Selection is exact on (fp64 score desc, id asc) throughout: per-block candidate
 // buffers pruned by the block's own k-th best, sorted lists per block, then sorted folds down to one list per query.
+// aur_kw_search_multi runs the same search over several stores (one per GPU) as one corpus: N, df and total_len are
+// summed over the stores' snapshots, every store scores its own prefix with the resulting idf / avgdl, and the per-store
+// lists are merged on the host (DESIGN.md section 10, "Sharded store").
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
@@ -50,6 +53,7 @@ constexpr int kKwBufCap = 256;            // candidate buffer per (block, query)
 constexpr int kKwQBlock = 256;            // queries per launch
 constexpr int kKwFoldCap = 2048;          // entries one fold block sorts
 constexpr int64_t kKwMaxTerm = int64_t(1) << 28;
+constexpr int kKwMaxStores = 64;         // stores one aur_kw_search_multi call takes
 
 #define KW_TRY(expr)                                                                                             \
   do {                                                                                                           \
@@ -388,6 +392,281 @@ int grow_postings(aur_kw* kw, int64_t need) {
   return AUR_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------- search
+// One search, over one store or several stores taken as one corpus, in the steps both entry points share: every store's
+// shared lock (in address order), a snapshot of each prefix and its statistics, the query blocks' launch tables built
+// once from the summed statistics, every store's passes enqueued on its own device and stream, then each store's top-k
+// collected.
+
+struct KwQuery {   // the arguments of one search (aur_kw_search)
+  const int32_t* terms; const int64_t* off; int32_t nq, k;
+  const int32_t* user; const int32_t* org; const int64_t* allow; int64_t n_allow;
+};
+
+int kw_check_query(const KwQuery& q, const double* scores_out, const int64_t* ids_out) {
+  if (!q.off || !scores_out || !ids_out) return report_error(AUR_ERR_INVALID, "null argument");
+  if (q.nq <= 0 || q.k <= 0) return report_error(AUR_ERR_INVALID, "nq and k must be positive");
+  if (q.k > kMaxK) return report_error(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
+  if (q.off[0] != 0) return report_error(AUR_ERR_INVALID, "q_offsets[0] must be 0");
+  for (int32_t i = 0; i < q.nq; ++i) if (q.off[i + 1] < q.off[i]) return report_error(AUR_ERR_INVALID, "q_offsets must be non-decreasing");
+  if (q.off[q.nq] > 0 && !q.terms) return report_error(AUR_ERR_INVALID, "q_terms is required");
+  if (q.n_allow < 0 || (q.n_allow > 0 && !q.allow)) return report_error(AUR_ERR_INVALID, "allow_ids / n_allow");
+  return AUR_OK;
+}
+
+struct KwSnap { int64_t n_rows = 0, N = 0, total_len = 0; std::vector<int64_t> udf; };
+
+// The published prefix and its statistics, df of the batch's distinct terms uniq, in one read.
+void kw_snapshot(aur_kw* kw, const std::vector<int32_t>& uniq, KwSnap* s) {
+  std::lock_guard<std::mutex> st(kw->mu_stat);
+  s->n_rows = kw->rows_pub; s->N = kw->n_live; s->total_len = kw->total_len;
+  s->udf.assign(uniq.size(), 0);
+  for (size_t i = 0; i < uniq.size(); ++i)
+    s->udf[i] = (uniq[i] >= 0 && uniq[i] < static_cast<int32_t>(kw->df.size())) ? kw->df[static_cast<size_t>(uniq[i])] : 0;
+}
+
+// One launch's query side, the same on every store: idf | hkey | hval | qoff | slot | q_user | q_org in one upload.
+struct KwBlock {
+  int q0 = 0, nqb = 0, nu = 0, hcap = 0;   // nu = 0: no query of the block has a live term
+  size_t b_hk = 0, b_hv = 0, b_qo = 0, b_sl = 0, b_qu = 0, b_qg = 0;
+  std::vector<unsigned char> tab;
+};
+
+// idf of every term with a live posting somewhere (N and udf: the corpus totals), then one table per kKwQBlock queries:
+// the block's unique terms in an open-addressing hash, every query's terms as unique indices in summation order.
+void kw_plan(const KwQuery& q, const std::vector<int32_t>& uniq, const std::vector<int64_t>& udf, int64_t N,
+             std::vector<KwBlock>* blocks) {
+  std::unordered_map<int32_t, double> idf;   // terms with a live posting (the loop path skips the others)
+  for (size_t i = 0; i < uniq.size(); ++i)
+    if (udf[i] > 0)
+      idf[uniq[i]] = std::log(1.0 + (static_cast<double>(N - udf[i]) + 0.5) / (static_cast<double>(udf[i]) + 0.5));
+  for (int32_t q0 = 0; q0 < q.nq; q0 += kKwQBlock) {
+    KwBlock b;
+    b.q0 = q0;
+    b.nqb = std::min(kKwQBlock, q.nq - q0);
+    const int nqb = b.nqb;
+    std::vector<int32_t> ukeys;
+    std::unordered_map<int32_t, int32_t> uidx;
+    std::vector<int32_t> qoff(static_cast<size_t>(nqb) + 1, 0), slot;
+    for (int i = 0; i < nqb; ++i) {
+      std::vector<int32_t> seen;
+      for (int64_t j = q.off[q0 + i]; j < q.off[q0 + i + 1]; ++j) {
+        const int32_t t = q.terms[j];
+        if (!idf.count(t) || std::find(seen.begin(), seen.end(), t) != seen.end()) continue;   // no live posting / repeated
+        seen.push_back(t);
+        auto it = uidx.find(t);
+        if (it == uidx.end()) { it = uidx.emplace(t, static_cast<int32_t>(ukeys.size())).first; ukeys.push_back(t); }
+        slot.push_back(it->second);
+      }
+      qoff[static_cast<size_t>(i) + 1] = static_cast<int32_t>(slot.size());
+    }
+    const int nu = b.nu = static_cast<int>(ukeys.size());
+    if (nu == 0) { blocks->push_back(std::move(b)); continue; }
+    int hcap = 16;
+    while (hcap < 2 * nu) hcap <<= 1;
+    b.hcap = hcap;
+    std::vector<int32_t> hkey(static_cast<size_t>(hcap), -1), hval(static_cast<size_t>(hcap), -1);
+    for (int u = 0; u < nu; ++u) {
+      uint32_t h = (static_cast<uint32_t>(ukeys[static_cast<size_t>(u)]) * 2654435761u) & static_cast<uint32_t>(hcap - 1);
+      while (hkey[h] >= 0) h = (h + 1) & static_cast<uint32_t>(hcap - 1);
+      hkey[h] = ukeys[static_cast<size_t>(u)]; hval[h] = u;
+    }
+    std::vector<double> uidf(static_cast<size_t>(nu));
+    for (int u = 0; u < nu; ++u) uidf[static_cast<size_t>(u)] = idf[ukeys[static_cast<size_t>(u)]];
+    b.b_hk = 8 * static_cast<size_t>(nu); b.b_hv = b.b_hk + 4 * static_cast<size_t>(hcap);
+    b.b_qo = b.b_hv + 4 * static_cast<size_t>(hcap); b.b_sl = b.b_qo + 4 * qoff.size();
+    b.b_qu = b.b_sl + 4 * std::max<size_t>(slot.size(), 1); b.b_qg = b.b_qu + 4 * static_cast<size_t>(nqb);
+    b.tab.assign(b.b_qg + 4 * static_cast<size_t>(nqb), 0);
+    unsigned char* tab = b.tab.data();
+    memcpy(tab, uidf.data(), 8 * static_cast<size_t>(nu));
+    memcpy(tab + b.b_hk, hkey.data(), 4 * static_cast<size_t>(hcap));
+    memcpy(tab + b.b_hv, hval.data(), 4 * static_cast<size_t>(hcap));
+    memcpy(tab + b.b_qo, qoff.data(), 4 * qoff.size());
+    if (!slot.empty()) memcpy(tab + b.b_sl, slot.data(), 4 * slot.size());
+    if (q.user) memcpy(tab + b.b_qu, q.user + q0, 4 * static_cast<size_t>(nqb));
+    std::vector<int32_t> qorg(static_cast<size_t>(nqb), -1);
+    if (q.org) std::copy(q.org + q0, q.org + q0 + nqb, qorg.begin());
+    memcpy(tab + b.b_qg, qorg.data(), 4 * static_cast<size_t>(nqb));
+    blocks->push_back(std::move(b));
+  }
+}
+
+// Enqueue one store's part of the search on c's stream: allow-list flags, then per block the table upload, the scoring
+// pass over the store's prefix n_rows and the folds into c's [nq][k] output.  Nothing waits.
+int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>& blocks, int64_t n_rows, int64_t N,
+              double avgdl) {
+  KW_TRY(cudaSetDevice(kw->device));
+  cudaStream_t s = c->stream;
+  const int k = q.k;
+  c->launches = 0; c->terms = 0; c->spilled = 0;
+  KW_TRY(cudaEventRecord(c->ev0, s));
+  const uint8_t* d_allow = nullptr;
+  if (q.allow) {
+    std::vector<int32_t> rows;
+    {
+      std::lock_guard<std::mutex> st(kw->mu_stat);    // writers change id2row under it (and tombstone only exclusively)
+      for (int64_t i = 0; i < q.n_allow; ++i) {
+        auto it = kw->id2row.find(q.allow[i]);
+        if (it != kw->id2row.end() && it->second < n_rows) rows.push_back(static_cast<int32_t>(it->second));
+      }
+    }
+    KW_TRY(c->allow.reserve(static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
+    KW_TRY(c->allow_rows.reserve(std::max<size_t>(rows.size(), 1)));
+    KW_TRY(cudaMemsetAsync(c->allow.p, 0, static_cast<size_t>(std::max<int64_t>(n_rows, 1)), s));
+    if (!rows.empty()) {
+      KW_TRY(cudaMemcpyAsync(c->allow_rows.p, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
+      kw_scatter_flag<<<static_cast<unsigned>((rows.size() + 255) / 256), 256, 0, s>>>(c->allow_rows.p, static_cast<int64_t>(rows.size()), c->allow.p, 1);
+      KW_TRY(cudaGetLastError());
+      c->launches += 1;
+    }
+    d_allow = c->allow.p;
+  }
+  const size_t nout = static_cast<size_t>(q.nq) * k;
+  KW_TRY(c->out_s.reserve(nout));
+  KW_TRY(c->out_ids.reserve(nout));
+  for (const KwBlock& b : blocks) {
+    const int nqb = b.nqb, nu = b.nu;
+    double* o_s = c->out_s.p + static_cast<size_t>(b.q0) * k;
+    int64_t* o_i = c->out_ids.p + static_cast<size_t>(b.q0) * k;
+    if (nu == 0 || n_rows == 0 || N == 0) {   // nothing can match: padding only
+      std::vector<double> ps(static_cast<size_t>(nqb) * k, -INFINITY);
+      std::vector<int64_t> pi(static_cast<size_t>(nqb) * k, -1);
+      KW_TRY(cudaMemcpyAsync(o_s, ps.data(), ps.size() * 8, cudaMemcpyHostToDevice, s));
+      KW_TRY(cudaMemcpyAsync(o_i, pi.data(), pi.size() * 8, cudaMemcpyHostToDevice, s));
+      continue;
+    }
+    KW_TRY(c->tab.reserve(b.tab.size()));
+    KW_TRY(cudaMemcpyAsync(c->tab.p, b.tab.data(), b.tab.size(), cudaMemcpyHostToDevice, s));   // pageable: staged before return
+    // geometry: blocks own contiguous row ranges of whole rounds
+    const int64_t rounds = (n_rows + kKwRoundRows - 1) / kKwRoundRows;
+    const int64_t grid = std::max<int64_t>(1, std::min<int64_t>(2 * kw->sm_count, rounds));
+    const int64_t rpb = (rounds + grid - 1) / grid * kKwRoundRows;
+    const int g = static_cast<int>((n_rows + rpb - 1) / rpb);
+    const int ksel = k;
+    size_t smem = static_cast<size_t>(nqb) * sizeof(Cand) + kKwWarps * kKwBufCap * sizeof(Cand) + 4 * static_cast<size_t>(nqb);
+    smem = (smem + 15) & ~size_t(15);
+    const size_t cval_smem = static_cast<size_t>(kKwWarps) * nu * 8;
+    const bool in_smem = smem + cval_smem <= kw->smem_optin;
+    c->terms = std::max(c->terms, nu);
+    if (!in_smem) ++c->spilled;
+    if (in_smem) smem += cval_smem;
+    else KW_TRY(c->cval.reserve(static_cast<size_t>(g) * kKwWarps * nu));
+    KW_TRY(c->buf.reserve(static_cast<size_t>(g) * nqb * kKwBufCap));
+    KW_TRY(c->lists_a.reserve(static_cast<size_t>(nqb) * g * ksel));
+    KwParams p{};
+    p.off = kw->d_off; p.post = kw->d_post; p.len = kw->d_len; p.ids = kw->d_ids; p.user = kw->d_user; p.org = kw->d_org;
+    p.live = kw->d_live; p.allow = d_allow; p.n_rows = n_rows;
+    p.idf = reinterpret_cast<const double*>(c->tab.p); p.n_uniq = nu;
+    p.hkey = reinterpret_cast<const int32_t*>(c->tab.p + b.b_hk); p.hval = reinterpret_cast<const int32_t*>(c->tab.p + b.b_hv);
+    p.hmask = b.hcap - 1;
+    p.q_off = reinterpret_cast<const int32_t*>(c->tab.p + b.b_qo); p.slot_u = reinterpret_cast<const int32_t*>(c->tab.p + b.b_sl);
+    p.q_user = q.user ? reinterpret_cast<const int32_t*>(c->tab.p + b.b_qu) : nullptr;
+    p.q_org = q.user ? reinterpret_cast<const int32_t*>(c->tab.p + b.b_qg) : nullptr;
+    p.nq = nqb; p.ksel = ksel; p.avgdl = avgdl;
+    p.cval_global = in_smem ? nullptr : c->cval.p;
+    p.buf = c->buf.p; p.lists = c->lists_a.p; p.rows_per_block = rpb;
+    kw_score_kernel<<<g, kKwThreads, smem, s>>>(p, in_smem ? 1 : 0);
+    KW_TRY(cudaGetLastError());
+    c->launches += 1;
+    // fold the per-block lists until one sorted list per query remains
+    int n_lists = g;
+    Cand* cur = c->lists_a.p;
+    bool in_a = true;
+    const int group = std::max(1, kKwFoldCap / ksel);
+    for (;;) {
+      const int n_groups = (n_lists + group - 1) / group;
+      const int gl = std::min(group, n_lists);
+      int sort_n = 1;
+      while (sort_n < gl * ksel) sort_n <<= 1;
+      const size_t fsmem = static_cast<size_t>(sort_n) * sizeof(Cand);
+      if (n_groups == 1) {
+        kw_fold_kernel<<<dim3(1, nqb), 256, fsmem, s>>>(cur, n_lists, ksel, group, sort_n, nullptr, o_s, o_i, k);
+        KW_TRY(cudaGetLastError());
+        c->launches += 1;
+        break;
+      }
+      KwBuf<Cand>& dst = in_a ? c->lists_b : c->lists_a;
+      KW_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
+      kw_fold_kernel<<<dim3(n_groups, nqb), 256, fsmem, s>>>(cur, n_lists, ksel, group, sort_n, dst.p, nullptr, nullptr, k);
+      KW_TRY(cudaGetLastError());
+      c->launches += 1;
+      cur = dst.p; n_lists = n_groups; in_a = !in_a;
+    }
+  }
+  KW_TRY(cudaEventRecord(c->ev1, s));
+  return AUR_OK;
+}
+
+// Wait for one store's part, copy its [nq][k] lists to the host and publish its last_* statistics.
+int kw_collect(aur_kw* kw, KwCtx* c, const KwQuery& q, double* scores_out, int64_t* ids_out) {
+  KW_TRY(cudaSetDevice(kw->device));
+  cudaStream_t s = c->stream;
+  const size_t nout = static_cast<size_t>(q.nq) * q.k;
+  KW_TRY(cudaMemcpyAsync(scores_out, c->out_s.p, nout * 8, cudaMemcpyDeviceToHost, s));
+  KW_TRY(cudaMemcpyAsync(ids_out, c->out_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
+  KW_TRY(cudaStreamSynchronize(s));
+  float ms = 0.f;
+  KW_TRY(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+  std::lock_guard<std::mutex> lk(kw->mu_pool);
+  kw->last_launches = c->launches; kw->last_ms = ms;
+  kw->last_terms = c->terms; kw->last_spilled = c->spilled;
+  return AUR_OK;
+}
+
+// Search stores[0 .. n) (distinct, arguments checked) as one corpus: store s's top-k lists land in
+// out_s / out_i + s * nq * k, scored with the idf and avgdl of the union of the snapshots.
+int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out_s, int64_t* out_i, int64_t* snapshot_rows) {
+  // shared locks for the whole search, in one order (by address) so that searches over overlapping store sets cannot
+  // deadlock behind a waiting writer
+  std::vector<aur_kw*> order(stores, stores + n);
+  std::sort(order.begin(), order.end(), std::less<aur_kw*>());
+  std::vector<std::shared_lock<std::shared_mutex>> locks;
+  locks.reserve(static_cast<size_t>(n));
+  for (aur_kw* kw : order) locks.emplace_back(kw->rw);
+  // the batch's distinct terms, each store's snapshot, the corpus totals
+  std::vector<int32_t> uniq(q.terms, q.terms + q.off[q.nq]);
+  std::sort(uniq.begin(), uniq.end());
+  uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
+  std::vector<KwSnap> snaps(static_cast<size_t>(n));
+  std::vector<int64_t> udf(uniq.size(), 0);
+  int64_t N = 0, total_len = 0;
+  for (int s = 0; s < n; ++s) {
+    kw_snapshot(stores[s], uniq, &snaps[static_cast<size_t>(s)]);
+    const KwSnap& sn = snaps[static_cast<size_t>(s)];
+    N += sn.N; total_len += sn.total_len;
+    for (size_t i = 0; i < uniq.size(); ++i) udf[i] += sn.udf[i];
+  }
+  const double avgdl = total_len ? static_cast<double>(total_len) / static_cast<double>(N) : 1.0;
+  std::vector<KwBlock> blocks;
+  kw_plan(q, uniq, udf, N, &blocks);
+  // every store's work enqueued before any is waited on; the contexts go back to their pools only once their streams
+  // are idle (also on an error), before the locks are released
+  struct Ctxs {
+    std::vector<std::pair<aur_kw*, KwCtx*>> v;
+    ~Ctxs() {
+      for (auto& e : v) { cudaSetDevice(e.first->device); cudaStreamSynchronize(e.second->stream); kw_ctx_release(e.first, e.second); }
+    }
+  } ctxs;
+  for (int s = 0; s < n; ++s) {
+    aur_kw* kw = stores[s];
+    KW_TRY(cudaSetDevice(kw->device));
+    KwCtx* c = nullptr;
+    int rc = kw_ctx_acquire(kw, &c);
+    if (rc != AUR_OK) return rc;
+    ctxs.v.emplace_back(kw, c);
+    const KwSnap& sn = snaps[static_cast<size_t>(s)];
+    if ((rc = kw_launch(kw, c, q, blocks, sn.n_rows, N, avgdl)) != AUR_OK) return rc;
+  }
+  const size_t nout = static_cast<size_t>(q.nq) * q.k;
+  for (int s = 0; s < n; ++s) {
+    const int rc = kw_collect(stores[s], ctxs.v[static_cast<size_t>(s)].second, q, out_s + s * nout, out_i + s * nout);
+    if (rc != AUR_OK) return rc;
+  }
+  if (snapshot_rows)
+    for (int s = 0; s < n; ++s) snapshot_rows[s] = snaps[static_cast<size_t>(s)].n_rows;
+  return AUR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -640,187 +919,35 @@ int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out) {
 int aur_kw_search(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k, const int32_t* q_user,
                   const int32_t* q_org, const int64_t* allow_ids, int64_t n_allow, double* scores_out, int64_t* ids_out,
                   int64_t* snapshot_rows_out) {
-  if (!kw || !q_offsets || !scores_out || !ids_out) return report_error(AUR_ERR_INVALID, "null argument");
-  if (nq <= 0 || k <= 0) return report_error(AUR_ERR_INVALID, "nq and k must be positive");
-  if (k > kMaxK) return report_error(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
-  if (q_offsets[0] != 0) return report_error(AUR_ERR_INVALID, "q_offsets[0] must be 0");
-  for (int32_t q = 0; q < nq; ++q) if (q_offsets[q + 1] < q_offsets[q]) return report_error(AUR_ERR_INVALID, "q_offsets must be non-decreasing");
-  if (q_offsets[nq] > 0 && !q_terms) return report_error(AUR_ERR_INVALID, "q_terms is required");
-  if (n_allow < 0 || (n_allow > 0 && !allow_ids)) return report_error(AUR_ERR_INVALID, "allow_ids / n_allow");
-  std::shared_lock<std::shared_mutex> rl(kw->rw);
-  KW_TRY(cudaSetDevice(kw->device));
-  // the batch's distinct terms, then one snapshot of the prefix and its statistics
-  std::vector<int32_t> uniq(q_terms, q_terms + q_offsets[nq]);
-  std::sort(uniq.begin(), uniq.end());
-  uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
-  std::vector<int64_t> udf(uniq.size(), 0);
-  int64_t n_rows, N, total_len;
-  {
-    std::lock_guard<std::mutex> st(kw->mu_stat);
-    n_rows = kw->rows_pub; N = kw->n_live; total_len = kw->total_len;
-    for (size_t i = 0; i < uniq.size(); ++i)
-      udf[i] = (uniq[i] >= 0 && uniq[i] < static_cast<int32_t>(kw->df.size())) ? kw->df[static_cast<size_t>(uniq[i])] : 0;
-  }
-  const double avgdl = total_len ? static_cast<double>(total_len) / static_cast<double>(N) : 1.0;
-  std::unordered_map<int32_t, double> idf;   // terms with a live posting (the loop path skips the others)
-  for (size_t i = 0; i < uniq.size(); ++i)
-    if (udf[i] > 0)
-      idf[uniq[i]] = std::log(1.0 + (static_cast<double>(N - udf[i]) + 0.5) / (static_cast<double>(udf[i]) + 0.5));
-  KwCtx* c = nullptr;
-  int rc = kw_ctx_acquire(kw, &c);
+  if (!kw) return report_error(AUR_ERR_INVALID, "null argument");
+  const KwQuery q{q_terms, q_offsets, nq, k, q_user, q_org, allow_ids, n_allow};
+  const int rc = kw_check_query(q, scores_out, ids_out);
   if (rc != AUR_OK) return rc;
-  struct Guard { aur_kw* kw; KwCtx* c; ~Guard() { kw_ctx_release(kw, c); } } guard{kw, c};
-  cudaStream_t s = c->stream;
-  c->launches = 0; c->terms = 0; c->spilled = 0;
-  KW_TRY(cudaEventRecord(c->ev0, s));
-  const uint8_t* d_allow = nullptr;
-  if (allow_ids) {
-    std::vector<int32_t> rows;
-    {
-      std::lock_guard<std::mutex> st(kw->mu_stat);    // writers change id2row under it (and tombstone only exclusively)
-      for (int64_t i = 0; i < n_allow; ++i) {
-        auto it = kw->id2row.find(allow_ids[i]);
-        if (it != kw->id2row.end() && it->second < n_rows) rows.push_back(static_cast<int32_t>(it->second));
-      }
-    }
-    KW_TRY(c->allow.reserve(static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
-    KW_TRY(c->allow_rows.reserve(std::max<size_t>(rows.size(), 1)));
-    KW_TRY(cudaMemsetAsync(c->allow.p, 0, static_cast<size_t>(std::max<int64_t>(n_rows, 1)), s));
-    if (!rows.empty()) {
-      KW_TRY(cudaMemcpyAsync(c->allow_rows.p, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
-      kw_scatter_flag<<<static_cast<unsigned>((rows.size() + 255) / 256), 256, 0, s>>>(c->allow_rows.p, static_cast<int64_t>(rows.size()), c->allow.p, 1);
-      KW_TRY(cudaGetLastError());
-      c->launches += 1;
-    }
-    d_allow = c->allow.p;
-  }
-  const size_t nout = static_cast<size_t>(nq) * k;
-  KW_TRY(c->out_s.reserve(nout));
-  KW_TRY(c->out_ids.reserve(nout));
-  for (int32_t q0 = 0; q0 < nq; q0 += kKwQBlock) {
-    const int nqb = std::min(kKwQBlock, nq - q0);
-    // launch term table: unique terms of this block, open-addressing hash, per-query slot lists in summation order
-    std::vector<int32_t> ukeys;
-    std::unordered_map<int32_t, int32_t> uidx;
-    std::vector<int32_t> qoff(static_cast<size_t>(nqb) + 1, 0), slot;
-    for (int q = 0; q < nqb; ++q) {
-      std::vector<int32_t> seen;
-      for (int64_t j = q_offsets[q0 + q]; j < q_offsets[q0 + q + 1]; ++j) {
-        const int32_t t = q_terms[j];
-        if (!idf.count(t) || std::find(seen.begin(), seen.end(), t) != seen.end()) continue;   // no live posting / repeated
-        seen.push_back(t);
-        auto it = uidx.find(t);
-        if (it == uidx.end()) { it = uidx.emplace(t, static_cast<int32_t>(ukeys.size())).first; ukeys.push_back(t); }
-        slot.push_back(it->second);
-      }
-      qoff[static_cast<size_t>(q) + 1] = static_cast<int32_t>(slot.size());
-    }
-    const int nu = static_cast<int>(ukeys.size());
-    double* o_s = c->out_s.p + static_cast<size_t>(q0) * k;
-    int64_t* o_i = c->out_ids.p + static_cast<size_t>(q0) * k;
-    if (nu == 0 || n_rows == 0 || N == 0) {   // nothing can match: padding only
-      std::vector<double> ps(static_cast<size_t>(nqb) * k, -INFINITY);
-      std::vector<int64_t> pi(static_cast<size_t>(nqb) * k, -1);
-      KW_TRY(cudaMemcpyAsync(o_s, ps.data(), ps.size() * 8, cudaMemcpyHostToDevice, s));
-      KW_TRY(cudaMemcpyAsync(o_i, pi.data(), pi.size() * 8, cudaMemcpyHostToDevice, s));
-      continue;
-    }
-    int hcap = 16;
-    while (hcap < 2 * nu) hcap <<= 1;
-    std::vector<int32_t> hkey(static_cast<size_t>(hcap), -1), hval(static_cast<size_t>(hcap), -1);
-    for (int u = 0; u < nu; ++u) {
-      uint32_t h = (static_cast<uint32_t>(ukeys[static_cast<size_t>(u)]) * 2654435761u) & static_cast<uint32_t>(hcap - 1);
-      while (hkey[h] >= 0) h = (h + 1) & static_cast<uint32_t>(hcap - 1);
-      hkey[h] = ukeys[static_cast<size_t>(u)]; hval[h] = u;
-    }
-    std::vector<double> uidf(static_cast<size_t>(nu));
-    for (int u = 0; u < nu; ++u) uidf[static_cast<size_t>(u)] = idf[ukeys[static_cast<size_t>(u)]];
-    // one upload: idf | hkey | hval | qoff | slot | q_user | q_org
-    const size_t b_idf = 0, b_hk = b_idf + 8 * static_cast<size_t>(nu), b_hv = b_hk + 4 * static_cast<size_t>(hcap);
-    const size_t b_qo = b_hv + 4 * static_cast<size_t>(hcap), b_sl = b_qo + 4 * qoff.size();
-    const size_t b_qu = b_sl + 4 * std::max<size_t>(slot.size(), 1), b_qg = b_qu + 4 * static_cast<size_t>(nqb);
-    const size_t bytes = b_qg + 4 * static_cast<size_t>(nqb);
-    std::vector<unsigned char> tab(bytes, 0);
-    memcpy(tab.data() + b_idf, uidf.data(), 8 * static_cast<size_t>(nu));
-    memcpy(tab.data() + b_hk, hkey.data(), 4 * static_cast<size_t>(hcap));
-    memcpy(tab.data() + b_hv, hval.data(), 4 * static_cast<size_t>(hcap));
-    memcpy(tab.data() + b_qo, qoff.data(), 4 * qoff.size());
-    if (!slot.empty()) memcpy(tab.data() + b_sl, slot.data(), 4 * slot.size());
-    if (q_user) memcpy(tab.data() + b_qu, q_user + q0, 4 * static_cast<size_t>(nqb));
-    std::vector<int32_t> qorg(static_cast<size_t>(nqb), -1);
-    if (q_org) std::copy(q_org + q0, q_org + q0 + nqb, qorg.begin());
-    memcpy(tab.data() + b_qg, qorg.data(), 4 * static_cast<size_t>(nqb));
-    KW_TRY(c->tab.reserve(bytes));
-    KW_TRY(cudaMemcpyAsync(c->tab.p, tab.data(), bytes, cudaMemcpyHostToDevice, s));   // pageable: staged before return
-    // geometry: blocks own contiguous row ranges of whole rounds
-    const int64_t rounds = (n_rows + kKwRoundRows - 1) / kKwRoundRows;
-    const int64_t grid = std::max<int64_t>(1, std::min<int64_t>(2 * kw->sm_count, rounds));
-    const int64_t rpb = (rounds + grid - 1) / grid * kKwRoundRows;
-    const int g = static_cast<int>((n_rows + rpb - 1) / rpb);
-    const int ksel = k;
-    size_t smem = static_cast<size_t>(nqb) * sizeof(Cand) + kKwWarps * kKwBufCap * sizeof(Cand) + 4 * static_cast<size_t>(nqb);
-    smem = (smem + 15) & ~size_t(15);
-    const size_t cval_smem = static_cast<size_t>(kKwWarps) * nu * 8;
-    const bool in_smem = smem + cval_smem <= kw->smem_optin;
-    c->terms = std::max(c->terms, nu);
-    if (!in_smem) ++c->spilled;
-    if (in_smem) smem += cval_smem;
-    else KW_TRY(c->cval.reserve(static_cast<size_t>(g) * kKwWarps * nu));
-    KW_TRY(c->buf.reserve(static_cast<size_t>(g) * nqb * kKwBufCap));
-    KW_TRY(c->lists_a.reserve(static_cast<size_t>(nqb) * g * ksel));
-    KwParams p{};
-    p.off = kw->d_off; p.post = kw->d_post; p.len = kw->d_len; p.ids = kw->d_ids; p.user = kw->d_user; p.org = kw->d_org;
-    p.live = kw->d_live; p.allow = d_allow; p.n_rows = n_rows;
-    p.idf = reinterpret_cast<const double*>(c->tab.p + b_idf); p.n_uniq = nu;
-    p.hkey = reinterpret_cast<const int32_t*>(c->tab.p + b_hk); p.hval = reinterpret_cast<const int32_t*>(c->tab.p + b_hv);
-    p.hmask = hcap - 1;
-    p.q_off = reinterpret_cast<const int32_t*>(c->tab.p + b_qo); p.slot_u = reinterpret_cast<const int32_t*>(c->tab.p + b_sl);
-    p.q_user = q_user ? reinterpret_cast<const int32_t*>(c->tab.p + b_qu) : nullptr;
-    p.q_org = q_user ? reinterpret_cast<const int32_t*>(c->tab.p + b_qg) : nullptr;
-    p.nq = nqb; p.ksel = ksel; p.avgdl = avgdl;
-    p.cval_global = in_smem ? nullptr : c->cval.p;
-    p.buf = c->buf.p; p.lists = c->lists_a.p; p.rows_per_block = rpb;
-    kw_score_kernel<<<g, kKwThreads, smem, s>>>(p, in_smem ? 1 : 0);
-    KW_TRY(cudaGetLastError());
-    c->launches += 1;
-    // fold the per-block lists until one sorted list per query remains
-    int n_lists = g;
-    Cand* cur = c->lists_a.p;
-    bool in_a = true;
-    const int group = std::max(1, kKwFoldCap / ksel);
-    for (;;) {
-      const int n_groups = (n_lists + group - 1) / group;
-      const int gl = std::min(group, n_lists);
-      int sort_n = 1;
-      while (sort_n < gl * ksel) sort_n <<= 1;
-      const size_t fsmem = static_cast<size_t>(sort_n) * sizeof(Cand);
-      if (n_groups == 1) {
-        kw_fold_kernel<<<dim3(1, nqb), 256, fsmem, s>>>(cur, n_lists, ksel, group, sort_n, nullptr, o_s, o_i, k);
-        KW_TRY(cudaGetLastError());
-        c->launches += 1;
-        break;
-      }
-      KwBuf<Cand>& dst = in_a ? c->lists_b : c->lists_a;
-      KW_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
-      kw_fold_kernel<<<dim3(n_groups, nqb), 256, fsmem, s>>>(cur, n_lists, ksel, group, sort_n, dst.p, nullptr, nullptr, k);
-      KW_TRY(cudaGetLastError());
-      c->launches += 1;
-      cur = dst.p; n_lists = n_groups; in_a = !in_a;
-    }
-  }
-  KW_TRY(cudaEventRecord(c->ev1, s));
-  KW_TRY(cudaMemcpyAsync(scores_out, c->out_s.p, nout * 8, cudaMemcpyDeviceToHost, s));
-  KW_TRY(cudaMemcpyAsync(ids_out, c->out_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
-  KW_TRY(cudaStreamSynchronize(s));
-  float ms = 0.f;
-  KW_TRY(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+  return kw_search_stores(&kw, 1, q, scores_out, ids_out, snapshot_rows_out);
+}
+
+int aur_kw_search_multi(aur_kw* const* stores, int32_t n_stores, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq,
+                        int32_t k, const int32_t* q_user, const int32_t* q_org, const int64_t* allow_ids, int64_t n_allow,
+                        double* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out) {
+  if (!stores) return report_error(AUR_ERR_INVALID, "null argument");
+  if (n_stores < 1 || n_stores > kKwMaxStores) return report_error(AUR_ERR_INVALID, "n_stores must be in 1 .. %d", kKwMaxStores);
+  for (int32_t s = 0; s < n_stores; ++s) if (!stores[s]) return report_error(AUR_ERR_INVALID, "store %d is NULL", s);
   {
-    std::lock_guard<std::mutex> lk(kw->mu_pool);
-    kw->last_launches = c->launches; kw->last_ms = ms;
-    kw->last_terms = c->terms; kw->last_spilled = c->spilled;
+    std::vector<aur_kw*> sorted(stores, stores + n_stores);
+    std::sort(sorted.begin(), sorted.end(), std::less<aur_kw*>());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+      return report_error(AUR_ERR_INVALID, "a store is listed twice (its statistics would count double)");
   }
-  if (snapshot_rows_out) *snapshot_rows_out = n_rows;
-  return AUR_OK;
+  const KwQuery q{q_terms, q_offsets, nq, k, q_user, q_org, allow_ids, n_allow};
+  int rc = kw_check_query(q, scores_out, ids_out);
+  if (rc != AUR_OK) return rc;
+  if (n_stores == 1) return kw_search_stores(stores, 1, q, scores_out, ids_out, snapshot_rows_out);
+  const size_t nout = static_cast<size_t>(nq) * k;
+  std::vector<double> ls(nout * n_stores);
+  std::vector<int64_t> li(nout * n_stores);
+  if ((rc = kw_search_stores(stores, n_stores, q, ls.data(), li.data(), snapshot_rows_out)) != AUR_OK) return rc;
+  // every store's lists are sorted by (fp64 score desc, id asc) with (-inf, -1) padding last: one k-way merge per query
+  return aur_merge_topk_host_f64(ls.data(), li.data(), n_stores, nq, k, k, scores_out, ids_out);
 }
 
 }  // extern "C"

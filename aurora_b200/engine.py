@@ -191,6 +191,13 @@ class Index:
         return {f: getattr(st, f) for f, _ in N.AurStats._fields_}
 
 
+def shard_capacity(capacity: int, n: int) -> int:
+    """Rows reserved on each of n shards of a store placed by ``id mod n`` (MultiIndex, MultiKeywordIndex): an even
+    share plus headroom, since id mod n is balanced only statistically."""
+    per = (int(capacity) + n - 1) // n
+    return per + max(64, per // 8)
+
+
 class MultiIndex:
     """One process, one shard per GPU of the host (the daemon's deployment on an 8-GPU box): the corpus is row-sharded
     by ``id mod n`` -- an upsert or a delete always lands on the shard that holds the old row -- every search runs on
@@ -209,8 +216,7 @@ class MultiIndex:
             raise RuntimeError("MultiIndex needs at least one device")
         self.dim, self.capacity, self.devices = int(dim), int(capacity), [int(d) for d in devices]
         n = len(self.devices)
-        per = (self.capacity + n - 1) // n
-        per += max(64, per // 8)                    # id mod n is balanced only statistically
+        per = shard_capacity(self.capacity, n)
         self._native_merge = shard_factory is None and _shards is None
         if shard_factory is None:
             shard_factory = lambda dim_, cap_, dev_: Index(dim_, cap_, dtype=dtype, device=dev_)   # noqa: E731
@@ -367,25 +373,128 @@ class KeywordIndex:
     def search(self, q_terms, q_offsets, k: int, q_user=None, q_org=None, allow_ids=None):
         """(ids [nq,k] int64, scores [nq,k] float64, snapshot rows).  Query q's term ids are
         q_terms[q_offsets[q]:q_offsets[q+1]] in summation order.  ``allow_ids``: None = every document."""
-        q_off = np.ascontiguousarray(q_offsets, dtype=np.int64)
-        nq = q_off.shape[0] - 1
-        qt = np.ascontiguousarray(q_terms, dtype=np.int32)
-        if qt.size == 0:
-            qt = np.zeros(1, dtype=np.int32)
-        scores = np.empty((nq, k), dtype=np.float64)
-        ids = np.empty((nq, k), dtype=np.int64)
-        u = None if q_user is None else np.ascontiguousarray(q_user, dtype=np.int32)
-        o = None if q_org is None else np.ascontiguousarray(q_org, dtype=np.int32)
-        allow, n_allow = None, 0
-        if allow_ids is not None:
-            allow = np.ascontiguousarray(allow_ids, dtype=np.int64)
-            n_allow = allow.shape[0]
-            if n_allow == 0:
-                allow = np.zeros(1, dtype=np.int64)     # a real pointer: "nothing is allowed"
+        a = _kw_query_args(q_terms, q_offsets, k, q_user, q_org, allow_ids)
         snap = C.c_int64(-1)
-        N.check(self._lib.aur_kw_search(self._h, _ptr(qt), _ptr(q_off), int(nq), int(k), _ptr(u), _ptr(o), _ptr(allow),
-                                        int(n_allow), _ptr(scores), _ptr(ids), C.byref(snap)))
-        return ids, scores, int(snap.value)
+        N.check(self._lib.aur_kw_search(self._h, *a["args"], C.byref(snap)))
+        return a["ids"], a["scores"], int(snap.value)
+
+
+def _kw_query_args(q_terms, q_offsets, k, q_user, q_org, allow_ids):
+    """The query-side arguments of aur_kw_search / aur_kw_search_multi and the output arrays they fill (kept alive in
+    the returned dict for the duration of the call)."""
+    q_off = np.ascontiguousarray(q_offsets, dtype=np.int64)
+    nq = q_off.shape[0] - 1
+    qt = np.ascontiguousarray(q_terms, dtype=np.int32)
+    if qt.size == 0:
+        qt = np.zeros(1, dtype=np.int32)
+    scores = np.empty((nq, k), dtype=np.float64)
+    ids = np.empty((nq, k), dtype=np.int64)
+    u = None if q_user is None else np.ascontiguousarray(q_user, dtype=np.int32)
+    o = None if q_org is None else np.ascontiguousarray(q_org, dtype=np.int32)
+    allow, n_allow = None, 0
+    if allow_ids is not None:
+        allow = np.ascontiguousarray(allow_ids, dtype=np.int64)
+        n_allow = allow.shape[0]
+        if n_allow == 0:
+            allow = np.zeros(1, dtype=np.int64)     # a real pointer: "nothing is allowed"
+    args = (_ptr(qt), _ptr(q_off), int(nq), int(k), _ptr(u), _ptr(o), _ptr(allow), int(n_allow), _ptr(scores), _ptr(ids))
+    return {"args": args, "ids": ids, "scores": scores, "keep": (qt, q_off, u, o, allow)}
+
+
+class MultiKeywordIndex:
+    """One BM25 keyword store per GPU of the host, searched as one corpus (aur_kw_search_multi): documents are placed by
+    ``id mod n`` like ``MultiIndex``'s rows -- an upsert or a delete always reaches the store that holds the old row --
+    and every search scores each store's prefix on its own GPU with the idf and avgdl of the union of the stores'
+    snapshots, so the answer is bit for bit that of a single ``KeywordIndex`` holding every document.  Same surface as
+    ``KeywordIndex``; ``search`` reports the snapshot rows of every store.  ``store_factory(capacity,
+    postings_capacity, device)`` builds one store (tests: a recording double)."""
+
+    _SUMMED = ("docs", "live", "capacity", "postings_used", "postings_allocated", "total_len")
+
+    def __init__(self, capacity: int, devices=None, postings_capacity: int = 0, store_factory=None):
+        from concurrent.futures import ThreadPoolExecutor
+
+        if devices is None:
+            devices = list(range(N.load().aur_device_count()))
+        if not devices:
+            raise RuntimeError("MultiKeywordIndex needs at least one device")
+        self.capacity, self.devices = int(capacity), [int(d) for d in devices]
+        n = len(self.devices)
+        if n > 64:
+            raise ValueError("MultiKeywordIndex takes at most 64 stores")
+        per = shard_capacity(self.capacity, n)
+        per_post = shard_capacity(postings_capacity, n) if postings_capacity else 0
+        if store_factory is None:
+            store_factory = lambda cap, post, dev: KeywordIndex(cap, postings_capacity=post, device=dev)   # noqa: E731
+        self.stores = [store_factory(per, per_post, d) for d in self.devices]
+        self._pool = ThreadPoolExecutor(max_workers=n, thread_name_prefix="aurora-b200-kw")
+
+    def _each(self, fn):
+        """fn(store index, store) on every store concurrently (each waits on its own GPU); results in store order."""
+        if len(self.stores) == 1:
+            return [fn(0, self.stores[0])]
+        return list(self._pool.map(lambda t: fn(*t), enumerate(self.stores)))
+
+    def _split(self, ids: np.ndarray):
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        owner = np.mod(ids, len(self.stores))
+        return ids, [np.nonzero(owner == s)[0] for s in range(len(self.stores))]
+
+    def add(self, ids, term_ids, tfs, offsets, user_codes=None, org_codes=None) -> None:
+        """KeywordIndex.add, each document to store ``id mod n``: its CSR rows are cut out and their offsets rebased."""
+        ids, sel = self._split(ids)
+        offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+        if offsets.shape != (ids.shape[0] + 1,):
+            raise ValueError("offsets must be [n + 1]")
+        t = np.ascontiguousarray(term_ids, dtype=np.int32)
+        f = np.ascontiguousarray(tfs, dtype=np.int32)
+        u = None if user_codes is None else np.asarray(user_codes, dtype=np.int32)
+        o = None if org_codes is None else np.asarray(org_codes, dtype=np.int32)
+
+        def put(s, store):
+            rows = sel[s]
+            if not len(rows):
+                return
+            lens = offsets[rows + 1] - offsets[rows]
+            sub_off = np.zeros(len(rows) + 1, dtype=np.int64)
+            np.cumsum(lens, out=sub_off[1:])
+            take = np.repeat(offsets[rows] - sub_off[:-1], lens) + np.arange(sub_off[-1], dtype=np.int64)
+            store.add(ids[rows], t[take], f[take], sub_off, None if u is None else u[rows], None if o is None else o[rows])
+        self._each(put)
+
+    def remove(self, ids) -> int:
+        ids, sel = self._split(ids)
+        return int(sum(self._each(lambda s, store: store.remove(ids[sel[s]]) if len(sel[s]) else 0)))
+
+    def compact(self) -> int:
+        return int(sum(self._each(lambda s, store: store.compact())))
+
+    def stats(self) -> dict:
+        """KeywordIndex.stats summed over the stores (the last search: launches and spills summed, terms and device time
+        the largest of any store); ``stores`` lists every store's own."""
+        per = self._each(lambda s, store: store.stats())
+        out = {key: int(sum(p[key] for p in per)) for key in self._SUMMED}
+        out["last_launches"] = int(sum(p["last_launches"] for p in per))
+        out["last_spilled"] = int(sum(p["last_spilled"] for p in per))
+        out["last_terms"] = max(p["last_terms"] for p in per)
+        out["last_ms"] = max(p["last_ms"] for p in per)
+        out["stores"] = per
+        return out
+
+    def search(self, q_terms, q_offsets, k: int, q_user=None, q_org=None, allow_ids=None):
+        """(ids [nq,k] int64, scores [nq,k] float64, snapshot rows [n stores]): KeywordIndex.search over the union of the
+        stores."""
+        a = _kw_query_args(q_terms, q_offsets, k, q_user, q_org, allow_ids)
+        handles = (C.c_void_p * len(self.stores))(*[st._h.value for st in self.stores])
+        snaps = np.full(len(self.stores), -1, dtype=np.int64)
+        N.check(N.load().aur_kw_search_multi(handles, len(self.stores), *a["args"], _ptr(snaps)))
+        return a["ids"], a["scores"], [int(x) for x in snaps]
+
+    def close(self) -> None:
+        for st in self.stores:
+            st.close()
+        self.stores = []
+        self._pool.shutdown(wait=False)
 
 
 def merge_topk_packed_dev(device: int, packed_ptr: int, n_shards: int, nq: int, k: int, out_scores_ptr: int,

@@ -95,16 +95,17 @@ class KnowledgeBase:
         self._scope_cache: Dict[Tuple[Optional[str], Optional[str]], tuple] = {}   # tenant -> (mutations, id set, sorted ids)
 
     def _keyword_store(self, capacity: int):
-        """``DeviceBM25`` on the vector index's GPU when that index is an ``engine.Index`` or a ``MultiIndex`` of them
-        (on its first shard's device), else ``BM25Index``.  Both score the same (DESIGN.md section 10)."""
+        """``DeviceBM25`` on the vector index's GPU when that index is an ``engine.Index``; over a ``MultiIndex`` of them,
+        one keyword store on each shard's GPU (``engine.MultiKeywordIndex``, searched as one corpus); else
+        ``BM25Index``.  All score the same (DESIGN.md section 10)."""
         from .bm25 import DeviceBM25
-        from .engine import Index, MultiIndex
+        from .engine import Index, MultiIndex, MultiKeywordIndex
 
         ix = self.index
         if isinstance(ix, Index):
             return DeviceBM25(capacity, device=ix.device)
         if isinstance(ix, MultiIndex) and ix.shards and all(isinstance(sh, Index) for sh in ix.shards):
-            return DeviceBM25(capacity, device=ix.shards[0].device)
+            return DeviceBM25(store=MultiKeywordIndex(capacity, devices=[sh.device for sh in ix.shards]))
         return BM25Index()
 
     def _scope_codes(self, user_id: Optional[str], org_id: Optional[str]) -> Tuple[int, int]:

@@ -191,6 +191,9 @@ int aur_merge_topk_packed_dev(int32_t device, const void* packed, int32_t n_shar
  * Stands in for the coordinator-side merge of a multi-shard Weaviate class (weaviate_client.py:252-259 call site). */
 int aur_merge_topk_host(const float* scores, const int64_t* ids, int32_t n_lists, int32_t nq, int32_t k_in,
                         int32_t k_out, float* out_scores, int64_t* out_ids);
+/* The same merge on fp64 scores (the keyword stores' exact BM25 scores, aur_kw_search_multi); padding -INFINITY / -1. */
+int aur_merge_topk_host_f64(const double* scores, const int64_t* ids, int32_t n_lists, int32_t nq, int32_t k_in,
+                            int32_t k_out, double* out_scores, int64_t* out_ids);
 
 /* Fused exchange (SURVEY.md 2c C1, "fused variant"): instead of a local top-k array + ncclAllGather + merge, the
  * kernel that produces a shard's exact top-k stores it straight into EVERY rank's exchange buffer over NVLink
@@ -276,6 +279,18 @@ int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out);
 int aur_kw_search(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k,
                   const int32_t* q_user, const int32_t* q_org, const int64_t* allow_ids, int64_t n_allow,
                   double* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out);
+/* aur_kw_search over n_stores (1 .. 64) stores taken as ONE corpus, e.g. one store per GPU of the host with documents
+ * placed by id mod n_stores; ids must be unique across the stores (the caller's placement keeps them so).  The answer
+ * equals aur_kw_search on a single store holding the union of every store's snapshot prefix: ids exact, fp64 scores
+ * bit-identical, padding (-1, -INFINITY).  N, df and total_len are summed over the stores' snapshots and idf / avgdl
+ * computed once from the sums; every store scores its own prefix on its own device with them, all stores at once, and
+ * the per-store lists are merged on the host by (score desc, id asc).  Every store's shared lock is held for the whole
+ * call, taken in address order.  q_user / q_org / allow_ids as for aur_kw_search (each store resolves allow_ids against
+ * its own documents).  snapshot_rows_out [n_stores] (nullable): the prefix store s scanned; each store's
+ * aur_kw_stats.last_* describe its part of the search.  NULL entries and a store listed twice: AUR_ERR_INVALID. */
+int aur_kw_search_multi(aur_kw* const* stores, int32_t n_stores, const int32_t* q_terms, const int64_t* q_offsets,
+                        int32_t nq, int32_t k, const int32_t* q_user, const int32_t* q_org, const int64_t* allow_ids,
+                        int64_t n_allow, double* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out);
 
 /* ------------------------------------------------------------------ text encoder
  * Replaces the text2vec-transformers sidecar: EmbeddingClient.embed / embed_batch

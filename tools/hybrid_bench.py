@@ -9,9 +9,13 @@ device keyword store (engine.KeywordIndex); 256 queries of 2-8 words are searche
   * the host BM25Index per-query time on the first --host-docs documents (stated; not extrapolated);
   * the host fusion + shaping time of a 256-request batch (bm25.ranked_fusion + result dicts);
   * the card's name and power limit, read in the same run.
-Parity: --parity sampled queries of the 256 batch are held to oracle/bm25_topk.py bit for bit; the run fails otherwise.
+--devices "0" (default) puts the corpus in one store on GPU 0; "all" or a list "0,1,..." shards it by id mod n over one
+store per listed device (engine.MultiKeywordIndex, searched as one corpus; a device may be listed more than once).  The
+device time of a sharded batch is the slowest store's; the line lists the stores' devices and postings.
+Parity: --parity sampled queries of the 256 batch are held to oracle/bm25_topk.py over the whole corpus bit for bit; the
+run fails otherwise.
 
-    python tools/hybrid_bench.py [--docs 1000000] [--tokens 250] [--reps 20]
+    python tools/hybrid_bench.py [--docs 1000000] [--tokens 250] [--reps 20] [--devices 0|all|0,1,...]
 """
 
 from __future__ import annotations
@@ -30,7 +34,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from aurora_b200 import bm25  # noqa: E402
-from aurora_b200.engine import KeywordIndex  # noqa: E402
+from aurora_b200 import _native as N  # noqa: E402
+from aurora_b200.engine import KeywordIndex, MultiKeywordIndex  # noqa: E402
 
 HBM_BYTES_PER_S = 3.35e12
 
@@ -81,7 +86,12 @@ def main():
     ap.add_argument("--host-queries", type=int, default=64)
     ap.add_argument("--parity", type=int, default=8)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--devices", default="0", help='"0" = one store on GPU 0; "all" or "0,1,..." = one store per device')
     args = ap.parse_args()
+    if args.devices == "all":
+        devices = list(range(N.load().aur_device_count()))
+    else:
+        devices = [int(d) for d in args.devices.split(",")]
     rng = np.random.default_rng(args.seed)
     t0 = time.perf_counter()
     terms, tfs, offsets = corpus(rng, args.docs, args.tokens, args.vocab)
@@ -89,7 +99,11 @@ def main():
     qt, qo = queries(rng, 256, args.vocab)
     ids = np.arange(args.docs, dtype=np.int64)
 
-    store = KeywordIndex(args.docs, postings_capacity=len(terms))
+    sharded = len(devices) > 1
+    if sharded:
+        store = MultiKeywordIndex(args.docs, devices=devices, postings_capacity=len(terms))
+    else:
+        store = KeywordIndex(args.docs, postings_capacity=len(terms), device=devices[0])
     t0 = time.perf_counter()
     step = 100_000
     for d0 in range(0, args.docs, step):
@@ -100,7 +114,8 @@ def main():
     st = store.stats()
 
     result = {"docs": args.docs, "mean_tokens": args.tokens, "vocab": args.vocab, "postings": int(st["postings_used"]),
-              "ingest_s": round(ingest_s, 2), "corpus_gen_s": round(gen_s, 2)}
+              "ingest_s": round(ingest_s, 2), "corpus_gen_s": round(gen_s, 2), "stores": len(devices), "devices": devices,
+              "postings_per_store": [int(p["postings_used"]) for p in st["stores"]] if sharded else [int(st["postings_used"])]}
     bytes_per_batch = int(st["postings_used"]) * 8 + args.docs * 13
     result["bytes_per_batch"] = bytes_per_batch
     k = 128
@@ -124,7 +139,8 @@ def main():
     from oracle.bm25_topk import Corpus, bm25_topk
 
     got_i, got_s, snap = store.search(qt, qo, k)
-    cp = Corpus(terms, tfs, offsets, ids, n_rows=snap)
+    assert (sum(snap) if sharded else snap) == args.docs
+    cp = Corpus(terms, tfs, offsets, ids)                    # the whole corpus, however it is sharded
     sample = np.linspace(0, 255, args.parity).astype(int)
     ok = True
     for q in sample:
