@@ -392,9 +392,28 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
     mbar_wait(q_ready, 0);   // the query block is in shared memory (and visible to the async proxy)
     const uint32_t qs_a = smem_u32(smem + L.off_qs);
     const uint32_t ring_a = smem_u32(smem);
-    int stage = 0; uint32_t phase = 0;
+    // One commit group per k-block, then wait_group 1: the next k-block's MMAs are queued while the previous ones run,
+    // so the tensor pipe drains once per tile instead of once per k-block.  The MMAs still accumulate in the order
+    // k-block 0 .. kbs - 1, K step 0 .. 3: the scores are bit-identical to waiting after every group.
+    // Stages are released in ring order (rel_stage trails stage), each exactly once and only after the wait_group that
+    // retires the group reading it: k-block kb's stage after k-block kb + 1 is issued, the tile's last one after the
+    // wait_group 0 that ends the tile.  So at most two stages are held (a 2-stage ring never waits on itself) and none
+    // across the acc_empty wait, where the epilogue may hold buffer 0 until the first certified threshold.  Without MMAs
+    // (dbg_flags & 2) the waits retire nothing and the same stages are released in the same order.  The wait_groups
+    // are unconditional: ptxas serialises every wgmma of the kernel when a group may be in flight where paths merge.
+    // (Overlapping the score-buffer store with the next tile's first k-block, through a second accumulator, makes
+    // ptxas serialise every wgmma too: it does not track which accumulator a wait_group 1 retires across loops.)
+    int stage = 0, rel_stage = 0; uint32_t phase = 0;
     long long tm_empty = 0, tm_full = 0;
     const long long tm_begin = TCLK();
+    // this CTA's tensor core is done with the oldest held stage; so may be the peer's producer
+    auto release = [&]() {
+      if (wt == 0) {
+        mbar_arrive(&empty_bar[rel_stage]);
+        if constexpr (kCtaGroup == 2) mbar_arrive_cluster(&empty_bar[rel_stage], rank ^ 1u);
+      }
+      if (++rel_stage == p.num_stages) rel_stage = 0;
+    };
     for (int it = 0; it < my_tiles; ++it) {
       const int b = (kEpiGroups == 2) ? (it & 1) : 0;
       float d[32];
@@ -413,15 +432,14 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
 #pragma unroll
           for (int k = 0; k < 4; ++k) wgmma_m64n64_ss(d, da + 2 * k, db + 2 * k, 1u);   // 4 x K=16 per 128-byte k-block
           wgmma_commit();
-          wgmma_wait<0>();
-          wgmma_fence_regs(d);
         }
-        if (wt == 0) {   // this CTA's tensor core is done with the stage; so may be the peer's producer
-          mbar_arrive(&empty_bar[stage]);
-          if constexpr (kCtaGroup == 2) mbar_arrive_cluster(&empty_bar[stage], rank ^ 1u);
-        }
+        wgmma_wait<1>();   // k-block kb - 1 has retired
+        if (kb > 0) release();
         if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
       }
+      wgmma_wait<0>();
+      wgmma_fence_regs(d);
+      release();
       {
         const long long t0 = TCLK();
         mbar_wait(&acc_empty[b], ((static_cast<uint32_t>(it / kEpiGroups)) & 1u) ^ 1u);
