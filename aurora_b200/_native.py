@@ -16,14 +16,14 @@ ABI_VERSION = 3         # must equal AUR_ABI_VERSION of the library that gets lo
 AUR_OK = 0
 AUR_ERR_INVALID, AUR_ERR_CUDA, AUR_ERR_NOMEM, AUR_ERR_UNSUPPORTED, AUR_ERR_NO_DEVICE = -1, -2, -3, -4, -5
 AUR_BF16, AUR_F32 = 0, 1
-KERNEL_AUTO, KERNEL_SIMT, KERNEL_TC1, KERNEL_TC2 = 0, 1, 2, 3
-KERNEL_NAMES = {0: "auto", 1: "simt", 2: "wgmma-cta1", 3: "wgmma-cluster2"}
+KERNEL_AUTO, KERNEL_SIMT, KERNEL_TC1, KERNEL_TC2, KERNEL_LIST = 0, 1, 2, 3, 4
+KERNEL_NAMES = {0: "auto", 1: "simt", 2: "wgmma-cta1", 3: "wgmma-cluster2", 4: "list"}
 TC_QUERY_ROWS = 64   # queries per CTA of the tensor-core kernel (kTcQRows, csrc/internal.h): the debug-score row count
 
 # every symbol include/aurora_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "aur_abi_version", "aur_last_error", "aur_device_count", "aur_open", "aur_close", "aur_get_stats",
-    "aur_set_option", "aur_sync", "aur_add", "aur_add_dev", "aur_export", "aur_read_rows", "aur_compact", "aur_remove", "aur_search", "aur_search_ex", "aur_search_subset", "aur_search_dev",
+    "aur_set_option", "aur_sync", "aur_add", "aur_add_dev", "aur_export", "aur_read_rows", "aur_compact", "aur_remove", "aur_search", "aur_search_ex", "aur_search_subset", "aur_search_lists", "aur_search_dev",
     "aur_merge_topk_dev", "aur_merge_topk_packed_dev", "aur_merge_topk_host", "aur_merge_topk_host_f64", "aur_exchange_create", "aur_exchange_connect", "aur_exchange_close",
     "aur_exchange_status", "aur_search_exchange_dev", "aur_cosine_pairs", "aur_dev_malloc", "aur_dev_free", "aur_memcpy_h2d", "aur_memcpy_d2h",
     "aur_debug_tc_scores",
@@ -107,6 +107,7 @@ def load():
         "aur_read_rows": (C.c_int, [vp, i64, i64, vp, vp]),
         "aur_search_ex": (C.c_int, [vp, vp, i32, i32, vp, vp, vp, vp, C.POINTER(i64)]),
         "aur_search_subset": (C.c_int, [vp, vp, i32, i32, vp, i64, vp, vp]),
+        "aur_search_lists": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, vp, vp, vp, C.POINTER(i64)]),
         "aur_search": (C.c_int, [vp, vp, i32, i32, vp, vp, vp, vp]),
         "aur_search_dev": (C.c_int, [vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]),
         "aur_merge_topk_dev": (C.c_int, [i32, vp, vp, i32, i32, i32, vp, vp, vp, vp]),

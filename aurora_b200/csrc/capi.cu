@@ -133,10 +133,12 @@ struct SearchCtx {
   DevBuf<int32_t> stage_quser, stage_qorg;
   DevBuf<float> stage_scores;
   DevBuf<int64_t> stage_ids;
+  DevBuf<int32_t> list_stage;    // list search: work items, their queries and the lists' resolved rows (one upload)
+  DevBuf<float> list_scores;     // list search: scores of a batch of work items, [slots][kSimtSeg]
   void release() {
     cand_a.release(); cand_b.release(); pub.release(); cand_count.release(); d_epoch.release(); cand_read.release(); score_chunk.release(); masked_inv.release();
     allow_rows.release(); row_mask.release(); scope_tab.release(); q_scope.release(); stage_q.release(); stage_quser.release(); stage_qorg.release(); stage_scores.release();
-    stage_ids.release();
+    stage_ids.release(); list_stage.release(); list_scores.release();
     if (ev_begin) cudaEventDestroy(ev_begin);
     if (ev_k0) cudaEventDestroy(ev_k0);
     if (ev_k1) cudaEventDestroy(ev_k1);
@@ -492,6 +494,23 @@ int check_search_args(aur_index* ix, const void* q, int32_t nq, int32_t k, const
   return AUR_OK;
 }
 
+// Pinned caller buffers are mapped into the device's address space (UVA): the re-rank kernel then writes its nq x k
+// results straight into them over PCIe and the two device-to-host copies (a launch + ~8 us of latency each) disappear.
+// Returns whether *d_scores / *d_ids now point at the caller's buffers (else they keep the staging buffers).
+bool direct_outputs(float* scores_out, int64_t* ids_out, float** d_scores, int64_t** d_ids) {
+  static const bool no_direct = getenv("AUR_NO_DIRECT_OUT") != nullptr;     // A/B switch
+  if (no_direct) return false;
+  cudaPointerAttributes as{}, ai{};
+  if (cudaPointerGetAttributes(&as, scores_out) == cudaSuccess && cudaPointerGetAttributes(&ai, ids_out) == cudaSuccess &&
+      as.type == cudaMemoryTypeHost && ai.type == cudaMemoryTypeHost && as.devicePointer && ai.devicePointer) {
+    *d_scores = static_cast<float*>(as.devicePointer);
+    *d_ids = static_cast<int64_t*>(ai.devicePointer);
+    return true;
+  }
+  cudaGetLastError();
+  return false;
+}
+
 // Host-buffer search: H2D of the queries, kernels, D2H of the results on a pool context's own stream.
 int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user, const int32_t* q_org,
                 const int64_t* allow_ids, int64_t n_allow, float* scores_out, int64_t* ids_out, int64_t* snapshot_out) {
@@ -569,27 +588,215 @@ int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, 
       }
     }
   }
-  // Pinned caller buffers are mapped into the device's address space (UVA): the re-rank kernel then writes its nq x k
-  // results straight into them over PCIe and the two device-to-host copies (a launch + ~8 us of latency each) disappear.
   float* d_scores = c->stage_scores.p;
   int64_t* d_ids = c->stage_ids.p;
-  bool direct = false;
-  static const bool no_direct = getenv("AUR_NO_DIRECT_OUT") != nullptr;     // A/B switch
-  if (!no_direct) {
-    cudaPointerAttributes as{}, ai{};
-    if (cudaPointerGetAttributes(&as, scores_out) == cudaSuccess && cudaPointerGetAttributes(&ai, ids_out) == cudaSuccess &&
-        as.type == cudaMemoryTypeHost && ai.type == cudaMemoryTypeHost && as.devicePointer && ai.devicePointer) {
-      d_scores = static_cast<float*>(as.devicePointer);
-      d_ids = static_cast<int64_t*>(ai.devicePointer);
-      direct = true;
-    } else {
-      cudaGetLastError();
-    }
-  }
+  const bool direct = direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
   rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, d_scores, d_ids, nullptr, s);
   if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
   if (!direct) {
     // into the caller's pageable buffers; nothing is written unless every kernel above was enqueued successfully
+    CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
+    CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
+  }
+  CU_TRY(cudaStreamSynchronize(s));
+  if (snapshot_out) *snapshot_out = n_rows;
+  return AUR_OK;
+}
+
+// Search with a pre-filter list per query (aur_search_lists).  The batch runs in blocks of kListQBlock queries (one
+// dense candidate buffer each, as on the generic path); a block's work items are (list, <= kListQMax of its queries
+// naming that list, kSimtSeg-row segment of the list), launched in batches whose score scratch stays within
+// kListScoreSlots rows of kSimtSeg floats.
+constexpr int kListQBlock = 1024;
+constexpr int64_t kListScoreSlots = 16384;   // 128 MB of scores
+
+int search_lists_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int64_t* list_ids,
+                      const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list, float* scores_out,
+                      int64_t* ids_out, int64_t* snapshot_out) {
+  int rc = check_search_args(ix, queries_host, nq, k, scores_out, ids_out);
+  if (rc != AUR_OK) return rc;
+  if (k > kMaxK) return fail(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
+  if (nq > 65535) return fail(AUR_ERR_UNSUPPORTED, "nq > 65535: split the batch");
+  if (ix->dtype != AUR_BF16) return fail(AUR_ERR_UNSUPPORTED, "list search needs a bf16 index");
+  if (!list_offsets || !q_list || n_lists < 1) return fail(AUR_ERR_INVALID, "list_offsets, q_list and n_lists >= 1 are required");
+  if (list_offsets[0] != 0) return fail(AUR_ERR_INVALID, "list_offsets[0] must be 0");
+  for (int32_t l = 0; l < n_lists; ++l)
+    if (list_offsets[l + 1] < list_offsets[l]) return fail(AUR_ERR_INVALID, "list_offsets decrease at list %d", l);
+  if (list_offsets[n_lists] > 0 && !list_ids) return fail(AUR_ERR_INVALID, "list_ids is required");
+  for (int32_t q = 0; q < nq; ++q)
+    if (q_list[q] < 0 || q_list[q] >= n_lists) return fail(AUR_ERR_INVALID, "q_list[%d] = %d is not a list", q, q_list[q]);
+
+  std::shared_lock<std::shared_mutex> rl(ix->rw);
+  CU_TRY(cudaSetDevice(ix->device));
+  SearchCtx* c = nullptr;
+  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
+  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
+  std::lock_guard<std::mutex> cl(c->mu);
+  cudaStream_t s = c->own_stream;
+  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
+  const int ksel = k + kSlack;
+
+  // ids -> rows of the published prefix (unknown / newer ids drop out), for the lists some query names
+  std::vector<std::vector<int32_t>> res(static_cast<size_t>(n_lists));
+  std::vector<char> named(static_cast<size_t>(n_lists), 0);
+  for (int32_t q = 0; q < nq; ++q) named[static_cast<size_t>(q_list[q])] = 1;
+  {
+    std::lock_guard<std::mutex> lk(ix->mu);
+    for (int32_t l = 0; l < n_lists; ++l) {
+      if (!named[static_cast<size_t>(l)]) continue;
+      std::vector<int32_t>& r = res[static_cast<size_t>(l)];
+      for (int64_t i = list_offsets[l]; i < list_offsets[l + 1]; ++i) {
+        auto it = ix->id2row.find(list_ids[i]);
+        if (it != ix->id2row.end() && it->second < n_rows) r.push_back(static_cast<int32_t>(it->second));
+      }
+    }
+  }
+  // staging (int32): [every named list's rows, sorted, once each][per block: its queries' positions, its items]
+  std::vector<int32_t> stage;
+  std::vector<int64_t> lrow0(static_cast<size_t>(n_lists), 0), llen(static_cast<size_t>(n_lists), 0);
+  for (int32_t l = 0; l < n_lists; ++l) {
+    std::vector<int32_t>& r = res[static_cast<size_t>(l)];
+    std::sort(r.begin(), r.end());
+    r.erase(std::unique(r.begin(), r.end()), r.end());
+    lrow0[static_cast<size_t>(l)] = static_cast<int64_t>(stage.size());
+    llen[static_cast<size_t>(l)] = static_cast<int64_t>(r.size());
+    stage.insert(stage.end(), r.begin(), r.end());
+    std::vector<int32_t>().swap(r);
+  }
+  struct Launch { size_t items; int n_items, max_nq; };
+  struct Block { int q0, nqb, n_segs; std::vector<Launch> launches; };
+  std::vector<Block> blocks;
+  constexpr int kItemWords = sizeof(ListItem) / 4;
+  size_t max_slots = 0, max_cand = 0;
+  std::vector<ListItem> items;
+  for (int q0 = 0; q0 < nq; q0 += kListQBlock) {
+    Block b{q0, std::min(kListQBlock, nq - q0), 1, {}};
+    std::vector<int32_t> order(static_cast<size_t>(b.nqb));
+    for (int i = 0; i < b.nqb; ++i) order[static_cast<size_t>(i)] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) { return q_list[q0 + x] < q_list[q0 + y]; });
+    const size_t qidx0 = stage.size();
+    stage.insert(stage.end(), order.begin(), order.end());
+    items.clear();
+    for (int i = 0; i < b.nqb;) {
+      const int32_t l = q_list[q0 + order[static_cast<size_t>(i)]];
+      int e = i;
+      while (e < b.nqb && q_list[q0 + order[static_cast<size_t>(e)]] == l) ++e;
+      const int64_t len = llen[static_cast<size_t>(l)];
+      const int segs = static_cast<int>((len + kSimtSeg - 1) / kSimtSeg);
+      b.n_segs = std::max(b.n_segs, segs);
+      for (int g = i; g < e; g += kListQMax)
+        for (int sg = 0; sg < segs; ++sg) {
+          ListItem it;
+          it.row0 = static_cast<int32_t>(lrow0[static_cast<size_t>(l)] + static_cast<int64_t>(sg) * kSimtSeg);
+          it.n_rows = static_cast<int32_t>(std::min<int64_t>(kSimtSeg, len - static_cast<int64_t>(sg) * kSimtSeg));
+          it.seg = sg;
+          it.q0 = static_cast<int32_t>(qidx0 + g);
+          it.nq = std::min(kListQMax, e - g);
+          it.out = 0;
+          items.push_back(it);
+        }
+      i = e;
+    }
+    // cut into launches; `out` = the item's first score row inside its launch
+    int64_t slots = 0;
+    for (size_t i = 0; i < items.size(); ++i) {
+      if (b.launches.empty() || slots + items[i].nq > kListScoreSlots) {
+        b.launches.push_back(Launch{stage.size() + i * kItemWords, 0, 0});
+        slots = 0;
+      }
+      Launch& ln = b.launches.back();
+      items[i].out = static_cast<int32_t>(slots);
+      slots += items[i].nq;
+      ++ln.n_items;
+      ln.max_nq = std::max(ln.max_nq, items[i].nq);
+      max_slots = std::max(max_slots, static_cast<size_t>(slots));
+    }
+    const int32_t* w = reinterpret_cast<const int32_t*>(items.data());
+    stage.insert(stage.end(), w, w + items.size() * kItemWords);
+    max_cand = std::max(max_cand, static_cast<size_t>(b.nqb) * b.n_segs * ksel);
+    blocks.push_back(std::move(b));
+  }
+  if (stage.size() > static_cast<size_t>(INT32_MAX))
+    return fail(AUR_ERR_UNSUPPORTED, "the lists of this batch are too long for one call: split the batch");
+
+  const size_t qbytes = static_cast<size_t>(nq) * ix->dim * 2;
+  const size_t nout = static_cast<size_t>(nq) * k;
+  CU_TRY(c->stage_q.reserve(qbytes));
+  CU_TRY(c->stage_scores.reserve(nout));
+  CU_TRY(c->stage_ids.reserve(nout));
+  CU_TRY(c->list_stage.reserve(stage.size()));
+  CU_TRY(c->list_scores.reserve(std::max<size_t>(max_slots, 1) * kSimtSeg));
+  CU_TRY(c->cand_a.reserve(max_cand));
+  CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
+  float* d_scores = c->stage_scores.p;
+  int64_t* d_ids = c->stage_ids.p;
+  const bool direct = direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
+
+  auto enqueue = [&]() -> int {
+    c->last_kernel = AUR_KERNEL_LIST;
+    c->last_launches = 0;
+    c->last_nq = nq;
+    c->snapshot_rows = n_rows;
+    CU_TRY(cudaEventRecord(c->ev_begin, s));
+    CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
+    CU_TRY(cudaMemcpyAsync(c->list_stage.p, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, s));
+    for (size_t bi = 0; bi < blocks.size(); ++bi) {
+      const Block& b = blocks[bi];
+      const uint8_t* qb = c->stage_q.p + static_cast<size_t>(b.q0) * ix->dim * 2;
+      int n_lists_c = b.n_segs;
+      CU_TRY(cudaMemsetAsync(c->cand_a.p, 0, static_cast<size_t>(b.nqb) * n_lists_c * ksel * 8, s));   // 0 = empty slot
+      if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k0, s));
+      for (const Launch& ln : b.launches) {
+        ListParams p{};
+        p.q = reinterpret_cast<const __nv_bfloat16*>(qb);
+        p.rows = static_cast<const __nv_bfloat16*>(ix->d_rows);
+        p.inv_norm = ix->d_inv_norm;
+        p.ids = ix->d_ids;
+        p.items = reinterpret_cast<const ListItem*>(c->list_stage.p + ln.items);
+        p.n_items = ln.n_items;
+        p.list_rows = c->list_stage.p;
+        p.qidx = c->list_stage.p;
+        p.scores = c->list_scores.p;
+        p.cand = c->cand_a.p;
+        p.dim = ix->dim; p.ksel = ksel; p.n_lists = n_lists_c;
+        CU_TRY(launch_list_search(p, ln.max_nq, s));
+        c->last_launches += 2;
+      }
+      if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k1, s));
+      // fold to <= 4096 keys per query, then the exact re-rank (the generic path's tail)
+      uint64_t* cur = c->cand_a.p;
+      bool in_a = true;
+      while (static_cast<int64_t>(n_lists_c) * ksel > 4096) {
+        const int group = 4096 / ksel;
+        const int n_groups = (n_lists_c + group - 1) / group;
+        DevBuf<uint64_t>& dst = in_a ? c->cand_b : c->cand_a;
+        CU_TRY(dst.reserve(static_cast<size_t>(b.nqb) * n_groups * ksel));
+        CU_TRY(launch_reduce_lists(cur, b.nqb, n_lists_c, ksel, group, ix->d_ids, dst.p, s));
+        c->last_launches += 1;
+        cur = dst.p; n_lists_c = n_groups; in_a = !in_a;
+      }
+      FinalizeArgs fa{};
+      fa.cand = cur; fa.n_lists = n_lists_c; fa.ksel = ksel;
+      fa.cand_read = c->cand_read.p + b.q0;
+      fa.q = qb; fa.rows = ix->d_rows; fa.dtype = ix->dtype; fa.dim = ix->dim; fa.nq = b.nqb; fa.k = k;
+      fa.ids = ix->d_ids;
+      fa.out_scores = d_scores + static_cast<size_t>(b.q0) * k;
+      fa.out_ids = d_ids + static_cast<size_t>(b.q0) * k;
+      CU_TRY(launch_finalize(fa, s));
+      c->last_launches += 1;
+    }
+    CU_TRY(cudaEventRecord(c->ev_fin, s));
+    CU_TRY(cudaEventRecord(c->ev_end, s));
+    c->have_timing = true;
+    {
+      std::lock_guard<std::mutex> lk(ix->mu);
+      ix->last_ctx = c;
+    }
+    return AUR_OK;
+  };
+  rc = enqueue();
+  if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
+  if (!direct) {
     CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
   }
@@ -903,6 +1110,13 @@ int aur_search_subset(aur_index* ix, const void* queries_host, int32_t nq, int32
   if (n_allow < 0) return fail(AUR_ERR_INVALID, "n_allow < 0");
   static const int64_t none = 0;
   return search_host(ix, queries_host, nq, k, nullptr, nullptr, allow_ids ? allow_ids : &none, n_allow, scores_out, ids_out, nullptr);
+}
+
+int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int64_t* list_ids,
+                     const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list, float* scores_out,
+                     int64_t* ids_out, int64_t* snapshot_rows_out) {
+  return search_lists_host(ix, queries_host, nq, k, list_ids, list_offsets, n_lists, q_list, scores_out, ids_out,
+                           snapshot_rows_out);
 }
 
 

@@ -168,6 +168,26 @@ cudaError_t launch_row_scope_mask(const int32_t* row_user, const int32_t* row_or
 cudaError_t launch_mask_inv_norm(const float* inv, const int32_t* row_user, const int32_t* row_org, int32_t u, int32_t o,
                                  int64_t n, float* out, cudaStream_t s);
 
+// ---------------------------------------------------------------- per-query pre-filter lists (listsearch.cu)
+constexpr int kListQMax = 64;     // queries of one work item (four m16 MMA row blocks)
+// One work item: rows list_rows[row0 .. row0 + n_rows) (n_rows <= kSimtSeg, segment `seg` of the list) against the
+// queries qidx[q0 .. q0 + nq) (nq <= kListQMax); their scores go to rows out .. out + nq of the score scratch.
+struct ListItem { int32_t row0, n_rows, seg, q0, nq, out; };
+struct ListParams {
+  const __nv_bfloat16* q;      // [nq of the query block, dim]
+  const __nv_bfloat16* rows;   // the shard's rows
+  const float* inv_norm;       // NaN = tombstone
+  const int64_t* ids;
+  const ListItem* items; int n_items;
+  const int32_t* list_rows;    // resolved rows of every list, each list sorted and without repeats
+  const int32_t* qidx;         // query (position in the block) of every item slot
+  float* scores;               // scratch [sum of the items' nq][kSimtSeg]
+  uint64_t* cand;              // [queries of the block, n_lists, ksel] candidate keys (slots no item writes: zero)
+  int dim, ksel, n_lists;
+};
+// Scores and per-segment selection of n_items work items; max_nq = the largest nq among them.
+cudaError_t launch_list_search(const ListParams& p, int max_nq, cudaStream_t s);
+
 // out[rows[i]] = inv[rows[i]] for the listed rows (out pre-filled with NaN): a resolved id subset as a row mask
 cudaError_t launch_scatter_inv_norm(const float* inv, const int32_t* rows, int64_t n, int64_t n_rows, float* out, cudaStream_t s);
 // compaction: rows map[0..n) (and their side arrays) -> bounce buffers

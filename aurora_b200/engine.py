@@ -165,6 +165,28 @@ class Index:
         N.check(self._lib.aur_search_subset(self._h, _ptr(q), nq, int(k), _ptr(allow), allow.shape[0], _ptr(scores), _ptr(ids)))
         return ids, scores
 
+    def search_lists(self, queries: np.ndarray, k: int, lists, q_list) -> Tuple[np.ndarray, np.ndarray]:
+        """Search with a pre-filter per query: query q sees only the rows whose ids are in ``lists[q_list[q]]`` (a
+        sequence of id arrays; several queries may name the same list).  Only the listed rows are read, so the cost
+        follows the lists' sizes, not the shard's.  bf16 indexes.  Returns (ids [nq,k] int64, scores [nq,k] float32)."""
+        ids, scores, _ = self.search_lists_snapshot(queries, k, lists, q_list)
+        return ids, scores
+
+    def search_lists_snapshot(self, queries: np.ndarray, k: int, lists, q_list):
+        """``search_lists`` together with the number of appended rows it saw (see ``search_snapshot``)."""
+        q = self._rows_buffer(queries)
+        nq = q.shape[0]
+        flat, offsets = lists_csr(lists)
+        ql = np.ascontiguousarray(q_list, dtype=np.int32)
+        if ql.shape != (nq,):
+            raise ValueError("q_list must be [nq]")
+        scores = np.empty((nq, k), dtype=np.float32)
+        ids = np.empty((nq, k), dtype=np.int64)
+        snap = C.c_int64(-1)
+        N.check(self._lib.aur_search_lists(self._h, _ptr(q), nq, int(k), _ptr(flat), _ptr(offsets), len(offsets) - 1,
+                                           _ptr(ql), _ptr(scores), _ptr(ids), C.byref(snap)))
+        return ids, scores, int(snap.value)
+
     def search_dev(self, q_ptr: int, nq: int, k: int, scores_ptr: int, ids_ptr: int, scores64_ptr: int = 0,
                    q_user_ptr: int = 0, q_org_ptr: int = 0, stream: int = 0) -> None:
         """Everything in HBM; asynchronous on ``stream`` (0 = the index's own stream)."""
@@ -189,6 +211,15 @@ class Index:
         st = N.AurStats()
         N.check(self._lib.aur_get_stats(self._h, C.byref(st)))
         return {f: getattr(st, f) for f, _ in N.AurStats._fields_}
+
+
+def lists_csr(lists):
+    """A sequence of id arrays as (ids int64, offsets int64 [len + 1]): list l = ids[offsets[l]:offsets[l + 1]]."""
+    parts = [np.asarray(a, dtype=np.int64).reshape(-1) for a in lists]
+    offsets = np.zeros(len(parts) + 1, dtype=np.int64)
+    np.cumsum([len(a) for a in parts], out=offsets[1:])
+    flat = np.ascontiguousarray(np.concatenate(parts)) if parts and offsets[-1] else np.zeros(1, dtype=np.int64)
+    return flat, offsets
 
 
 def shard_capacity(capacity: int, n: int) -> int:
@@ -276,6 +307,12 @@ class MultiIndex:
     def search_subset(self, queries: np.ndarray, k: int, allow_ids: np.ndarray):
         allow, sel = self._split(allow_ids)
         return self._merge(self._each(lambda s, shard: shard.search_subset(queries, k, allow[sel[s]])), k)
+
+    def search_lists(self, queries: np.ndarray, k: int, lists, q_list):
+        """Index.search_lists over every shard: each list is split by ``id mod n``, each shard searches its part."""
+        split = [self._split(a) for a in lists]
+        return self._merge(self._each(lambda s, shard: shard.search_lists(
+            queries, k, [ids[sel[s]] for ids, sel in split], q_list)), k)
 
     # -------------------------------------------------------------- maintenance
     def stats(self) -> dict:

@@ -41,6 +41,10 @@ logger = logging.getLogger(__name__)
 
 COLLECTION_NAME = "KnowledgeBaseChunk"  # weaviate_client.py:23
 _MAX_FETCH = 128                        # engine's largest k
+# A filtered query reads only its allowed rows (Index.search_lists) while they are at most this fraction of the live
+# objects; above it the masked full scan (search_subset) answers sooner.  Measured at one query over 1M x 768 bf16
+# (DESIGN.md section 9, tools/list_bench.py): the list path wins at 3 000 rows (0.3 %), the full scan at 10 000 (1 %).
+_LIST_MAX_FRACTION = 0.005
 
 
 def _sanitize(value: Any) -> str:
@@ -316,7 +320,11 @@ class KnowledgeBase:
                 dense = [(rid, sc) for rid, sc in _dense if rid in self._props]
             elif qv is not None and (allowed is None or allowed):
                 fetch = max(1, min(_MAX_FETCH, limit if not hybrid else _MAX_FETCH))
-                if allowed is not None:
+                if (allowed is not None and hasattr(self.index, "search_lists")
+                        and len(allowed) <= _LIST_MAX_FRACTION * len(self._props)):   # reads only the allowed rows
+                    ids, scores = self.index.search_lists(qv, fetch, [np.asarray(allowed, dtype=np.int64)],
+                                                          np.zeros(1, np.int32))
+                elif allowed is not None:
                     ids, scores = self.index.search_subset(qv, fetch, np.asarray(allowed, dtype=np.int64))
                 else:
                     q_user = q_org = None
@@ -394,11 +402,26 @@ class KnowledgeBase:
                 co = self._code(self._org_code, o, False) if o else -1
                 groups.setdefault(fetch, []).append((pos, cu, -1 if co == -2 else co))
             for fetch, members in groups.items():
-                # one launch for the whole group: up to 32 distinct tenant scopes per batch ride on the tensor-core
-                # kernel as per-row bit masks (csrc/capi.cu search_host); the library falls back by itself beyond that
                 pos = [m[0] for m in members]
-                ids, scores = self.index.search(vecs[pos], fetch, np.array([m[1] for m in members], np.int32),
-                                                np.array([m[2] for m in members], np.int32))
+                scopes: Dict[Tuple[int, int], int] = {}
+                for m in members:
+                    scopes.setdefault((m[1], m[2]), len(scopes))
+                if len(scopes) > 32 and hasattr(self.index, "search_lists"):
+                    # more scopes than the tensor-core kernel's row bit masks hold: one id list per scope (the rows
+                    # _tenant_scope gives the keyword leg) and one list search that reads only those rows
+                    lists: List[np.ndarray] = [np.empty(0, np.int64)] * len(scopes)
+                    for m in members:
+                        slot = scopes[(m[1], m[2])]
+                        if not len(lists[slot]):
+                            u, o = reqs[need[m[0]]][0], reqs[need[m[0]]][4]
+                            lists[slot] = self._tenant_scope(u, o)[1]
+                    ids, scores = self.index.search_lists(vecs[pos], fetch, lists,
+                                                          np.array([scopes[(m[1], m[2])] for m in members], np.int32))
+                else:
+                    # one launch for the whole group: up to 32 distinct tenant scopes per batch ride on the tensor-core
+                    # kernel as per-row bit masks (csrc/capi.cu search_host); the library falls back by itself beyond
+                    ids, scores = self.index.search(vecs[pos], fetch, np.array([m[1] for m in members], np.int32),
+                                                    np.array([m[2] for m in members], np.int32))
                 for row, p_ in enumerate(pos):
                     dense[need[p_]] = [(int(r), float(s_)) for r, s_ in zip(ids[row], scores[row]) if r >= 0]
         out = []

@@ -58,7 +58,8 @@ typedef enum aur_kernel {
   AUR_KERNEL_AUTO = 0,   /* tensor-core path when the shape allows it, else SIMT      */
   AUR_KERNEL_SIMT = 1,   /* generic CUDA-core path (any dim / dtype / filter)     */
   AUR_KERNEL_TC1 = 2,    /* wgmma, single CTAs                                    */
-  AUR_KERNEL_TC2 = 3     /* wgmma, two-CTA clusters sharing tiles by TMA multicast */
+  AUR_KERNEL_TC2 = 3,    /* wgmma, two-CTA clusters sharing tiles by TMA multicast */
+  AUR_KERNEL_LIST = 4    /* per-query list gather (aur_search_lists only; not an option value) */
 } aur_kernel;
 
 typedef struct aur_index aur_index; /* opaque: one corpus shard resident on one GPU */
@@ -163,6 +164,17 @@ int aur_search_ex(aur_index* ix, const void* queries_host, int32_t nq, int32_t k
 int aur_search_subset(aur_index* ix, const void* queries_host, int32_t nq, int32_t k,
                       const int64_t* allow_ids, int64_t n_allow,
                       float* scores_out, int64_t* ids_out);
+/* Search with a pre-filter per query: query q sees only the rows whose ids are in list q_list[q], list l being
+ * list_ids[list_offsets[l] .. list_offsets[l + 1]).  Several queries may name the same list.  Unknown ids, tombstoned ids
+ * and ids appended after the search's snapshot are ignored; an id listed twice counts once; an empty list yields padding.
+ * Cost grows with the listed rows, not the shard.  bf16 indexes (any dim the index accepts); 1 <= k <= 128.
+ * Many tenants' pre-filtered requests (Aurora Learn's org or user scope, incident_knowledge.py:128-133; the
+ * prediscovery `org_id AND document_id LIKE "discovery:*"` filter, rca_prompt_builder.py:286-298) share one call.
+ * Threading, snapshot (*snapshot_rows_out, nullable) and page-locked outputs as for aur_search_ex; aur_stats reports
+ * last_kernel = AUR_KERNEL_LIST.  The "kernel" option does not apply. */
+int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_t k,
+                     const int64_t* list_ids, const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list,
+                     float* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out);
 /* Device variant: everything in HBM; scores64_dev (nullable) additionally receives the
  * fp64 ranking keys needed for an exact cross-shard merge. */
 int aur_search_dev(aur_index* ix, const void* queries_dev, int32_t nq, int32_t k,
