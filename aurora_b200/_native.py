@@ -45,7 +45,7 @@ class AurStats(C.Structure):
                 ("dtype", C.c_int32), ("last_kernel", C.c_int32), ("last_launches", C.c_int32),
                 ("last_kernel_ms", C.c_float), ("last_total_ms", C.c_float), ("last_finalize_ms", C.c_float),
                 ("last_merge_ms", C.c_float), ("last_candidates", C.c_int64), ("last_candidates_max", C.c_int32),
-                ("reserved", C.c_int32)]
+                ("last_tile_n", C.c_int32)]
 
 
 class AurKwStats(C.Structure):

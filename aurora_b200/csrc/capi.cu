@@ -117,6 +117,7 @@ struct SearchCtx {
   cudaEvent_t ev_begin = nullptr, ev_k0 = nullptr, ev_k1 = nullptr, ev_fin = nullptr, ev_end = nullptr;
   bool have_timing = false;
   int last_kernel = 0, last_launches = 0, last_nq = 0;
+  int last_tile_n = 0;             // corpus rows per tile of the last tensor-core launch (0: none)
   int64_t snapshot_rows = 0;
   uint32_t epoch = 0;
   DevBuf<uint64_t> cand_a, cand_b;
@@ -164,13 +165,14 @@ struct aur_index {
   std::unordered_map<int64_t, int64_t> id2row;
   cudaStream_t stream = nullptr;         // the index's own stream: device-pointer calls with stream == NULL
   cudaStream_t ingest_stream = nullptr;  // host appends / tombstones, lowest priority so queries overtake them
-  CUtensorMap tmap[2];  // box rows 64 (cta_group::1) and 32 (cta_group::2)
+  CUtensorMap tmap[2][2];  // [64-row, 128-row tiles][cta_group 1, 2]: box rows tile / cta_group
   bool tmap_ok = false;
   int sm_count = 0;
   size_t smem_optin = 0;
   int opt_kernel = AUR_KERNEL_AUTO;
   int opt_dbg_flags = 0;
   int opt_epi_groups = 0;        // 0 = auto
+  int opt_tc_tile = 0;           // corpus rows per tile: 0 = auto, 64, 128
   std::atomic<uint32_t> opt_dbg_epoch{0};   // bring-up: start value of the contexts' launch counters (0 = 1)
   std::vector<std::unique_ptr<SearchCtx>> ctxs;
   std::vector<SearchCtx*> free_ctxs;   // idle pool contexts
@@ -184,16 +186,19 @@ int build_tmaps(aur_index* ix) {
   if (ix->dtype != AUR_BF16 || ix->dim % kTcKBlock != 0 || ix->dim > kTcMaxDim) return AUR_OK;  // SIMT only
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
-  for (int g = 1; g <= 2; ++g) {
-    cuuint64_t gdim[2] = {static_cast<cuuint64_t>(ix->dim), static_cast<cuuint64_t>(ix->capacity)};
-    cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ix->dim) * 2};
-    cuuint32_t box[2] = {static_cast<cuuint32_t>(kTcKBlock), static_cast<cuuint32_t>(kTcTileN / g)};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&ix->tmap[g - 1], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ix->d_rows, gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
-  }
+  // rows past the capacity (a tile's tail, a whole half of the last tile of a pair) arrive as zeros
+  for (int w = 0; w < 2; ++w)
+    for (int g = 1; g <= 2; ++g) {
+      const int tile_n = w ? kTcTileWide : kTcTileN;
+      cuuint64_t gdim[2] = {static_cast<cuuint64_t>(ix->dim), static_cast<cuuint64_t>(ix->capacity)};
+      cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ix->dim) * 2};
+      cuuint32_t box[2] = {static_cast<cuuint32_t>(kTcKBlock), static_cast<cuuint32_t>(tile_n / g)};
+      cuuint32_t estr[2] = {1, 1};
+      CUresult r = enc(&ix->tmap[w][g - 1], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ix->d_rows, gdim, gstride, box, estr,
+                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (r != CUDA_SUCCESS) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
+    }
   ix->tmap_ok = true;
   return AUR_OK;
 }
@@ -202,7 +207,7 @@ bool tc_shape_ok(const aur_index* ix, int k, bool filtered) {
   if (!ix->tmap_ok || filtered || k > kMaxK) return false;
   // candidate lists (k + slack per query) and the query block share the SM's shared memory with
   // the TMA ring: large k at large dim leaves no room for a pipeline
-  return tc_pick_stages(1, k + kSlack, ix->dim, ix->smem_optin) >= 2;
+  return tc_pick_stages(1, k + kSlack, ix->dim, ix->smem_optin, kTcTileN, true) >= 2;
 }
 
 int ctx_init(aur_index* ix, SearchCtx* c) {
@@ -239,6 +244,15 @@ void release_ctx(aur_index* ix, SearchCtx* c) {
   if (!c->bound) ix->free_ctxs.push_back(c);
 }
 
+// Corpus rows per tile when the index leaves it to the launch.  A 128-row tile (wgmma m64n128) fetches each operand for
+// twice the work of a 64-row one, but its layout leaves fewer, larger ring stages: it runs with one epilogue group and
+// at least kTcWideMinStages stages, so at dim 1024, at large k and for most tenant-scoped batches the 64-row kernel
+// stays.  The bring-up score dump (dbg) keeps the 64-row tile it documents.
+int tc_auto_tile(int epi_groups, int ksel, int dim, size_t smem_optin, bool mask, bool dbg) {
+  if (dbg || epi_groups != 1) return kTcTileN;
+  return tc_pick_stages(1, ksel, dim, smem_optin, kTcTileWide, mask) >= kTcWideMinStages ? kTcTileWide : kTcTileN;
+}
+
 // Runs one block of queries (<= 128 single CTAs, <= 512 pairs) through the tensor-core kernel over the first n_rows rows.  Leaves candidate keys
 // in c->cand_a as [nqb_pad, n_lists, ksel]; returns n_lists.
 int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, int nqb, int ksel, int64_t n_rows, float* dbg,
@@ -260,9 +274,13 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   // epilogue groups: 1 by default; 2 (alternating tiles) stays selectable for experiments
   int epi_groups = ix->opt_epi_groups;
   if (epi_groups == 0) epi_groups = 1;   // one group leaves the most shared memory to the TMA ring
-  const int stages = tc_pick_stages(epi_groups, ksel, ix->dim, ix->smem_optin);
+  const bool mask = row_mask != nullptr;
+  int tile_n = ix->opt_tc_tile;
+  if (tile_n == 0) tile_n = tc_auto_tile(epi_groups, ksel, ix->dim, ix->smem_optin, mask, dbg != nullptr);
+  if (tile_n == kTcTileWide && epi_groups != 1) return fail(AUR_ERR_UNSUPPORTED, "128-row tiles need epi_groups 1");
+  const int stages = tc_pick_stages(epi_groups, ksel, ix->dim, ix->smem_optin, tile_n, mask);
   if (stages < 2) return fail(AUR_ERR_UNSUPPORTED, "k too large for the tensor-core path's shared memory");
-  const size_t smem = tc_smem_bytes(epi_groups, stages, ksel, ix->dim);
+  const size_t smem = tc_smem_bytes(epi_groups, stages, ksel, ix->dim, tile_n, mask);
   const int n_lists = n_tsets * epi_groups;   // candidate lists per query
   const size_t ncand = static_cast<size_t>(n_qblocks) * kTcQRows * n_lists * ksel;
   CU_TRY(c->cand_a.reserve(ncand));
@@ -298,8 +316,9 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   p.nq = nqb; p.dim = ix->dim; p.ksel = ksel; p.n_lists = n_lists; p.n_qblocks = n_qblocks;
   p.num_stages = stages;
   p.dbg_flags = ix->opt_dbg_flags;
-  p.n_tiles = static_cast<int>((n_rows + kTcTileN - 1) / kTcTileN);
-  CU_TRY(tc_launch(cta_group, epi_groups, grid, &ix->tmap[cta_group - 1], p, smem, s));
+  p.n_tiles = static_cast<int>((n_rows + tile_n - 1) / tile_n);
+  CU_TRY(tc_launch(cta_group, epi_groups, tile_n, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
+  c->last_tile_n = tile_n;
   *n_lists_out = n_lists;
   return AUR_OK;
 }
@@ -337,6 +356,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
   c->last_kernel = kernel;
   c->last_launches = 0;
   c->last_nq = nq;
+  c->last_tile_n = 0;
   CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
   c->snapshot_rows = n_rows;
   CU_TRY(cudaEventRecord(c->ev_begin, s));
@@ -735,6 +755,7 @@ int search_lists_host(aur_index* ix, const void* queries_host, int32_t nq, int32
   auto enqueue = [&]() -> int {
     c->last_kernel = AUR_KERNEL_LIST;
     c->last_launches = 0;
+    c->last_tile_n = 0;
     c->last_nq = nq;
     c->snapshot_rows = n_rows;
     CU_TRY(cudaEventRecord(c->ev_begin, s));
@@ -883,7 +904,7 @@ int aur_get_stats(aur_index* ix, aur_stats* out) {
   }
   if (c) {
     std::lock_guard<std::mutex> cl(c->mu);
-    out->last_kernel = c->last_kernel; out->last_launches = c->last_launches;
+    out->last_kernel = c->last_kernel; out->last_launches = c->last_launches; out->last_tile_n = c->last_tile_n;
     if (c->have_timing) {
       CU_TRY(cudaSetDevice(ix->device));
       CU_TRY(cudaEventSynchronize(c->ev_end));
@@ -1024,6 +1045,11 @@ int aur_set_option(aur_index* ix, const char* key, int64_t value) {
   if (strcmp(key, "epi_groups") == 0) {
     if (value < 0 || value > 2) return fail(AUR_ERR_INVALID, "epi_groups must be 0 (auto), 1 or 2");
     ix->opt_epi_groups = static_cast<int>(value);
+    return AUR_OK;
+  }
+  if (strcmp(key, "tc_tile") == 0) {
+    if (value != 0 && value != kTcTileN && value != kTcTileWide) return fail(AUR_ERR_INVALID, "tc_tile must be 0 (auto), 64 or 128");
+    ix->opt_tc_tile = static_cast<int>(value);
     return AUR_OK;
   }
   if (strcmp(key, "dbg_flags") == 0) { ix->opt_dbg_flags = static_cast<int>(value); return AUR_OK; }

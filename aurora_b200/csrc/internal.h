@@ -48,7 +48,9 @@ __device__ __forceinline__ bool key_before(uint64_t a, uint64_t b, const int64_t
 #endif
 
 // ---------------------------------------------------------------- wgmma similarity kernel
-constexpr int kTcTileN = 64;       // corpus rows per tile  (MMA N)
+constexpr int kTcTileN = 64;       // corpus rows per tile  (MMA N); the bring-up score dump keeps this width
+constexpr int kTcTileWide = 128;   // the wide tile (wgmma m64n128), picked per launch when its layout fits
+constexpr int kTcWideMinStages = 4;   // with three 16 KB stages the wide tile measured no faster than the 64-row one
 constexpr int kTcKBlock = 64;      // bf16 per 128-byte swizzled smem row (one pipeline stage)
 constexpr int kTcQRows = 64;       // queries per CTA (MMA M of one warpgroup)
 constexpr int kTcChunk = 16;       // scores examined per threshold test
@@ -90,11 +92,12 @@ constexpr uint32_t kSearchEpochMax = 0x7FFFFFFFu;
 
 // epi_groups: 1 = two epilogue warps take every tile; 2 = two pairs of warps alternate tiles
 // (each pair owns one score buffer and its own candidate lists).
-size_t tc_smem_bytes(int epi_groups, int num_stages, int ksel, int dim);
-int tc_pick_stages(int epi_groups, int ksel, int dim, size_t smem_limit);
+// tile_n: corpus rows per tile, kTcTileN or kTcTileWide (epi_groups 1 only); mask: a kMask launch (row_mask set).
+size_t tc_smem_bytes(int epi_groups, int num_stages, int ksel, int dim, int tile_n, bool mask);
+int tc_pick_stages(int epi_groups, int ksel, int dim, size_t smem_limit, int tile_n, bool mask);
 // Launches the fused similarity + top-k kernel; cta_group 2 = two-CTA clusters sharing every corpus tile by TMA
-// multicast.  tmap: CUtensorMap over the corpus with a {64, 64 / cta_group} box and 128-byte swizzle.
-cudaError_t tc_launch(int cta_group, int epi_groups, int grid, const void* tmap, const TcParams& p, size_t smem,
+// multicast.  tmap: CUtensorMap over the corpus with a {64, tile_n / cta_group} box and 128-byte swizzle.
+cudaError_t tc_launch(int cta_group, int epi_groups, int tile_n, int grid, const void* tmap, const TcParams& p, size_t smem,
                       cudaStream_t s);
 
 // ---------------------------------------------------------------- SIMT kernels

@@ -6,21 +6,27 @@
 // reference sends to Weaviate (server/routes/knowledge_base/weaviate_client.py:252-259,
 // server/routes/incident_feedback/weaviate_client.py:286-291).
 //
+// Tile width N = 64 or 128 corpus rows (kTileN, chosen per launch on the host, tc_auto_tile in capi.cu): 128 when its
+// layout keeps at least four 16 KB ring stages and there is one epilogue group -- at dim 768 / top-32 four stages against
+// eight 8 KB ones -- else 64.  The wide tile runs wgmma m64n128k16: the query operand is fetched from shared memory once
+// per 128 corpus rows instead of once per 64, and the drain, score-buffer hand-off and threshold read happen once per
+// 128 rows.  Its epilogue examines a tile 64 scores at a time with the 64-row code.
+//
 // One CTA, persistent, 1 CTA / SM (G = 1 or 2 epilogue groups):
-//   warps 1..2G  epilogue  : thread r of a group owns query r (score-buffer row r): reads its 64 scores of a
+//   warps 1..2G  epilogue  : thread r of a group owns query r (score-buffer row r): reads its N scores of a
 //                            tile, scales them by the rows' inverse norms, keeps one max per 16 scores and
 //                            compares it with the query's threshold; a four-score group that reaches it is
 //                            parked in a per-thread FIFO in shared memory and examined later, out of line and
 //                            rarely (drain_fifo); large k without room for the FIFO pushes at once (push_group4).
 //   warp 0      threshold  : serves the certified global threshold of the queries assigned to this CTA (see
 //                            "Threshold exchange").
-//   warp 2G+1   TMA producer: corpus tiles [64 rows x 64 k] -> smem ring (SWIZZLE_128B)
-//   warpgroup   MMA        : wgmma m64n64k16, A = the CTA's 64 queries (K-major tiles in shared memory), B =
-//                            corpus tile from the ring; the [64 queries x 64 rows] fp32 accumulator lives in
+//   warp 2G+1   TMA producer: corpus tiles [N rows x 64 k] -> smem ring (SWIZZLE_128B)
+//   warpgroup   MMA        : wgmma m64nNk16, A = the CTA's 64 queries (K-major tiles in shared memory), B =
+//                            corpus tile from the ring; the [64 queries x N rows] fp32 accumulator lives in
 //                            registers for the whole tile and is then stored to a padded score buffer that the
 //                            epilogue group of that tile reads row-wise (one buffer per group).  The MMA of the
 //                            next tile runs while the epilogue works on the buffer it just released.
-// Two-CTA clusters (AUR_KERNEL_TC2): the pair shares every corpus tile -- each CTA TMA-loads 32 of the 64 rows and
+// Two-CTA clusters (AUR_KERNEL_TC2): the pair shares every corpus tile -- each CTA TMA-loads N / 2 of the N rows and
 // multicasts them to both, so a tile crosses L2 -> SM once per pair; each CTA scores its own 64 queries.
 // Single CTAs: when nq > 64 several CTAs take the same tiles for different query blocks (sharing through L2).
 //
@@ -65,27 +71,31 @@ constexpr int kThrWarps = 1;
 // bytes in that variant.
 __host__ __device__ constexpr int tc_mma_warp0(int epi_groups) { return (kThrWarps + 2 * epi_groups + 1 + 3) / 4 * 4; }
 constexpr uint32_t kSlot = kTcQRows * 8u;   // byte stride between list slots of one query
-constexpr uint32_t kStageBytes = kTcTileN * 128u;   // one 64-dim k-block of a 64-row corpus tile
 constexpr uint32_t kQTileBytes = kTcQRows * 128u;   // one 64-dim k-block of the query block
-constexpr int kScStride = kTcTileN + 4;             // floats per score-buffer row (padding spreads the banks)
-constexpr uint32_t kScBytes = kTcQRows * kScStride * 4u;
+// one 64-dim k-block of a corpus tile (a ring stage); floats per score-buffer row (padding spreads the banks)
+__host__ __device__ constexpr uint32_t stage_bytes(int tile_n) { return static_cast<uint32_t>(tile_n) * 128u; }
+__host__ __device__ constexpr int sc_stride(int tile_n) { return tile_n + 4; }
+__host__ __device__ constexpr uint32_t sc_bytes(int tile_n) { return kTcQRows * sc_stride(tile_n) * 4u; }
 
 struct SmemLayout {
   uint32_t lcap, fifo_recs;
   uint32_t off_qs, off_sc, off_list, off_norm, off_mask, off_fifo, off_tau, off_bar, total;
 };
-__host__ __device__ inline SmemLayout make_layout(int epi_groups, int num_stages, int ksel, int dim) {
+// The 128-row layout fits a fourth 16 KB ring stage at dim 768 / ksel 40 only without what the 64-row one can afford:
+// it reserves the tenant-scope masks for kMask launches alone and parks half as many groups per thread in the FIFO.
+__host__ __device__ inline SmemLayout make_layout(int epi_groups, int num_stages, int ksel, int dim, int tile_n, bool mask) {
   SmemLayout L;
+  const bool wide = tile_n == kTcTileWide;
   L.lcap = static_cast<uint32_t>(ksel);
-  uint32_t o = kStageBytes * num_stages;
+  uint32_t o = stage_bytes(tile_n) * num_stages;
   // the query block: [64 queries x 64] bf16 K-major SWIZZLE_128B tiles, one per k-block (the wgmma A operand)
   L.off_qs = o;     o += static_cast<uint32_t>(dim / kTcKBlock) * kQTileBytes;
-  L.off_sc = o;     o += static_cast<uint32_t>(epi_groups) * kScBytes;
+  L.off_sc = o;     o += static_cast<uint32_t>(epi_groups) * sc_bytes(tile_n);
   L.off_list = o;   o += static_cast<uint32_t>(epi_groups) * L.lcap * kSlot;
-  L.off_norm = o;   o += static_cast<uint32_t>(epi_groups) * 2u * 2u * kTcTileN * 4u;
-  L.off_mask = o;   o += static_cast<uint32_t>(epi_groups) * 2u * 2u * kTcTileN * 4u;   // per-row tenant-scope bit masks (kMask launches)
+  L.off_norm = o;   o += static_cast<uint32_t>(epi_groups) * 2u * 2u * tile_n * 4u;
+  L.off_mask = o;   if (mask || !wide) o += static_cast<uint32_t>(epi_groups) * 2u * 2u * tile_n * 4u;   // per-row tenant-scope bit masks (kMask launches)
   // deferred-candidate FIFO: per thread kTcFifoRecs records of four adjacent scores (16 B) + a row tag
-  L.fifo_recs = (epi_groups == 1 && ksel <= kTcFifoMaxKsel) ? kTcFifoRecs : 0u;
+  L.fifo_recs = (epi_groups == 1 && ksel <= kTcFifoMaxKsel) ? (wide ? kTcFifoRecs / 2 : kTcFifoRecs) : 0u;
   L.off_fifo = o;   o += L.fifo_recs * kTcQRows * (16u + 4u);
   L.off_tau = o;    o += kTcQRows * 4u;   // certified thresholds of this CTA's queries, refreshed by the threshold warp
   L.off_bar = o;    o += (2u * kTcMaxStages + 2u + 2u + 1u) * 8u + 16u;
@@ -267,21 +277,26 @@ constexpr uint32_t kNaNBits = 0x7FC00000u;
 // batch may see the row -- and every query knows its scope's bit: scores of invisible rows become NaN before anything
 // else looks at them, exactly like tombstones.  (One scope for the whole batch needs none of this: it folds into the
 // inverse norms.)
-template <int kCtaGroup, int kEpiGroups, bool kMask>
+template <int kCtaGroup, int kEpiGroups, bool kMask, int kTileN>
 __global__ void __launch_bounds__(32 * (tc_mma_warp0(kEpiGroups) + 4), 1)
 simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
+  static_assert(kTileN == kTcTileN || (kTileN == kTcTileWide && kEpiGroups == 1), "tile width");
   constexpr int kEpiWarps = 2 * kEpiGroups;
   constexpr int kProducerWarp = kEpiWarps + kThrWarps;
   constexpr int kMmaWarp0 = tc_mma_warp0(kEpiGroups);   // first warp of the MMA warpgroup (warpgroup-aligned)
+  constexpr uint32_t kStageBytes = stage_bytes(kTileN);
+  constexpr int kScStride = sc_stride(kTileN);
+  constexpr uint32_t kScBytes = sc_bytes(kTileN);
+  constexpr int kHalves = kTileN / 64;   // the epilogue examines a tile 64 scores (four 16-score chunks) at a time
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment; the runtime only guarantees 16.  Offsetting
   // the declared array (rather than round-tripping through an integer) keeps the compiler's
   // shared-address-space inference, i.e. LDS/STS instead of generic loads.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
 
-  const SmemLayout L = make_layout(kEpiGroups, p.num_stages, p.ksel, p.dim);
-  float* normbuf = reinterpret_cast<float*>(smem + L.off_norm);      // [2G warps][2][64]
-  uint32_t* maskbuf = reinterpret_cast<uint32_t*>(smem + L.off_mask);  // [2G warps][2][64]
+  const SmemLayout L = make_layout(kEpiGroups, p.num_stages, p.ksel, p.dim, kTileN, kMask);
+  float* normbuf = reinterpret_cast<float*>(smem + L.off_norm);      // [2G warps][2][kTileN]
+  uint32_t* maskbuf = reinterpret_cast<uint32_t*>(smem + L.off_mask);  // [2G warps][2][kTileN]
   float* scbuf = reinterpret_cast<float*>(smem + L.off_sc);          // [G][64 queries][kScStride]
   volatile float* tau_s = reinterpret_cast<volatile float*>(smem + L.off_tau);   // [64]
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bar);
@@ -358,7 +373,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
 #endif
       for (int it = 0; it < my_tiles; ++it) {
         const int tile = tset + it * n_tsets;
-        const int row0 = tile * kTcTileN + static_cast<int>(rank) * (kTcTileN / kCtaGroup);
+        const int row0 = tile * kTileN + static_cast<int>(rank) * (kTileN / kCtaGroup);
         for (int kb = 0; kb < kbs; ++kb) {
           {
             const long long t0 = TCLK();
@@ -385,8 +400,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
     }
   } else if (warp >= kMmaWarp0) {
     // ============================== MMA warpgroup ==============================
-    // wgmma accumulator layout (m64n64): thread t = 32 w + l holds rows 16 w + l / 4 (+ 8) and columns
-    // 8 j + 2 (l % 4) (+ 1), j = 0..7 -- stored into the score buffer as [query][corpus row].
+    // wgmma accumulator layout (m64nN): thread t = 32 w + l holds rows 16 w + l / 4 (+ 8) and columns
+    // 8 j + 2 (l % 4) (+ 1), j = 0..N/8-1 -- stored into the score buffer as [query][corpus row].
     const int wt = threadIdx.x - kMmaWarp0 * 32;
     const int w4 = wt >> 5, l4 = wt & 31;
     mbar_wait(q_ready, 0);   // the query block is in shared memory (and visible to the async proxy)
@@ -416,9 +431,9 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
     };
     for (int it = 0; it < my_tiles; ++it) {
       const int b = (kEpiGroups == 2) ? (it & 1) : 0;
-      float d[32];
+      float d[kTileN / 2];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) d[i] = 0.f;
+      for (int i = 0; i < kTileN / 2; ++i) d[i] = 0.f;
       for (int kb = 0; kb < kbs; ++kb) {
         {
           const long long t0 = TCLK();
@@ -430,7 +445,10 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
           const uint64_t da = wgmma_desc_sw128(qs_a + static_cast<uint32_t>(kb) * kQTileBytes);
           const uint64_t db = wgmma_desc_sw128(ring_a + static_cast<uint32_t>(stage) * kStageBytes);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) wgmma_m64n64_ss(d, da + 2 * k, db + 2 * k, 1u);   // 4 x K=16 per 128-byte k-block
+          for (int k = 0; k < 4; ++k) {   // 4 x K=16 per 128-byte k-block
+            if constexpr (kTileN == kTcTileWide) wgmma_m64n128_ss(d, da + 2 * k, db + 2 * k, 1u);
+            else wgmma_m64n64_ss(d, da + 2 * k, db + 2 * k, 1u);
+          }
           wgmma_commit();
         }
         wgmma_wait<1>();   // k-block kb - 1 has retired
@@ -447,7 +465,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       }
       float* sc = scbuf + b * (kScBytes / 4);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
+      for (int j = 0; j < kTileN / 8; ++j) {
         const int row = 16 * w4 + (l4 >> 2), col = 8 * j + 2 * (l4 & 3);
         *reinterpret_cast<float2*>(sc + row * kScStride + col) = make_float2(d[4 * j + 0], d[4 * j + 1]);
         *reinterpret_cast<float2*>(sc + (row + 8) * kScStride + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
@@ -564,18 +582,18 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
         if (lane == 0) mbar_arrive(q_ready);
       }
       const float* myrow = scbuf + grp * (kScBytes / 4) + r * kScStride;   // this query's row of the group's score buffer
-      auto load_scores = [&](uint32_t (&acc)[4][16]) {
+      auto load_scores = [&](uint32_t (&acc)[4][16], int h) {   // scores 64 h .. 64 h + 63 of the tile
 #pragma unroll
         for (int c = 0; c < 4; ++c)
 #pragma unroll
           for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 v = *reinterpret_cast<const float4*>(myrow + c * 16 + j4 * 4);
+            const float4 v = *reinterpret_cast<const float4*>(myrow + h * 64 + c * 16 + j4 * 4);
             acc[c][j4 * 4 + 0] = __float_as_uint(v.x); acc[c][j4 * 4 + 1] = __float_as_uint(v.y);
             acc[c][j4 * 4 + 2] = __float_as_uint(v.z); acc[c][j4 * 4 + 3] = __float_as_uint(v.w);
           }
       };
-      float* mynorm = normbuf + ew * 2 * kTcTileN;
-      uint32_t* mymask = maskbuf + ew * 2 * kTcTileN;
+      float* mynorm = normbuf + ew * 2 * kTileN;
+      uint32_t* mymask = maskbuf + ew * 2 * kTileN;
       uint32_t mybit = 0u;                                       // this query's tenant-scope bit
       if constexpr (kMask) { if (qglob < p.nq) mybit = 1u << (p.q_scope[qglob] & 31); }
       const uint32_t list_a = smem_u32(smem + L.off_list) + (static_cast<uint32_t>(grp) * L.lcap * kTcQRows + r) * 8u;
@@ -595,27 +613,36 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       const long long t_begin = TCLK();
       long long t_boot = 0, t_loop_end = 0;
 
-      // inverse norms: tile(0) into buffer 0, tile(1) in flight in registers
-      uint32_t mm0 = 0u, mm1 = 0u;                              // (masks of the tile in flight, beside its norms)
-      auto load_norms = [&](int li2, float& a, float& b2) {
-        a = __uint_as_float(kNaNBits); b2 = a;
-        mm0 = 0u; mm1 = 0u;
+      // inverse norms: tile(0) into buffer 0, tile(1) in flight in registers (lane takes rows lane + 32 i)
+      constexpr int kNv = kTileN / 32;
+      float nn[kNv];
+      uint32_t mm[kNv];                                         // (masks of the tile in flight, beside its norms)
+      auto load_norms = [&](int li2) {
+#pragma unroll
+        for (int i = 0; i < kNv; ++i) { nn[i] = __uint_as_float(kNaNBits); mm[i] = 0u; }
         const int it2 = grp + li2 * kEpiGroups;
         if (it2 < my_tiles) {
-          const int64_t rbase = static_cast<int64_t>(tset + it2 * n_tsets) * kTcTileN;
-          if (rbase + lane < p.n_rows) a = __ldg(p.inv_norm + rbase + lane);
-          if (rbase + lane + 32 < p.n_rows) b2 = __ldg(p.inv_norm + rbase + lane + 32);
+          const int64_t rbase = static_cast<int64_t>(tset + it2 * n_tsets) * kTileN;
+#pragma unroll
+          for (int i = 0; i < kNv; ++i)
+            if (rbase + lane + 32 * i < p.n_rows) nn[i] = __ldg(p.inv_norm + rbase + lane + 32 * i);
           if constexpr (kMask) {
-            if (rbase + lane < p.n_rows) mm0 = __ldg(p.row_mask + rbase + lane);
-            if (rbase + lane + 32 < p.n_rows) mm1 = __ldg(p.row_mask + rbase + lane + 32);
+#pragma unroll
+            for (int i = 0; i < kNv; ++i)
+              if (rbase + lane + 32 * i < p.n_rows) mm[i] = __ldg(p.row_mask + rbase + lane + 32 * i);
           }
         }
       };
-      float nn0, nn1;
-      load_norms(0, nn0, nn1);
-      mynorm[lane] = nn0; mynorm[lane + 32] = nn1;
-      if constexpr (kMask) { mymask[lane] = mm0; mymask[lane + 32] = mm1; }
-      load_norms(1, nn0, nn1);
+      auto store_norms = [&](int buf) {
+#pragma unroll
+        for (int i = 0; i < kNv; ++i) {
+          mynorm[buf * kTileN + lane + 32 * i] = nn[i];
+          if constexpr (kMask) mymask[buf * kTileN + lane + 32 * i] = mm[i];
+        }
+      };
+      load_norms(0);
+      store_norms(0);
+      load_norms(1);
       __syncwarp();
 
       // Bootstrap on the first tile: nobody has a threshold yet, and pushing 64 arbitrary rows
@@ -626,7 +653,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       if (xchg && grp < my_tiles) {
         mbar_wait(&acc_full[grp], 0);
 #pragma unroll 1
-        for (int c = 0; c < 4; ++c) {
+        for (int c = 0; c < kTileN / 16; ++c) {
           uint32_t a16[16];
 #pragma unroll
           for (int j4 = 0; j4 < 4; ++j4) {
@@ -662,19 +689,17 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       int li = 0;  // this group's iteration count
       for (int it = grp; it < my_tiles; it += kEpiGroups, ++li) {
         const int tile = tset + it * n_tsets;
-        const int row0 = tile * kTcTileN;
+        const int row0 = tile * kTileN;
         const int b = grp;
-        const float* nb = mynorm + (li & 1) * kTcTileN;
+        const float* nbt = mynorm + (li & 1) * kTileN;
         const long long t_top0 = TCLK();
         const float thr_now = (xchg && !(p.dbg_flags & 16)) ? tau_s[r] : -INFINITY;   // shared-memory copy kept by the threshold warp
 
         // norms of the next tile (loaded one iteration ago) -> the other buffer; start the
         // loads for the tile after that.  A whole tile period hides the HBM latency.
         if (!(p.dbg_flags & 32)) {
-          float* nnext = mynorm + ((li + 1) & 1) * kTcTileN;
-          nnext[lane] = nn0; nnext[lane + 32] = nn1;
-          if constexpr (kMask) { uint32_t* mnext = mymask + ((li + 1) & 1) * kTcTileN; mnext[lane] = mm0; mnext[lane + 32] = mm1; }
-          load_norms(li + 2, nn0, nn1);
+          store_norms((li + 1) & 1);
+          load_norms(li + 2);
           __syncwarp();
         }
 
@@ -683,109 +708,118 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
           mbar_wait(&acc_full[b], (static_cast<uint32_t>(li)) & 1u);
           t_wait += TCLK() - t0;
         }
-        const long long t_ld0 = TCLK();
-        uint32_t acc[4][16];
-        if (!(p.dbg_flags & 1)) load_scores(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[b]);   // scores in registers: hand the buffer back to the MMA warpgroup
-        t_ld += TCLK() - t_ld0;
-        if (p.dbg_flags & (1 | 4)) continue;
-        const long long t_fast0 = TCLK();
-
-        // Fast path: scale by 1/|c_j| in place and keep one running max per 16
-        // scores.  (NaN norm = tombstone / out of range: fmaxf drops it, `>=` rejects it.)
-        if constexpr (kMask) {   // rows this query's tenant scope may not see: NaN, like tombstones
-          const uint32_t* mb = mymask + (li & 1) * kTcTileN;
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-#pragma unroll
-            for (int j4 = 0; j4 < 4; ++j4) {
-              const uint4 mk = *reinterpret_cast<const uint4*>(mb + c * 16 + j4 * 4);
-              if (!(mk.x & mybit)) acc[c][j4 * 4 + 0] = kNaNBits;
-              if (!(mk.y & mybit)) acc[c][j4 * 4 + 1] = kNaNBits;
-              if (!(mk.z & mybit)) acc[c][j4 * 4 + 2] = kNaNBits;
-              if (!(mk.w & mybit)) acc[c][j4 * 4 + 3] = kNaNBits;
-            }
-        }
-        float cmax[4];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          float m = -INFINITY;
-#pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4) {
-            const float4 nv = *reinterpret_cast<const float4*>(nb + c * 16 + j4 * 4);
-            acc[c][j4 * 4 + 0] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 0]), nv.x));
-            acc[c][j4 * 4 + 1] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 1]), nv.y));
-            acc[c][j4 * 4 + 2] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 2]), nv.z));
-            acc[c][j4 * 4 + 3] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 3]), nv.w));
-            m = fmaxf(fmaxf(m, fmaxf(__uint_as_float(acc[c][j4 * 4 + 0]), __uint_as_float(acc[c][j4 * 4 + 1]))),
-                      fmaxf(__uint_as_float(acc[c][j4 * 4 + 2]), __uint_as_float(acc[c][j4 * 4 + 3])));
+        // A wide tile is examined 64 scores at a time by the same code, half 0 while the buffer is still held.
+#pragma unroll 1
+        for (int h = 0; h < kHalves; ++h) {
+          const int hrow0 = row0 + 64 * h;
+          const float* nb = nbt + 64 * h;
+          const long long t_ld0 = TCLK();
+          uint32_t acc[4][16];
+          if (!(p.dbg_flags & 1)) load_scores(acc, h);
+          if (h == kHalves - 1) {   // the whole tile in registers or examined: hand the buffer back to the MMA warpgroup
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&acc_empty[b]);
           }
-          cmax[c] = m;
-        }
-        if (p.dbg_scores != nullptr && it == 0 && !(p.dbg_flags & 64)) {  // (group 0 owns tile 0)
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-              p.dbg_scores[(static_cast<size_t>(blockIdx.x) * kTcQRows + r) * kTcTileN + c * 16 + j] =
-                  __uint_as_float(acc[c][j]);
-        }
+          t_ld += TCLK() - t_ld0;
+          if (p.dbg_flags & (1 | 4)) continue;
+          const long long t_fast0 = TCLK();
 
-        t_fast += TCLK() - t_fast0;
-        // what this CTA can vouch for (published below): chunk maxima are distinct rows
-        if (!(booted && li == 0)) {
-          if (xm == 1) st.top[0] = fmaxf(st.top[0], fmaxf(fmaxf(cmax[0], cmax[1]), fmaxf(cmax[2], cmax[3])));
-          else { top4_insert(st.top, cmax[0]); top4_insert(st.top, cmax[1]); top4_insert(st.top, cmax[2]); top4_insert(st.top, cmax[3]); }
-        }
-        if (p.dbg_flags & 8) continue;
-        const long long t_ch0 = TCLK();
-        // A group of four scores whose max reaches this query's threshold goes out of line.
-        st.tau = fmaxf(st.tau, thr_now);
-        if (use_fifo) {
+          // Fast path: scale by 1/|c_j| in place and keep one running max per 16
+          // scores.  (NaN norm = tombstone / out of range: fmaxf drops it, `>=` rejects it.)
+          if constexpr (kMask) {   // rows this query's tenant scope may not see: NaN, like tombstones
+            const uint32_t* mb = mymask + (li & 1) * kTileN + h * 64;
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+#pragma unroll
+              for (int j4 = 0; j4 < 4; ++j4) {
+                const uint4 mk = *reinterpret_cast<const uint4*>(mb + c * 16 + j4 * 4);
+                if (!(mk.x & mybit)) acc[c][j4 * 4 + 0] = kNaNBits;
+                if (!(mk.y & mybit)) acc[c][j4 * 4 + 1] = kNaNBits;
+                if (!(mk.z & mybit)) acc[c][j4 * 4 + 2] = kNaNBits;
+                if (!(mk.w & mybit)) acc[c][j4 * 4 + 3] = kNaNBits;
+              }
+          }
+          float cmax[4];
 #pragma unroll
           for (int c = 0; c < 4; ++c) {
-            if (cmax[c] >= st.tau) {
-              if (fcnt > static_cast<int>(L.fifo_recs) - 4) {   // no room for four more groups: make room (rare)
-                const long long t0 = TCLK();
-                st = drain_fifo(st, fifo_a, ftag_a, fcnt, list_a, ksel, p.ids);
-                fcnt = 0;
-                ++nslow;
-                t_slow += TCLK() - t0;
-              }
+            float m = -INFINITY;
 #pragma unroll
-              for (int g = 0; g < 4; ++g) {   // park the groups that reach the threshold: two stores each, no call
-                const float m4 = fmaxf(fmaxf(__uint_as_float(acc[c][4 * g]), __uint_as_float(acc[c][4 * g + 1])),
-                                       fmaxf(__uint_as_float(acc[c][4 * g + 2]), __uint_as_float(acc[c][4 * g + 3])));
-                if (m4 >= st.tau) {
-                  asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(fifo_a + static_cast<uint32_t>(fcnt) * (kTcQRows * 16u)),
-                               "r"(acc[c][4 * g]), "r"(acc[c][4 * g + 1]), "r"(acc[c][4 * g + 2]), "r"(acc[c][4 * g + 3]) : "memory");
-                  asm volatile("st.shared.b32 [%0], %1;" ::"r"(ftag_a + static_cast<uint32_t>(fcnt) * (kTcQRows * 4u)),
-                               "r"(row0 + c * 16 + 4 * g) : "memory");
-                  ++fcnt;
+            for (int j4 = 0; j4 < 4; ++j4) {
+              const float4 nv = *reinterpret_cast<const float4*>(nb + c * 16 + j4 * 4);
+              acc[c][j4 * 4 + 0] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 0]), nv.x));
+              acc[c][j4 * 4 + 1] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 1]), nv.y));
+              acc[c][j4 * 4 + 2] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 2]), nv.z));
+              acc[c][j4 * 4 + 3] = __float_as_uint(__fmul_rn(__uint_as_float(acc[c][j4 * 4 + 3]), nv.w));
+              m = fmaxf(fmaxf(m, fmaxf(__uint_as_float(acc[c][j4 * 4 + 0]), __uint_as_float(acc[c][j4 * 4 + 1]))),
+                        fmaxf(__uint_as_float(acc[c][j4 * 4 + 2]), __uint_as_float(acc[c][j4 * 4 + 3])));
+            }
+            cmax[c] = m;
+          }
+          if (p.dbg_scores != nullptr && it == 0 && h == 0 && !(p.dbg_flags & 64)) {  // (group 0 owns tile 0)
+#pragma unroll
+            for (int c = 0; c < 4; ++c)
+#pragma unroll
+              for (int j = 0; j < 16; ++j)
+                p.dbg_scores[(static_cast<size_t>(blockIdx.x) * kTcQRows + r) * kTcTileN + c * 16 + j] =
+                    __uint_as_float(acc[c][j]);
+          }
+
+          t_fast += TCLK() - t_fast0;
+          // what this CTA can vouch for (published below): chunk maxima are distinct rows
+          if (!(booted && li == 0)) {
+            if (xm == 1) st.top[0] = fmaxf(st.top[0], fmaxf(fmaxf(cmax[0], cmax[1]), fmaxf(cmax[2], cmax[3])));
+            else { top4_insert(st.top, cmax[0]); top4_insert(st.top, cmax[1]); top4_insert(st.top, cmax[2]); top4_insert(st.top, cmax[3]); }
+          }
+          if (p.dbg_flags & 8) continue;
+          const long long t_ch0 = TCLK();
+          // A group of four scores whose max reaches this query's threshold goes out of line.
+          st.tau = fmaxf(st.tau, thr_now);
+          if (use_fifo) {
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              if (cmax[c] >= st.tau) {
+                if (fcnt > static_cast<int>(L.fifo_recs) - 4) {   // no room for four more groups: make room (rare)
+                  const long long t0 = TCLK();
+                  st = drain_fifo(st, fifo_a, ftag_a, fcnt, list_a, ksel, p.ids);
+                  fcnt = 0;
+                  ++nslow;
+                  t_slow += TCLK() - t0;
+                }
+#pragma unroll
+                for (int g = 0; g < 4; ++g) {   // park the groups that reach the threshold: two stores each, no call
+                  const float m4 = fmaxf(fmaxf(__uint_as_float(acc[c][4 * g]), __uint_as_float(acc[c][4 * g + 1])),
+                                         fmaxf(__uint_as_float(acc[c][4 * g + 2]), __uint_as_float(acc[c][4 * g + 3])));
+                  if (m4 >= st.tau) {
+                    asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(fifo_a + static_cast<uint32_t>(fcnt) * (kTcQRows * 16u)),
+                                 "r"(acc[c][4 * g]), "r"(acc[c][4 * g + 1]), "r"(acc[c][4 * g + 2]), "r"(acc[c][4 * g + 3]) : "memory");
+                    asm volatile("st.shared.b32 [%0], %1;" ::"r"(ftag_a + static_cast<uint32_t>(fcnt) * (kTcQRows * 4u)),
+                                 "r"(hrow0 + c * 16 + 4 * g) : "memory");
+                    ++fcnt;
+                  }
                 }
               }
             }
-          }
-        } else {
+          } else {
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          if (cmax[c] >= st.tau) {
-            const long long t0 = TCLK();
+          for (int c = 0; c < 4; ++c) {
+            if (cmax[c] >= st.tau) {
+              const long long t0 = TCLK();
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              const float s0 = __uint_as_float(acc[c][4 * g]), s1 = __uint_as_float(acc[c][4 * g + 1]);
-              const float s2 = __uint_as_float(acc[c][4 * g + 2]), s3 = __uint_as_float(acc[c][4 * g + 3]);
-              if (fmaxf(fmaxf(s0, s1), fmaxf(s2, s3)) >= st.tau)
-                st = push_group4(st, s0, s1, s2, s3, row0 + c * 16 + 4 * g, list_a, ksel, p.ids);
+              for (int g = 0; g < 4; ++g) {
+                const float s0 = __uint_as_float(acc[c][4 * g]), s1 = __uint_as_float(acc[c][4 * g + 1]);
+                const float s2 = __uint_as_float(acc[c][4 * g + 2]), s3 = __uint_as_float(acc[c][4 * g + 3]);
+                if (fmaxf(fmaxf(s0, s1), fmaxf(s2, s3)) >= st.tau)
+                  st = push_group4(st, s0, s1, s2, s3, hrow0 + c * 16 + 4 * g, list_a, ksel, p.ids);
+              }
+              ++nslow;
+              t_slow += TCLK() - t0;
             }
-            ++nslow;
-            t_slow += TCLK() - t0;
           }
-        }
-        }
+          }
 
-        if (li < 8) t_top += TCLK() - t_ch0; else t_chunks += TCLK() - t_ch0;   // t_top reused: early tiles
+          if (li < 8) t_top += TCLK() - t_ch0; else t_chunks += TCLK() - t_ch0;   // t_top reused: early tiles
+        }
+        if (p.dbg_flags & (1 | 4 | 8)) continue;
         const long long t_pub0 = TCLK();
         // publish this CTA's m-th best for the exchange (monotone, so stale reads stay valid)
         const float pv = top4_get(st.top, xm);
@@ -839,9 +873,9 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   if constexpr (kCtaGroup == 2) cluster_sync_all();
 }
 
-template <int kCtaGroup, int kEpiGroups, bool kMask>
+template <int kCtaGroup, int kEpiGroups, bool kMask, int kTileN>
 cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm, const TcParams& p, size_t smem) {
-  auto kern = simtopk_tc_kernel<kCtaGroup, kEpiGroups, kMask>;
+  auto kern = simtopk_tc_kernel<kCtaGroup, kEpiGroups, kMask, kTileN>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
   return cudaLaunchKernelEx(&cfg, kern, tm, p);
@@ -849,17 +883,17 @@ cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm,
 
 }  // namespace
 
-size_t tc_smem_bytes(int epi_groups, int num_stages, int ksel, int dim) {
-  return make_layout(epi_groups, num_stages, ksel, dim).total + 1024;  // + alignment slack
+size_t tc_smem_bytes(int epi_groups, int num_stages, int ksel, int dim, int tile_n, bool mask) {
+  return make_layout(epi_groups, num_stages, ksel, dim, tile_n, mask).total + 1024;  // + alignment slack
 }
 
-int tc_pick_stages(int epi_groups, int ksel, int dim, size_t smem_limit) {
+int tc_pick_stages(int epi_groups, int ksel, int dim, size_t smem_limit, int tile_n, bool mask) {
   for (int s = kTcMaxStages; s >= 2; --s)
-    if (tc_smem_bytes(epi_groups, s, ksel, dim) <= smem_limit) return s;
+    if (tc_smem_bytes(epi_groups, s, ksel, dim, tile_n, mask) <= smem_limit) return s;
   return 0;
 }
 
-cudaError_t tc_launch(int cta_group, int epi_groups, int grid, const void* tmap, const TcParams& p, size_t smem,
+cudaError_t tc_launch(int cta_group, int epi_groups, int tile_n, int grid, const void* tmap, const TcParams& p, size_t smem,
                       cudaStream_t s) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
@@ -875,12 +909,17 @@ cudaError_t tc_launch(int cta_group, int epi_groups, int grid, const void* tmap,
   cfg.numAttrs = 1;
   const CUtensorMap& tm = *reinterpret_cast<const CUtensorMap*>(tmap);
   const bool mask = p.row_mask != nullptr;
-  if (cta_group == 2) {
-    if (epi_groups == 2) return mask ? launch_variant<2, 2, true>(cfg, tm, p, smem) : launch_variant<2, 2, false>(cfg, tm, p, smem);
-    return mask ? launch_variant<2, 1, true>(cfg, tm, p, smem) : launch_variant<2, 1, false>(cfg, tm, p, smem);
+  if (tile_n == kTcTileWide) {   // one epilogue group only
+    if (epi_groups != 1) return cudaErrorInvalidValue;
+    if (cta_group == 2) return mask ? launch_variant<2, 1, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<2, 1, false, kTcTileWide>(cfg, tm, p, smem);
+    return mask ? launch_variant<1, 1, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<1, 1, false, kTcTileWide>(cfg, tm, p, smem);
   }
-  if (epi_groups == 2) return mask ? launch_variant<1, 2, true>(cfg, tm, p, smem) : launch_variant<1, 2, false>(cfg, tm, p, smem);
-  return mask ? launch_variant<1, 1, true>(cfg, tm, p, smem) : launch_variant<1, 1, false>(cfg, tm, p, smem);
+  if (cta_group == 2) {
+    if (epi_groups == 2) return mask ? launch_variant<2, 2, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<2, 2, false, kTcTileN>(cfg, tm, p, smem);
+    return mask ? launch_variant<2, 1, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<2, 1, false, kTcTileN>(cfg, tm, p, smem);
+  }
+  if (epi_groups == 2) return mask ? launch_variant<1, 2, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<1, 2, false, kTcTileN>(cfg, tm, p, smem);
+  return mask ? launch_variant<1, 1, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<1, 1, false, kTcTileN>(cfg, tm, p, smem);
 }
 
 }  // namespace aur

@@ -86,7 +86,7 @@ typedef struct aur_stats {
   float   last_merge_ms; /* aur_search_exchange_dev: delivery wait + cross-shard merge; else ~0           */
   int64_t last_candidates;     /* candidate keys the last search's exact re-rank read, summed over its queries */
   int32_t last_candidates_max; /* the most any one query of the last search carried into the re-rank          */
-  int32_t reserved;
+  int32_t last_tile_n;   /* corpus rows per tile of the last search's tensor-core kernel (64, 128; 0: none) */
 } aur_stats;
 
 int aur_abi_version(void);
@@ -98,7 +98,8 @@ int aur_device_count(void);
 int aur_open(const aur_config* cfg, aur_index** out);
 int aur_close(aur_index* ix);
 int aur_get_stats(aur_index* ix, aur_stats* out);
-/* Options: "kernel" (aur_kernel), "epi_groups"; bring-up only: "dbg_flags", and "dbg_epoch" (1 .. 2^31 - 1), which
+/* Options: "kernel" (aur_kernel), "epi_groups", "tc_tile" (corpus rows per tensor-core tile: 0 = auto, 64 or 128;
+ * 128 needs epi_groups 1, and a search it does not fit fails); bring-up only: "dbg_flags", and "dbg_epoch" (1 .. 2^31 - 1), which
  * sets the tensor-core kernel's launch counter of every search context of the index, e.g. just before it wraps. */
 int aur_set_option(aur_index* ix, const char* key, int64_t value);
 int aur_sync(aur_index* ix);
