@@ -18,12 +18,13 @@ AUR_ERR_INVALID, AUR_ERR_CUDA, AUR_ERR_NOMEM, AUR_ERR_UNSUPPORTED, AUR_ERR_NO_DE
 AUR_BF16, AUR_F32 = 0, 1
 KERNEL_AUTO, KERNEL_SIMT, KERNEL_TC1, KERNEL_TC2, KERNEL_LIST = 0, 1, 2, 3, 4
 KERNEL_NAMES = {0: "auto", 1: "simt", 2: "wgmma-cta1", 3: "wgmma-cluster2", 4: "list"}
+FILTER_LEAF, FILTER_AND, FILTER_OR = 0, 1, 2   # filter program tokens (AUR_FILTER_*)
 TC_QUERY_ROWS = 64   # queries per CTA of the tensor-core kernel (kTcQRows, csrc/internal.h): the debug-score row count
 
 # every symbol include/aurora_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "aur_abi_version", "aur_last_error", "aur_device_count", "aur_open", "aur_close", "aur_get_stats",
-    "aur_set_option", "aur_sync", "aur_add", "aur_add_dev", "aur_export", "aur_read_rows", "aur_compact", "aur_remove", "aur_search", "aur_search_ex", "aur_search_subset", "aur_search_lists", "aur_search_dev",
+    "aur_set_option", "aur_sync", "aur_add", "aur_add_dev", "aur_export", "aur_read_rows", "aur_compact", "aur_remove", "aur_search", "aur_search_ex", "aur_search_subset", "aur_search_lists", "aur_set_attrs", "aur_search_filtered", "aur_filter_ids", "aur_search_dev",
     "aur_merge_topk_dev", "aur_merge_topk_packed_dev", "aur_merge_topk_host", "aur_merge_topk_host_f64", "aur_exchange_create", "aur_exchange_connect", "aur_exchange_close",
     "aur_exchange_status", "aur_search_exchange_dev", "aur_cosine_pairs", "aur_dev_malloc", "aur_dev_free", "aur_memcpy_h2d", "aur_memcpy_d2h",
     "aur_debug_tc_scores",
@@ -109,6 +110,9 @@ def load():
         "aur_search_subset": (C.c_int, [vp, vp, i32, i32, vp, i64, vp, vp]),
         "aur_search_lists": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, vp, vp, vp, C.POINTER(i64)]),
         "aur_search": (C.c_int, [vp, vp, i32, i32, vp, vp, vp, vp]),
+        "aur_set_attrs": (C.c_int, [vp, i32, vp, vp, i64]),
+        "aur_search_filtered": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, vp, i64, vp, i64, vp, vp, vp, C.POINTER(i64)]),
+        "aur_filter_ids": (C.c_int, [vp, vp, i32, vp, i64, vp, i64, C.POINTER(i64)]),
         "aur_search_dev": (C.c_int, [vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]),
         "aur_merge_topk_dev": (C.c_int, [i32, vp, vp, i32, i32, i32, vp, vp, vp, vp]),
         "aur_merge_topk_host": (C.c_int, [vp, vp, i32, i32, i32, i32, vp, vp]),

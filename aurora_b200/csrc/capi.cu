@@ -3,6 +3,7 @@
 //                              coalesced for everything else)
 //   inv_norm  [capacity] f32   1/|row|; 0 for zero rows; NaN marks a tombstone
 //   ids       [capacity] i64   caller ids;  user / org [capacity] i32 tenant codes
+//   attr      up to 16 x [capacity] i32 attribute codes for device-evaluated filters (allocated on first aur_set_attrs)
 // plus grow-only scratch for candidate lists.  No CPU compute path exists here: without
 // a CUDA device every entry point fails with AUR_ERR_NO_DEVICE.
 //
@@ -136,10 +137,16 @@ struct SearchCtx {
   DevBuf<int64_t> stage_ids;
   DevBuf<int32_t> list_stage;    // list search: work items, their queries and the lists' resolved rows (one upload)
   DevBuf<float> list_scores;     // list search: scores of a batch of work items, [slots][kSimtSeg]
+  DevBuf<int32_t> filt_stage;    // filtered search: the programs' tokens, offsets and bitmaps (one upload)
+  DevBuf<uint32_t> filt_mask;    // filtered search: per row, bit q = program q matches
+  DevBuf<uint32_t> filt_counts;  // filtered search: [32] totals, then [n_programs][blocks] counts (scanned into offsets)
+  DevBuf<int32_t> filt_rows;     // filtered search: every program's matching rows, ascending, program after program
+  DevBuf<int64_t> filt_ids;      // aur_filter_ids: their ids
   void release() {
     cand_a.release(); cand_b.release(); pub.release(); cand_count.release(); d_epoch.release(); cand_read.release(); score_chunk.release(); masked_inv.release();
     allow_rows.release(); row_mask.release(); scope_tab.release(); q_scope.release(); stage_q.release(); stage_quser.release(); stage_qorg.release(); stage_scores.release();
     stage_ids.release(); list_stage.release(); list_scores.release();
+    filt_stage.release(); filt_mask.release(); filt_counts.release(); filt_rows.release(); filt_ids.release();
     if (ev_begin) cudaEventDestroy(ev_begin);
     if (ev_k0) cudaEventDestroy(ev_k0);
     if (ev_k1) cudaEventDestroy(ev_k1);
@@ -162,6 +169,8 @@ struct aur_index {
   int64_t* d_ids = nullptr;
   int32_t* d_user = nullptr;
   int32_t* d_org = nullptr;
+  int32_t* d_attr[kFiltAttrCols] = {};   // attribute columns (program columns 2..), allocated on first aur_set_attrs; guarded by mu
+  DevBuf<int32_t> attr_stage;            // aur_set_attrs: (row, code) pairs (writers hold mu_write)
   std::unordered_map<int64_t, int64_t> id2row;
   cudaStream_t stream = nullptr;         // the index's own stream: device-pointer calls with stream == NULL
   cudaStream_t ingest_stream = nullptr;  // host appends / tombstones, lowest priority so queries overtake them
@@ -335,12 +344,13 @@ struct Scope {
   const int32_t* scope_tab = nullptr;    // device [n_scopes][2]: the batch's distinct tenant scopes, when there are <= 32
   const int32_t* q_scope = nullptr;      // device [nq]: scope index of every query
   int n_scopes = 0;
+  const uint32_t* match_mask = nullptr;  // device [n_rows]: rows with bit 0 set stay visible (a device-evaluated filter)
 };
 
 // Enqueues one search over the published prefix `n_rows` on stream s using context c.
 int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k, const Scope& sc, int64_t n_rows,
                    float* scores, int64_t* ids, double* scores64, cudaStream_t s,
-                   const FinalizeArgs::ExchangeOut* ex = nullptr) {
+                   const FinalizeArgs::ExchangeOut* ex = nullptr, bool begun = false) {
   if (nq <= 0 || k <= 0) return fail(AUR_ERR_INVALID, "nq and k must be positive");
   if (k > kMaxK) return fail(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
   if (nq > 65535) return fail(AUR_ERR_UNSUPPORTED, "nq > 65535: split the batch");
@@ -354,12 +364,12 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
     return fail(AUR_ERR_UNSUPPORTED, "tensor-core path needs bf16, dim %% 64 == 0, dim <= %d, no per-query tenant filter, and k small "
                 "enough for its shared-memory lists at this dim", kTcMaxDim);
   c->last_kernel = kernel;
-  c->last_launches = 0;
+  if (!begun) c->last_launches = 0;
   c->last_nq = nq;
   c->last_tile_n = 0;
   CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
   c->snapshot_rows = n_rows;
-  CU_TRY(cudaEventRecord(c->ev_begin, s));
+  if (!begun) CU_TRY(cudaEventRecord(c->ev_begin, s));
   bool k_timed = false;
   const float* inv = nullptr;   // masked inverse norms (nullptr = the shard's own)
   if (subset && n_rows > 0) {
@@ -367,6 +377,11 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
     CU_TRY(launch_fill_f32(c->masked_inv.p, nanf(""), n_rows, s));
     CU_TRY(launch_scatter_inv_norm(ix->d_inv_norm, sc.allow_rows, sc.n_allow, n_rows, c->masked_inv.p, s));
     c->last_launches += 2;
+    inv = c->masked_inv.p;
+  } else if (sc.match_mask && n_rows > 0) {
+    CU_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
+    CU_TRY(launch_mask_match(ix->d_inv_norm, sc.match_mask, n_rows, c->masked_inv.p, s));
+    ++c->last_launches;
     inv = c->masked_inv.p;
   } else if (kernel != AUR_KERNEL_SIMT && scoped_tc && n_rows > 0) {              // up to 32 scopes in the batch: row bit masks
     CU_TRY(c->row_mask.reserve(static_cast<size_t>(ix->capacity) + 64));
@@ -630,59 +645,25 @@ int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, 
 constexpr int kListQBlock = 1024;
 constexpr int64_t kListScoreSlots = 16384;   // 128 MB of scores
 
-int search_lists_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int64_t* list_ids,
-                      const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list, float* scores_out,
-                      int64_t* ids_out, int64_t* snapshot_out) {
-  int rc = check_search_args(ix, queries_host, nq, k, scores_out, ids_out);
+int check_list_args(aur_index* ix, const void* q, int32_t nq, int32_t k, const void* s_out, const void* i_out) {
+  int rc = check_search_args(ix, q, nq, k, s_out, i_out);
   if (rc != AUR_OK) return rc;
   if (k > kMaxK) return fail(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
   if (nq > 65535) return fail(AUR_ERR_UNSUPPORTED, "nq > 65535: split the batch");
   if (ix->dtype != AUR_BF16) return fail(AUR_ERR_UNSUPPORTED, "list search needs a bf16 index");
-  if (!list_offsets || !q_list || n_lists < 1) return fail(AUR_ERR_INVALID, "list_offsets, q_list and n_lists >= 1 are required");
-  if (list_offsets[0] != 0) return fail(AUR_ERR_INVALID, "list_offsets[0] must be 0");
-  for (int32_t l = 0; l < n_lists; ++l)
-    if (list_offsets[l + 1] < list_offsets[l]) return fail(AUR_ERR_INVALID, "list_offsets decrease at list %d", l);
-  if (list_offsets[n_lists] > 0 && !list_ids) return fail(AUR_ERR_INVALID, "list_ids is required");
-  for (int32_t q = 0; q < nq; ++q)
-    if (q_list[q] < 0 || q_list[q] >= n_lists) return fail(AUR_ERR_INVALID, "q_list[%d] = %d is not a list", q, q_list[q]);
+  return AUR_OK;
+}
 
-  std::shared_lock<std::shared_mutex> rl(ix->rw);
-  CU_TRY(cudaSetDevice(ix->device));
-  SearchCtx* c = nullptr;
-  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
-  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
-  std::lock_guard<std::mutex> cl(c->mu);
-  cudaStream_t s = c->own_stream;
-  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
+// The device side of a list search once every list's rows are known: work items built on the host from the lists'
+// lengths alone, launched in batches, folded and re-ranked exactly, results copied to the caller's buffers.  List l is
+// rows list_rows[lrow0[l] .. lrow0[l] + llen[l]), ascending and without repeats; list_rows = nullptr means the rows sit
+// at the front of `stage` (which is uploaded in one copy and extended here with the work items).  `begun`: the caller
+// already recorded ev_begin (its own kernels ran first on this stream).
+int run_list_search(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k,
+                    const int32_t* q_list, int32_t n_lists, const std::vector<int64_t>& lrow0, const std::vector<int64_t>& llen,
+                    std::vector<int32_t>& stage, const int32_t* list_rows, int64_t n_rows, bool begun, float* scores_out,
+                    int64_t* ids_out) {
   const int ksel = k + kSlack;
-
-  // ids -> rows of the published prefix (unknown / newer ids drop out), for the lists some query names
-  std::vector<std::vector<int32_t>> res(static_cast<size_t>(n_lists));
-  std::vector<char> named(static_cast<size_t>(n_lists), 0);
-  for (int32_t q = 0; q < nq; ++q) named[static_cast<size_t>(q_list[q])] = 1;
-  {
-    std::lock_guard<std::mutex> lk(ix->mu);
-    for (int32_t l = 0; l < n_lists; ++l) {
-      if (!named[static_cast<size_t>(l)]) continue;
-      std::vector<int32_t>& r = res[static_cast<size_t>(l)];
-      for (int64_t i = list_offsets[l]; i < list_offsets[l + 1]; ++i) {
-        auto it = ix->id2row.find(list_ids[i]);
-        if (it != ix->id2row.end() && it->second < n_rows) r.push_back(static_cast<int32_t>(it->second));
-      }
-    }
-  }
-  // staging (int32): [every named list's rows, sorted, once each][per block: its queries' positions, its items]
-  std::vector<int32_t> stage;
-  std::vector<int64_t> lrow0(static_cast<size_t>(n_lists), 0), llen(static_cast<size_t>(n_lists), 0);
-  for (int32_t l = 0; l < n_lists; ++l) {
-    std::vector<int32_t>& r = res[static_cast<size_t>(l)];
-    std::sort(r.begin(), r.end());
-    r.erase(std::unique(r.begin(), r.end()), r.end());
-    lrow0[static_cast<size_t>(l)] = static_cast<int64_t>(stage.size());
-    llen[static_cast<size_t>(l)] = static_cast<int64_t>(r.size());
-    stage.insert(stage.end(), r.begin(), r.end());
-    std::vector<int32_t>().swap(r);
-  }
   struct Launch { size_t items; int n_items, max_nq; };
   struct Block { int q0, nqb, n_segs; std::vector<Launch> launches; };
   std::vector<Block> blocks;
@@ -754,11 +735,11 @@ int search_lists_host(aur_index* ix, const void* queries_host, int32_t nq, int32
 
   auto enqueue = [&]() -> int {
     c->last_kernel = AUR_KERNEL_LIST;
-    c->last_launches = 0;
+    if (!begun) c->last_launches = 0;
     c->last_tile_n = 0;
     c->last_nq = nq;
     c->snapshot_rows = n_rows;
-    CU_TRY(cudaEventRecord(c->ev_begin, s));
+    if (!begun) CU_TRY(cudaEventRecord(c->ev_begin, s));
     CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
     CU_TRY(cudaMemcpyAsync(c->list_stage.p, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, s));
     for (size_t bi = 0; bi < blocks.size(); ++bi) {
@@ -775,7 +756,7 @@ int search_lists_host(aur_index* ix, const void* queries_host, int32_t nq, int32
         p.ids = ix->d_ids;
         p.items = reinterpret_cast<const ListItem*>(c->list_stage.p + ln.items);
         p.n_items = ln.n_items;
-        p.list_rows = c->list_stage.p;
+        p.list_rows = list_rows ? list_rows : c->list_stage.p;
         p.qidx = c->list_stage.p;
         p.scores = c->list_scores.p;
         p.cand = c->cand_a.p;
@@ -815,14 +796,174 @@ int search_lists_host(aur_index* ix, const void* queries_host, int32_t nq, int32
     }
     return AUR_OK;
   };
-  rc = enqueue();
+  int rc = enqueue();
   if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
   if (!direct) {
     CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
     CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
   }
   CU_TRY(cudaStreamSynchronize(s));
+  return AUR_OK;
+}
+
+int search_lists_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int64_t* list_ids,
+                      const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list, float* scores_out,
+                      int64_t* ids_out, int64_t* snapshot_out) {
+  int rc = check_list_args(ix, queries_host, nq, k, scores_out, ids_out);
+  if (rc != AUR_OK) return rc;
+  if (!list_offsets || !q_list || n_lists < 1) return fail(AUR_ERR_INVALID, "list_offsets, q_list and n_lists >= 1 are required");
+  if (list_offsets[0] != 0) return fail(AUR_ERR_INVALID, "list_offsets[0] must be 0");
+  for (int32_t l = 0; l < n_lists; ++l)
+    if (list_offsets[l + 1] < list_offsets[l]) return fail(AUR_ERR_INVALID, "list_offsets decrease at list %d", l);
+  if (list_offsets[n_lists] > 0 && !list_ids) return fail(AUR_ERR_INVALID, "list_ids is required");
+  for (int32_t q = 0; q < nq; ++q)
+    if (q_list[q] < 0 || q_list[q] >= n_lists) return fail(AUR_ERR_INVALID, "q_list[%d] = %d is not a list", q, q_list[q]);
+
+  std::shared_lock<std::shared_mutex> rl(ix->rw);
+  CU_TRY(cudaSetDevice(ix->device));
+  SearchCtx* c = nullptr;
+  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
+  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
+  std::lock_guard<std::mutex> cl(c->mu);
+  cudaStream_t s = c->own_stream;
+  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
+
+  // ids -> rows of the published prefix (unknown / newer ids drop out), for the lists some query names
+  std::vector<std::vector<int32_t>> res(static_cast<size_t>(n_lists));
+  std::vector<char> named(static_cast<size_t>(n_lists), 0);
+  for (int32_t q = 0; q < nq; ++q) named[static_cast<size_t>(q_list[q])] = 1;
+  {
+    std::lock_guard<std::mutex> lk(ix->mu);
+    for (int32_t l = 0; l < n_lists; ++l) {
+      if (!named[static_cast<size_t>(l)]) continue;
+      std::vector<int32_t>& r = res[static_cast<size_t>(l)];
+      for (int64_t i = list_offsets[l]; i < list_offsets[l + 1]; ++i) {
+        auto it = ix->id2row.find(list_ids[i]);
+        if (it != ix->id2row.end() && it->second < n_rows) r.push_back(static_cast<int32_t>(it->second));
+      }
+    }
+  }
+  // staging (int32): [every named list's rows, sorted, once each][per block: its queries' positions, its items]
+  std::vector<int32_t> stage;
+  std::vector<int64_t> lrow0(static_cast<size_t>(n_lists), 0), llen(static_cast<size_t>(n_lists), 0);
+  for (int32_t l = 0; l < n_lists; ++l) {
+    std::vector<int32_t>& r = res[static_cast<size_t>(l)];
+    std::sort(r.begin(), r.end());
+    r.erase(std::unique(r.begin(), r.end()), r.end());
+    lrow0[static_cast<size_t>(l)] = static_cast<int64_t>(stage.size());
+    llen[static_cast<size_t>(l)] = static_cast<int64_t>(r.size());
+    stage.insert(stage.end(), r.begin(), r.end());
+    std::vector<int32_t>().swap(r);
+  }
+  rc = run_list_search(ix, c, s, queries_host, nq, k, q_list, n_lists, lrow0, llen, stage, nullptr, n_rows, false, scores_out,
+                       ids_out);
+  if (rc != AUR_OK) return rc;
   if (snapshot_out) *snapshot_out = n_rows;
+  return AUR_OK;
+}
+
+// Filter programs (aur_search_filtered, aur_filter_ids): n_programs programs, program q = tokens
+// prog[4 * prog_off[q] .. 4 * prog_off[q + 1]), each token {kind, column, bitmap offset, bitmap length}.
+int check_programs(aur_index* ix, const int32_t* prog, const int32_t* prog_off, int32_t n_programs, const uint32_t* bitmap,
+                   int64_t bitmap_words) {
+  if (!prog || !prog_off) return fail(AUR_ERR_INVALID, "null program");
+  if (n_programs < 1 || n_programs > kFiltCallPrograms) return fail(AUR_ERR_INVALID, "1 <= n_programs <= %d", kFiltCallPrograms);
+  if (bitmap_words < 0 || (bitmap_words > 0 && !bitmap)) return fail(AUR_ERR_INVALID, "bitmap / bitmap_words");
+  if (prog_off[0] != 0) return fail(AUR_ERR_INVALID, "program offsets must start at 0");
+  std::lock_guard<std::mutex> lk(ix->mu);   // the attribute columns that exist
+  for (int32_t q = 0; q < n_programs; ++q) {
+    if (prog_off[q + 1] < prog_off[q]) return fail(AUR_ERR_INVALID, "program offsets decrease at program %d", q);
+    int depth = 0, leaves = 0;
+    for (int32_t t = prog_off[q]; t < prog_off[q + 1]; ++t) {
+      const int32_t* tk = prog + 4 * static_cast<int64_t>(t);
+      if (tk[0] == kFiltLeaf) {
+        if (++leaves > kFiltMaxLeaves) return fail(AUR_ERR_INVALID, "program %d has more than %d leaves", q, kFiltMaxLeaves);
+        if (tk[1] < 0 || tk[1] >= kFiltCols) return fail(AUR_ERR_INVALID, "program %d: column %d out of range", q, tk[1]);
+        if (tk[1] >= 2 && !ix->d_attr[tk[1] - 2]) return fail(AUR_ERR_INVALID, "program %d: column %d was never set", q, tk[1]);
+        if (tk[2] < 0 || tk[3] < 0 || static_cast<int64_t>(tk[2]) + tk[3] > bitmap_words * 32)
+          return fail(AUR_ERR_INVALID, "program %d: bitmap slice [%d, +%d) outside the bitmap", q, tk[2], tk[3]);
+        ++depth;
+      } else if (tk[0] == kFiltAnd || tk[0] == kFiltOr) {
+        if (depth < 2) return fail(AUR_ERR_INVALID, "program %d: operator without two operands", q);
+        --depth;
+      } else {
+        return fail(AUR_ERR_INVALID, "program %d: unknown token kind %d", q, tk[0]);
+      }
+    }
+    if (depth != 1) return fail(AUR_ERR_INVALID, "program %d leaves %d values, not one", q, depth);
+  }
+  return AUR_OK;
+}
+
+// Where pass `ps` of a filter evaluation (programs 32 ps .. 32 ps + 31) keeps its data: c->filt_mask holds one mask per
+// pass, c->filt_counts every pass's 32 totals and then every pass's block counts.
+struct FiltPass { uint32_t* mask; uint32_t* totals; uint32_t* counts; int n_programs; };
+FiltPass filt_pass(SearchCtx* c, int ps, int n_programs, int64_t n_rows) {
+  const int n_passes = (n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms;
+  const size_t rows = static_cast<size_t>(std::max<int64_t>(n_rows, 1)), nb = static_cast<size_t>(std::max(filter_blocks(n_rows), 1));
+  return FiltPass{c->filt_mask.p + ps * rows, c->filt_counts.p + ps * kFiltMaxPrograms,
+                  c->filt_counts.p + static_cast<size_t>(n_passes) * kFiltMaxPrograms + ps * kFiltMaxPrograms * nb,
+                  std::min(kFiltMaxPrograms, n_programs - ps * kFiltMaxPrograms)};
+}
+
+// Uploads checked programs, evaluates them over the snapshot's rows [0, n_rows) in passes of up to 32 programs (masks
+// and counts in c->filt_mask / c->filt_counts, filt_pass) and reads back each program's number of matching rows (one
+// small copy and a sync for all passes).
+int filter_count(aur_index* ix, SearchCtx* c, cudaStream_t s, const int32_t* prog, const int32_t* prog_off, int32_t n_programs,
+                 const uint32_t* bitmap, int64_t bitmap_words, int64_t n_rows, std::vector<int64_t>* totals) {
+  const size_t n_tok = static_cast<size_t>(prog_off[n_programs]);
+  std::vector<int32_t> st(n_tok * 4 + static_cast<size_t>(n_programs) + 1 + static_cast<size_t>(bitmap_words));
+  if (n_tok) memcpy(st.data(), prog, n_tok * 16);
+  memcpy(st.data() + n_tok * 4, prog_off, (static_cast<size_t>(n_programs) + 1) * 4);
+  if (bitmap_words) memcpy(st.data() + n_tok * 4 + n_programs + 1, bitmap, static_cast<size_t>(bitmap_words) * 4);
+  const int n_passes = (n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms;
+  const size_t nb = static_cast<size_t>(std::max(filter_blocks(n_rows), 1));
+  CU_TRY(c->filt_stage.reserve(st.size()));
+  CU_TRY(c->filt_mask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
+  CU_TRY(c->filt_counts.reserve(static_cast<size_t>(n_passes) * kFiltMaxPrograms * (1 + nb)));
+  CU_TRY(cudaMemcpyAsync(c->filt_stage.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice, s));   // pageable: staged on return
+  FiltParams p{};
+  p.cols[0] = ix->d_user; p.cols[1] = ix->d_org;
+  {
+    std::lock_guard<std::mutex> lk(ix->mu);
+    for (int i = 0; i < kFiltAttrCols; ++i) p.cols[2 + i] = ix->d_attr[i];
+  }
+  const int32_t* d_off = c->filt_stage.p + n_tok * 4;   // token indices stay absolute: a pass starts at its first offset
+  p.tok = reinterpret_cast<const FiltToken*>(c->filt_stage.p);
+  p.bitmap = reinterpret_cast<const uint32_t*>(d_off + n_programs + 1);
+  p.inv_norm = ix->d_inv_norm;
+  p.n_rows = n_rows;
+  for (int ps = 0; ps < n_passes; ++ps) {
+    const FiltPass fp = filt_pass(c, ps, n_programs, n_rows);
+    p.prog_off = d_off + ps * kFiltMaxPrograms;
+    p.n_programs = fp.n_programs;
+    CU_TRY(launch_filter_count(p, fp.mask, fp.counts, fp.totals, s));
+    ++c->last_launches;
+  }
+  std::vector<uint32_t> h(static_cast<size_t>(n_passes) * kFiltMaxPrograms);
+  CU_TRY(cudaMemcpyAsync(h.data(), c->filt_counts.p, h.size() * 4, cudaMemcpyDeviceToHost, s));
+  CU_TRY(cudaStreamSynchronize(s));
+  totals->assign(h.begin(), h.begin() + n_programs);   // pass ps's totals are words 32 ps .. 32 ps + 31: program order
+  return AUR_OK;
+}
+
+// After filter_count: every program's matching rows, ascending, program after program, into c->filt_rows (and with
+// `with_ids` their ids into c->filt_ids).
+int filter_write(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t n_programs, const std::vector<int64_t>& tot, int64_t n_rows,
+                 bool with_ids) {
+  int64_t total = 0;
+  for (int64_t t : tot) total += t;
+  if (total > INT32_MAX) return fail(AUR_ERR_UNSUPPORTED, "the programs of this call match too many rows for one call: split it");
+  CU_TRY(c->filt_rows.reserve(static_cast<size_t>(std::max<int64_t>(total, 1))));
+  if (with_ids) CU_TRY(c->filt_ids.reserve(static_cast<size_t>(std::max<int64_t>(total, 1))));
+  int64_t base = 0;
+  for (int ps = 0; ps * kFiltMaxPrograms < n_programs; ++ps) {
+    const FiltPass fp = filt_pass(c, ps, n_programs, n_rows);
+    CU_TRY(launch_filter_write(fp.mask, fp.counts, fp.totals, fp.n_programs, n_rows, with_ids ? ix->d_ids : nullptr,
+                               c->filt_rows.p + base, with_ids ? c->filt_ids.p + base : nullptr, s));
+    if (n_rows > 0) c->last_launches += 2;
+    for (int q = 0; q < fp.n_programs; ++q) base += tot[static_cast<size_t>(ps * kFiltMaxPrograms + q)];
+  }
   return AUR_OK;
 }
 
@@ -885,6 +1026,8 @@ int aur_close(aur_index* ix) {
   cudaSetDevice(ix->device);
   cudaDeviceSynchronize();   // searches bound to caller streams may still be in flight
   cudaFree(ix->d_rows); cudaFree(ix->d_inv_norm); cudaFree(ix->d_ids); cudaFree(ix->d_user); cudaFree(ix->d_org);
+  for (int32_t* a : ix->d_attr) cudaFree(a);
+  ix->attr_stage.release();
   for (auto& c : ix->ctxs) c->release();
   if (ix->stream) cudaStreamDestroy(ix->stream);
   if (ix->ingest_stream) cudaStreamDestroy(ix->ingest_stream);
@@ -977,14 +1120,20 @@ int aur_compact(aur_index* ix, int64_t* reclaimed) {
   // Stable compaction in place, a bounce buffer at a time: live row j moves down to row j.  Chunk [i0, i1) only
   // overwrites rows < i1 <= old(i1), i.e. rows whose content has already been gathered or moved.
   const int64_t chunk = 65536;
-  DevBuf<int32_t> d_map; DevBuf<uint8_t> bounce; DevBuf<float> b_inv; DevBuf<int64_t> b_ids; DevBuf<int32_t> b_user, b_org;
+  DevBuf<int32_t> d_map; DevBuf<uint8_t> bounce; DevBuf<float> b_inv; DevBuf<int64_t> b_ids; DevBuf<int32_t> b_user, b_org, b_attr;
+  std::vector<int32_t*> attrs;
+  {
+    std::lock_guard<std::mutex> lk(ix->mu);
+    for (int32_t* a : ix->d_attr) if (a) attrs.push_back(a);
+  }
   cudaError_t e = d_map.reserve(static_cast<size_t>(chunk));
   if (e == cudaSuccess) e = bounce.reserve(static_cast<size_t>(chunk) * ix->dim * ix->elt);
   if (e == cudaSuccess) e = b_inv.reserve(chunk);
   if (e == cudaSuccess) e = b_ids.reserve(chunk);
   if (e == cudaSuccess) e = b_user.reserve(chunk);
   if (e == cudaSuccess) e = b_org.reserve(chunk);
-  auto drop = [&]() { d_map.release(); bounce.release(); b_inv.release(); b_ids.release(); b_user.release(); b_org.release(); };
+  if (e == cudaSuccess && !attrs.empty()) e = b_attr.reserve(chunk);
+  auto drop = [&]() { d_map.release(); bounce.release(); b_inv.release(); b_ids.release(); b_user.release(); b_org.release(); b_attr.release(); };
   if (e != cudaSuccess) { drop(); return fail(AUR_ERR_NOMEM, "aur_compact: %s", cudaGetErrorString(e)); }
   cudaStream_t s = ix->ingest_stream;
   std::vector<int32_t> map_host(static_cast<size_t>(chunk));
@@ -1002,8 +1151,16 @@ int aur_compact(aur_index* ix, int64_t* reclaimed) {
     if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_ids + i0, b_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_user + i0, b_user.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_org + i0, b_org.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
+    for (int32_t* a : attrs) {
+      if (e == cudaSuccess) e = launch_gather_i32(a, d_map.p, m, b_attr.p, s);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(a + i0, b_attr.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
+    }
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);   // map_host is reused by the next chunk
   }
+  // the freed rows are appended to again: their attributes start absent, as in a fresh column
+  for (int32_t* a : attrs)
+    if (e == cudaSuccess) e = cudaMemsetAsync(a + nlive, 0xFF, static_cast<size_t>(rows - nlive) * 4, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   drop();
   if (e != cudaSuccess) return fail(AUR_ERR_CUDA, "aur_compact: %s (the shard may be inconsistent: restore the last snapshot)", cudaGetErrorString(e));
   {
@@ -1143,6 +1300,134 @@ int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_
                      int64_t* ids_out, int64_t* snapshot_rows_out) {
   return search_lists_host(ix, queries_host, nq, k, list_ids, list_offsets, n_lists, q_list, scores_out, ids_out,
                            snapshot_rows_out);
+}
+
+int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t* codes, int64_t n) {
+  if (!ix || n < 0 || (n > 0 && (!ids || !codes))) return fail(AUR_ERR_INVALID, "null argument");
+  if (col < 2 || col >= kFiltCols) return fail(AUR_ERR_INVALID, "attribute columns are 2 .. %d", kFiltCols - 1);
+  std::shared_lock<std::shared_mutex> rl(ix->rw);
+  std::lock_guard<std::mutex> wk(ix->mu_write);
+  CU_TRY(cudaSetDevice(ix->device));
+  cudaStream_t s = ix->ingest_stream;
+  int32_t* a = nullptr;
+  {
+    std::lock_guard<std::mutex> lk(ix->mu);
+    a = ix->d_attr[col - 2];
+  }
+  if (!a) {   // first use: every row absent (-1), at the padded capacity like the tenant codes
+    const int64_t cap_pad = (ix->capacity + kTcTileN - 1) / kTcTileN * kTcTileN;
+    cudaError_t e = cudaMalloc(&a, static_cast<size_t>(cap_pad) * 4);
+    if (e != cudaSuccess) return fail(AUR_ERR_NOMEM, "attribute column: %s", cudaGetErrorString(e));
+    e = cudaMemsetAsync(a, 0xFF, static_cast<size_t>(cap_pad) * 4, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { cudaFree(a); return fail(AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e)); }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    ix->d_attr[col - 2] = a;
+  }
+  std::vector<int32_t> pairs;
+  pairs.reserve(2 * static_cast<size_t>(n));
+  {
+    std::lock_guard<std::mutex> lk(ix->mu);
+    for (int64_t i = 0; i < n; ++i) {
+      auto it = ix->id2row.find(ids[i]);
+      if (it == ix->id2row.end()) continue;
+      pairs.push_back(static_cast<int32_t>(it->second));
+      pairs.push_back(codes[i]);
+    }
+  }
+  if (pairs.empty()) return AUR_OK;
+  CU_TRY(ix->attr_stage.reserve(pairs.size()));
+  CU_TRY(cudaMemcpyAsync(ix->attr_stage.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s));
+  CU_TRY(launch_scatter_codes(ix->attr_stage.p, static_cast<int64_t>(pairs.size() / 2), a, s));
+  CU_TRY(cudaStreamSynchronize(s));
+  return AUR_OK;
+}
+
+int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* prog,
+                        const int32_t* prog_offsets, int32_t n_programs, const uint32_t* bitmap, int64_t bitmap_words,
+                        const int32_t* q_program, int64_t max_list_rows, float* scores_out, int64_t* ids_out,
+                        int64_t* matched_out, int64_t* snapshot_rows_out) {
+  int rc = check_list_args(ix, queries_host, nq, k, scores_out, ids_out);
+  if (rc != AUR_OK) return rc;
+  if ((rc = check_programs(ix, prog, prog_offsets, n_programs, bitmap, bitmap_words)) != AUR_OK) return rc;
+  if (!q_program) return fail(AUR_ERR_INVALID, "q_program is required");
+  for (int32_t q = 0; q < nq; ++q)
+    if (q_program[q] < 0 || q_program[q] >= n_programs) return fail(AUR_ERR_INVALID, "q_program[%d] = %d is not a program", q, q_program[q]);
+  if (max_list_rows < 0) return fail(AUR_ERR_INVALID, "max_list_rows < 0");
+
+  std::shared_lock<std::shared_mutex> rl(ix->rw);
+  CU_TRY(cudaSetDevice(ix->device));
+  SearchCtx* c = nullptr;
+  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
+  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
+  std::lock_guard<std::mutex> cl(c->mu);
+  cudaStream_t s = c->own_stream;
+  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
+  c->last_launches = 0;
+  CU_TRY(cudaEventRecord(c->ev_begin, s));
+  std::vector<int64_t> tot;
+  if ((rc = filter_count(ix, c, s, prog, prog_offsets, n_programs, bitmap, bitmap_words, n_rows, &tot)) != AUR_OK) return rc;
+  if (n_programs == 1 && tot[0] > max_list_rows) {
+    // dense: the matching rows as a row mask, and the masked scan aur_search_subset runs
+    const size_t qbytes = static_cast<size_t>(nq) * ix->dim * 2;
+    const size_t nout = static_cast<size_t>(nq) * k;
+    CU_TRY(c->stage_q.reserve(qbytes));
+    CU_TRY(c->stage_scores.reserve(nout));
+    CU_TRY(c->stage_ids.reserve(nout));
+    CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
+    Scope sc;
+    sc.match_mask = c->filt_mask.p;
+    float* d_scores = c->stage_scores.p;
+    int64_t* d_ids = c->stage_ids.p;
+    const bool direct = direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
+    rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, d_scores, d_ids, nullptr, s, nullptr, true);
+    if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
+    if (!direct) {
+      CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
+      CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
+    }
+    CU_TRY(cudaStreamSynchronize(s));
+  } else {
+    // lists: every program's rows written on the device, in the order the host path stages them; items from the lengths
+    std::vector<int64_t> lrow0(static_cast<size_t>(n_programs), 0);
+    for (int32_t q = 1; q < n_programs; ++q)
+      lrow0[static_cast<size_t>(q)] = lrow0[static_cast<size_t>(q - 1)] + tot[static_cast<size_t>(q - 1)];
+    if ((rc = filter_write(ix, c, s, n_programs, tot, n_rows, false)) != AUR_OK) return rc;
+    std::vector<int32_t> stage;
+    rc = run_list_search(ix, c, s, queries_host, nq, k, q_program, n_programs, lrow0, tot, stage, c->filt_rows.p, n_rows, true,
+                         scores_out, ids_out);
+    if (rc != AUR_OK) return rc;
+  }
+  if (matched_out) for (int32_t q = 0; q < n_programs; ++q) matched_out[q] = tot[static_cast<size_t>(q)];
+  if (snapshot_rows_out) *snapshot_rows_out = n_rows;
+  return AUR_OK;
+}
+
+int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,
+                   int64_t* ids_out, int64_t cap, int64_t* n_out) {
+  if (!ix || !n_out || cap < 0 || (cap > 0 && !ids_out)) return fail(AUR_ERR_INVALID, "null argument");
+  if (n_tokens < 0) return fail(AUR_ERR_INVALID, "n_tokens < 0");
+  const int32_t off[2] = {0, n_tokens};
+  int rc = check_programs(ix, prog, off, 1, bitmap, bitmap_words);
+  if (rc != AUR_OK) return rc;
+  std::shared_lock<std::shared_mutex> rl(ix->rw);
+  CU_TRY(cudaSetDevice(ix->device));
+  SearchCtx* c = nullptr;
+  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
+  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
+  std::lock_guard<std::mutex> cl(c->mu);
+  cudaStream_t s = c->own_stream;
+  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
+  std::vector<int64_t> tot;
+  if ((rc = filter_count(ix, c, s, prog, off, 1, bitmap, bitmap_words, n_rows, &tot)) != AUR_OK) return rc;
+  const int64_t n = tot[0], m = std::min(n, cap);
+  if ((rc = filter_write(ix, c, s, 1, tot, n_rows, true)) != AUR_OK) return rc;
+  std::vector<int64_t> got(static_cast<size_t>(m));
+  if (m) CU_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToHost, s));
+  CU_TRY(cudaStreamSynchronize(s));
+  if (m) memcpy(ids_out, got.data(), static_cast<size_t>(m) * 8);
+  *n_out = n;
+  return AUR_OK;
 }
 
 

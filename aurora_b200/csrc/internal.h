@@ -191,6 +191,38 @@ struct ListParams {
 // Scores and per-segment selection of n_items work items; max_nq = the largest nq among them.
 cudaError_t launch_list_search(const ListParams& p, int max_nq, cudaStream_t s);
 
+// ---------------------------------------------------------------- metadata pre-filters (filter.cu)
+constexpr int kFiltAttrCols = 16;             // attribute columns per shard
+constexpr int kFiltCols = 2 + kFiltAttrCols;  // program columns: 0 = tenant user codes, 1 = org codes, 2.. attributes
+constexpr int kFiltMaxLeaves = 32;            // leaves per program (its evaluation stack is one 32-bit word)
+constexpr int kFiltMaxPrograms = 32;          // programs per pass (bit p of a row's match mask)
+constexpr int kFiltCallPrograms = 1024;       // programs per call, evaluated in passes of kFiltMaxPrograms
+constexpr int kFiltBlockRows = 2048;          // rows per CTA of the count and write kernels
+enum { kFiltLeaf = 0, kFiltAnd = 1, kFiltOr = 2 };
+struct FiltToken { int32_t kind, col, bm_off, bm_len; };   // bm_off / bm_len in bits; AND / OR ignore the rest
+struct FiltParams {
+  const int32_t* cols[kFiltCols];   // [n_rows] codes per column (only the columns the programs name are read)
+  const FiltToken* tok;             // every program's tokens, postfix
+  const int32_t* prog_off;          // [n_programs + 1] program q = tok[prog_off[q] .. prog_off[q + 1])
+  const uint32_t* bitmap;           // leaf bitmaps
+  const float* inv_norm;            // NaN = tombstone (never matches)
+  int64_t n_rows;                   // the search's snapshot
+  int n_programs;
+};
+int filter_blocks(int64_t n_rows);
+// mask [n_rows] (bit q = program q), block_counts [n_programs][filter_blocks(n_rows)], totals [32] (zeroed here)
+cudaError_t launch_filter_count(const FiltParams& p, uint32_t* mask, uint32_t* block_counts, uint32_t* totals, cudaStream_t s);
+// rows_out [sum of totals]: program q's matching rows, ascending, after those of programs < q; ids_out (nullable) their ids.
+// Scans block_counts in place.
+cudaError_t launch_filter_write(const uint32_t* mask, uint32_t* block_counts, const uint32_t* totals, int n_programs, int64_t n_rows,
+                                const int64_t* ids, int32_t* rows_out, int64_t* ids_out, cudaStream_t s);
+// out[i] = (mask[i] & 1) ? inv[i] : NaN
+cudaError_t launch_mask_match(const float* inv, const uint32_t* mask, int64_t n, float* out, cudaStream_t s);
+// col[pairs[2i]] = pairs[2i + 1]
+cudaError_t launch_scatter_codes(const int32_t* pairs, int64_t n, int32_t* col, cudaStream_t s);
+// out[i] = src[map[i]] (compaction of an attribute column)
+cudaError_t launch_gather_i32(const int32_t* src, const int32_t* map, int64_t n, int32_t* out, cudaStream_t s);
+
 // out[rows[i]] = inv[rows[i]] for the listed rows (out pre-filled with NaN): a resolved id subset as a row mask
 cudaError_t launch_scatter_inv_norm(const float* inv, const int32_t* rows, int64_t n, int64_t n_rows, float* out, cudaStream_t s);
 // compaction: rows map[0..n) (and their side arrays) -> bounce buffers

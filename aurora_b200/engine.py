@@ -187,6 +187,53 @@ class Index:
                                            _ptr(ql), _ptr(scores), _ptr(ids), C.byref(snap)))
         return ids, scores, int(snap.value)
 
+    # -------------------------------------------------------------- device-evaluated filters
+    def set_attrs(self, col: int, ids, codes) -> None:
+        """Attribute column ``col`` (2 .. 17) of the rows ``ids`` := ``codes`` (int32, -1 = absent); unknown ids are
+        ignored.  The column starts all absent on first use."""
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        codes = np.ascontiguousarray(codes, dtype=np.int32)
+        if codes.shape != ids.shape:
+            raise ValueError("ids and codes must have the same length")
+        N.check(self._lib.aur_set_attrs(self._h, int(col), _ptr(ids), _ptr(codes), ids.shape[0]))
+
+    def search_filtered(self, queries: np.ndarray, k: int, programs, q_program=None, max_list_rows: int = 0):
+        """Search with pre-filters evaluated on the device: query q sees the live rows ``programs[q_program[q]]`` matches
+        (``filters.compile_program`` outputs, at most 32; ``q_program`` None = every query on program 0).  One program
+        matching more than ``max_list_rows`` rows runs the masked full scan, anything else the list kernels.  Returns
+        (ids [nq,k] int64, scores [nq,k] float32, matching rows per program int64, snapshot rows)."""
+        from .filters import pack_programs
+
+        q = self._rows_buffer(queries)
+        nq = q.shape[0]
+        tok, off, bm = pack_programs(programs)
+        ql = np.zeros(nq, np.int32) if q_program is None else np.ascontiguousarray(q_program, dtype=np.int32)
+        if ql.shape != (nq,):
+            raise ValueError("q_program must be [nq]")
+        scores = np.empty((nq, k), dtype=np.float32)
+        ids = np.empty((nq, k), dtype=np.int64)
+        matched = np.zeros(len(programs), dtype=np.int64)
+        snap = C.c_int64(-1)
+        N.check(self._lib.aur_search_filtered(self._h, _ptr(q), nq, int(k), _ptr(tok), _ptr(off), len(programs), _ptr(bm),
+                                              bm.shape[0], _ptr(ql), int(max_list_rows), _ptr(scores), _ptr(ids),
+                                              _ptr(matched), C.byref(snap)))
+        return ids, scores, matched, int(snap.value)
+
+    def filter_ids(self, program) -> np.ndarray:
+        """Ids of the live rows one ``filters.compile_program`` program matches, in row order."""
+        from .filters import pack_programs
+
+        tok, _, bm = pack_programs([program])
+        cap = 1 << 16
+        while True:                 # the call reports the count: one retry with room for every match (more if rows arrive)
+            out = np.empty(cap, dtype=np.int64)
+            n = C.c_int64(0)
+            N.check(self._lib.aur_filter_ids(self._h, _ptr(tok), tok.shape[0], _ptr(bm), bm.shape[0], _ptr(out), cap,
+                                             C.byref(n)))
+            if n.value <= cap:
+                return out[:n.value]
+            cap = int(n.value)
+
     def search_dev(self, q_ptr: int, nq: int, k: int, scores_ptr: int, ids_ptr: int, scores64_ptr: int = 0,
                    q_user_ptr: int = 0, q_org_ptr: int = 0, stream: int = 0) -> None:
         """Everything in HBM; asynchronous on ``stream`` (0 = the index's own stream)."""
@@ -313,6 +360,22 @@ class MultiIndex:
         split = [self._split(a) for a in lists]
         return self._merge(self._each(lambda s, shard: shard.search_lists(
             queries, k, [ids[sel[s]] for ids, sel in split], q_list)), k)
+
+    def set_attrs(self, col: int, ids, codes) -> None:
+        ids, sel = self._split(ids)
+        codes = np.asarray(codes, dtype=np.int32)
+        self._each(lambda s, shard: shard.set_attrs(col, ids[sel[s]], codes[sel[s]]))   # every shard gets the column
+
+    def search_filtered(self, queries: np.ndarray, k: int, programs, q_program=None, max_list_rows: int = 0):
+        """Index.search_filtered on every shard, each with an even share of ``max_list_rows``; merged as search_lists.
+        Returns (ids, scores, matching rows per program summed over the shards, snapshot rows per shard)."""
+        share = int(max_list_rows) // len(self.shards)
+        parts = self._each(lambda s, shard: shard.search_filtered(queries, k, programs, q_program, share))
+        ids, sc = self._merge([(p[0], p[1]) for p in parts], k)
+        return ids, sc, np.sum([p[2] for p in parts], axis=0), [p[3] for p in parts]
+
+    def filter_ids(self, program) -> np.ndarray:
+        return np.concatenate(self._each(lambda s, shard: shard.filter_ids(program)))
 
     # -------------------------------------------------------------- maintenance
     def stats(self) -> dict:

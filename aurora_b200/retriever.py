@@ -34,8 +34,9 @@ from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import numpy as np
 
+from ._native import AUR_BF16
 from .bm25 import BM25Index
-from .filters import Filter, HybridFusion  # noqa: F401  (re-exported for call sites)
+from .filters import AttrColumn, Filter, HybridFusion, compile_program  # noqa: F401  (Filter, HybridFusion: re-exported)
 
 logger = logging.getLogger(__name__)
 
@@ -45,6 +46,7 @@ _MAX_FETCH = 128                        # engine's largest k
 # objects; above it the masked full scan (search_subset) answers sooner.  Measured at one query over 1M x 768 bf16
 # (DESIGN.md section 9, tools/list_bench.py): the list path wins at 3 000 rows (0.3 %), the full scan at 10 000 (1 %).
 _LIST_MAX_FRACTION = 0.005
+_ATTR_COLS = range(2, 18)               # the shard's attribute columns (include/aurora_b200.h, aur_set_attrs)
 
 
 def _sanitize(value: Any) -> str:
@@ -97,6 +99,11 @@ class KnowledgeBase:
         self._wal_sync = True
         self._replaying = False
         self._scope_cache: Dict[Tuple[Optional[str], Optional[str]], tuple] = {}   # tenant -> (mutations, id set, sorted ids)
+        # filters evaluated on the device: a property gets an attribute column of the shard the first time a filter names
+        # it, and keeps it current from then on (insert_objects)
+        self._attr_cols: Dict[str, AttrColumn] = {}
+        self._attr_free = list(_ATTR_COLS)
+        self._attr_host: set = set()    # properties with a value that has no code (unhashable): their filters stay on the host
 
     def _keyword_store(self, capacity: int):
         """``DeviceBM25`` on the vector index's GPU when that index is an ``engine.Index``; over a ``MultiIndex`` of them,
@@ -241,6 +248,8 @@ class KnowledgeBase:
                     self.sparse.add(rid, text)
             if self._kw_device:
                 self.sparse.add_many(ids, texts, ucode, ocode)
+            if self._attr_cols:             # before the lock is released: no query sees the new rows without their codes
+                self._set_attr_codes(np.unique(ids))
             self.mutations += len(objs)
             self._log({"op": "put", "gen": gen, "user": user_id, "org": org_id, "objs": [list(o) for o in objs]})
         return len(objs)
@@ -262,6 +271,66 @@ class KnowledgeBase:
         self._scope_cache[key] = (self.mutations, ids, arr)
         return ids, arr
 
+    # ------------------------------------------------------------------ device filters
+    def _set_attr_codes(self, rids: np.ndarray) -> None:
+        """Every attribute column's codes of the rows ``rids`` from their current properties.  Caller holds the lock."""
+        for name, col in list(self._attr_cols.items()):
+            try:
+                codes = np.array([col.code(self._props[int(r)]) for r in rids], dtype=np.int32)
+            except TypeError:               # a value without a code: this property's filters go back to the host path
+                del self._attr_cols[name]
+                self._attr_host.add(name)
+                self._attr_free.append(col.col)   # the slot serves the next property (its codes are rewritten then)
+                continue
+            self.index.set_attrs(col.col, rids, codes)
+
+    def _attr_column(self, name: str) -> AttrColumn:
+        """The attribute column of property ``name``, built from the whole table on first use.  Caller holds the lock."""
+        col = self._attr_cols.get(name)
+        if col is not None:
+            return col
+        if name in self._attr_host or not self._attr_free:
+            raise KeyError(name)
+        col = AttrColumn(name, self._attr_free[0])
+        rids = np.fromiter(self._props.keys(), dtype=np.int64, count=len(self._props))
+        try:
+            codes = np.array([col.code(self._props[int(r)]) for r in rids], dtype=np.int32)
+        except TypeError:
+            self._attr_host.add(name)
+            raise
+        self.index.set_attrs(col.col, rids, codes)
+        self._attr_free.pop(0)
+        self._attr_cols[name] = col
+        return col
+
+    def _device_program(self, filters, tenant: bool, user_id: Optional[str], org_id: Optional[str]):
+        """``filters`` AND the tenant scope as a device program over attribute columns, or None when the query is
+        resolved on the host: an index without device filters (CPU doubles, f32 shards), a property without a column, or
+        a leaf whose evaluation raises (the host path then raises as it always has).  The tenant scope is written over
+        the ``user_id`` / ``org_id`` properties, exactly as the host predicate reads it.  Caller holds the lock."""
+        if not hasattr(self.index, "search_filtered") or getattr(self.index, "dtype", None) != AUR_BF16:
+            return None
+        expr = filters
+        if tenant:
+            terms = ([Filter.by_property("user_id").equal(user_id)] if user_id else []) + \
+                    ([Filter.by_property("org_id").equal(org_id)] if org_id else [])
+            if not terms:
+                return None                 # matches nothing: the host path answers without a search
+            expr = filters & (terms[0] if len(terms) == 1 else terms[0] | terms[1])
+        names: List[str] = []
+
+        def walk(t):
+            if t[0] in ("and", "or"):
+                walk(t[1])
+                walk(t[2])
+            elif t[1] not in names:
+                names.append(t[1])
+        try:
+            walk(expr.tree)
+            return compile_program(expr, {n: self._attr_column(n) for n in names})
+        except Exception:                   # noqa: BLE001 - any failure keeps the host path and its behaviour
+            return None
+
     def _unindex(self, rid: int, props: Dict[str, Any]) -> None:
         self._by_user.get(props.get("user_id"), set()).discard(rid)
         if props.get("org_id"):
@@ -278,9 +347,10 @@ class KnowledgeBase:
         (1-alpha)/(rank+60), ``score`` = the fused score.
 
         Filters are PRE-filters, as in Weaviate: the tenant scope (user OR org) runs inside the kernel;
-        a ``filters`` expression is resolved against the metadata table to the set of allowed ids, and
-        the kernel then searches only those rows (``Index.search_subset``), so a small tenant's chunks
-        are found even when the global top-k belongs to other tenants.
+        a ``filters`` expression on a CUDA shard is compiled to a program over the shard's attribute
+        columns and evaluated there (``Index.search_filtered``); elsewhere it is resolved against the
+        metadata table to the set of allowed ids.  Either way the kernel searches only the matching rows,
+        so a small tenant's chunks are found even when the global top-k belongs to other tenants.
 
         ``scoped``: the caller is a tenant-facing entry point (search_knowledge_base): a missing user AND
         org matches nothing instead of everything (the reference always applies ``user_id == u``,
@@ -302,7 +372,8 @@ class KnowledgeBase:
                        (bool(org_id) and props.get("org_id") == org_id)
 
             allowed: Optional[List[int]] = None
-            if filters is not None:
+            prog = self._device_program(filters, tenant, user_id, org_id) if filters is not None else None
+            if filters is not None and prog is None:
                 # narrow the scan with the filter's own equality terms and the tenant scope, then run the predicate
                 eq = filters.required_equalities()
                 pools = []
@@ -318,9 +389,12 @@ class KnowledgeBase:
             dense: List[Tuple[int, float]] = []
             if _dense is not None:          # dense leg already computed by query_batch (same scope, same fetch)
                 dense = [(rid, sc) for rid, sc in _dense if rid in self._props]
-            elif qv is not None and (allowed is None or allowed):
+            elif qv is not None and (prog is not None or allowed is None or allowed):
                 fetch = max(1, min(_MAX_FETCH, limit if not hybrid else _MAX_FETCH))
-                if (allowed is not None and hasattr(self.index, "search_lists")
+                if prog is not None:        # no id crosses PCIe; the list-vs-scan rule is the host path's
+                    ids, scores, _, _ = self.index.search_filtered(
+                        qv, fetch, [prog], max_list_rows=int(_LIST_MAX_FRACTION * len(self._props)))
+                elif (allowed is not None and hasattr(self.index, "search_lists")
                         and len(allowed) <= _LIST_MAX_FRACTION * len(self._props)):   # reads only the allowed rows
                     ids, scores = self.index.search_lists(qv, fetch, [np.asarray(allowed, dtype=np.int64)],
                                                           np.zeros(1, np.int32))
@@ -343,6 +417,8 @@ class KnowledgeBase:
                 picked = [(rid, sc, sc) for rid, sc in dense[:limit]]
             else:
                 # keyword leg under the same pre-filter: the resolved filter's ids, else the tenant's own inverted lists
+                if prog is not None and _sparse is None:
+                    allowed = self.index.filter_ids(prog).tolist()
                 if _sparse is not None:     # keyword leg already computed by query_batch (same scope, same fetch);
                     # objects deleted since then drop out, as for the dense leg
                     sparse = [(rid, sc) for rid, sc in _sparse if rid in self._props]

@@ -176,6 +176,41 @@ int aur_search_subset(aur_index* ix, const void* queries_host, int32_t nq, int32
 int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_t k,
                      const int64_t* list_ids, const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list,
                      float* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out);
+/* Attribute columns and device-evaluated pre-filters.
+ *
+ * A shard carries up to 16 int32 attribute columns, numbered 2 .. 17 (columns 0 and 1 are the tenant user / org codes
+ * of aur_add).  A column is allocated on its first aur_set_attrs with every row absent (-1); rows appended later, the new
+ * row of an upsert and the rows compaction frees start absent too.  aur_set_attrs writes codes by id (unknown ids are
+ * ignored) and is serialised with the other writers.  A search sees a row's codes as they were when its filter kernel read
+ * them: a caller that must never answer from a row without its codes sets them before it lets searches name them.
+ *
+ * A filter program is a postfix sequence of tokens, 4 int32 each: {AUR_FILTER_LEAF, column, bitmap offset, bitmap length}
+ * or {AUR_FILTER_AND | AUR_FILTER_OR, 0, 0, 0}.  Offsets and lengths count bits of `bitmap` (bitmap_words uint32 words,
+ * bit i = word i / 32, bit i % 32).  A leaf is true for a row whose code c in that column has bit c + 1 of its slice set
+ * (bit 0: absent), so the tenant scope of aur_search, row_user == u OR (o >= 0 AND row_org == o), is the program
+ * [leaf(0, bit u + 1), leaf(1, bit o + 1), OR].  At most 32 leaves per program; only live rows of the search's snapshot
+ * match.  Malformed programs (stack underflow, not exactly one value left, more than 32 leaves, unknown token, a column
+ * out of range or never set, a slice outside the bitmap) are AUR_ERR_INVALID. */
+#define AUR_FILTER_LEAF 0
+#define AUR_FILTER_AND 1
+#define AUR_FILTER_OR 2
+int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t* codes, int64_t n);
+/* aur_search_lists with every list given as a filter program evaluated on the device: program p
+ * (tokens prog[4 * prog_offsets[p] .. 4 * prog_offsets[p + 1]), 1 <= n_programs <= 1024) selects the rows query q searches
+ * when q_program[q] = p.  The matching rows never leave the device, and no id is resolved on the host.  The programs are
+ * counted first, 32 per pass over the rows, with one small read-back for all passes; a call with one program whose matching rows exceed max_list_rows runs the masked
+ * full scan of aur_search_subset (aur_stats.last_kernel = the tensor-core or SIMT kernel), every other call the list kernels
+ * of aur_search_lists (AUR_KERNEL_LIST).  Either way the answer is bit for bit that of the corresponding host-resolved call
+ * over the matching ids.  matched_out [n_programs] (nullable) receives each program's matching rows.  bf16 indexes;
+ * threading, snapshot and page-locked outputs as for aur_search_lists. */
+int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* prog,
+                        const int32_t* prog_offsets, int32_t n_programs, const uint32_t* bitmap, int64_t bitmap_words,
+                        const int32_t* q_program, int64_t max_list_rows, float* scores_out, int64_t* ids_out,
+                        int64_t* matched_out, int64_t* snapshot_rows_out);
+/* The ids of the live rows one program (n_tokens tokens) matches, in row order: the first min(*n_out, cap) go to ids_out,
+ * *n_out receives how many there are (call again with a larger cap when it exceeds cap). */
+int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,
+                   int64_t* ids_out, int64_t cap, int64_t* n_out);
 /* Device variant: everything in HBM; scores64_dev (nullable) additionally receives the
  * fp64 ranking keys needed for an exact cross-shard merge. */
 int aur_search_dev(aur_index* ix, const void* queries_dev, int32_t nq, int32_t k,
