@@ -40,18 +40,6 @@ using namespace aur;
 namespace {
 
 thread_local std::string g_err;
-int fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);
-  g_err = buf;
-  return code;
-}
-#define CU_TRY(expr)                                                                               \
-  do {                                                                                             \
-    cudaError_t e_ = (expr);                                                                       \
-    if (e_ != cudaSuccess) return fail(AUR_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e_), \
-                                       __FILE__, __LINE__);                                        \
-  } while (0)
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -69,20 +57,6 @@ EncodeTiledFn get_encode_fn() {
   });
   return fn;
 }
-
-template <typename T>
-struct DevBuf {  // grow-only device scratch
-  T* p = nullptr; size_t n = 0;
-  cudaError_t reserve(size_t want) {
-    if (want <= n) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; n = 0;
-    cudaError_t e = cudaMalloc(&p, want * sizeof(T));
-    if (e == cudaSuccess) n = want;
-    return e;
-  }
-  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-};
 
 }  // namespace
 
@@ -107,6 +81,16 @@ int encode_tmap_2d_bf16(void* tmap, const void* base, uint64_t cols, uint64_t ro
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
 }
 }  // namespace aur
+
+namespace {
+int (&fail)(int, const char*, ...) = report_error;
+#define CU_TRY(expr)                                                                               \
+  do {                                                                                             \
+    cudaError_t e_ = (expr);                                                                       \
+    if (e_ != cudaSuccess) return fail(AUR_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e_), \
+                                       __FILE__, __LINE__);                                        \
+  } while (0)
+}  // namespace
 
 // Scratch and bookkeeping of ONE in-flight search.  Device-pointer searches are bound to the caller's stream
 // (same stream -> same context -> stream order protects the scratch); host-buffer searches take a context from a
@@ -162,6 +146,8 @@ struct aur_index {
   std::mutex mu_write;           // one writer at a time (append / remove)
   int device = 0, dim = 0, dtype = 0;
   int64_t capacity = 0, live = 0;
+  int64_t cap_pad = 0;                // capacity rounded up to a whole tile (TMA boxes never straddle an allocation):
+                                      // the length of every per-row array
   std::atomic<int64_t> rows_pub{0};   // rows visible to searches (published after the data landed)
   size_t elt = 2;
   void* d_rows = nullptr;
@@ -180,7 +166,6 @@ struct aur_index {
   size_t smem_optin = 0;
   int opt_kernel = AUR_KERNEL_AUTO;
   int opt_dbg_flags = 0;
-  int opt_epi_groups = 0;        // 0 = auto
   int opt_tc_tile = 0;           // corpus rows per tile: 0 = auto, 64, 128
   std::atomic<uint32_t> opt_dbg_epoch{0};   // bring-up: start value of the contexts' launch counters (0 = 1)
   std::vector<std::unique_ptr<SearchCtx>> ctxs;
@@ -193,20 +178,15 @@ namespace {
 int build_tmaps(aur_index* ix) {
   ix->tmap_ok = false;
   if (ix->dtype != AUR_BF16 || ix->dim % kTcKBlock != 0 || ix->dim > kTcMaxDim) return AUR_OK;  // SIMT only
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
   // rows past the capacity (a tile's tail, a whole half of the last tile of a pair) arrive as zeros
   for (int w = 0; w < 2; ++w)
     for (int g = 1; g <= 2; ++g) {
       const int tile_n = w ? kTcTileWide : kTcTileN;
-      cuuint64_t gdim[2] = {static_cast<cuuint64_t>(ix->dim), static_cast<cuuint64_t>(ix->capacity)};
-      cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ix->dim) * 2};
-      cuuint32_t box[2] = {static_cast<cuuint32_t>(kTcKBlock), static_cast<cuuint32_t>(tile_n / g)};
-      cuuint32_t estr[2] = {1, 1};
-      CUresult r = enc(&ix->tmap[w][g - 1], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ix->d_rows, gdim, gstride, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-      if (r != CUDA_SUCCESS) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", static_cast<int>(r));
+      const int r = encode_tmap_2d_bf16(&ix->tmap[w][g - 1], ix->d_rows, static_cast<uint64_t>(ix->dim),
+                                        static_cast<uint64_t>(ix->capacity), static_cast<uint64_t>(ix->dim) * 2, kTcKBlock,
+                                        static_cast<uint32_t>(tile_n / g));
+      if (r < 0) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
+      if (r != CUDA_SUCCESS) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", r);
     }
   ix->tmap_ok = true;
   return AUR_OK;
@@ -216,17 +196,16 @@ bool tc_shape_ok(const aur_index* ix, int k, bool filtered) {
   if (!ix->tmap_ok || filtered || k > kMaxK) return false;
   // candidate lists (k + slack per query) and the query block share the SM's shared memory with
   // the TMA ring: large k at large dim leaves no room for a pipeline
-  return tc_pick_stages(1, k + kSlack, ix->dim, ix->smem_optin, kTcTileN, true) >= 2;
+  return tc_pick_stages(k + kSlack, ix->dim, ix->smem_optin, kTcTileN, true) >= 2;
 }
 
-int ctx_init(aur_index* ix, SearchCtx* c) {
+int ctx_init(SearchCtx* c) {
   int lo = 0, hi = 0;
   CU_TRY(cudaDeviceGetStreamPriorityRange(&lo, &hi));   // hi = numerically lowest = highest priority
   CU_TRY(cudaStreamCreateWithPriority(&c->own_stream, cudaStreamNonBlocking, hi));
   CU_TRY(cudaEventCreate(&c->ev_begin)); CU_TRY(cudaEventCreate(&c->ev_k0));
   CU_TRY(cudaEventCreate(&c->ev_k1));    CU_TRY(cudaEventCreate(&c->ev_end));
   CU_TRY(cudaEventCreate(&c->ev_fin));
-  (void)ix;
   return AUR_OK;
 }
 
@@ -241,7 +220,7 @@ int acquire_ctx(aur_index* ix, cudaStream_t s, SearchCtx** out) {
     return AUR_OK;
   }
   std::unique_ptr<SearchCtx> c(new SearchCtx());
-  int rc = ctx_init(ix, c.get());
+  int rc = ctx_init(c.get());
   if (rc != AUR_OK) { c->release(); return rc; }
   c->bound = s;
   *out = c.get();
@@ -253,13 +232,106 @@ void release_ctx(aur_index* ix, SearchCtx* c) {
   if (!c->bound) ix->free_ctxs.push_back(c);
 }
 
+// Pinned caller buffers are mapped into the device's address space (UVA): the re-rank kernel then writes its nq x k
+// results straight into them over PCIe and the two device-to-host copies (a launch + ~8 us of latency each) disappear.
+// Returns whether *d_scores / *d_ids now point at the caller's buffers (else they keep the staging buffers).
+bool direct_outputs(float* scores_out, int64_t* ids_out, float** d_scores, int64_t** d_ids) {
+  cudaPointerAttributes as{}, ai{};
+  if (cudaPointerGetAttributes(&as, scores_out) == cudaSuccess && cudaPointerGetAttributes(&ai, ids_out) == cudaSuccess &&
+      as.type == cudaMemoryTypeHost && ai.type == cudaMemoryTypeHost && as.devicePointer && ai.devicePointer) {
+    *d_scores = static_cast<float*>(as.devicePointer);
+    *d_ids = static_cast<int64_t*>(ai.devicePointer);
+    return true;
+  }
+  cudaGetLastError();
+  return false;
+}
+
+// One call with host buffers: the index's shared lock, its device, an idle pool context locked for the call and given
+// back when the call ends, the context's own stream, and the prefix published when the call began (open()).  A search
+// call stages its queries and outputs with stage() and ends with finish().
+struct HostCall {
+  aur_index* ix;
+  std::shared_lock<std::shared_mutex> rl;
+  SearchCtx* c = nullptr;
+  std::unique_lock<std::mutex> cl;
+  cudaStream_t s = nullptr;
+  int64_t n_rows = 0;
+  float* d_scores = nullptr;   // where the search writes its results: the caller's pinned buffers or the staging buffers
+  int64_t* d_ids = nullptr;
+  bool direct = false;
+
+  explicit HostCall(aur_index* index) : ix(index), rl(index->rw) {}
+  HostCall(const HostCall&) = delete;
+  HostCall& operator=(const HostCall&) = delete;
+  ~HostCall() {
+    if (!c) return;
+    cl.unlock();
+    release_ctx(ix, c);
+  }
+  int open() {
+    CU_TRY(cudaSetDevice(ix->device));
+    const int rc = acquire_ctx(ix, nullptr, &c);
+    if (rc != AUR_OK) return rc;
+    cl = std::unique_lock<std::mutex>(c->mu);
+    s = c->own_stream;
+    n_rows = ix->rows_pub.load(std::memory_order_acquire);
+    return AUR_OK;
+  }
+  // Uploads the queries to c->stage_q and picks the outputs (direct_outputs).
+  int stage(const void* queries_host, int32_t nq, int32_t k, float* scores_out, int64_t* ids_out) {
+    const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->elt;
+    const size_t nout = static_cast<size_t>(nq) * k;
+    CU_TRY(c->stage_q.reserve(qbytes));
+    CU_TRY(c->stage_scores.reserve(nout));
+    CU_TRY(c->stage_ids.reserve(nout));
+    CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
+    d_scores = c->stage_scores.p;
+    d_ids = c->stage_ids.p;
+    direct = direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
+    return AUR_OK;
+  }
+  // Ends a search whose enqueue returned rc.  The caller's buffers are written only when every kernel of the search was
+  // enqueued successfully; on any failure the stream drains and they are left untouched.
+  int finish(int rc, int32_t nq, int32_t k, float* scores_out, int64_t* ids_out) {
+    if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
+    if (!direct) {   // into the caller's pageable buffers
+      const size_t nout = static_cast<size_t>(nq) * k;
+      CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
+      CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
+    }
+    CU_TRY(cudaStreamSynchronize(s));
+    return AUR_OK;
+  }
+};
+
+// Calls f(i, row) for every ids[i] (i < n) that names a row of the prefix [0, n_rows); unknown and newer ids drop out.
+template <typename F>
+void resolve_ids(aur_index* ix, const int64_t* ids, int64_t n, int64_t n_rows, F&& f) {
+  std::lock_guard<std::mutex> lk(ix->mu);
+  for (int64_t i = 0; i < n; ++i) {
+    auto it = ix->id2row.find(ids[i]);
+    if (it != ix->id2row.end() && it->second < n_rows) f(i, static_cast<int32_t>(it->second));
+  }
+}
+
 // Corpus rows per tile when the index leaves it to the launch.  A 128-row tile (wgmma m64n128) fetches each operand for
-// twice the work of a 64-row one, but its layout leaves fewer, larger ring stages: it runs with one epilogue group and
-// at least kTcWideMinStages stages, so at dim 1024, at large k and for most tenant-scoped batches the 64-row kernel
-// stays.  The bring-up score dump (dbg) keeps the 64-row tile it documents.
-int tc_auto_tile(int epi_groups, int ksel, int dim, size_t smem_optin, bool mask, bool dbg) {
-  if (dbg || epi_groups != 1) return kTcTileN;
-  return tc_pick_stages(1, ksel, dim, smem_optin, kTcTileWide, mask) >= kTcWideMinStages ? kTcTileWide : kTcTileN;
+// twice the work of a 64-row one, but its layout leaves fewer, larger ring stages: it runs with at least
+// kTcWideMinStages stages, so at dim 1024, at large k and for most tenant-scoped batches the 64-row kernel stays.  The
+// bring-up score dump (dbg) keeps the 64-row tile it documents.
+int tc_auto_tile(int ksel, int dim, size_t smem_optin, bool mask, bool dbg) {
+  if (dbg) return kTcTileN;
+  return tc_pick_stages(ksel, dim, smem_optin, kTcTileWide, mask) >= kTcWideMinStages ? kTcTileWide : kTcTileN;
+}
+
+// Query super-blocks of a two-CTA launch (CTA pairs of 128 queries each that walk the same tiles side by side, sharing
+// them through L2): at most `want`, fewer while the threshold exchange would need more than ceil(ksel / tile sets) = 4
+// rows vouched for per CTA.
+int tc2_super_blocks(const aur_index* ix, int ksel, int want) {
+  const int pairs = ix->sm_count / 2;
+  int n_super = want;
+  while (n_super > 1 && (ksel + pairs / n_super - 1) / (pairs / n_super) > 4) --n_super;
+  return n_super;
 }
 
 // Runs one block of queries (<= 128 single CTAs, <= 512 pairs) through the tensor-core kernel over the first n_rows rows.  Leaves candidate keys
@@ -270,30 +342,23 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   int n_qblocks = (nqb > kTcQRows) ? 2 : 1;
   if (cta_group == 2 && nqb <= kTcQRows) cta_group = 1;   // a pair works on 128 query rows: a short tail runs as single CTAs
   const int pairs = ix->sm_count / 2;
-  int n_super = 1;   // query super-blocks of 128 (CTA pairs that walk the same tiles side by side, sharing them through L2)
+  int n_super = 1;
   if (cta_group == 2) {
-    n_super = (nqb + 2 * kTcQRows - 1) / (2 * kTcQRows);
-    // the threshold exchange needs ceil(ksel / tile sets) <= 4 rows vouched for per CTA
-    while (n_super > 1 && (ksel + pairs / n_super - 1) / (pairs / n_super) > 4) --n_super;
+    n_super = tc2_super_blocks(ix, ksel, (nqb + 2 * kTcQRows - 1) / (2 * kTcQRows));
     if (nqb > n_super * 2 * kTcQRows) return fail(AUR_ERR_INVALID, "internal: query block larger than the launch geometry");
     n_qblocks = 2 * n_super;
   }
   int grid = (cta_group == 2) ? (pairs / n_super) * n_super * 2 : (ix->sm_count & ~1);
-  const int n_tsets = (cta_group == 2) ? pairs / n_super : grid / n_qblocks;
-  // epilogue groups: 1 by default; 2 (alternating tiles) stays selectable for experiments
-  int epi_groups = ix->opt_epi_groups;
-  if (epi_groups == 0) epi_groups = 1;   // one group leaves the most shared memory to the TMA ring
+  const int n_lists = (cta_group == 2) ? pairs / n_super : grid / n_qblocks;   // tile sets = candidate lists per query
   const bool mask = row_mask != nullptr;
   int tile_n = ix->opt_tc_tile;
-  if (tile_n == 0) tile_n = tc_auto_tile(epi_groups, ksel, ix->dim, ix->smem_optin, mask, dbg != nullptr);
-  if (tile_n == kTcTileWide && epi_groups != 1) return fail(AUR_ERR_UNSUPPORTED, "128-row tiles need epi_groups 1");
-  const int stages = tc_pick_stages(epi_groups, ksel, ix->dim, ix->smem_optin, tile_n, mask);
+  if (tile_n == 0) tile_n = tc_auto_tile(ksel, ix->dim, ix->smem_optin, mask, dbg != nullptr);
+  const int stages = tc_pick_stages(ksel, ix->dim, ix->smem_optin, tile_n, mask);
   if (stages < 2) return fail(AUR_ERR_UNSUPPORTED, "k too large for the tensor-core path's shared memory");
-  const size_t smem = tc_smem_bytes(epi_groups, stages, ksel, ix->dim, tile_n, mask);
-  const int n_lists = n_tsets * epi_groups;   // candidate lists per query
+  const size_t smem = tc_smem_bytes(stages, ksel, ix->dim, tile_n, mask);
   const size_t ncand = static_cast<size_t>(n_qblocks) * kTcQRows * n_lists * ksel;
   CU_TRY(c->cand_a.reserve(ncand));
-  const size_t npub = static_cast<size_t>(n_qblocks) * kTcQRows * (((n_tsets + 1) & ~1) + 1);
+  const size_t npub = static_cast<size_t>(n_qblocks) * kTcQRows * (((n_lists + 1) & ~1) + 1);
   if (npub > c->pub.n) {
     CU_TRY(c->pub.reserve(npub));
     CU_TRY(cudaMemsetAsync(c->pub.p, 0, npub * 8, s));  // epoch 0 is never used by a launch
@@ -326,7 +391,7 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   p.num_stages = stages;
   p.dbg_flags = ix->opt_dbg_flags;
   p.n_tiles = static_cast<int>((n_rows + tile_n - 1) / tile_n);
-  CU_TRY(tc_launch(cta_group, epi_groups, tile_n, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
+  CU_TRY(tc_launch(cta_group, tile_n, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
   c->last_tile_n = tile_n;
   *n_lists_out = n_lists;
   return AUR_OK;
@@ -347,13 +412,65 @@ struct Scope {
   const uint32_t* match_mask = nullptr;  // device [n_rows]: rows with bit 0 set stay visible (a device-evaluated filter)
 };
 
-// Enqueues one search over the published prefix `n_rows` on stream s using context c.
+// Stats of one search call (aur_get_stats), kept on the context that runs it.  The call opens them with stats_begin
+// (counters reset, ev_begin) and closes them with stats_end (ev_fin, ev_end; the context becomes the one aur_get_stats
+// reads).  In between the search sets last_kernel, counts every launch in last_launches and brackets the main kernels
+// of its first block of queries with ev_k0 / ev_k1.
+int stats_begin(SearchCtx* c, cudaStream_t s, int nq, int64_t n_rows) {
+  c->last_launches = 0;
+  c->last_tile_n = 0;
+  c->last_nq = nq;
+  c->snapshot_rows = n_rows;
+  CU_TRY(cudaEventRecord(c->ev_begin, s));
+  return AUR_OK;
+}
+int stats_end(aur_index* ix, SearchCtx* c, cudaStream_t s) {
+  CU_TRY(cudaEventRecord(c->ev_fin, s));
+  CU_TRY(cudaEventRecord(c->ev_end, s));
+  c->have_timing = true;
+  std::lock_guard<std::mutex> lk(ix->mu);
+  ix->last_ctx = c;
+  return AUR_OK;
+}
+
+// The tail of one block of queries q0 .. q0 + nqb: its candidate lists [nqb, n_lists, ksel] in c->cand_a are folded
+// until one sort of <= 4096 keys finishes them, then re-ranked exactly into the block's rows of the outputs.  compact:
+// the tensor-core kernel already compacted its survivors per query (counted in c->cand_count), nothing to fold.
+int candidate_tail(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* qb, int q0, int nqb, int k, int n_lists, bool compact,
+                   float* scores, int64_t* ids, double* scores64, const FinalizeArgs::ExchangeOut* ex) {
+  const int ksel = k + kSlack;
+  uint64_t* cur = c->cand_a.p;
+  bool in_a = true;
+  while (!compact && static_cast<int64_t>(n_lists) * ksel > 4096) {
+    const int group = 4096 / ksel;
+    const int n_groups = (n_lists + group - 1) / group;
+    DevBuf<uint64_t>& dst = in_a ? c->cand_b : c->cand_a;
+    // rows of cand are indexed by the query position inside the block (TC pads to 128/256)
+    CU_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
+    CU_TRY(launch_reduce_lists(cur, nqb, n_lists, ksel, group, ix->d_ids, dst.p, s));
+    c->last_launches += 1;
+    cur = dst.p; n_lists = n_groups; in_a = !in_a;
+  }
+  FinalizeArgs fa{};
+  fa.cand = cur; fa.n_lists = n_lists; fa.ksel = ksel;
+  fa.counts = compact ? c->cand_count.p : nullptr;
+  fa.epoch_bump = compact ? c->d_epoch.p : nullptr;
+  fa.cand_read = c->cand_read.p + q0;
+  fa.q = qb; fa.rows = ix->d_rows; fa.dtype = ix->dtype; fa.dim = ix->dim; fa.nq = nqb; fa.k = k;
+  fa.ids = ix->d_ids;
+  fa.out_scores = scores ? scores + static_cast<size_t>(q0) * k : nullptr;
+  fa.out_ids = ids ? ids + static_cast<size_t>(q0) * k : nullptr;
+  fa.out_scores64 = scores64 ? scores64 + static_cast<size_t>(q0) * k : nullptr;
+  if (ex) { fa.ex = *ex; fa.ex.q0 = q0; }
+  CU_TRY(launch_finalize(fa, s));
+  c->last_launches += 1;
+  return AUR_OK;
+}
+
+// Enqueues one search over the published prefix `n_rows` on stream s using context c, inside the call's stats.
 int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k, const Scope& sc, int64_t n_rows,
                    float* scores, int64_t* ids, double* scores64, cudaStream_t s,
-                   const FinalizeArgs::ExchangeOut* ex = nullptr, bool begun = false) {
-  if (nq <= 0 || k <= 0) return fail(AUR_ERR_INVALID, "nq and k must be positive");
-  if (k > kMaxK) return fail(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
-  if (nq > 65535) return fail(AUR_ERR_UNSUPPORTED, "nq > 65535: split the batch");
+                   const FinalizeArgs::ExchangeOut* ex = nullptr) {
   const bool subset = sc.n_allow >= 0;
   const bool scoped_tc = sc.n_scopes > 0 && !subset && sc.uniform == nullptr;        // per-query scopes through bit masks
   const bool filtered = sc.q_user != nullptr && sc.uniform == nullptr && !subset && !scoped_tc;   // else: generic kernel only
@@ -364,12 +481,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
     return fail(AUR_ERR_UNSUPPORTED, "tensor-core path needs bf16, dim %% 64 == 0, dim <= %d, no per-query tenant filter, and k small "
                 "enough for its shared-memory lists at this dim", kTcMaxDim);
   c->last_kernel = kernel;
-  if (!begun) c->last_launches = 0;
-  c->last_nq = nq;
-  c->last_tile_n = 0;
   CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
-  c->snapshot_rows = n_rows;
-  if (!begun) CU_TRY(cudaEventRecord(c->ev_begin, s));
   bool k_timed = false;
   const float* inv = nullptr;   // masked inverse norms (nullptr = the shard's own)
   if (subset && n_rows > 0) {
@@ -398,17 +510,11 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
   // side on the same corpus tiles (fewer when k + slack is too large for the threshold exchange of that geometry)
   int qstep = 1024;
   if (kernel == AUR_KERNEL_TC1) qstep = 2 * kTcQRows;
-  else if (kernel == AUR_KERNEL_TC2) {
-    const int pairs = ix->sm_count / 2;
-    int n_super = 4;
-    while (n_super > 1 && (ksel + pairs / n_super - 1) / (pairs / n_super) > 4) --n_super;
-    qstep = n_super * 2 * kTcQRows;
-  }
+  else if (kernel == AUR_KERNEL_TC2) qstep = tc2_super_blocks(ix, ksel, 4) * 2 * kTcQRows;
   for (int q0 = 0; q0 < nq; q0 += qstep) {
     const int nqb = (nq - q0 < qstep) ? nq - q0 : qstep;
     const uint8_t* qb = static_cast<const uint8_t*>(q_dev) + static_cast<size_t>(q0) * ix->dim * ix->elt;
     int n_lists = 0;
-    uint64_t* cur = nullptr;
     if (kernel == AUR_KERNEL_SIMT) {
       if (n_rows == 0) {
         n_lists = 1;
@@ -432,7 +538,6 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
         }
         if (!k_timed) { CU_TRY(cudaEventRecord(c->ev_k1, s)); k_timed = true; }
       }
-      cur = c->cand_a.p;
     } else {
       if (!k_timed) CU_TRY(cudaEventRecord(c->ev_k0, s));
       const bool use_mask = scoped_tc && n_rows > 0;
@@ -441,44 +546,11 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
       if (rc != AUR_OK) return rc;
       if (!k_timed) { CU_TRY(cudaEventRecord(c->ev_k1, s)); k_timed = true; }
       c->last_launches += 1;
-      cur = c->cand_a.p;
     }
-    // dense candidate lists (SIMT path): fold until one sort of <= 4096 keys finishes the
-    // job.  The tensor-core kernel already compacted its survivors per query.
-    const bool compact = kernel != AUR_KERNEL_SIMT;
-    bool in_a = true;
-    while (!compact && static_cast<int64_t>(n_lists) * ksel > 4096) {
-      const int group = 4096 / ksel;
-      const int n_groups = (n_lists + group - 1) / group;
-      DevBuf<uint64_t>& dst = in_a ? c->cand_b : c->cand_a;
-      // rows of cand are indexed by the query position inside the block (TC pads to 128/256)
-      CU_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
-      CU_TRY(launch_reduce_lists(cur, nqb, n_lists, ksel, group, ix->d_ids, dst.p, s));
-      c->last_launches += 1;
-      cur = dst.p; n_lists = n_groups; in_a = !in_a;
-    }
-    FinalizeArgs fa{};
-    fa.cand = cur; fa.n_lists = n_lists; fa.ksel = ksel;
-    fa.counts = compact ? c->cand_count.p : nullptr;
-    fa.epoch_bump = compact ? c->d_epoch.p : nullptr;
-    fa.cand_read = c->cand_read.p + q0;
-    fa.q = qb; fa.rows = ix->d_rows; fa.dtype = ix->dtype; fa.dim = ix->dim; fa.nq = nqb; fa.k = k;
-    fa.ids = ix->d_ids;
-    fa.out_scores = scores ? scores + static_cast<size_t>(q0) * k : nullptr;
-    fa.out_ids = ids ? ids + static_cast<size_t>(q0) * k : nullptr;
-    fa.out_scores64 = scores64 ? scores64 + static_cast<size_t>(q0) * k : nullptr;
-    if (ex) { fa.ex = *ex; fa.ex.q0 = q0; }
-    CU_TRY(launch_finalize(fa, s));
-    c->last_launches += 1;
+    const int rc = candidate_tail(ix, c, s, qb, q0, nqb, k, n_lists, kernel != AUR_KERNEL_SIMT, scores, ids, scores64, ex);
+    if (rc != AUR_OK) return rc;
   }
   if (!k_timed) { CU_TRY(cudaEventRecord(c->ev_k0, s)); CU_TRY(cudaEventRecord(c->ev_k1, s)); }
-  CU_TRY(cudaEventRecord(c->ev_fin, s));
-  CU_TRY(cudaEventRecord(c->ev_end, s));
-  c->have_timing = true;
-  {
-    std::lock_guard<std::mutex> lk(ix->mu);
-    ix->last_ctx = c;
-  }
   return AUR_OK;
 }
 
@@ -529,21 +601,11 @@ int check_search_args(aur_index* ix, const void* q, int32_t nq, int32_t k, const
   return AUR_OK;
 }
 
-// Pinned caller buffers are mapped into the device's address space (UVA): the re-rank kernel then writes its nq x k
-// results straight into them over PCIe and the two device-to-host copies (a launch + ~8 us of latency each) disappear.
-// Returns whether *d_scores / *d_ids now point at the caller's buffers (else they keep the staging buffers).
-bool direct_outputs(float* scores_out, int64_t* ids_out, float** d_scores, int64_t** d_ids) {
-  static const bool no_direct = getenv("AUR_NO_DIRECT_OUT") != nullptr;     // A/B switch
-  if (no_direct) return false;
-  cudaPointerAttributes as{}, ai{};
-  if (cudaPointerGetAttributes(&as, scores_out) == cudaSuccess && cudaPointerGetAttributes(&ai, ids_out) == cudaSuccess &&
-      as.type == cudaMemoryTypeHost && ai.type == cudaMemoryTypeHost && as.devicePointer && ai.devicePointer) {
-    *d_scores = static_cast<float*>(as.devicePointer);
-    *d_ids = static_cast<int64_t*>(ai.devicePointer);
-    return true;
-  }
-  cudaGetLastError();
-  return false;
+// Limits of one search batch: top-k lists of at most kMaxK, and no more queries than the kernels' grids index.
+int check_batch(int32_t nq, int32_t k) {
+  if (k > kMaxK) return fail(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
+  if (nq > 65535) return fail(AUR_ERR_UNSUPPORTED, "nq > 65535: split the batch");
+  return AUR_OK;
 }
 
 // Host-buffer search: H2D of the queries, kernels, D2H of the results on a pool context's own stream.
@@ -551,34 +613,22 @@ int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, 
                 const int64_t* allow_ids, int64_t n_allow, float* scores_out, int64_t* ids_out, int64_t* snapshot_out) {
   int rc = check_search_args(ix, queries_host, nq, k, scores_out, ids_out);
   if (rc != AUR_OK) return rc;
-  std::shared_lock<std::shared_mutex> rl(ix->rw);
-  CU_TRY(cudaSetDevice(ix->device));
-  SearchCtx* c = nullptr;
-  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
-  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
-  std::lock_guard<std::mutex> cl(c->mu);
-  cudaStream_t s = c->own_stream;
-  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
-  const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->elt;
-  const size_t nout = static_cast<size_t>(nq) * k;
-  CU_TRY(c->stage_q.reserve(qbytes));
-  CU_TRY(c->stage_scores.reserve(nout));
-  CU_TRY(c->stage_ids.reserve(nout));
-  CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
+  const bool subset = allow_ids || n_allow > 0;
+  if (subset && (n_allow < 0 || (n_allow > 0 && !allow_ids))) return fail(AUR_ERR_INVALID, "allow_ids / n_allow");
+  if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
+  HostCall call(ix);
+  if ((rc = call.open()) != AUR_OK) return rc;
+  SearchCtx* c = call.c;
+  cudaStream_t s = call.s;
+  const int64_t n_rows = call.n_rows;
+  if ((rc = call.stage(queries_host, nq, k, scores_out, ids_out)) != AUR_OK) return rc;
   Scope sc;
   int32_t scope[2] = {0, -1};
   std::vector<int32_t> rows_host;
-  if (allow_ids || n_allow > 0) {
+  if (subset) {
     // resolved metadata pre-filter: ids -> rows of the published prefix (unknown / newer ids drop out)
-    if (n_allow < 0 || (n_allow > 0 && !allow_ids)) return fail(AUR_ERR_INVALID, "allow_ids / n_allow");
     rows_host.reserve(static_cast<size_t>(n_allow));
-    {
-      std::lock_guard<std::mutex> lk(ix->mu);
-      for (int64_t i = 0; i < n_allow; ++i) {
-        auto it = ix->id2row.find(allow_ids[i]);
-        if (it != ix->id2row.end() && it->second < n_rows) rows_host.push_back(static_cast<int32_t>(it->second));
-      }
-    }
+    resolve_ids(ix, allow_ids, n_allow, n_rows, [&](int64_t, int32_t row) { rows_host.push_back(row); });
     CU_TRY(c->allow_rows.reserve(rows_host.size() + 1));
     if (!rows_host.empty())
       CU_TRY(cudaMemcpyAsync(c->allow_rows.p, rows_host.data(), rows_host.size() * 4, cudaMemcpyHostToDevice, s));
@@ -623,17 +673,10 @@ int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, 
       }
     }
   }
-  float* d_scores = c->stage_scores.p;
-  int64_t* d_ids = c->stage_ids.p;
-  const bool direct = direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
-  rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, d_scores, d_ids, nullptr, s);
-  if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
-  if (!direct) {
-    // into the caller's pageable buffers; nothing is written unless every kernel above was enqueued successfully
-    CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
-  }
-  CU_TRY(cudaStreamSynchronize(s));
+  rc = stats_begin(c, s, nq, n_rows);
+  if (rc == AUR_OK) rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, call.d_scores, call.d_ids, nullptr, s);
+  if (rc == AUR_OK) rc = stats_end(ix, c, s);
+  if ((rc = call.finish(rc, nq, k, scores_out, ids_out)) != AUR_OK) return rc;
   if (snapshot_out) *snapshot_out = n_rows;
   return AUR_OK;
 }
@@ -648,35 +691,34 @@ constexpr int64_t kListScoreSlots = 16384;   // 128 MB of scores
 int check_list_args(aur_index* ix, const void* q, int32_t nq, int32_t k, const void* s_out, const void* i_out) {
   int rc = check_search_args(ix, q, nq, k, s_out, i_out);
   if (rc != AUR_OK) return rc;
-  if (k > kMaxK) return fail(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
-  if (nq > 65535) return fail(AUR_ERR_UNSUPPORTED, "nq > 65535: split the batch");
+  if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
   if (ix->dtype != AUR_BF16) return fail(AUR_ERR_UNSUPPORTED, "list search needs a bf16 index");
   return AUR_OK;
 }
 
-// The device side of a list search once every list's rows are known: work items built on the host from the lists'
-// lengths alone, launched in batches, folded and re-ranked exactly, results copied to the caller's buffers.  List l is
-// rows list_rows[lrow0[l] .. lrow0[l] + llen[l]), ascending and without repeats; list_rows = nullptr means the rows sit
-// at the front of `stage` (which is uploaded in one copy and extended here with the work items).  `begun`: the caller
-// already recorded ev_begin (its own kernels ran first on this stream).
-int run_list_search(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k,
-                    const int32_t* q_list, int32_t n_lists, const std::vector<int64_t>& lrow0, const std::vector<int64_t>& llen,
-                    std::vector<int32_t>& stage, const int32_t* list_rows, int64_t n_rows, bool begun, float* scores_out,
-                    int64_t* ids_out) {
-  const int ksel = k + kSlack;
-  struct Launch { size_t items; int n_items, max_nq; };
+// The host side of a list search, built from the lists' lengths alone: blocks of queries, each with its work items cut
+// into launches, and the int32 staging the device side uploads in one copy.
+struct ListPlan {
+  struct Launch { size_t items; int n_items, max_nq; };   // items: offset of the launch's first item in `stage`
   struct Block { int q0, nqb, n_segs; std::vector<Launch> launches; };
   std::vector<Block> blocks;
-  constexpr int kItemWords = sizeof(ListItem) / 4;
+  std::vector<int32_t> stage;   // [the lists' rows, when the host resolved them][per block: its queries' positions, its items]
   size_t max_slots = 0, max_cand = 0;
+};
+
+// List l is rows lrow0[l] .. lrow0[l] + llen[l] of the lists' rows, ascending and without repeats.
+int plan_list_search(int32_t nq, int32_t k, const int32_t* q_list, const std::vector<int64_t>& lrow0,
+                     const std::vector<int64_t>& llen, ListPlan* pl) {
+  const int ksel = k + kSlack;
+  constexpr int kItemWords = sizeof(ListItem) / 4;
   std::vector<ListItem> items;
   for (int q0 = 0; q0 < nq; q0 += kListQBlock) {
-    Block b{q0, std::min(kListQBlock, nq - q0), 1, {}};
+    ListPlan::Block b{q0, std::min(kListQBlock, nq - q0), 1, {}};
     std::vector<int32_t> order(static_cast<size_t>(b.nqb));
     for (int i = 0; i < b.nqb; ++i) order[static_cast<size_t>(i)] = i;
     std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) { return q_list[q0 + x] < q_list[q0 + y]; });
-    const size_t qidx0 = stage.size();
-    stage.insert(stage.end(), order.begin(), order.end());
+    const size_t qidx0 = pl->stage.size();
+    pl->stage.insert(pl->stage.end(), order.begin(), order.end());
     items.clear();
     for (int i = 0; i < b.nqb;) {
       const int32_t l = q_list[q0 + order[static_cast<size_t>(i)]];
@@ -702,163 +744,63 @@ int run_list_search(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* que
     int64_t slots = 0;
     for (size_t i = 0; i < items.size(); ++i) {
       if (b.launches.empty() || slots + items[i].nq > kListScoreSlots) {
-        b.launches.push_back(Launch{stage.size() + i * kItemWords, 0, 0});
+        b.launches.push_back(ListPlan::Launch{pl->stage.size() + i * kItemWords, 0, 0});
         slots = 0;
       }
-      Launch& ln = b.launches.back();
+      ListPlan::Launch& ln = b.launches.back();
       items[i].out = static_cast<int32_t>(slots);
       slots += items[i].nq;
       ++ln.n_items;
       ln.max_nq = std::max(ln.max_nq, items[i].nq);
-      max_slots = std::max(max_slots, static_cast<size_t>(slots));
+      pl->max_slots = std::max(pl->max_slots, static_cast<size_t>(slots));
     }
     const int32_t* w = reinterpret_cast<const int32_t*>(items.data());
-    stage.insert(stage.end(), w, w + items.size() * kItemWords);
-    max_cand = std::max(max_cand, static_cast<size_t>(b.nqb) * b.n_segs * ksel);
-    blocks.push_back(std::move(b));
+    pl->stage.insert(pl->stage.end(), w, w + items.size() * kItemWords);
+    pl->max_cand = std::max(pl->max_cand, static_cast<size_t>(b.nqb) * b.n_segs * ksel);
+    pl->blocks.push_back(std::move(b));
   }
-  if (stage.size() > static_cast<size_t>(INT32_MAX))
+  if (pl->stage.size() > static_cast<size_t>(INT32_MAX))
     return fail(AUR_ERR_UNSUPPORTED, "the lists of this batch are too long for one call: split the batch");
-
-  const size_t qbytes = static_cast<size_t>(nq) * ix->dim * 2;
-  const size_t nout = static_cast<size_t>(nq) * k;
-  CU_TRY(c->stage_q.reserve(qbytes));
-  CU_TRY(c->stage_scores.reserve(nout));
-  CU_TRY(c->stage_ids.reserve(nout));
-  CU_TRY(c->list_stage.reserve(stage.size()));
-  CU_TRY(c->list_scores.reserve(std::max<size_t>(max_slots, 1) * kSimtSeg));
-  CU_TRY(c->cand_a.reserve(max_cand));
-  CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
-  float* d_scores = c->stage_scores.p;
-  int64_t* d_ids = c->stage_ids.p;
-  const bool direct = direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
-
-  auto enqueue = [&]() -> int {
-    c->last_kernel = AUR_KERNEL_LIST;
-    if (!begun) c->last_launches = 0;
-    c->last_tile_n = 0;
-    c->last_nq = nq;
-    c->snapshot_rows = n_rows;
-    if (!begun) CU_TRY(cudaEventRecord(c->ev_begin, s));
-    CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
-    CU_TRY(cudaMemcpyAsync(c->list_stage.p, stage.data(), stage.size() * 4, cudaMemcpyHostToDevice, s));
-    for (size_t bi = 0; bi < blocks.size(); ++bi) {
-      const Block& b = blocks[bi];
-      const uint8_t* qb = c->stage_q.p + static_cast<size_t>(b.q0) * ix->dim * 2;
-      int n_lists_c = b.n_segs;
-      CU_TRY(cudaMemsetAsync(c->cand_a.p, 0, static_cast<size_t>(b.nqb) * n_lists_c * ksel * 8, s));   // 0 = empty slot
-      if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k0, s));
-      for (const Launch& ln : b.launches) {
-        ListParams p{};
-        p.q = reinterpret_cast<const __nv_bfloat16*>(qb);
-        p.rows = static_cast<const __nv_bfloat16*>(ix->d_rows);
-        p.inv_norm = ix->d_inv_norm;
-        p.ids = ix->d_ids;
-        p.items = reinterpret_cast<const ListItem*>(c->list_stage.p + ln.items);
-        p.n_items = ln.n_items;
-        p.list_rows = list_rows ? list_rows : c->list_stage.p;
-        p.qidx = c->list_stage.p;
-        p.scores = c->list_scores.p;
-        p.cand = c->cand_a.p;
-        p.dim = ix->dim; p.ksel = ksel; p.n_lists = n_lists_c;
-        CU_TRY(launch_list_search(p, ln.max_nq, s));
-        c->last_launches += 2;
-      }
-      if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k1, s));
-      // fold to <= 4096 keys per query, then the exact re-rank (the generic path's tail)
-      uint64_t* cur = c->cand_a.p;
-      bool in_a = true;
-      while (static_cast<int64_t>(n_lists_c) * ksel > 4096) {
-        const int group = 4096 / ksel;
-        const int n_groups = (n_lists_c + group - 1) / group;
-        DevBuf<uint64_t>& dst = in_a ? c->cand_b : c->cand_a;
-        CU_TRY(dst.reserve(static_cast<size_t>(b.nqb) * n_groups * ksel));
-        CU_TRY(launch_reduce_lists(cur, b.nqb, n_lists_c, ksel, group, ix->d_ids, dst.p, s));
-        c->last_launches += 1;
-        cur = dst.p; n_lists_c = n_groups; in_a = !in_a;
-      }
-      FinalizeArgs fa{};
-      fa.cand = cur; fa.n_lists = n_lists_c; fa.ksel = ksel;
-      fa.cand_read = c->cand_read.p + b.q0;
-      fa.q = qb; fa.rows = ix->d_rows; fa.dtype = ix->dtype; fa.dim = ix->dim; fa.nq = b.nqb; fa.k = k;
-      fa.ids = ix->d_ids;
-      fa.out_scores = d_scores + static_cast<size_t>(b.q0) * k;
-      fa.out_ids = d_ids + static_cast<size_t>(b.q0) * k;
-      CU_TRY(launch_finalize(fa, s));
-      c->last_launches += 1;
-    }
-    CU_TRY(cudaEventRecord(c->ev_fin, s));
-    CU_TRY(cudaEventRecord(c->ev_end, s));
-    c->have_timing = true;
-    {
-      std::lock_guard<std::mutex> lk(ix->mu);
-      ix->last_ctx = c;
-    }
-    return AUR_OK;
-  };
-  int rc = enqueue();
-  if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
-  if (!direct) {
-    CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
-    CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
-  }
-  CU_TRY(cudaStreamSynchronize(s));
   return AUR_OK;
 }
 
-int search_lists_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int64_t* list_ids,
-                      const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list, float* scores_out,
-                      int64_t* ids_out, int64_t* snapshot_out) {
-  int rc = check_list_args(ix, queries_host, nq, k, scores_out, ids_out);
-  if (rc != AUR_OK) return rc;
-  if (!list_offsets || !q_list || n_lists < 1) return fail(AUR_ERR_INVALID, "list_offsets, q_list and n_lists >= 1 are required");
-  if (list_offsets[0] != 0) return fail(AUR_ERR_INVALID, "list_offsets[0] must be 0");
-  for (int32_t l = 0; l < n_lists; ++l)
-    if (list_offsets[l + 1] < list_offsets[l]) return fail(AUR_ERR_INVALID, "list_offsets decrease at list %d", l);
-  if (list_offsets[n_lists] > 0 && !list_ids) return fail(AUR_ERR_INVALID, "list_ids is required");
-  for (int32_t q = 0; q < nq; ++q)
-    if (q_list[q] < 0 || q_list[q] >= n_lists) return fail(AUR_ERR_INVALID, "q_list[%d] = %d is not a list", q, q_list[q]);
-
-  std::shared_lock<std::shared_mutex> rl(ix->rw);
-  CU_TRY(cudaSetDevice(ix->device));
-  SearchCtx* c = nullptr;
-  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
-  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
-  std::lock_guard<std::mutex> cl(c->mu);
-  cudaStream_t s = c->own_stream;
-  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
-
-  // ids -> rows of the published prefix (unknown / newer ids drop out), for the lists some query names
-  std::vector<std::vector<int32_t>> res(static_cast<size_t>(n_lists));
-  std::vector<char> named(static_cast<size_t>(n_lists), 0);
-  for (int32_t q = 0; q < nq; ++q) named[static_cast<size_t>(q_list[q])] = 1;
-  {
-    std::lock_guard<std::mutex> lk(ix->mu);
-    for (int32_t l = 0; l < n_lists; ++l) {
-      if (!named[static_cast<size_t>(l)]) continue;
-      std::vector<int32_t>& r = res[static_cast<size_t>(l)];
-      for (int64_t i = list_offsets[l]; i < list_offsets[l + 1]; ++i) {
-        auto it = ix->id2row.find(list_ids[i]);
-        if (it != ix->id2row.end() && it->second < n_rows) r.push_back(static_cast<int32_t>(it->second));
-      }
+// The device side of a planned list search over the queries in c->stage_q: the plan is uploaded, every block's work
+// items launched, and its candidates folded and re-ranked exactly into d_scores / d_ids.  list_rows: the lists' rows on
+// the device (nullptr: at the front of the plan's staging).
+int run_list_search(aur_index* ix, SearchCtx* c, cudaStream_t s, const ListPlan& pl, int32_t nq, int32_t k,
+                    const int32_t* list_rows, float* d_scores, int64_t* d_ids) {
+  const int ksel = k + kSlack;
+  CU_TRY(c->list_stage.reserve(pl.stage.size()));
+  CU_TRY(c->list_scores.reserve(std::max<size_t>(pl.max_slots, 1) * kSimtSeg));
+  CU_TRY(c->cand_a.reserve(pl.max_cand));
+  CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
+  c->last_kernel = AUR_KERNEL_LIST;
+  CU_TRY(cudaMemcpyAsync(c->list_stage.p, pl.stage.data(), pl.stage.size() * 4, cudaMemcpyHostToDevice, s));
+  for (size_t bi = 0; bi < pl.blocks.size(); ++bi) {
+    const ListPlan::Block& b = pl.blocks[bi];
+    const uint8_t* qb = c->stage_q.p + static_cast<size_t>(b.q0) * ix->dim * 2;
+    CU_TRY(cudaMemsetAsync(c->cand_a.p, 0, static_cast<size_t>(b.nqb) * b.n_segs * ksel * 8, s));   // 0 = empty slot
+    if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k0, s));
+    for (const ListPlan::Launch& ln : b.launches) {
+      ListParams p{};
+      p.q = reinterpret_cast<const __nv_bfloat16*>(qb);
+      p.rows = static_cast<const __nv_bfloat16*>(ix->d_rows);
+      p.inv_norm = ix->d_inv_norm;
+      p.ids = ix->d_ids;
+      p.items = reinterpret_cast<const ListItem*>(c->list_stage.p + ln.items);
+      p.n_items = ln.n_items;
+      p.list_rows = list_rows ? list_rows : c->list_stage.p;
+      p.qidx = c->list_stage.p;
+      p.scores = c->list_scores.p;
+      p.cand = c->cand_a.p;
+      p.dim = ix->dim; p.ksel = ksel; p.n_lists = b.n_segs;
+      CU_TRY(launch_list_search(p, ln.max_nq, s));
+      c->last_launches += 2;
     }
+    if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k1, s));
+    const int rc = candidate_tail(ix, c, s, qb, b.q0, b.nqb, k, b.n_segs, false, d_scores, d_ids, nullptr, nullptr);
+    if (rc != AUR_OK) return rc;
   }
-  // staging (int32): [every named list's rows, sorted, once each][per block: its queries' positions, its items]
-  std::vector<int32_t> stage;
-  std::vector<int64_t> lrow0(static_cast<size_t>(n_lists), 0), llen(static_cast<size_t>(n_lists), 0);
-  for (int32_t l = 0; l < n_lists; ++l) {
-    std::vector<int32_t>& r = res[static_cast<size_t>(l)];
-    std::sort(r.begin(), r.end());
-    r.erase(std::unique(r.begin(), r.end()), r.end());
-    lrow0[static_cast<size_t>(l)] = static_cast<int64_t>(stage.size());
-    llen[static_cast<size_t>(l)] = static_cast<int64_t>(r.size());
-    stage.insert(stage.end(), r.begin(), r.end());
-    std::vector<int32_t>().swap(r);
-  }
-  rc = run_list_search(ix, c, s, queries_host, nq, k, q_list, n_lists, lrow0, llen, stage, nullptr, n_rows, false, scores_out,
-                       ids_out);
-  if (rc != AUR_OK) return rc;
-  if (snapshot_out) *snapshot_out = n_rows;
   return AUR_OK;
 }
 
@@ -1007,13 +949,13 @@ int aur_open(const aur_config* cfg, aur_index** out) {
   OPEN_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
   OPEN_TRY(cudaStreamCreateWithPriority(&ix->stream, cudaStreamNonBlocking, prio_hi));
   OPEN_TRY(cudaStreamCreateWithPriority(&ix->ingest_stream, cudaStreamNonBlocking, prio_lo));
-  // round the row store up to a whole tile so TMA boxes never straddle the allocation
-  const int64_t cap_pad = (cfg->capacity + kTcTileN - 1) / kTcTileN * kTcTileN;
-  OPEN_TRY(cudaMalloc(&ix->d_rows, static_cast<size_t>(cap_pad) * ix->dim * ix->elt));
-  OPEN_TRY(cudaMalloc(&ix->d_inv_norm, static_cast<size_t>(cap_pad) * 4));
-  OPEN_TRY(cudaMalloc(&ix->d_ids, static_cast<size_t>(cap_pad) * 8));
-  OPEN_TRY(cudaMalloc(&ix->d_user, static_cast<size_t>(cap_pad) * 4));
-  OPEN_TRY(cudaMalloc(&ix->d_org, static_cast<size_t>(cap_pad) * 4));
+  ix->cap_pad = (cfg->capacity + kTcTileN - 1) / kTcTileN * kTcTileN;
+  const size_t cap_pad = static_cast<size_t>(ix->cap_pad);
+  OPEN_TRY(cudaMalloc(&ix->d_rows, cap_pad * ix->dim * ix->elt));
+  OPEN_TRY(cudaMalloc(&ix->d_inv_norm, cap_pad * 4));
+  OPEN_TRY(cudaMalloc(&ix->d_ids, cap_pad * 8));
+  OPEN_TRY(cudaMalloc(&ix->d_user, cap_pad * 4));
+  OPEN_TRY(cudaMalloc(&ix->d_org, cap_pad * 4));
 #undef OPEN_TRY
   int rc = build_tmaps(ix);
   if (rc != AUR_OK) return bail(rc);
@@ -1199,11 +1141,6 @@ int aur_set_option(aur_index* ix, const char* key, int64_t value) {
     ix->opt_kernel = static_cast<int>(value);
     return AUR_OK;
   }
-  if (strcmp(key, "epi_groups") == 0) {
-    if (value < 0 || value > 2) return fail(AUR_ERR_INVALID, "epi_groups must be 0 (auto), 1 or 2");
-    ix->opt_epi_groups = static_cast<int>(value);
-    return AUR_OK;
-  }
   if (strcmp(key, "tc_tile") == 0) {
     if (value != 0 && value != kTcTileN && value != kTcTileWide) return fail(AUR_ERR_INVALID, "tc_tile must be 0 (auto), 64 or 128");
     ix->opt_tc_tile = static_cast<int>(value);
@@ -1266,16 +1203,19 @@ int aur_search_dev(aur_index* ix, const void* queries_dev, int32_t nq, int32_t k
                    const int32_t* q_org_dev, float* scores_dev, int64_t* ids_dev, double* scores64_dev, void* stream) {
   int rc = check_search_args(ix, queries_dev, nq, k, scores_dev, ids_dev);
   if (rc != AUR_OK) return rc;
+  if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   CU_TRY(cudaSetDevice(ix->device));
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
   SearchCtx* c = nullptr;
   if ((rc = acquire_ctx(ix, s, &c)) != AUR_OK) return rc;
   std::lock_guard<std::mutex> cl(c->mu);
+  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
   Scope sc;
   sc.q_user = q_user_dev; sc.q_org = q_org_dev;
-  return search_enqueue(ix, c, queries_dev, nq, k, sc, ix->rows_pub.load(std::memory_order_acquire), scores_dev, ids_dev,
-                        scores64_dev, s);
+  if ((rc = stats_begin(c, s, nq, n_rows)) != AUR_OK) return rc;
+  if ((rc = search_enqueue(ix, c, queries_dev, nq, k, sc, n_rows, scores_dev, ids_dev, scores64_dev, s)) != AUR_OK) return rc;
+  return stats_end(ix, c, s);
 }
 
 int aur_search(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
@@ -1298,8 +1238,43 @@ int aur_search_subset(aur_index* ix, const void* queries_host, int32_t nq, int32
 int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int64_t* list_ids,
                      const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list, float* scores_out,
                      int64_t* ids_out, int64_t* snapshot_rows_out) {
-  return search_lists_host(ix, queries_host, nq, k, list_ids, list_offsets, n_lists, q_list, scores_out, ids_out,
-                           snapshot_rows_out);
+  int rc = check_list_args(ix, queries_host, nq, k, scores_out, ids_out);
+  if (rc != AUR_OK) return rc;
+  if (!list_offsets || !q_list || n_lists < 1) return fail(AUR_ERR_INVALID, "list_offsets, q_list and n_lists >= 1 are required");
+  if (list_offsets[0] != 0) return fail(AUR_ERR_INVALID, "list_offsets[0] must be 0");
+  for (int32_t l = 0; l < n_lists; ++l)
+    if (list_offsets[l + 1] < list_offsets[l]) return fail(AUR_ERR_INVALID, "list_offsets decrease at list %d", l);
+  if (list_offsets[n_lists] > 0 && !list_ids) return fail(AUR_ERR_INVALID, "list_ids is required");
+  for (int32_t q = 0; q < nq; ++q)
+    if (q_list[q] < 0 || q_list[q] >= n_lists) return fail(AUR_ERR_INVALID, "q_list[%d] = %d is not a list", q, q_list[q]);
+
+  HostCall call(ix);
+  if ((rc = call.open()) != AUR_OK) return rc;
+  SearchCtx* c = call.c;
+  cudaStream_t s = call.s;
+  // staging (int32): [every named list's rows of the published prefix, sorted, once each][the plan's blocks]
+  std::vector<char> named(static_cast<size_t>(n_lists), 0);
+  for (int32_t q = 0; q < nq; ++q) named[static_cast<size_t>(q_list[q])] = 1;
+  ListPlan pl;
+  std::vector<int64_t> lrow0(static_cast<size_t>(n_lists), 0), llen(static_cast<size_t>(n_lists), 0);
+  for (int32_t l = 0; l < n_lists; ++l) {
+    const size_t r0 = pl.stage.size();
+    lrow0[static_cast<size_t>(l)] = static_cast<int64_t>(r0);
+    if (!named[static_cast<size_t>(l)]) continue;
+    resolve_ids(ix, list_ids + list_offsets[l], list_offsets[l + 1] - list_offsets[l], call.n_rows,
+                [&](int64_t, int32_t row) { pl.stage.push_back(row); });
+    std::sort(pl.stage.begin() + r0, pl.stage.end());
+    pl.stage.erase(std::unique(pl.stage.begin() + r0, pl.stage.end()), pl.stage.end());
+    llen[static_cast<size_t>(l)] = static_cast<int64_t>(pl.stage.size() - r0);
+  }
+  if ((rc = plan_list_search(nq, k, q_list, lrow0, llen, &pl)) != AUR_OK) return rc;
+  rc = stats_begin(c, s, nq, call.n_rows);
+  if (rc == AUR_OK) rc = call.stage(queries_host, nq, k, scores_out, ids_out);
+  if (rc == AUR_OK) rc = run_list_search(ix, c, s, pl, nq, k, nullptr, call.d_scores, call.d_ids);
+  if (rc == AUR_OK) rc = stats_end(ix, c, s);
+  if ((rc = call.finish(rc, nq, k, scores_out, ids_out)) != AUR_OK) return rc;
+  if (snapshot_rows_out) *snapshot_rows_out = call.n_rows;
+  return AUR_OK;
 }
 
 int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t* codes, int64_t n) {
@@ -1315,10 +1290,9 @@ int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t*
     a = ix->d_attr[col - 2];
   }
   if (!a) {   // first use: every row absent (-1), at the padded capacity like the tenant codes
-    const int64_t cap_pad = (ix->capacity + kTcTileN - 1) / kTcTileN * kTcTileN;
-    cudaError_t e = cudaMalloc(&a, static_cast<size_t>(cap_pad) * 4);
+    cudaError_t e = cudaMalloc(&a, static_cast<size_t>(ix->cap_pad) * 4);
     if (e != cudaSuccess) return fail(AUR_ERR_NOMEM, "attribute column: %s", cudaGetErrorString(e));
-    e = cudaMemsetAsync(a, 0xFF, static_cast<size_t>(cap_pad) * 4, s);
+    e = cudaMemsetAsync(a, 0xFF, static_cast<size_t>(ix->cap_pad) * 4, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) { cudaFree(a); return fail(AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e)); }
     std::lock_guard<std::mutex> lk(ix->mu);
@@ -1326,15 +1300,7 @@ int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t*
   }
   std::vector<int32_t> pairs;
   pairs.reserve(2 * static_cast<size_t>(n));
-  {
-    std::lock_guard<std::mutex> lk(ix->mu);
-    for (int64_t i = 0; i < n; ++i) {
-      auto it = ix->id2row.find(ids[i]);
-      if (it == ix->id2row.end()) continue;
-      pairs.push_back(static_cast<int32_t>(it->second));
-      pairs.push_back(codes[i]);
-    }
-  }
+  resolve_ids(ix, ids, n, INT64_MAX, [&](int64_t i, int32_t row) { pairs.push_back(row); pairs.push_back(codes[i]); });
   if (pairs.empty()) return AUR_OK;
   CU_TRY(ix->attr_stage.reserve(pairs.size()));
   CU_TRY(cudaMemcpyAsync(ix->attr_stage.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s));
@@ -1355,49 +1321,33 @@ int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int
     if (q_program[q] < 0 || q_program[q] >= n_programs) return fail(AUR_ERR_INVALID, "q_program[%d] = %d is not a program", q, q_program[q]);
   if (max_list_rows < 0) return fail(AUR_ERR_INVALID, "max_list_rows < 0");
 
-  std::shared_lock<std::shared_mutex> rl(ix->rw);
-  CU_TRY(cudaSetDevice(ix->device));
-  SearchCtx* c = nullptr;
-  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
-  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
-  std::lock_guard<std::mutex> cl(c->mu);
-  cudaStream_t s = c->own_stream;
-  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
-  c->last_launches = 0;
-  CU_TRY(cudaEventRecord(c->ev_begin, s));
+  HostCall call(ix);
+  if ((rc = call.open()) != AUR_OK) return rc;
+  SearchCtx* c = call.c;
+  cudaStream_t s = call.s;
+  const int64_t n_rows = call.n_rows;
+  if ((rc = stats_begin(c, s, nq, n_rows)) != AUR_OK) return rc;
   std::vector<int64_t> tot;
   if ((rc = filter_count(ix, c, s, prog, prog_offsets, n_programs, bitmap, bitmap_words, n_rows, &tot)) != AUR_OK) return rc;
   if (n_programs == 1 && tot[0] > max_list_rows) {
     // dense: the matching rows as a row mask, and the masked scan aur_search_subset runs
-    const size_t qbytes = static_cast<size_t>(nq) * ix->dim * 2;
-    const size_t nout = static_cast<size_t>(nq) * k;
-    CU_TRY(c->stage_q.reserve(qbytes));
-    CU_TRY(c->stage_scores.reserve(nout));
-    CU_TRY(c->stage_ids.reserve(nout));
-    CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
     Scope sc;
     sc.match_mask = c->filt_mask.p;
-    float* d_scores = c->stage_scores.p;
-    int64_t* d_ids = c->stage_ids.p;
-    const bool direct = direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
-    rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, d_scores, d_ids, nullptr, s, nullptr, true);
-    if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
-    if (!direct) {
-      CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
-      CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
-    }
-    CU_TRY(cudaStreamSynchronize(s));
+    rc = call.stage(queries_host, nq, k, scores_out, ids_out);
+    if (rc == AUR_OK) rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, call.d_scores, call.d_ids, nullptr, s);
   } else {
     // lists: every program's rows written on the device, in the order the host path stages them; items from the lengths
     std::vector<int64_t> lrow0(static_cast<size_t>(n_programs), 0);
     for (int32_t q = 1; q < n_programs; ++q)
       lrow0[static_cast<size_t>(q)] = lrow0[static_cast<size_t>(q - 1)] + tot[static_cast<size_t>(q - 1)];
     if ((rc = filter_write(ix, c, s, n_programs, tot, n_rows, false)) != AUR_OK) return rc;
-    std::vector<int32_t> stage;
-    rc = run_list_search(ix, c, s, queries_host, nq, k, q_program, n_programs, lrow0, tot, stage, c->filt_rows.p, n_rows, true,
-                         scores_out, ids_out);
-    if (rc != AUR_OK) return rc;
+    ListPlan pl;
+    rc = plan_list_search(nq, k, q_program, lrow0, tot, &pl);
+    if (rc == AUR_OK) rc = call.stage(queries_host, nq, k, scores_out, ids_out);
+    if (rc == AUR_OK) rc = run_list_search(ix, c, s, pl, nq, k, c->filt_rows.p, call.d_scores, call.d_ids);
   }
+  if (rc == AUR_OK) rc = stats_end(ix, c, s);
+  if ((rc = call.finish(rc, nq, k, scores_out, ids_out)) != AUR_OK) return rc;
   if (matched_out) for (int32_t q = 0; q < n_programs; ++q) matched_out[q] = tot[static_cast<size_t>(q)];
   if (snapshot_rows_out) *snapshot_rows_out = n_rows;
   return AUR_OK;
@@ -1410,18 +1360,14 @@ int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const u
   const int32_t off[2] = {0, n_tokens};
   int rc = check_programs(ix, prog, off, 1, bitmap, bitmap_words);
   if (rc != AUR_OK) return rc;
-  std::shared_lock<std::shared_mutex> rl(ix->rw);
-  CU_TRY(cudaSetDevice(ix->device));
-  SearchCtx* c = nullptr;
-  if ((rc = acquire_ctx(ix, nullptr, &c)) != AUR_OK) return rc;
-  struct Guard { aur_index* ix; SearchCtx* c; ~Guard() { release_ctx(ix, c); } } guard{ix, c};
-  std::lock_guard<std::mutex> cl(c->mu);
-  cudaStream_t s = c->own_stream;
-  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
+  HostCall call(ix);
+  if ((rc = call.open()) != AUR_OK) return rc;
+  SearchCtx* c = call.c;
+  cudaStream_t s = call.s;
   std::vector<int64_t> tot;
-  if ((rc = filter_count(ix, c, s, prog, off, 1, bitmap, bitmap_words, n_rows, &tot)) != AUR_OK) return rc;
+  if ((rc = filter_count(ix, c, s, prog, off, 1, bitmap, bitmap_words, call.n_rows, &tot)) != AUR_OK) return rc;
   const int64_t n = tot[0], m = std::min(n, cap);
-  if ((rc = filter_write(ix, c, s, 1, tot, n_rows, true)) != AUR_OK) return rc;
+  if ((rc = filter_write(ix, c, s, 1, tot, call.n_rows, true)) != AUR_OK) return rc;
   std::vector<int64_t> got(static_cast<size_t>(m));
   if (m) CU_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToHost, s));
   CU_TRY(cudaStreamSynchronize(s));
@@ -1552,6 +1498,7 @@ int aur_search_exchange_dev(aur_index* ix, aur_exchange* ex, const void* queries
   if (ex->device != ix->device) return fail(AUR_ERR_INVALID, "exchange and index live on different devices");
   if (nq > ex->nq_max || k > ex->k_max || static_cast<size_t>(nq) * k > ex->entries)
     return fail(AUR_ERR_INVALID, "batch %d x top-%d exceeds the exchange's %d x %d", nq, k, ex->nq_max, ex->k_max);
+  if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   CU_TRY(cudaSetDevice(ix->device));
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
@@ -1563,9 +1510,11 @@ int aur_search_exchange_dev(aur_index* ix, aur_exchange* ex, const void* queries
   for (int r = 0; r < ex->world; ++r) eo.slot[r] = ex->peer[r] + static_cast<size_t>(ex->rank) * ex->slot_stride;
   eo.seq = ex->d_seq;
   eo.parity_stride = ex->parity_stride;
+  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
   Scope sc;
-  rc = search_enqueue(ix, c, queries_dev, nq, k, sc, ix->rows_pub.load(std::memory_order_acquire), nullptr, nullptr, nullptr, s, &eo);
-  if (rc != AUR_OK) return rc;
+  if ((rc = stats_begin(c, s, nq, n_rows)) != AUR_OK) return rc;
+  if ((rc = search_enqueue(ix, c, queries_dev, nq, k, sc, n_rows, nullptr, nullptr, nullptr, s, &eo)) != AUR_OK) return rc;
+  if ((rc = stats_end(ix, c, s)) != AUR_OK) return rc;
   ExchangeParams p{};
   p.slots = ex->local;
   p.seq = ex->d_seq; p.done = ex->d_done; p.status = ex->d_done + 1;

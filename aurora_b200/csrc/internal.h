@@ -90,15 +90,12 @@ constexpr int kTcPubMax = 74;      // published values a thread folds into its t
 // other's entries as its own.  0 is never a tag: it marks a zeroed table.
 constexpr uint32_t kSearchEpochMax = 0x7FFFFFFFu;
 
-// epi_groups: 1 = two epilogue warps take every tile; 2 = two pairs of warps alternate tiles
-// (each pair owns one score buffer and its own candidate lists).
-// tile_n: corpus rows per tile, kTcTileN or kTcTileWide (epi_groups 1 only); mask: a kMask launch (row_mask set).
-size_t tc_smem_bytes(int epi_groups, int num_stages, int ksel, int dim, int tile_n, bool mask);
-int tc_pick_stages(int epi_groups, int ksel, int dim, size_t smem_limit, int tile_n, bool mask);
+// tile_n: corpus rows per tile, kTcTileN or kTcTileWide; mask: a kMask launch (row_mask set).
+size_t tc_smem_bytes(int num_stages, int ksel, int dim, int tile_n, bool mask);
+int tc_pick_stages(int ksel, int dim, size_t smem_limit, int tile_n, bool mask);
 // Launches the fused similarity + top-k kernel; cta_group 2 = two-CTA clusters sharing every corpus tile by TMA
 // multicast.  tmap: CUtensorMap over the corpus with a {64, tile_n / cta_group} box and 128-byte swizzle.
-cudaError_t tc_launch(int cta_group, int epi_groups, int tile_n, int grid, const void* tmap, const TcParams& p, size_t smem,
-                      cudaStream_t s);
+cudaError_t tc_launch(int cta_group, int tile_n, int grid, const void* tmap, const TcParams& p, size_t smem, cudaStream_t s);
 
 // ---------------------------------------------------------------- SIMT kernels
 struct FilterArgs {
@@ -286,6 +283,20 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   cfg.attrs = attr; cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
+
+template <typename T>
+struct DevBuf {   // grow-only device scratch
+  T* p = nullptr; size_t n = 0;
+  cudaError_t reserve(size_t want) {
+    if (want <= n) return cudaSuccess;
+    if (p) cudaFree(p);
+    p = nullptr; n = 0;
+    cudaError_t e = cudaMalloc(&p, want * sizeof(T));
+    if (e == cudaSuccess) n = want;
+    return e;
+  }
+  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
+};
 
 // Error reporting shared by the translation units behind the C ABI (thread-local message).
 int report_error(int code, const char* fmt, ...);

@@ -245,30 +245,16 @@ __global__ void kw_gather_postings(const uint2* post, const int64_t* old_off, co
   for (int64_t i = lane; i < o1 - o0; i += 32) out[d + i] = post[o0 + i];
 }
 
-template <typename T>
-struct KwBuf {   // grow-only device scratch
-  T* p = nullptr; size_t n = 0;
-  cudaError_t reserve(size_t want) {
-    if (want <= n) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; n = 0;
-    cudaError_t e = cudaMalloc(&p, want * sizeof(T));
-    if (e == cudaSuccess) n = want;
-    return e;
-  }
-  void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-};
-
 // Scratch of one in-flight search (a pool, so several host threads can search at once).
 struct KwCtx {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  KwBuf<unsigned char> tab;     // launch term table
-  KwBuf<Cand> buf, lists_a, lists_b;
-  KwBuf<double> cval, out_s;
-  KwBuf<int64_t> out_ids;
-  KwBuf<uint8_t> allow;
-  KwBuf<int32_t> allow_rows;
+  DevBuf<unsigned char> tab;     // launch term table
+  DevBuf<Cand> buf, lists_a, lists_b;
+  DevBuf<double> cval, out_s;
+  DevBuf<int64_t> out_ids;
+  DevBuf<uint8_t> allow;
+  DevBuf<int32_t> allow_rows;
   int launches = 0, terms = 0, spilled = 0;   // of the last search: kernels, most distinct terms in one launch,
                                               // launches whose contribution table spilled to global memory
   void release() {
@@ -352,7 +338,7 @@ int tombstone_rows(aur_kw* kw, const std::vector<int64_t>& rows) {
     noff[j + 1] = noff[j] + (kw->h_off[r + 1] - kw->h_off[r]);
   }
   std::vector<uint2> terms(static_cast<size_t>(noff[m]));
-  KwBuf<int32_t> d_map; KwBuf<int64_t> d_noff; KwBuf<uint2> d_terms;
+  DevBuf<int32_t> d_map; DevBuf<int64_t> d_noff; DevBuf<uint2> d_terms;
   cudaStream_t s = kw->stream;
   cudaError_t e = d_map.reserve(m);
   if (e == cudaSuccess) e = d_noff.reserve(m + 1);
@@ -585,7 +571,7 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
         c->launches += 1;
         break;
       }
-      KwBuf<Cand>& dst = in_a ? c->lists_b : c->lists_a;
+      DevBuf<Cand>& dst = in_a ? c->lists_b : c->lists_a;
       KW_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
       kw_fold_kernel<<<dim3(n_groups, nqb), 256, fsmem, s>>>(cur, n_lists, ksel, group, sort_n, dst.p, nullptr, nullptr, k);
       KW_TRY(cudaGetLastError());

@@ -7,25 +7,24 @@
 // server/routes/incident_feedback/weaviate_client.py:286-291).
 //
 // Tile width N = 64 or 128 corpus rows (kTileN, chosen per launch on the host, tc_auto_tile in capi.cu): 128 when its
-// layout keeps at least four 16 KB ring stages and there is one epilogue group -- at dim 768 / top-32 four stages against
-// eight 8 KB ones -- else 64.  The wide tile runs wgmma m64n128k16: the query operand is fetched from shared memory once
+// layout keeps at least four 16 KB ring stages -- at dim 768 / top-32 four stages against eight 8 KB ones -- else 64.  The wide tile runs wgmma m64n128k16: the query operand is fetched from shared memory once
 // per 128 corpus rows instead of once per 64, and the drain, score-buffer hand-off and threshold read happen once per
 // 128 rows.  Its epilogue examines a tile 64 scores at a time with the 64-row code.
 //
-// One CTA, persistent, 1 CTA / SM (G = 1 or 2 epilogue groups):
-//   warps 1..2G  epilogue  : thread r of a group owns query r (score-buffer row r): reads its N scores of a
+// One CTA, persistent, 1 CTA / SM:
+//   warps 1..2   epilogue  : thread r of the two warps owns query r (score-buffer row r): reads its N scores of a
 //                            tile, scales them by the rows' inverse norms, keeps one max per 16 scores and
 //                            compares it with the query's threshold; a four-score group that reaches it is
 //                            parked in a per-thread FIFO in shared memory and examined later, out of line and
 //                            rarely (drain_fifo); large k without room for the FIFO pushes at once (push_group4).
 //   warp 0      threshold  : serves the certified global threshold of the queries assigned to this CTA (see
 //                            "Threshold exchange").
-//   warp 2G+1   TMA producer: corpus tiles [N rows x 64 k] -> smem ring (SWIZZLE_128B)
-//   warpgroup   MMA        : wgmma m64nNk16, A = the CTA's 64 queries (K-major tiles in shared memory), B =
+//   warp 3      TMA producer: corpus tiles [N rows x 64 k] -> smem ring (SWIZZLE_128B)
+//   warps 4..7  MMA        : wgmma m64nNk16, A = the CTA's 64 queries (K-major tiles in shared memory), B =
 //                            corpus tile from the ring; the [64 queries x N rows] fp32 accumulator lives in
 //                            registers for the whole tile and is then stored to a padded score buffer that the
-//                            epilogue group of that tile reads row-wise (one buffer per group).  The MMA of the
-//                            next tile runs while the epilogue works on the buffer it just released.
+//                            epilogue warps read row-wise.  The MMA of the next tile runs while the epilogue
+//                            works on the buffer it just released.
 // Two-CTA clusters (AUR_KERNEL_TC2): the pair shares every corpus tile -- each CTA TMA-loads N / 2 of the N rows and
 // multicasts them to both, so a tile crosses L2 -> SM once per pair; each CTA scores its own 64 queries.
 // Single CTAs: when nq > 64 several CTAs take the same tiles for different query blocks (sharing through L2).
@@ -64,12 +63,13 @@ using namespace ptx;
 
 namespace {
 
+// warps: threshold, two epilogue, producer, then the MMA warpgroup at the next multiple of four: 8 warps, two per SM
+// sub-partition, up to 255 registers a thread (no spills).
 constexpr int kThrWarps = 1;
-// warps: threshold, 2G epilogue, producer, then the MMA warpgroup at the next multiple of four.  G = 1: 8 warps, two per
-// SM sub-partition, up to 255 registers a thread (no spills).  G = 2 (selectable for experiments) needs 10 live warps,
-// three on some sub-partition, which caps a thread at 168 registers whatever the order of the roles: a spill of a few
-// bytes in that variant.
-__host__ __device__ constexpr int tc_mma_warp0(int epi_groups) { return (kThrWarps + 2 * epi_groups + 1 + 3) / 4 * 4; }
+constexpr int kEpiWarps = 2;
+constexpr int kProducerWarp = kThrWarps + kEpiWarps;
+constexpr int kMmaWarp0 = (kProducerWarp + 1 + 3) / 4 * 4;   // first warp of the MMA warpgroup (warpgroup-aligned)
+constexpr int kThreads = 32 * (kMmaWarp0 + 4);
 constexpr uint32_t kSlot = kTcQRows * 8u;   // byte stride between list slots of one query
 constexpr uint32_t kQTileBytes = kTcQRows * 128u;   // one 64-dim k-block of the query block
 // one 64-dim k-block of a corpus tile (a ring stage); floats per score-buffer row (padding spreads the banks)
@@ -83,19 +83,19 @@ struct SmemLayout {
 };
 // The 128-row layout fits a fourth 16 KB ring stage at dim 768 / ksel 40 only without what the 64-row one can afford:
 // it reserves the tenant-scope masks for kMask launches alone and parks half as many groups per thread in the FIFO.
-__host__ __device__ inline SmemLayout make_layout(int epi_groups, int num_stages, int ksel, int dim, int tile_n, bool mask) {
+__host__ __device__ inline SmemLayout make_layout(int num_stages, int ksel, int dim, int tile_n, bool mask) {
   SmemLayout L;
   const bool wide = tile_n == kTcTileWide;
   L.lcap = static_cast<uint32_t>(ksel);
   uint32_t o = stage_bytes(tile_n) * num_stages;
   // the query block: [64 queries x 64] bf16 K-major SWIZZLE_128B tiles, one per k-block (the wgmma A operand)
   L.off_qs = o;     o += static_cast<uint32_t>(dim / kTcKBlock) * kQTileBytes;
-  L.off_sc = o;     o += static_cast<uint32_t>(epi_groups) * sc_bytes(tile_n);
-  L.off_list = o;   o += static_cast<uint32_t>(epi_groups) * L.lcap * kSlot;
-  L.off_norm = o;   o += static_cast<uint32_t>(epi_groups) * 2u * 2u * tile_n * 4u;
-  L.off_mask = o;   if (mask || !wide) o += static_cast<uint32_t>(epi_groups) * 2u * 2u * tile_n * 4u;   // per-row tenant-scope bit masks (kMask launches)
+  L.off_sc = o;     o += sc_bytes(tile_n);
+  L.off_list = o;   o += L.lcap * kSlot;
+  L.off_norm = o;   o += 2u * 2u * tile_n * 4u;
+  L.off_mask = o;   if (mask || !wide) o += 2u * 2u * tile_n * 4u;   // per-row tenant-scope bit masks (kMask launches)
   // deferred-candidate FIFO: per thread kTcFifoRecs records of four adjacent scores (16 B) + a row tag
-  L.fifo_recs = (epi_groups == 1 && ksel <= kTcFifoMaxKsel) ? (wide ? kTcFifoRecs / 2 : kTcFifoRecs) : 0u;
+  L.fifo_recs = ksel <= kTcFifoMaxKsel ? (wide ? kTcFifoRecs / 2 : kTcFifoRecs) : 0u;
   L.off_fifo = o;   o += L.fifo_recs * kTcQRows * (16u + 4u);
   L.off_tau = o;    o += kTcQRows * 4u;   // certified thresholds of this CTA's queries, refreshed by the threshold warp
   L.off_bar = o;    o += (2u * kTcMaxStages + 2u + 2u + 1u) * 8u + 16u;
@@ -261,9 +261,7 @@ __device__ __forceinline__ float read_threshold(const unsigned long long* tq, ui
 // Publishes value v of this launch into a CTA's exchange slot.  The slot's first publish of a launch REPLACES the entry
 // (atomicExch), later ones keep the max.  A plain atomicMax would never get past an entry that another launch left with
 // a numerically larger tag -- a bring-up launch (upper half of the tags) or any search before the counter wrapped --
-// and the exchange would stay without a valid value for that slot until the table is reallocated.  With two epilogue
-// groups both groups' first publishes replace: the slot may drop to the smaller of their values for a moment, which is
-// still a value the CTA vouches for, so every threshold derived from it stays certified.
+// and the exchange would stay without a valid value for that slot until the table is reallocated.
 __device__ __forceinline__ void publish_value(unsigned long long* slot, uint32_t epoch, float v, bool first) {
   const unsigned long long e = (static_cast<unsigned long long>(epoch) << 32) | f32_to_ord(v);
   if (first) atomicExch(slot, e);
@@ -277,16 +275,12 @@ constexpr uint32_t kNaNBits = 0x7FC00000u;
 // batch may see the row -- and every query knows its scope's bit: scores of invisible rows become NaN before anything
 // else looks at them, exactly like tombstones.  (One scope for the whole batch needs none of this: it folds into the
 // inverse norms.)
-template <int kCtaGroup, int kEpiGroups, bool kMask, int kTileN>
-__global__ void __launch_bounds__(32 * (tc_mma_warp0(kEpiGroups) + 4), 1)
+template <int kCtaGroup, bool kMask, int kTileN>
+__global__ void __launch_bounds__(kThreads, 1)
 simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
-  static_assert(kTileN == kTcTileN || (kTileN == kTcTileWide && kEpiGroups == 1), "tile width");
-  constexpr int kEpiWarps = 2 * kEpiGroups;
-  constexpr int kProducerWarp = kEpiWarps + kThrWarps;
-  constexpr int kMmaWarp0 = tc_mma_warp0(kEpiGroups);   // first warp of the MMA warpgroup (warpgroup-aligned)
+  static_assert(kTileN == kTcTileN || kTileN == kTcTileWide, "tile width");
   constexpr uint32_t kStageBytes = stage_bytes(kTileN);
   constexpr int kScStride = sc_stride(kTileN);
-  constexpr uint32_t kScBytes = sc_bytes(kTileN);
   constexpr int kHalves = kTileN / 64;   // the epilogue examines a tile 64 scores (four 16-score chunks) at a time
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment; the runtime only guarantees 16.  Offsetting
@@ -294,16 +288,16 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   // shared-address-space inference, i.e. LDS/STS instead of generic loads.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
 
-  const SmemLayout L = make_layout(kEpiGroups, p.num_stages, p.ksel, p.dim, kTileN, kMask);
-  float* normbuf = reinterpret_cast<float*>(smem + L.off_norm);      // [2G warps][2][kTileN]
-  uint32_t* maskbuf = reinterpret_cast<uint32_t*>(smem + L.off_mask);  // [2G warps][2][kTileN]
-  float* scbuf = reinterpret_cast<float*>(smem + L.off_sc);          // [G][64 queries][kScStride]
+  const SmemLayout L = make_layout(p.num_stages, p.ksel, p.dim, kTileN, kMask);
+  float* normbuf = reinterpret_cast<float*>(smem + L.off_norm);      // [2 warps][2][kTileN]
+  uint32_t* maskbuf = reinterpret_cast<uint32_t*>(smem + L.off_mask);  // [2 warps][2][kTileN]
+  float* scbuf = reinterpret_cast<float*>(smem + L.off_sc);          // [64 queries][kScStride]
   volatile float* tau_s = reinterpret_cast<volatile float*>(smem + L.off_tau);   // [64]
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.off_bar);
   uint64_t* full_bar = bars;                              // [kTcMaxStages]
   uint64_t* empty_bar = bars + kTcMaxStages;              // [kTcMaxStages]
-  uint64_t* acc_full = bars + 2 * kTcMaxStages;           // [2] score buffer g written
-  uint64_t* acc_empty = bars + 2 * kTcMaxStages + 2;      // [2] score buffer g read into registers
+  uint64_t* acc_full = bars + 2 * kTcMaxStages;           // [1] score buffer written
+  uint64_t* acc_empty = bars + 2 * kTcMaxStages + 2;      // [1] score buffer read into registers
   uint64_t* q_ready = bars + 2 * kTcMaxStages + 4;        // [1] the query block is in shared memory
   volatile int* epi_done = reinterpret_cast<volatile int*>(bars + 2 * kTcMaxStages + 5);
 
@@ -346,10 +340,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       mbar_init(&full_bar[i], 1);          // this CTA's expect_tx arrive (the bytes may come from both CTAs)
       mbar_init(&empty_bar[i], kCtaGroup); // the MMA warpgroup of every CTA the stage is multicast to
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 128);        // every thread of the MMA warpgroup stores its part
-      mbar_init(&acc_empty[i], 2);         // the two warps of the epilogue group that reads this buffer
-    }
+    mbar_init(acc_full, 128);              // every thread of the MMA warpgroup stores its part
+    mbar_init(acc_empty, kEpiWarps);       // the epilogue warps read the buffer
     mbar_init(q_ready, kEpiWarps);
     *epi_done = 0;
     fence_mbar_init();
@@ -430,7 +422,6 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       if (++rel_stage == p.num_stages) rel_stage = 0;
     };
     for (int it = 0; it < my_tiles; ++it) {
-      const int b = (kEpiGroups == 2) ? (it & 1) : 0;
       float d[kTileN / 2];
 #pragma unroll
       for (int i = 0; i < kTileN / 2; ++i) d[i] = 0.f;
@@ -460,17 +451,16 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       release();
       {
         const long long t0 = TCLK();
-        mbar_wait(&acc_empty[b], ((static_cast<uint32_t>(it / kEpiGroups)) & 1u) ^ 1u);
+        mbar_wait(acc_empty, (static_cast<uint32_t>(it) & 1u) ^ 1u);
         tm_empty += TCLK() - t0;
       }
-      float* sc = scbuf + b * (kScBytes / 4);
 #pragma unroll
       for (int j = 0; j < kTileN / 8; ++j) {
         const int row = 16 * w4 + (l4 >> 2), col = 8 * j + 2 * (l4 & 3);
-        *reinterpret_cast<float2*>(sc + row * kScStride + col) = make_float2(d[4 * j + 0], d[4 * j + 1]);
-        *reinterpret_cast<float2*>(sc + (row + 8) * kScStride + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+        *reinterpret_cast<float2*>(scbuf + row * kScStride + col) = make_float2(d[4 * j + 0], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(scbuf + (row + 8) * kScStride + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
       }
-      mbar_arrive(&acc_full[b]);
+      mbar_arrive(acc_full);
     }
     if ((p.dbg_flags & 64) && p.dbg_scores != nullptr && wt == 0) {
       float* dd = p.dbg_scores + static_cast<size_t>(blockIdx.x) * kTcQRows * kTcTileN + 32;
@@ -478,8 +468,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       dd[2] = static_cast<float>(TCLK() - tm_begin);
     }
   } else if (warp < kProducerWarp) {
-    // ================= threshold warp (0) and epilogue warps (1-2G) =================
-    const int ew = warp - kThrWarps;           // epilogue warp 0 .. 2G-1 (the threshold warp: -1)
+    // ================= threshold warp (0) and epilogue warps (1-2) =================
+    const int ew = warp - kThrWarps;           // epilogue warp 0 .. 1 (the threshold warp: -1)
     const int quarter = ew & 1;                // which 32 queries of the block this warp owns
     const int r = (warp < kThrWarps) ? lane : quarter * 32 + lane;   // query row inside the CTA
     const int qglob = qblock * kTcQRows + r;   // query index inside this launch
@@ -537,10 +527,9 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       }
     } else {
       // ============================== epilogue warps ==============================
-      const int grp = ew >> 1;   // epilogue group: takes tiles grp, grp + groups, ...
       const long long t_kernel0 = TCLK();
       // ---- the query block into shared memory: [64 queries x 128 B] K-major tiles with the 128-byte swizzle TMA
-      //      would produce (16-byte chunk c of row r at c ^ (r & 7)); with two groups each loads every other k-block.
+      //      would produce (16-byte chunk c of row r at c ^ (r & 7)).
       //      A warp reads its 32 rows coalesced (lane l takes 16-byte piece l of 4 consecutive rows per instruction).
       {
         const uint8_t* qbase = reinterpret_cast<const uint8_t*>(p.q);
@@ -556,19 +545,18 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
         };
         // every CTA of a query block reads the same block at the same moment: start each at a different
         // k-block (rotation by tile set) so they do not all queue on the same L2 lines
-        const int n_j = (kbs - grp + kEpiGroups - 1) / kEpiGroups;      // k-blocks this group loads
-        const int rot = n_j > 0 ? tset % n_j : 0;
-        auto kb_of = [&](int j) { return (j < n_j) ? grp + ((j + rot) % n_j) * kEpiGroups : kbs; };
+        const int rot = kbs > 0 ? tset % kbs : 0;
+        auto kb_of = [&](int j) { return (j < kbs) ? (j + rot) % kbs : kbs; };
         // four k-blocks of loads (32 x 16 B per lane) are issued before the first is consumed
         constexpr int kDepth = 4;
         uint4 x[kDepth][8];
-        for (int j0 = 0; j0 < n_j; j0 += kDepth) {
+        for (int j0 = 0; j0 < kbs; j0 += kDepth) {
 #pragma unroll
           for (int u = 0; u < kDepth; ++u) load_kb(kb_of(j0 + u), x[u]);
 #pragma unroll
           for (int u = 0; u < kDepth; ++u) {
             const int j = j0 + u;
-            if (j >= n_j) break;
+            if (j >= kbs) break;
             uint8_t* tile = smem + L.off_qs + static_cast<uint32_t>(kb_of(j)) * kQTileBytes + quarter * 32 * 128;
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
@@ -581,7 +569,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
         __syncwarp();
         if (lane == 0) mbar_arrive(q_ready);
       }
-      const float* myrow = scbuf + grp * (kScBytes / 4) + r * kScStride;   // this query's row of the group's score buffer
+      const float* myrow = scbuf + r * kScStride;   // this query's row of the score buffer
       auto load_scores = [&](uint32_t (&acc)[4][16], int h) {   // scores 64 h .. 64 h + 63 of the tile
 #pragma unroll
         for (int c = 0; c < 4; ++c)
@@ -596,7 +584,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       uint32_t* mymask = maskbuf + ew * 2 * kTileN;
       uint32_t mybit = 0u;                                       // this query's tenant-scope bit
       if constexpr (kMask) { if (qglob < p.nq) mybit = 1u << (p.q_scope[qglob] & 31); }
-      const uint32_t list_a = smem_u32(smem + L.off_list) + (static_cast<uint32_t>(grp) * L.lcap * kTcQRows + r) * 8u;
+      const uint32_t list_a = smem_u32(smem + L.off_list) + static_cast<uint32_t>(r) * 8u;
       // deferred-candidate FIFO (see drain_fifo) whenever shared memory has room for it
       const bool use_fifo = L.fifo_recs > 0;
       const uint32_t fifo_a = smem_u32(smem + L.off_fifo) + r * 16u;
@@ -617,10 +605,9 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       constexpr int kNv = kTileN / 32;
       float nn[kNv];
       uint32_t mm[kNv];                                         // (masks of the tile in flight, beside its norms)
-      auto load_norms = [&](int li2) {
+      auto load_norms = [&](int it2) {
 #pragma unroll
         for (int i = 0; i < kNv; ++i) { nn[i] = __uint_as_float(kNaNBits); mm[i] = 0u; }
-        const int it2 = grp + li2 * kEpiGroups;
         if (it2 < my_tiles) {
           const int64_t rbase = static_cast<int64_t>(tset + it2 * n_tsets) * kTileN;
 #pragma unroll
@@ -650,8 +637,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       // publish them, wait until enough CTAs have done the same (~5 us, once), and let the
       // main loop examine the tile against the first certified threshold.  The accumulator
       // buffer is not released here, so the MMA cannot overwrite it before the loop reads it again.
-      if (xchg && grp < my_tiles) {
-        mbar_wait(&acc_full[grp], 0);
+      if (xchg && my_tiles > 0) {
+        mbar_wait(acc_full, 0);
 #pragma unroll 1
         for (int c = 0; c < kTileN / 16; ++c) {
           uint32_t a16[16];
@@ -686,26 +673,24 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
         t_boot = TCLK() - t_begin;
       }
 
-      int li = 0;  // this group's iteration count
-      for (int it = grp; it < my_tiles; it += kEpiGroups, ++li) {
+      for (int it = 0; it < my_tiles; ++it) {
         const int tile = tset + it * n_tsets;
         const int row0 = tile * kTileN;
-        const int b = grp;
-        const float* nbt = mynorm + (li & 1) * kTileN;
+        const float* nbt = mynorm + (it & 1) * kTileN;
         const long long t_top0 = TCLK();
         const float thr_now = (xchg && !(p.dbg_flags & 16)) ? tau_s[r] : -INFINITY;   // shared-memory copy kept by the threshold warp
 
         // norms of the next tile (loaded one iteration ago) -> the other buffer; start the
         // loads for the tile after that.  A whole tile period hides the HBM latency.
         if (!(p.dbg_flags & 32)) {
-          store_norms((li + 1) & 1);
-          load_norms(li + 2);
+          store_norms((it + 1) & 1);
+          load_norms(it + 2);
           __syncwarp();
         }
 
         {
           const long long t0 = TCLK();
-          mbar_wait(&acc_full[b], (static_cast<uint32_t>(li)) & 1u);
+          mbar_wait(acc_full, (static_cast<uint32_t>(it)) & 1u);
           t_wait += TCLK() - t0;
         }
         // A wide tile is examined 64 scores at a time by the same code, half 0 while the buffer is still held.
@@ -718,7 +703,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
           if (!(p.dbg_flags & 1)) load_scores(acc, h);
           if (h == kHalves - 1) {   // the whole tile in registers or examined: hand the buffer back to the MMA warpgroup
             __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[b]);
+            if (lane == 0) mbar_arrive(acc_empty);
           }
           t_ld += TCLK() - t_ld0;
           if (p.dbg_flags & (1 | 4)) continue;
@@ -727,7 +712,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
           // Fast path: scale by 1/|c_j| in place and keep one running max per 16
           // scores.  (NaN norm = tombstone / out of range: fmaxf drops it, `>=` rejects it.)
           if constexpr (kMask) {   // rows this query's tenant scope may not see: NaN, like tombstones
-            const uint32_t* mb = mymask + (li & 1) * kTileN + h * 64;
+            const uint32_t* mb = mymask + (it & 1) * kTileN + h * 64;
 #pragma unroll
             for (int c = 0; c < 4; ++c)
 #pragma unroll
@@ -755,7 +740,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
             }
             cmax[c] = m;
           }
-          if (p.dbg_scores != nullptr && it == 0 && h == 0 && !(p.dbg_flags & 64)) {  // (group 0 owns tile 0)
+          if (p.dbg_scores != nullptr && it == 0 && h == 0 && !(p.dbg_flags & 64)) {
 #pragma unroll
             for (int c = 0; c < 4; ++c)
 #pragma unroll
@@ -766,7 +751,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
 
           t_fast += TCLK() - t_fast0;
           // what this CTA can vouch for (published below): chunk maxima are distinct rows
-          if (!(booted && li == 0)) {
+          if (!(booted && it == 0)) {
             if (xm == 1) st.top[0] = fmaxf(st.top[0], fmaxf(fmaxf(cmax[0], cmax[1]), fmaxf(cmax[2], cmax[3])));
             else { top4_insert(st.top, cmax[0]); top4_insert(st.top, cmax[1]); top4_insert(st.top, cmax[2]); top4_insert(st.top, cmax[3]); }
           }
@@ -817,7 +802,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
           }
           }
 
-          if (li < 8) t_top += TCLK() - t_ch0; else t_chunks += TCLK() - t_ch0;   // t_top reused: early tiles
+          if (it < 8) t_top += TCLK() - t_ch0; else t_chunks += TCLK() - t_ch0;   // t_top reused: early tiles
         }
         if (p.dbg_flags & (1 | 4 | 8)) continue;
         const long long t_pub0 = TCLK();
@@ -845,14 +830,14 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       //      to this query's compact candidate row
       st = compact_list(st, list_a, ksel, p.ids);
       {
-        const size_t cap = static_cast<size_t>(n_tsets) * kEpiGroups * ksel;
+        const size_t cap = static_cast<size_t>(n_tsets) * ksel;
         uint64_t* out = p.cand + static_cast<size_t>(qglob) * cap;
         if (st.nfill > 0 && qglob < p.nq) {
           const uint32_t slot0 = atomicAdd(p.cand_count + qglob, static_cast<uint32_t>(st.nfill));
           for (int t = 0; t < st.nfill; ++t) out[slot0 + t] = lds_u64(list_a + t * kSlot);
         }
       }
-      if ((p.dbg_flags & 64) && p.dbg_scores != nullptr && grp == 0) {
+      if ((p.dbg_flags & 64) && p.dbg_scores != nullptr) {
         float* d = p.dbg_scores + (static_cast<size_t>(blockIdx.x) * kTcQRows + r) * kTcTileN;
         d[0] = static_cast<float>(st.nfill); d[1] = static_cast<float>(nslow);
         d[2] = tau_end; d[3] = st.tau_local;
@@ -873,9 +858,9 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   if constexpr (kCtaGroup == 2) cluster_sync_all();
 }
 
-template <int kCtaGroup, int kEpiGroups, bool kMask, int kTileN>
+template <int kCtaGroup, bool kMask, int kTileN>
 cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm, const TcParams& p, size_t smem) {
-  auto kern = simtopk_tc_kernel<kCtaGroup, kEpiGroups, kMask, kTileN>;
+  auto kern = simtopk_tc_kernel<kCtaGroup, kMask, kTileN>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
   return cudaLaunchKernelEx(&cfg, kern, tm, p);
@@ -883,21 +868,20 @@ cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm,
 
 }  // namespace
 
-size_t tc_smem_bytes(int epi_groups, int num_stages, int ksel, int dim, int tile_n, bool mask) {
-  return make_layout(epi_groups, num_stages, ksel, dim, tile_n, mask).total + 1024;  // + alignment slack
+size_t tc_smem_bytes(int num_stages, int ksel, int dim, int tile_n, bool mask) {
+  return make_layout(num_stages, ksel, dim, tile_n, mask).total + 1024;  // + alignment slack
 }
 
-int tc_pick_stages(int epi_groups, int ksel, int dim, size_t smem_limit, int tile_n, bool mask) {
+int tc_pick_stages(int ksel, int dim, size_t smem_limit, int tile_n, bool mask) {
   for (int s = kTcMaxStages; s >= 2; --s)
-    if (tc_smem_bytes(epi_groups, s, ksel, dim, tile_n, mask) <= smem_limit) return s;
+    if (tc_smem_bytes(s, ksel, dim, tile_n, mask) <= smem_limit) return s;
   return 0;
 }
 
-cudaError_t tc_launch(int cta_group, int epi_groups, int tile_n, int grid, const void* tmap, const TcParams& p, size_t smem,
-                      cudaStream_t s) {
+cudaError_t tc_launch(int cta_group, int tile_n, int grid, const void* tmap, const TcParams& p, size_t smem, cudaStream_t s) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(32 * (tc_mma_warp0(epi_groups) + 4));
+  cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
   cudaLaunchAttribute attr[1];
@@ -909,17 +893,12 @@ cudaError_t tc_launch(int cta_group, int epi_groups, int tile_n, int grid, const
   cfg.numAttrs = 1;
   const CUtensorMap& tm = *reinterpret_cast<const CUtensorMap*>(tmap);
   const bool mask = p.row_mask != nullptr;
-  if (tile_n == kTcTileWide) {   // one epilogue group only
-    if (epi_groups != 1) return cudaErrorInvalidValue;
-    if (cta_group == 2) return mask ? launch_variant<2, 1, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<2, 1, false, kTcTileWide>(cfg, tm, p, smem);
-    return mask ? launch_variant<1, 1, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<1, 1, false, kTcTileWide>(cfg, tm, p, smem);
+  if (tile_n == kTcTileWide) {
+    if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileWide>(cfg, tm, p, smem);
+    return mask ? launch_variant<1, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileWide>(cfg, tm, p, smem);
   }
-  if (cta_group == 2) {
-    if (epi_groups == 2) return mask ? launch_variant<2, 2, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<2, 2, false, kTcTileN>(cfg, tm, p, smem);
-    return mask ? launch_variant<2, 1, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<2, 1, false, kTcTileN>(cfg, tm, p, smem);
-  }
-  if (epi_groups == 2) return mask ? launch_variant<1, 2, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<1, 2, false, kTcTileN>(cfg, tm, p, smem);
-  return mask ? launch_variant<1, 1, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<1, 1, false, kTcTileN>(cfg, tm, p, smem);
+  if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileN>(cfg, tm, p, smem);
+  return mask ? launch_variant<1, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileN>(cfg, tm, p, smem);
 }
 
 }  // namespace aur

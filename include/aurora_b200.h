@@ -98,8 +98,8 @@ int aur_device_count(void);
 int aur_open(const aur_config* cfg, aur_index** out);
 int aur_close(aur_index* ix);
 int aur_get_stats(aur_index* ix, aur_stats* out);
-/* Options: "kernel" (aur_kernel), "epi_groups", "tc_tile" (corpus rows per tensor-core tile: 0 = auto, 64 or 128;
- * 128 needs epi_groups 1, and a search it does not fit fails); bring-up only: "dbg_flags", and "dbg_epoch" (1 .. 2^31 - 1), which
+/* Options: "kernel" (aur_kernel), "tc_tile" (corpus rows per tensor-core tile: 0 = auto, 64 or 128;
+ * a search the 128-row layout does not fit fails); bring-up only: "dbg_flags", and "dbg_epoch" (1 .. 2^31 - 1), which
  * sets the tensor-core kernel's launch counter of every search context of the index, e.g. just before it wraps. */
 int aur_set_option(aur_index* ix, const char* key, int64_t value);
 int aur_sync(aur_index* ix);

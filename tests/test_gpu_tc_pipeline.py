@@ -19,11 +19,11 @@ SMEM_OPTIN = 227 * 1024   # sm_90 opt-in shared memory per block
 KSLACK, QROWS, TILE_N, MAX_STAGES = 8, 64, 64, 12   # kSlack, kTcQRows, kTcTileN, kTcMaxStages (csrc/internal.h)
 
 
-def tc_stages(dim: int, ksel: int, epi_groups: int = 1) -> int:
+def tc_stages(dim: int, ksel: int) -> int:
     """tc_pick_stages (csrc/simtopk_tc.cu): the deepest TMA ring make_layout fits into the opt-in shared memory."""
-    fifo = 16 * QROWS * 20 if (epi_groups == 1 and ksel <= 64) else 0
-    rest = ((dim // 64) * QROWS * 128 + epi_groups * QROWS * (TILE_N + 4) * 4 + epi_groups * ksel * QROWS * 8
-            + 2 * epi_groups * 2 * 2 * TILE_N * 4 + fifo + QROWS * 4 + (2 * MAX_STAGES + 5) * 8 + 16 + 1024)
+    fifo = 16 * QROWS * 20 if ksel <= 64 else 0
+    rest = ((dim // 64) * QROWS * 128 + QROWS * (TILE_N + 4) * 4 + ksel * QROWS * 8
+            + 2 * 2 * 2 * TILE_N * 4 + fifo + QROWS * 4 + (2 * MAX_STAGES + 5) * 8 + 16 + 1024)
     for s in range(MAX_STAGES, 1, -1):
         if TILE_N * 128 * s + rest <= SMEM_OPTIN:
             return s
@@ -56,14 +56,12 @@ def _data(n, d, nq, seed):
     return O.round_to_bf16(C), O.round_to_bf16(Q)
 
 
-def _run_both(C, Q, k, epi_groups=0):
+def _run_both(C, Q, k):
     n, d = C.shape
     want = O.cosine_topk(Q, C, k, return_f64=True)
     got = {}
     with Index(d, n) as ix:
         ix.add(C, np.arange(n, dtype=np.int64))
-        if epi_groups:
-            N.check(ix._lib.aur_set_option(ix._h, b"epi_groups", epi_groups))
         for kern in (N.KERNEL_TC1, N.KERNEL_TC2):
             ix.set_kernel(kern)
             got[kern] = dev_search(ix, Q, k)
@@ -99,10 +97,7 @@ def test_two_stage_ring_at_dim_1024(kernel, nq):
     _run_both(C, Q, k)
 
 
-def test_two_epilogue_groups_many_tiles():
-    """epi_groups = 2: the MMA warpgroup alternates the two score buffers tile by tile."""
-    d, nq, k = 768, 128, 16
-    ts = tile_sets(N.KERNEL_TC1, nq, k + KSLACK, _sm_count())
-    n = (ts * 7 + ts // 2) * TILE_N
-    C, Q = _data(n, d, nq, seed=7)
-    _run_both(C, Q, k, epi_groups=2)
+def test_epi_groups_option_is_rejected():
+    """The kernel has one epilogue group: "epi_groups" is not an option."""
+    with Index(64, 64) as ix:
+        assert ix._lib.aur_set_option(ix._h, b"epi_groups", 2) == N.AUR_ERR_INVALID

@@ -12,27 +12,27 @@ QROWS, MAX_STAGES, FIFO_RECS, FIFO_MAX_KSEL = 64, 12, 16, 64   # kTcQRows, kTcMa
 NARROW, WIDE, WIDE_MIN_STAGES = 64, 128, 4                      # kTcTileN, kTcTileWide, kTcWideMinStages
 
 
-def smem_bytes(dim: int, ksel: int, stages: int, tile: int, mask: bool, epi_groups: int = 1) -> int:
+def smem_bytes(dim: int, ksel: int, stages: int, tile: int, mask: bool) -> int:
     """tc_smem_bytes: make_layout's total plus the 1 KB alignment slack."""
     wide = tile == WIDE
-    fifo = ((FIFO_RECS // 2 if wide else FIFO_RECS) if epi_groups == 1 and ksel <= FIFO_MAX_KSEL else 0) * QROWS * 20
-    rows_buf = 2 * epi_groups * 2 * tile * 4                     # inverse norms (and tenant masks): [2G warps][2][tile]
-    return (tile * 128 * stages + (dim // 64) * QROWS * 128 + epi_groups * QROWS * (tile + 4) * 4
-            + epi_groups * ksel * QROWS * 8 + rows_buf + (rows_buf if mask or not wide else 0) + fifo
+    fifo = ((FIFO_RECS // 2 if wide else FIFO_RECS) if ksel <= FIFO_MAX_KSEL else 0) * QROWS * 20
+    rows_buf = 2 * 2 * tile * 4                                  # inverse norms (and tenant masks): [2 warps][2][tile]
+    return (tile * 128 * stages + (dim // 64) * QROWS * 128 + QROWS * (tile + 4) * 4
+            + ksel * QROWS * 8 + rows_buf + (rows_buf if mask or not wide else 0) + fifo
             + QROWS * 4 + (2 * MAX_STAGES + 5) * 8 + 16 + 1024)
 
 
-def stages(dim: int, ksel: int, tile: int, mask: bool = False, epi_groups: int = 1) -> int:
+def stages(dim: int, ksel: int, tile: int, mask: bool = False) -> int:
     """tc_pick_stages: the deepest ring that fits, 0 when not even two stages do."""
     for s in range(MAX_STAGES, 1, -1):
-        if smem_bytes(dim, ksel, s, tile, mask, epi_groups) <= SMEM_OPTIN:
+        if smem_bytes(dim, ksel, s, tile, mask) <= SMEM_OPTIN:
             return s
     return 0
 
 
-def auto_tile(dim: int, ksel: int, mask: bool = False, epi_groups: int = 1) -> int:
+def auto_tile(dim: int, ksel: int, mask: bool = False) -> int:
     """tc_auto_tile for a search (the bring-up score dump always takes 64-row tiles)."""
-    return WIDE if epi_groups == 1 and stages(dim, ksel, WIDE, mask) >= WIDE_MIN_STAGES else NARROW
+    return WIDE if stages(dim, ksel, WIDE, mask) >= WIDE_MIN_STAGES else NARROW
 
 
 def largest_wide_k(dim: int, mask: bool = False) -> int:
@@ -65,4 +65,3 @@ def test_wide_layout_is_never_picked_where_it_does_not_fit():
                 if auto_tile(dim, k + 8, mask) == WIDE:
                     assert smem_bytes(dim, k + 8, WIDE_MIN_STAGES, WIDE, mask) <= SMEM_OPTIN
     assert largest_wide_k(768) == 33
-    assert auto_tile(768, 40, epi_groups=2) == NARROW

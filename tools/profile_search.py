@@ -37,8 +37,6 @@ def main():
         flags = int(os.environ.get("AUR_DBG_FLAGS", "0"))
         if flags:
             N.check(ix._lib.aur_set_option(ix._h, b"dbg_flags", flags))
-        if os.environ.get("AUR_EPI_GROUPS"):
-            N.check(ix._lib.aur_set_option(ix._h, b"epi_groups", int(os.environ["AUR_EPI_GROUPS"])))
         dq = DeviceBuffer(q.nbytes).upload(q)
         ds = DeviceBuffer(nq * k * 4)
         di = DeviceBuffer(nq * k * 8)

@@ -5,7 +5,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from aurora_b200 import _native as N
 from aurora_b200.engine import DeviceBuffer, Index, to_bf16_bits
-Q = N.TC_QUERY_ROWS                  # queries per CTA = epilogue threads per group
+Q = N.TC_QUERY_ROWS                  # queries per CTA = epilogue threads
 MAX_CTAS = 1024                      # buffer sized for more CTAs than any GPU has SMs; the call returns the real count
 n, d, nq = int(sys.argv[1]) if len(sys.argv) > 1 else 1_000_000, 768, 2 * Q   # one query block per CTA of a pair
 rng = np.random.default_rng(1002)
@@ -16,26 +16,21 @@ with Index(d, n) as ix:
         m = min(50_000, n - lo)
         ix.add(np.roll(block[:m], lo // 50_000, axis=1), np.arange(lo, lo + m, dtype=np.int64))
     N.check(ix._lib.aur_set_option(ix._h, b"dbg_flags", 64 | int(os.environ.get("AUR_DBG_FLAGS", "0"))))
-    g = 1
-    if os.environ.get("AUR_EPI_GROUPS"):
-        N.check(ix._lib.aur_set_option(ix._h, b"epi_groups", int(os.environ["AUR_EPI_GROUPS"])))
     dq = DeviceBuffer(q.nbytes).upload(q)
     dout = DeviceBuffer(MAX_CTAS * Q * 64 * 4)
     for _ in range(3):
         n_ctas = ix.debug_tc_scores(dq.ptr, nq, 2, dout.ptr)
     out = dout.download(np.empty((MAX_CTAS, Q, 64), dtype=np.float32))[:n_ctas]
 tiles = -(-(-(-n // 64)) // (n_ctas // 2))       # corpus tiles per CTA pair (one tile set per pair)
-for grp in range(g):
-    npush, nslow, tg, tl = (out[:, :, grp * 4 + i] for i in range(4))
-    print(f"group {grp}: final list entries/thread mean {npush.mean():.1f} max {npush.max():.0f} p50 {np.median(npush):.0f}; "
-          f"slow-chunk entries/thread mean {nslow.mean():.1f} max {nslow.max():.0f} (of {4 * tiles // g} chunks); "
-          f"tau_glob mean {tg.mean():.3f} tau_local mean {tl.mean():.3f}")
+npush, nslow, tg, tl = (out[:, :, i] for i in range(4))
+print(f"final list entries/thread mean {npush.mean():.1f} max {npush.max():.0f} p50 {np.median(npush):.0f}; "
+      f"slow-chunk entries/thread mean {nslow.mean():.1f} max {nslow.max():.0f} (of {4 * tiles} chunks); "
+      f"tau_glob mean {tg.mean():.3f} tau_local mean {tl.mean():.3f}")
 
-for grp in range(g):
-    tw, ts, tx, tl, tt = (out[:, :, 8 + grp * 8 + i] for i in range(5))
-    print(f"group {grp} cycles/thread: total {tt.mean():.0f} wait_full {tw.mean():.0f} ({100*tw.mean()/tt.mean():.0f}%) "
-          f"slow {ts.mean():.0f} ({100*ts.mean()/tt.mean():.0f}%) xchg {tx.mean():.0f} ({100*tx.mean()/tt.mean():.0f}%) "
-          f"ld_scores {tl.mean():.0f} ({100*tl.mean()/tt.mean():.0f}%)  slow max {ts.max():.0f}")
+tw, ts, tx, tl, tt = (out[:, :, 8 + i] for i in range(5))
+print(f"cycles/thread: total {tt.mean():.0f} wait_full {tw.mean():.0f} ({100*tw.mean()/tt.mean():.0f}%) "
+      f"slow {ts.mean():.0f} ({100*ts.mean()/tt.mean():.0f}%) xchg {tx.mean():.0f} ({100*tx.mean()/tt.mean():.0f}%) "
+      f"ld_scores {tl.mean():.0f} ({100*tl.mean()/tt.mean():.0f}%)  slow max {ts.max():.0f}")
 mm = out[:, 0, 32:35]
 print(f"MMA warpgroup cycles: total {mm[:,2].mean():.0f} wait_score_buffer {mm[:,0].mean():.0f} ({100*mm[:,0].mean()/mm[:,2].mean():.0f}%) "
       f"wait_smem_full {mm[:,1].mean():.0f} ({100*mm[:,1].mean()/mm[:,2].mean():.0f}%)")
