@@ -9,7 +9,9 @@ b = 0.75, "word" tokenisation (lower-case, split on non-alphanumerics), idf = ln
 (n + 0.5)); rankedFusion with the constant 60 and 0-based ranks.  Unpinned: the reference has no test
 at this boundary (SURVEY.md section 8c).  ``BM25Index`` is the host index (the path of the test doubles and
 the definition the device is held to); ``DeviceBM25`` keeps the vocabulary and tokenisation on the host and the
-postings, scoring and top-k in the GPU keyword store (csrc/keyword.cu, DESIGN.md section 10).
+postings, scoring and top-k in the GPU keyword store (csrc/keyword.cu, DESIGN.md section 10).  ``ranked_fusion`` and
+``relative_score_fusion`` (Weaviate's other fusion, HybridFusion.RELATIVE_SCORE) define the fused score; the device
+fusion of ``DeviceBM25.search_batch(..., dense=...)`` (csrc/hybrid.cu, DESIGN.md section 11) equals them bit for bit.
 """
 
 from __future__ import annotations
@@ -250,14 +252,35 @@ class DeviceBM25:
             allow_ids = [d for d in base if allow(d)]
         return self._run([query], limit, None, None, allow_ids)[0]
 
-    def search_batch(self, queries: List[str], limit: int, q_user=None, q_org=None) -> List[List[Tuple[int, float]]]:
+    def search_batch(self, queries: List[str], limit: int, q_user=None, q_org=None, dense=None) -> List[list]:
         """All queries in one device search; ``q_user`` / ``q_org``: per-query tenant codes (row_user == u or, for
-        org >= 0, row_org == o), None = unscoped."""
+        org >= 0, row_org == o), None = unscoped.
+
+        ``dense = (index, vectors, w_dense, fusion, k_out)``: the whole hybrid query in one device call
+        (``engine.hybrid_search``): the keyword leg's top-``limit`` stays in HBM and is fused there with the dense leg's
+        top-``limit`` of ``vectors`` over the ``engine.Index`` ``index`` (same scopes), weights ``w_dense`` (per query)
+        and ``1 - w_dense``, ``fusion`` an ``AUR_FUSION_*`` value.  Each query's list then holds its best ``k_out``
+        pairs ``(id, (fused score, dense cosine or None))``."""
         if not queries:
             return []
+        if dense is not None:
+            return self._run_hybrid(queries, limit, q_user, q_org, *dense)
         if limit <= 0 or not self._docs:
             return [[] for _ in queries]
         return self._run(queries, limit, q_user, q_org, None)
+
+    def _run_hybrid(self, queries, fetch, q_user, q_org, index, vectors, w_dense, fusion, k_out):
+        from .engine import hybrid_search
+
+        q_terms, q_off = query_csr(self.vocab, queries)
+        ids, scores, cosine, _ = hybrid_search(index, self.store, vectors, fetch, q_terms, q_off, w_dense, None, fusion,
+                                               k_out, q_user, q_org)
+        out = []
+        for row_i, row_s, row_c in zip(ids, scores, cosine):
+            n = int((row_i >= 0).sum())
+            out.append([(int(d), (float(s), None if c != c else float(c)))
+                        for d, s, c in zip(row_i[:n].tolist(), row_s[:n].tolist(), row_c[:n].tolist())])
+        return out
 
     def _run(self, queries, limit, q_user, q_org, allow_ids):
         q_terms, q_off = query_csr(self.vocab, queries)
@@ -278,4 +301,21 @@ def ranked_fusion(legs: Iterable[Tuple[float, List[int]]], limit: int) -> List[T
             continue
         for rank, doc in enumerate(ids):
             fused[doc] += weight / (rank + RANK_CONSTANT)
+    return sorted(fused.items(), key=lambda kv: (-kv[1], kv[0]))[:limit]
+
+
+def relative_score_fusion(legs: Iterable[Tuple[float, List[Tuple[int, float]]]], limit: int) -> List[Tuple[int, float]]:
+    """Weaviate relativeScoreFusion: ``legs`` = (weight, [(id, score)] best-first); each leg's scores are min-max
+    normalised over its own list, score(id) = sum over legs of weight * (s - lo) / (hi - lo) (weight when hi == lo),
+    summed in leg order from 0.0 in fp64.  A leg with weight <= 0 or no entries takes no part.  Returns the top ``limit``
+    (id, fused score), ties by id.  The hi == lo rule, the fp64 arithmetic and the id tie-break are this project's
+    reading of Weaviate's documentation (parity unpinned, DESIGN.md section 11)."""
+    fused: Dict[int, float] = defaultdict(float)
+    for weight, entries in legs:
+        if weight <= 0.0 or not entries:
+            continue
+        scores = [s for _, s in entries]
+        lo, hi = min(scores), max(scores)
+        for doc, s in entries:
+            fused[doc] += weight if hi == lo else weight * ((s - lo) / (hi - lo))
     return sorted(fused.items(), key=lambda kv: (-kv[1], kv[0]))[:limit]

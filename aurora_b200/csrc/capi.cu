@@ -608,6 +608,44 @@ int check_batch(int32_t nq, int32_t k) {
   return AUR_OK;
 }
 
+// Per-query tenant codes (host) of a search into c's staging on stream s, and how the search applies them: the reference
+// asks one tenant's question at a time (weaviate_client.py:244-249), so when every query of the batch carries the same
+// (user, org) scope the filter folds into the row scale and the tensor-core kernel serves it (sc->uniform = scope, which
+// must outlive the search's enqueue); a coalesced batch of several tenants' questions with at most 32 distinct scopes
+// gives every corpus row a bit mask (one pre-pass) on the same kernel; more scopes -> the generic kernel.
+int stage_tenant_scope(SearchCtx* c, cudaStream_t s, int32_t nq, const int32_t* q_user, const int32_t* q_org, int32_t* scope,
+                       Scope* sc) {
+  CU_TRY(c->stage_quser.reserve(nq));
+  CU_TRY(cudaMemcpyAsync(c->stage_quser.p, q_user, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
+  sc->q_user = c->stage_quser.p;
+  if (q_org) {
+    CU_TRY(c->stage_qorg.reserve(nq));
+    CU_TRY(cudaMemcpyAsync(c->stage_qorg.p, q_org, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
+    sc->q_org = c->stage_qorg.p;
+  }
+  bool uniform = true;
+  scope[0] = q_user[0]; scope[1] = q_org ? q_org[0] : -1;
+  for (int i = 1; i < nq && uniform; ++i) uniform = q_user[i] == scope[0] && (q_org ? q_org[i] : -1) == scope[1];
+  if (uniform) { sc->uniform = scope; return AUR_OK; }
+  std::vector<int32_t> tab; std::vector<int32_t> qs(static_cast<size_t>(nq));
+  for (int i = 0; i < nq; ++i) {
+    const int32_t u = q_user[i], o = q_org ? q_org[i] : -1;
+    int found = -1;
+    for (size_t t = 0; t < tab.size() / 2; ++t) if (tab[2 * t] == u && tab[2 * t + 1] == o) { found = static_cast<int>(t); break; }
+    if (found < 0) {
+      if (tab.size() / 2 == 32) return AUR_OK;
+      found = static_cast<int>(tab.size() / 2); tab.push_back(u); tab.push_back(o);
+    }
+    qs[static_cast<size_t>(i)] = found;
+  }
+  CU_TRY(c->scope_tab.reserve(64)); CU_TRY(c->q_scope.reserve(static_cast<size_t>(nq)));
+  CU_TRY(cudaMemcpyAsync(c->scope_tab.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, s));
+  CU_TRY(cudaMemcpyAsync(c->q_scope.p, qs.data(), static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
+  CU_TRY(cudaStreamSynchronize(s));          // tab / qs are host temporaries
+  sc->scope_tab = c->scope_tab.p; sc->q_scope = c->q_scope.p; sc->n_scopes = static_cast<int>(tab.size() / 2);
+  return AUR_OK;
+}
+
 // Host-buffer search: H2D of the queries, kernels, D2H of the results on a pool context's own stream.
 int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user, const int32_t* q_org,
                 const int64_t* allow_ids, int64_t n_allow, float* scores_out, int64_t* ids_out, int64_t* snapshot_out) {
@@ -634,44 +672,8 @@ int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, 
       CU_TRY(cudaMemcpyAsync(c->allow_rows.p, rows_host.data(), rows_host.size() * 4, cudaMemcpyHostToDevice, s));
     sc.allow_rows = c->allow_rows.p;
     sc.n_allow = static_cast<int64_t>(rows_host.size());
-  } else if (q_user) {
-    CU_TRY(c->stage_quser.reserve(nq));
-    CU_TRY(cudaMemcpyAsync(c->stage_quser.p, q_user, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
-    sc.q_user = c->stage_quser.p;
-    if (q_org) {
-      CU_TRY(c->stage_qorg.reserve(nq));
-      CU_TRY(cudaMemcpyAsync(c->stage_qorg.p, q_org, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
-      sc.q_org = c->stage_qorg.p;
-    }
-    // the reference asks one tenant's question at a time (weaviate_client.py:244-249): when every query of the
-    // batch carries the same (user, org) scope the filter folds into the row scale and the tensor-core kernel serves it
-    bool uniform = true;
-    scope[0] = q_user[0]; scope[1] = q_org ? q_org[0] : -1;
-    for (int i = 1; i < nq && uniform; ++i) uniform = q_user[i] == scope[0] && (q_org ? q_org[i] : -1) == scope[1];
-    if (uniform) sc.uniform = scope;
-    else {
-      // a coalesced batch of several tenants' questions: with at most 32 distinct scopes every corpus row gets a bit
-      // mask (one pre-pass) and the tensor-core kernel serves the batch; more scopes -> the generic kernel
-      std::vector<int32_t> tab; std::vector<int32_t> qs(static_cast<size_t>(nq));
-      bool fits = true;
-      for (int i = 0; i < nq && fits; ++i) {
-        const int32_t u = q_user[i], o = q_org ? q_org[i] : -1;
-        int found = -1;
-        for (size_t t = 0; t < tab.size() / 2; ++t) if (tab[2 * t] == u && tab[2 * t + 1] == o) { found = static_cast<int>(t); break; }
-        if (found < 0) {
-          if (tab.size() / 2 == 32) { fits = false; break; }
-          found = static_cast<int>(tab.size() / 2); tab.push_back(u); tab.push_back(o);
-        }
-        qs[static_cast<size_t>(i)] = found;
-      }
-      if (fits) {
-        CU_TRY(c->scope_tab.reserve(64)); CU_TRY(c->q_scope.reserve(static_cast<size_t>(nq)));
-        CU_TRY(cudaMemcpyAsync(c->scope_tab.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, s));
-        CU_TRY(cudaMemcpyAsync(c->q_scope.p, qs.data(), static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
-        CU_TRY(cudaStreamSynchronize(s));          // tab / qs are host temporaries
-        sc.scope_tab = c->scope_tab.p; sc.q_scope = c->q_scope.p; sc.n_scopes = static_cast<int>(tab.size() / 2);
-      }
-    }
+  } else if (q_user && (rc = stage_tenant_scope(c, s, nq, q_user, q_org, scope, &sc)) != AUR_OK) {
+    return rc;
   }
   rc = stats_begin(c, s, nq, n_rows);
   if (rc == AUR_OK) rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, call.d_scores, call.d_ids, nullptr, s);
@@ -910,6 +912,33 @@ int filter_write(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t n_programs
 }
 
 }  // namespace
+
+namespace aur {
+int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
+              const int32_t* q_org, float* scores, int64_t* ids, int64_t* snapshot_rows) {
+  if (ix->dtype != AUR_BF16) return fail(AUR_ERR_UNSUPPORTED, "hybrid search needs a bf16 index");
+  if (ix->device != device) return fail(AUR_ERR_INVALID, "the keyword store is on device %d, the index on device %d", device, ix->device);
+  int rc = check_batch(nq, k);
+  if (rc != AUR_OK) return rc;
+  std::shared_lock<std::shared_mutex> rl(ix->rw);   // (compaction waits for the device before it moves a row)
+  CU_TRY(cudaSetDevice(ix->device));
+  SearchCtx* c = nullptr;
+  if ((rc = acquire_ctx(ix, s, &c)) != AUR_OK) return rc;
+  std::lock_guard<std::mutex> cl(c->mu);
+  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
+  const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->elt;
+  CU_TRY(c->stage_q.reserve(qbytes));
+  CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
+  Scope sc;
+  int32_t scope[2] = {0, -1};
+  if (q_user && (rc = stage_tenant_scope(c, s, nq, q_user, q_org, scope, &sc)) != AUR_OK) return rc;
+  if ((rc = stats_begin(c, s, nq, n_rows)) != AUR_OK) return rc;
+  if ((rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, scores, ids, nullptr, s)) != AUR_OK) return rc;
+  if ((rc = stats_end(ix, c, s)) != AUR_OK) return rc;
+  *snapshot_rows = n_rows;
+  return AUR_OK;
+}
+}  // namespace aur
 
 extern "C" {
 

@@ -5,6 +5,11 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <functional>
+
+struct aur_index;
+struct aur_kw;
+
 namespace aur {
 
 // ---------------------------------------------------------------- candidate keys
@@ -297,6 +302,21 @@ struct DevBuf {   // grow-only device scratch
   }
   void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
 };
+
+// ---------------------------------------------------------------- the two legs of a hybrid query (hybrid.cu)
+// Dense leg: the search aur_search_ex runs for these host queries and per-query tenant codes (same scope handling, same
+// kernels, same answer), enqueued on stream s of `device` over the prefix published now, into the device arrays
+// scores / ids [nq * k].  Nothing waits; *snapshot_rows receives the prefix.  A bf16 index on `device` only
+// (else AUR_ERR_UNSUPPORTED / AUR_ERR_INVALID).  The leg's aur_stats.last_* are the index's last search.  (capi.cu)
+int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
+              const int32_t* q_org, float* scores, int64_t* ids, int64_t* snapshot_rows);
+// Keyword leg: aur_kw_search's search (no allow-list) enqueued on the store's own context and stream, then
+// then(device, stream, scores, ids, snapshot_rows) runs with the leg's results -- device arrays [nq * k], valid once the
+// stream reaches them -- while the store's shared lock and the context are held.  The leg's aur_kw_stats.last_* are
+// published after then() returns AUR_OK.  (keyword.cu)
+using KwLegThen = std::function<int(int device, cudaStream_t s, const double* scores, const int64_t* ids, int64_t snapshot_rows)>;
+int kw_leg(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k, const int32_t* q_user,
+           const int32_t* q_org, const KwLegThen& then);
 
 // Error reporting shared by the translation units behind the C ABI (thread-local message).
 int report_error(int code, const char* fmt, ...);

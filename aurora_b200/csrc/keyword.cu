@@ -389,8 +389,8 @@ struct KwQuery {   // the arguments of one search (aur_kw_search)
   const int32_t* user; const int32_t* org; const int64_t* allow; int64_t n_allow;
 };
 
-int kw_check_query(const KwQuery& q, const double* scores_out, const int64_t* ids_out) {
-  if (!q.off || !scores_out || !ids_out) return report_error(AUR_ERR_INVALID, "null argument");
+int kw_check_query(const KwQuery& q) {
+  if (!q.off) return report_error(AUR_ERR_INVALID, "null argument");
   if (q.nq <= 0 || q.k <= 0) return report_error(AUR_ERR_INVALID, "nq and k must be positive");
   if (q.k > kMaxK) return report_error(AUR_ERR_UNSUPPORTED, "k > %d", kMaxK);
   if (q.off[0] != 0) return report_error(AUR_ERR_INVALID, "q_offsets[0] must be 0");
@@ -583,6 +583,16 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
   return AUR_OK;
 }
 
+// Publish the last_* statistics of a search whose part on c's stream has completed.
+int kw_publish(aur_kw* kw, KwCtx* c) {
+  float ms = 0.f;
+  KW_TRY(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+  std::lock_guard<std::mutex> lk(kw->mu_pool);
+  kw->last_launches = c->launches; kw->last_ms = ms;
+  kw->last_terms = c->terms; kw->last_spilled = c->spilled;
+  return AUR_OK;
+}
+
 // Wait for one store's part, copy its [nq][k] lists to the host and publish its last_* statistics.
 int kw_collect(aur_kw* kw, KwCtx* c, const KwQuery& q, double* scores_out, int64_t* ids_out) {
   KW_TRY(cudaSetDevice(kw->device));
@@ -591,12 +601,33 @@ int kw_collect(aur_kw* kw, KwCtx* c, const KwQuery& q, double* scores_out, int64
   KW_TRY(cudaMemcpyAsync(scores_out, c->out_s.p, nout * 8, cudaMemcpyDeviceToHost, s));
   KW_TRY(cudaMemcpyAsync(ids_out, c->out_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
   KW_TRY(cudaStreamSynchronize(s));
-  float ms = 0.f;
-  KW_TRY(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-  std::lock_guard<std::mutex> lk(kw->mu_pool);
-  kw->last_launches = c->launches; kw->last_ms = ms;
-  kw->last_terms = c->terms; kw->last_spilled = c->spilled;
-  return AUR_OK;
+  return kw_publish(kw, c);
+}
+
+// Each store's snapshot and the launch tables of a search over stores[0 .. n) taken as one corpus: the batch's distinct
+// terms, idf and avgdl from the summed statistics.  Caller holds every store's shared lock.
+struct KwPlan {
+  std::vector<KwSnap> snaps;
+  std::vector<KwBlock> blocks;
+  int64_t N = 0;
+  double avgdl = 1.0;
+};
+void kw_prepare(aur_kw* const* stores, int n, const KwQuery& q, KwPlan* pl) {
+  std::vector<int32_t> uniq(q.terms, q.terms + q.off[q.nq]);
+  std::sort(uniq.begin(), uniq.end());
+  uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
+  pl->snaps.assign(static_cast<size_t>(n), KwSnap());
+  std::vector<int64_t> udf(uniq.size(), 0);
+  int64_t N = 0, total_len = 0;
+  for (int s = 0; s < n; ++s) {
+    kw_snapshot(stores[s], uniq, &pl->snaps[static_cast<size_t>(s)]);
+    const KwSnap& sn = pl->snaps[static_cast<size_t>(s)];
+    N += sn.N; total_len += sn.total_len;
+    for (size_t i = 0; i < uniq.size(); ++i) udf[i] += sn.udf[i];
+  }
+  pl->N = N;
+  pl->avgdl = total_len ? static_cast<double>(total_len) / static_cast<double>(N) : 1.0;
+  kw_plan(q, uniq, udf, N, &pl->blocks);
 }
 
 // Search stores[0 .. n) (distinct, arguments checked) as one corpus: store s's top-k lists land in
@@ -609,22 +640,9 @@ int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out
   std::vector<std::shared_lock<std::shared_mutex>> locks;
   locks.reserve(static_cast<size_t>(n));
   for (aur_kw* kw : order) locks.emplace_back(kw->rw);
-  // the batch's distinct terms, each store's snapshot, the corpus totals
-  std::vector<int32_t> uniq(q.terms, q.terms + q.off[q.nq]);
-  std::sort(uniq.begin(), uniq.end());
-  uniq.erase(std::unique(uniq.begin(), uniq.end()), uniq.end());
-  std::vector<KwSnap> snaps(static_cast<size_t>(n));
-  std::vector<int64_t> udf(uniq.size(), 0);
-  int64_t N = 0, total_len = 0;
-  for (int s = 0; s < n; ++s) {
-    kw_snapshot(stores[s], uniq, &snaps[static_cast<size_t>(s)]);
-    const KwSnap& sn = snaps[static_cast<size_t>(s)];
-    N += sn.N; total_len += sn.total_len;
-    for (size_t i = 0; i < uniq.size(); ++i) udf[i] += sn.udf[i];
-  }
-  const double avgdl = total_len ? static_cast<double>(total_len) / static_cast<double>(N) : 1.0;
-  std::vector<KwBlock> blocks;
-  kw_plan(q, uniq, udf, N, &blocks);
+  KwPlan pl;
+  kw_prepare(stores, n, q, &pl);
+  const std::vector<KwSnap>& snaps = pl.snaps;
   // every store's work enqueued before any is waited on; the contexts go back to their pools only once their streams
   // are idle (also on an error), before the locks are released
   struct Ctxs {
@@ -641,7 +659,7 @@ int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out
     if (rc != AUR_OK) return rc;
     ctxs.v.emplace_back(kw, c);
     const KwSnap& sn = snaps[static_cast<size_t>(s)];
-    if ((rc = kw_launch(kw, c, q, blocks, sn.n_rows, N, avgdl)) != AUR_OK) return rc;
+    if ((rc = kw_launch(kw, c, q, pl.blocks, sn.n_rows, pl.N, pl.avgdl)) != AUR_OK) return rc;
   }
   const size_t nout = static_cast<size_t>(q.nq) * q.k;
   for (int s = 0; s < n; ++s) {
@@ -654,6 +672,32 @@ int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out
 }
 
 }  // namespace
+
+namespace aur {
+int kw_leg(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k, const int32_t* q_user,
+           const int32_t* q_org, const KwLegThen& then) {
+  if (!kw) return report_error(AUR_ERR_INVALID, "null store");
+  const KwQuery q{q_terms, q_offsets, nq, k, q_user, q_org, nullptr, 0};
+  int rc = kw_check_query(q);
+  if (rc != AUR_OK) return rc;
+  std::shared_lock<std::shared_mutex> rl(kw->rw);   // held until the leg's kernels have finished (then() waits for them)
+  KwPlan pl;
+  kw_prepare(&kw, 1, q, &pl);
+  KW_TRY(cudaSetDevice(kw->device));
+  KwCtx* c = nullptr;
+  if ((rc = kw_ctx_acquire(kw, &c)) != AUR_OK) return rc;
+  struct Back {   // the context goes back to the pool once its stream is idle, also on an error
+    aur_kw* kw; KwCtx* c;
+    ~Back() { cudaSetDevice(kw->device); cudaStreamSynchronize(c->stream); kw_ctx_release(kw, c); }
+  } back{kw, c};
+  const int64_t n_rows = pl.snaps[0].n_rows;
+  if ((rc = kw_launch(kw, c, q, pl.blocks, n_rows, pl.N, pl.avgdl)) != AUR_OK) return rc;
+  if ((rc = then(kw->device, c->stream, c->out_s.p, c->out_ids.p, n_rows)) != AUR_OK) return rc;
+  KW_TRY(cudaSetDevice(kw->device));
+  KW_TRY(cudaStreamSynchronize(c->stream));
+  return kw_publish(kw, c);
+}
+}  // namespace aur
 
 extern "C" {
 
@@ -905,9 +949,9 @@ int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out) {
 int aur_kw_search(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k, const int32_t* q_user,
                   const int32_t* q_org, const int64_t* allow_ids, int64_t n_allow, double* scores_out, int64_t* ids_out,
                   int64_t* snapshot_rows_out) {
-  if (!kw) return report_error(AUR_ERR_INVALID, "null argument");
+  if (!kw || !scores_out || !ids_out) return report_error(AUR_ERR_INVALID, "null argument");
   const KwQuery q{q_terms, q_offsets, nq, k, q_user, q_org, allow_ids, n_allow};
-  const int rc = kw_check_query(q, scores_out, ids_out);
+  const int rc = kw_check_query(q);
   if (rc != AUR_OK) return rc;
   return kw_search_stores(&kw, 1, q, scores_out, ids_out, snapshot_rows_out);
 }
@@ -924,8 +968,9 @@ int aur_kw_search_multi(aur_kw* const* stores, int32_t n_stores, const int32_t* 
     if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
       return report_error(AUR_ERR_INVALID, "a store is listed twice (its statistics would count double)");
   }
+  if (!scores_out || !ids_out) return report_error(AUR_ERR_INVALID, "null argument");
   const KwQuery q{q_terms, q_offsets, nq, k, q_user, q_org, allow_ids, n_allow};
-  int rc = kw_check_query(q, scores_out, ids_out);
+  int rc = kw_check_query(q);
   if (rc != AUR_OK) return rc;
   if (n_stores == 1) return kw_search_stores(stores, 1, q, scores_out, ids_out, snapshot_rows_out);
   const size_t nout = static_cast<size_t>(nq) * k;

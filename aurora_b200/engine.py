@@ -479,6 +479,33 @@ class KeywordIndex:
         return a["ids"], a["scores"], int(snap.value)
 
 
+def hybrid_search(index: Index, kw_index: KeywordIndex, queries: np.ndarray, fetch: int, q_terms, q_offsets,
+                  w_dense, w_sparse=None, fusion: int = N.FUSION_RANKED, k_out: Optional[int] = None, q_user=None,
+                  q_org=None):
+    """Both legs of the hybrid query and their fusion in one device call (aur_hybrid_search): the dense leg's top-``fetch``
+    of ``queries`` over ``index`` and the keyword leg's top-``fetch`` of ``q_terms`` / ``q_offsets`` over ``kw_index``
+    (same tenant scope), fused per query with weights ``w_dense`` / ``w_sparse`` (default ``1 - w_dense``).  Returns
+    (ids [nq, k_out] int64, fused scores [nq, k_out] float64, dense cosines [nq, k_out] float32 (NaN: not in the dense
+    list), (dense snapshot rows, keyword snapshot rows)); padding (-1, -inf, NaN)."""
+    q = index._rows_buffer(queries)
+    nq = q.shape[0]
+    k_out = 2 * int(fetch) if k_out is None else int(k_out)
+    wd = np.ascontiguousarray(np.broadcast_to(np.asarray(w_dense, dtype=np.float64), (nq,)))
+    ws = 1.0 - wd if w_sparse is None else np.ascontiguousarray(np.broadcast_to(np.asarray(w_sparse, dtype=np.float64), (nq,)))
+    a = _kw_query_args(q_terms, q_offsets, 1, q_user, q_org, None)
+    qt, q_off, u, o, _ = a["keep"]
+    if q_off.shape[0] - 1 != nq:
+        raise ValueError(f"{nq} query vectors but {q_off.shape[0] - 1} keyword queries")
+    scores = np.empty((nq, k_out), dtype=np.float64)
+    ids = np.empty((nq, k_out), dtype=np.int64)
+    cosine = np.empty((nq, k_out), dtype=np.float32)
+    snaps = (C.c_int64 * 2)(-1, -1)
+    N.check(index._lib.aur_hybrid_search(index._h, kw_index._h, _ptr(q), nq, int(fetch), _ptr(qt), _ptr(q_off), _ptr(u),
+                                         _ptr(o), _ptr(wd), _ptr(ws), int(fusion), k_out, _ptr(scores), _ptr(ids),
+                                         _ptr(cosine), snaps))
+    return ids, scores, cosine, (int(snaps[0]), int(snaps[1]))
+
+
 def _kw_query_args(q_terms, q_offsets, k, q_user, q_org, allow_ids):
     """The query-side arguments of aur_kw_search / aur_kw_search_multi and the output arrays they fill (kept alive in
     the returned dict for the duration of the call)."""

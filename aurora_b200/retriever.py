@@ -34,7 +34,7 @@ from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import numpy as np
 
-from ._native import AUR_BF16
+from ._native import AUR_BF16, FUSION_RANKED, FUSION_RELATIVE_SCORE
 from .bm25 import BM25Index
 from .filters import AttrColumn, Filter, HybridFusion, compile_program  # noqa: F401  (Filter, HybridFusion: re-exported)
 
@@ -47,6 +47,8 @@ _MAX_FETCH = 128                        # engine's largest k
 # (DESIGN.md section 9, tools/list_bench.py): the list path wins at 3 000 rows (0.3 %), the full scan at 10 000 (1 %).
 _LIST_MAX_FRACTION = 0.005
 _ATTR_COLS = range(2, 18)               # the shard's attribute columns (include/aurora_b200.h, aur_set_attrs)
+# hybrid fusions the knowledge base implements, as aur_hybrid_search's AUR_FUSION_* values
+_FUSION = {HybridFusion.RANKED: FUSION_RANKED, HybridFusion.RELATIVE_SCORE: FUSION_RELATIVE_SCORE}
 
 
 def _sanitize(value: Any) -> str:
@@ -83,6 +85,7 @@ class KnowledgeBase:
         # keyword leg of the hybrid query: on the GPU beside a CUDA vector index, else the host index
         self.sparse = self._keyword_store(int(capacity))
         self._kw_device = not isinstance(self.sparse, BM25Index)
+        self._hybrid_device = self._fuses_on_device()
         self._lock = threading.RLock()  # the reference's module globals are unlocked (weaviate_client.py:31-32)
         self._props: Dict[int, Dict[str, Any]] = {}   # id -> properties
         self._key2id: Dict[str, int] = {}             # uuid5 -> id
@@ -118,6 +121,18 @@ class KnowledgeBase:
         if isinstance(ix, MultiIndex) and ix.shards and all(isinstance(sh, Index) for sh in ix.shards):
             return DeviceBM25(store=MultiKeywordIndex(capacity, devices=[sh.device for sh in ix.shards]))
         return BM25Index()
+
+    def _fuses_on_device(self) -> bool:
+        """Whether an unfiltered hybrid query runs as one device call, both legs and their fusion
+        (``engine.hybrid_search``): a bf16 ``engine.Index`` and a ``DeviceBM25`` over a ``KeywordIndex`` on its GPU.
+        ``MultiIndex``, f32 shards and the CPU doubles fuse on the host (``bm25.ranked_fusion`` /
+        ``relative_score_fusion``), as do filtered queries."""
+        from .bm25 import DeviceBM25
+        from .engine import Index, KeywordIndex
+
+        ix, sp = self.index, self.sparse
+        return (isinstance(ix, Index) and ix.dtype == AUR_BF16 and isinstance(sp, DeviceBM25)
+                and isinstance(sp.store, KeywordIndex) and sp.store.device == ix.device)
 
     def _scope_codes(self, user_id: Optional[str], org_id: Optional[str]) -> Tuple[int, int]:
         """Tenant scope as the kernels take it: (user code, org code); -2 matches no row, org -1 = no org."""
@@ -339,18 +354,26 @@ class KnowledgeBase:
     # ------------------------------------------------------------------ search
     def query(self, query: str, limit: int, filters=None, user_id: Optional[str] = None,
               org_id: Optional[str] = None, alpha: Optional[float] = None, scoped: bool = False,
+              fusion: str = HybridFusion.RANKED,
               _dense: Optional[List[Tuple[int, float]]] = None,
-              _sparse: Optional[List[Tuple[int, float]]] = None) -> List[SimpleNamespace]:
+              _sparse: Optional[List[Tuple[int, float]]] = None,
+              _fused: Optional[list] = None) -> List[SimpleNamespace]:
         """Top-``limit`` objects.  ``alpha`` None or >= 1: pure vector search, ``score`` = cosine
-        (near_text, incident_feedback/weaviate_client.py:286-297).  ``alpha`` < 1: hybrid with ranked
-        fusion (weaviate_client.py:252-259): dense and BM25 lists fused as alpha/(rank+60) +
-        (1-alpha)/(rank+60), ``score`` = the fused score.
+        (near_text, incident_feedback/weaviate_client.py:286-297).  ``alpha`` < 1: hybrid
+        (weaviate_client.py:252-259), ``score`` = the fused score of the dense and BM25 lists with weights
+        alpha and 1 - alpha: ``fusion`` = ``HybridFusion.RANKED`` (weight / (rank + 60) per list) or
+        ``HybridFusion.RELATIVE_SCORE`` (weight times the score min-max normalised over its list).
 
         Filters are PRE-filters, as in Weaviate: the tenant scope (user OR org) runs inside the kernel;
         a ``filters`` expression on a CUDA shard is compiled to a program over the shard's attribute
         columns and evaluated there (``Index.search_filtered``); elsewhere it is resolved against the
         metadata table to the set of allowed ids.  Either way the kernel searches only the matching rows,
         so a small tenant's chunks are found even when the global top-k belongs to other tenants.
+
+        An unfiltered hybrid query on a CUDA shard is one device call (``DeviceBM25.search_batch`` with ``dense``):
+        both legs and their fusion run on the GPU and only the fused top-``limit`` comes back.  Objects deleted after
+        that call drop out of the answer; the others keep the scores the device computed (the answer as of the
+        search).  Elsewhere the two lists come back and are fused on the host.
 
         ``scoped``: the caller is a tenant-facing entry point (search_knowledge_base): a missing user AND
         org matches nothing instead of everything (the reference always applies ``user_id == u``,
@@ -359,11 +382,30 @@ class KnowledgeBase:
             return []
         if scoped and not user_id and not org_id:
             return []
+        if fusion is None:
+            fusion = HybridFusion.RANKED
+        if fusion not in _FUSION:
+            raise NotImplementedError(f"hybrid fusion {fusion!r}: only HybridFusion.RANKED and RELATIVE_SCORE are implemented")
         hybrid = alpha is not None and alpha < 1.0
         dense_w = 1.0 if not hybrid else max(0.0, float(alpha))
-        qv = self.encoder.encode([query]) if (dense_w > 0.0 and _dense is None) else None
+        on_device = (_fused is None and _dense is None and _sparse is None and hybrid and filters is None
+                     and self._hybrid_device)
+        if on_device:                       # a query whose dense leg is ignored still passes a vector: zeros
+            qv = self.encoder.encode([query]) if dense_w > 0.0 else np.zeros((1, self.dim), np.float32)
+        else:
+            qv = self.encoder.encode([query]) if (dense_w > 0.0 and _dense is None and _fused is None) else None
         with self._lock:
             tenant = scoped or user_id is not None or org_id is not None
+            if on_device:
+                q_user = q_org = None
+                if tenant:
+                    cu, co = self._scope_codes(user_id, org_id)
+                    q_user, q_org = np.array([cu], np.int32), np.array([co], np.int32)
+                _fused = self.sparse.search_batch([query], _MAX_FETCH, q_user, q_org,
+                                                  dense=(self.index, qv, np.array([dense_w]), _FUSION[fusion],
+                                                         min(limit, 2 * _MAX_FETCH)))[0]
+            if _fused is not None:          # fused on the device (here or by query_batch)
+                return self._shape([(rid, fs, cos) for rid, (fs, cos) in _fused if rid in self._props][:limit])
 
             def tenant_ok(props) -> bool:
                 if not tenant:
@@ -440,29 +482,55 @@ class KnowledgeBase:
                     else:
                         allowed_set = None
                     sparse = self.sparse.search(query, _MAX_FETCH, allowed=allowed_set, allowed_sorted=allowed_arr)
-                from .bm25 import ranked_fusion
+                from . import bm25
 
                 cos = dict(dense)
-                fused = ranked_fusion([(dense_w, [d for d, _ in dense]), (1.0 - dense_w, [d for d, _ in sparse])], limit)
+                if fusion == HybridFusion.RELATIVE_SCORE:
+                    fused = bm25.relative_score_fusion([(dense_w, dense), (1.0 - dense_w, sparse)], limit)
+                else:
+                    fused = bm25.ranked_fusion([(dense_w, [d for d, _ in dense]), (1.0 - dense_w, [d for d, _ in sparse])],
+                                               limit)
                 picked = [(rid, fs, cos.get(rid)) for rid, fs in fused]
-            out = []
-            for rid, score, cosine in picked:
-                meta = SimpleNamespace(score=float(score), distance=None if cosine is None else 1.0 - float(cosine))
-                out.append(SimpleNamespace(properties=dict(self._props[rid]), uuid=self._id2key.get(rid), metadata=meta))
-            return out
+            return self._shape(picked)
+
+    def _shape(self, picked) -> List[SimpleNamespace]:
+        """(id, score, dense cosine or None) -> result objects.  Caller holds the lock."""
+        out = []
+        for rid, score, cosine in picked:
+            meta = SimpleNamespace(score=float(score), distance=None if cosine is None else 1.0 - float(cosine))
+            out.append(SimpleNamespace(properties=dict(self._props[rid]), uuid=self._id2key.get(rid), metadata=meta))
+        return out
 
     def query_batch(self, reqs: List[Tuple[Optional[str], str, int, Optional[float], Optional[str]]]) -> List[List[SimpleNamespace]]:
         """Several tenant-scoped searches at once: ``(user_id, query, limit, alpha, org_id)`` each.  All query texts go
         through ONE encoder batch; the dense leg is ONE kernel launch per result size (the tenant scopes of the batch ride
         along as per-row bit masks on the tensor-core kernel); on a GPU keyword store the keyword leg of every hybrid request
-        (alpha < 1) is ONE device search with per-request tenant codes; fusion / shaping per request as in ``query``."""
+        (alpha < 1) is ONE device search with per-request tenant codes; fusion / shaping per request as in ``query``.
+        On a CUDA shard whose hybrid requests carry at most 32 distinct tenant scopes, those requests are instead ONE device
+        call for both legs and their ranked fusion (``DeviceBM25.search_batch`` with ``dense``, per-request weights), and
+        only shaping is left per request."""
         need = [i for i, (u, q, lim, a, o) in enumerate(reqs) if lim > 0 and (u or o) and (a is None or a > 0.0)]
-        kw_need = [i for i, (u, q, lim, a, o) in enumerate(reqs)
-                   if lim > 0 and (u or o) and a is not None and a < 1.0] if self._kw_device else []
+        hyb = [i for i, (u, q, lim, a, o) in enumerate(reqs) if lim > 0 and (u or o) and a is not None and a < 1.0]
         vecs = self.encoder.encode([reqs[i][1] for i in need]) if need else None
         dense: Dict[int, List[Tuple[int, float]]] = {}
         sparse: Dict[int, List[Tuple[int, float]]] = {}
+        fused: Dict[int, list] = {}
         with self._lock:
+            if hyb and self._hybrid_device:
+                codes = [self._scope_codes(reqs[i][0], reqs[i][4]) for i in hyb]
+                if len(set(codes)) <= 32:   # the tensor-core kernel's per-row scope masks hold them
+                    row = {i: pos for pos, i in enumerate(need)}
+                    hv = np.zeros((len(hyb), self.dim), vecs.dtype if vecs is not None else np.float32)
+                    for j, i in enumerate(hyb):
+                        if i in row:        # alpha <= 0: the dense leg is ignored, its vector stays zero
+                            hv[j] = vecs[row[i]]
+                    lists = self.sparse.search_batch(
+                        [reqs[i][1] for i in hyb], _MAX_FETCH, np.array([c[0] for c in codes], np.int32),
+                        np.array([c[1] for c in codes], np.int32),
+                        dense=(self.index, hv, np.array([max(0.0, float(reqs[i][3])) for i in hyb]), FUSION_RANKED,
+                               min(max(reqs[i][2] for i in hyb), 2 * _MAX_FETCH)))
+                    fused = dict(zip(hyb, lists))
+            kw_need = [i for i in hyb if i not in fused] if self._kw_device else []
             if kw_need:
                 codes = [self._scope_codes(reqs[i][0], reqs[i][4]) for i in kw_need]
                 lists = self.sparse.search_batch([reqs[i][1] for i in kw_need], _MAX_FETCH,
@@ -471,6 +539,8 @@ class KnowledgeBase:
                 sparse = dict(zip(kw_need, lists))
             groups: Dict[int, List[Tuple[int, int, int]]] = {}      # fetch size -> [(position, user code, org code)]
             for pos, i in enumerate(need):
+                if i in fused:
+                    continue
                 u, _, lim, a, o = reqs[i]
                 hybrid = a is not None and a < 1.0
                 fetch = max(1, min(_MAX_FETCH, lim if not hybrid else _MAX_FETCH))
@@ -503,7 +573,7 @@ class KnowledgeBase:
         out = []
         for i, (u, q, lim, a, o) in enumerate(reqs):
             out.append(self.query(q, lim, user_id=u, org_id=o, alpha=a, scoped=True, _dense=dense.get(i),
-                                  _sparse=sparse.get(i)))
+                                  _sparse=sparse.get(i), _fused=fused.get(i)))
         return out
 
     # ------------------------------------------------------------------ persistence
@@ -622,9 +692,12 @@ class _QueryFacade:
 
     def hybrid(self, query: str, limit: int = 10, alpha: float = 0.5, fusion_type=None, filters=None,
                return_metadata=None, **_):
-        if fusion_type not in (None, HybridFusion.RANKED):
-            raise NotImplementedError("only HybridFusion.RANKED (what the reference requests) is implemented")
-        return SimpleNamespace(objects=self._kb.query(query, limit, filters=filters, alpha=alpha))
+        """``fusion_type`` None means RANKED, what the reference requests (Weaviate's own default since 1.24 is
+        RELATIVE_SCORE); RELATIVE_SCORE is implemented too, anything else raises NotImplementedError."""
+        if fusion_type not in (None, HybridFusion.RANKED, HybridFusion.RELATIVE_SCORE):
+            raise NotImplementedError("only HybridFusion.RANKED (what the reference requests) and RELATIVE_SCORE are implemented")
+        return SimpleNamespace(objects=self._kb.query(query, limit, filters=filters, alpha=alpha,
+                                                      fusion=fusion_type or HybridFusion.RANKED))
 
     def near_text(self, query: str, limit: int = 10, filters=None, return_metadata=None, **_):
         return SimpleNamespace(objects=self._kb.query(query, limit, filters=filters))

@@ -340,6 +340,30 @@ int aur_kw_search_multi(aur_kw* const* stores, int32_t n_stores, const int32_t* 
                         int32_t nq, int32_t k, const int32_t* q_user, const int32_t* q_org, const int64_t* allow_ids,
                         int64_t n_allow, double* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out);
 
+/* ------------------------------------------------------------------ hybrid query
+ * collection.query.hybrid (weaviate_client.py:252-259) in one call: the dense leg (aur_search_ex of queries_host over
+ * ix, top-fetch cosines) and the keyword leg (aur_kw_search of q_terms / q_offsets over kw, top-fetch BM25 scores) run
+ * on the GPU, both enqueued before either is waited on, with the same per-query tenant scope q_user / q_org (as in
+ * aur_search; NULL = unscoped); each leg's answer is the one those calls give for the snapshot it reports.  A kernel
+ * then fuses query q's two lists with weights w_dense[q] / w_sparse[q] (finite; a leg whose weight is <= 0 takes no
+ * part, so with w_dense <= 0 the dense leg is searched but ignored) and one copy returns the best k_out entries by
+ * (fused score desc, id asc):
+ *   AUR_FUSION_RANKED          Weaviate's rankedFusion: an entry at 0-based rank r of a leg adds w / (r + 60);
+ *   AUR_FUSION_RELATIVE_SCORE  relativeScoreFusion: an entry with score s adds w * (s - lo) / (hi - lo), lo / hi the
+ *                              min / max score of its leg's list (w when hi == lo), cosines taken as fp64;
+ * summed in fp64 from 0.0, dense part first -- bit for bit aurora_b200.bm25.ranked_fusion / relative_score_fusion.
+ * scores_out [nq * k_out] fp64 fused scores, ids_out [nq * k_out], cosine_out [nq * k_out] the dense leg's fp32 cosine
+ * of the id (NaN when the id is not in the dense list); padding (-INFINITY, -1, NaN).  snapshot_rows_out [2] (nullable):
+ * the prefix the dense and the keyword leg saw.  1 <= fetch <= 128, 1 <= k_out <= 2 * fetch; a bf16 index and a
+ * keyword store on its device (else AUR_ERR_UNSUPPORTED / AUR_ERR_INVALID).  aur_stats.last_* and aur_kw_stats.last_*
+ * describe the two legs. */
+#define AUR_FUSION_RANKED 0
+#define AUR_FUSION_RELATIVE_SCORE 1
+int aur_hybrid_search(aur_index* ix, aur_kw* kw, const void* queries_host, int32_t nq, int32_t fetch,
+                      const int32_t* q_terms, const int64_t* q_offsets, const int32_t* q_user, const int32_t* q_org,
+                      const double* w_dense, const double* w_sparse, int32_t fusion, int32_t k_out,
+                      double* scores_out, int64_t* ids_out, float* cosine_out, int64_t* snapshot_rows_out);
+
 /* ------------------------------------------------------------------ text encoder
  * Replaces the text2vec-transformers sidecar: EmbeddingClient.embed / embed_batch
  * (server/services/correlation/embedding_client.py:39-78, POST {base}/vectors) and the
