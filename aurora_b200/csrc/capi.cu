@@ -938,6 +938,9 @@ int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_hos
   *snapshot_rows = n_rows;
   return AUR_OK;
 }
+
+int index_device(const aur_index* ix) { return ix->device; }
+int index_is_bf16(const aur_index* ix) { return ix->dtype == AUR_BF16; }
 }  // namespace aur
 
 extern "C" {

@@ -6,6 +6,7 @@
 #include <stdlib.h>
 
 #include <functional>
+#include <vector>
 
 struct aur_index;
 struct aur_kw;
@@ -310,13 +311,19 @@ struct DevBuf {   // grow-only device scratch
 // (else AUR_ERR_UNSUPPORTED / AUR_ERR_INVALID).  The leg's aur_stats.last_* are the index's last search.  (capi.cu)
 int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
               const int32_t* q_org, float* scores, int64_t* ids, int64_t* snapshot_rows);
-// Keyword leg: aur_kw_search's search (no allow-list) enqueued on the store's own context and stream, then
-// then(device, stream, scores, ids, snapshot_rows) runs with the leg's results -- device arrays [nq * k], valid once the
-// stream reaches them -- while the store's shared lock and the context are held.  The leg's aur_kw_stats.last_* are
-// published after then() returns AUR_OK.  (keyword.cu)
-using KwLegThen = std::function<int(int device, cudaStream_t s, const double* scores, const int64_t* ids, int64_t snapshot_rows)>;
-int kw_leg(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k, const int32_t* q_user,
-           const int32_t* q_org, const KwLegThen& then);
+int index_device(const aur_index* ix);
+int index_is_bf16(const aur_index* ix);
+// Keyword legs: aur_kw_search_multi's search (no allow-list) over stores[0 .. n) (distinct, non-NULL, 1 <= n <= 64)
+// taken as one corpus, each store's part enqueued on its own context and stream; then then(legs) runs with every
+// store's (device, stream, top-k lists, snapshot) -- device arrays [nq * k], valid once the stream reaches them,
+// sorted by (fp64 score desc, id asc) -- while every store's shared lock and every context are held.  Each store's
+// aur_kw_stats.last_* are published after then() returns AUR_OK.  The query arguments are checked by kw_check.  (keyword.cu)
+struct KwLeg { int device; cudaStream_t stream; const double* scores; const int64_t* ids; int64_t snapshot_rows; };
+using KwLegsThen = std::function<int(const std::vector<KwLeg>& legs)>;
+int kw_legs(aur_kw* const* stores, int n, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k,
+            const int32_t* q_user, const int32_t* q_org, const KwLegsThen& then);
+int kw_check(const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k);   // aur_kw_search's query checks
+int kw_device(const aur_kw* kw);
 
 // Error reporting shared by the translation units behind the C ABI (thread-local message).
 int report_error(int code, const char* fmt, ...);

@@ -21,7 +21,8 @@
 // buffers pruned by the block's own k-th best, sorted lists per block, then sorted folds down to one list per query.
 // aur_kw_search_multi runs the same search over several stores (one per GPU) as one corpus: N, df and total_len are
 // summed over the stores' snapshots, every store scores its own prefix with the resulting idf / avgdl, and the per-store
-// lists are merged on the host (DESIGN.md section 10, "Sharded store").
+// lists are merged on the host (DESIGN.md section 10, "Sharded store").  The hybrid query (hybrid.cu) runs the same
+// steps through kw_legs and merges the per-store lists on the device instead.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
@@ -630,9 +631,12 @@ void kw_prepare(aur_kw* const* stores, int n, const KwQuery& q, KwPlan* pl) {
   kw_plan(q, uniq, udf, N, &pl->blocks);
 }
 
-// Search stores[0 .. n) (distinct, arguments checked) as one corpus: store s's top-k lists land in
-// out_s / out_i + s * nq * k, scored with the idf and avgdl of the union of the snapshots.
-int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out_s, int64_t* out_i, int64_t* snapshot_rows) {
+// Search stores[0 .. n) (distinct, arguments checked) as one corpus and hand the enqueued parts to
+// after(ctxs, snaps): ctxs[s] = store s's context, whose stream computes its top-k lists into out_s / out_ids, scored
+// with the idf and avgdl of the union of the snapshots snaps.  Every store's shared lock is held, and every context
+// stays out of its pool, until after() has returned and the context's stream is idle (also on an error).
+template <typename After>
+int kw_run(aur_kw* const* stores, int n, const KwQuery& q, After&& after) {
   // shared locks for the whole search, in one order (by address) so that searches over overlapping store sets cannot
   // deadlock behind a waiting writer
   std::vector<aur_kw*> order(stores, stores + n);
@@ -642,7 +646,6 @@ int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out
   for (aur_kw* kw : order) locks.emplace_back(kw->rw);
   KwPlan pl;
   kw_prepare(stores, n, q, &pl);
-  const std::vector<KwSnap>& snaps = pl.snaps;
   // every store's work enqueued before any is waited on; the contexts go back to their pools only once their streams
   // are idle (also on an error), before the locks are released
   struct Ctxs {
@@ -651,6 +654,7 @@ int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out
       for (auto& e : v) { cudaSetDevice(e.first->device); cudaStreamSynchronize(e.second->stream); kw_ctx_release(e.first, e.second); }
     }
   } ctxs;
+  std::vector<KwCtx*> cs;
   for (int s = 0; s < n; ++s) {
     aur_kw* kw = stores[s];
     KW_TRY(cudaSetDevice(kw->device));
@@ -658,45 +662,55 @@ int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out
     int rc = kw_ctx_acquire(kw, &c);
     if (rc != AUR_OK) return rc;
     ctxs.v.emplace_back(kw, c);
-    const KwSnap& sn = snaps[static_cast<size_t>(s)];
+    cs.push_back(c);
+    const KwSnap& sn = pl.snaps[static_cast<size_t>(s)];
     if ((rc = kw_launch(kw, c, q, pl.blocks, sn.n_rows, pl.N, pl.avgdl)) != AUR_OK) return rc;
   }
-  const size_t nout = static_cast<size_t>(q.nq) * q.k;
-  for (int s = 0; s < n; ++s) {
-    const int rc = kw_collect(stores[s], ctxs.v[static_cast<size_t>(s)].second, q, out_s + s * nout, out_i + s * nout);
-    if (rc != AUR_OK) return rc;
-  }
-  if (snapshot_rows)
-    for (int s = 0; s < n; ++s) snapshot_rows[s] = snaps[static_cast<size_t>(s)].n_rows;
-  return AUR_OK;
+  return after(cs, pl.snaps);
+}
+
+// kw_run whose parts are copied to the host: store s's top-k lists land in out_s / out_i + s * nq * k.
+int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out_s, int64_t* out_i, int64_t* snapshot_rows) {
+  return kw_run(stores, n, q, [&](const std::vector<KwCtx*>& cs, const std::vector<KwSnap>& snaps) -> int {
+    const size_t nout = static_cast<size_t>(q.nq) * q.k;
+    for (int s = 0; s < n; ++s) {
+      const int rc = kw_collect(stores[s], cs[static_cast<size_t>(s)], q, out_s + s * nout, out_i + s * nout);
+      if (rc != AUR_OK) return rc;
+    }
+    if (snapshot_rows)
+      for (int s = 0; s < n; ++s) snapshot_rows[s] = snaps[static_cast<size_t>(s)].n_rows;
+    return AUR_OK;
+  });
 }
 
 }  // namespace
 
 namespace aur {
-int kw_leg(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k, const int32_t* q_user,
-           const int32_t* q_org, const KwLegThen& then) {
-  if (!kw) return report_error(AUR_ERR_INVALID, "null store");
+int kw_legs(aur_kw* const* stores, int n, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k,
+            const int32_t* q_user, const int32_t* q_org, const KwLegsThen& then) {
   const KwQuery q{q_terms, q_offsets, nq, k, q_user, q_org, nullptr, 0};
-  int rc = kw_check_query(q);
-  if (rc != AUR_OK) return rc;
-  std::shared_lock<std::shared_mutex> rl(kw->rw);   // held until the leg's kernels have finished (then() waits for them)
-  KwPlan pl;
-  kw_prepare(&kw, 1, q, &pl);
-  KW_TRY(cudaSetDevice(kw->device));
-  KwCtx* c = nullptr;
-  if ((rc = kw_ctx_acquire(kw, &c)) != AUR_OK) return rc;
-  struct Back {   // the context goes back to the pool once its stream is idle, also on an error
-    aur_kw* kw; KwCtx* c;
-    ~Back() { cudaSetDevice(kw->device); cudaStreamSynchronize(c->stream); kw_ctx_release(kw, c); }
-  } back{kw, c};
-  const int64_t n_rows = pl.snaps[0].n_rows;
-  if ((rc = kw_launch(kw, c, q, pl.blocks, n_rows, pl.N, pl.avgdl)) != AUR_OK) return rc;
-  if ((rc = then(kw->device, c->stream, c->out_s.p, c->out_ids.p, n_rows)) != AUR_OK) return rc;
-  KW_TRY(cudaSetDevice(kw->device));
-  KW_TRY(cudaStreamSynchronize(c->stream));
-  return kw_publish(kw, c);
+  return kw_run(stores, n, q, [&](const std::vector<KwCtx*>& cs, const std::vector<KwSnap>& snaps) -> int {
+    std::vector<KwLeg> legs(static_cast<size_t>(n));
+    for (int s = 0; s < n; ++s) {
+      const KwCtx* c = cs[static_cast<size_t>(s)];
+      legs[static_cast<size_t>(s)] = KwLeg{stores[s]->device, c->stream, c->out_s.p, c->out_ids.p, snaps[static_cast<size_t>(s)].n_rows};
+    }
+    int rc = then(legs);
+    if (rc != AUR_OK) return rc;
+    for (int s = 0; s < n; ++s) {
+      KW_TRY(cudaSetDevice(stores[s]->device));
+      KW_TRY(cudaStreamSynchronize(cs[static_cast<size_t>(s)]->stream));
+      if ((rc = kw_publish(stores[s], cs[static_cast<size_t>(s)])) != AUR_OK) return rc;
+    }
+    return AUR_OK;
+  });
 }
+
+int kw_check(const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k) {
+  return kw_check_query(KwQuery{q_terms, q_offsets, nq, k, nullptr, nullptr, nullptr, 0});
+}
+
+int kw_device(const aur_kw* kw) { return kw->device; }
 }  // namespace aur
 
 extern "C" {

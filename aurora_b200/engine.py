@@ -479,15 +479,30 @@ class KeywordIndex:
         return a["ids"], a["scores"], int(snap.value)
 
 
-def hybrid_search(index: Index, kw_index: KeywordIndex, queries: np.ndarray, fetch: int, q_terms, q_offsets,
+def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_offsets,
                   w_dense, w_sparse=None, fusion: int = N.FUSION_RANKED, k_out: Optional[int] = None, q_user=None,
                   q_org=None):
     """Both legs of the hybrid query and their fusion in one device call (aur_hybrid_search): the dense leg's top-``fetch``
     of ``queries`` over ``index`` and the keyword leg's top-``fetch`` of ``q_terms`` / ``q_offsets`` over ``kw_index``
     (same tenant scope), fused per query with weights ``w_dense`` / ``w_sparse`` (default ``1 - w_dense``).  Returns
     (ids [nq, k_out] int64, fused scores [nq, k_out] float64, dense cosines [nq, k_out] float32 (NaN: not in the dense
-    list), (dense snapshot rows, keyword snapshot rows)); padding (-1, -inf, NaN)."""
-    q = index._rows_buffer(queries)
+    list), (dense snapshot rows, keyword snapshot rows)); padding (-1, -inf, NaN).
+
+    ``index`` / ``kw_index`` are an ``Index`` and a ``KeywordIndex``, or a ``MultiIndex`` of bf16 ``Index`` shards and a
+    ``MultiKeywordIndex`` on the same devices in the same order (aur_hybrid_search_multi): each leg is then the global
+    top-``fetch`` of ``MultiIndex.search`` / ``MultiKeywordIndex.search``, merged and fused on shard 0's GPU, and the
+    snapshots are (one per shard, one per store)."""
+    multi = isinstance(index, MultiIndex)
+    if multi:
+        if not isinstance(kw_index, MultiKeywordIndex):
+            raise TypeError("a MultiIndex is searched together with a MultiKeywordIndex")
+        if not index.shards or not all(isinstance(sh, Index) and sh.dtype == N.AUR_BF16 for sh in index.shards):
+            raise TypeError("hybrid_search over a MultiIndex needs bf16 engine.Index shards")
+        if kw_index.devices != index.devices or len(kw_index.stores) != len(index.shards):
+            raise ValueError(f"keyword stores on devices {kw_index.devices}, vector shards on {index.devices}")
+        q = index.shards[0]._rows_buffer(queries)
+    else:
+        q = index._rows_buffer(queries)
     nq = q.shape[0]
     k_out = 2 * int(fetch) if k_out is None else int(k_out)
     wd = np.ascontiguousarray(np.broadcast_to(np.asarray(w_dense, dtype=np.float64), (nq,)))
@@ -499,6 +514,15 @@ def hybrid_search(index: Index, kw_index: KeywordIndex, queries: np.ndarray, fet
     scores = np.empty((nq, k_out), dtype=np.float64)
     ids = np.empty((nq, k_out), dtype=np.int64)
     cosine = np.empty((nq, k_out), dtype=np.float32)
+    if multi:
+        n = len(index.shards)
+        shards = (C.c_void_p * n)(*[sh._h.value for sh in index.shards])
+        stores = (C.c_void_p * n)(*[st._h.value for st in kw_index.stores])
+        snaps = np.full(2 * n, -1, dtype=np.int64)
+        N.check(N.load().aur_hybrid_search_multi(shards, stores, n, _ptr(q), nq, int(fetch), _ptr(qt), _ptr(q_off), _ptr(u),
+                                                 _ptr(o), _ptr(wd), _ptr(ws), int(fusion), k_out, _ptr(scores), _ptr(ids),
+                                                 _ptr(cosine), _ptr(snaps)))
+        return ids, scores, cosine, (snaps[:n].tolist(), snaps[n:].tolist())
     snaps = (C.c_int64 * 2)(-1, -1)
     N.check(index._lib.aur_hybrid_search(index._h, kw_index._h, _ptr(q), nq, int(fetch), _ptr(qt), _ptr(q_off), _ptr(u),
                                          _ptr(o), _ptr(wd), _ptr(ws), int(fusion), k_out, _ptr(scores), _ptr(ids),

@@ -124,15 +124,22 @@ class KnowledgeBase:
 
     def _fuses_on_device(self) -> bool:
         """Whether an unfiltered hybrid query runs as one device call, both legs and their fusion
-        (``engine.hybrid_search``): a bf16 ``engine.Index`` and a ``DeviceBM25`` over a ``KeywordIndex`` on its GPU.
-        ``MultiIndex``, f32 shards and the CPU doubles fuse on the host (``bm25.ranked_fusion`` /
+        (``engine.hybrid_search``): a bf16 ``engine.Index`` and a ``DeviceBM25`` over a ``KeywordIndex`` on its GPU, or
+        a ``MultiIndex`` of bf16 ``engine.Index`` shards and a ``DeviceBM25`` over a ``MultiKeywordIndex`` on the same
+        devices in the same order.  f32 shards and the CPU doubles fuse on the host (``bm25.ranked_fusion`` /
         ``relative_score_fusion``), as do filtered queries."""
         from .bm25 import DeviceBM25
-        from .engine import Index, KeywordIndex
+        from .engine import Index, KeywordIndex, MultiIndex, MultiKeywordIndex
 
         ix, sp = self.index, self.sparse
-        return (isinstance(ix, Index) and ix.dtype == AUR_BF16 and isinstance(sp, DeviceBM25)
-                and isinstance(sp.store, KeywordIndex) and sp.store.device == ix.device)
+        if not isinstance(sp, DeviceBM25):
+            return False
+        if isinstance(ix, MultiIndex):
+            return (bool(ix.shards) and all(isinstance(sh, Index) and sh.dtype == AUR_BF16 for sh in ix.shards)
+                    and isinstance(sp.store, MultiKeywordIndex) and sp.store.devices == ix.devices
+                    and len(sp.store.stores) == len(ix.shards))
+        return (isinstance(ix, Index) and ix.dtype == AUR_BF16 and isinstance(sp.store, KeywordIndex)
+                and sp.store.device == ix.device)
 
     def _scope_codes(self, user_id: Optional[str], org_id: Optional[str]) -> Tuple[int, int]:
         """Tenant scope as the kernels take it: (user code, org code); -2 matches no row, org -1 = no org."""

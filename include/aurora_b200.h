@@ -363,6 +363,25 @@ int aur_hybrid_search(aur_index* ix, aur_kw* kw, const void* queries_host, int32
                       const int32_t* q_terms, const int64_t* q_offsets, const int32_t* q_user, const int32_t* q_org,
                       const double* w_dense, const double* w_sparse, int32_t fusion, int32_t k_out,
                       double* scores_out, int64_t* ids_out, float* cosine_out, int64_t* snapshot_rows_out);
+/* aur_hybrid_search over n (1 .. 64) vector shards and n keyword stores taken as one corpus, e.g. one shard and one store
+ * per GPU of the host with documents placed by id mod n (engine.MultiIndex + engine.MultiKeywordIndex); shard s and
+ * store s must be on the same device, shards bf16, ids unique across the shards.  Every shard's dense leg and every
+ * store's keyword leg (the stores scored with corpus-wide statistics, as aur_kw_search_multi) run on their own devices,
+ * all enqueued before any is waited on; the lists of shards 1 .. n-1 are copied to shard 0's device (peer copies;
+ * peer access is neither required nor enabled), where one kernel merges each leg's lists into its global top-fetch and
+ * fuses the two as aur_hybrid_search does.  Each leg's merged list is exactly the host merge's: aur_merge_topk_host on
+ * the shards' fp32 cosines (engine.MultiIndex.search), aur_merge_topk_host_f64 on the stores' fp64 scores
+ * (aur_kw_search_multi) -- best head first by (score desc, id asc, list asc), a list ending at its first id < 0.
+ * snapshot_rows_out [2n] (nullable): entries 0 .. n-1 the prefix each shard's dense leg saw, n .. 2n-1 the prefix each
+ * store's keyword leg saw.  Each shard's aur_stats.last_* and each store's aur_kw_stats.last_* describe its own part.
+ * NULL entries, a shard or a store listed twice, n out of range: AUR_ERR_INVALID; an f32 shard: AUR_ERR_UNSUPPORTED; a
+ * store on another device than its shard: AUR_ERR_INVALID; the other arguments as for aur_hybrid_search.  Every
+ * rejection happens before any device work.  aur_hybrid_search is this call with n = 1. */
+int aur_hybrid_search_multi(aur_index* const* shards, aur_kw* const* stores, int32_t n, const void* queries_host,
+                            int32_t nq, int32_t fetch, const int32_t* q_terms, const int64_t* q_offsets,
+                            const int32_t* q_user, const int32_t* q_org, const double* w_dense, const double* w_sparse,
+                            int32_t fusion, int32_t k_out, double* scores_out, int64_t* ids_out, float* cosine_out,
+                            int64_t* snapshot_rows_out /* [2n] */);
 
 /* ------------------------------------------------------------------ text encoder
  * Replaces the text2vec-transformers sidecar: EmbeddingClient.embed / embed_batch
