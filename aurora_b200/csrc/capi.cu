@@ -167,6 +167,8 @@ struct aur_index {
   int opt_kernel = AUR_KERNEL_AUTO;
   int opt_dbg_flags = 0;
   int opt_tc_tile = 0;           // corpus rows per tile: 0 = auto, 64, 128
+  int opt_tc_stages = 0;         // cap on the TMA ring's depth: 0 = the deepest that fits
+  int opt_tc_qregs = -1;         // query k-blocks in the MMA warpgroup's registers: -1 = auto, 0 = none, kTcQRegs
   std::atomic<uint32_t> opt_dbg_epoch{0};   // bring-up: start value of the contexts' launch counters (0 = 1)
   std::vector<std::unique_ptr<SearchCtx>> ctxs;
   std::vector<SearchCtx*> free_ctxs;   // idle pool contexts
@@ -353,9 +355,16 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   const bool mask = row_mask != nullptr;
   int tile_n = ix->opt_tc_tile;
   if (tile_n == 0) tile_n = tc_auto_tile(ksel, ix->dim, ix->smem_optin, mask, dbg != nullptr);
-  const int stages = tc_pick_stages(ksel, ix->dim, ix->smem_optin, tile_n, mask);
-  if (stages < 2) return fail(AUR_ERR_UNSUPPORTED, "k too large for the tensor-core path's shared memory");
-  const size_t smem = tc_smem_bytes(stages, ksel, ix->dim, tile_n, mask);
+  // The width is settled (from the all-in-shared-memory layout); a 128-row launch then moves its first query k-blocks
+  // into registers and spends the shared memory they leave on ring stages.
+  // The bring-up switch that issues no MMAs (dbg_flags & 2) keeps the whole block in shared memory: without MMAs
+  // nothing holds the warpgroup's four warps in step, and the one such run with register k-blocks stopped making progress.
+  const int qregs = (tile_n == kTcTileWide && ix->opt_tc_qregs != 0 && !(ix->opt_dbg_flags & 2) && ix->dim / kTcKBlock >= kTcQRegs) ? kTcQRegs : 0;
+  // (what fits is decided without the registers too: they deepen a ring, they do not admit a larger k)
+  if (tc_pick_stages(ksel, ix->dim, ix->smem_optin, tile_n, mask) < 2) return fail(AUR_ERR_UNSUPPORTED, "k too large for the tensor-core path's shared memory");
+  int stages = tc_pick_stages(ksel, ix->dim, ix->smem_optin, tile_n, mask, qregs);
+  if (ix->opt_tc_stages >= 2 && ix->opt_tc_stages < stages) stages = ix->opt_tc_stages;
+  const size_t smem = tc_smem_bytes(stages, ksel, ix->dim, tile_n, mask, qregs);
   const size_t ncand = static_cast<size_t>(n_qblocks) * kTcQRows * n_lists * ksel;
   CU_TRY(c->cand_a.reserve(ncand));
   const size_t npub = static_cast<size_t>(n_qblocks) * kTcQRows * (((n_lists + 1) & ~1) + 1);
@@ -391,7 +400,7 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   p.num_stages = stages;
   p.dbg_flags = ix->opt_dbg_flags;
   p.n_tiles = static_cast<int>((n_rows + tile_n - 1) / tile_n);
-  CU_TRY(tc_launch(cta_group, tile_n, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
+  CU_TRY(tc_launch(cta_group, tile_n, qregs, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
   c->last_tile_n = tile_n;
   *n_lists_out = n_lists;
   return AUR_OK;
@@ -1176,6 +1185,17 @@ int aur_set_option(aur_index* ix, const char* key, int64_t value) {
   if (strcmp(key, "tc_tile") == 0) {
     if (value != 0 && value != kTcTileN && value != kTcTileWide) return fail(AUR_ERR_INVALID, "tc_tile must be 0 (auto), 64 or 128");
     ix->opt_tc_tile = static_cast<int>(value);
+    return AUR_OK;
+  }
+  if (strcmp(key, "tc_stages") == 0) {
+    if (value != 0 && (value < 2 || value > kTcMaxStages)) return fail(AUR_ERR_INVALID, "tc_stages must be 0 (deepest) or 2 .. %d", kTcMaxStages);
+    ix->opt_tc_stages = static_cast<int>(value);
+    return AUR_OK;
+  }
+  if (strcmp(key, "tc_qregs") == 0) {
+    if (value != -1 && value != 0 && (value != kTcQRegs || ix->dim / kTcKBlock < kTcQRegs))
+      return fail(AUR_ERR_INVALID, "tc_qregs must be -1 (auto), 0, or %d at dim >= %d", kTcQRegs, kTcQRegs * kTcKBlock);
+    ix->opt_tc_qregs = static_cast<int>(value);
     return AUR_OK;
   }
   if (strcmp(key, "dbg_flags") == 0) { ix->opt_dbg_flags = static_cast<int>(value); return AUR_OK; }

@@ -58,6 +58,9 @@ constexpr int kTcTileN = 64;       // corpus rows per tile  (MMA N); the bring-u
 constexpr int kTcTileWide = 128;   // the wide tile (wgmma m64n128), picked per launch when its layout fits
 constexpr int kTcWideMinStages = 4;   // with three 16 KB stages the wide tile measured no faster than the 64-row one
 constexpr int kTcKBlock = 64;      // bf16 per 128-byte swizzled smem row (one pipeline stage)
+// Leading query k-blocks a 128-row launch keeps in the MMA warpgroup's registers (16 registers a thread each) when
+// dim / 64 has that many, instead of 8 KB shared-memory tiles: every two of them buy one more 16 KB ring stage.
+constexpr int kTcQRegs = 6;   // 4 measured slower (six ring stages at dim 768 / top-32 against seven), 8 spills
 constexpr int kTcQRows = 64;       // queries per CTA (MMA M of one warpgroup)
 constexpr int kTcChunk = 16;       // scores examined per threshold test
 constexpr int kTcListMin = 64;     // list slots per query: max(ksel, this) so a whole first tile appends
@@ -96,12 +99,13 @@ constexpr int kTcPubMax = 74;      // published values a thread folds into its t
 // other's entries as its own.  0 is never a tag: it marks a zeroed table.
 constexpr uint32_t kSearchEpochMax = 0x7FFFFFFFu;
 
-// tile_n: corpus rows per tile, kTcTileN or kTcTileWide; mask: a kMask launch (row_mask set).
-size_t tc_smem_bytes(int num_stages, int ksel, int dim, int tile_n, bool mask);
-int tc_pick_stages(int ksel, int dim, size_t smem_limit, int tile_n, bool mask);
+// tile_n: corpus rows per tile, kTcTileN or kTcTileWide; mask: a kMask launch (row_mask set); qregs: leading query
+// k-blocks held in registers, which take no shared memory (0 or kTcQRegs, the latter with 128-row tiles only).
+size_t tc_smem_bytes(int num_stages, int ksel, int dim, int tile_n, bool mask, int qregs = 0);
+int tc_pick_stages(int ksel, int dim, size_t smem_limit, int tile_n, bool mask, int qregs = 0);
 // Launches the fused similarity + top-k kernel; cta_group 2 = two-CTA clusters sharing every corpus tile by TMA
 // multicast.  tmap: CUtensorMap over the corpus with a {64, tile_n / cta_group} box and 128-byte swizzle.
-cudaError_t tc_launch(int cta_group, int tile_n, int grid, const void* tmap, const TcParams& p, size_t smem, cudaStream_t s);
+cudaError_t tc_launch(int cta_group, int tile_n, int qregs, int grid, const void* tmap, const TcParams& p, size_t smem, cudaStream_t s);
 
 // ---------------------------------------------------------------- SIMT kernels
 struct FilterArgs {

@@ -177,6 +177,18 @@ __device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t a, uin
       : AUR_R8(0), AUR_R8(8), AUR_R8(16), AUR_R8(24), AUR_R8(32), AUR_R8(40), AUR_R8(48), AUR_R8(56)
       : "l"(a), "l"(b), "r"(accumulate));
 }
+// Same, N = 128, A from registers: four bf16x2 per thread, the m64k16 A fragment (rows 16 w + l / 4 and + 8, columns
+// 2 (l % 4) and + 8).  B in shared memory, K-major.
+__device__ __forceinline__ void wgmma_m64n128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63},"
+      " {%64,%65,%66,%67}, %68, p, 1, 1, 0;\n\t}"
+      : AUR_R8(0), AUR_R8(8), AUR_R8(16), AUR_R8(24), AUR_R8(32), AUR_R8(40), AUR_R8(48), AUR_R8(56)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(accumulate));
+}
 // Same, N = 256.
 __device__ __forceinline__ void wgmma_m64n256_ss(float (&d)[128], uint64_t a, uint64_t b, uint32_t accumulate) {
   asm volatile(

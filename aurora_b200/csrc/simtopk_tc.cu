@@ -1,15 +1,18 @@
 // Fused similarity + top-k for sm_90a: S = Q . C^T on wgmma tensor cores with the query
-// block resident in shared memory, the corpus streamed once from HBM by TMA, and a per-query
-// candidate list kept in shared memory by the epilogue warps.
+// block resident on the SM (shared memory, and for 128-row tiles its first k-blocks in the MMA warpgroup's registers),
+// the corpus streamed once from HBM by TMA, and a per-query candidate list kept in shared memory by the epilogue warps.
 //
 // Replaces the dense leg of collection.query.hybrid(...) / near_text(...) that the
 // reference sends to Weaviate (server/routes/knowledge_base/weaviate_client.py:252-259,
 // server/routes/incident_feedback/weaviate_client.py:286-291).
 //
 // Tile width N = 64 or 128 corpus rows (kTileN, chosen per launch on the host, tc_auto_tile in capi.cu): 128 when its
-// layout keeps at least four 16 KB ring stages -- at dim 768 / top-32 four stages against eight 8 KB ones -- else 64.  The wide tile runs wgmma m64n128k16: the query operand is fetched from shared memory once
-// per 128 corpus rows instead of once per 64, and the drain, score-buffer hand-off and threshold read happen once per
-// 128 rows.  Its epilogue examines a tile 64 scores at a time with the 64-row code.
+// layout with the whole query block in shared memory keeps at least four 16 KB ring stages, else 64.  The wide tile runs
+// wgmma m64n128k16: the query operand is fetched once per 128 corpus rows instead of once per 64, and the drain,
+// score-buffer hand-off and threshold read happen once per 128 rows.  Its epilogue examines a tile 64 scores at a time
+// with the 64-row code.  A wide launch then keeps its first kTcQRegs query k-blocks as wgmma's register A operand (kQReg,
+// when dim / 64 has that many) and spends the 8 KB of shared memory each one leaves on the ring: at dim 768 / top-32
+// seven 16 KB stages against the eight 8 KB ones of the 64-row kernel, in the same footprint as four.
 //
 // One CTA, persistent, 1 CTA / SM:
 //   warps 1..2   epilogue  : thread r of the two warps owns query r (score-buffer row r): reads its N scores of a
@@ -20,7 +23,8 @@
 //   warp 0      threshold  : serves the certified global threshold of the queries assigned to this CTA (see
 //                            "Threshold exchange").
 //   warp 3      TMA producer: corpus tiles [N rows x 64 k] -> smem ring (SWIZZLE_128B)
-//   warps 4..7  MMA        : wgmma m64nNk16, A = the CTA's 64 queries (K-major tiles in shared memory), B =
+//   warps 4..7  MMA        : wgmma m64nNk16, A = the CTA's 64 queries (K-major tiles in shared memory; k-blocks
+//                            0 .. kQReg - 1 as register fragments loaded once from global memory), B =
 //                            corpus tile from the ring; the [64 queries x N rows] fp32 accumulator lives in
 //                            registers for the whole tile and is then stored to a padded score buffer that the
 //                            epilogue warps read row-wise.  The MMA of the next tile runs while the epilogue
@@ -83,13 +87,14 @@ struct SmemLayout {
 };
 // The 128-row layout fits a fourth 16 KB ring stage at dim 768 / ksel 40 only without what the 64-row one can afford:
 // it reserves the tenant-scope masks for kMask launches alone and parks half as many groups per thread in the FIFO.
-__host__ __device__ inline SmemLayout make_layout(int num_stages, int ksel, int dim, int tile_n, bool mask) {
+// qregs: leading query k-blocks the MMA warpgroup keeps in registers; only the others have a tile at off_qs.
+__host__ __device__ inline SmemLayout make_layout(int num_stages, int ksel, int dim, int tile_n, bool mask, int qregs) {
   SmemLayout L;
   const bool wide = tile_n == kTcTileWide;
   L.lcap = static_cast<uint32_t>(ksel);
   uint32_t o = stage_bytes(tile_n) * num_stages;
   // the query block: [64 queries x 64] bf16 K-major SWIZZLE_128B tiles, one per k-block (the wgmma A operand)
-  L.off_qs = o;     o += static_cast<uint32_t>(dim / kTcKBlock) * kQTileBytes;
+  L.off_qs = o;     o += static_cast<uint32_t>(dim / kTcKBlock - qregs) * kQTileBytes;
   L.off_sc = o;     o += sc_bytes(tile_n);
   L.off_list = o;   o += L.lcap * kSlot;
   L.off_norm = o;   o += 2u * 2u * tile_n * 4u;
@@ -275,10 +280,14 @@ constexpr uint32_t kNaNBits = 0x7FC00000u;
 // batch may see the row -- and every query knows its scope's bit: scores of invisible rows become NaN before anything
 // else looks at them, exactly like tombstones.  (One scope for the whole batch needs none of this: it folds into the
 // inverse norms.)
-template <int kCtaGroup, bool kMask, int kTileN>
+//
+// kQReg: the first kQReg query k-blocks are the MMA warpgroup's register A operand instead of shared-memory tiles
+// (128-row tiles only; the host launches it only when dim / 64 >= kQReg).  Every two of them free one 16 KB ring stage.
+template <int kCtaGroup, bool kMask, int kTileN, int kQReg>
 __global__ void __launch_bounds__(kThreads, 1)
 simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   static_assert(kTileN == kTcTileN || kTileN == kTcTileWide, "tile width");
+  static_assert(kQReg == 0 || kTileN == kTcTileWide, "register-resident query k-blocks: 128-row tiles only");
   constexpr uint32_t kStageBytes = stage_bytes(kTileN);
   constexpr int kScStride = sc_stride(kTileN);
   constexpr int kHalves = kTileN / 64;   // the epilogue examines a tile 64 scores (four 16-score chunks) at a time
@@ -288,7 +297,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   // shared-address-space inference, i.e. LDS/STS instead of generic loads.
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
 
-  const SmemLayout L = make_layout(p.num_stages, p.ksel, p.dim, kTileN, kMask);
+  const SmemLayout L = make_layout(p.num_stages, p.ksel, p.dim, kTileN, kMask, kQReg);
   float* normbuf = reinterpret_cast<float*>(smem + L.off_norm);      // [2 warps][2][kTileN]
   uint32_t* maskbuf = reinterpret_cast<uint32_t*>(smem + L.off_mask);  // [2 warps][2][kTileN]
   float* scbuf = reinterpret_cast<float*>(smem + L.off_sc);          // [64 queries][kScStride]
@@ -396,7 +405,28 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
     // 8 j + 2 (l % 4) (+ 1), j = 0..N/8-1 -- stored into the score buffer as [query][corpus row].
     const int wt = threadIdx.x - kMmaWarp0 * 32;
     const int w4 = wt >> 5, l4 = wt & 31;
-    mbar_wait(q_ready, 0);   // the query block is in shared memory (and visible to the async proxy)
+    // Register A operand: per k-block and K step the m64k16 fragment of this thread -- rows 16 w + l / 4 (+ 8), the
+    // bf16 pairs at columns 16 s + 2 (l % 4) (+ 8) -- read straight from global memory while the epilogue warps stage
+    // the other k-blocks.  Rows past nq are zeros, as in the staged tiles.  Written here and never again, and indexed by
+    // compile-time constants only (a dynamic index would put the array in local memory).
+    uint32_t qa[kQReg > 0 ? kQReg : 1][4][4];
+    if constexpr (kQReg > 0) {
+      const int qrow = qblock * kTcQRows + 16 * w4 + (l4 >> 2);
+      const uint32_t* q0 = reinterpret_cast<const uint32_t*>(p.q + static_cast<size_t>(qrow) * p.dim) + (l4 & 3);
+      const uint32_t* q8 = q0 + 4 * p.dim;   // row + 8, in 32-bit words
+      const bool ok0 = qrow < p.nq, ok8 = qrow + 8 < p.nq;
+#pragma unroll
+      for (int kb = 0; kb < kQReg; ++kb)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int wofs = kb * 32 + k * 8;
+          qa[kb][k][0] = ok0 ? __ldg(q0 + wofs) : 0u;
+          qa[kb][k][1] = ok8 ? __ldg(q8 + wofs) : 0u;
+          qa[kb][k][2] = ok0 ? __ldg(q0 + wofs + 4) : 0u;
+          qa[kb][k][3] = ok8 ? __ldg(q8 + wofs + 4) : 0u;
+        }
+    }
+    mbar_wait(q_ready, 0);   // the staged query k-blocks are in shared memory (and visible to the async proxy)
     const uint32_t qs_a = smem_u32(smem + L.off_qs);
     const uint32_t ring_a = smem_u32(smem);
     // One commit group per k-block, then wait_group 1: the next k-block's MMAs are queued while the previous ones run,
@@ -410,6 +440,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
     // are unconditional: ptxas serialises every wgmma of the kernel when a group may be in flight where paths merge.
     // (Overlapping the score-buffer store with the next tile's first k-block, through a second accumulator, makes
     // ptxas serialise every wgmma too: it does not track which accumulator a wait_group 1 retires across loops.)
+    // A tile is kQReg unrolled k-blocks with register A, then the runtime loop with shared-memory A; both run the one
+    // body below, so the stage, phase and release bookkeeping is the same for either operand source.
     int stage = 0, rel_stage = 0; uint32_t phase = 0;
     long long tm_empty = 0, tm_full = 0;
     const long long tm_begin = TCLK();
@@ -421,31 +453,43 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       }
       if (++rel_stage == p.num_stages) rel_stage = 0;
     };
+    // one k-block: mmas(db) issues its four K = 16 MMAs against the ring stage behind descriptor db
+    auto kblock = [&](int kb, auto&& mmas) {
+      {
+        const long long t0 = TCLK();
+        mbar_wait(&full_bar[stage], phase);
+        tm_full += TCLK() - t0;
+      }
+      if (!(p.dbg_flags & 2)) {
+        wgmma_fence();
+        mmas(wgmma_desc_sw128(ring_a + static_cast<uint32_t>(stage) * kStageBytes));
+        wgmma_commit();
+      }
+      wgmma_wait<1>();   // k-block kb - 1 has retired
+      if (kb > 0) release();
+      if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
+    };
     for (int it = 0; it < my_tiles; ++it) {
       float d[kTileN / 2];
 #pragma unroll
       for (int i = 0; i < kTileN / 2; ++i) d[i] = 0.f;
-      for (int kb = 0; kb < kbs; ++kb) {
-        {
-          const long long t0 = TCLK();
-          mbar_wait(&full_bar[stage], phase);
-          tm_full += TCLK() - t0;
-        }
-        if (!(p.dbg_flags & 2)) {
-          wgmma_fence();
-          const uint64_t da = wgmma_desc_sw128(qs_a + static_cast<uint32_t>(kb) * kQTileBytes);
-          const uint64_t db = wgmma_desc_sw128(ring_a + static_cast<uint32_t>(stage) * kStageBytes);
+      if constexpr (kQReg > 0) {
+#pragma unroll
+        for (int kb = 0; kb < kQReg; ++kb)
+          kblock(kb, [&](uint64_t db) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_m64n128_rs(d, qa[kb][k], db + 2 * k, 1u);
+          });
+      }
+      for (int kb = kQReg; kb < kbs; ++kb)
+        kblock(kb, [&](uint64_t db) {
+          const uint64_t da = wgmma_desc_sw128(qs_a + static_cast<uint32_t>(kb - kQReg) * kQTileBytes);
 #pragma unroll
           for (int k = 0; k < 4; ++k) {   // 4 x K=16 per 128-byte k-block
             if constexpr (kTileN == kTcTileWide) wgmma_m64n128_ss(d, da + 2 * k, db + 2 * k, 1u);
             else wgmma_m64n64_ss(d, da + 2 * k, db + 2 * k, 1u);
           }
-          wgmma_commit();
-        }
-        wgmma_wait<1>();   // k-block kb - 1 has retired
-        if (kb > 0) release();
-        if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
-      }
+        });
       wgmma_wait<0>();
       wgmma_fence_regs(d);
       release();
@@ -545,19 +589,21 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
         };
         // every CTA of a query block reads the same block at the same moment: start each at a different
         // k-block (rotation by tile set) so they do not all queue on the same L2 lines
-        const int rot = kbs > 0 ? tset % kbs : 0;
-        auto kb_of = [&](int j) { return (j < kbs) ? (j + rot) % kbs : kbs; };
+        // (only the k-blocks the MMA warpgroup does not hold in registers: kQReg .. kbs - 1, tile index kb - kQReg)
+        const int nst = kbs - kQReg;
+        const int rot = nst > 0 ? tset % nst : 0;
+        auto kb_of = [&](int j) { return (j < nst) ? kQReg + (j + rot) % nst : kbs; };
         // four k-blocks of loads (32 x 16 B per lane) are issued before the first is consumed
         constexpr int kDepth = 4;
         uint4 x[kDepth][8];
-        for (int j0 = 0; j0 < kbs; j0 += kDepth) {
+        for (int j0 = 0; j0 < nst; j0 += kDepth) {
 #pragma unroll
           for (int u = 0; u < kDepth; ++u) load_kb(kb_of(j0 + u), x[u]);
 #pragma unroll
           for (int u = 0; u < kDepth; ++u) {
             const int j = j0 + u;
-            if (j >= kbs) break;
-            uint8_t* tile = smem + L.off_qs + static_cast<uint32_t>(kb_of(j)) * kQTileBytes + quarter * 32 * 128;
+            if (j >= nst) break;
+            uint8_t* tile = smem + L.off_qs + static_cast<uint32_t>(kb_of(j) - kQReg) * kQTileBytes + quarter * 32 * 128;
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               const int id = i * 32 + lane, row = id >> 3, c = id & 7;
@@ -858,9 +904,9 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   if constexpr (kCtaGroup == 2) cluster_sync_all();
 }
 
-template <int kCtaGroup, bool kMask, int kTileN>
+template <int kCtaGroup, bool kMask, int kTileN, int kQReg = 0>
 cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm, const TcParams& p, size_t smem) {
-  auto kern = simtopk_tc_kernel<kCtaGroup, kMask, kTileN>;
+  auto kern = simtopk_tc_kernel<kCtaGroup, kMask, kTileN, kQReg>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
   return cudaLaunchKernelEx(&cfg, kern, tm, p);
@@ -868,17 +914,17 @@ cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm,
 
 }  // namespace
 
-size_t tc_smem_bytes(int num_stages, int ksel, int dim, int tile_n, bool mask) {
-  return make_layout(num_stages, ksel, dim, tile_n, mask).total + 1024;  // + alignment slack
+size_t tc_smem_bytes(int num_stages, int ksel, int dim, int tile_n, bool mask, int qregs) {
+  return make_layout(num_stages, ksel, dim, tile_n, mask, qregs).total + 1024;  // + alignment slack
 }
 
-int tc_pick_stages(int ksel, int dim, size_t smem_limit, int tile_n, bool mask) {
+int tc_pick_stages(int ksel, int dim, size_t smem_limit, int tile_n, bool mask, int qregs) {
   for (int s = kTcMaxStages; s >= 2; --s)
-    if (tc_smem_bytes(s, ksel, dim, tile_n, mask) <= smem_limit) return s;
+    if (tc_smem_bytes(s, ksel, dim, tile_n, mask, qregs) <= smem_limit) return s;
   return 0;
 }
 
-cudaError_t tc_launch(int cta_group, int tile_n, int grid, const void* tmap, const TcParams& p, size_t smem, cudaStream_t s) {
+cudaError_t tc_launch(int cta_group, int tile_n, int qregs, int grid, const void* tmap, const TcParams& p, size_t smem, cudaStream_t s) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(kThreads);
@@ -893,6 +939,11 @@ cudaError_t tc_launch(int cta_group, int tile_n, int grid, const void* tmap, con
   cfg.numAttrs = 1;
   const CUtensorMap& tm = *reinterpret_cast<const CUtensorMap*>(tmap);
   const bool mask = p.row_mask != nullptr;
+  if (qregs != 0) {   // smem was sized without these k-blocks' tiles: only the matching kernel may run
+    if (qregs != kTcQRegs || tile_n != kTcTileWide || p.dim / kTcKBlock < qregs) return cudaErrorInvalidValue;
+    if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileWide, kTcQRegs>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileWide, kTcQRegs>(cfg, tm, p, smem);
+    return mask ? launch_variant<1, true, kTcTileWide, kTcQRegs>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileWide, kTcQRegs>(cfg, tm, p, smem);
+  }
   if (tile_n == kTcTileWide) {
     if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileWide>(cfg, tm, p, smem);
     return mask ? launch_variant<1, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileWide>(cfg, tm, p, smem);

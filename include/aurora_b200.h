@@ -99,7 +99,9 @@ int aur_open(const aur_config* cfg, aur_index** out);
 int aur_close(aur_index* ix);
 int aur_get_stats(aur_index* ix, aur_stats* out);
 /* Options: "kernel" (aur_kernel), "tc_tile" (corpus rows per tensor-core tile: 0 = auto, 64 or 128;
- * a search the 128-row layout does not fit fails); bring-up only: "dbg_flags", and "dbg_epoch" (1 .. 2^31 - 1), which
+ * a search the 128-row layout does not fit fails), "tc_stages" (cap on the tensor-core kernel's TMA ring: 0 = the
+ * deepest that fits, 2 .. 12), "tc_qregs" (query k-blocks a 128-row launch holds in registers: -1 = auto, 0 = none, or
+ * the depth the library is built with where dim / 64 reaches it); bring-up only: "dbg_flags", and "dbg_epoch" (1 .. 2^31 - 1), which
  * sets the tensor-core kernel's launch counter of every search context of the index, e.g. just before it wraps. */
 int aur_set_option(aur_index* ix, const char* key, int64_t value);
 int aur_sync(aur_index* ix);

@@ -2,7 +2,11 @@
 """Timing decomposition of simtopk_tc_kernel with the bring-up switches (dbg_flags, internal.h): same box,
 same corpus, one process -- what each part of the pipeline costs when the others are switched off.
 
-  python tools/decompose.py [n_rows] [out.json]
+  python tools/decompose.py [n_rows] [out.json] [--flags 0,1,3] [--configs tile:stages:qregs,...]
+
+--flags keeps only those dbg_flags values; --configs repeats the table under several kernel configurations
+(aur_set_option tc_tile : tc_stages : tc_qregs, default 0:0:-1 = what a search picks by itself), e.g. 128:2:0,128:3:0 for
+the slope of kernel time against ring depth.
 """
 from __future__ import annotations
 
@@ -41,9 +45,21 @@ def sm_clock():
         return None, None
 
 
+def _opt(args, name, default):
+    if name not in args:
+        return default
+    i = args.index(name)
+    v = args[i + 1]
+    del args[i:i + 2]
+    return v
+
+
 def main():
+    keep = [int(f) for f in _opt(sys.argv, "--flags", "").split(",") if f]
+    configs = [tuple(int(x) for x in c.split(":")) for c in _opt(sys.argv, "--configs", "0:0:-1").split(",")]
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 1_000_000
     out = sys.argv[2] if len(sys.argv) > 2 else "gpurun_out/decompose.json"
+    variants = [v for v in VARIANTS if not keep or v[0] in keep]
     d, nq, k = 768, 256, 32
     rng = np.random.default_rng(1002)
     block = to_bf16_bits(rng.standard_normal((50_000, d)).astype(np.float32))
@@ -56,8 +72,9 @@ def main():
         dq = DeviceBuffer(q.nbytes).upload(q)
         ds = DeviceBuffer(nq * k * 4)
         di = DeviceBuffer(nq * k * 8)
-        for flags, name in VARIANTS:
-            N.check(ix._lib.aur_set_option(ix._h, b"dbg_flags", flags))
+        for (tile, stages, qregs), (flags, name) in ((c, v) for c in configs for v in variants):
+            for key, val in ((b"tc_tile", tile), (b"tc_stages", stages), (b"tc_qregs", qregs), (b"dbg_flags", flags)):
+                N.check(ix._lib.aur_set_option(ix._h, key, val))
             for _ in range(150):                       # back to back: the clock settles where the power cap puts it
                 ix.search_dev(dq.ptr, nq, k, ds.ptr, di.ptr)
             clk, pw = sm_clock()
@@ -68,10 +85,10 @@ def main():
                 ix.search_dev(dq.ptr, nq, k, ds.ptr, di.ptr)
                 ix.sync()
                 ks.append(ix.stats()["last_kernel_ms"])
-            r = {"flags": flags, "what": name, "kernel_ms": float(np.median(ks)), "kernel_ms_min": float(np.min(ks)),
+            r = {"tc_tile": tile, "tc_stages": stages, "tc_qregs": qregs, "tile_n": ix.stats()["last_tile_n"], "flags": flags, "what": name, "kernel_ms": float(np.median(ks)), "kernel_ms_min": float(np.min(ks)),
                  "sm_mhz_under_load": clk, "power_w": pw}
             res.append(r)
-            print(f"flags {flags:3d}  {r['kernel_ms']:.4f} ms (min {r['kernel_ms_min']:.4f})  sm {clk} MHz  {pw} W   {name}", flush=True)
+            print(f"tile {tile:3d} stages {stages:2d} qregs {qregs:2d}  flags {flags:3d}  {r['kernel_ms']:.4f} ms (min {r['kernel_ms_min']:.4f})  sm {clk} MHz  {pw} W   {name}", flush=True)
     os.makedirs(os.path.dirname(out) or ".", exist_ok=True)
     json.dump({"rows": n, "dim": d, "nq": nq, "k": k, "variants": res}, open(out, "w"), indent=1)
 

@@ -4,8 +4,9 @@ the MMA warpgroup's cycles over its tile count, and how much of them it spent wa
 epilogue (tm_empty); the producer's wait for free ring stages (tp_wait); the SM clock from the globaltimer.  1M x 768
 corpus, 128 queries on CTA pairs (the bring-up entry point's largest batch).
 
-  AURORA_B200_LIB=lib_prof.so python tools/tile_cycles.py [tc_tile: 0 | 64 | 128] [n_rows]
-prints one JSON line."""
+  AURORA_B200_LIB=lib_prof.so python tools/tile_cycles.py [tc_tile: 0 | 64 | 128] [n_rows] [tc_stages] [tc_qregs]
+prints one JSON line.  tc_stages (0 = the deepest ring that fits) and tc_qregs (-1 = auto, 0 = the whole query block in
+shared memory) are set only when given, so a library without those options can be measured too."""
 import json
 import os
 import sys
@@ -34,6 +35,9 @@ def main():
         N.check(ix._lib.aur_set_option(ix._h, b"dbg_flags", 64))
         if tile:
             N.check(ix._lib.aur_set_option(ix._h, b"tc_tile", tile))
+        for key, arg in ((b"tc_stages", 3), (b"tc_qregs", 4)):
+            if len(sys.argv) > arg:
+                N.check(ix._lib.aur_set_option(ix._h, key, int(sys.argv[arg])))
         dq = DeviceBuffer(q.nbytes).upload(q)
         dout = DeviceBuffer(MAX_CTAS * Q * 64 * 4)
         for _ in range(20):
@@ -45,7 +49,8 @@ def main():
     mm, pp = out[:, 0, 32:35].astype(np.float64), out[:, 0, 36:39].astype(np.float64)
     total, full, empty = mm[:, 2].mean(), mm[:, 1].mean(), mm[:, 0].mean()
     mhz = pp[:, 1].mean() / max(pp[:, 2].mean(), 1) * 1e3
-    r = {"tile_n": tile_n, "tiles_per_cta": tiles, "mma_cycles": total, "cycles_per_tile": total / tiles,
+    r = {"tile_n": tile_n, "tc_stages": int(sys.argv[3]) if len(sys.argv) > 3 else 0,
+         "tc_qregs": int(sys.argv[4]) if len(sys.argv) > 4 else -1, "tiles_per_cta": tiles, "mma_cycles": total, "cycles_per_tile": total / tiles,
          "cycles_per_64_rows": total / tiles * 64 / tile_n, "tm_full_share": full / total, "tm_empty_share": empty / total,
          "tp_wait_share": pp[:, 0].mean() / max(pp[:, 1].mean(), 1), "sm_mhz": mhz,
          "us_per_64_rows": total / tiles * 64 / tile_n / mhz}
