@@ -29,8 +29,8 @@ EXPORTS = [
     "aur_merge_topk_dev", "aur_merge_topk_packed_dev", "aur_merge_topk_host", "aur_merge_topk_host_f64", "aur_exchange_create", "aur_exchange_connect", "aur_exchange_close",
     "aur_exchange_status", "aur_search_exchange_dev", "aur_cosine_pairs", "aur_dev_malloc", "aur_dev_free", "aur_memcpy_h2d", "aur_memcpy_d2h",
     "aur_debug_tc_scores",
-    "aur_kw_open", "aur_kw_close", "aur_kw_add", "aur_kw_remove", "aur_kw_compact", "aur_kw_get_stats", "aur_kw_search",
-    "aur_kw_search_multi", "aur_hybrid_search", "aur_hybrid_search_multi",
+    "aur_kw_open", "aur_kw_close", "aur_kw_add", "aur_kw_remove", "aur_kw_compact", "aur_kw_get_stats", "aur_kw_set_attrs",
+    "aur_kw_search", "aur_kw_search_multi", "aur_hybrid_search", "aur_hybrid_search_multi", "aur_hybrid_search_filtered",
     "aur_encoder_open", "aur_encoder_close", "aur_encoder_load", "aur_encode", "aur_encode_append",
     "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
     "aur_tokenize", "aur_encode_text_append", "aur_debug_gemm", "aur_debug_attention", "aur_debug_encoder_hidden",
@@ -136,10 +136,13 @@ def load():
         "aur_kw_remove": (C.c_int, [vp, vp, i64, C.POINTER(i64)]),
         "aur_kw_compact": (C.c_int, [vp, C.POINTER(i64)]),
         "aur_kw_get_stats": (C.c_int, [vp, C.POINTER(AurKwStats)]),
+        "aur_kw_set_attrs": (C.c_int, [vp, i32, vp, vp, i64]),
         "aur_kw_search": (C.c_int, [vp, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, C.POINTER(i64)]),
         "aur_kw_search_multi": (C.c_int, [vp, i32, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, vp]),
         "aur_hybrid_search": (C.c_int, [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]),
         "aur_hybrid_search_multi": (C.c_int, [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]),
+        "aur_hybrid_search_filtered": (C.c_int, [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, i32, vp, i64, vp, i64, vp, vp,
+                                                 i32, i32, vp, vp, vp, vp]),
         "aur_encoder_open": (C.c_int, [C.POINTER(AurEncoderConfig), C.POINTER(vp)]),
         "aur_encoder_close": (C.c_int, [vp]),
         "aur_encoder_load": (C.c_int, [vp, C.c_char_p, vp, i64]),

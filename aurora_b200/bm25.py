@@ -252,7 +252,8 @@ class DeviceBM25:
             allow_ids = [d for d in base if allow(d)]
         return self._run([query], limit, None, None, allow_ids)[0]
 
-    def search_batch(self, queries: List[str], limit: int, q_user=None, q_org=None, dense=None) -> List[list]:
+    def search_batch(self, queries: List[str], limit: int, q_user=None, q_org=None, dense=None, programs=None,
+                     q_program=None, max_list_rows: int = 0) -> List[list]:
         """All queries in one device search; ``q_user`` / ``q_org``: per-query tenant codes (row_user == u or, for
         org >= 0, row_org == o), None = unscoped.
 
@@ -260,21 +261,26 @@ class DeviceBM25:
         (``engine.hybrid_search``): the keyword leg's top-``limit`` stays in HBM and is fused there with the dense leg's
         top-``limit`` of ``vectors`` over the ``engine.Index`` ``index`` (same scopes), weights ``w_dense`` (per query)
         and ``1 - w_dense``, ``fusion`` an ``AUR_FUSION_*`` value.  Each query's list then holds its best ``k_out``
-        pairs ``(id, (fused score, dense cosine or None))``."""
+        pairs ``(id, (fused score, dense cosine or None))``.  With ``dense``, ``programs`` / ``q_program`` /
+        ``max_list_rows`` scope both legs by filter programs instead of tenant codes (``engine.hybrid_search``)."""
         if not queries:
             return []
         if dense is not None:
-            return self._run_hybrid(queries, limit, q_user, q_org, *dense)
+            return self._run_hybrid(queries, limit, q_user, q_org, *dense, programs=programs, q_program=q_program,
+                                    max_list_rows=max_list_rows)
+        if programs is not None:
+            raise ValueError("programs scope the fused hybrid query only (pass dense=...)")
         if limit <= 0 or not self._docs:
             return [[] for _ in queries]
         return self._run(queries, limit, q_user, q_org, None)
 
-    def _run_hybrid(self, queries, fetch, q_user, q_org, index, vectors, w_dense, fusion, k_out):
+    def _run_hybrid(self, queries, fetch, q_user, q_org, index, vectors, w_dense, fusion, k_out, programs=None,
+                    q_program=None, max_list_rows=0):
         from .engine import hybrid_search
 
         q_terms, q_off = query_csr(self.vocab, queries)
         ids, scores, cosine, _ = hybrid_search(index, self.store, vectors, fetch, q_terms, q_off, w_dense, None, fusion,
-                                               k_out, q_user, q_org)
+                                               k_out, q_user, q_org, programs, q_program, max_list_rows)
         out = []
         for row_i, row_s, row_c in zip(ids, scores, cosine):
             n = int((row_i >= 0).sum())

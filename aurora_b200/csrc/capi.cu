@@ -126,7 +126,10 @@ struct SearchCtx {
   DevBuf<uint32_t> filt_counts;  // filtered search: [32] totals, then [n_programs][blocks] counts (scanned into offsets)
   DevBuf<int32_t> filt_rows;     // filtered search: every program's matching rows, ascending, program after program
   DevBuf<int64_t> filt_ids;      // aur_filter_ids: their ids
+  uint32_t* h_totals = nullptr;  // page-locked landing area of the count pass's totals (kFiltCallPrograms words)
   void release() {
+    if (h_totals) cudaFreeHost(h_totals);
+    h_totals = nullptr;
     cand_a.release(); cand_b.release(); pub.release(); cand_count.release(); d_epoch.release(); cand_read.release(); score_chunk.release(); masked_inv.release();
     allow_rows.release(); row_mask.release(); scope_tab.release(); q_scope.release(); stage_q.release(); stage_quser.release(); stage_qorg.release(); stage_scores.release();
     stage_ids.release(); list_stage.release(); list_scores.release();
@@ -860,17 +863,19 @@ FiltPass filt_pass(SearchCtx* c, int ps, int n_programs, int64_t n_rows) {
 }
 
 // Uploads checked programs, evaluates them over the snapshot's rows [0, n_rows) in passes of up to 32 programs (masks
-// and counts in c->filt_mask / c->filt_counts, filt_pass) and reads back each program's number of matching rows (one
-// small copy and a sync for all passes).
-int filter_count(aur_index* ix, SearchCtx* c, cudaStream_t s, const int32_t* prog, const int32_t* prog_off, int32_t n_programs,
-                 const uint32_t* bitmap, int64_t bitmap_words, int64_t n_rows, std::vector<int64_t>* totals) {
-  const size_t n_tok = static_cast<size_t>(prog_off[n_programs]);
-  std::vector<int32_t> st(n_tok * 4 + static_cast<size_t>(n_programs) + 1 + static_cast<size_t>(bitmap_words));
-  if (n_tok) memcpy(st.data(), prog, n_tok * 16);
-  memcpy(st.data() + n_tok * 4, prog_off, (static_cast<size_t>(n_programs) + 1) * 4);
-  if (bitmap_words) memcpy(st.data() + n_tok * 4 + n_programs + 1, bitmap, static_cast<size_t>(bitmap_words) * 4);
+// and counts in c->filt_mask / c->filt_counts, filt_pass) and enqueues the read-back of each program's number of
+// matching rows into c->h_totals (one small copy for all passes).  Nothing waits: filter_totals reads them once the
+// stream is idle.
+int filter_count(aur_index* ix, SearchCtx* c, cudaStream_t s, const FiltProgs& fp, int64_t n_rows) {
+  const int32_t n_programs = fp.n_programs;
+  const size_t n_tok = static_cast<size_t>(fp.prog_off[n_programs]);
+  std::vector<int32_t> st(n_tok * 4 + static_cast<size_t>(n_programs) + 1 + static_cast<size_t>(fp.bitmap_words));
+  if (n_tok) memcpy(st.data(), fp.prog, n_tok * 16);
+  memcpy(st.data() + n_tok * 4, fp.prog_off, (static_cast<size_t>(n_programs) + 1) * 4);
+  if (fp.bitmap_words) memcpy(st.data() + n_tok * 4 + n_programs + 1, fp.bitmap, static_cast<size_t>(fp.bitmap_words) * 4);
   const int n_passes = (n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms;
   const size_t nb = static_cast<size_t>(std::max(filter_blocks(n_rows), 1));
+  if (!c->h_totals) CU_TRY(cudaHostAlloc(reinterpret_cast<void**>(&c->h_totals), kFiltCallPrograms * 4, cudaHostAllocPortable));
   CU_TRY(c->filt_stage.reserve(st.size()));
   CU_TRY(c->filt_mask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
   CU_TRY(c->filt_counts.reserve(static_cast<size_t>(n_passes) * kFiltMaxPrograms * (1 + nb)));
@@ -887,17 +892,21 @@ int filter_count(aur_index* ix, SearchCtx* c, cudaStream_t s, const int32_t* pro
   p.inv_norm = ix->d_inv_norm;
   p.n_rows = n_rows;
   for (int ps = 0; ps < n_passes; ++ps) {
-    const FiltPass fp = filt_pass(c, ps, n_programs, n_rows);
+    const FiltPass pass = filt_pass(c, ps, n_programs, n_rows);
     p.prog_off = d_off + ps * kFiltMaxPrograms;
-    p.n_programs = fp.n_programs;
-    CU_TRY(launch_filter_count(p, fp.mask, fp.counts, fp.totals, s));
+    p.n_programs = pass.n_programs;
+    CU_TRY(launch_filter_count(p, pass.mask, pass.counts, pass.totals, s));
     ++c->last_launches;
   }
-  std::vector<uint32_t> h(static_cast<size_t>(n_passes) * kFiltMaxPrograms);
-  CU_TRY(cudaMemcpyAsync(h.data(), c->filt_counts.p, h.size() * 4, cudaMemcpyDeviceToHost, s));
-  CU_TRY(cudaStreamSynchronize(s));
-  totals->assign(h.begin(), h.begin() + n_programs);   // pass ps's totals are words 32 ps .. 32 ps + 31: program order
+  CU_TRY(cudaMemcpyAsync(c->h_totals, c->filt_counts.p, static_cast<size_t>(n_passes) * kFiltMaxPrograms * 4,
+                         cudaMemcpyDeviceToHost, s));
   return AUR_OK;
+}
+
+// After filter_count, with the stream idle: every program's number of matching rows (pass ps's totals are words
+// 32 ps .. 32 ps + 31: program order).
+void filter_totals(const SearchCtx* c, int32_t n_programs, std::vector<int64_t>* totals) {
+  totals->assign(c->h_totals, c->h_totals + n_programs);
 }
 
 // After filter_count: every program's matching rows, ascending, program after program, into c->filt_rows (and with
@@ -918,6 +927,27 @@ int filter_write(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t n_programs
     for (int q = 0; q < fp.n_programs; ++q) base += tot[static_cast<size_t>(ps * kFiltMaxPrograms + q)];
   }
   return AUR_OK;
+}
+
+// After filter_count and its totals: the search of the queries in c->stage_q under the programs, into scores / ids.  One
+// program matching more than max_list_rows rows runs the masked scan of aur_search_subset, anything else the list kernels.
+int filtered_search(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t nq, int32_t k, const FiltProgs& fp,
+                    const std::vector<int64_t>& tot, int64_t max_list_rows, int64_t n_rows, float* scores, int64_t* ids) {
+  if (fp.n_programs == 1 && tot[0] > max_list_rows) {
+    // dense: the matching rows as a row mask, and the masked scan aur_search_subset runs
+    Scope sc;
+    sc.match_mask = c->filt_mask.p;
+    return search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, scores, ids, nullptr, s);
+  }
+  // lists: every program's rows written on the device, in the order the host path stages them; items from the lengths
+  std::vector<int64_t> lrow0(static_cast<size_t>(fp.n_programs), 0);
+  for (int32_t q = 1; q < fp.n_programs; ++q)
+    lrow0[static_cast<size_t>(q)] = lrow0[static_cast<size_t>(q - 1)] + tot[static_cast<size_t>(q - 1)];
+  int rc = filter_write(ix, c, s, fp.n_programs, tot, n_rows, false);
+  if (rc != AUR_OK) return rc;
+  ListPlan pl;
+  if ((rc = plan_list_search(nq, k, fp.q_program, lrow0, tot, &pl)) != AUR_OK) return rc;
+  return run_list_search(ix, c, s, pl, nq, k, c->filt_rows.p, scores, ids);
 }
 
 }  // namespace
@@ -950,6 +980,64 @@ int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_hos
 
 int index_device(const aur_index* ix) { return ix->device; }
 int index_is_bf16(const aur_index* ix) { return ix->dtype == AUR_BF16; }
+
+int filter_check(aur_index* ix, const FiltProgs& fp) {
+  return check_programs(ix, fp.prog, fp.prog_off, fp.n_programs, fp.bitmap, fp.bitmap_words);
+}
+
+int filtered_legs(aur_index* const* shards, int n, const void* queries_host, int32_t nq, int32_t k, const FiltProgs& fp,
+                  int64_t max_list_rows, const DenseLegsThen& then, float* scores_host, int64_t* ids_host) {
+  struct Part { std::unique_ptr<HostCall> call; std::vector<int64_t> tot; };
+  std::vector<Part> parts(static_cast<size_t>(n));
+  // every stream drains before its context goes back to the pool (also on an error): declared after `parts`, so it
+  // runs before their destructors
+  struct Drain {
+    std::vector<Part>& v;
+    ~Drain() {
+      for (Part& p : v)
+        if (p.call && p.call->c) { cudaSetDevice(p.call->ix->device); cudaStreamSynchronize(p.call->s); }
+    }
+  } drain{parts};
+  // shared locks in one order (by address), as the keyword legs take theirs
+  std::vector<int> order(static_cast<size_t>(n));
+  for (int s = 0; s < n; ++s) order[static_cast<size_t>(s)] = s;
+  std::sort(order.begin(), order.end(), [&](int a, int b) { return std::less<aur_index*>()(shards[a], shards[b]); });
+  for (int s : order) parts[static_cast<size_t>(s)].call.reset(new HostCall(shards[s]));
+  const size_t nout = static_cast<size_t>(nq) * k;
+  int rc = AUR_OK;
+  // every shard's queries and count pass, then one wait for all the counts
+  for (Part& pt : parts) {
+    HostCall& call = *pt.call;
+    if ((rc = call.open()) != AUR_OK) return rc;
+    SearchCtx* c = call.c;
+    const size_t qbytes = static_cast<size_t>(nq) * call.ix->dim * call.ix->elt;
+    CU_TRY(c->stage_q.reserve(qbytes));
+    CU_TRY(c->stage_scores.reserve(nout));
+    CU_TRY(c->stage_ids.reserve(nout));
+    CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, call.s));
+    call.d_scores = c->stage_scores.p;
+    call.d_ids = c->stage_ids.p;
+    if (n == 1 && scores_host && ids_host) call.direct = direct_outputs(scores_host, ids_host, &call.d_scores, &call.d_ids);
+    if ((rc = stats_begin(c, call.s, nq, call.n_rows)) != AUR_OK) return rc;
+    if ((rc = filter_count(call.ix, c, call.s, fp, call.n_rows)) != AUR_OK) return rc;
+  }
+  for (Part& pt : parts) {
+    CU_TRY(cudaSetDevice(pt.call->ix->device));
+    CU_TRY(cudaStreamSynchronize(pt.call->s));
+    filter_totals(pt.call->c, fp.n_programs, &pt.tot);
+  }
+  std::vector<DenseLeg> legs;
+  for (Part& pt : parts) {
+    HostCall& call = *pt.call;
+    SearchCtx* c = call.c;
+    CU_TRY(cudaSetDevice(call.ix->device));
+    rc = filtered_search(call.ix, c, call.s, nq, k, fp, pt.tot, max_list_rows, call.n_rows, call.d_scores, call.d_ids);
+    if (rc == AUR_OK) rc = stats_end(call.ix, c, call.s);
+    if (rc != AUR_OK) return rc;
+    legs.push_back(DenseLeg{call.ix->device, call.s, call.d_scores, call.d_ids, call.n_rows, &pt.tot, call.direct});
+  }
+  return then(legs);
+}
 }  // namespace aur
 
 extern "C" {
@@ -1372,37 +1460,20 @@ int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int
   for (int32_t q = 0; q < nq; ++q)
     if (q_program[q] < 0 || q_program[q] >= n_programs) return fail(AUR_ERR_INVALID, "q_program[%d] = %d is not a program", q, q_program[q]);
   if (max_list_rows < 0) return fail(AUR_ERR_INVALID, "max_list_rows < 0");
-
-  HostCall call(ix);
-  if ((rc = call.open()) != AUR_OK) return rc;
-  SearchCtx* c = call.c;
-  cudaStream_t s = call.s;
-  const int64_t n_rows = call.n_rows;
-  if ((rc = stats_begin(c, s, nq, n_rows)) != AUR_OK) return rc;
-  std::vector<int64_t> tot;
-  if ((rc = filter_count(ix, c, s, prog, prog_offsets, n_programs, bitmap, bitmap_words, n_rows, &tot)) != AUR_OK) return rc;
-  if (n_programs == 1 && tot[0] > max_list_rows) {
-    // dense: the matching rows as a row mask, and the masked scan aur_search_subset runs
-    Scope sc;
-    sc.match_mask = c->filt_mask.p;
-    rc = call.stage(queries_host, nq, k, scores_out, ids_out);
-    if (rc == AUR_OK) rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, call.d_scores, call.d_ids, nullptr, s);
-  } else {
-    // lists: every program's rows written on the device, in the order the host path stages them; items from the lengths
-    std::vector<int64_t> lrow0(static_cast<size_t>(n_programs), 0);
-    for (int32_t q = 1; q < n_programs; ++q)
-      lrow0[static_cast<size_t>(q)] = lrow0[static_cast<size_t>(q - 1)] + tot[static_cast<size_t>(q - 1)];
-    if ((rc = filter_write(ix, c, s, n_programs, tot, n_rows, false)) != AUR_OK) return rc;
-    ListPlan pl;
-    rc = plan_list_search(nq, k, q_program, lrow0, tot, &pl);
-    if (rc == AUR_OK) rc = call.stage(queries_host, nq, k, scores_out, ids_out);
-    if (rc == AUR_OK) rc = run_list_search(ix, c, s, pl, nq, k, c->filt_rows.p, call.d_scores, call.d_ids);
-  }
-  if (rc == AUR_OK) rc = stats_end(ix, c, s);
-  if ((rc = call.finish(rc, nq, k, scores_out, ids_out)) != AUR_OK) return rc;
-  if (matched_out) for (int32_t q = 0; q < n_programs; ++q) matched_out[q] = tot[static_cast<size_t>(q)];
-  if (snapshot_rows_out) *snapshot_rows_out = n_rows;
-  return AUR_OK;
+  const FiltProgs fp{prog, prog_offsets, n_programs, bitmap, bitmap_words, q_program};
+  return filtered_legs(&ix, 1, queries_host, nq, k, fp, max_list_rows, [&](const std::vector<DenseLeg>& legs) -> int {
+    const DenseLeg& l = legs[0];
+    const size_t nout = static_cast<size_t>(nq) * k;
+    // (reached only when every kernel of the search was enqueued: on any failure the pageable outputs stay untouched)
+    if (!l.direct) {   // page-locked outputs were written by the re-rank kernel itself
+      CU_TRY(cudaMemcpyAsync(scores_out, l.scores, nout * 4, cudaMemcpyDeviceToHost, l.stream));
+      CU_TRY(cudaMemcpyAsync(ids_out, l.ids, nout * 8, cudaMemcpyDeviceToHost, l.stream));
+    }
+    CU_TRY(cudaStreamSynchronize(l.stream));
+    if (matched_out) for (int32_t q = 0; q < n_programs; ++q) matched_out[q] = (*l.matched)[static_cast<size_t>(q)];
+    if (snapshot_rows_out) *snapshot_rows_out = l.snapshot_rows;
+    return AUR_OK;
+  }, scores_out, ids_out);
 }
 
 int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,
@@ -1417,7 +1488,9 @@ int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const u
   SearchCtx* c = call.c;
   cudaStream_t s = call.s;
   std::vector<int64_t> tot;
-  if ((rc = filter_count(ix, c, s, prog, off, 1, bitmap, bitmap_words, call.n_rows, &tot)) != AUR_OK) return rc;
+  if ((rc = filter_count(ix, c, s, FiltProgs{prog, off, 1, bitmap, bitmap_words, nullptr}, call.n_rows)) != AUR_OK) return rc;
+  CU_TRY(cudaStreamSynchronize(s));
+  filter_totals(c, 1, &tot);
   const int64_t n = tot[0], m = std::min(n, cap);
   if ((rc = filter_write(ix, c, s, 1, tot, call.n_rows, true)) != AUR_OK) return rc;
   std::vector<int64_t> got(static_cast<size_t>(m));

@@ -1,10 +1,12 @@
-// Metadata pre-filters evaluated on the device (aur_search_filtered, aur_filter_ids).
+// Metadata pre-filters evaluated on the device (aur_search_filtered, aur_filter_ids, aur_hybrid_search_filtered).
 //
 // A program is a postfix sequence of leaves and AND / OR tokens (FiltToken).  A leaf (column, bitmap offset, bitmap length)
 // is true for a row when bit code + 1 of its bitmap slice is set, code being the row's int32 value in that column (-1 =
-// property absent).  Columns 0 / 1 are the shard's tenant codes, 2.. its attribute columns.  Three kernels:
+// property absent).  Columns 0 / 1 are the shard's (or keyword store's) tenant codes, 2.. its attribute columns.  Three
+// kernels:
 //   filter_count_kernel  one pass over the snapshot's rows: every live row's match bits (bit p = program p, up to 32
-//                        programs) into a per-row mask, per-block counts per program and the per-program totals;
+//                        programs) into a per-row mask, per-block counts per program and the per-program totals; over a
+//                        keyword store's rows (the hybrid query's keyword leg) the mask alone;
 //   filter_scan_kernel   exclusive scan of each program's block counts, offset by the programs before it;
 //   filter_write_kernel  each program's matching rows in ascending row order (and optionally their ids) into one buffer:
 //                        the rows the host path stages after its sort and unique.
@@ -46,9 +48,20 @@ __device__ __forceinline__ uint32_t row_match(const FiltParams& p, int64_t row) 
   return m;
 }
 
+// kMaskOnly: a keyword store's rows (liveness from p.live), the mask alone -- its consumer is a kernel, so nothing is
+// counted for the host.  Otherwise a vector shard's rows (liveness from p.inv_norm), mask and counts.
+template <bool kMaskOnly>
 __global__ void __launch_bounds__(kFiltThreads) filter_count_kernel(FiltParams p, uint32_t* __restrict__ mask,
                                                                     uint32_t* __restrict__ block_counts,
                                                                     uint32_t* __restrict__ totals, int n_blocks) {
+  if constexpr (kMaskOnly) {
+    const int64_t base = static_cast<int64_t>(blockIdx.x) * kFiltBlockRows;
+    for (int it = 0; it < kFiltBlockRows / kFiltThreads; ++it) {
+      const int64_t row = base + it * kFiltThreads + threadIdx.x;
+      if (row < p.n_rows) mask[row] = __ldg(p.live + row) ? row_match(p, row) : 0u;
+    }
+    return;
+  }
   __shared__ uint32_t s_cnt[32];
   if (threadIdx.x < 32) s_cnt[threadIdx.x] = 0u;
   __syncthreads();
@@ -182,7 +195,14 @@ cudaError_t launch_filter_count(const FiltParams& p, uint32_t* mask, uint32_t* b
   cudaError_t e = cudaMemsetAsync(totals, 0, 32 * sizeof(uint32_t), s);
   if (e != cudaSuccess || p.n_rows <= 0) return e;
   const int nb = filter_blocks(p.n_rows);
-  filter_count_kernel<<<nb, kFiltThreads, 0, s>>>(p, mask, block_counts, totals, nb);
+  filter_count_kernel<false><<<nb, kFiltThreads, 0, s>>>(p, mask, block_counts, totals, nb);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_filter_mask(const FiltParams& p, uint32_t* mask, cudaStream_t s) {
+  if (p.n_rows <= 0) return cudaSuccess;
+  const int nb = filter_blocks(p.n_rows);
+  filter_count_kernel<true><<<nb, kFiltThreads, 0, s>>>(p, mask, nullptr, nullptr, nb);
   return cudaGetLastError();
 }
 

@@ -319,10 +319,62 @@ struct HybridArgs {
   const int32_t* q_user; const int32_t* q_org;
   std::vector<double> w;   // [nq][2]
   int32_t fusion, k_out;
+  const FiltProgs* fp;     // nullable: every query's scope as a program (aur_hybrid_search_filtered)
+  int64_t max_list_rows;   // with fp: the dense legs' list-vs-scan bound, an even share per shard
 };
 
-// Inside the keyword legs: every shard's dense leg, the join and gather on shard 0's device, the merge + fusion and the
-// copy into hs[0]->host.  hs[s] is on shard s's device; rows[s] receives shard s's snapshot.
+// One shard's dense list [nq][fetch] on its device, valid once `stream` reaches it.
+struct DenseList { cudaStream_t stream; const float* cos; const int64_t* ids; };
+
+// The join on shard 0's device (every keyword leg, every dense leg not on its stream), the gather of the other shards'
+// lists, the merge + fusion and the copy into hs[0]->host.  Shard 0's buffers were prepared by run_on_devices.
+int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const std::vector<KwLeg>& kl,
+                  const std::vector<DenseList>& dl) {
+  const int n = a.n;
+  const size_t nl = static_cast<size_t>(a.nq) * a.fetch, no = static_cast<size_t>(a.nq) * a.k_out;
+  HybridCtx* h = hs[0];
+  cudaStream_t st = h->stream;
+  for (int s = 0; s < n; ++s) {
+    HybridCtx* o = hs[static_cast<size_t>(s)];
+    HYB_TRY(cudaSetDevice(o->device));
+    if (dl[static_cast<size_t>(s)].stream != st) HYB_TRY(cudaEventRecord(o->dense_done, dl[static_cast<size_t>(s)].stream));
+    HYB_TRY(cudaEventRecord(o->kw_done, kl[static_cast<size_t>(s)].stream));   // the store shares the shard's device
+  }
+  HYB_TRY(cudaSetDevice(h->device));
+  // their lists come over by peer copies (also between shards of one device, so that every shard count runs the same code)
+  for (int s = 0; s < n; ++s) {
+    const HybridCtx* o = hs[static_cast<size_t>(s)];
+    const KwLeg& k = kl[static_cast<size_t>(s)];
+    const DenseList& d = dl[static_cast<size_t>(s)];
+    HYB_TRY(cudaStreamWaitEvent(st, o->kw_done, 0));
+    if (d.stream != st) HYB_TRY(cudaStreamWaitEvent(st, o->dense_done, 0));
+    if (s == 0) continue;
+    const size_t at = static_cast<size_t>(s - 1) * nl;
+    HYB_TRY(cudaMemcpyPeerAsync(h->g_cos.p + at, h->device, d.cos, o->device, nl * 4, st));
+    HYB_TRY(cudaMemcpyPeerAsync(h->g_did.p + at, h->device, d.ids, o->device, nl * 8, st));
+    HYB_TRY(cudaMemcpyPeerAsync(h->g_ks.p + at, h->device, k.scores, k.device, nl * 8, st));
+    HYB_TRY(cudaMemcpyPeerAsync(h->g_kid.p + at, h->device, k.ids, k.device, nl * 8, st));
+  }
+  FuseParams p;
+  p.dense = LegLists{dl[0].ids, dl[0].cos, h->g_did.p, h->g_cos.p, h->run_max.p};
+  p.kw = LegLists{kl[0].ids, kl[0].scores, h->g_kid.p, h->g_ks.p, n > 1 ? h->run_max.p + static_cast<size_t>(n) * nl : nullptr};
+  p.w = h->w.p;
+  p.n = n; p.nq = a.nq; p.fetch = a.fetch; p.k_out = a.k_out; p.fusion = a.fusion;
+  p.sort_n = 2;
+  while (p.sort_n < 2 * a.fetch) p.sort_n <<= 1;
+  p.o_s = reinterpret_cast<double*>(h->out.p);
+  p.o_i = reinterpret_cast<int64_t*>(h->out.p + no * 8);
+  p.o_c = reinterpret_cast<float*>(h->out.p + no * 16);
+  hybrid_merge_fuse_kernel<<<static_cast<unsigned>(a.nq), kFuseThreads, 0, st>>>(p);
+  HYB_TRY(cudaGetLastError());
+  HYB_TRY(cudaMemcpyAsync(h->host, h->out.p, no * kOutBytes, cudaMemcpyDeviceToHost, st));
+  HYB_TRY(cudaStreamSynchronize(st));
+  return AUR_OK;
+}
+
+// Inside the keyword legs: shard 0's device takes the weights and the output space, every shard's dense leg is enqueued
+// (aur_search_ex's search on the shard's hybrid context, or with programs aur_search_filtered's on a pooled search
+// context: filtered_legs), then join_and_fuse.  hs[s] is on shard s's device; rows[s] receives shard s's snapshot.
 int run_on_devices(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const std::vector<KwLeg>& kl, int64_t* rows) {
   const int n = a.n;
   const size_t nl = static_cast<size_t>(a.nq) * a.fetch, no = static_cast<size_t>(a.nq) * a.k_out;
@@ -347,6 +399,19 @@ int run_on_devices(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const
   }
   HYB_TRY(cudaMemcpyAsync(h->w.p, a.w.data(), a.w.size() * 8, cudaMemcpyHostToDevice, st));
   // (pageable: staged before the call returns; behind the dense legs it would wait for their kernels)
+  if (a.fp) {
+    return filtered_legs(a.shards, n, a.queries_host, a.nq, a.fetch, *a.fp, a.max_list_rows / n,
+                         [&](const std::vector<DenseLeg>& legs) -> int {
+                           std::vector<DenseList> dl;
+                           for (int s = 0; s < n; ++s) {
+                             const DenseLeg& l = legs[static_cast<size_t>(s)];
+                             rows[s] = l.snapshot_rows;
+                             dl.push_back(DenseList{l.stream, l.scores, l.ids});
+                           }
+                           return join_and_fuse(a, hs, kl, dl);
+                         });
+  }
+  std::vector<DenseList> dl;
   for (int s = 0; s < n; ++s) {
     HybridCtx* o = hs[static_cast<size_t>(s)];
     HYB_TRY(cudaSetDevice(o->device));
@@ -355,39 +420,9 @@ int run_on_devices(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const
     const int rc = dense_leg(a.shards[s], o->device, o->stream, a.queries_host, a.nq, a.fetch, a.q_user, a.q_org, o->cos.p,
                              o->ids.p, &rows[s]);
     if (rc != AUR_OK) return rc;
-    if (s > 0) HYB_TRY(cudaEventRecord(o->dense_done, o->stream));
-    HYB_TRY(cudaEventRecord(o->kw_done, kl[static_cast<size_t>(s)].stream));   // the store shares the shard's device
+    dl.push_back(DenseList{o->stream, o->cos.p, o->ids.p});
   }
-  HYB_TRY(cudaSetDevice(h->device));
-  // the join: every keyword leg, every other shard's dense leg; their lists come over by peer copies (also between
-  // shards of one device, so that every shard count runs the same code)
-  for (int s = 0; s < n; ++s) {
-    const HybridCtx* o = hs[static_cast<size_t>(s)];
-    const KwLeg& k = kl[static_cast<size_t>(s)];
-    HYB_TRY(cudaStreamWaitEvent(st, o->kw_done, 0));
-    if (s == 0) continue;
-    HYB_TRY(cudaStreamWaitEvent(st, o->dense_done, 0));
-    const size_t at = static_cast<size_t>(s - 1) * nl;
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_cos.p + at, h->device, o->cos.p, o->device, nl * 4, st));
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_did.p + at, h->device, o->ids.p, o->device, nl * 8, st));
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_ks.p + at, h->device, k.scores, k.device, nl * 8, st));
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_kid.p + at, h->device, k.ids, k.device, nl * 8, st));
-  }
-  FuseParams p;
-  p.dense = LegLists{h->ids.p, h->cos.p, h->g_did.p, h->g_cos.p, h->run_max.p};
-  p.kw = LegLists{kl[0].ids, kl[0].scores, h->g_kid.p, h->g_ks.p, n > 1 ? h->run_max.p + static_cast<size_t>(n) * nl : nullptr};
-  p.w = h->w.p;
-  p.n = n; p.nq = a.nq; p.fetch = a.fetch; p.k_out = a.k_out; p.fusion = a.fusion;
-  p.sort_n = 2;
-  while (p.sort_n < 2 * a.fetch) p.sort_n <<= 1;
-  p.o_s = reinterpret_cast<double*>(h->out.p);
-  p.o_i = reinterpret_cast<int64_t*>(h->out.p + no * 8);
-  p.o_c = reinterpret_cast<float*>(h->out.p + no * 16);
-  hybrid_merge_fuse_kernel<<<static_cast<unsigned>(a.nq), kFuseThreads, 0, st>>>(p);
-  HYB_TRY(cudaGetLastError());
-  HYB_TRY(cudaMemcpyAsync(h->host, h->out.p, no * kOutBytes, cudaMemcpyDeviceToHost, st));
-  HYB_TRY(cudaStreamSynchronize(st));
-  return AUR_OK;
+  return join_and_fuse(a, hs, kl, dl);
 }
 
 template <typename T>
@@ -397,18 +432,21 @@ bool has_repeat(T* const* v, int n) {
   return std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end();
 }
 
-// Both entry points: arguments already checked up to the handle lists (non-NULL, distinct, 1 <= n <= kMaxLists).
+// Every entry point: arguments already checked up to the handle lists (non-NULL, distinct, 1 <= n <= kMaxLists).
+// fp (nullable): the queries' programs (q_user / q_org are then NULL), max_list_rows their dense legs' bound.
 int hybrid_search(aur_index* const* shards, aur_kw* const* stores, int32_t n, const void* queries_host, int32_t nq,
                   int32_t fetch, const int32_t* q_terms, const int64_t* q_offsets, const int32_t* q_user,
-                  const int32_t* q_org, const double* w_dense, const double* w_sparse, int32_t fusion, int32_t k_out,
-                  double* scores_out, int64_t* ids_out, float* cosine_out, int64_t* snapshot_rows_out) {
+                  const int32_t* q_org, const FiltProgs* fp, int64_t max_list_rows, const double* w_dense,
+                  const double* w_sparse, int32_t fusion, int32_t k_out, double* scores_out, int64_t* ids_out,
+                  float* cosine_out, int64_t* snapshot_rows_out) {
   if (nq <= 0) return report_error(AUR_ERR_INVALID, "nq must be positive");
   if (nq > 65535) return report_error(AUR_ERR_UNSUPPORTED, "nq > 65535: split the batch");
   if (fetch < 1) return report_error(AUR_ERR_INVALID, "fetch must be positive");
   if (fetch > kMaxK) return report_error(AUR_ERR_UNSUPPORTED, "fetch > %d", kMaxK);
   if (k_out < 1 || k_out > 2 * fetch) return report_error(AUR_ERR_INVALID, "k_out must be in 1 .. 2 * fetch (%d)", 2 * fetch);
   if (fusion != AUR_FUSION_RANKED && fusion != AUR_FUSION_RELATIVE_SCORE) return report_error(AUR_ERR_INVALID, "unknown fusion %d", fusion);
-  HybridArgs a{shards, n, queries_host, nq, fetch, q_user, q_org, std::vector<double>(2 * static_cast<size_t>(nq)), fusion, k_out};
+  HybridArgs a{shards, n, queries_host, nq, fetch, q_user, q_org, std::vector<double>(2 * static_cast<size_t>(nq)), fusion, k_out,
+               fp, max_list_rows};
   for (int32_t i = 0; i < nq; ++i) {
     if (!std::isfinite(w_dense[i]) || !std::isfinite(w_sparse[i])) return report_error(AUR_ERR_INVALID, "weights must be finite (query %d)", i);
     a.w[2 * static_cast<size_t>(i)] = w_dense[i];
@@ -422,9 +460,20 @@ int hybrid_search(aur_index* const* shards, aur_kw* const* stores, int32_t n, co
       return report_error(AUR_ERR_INVALID, "keyword store %d is on device %d, its shard on device %d", s, kw_device(stores[s]),
                           index_device(shards[s]));
   }
+  if (fp) {   // every shard and every store must hold every column the programs name
+    for (int s = 0; s < n; ++s) {
+      if ((rc = filter_check(shards[s], *fp)) != AUR_OK) return rc;
+      if ((rc = kw_check_columns(stores[s], *fp)) != AUR_OK) return rc;
+    }
+    if (!fp->q_program) return report_error(AUR_ERR_INVALID, "q_program is required");
+    for (int32_t q = 0; q < nq; ++q)
+      if (fp->q_program[q] < 0 || fp->q_program[q] >= fp->n_programs)
+        return report_error(AUR_ERR_INVALID, "q_program[%d] = %d is not a program", q, fp->q_program[q]);
+    if (max_list_rows < 0) return report_error(AUR_ERR_INVALID, "max_list_rows < 0");
+  }
   std::vector<HybridCtx*> hs;
   std::vector<int64_t> rows(2 * static_cast<size_t>(n), 0);
-  rc = kw_legs(stores, n, q_terms, q_offsets, nq, fetch, q_user, q_org, [&](const std::vector<KwLeg>& kl) {
+  rc = kw_legs(stores, n, q_terms, q_offsets, nq, fetch, q_user, q_org, fp, [&](const std::vector<KwLeg>& kl) {
     int r = AUR_OK;
     for (int s = 0; s < n && r == AUR_OK; ++s) {
       HybridCtx* h = nullptr;
@@ -446,6 +495,16 @@ int hybrid_search(aur_index* const* shards, aur_kw* const* stores, int32_t n, co
   return rc;
 }
 
+// The handle checks of the multi-shard entry points.
+int check_handles(aur_index* const* shards, aur_kw* const* stores, int32_t n) {
+  if (n < 1 || n > kMaxLists) return report_error(AUR_ERR_INVALID, "n must be in 1 .. %d", kMaxLists);
+  for (int32_t s = 0; s < n; ++s)
+    if (!shards[s] || !stores[s]) return report_error(AUR_ERR_INVALID, "shard or store %d is NULL", s);
+  if (has_repeat(shards, n)) return report_error(AUR_ERR_INVALID, "a shard is listed twice");
+  if (has_repeat(stores, n)) return report_error(AUR_ERR_INVALID, "a keyword store is listed twice (its statistics would count double)");
+  return AUR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -456,8 +515,8 @@ int aur_hybrid_search(aur_index* ix, aur_kw* kw, const void* queries_host, int32
                       float* cosine_out, int64_t* snapshot_rows_out) {
   if (!ix || !kw || !queries_host || !q_offsets || !w_dense || !w_sparse || !scores_out || !ids_out || !cosine_out)
     return report_error(AUR_ERR_INVALID, "null argument");
-  return hybrid_search(&ix, &kw, 1, queries_host, nq, fetch, q_terms, q_offsets, q_user, q_org, w_dense, w_sparse, fusion,
-                       k_out, scores_out, ids_out, cosine_out, snapshot_rows_out);
+  return hybrid_search(&ix, &kw, 1, queries_host, nq, fetch, q_terms, q_offsets, q_user, q_org, nullptr, 0, w_dense, w_sparse,
+                       fusion, k_out, scores_out, ids_out, cosine_out, snapshot_rows_out);
 }
 
 int aur_hybrid_search_multi(aur_index* const* shards, aur_kw* const* stores, int32_t n, const void* queries_host, int32_t nq,
@@ -467,13 +526,25 @@ int aur_hybrid_search_multi(aur_index* const* shards, aur_kw* const* stores, int
                             int64_t* snapshot_rows_out) {
   if (!shards || !stores || !queries_host || !q_offsets || !w_dense || !w_sparse || !scores_out || !ids_out || !cosine_out)
     return report_error(AUR_ERR_INVALID, "null argument");
-  if (n < 1 || n > kMaxLists) return report_error(AUR_ERR_INVALID, "n must be in 1 .. %d", kMaxLists);
-  for (int32_t s = 0; s < n; ++s)
-    if (!shards[s] || !stores[s]) return report_error(AUR_ERR_INVALID, "shard or store %d is NULL", s);
-  if (has_repeat(shards, n)) return report_error(AUR_ERR_INVALID, "a shard is listed twice");
-  if (has_repeat(stores, n)) return report_error(AUR_ERR_INVALID, "a keyword store is listed twice (its statistics would count double)");
-  return hybrid_search(shards, stores, n, queries_host, nq, fetch, q_terms, q_offsets, q_user, q_org, w_dense, w_sparse, fusion,
-                       k_out, scores_out, ids_out, cosine_out, snapshot_rows_out);
+  const int rc = check_handles(shards, stores, n);
+  if (rc != AUR_OK) return rc;
+  return hybrid_search(shards, stores, n, queries_host, nq, fetch, q_terms, q_offsets, q_user, q_org, nullptr, 0, w_dense,
+                       w_sparse, fusion, k_out, scores_out, ids_out, cosine_out, snapshot_rows_out);
+}
+
+int aur_hybrid_search_filtered(aur_index* const* shards, aur_kw* const* stores, int32_t n, const void* queries_host,
+                               int32_t nq, int32_t fetch, const int32_t* q_terms, const int64_t* q_offsets,
+                               const int32_t* prog, const int32_t* prog_offsets, int32_t n_programs, const uint32_t* bitmap,
+                               int64_t bitmap_words, const int32_t* q_program, int64_t max_list_rows,
+                               const double* w_dense, const double* w_sparse, int32_t fusion, int32_t k_out,
+                               double* scores_out, int64_t* ids_out, float* cosine_out, int64_t* snapshot_rows_out) {
+  if (!shards || !stores || !queries_host || !q_offsets || !w_dense || !w_sparse || !scores_out || !ids_out || !cosine_out)
+    return report_error(AUR_ERR_INVALID, "null argument");
+  const int rc = check_handles(shards, stores, n);
+  if (rc != AUR_OK) return rc;
+  const FiltProgs fp{prog, prog_offsets, n_programs, bitmap, bitmap_words, q_program};
+  return hybrid_search(shards, stores, n, queries_host, nq, fetch, q_terms, q_offsets, nullptr, nullptr, &fp, max_list_rows,
+                       w_dense, w_sparse, fusion, k_out, scores_out, ids_out, cosine_out, snapshot_rows_out);
 }
 
 }  // extern "C"

@@ -212,13 +212,22 @@ struct FiltParams {
   const FiltToken* tok;             // every program's tokens, postfix
   const int32_t* prog_off;          // [n_programs + 1] program q = tok[prog_off[q] .. prog_off[q + 1])
   const uint32_t* bitmap;           // leaf bitmaps
-  const float* inv_norm;            // NaN = tombstone (never matches)
+  const float* inv_norm;            // a vector shard's rows: NaN = tombstone (never matches)
+  const uint8_t* live;              // a keyword store's rows (launch_filter_mask): 0 = tombstone (never matches)
   int64_t n_rows;                   // the search's snapshot
   int n_programs;
 };
 int filter_blocks(int64_t n_rows);
 // mask [n_rows] (bit q = program q), block_counts [n_programs][filter_blocks(n_rows)], totals [32] (zeroed here)
 cudaError_t launch_filter_count(const FiltParams& p, uint32_t* mask, uint32_t* block_counts, uint32_t* totals, cudaStream_t s);
+// The same pass over a keyword store's rows (liveness from p.live): mask [n_rows] only, no counts, nothing read back.
+cudaError_t launch_filter_mask(const FiltParams& p, uint32_t* mask, cudaStream_t s);
+// The programs of one call (aur_search_filtered, aur_hybrid_search_filtered), as the C ABI takes them; q_program [nq].
+struct FiltProgs {
+  const int32_t* prog; const int32_t* prog_off; int32_t n_programs;
+  const uint32_t* bitmap; int64_t bitmap_words;
+  const int32_t* q_program;
+};
 // rows_out [sum of totals]: program q's matching rows, ascending, after those of programs < q; ids_out (nullable) their ids.
 // Scans block_counts in place.
 cudaError_t launch_filter_write(const uint32_t* mask, uint32_t* block_counts, const uint32_t* totals, int n_programs, int64_t n_rows,
@@ -317,16 +326,36 @@ int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_hos
               const int32_t* q_org, float* scores, int64_t* ids, int64_t* snapshot_rows);
 int index_device(const aur_index* ix);
 int index_is_bf16(const aur_index* ix);
-// Keyword legs: aur_kw_search_multi's search (no allow-list) over stores[0 .. n) (distinct, non-NULL, 1 <= n <= 64)
-// taken as one corpus, each store's part enqueued on its own context and stream; then then(legs) runs with every
+// Filtered dense legs: aur_search_filtered's search of the host queries under the checked programs fp on every shard
+// of shards[0 .. n) (bf16, distinct), max_list_rows applied per shard, each shard's part on a pooled search context of
+// its device and that context's stream.  Every shard's count pass is enqueued before any is waited on; their read-back
+// is the only host sync.  Then every shard's search (list kernels or masked scan, as aur_search_filtered picks) is
+// enqueued and then(legs) runs with every shard's (device, stream, top-k lists [nq * k] in device memory, valid once the
+// stream reaches them, snapshot, matching rows per program) while the shards' shared locks and contexts are held; the
+// streams are idle again before this returns.  aur_stats.last_* of each shard describe its part.  scores_host /
+// ids_host (n = 1, nullable): the caller's host outputs; when both are page-locked and mapped, the search writes its
+// lists straight into them (DenseLeg.direct) instead of into device staging.  (capi.cu)
+struct DenseLeg { int device; cudaStream_t stream; const float* scores; const int64_t* ids; int64_t snapshot_rows;
+                  const std::vector<int64_t>* matched; bool direct; };
+using DenseLegsThen = std::function<int(const std::vector<DenseLeg>& legs)>;
+int filtered_legs(aur_index* const* shards, int n, const void* queries_host, int32_t nq, int32_t k, const FiltProgs& fp,
+                  int64_t max_list_rows, const DenseLegsThen& then, float* scores_host = nullptr,
+                  int64_t* ids_host = nullptr);
+// aur_search_filtered's program checks against one shard: structure, 1 <= n_programs <= 1024, columns set on it.
+int filter_check(aur_index* ix, const FiltProgs& fp);
+// Keyword legs: aur_kw_search_multi's search over stores[0 .. n) (distinct, non-NULL, 1 <= n <= 64) taken as one
+// corpus, each store's part enqueued on its own context and stream; fp (nullable; programs checked by filter_check and
+// kw_check_columns) restricts query q to the live rows program fp->q_program[q] matches on each store, evaluated there
+// (no allow-list, no read-back).  then(legs) runs with every
 // store's (device, stream, top-k lists, snapshot) -- device arrays [nq * k], valid once the stream reaches them,
 // sorted by (fp64 score desc, id asc) -- while every store's shared lock and every context are held.  Each store's
 // aur_kw_stats.last_* are published after then() returns AUR_OK.  The query arguments are checked by kw_check.  (keyword.cu)
 struct KwLeg { int device; cudaStream_t stream; const double* scores; const int64_t* ids; int64_t snapshot_rows; };
 using KwLegsThen = std::function<int(const std::vector<KwLeg>& legs)>;
 int kw_legs(aur_kw* const* stores, int n, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k,
-            const int32_t* q_user, const int32_t* q_org, const KwLegsThen& then);
+            const int32_t* q_user, const int32_t* q_org, const FiltProgs* fp, const KwLegsThen& then);
 int kw_check(const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k);   // aur_kw_search's query checks
+int kw_check_columns(aur_kw* kw, const FiltProgs& fp);   // every attribute column fp's leaves name was set on kw
 int kw_device(const aur_kw* kw);
 
 // Error reporting shared by the translation units behind the C ABI (thread-local message).

@@ -22,7 +22,8 @@
 // aur_kw_search_multi runs the same search over several stores (one per GPU) as one corpus: N, df and total_len are
 // summed over the stores' snapshots, every store scores its own prefix with the resulting idf / avgdl, and the per-store
 // lists are merged on the host (DESIGN.md section 10, "Sharded store").  The hybrid query (hybrid.cu) runs the same
-// steps through kw_legs and merges the per-store lists on the device instead.
+// steps through kw_legs and merges the per-store lists on the device instead; its filtered form evaluates filter programs
+// over the store's tenant codes and attribute columns (aur_kw_set_attrs, filter.cu) and scores only the matching rows.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
@@ -104,6 +105,10 @@ struct KwParams {
   Cand* buf;             // [grid][nq][kKwBufCap]
   Cand* lists;           // out: [nq][grid][ksel]
   int64_t rows_per_block;
+  // filtered launches (kw_score_kernel<true>): fmask [n_passes][fmask_stride] program match bits of every row (bit p of
+  // word ps = program 32 ps + p), prog_used [n_passes] the programs this launch's queries name, q_prog [nq] each one's
+  const uint32_t* fmask; const uint32_t* prog_used; const int32_t* q_prog;
+  int64_t fmask_stride; int n_passes;
 };
 
 __device__ __forceinline__ int lookup(const KwParams& p, int32_t term) {
@@ -136,6 +141,9 @@ __device__ int warp_flush(const KwParams& p, Cand* area, Cand* gbuf, int cnt, in
   return keep;
 }
 
+// kFilt: query q admits a row only when the row matches program q_prog[q]; a row that matches no program of the launch is
+// skipped before its postings are read.
+template <bool kFilt>
 __global__ void __launch_bounds__(kKwThreads) kw_score_kernel(KwParams p, int cval_in_smem) {
   extern __shared__ __align__(16) unsigned char smem[];
   Cand* thr = reinterpret_cast<Cand*>(smem);                         // [nq] block's ksel-th best so far
@@ -157,6 +165,11 @@ __global__ void __launch_bounds__(kKwThreads) kw_score_kernel(KwParams p, int cv
       const int64_t row = r0 + warp * kKwRowsPerWarp + j;
       if (row >= r_end) break;
       if (!__ldg(p.live + row) || (p.allow && !__ldg(p.allow + row))) continue;
+      if constexpr (kFilt) {
+        uint32_t any = 0u;
+        for (int ps = 0; ps < p.n_passes; ++ps) any |= __ldg(p.fmask + ps * p.fmask_stride + row) & __ldg(p.prog_used + ps);
+        if (!any) continue;
+      }
       const int64_t o0 = __ldg(p.off + row), o1 = __ldg(p.off + row + 1);
       const int32_t dl = __ldg(p.len + row);
       bool hit = false;
@@ -176,6 +189,10 @@ __global__ void __launch_bounds__(kKwThreads) kw_score_kernel(KwParams p, int cv
         if (p.q_user) {
           const int32_t qu = __ldg(p.q_user + q), qo = p.q_org ? __ldg(p.q_org + q) : -1;
           if (!(ru == qu || (qo >= 0 && ro == qo))) continue;
+        }
+        if constexpr (kFilt) {
+          const int32_t pg = __ldg(p.q_prog + q);
+          if (!((__ldg(p.fmask + (pg >> 5) * p.fmask_stride + row) >> (pg & 31)) & 1u)) continue;
         }
         const Cand c{s, rid};
         if (!better(c, thr[q])) continue;
@@ -256,11 +273,13 @@ struct KwCtx {
   DevBuf<int64_t> out_ids;
   DevBuf<uint8_t> allow;
   DevBuf<int32_t> allow_rows;
+  DevBuf<int32_t> fstage;        // filtered search: the programs' tokens, offsets and bitmaps (one upload)
+  DevBuf<uint32_t> fmask;        // filtered search: [passes][rows] program match bits
   int launches = 0, terms = 0, spilled = 0;   // of the last search: kernels, most distinct terms in one launch,
                                               // launches whose contribution table spilled to global memory
   void release() {
     tab.release(); buf.release(); lists_a.release(); lists_b.release(); cval.release(); out_s.release(); out_ids.release();
-    allow.release(); allow_rows.release();
+    allow.release(); allow_rows.release(); fstage.release(); fmask.release();
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (stream) cudaStreamDestroy(stream);
@@ -288,6 +307,9 @@ struct aur_kw {
   int64_t* d_off = nullptr; int32_t* d_len = nullptr; int64_t* d_ids = nullptr;
   int32_t* d_user = nullptr; int32_t* d_org = nullptr; uint8_t* d_live = nullptr;
   uint2* d_post = nullptr; int64_t post_cap = 0;
+  int32_t* d_attr[kFiltAttrCols] = {};   // attribute columns (program columns 2..), allocated on first aur_kw_set_attrs;
+                                         // the pointers are read and written under mu_stat
+  DevBuf<int32_t> attr_stage;            // aur_kw_set_attrs: (row, code) pairs (writers hold mu_write)
   // host mirrors (the writer's bookkeeping; searches read only the published statistics)
   std::vector<int64_t> h_off{0};
   std::vector<int32_t> h_len, h_user, h_org;
@@ -385,9 +407,10 @@ int grow_postings(aur_kw* kw, int64_t need) {
 // once from the summed statistics, every store's passes enqueued on its own device and stream, then each store's top-k
 // collected.
 
-struct KwQuery {   // the arguments of one search (aur_kw_search)
+struct KwQuery {   // the arguments of one search (aur_kw_search; fp: the hybrid query's programs, nullable)
   const int32_t* terms; const int64_t* off; int32_t nq, k;
   const int32_t* user; const int32_t* org; const int64_t* allow; int64_t n_allow;
+  const FiltProgs* fp;
 };
 
 int kw_check_query(const KwQuery& q) {
@@ -412,10 +435,11 @@ void kw_snapshot(aur_kw* kw, const std::vector<int32_t>& uniq, KwSnap* s) {
     s->udf[i] = (uniq[i] >= 0 && uniq[i] < static_cast<int32_t>(kw->df.size())) ? kw->df[static_cast<size_t>(uniq[i])] : 0;
 }
 
-// One launch's query side, the same on every store: idf | hkey | hval | qoff | slot | q_user | q_org in one upload.
+// One launch's query side, the same on every store: idf | hkey | hval | qoff | slot | q_user | q_org [| q_prog |
+// programs used] in one upload.
 struct KwBlock {
   int q0 = 0, nqb = 0, nu = 0, hcap = 0;   // nu = 0: no query of the block has a live term
-  size_t b_hk = 0, b_hv = 0, b_qo = 0, b_sl = 0, b_qu = 0, b_qg = 0;
+  size_t b_hk = 0, b_hv = 0, b_qo = 0, b_sl = 0, b_qu = 0, b_qg = 0, b_qp = 0, b_pu = 0;
   std::vector<unsigned char> tab;
 };
 
@@ -463,7 +487,9 @@ void kw_plan(const KwQuery& q, const std::vector<int32_t>& uniq, const std::vect
     b.b_hk = 8 * static_cast<size_t>(nu); b.b_hv = b.b_hk + 4 * static_cast<size_t>(hcap);
     b.b_qo = b.b_hv + 4 * static_cast<size_t>(hcap); b.b_sl = b.b_qo + 4 * qoff.size();
     b.b_qu = b.b_sl + 4 * std::max<size_t>(slot.size(), 1); b.b_qg = b.b_qu + 4 * static_cast<size_t>(nqb);
-    b.tab.assign(b.b_qg + 4 * static_cast<size_t>(nqb), 0);
+    b.b_qp = b.b_qg + 4 * static_cast<size_t>(nqb); b.b_pu = b.b_qp + 4 * static_cast<size_t>(nqb);
+    const int n_passes = q.fp ? (q.fp->n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms : 0;
+    b.tab.assign(q.fp ? b.b_pu + 4 * static_cast<size_t>(n_passes) : b.b_qp, 0);
     unsigned char* tab = b.tab.data();
     memcpy(tab, uidf.data(), 8 * static_cast<size_t>(nu));
     memcpy(tab + b.b_hk, hkey.data(), 4 * static_cast<size_t>(hcap));
@@ -474,6 +500,15 @@ void kw_plan(const KwQuery& q, const std::vector<int32_t>& uniq, const std::vect
     std::vector<int32_t> qorg(static_cast<size_t>(nqb), -1);
     if (q.org) std::copy(q.org + q0, q.org + q0 + nqb, qorg.begin());
     memcpy(tab + b.b_qg, qorg.data(), 4 * static_cast<size_t>(nqb));
+    if (q.fp) {
+      std::vector<uint32_t> used(static_cast<size_t>(n_passes), 0u);
+      for (int i = 0; i < nqb; ++i) {
+        const int32_t pg = q.fp->q_program[q0 + i];
+        used[static_cast<size_t>(pg / kFiltMaxPrograms)] |= 1u << (pg % kFiltMaxPrograms);
+      }
+      memcpy(tab + b.b_qp, q.fp->q_program + q0, 4 * static_cast<size_t>(nqb));
+      memcpy(tab + b.b_pu, used.data(), 4 * used.size());
+    }
     blocks->push_back(std::move(b));
   }
 }
@@ -507,6 +542,40 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
       c->launches += 1;
     }
     d_allow = c->allow.p;
+  }
+  // programs: every row's match bits over the snapshot, 32 programs a pass; the scoring kernel reads them in place
+  const uint32_t* d_fmask = nullptr;
+  int n_passes = 0;
+  const bool scores = n_rows > 0 && N > 0 && std::any_of(blocks.begin(), blocks.end(), [](const KwBlock& b) { return b.nu > 0; });
+  if (q.fp && scores) {
+    const FiltProgs& fp = *q.fp;
+    n_passes = (fp.n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms;
+    const size_t n_tok = static_cast<size_t>(fp.prog_off[fp.n_programs]);
+    std::vector<int32_t> st(n_tok * 4 + static_cast<size_t>(fp.n_programs) + 1 + static_cast<size_t>(fp.bitmap_words));
+    if (n_tok) memcpy(st.data(), fp.prog, n_tok * 16);
+    memcpy(st.data() + n_tok * 4, fp.prog_off, (static_cast<size_t>(fp.n_programs) + 1) * 4);
+    if (fp.bitmap_words) memcpy(st.data() + n_tok * 4 + fp.n_programs + 1, fp.bitmap, static_cast<size_t>(fp.bitmap_words) * 4);
+    KW_TRY(c->fstage.reserve(st.size()));
+    KW_TRY(c->fmask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(n_rows)));
+    KW_TRY(cudaMemcpyAsync(c->fstage.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice, s));   // pageable: staged on return
+    FiltParams fpp{};
+    fpp.cols[0] = kw->d_user; fpp.cols[1] = kw->d_org;
+    {
+      std::lock_guard<std::mutex> lk(kw->mu_stat);
+      for (int i = 0; i < kFiltAttrCols; ++i) fpp.cols[2 + i] = kw->d_attr[i];
+    }
+    const int32_t* d_off = c->fstage.p + n_tok * 4;   // token indices stay absolute: a pass starts at its first offset
+    fpp.tok = reinterpret_cast<const FiltToken*>(c->fstage.p);
+    fpp.bitmap = reinterpret_cast<const uint32_t*>(d_off + fp.n_programs + 1);
+    fpp.live = kw->d_live;
+    fpp.n_rows = n_rows;
+    for (int ps = 0; ps < n_passes; ++ps) {
+      fpp.prog_off = d_off + ps * kFiltMaxPrograms;
+      fpp.n_programs = std::min(kFiltMaxPrograms, fp.n_programs - ps * kFiltMaxPrograms);
+      KW_TRY(launch_filter_mask(fpp, c->fmask.p + static_cast<size_t>(ps) * n_rows, s));
+      c->launches += 1;
+    }
+    d_fmask = c->fmask.p;
   }
   const size_t nout = static_cast<size_t>(q.nq) * k;
   KW_TRY(c->out_s.reserve(nout));
@@ -552,7 +621,14 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
     p.nq = nqb; p.ksel = ksel; p.avgdl = avgdl;
     p.cval_global = in_smem ? nullptr : c->cval.p;
     p.buf = c->buf.p; p.lists = c->lists_a.p; p.rows_per_block = rpb;
-    kw_score_kernel<<<g, kKwThreads, smem, s>>>(p, in_smem ? 1 : 0);
+    if (d_fmask) {
+      p.fmask = d_fmask; p.fmask_stride = n_rows; p.n_passes = n_passes;
+      p.q_prog = reinterpret_cast<const int32_t*>(c->tab.p + b.b_qp);
+      p.prog_used = reinterpret_cast<const uint32_t*>(c->tab.p + b.b_pu);
+      kw_score_kernel<true><<<g, kKwThreads, smem, s>>>(p, in_smem ? 1 : 0);
+    } else {
+      kw_score_kernel<false><<<g, kKwThreads, smem, s>>>(p, in_smem ? 1 : 0);
+    }
     KW_TRY(cudaGetLastError());
     c->launches += 1;
     // fold the per-block lists until one sorted list per query remains
@@ -687,8 +763,8 @@ int kw_search_stores(aur_kw* const* stores, int n, const KwQuery& q, double* out
 
 namespace aur {
 int kw_legs(aur_kw* const* stores, int n, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k,
-            const int32_t* q_user, const int32_t* q_org, const KwLegsThen& then) {
-  const KwQuery q{q_terms, q_offsets, nq, k, q_user, q_org, nullptr, 0};
+            const int32_t* q_user, const int32_t* q_org, const FiltProgs* fp, const KwLegsThen& then) {
+  const KwQuery q{q_terms, q_offsets, nq, k, q_user, q_org, nullptr, 0, fp};
   return kw_run(stores, n, q, [&](const std::vector<KwCtx*>& cs, const std::vector<KwSnap>& snaps) -> int {
     std::vector<KwLeg> legs(static_cast<size_t>(n));
     for (int s = 0; s < n; ++s) {
@@ -708,6 +784,16 @@ int kw_legs(aur_kw* const* stores, int n, const int32_t* q_terms, const int64_t*
 
 int kw_check(const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k) {
   return kw_check_query(KwQuery{q_terms, q_offsets, nq, k, nullptr, nullptr, nullptr, 0});
+}
+
+int kw_check_columns(aur_kw* kw, const FiltProgs& fp) {
+  std::lock_guard<std::mutex> st(kw->mu_stat);   // the attribute columns that exist
+  for (int32_t t = 0; t < fp.prog_off[fp.n_programs]; ++t) {
+    const int32_t* tk = fp.prog + 4 * static_cast<int64_t>(t);
+    if (tk[0] == kFiltLeaf && tk[1] >= 2 && !kw->d_attr[tk[1] - 2])
+      return report_error(AUR_ERR_INVALID, "column %d was never set on the keyword store", tk[1]);
+  }
+  return AUR_OK;
 }
 
 int kw_device(const aur_kw* kw) { return kw->device; }
@@ -748,7 +834,9 @@ int aur_kw_open(int32_t device, int64_t doc_capacity, int64_t postings_capacity,
   if (e == cudaSuccess) e = cudaMemset(kw->d_off, 0, 8);
   // once, at the device's limit: the attribute belongs to the kernel, not to a search, and searches run concurrently
   if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(kw_score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kw->smem_optin));
+    e = cudaFuncSetAttribute(kw_score_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kw->smem_optin));
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(kw_score_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kw->smem_optin));
   if (e != cudaSuccess) return bail(e);
   *out = kw.release();
   return AUR_OK;
@@ -761,6 +849,8 @@ int aur_kw_close(aur_kw* kw) {
   for (auto& c : kw->ctxs) cudaStreamSynchronize(c->stream);
   cudaFree(kw->d_off); cudaFree(kw->d_len); cudaFree(kw->d_ids); cudaFree(kw->d_user); cudaFree(kw->d_org);
   cudaFree(kw->d_live); cudaFree(kw->d_post);
+  for (int32_t* a : kw->d_attr) cudaFree(a);
+  kw->attr_stage.release();
   for (auto& c : kw->ctxs) c->release();
   if (kw->stream) cudaStreamDestroy(kw->stream);
   delete kw;
@@ -918,8 +1008,19 @@ int aur_kw_compact(aur_kw* kw, int64_t* reclaimed) {
     kw_gather_postings<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, kw->stream>>>(kw->d_post, kw->d_off, d_map, d_noff, nl, np_);
     e = cudaGetLastError();
   }
+  // attribute codes move with their rows (through a bounce buffer); the rows compaction frees start absent again
+  int32_t* bounce = nullptr;
+  const bool any_attr = std::any_of(std::begin(kw->d_attr), std::end(kw->d_attr), [](const int32_t* a) { return a != nullptr; });
+  if (e == cudaSuccess && any_attr && nl) e = cudaMalloc(&bounce, static_cast<size_t>(nl) * 4);
+  for (int32_t* a : kw->d_attr) {
+    if (!a) continue;
+    if (e == cudaSuccess && nl) e = launch_gather_i32(a, d_map, nl, bounce, kw->stream);
+    if (e == cudaSuccess && nl) e = cudaMemcpyAsync(a, bounce, static_cast<size_t>(nl) * 4, cudaMemcpyDeviceToDevice, kw->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(a + nl, 0xFF, static_cast<size_t>(rows - nl) * 4, kw->stream);
+  }
   if (e == cudaSuccess) e = cudaStreamSynchronize(kw->stream);
   cudaFree(d_map);
+  cudaFree(bounce);
   if (e != cudaSuccess) { cudaFree(np_); cudaFree(d_noff); return report_error(AUR_ERR_CUDA, "aur_kw_compact: %s", cudaGetErrorString(e)); }
   cudaFree(kw->d_post);
   kw->d_post = np_;
@@ -957,6 +1058,40 @@ int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out) {
   out->last_ms = kw->last_ms;
   out->last_terms = kw->last_terms;
   out->last_spilled = kw->last_spilled;
+  return AUR_OK;
+}
+
+int aur_kw_set_attrs(aur_kw* kw, int32_t col, const int64_t* ids, const int32_t* codes, int64_t n) {
+  if (!kw || n < 0 || (n > 0 && (!ids || !codes))) return report_error(AUR_ERR_INVALID, "null argument");
+  if (col < 2 || col >= kFiltCols) return report_error(AUR_ERR_INVALID, "attribute columns are 2 .. %d", kFiltCols - 1);
+  std::lock_guard<std::mutex> wk(kw->mu_write);
+  std::shared_lock<std::shared_mutex> rl(kw->rw);
+  KW_TRY(cudaSetDevice(kw->device));
+  cudaStream_t s = kw->stream;
+  int32_t* a = nullptr;
+  {
+    std::lock_guard<std::mutex> st(kw->mu_stat);
+    a = kw->d_attr[col - 2];
+  }
+  if (!a) {   // first use: every row absent (-1), at the store's capacity like its tenant codes
+    KW_TRY(cudaMalloc(&a, static_cast<size_t>(kw->capacity) * 4));
+    cudaError_t e = cudaMemsetAsync(a, 0xFF, static_cast<size_t>(kw->capacity) * 4, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { cudaFree(a); return report_error(AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e)); }
+    std::lock_guard<std::mutex> st(kw->mu_stat);
+    kw->d_attr[col - 2] = a;
+  }
+  std::vector<int32_t> pairs;   // (row, code); id2row changes only under mu_write, which this call holds
+  pairs.reserve(2 * static_cast<size_t>(n));
+  for (int64_t i = 0; i < n; ++i) {
+    auto it = kw->id2row.find(ids[i]);
+    if (it != kw->id2row.end()) { pairs.push_back(static_cast<int32_t>(it->second)); pairs.push_back(codes[i]); }
+  }
+  if (pairs.empty()) return AUR_OK;
+  KW_TRY(kw->attr_stage.reserve(pairs.size()));
+  KW_TRY(cudaMemcpyAsync(kw->attr_stage.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s));
+  KW_TRY(launch_scatter_codes(kw->attr_stage.p, static_cast<int64_t>(pairs.size() / 2), a, s));
+  KW_TRY(cudaStreamSynchronize(s));
   return AUR_OK;
 }
 

@@ -470,6 +470,15 @@ class KeywordIndex:
         N.check(self._lib.aur_kw_get_stats(self._h, C.byref(st)))
         return {f: getattr(st, f) for f, _ in N.AurKwStats._fields_}
 
+    def set_attrs(self, col: int, ids, codes) -> None:
+        """``Index.set_attrs`` for the keyword store: attribute column ``col`` (2 .. 17) of the documents ``ids`` :=
+        ``codes`` (int32, -1 = absent); unknown ids are ignored.  Read by ``hybrid_search``'s programs."""
+        ids = np.ascontiguousarray(ids, dtype=np.int64)
+        codes = np.ascontiguousarray(codes, dtype=np.int32)
+        if codes.shape != ids.shape:
+            raise ValueError("ids and codes must have the same length")
+        N.check(self._lib.aur_kw_set_attrs(self._h, int(col), _ptr(ids), _ptr(codes), ids.shape[0]))
+
     def search(self, q_terms, q_offsets, k: int, q_user=None, q_org=None, allow_ids=None):
         """(ids [nq,k] int64, scores [nq,k] float64, snapshot rows).  Query q's term ids are
         q_terms[q_offsets[q]:q_offsets[q+1]] in summation order.  ``allow_ids``: None = every document."""
@@ -481,7 +490,7 @@ class KeywordIndex:
 
 def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_offsets,
                   w_dense, w_sparse=None, fusion: int = N.FUSION_RANKED, k_out: Optional[int] = None, q_user=None,
-                  q_org=None):
+                  q_org=None, programs=None, q_program=None, max_list_rows: int = 0):
     """Both legs of the hybrid query and their fusion in one device call (aur_hybrid_search): the dense leg's top-``fetch``
     of ``queries`` over ``index`` and the keyword leg's top-``fetch`` of ``q_terms`` / ``q_offsets`` over ``kw_index``
     (same tenant scope), fused per query with weights ``w_dense`` / ``w_sparse`` (default ``1 - w_dense``).  Returns
@@ -491,7 +500,13 @@ def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_o
     ``index`` / ``kw_index`` are an ``Index`` and a ``KeywordIndex``, or a ``MultiIndex`` of bf16 ``Index`` shards and a
     ``MultiKeywordIndex`` on the same devices in the same order (aur_hybrid_search_multi): each leg is then the global
     top-``fetch`` of ``MultiIndex.search`` / ``MultiKeywordIndex.search``, merged and fused on shard 0's GPU, and the
-    snapshots are (one per shard, one per store)."""
+    snapshots are (one per shard, one per store).
+
+    ``programs`` (``filters.compile_program`` outputs, at most 1024) scope the queries instead of ``q_user`` / ``q_org``
+    (aur_hybrid_search_filtered): query q sees the rows ``programs[q_program[q]]`` matches (``q_program`` None = every
+    query on program 0), in both legs -- the dense leg is ``Index.search_filtered`` / ``MultiIndex.search_filtered`` with
+    ``max_list_rows``, the keyword leg the search over the live documents whose ``KeywordIndex.set_attrs`` codes satisfy
+    the program, evaluated on each store's GPU.  Every column a program names must be set on every shard and store."""
     multi = isinstance(index, MultiIndex)
     if multi:
         if not isinstance(kw_index, MultiKeywordIndex):
@@ -514,6 +529,28 @@ def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_o
     scores = np.empty((nq, k_out), dtype=np.float64)
     ids = np.empty((nq, k_out), dtype=np.int64)
     cosine = np.empty((nq, k_out), dtype=np.float32)
+    if programs is not None:
+        from .filters import pack_programs
+
+        if q_user is not None or q_org is not None:
+            raise ValueError("programs replace q_user / q_org: write the tenant scope into the programs")
+        tok, off, bm = pack_programs(programs)
+        ql = np.zeros(nq, np.int32) if q_program is None else np.ascontiguousarray(q_program, dtype=np.int32)
+        if ql.shape != (nq,):
+            raise ValueError("q_program must be [nq]")
+        shard_list = index.shards if multi else [index]
+        store_list = kw_index.stores if multi else [kw_index]
+        n = len(shard_list)
+        shards = (C.c_void_p * n)(*[sh._h.value for sh in shard_list])
+        stores = (C.c_void_p * n)(*[st._h.value for st in store_list])
+        snaps = np.full(2 * n, -1, dtype=np.int64)
+        N.check(N.load().aur_hybrid_search_filtered(shards, stores, n, _ptr(q), nq, int(fetch), _ptr(qt), _ptr(q_off),
+                                                    _ptr(tok), _ptr(off), len(programs), _ptr(bm), bm.shape[0], _ptr(ql),
+                                                    int(max_list_rows), _ptr(wd), _ptr(ws), int(fusion), k_out,
+                                                    _ptr(scores), _ptr(ids), _ptr(cosine), _ptr(snaps)))
+        if multi:
+            return ids, scores, cosine, (snaps[:n].tolist(), snaps[n:].tolist())
+        return ids, scores, cosine, (int(snaps[0]), int(snaps[1]))
     if multi:
         n = len(index.shards)
         shards = (C.c_void_p * n)(*[sh._h.value for sh in index.shards])
@@ -616,6 +653,12 @@ class MultiKeywordIndex:
     def remove(self, ids) -> int:
         ids, sel = self._split(ids)
         return int(sum(self._each(lambda s, store: store.remove(ids[sel[s]]) if len(sel[s]) else 0)))
+
+    def set_attrs(self, col: int, ids, codes) -> None:
+        """KeywordIndex.set_attrs, each document's code to store ``id mod n``; every store gets the column."""
+        ids, sel = self._split(ids)
+        codes = np.asarray(codes, dtype=np.int32)
+        self._each(lambda s, store: store.set_attrs(col, ids[sel[s]], codes[sel[s]]))
 
     def compact(self) -> int:
         return int(sum(self._each(lambda s, store: store.compact())))

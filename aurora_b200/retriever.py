@@ -123,11 +123,12 @@ class KnowledgeBase:
         return BM25Index()
 
     def _fuses_on_device(self) -> bool:
-        """Whether an unfiltered hybrid query runs as one device call, both legs and their fusion
-        (``engine.hybrid_search``): a bf16 ``engine.Index`` and a ``DeviceBM25`` over a ``KeywordIndex`` on its GPU, or
-        a ``MultiIndex`` of bf16 ``engine.Index`` shards and a ``DeviceBM25`` over a ``MultiKeywordIndex`` on the same
-        devices in the same order.  f32 shards and the CPU doubles fuse on the host (``bm25.ranked_fusion`` /
-        ``relative_score_fusion``), as do filtered queries."""
+        """Whether a hybrid query runs as one device call, both legs and their fusion (``engine.hybrid_search``): a bf16
+        ``engine.Index`` and a ``DeviceBM25`` over a ``KeywordIndex`` on its GPU, or a ``MultiIndex`` of bf16
+        ``engine.Index`` shards and a ``DeviceBM25`` over a ``MultiKeywordIndex`` on the same devices in the same order.
+        Filtered queries too, when their filter compiles to a device program (attribute columns are then kept on the
+        keyword store as well).  f32 shards, the CPU doubles and filters that stay on the host fuse on the host
+        (``bm25.ranked_fusion`` / ``relative_score_fusion``)."""
         from .bm25 import DeviceBM25
         from .engine import Index, KeywordIndex, MultiIndex, MultiKeywordIndex
 
@@ -304,7 +305,14 @@ class KnowledgeBase:
                 self._attr_host.add(name)
                 self._attr_free.append(col.col)   # the slot serves the next property (its codes are rewritten then)
                 continue
-            self.index.set_attrs(col.col, rids, codes)
+            self._write_attr(col.col, rids, codes)
+
+    def _write_attr(self, col: int, rids: np.ndarray, codes: np.ndarray) -> None:
+        """Attribute column ``col`` of the rows ``rids`` on the vector index and, when hybrid queries fuse on the device
+        (their filter programs then run on the keyword store too), on the keyword store.  Caller holds the lock."""
+        self.index.set_attrs(col, rids, codes)
+        if self._hybrid_device:
+            self.sparse.store.set_attrs(col, rids, codes)
 
     def _attr_column(self, name: str) -> AttrColumn:
         """The attribute column of property ``name``, built from the whole table on first use.  Caller holds the lock."""
@@ -320,7 +328,7 @@ class KnowledgeBase:
         except TypeError:
             self._attr_host.add(name)
             raise
-        self.index.set_attrs(col.col, rids, codes)
+        self._write_attr(col.col, rids, codes)     # a slot handed back by another property is rewritten on every row
         self._attr_free.pop(0)
         self._attr_cols[name] = col
         return col
@@ -377,8 +385,9 @@ class KnowledgeBase:
         metadata table to the set of allowed ids.  Either way the kernel searches only the matching rows,
         so a small tenant's chunks are found even when the global top-k belongs to other tenants.
 
-        An unfiltered hybrid query on a CUDA shard is one device call (``DeviceBM25.search_batch`` with ``dense``):
-        both legs and their fusion run on the GPU and only the fused top-``limit`` comes back.  Objects deleted after
+        A hybrid query on a CUDA shard is one device call (``DeviceBM25.search_batch`` with ``dense``): both legs and
+        their fusion run on the GPU and only the fused top-``limit`` comes back.  A filtered one goes the same way when
+        its filter compiles to a device program, which both legs then evaluate on the GPU.  Objects deleted after
         that call drop out of the answer; the others keep the scores the device computed (the answer as of the
         search).  Elsewhere the two lists come back and are fused on the host.
 
@@ -422,6 +431,14 @@ class KnowledgeBase:
 
             allowed: Optional[List[int]] = None
             prog = self._device_program(filters, tenant, user_id, org_id) if filters is not None else None
+            if prog is not None and hybrid and self._hybrid_device and _dense is None and _sparse is None:
+                # the whole filtered hybrid query in one device call: both legs evaluate the program on the GPU
+                if qv is None:              # the dense leg is ignored (alpha <= 0) but still takes a vector
+                    qv = np.zeros((1, self.dim), np.float32)
+                fused = self.sparse.search_batch(
+                    [query], _MAX_FETCH, dense=(self.index, qv, np.array([dense_w]), _FUSION[fusion], min(limit, 2 * _MAX_FETCH)),
+                    programs=[prog], max_list_rows=int(_LIST_MAX_FRACTION * len(self._props)))[0]
+                return self._shape([(rid, fs, cos) for rid, (fs, cos) in fused if rid in self._props][:limit])
             if filters is not None and prog is None:
                 # narrow the scan with the filter's own equality terms and the tenant scope, then run the predicate
                 eq = filters.required_equalities()
@@ -465,7 +482,9 @@ class KnowledgeBase:
             if not hybrid:
                 picked = [(rid, sc, sc) for rid, sc in dense[:limit]]
             else:
-                # keyword leg under the same pre-filter: the resolved filter's ids, else the tenant's own inverted lists
+                # keyword leg under the same pre-filter: the resolved filter's ids, else the tenant's own inverted lists.
+                # A device program reaches here only with the keyword leg on the host (BM25Index beside an index that
+                # evaluates programs, e.g. a MultiIndex of CPU shard doubles): the device knowledge base fused above.
                 if prog is not None and _sparse is None:
                     allowed = self.index.filter_ids(prog).tolist()
                 if _sparse is not None:     # keyword leg already computed by query_batch (same scope, same fetch);

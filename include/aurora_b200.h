@@ -320,6 +320,13 @@ int aur_kw_remove(aur_kw* kw, const int64_t* ids, int64_t n, int64_t* removed);
 /* Stable compaction of the tombstones, as aur_compact; *reclaimed (nullable) = rows freed. */
 int aur_kw_compact(aur_kw* kw, int64_t* reclaimed);
 int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out);
+/* Attribute columns of the keyword store, exactly as aur_set_attrs for an aur_index: columns 2 .. 17 (0 and 1 are the
+ * store's user / org codes of aur_kw_add), allocated on first use at the store's capacity with every row absent (-1);
+ * codes are written by id (unknown ids are ignored); rows appended later, the new row of an upsert and the rows compaction
+ * frees start absent, and compaction carries every row's codes with it.  Serialised with the store's other writers.  A
+ * search sees a row's codes as they were when its filter kernel read them: a caller that must never answer from a row
+ * without its codes sets them before it lets searches name them.  Read by aur_hybrid_search_filtered's programs. */
+int aur_kw_set_attrs(aur_kw* kw, int32_t col, const int64_t* ids, const int32_t* codes, int64_t n);
 /* The BM25 leg of collection.query.hybrid (weaviate_client.py:252-259), batched: query q's term ids are
  * q_terms[q_offsets[q] .. q_offsets[q + 1]) in summation order (repeats and unknown ids are ignored); top-k each,
  * 1 <= k <= 128 (larger: AUR_ERR_UNSUPPORTED).  q_user / q_org: per-query tenant scope as in aur_search
@@ -384,6 +391,27 @@ int aur_hybrid_search_multi(aur_index* const* shards, aur_kw* const* stores, int
                             const int32_t* q_user, const int32_t* q_org, const double* w_dense, const double* w_sparse,
                             int32_t fusion, int32_t k_out, double* scores_out, int64_t* ids_out, float* cosine_out,
                             int64_t* snapshot_rows_out /* [2n] */);
+/* aur_hybrid_search_multi with every query's scope given as a filter program instead of q_user / q_org: query q sees
+ * the rows program q_program[q] matches (programs, bitmap and 1 <= n_programs <= 1024 as for aur_search_filtered; the
+ * tenant scope is the program [leaf(0, bit u + 1), leaf(1, bit o + 1), OR]).  n = 1 is the single-shard call.
+ *   dense leg of shard s   exactly aur_search_filtered on that shard with max_list_rows / n as its bound;
+ *   keyword leg of store s exactly aur_kw_search_multi with, for query q, the allow-list of the store's live rows whose
+ *                          codes (tenant codes and aur_kw_set_attrs columns) satisfy program q_program[q]; idf and
+ *                          avgdl stay corpus-wide, unaffected by the filter.
+ * The programs are evaluated on every store's device and the match bits read in place by its scoring kernel (a row that
+ * matches no program of a launch is skipped before its postings are read), so the keyword legs need no host sync.  The
+ * keyword legs are enqueued first, then every shard's count pass; their small read-back (the list planning needs it) is
+ * the call's only host sync before the final copy.  The lists are then merged and fused as aur_hybrid_search_multi does.
+ * A column a leaf names must have been set on every shard and every store; q_program [nq] must name programs and
+ * max_list_rows be >= 0; every other argument as for aur_hybrid_search_multi (all AUR_ERR_INVALID / _UNSUPPORTED before
+ * any device work, the outputs untouched).  snapshot_rows_out [2n] as for aur_hybrid_search_multi. */
+int aur_hybrid_search_filtered(aur_index* const* shards, aur_kw* const* stores, int32_t n, const void* queries_host,
+                               int32_t nq, int32_t fetch, const int32_t* q_terms, const int64_t* q_offsets,
+                               const int32_t* prog, const int32_t* prog_offsets, int32_t n_programs, const uint32_t* bitmap,
+                               int64_t bitmap_words, const int32_t* q_program, int64_t max_list_rows,
+                               const double* w_dense, const double* w_sparse, int32_t fusion, int32_t k_out,
+                               double* scores_out, int64_t* ids_out, float* cosine_out,
+                               int64_t* snapshot_rows_out /* [2n] */);
 
 /* ------------------------------------------------------------------ text encoder
  * Replaces the text2vec-transformers sidecar: EmbeddingClient.embed / embed_batch
