@@ -30,7 +30,8 @@ EXPORTS = [
     "aur_exchange_status", "aur_search_exchange_dev", "aur_cosine_pairs", "aur_dev_malloc", "aur_dev_free", "aur_memcpy_h2d", "aur_memcpy_d2h",
     "aur_debug_tc_scores",
     "aur_kw_open", "aur_kw_close", "aur_kw_add", "aur_kw_remove", "aur_kw_compact", "aur_kw_get_stats", "aur_kw_set_attrs",
-    "aur_kw_search", "aur_kw_search_multi", "aur_hybrid_search", "aur_hybrid_search_multi", "aur_hybrid_search_filtered",
+    "aur_kw_search", "aur_kw_search_multi", "aur_kw_reindex", "aur_kw_set_option", "aur_kw_get_index_stats",
+    "aur_hybrid_search", "aur_hybrid_search_multi", "aur_hybrid_search_filtered",
     "aur_encoder_open", "aur_encoder_close", "aur_encoder_load", "aur_encode", "aur_encode_append",
     "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
     "aur_tokenize", "aur_encode_text_append", "aur_debug_gemm", "aur_debug_attention", "aur_debug_encoder_hidden",
@@ -54,6 +55,16 @@ class AurKwStats(C.Structure):
     _fields_ = [("docs", C.c_int64), ("live", C.c_int64), ("capacity", C.c_int64), ("postings_used", C.c_int64),
                 ("postings_allocated", C.c_int64), ("total_len", C.c_int64), ("last_launches", C.c_int32),
                 ("last_ms", C.c_float), ("last_terms", C.c_int32), ("last_spilled", C.c_int32)]
+
+
+class AurKwIndexStats(C.Structure):
+    _fields_ = [("indexed_rows", C.c_int64), ("index_postings", C.c_int64), ("index_bytes", C.c_int64),
+                ("builds", C.c_int64), ("last_build_ms", C.c_float), ("last_path", C.c_int32),
+                ("last_postings", C.c_int64)]
+
+
+KW_PATH_FORWARD, KW_PATH_INDEX = 1, 2   # AUR_KW_PATH_* bits of AurKwIndexStats.last_path
+KW_PATH_AUTO_OPT, KW_PATH_FORWARD_OPT, KW_PATH_INDEX_OPT = 0, 1, 2   # aur_kw_set_option "kw_path" values
 
 
 class AurEncoderConfig(C.Structure):
@@ -139,6 +150,9 @@ def load():
         "aur_kw_set_attrs": (C.c_int, [vp, i32, vp, vp, i64]),
         "aur_kw_search": (C.c_int, [vp, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, C.POINTER(i64)]),
         "aur_kw_search_multi": (C.c_int, [vp, i32, vp, vp, i32, i32, vp, vp, vp, i64, vp, vp, vp]),
+        "aur_kw_reindex": (C.c_int, [vp]),
+        "aur_kw_set_option": (C.c_int, [vp, C.c_char_p, i64]),
+        "aur_kw_get_index_stats": (C.c_int, [vp, C.POINTER(AurKwIndexStats)]),
         "aur_hybrid_search": (C.c_int, [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]),
         "aur_hybrid_search_multi": (C.c_int, [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]),
         "aur_hybrid_search_filtered": (C.c_int, [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, i32, vp, i64, vp, i64, vp, vp,

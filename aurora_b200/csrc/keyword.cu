@@ -19,6 +19,9 @@
 // term up in the launch's term table and parks the row's contribution per unique term; then every lane sums its
 // queries' terms in their order.  Selection is exact on (fp64 score desc, id asc) throughout: per-block candidate
 // buffers pruned by the block's own k-th best, sorted lists per block, then sorted folds down to one list per query.
+// A term-major index of the store's first R rows (DESIGN.md section 10, "Term-major index") lets a launch score those
+// rows from its own terms' posting lists instead, into per-query accumulators, when the path rule estimates it cheaper;
+// the rows behind R are always scanned forward, and both parts' lists are folded together.
 // aur_kw_search_multi runs the same search over several stores (one per GPU) as one corpus: N, df and total_len are
 // summed over the stores' snapshots, every store scores its own prefix with the resulting idf / avgdl, and the per-store
 // lists are merged on the host (DESIGN.md section 10, "Sharded store").  The hybrid query (hybrid.cu) runs the same
@@ -33,6 +36,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <chrono>
 #include <memory>
 #include <mutex>
 #include <shared_mutex>
@@ -56,6 +60,16 @@ constexpr int kKwQBlock = 256;            // queries per launch
 constexpr int kKwFoldCap = 2048;          // entries one fold block sorts
 constexpr int64_t kKwMaxTerm = int64_t(1) << 28;
 constexpr int kKwMaxStores = 64;         // stores one aur_kw_search_multi call takes
+// term-major index (DESIGN.md section 10, "Term-major index")
+constexpr int64_t kKwMaxRows = 0x7FFFFFC0ll;              // aur_kw_open's capacity limit: every row id fits the index's u32
+static_assert(kKwMaxRows <= 0xFFFFFFFFll, "indexed rows are u32");
+constexpr int64_t kIxTailFrac = 8;                         // the writer rebuilds once the tail holds > 1/8 of the indexed postings
+constexpr int kIxMaxTermPos = 64;                          // term positions (one launch each) a query group takes through the index
+constexpr int64_t kIxAccBytes = int64_t(256) << 20;        // fp64 accumulators of one query group: more queries are split
+constexpr int kIxSelBlocksPerSm = 4;                       // selection grid over the indexed rows
+// the path rule's cost model, in ns of H100 time: forward scan per posting of [0, R); index per list posting, per
+// accumulator entry scanned, per launch
+constexpr double kFwdNsPerPosting = 0.02, kIxNsPerPosting = 0.05, kIxNsPerAcc = 0.005, kIxNsPerLaunch = 3000.0;
 
 #define KW_TRY(expr)                                                                                             \
   do {                                                                                                           \
@@ -141,6 +155,54 @@ __device__ int warp_flush(const KwParams& p, Cand* area, Cand* gbuf, int cnt, in
   return keep;
 }
 
+// Selection state of one block in shared memory (kw_score_kernel, kw_ix_select_kernel): thr [nq] the block's ksel-th
+// best so far, sort_area [warps][kKwBufCap], cnt [nq] entries in each query's candidate buffer.
+struct KwSel { Cand* thr; Cand* sort_area; int* cnt; };
+
+// Query q's admission of a row with score s > 0 (row: index into the row-indexed arrays of p; ru / ro / rid: the row's
+// tenant codes and id): the query's tenant scope, its filter program (kFilt), then the block's threshold; an admitted
+// row joins the query's candidate buffer.
+template <bool kFilt>
+__device__ __forceinline__ void kw_offer(const KwParams& p, const KwSel& sl, Cand* gbuf, int q, int64_t row, int32_t ru,
+                                         int32_t ro, int64_t rid, double s) {
+  if (p.q_user) {
+    const int32_t qu = __ldg(p.q_user + q), qo = p.q_org ? __ldg(p.q_org + q) : -1;
+    if (!(ru == qu || (qo >= 0 && ro == qo))) return;
+  }
+  if constexpr (kFilt) {
+    const int32_t pg = __ldg(p.q_prog + q);
+    if (!((__ldg(p.fmask + (pg >> 5) * p.fmask_stride + row) >> (pg & 31)) & 1u)) return;
+  }
+  const Cand c{s, rid};
+  if (!better(c, sl.thr[q])) return;
+  const int pos = atomicAdd(sl.cnt + q, 1);
+  gbuf[static_cast<size_t>(q) * kKwBufCap + pos] = c;
+}
+
+// End of a round (at most kKwRoundRows appends per query since the last): buffers that could overflow next round are
+// cut to their best ksel, which raises the threshold.  Between two __syncthreads.
+__device__ __forceinline__ void kw_round_flush(const KwParams& p, const KwSel& sl, Cand* gbuf, int warp, int lane) {
+  for (int q = warp; q < p.nq; q += kKwWarps) {
+    const int c = sl.cnt[q];
+    if (c > kKwBufCap - kKwRoundRows) {
+      Cand t = sl.thr[q];
+      const int keep = warp_flush(p, sl.sort_area + warp * kKwBufCap, gbuf + static_cast<size_t>(q) * kKwBufCap, c, lane, &t);
+      if (lane == 0) { sl.cnt[q] = keep; sl.thr[q] = t; }
+    }
+  }
+}
+
+// The block's sorted best ksel per query: query q's list is list `list` of n_lists at p.lists + (q * n_lists + list) * ksel.
+__device__ __forceinline__ void kw_block_lists(const KwParams& p, const KwSel& sl, Cand* gbuf, int warp, int lane,
+                                               unsigned n_lists, unsigned list) {
+  for (int q = warp; q < p.nq; q += kKwWarps) {
+    Cand* area = sl.sort_area + warp * kKwBufCap;
+    const int keep = warp_flush(p, area, gbuf + static_cast<size_t>(q) * kKwBufCap, sl.cnt[q], lane, nullptr);
+    Cand* out = p.lists + (static_cast<size_t>(q) * n_lists + list) * p.ksel;
+    for (int i = lane; i < p.ksel; i += 32) out[i] = i < keep ? area[i] : sentinel();
+  }
+}
+
 // kFilt: query q admits a row only when the row matches program q_prog[q]; a row that matches no program of the launch is
 // skipped before its postings are read.
 template <bool kFilt>
@@ -154,6 +216,7 @@ __global__ void __launch_bounds__(kKwThreads) kw_score_kernel(KwParams p, int cv
   double* cval = cval_in_smem ? cval_s + static_cast<size_t>(warp) * p.n_uniq
                               : p.cval_global + (static_cast<size_t>(blockIdx.x) * kKwWarps + warp) * p.n_uniq;
   for (int q = threadIdx.x; q < p.nq; q += blockDim.x) { thr[q] = sentinel(); cnt[q] = 0; }
+  const KwSel sl{thr, sort_area, cnt};
   for (int u = lane; u < p.n_uniq; u += 32) cval[u] = 0.0;
   __syncthreads();
   Cand* gbuf = p.buf + static_cast<size_t>(blockIdx.x) * p.nq * kKwBufCap;
@@ -186,18 +249,7 @@ __global__ void __launch_bounds__(kKwThreads) kw_score_kernel(KwParams p, int cv
         double s = 0.0;   // the loop path's defaultdict(float) start; adding a miss (0.0) leaves s bit-identical
         for (int g = __ldg(p.q_off + q), g1 = __ldg(p.q_off + q + 1); g < g1; ++g) s = __dadd_rn(s, cval[__ldg(p.slot_u + g)]);
         if (!(s > 0.0)) continue;
-        if (p.q_user) {
-          const int32_t qu = __ldg(p.q_user + q), qo = p.q_org ? __ldg(p.q_org + q) : -1;
-          if (!(ru == qu || (qo >= 0 && ro == qo))) continue;
-        }
-        if constexpr (kFilt) {
-          const int32_t pg = __ldg(p.q_prog + q);
-          if (!((__ldg(p.fmask + (pg >> 5) * p.fmask_stride + row) >> (pg & 31)) & 1u)) continue;
-        }
-        const Cand c{s, rid};
-        if (!better(c, thr[q])) continue;
-        const int pos = atomicAdd(cnt + q, 1);
-        gbuf[static_cast<size_t>(q) * kKwBufCap + pos] = c;
+        kw_offer<kFilt>(p, sl, gbuf, q, row, ru, ro, rid, s);
       }
       __syncwarp();
       if (hit)
@@ -208,23 +260,125 @@ __global__ void __launch_bounds__(kKwThreads) kw_score_kernel(KwParams p, int cv
       __syncwarp();
     }
     __syncthreads();
-    for (int q = warp; q < p.nq; q += kKwWarps) {
-      const int c = cnt[q];
-      if (c > kKwBufCap - kKwRoundRows) {
-        Cand t = thr[q];
-        const int keep = warp_flush(p, sort_area + warp * kKwBufCap, gbuf + static_cast<size_t>(q) * kKwBufCap, c, lane, &t);
-        if (lane == 0) { cnt[q] = keep; thr[q] = t; }
+    kw_round_flush(p, sl, gbuf, warp, lane);
+    __syncthreads();
+  }
+  kw_block_lists(p, sl, gbuf, warp, lane, gridDim.x, blockIdx.x);
+}
+
+// ------------------------------------------------------------------------------------------- term-major index
+// The store's first R rows, term by term: term t's postings are tpost[toff[t] .. toff[t + 1]) as (row, tf), in no
+// particular order within a term.  Built by a counting sort of the forward postings of rows [0, R): kw_ix_count,
+// kw_ix_scan, kw_ix_scatter.
+
+// cnt[t] += postings of term t in rows [0, R); one warp per row.
+__global__ void kw_ix_count(const int64_t* off, const uint2* post, int64_t R, unsigned* cnt) {
+  const int64_t w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  if (w >= R) return;
+  for (int64_t i = off[w] + (threadIdx.x & 31); i < off[w + 1]; i += 32) atomicAdd(cnt + post[i].x, 1u);
+}
+
+// toff[0 .. T] = exclusive scan of cnt[0 .. T) (toff[T] = every posting), cur = toff[0 .. T); one block, each thread a
+// contiguous chunk of terms.
+__global__ void __launch_bounds__(1024) kw_ix_scan(const unsigned* cnt, int64_t T, int64_t* toff, unsigned long long* cur) {
+  __shared__ int64_t part[1024];
+  const int t = threadIdx.x;
+  const int64_t chunk = (T + 1023) / 1024;
+  const int64_t a = t * chunk, b = a + chunk < T ? a + chunk : T;
+  int64_t s = 0;
+  for (int64_t i = a; i < b; ++i) s += cnt[i];
+  part[t] = s;
+  __syncthreads();
+  for (int d = 1; d < 1024; d <<= 1) {   // inclusive scan of the chunk sums
+    const int64_t v = t >= d ? part[t - d] : 0;
+    __syncthreads();
+    part[t] += v;
+    __syncthreads();
+  }
+  int64_t run = part[t] - s;
+  for (int64_t i = a; i < b; ++i) { toff[i] = run; cur[i] = static_cast<unsigned long long>(run); run += cnt[i]; }
+  if (t == 1023) toff[T] = part[1023];
+}
+
+// tpost[cur[t]++] = (row, tf) for every posting of rows [0, R); one warp per row.
+__global__ void kw_ix_scatter(const int64_t* off, const uint2* post, int64_t R, unsigned long long* cur, uint2* tpost) {
+  const int64_t w = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  if (w >= R) return;
+  for (int64_t i = off[w] + (threadIdx.x & 31); i < off[w + 1]; i += 32) {
+    const uint2 pt = post[i];
+    tpost[atomicAdd(cur + pt.x, 1ull)] = make_uint2(static_cast<uint32_t>(w), pt.y);
+  }
+}
+
+// One term position of a query group scored from the index: query q (blockIdx.y) of the group adds the contribution of
+// its j-th term u (summation order) to acc[q * R + row] for every (row, tf) of u's list.  A list holds a row once and a
+// query has one j-th term, so no two threads of a launch touch one entry; launches j = 0, 1, ... run in stream order,
+// so acc[q][row] is summed in the query's term order, as kw_score_kernel sums it.
+struct KwIxTerm {
+  const uint2* tpost; const int64_t* toff; int64_t n_terms;   // the index (terms 0 .. n_terms - 1)
+  const int32_t* len; const int32_t* ukey; const double* idf;   // ukey [n_uniq]: unique index -> term id
+  const int32_t* q_off; const int32_t* slot_u;                  // the group's first query at q_off[0]
+  double* acc; int64_t R; double avgdl; int j;
+};
+
+__global__ void __launch_bounds__(256) kw_ix_term_kernel(KwIxTerm t) {
+  const int q = blockIdx.y;
+  const int g = __ldg(t.q_off + q) + t.j;
+  if (g >= __ldg(t.q_off + q + 1)) return;
+  const int u = __ldg(t.slot_u + g);
+  const int32_t term = __ldg(t.ukey + u);
+  if (term >= t.n_terms) return;   // first seen after the build: no indexed row has it
+  const int64_t hi = __ldg(t.toff + term + 1);
+  const double idf = __ldg(t.idf + u);
+  double* acc = t.acc + static_cast<size_t>(q) * t.R;
+  for (int64_t i = __ldg(t.toff + term) + static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < hi;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const uint2 pt = __ldg(t.tpost + i);
+    acc[pt.x] = __dadd_rn(acc[pt.x], contribution(idf, pt.y, __ldg(t.len + pt.x), t.avgdl));
+  }
+}
+
+// Selection over the indexed rows [0, p.n_rows): query q's score of row r is acc[q * R + r] (0.0: none of its terms);
+// every entry is read once and reset to 0.0 for the next search.  Rows are admitted by kw_score_kernel's tests and
+// selected into the same per-block lists: query q's list of block b at p.lists + (q * n_lists + b) * ksel.  A round
+// is kKwRoundRows rows, one per lane; warp w takes queries w, w + 8, ...
+template <bool kFilt>
+__global__ void __launch_bounds__(kKwThreads) kw_ix_select_kernel(KwParams p, double* acc, int64_t R, int n_lists) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  Cand* thr = reinterpret_cast<Cand*>(smem);   // kw_score_kernel's layout, without the contribution table
+  Cand* sort_area = thr + p.nq;
+  int* cnt = reinterpret_cast<int*>(sort_area + kKwWarps * kKwBufCap);
+  const KwSel sl{thr, sort_area, cnt};
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int q = threadIdx.x; q < p.nq; q += blockDim.x) { thr[q] = sentinel(); cnt[q] = 0; }
+  __syncthreads();
+  Cand* gbuf = p.buf + static_cast<size_t>(blockIdx.x) * p.nq * kKwBufCap;
+  const int64_t r_begin = static_cast<int64_t>(blockIdx.x) * p.rows_per_block;
+  int64_t r_end = r_begin + p.rows_per_block;
+  if (r_end > p.n_rows) r_end = p.n_rows;
+  for (int64_t r0 = r_begin; r0 < r_end; r0 += kKwRoundRows) {
+    const int64_t row = r0 + lane;
+    if (row < r_end) {
+      int state = -1;   // the row's live / allow test, once a query scores it: 1 admitted, 0 not
+      int32_t ru = 0, ro = 0;
+      int64_t rid = 0;
+      for (int q = warp; q < p.nq; q += kKwWarps) {
+        double* a = acc + static_cast<size_t>(q) * R + row;
+        const double s = *a;
+        if (s == 0.0) continue;
+        *a = 0.0;
+        if (state < 0) {
+          state = __ldg(p.live + row) && !(p.allow && !__ldg(p.allow + row));
+          if (state) { ru = __ldg(p.user + row); ro = __ldg(p.org + row); rid = __ldg(p.ids + row); }
+        }
+        if (state && s > 0.0) kw_offer<kFilt>(p, sl, gbuf, q, row, ru, ro, rid, s);
       }
     }
     __syncthreads();
+    kw_round_flush(p, sl, gbuf, warp, lane);
+    __syncthreads();
   }
-  // the block's sorted best ksel per query
-  for (int q = warp; q < p.nq; q += kKwWarps) {
-    Cand* area = sort_area + warp * kKwBufCap;
-    const int keep = warp_flush(p, area, gbuf + static_cast<size_t>(q) * kKwBufCap, cnt[q], lane, nullptr);
-    Cand* out = p.lists + (static_cast<size_t>(q) * gridDim.x + blockIdx.x) * p.ksel;
-    for (int i = lane; i < p.ksel; i += 32) out[i] = i < keep ? area[i] : sentinel();
-  }
+  kw_block_lists(p, sl, gbuf, warp, lane, static_cast<unsigned>(n_lists), blockIdx.x);
 }
 
 // [nq][n_lists][ksel] sorted lists -> [nq][ceil(n_lists / group)][ksel]; final: top-k as (fp64 score, id) with
@@ -275,11 +429,15 @@ struct KwCtx {
   DevBuf<int32_t> allow_rows;
   DevBuf<int32_t> fstage;        // filtered search: the programs' tokens, offsets and bitmaps (one upload)
   DevBuf<uint32_t> fmask;        // filtered search: [passes][rows] program match bits
+  DevBuf<double> acc;            // index path: [group][R] per-query scores, all 0.0 between searches
+  bool acc_clean = true;         // false while a search's index part is in flight (an error leaves it dirty)
   int launches = 0, terms = 0, spilled = 0;   // of the last search: kernels, most distinct terms in one launch,
                                               // launches whose contribution table spilled to global memory
+  int path = 0;                  // of the last search: AUR_KW_PATH_* bits
+  int64_t postings = 0;          // of the last search: postings it read
   void release() {
     tab.release(); buf.release(); lists_a.release(); lists_b.release(); cval.release(); out_s.release(); out_ids.release();
-    allow.release(); allow_rows.release(); fstage.release(); fmask.release();
+    allow.release(); allow_rows.release(); fstage.release(); fmask.release(); acc.release();
     if (ev0) cudaEventDestroy(ev0);
     if (ev1) cudaEventDestroy(ev1);
     if (stream) cudaStreamDestroy(stream);
@@ -319,10 +477,18 @@ struct aur_kw {
   // published under mu_stat
   int64_t rows_pub = 0, post_pub = 0, n_live = 0, total_len = 0;
   std::vector<int64_t> df;
+  // term-major index of rows [0, ix_rows) (ix_post postings), published under mu_stat and replaced only under the
+  // exclusive lock: d_toff [ix_terms + 1], d_tpost [ix_post]; h_toff mirrors d_toff
+  int64_t* d_toff = nullptr; uint2* d_tpost = nullptr;
+  int64_t ix_rows = 0, ix_post = 0, ix_terms = 0, ix_builds = 0;
+  std::vector<int64_t> h_toff;
+  float ix_build_ms = 0.f;
+  std::atomic<int> kw_path{0};   // aur_kw_set_option "kw_path": 0 auto, 1 forward, 2 index
   // search pool + last search's stats
   std::vector<std::unique_ptr<KwCtx>> ctxs;
   std::vector<KwCtx*> idle;
-  int last_launches = 0, last_terms = 0, last_spilled = 0;
+  int last_launches = 0, last_terms = 0, last_spilled = 0, last_path = 0;
+  int64_t last_postings = 0;
   float last_ms = 0.f;
 };
 
@@ -401,6 +567,71 @@ int grow_postings(aur_kw* kw, int64_t need) {
   return AUR_OK;
 }
 
+// Drop the term-major index (rows are about to move).  Caller holds the exclusive lock.
+void drop_index(aur_kw* kw) {
+  int64_t* toff = nullptr; uint2* tpost = nullptr;
+  {
+    std::lock_guard<std::mutex> st(kw->mu_stat);
+    std::swap(toff, kw->d_toff); std::swap(tpost, kw->d_tpost);
+    kw->ix_rows = kw->ix_post = kw->ix_terms = 0;
+    kw->h_toff.clear();
+  }
+  cudaFree(toff); cudaFree(tpost);
+}
+
+// Build the term-major index of every appended row into fresh buffers on the store's stream and publish it.  The
+// caller holds mu_write and no rw lock: the forward postings of the rows being indexed only change under mu_write, so
+// searches go on while the index is built, and publishing waits for the searches in flight (exclusive lock).
+int build_index(aur_kw* kw) {
+  const auto t0 = std::chrono::steady_clock::now();
+  const int64_t R = static_cast<int64_t>(kw->h_len.size()), P = kw->h_off.back();
+  const int64_t T = static_cast<int64_t>(kw->df.size());   // every term id seen so far (writers resize df)
+  KW_TRY(cudaSetDevice(kw->device));
+  cudaStream_t s = kw->stream;
+  int64_t* toff = nullptr; uint2* tpost = nullptr;
+  DevBuf<unsigned> cnt; DevBuf<unsigned long long> cur;
+  std::vector<int64_t> h_toff(static_cast<size_t>(T) + 1);
+  const unsigned row_blocks = static_cast<unsigned>((R * 32 + 255) / 256);
+  cudaError_t e = cudaMalloc(&toff, (static_cast<size_t>(T) + 1) * 8);
+  if (e == cudaSuccess) e = cudaMalloc(&tpost, static_cast<size_t>(std::max<int64_t>(P, 1)) * 8);
+  if (e == cudaSuccess) e = cnt.reserve(static_cast<size_t>(std::max<int64_t>(T, 1)));
+  if (e == cudaSuccess) e = cur.reserve(static_cast<size_t>(std::max<int64_t>(T, 1)));
+  if (e == cudaSuccess) e = cudaMemsetAsync(cnt.p, 0, static_cast<size_t>(T) * 4, s);
+  if (e == cudaSuccess) {
+    if (R) kw_ix_count<<<row_blocks, 256, 0, s>>>(kw->d_off, kw->d_post, R, cnt.p);
+    kw_ix_scan<<<1, 1024, 0, s>>>(cnt.p, T, toff, cur.p);
+    if (R) kw_ix_scatter<<<row_blocks, 256, 0, s>>>(kw->d_off, kw->d_post, R, cur.p, tpost);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(h_toff.data(), toff, h_toff.size() * 8, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  cnt.release(); cur.release();
+  if (e != cudaSuccess) {
+    cudaFree(toff); cudaFree(tpost);
+    return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "keyword index build: %s",
+                        cudaGetErrorString(e));
+  }
+  const float ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  {
+    std::unique_lock<std::shared_mutex> xl(kw->rw);
+    std::lock_guard<std::mutex> st(kw->mu_stat);
+    std::swap(toff, kw->d_toff); std::swap(tpost, kw->d_tpost);
+    kw->h_toff.swap(h_toff);
+    kw->ix_rows = R; kw->ix_post = P; kw->ix_terms = T;
+    ++kw->ix_builds;
+    kw->ix_build_ms = ms;
+  }
+  cudaFree(toff); cudaFree(tpost);   // the previous index: no search holds it any more
+  return AUR_OK;
+}
+
+// The writer's rule: rebuild once the unindexed tail holds more than 1 / kIxTailFrac of the indexed postings (any
+// postings at all when nothing is indexed).  Caller holds mu_write.
+bool index_due(const aur_kw* kw) {
+  const int64_t tail = kw->h_off.back() - kw->ix_post;
+  return tail > 0 && tail * kIxTailFrac > kw->ix_post;
+}
+
 // ---------------------------------------------------------------------------------------------------------- search
 // One search, over one store or several stores taken as one corpus, in the steps both entry points share: every store's
 // shared lock (in address order), a snapshot of each prefix and its statistics, the query blocks' launch tables built
@@ -424,23 +655,38 @@ int kw_check_query(const KwQuery& q) {
   return AUR_OK;
 }
 
-struct KwSnap { int64_t n_rows = 0, N = 0, total_len = 0; std::vector<int64_t> udf; };
+struct KwSnap {
+  int64_t n_rows = 0, N = 0, total_len = 0, post = 0;
+  std::vector<int64_t> udf;
+  // the term-major index of rows [0, ix_rows) (ix_post postings, terms 0 .. ix_terms - 1); ulen: list length of each
+  // distinct term of the batch
+  const int64_t* toff = nullptr; const uint2* tpost = nullptr;
+  int64_t ix_rows = 0, ix_post = 0, ix_terms = 0;
+  std::vector<int64_t> ulen;
+};
 
-// The published prefix and its statistics, df of the batch's distinct terms uniq, in one read.
+// The published prefix, its statistics, df of the batch's distinct terms uniq and the index, in one read.
 void kw_snapshot(aur_kw* kw, const std::vector<int32_t>& uniq, KwSnap* s) {
   std::lock_guard<std::mutex> st(kw->mu_stat);
-  s->n_rows = kw->rows_pub; s->N = kw->n_live; s->total_len = kw->total_len;
+  s->n_rows = kw->rows_pub; s->N = kw->n_live; s->total_len = kw->total_len; s->post = kw->post_pub;
   s->udf.assign(uniq.size(), 0);
   for (size_t i = 0; i < uniq.size(); ++i)
     s->udf[i] = (uniq[i] >= 0 && uniq[i] < static_cast<int32_t>(kw->df.size())) ? kw->df[static_cast<size_t>(uniq[i])] : 0;
+  s->toff = kw->d_toff; s->tpost = kw->d_tpost;
+  s->ix_rows = kw->ix_rows; s->ix_post = kw->ix_post; s->ix_terms = kw->ix_terms;
+  s->ulen.assign(uniq.size(), 0);
+  for (size_t i = 0; i < uniq.size(); ++i)
+    if (uniq[i] >= 0 && uniq[i] < kw->ix_terms)
+      s->ulen[i] = kw->h_toff[static_cast<size_t>(uniq[i]) + 1] - kw->h_toff[static_cast<size_t>(uniq[i])];
 }
 
 // One launch's query side, the same on every store: idf | hkey | hval | qoff | slot | q_user | q_org [| q_prog |
 // programs used] in one upload.
 struct KwBlock {
   int q0 = 0, nqb = 0, nu = 0, hcap = 0;   // nu = 0: no query of the block has a live term
-  size_t b_hk = 0, b_hv = 0, b_qo = 0, b_sl = 0, b_qu = 0, b_qg = 0, b_qp = 0, b_pu = 0;
+  size_t b_hk = 0, b_hv = 0, b_qo = 0, b_sl = 0, b_qu = 0, b_qg = 0, b_qp = 0, b_pu = 0, b_uk = 0;
   std::vector<unsigned char> tab;
+  std::vector<int32_t> qoff, slot, ug;     // host copies of qoff / slot; ug: unique index -> index into the batch's uniq
 };
 
 // idf of every term with a live posting somewhere (N and udf: the corpus totals), then one table per kKwQBlock queries:
@@ -489,8 +735,14 @@ void kw_plan(const KwQuery& q, const std::vector<int32_t>& uniq, const std::vect
     b.b_qu = b.b_sl + 4 * std::max<size_t>(slot.size(), 1); b.b_qg = b.b_qu + 4 * static_cast<size_t>(nqb);
     b.b_qp = b.b_qg + 4 * static_cast<size_t>(nqb); b.b_pu = b.b_qp + 4 * static_cast<size_t>(nqb);
     const int n_passes = q.fp ? (q.fp->n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms : 0;
-    b.tab.assign(q.fp ? b.b_pu + 4 * static_cast<size_t>(n_passes) : b.b_qp, 0);
+    b.b_uk = q.fp ? b.b_pu + 4 * static_cast<size_t>(n_passes) : b.b_qp;
+    b.tab.assign(b.b_uk + 4 * static_cast<size_t>(nu), 0);
     unsigned char* tab = b.tab.data();
+    memcpy(tab + b.b_uk, ukeys.data(), 4 * static_cast<size_t>(nu));
+    b.ug.resize(static_cast<size_t>(nu));
+    for (int u = 0; u < nu; ++u)
+      b.ug[static_cast<size_t>(u)] = static_cast<int32_t>(std::lower_bound(uniq.begin(), uniq.end(), ukeys[static_cast<size_t>(u)]) - uniq.begin());
+    b.qoff = qoff; b.slot = slot;
     memcpy(tab, uidf.data(), 8 * static_cast<size_t>(nu));
     memcpy(tab + b.b_hk, hkey.data(), 4 * static_cast<size_t>(hcap));
     memcpy(tab + b.b_hv, hval.data(), 4 * static_cast<size_t>(hcap));
@@ -513,14 +765,51 @@ void kw_plan(const KwQuery& q, const std::vector<int32_t>& uniq, const std::vect
   }
 }
 
+// Blocks that own contiguous ranges of whole rounds of n rows, at most max_blocks of them; *rpb = rows per block.
+int kw_grid(int64_t n, int64_t max_blocks, int64_t* rpb) {
+  const int64_t rounds = (n + kKwRoundRows - 1) / kKwRoundRows;
+  const int64_t grid = std::max<int64_t>(1, std::min<int64_t>(max_blocks, rounds));
+  *rpb = (rounds + grid - 1) / grid * kKwRoundRows;
+  return static_cast<int>((n + *rpb - 1) / *rpb);
+}
+
+// How one launch (query block b) scores the indexed rows [0, rows) of the snapshot: rows = 0 leaves every row to the
+// forward scan.  The index serves a block whose queries have at most kIxMaxTermPos terms, in groups of `group` queries
+// whose accumulators fit kIxAccBytes, and (kw_path auto) when its estimated time -- a launch per term position and
+// group, the lists it reads (`postings`, dead rows included), the accumulator scan -- is below the forward scan's of the
+// same rows.
+struct KwIxPlan { int64_t rows = 0, postings = 0; int group = 0; };
+KwIxPlan kw_ix_plan(const aur_kw* kw, const KwSnap& sn, const KwBlock& b) {
+  KwIxPlan x;
+  const int mode = kw->kw_path.load(std::memory_order_relaxed);
+  const int64_t R = sn.ix_rows;
+  if (mode == 1 || R == 0) return x;
+  int J = 0;
+  for (int i = 0; i < b.nqb; ++i) J = std::max(J, b.qoff[static_cast<size_t>(i) + 1] - b.qoff[static_cast<size_t>(i)]);
+  const int64_t gmax = kIxAccBytes / (8 * R);
+  if (J > kIxMaxTermPos || gmax < 1) return x;
+  const int group = static_cast<int>(std::min<int64_t>(b.nqb, gmax));
+  int64_t L = 0;
+  for (int32_t u : b.slot) L += sn.ulen[static_cast<size_t>(b.ug[static_cast<size_t>(u)])];
+  if (mode == 0) {
+    const int n_groups = (b.nqb + group - 1) / group;
+    const double t_ix = n_groups * (J + 1) * kIxNsPerLaunch + static_cast<double>(L) * kIxNsPerPosting +
+                        static_cast<double>(b.nqb) * static_cast<double>(R) * kIxNsPerAcc;
+    if (!(t_ix < static_cast<double>(sn.ix_post) * kFwdNsPerPosting)) return x;
+  }
+  x.rows = R; x.postings = L; x.group = group;
+  return x;
+}
+
 // Enqueue one store's part of the search on c's stream: allow-list flags, then per block the table upload, the scoring
-// pass over the store's prefix n_rows and the folds into c's [nq][k] output.  Nothing waits.
-int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>& blocks, int64_t n_rows, int64_t N,
+// of the store's prefix sn.n_rows (index and / or forward scan) and the folds into c's [nq][k] output.  Nothing waits.
+int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>& blocks, const KwSnap& sn, int64_t N,
               double avgdl) {
   KW_TRY(cudaSetDevice(kw->device));
   cudaStream_t s = c->stream;
   const int k = q.k;
-  c->launches = 0; c->terms = 0; c->spilled = 0;
+  const int64_t n_rows = sn.n_rows;
+  c->launches = 0; c->terms = 0; c->spilled = 0; c->path = 0; c->postings = 0;
   KW_TRY(cudaEventRecord(c->ev0, s));
   const uint8_t* d_allow = nullptr;
   if (q.allow) {
@@ -593,22 +882,18 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
     }
     KW_TRY(c->tab.reserve(b.tab.size()));
     KW_TRY(cudaMemcpyAsync(c->tab.p, b.tab.data(), b.tab.size(), cudaMemcpyHostToDevice, s));   // pageable: staged before return
-    // geometry: blocks own contiguous row ranges of whole rounds
-    const int64_t rounds = (n_rows + kKwRoundRows - 1) / kKwRoundRows;
-    const int64_t grid = std::max<int64_t>(1, std::min<int64_t>(2 * kw->sm_count, rounds));
-    const int64_t rpb = (rounds + grid - 1) / grid * kKwRoundRows;
-    const int g = static_cast<int>((n_rows + rpb - 1) / rpb);
     const int ksel = k;
-    size_t smem = static_cast<size_t>(nqb) * sizeof(Cand) + kKwWarps * kKwBufCap * sizeof(Cand) + 4 * static_cast<size_t>(nqb);
-    smem = (smem + 15) & ~size_t(15);
-    const size_t cval_smem = static_cast<size_t>(kKwWarps) * nu * 8;
-    const bool in_smem = smem + cval_smem <= kw->smem_optin;
     c->terms = std::max(c->terms, nu);
-    if (!in_smem) ++c->spilled;
-    if (in_smem) smem += cval_smem;
-    else KW_TRY(c->cval.reserve(static_cast<size_t>(g) * kKwWarps * nu));
-    KW_TRY(c->buf.reserve(static_cast<size_t>(g) * nqb * kKwBufCap));
-    KW_TRY(c->lists_a.reserve(static_cast<size_t>(nqb) * g * ksel));
+    // rows [0, R) from the term-major index when the path rule picks it, rows [R, n_rows) by the forward scan; the
+    // index part's per-block lists come first, the forward part's after them
+    const KwIxPlan ix = kw_ix_plan(kw, sn, b);
+    const int64_t R = ix.rows, tail = n_rows - R;
+    int64_t rpb_i = 0, rpb_t = 0;
+    const int gi = R > 0 ? kw_grid(R, kIxSelBlocksPerSm * static_cast<int64_t>(kw->sm_count), &rpb_i) : 0;
+    const int gt = tail > 0 ? kw_grid(tail, 2 * static_cast<int64_t>(kw->sm_count), &rpb_t) : 0;
+    int n_lists = gi + gt;   // folded below
+    KW_TRY(c->buf.reserve(static_cast<size_t>(std::max(gi, gt)) * nqb * kKwBufCap));
+    KW_TRY(c->lists_a.reserve(static_cast<size_t>(nqb) * n_lists * ksel));
     KwParams p{};
     p.off = kw->d_off; p.post = kw->d_post; p.len = kw->d_len; p.ids = kw->d_ids; p.user = kw->d_user; p.org = kw->d_org;
     p.live = kw->d_live; p.allow = d_allow; p.n_rows = n_rows;
@@ -619,20 +904,83 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
     p.q_user = q.user ? reinterpret_cast<const int32_t*>(c->tab.p + b.b_qu) : nullptr;
     p.q_org = q.user ? reinterpret_cast<const int32_t*>(c->tab.p + b.b_qg) : nullptr;
     p.nq = nqb; p.ksel = ksel; p.avgdl = avgdl;
-    p.cval_global = in_smem ? nullptr : c->cval.p;
-    p.buf = c->buf.p; p.lists = c->lists_a.p; p.rows_per_block = rpb;
+    p.buf = c->buf.p; p.lists = c->lists_a.p;
     if (d_fmask) {
       p.fmask = d_fmask; p.fmask_stride = n_rows; p.n_passes = n_passes;
       p.q_prog = reinterpret_cast<const int32_t*>(c->tab.p + b.b_qp);
       p.prog_used = reinterpret_cast<const uint32_t*>(c->tab.p + b.b_pu);
-      kw_score_kernel<true><<<g, kKwThreads, smem, s>>>(p, in_smem ? 1 : 0);
-    } else {
-      kw_score_kernel<false><<<g, kKwThreads, smem, s>>>(p, in_smem ? 1 : 0);
     }
-    KW_TRY(cudaGetLastError());
-    c->launches += 1;
+    if (R > 0) {
+      const size_t acc_n = static_cast<size_t>(ix.group) * static_cast<size_t>(R);
+      if (c->acc.n < acc_n) { KW_TRY(c->acc.reserve(acc_n)); c->acc_clean = false; }
+      if (!c->acc_clean) KW_TRY(cudaMemsetAsync(c->acc.p, 0, c->acc.n * 8, s));
+      c->acc_clean = false;   // until every group's selection has been enqueued
+      for (int g0 = 0; g0 < nqb; g0 += ix.group) {
+        const int ng = std::min(ix.group, nqb - g0);
+        int J = 0;
+        for (int i = g0; i < g0 + ng; ++i) J = std::max(J, b.qoff[static_cast<size_t>(i) + 1] - b.qoff[static_cast<size_t>(i)]);
+        KwIxTerm t{sn.tpost, sn.toff, sn.ix_terms, kw->d_len, reinterpret_cast<const int32_t*>(c->tab.p + b.b_uk), p.idf,
+                   p.q_off + g0, p.slot_u, c->acc.p, R, avgdl, 0};
+        for (int j = 0; j < J; ++j) {
+          int64_t longest = 0;   // the longest list this launch reads
+          for (int i = g0; i < g0 + ng; ++i) {
+            const int32_t g = b.qoff[static_cast<size_t>(i)] + j;
+            if (g < b.qoff[static_cast<size_t>(i) + 1])
+              longest = std::max(longest, sn.ulen[static_cast<size_t>(b.ug[static_cast<size_t>(b.slot[static_cast<size_t>(g)])])]);
+          }
+          if (longest == 0) continue;   // nothing to add at this position
+          t.j = j;
+          const unsigned gx = static_cast<unsigned>(std::min<int64_t>((longest + 1023) / 1024, 65535));
+          kw_ix_term_kernel<<<dim3(gx, static_cast<unsigned>(ng)), 256, 0, s>>>(t);
+          KW_TRY(cudaGetLastError());
+          c->launches += 1;
+        }
+        KwParams ps = p;
+        ps.n_rows = R; ps.nq = ng; ps.rows_per_block = rpb_i;
+        ps.lists = c->lists_a.p + static_cast<size_t>(g0) * n_lists * ksel;
+        if (p.q_user) { ps.q_user = p.q_user + g0; ps.q_org = p.q_org + g0; }
+        if (p.q_prog) ps.q_prog = p.q_prog + g0;
+        const size_t smem = static_cast<size_t>(ng) * sizeof(Cand) + kKwWarps * kKwBufCap * sizeof(Cand) + 4 * static_cast<size_t>(ng);
+        if (d_fmask) kw_ix_select_kernel<true><<<gi, kKwThreads, smem, s>>>(ps, c->acc.p, R, n_lists);
+        else kw_ix_select_kernel<false><<<gi, kKwThreads, smem, s>>>(ps, c->acc.p, R, n_lists);
+        KW_TRY(cudaGetLastError());
+        c->launches += 1;
+      }
+      c->acc_clean = true;
+      c->path |= AUR_KW_PATH_INDEX;
+      c->postings += ix.postings;
+    }
+    if (tail > 0) {
+      // kw_score_kernel over rows [R, n_rows): every row-indexed array starts at row R
+      const int g = gt;
+      size_t smem = static_cast<size_t>(nqb) * sizeof(Cand) + kKwWarps * kKwBufCap * sizeof(Cand) + 4 * static_cast<size_t>(nqb);
+      smem = (smem + 15) & ~size_t(15);
+      const size_t cval_smem = static_cast<size_t>(kKwWarps) * nu * 8;
+      const bool in_smem = smem + cval_smem <= kw->smem_optin;
+      if (!in_smem) ++c->spilled;
+      if (in_smem) smem += cval_smem;
+      else KW_TRY(c->cval.reserve(static_cast<size_t>(g) * kKwWarps * nu));
+      if (gi) KW_TRY(c->lists_b.reserve(static_cast<size_t>(nqb) * g * ksel));
+      KwParams pf = p;
+      pf.off += R; pf.len += R; pf.ids += R; pf.user += R; pf.org += R; pf.live += R;
+      if (pf.allow) pf.allow += R;
+      if (pf.fmask) pf.fmask += R;
+      pf.n_rows = tail; pf.rows_per_block = rpb_t;
+      pf.cval_global = in_smem ? nullptr : c->cval.p;
+      pf.lists = gi ? c->lists_b.p : c->lists_a.p;
+      if (d_fmask) kw_score_kernel<true><<<g, kKwThreads, smem, s>>>(pf, in_smem ? 1 : 0);
+      else kw_score_kernel<false><<<g, kKwThreads, smem, s>>>(pf, in_smem ? 1 : 0);
+      KW_TRY(cudaGetLastError());
+      c->launches += 1;
+      if (gi) {   // into lists gi .. n_lists - 1 of every query
+        const size_t w = static_cast<size_t>(g) * ksel * sizeof(Cand);
+        KW_TRY(cudaMemcpy2DAsync(c->lists_a.p + static_cast<size_t>(gi) * ksel, static_cast<size_t>(n_lists) * ksel * sizeof(Cand),
+                                 c->lists_b.p, w, w, static_cast<size_t>(nqb), cudaMemcpyDeviceToDevice, s));
+      }
+      c->path |= AUR_KW_PATH_FORWARD;
+      c->postings += sn.post - (R > 0 ? sn.ix_post : 0);
+    }
     // fold the per-block lists until one sorted list per query remains
-    int n_lists = g;
     Cand* cur = c->lists_a.p;
     bool in_a = true;
     const int group = std::max(1, kKwFoldCap / ksel);
@@ -667,6 +1015,7 @@ int kw_publish(aur_kw* kw, KwCtx* c) {
   std::lock_guard<std::mutex> lk(kw->mu_pool);
   kw->last_launches = c->launches; kw->last_ms = ms;
   kw->last_terms = c->terms; kw->last_spilled = c->spilled;
+  kw->last_path = c->path; kw->last_postings = c->postings;
   return AUR_OK;
 }
 
@@ -740,7 +1089,7 @@ int kw_run(aur_kw* const* stores, int n, const KwQuery& q, After&& after) {
     ctxs.v.emplace_back(kw, c);
     cs.push_back(c);
     const KwSnap& sn = pl.snaps[static_cast<size_t>(s)];
-    if ((rc = kw_launch(kw, c, q, pl.blocks, sn.n_rows, pl.N, pl.avgdl)) != AUR_OK) return rc;
+    if ((rc = kw_launch(kw, c, q, pl.blocks, sn, pl.N, pl.avgdl)) != AUR_OK) return rc;
   }
   return after(cs, pl.snaps);
 }
@@ -799,6 +1148,11 @@ int kw_check_columns(aur_kw* kw, const FiltProgs& fp) {
 int kw_device(const aur_kw* kw) { return kw->device; }
 }  // namespace aur
 
+namespace {
+int kw_append(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes, const int32_t* term_ids,
+              const int32_t* tfs, const int64_t* offsets, int64_t n, int64_t total, int32_t max_term);
+}  // namespace
+
 extern "C" {
 
 int aur_kw_open(int32_t device, int64_t doc_capacity, int64_t postings_capacity, aur_kw** out) {
@@ -848,7 +1202,7 @@ int aur_kw_close(aur_kw* kw) {
   if (kw->stream) cudaStreamSynchronize(kw->stream);   // this store's work only: other users of the GPU are not waited on
   for (auto& c : kw->ctxs) cudaStreamSynchronize(c->stream);
   cudaFree(kw->d_off); cudaFree(kw->d_len); cudaFree(kw->d_ids); cudaFree(kw->d_user); cudaFree(kw->d_org);
-  cudaFree(kw->d_live); cudaFree(kw->d_post);
+  cudaFree(kw->d_live); cudaFree(kw->d_post); cudaFree(kw->d_toff); cudaFree(kw->d_tpost);
   for (int32_t* a : kw->d_attr) cudaFree(a);
   kw->attr_stage.release();
   for (auto& c : kw->ctxs) c->release();
@@ -884,6 +1238,19 @@ int aur_kw_add(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const 
     if (dl > 0x7FFFFFFF) return report_error(AUR_ERR_INVALID, "document longer than 2^31 - 1 tokens");
   }
   std::lock_guard<std::mutex> wk(kw->mu_write);
+  const int rc = kw_append(kw, ids, user_codes, org_codes, term_ids, tfs, offsets, n, total, max_term);
+  // a failed rebuild (out of memory, say) keeps the previous index and leaves the appended rows to the forward scan:
+  // the documents are in, and aur_kw_reindex reports the error
+  if (rc == AUR_OK && index_due(kw)) build_index(kw);
+  return rc;
+}
+
+}  // extern "C"
+
+namespace {
+// aur_kw_add's append and publication of n checked documents; the caller holds mu_write.
+int kw_append(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes, const int32_t* term_ids,
+              const int32_t* tfs, const int64_t* offsets, int64_t n, int64_t total, int32_t max_term) {
   const int64_t base = static_cast<int64_t>(kw->h_len.size());
   if (base + n > kw->capacity)
     return report_error(AUR_ERR_NOMEM, "keyword store full: %lld + %lld > capacity %lld (aur_kw_compact reclaims tombstones)",
@@ -954,6 +1321,9 @@ int aur_kw_add(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const 
   kw->post_pub = post0 + total;
   return AUR_OK;
 }
+}  // namespace
+
+extern "C" {
 
 int aur_kw_remove(aur_kw* kw, const int64_t* ids, int64_t n, int64_t* removed) {
   if (!kw || (n > 0 && !ids) || n < 0) return report_error(AUR_ERR_INVALID, "null argument or n < 0");
@@ -986,6 +1356,8 @@ int aur_kw_compact(aur_kw* kw, int64_t* reclaimed) {
   for (int64_t r = 0; r < rows; ++r) if (kw->h_live[static_cast<size_t>(r)]) map.push_back(static_cast<int32_t>(r));
   const int64_t nl = static_cast<int64_t>(map.size());
   if (nl == rows) return AUR_OK;
+  const bool reindex = kw->ix_rows > 0;   // rows move: the index is rebuilt over the compacted store
+  drop_index(kw);
   // stable: live rows keep their order; postings go to a fresh array of the same capacity
   std::vector<int64_t> off(static_cast<size_t>(nl) + 1, 0), ids(static_cast<size_t>(nl));
   std::vector<int32_t> len(static_cast<size_t>(nl)), user(static_cast<size_t>(nl)), org(static_cast<size_t>(nl));
@@ -1036,11 +1408,14 @@ int aur_kw_compact(aur_kw* kw, int64_t* reclaimed) {
   kw->h_off = off; kw->h_len = len; kw->h_ids = ids; kw->h_user = user; kw->h_org = org; kw->h_live = live;
   kw->id2row.clear();
   for (int64_t j = 0; j < nl; ++j) kw->id2row[ids[static_cast<size_t>(j)]] = j;
-  std::lock_guard<std::mutex> st(kw->mu_stat);
-  kw->rows_pub = nl;
-  kw->post_pub = off.back();
+  {
+    std::lock_guard<std::mutex> st(kw->mu_stat);
+    kw->rows_pub = nl;
+    kw->post_pub = off.back();
+  }
   if (reclaimed) *reclaimed = rows - nl;
-  return AUR_OK;
+  xl.unlock();
+  return reindex ? build_index(kw) : AUR_OK;
 }
 
 int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out) {
@@ -1128,6 +1503,39 @@ int aur_kw_search_multi(aur_kw* const* stores, int32_t n_stores, const int32_t* 
   if ((rc = kw_search_stores(stores, n_stores, q, ls.data(), li.data(), snapshot_rows_out)) != AUR_OK) return rc;
   // every store's lists are sorted by (fp64 score desc, id asc) with (-inf, -1) padding last: one k-way merge per query
   return aur_merge_topk_host_f64(ls.data(), li.data(), n_stores, nq, k, k, scores_out, ids_out);
+}
+
+int aur_kw_reindex(aur_kw* kw) {
+  if (!kw) return report_error(AUR_ERR_INVALID, "null store");
+  std::lock_guard<std::mutex> wk(kw->mu_write);
+  return build_index(kw);
+}
+
+int aur_kw_set_option(aur_kw* kw, const char* name, int64_t value) {
+  if (!kw || !name) return report_error(AUR_ERR_INVALID, "null argument");
+  if (strcmp(name, "kw_path") == 0) {
+    if (value < 0 || value > 2) return report_error(AUR_ERR_INVALID, "kw_path must be 0 (auto), 1 (forward) or 2 (index)");
+    kw->kw_path.store(static_cast<int>(value));
+    return AUR_OK;
+  }
+  return report_error(AUR_ERR_INVALID, "unknown keyword store option '%s'", name);
+}
+
+int aur_kw_get_index_stats(aur_kw* kw, aur_kw_index_stats* out) {
+  if (!kw || !out) return report_error(AUR_ERR_INVALID, "null argument");
+  memset(out, 0, sizeof *out);
+  {
+    std::lock_guard<std::mutex> st(kw->mu_stat);
+    out->indexed_rows = kw->ix_rows;
+    out->index_postings = kw->ix_post;
+    out->index_bytes = kw->d_toff ? kw->ix_post * 8 + (kw->ix_terms + 1) * 8 : 0;
+    out->builds = kw->ix_builds;
+    out->last_build_ms = kw->ix_build_ms;
+  }
+  std::lock_guard<std::mutex> lk(kw->mu_pool);
+  out->last_path = kw->last_path;
+  out->last_postings = kw->last_postings;
+  return AUR_OK;
 }
 
 }  // extern "C"

@@ -487,6 +487,23 @@ class KeywordIndex:
         N.check(self._lib.aur_kw_search(self._h, *a["args"], C.byref(snap)))
         return a["ids"], a["scores"], int(snap.value)
 
+    def reindex(self) -> None:
+        """Build the term-major index over every document now (aur_kw_reindex); the writer path also does this on its
+        own once the unindexed documents hold more than 1/8 of the indexed postings."""
+        N.check(self._lib.aur_kw_reindex(self._h))
+
+    def index_stats(self) -> dict:
+        """The term-major index (indexed rows, postings, bytes, builds, last build ms) and the last search's path
+        (``last_path``: N.KW_PATH_* bits) and postings read."""
+        st = N.AurKwIndexStats()
+        N.check(self._lib.aur_kw_get_index_stats(self._h, C.byref(st)))
+        return {f: getattr(st, f) for f, _ in N.AurKwIndexStats._fields_}
+
+    def set_path(self, path: int) -> None:
+        """Force how searches score the indexed rows, for tests and A/B runs: N.KW_PATH_AUTO_OPT (the cost rule),
+        N.KW_PATH_FORWARD_OPT or N.KW_PATH_INDEX_OPT.  Answers do not depend on it."""
+        N.check(self._lib.aur_kw_set_option(self._h, b"kw_path", int(path)))
+
 
 def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_offsets,
                   w_dense, w_sparse=None, fusion: int = N.FUSION_RANKED, k_out: Optional[int] = None, q_user=None,
@@ -674,6 +691,16 @@ class MultiKeywordIndex:
         out["last_ms"] = max(p["last_ms"] for p in per)
         out["stores"] = per
         return out
+
+    def reindex(self) -> None:
+        self._each(lambda s, store: store.reindex())
+
+    def index_stats(self) -> list:
+        """KeywordIndex.index_stats of every store (each store is indexed and searched on its own path)."""
+        return self._each(lambda s, store: store.index_stats())
+
+    def set_path(self, path: int) -> None:
+        self._each(lambda s, store: store.set_path(path))
 
     def search(self, q_terms, q_offsets, k: int, q_user=None, q_org=None, allow_ids=None):
         """(ids [nq,k] int64, scores [nq,k] float64, snapshot rows [n stores]): KeywordIndex.search over the union of the

@@ -349,6 +349,33 @@ int aur_kw_search_multi(aur_kw* const* stores, int32_t n_stores, const int32_t* 
                         int32_t nq, int32_t k, const int32_t* q_user, const int32_t* q_org, const int64_t* allow_ids,
                         int64_t n_allow, double* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out);
 
+/* Term-major index (DESIGN.md section 10): besides its forward postings, a store holds an index of its first R rows
+ * (the indexed prefix), every term's (row, tf) list, from which a search reads only its own terms' postings; rows
+ * [R, rows) are scanned forward.  Answers are bit-identical whichever way a row is scored.  The index is built on the
+ * store's stream by aur_kw_reindex, by aur_kw_add once the unindexed rows hold more than 1/8 of the indexed postings
+ * (a build that fails there leaves the previous index in place; the add still succeeds), and by aur_kw_compact.  A
+ * build runs beside searches and waits for those in flight before it is published; it takes 8 B per indexed posting
+ * plus 8 B per term id, twice that while the old index is still held. */
+typedef struct aur_kw_index_stats {
+  int64_t indexed_rows;       /* R                                                   */
+  int64_t index_postings;     /* postings in the index (those of rows [0, R))        */
+  int64_t index_bytes;        /* HBM the index holds                                 */
+  int64_t builds;             /* builds published since open                         */
+  float   last_build_ms;      /* host time of the last one, device work included     */
+  int32_t last_path;          /* the last search's AUR_KW_PATH_* bits (0: it scored nothing) */
+  int64_t last_postings;      /* postings the last search read: its terms' lists in the index, every posting of
+                                 the rows it scanned forward                         */
+} aur_kw_index_stats;
+#define AUR_KW_PATH_FORWARD 1  /* some rows scanned forward */
+#define AUR_KW_PATH_INDEX 2    /* some rows scored from the index */
+/* Index every appended row now (the writers' serialisation is held while it builds). */
+int aur_kw_reindex(aur_kw* kw);
+/* "kw_path": 0 auto (the cost rule picks per launch), 1 forward scan only, 2 the index wherever it can serve (a launch
+ * whose queries have more than 64 terms is still scanned forward).  For tests and A/B runs: answers do not change.
+ * Unknown names and values: AUR_ERR_INVALID. */
+int aur_kw_set_option(aur_kw* kw, const char* name, int64_t value);
+int aur_kw_get_index_stats(aur_kw* kw, aur_kw_index_stats* out);
+
 /* ------------------------------------------------------------------ hybrid query
  * collection.query.hybrid (weaviate_client.py:252-259) in one call: the dense leg (aur_search_ex of queries_host over
  * ix, top-fetch cosines) and the keyword leg (aur_kw_search of q_terms / q_offsets over kw, top-fetch BM25 scores) run
