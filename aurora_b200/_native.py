@@ -31,6 +31,8 @@ EXPORTS = [
     "aur_debug_tc_scores",
     "aur_kw_open", "aur_kw_close", "aur_kw_add", "aur_kw_remove", "aur_kw_compact", "aur_kw_get_stats", "aur_kw_set_attrs",
     "aur_kw_search", "aur_kw_search_multi", "aur_kw_reindex", "aur_kw_set_option", "aur_kw_get_index_stats",
+    "aur_kw_read_rows", "aur_kw_vocab_open", "aur_kw_vocab_close", "aur_kw_vocab_size", "aur_kw_vocab_read",
+    "aur_kw_vocab_set_option", "aur_kw_add_text",
     "aur_hybrid_search", "aur_hybrid_search_multi", "aur_hybrid_search_filtered",
     "aur_encoder_open", "aur_encoder_close", "aur_encoder_load", "aur_encode", "aur_encode_append",
     "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
@@ -153,6 +155,13 @@ def load():
         "aur_kw_reindex": (C.c_int, [vp]),
         "aur_kw_set_option": (C.c_int, [vp, C.c_char_p, i64]),
         "aur_kw_get_index_stats": (C.c_int, [vp, C.POINTER(AurKwIndexStats)]),
+        "aur_kw_read_rows": (C.c_int, [vp, i64, i64, vp, vp, vp, vp, i64, C.POINTER(i64)]),
+        "aur_kw_vocab_open": (C.c_int, [i32, C.POINTER(vp)]),
+        "aur_kw_vocab_close": (C.c_int, [vp]),
+        "aur_kw_vocab_size": (C.c_int, [vp, C.POINTER(i64), C.POINTER(i64)]),
+        "aur_kw_vocab_read": (C.c_int, [vp, i64, i64, vp, i64, vp]),
+        "aur_kw_vocab_set_option": (C.c_int, [vp, C.c_char_p, i64]),
+        "aur_kw_add_text": (C.c_int, [vp, i32, vp, vp, vp, vp, C.c_char_p, vp, i64]),
         "aur_hybrid_search": (C.c_int, [vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]),
         "aur_hybrid_search_multi": (C.c_int, [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp, vp]),
         "aur_hybrid_search_filtered": (C.c_int, [vp, vp, i32, vp, i32, i32, vp, vp, vp, vp, i32, vp, i64, vp, i64, vp, vp,

@@ -8,8 +8,9 @@ not in /root/reference -- so this restates Weaviate 1.27's documented behaviour:
 b = 0.75, "word" tokenisation (lower-case, split on non-alphanumerics), idf = ln(1 + (N - n + 0.5) /
 (n + 0.5)); rankedFusion with the constant 60 and 0-based ranks.  Unpinned: the reference has no test
 at this boundary (SURVEY.md section 8c).  ``BM25Index`` is the host index (the path of the test doubles and
-the definition the device is held to); ``DeviceBM25`` keeps the vocabulary and tokenisation on the host and the
-postings, scoring and top-k in the GPU keyword store (csrc/keyword.cu, DESIGN.md section 10).  ``ranked_fusion`` and
+the definition the device is held to); ``DeviceBM25`` analyses text into the GPU keyword store on the device
+(csrc/kw_text.cu, ``build_csr``'s ids and rows bit for bit) and keeps postings, scoring and top-k there
+(csrc/keyword.cu, DESIGN.md section 10), with a host mirror of the vocabulary that maps queries.  ``ranked_fusion`` and
 ``relative_score_fusion`` (Weaviate's other fusion, HybridFusion.RELATIVE_SCORE) define the fused score; the device
 fusion of ``DeviceBM25.search_batch(..., dense=...)`` (csrc/hybrid.cu, DESIGN.md section 11) equals them bit for bit.
 """
@@ -188,18 +189,32 @@ def query_csr(vocab: Dict[str, int], queries: Iterable[str]):
 class DeviceBM25:
     """The keyword leg on the GPU (``engine.KeywordIndex``), with ``BM25Index``'s surface plus ``search_batch``.
 
-    Scores and order are those of ``BM25Index.search`` on its loop path, bit for bit (DESIGN.md section 10).  Holds the
-    vocabulary (word -> int32 term id, grow-only; a reloaded knowledge base rebuilds it from the texts) and tenant codes
-    per document, so a tenant scope is applied on the device like the dense leg's."""
+    Scores and order are those of ``BM25Index.search`` on its loop path, bit for bit (DESIGN.md section 10).  The
+    vocabulary (word -> int32 term id, grow-only; a reloaded knowledge base rebuilds it from the texts) lives on the
+    store's GPU (``engine.KeywordVocab``; store 0's for a ``MultiKeywordIndex``), where ``add_many`` analyses the text;
+    ``vocab`` is its host mirror, brought up to date after every add.  A store without ``add_text`` (the CPU test
+    doubles) is fed ``build_csr`` instead.  Tenant codes are kept per document, so a tenant scope is applied on the
+    device like the dense leg's.  Safe to use from several threads."""
 
     def __init__(self, capacity: int = 1 << 20, device: int = 0, postings_capacity: int = 0, store=None):
+        import threading
+
         if store is None:
             from .engine import KeywordIndex
 
             store = KeywordIndex(capacity, postings_capacity=postings_capacity, device=device)
         self.store = store
-        self.vocab: Dict[str, int] = {}
+        self.vocab: Dict[str, int] = {}     # host mirror of the device vocabulary: query_csr maps queries with it
         self._docs: set = set()
+        # a store that analyses text on the GPU gets a device vocabulary on its (first store's) device
+        self._dvocab = None
+        if hasattr(store, "add_text"):
+            from .engine import KeywordVocab
+
+            self._dvocab = KeywordVocab(store.stores[0].device if hasattr(store, "stores") else store.device)
+        # held across an add and the mirror's update, and across a query's mapping and its search, so a search never
+        # maps its terms with a mirror that is behind the rows it scores
+        self._lock = threading.RLock()
 
     def __len__(self) -> int:
         return len(self._docs)
@@ -214,9 +229,27 @@ class DeviceBM25:
         doc_ids = np.asarray(doc_ids, dtype=np.int64)
         if len(doc_ids) == 0:
             return
-        terms, tfs, offsets = build_csr(self.vocab, texts)
-        self.store.add(doc_ids, terms, tfs, offsets, user_codes, org_codes)
-        self._docs.update(int(d) for d in doc_ids)
+        with self._lock:
+            if self._dvocab is None:
+                terms, tfs, offsets = build_csr(self.vocab, texts)
+                self.store.add(doc_ids, terms, tfs, offsets, user_codes, org_codes)
+            else:
+                try:
+                    self.store.add_text(self._dvocab, doc_ids, texts, user_codes, org_codes)
+                except BaseException:
+                    try:    # a failed add may still have added words (as build_csr does)
+                        self._sync_vocab()
+                    except Exception:
+                        pass    # the add's error is the one to report; the next add brings the mirror up to date
+                    raise
+                self._sync_vocab()
+            self._docs.update(int(d) for d in doc_ids)
+
+    def _sync_vocab(self) -> None:
+        """Bring the host mirror up to date: read only the ids it does not have yet."""
+        have = len(self.vocab)
+        for i, w in enumerate(self._dvocab.read(have), have):
+            self.vocab[w] = i
 
     def remove(self, doc_id: int) -> bool:
         return self.remove_many([doc_id]) > 0
@@ -278,9 +311,10 @@ class DeviceBM25:
                     q_program=None, max_list_rows=0):
         from .engine import hybrid_search
 
-        q_terms, q_off = query_csr(self.vocab, queries)
-        ids, scores, cosine, _ = hybrid_search(index, self.store, vectors, fetch, q_terms, q_off, w_dense, None, fusion,
-                                               k_out, q_user, q_org, programs, q_program, max_list_rows)
+        with self._lock:
+            q_terms, q_off = query_csr(self.vocab, queries)
+            ids, scores, cosine, _ = hybrid_search(index, self.store, vectors, fetch, q_terms, q_off, w_dense, None, fusion,
+                                                   k_out, q_user, q_org, programs, q_program, max_list_rows)
         out = []
         for row_i, row_s, row_c in zip(ids, scores, cosine):
             n = int((row_i >= 0).sum())
@@ -289,8 +323,9 @@ class DeviceBM25:
         return out
 
     def _run(self, queries, limit, q_user, q_org, allow_ids):
-        q_terms, q_off = query_csr(self.vocab, queries)
-        ids, scores, _ = self.store.search(q_terms, q_off, int(limit), q_user, q_org, allow_ids)
+        with self._lock:
+            q_terms, q_off = query_csr(self.vocab, queries)
+            ids, scores, _ = self.store.search(q_terms, q_off, int(limit), q_user, q_org, allow_ids)
         out = []
         for row_i, row_s in zip(ids, scores):
             n = int((row_i >= 0).sum())

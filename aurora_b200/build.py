@@ -14,7 +14,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libaurora_b200.so")
-SOURCES = ["capi.cu", "kernels_simt.cu", "simtopk_tc.cu", "encoder.cu", "encoder_simt.cu", "gemm_tc.cu", "attn_tc.cu", "keyword.cu", "hybrid.cu", "listsearch.cu", "filter.cu", "tokenizer.cpp", "host_merge.cpp"]
+SOURCES = ["capi.cu", "kernels_simt.cu", "simtopk_tc.cu", "encoder.cu", "encoder_simt.cu", "gemm_tc.cu", "attn_tc.cu", "keyword.cu", "kw_text.cu", "hybrid.cu", "listsearch.cu", "filter.cu", "tokenizer.cpp", "host_merge.cpp"]
 HEADERS = ["internal.h", "ptx.cuh", "unicode_tables.inc", os.path.join("..", "..", "include", "aurora_b200.h")]
 
 PROFILE = bool(int(os.environ.get("AUR_TC_PROFILE", "0")))   # bring-up timers in the tensor-core similarity kernel

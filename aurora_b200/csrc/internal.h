@@ -6,6 +6,7 @@
 #include <stdlib.h>
 
 #include <functional>
+#include <mutex>
 #include <vector>
 
 struct aur_index;
@@ -357,6 +358,22 @@ int kw_legs(aur_kw* const* stores, int n, const int32_t* q_terms, const int64_t*
 int kw_check(const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k);   // aur_kw_search's query checks
 int kw_check_columns(aur_kw* kw, const FiltProgs& fp);   // every attribute column fp's leaves name was set on kw
 int kw_device(const aur_kw* kw);
+// The store side of a text add (kw_text.cu): the rows of one batch as aur_kw_add publishes them.  Callers hold the
+// store's mu_write (kw_write_mutex) and have checked the arguments and the room (kw_check_room).  land(dst, stream)
+// enqueues the copy of the rows' total postings (term id, tf) to the store's device memory dst on the store's stream.
+struct KwRows {
+  const int64_t* ids; const int32_t* user; const int32_t* org;   // [n]; user / org nullable (0 / -1)
+  const int64_t* offsets;    // [n + 1] from 0: row i's postings
+  const int32_t* term_ids;   // [total] host copy of the postings' term ids (df)
+  const int32_t* len;        // [n] document lengths (sum of tf)
+  int64_t n, total; int32_t max_term;
+};
+using KwLand = std::function<cudaError_t(uint2* dst, cudaStream_t s)>;
+int kw_check_room(aur_kw* kw, int64_t n);                         // AUR_ERR_NOMEM when n more rows do not fit
+int kw_append_rows(aur_kw* kw, const KwRows& r, const KwLand& land);
+void kw_after_append(aur_kw* kw, int rc);                         // the writer's index rebuild rule (index_due)
+std::mutex& kw_write_mutex(aur_kw* kw);
+int64_t kw_rows_appended(const aur_kw* kw);
 
 // Error reporting shared by the translation units behind the C ABI (thread-local message).
 int report_error(int code, const char* fmt, ...);

@@ -1148,10 +1148,6 @@ int kw_check_columns(aur_kw* kw, const FiltProgs& fp) {
 int kw_device(const aur_kw* kw) { return kw->device; }
 }  // namespace aur
 
-namespace {
-int kw_append(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes, const int32_t* term_ids,
-              const int32_t* tfs, const int64_t* offsets, int64_t n, int64_t total, int32_t max_term);
-}  // namespace
 
 extern "C" {
 
@@ -1237,24 +1233,42 @@ int aur_kw_add(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const 
     }
     if (dl > 0x7FFFFFFF) return report_error(AUR_ERR_INVALID, "document longer than 2^31 - 1 tokens");
   }
+  std::vector<uint2> post(static_cast<size_t>(total));
+  for (int64_t j = 0; j < total; ++j) post[static_cast<size_t>(j)] = make_uint2(static_cast<uint32_t>(term_ids[j]), static_cast<uint32_t>(tfs[j]));
+  std::vector<int32_t> len(static_cast<size_t>(n));
+  for (int64_t i = 0; i < n; ++i) {
+    int64_t dl = 0;
+    for (int64_t j = offsets[i]; j < offsets[i + 1]; ++j) dl += tfs[j];
+    len[static_cast<size_t>(i)] = static_cast<int32_t>(dl);
+  }
   std::lock_guard<std::mutex> wk(kw->mu_write);
-  const int rc = kw_append(kw, ids, user_codes, org_codes, term_ids, tfs, offsets, n, total, max_term);
-  // a failed rebuild (out of memory, say) keeps the previous index and leaves the appended rows to the forward scan:
-  // the documents are in, and aur_kw_reindex reports the error
-  if (rc == AUR_OK && index_due(kw)) build_index(kw);
+  const KwRows rows{ids, user_codes, org_codes, offsets, term_ids, len.data(), n, total, max_term};
+  int rc = kw_check_room(kw, n);
+  if (rc == AUR_OK)
+    rc = kw_append_rows(kw, rows, [&](uint2* dst, cudaStream_t s) {
+      return total ? cudaMemcpyAsync(dst, post.data(), static_cast<size_t>(total) * 8, cudaMemcpyHostToDevice, s) : cudaSuccess;
+    });
+  kw_after_append(kw, rc);
   return rc;
 }
 
 }  // extern "C"
 
-namespace {
-// aur_kw_add's append and publication of n checked documents; the caller holds mu_write.
-int kw_append(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes, const int32_t* term_ids,
-              const int32_t* tfs, const int64_t* offsets, int64_t n, int64_t total, int32_t max_term) {
+namespace aur {
+int kw_check_room(aur_kw* kw, int64_t n) {
   const int64_t base = static_cast<int64_t>(kw->h_len.size());
   if (base + n > kw->capacity)
     return report_error(AUR_ERR_NOMEM, "keyword store full: %lld + %lld > capacity %lld (aur_kw_compact reclaims tombstones)",
                         (long long)base, (long long)n, (long long)kw->capacity);
+  return AUR_OK;
+}
+
+// The append and publication of r (checked, room checked) shared by aur_kw_add and aur_kw_add_text; the caller holds
+// mu_write.  land(dst, stream) enqueues the copy of the rows' r.total postings to dst on the store's stream.
+int kw_append_rows(aur_kw* kw, const KwRows& r, const KwLand& land) {
+  const int64_t n = r.n, total = r.total;
+  const int64_t* ids = r.ids;
+  const int64_t base = static_cast<int64_t>(kw->h_len.size());
   const int64_t post0 = kw->h_off.back();
   bool replaces = false;
   for (int64_t i = 0; i < n && !replaces; ++i) replaces = kw->id2row.count(ids[i]) != 0;
@@ -1265,27 +1279,22 @@ int kw_append(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const i
   KW_TRY(cudaSetDevice(kw->device));
   int rc = grow_postings(kw, post0 + total);
   if (rc != AUR_OK) return rc;
-  std::vector<uint2> post(static_cast<size_t>(total));
-  for (int64_t j = 0; j < total; ++j) post[static_cast<size_t>(j)] = make_uint2(static_cast<uint32_t>(term_ids[j]), static_cast<uint32_t>(tfs[j]));
   std::vector<int64_t> off(static_cast<size_t>(n));
-  std::vector<int32_t> len(static_cast<size_t>(n)), user(static_cast<size_t>(n)), org(static_cast<size_t>(n));
+  std::vector<int32_t> user(static_cast<size_t>(n)), org(static_cast<size_t>(n));
   std::vector<uint8_t> live(static_cast<size_t>(n), 1);
   for (int64_t i = 0; i < n; ++i) {
-    off[static_cast<size_t>(i)] = post0 + offsets[i + 1];
-    int64_t dl = 0;
-    for (int64_t j = offsets[i]; j < offsets[i + 1]; ++j) dl += tfs[j];
-    len[static_cast<size_t>(i)] = static_cast<int32_t>(dl);
-    user[static_cast<size_t>(i)] = user_codes ? user_codes[i] : 0;
-    org[static_cast<size_t>(i)] = org_codes ? org_codes[i] : -1;
+    off[static_cast<size_t>(i)] = post0 + r.offsets[i + 1];
+    user[static_cast<size_t>(i)] = r.user ? r.user[i] : 0;
+    org[static_cast<size_t>(i)] = r.org ? r.org[i] : -1;
   }
   // an id repeated inside the batch: its last occurrence wins (the earlier rows land as tombstones)
   std::unordered_map<int64_t, int64_t> last;
   for (int64_t i = 0; i < n; ++i) last[ids[i]] = i;
   for (int64_t i = 0; i < n; ++i) if (last[ids[i]] != i) live[static_cast<size_t>(i)] = 0;
   cudaStream_t s = kw->stream;
-  if (total) KW_TRY(cudaMemcpyAsync(kw->d_post + post0, post.data(), static_cast<size_t>(total) * 8, cudaMemcpyHostToDevice, s));
+  KW_TRY(land(kw->d_post + post0, s));
   KW_TRY(cudaMemcpyAsync(kw->d_off + base + 1, off.data(), static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_len + base, len.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  KW_TRY(cudaMemcpyAsync(kw->d_len + base, r.len, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
   KW_TRY(cudaMemcpyAsync(kw->d_ids + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
   KW_TRY(cudaMemcpyAsync(kw->d_user + base, user.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
   KW_TRY(cudaMemcpyAsync(kw->d_org + base, org.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
@@ -1293,14 +1302,14 @@ int kw_append(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const i
   KW_TRY(cudaStreamSynchronize(s));
   for (int64_t i = 0; i < n; ++i) {
     kw->h_off.push_back(off[static_cast<size_t>(i)]);
-    kw->h_len.push_back(len[static_cast<size_t>(i)]);
+    kw->h_len.push_back(r.len[i]);
     kw->h_ids.push_back(ids[i]);
     kw->h_user.push_back(user[static_cast<size_t>(i)]);
     kw->h_org.push_back(org[static_cast<size_t>(i)]);
     kw->h_live.push_back(live[static_cast<size_t>(i)]);
   }
   std::lock_guard<std::mutex> st(kw->mu_stat);
-  if (static_cast<int64_t>(kw->df.size()) <= max_term) kw->df.resize(static_cast<size_t>(max_term) + 1, 0);
+  if (static_cast<int64_t>(kw->df.size()) <= r.max_term) kw->df.resize(static_cast<size_t>(r.max_term) + 1, 0);
   if (replaces) {   // exclusive: no search is running, so the old rows and their statistics leave together
     std::vector<int64_t> old;
     for (int64_t i = 0; i < n; ++i) {
@@ -1313,15 +1322,24 @@ int kw_append(aur_kw* kw, const int64_t* ids, const int32_t* user_codes, const i
   for (int64_t i = 0; i < n; ++i) {
     if (!live[static_cast<size_t>(i)]) continue;
     kw->id2row[ids[i]] = base + i;
-    for (int64_t j = offsets[i]; j < offsets[i + 1]; ++j) ++kw->df[term_ids[j]];
+    for (int64_t j = r.offsets[i]; j < r.offsets[i + 1]; ++j) ++kw->df[r.term_ids[j]];
     ++kw->n_live;
-    kw->total_len += len[static_cast<size_t>(i)];
+    kw->total_len += r.len[i];
   }
   kw->rows_pub = base + n;
   kw->post_pub = post0 + total;
   return AUR_OK;
 }
-}  // namespace
+
+void kw_after_append(aur_kw* kw, int rc) {
+  // a failed rebuild (out of memory, say) keeps the previous index and leaves the appended rows to the forward scan:
+  // the documents are in, and aur_kw_reindex reports the error
+  if (rc == AUR_OK && index_due(kw)) build_index(kw);
+}
+
+std::mutex& kw_write_mutex(aur_kw* kw) { return kw->mu_write; }
+int64_t kw_rows_appended(const aur_kw* kw) { return static_cast<int64_t>(kw->h_len.size()); }
+}  // namespace aur
 
 extern "C" {
 
@@ -1503,6 +1521,35 @@ int aur_kw_search_multi(aur_kw* const* stores, int32_t n_stores, const int32_t* 
   if ((rc = kw_search_stores(stores, n_stores, q, ls.data(), li.data(), snapshot_rows_out)) != AUR_OK) return rc;
   // every store's lists are sorted by (fp64 score desc, id asc) with (-inf, -1) padding last: one k-way merge per query
   return aur_merge_topk_host_f64(ls.data(), li.data(), n_stores, nq, k, k, scores_out, ids_out);
+}
+
+int aur_kw_read_rows(aur_kw* kw, int64_t row0, int64_t n, int64_t* ids_out, int64_t* offsets_out, int32_t* term_ids_out,
+                     int32_t* tfs_out, int64_t cap, int64_t* postings_out) {
+  if (!kw || !offsets_out || !postings_out) return report_error(AUR_ERR_INVALID, "null argument");
+  std::lock_guard<std::mutex> wk(kw->mu_write);   // the host mirrors change only under mu_write
+  std::shared_lock<std::shared_mutex> rl(kw->rw);
+  int64_t rows = 0;
+  {
+    std::lock_guard<std::mutex> st(kw->mu_stat);
+    rows = kw->rows_pub;
+  }
+  if (row0 < 0 || n < 0 || row0 + n > rows)
+    return report_error(AUR_ERR_INVALID, "rows [%lld, %lld) outside the published %lld", (long long)row0, (long long)(row0 + n),
+                        (long long)rows);
+  const int64_t p0 = kw->h_off[static_cast<size_t>(row0)], total = kw->h_off[static_cast<size_t>(row0 + n)] - p0;
+  for (int64_t i = 0; i <= n; ++i) offsets_out[i] = kw->h_off[static_cast<size_t>(row0 + i)] - p0;
+  if (ids_out) std::copy(kw->h_ids.begin() + row0, kw->h_ids.begin() + row0 + n, ids_out);
+  *postings_out = total;
+  if (!term_ids_out || !tfs_out || cap < total || total == 0) return AUR_OK;   // count mode
+  KW_TRY(cudaSetDevice(kw->device));
+  std::vector<uint2> post(static_cast<size_t>(total));
+  KW_TRY(cudaMemcpyAsync(post.data(), kw->d_post + p0, static_cast<size_t>(total) * 8, cudaMemcpyDeviceToHost, kw->stream));
+  KW_TRY(cudaStreamSynchronize(kw->stream));
+  for (int64_t j = 0; j < total; ++j) {
+    term_ids_out[j] = static_cast<int32_t>(post[static_cast<size_t>(j)].x);
+    tfs_out[j] = static_cast<int32_t>(post[static_cast<size_t>(j)].y);
+  }
+  return AUR_OK;
 }
 
 int aur_kw_reindex(aur_kw* kw) {

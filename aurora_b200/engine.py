@@ -422,7 +422,8 @@ class MultiIndex:
 
 class KeywordIndex:
     """BM25 keyword store resident on one GPU (aur_kw_*): documents as (term id, tf) postings, keyed by the same ids and
-    tenant codes as ``Index``.  The vocabulary (text -> term ids) lives in ``bm25.DeviceBM25``."""
+    tenant codes as ``Index``.  Term ids come from ``bm25.build_csr`` (``add``) or from a ``KeywordVocab`` on the GPU
+    (``add_text``)."""
 
     def __init__(self, capacity: int, postings_capacity: int = 0, device: int = 0):
         self._lib = N.load()
@@ -487,6 +488,24 @@ class KeywordIndex:
         N.check(self._lib.aur_kw_search(self._h, *a["args"], C.byref(snap)))
         return a["ids"], a["scores"], int(snap.value)
 
+    def add_text(self, vocab: "KeywordVocab", ids, texts, user_codes=None, org_codes=None) -> None:
+        """Upsert len(ids) documents from their text, analysed on ``vocab``'s GPU (aur_kw_add_text): the rows and the
+        new term ids are those ``bm25.build_csr(vocab words, texts)`` gives, new words added to ``vocab``."""
+        _add_text([self], vocab, ids, texts, user_codes, org_codes)
+
+    def read_rows(self, row0: int, n: int):
+        """Rows [row0, row0 + n) of the published prefix (tombstones included): (ids int64 [n], offsets int64 [n + 1],
+        term ids int32, tfs int32), the postings of row i at [offsets[i], offsets[i + 1])."""
+        ids = np.empty(int(n), dtype=np.int64)
+        off = np.empty(int(n) + 1, dtype=np.int64)
+        total = C.c_int64(0)
+        N.check(self._lib.aur_kw_read_rows(self._h, int(row0), int(n), _ptr(ids), _ptr(off), None, None, 0, C.byref(total)))
+        terms = np.empty(max(total.value, 1), dtype=np.int32)
+        tfs = np.empty(max(total.value, 1), dtype=np.int32)
+        N.check(self._lib.aur_kw_read_rows(self._h, int(row0), int(n), _ptr(ids), _ptr(off), _ptr(terms), _ptr(tfs),
+                                           total.value, C.byref(total)))
+        return ids, off, terms[:total.value], tfs[:total.value]
+
     def reindex(self) -> None:
         """Build the term-major index over every document now (aur_kw_reindex); the writer path also does this on its
         own once the unindexed documents hold more than 1/8 of the indexed postings."""
@@ -503,6 +522,67 @@ class KeywordIndex:
         """Force how searches score the indexed rows, for tests and A/B runs: N.KW_PATH_AUTO_OPT (the cost rule),
         N.KW_PATH_FORWARD_OPT or N.KW_PATH_INDEX_OPT.  Answers do not depend on it."""
         N.check(self._lib.aur_kw_set_option(self._h, b"kw_path", int(path)))
+
+
+class KeywordVocab:
+    """The keyword vocabulary (word -> term id, grow-only) held on one GPU (aur_kw_vocab_*): ``KeywordIndex.add_text``
+    and ``MultiKeywordIndex.add_text`` analyse text into it, with the ids ``bm25.build_csr`` would give."""
+
+    def __init__(self, device: int = 0):
+        self._lib = N.load()
+        self.device = int(device)
+        self._h = C.c_void_p()
+        N.check(self._lib.aur_kw_vocab_open(self.device, C.byref(self._h)))
+
+    def close(self) -> None:
+        if getattr(self, "_h", None) is not None and self._h.value:
+            self._lib.aur_kw_vocab_close(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __len__(self) -> int:
+        return self.size()[0]
+
+    def size(self) -> Tuple[int, int]:
+        """(words, bytes)."""
+        words, nbytes = C.c_int64(0), C.c_int64(0)
+        N.check(self._lib.aur_kw_vocab_size(self._h, C.byref(words), C.byref(nbytes)))
+        return int(words.value), int(nbytes.value)
+
+    def read(self, id0: int = 0, n: Optional[int] = None) -> list:
+        """The words with ids [id0, id0 + n) (default: to the end), in id order."""
+        if n is None:
+            n = self.size()[0] - int(id0)
+        off = np.empty(int(n) + 1, dtype=np.int64)
+        N.check(self._lib.aur_kw_vocab_read(self._h, int(id0), int(n), None, 0, _ptr(off)))
+        buf = C.create_string_buffer(max(int(off[-1]), 1))
+        N.check(self._lib.aur_kw_vocab_read(self._h, int(id0), int(n), buf, int(off[-1]), _ptr(off)))
+        raw = buf.raw
+        return [raw[off[i]:off[i + 1]].decode("ascii") for i in range(int(n))]
+
+    def set_option(self, name: str, value: int) -> None:
+        """``hash_bits`` (1 .. 64), on an empty vocabulary: a test hook that forces hash collisions."""
+        N.check(self._lib.aur_kw_vocab_set_option(self._h, name.encode(), int(value)))
+
+
+def _add_text(stores, vocab: KeywordVocab, ids, texts, user_codes, org_codes) -> None:
+    """aur_kw_add_text over ``stores`` (``KeywordIndex`` objects): the texts as one UTF-8 buffer plus byte offsets."""
+    ids = np.ascontiguousarray(ids, dtype=np.int64)
+    enc = [t.encode("utf-8", "surrogatepass") for t in texts]   # a lone surrogate (ED xx xx) is a break, as in tokenize
+    if len(enc) != ids.shape[0]:
+        raise ValueError(f"{ids.shape[0]} ids but {len(enc)} texts")
+    off = np.zeros(len(enc) + 1, dtype=np.int64)
+    np.cumsum([len(b) for b in enc], out=off[1:])
+    u = None if user_codes is None else np.ascontiguousarray(user_codes, dtype=np.int32)
+    o = None if org_codes is None else np.ascontiguousarray(org_codes, dtype=np.int32)
+    handles = (C.c_void_p * len(stores))(*[st._h.value for st in stores])
+    N.check(N.load().aur_kw_add_text(handles, len(stores), vocab._h, _ptr(ids), _ptr(u), _ptr(o), b"".join(enc),
+                                     _ptr(off), ids.shape[0]))
 
 
 def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_offsets,
@@ -666,6 +746,11 @@ class MultiKeywordIndex:
             take = np.repeat(offsets[rows] - sub_off[:-1], lens) + np.arange(sub_off[-1], dtype=np.int64)
             store.add(ids[rows], t[take], f[take], sub_off, None if u is None else u[rows], None if o is None else o[rows])
         self._each(put)
+
+    def add_text(self, vocab: "KeywordVocab", ids, texts, user_codes=None, org_codes=None) -> None:
+        """KeywordIndex.add_text, each document to store ``id mod n``, all stores in one call (aur_kw_add_text): the text
+        is analysed once on ``vocab``'s GPU and every store's rows are copied to its own."""
+        _add_text(self.stores, vocab, ids, texts, user_codes, org_codes)
 
     def remove(self, ids) -> int:
         ids, sel = self._split(ids)

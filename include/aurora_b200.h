@@ -376,6 +376,49 @@ int aur_kw_reindex(aur_kw* kw);
 int aur_kw_set_option(aur_kw* kw, const char* name, int64_t value);
 int aur_kw_get_index_stats(aur_kw* kw, aur_kw_index_stats* out);
 
+/* Reads back the forward rows [row0, row0 + n) of the published prefix (append order, tombstones included), the keyword
+ * counterpart of aur_read_rows: ids_out [n] (nullable), offsets_out [n + 1] from 0, and row i's postings
+ * term_ids_out / tfs_out [offsets_out[i] .. offsets_out[i + 1]) (term id ascending).  *postings_out = the rows'
+ * postings; when term_ids_out or tfs_out is NULL or cap is smaller, only ids and offsets are written (count mode). */
+int aur_kw_read_rows(aur_kw* kw, int64_t row0, int64_t n, int64_t* ids_out, int64_t* offsets_out, int32_t* term_ids_out,
+                     int32_t* tfs_out, int64_t cap, int64_t* postings_out);
+
+/* Keyword analysis on the device (DESIGN.md section 10, "Text analysis"): the vocabulary (word -> term id, grow-only,
+ * at most 2^28 words) lives in HBM on one device, and aur_kw_add_text turns UTF-8 text into keyword-store rows there.
+ * Words are Python's re.findall(r"[0-9a-z]+", text.lower()) on the bytes: ASCII letters (lowered) and digits are word
+ * characters, E2 84 AA (U+212A KELVIN SIGN) is "k" inside a word, C4 B0 (U+0130) is "i" followed by a break, every
+ * other byte (NUL, other non-ASCII, stray or truncated sequences) is a break.  A word the vocabulary has never seen gets
+ * the next free id in order of its first occurrence in the batch (document order, then position); each document's row
+ * lists (term id ascending, tf).  For the same texts in the same order the ids and rows equal bm25.build_csr's. */
+typedef struct aur_kw_vocab aur_kw_vocab;
+/* Without a device: AUR_ERR_NO_DEVICE. */
+int aur_kw_vocab_open(int32_t device, aur_kw_vocab** out);
+int aur_kw_vocab_close(aur_kw_vocab* v);
+/* words (nullable) = words held, bytes (nullable) = their bytes. */
+int aur_kw_vocab_size(aur_kw_vocab* v, int64_t* words, int64_t* bytes);
+/* The words with ids [id0, id0 + n), concatenated into bytes_out, word i at [offsets_out[i], offsets_out[i + 1]) (from
+ * 0).  bytes_out NULL: only the offsets are written (count mode, as aur_tokenize); bytes_cap too small: AUR_ERR_INVALID
+ * and nothing is written. */
+int aur_kw_vocab_read(aur_kw_vocab* v, int64_t id0, int64_t n, char* bytes_out, int64_t bytes_cap, int64_t* offsets_out);
+/* "hash_bits" (1 .. 64, default 64): a test hook that truncates the word hash to that many bits so that distinct words
+ * collide; equality is always decided on the bytes, so results do not change.  Only on an empty vocabulary.  Unknown
+ * names and values: AUR_ERR_INVALID. */
+int aur_kw_vocab_set_option(aur_kw_vocab* v, const char* name, int64_t value);
+/* aur_kw_add of n texts analysed on v's device: document i (bytes texts_utf8[text_offsets[i] .. text_offsets[i + 1]),
+ * text_offsets[0] = 0)
+ * goes to store ids[i] mod n_stores, as engine.MultiKeywordIndex places it, an id repeated in the batch keeps its last
+ * occurrence, user_codes / org_codes as for aur_kw_add.  Stores may live on other devices than v; their rows are
+ * peer-copied (cudaMemcpyPeerAsync; peer access is neither required nor enabled).  The argument checks, every store's
+ * capacity and the 2^28 word limit are checked before anything is written: such a failure leaves the stores and the
+ * vocabulary unchanged.  A later failure (out of memory growing the postings, say) may leave new words in the
+ * vocabulary, as bm25.build_csr does, but never a partial row in a store.  Batches larger than 64 MB of text are
+ * analysed in slices of whole documents, each published before the next: the word limit of a later slice is checked
+ * when it is reached.  Writers serialise as for aur_kw_add: every store's writer lock in address order, then the
+ * vocabulary's.  NULL or repeated stores and n_stores outside 1 .. 64: AUR_ERR_INVALID. */
+int aur_kw_add_text(aur_kw* const* stores, int32_t n_stores, aur_kw_vocab* v, const int64_t* ids,
+                    const int32_t* user_codes, const int32_t* org_codes, const char* texts_utf8,
+                    const int64_t* text_offsets, int64_t n);
+
 /* ------------------------------------------------------------------ hybrid query
  * collection.query.hybrid (weaviate_client.py:252-259) in one call: the dense leg (aur_search_ex of queries_host over
  * ix, top-fetch cosines) and the keyword leg (aur_kw_search of q_terms / q_offsets over kw, top-fetch BM25 scores) run
