@@ -15,7 +15,7 @@ LIB_PATH = os.environ.get("AURORA_B200_LIB") or os.path.join(HERE, "libaurora_b2
 ABI_VERSION = 3         # must equal AUR_ABI_VERSION of the library that gets loaded (struct layouts below)
 AUR_OK = 0
 AUR_ERR_INVALID, AUR_ERR_CUDA, AUR_ERR_NOMEM, AUR_ERR_UNSUPPORTED, AUR_ERR_NO_DEVICE = -1, -2, -3, -4, -5
-AUR_BF16, AUR_F32 = 0, 1
+AUR_BF16, AUR_F32, AUR_I8 = 0, 1, 2
 KERNEL_AUTO, KERNEL_SIMT, KERNEL_TC1, KERNEL_TC2, KERNEL_LIST = 0, 1, 2, 3, 4
 KERNEL_NAMES = {0: "auto", 1: "simt", 2: "wgmma-cta1", 3: "wgmma-cluster2", 4: "list"}
 FILTER_LEAF, FILTER_AND, FILTER_OR = 0, 1, 2   # filter program tokens (AUR_FILTER_*)

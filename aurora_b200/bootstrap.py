@@ -7,7 +7,8 @@ behind the reference's module API.  Used as the daemon's boot hook:
 
 Variables: AURORA_B200_MODEL (bge-base | bge-large | minilm-l6, default bge-base), AURORA_B200_ENCODER_WEIGHTS
 (HuggingFace BertModel safetensors), AURORA_B200_VOCAB (WordPiece vocab.txt), AURORA_B200_DEVICE (0),
-AURORA_B200_CAPACITY (rows of HBM to reserve, default 1048576), AURORA_B200_SNAPSHOT (directory: restored at
+AURORA_B200_CAPACITY (rows of HBM to reserve, default 1048576), AURORA_B200_DTYPE (row format of the shards: bf16, the
+default, or int8 for half the HBM), AURORA_B200_SNAPSHOT (directory: restored at
 start when present; see KnowledgeBase.save), AURORA_B200_MAX_TOKENS / AURORA_B200_MAX_SEQS (encoder workspace).
 There is no CPU fallback: without a CUDA device or with a variable missing this raises.
 """
@@ -37,6 +38,7 @@ def configure_from_env() -> None:
     cfg = _model_config(os.environ.get("AURORA_B200_MODEL", "bge-base"))
     device = int(os.environ.get("AURORA_B200_DEVICE", "0"))
     capacity = int(os.environ.get("AURORA_B200_CAPACITY", str(1 << 20)))
+    dtype = os.environ.get("AURORA_B200_DTYPE", "bf16")
     enc = Encoder(cfg, max_tokens=int(os.environ.get("AURORA_B200_MAX_TOKENS", "32768")),
                   max_seqs=int(os.environ.get("AURORA_B200_MAX_SEQS", "2048")), device=device)
     enc.load_weights(from_hf_bert(read_safetensors(os.environ["AURORA_B200_ENCODER_WEIGHTS"]), cfg))
@@ -55,14 +57,14 @@ def configure_from_env() -> None:
         from .engine import MultiIndex
 
         devices = None if devs == "all" else [int(x) for x in devs.split(",")]
-        factory = lambda dim, cap: MultiIndex(dim, cap, devices=devices)                    # noqa: E731
+        factory = lambda dim, cap: MultiIndex(dim, cap, devices=devices, dtype=dtype)       # noqa: E731
         loader = lambda path, cap: MultiIndex.load(path, capacity=cap, devices=devices)     # noqa: E731
 
     def make():
         if snap and os.path.exists(os.path.join(snap, "meta.json")):
             kb = retriever.KnowledgeBase.load(snap, text_encoder, capacity=capacity, device=device, index_loader=loader)
         else:
-            kb = retriever.KnowledgeBase(text_encoder, capacity=capacity, device=device, index_factory=factory)
+            kb = retriever.KnowledgeBase(text_encoder, capacity=capacity, device=device, index_factory=factory, dtype=dtype)
         if snap and wal:
             os.makedirs(snap, exist_ok=True)
             kb.attach_wal(os.path.join(snap, "mutations.log"))

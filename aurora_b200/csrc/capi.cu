@@ -1,6 +1,6 @@
 // Host runtime + C ABI (include/aurora_b200.h).  Owns one corpus shard in HBM:
-//   rows      [capacity, dim]  bf16 or f32, row-major (K-major for the MMA, 128-bit
-//                              coalesced for everything else)
+//   rows      [capacity, dim]  bf16, f32 or int8 (AUR_I8: quantized from bf16 on ingest), row-major (K-major for the
+//                              MMA, 128-bit coalesced for everything else)
 //   inv_norm  [capacity] f32   1/|row|; 0 for zero rows; NaN marks a tombstone
 //   ids       [capacity] i64   caller ids;  user / org [capacity] i32 tenant codes
 //   attr      up to 16 x [capacity] i32 attribute codes for device-evaluated filters (allocated on first aur_set_attrs)
@@ -67,18 +67,28 @@ int report_error(int code, const char* fmt, ...) {
   g_err = buf;
   return code;
 }
-int encode_tmap_2d_bf16(void* tmap, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride_bytes,
-                        uint32_t box_cols, uint32_t box_rows) {
+namespace {
+int encode_tmap_2d(CUtensorMapDataType type, void* tmap, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride_bytes,
+                   uint32_t box_cols, uint32_t box_rows) {
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) return -1;
   cuuint64_t gdim[2] = {cols, rows};
   cuuint64_t gstride[1] = {row_stride_bytes};
   cuuint32_t box[2] = {box_cols, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  return static_cast<int>(enc(static_cast<CUtensorMap*>(tmap), CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+  return static_cast<int>(enc(static_cast<CUtensorMap*>(tmap), type, 2,
                               const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE));
+}
+}  // namespace
+int encode_tmap_2d_bf16(void* tmap, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride_bytes,
+                        uint32_t box_cols, uint32_t box_rows) {
+  return encode_tmap_2d(CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, tmap, base, cols, rows, row_stride_bytes, box_cols, box_rows);
+}
+int encode_tmap_2d_u8(void* tmap, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride_bytes,
+                      uint32_t box_cols, uint32_t box_rows) {
+  return encode_tmap_2d(CU_TENSOR_MAP_DATA_TYPE_UINT8, tmap, base, cols, rows, row_stride_bytes, box_cols, box_rows);
 }
 }  // namespace aur
 
@@ -110,6 +120,7 @@ struct SearchCtx {
   DevBuf<uint32_t> cand_count;   // compacted candidates per query (self-resetting)
   DevBuf<uint32_t> d_epoch;      // the tensor-core kernel's launch counter, device resident (CUDA-graph replays advance it)
   DevBuf<uint32_t> cand_read;    // per query of the last search: candidate keys its exact re-rank read
+  DevBuf<int8_t> q_img;          // int8 shards: the tensor-core kernel's query image (launch_query_image_i8)
   DevBuf<float> score_chunk;
   DevBuf<float> masked_inv;      // inverse norms with the invisible rows turned into NaN (tenant scope / id subset)
   DevBuf<int32_t> allow_rows;    // subset search: rows that stay visible
@@ -130,7 +141,7 @@ struct SearchCtx {
   void release() {
     if (h_totals) cudaFreeHost(h_totals);
     h_totals = nullptr;
-    cand_a.release(); cand_b.release(); pub.release(); cand_count.release(); d_epoch.release(); cand_read.release(); score_chunk.release(); masked_inv.release();
+    cand_a.release(); cand_b.release(); pub.release(); cand_count.release(); d_epoch.release(); cand_read.release(); q_img.release(); score_chunk.release(); masked_inv.release();
     allow_rows.release(); row_mask.release(); scope_tab.release(); q_scope.release(); stage_q.release(); stage_quser.release(); stage_qorg.release(); stage_scores.release();
     stage_ids.release(); list_stage.release(); list_scores.release();
     filt_stage.release(); filt_mask.release(); filt_counts.release(); filt_rows.release(); filt_ids.release();
@@ -152,7 +163,9 @@ struct aur_index {
   int64_t cap_pad = 0;                // capacity rounded up to a whole tile (TMA boxes never straddle an allocation):
                                       // the length of every per-row array
   std::atomic<int64_t> rows_pub{0};   // rows visible to searches (published after the data landed)
-  size_t elt = 2;
+  size_t elt = 2;                        // bytes per stored row element (int8 rows: 1)
+  size_t qelt = 2;                       // bytes per query / input row element (bf16 for bf16 and int8 rows, f32 for f32)
+  DevBuf<uint8_t> i8_stage;              // int8 shards: host bf16 rows on their way to the quantizer (writers hold mu_write)
   void* d_rows = nullptr;
   float* d_inv_norm = nullptr;
   int64_t* d_ids = nullptr;
@@ -182,14 +195,17 @@ namespace {
 
 int build_tmaps(aur_index* ix) {
   ix->tmap_ok = false;
-  if (ix->dtype != AUR_BF16 || ix->dim % kTcKBlock != 0 || ix->dim > kTcMaxDim) return AUR_OK;  // SIMT only
+  const bool i8 = ix->dtype == AUR_I8;
+  // int8 rows: 128 of them per 128-byte k-block, so the path needs dim % 128 == 0
+  if (ix->dtype == AUR_F32 || ix->dim % (i8 ? kTcKBlockI8 : kTcKBlock) != 0 || ix->dim > kTcMaxDim) return AUR_OK;  // SIMT only
   // rows past the capacity (a tile's tail, a whole half of the last tile of a pair) arrive as zeros
   for (int w = 0; w < 2; ++w)
     for (int g = 1; g <= 2; ++g) {
       const int tile_n = w ? kTcTileWide : kTcTileN;
-      const int r = encode_tmap_2d_bf16(&ix->tmap[w][g - 1], ix->d_rows, static_cast<uint64_t>(ix->dim),
-                                        static_cast<uint64_t>(ix->capacity), static_cast<uint64_t>(ix->dim) * 2, kTcKBlock,
-                                        static_cast<uint32_t>(tile_n / g));
+      const uint64_t cols = static_cast<uint64_t>(ix->dim), rows = static_cast<uint64_t>(ix->capacity);
+      const uint32_t box_rows = static_cast<uint32_t>(tile_n / g);
+      const int r = i8 ? encode_tmap_2d_u8(&ix->tmap[w][g - 1], ix->d_rows, cols, rows, cols, kTcKBlockI8, box_rows)
+                       : encode_tmap_2d_bf16(&ix->tmap[w][g - 1], ix->d_rows, cols, rows, cols * 2, kTcKBlock, box_rows);
       if (r < 0) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
       if (r != CUDA_SUCCESS) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", r);
     }
@@ -285,7 +301,7 @@ struct HostCall {
   }
   // Uploads the queries to c->stage_q and picks the outputs (direct_outputs).
   int stage(const void* queries_host, int32_t nq, int32_t k, float* scores_out, int64_t* ids_out) {
-    const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->elt;
+    const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->qelt;
     const size_t nout = static_cast<size_t>(nq) * k;
     CU_TRY(c->stage_q.reserve(qbytes));
     CU_TRY(c->stage_scores.reserve(nout));
@@ -362,7 +378,8 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   // into registers and spends the shared memory they leave on ring stages.
   // The bring-up switch that issues no MMAs (dbg_flags & 2) keeps the whole block in shared memory: without MMAs
   // nothing holds the warpgroup's four warps in step, and the one such run with register k-blocks stopped making progress.
-  const int qregs = (tile_n == kTcTileWide && ix->opt_tc_qregs != 0 && !(ix->opt_dbg_flags & 2) && ix->dim / kTcKBlock >= kTcQRegs) ? kTcQRegs : 0;
+  const bool i8 = ix->dtype == AUR_I8;   // (its launches keep the whole query image in shared memory: no tc_qregs)
+  const int qregs = (!i8 && tile_n == kTcTileWide && ix->opt_tc_qregs != 0 && !(ix->opt_dbg_flags & 2) && ix->dim / kTcKBlock >= kTcQRegs) ? kTcQRegs : 0;
   // (what fits is decided without the registers too: they deepen a ring, they do not admit a larger k)
   if (tc_pick_stages(ksel, ix->dim, ix->smem_optin, tile_n, mask) < 2) return fail(AUR_ERR_UNSUPPORTED, "k too large for the tensor-core path's shared memory");
   int stages = tc_pick_stages(ksel, ix->dim, ix->smem_optin, tile_n, mask, qregs);
@@ -384,9 +401,14 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
     CU_TRY(c->d_epoch.reserve(1));
     CU_TRY(cudaMemcpyAsync(c->d_epoch.p, &e0, 4, cudaMemcpyHostToDevice, s));   // pageable source: staged before return
   }
+  if (i8) {
+    CU_TRY(c->q_img.reserve(static_cast<size_t>(nqb) * ix->dim * 2));
+    CU_TRY(launch_query_image_i8(static_cast<const __nv_bfloat16*>(q_dev), ix->dim, nqb, c->q_img.p, s));
+    c->last_launches += 1;
+  }
   ++c->epoch;
   TcParams p;
-  p.q = static_cast<const __nv_bfloat16*>(q_dev);
+  p.q = i8 ? reinterpret_cast<const __nv_bfloat16*>(c->q_img.p) : static_cast<const __nv_bfloat16*>(q_dev);
   p.inv_norm = inv_norm ? inv_norm : ix->d_inv_norm;
   p.row_mask = row_mask; p.q_scope = q_scope;
   p.ids = ix->d_ids;
@@ -403,7 +425,7 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   p.num_stages = stages;
   p.dbg_flags = ix->opt_dbg_flags;
   p.n_tiles = static_cast<int>((n_rows + tile_n - 1) / tile_n);
-  CU_TRY(tc_launch(cta_group, tile_n, qregs, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
+  CU_TRY(tc_launch(cta_group, tile_n, qregs, i8, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
   c->last_tile_n = tile_n;
   *n_lists_out = n_lists;
   return AUR_OK;
@@ -490,8 +512,8 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
   int kernel = ix->opt_kernel;
   if (kernel == AUR_KERNEL_AUTO) kernel = tc_shape_ok(ix, k, filtered) ? AUR_KERNEL_TC2 : AUR_KERNEL_SIMT;
   if (kernel != AUR_KERNEL_SIMT && !tc_shape_ok(ix, k, filtered))
-    return fail(AUR_ERR_UNSUPPORTED, "tensor-core path needs bf16, dim %% 64 == 0, dim <= %d, no per-query tenant filter, and k small "
-                "enough for its shared-memory lists at this dim", kTcMaxDim);
+    return fail(AUR_ERR_UNSUPPORTED, "tensor-core path needs bf16 rows with dim %% 64 == 0 or int8 rows with dim %% 128 == 0, dim <= %d, "
+                "no per-query tenant filter, and k small enough for its shared-memory lists at this dim", kTcMaxDim);
   c->last_kernel = kernel;
   CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
   bool k_timed = false;
@@ -525,7 +547,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
   else if (kernel == AUR_KERNEL_TC2) qstep = tc2_super_blocks(ix, ksel, 4) * 2 * kTcQRows;
   for (int q0 = 0; q0 < nq; q0 += qstep) {
     const int nqb = (nq - q0 < qstep) ? nq - q0 : qstep;
-    const uint8_t* qb = static_cast<const uint8_t*>(q_dev) + static_cast<size_t>(q0) * ix->dim * ix->elt;
+    const uint8_t* qb = static_cast<const uint8_t*>(q_dev) + static_cast<size_t>(q0) * ix->dim * ix->qelt;
     int n_lists = 0;
     if (kernel == AUR_KERNEL_SIMT) {
       if (n_rows == 0) {
@@ -579,8 +601,26 @@ int add_common(aur_index* ix, const void* rows, bool rows_on_device, const int64
   for (int64_t i = 0; i < n; ++i)
     if (ids[i] < 0) return fail(AUR_ERR_INVALID, "ids must be >= 0");
   uint8_t* dst = static_cast<uint8_t*>(ix->d_rows) + static_cast<size_t>(base) * ix->dim * ix->elt;
-  CU_TRY(cudaMemcpyAsync(dst, rows, static_cast<size_t>(n) * ix->dim * ix->elt,
-                         rows_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+  if (ix->dtype == AUR_I8) {
+    // bf16 rows in, quantized on s before the publish below: a search never sees an unquantized row.  Host rows pass
+    // through a bounded device staging buffer, a slice at a time (stream order keeps the slices apart).
+    const int64_t slice = rows_on_device ? n : std::min<int64_t>(n, 65536);
+    const size_t in_row = static_cast<size_t>(ix->dim) * 2;
+    if (!rows_on_device) CU_TRY(ix->i8_stage.reserve(static_cast<size_t>(slice) * in_row));
+    for (int64_t r0 = 0; r0 < n; r0 += slice) {
+      const int64_t m = std::min(slice, n - r0);
+      const uint8_t* src = static_cast<const uint8_t*>(rows) + static_cast<size_t>(r0) * in_row;
+      if (!rows_on_device) {
+        CU_TRY(cudaMemcpyAsync(ix->i8_stage.p, src, static_cast<size_t>(m) * in_row, cudaMemcpyHostToDevice, s));
+        src = ix->i8_stage.p;
+      }
+      CU_TRY(launch_quantize_rows_i8(reinterpret_cast<const __nv_bfloat16*>(src), ix->dim, m,
+                                     reinterpret_cast<int8_t*>(dst) + static_cast<size_t>(r0) * ix->dim, ix->d_inv_norm + base + r0, s));
+    }
+  } else {
+    CU_TRY(cudaMemcpyAsync(dst, rows, static_cast<size_t>(n) * ix->dim * ix->elt,
+                           rows_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+  }
   CU_TRY(cudaMemcpyAsync(ix->d_ids + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
   std::vector<int32_t> fill;
   if (!users) { fill.assign(static_cast<size_t>(n), 0); users = fill.data(); }
@@ -588,7 +628,7 @@ int add_common(aur_index* ix, const void* rows, bool rows_on_device, const int64
   std::vector<int32_t> fill2;
   if (!orgs) { fill2.assign(static_cast<size_t>(n), -1); orgs = fill2.data(); }
   CU_TRY(cudaMemcpyAsync(ix->d_org + base, orgs, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  CU_TRY(launch_row_inv_norms(dst, ix->dtype, ix->dim, n, ix->d_inv_norm + base, s));
+  if (ix->dtype != AUR_I8) CU_TRY(launch_row_inv_norms(dst, ix->dtype, ix->dim, n, ix->d_inv_norm + base, s));
   // upsert: an id that already exists loses its old row (weaviate_client.py:172 uuid5 semantics).  The old rows
   // are tombstoned before the new ones are published: a racing search may briefly miss the object, never see it twice.
   std::vector<int64_t> dead;
@@ -706,7 +746,7 @@ int check_list_args(aur_index* ix, const void* q, int32_t nq, int32_t k, const v
   int rc = check_search_args(ix, q, nq, k, s_out, i_out);
   if (rc != AUR_OK) return rc;
   if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
-  if (ix->dtype != AUR_BF16) return fail(AUR_ERR_UNSUPPORTED, "list search needs a bf16 index");
+  if (ix->dtype == AUR_F32) return fail(AUR_ERR_UNSUPPORTED, "list search needs a bf16 or int8 index");
   return AUR_OK;
 }
 
@@ -798,7 +838,8 @@ int run_list_search(aur_index* ix, SearchCtx* c, cudaStream_t s, const ListPlan&
     for (const ListPlan::Launch& ln : b.launches) {
       ListParams p{};
       p.q = reinterpret_cast<const __nv_bfloat16*>(qb);
-      p.rows = static_cast<const __nv_bfloat16*>(ix->d_rows);
+      p.rows = ix->d_rows;
+      p.rows_i8 = ix->dtype == AUR_I8;
       p.inv_norm = ix->d_inv_norm;
       p.ids = ix->d_ids;
       p.items = reinterpret_cast<const ListItem*>(c->list_stage.p + ln.items);
@@ -955,7 +996,7 @@ int filtered_search(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t nq, int
 namespace aur {
 int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
               const int32_t* q_org, float* scores, int64_t* ids, int64_t* snapshot_rows) {
-  if (ix->dtype != AUR_BF16) return fail(AUR_ERR_UNSUPPORTED, "hybrid search needs a bf16 index");
+  if (ix->dtype == AUR_F32) return fail(AUR_ERR_UNSUPPORTED, "hybrid search needs a bf16 or int8 index");
   if (ix->device != device) return fail(AUR_ERR_INVALID, "the keyword store is on device %d, the index on device %d", device, ix->device);
   int rc = check_batch(nq, k);
   if (rc != AUR_OK) return rc;
@@ -965,7 +1006,7 @@ int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_hos
   if ((rc = acquire_ctx(ix, s, &c)) != AUR_OK) return rc;
   std::lock_guard<std::mutex> cl(c->mu);
   const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
-  const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->elt;
+  const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->qelt;
   CU_TRY(c->stage_q.reserve(qbytes));
   CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
   Scope sc;
@@ -979,7 +1020,7 @@ int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_hos
 }
 
 int index_device(const aur_index* ix) { return ix->device; }
-int index_is_bf16(const aur_index* ix) { return ix->dtype == AUR_BF16; }
+int index_bf16_queries(const aur_index* ix) { return ix->dtype == AUR_BF16 || ix->dtype == AUR_I8; }
 
 int filter_check(aur_index* ix, const FiltProgs& fp) {
   return check_programs(ix, fp.prog, fp.prog_off, fp.n_programs, fp.bitmap, fp.bitmap_words);
@@ -1010,7 +1051,7 @@ int filtered_legs(aur_index* const* shards, int n, const void* queries_host, int
     HostCall& call = *pt.call;
     if ((rc = call.open()) != AUR_OK) return rc;
     SearchCtx* c = call.c;
-    const size_t qbytes = static_cast<size_t>(nq) * call.ix->dim * call.ix->elt;
+    const size_t qbytes = static_cast<size_t>(nq) * call.ix->dim * call.ix->qelt;
     CU_TRY(c->stage_q.reserve(qbytes));
     CU_TRY(c->stage_scores.reserve(nout));
     CU_TRY(c->stage_ids.reserve(nout));
@@ -1055,8 +1096,10 @@ int aur_open(const aur_config* cfg, aur_index** out) {
   if (!cfg || !out) return fail(AUR_ERR_INVALID, "null argument");
   *out = nullptr;
   if (cfg->dim <= 0 || cfg->capacity <= 0) return fail(AUR_ERR_INVALID, "dim and capacity must be positive");
-  if (cfg->dtype != AUR_BF16 && cfg->dtype != AUR_F32) return fail(AUR_ERR_INVALID, "dtype must be AUR_BF16 or AUR_F32");
+  if (cfg->dtype != AUR_BF16 && cfg->dtype != AUR_F32 && cfg->dtype != AUR_I8)
+    return fail(AUR_ERR_INVALID, "dtype must be AUR_BF16, AUR_F32 or AUR_I8");
   if (cfg->dtype == AUR_BF16 && cfg->dim % 8 != 0) return fail(AUR_ERR_INVALID, "bf16 rows need dim %% 8 == 0");
+  if (cfg->dtype == AUR_I8 && cfg->dim % 16 != 0) return fail(AUR_ERR_INVALID, "int8 rows need dim %% 16 == 0");
   if (cfg->capacity > 0x7FFFFFC0ll) return fail(AUR_ERR_INVALID, "capacity exceeds int32 row indexing");
   int ndev = aur_device_count();
   if (ndev == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device: aurora_b200 has no CPU fallback");
@@ -1067,7 +1110,8 @@ int aur_open(const aur_config* cfg, aur_index** out) {
   if (prop.major != 9) return fail(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
   aur_index* ix = new aur_index();
   ix->device = cfg->device; ix->dim = cfg->dim; ix->dtype = cfg->dtype; ix->capacity = cfg->capacity;
-  ix->elt = cfg->dtype == AUR_BF16 ? 2 : 4;
+  ix->elt = cfg->dtype == AUR_BF16 ? 2 : (cfg->dtype == AUR_I8 ? 1 : 4);
+  ix->qelt = cfg->dtype == AUR_F32 ? 4 : 2;
   ix->sm_count = prop.multiProcessorCount;
   ix->smem_optin = prop.sharedMemPerBlockOptin;
   auto bail = [&](int rc) { aur_close(ix); return rc; };
@@ -1099,6 +1143,7 @@ int aur_close(aur_index* ix) {
   cudaFree(ix->d_rows); cudaFree(ix->d_inv_norm); cudaFree(ix->d_ids); cudaFree(ix->d_user); cudaFree(ix->d_org);
   for (int32_t* a : ix->d_attr) cudaFree(a);
   ix->attr_stage.release();
+  ix->i8_stage.release();
   for (auto& c : ix->ctxs) c->release();
   if (ix->stream) cudaStreamDestroy(ix->stream);
   if (ix->ingest_stream) cudaStreamDestroy(ix->ingest_stream);
@@ -1152,7 +1197,11 @@ int aur_export(aur_index* ix, void* rows_out, int64_t* ids_out, int32_t* user_ou
   CU_TRY(cudaMemcpy(ids_out, ix->d_ids, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
   if (user_out) CU_TRY(cudaMemcpy(user_out, ix->d_user, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
   if (org_out) CU_TRY(cudaMemcpy(org_out, ix->d_org, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
-  for (int64_t i = 0; i < n; ++i) live_out[i] = inv[static_cast<size_t>(i)] == inv[static_cast<size_t>(i)];   // NaN = tombstone
+  // NaN = tombstone; an int8 row stored from a row with a NaN / inf (scale +inf, never returned) is live, reported as 2
+  for (int64_t i = 0; i < n; ++i) {
+    const float v = inv[static_cast<size_t>(i)];
+    live_out[i] = v != v ? 0 : (ix->dtype == AUR_I8 && isinf(v) ? 2 : 1);
+  }
   return AUR_OK;
 }
 
@@ -1715,6 +1764,7 @@ int aur_debug_tc_scores(aur_index* ix, const void* queries_dev, int32_t nq, int3
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   CU_TRY(cudaSetDevice(ix->device));
   if (!ix->tmap_ok) return fail(AUR_ERR_UNSUPPORTED, "index shape has no tensor-core path");
+  if (ix->dtype == AUR_I8) return fail(AUR_ERR_UNSUPPORTED, "the tensor-core score dump is for bf16 shards");
   if (nq <= 0 || nq > 2 * kTcQRows) return fail(AUR_ERR_INVALID, "1..%d queries", 2 * kTcQRows);
   int n_lists = 0;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ix->stream;

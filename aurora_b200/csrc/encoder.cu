@@ -370,7 +370,7 @@ int aur_encode_append(aur_encoder* e, aur_index* ix, const int32_t* tokens, cons
   aur_stats st{};
   int rc;
   if ((rc = aur_get_stats(ix, &st))) return rc;
-  if (st.dim != e->cfg.hidden || st.dtype != AUR_BF16)
+  if (st.dim != e->cfg.hidden || st.dtype == AUR_F32)   // (an int8 index quantizes the bf16 rows as it adds them)
     return report_error(AUR_ERR_INVALID, "index is %d-d dtype %d; the encoder produces %d-d bf16", st.dim, st.dtype, e->cfg.hidden);
   int n_items = 0;
   if ((rc = stage_inputs(e, tokens, cu, n_seq, &n_items))) return rc;

@@ -455,7 +455,7 @@ int hybrid_search(aur_index* const* shards, aur_kw* const* stores, int32_t n, co
   int rc = kw_check(q_terms, q_offsets, nq, fetch);
   if (rc != AUR_OK) return rc;
   for (int s = 0; s < n; ++s) {
-    if (!index_is_bf16(shards[s])) return report_error(AUR_ERR_UNSUPPORTED, "hybrid search needs bf16 shards (shard %d)", s);
+    if (!index_bf16_queries(shards[s])) return report_error(AUR_ERR_UNSUPPORTED, "hybrid search needs bf16 or int8 shards (shard %d)", s);
     if (index_device(shards[s]) != kw_device(stores[s]))
       return report_error(AUR_ERR_INVALID, "keyword store %d is on device %d, its shard on device %d", s, kw_device(stores[s]),
                           index_device(shards[s]));

@@ -59,6 +59,7 @@ constexpr int kTcTileN = 64;       // corpus rows per tile  (MMA N); the bring-u
 constexpr int kTcTileWide = 128;   // the wide tile (wgmma m64n128), picked per launch when its layout fits
 constexpr int kTcWideMinStages = 4;   // with three 16 KB stages the wide tile measured no faster than the 64-row one
 constexpr int kTcKBlock = 64;      // bf16 per 128-byte swizzled smem row (one pipeline stage)
+constexpr int kTcKBlockI8 = 128;   // int8 per 128-byte swizzled smem row (a stage of an int8 shard: twice the dimensions)
 // Leading query k-blocks a 128-row launch keeps in the MMA warpgroup's registers (16 registers a thread each) when
 // dim / 64 has that many, instead of 8 KB shared-memory tiles: every two of them buy one more 16 KB ring stage.
 constexpr int kTcQRegs = 6;   // 4 measured slower (six ring stages at dim 768 / top-32 against seven), 8 spills
@@ -105,8 +106,10 @@ constexpr uint32_t kSearchEpochMax = 0x7FFFFFFFu;
 size_t tc_smem_bytes(int num_stages, int ksel, int dim, int tile_n, bool mask, int qregs = 0);
 int tc_pick_stages(int ksel, int dim, size_t smem_limit, int tile_n, bool mask, int qregs = 0);
 // Launches the fused similarity + top-k kernel; cta_group 2 = two-CTA clusters sharing every corpus tile by TMA
-// multicast.  tmap: CUtensorMap over the corpus with a {64, tile_n / cta_group} box and 128-byte swizzle.
-cudaError_t tc_launch(int cta_group, int tile_n, int qregs, int grid, const void* tmap, const TcParams& p, size_t smem, cudaStream_t s);
+// multicast.  tmap: CUtensorMap over the corpus with a {64, tile_n / cta_group} box (i8: int8 rows, a {128, ...} UINT8
+// box, p.q the query image of launch_query_image_i8) and 128-byte swizzle.
+cudaError_t tc_launch(int cta_group, int tile_n, int qregs, bool i8, int grid, const void* tmap, const TcParams& p, size_t smem,
+                      cudaStream_t s);
 
 // ---------------------------------------------------------------- SIMT kernels
 struct FilterArgs {
@@ -117,6 +120,11 @@ struct FilterArgs {
 };
 
 cudaError_t launch_row_inv_norms(const void* rows, int dtype, int dim, int64_t n, float* inv_norm, cudaStream_t s);
+// The tensor-core kernel's query operand for int8 rows: per bf16 query q16 = rint(q * 32512 / max|q|) (0 for a zero query)
+// split as q16 = 256 hi + lo, hi = (q16 + 128) >> 8, both int8; written [nq][dim / 128][hi 128 B | lo 128 B].
+cudaError_t launch_query_image_i8(const __nv_bfloat16* q, int dim, int nq, int8_t* out, cudaStream_t s);
+// Ingest into an int8 shard: bf16 rows in -> int8 rows and their inverse norms out (oracle/quantize.py's rule).
+cudaError_t launch_quantize_rows_i8(const __nv_bfloat16* in, int dim, int64_t n, int8_t* out, float* inv_norm, cudaStream_t s);
 // Generic path: scores of a chunk of rows for all queries, then per-segment selection.
 constexpr int kSimtSeg = 2048;    // corpus rows per selection segment (one candidate list)
 cudaError_t launch_simt_scores(const void* q, const void* rows, int dtype, int dim, int nq, int64_t row0,
@@ -135,7 +143,7 @@ struct FinalizeArgs {
                      // (reset to 0 by the kernel); null = all n_lists * ksel slots are keys
   uint32_t* epoch_bump;  // nullable: the tensor-core kernel's device-resident launch counter, advanced here (never 0)
   uint32_t* cand_read;   // nullable: per query, the number of candidate keys the re-rank read (aur_stats.last_candidates)
-  const void* q; const void* rows; int dtype; int dim; int nq; int k;
+  const void* q; const void* rows; int dtype; int dim; int nq; int k;   // q: bf16 for bf16 and int8 rows, f32 for f32
   const int64_t* ids;
   float* out_scores; int64_t* out_ids; double* out_scores64;   // (out_scores / out_ids nullable in exchange mode)
   int sort_cap;      // set by launch_finalize: keys the shared sort buffer holds
@@ -186,7 +194,7 @@ constexpr int kListQMax = 64;     // queries of one work item (four m16 MMA row 
 struct ListItem { int32_t row0, n_rows, seg, q0, nq, out; };
 struct ListParams {
   const __nv_bfloat16* q;      // [nq of the query block, dim]
-  const __nv_bfloat16* rows;   // the shard's rows
+  const void* rows;            // the shard's rows: bf16, or int8 when rows_i8 (converted exactly to bf16 on the gather)
   const float* inv_norm;       // NaN = tombstone
   const int64_t* ids;
   const ListItem* items; int n_items;
@@ -195,6 +203,7 @@ struct ListParams {
   float* scores;               // scratch [sum of the items' nq][kSimtSeg]
   uint64_t* cand;              // [queries of the block, n_lists, ksel] candidate keys (slots no item writes: zero)
   int dim, ksel, n_lists;
+  bool rows_i8;
 };
 // Scores and per-segment selection of n_items work items; max_nq = the largest nq among them.
 cudaError_t launch_list_search(const ListParams& p, int max_nq, cudaStream_t s);
@@ -321,12 +330,12 @@ struct DevBuf {   // grow-only device scratch
 // ---------------------------------------------------------------- the two legs of a hybrid query (hybrid.cu)
 // Dense leg: the search aur_search_ex runs for these host queries and per-query tenant codes (same scope handling, same
 // kernels, same answer), enqueued on stream s of `device` over the prefix published now, into the device arrays
-// scores / ids [nq * k].  Nothing waits; *snapshot_rows receives the prefix.  A bf16 index on `device` only
+// scores / ids [nq * k].  Nothing waits; *snapshot_rows receives the prefix.  A bf16 or int8 index on `device` only
 // (else AUR_ERR_UNSUPPORTED / AUR_ERR_INVALID).  The leg's aur_stats.last_* are the index's last search.  (capi.cu)
 int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
               const int32_t* q_org, float* scores, int64_t* ids, int64_t* snapshot_rows);
 int index_device(const aur_index* ix);
-int index_is_bf16(const aur_index* ix);
+int index_bf16_queries(const aur_index* ix);   // the index takes bf16 queries: bf16 or int8 rows
 // Filtered dense legs: aur_search_filtered's search of the host queries under the checked programs fp on every shard
 // of shards[0 .. n) (bf16, distinct), max_list_rows applied per shard, each shard's part on a pooled search context of
 // its device and that context's stream.  Every shard's count pass is enqueued before any is waited on; their read-back
@@ -380,5 +389,8 @@ int report_error(int code, const char* fmt, ...);
 // 2-D bf16 tensor map, 128-byte swizzle; returns 0 or a CUresult.
 int encode_tmap_2d_bf16(void* tmap, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride_bytes,
                         uint32_t box_cols, uint32_t box_rows);
+// The same over uint8 elements (an int8 shard's rows).
+int encode_tmap_2d_u8(void* tmap, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride_bytes,
+                      uint32_t box_cols, uint32_t box_rows);
 
 }  // namespace aur

@@ -4,6 +4,7 @@
 // the pairwise cosine that mirrors SimilarityStrategy._cosine_similarity.
 #include <math.h>
 #include <string.h>
+#include <type_traits>
 #include "internal.h"
 
 namespace aur {
@@ -12,6 +13,7 @@ namespace {
 template <typename T> __device__ __forceinline__ float to_f32(T v);
 template <> __device__ __forceinline__ float to_f32<float>(float v) { return v; }
 template <> __device__ __forceinline__ float to_f32<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <> __device__ __forceinline__ float to_f32<int8_t>(int8_t v) { return static_cast<float>(v); }
 
 __device__ __forceinline__ double warp_sum_lane0(double v) {
   // shfl_down tree: lane 0 ends with a value whose association order is fixed, so the
@@ -44,12 +46,77 @@ __global__ void row_inv_norm_kernel(const T* __restrict__ rows, int dim, int64_t
   if (lane == 0) inv_norm[row] = ss > 0.f ? 1.0f / sqrtf(ss) : 0.f;
 }
 
+// Ingest into an int8 shard (AUR_I8), one warp per row: amax = max |x| (exact), q = rint(x * 127 / amax) with an exact
+// fp64 product and one correctly rounded fp64 division (oracle/quantize.py), then the inverse norm of the int8 row in
+// row_inv_norm_kernel's summation order, so an int8 row and the same values stored as bf16 get the same scale bit for
+// bit.  An all-zero row stays zero with scale 0.  A row holding a NaN or +-inf is stored as zeros with scale +inf: its
+// first-pass score 0 * inf is NaN on every path, which no selection admits -- never returned, as in a bf16 shard, where
+// such a row scores NaN -- while it stays live for exports and filters (a tombstone is a NaN scale).
+__global__ void quantize_rows_i8_kernel(const __nv_bfloat16* __restrict__ in, int dim, int64_t n, int8_t* __restrict__ out,
+                                        float* __restrict__ inv_norm) {
+  const int64_t row = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (row >= n) return;
+  const __nv_bfloat16* p = in + row * dim;
+  int8_t* o = out + row * dim;
+  float amax = 0.f;
+  bool finite = true;
+  for (int i = lane; i < dim; i += 32) {
+    const float v = __bfloat162float(p[i]);
+    finite = finite && isfinite(v);
+    amax = fmaxf(amax, fabsf(v));
+  }
+#pragma unroll
+  for (int o2 = 16; o2 > 0; o2 >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o2));
+  finite = __all_sync(0xffffffffu, finite);
+  const double a = static_cast<double>(amax);
+  float ss = 0.f;
+  for (int i = lane; i < dim; i += 32) {
+    int8_t q = 0;
+    if (finite && amax > 0.f)
+      q = static_cast<int8_t>(rint(__ddiv_rn(__dmul_rn(static_cast<double>(__bfloat162float(p[i])), 127.0), a)));
+    o[i] = q;
+    const float v = static_cast<float>(q);
+    ss = fmaf(v, v, ss);
+  }
+#pragma unroll
+  for (int o2 = 16; o2 > 0; o2 >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o2);
+  if (lane == 0) inv_norm[row] = !finite ? INFINITY : (ss > 0.f ? 1.0f / sqrtf(ss) : 0.f);
+}
+
+// The tensor-core kernel's query operand for an int8 shard, one warp per query: q16 = rint(q * 32512 / amax) (exact
+// fp64 product, one rounded division; a zero query stays 0), split exactly as q16 = 256 hi + lo with hi = (q16 + 128) >> 8
+// in [-127, 127] and lo in [-128, 127].  Row q of the output is [dim / 128][hi 128 B | lo 128 B]: dim * 2 bytes, the size
+// of the bf16 query row the kernel's staging copies.  Rounding to 16 bits moves a cosine by at most about
+// sqrt(dim) / 65024 relative to |q|: the re-rank's k + 8 slack covers it as it covers fp32 noise on bf16 rows.
+__global__ void query_image_i8_kernel(const __nv_bfloat16* __restrict__ q, int dim, int nq, int8_t* __restrict__ out) {
+  const int64_t qi = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (qi >= nq) return;
+  const __nv_bfloat16* p = q + qi * dim;
+  int8_t* o = out + qi * dim * 2;
+  float amax = 0.f;
+  for (int i = lane; i < dim; i += 32) amax = fmaxf(amax, fabsf(__bfloat162float(p[i])));
+#pragma unroll
+  for (int o2 = 16; o2 > 0; o2 >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o2));
+  const double a = static_cast<double>(amax);
+  for (int i = lane; i < dim; i += 32) {
+    int v = 0;
+    if (amax > 0.f && isfinite(amax))
+      v = static_cast<int>(rint(__ddiv_rn(__dmul_rn(static_cast<double>(__bfloat162float(p[i])), 32512.0), a)));
+    const int hi = (v + 128) >> 8, lo = v - 256 * hi;
+    int8_t* blk = o + (i / 128) * 256 + (i % 128);
+    blk[0] = static_cast<int8_t>(hi);
+    blk[128] = static_cast<int8_t>(lo);
+  }
+}
+
 // --------------------------------------------------------------------------------------
 // Generic similarity: 64 queries x 64 rows per block, 4x4 per thread, fp32 FMA.
 constexpr int kSB = 64, kSK = 16;
-template <typename T>
+template <typename T, typename TR = T>
 __global__ void __launch_bounds__(256)
-simt_scores_kernel(const T* __restrict__ q, const T* __restrict__ rows, int dim, int nq, int64_t row0,
+simt_scores_kernel(const T* __restrict__ q, const TR* __restrict__ rows, int dim, int nq, int64_t row0,
                    int64_t nrows_chunk, int64_t n_rows, const float* __restrict__ inv_norm, FilterArgs f,
                    float* __restrict__ scores) {
   __shared__ float Qs[kSK][kSB + 1];
@@ -211,7 +278,8 @@ reduce_lists_kernel(const uint64_t* __restrict__ in, int n_lists, int ksel, int 
 
 // --------------------------------------------------------------------------------------
 // Finalize: best ksel approximate candidates -> exact fp64 cosine -> (score desc, id asc).
-template <typename T>
+// T: the query's element type, TR: the rows' (int8 rows take bf16 queries).
+template <typename T, typename TR = T>
 __global__ void __launch_bounds__(256, 2)
 finalize_kernel(FinalizeArgs a) {
   extern __shared__ uint64_t skeys[];
@@ -223,7 +291,7 @@ finalize_kernel(FinalizeArgs a) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
   // ---- prologue, independent of the similarity kernel (launched with programmatic dependent launch, so this part
   //      overlaps that kernel's tail): the query goes to shared memory once (as fp32, exact for bf16 / f32), |q|^2
-  const T* rows = static_cast<const T*>(a.rows);
+  const TR* rows = static_cast<const TR*>(a.rows);
   const T* qv = static_cast<const T*>(a.q) + static_cast<size_t>(qi) * a.dim;
   float* qs = reinterpret_cast<float*>(skeys + a.sort_cap);      // [dim] behind the sort buffer
   for (int i = threadIdx.x; i < a.dim; i += blockDim.x) qs[i] = to_f32(qv[i]);
@@ -283,7 +351,10 @@ finalize_kernel(FinalizeArgs a) {
   const int ncand = min(a.ksel, P);
   for (int c = threadIdx.x; c < ncand; c += blockDim.x) topkeys[c] = skeys[c];
   __syncthreads();
-  constexpr int kVec = 16 / static_cast<int>(sizeof(T));          // elements per 16-byte piece
+  // elements per piece: a 16-byte piece of bf16 / f32 rows; int8 rows are read 8 bytes at a time, so that every lane
+  // sums the same elements in the same order as for the row stored as bf16
+  constexpr int kVec = sizeof(TR) == 1 ? 8 : 16 / static_cast<int>(sizeof(TR));
+  using Piece = typename std::conditional<sizeof(TR) == 1, uint2, uint4>::type;
   const bool vec_ok = (a.dim % kVec) == 0;
   // kRe candidates per warp and step, strided by the warp count, with every row load (and the id load)
   // issued before any arithmetic: at k+slack = 40 and 8 warps x 5 all candidate rows of the query are in
@@ -292,7 +363,7 @@ finalize_kernel(FinalizeArgs a) {
   const int n_chunks = vec_ok ? a.dim / kVec : 0;
   const bool reg_path = vec_ok && n_chunks <= 32 * kMaxCh;
   for (int c0 = warp; c0 < ncand; c0 += kRe * nwarps) {
-    int32_t row[kRe]; const T* rv[kRe]; int64_t idv[kRe];
+    int32_t row[kRe]; const TR* rv[kRe]; int64_t idv[kRe];
     double dot[kRe], cc[kRe];
 #pragma unroll
     for (int h = 0; h < kRe; ++h) {
@@ -303,13 +374,13 @@ finalize_kernel(FinalizeArgs a) {
       dot[h] = 0.0; cc[h] = 0.0;
     }
     if (reg_path) {
-      uint4 raw[kRe][kMaxCh];
+      Piece raw[kRe][kMaxCh];
 #pragma unroll
       for (int h = 0; h < kRe; ++h)
 #pragma unroll
         for (int i = 0; i < kMaxCh; ++i) {
           const int ch = lane + 32 * i;
-          raw[h][i] = (row[h] >= 0 && ch < n_chunks) ? __ldg(reinterpret_cast<const uint4*>(rv[h]) + ch) : make_uint4(0, 0, 0, 0);
+          raw[h][i] = (row[h] >= 0 && ch < n_chunks) ? __ldg(reinterpret_cast<const Piece*>(rv[h]) + ch) : Piece{};
         }
 #pragma unroll
       for (int h = 0; h < kRe; ++h) idv[h] = (row[h] >= 0) ? __ldg(a.ids + row[h]) : -1;
@@ -319,8 +390,8 @@ finalize_kernel(FinalizeArgs a) {
         for (int i = 0; i < kMaxCh; ++i) {
           const int ch = lane + 32 * i;
           if (ch < n_chunks) {
-            T el[kVec];
-            memcpy(el, &raw[h][i], 16);
+            TR el[kVec];
+            memcpy(el, &raw[h][i], sizeof(Piece));
 #pragma unroll
             for (int e = 0; e < kVec; ++e) {
               const double x = static_cast<double>(qs[ch * kVec + e]), y = static_cast<double>(to_f32(el[e]));
@@ -544,6 +615,7 @@ cudaError_t launch_row_inv_norms(const void* rows, int dtype, int dim, int64_t n
   if (n <= 0) return cudaSuccess;
   const int threads = 256;
   const int64_t blocks = (n * 32 + threads - 1) / threads;
+  if (dtype == 2) return cudaErrorInvalidValue;   // int8 rows get their scale from launch_quantize_rows_i8
   if (dtype == 0)
     row_inv_norm_kernel<__nv_bfloat16><<<static_cast<unsigned>(blocks), threads, 0, s>>>(
         static_cast<const __nv_bfloat16*>(rows), dim, n, inv_norm);
@@ -553,11 +625,29 @@ cudaError_t launch_row_inv_norms(const void* rows, int dtype, int dim, int64_t n
   return cudaGetLastError();
 }
 
+cudaError_t launch_query_image_i8(const __nv_bfloat16* q, int dim, int nq, int8_t* out, cudaStream_t s) {
+  if (nq <= 0) return cudaSuccess;
+  const int64_t blocks = (static_cast<int64_t>(nq) * 32 + 255) / 256;
+  query_image_i8_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(q, dim, nq, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_quantize_rows_i8(const __nv_bfloat16* in, int dim, int64_t n, int8_t* out, float* inv_norm, cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  const int64_t blocks = (n * 32 + 255) / 256;
+  quantize_rows_i8_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(in, dim, n, out, inv_norm);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_simt_scores(const void* q, const void* rows, int dtype, int dim, int nq, int64_t row0,
                                int64_t nrows_chunk, int64_t n_rows, const float* inv_norm, FilterArgs f, float* scores,
                                cudaStream_t s) {
   dim3 grid(static_cast<unsigned>((nrows_chunk + kSB - 1) / kSB), static_cast<unsigned>((nq + kSB - 1) / kSB));
-  if (dtype == 0)
+  if (dtype == 2)
+    simt_scores_kernel<__nv_bfloat16, int8_t><<<grid, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(q),
+                                                                  static_cast<const int8_t*>(rows), dim, nq, row0,
+                                                                  nrows_chunk, n_rows, inv_norm, f, scores);
+  else if (dtype == 0)
     simt_scores_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(q),
                                                           static_cast<const __nv_bfloat16*>(rows), dim, nq, row0,
                                                           nrows_chunk, n_rows, inv_norm, f, scores);
@@ -594,12 +684,14 @@ cudaError_t launch_finalize(const FinalizeArgs& a_in, cudaStream_t s) {
   const size_t smem = static_cast<size_t>(P) * 8 + static_cast<size_t>(a.dim) * 4;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(a.dtype == 0 ? (const void*)finalize_kernel<__nv_bfloat16>
-                                                      : (const void*)finalize_kernel<float>,
+                                         : a.dtype == 2 ? (const void*)finalize_kernel<__nv_bfloat16, int8_t>
+                                                        : (const void*)finalize_kernel<float>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
     if (e != cudaSuccess) return e;
   }
   // programmatic dependent launch: blocks start (query -> shared memory, |q|^2) while the similarity kernel drains
   if (a.dtype == 0) return launch_pdl(finalize_kernel<__nv_bfloat16>, dim3(a.nq), dim3(256), smem, s, 1, a);
+  if (a.dtype == 2) return launch_pdl(finalize_kernel<__nv_bfloat16, int8_t>, dim3(a.nq), dim3(256), smem, s, 1, a);
   return launch_pdl(finalize_kernel<float>, dim3(a.nq), dim3(256), smem, s, 1, a);
 }
 

@@ -46,6 +46,10 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4],
 
 // One CTA per (item, 64-row tile of its segment): the tile's k-chunks stream through the ring, so a short list is
 // spread over many SMs instead of being one CTA's chain of dependent loads.
+// TR: the rows' element type.  int8 rows are read 8 bytes (8 elements) per piece and stored into the ring as the 8
+// bf16 values they are exactly (plain loads and stores: the barrier that publishes a chunk orders them as it orders the
+// cp.async groups), so the MMAs see the same operands as for the rows stored as bf16.
+template <typename TR>
 __global__ void __launch_bounds__(kLThreads) list_scores_kernel(ListParams p) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __nv_bfloat16* ring = reinterpret_cast<__nv_bfloat16*>(smem_raw);
@@ -58,6 +62,7 @@ __global__ void __launch_bounds__(kLThreads) list_scores_kernel(ListParams p) {
   for (int i = threadIdx.x; i < t_rows; i += kLThreads) s_rows[i] = p.list_rows[it.row0 + j0 + i];
   for (int i = threadIdx.x; i < it.nq; i += kLThreads) s_q[i] = p.qidx[it.q0 + i];
   __syncthreads();
+  const TR* rows = static_cast<const TR*>(p.rows);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tiles = (it.nq + 15) >> 4;     // 16-query MMA row blocks in use
   const int qrows = m_tiles * 16;
@@ -76,7 +81,24 @@ __global__ void __launch_bounds__(kLThreads) list_scores_kernel(ListParams p) {
           if (r < it.nq && k < p.dim) { src = p.q + static_cast<size_t>(s_q[r]) * p.dim + k; bytes = 16; }
         } else {
           dst_row = kListQMax + (r - qrows);
-          if (k < p.dim) { src = p.rows + static_cast<size_t>(s_rows[r - qrows]) * p.dim + k; bytes = 16; }
+          if constexpr (sizeof(TR) == 1) {
+            uint32_t w[4] = {0u, 0u, 0u, 0u};   // 8 bf16 values, zeros for k beyond dim
+            if (k < p.dim) {
+              const uint2 v = __ldg(reinterpret_cast<const uint2*>(rows + static_cast<size_t>(s_rows[r - qrows]) * p.dim + k));
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const uint32_t b = (e < 2 ? v.x : v.y) >> (16 * (e & 1));
+                const __nv_bfloat162 h2 = __floats2bfloat162_rn(static_cast<float>(static_cast<int8_t>(b)),
+                                                                static_cast<float>(static_cast<int8_t>(b >> 8)));
+                w[e] = *reinterpret_cast<const uint32_t*>(&h2);
+              }
+            }
+            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(base + (dst_row * kLPitch + (i & 7) * 8) * 2),
+                         "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
+            continue;
+          } else if (k < p.dim) {
+            src = rows + static_cast<size_t>(s_rows[r - qrows]) * p.dim + k; bytes = 16;
+          }
         }
         cp_async16(base + (dst_row * kLPitch + (i & 7) * 8) * 2, src, bytes);
       }
@@ -175,9 +197,10 @@ __global__ void __launch_bounds__(256) list_select_kernel(ListParams p) {
 
 cudaError_t launch_list_search(const ListParams& p, int max_nq, cudaStream_t s) {
   if (p.n_items <= 0) return cudaSuccess;
-  cudaError_t e = cudaFuncSetAttribute(list_scores_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kLSmem));
+  auto kern = p.rows_i8 ? list_scores_kernel<int8_t> : list_scores_kernel<__nv_bfloat16>;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kLSmem));
   if (e != cudaSuccess) return e;
-  list_scores_kernel<<<dim3(p.n_items, kSimtSeg / kLTile), kLThreads, kLSmem, s>>>(p);
+  kern<<<dim3(p.n_items, kSimtSeg / kLTile), kLThreads, kLSmem, s>>>(p);
   list_select_kernel<<<dim3(p.n_items, max_nq), 256, 0, s>>>(p);
   return cudaGetLastError();
 }

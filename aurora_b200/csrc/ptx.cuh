@@ -214,6 +214,35 @@ __device__ __forceinline__ void wgmma_m64n64_rs_tb(float (&d)[32], const uint32_
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
 }
 #undef AUR_R8
+#define AUR_I8R(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
+// D[64 x 64] (+)= A[smem, K-major] . B[smem, K-major]^T, s8 in, s32 accumulate; one K = 32 step (32 bytes of K, the
+// same descriptor advance as a bf16 K = 16 step).
+__device__ __forceinline__ void wgmma_m64n64_s8(int32_t (&d)[32], uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31},"
+      " %32, %33, p;\n\t}"
+      : AUR_I8R(0), AUR_I8R(8), AUR_I8R(16), AUR_I8R(24)
+      : "l"(a), "l"(b), "r"(accumulate));
+}
+// Same, N = 128.
+__device__ __forceinline__ void wgmma_m64n128_s8(int32_t (&d)[64], uint64_t a, uint64_t b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63},"
+      " %64, %65, p;\n\t}"
+      : AUR_I8R(0), AUR_I8R(8), AUR_I8R(16), AUR_I8R(24), AUR_I8R(32), AUR_I8R(40), AUR_I8R(48), AUR_I8R(56)
+      : "l"(a), "l"(b), "r"(accumulate));
+}
+#undef AUR_I8R
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(int32_t (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
 
 __device__ __forceinline__ void unpack_u64(uint64_t v, uint32_t& lo, uint32_t& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v));

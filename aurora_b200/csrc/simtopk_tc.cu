@@ -283,11 +283,21 @@ constexpr uint32_t kNaNBits = 0x7FC00000u;
 //
 // kQReg: the first kQReg query k-blocks are the MMA warpgroup's register A operand instead of shared-memory tiles
 // (128-row tiles only; the host launches it only when dim / 64 >= kQReg).  Every two of them free one 16 KB ring stage.
-template <int kCtaGroup, bool kMask, int kTileN, int kQReg>
+//
+// kI8: int8 corpus rows (AUR_I8).  A corpus k-block is still one 128-byte swizzled row of a ring stage, now 128 int8
+// (UINT8 tensor map), so a stage carries twice the dimensions.  p.q is then the query image of launch_query_image_i8:
+// each query as q16 = 256 hi + lo (hi, lo int8), laid out [dim / 128][hi 128 B | lo 128 B], dim * 2 bytes a query like
+// a bf16 query row -- the staging below copies it unchanged, so query tile 2 kb is hi and 2 kb + 1 is lo of corpus
+// k-block kb.  Per k-block the MMA warpgroup issues 4 wgmma m64nNk32 s8 into acc_hi and 4 into acc_lo, one commit group,
+// and hands the epilogue fmaf(acc_hi, 256, acc_lo): |acc| <= 127 * 128 * 1024 < 2^24, so both convert exactly and the
+// combination rounds once.  That is q16 . c, the cosine times a positive per-query factor: every comparison the
+// epilogue, the threshold exchange and the candidate keys make is between scores of one query, so nothing else changes.
+template <int kCtaGroup, bool kMask, int kTileN, int kQReg, bool kI8 = false>
 __global__ void __launch_bounds__(kThreads, 1)
 simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   static_assert(kTileN == kTcTileN || kTileN == kTcTileWide, "tile width");
   static_assert(kQReg == 0 || kTileN == kTcTileWide, "register-resident query k-blocks: 128-row tiles only");
+  static_assert(!(kI8 && kQReg), "int8 rows: query image in shared memory only");
   constexpr uint32_t kStageBytes = stage_bytes(kTileN);
   constexpr int kScStride = sc_stride(kTileN);
   constexpr int kHalves = kTileN / 64;   // the epilogue examines a tile 64 scores (four 16-score chunks) at a time
@@ -333,7 +343,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
     n_tsets = gridDim.x / p.n_qblocks;
   }
   const int my_tiles = (p.n_tiles > tset) ? (p.n_tiles - tset + n_tsets - 1) / n_tsets : 0;
-  const int kbs = p.dim / kTcKBlock;  // 128-byte k-blocks per row
+  const int kbs = p.dim / kTcKBlock;  // 128-byte k-blocks per query row (bf16 row, or int8 query image)
+  const int kbs_c = kI8 ? p.dim / kTcKBlockI8 : kbs;   // 128-byte k-blocks per corpus row
 
   // exchange geometry: R-th largest of the m-th best of `nuse` CTAs is a valid threshold
   const int ksel = p.ksel;
@@ -375,7 +386,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
       for (int it = 0; it < my_tiles; ++it) {
         const int tile = tset + it * n_tsets;
         const int row0 = tile * kTileN + static_cast<int>(rank) * (kTileN / kCtaGroup);
-        for (int kb = 0; kb < kbs; ++kb) {
+        for (int kb = 0; kb < kbs_c; ++kb) {
           {
             const long long t0 = TCLK();
             mbar_wait(&empty_bar[stage], phase ^ 1u);
@@ -383,10 +394,11 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
           }
           uint8_t* dst = smem + static_cast<uint32_t>(stage) * kStageBytes;
           mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);   // the whole tile lands here, half of it from the peer
+          constexpr int kKb = kI8 ? kTcKBlockI8 : kTcKBlock;   // elements of a 128-byte k-block
           if constexpr (kCtaGroup == 1)
-            tma_load_2d(dst, &tmap, &full_bar[stage], kb * kTcKBlock, row0, hint);
+            tma_load_2d(dst, &tmap, &full_bar[stage], kb * kKb, row0, hint);
           else
-            tma_load_2d_mc(dst + rank * (kStageBytes / 2), &tmap, &full_bar[stage], kb * kTcKBlock, row0, 0x3, hint);
+            tma_load_2d_mc(dst + rank * (kStageBytes / 2), &tmap, &full_bar[stage], kb * kKb, row0, 0x3, hint);
           if (++stage == p.num_stages) { stage = 0; phase ^= 1u; }
         }
       }
@@ -471,6 +483,31 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
     };
     for (int it = 0; it < my_tiles; ++it) {
       float d[kTileN / 2];
+      if constexpr (kI8) {
+        int32_t dh[kTileN / 2], dl[kTileN / 2];
+#pragma unroll
+        for (int i = 0; i < kTileN / 2; ++i) { dh[i] = 0; dl[i] = 0; }
+        for (int kb = 0; kb < kbs_c; ++kb)
+          kblock(kb, [&](uint64_t db) {
+            const uint64_t dah = wgmma_desc_sw128(qs_a + static_cast<uint32_t>(2 * kb) * kQTileBytes);
+            const uint64_t dal = wgmma_desc_sw128(qs_a + static_cast<uint32_t>(2 * kb + 1) * kQTileBytes);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {   // 4 x K=32 per 128-byte k-block, hi then lo
+              if constexpr (kTileN == kTcTileWide) wgmma_m64n128_s8(dh, dah + 2 * k, db + 2 * k, 1u);
+              else wgmma_m64n64_s8(dh, dah + 2 * k, db + 2 * k, 1u);
+            }
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              if constexpr (kTileN == kTcTileWide) wgmma_m64n128_s8(dl, dal + 2 * k, db + 2 * k, 1u);
+              else wgmma_m64n64_s8(dl, dal + 2 * k, db + 2 * k, 1u);
+            }
+          });
+        wgmma_wait<0>();
+        wgmma_fence_regs(dh);
+        wgmma_fence_regs(dl);
+#pragma unroll
+        for (int i = 0; i < kTileN / 2; ++i) d[i] = fmaf(static_cast<float>(dh[i]), 256.f, static_cast<float>(dl[i]));
+      } else {
 #pragma unroll
       for (int i = 0; i < kTileN / 2; ++i) d[i] = 0.f;
       if constexpr (kQReg > 0) {
@@ -492,6 +529,7 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
         });
       wgmma_wait<0>();
       wgmma_fence_regs(d);
+      }
       release();
       {
         const long long t0 = TCLK();
@@ -904,9 +942,9 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   if constexpr (kCtaGroup == 2) cluster_sync_all();
 }
 
-template <int kCtaGroup, bool kMask, int kTileN, int kQReg = 0>
+template <int kCtaGroup, bool kMask, int kTileN, int kQReg = 0, bool kI8 = false>
 cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm, const TcParams& p, size_t smem) {
-  auto kern = simtopk_tc_kernel<kCtaGroup, kMask, kTileN, kQReg>;
+  auto kern = simtopk_tc_kernel<kCtaGroup, kMask, kTileN, kQReg, kI8>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
   if (e != cudaSuccess) return e;
   return cudaLaunchKernelEx(&cfg, kern, tm, p);
@@ -924,7 +962,8 @@ int tc_pick_stages(int ksel, int dim, size_t smem_limit, int tile_n, bool mask, 
   return 0;
 }
 
-cudaError_t tc_launch(int cta_group, int tile_n, int qregs, int grid, const void* tmap, const TcParams& p, size_t smem, cudaStream_t s) {
+cudaError_t tc_launch(int cta_group, int tile_n, int qregs, bool i8, int grid, const void* tmap, const TcParams& p, size_t smem,
+                      cudaStream_t s) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(kThreads);
@@ -939,6 +978,15 @@ cudaError_t tc_launch(int cta_group, int tile_n, int qregs, int grid, const void
   cfg.numAttrs = 1;
   const CUtensorMap& tm = *reinterpret_cast<const CUtensorMap*>(tmap);
   const bool mask = p.row_mask != nullptr;
+  if (i8) {
+    if (qregs != 0 || p.dim % kTcKBlockI8 != 0) return cudaErrorInvalidValue;
+    if (tile_n == kTcTileWide) {
+      if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileWide, 0, true>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileWide, 0, true>(cfg, tm, p, smem);
+      return mask ? launch_variant<1, true, kTcTileWide, 0, true>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileWide, 0, true>(cfg, tm, p, smem);
+    }
+    if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileN, 0, true>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileN, 0, true>(cfg, tm, p, smem);
+    return mask ? launch_variant<1, true, kTcTileN, 0, true>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileN, 0, true>(cfg, tm, p, smem);
+  }
   if (qregs != 0) {   // smem was sized without these k-blocks' tiles: only the matching kernel may run
     if (qregs != kTcQRegs || tile_n != kTcTileWide || p.dim / kTcKBlock < qregs) return cudaErrorInvalidValue;
     if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileWide, kTcQRegs>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileWide, kTcQRegs>(cfg, tm, p, smem);

@@ -26,13 +26,31 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+_DTYPES = {"bf16": N.AUR_BF16, "f32": N.AUR_F32, "int8": N.AUR_I8}
+_DTYPE_NAMES = {v: k for k, v in _DTYPES.items()}
+
+
+def _row_dtype(dtype: int):
+    """numpy element type of the rows an index stores (export / read_rows)."""
+    return {N.AUR_BF16: np.uint16, N.AUR_F32: np.float32, N.AUR_I8: np.int8}[dtype]
+
+
 class Index:
-    """One row-shard of the corpus, resident on one GPU."""
+    """One row-shard of the corpus, resident on one GPU.
+
+    ``dtype="int8"`` stores every row as int8 (half the memory of bf16): rows and queries go in as floats or bf16 bits,
+    and each row is quantized on the device as it is added (``oracle/quantize.py``).  Scores are exact cosines against
+    the stored int8 rows; ``export`` / ``read_rows`` / ``save`` return them as int8."""
 
     def __init__(self, dim: int, capacity: int, dtype: str = "bf16", device: int = 0):
+        if dtype not in _DTYPES:
+            raise ValueError(f"dtype must be one of {sorted(_DTYPES)}, not {dtype!r}")
+        dim = int(dim)
+        if dtype == "int8" and dim % 16:
+            raise ValueError("int8 rows need dim % 16 == 0")
         self._lib = N.load()
-        self.dim, self.capacity, self.device = int(dim), int(capacity), int(device)
-        self.dtype = {"bf16": N.AUR_BF16, "f32": N.AUR_F32}[dtype]
+        self.dim, self.capacity, self.device = dim, int(capacity), int(device)
+        self.dtype = _DTYPES[dtype]
         self._h = C.c_void_p()
         cfg = N.AurConfig(device=self.device, dim=self.dim, dtype=self.dtype, reserved=0, capacity=self.capacity)
         N.check(self._lib.aur_open(C.byref(cfg), C.byref(self._h)))
@@ -60,10 +78,10 @@ class Index:
         x = np.asarray(x)
         if x.ndim != 2 or x.shape[1] != self.dim:
             raise ValueError(f"expected [n, {self.dim}] rows, got {x.shape}")
-        if self.dtype == N.AUR_BF16:
+        if self.dtype in (N.AUR_BF16, N.AUR_I8):     # int8 shards take bf16 rows and queries
             if x.dtype == np.uint16:
                 return np.ascontiguousarray(x)
-            return to_bf16_bits(x)
+            return to_bf16_bits(x)      # (int8 rows of a snapshot are exact in bf16)
         return np.ascontiguousarray(x, dtype=np.float32)
 
     # -------------------------------------------------------------- ingest
@@ -92,29 +110,36 @@ class Index:
 
     # -------------------------------------------------------------- snapshot
     def export(self):
-        """All appended rows in append order: (rows [n, dim] uint16 bf16 bits or float32, ids, user codes,
+        """All appended rows in append order: (rows [n, dim] uint16 bf16 bits, float32 or int8, ids, user codes,
         org codes, live mask).  Tombstoned rows are included with live = False."""
+        rows, ids, user, org, live = self.export_raw()
+        return rows, ids, user, org, live.astype(bool)
+
+    def export_raw(self):
+        """``export`` with aur_export's live flags as they are: 0 tombstone, 1 live, 2 live int8 row stored from a row
+        holding a NaN or inf (zeros that no search returns)."""
         n = self.stats()["rows"]
-        rows = np.empty((n, self.dim), dtype=np.uint16 if self.dtype == N.AUR_BF16 else np.float32)
+        rows = np.empty((n, self.dim), dtype=_row_dtype(self.dtype))
         ids = np.empty(n, dtype=np.int64)
         user, org = np.empty(n, dtype=np.int32), np.empty(n, dtype=np.int32)
         live = np.empty(n, dtype=np.uint8)
         N.check(self._lib.aur_export(self._h, _ptr(rows), _ptr(ids), _ptr(user), _ptr(org), _ptr(live), n))
-        return rows, ids, user, org, live.astype(bool)
+        return rows, ids, user, org, live
 
     def save(self, path: str) -> None:
         """Snapshot of the live rows (tombstones are compacted away) as one .npz file."""
-        rows, ids, user, org, live = self.export()
-        np.savez(path, rows=rows[live], ids=ids[live], user=user[live], org=org[live], dim=self.dim,
-                 dtype=self.dtype, capacity=self.capacity)
+        rows, ids, user, org, live = self.export_raw()
+        keep = live > 0
+        np.savez(path, rows=rows[keep], ids=ids[keep], user=user[keep], org=org[keep], nonfinite=live[keep] == 2,
+                 dim=self.dim, dtype=self.dtype, capacity=self.capacity)
 
     @classmethod
     def load(cls, path: str, capacity: Optional[int] = None, device: int = 0) -> "Index":
         z = np.load(path if path.endswith(".npz") else path + ".npz")
-        dtype = "bf16" if int(z["dtype"]) == N.AUR_BF16 else "f32"
+        dtype = _DTYPE_NAMES[int(z["dtype"])]
         ix = cls(int(z["dim"]), int(capacity or z["capacity"]), dtype=dtype, device=device)
         if len(z["ids"]):
-            ix.add(z["rows"], z["ids"], z["user"], z["org"])
+            ix.add(_snapshot_rows(z), z["ids"], z["user"], z["org"])
         return ix
 
     # -------------------------------------------------------------- search
@@ -142,8 +167,8 @@ class Index:
         return ids, scores, int(snap.value)
 
     def read_rows(self, row0: int, n: int):
-        """(rows [n, dim] uint16 bf16 bits or float32, ids [n]) of appended rows row0 .. row0 + n."""
-        rows = np.empty((n, self.dim), dtype=np.uint16 if self.dtype == N.AUR_BF16 else np.float32)
+        """(rows [n, dim] uint16 bf16 bits, float32 or int8, ids [n]) of appended rows row0 .. row0 + n."""
+        rows = np.empty((n, self.dim), dtype=_row_dtype(self.dtype))
         ids = np.empty(n, dtype=np.int64)
         N.check(self._lib.aur_read_rows(self._h, int(row0), int(n), _ptr(rows), _ptr(ids)))
         return rows, ids
@@ -267,6 +292,16 @@ def lists_csr(lists):
     np.cumsum([len(a) for a in parts], out=offsets[1:])
     flat = np.ascontiguousarray(np.concatenate(parts)) if parts and offsets[-1] else np.zeros(1, dtype=np.int64)
     return flat, offsets
+
+
+def _snapshot_rows(z) -> np.ndarray:
+    """The rows of a snapshot as ``add`` takes them.  An int8 row stored from a row holding a NaN or inf (zeros, never
+    returned) is re-added as a bf16 row holding a NaN, so the restored shard stores it, and answers, as before."""
+    rows = z["rows"]
+    if "nonfinite" in z.files and z["nonfinite"].any():
+        rows = to_bf16_bits(np.asarray(rows, dtype=np.float32))     # int8 values are exact in bf16
+        rows[z["nonfinite"], 0] = 0x7FC0
+    return rows
 
 
 def shard_capacity(capacity: int, n: int) -> int:
@@ -394,17 +429,20 @@ class MultiIndex:
 
     def save(self, path: str) -> None:
         """One .npz like Index.save (live rows of all shards): a snapshot restores onto any number of devices."""
-        parts = self._each(lambda s, shard: shard.export())
-        cat = lambda i: np.concatenate([np.asarray(p[i])[p[4]] for p in parts])   # noqa: E731
-        np.savez(path, rows=cat(0), ids=cat(1), user=cat(2), org=cat(3), dim=self.dim, dtype=self.dtype, capacity=self.capacity)
+        parts = self._each(lambda s, shard: shard.export_raw() if hasattr(shard, "export_raw") else shard.export())
+        keep = [np.asarray(p[4]) > 0 for p in parts]
+        cat = lambda i: np.concatenate([np.asarray(p[i])[m] for p, m in zip(parts, keep)])   # noqa: E731
+        nonfinite = np.concatenate([np.asarray(p[4])[m] == 2 for p, m in zip(parts, keep)])
+        np.savez(path, rows=cat(0), ids=cat(1), user=cat(2), org=cat(3), nonfinite=nonfinite, dim=self.dim, dtype=self.dtype,
+                 capacity=self.capacity)
 
     @classmethod
     def load(cls, path: str, capacity: Optional[int] = None, devices=None, shard_factory=None) -> "MultiIndex":
         z = np.load(path if path.endswith(".npz") else path + ".npz")
-        dtype = "bf16" if int(z["dtype"]) == N.AUR_BF16 else "f32"
+        dtype = _DTYPE_NAMES[int(z["dtype"])]
         mi = cls(int(z["dim"]), int(capacity or z["capacity"]), devices=devices, dtype=dtype, shard_factory=shard_factory)
         if len(z["ids"]):
-            mi.add(z["rows"], z["ids"], z["user"], z["org"])
+            mi.add(_snapshot_rows(z), z["ids"], z["user"], z["org"])
         return mi
 
     def close(self) -> None:
@@ -608,8 +646,8 @@ def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_o
     if multi:
         if not isinstance(kw_index, MultiKeywordIndex):
             raise TypeError("a MultiIndex is searched together with a MultiKeywordIndex")
-        if not index.shards or not all(isinstance(sh, Index) and sh.dtype == N.AUR_BF16 for sh in index.shards):
-            raise TypeError("hybrid_search over a MultiIndex needs bf16 engine.Index shards")
+        if not index.shards or not all(isinstance(sh, Index) and sh.dtype in (N.AUR_BF16, N.AUR_I8) for sh in index.shards):
+            raise TypeError("hybrid_search over a MultiIndex needs bf16 or int8 engine.Index shards")
         if kw_index.devices != index.devices or len(kw_index.stores) != len(index.shards):
             raise ValueError(f"keyword stores on devices {kw_index.devices}, vector shards on {index.devices}")
         q = index.shards[0]._rows_buffer(queries)

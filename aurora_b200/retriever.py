@@ -34,7 +34,7 @@ from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import numpy as np
 
-from ._native import AUR_BF16, FUSION_RANKED, FUSION_RELATIVE_SCORE
+from ._native import AUR_BF16, AUR_I8, FUSION_RANKED, FUSION_RELATIVE_SCORE
 from .bm25 import BM25Index
 from .filters import AttrColumn, Filter, HybridFusion, compile_program  # noqa: F401  (Filter, HybridFusion: re-exported)
 
@@ -71,7 +71,7 @@ class KnowledgeBase:
     """
 
     def __init__(self, encoder, capacity: int = 1 << 20, device: int = 0,
-                 index_factory: Optional[Callable[[int, int], Any]] = None):
+                 index_factory: Optional[Callable[[int, int], Any]] = None, dtype: str = "bf16"):
         if encoder is None:
             raise RuntimeError("aurora_b200.retriever needs an encoder (text -> vector); none configured")
         self.encoder = encoder
@@ -80,7 +80,7 @@ class KnowledgeBase:
             from .engine import Index  # raises loudly if the CUDA library is missing
 
             def index_factory(dim, cap):
-                return Index(dim, cap, dtype="bf16", device=device)
+                return Index(dim, cap, dtype=dtype, device=device)   # "int8": half the HBM, exact over the int8 rows
         self.index = index_factory(self.dim, int(capacity))
         # keyword leg of the hybrid query: on the GPU beside a CUDA vector index, else the host index
         self.sparse = self._keyword_store(int(capacity))
@@ -124,7 +124,7 @@ class KnowledgeBase:
 
     def _fuses_on_device(self) -> bool:
         """Whether a hybrid query runs as one device call, both legs and their fusion (``engine.hybrid_search``): a bf16
-        ``engine.Index`` and a ``DeviceBM25`` over a ``KeywordIndex`` on its GPU, or a ``MultiIndex`` of bf16
+        or int8 ``engine.Index`` and a ``DeviceBM25`` over a ``KeywordIndex`` on its GPU, or a ``MultiIndex`` of such
         ``engine.Index`` shards and a ``DeviceBM25`` over a ``MultiKeywordIndex`` on the same devices in the same order.
         Filtered queries too, when their filter compiles to a device program (attribute columns are then kept on the
         keyword store as well).  f32 shards, the CPU doubles and filters that stay on the host fuse on the host
@@ -136,10 +136,10 @@ class KnowledgeBase:
         if not isinstance(sp, DeviceBM25):
             return False
         if isinstance(ix, MultiIndex):
-            return (bool(ix.shards) and all(isinstance(sh, Index) and sh.dtype == AUR_BF16 for sh in ix.shards)
+            return (bool(ix.shards) and all(isinstance(sh, Index) and sh.dtype in (AUR_BF16, AUR_I8) for sh in ix.shards)
                     and isinstance(sp.store, MultiKeywordIndex) and sp.store.devices == ix.devices
                     and len(sp.store.stores) == len(ix.shards))
-        return (isinstance(ix, Index) and ix.dtype == AUR_BF16 and isinstance(sp.store, KeywordIndex)
+        return (isinstance(ix, Index) and ix.dtype in (AUR_BF16, AUR_I8) and isinstance(sp.store, KeywordIndex)
                 and sp.store.device == ix.device)
 
     def _scope_codes(self, user_id: Optional[str], org_id: Optional[str]) -> Tuple[int, int]:
@@ -338,7 +338,7 @@ class KnowledgeBase:
         resolved on the host: an index without device filters (CPU doubles, f32 shards), a property without a column, or
         a leaf whose evaluation raises (the host path then raises as it always has).  The tenant scope is written over
         the ``user_id`` / ``org_id`` properties, exactly as the host predicate reads it.  Caller holds the lock."""
-        if not hasattr(self.index, "search_filtered") or getattr(self.index, "dtype", None) != AUR_BF16:
+        if not hasattr(self.index, "search_filtered") or getattr(self.index, "dtype", None) not in (AUR_BF16, AUR_I8):
             return None
         expr = filters
         if tenant:
@@ -752,8 +752,9 @@ _state_lock = threading.Lock()
 
 
 def configure(encoder=None, capacity: Optional[int] = None, device: Optional[int] = None, index_factory=None,
-              factory: Optional[Callable[[], KnowledgeBase]] = None) -> None:
-    """Install the backend.  Environment: AURORA_B200_CAPACITY, AURORA_B200_DEVICE."""
+              factory: Optional[Callable[[], KnowledgeBase]] = None, dtype: Optional[str] = None) -> None:
+    """Install the backend.  Environment: AURORA_B200_CAPACITY, AURORA_B200_DEVICE, AURORA_B200_DTYPE (the shard's row
+    format: bf16, the default, or int8)."""
     global _kb, _kb_factory
     with _state_lock:
         _kb = None
@@ -762,7 +763,8 @@ def configure(encoder=None, capacity: Optional[int] = None, device: Optional[int
             return
         cap = capacity if capacity is not None else int(os.getenv("AURORA_B200_CAPACITY", str(1 << 20)))
         dev = device if device is not None else int(os.getenv("AURORA_B200_DEVICE", "0"))
-        _kb_factory = lambda: KnowledgeBase(encoder, capacity=cap, device=dev, index_factory=index_factory)  # noqa: E731
+        dt = dtype if dtype is not None else os.getenv("AURORA_B200_DTYPE", "bf16")
+        _kb_factory = lambda: KnowledgeBase(encoder, capacity=cap, device=dev, index_factory=index_factory, dtype=dt)  # noqa: E731
 
 
 def _get_kb() -> KnowledgeBase:

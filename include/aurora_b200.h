@@ -17,7 +17,7 @@
  *     passed as void* (NULL = the index's own stream; pass cudaStreamLegacy, (void*)1, for
  *     the legacy default stream) and do not synchronise;
  *   - vectors are row-major [n, dim]; dtype is fixed per index (AUR_BF16: raw uint16
- *     bfloat16 bits; AUR_F32: IEEE float);
+ *     bfloat16 bits; AUR_F32: IEEE float; AUR_I8: rows are stored as int8, see aur_dtype);
  *   - ids are caller-chosen int64 (>= 0), unique per index; adding an existing id
  *     replaces the old row (reference: deterministic uuid5 upsert,
  *     weaviate_client.py:172);
@@ -51,7 +51,14 @@ typedef enum aur_status {
   AUR_ERR_NO_DEVICE = -5    /* no CUDA device (the library has no CPU path)   */
 } aur_status;
 
-typedef enum aur_dtype { AUR_BF16 = 0, AUR_F32 = 1 } aur_dtype;
+/* AUR_I8: rows are stored as int8 [capacity, dim] (dim % 16 == 0), half the memory of bf16.  Rows and queries go in
+ * as bf16 bits, as for AUR_BF16; each row is quantized on the device when it is added:
+ * q = rint(x * 127 / max|x|) in fp64 (half to even), a zero row stays zero, and a row holding a NaN or +-inf is stored
+ * as zeros and never returned by a search (as in a bf16 shard).  Cosine ignores the per-row scale, so scores are exact
+ * cosines against the stored int8 rows.  aur_export / aur_read_rows return the int8 rows.  The tensor-core kernel
+ * serves int8 shards with dim % 128 == 0 and dim <= 1024 (wgmma s8 over a two-byte query image); "tc_qregs" does not
+ * apply to them, and aur_debug_tc_scores is unsupported. */
+typedef enum aur_dtype { AUR_BF16 = 0, AUR_F32 = 1, AUR_I8 = 2 } aur_dtype;
 
 /* Which similarity kernel serves a search (aur_set_option "kernel"). */
 typedef enum aur_kernel {
@@ -120,7 +127,8 @@ int aur_add_dev(aur_index* ix, const void* rows_dev, const int64_t* ids_host,
 /* Snapshot.  Replaces the Weaviate data volume (docker-compose.yaml:477-478) as the durable copy of
  * the shard: copies all n = aur_stats.rows appended rows (tombstones included, live_out[i] = 0 for
  * them) back to the host in append order.  Restore = aur_open + aur_add of the live rows, which also
- * compacts the tombstones away.  user_out / org_out may be NULL. */
+ * compacts the tombstones away.  user_out / org_out may be NULL.  AUR_I8: live_out[i] = 2 for a live row stored from a
+ * row holding a NaN or +-inf (zeros that no search returns); a restore re-adds it as a row holding a NaN. */
 int aur_export(aur_index* ix, void* rows_out, int64_t* ids_out, int32_t* user_out,
                int32_t* org_out, uint8_t* live_out, int64_t n);
 
