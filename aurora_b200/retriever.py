@@ -30,10 +30,11 @@ import threading
 import uuid
 from datetime import datetime, timezone
 from types import SimpleNamespace
-from typing import Any, Callable, Dict, List, Optional, Tuple
+from typing import Any, Callable, Dict, List, NamedTuple, Optional, Tuple
 
 import numpy as np
 
+from . import bm25
 from ._native import AUR_BF16, AUR_I8, FUSION_RANKED, FUSION_RELATIVE_SCORE
 from .bm25 import BM25Index
 from .filters import AttrColumn, Filter, HybridFusion, compile_program  # noqa: F401  (Filter, HybridFusion: re-exported)
@@ -54,6 +55,32 @@ _FUSION = {HybridFusion.RANKED: FUSION_RANKED, HybridFusion.RELATIVE_SCORE: FUSI
 def _sanitize(value: Any) -> str:
     """utils.log_sanitizer.sanitize stand-in: strip control characters from logged values."""
     return "".join(ch if ch.isprintable() else "?" for ch in str(value))
+
+
+class _Request(NamedTuple):
+    """One search as ``KnowledgeBase.query`` takes it (``fusion`` None already read as RANKED)."""
+    text: str
+    limit: int
+    alpha: Optional[float]
+    fusion: str
+    filters: Any
+    user: Optional[str]
+    org: Optional[str]
+    scoped: bool
+
+    @property
+    def searchable(self) -> bool:
+        """False when the answer is [] without a search: no result asked for, or a tenant-facing search without a tenant."""
+        return self.limit > 0 and bool(self.user or self.org or not self.scoped)
+
+    @property
+    def hybrid(self) -> bool:
+        return self.alpha is not None and self.alpha < 1.0
+
+    @property
+    def dense_w(self) -> float:
+        """The dense leg's weight: 1 for a vector search, else alpha (at least 0; 0 leaves the dense leg unsearched)."""
+        return max(0.0, float(self.alpha)) if self.hybrid else 1.0
 
 
 def generate_uuid5(identifier: str) -> str:
@@ -369,10 +396,7 @@ class KnowledgeBase:
     # ------------------------------------------------------------------ search
     def query(self, query: str, limit: int, filters=None, user_id: Optional[str] = None,
               org_id: Optional[str] = None, alpha: Optional[float] = None, scoped: bool = False,
-              fusion: str = HybridFusion.RANKED,
-              _dense: Optional[List[Tuple[int, float]]] = None,
-              _sparse: Optional[List[Tuple[int, float]]] = None,
-              _fused: Optional[list] = None) -> List[SimpleNamespace]:
+              fusion: str = HybridFusion.RANKED) -> List[SimpleNamespace]:
         """Top-``limit`` objects.  ``alpha`` None or >= 1: pure vector search, ``score`` = cosine
         (near_text, incident_feedback/weaviate_client.py:286-297).  ``alpha`` < 1: hybrid
         (weaviate_client.py:252-259), ``score`` = the fused score of the dense and BM25 lists with weights
@@ -394,130 +418,163 @@ class KnowledgeBase:
         ``scoped``: the caller is a tenant-facing entry point (search_knowledge_base): a missing user AND
         org matches nothing instead of everything (the reference always applies ``user_id == u``,
         weaviate_client.py:244-249)."""
-        if limit <= 0:
-            return []
-        if scoped and not user_id and not org_id:
-            return []
-        if fusion is None:
-            fusion = HybridFusion.RANKED
-        if fusion not in _FUSION:
+        req = _Request(query, limit, alpha, HybridFusion.RANKED if fusion is None else fusion, filters, user_id, org_id,
+                       scoped)
+        if req.searchable and req.fusion not in _FUSION:
             raise NotImplementedError(f"hybrid fusion {fusion!r}: only HybridFusion.RANKED and RELATIVE_SCORE are implemented")
-        hybrid = alpha is not None and alpha < 1.0
-        dense_w = 1.0 if not hybrid else max(0.0, float(alpha))
-        on_device = (_fused is None and _dense is None and _sparse is None and hybrid and filters is None
-                     and self._hybrid_device)
-        if on_device:                       # a query whose dense leg is ignored still passes a vector: zeros
-            qv = self.encoder.encode([query]) if dense_w > 0.0 else np.zeros((1, self.dim), np.float32)
-        else:
-            qv = self.encoder.encode([query]) if (dense_w > 0.0 and _dense is None and _fused is None) else None
+        return self._search([req])[0]
+
+    def query_batch(self, reqs: List[Tuple[Optional[str], str, int, Optional[float], Optional[str]]]) -> List[List[SimpleNamespace]]:
+        """Several tenant-scoped searches at once: ``(user_id, query, limit, alpha, org_id)`` each, answered as ``query``
+        answers them with ``scoped=True``.  All query texts go through ONE encoder batch; the dense leg is ONE kernel
+        launch per result size (the tenant scopes of the batch ride along as per-row bit masks on the tensor-core kernel);
+        on a GPU keyword store the keyword leg of every hybrid request (alpha < 1) is ONE device search with per-request
+        tenant codes.  On a CUDA shard whose hybrid requests carry at most 32 distinct tenant scopes, those requests are
+        instead ONE device call for both legs and their ranked fusion (``DeviceBM25.search_batch`` with ``dense``,
+        per-request weights), and only shaping is left per request."""
+        return self._search([_Request(q, lim, a, HybridFusion.RANKED, None, u, o, True) for u, q, lim, a, o in reqs])
+
+    def _search(self, reqs: List[_Request]) -> List[List[SimpleNamespace]]:
+        """The answers to ``reqs``.  Encode every dense leg in one call; under the lock resolve each request's scope;
+        answer on the device the hybrid requests that fuse there, one call per kind of scope and fusion; search the other
+        requests' legs, batched per kind of scope (and result size for the dense leg); fuse and shape on the host."""
+        live = [i for i, r in enumerate(reqs) if r.searchable]
+        enc = [i for i in live if reqs[i].dense_w > 0.0]
+        vecs = self.encoder.encode([reqs[i].text for i in enc]) if enc else None
+        row = {i: j for j, i in enumerate(enc)}
+        out: List[List[SimpleNamespace]] = [[] for _ in reqs]
         with self._lock:
-            tenant = scoped or user_id is not None or org_id is not None
-            if on_device:
-                q_user = q_org = None
-                if tenant:
-                    cu, co = self._scope_codes(user_id, org_id)
-                    q_user, q_org = np.array([cu], np.int32), np.array([co], np.int32)
-                _fused = self.sparse.search_batch([query], _MAX_FETCH, q_user, q_org,
-                                                  dense=(self.index, qv, np.array([dense_w]), _FUSION[fusion],
-                                                         min(limit, 2 * _MAX_FETCH)))[0]
-            if _fused is not None:          # fused on the device (here or by query_batch)
-                return self._shape([(rid, fs, cos) for rid, (fs, cos) in _fused if rid in self._props][:limit])
+            scope = {i: self._resolve_scope(reqs[i]) for i in live}
+            fused: Dict[int, list] = {}
+            calls: Dict[tuple, List[int]] = {}
+            for i in live:
+                if reqs[i].hybrid and self._hybrid_device and scope[i][0] != "ids":
+                    calls.setdefault((scope[i][0], reqs[i].fusion), []).append(i)
+            for (kind, fusion), g in calls.items():
+                vals = [scope[i][1] for i in g]
+                if kind == "codes" and len(set(vals)) > 32:   # more than the tensor-core kernel's per-row scope masks hold
+                    continue
+                hv = np.zeros((len(g), self.dim), vecs.dtype if vecs is not None else np.float32)
+                for j, i in enumerate(g):
+                    if i in row:            # alpha <= 0: the dense leg is ignored, its vector stays zero
+                        hv[j] = vecs[row[i]]
+                w = np.array([reqs[i].dense_w for i in g])
+                lists = self.sparse.search_batch([reqs[i].text for i in g], _MAX_FETCH, **self._scope_args(kind, vals),
+                                                 dense=(self.index, hv, w, _FUSION[fusion],
+                                                        min(max(reqs[i].limit for i in g), 2 * _MAX_FETCH)))
+                fused.update(zip(g, lists))
 
-            def tenant_ok(props) -> bool:
-                if not tenant:
-                    return True
-                return (bool(user_id) and props.get("user_id") == user_id) or \
-                       (bool(org_id) and props.get("org_id") == org_id)
-
-            allowed: Optional[List[int]] = None
-            prog = self._device_program(filters, tenant, user_id, org_id) if filters is not None else None
-            if prog is not None and hybrid and self._hybrid_device and _dense is None and _sparse is None:
-                # the whole filtered hybrid query in one device call: both legs evaluate the program on the GPU
-                if qv is None:              # the dense leg is ignored (alpha <= 0) but still takes a vector
-                    qv = np.zeros((1, self.dim), np.float32)
-                fused = self.sparse.search_batch(
-                    [query], _MAX_FETCH, dense=(self.index, qv, np.array([dense_w]), _FUSION[fusion], min(limit, 2 * _MAX_FETCH)),
-                    programs=[prog], max_list_rows=int(_LIST_MAX_FRACTION * len(self._props)))[0]
-                return self._shape([(rid, fs, cos) for rid, (fs, cos) in fused if rid in self._props][:limit])
-            if filters is not None and prog is None:
-                # narrow the scan with the filter's own equality terms and the tenant scope, then run the predicate
-                eq = filters.required_equalities()
-                pools = []
-                if "org_id" in eq:
-                    pools.append(self._by_org.get(eq["org_id"], set()))
-                if "user_id" in eq:
-                    pools.append(self._by_user.get(eq["user_id"], set()))
-                if tenant:
-                    pools.append(self._by_user.get(user_id, set()) | (self._by_org.get(org_id, set()) if org_id else set()))
-                cand = set.intersection(*pools) if pools else self._props.keys()
-                allowed = [rid for rid in cand if filters.matches(self._props[rid]) and tenant_ok(self._props[rid])]
-
-            dense: List[Tuple[int, float]] = []
-            if _dense is not None:          # dense leg already computed by query_batch (same scope, same fetch)
-                dense = [(rid, sc) for rid, sc in _dense if rid in self._props]
-            elif qv is not None and (prog is not None or allowed is None or allowed):
-                fetch = max(1, min(_MAX_FETCH, limit if not hybrid else _MAX_FETCH))
-                if prog is not None:        # no id crosses PCIe; the list-vs-scan rule is the host path's
-                    ids, scores, _, _ = self.index.search_filtered(
-                        qv, fetch, [prog], max_list_rows=int(_LIST_MAX_FRACTION * len(self._props)))
-                elif (allowed is not None and hasattr(self.index, "search_lists")
-                        and len(allowed) <= _LIST_MAX_FRACTION * len(self._props)):   # reads only the allowed rows
-                    ids, scores = self.index.search_lists(qv, fetch, [np.asarray(allowed, dtype=np.int64)],
-                                                          np.zeros(1, np.int32))
-                elif allowed is not None:
-                    ids, scores = self.index.search_subset(qv, fetch, np.asarray(allowed, dtype=np.int64))
-                else:
-                    q_user = q_org = None
-                    if tenant:
-                        q_user = np.array([self._code(self._user_code, user_id, False) if user_id else -2], dtype=np.int32)
-                        q_org = np.array([self._code(self._org_code, org_id, False) if org_id else -1], dtype=np.int32)
-                        if q_org[0] == -2:
-                            q_org[0] = -1
-                    ids, scores = self.index.search(qv, fetch, q_user, q_org)
-                for rid, sc in zip(ids[0], scores[0]):
-                    if rid < 0:
-                        break
-                    if int(rid) in self._props:
-                        dense.append((int(rid), float(sc)))
-            if not hybrid:
-                picked = [(rid, sc, sc) for rid, sc in dense[:limit]]
-            else:
-                # keyword leg under the same pre-filter: the resolved filter's ids, else the tenant's own inverted lists.
-                # A device program reaches here only with the keyword leg on the host (BM25Index beside an index that
-                # evaluates programs, e.g. a MultiIndex of CPU shard doubles): the device knowledge base fused above.
-                if prog is not None and _sparse is None:
-                    allowed = self.index.filter_ids(prog).tolist()
-                if _sparse is not None:     # keyword leg already computed by query_batch (same scope, same fetch);
-                    # objects deleted since then drop out, as for the dense leg
-                    sparse = [(rid, sc) for rid, sc in _sparse if rid in self._props]
-                elif self._kw_device:       # the device applies the tenant scope itself, as the dense leg does
-                    if allowed is not None:
-                        sparse = self.sparse.search(query, _MAX_FETCH, allowed=allowed)
-                    elif tenant:
-                        cu, co = self._scope_codes(user_id, org_id)
-                        sparse = self.sparse.search_batch([query], _MAX_FETCH, np.array([cu], np.int32),
-                                                          np.array([co], np.int32))[0]
+            groups: Dict[tuple, List[int]] = {}     # (fetch size, kind of scope, request of an allow-list) -> requests
+            for i in live:
+                kind, val = scope[i]
+                if i in row and i not in fused and (kind != "ids" or val):
+                    fetch = max(1, min(_MAX_FETCH, _MAX_FETCH if reqs[i].hybrid else reqs[i].limit))
+                    groups.setdefault((fetch, kind, i if kind == "ids" else None), []).append(i)
+            dense: Dict[int, List[Tuple[int, float]]] = {}
+            for (fetch, kind, _), g in groups.items():
+                q, vals = vecs[[row[i] for i in g]], [scope[i][1] for i in g]
+                if kind == "ids":
+                    allowed = np.asarray(vals[0], dtype=np.int64)
+                    if hasattr(self.index, "search_lists") and len(allowed) <= _LIST_MAX_FRACTION * len(self._props):
+                        ids, scores = self.index.search_lists(q, fetch, [allowed], np.zeros(1, np.int32))  # reads only those rows
                     else:
-                        sparse = self.sparse.search(query, _MAX_FETCH)
+                        ids, scores = self.index.search_subset(q, fetch, allowed)
+                elif kind == "program":     # no id crosses PCIe; the list-vs-scan rule is the host path's
+                    ids, scores, _, _ = self.index.search_filtered(q, fetch, **self._scope_args(kind, vals))
+                elif kind == "codes" and len(set(vals)) > 32 and hasattr(self.index, "search_lists"):
+                    # more scopes than the tensor-core kernel's row bit masks hold: one id list per scope (the rows
+                    # _tenant_scope gives the keyword leg) and one list search that reads only those rows
+                    slots: Dict[Tuple[int, int], int] = {}
+                    lists = []
+                    for i, v in zip(g, vals):
+                        if v not in slots:
+                            slots[v] = len(slots)
+                            lists.append(self._tenant_scope(reqs[i].user, reqs[i].org)[1])
+                    ids, scores = self.index.search_lists(q, fetch, lists, np.array([slots[v] for v in vals], np.int32))
                 else:
-                    allowed_arr = None
-                    if allowed is not None:
-                        allowed_set = set(allowed)
-                    elif tenant:
-                        allowed_set, allowed_arr = self._tenant_scope(user_id, org_id)
-                    else:
-                        allowed_set = None
-                    sparse = self.sparse.search(query, _MAX_FETCH, allowed=allowed_set, allowed_sorted=allowed_arr)
-                from . import bm25
+                    # one launch for the whole group: up to 32 distinct tenant scopes per batch ride on the tensor-core
+                    # kernel as per-row bit masks (csrc/capi.cu search_host); the library falls back by itself beyond
+                    ids, scores = self.index.search(q, fetch, **self._scope_args(kind, vals))
+                for i, r_ids, r_scores in zip(g, ids, scores):
+                    dense[i] = [(int(d), float(s)) for d, s in zip(r_ids, r_scores) if d >= 0]
 
-                cos = dict(dense)
-                if fusion == HybridFusion.RELATIVE_SCORE:
-                    fused = bm25.relative_score_fusion([(dense_w, dense), (1.0 - dense_w, sparse)], limit)
+            # keyword leg under the same pre-filter: a program's or the filter's ids, else the tenant scope (on the device
+            # by codes, as the dense leg applies it; on the host by the tenant's own inverted lists)
+            sparse: Dict[int, List[Tuple[int, float]]] = {}
+            kw_calls: Dict[str, List[int]] = {}
+            for i in live:
+                if not reqs[i].hybrid or i in fused:
+                    continue
+                kind, val = scope[i]
+                if kind == "program":       # only beside a keyword leg that cannot evaluate it (the others fused above)
+                    kind, val = "ids", self.index.filter_ids(val).tolist()
+                if kind == "ids":
+                    sparse[i] = self.sparse.search(reqs[i].text, _MAX_FETCH,
+                                                   allowed=val if self._kw_device else set(val))
+                elif self._kw_device:
+                    kw_calls.setdefault(kind, []).append(i)
                 else:
-                    fused = bm25.ranked_fusion([(dense_w, [d for d, _ in dense]), (1.0 - dense_w, [d for d, _ in sparse])],
-                                               limit)
-                picked = [(rid, fs, cos.get(rid)) for rid, fs in fused]
-            return self._shape(picked)
+                    allowed_set, allowed_arr = self._tenant_scope(reqs[i].user, reqs[i].org) if kind == "codes" else (None, None)
+                    sparse[i] = self.sparse.search(reqs[i].text, _MAX_FETCH, allowed=allowed_set, allowed_sorted=allowed_arr)
+            for kind, g in kw_calls.items():
+                sparse.update(zip(g, self.sparse.search_batch([reqs[i].text for i in g], _MAX_FETCH,
+                                                              **self._scope_args(kind, [scope[i][1] for i in g]))))
+
+            # objects deleted since a leg's search (the keyword store's own call may delete) drop out of the answer
+            for i in live:
+                r = reqs[i]
+                if i in fused:              # the device's scores: the answer as of the search
+                    out[i] = self._shape([(d, fs, cos) for d, (fs, cos) in fused[i] if d in self._props][:r.limit])
+                    continue
+                d_leg = [(d, s) for d, s in dense.get(i, []) if d in self._props]
+                if not r.hybrid:
+                    out[i] = self._shape([(d, s, s) for d, s in d_leg[:r.limit]])
+                    continue
+                s_leg = [(d, s) for d, s in sparse[i] if d in self._props]
+                if r.fusion == HybridFusion.RELATIVE_SCORE:
+                    picked = bm25.relative_score_fusion([(r.dense_w, d_leg), (1.0 - r.dense_w, s_leg)], r.limit)
+                else:
+                    picked = bm25.ranked_fusion([(r.dense_w, [d for d, _ in d_leg]),
+                                                 (1.0 - r.dense_w, [d for d, _ in s_leg])], r.limit)
+                cos = dict(d_leg)
+                out[i] = self._shape([(d, fs, cos.get(d)) for d, fs in picked])
+        return out
+
+    def _resolve_scope(self, r: _Request):
+        """The rows ``r`` may see, as ``(kind, value)``: ``("all", None)``, ``("codes", (user code, org code))``,
+        ``("program", device program)`` or ``("ids", allowed id list)`` (a filter resolved on the host).  Caller holds
+        the lock."""
+        tenant = r.scoped or r.user is not None or r.org is not None
+        if r.filters is None:
+            return ("codes", self._scope_codes(r.user, r.org)) if tenant else ("all", None)
+        prog = self._device_program(r.filters, tenant, r.user, r.org)
+        if prog is not None:
+            return "program", prog
+        # narrow the scan with the filter's own equality terms and the tenant scope, then run the predicate
+        eq = r.filters.required_equalities()
+        pools = []
+        if "org_id" in eq:
+            pools.append(self._by_org.get(eq["org_id"], set()))
+        if "user_id" in eq:
+            pools.append(self._by_user.get(eq["user_id"], set()))
+        if tenant:
+            pools.append(self._by_user.get(r.user, set()) | (self._by_org.get(r.org, set()) if r.org else set()))
+        cand = set.intersection(*pools) if pools else self._props.keys()
+
+        def tenant_ok(props) -> bool:
+            return not tenant or (bool(r.user) and props.get("user_id") == r.user) or \
+                (bool(r.org) and props.get("org_id") == r.org)
+        return "ids", [rid for rid in cand if r.filters.matches(self._props[rid]) and tenant_ok(self._props[rid])]
+
+    def _scope_args(self, kind: str, vals: list) -> Dict[str, Any]:
+        """The scopes of one batch of a kind as the index's and the keyword store's searches take them.  Caller holds
+        the lock."""
+        if kind == "codes":
+            return {"q_user": np.array([v[0] for v in vals], np.int32), "q_org": np.array([v[1] for v in vals], np.int32)}
+        if kind == "program":               # q_program None: every query on program 0
+            return {"programs": vals, "q_program": np.arange(len(vals), dtype=np.int32) if len(vals) > 1 else None,
+                    "max_list_rows": int(_LIST_MAX_FRACTION * len(self._props))}
+        return {}
 
     def _shape(self, picked) -> List[SimpleNamespace]:
         """(id, score, dense cosine or None) -> result objects.  Caller holds the lock."""
@@ -525,81 +582,6 @@ class KnowledgeBase:
         for rid, score, cosine in picked:
             meta = SimpleNamespace(score=float(score), distance=None if cosine is None else 1.0 - float(cosine))
             out.append(SimpleNamespace(properties=dict(self._props[rid]), uuid=self._id2key.get(rid), metadata=meta))
-        return out
-
-    def query_batch(self, reqs: List[Tuple[Optional[str], str, int, Optional[float], Optional[str]]]) -> List[List[SimpleNamespace]]:
-        """Several tenant-scoped searches at once: ``(user_id, query, limit, alpha, org_id)`` each.  All query texts go
-        through ONE encoder batch; the dense leg is ONE kernel launch per result size (the tenant scopes of the batch ride
-        along as per-row bit masks on the tensor-core kernel); on a GPU keyword store the keyword leg of every hybrid request
-        (alpha < 1) is ONE device search with per-request tenant codes; fusion / shaping per request as in ``query``.
-        On a CUDA shard whose hybrid requests carry at most 32 distinct tenant scopes, those requests are instead ONE device
-        call for both legs and their ranked fusion (``DeviceBM25.search_batch`` with ``dense``, per-request weights), and
-        only shaping is left per request."""
-        need = [i for i, (u, q, lim, a, o) in enumerate(reqs) if lim > 0 and (u or o) and (a is None or a > 0.0)]
-        hyb = [i for i, (u, q, lim, a, o) in enumerate(reqs) if lim > 0 and (u or o) and a is not None and a < 1.0]
-        vecs = self.encoder.encode([reqs[i][1] for i in need]) if need else None
-        dense: Dict[int, List[Tuple[int, float]]] = {}
-        sparse: Dict[int, List[Tuple[int, float]]] = {}
-        fused: Dict[int, list] = {}
-        with self._lock:
-            if hyb and self._hybrid_device:
-                codes = [self._scope_codes(reqs[i][0], reqs[i][4]) for i in hyb]
-                if len(set(codes)) <= 32:   # the tensor-core kernel's per-row scope masks hold them
-                    row = {i: pos for pos, i in enumerate(need)}
-                    hv = np.zeros((len(hyb), self.dim), vecs.dtype if vecs is not None else np.float32)
-                    for j, i in enumerate(hyb):
-                        if i in row:        # alpha <= 0: the dense leg is ignored, its vector stays zero
-                            hv[j] = vecs[row[i]]
-                    lists = self.sparse.search_batch(
-                        [reqs[i][1] for i in hyb], _MAX_FETCH, np.array([c[0] for c in codes], np.int32),
-                        np.array([c[1] for c in codes], np.int32),
-                        dense=(self.index, hv, np.array([max(0.0, float(reqs[i][3])) for i in hyb]), FUSION_RANKED,
-                               min(max(reqs[i][2] for i in hyb), 2 * _MAX_FETCH)))
-                    fused = dict(zip(hyb, lists))
-            kw_need = [i for i in hyb if i not in fused] if self._kw_device else []
-            if kw_need:
-                codes = [self._scope_codes(reqs[i][0], reqs[i][4]) for i in kw_need]
-                lists = self.sparse.search_batch([reqs[i][1] for i in kw_need], _MAX_FETCH,
-                                                 np.array([c[0] for c in codes], np.int32),
-                                                 np.array([c[1] for c in codes], np.int32))
-                sparse = dict(zip(kw_need, lists))
-            groups: Dict[int, List[Tuple[int, int, int]]] = {}      # fetch size -> [(position, user code, org code)]
-            for pos, i in enumerate(need):
-                if i in fused:
-                    continue
-                u, _, lim, a, o = reqs[i]
-                hybrid = a is not None and a < 1.0
-                fetch = max(1, min(_MAX_FETCH, lim if not hybrid else _MAX_FETCH))
-                cu = self._code(self._user_code, u, False) if u else -2
-                co = self._code(self._org_code, o, False) if o else -1
-                groups.setdefault(fetch, []).append((pos, cu, -1 if co == -2 else co))
-            for fetch, members in groups.items():
-                pos = [m[0] for m in members]
-                scopes: Dict[Tuple[int, int], int] = {}
-                for m in members:
-                    scopes.setdefault((m[1], m[2]), len(scopes))
-                if len(scopes) > 32 and hasattr(self.index, "search_lists"):
-                    # more scopes than the tensor-core kernel's row bit masks hold: one id list per scope (the rows
-                    # _tenant_scope gives the keyword leg) and one list search that reads only those rows
-                    lists: List[np.ndarray] = [np.empty(0, np.int64)] * len(scopes)
-                    for m in members:
-                        slot = scopes[(m[1], m[2])]
-                        if not len(lists[slot]):
-                            u, o = reqs[need[m[0]]][0], reqs[need[m[0]]][4]
-                            lists[slot] = self._tenant_scope(u, o)[1]
-                    ids, scores = self.index.search_lists(vecs[pos], fetch, lists,
-                                                          np.array([scopes[(m[1], m[2])] for m in members], np.int32))
-                else:
-                    # one launch for the whole group: up to 32 distinct tenant scopes per batch ride on the tensor-core
-                    # kernel as per-row bit masks (csrc/capi.cu search_host); the library falls back by itself beyond
-                    ids, scores = self.index.search(vecs[pos], fetch, np.array([m[1] for m in members], np.int32),
-                                                    np.array([m[2] for m in members], np.int32))
-                for row, p_ in enumerate(pos):
-                    dense[need[p_]] = [(int(r), float(s_)) for r, s_ in zip(ids[row], scores[row]) if r >= 0]
-        out = []
-        for i, (u, q, lim, a, o) in enumerate(reqs):
-            out.append(self.query(q, lim, user_id=u, org_id=o, alpha=a, scoped=True, _dense=dense.get(i),
-                                  _sparse=sparse.get(i), _fused=fused.get(i)))
         return out
 
     # ------------------------------------------------------------------ persistence
@@ -807,21 +789,8 @@ def search_knowledge_base(user_id: str, query: str, limit: int = 5, alpha: float
     if not query.strip():
         return []
     try:
-        objs = _get_kb().query(query, limit, user_id=user_id, org_id=org_id, alpha=alpha, scoped=True)
-        results = []
-        for obj in objs:
-            score = obj.metadata.score if obj.metadata else 0.0
-            if min_score > 0.0 and score < min_score:
-                continue
-            p = obj.properties
-            results.append({
-                "content": p.get("content", ""),
-                "heading_context": p.get("heading_context", ""),
-                "source_filename": p.get("source_filename", ""),
-                "document_id": p.get("document_id", ""),
-                "chunk_index": p.get("chunk_index", 0),
-                "score": score,
-            })
+        results = _shape_results(_get_kb().query(query, limit, user_id=user_id, org_id=org_id, alpha=alpha, scoped=True),
+                                 min_score)
         logger.info(f"[KB B200] Search for '{_sanitize(query)[:50]}...' returned {len(results)} results")
         return results
     except Exception as e:
