@@ -171,8 +171,7 @@ struct aur_index {
   int64_t* d_ids = nullptr;
   int32_t* d_user = nullptr;
   int32_t* d_org = nullptr;
-  int32_t* d_attr[kFiltAttrCols] = {};   // attribute columns (program columns 2..), allocated on first aur_set_attrs; guarded by mu
-  DevBuf<int32_t> attr_stage;            // aur_set_attrs: (row, code) pairs (writers hold mu_write)
+  AttrColumns attrs;                     // program columns 2.., cap_pad rows each (aur_set_attrs, writers hold mu_write)
   std::unordered_map<int64_t, int64_t> id2row;
   cudaStream_t stream = nullptr;         // the index's own stream: device-pointer calls with stream == NULL
   cudaStream_t ingest_stream = nullptr;  // host appends / tombstones, lowest priority so queries overtake them
@@ -859,48 +858,14 @@ int run_list_search(aur_index* ix, SearchCtx* c, cudaStream_t s, const ListPlan&
   return AUR_OK;
 }
 
-// Filter programs (aur_search_filtered, aur_filter_ids): n_programs programs, program q = tokens
-// prog[4 * prog_off[q] .. 4 * prog_off[q + 1]), each token {kind, column, bitmap offset, bitmap length}.
-int check_programs(aur_index* ix, const int32_t* prog, const int32_t* prog_off, int32_t n_programs, const uint32_t* bitmap,
-                   int64_t bitmap_words) {
-  if (!prog || !prog_off) return fail(AUR_ERR_INVALID, "null program");
-  if (n_programs < 1 || n_programs > kFiltCallPrograms) return fail(AUR_ERR_INVALID, "1 <= n_programs <= %d", kFiltCallPrograms);
-  if (bitmap_words < 0 || (bitmap_words > 0 && !bitmap)) return fail(AUR_ERR_INVALID, "bitmap / bitmap_words");
-  if (prog_off[0] != 0) return fail(AUR_ERR_INVALID, "program offsets must start at 0");
-  std::lock_guard<std::mutex> lk(ix->mu);   // the attribute columns that exist
-  for (int32_t q = 0; q < n_programs; ++q) {
-    if (prog_off[q + 1] < prog_off[q]) return fail(AUR_ERR_INVALID, "program offsets decrease at program %d", q);
-    int depth = 0, leaves = 0;
-    for (int32_t t = prog_off[q]; t < prog_off[q + 1]; ++t) {
-      const int32_t* tk = prog + 4 * static_cast<int64_t>(t);
-      if (tk[0] == kFiltLeaf) {
-        if (++leaves > kFiltMaxLeaves) return fail(AUR_ERR_INVALID, "program %d has more than %d leaves", q, kFiltMaxLeaves);
-        if (tk[1] < 0 || tk[1] >= kFiltCols) return fail(AUR_ERR_INVALID, "program %d: column %d out of range", q, tk[1]);
-        if (tk[1] >= 2 && !ix->d_attr[tk[1] - 2]) return fail(AUR_ERR_INVALID, "program %d: column %d was never set", q, tk[1]);
-        if (tk[2] < 0 || tk[3] < 0 || static_cast<int64_t>(tk[2]) + tk[3] > bitmap_words * 32)
-          return fail(AUR_ERR_INVALID, "program %d: bitmap slice [%d, +%d) outside the bitmap", q, tk[2], tk[3]);
-        ++depth;
-      } else if (tk[0] == kFiltAnd || tk[0] == kFiltOr) {
-        if (depth < 2) return fail(AUR_ERR_INVALID, "program %d: operator without two operands", q);
-        --depth;
-      } else {
-        return fail(AUR_ERR_INVALID, "program %d: unknown token kind %d", q, tk[0]);
-      }
-    }
-    if (depth != 1) return fail(AUR_ERR_INVALID, "program %d leaves %d values, not one", q, depth);
-  }
-  return AUR_OK;
-}
-
 // Where pass `ps` of a filter evaluation (programs 32 ps .. 32 ps + 31) keeps its data: c->filt_mask holds one mask per
 // pass, c->filt_counts every pass's 32 totals and then every pass's block counts.
 struct FiltPass { uint32_t* mask; uint32_t* totals; uint32_t* counts; int n_programs; };
 FiltPass filt_pass(SearchCtx* c, int ps, int n_programs, int64_t n_rows) {
-  const int n_passes = (n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms;
   const size_t rows = static_cast<size_t>(std::max<int64_t>(n_rows, 1)), nb = static_cast<size_t>(std::max(filter_blocks(n_rows), 1));
   return FiltPass{c->filt_mask.p + ps * rows, c->filt_counts.p + ps * kFiltMaxPrograms,
-                  c->filt_counts.p + static_cast<size_t>(n_passes) * kFiltMaxPrograms + ps * kFiltMaxPrograms * nb,
-                  std::min(kFiltMaxPrograms, n_programs - ps * kFiltMaxPrograms)};
+                  c->filt_counts.p + static_cast<size_t>(filter_passes(n_programs)) * kFiltMaxPrograms + ps * kFiltMaxPrograms * nb,
+                  filter_pass_programs(n_programs, ps)};
 }
 
 // Uploads checked programs, evaluates them over the snapshot's rows [0, n_rows) in passes of up to 32 programs (masks
@@ -908,35 +873,17 @@ FiltPass filt_pass(SearchCtx* c, int ps, int n_programs, int64_t n_rows) {
 // matching rows into c->h_totals (one small copy for all passes).  Nothing waits: filter_totals reads them once the
 // stream is idle.
 int filter_count(aur_index* ix, SearchCtx* c, cudaStream_t s, const FiltProgs& fp, int64_t n_rows) {
-  const int32_t n_programs = fp.n_programs;
-  const size_t n_tok = static_cast<size_t>(fp.prog_off[n_programs]);
-  std::vector<int32_t> st(n_tok * 4 + static_cast<size_t>(n_programs) + 1 + static_cast<size_t>(fp.bitmap_words));
-  if (n_tok) memcpy(st.data(), fp.prog, n_tok * 16);
-  memcpy(st.data() + n_tok * 4, fp.prog_off, (static_cast<size_t>(n_programs) + 1) * 4);
-  if (fp.bitmap_words) memcpy(st.data() + n_tok * 4 + n_programs + 1, fp.bitmap, static_cast<size_t>(fp.bitmap_words) * 4);
-  const int n_passes = (n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms;
+  const int n_passes = filter_passes(fp.n_programs);
   const size_t nb = static_cast<size_t>(std::max(filter_blocks(n_rows), 1));
   if (!c->h_totals) CU_TRY(cudaHostAlloc(reinterpret_cast<void**>(&c->h_totals), kFiltCallPrograms * 4, cudaHostAllocPortable));
-  CU_TRY(c->filt_stage.reserve(st.size()));
   CU_TRY(c->filt_mask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
   CU_TRY(c->filt_counts.reserve(static_cast<size_t>(n_passes) * kFiltMaxPrograms * (1 + nb)));
-  CU_TRY(cudaMemcpyAsync(c->filt_stage.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice, s));   // pageable: staged on return
-  FiltParams p{};
-  p.cols[0] = ix->d_user; p.cols[1] = ix->d_org;
-  {
-    std::lock_guard<std::mutex> lk(ix->mu);
-    for (int i = 0; i < kFiltAttrCols; ++i) p.cols[2 + i] = ix->d_attr[i];
-  }
-  const int32_t* d_off = c->filt_stage.p + n_tok * 4;   // token indices stay absolute: a pass starts at its first offset
-  p.tok = reinterpret_cast<const FiltToken*>(c->filt_stage.p);
-  p.bitmap = reinterpret_cast<const uint32_t*>(d_off + n_programs + 1);
-  p.inv_norm = ix->d_inv_norm;
-  p.n_rows = n_rows;
+  FiltParams p;
+  CU_TRY(filter_upload(fp, ix->d_user, ix->d_org, ix->attrs, c->filt_stage, s, &p));
+  p.inv_norm = ix->d_inv_norm; p.n_rows = n_rows;
   for (int ps = 0; ps < n_passes; ++ps) {
-    const FiltPass pass = filt_pass(c, ps, n_programs, n_rows);
-    p.prog_off = d_off + ps * kFiltMaxPrograms;
-    p.n_programs = pass.n_programs;
-    CU_TRY(launch_filter_count(p, pass.mask, pass.counts, pass.totals, s));
+    const FiltPass pass = filt_pass(c, ps, fp.n_programs, n_rows);
+    CU_TRY(launch_filter_count(filter_pass(p, ps), pass.mask, pass.counts, pass.totals, s));
     ++c->last_launches;
   }
   CU_TRY(cudaMemcpyAsync(c->h_totals, c->filt_counts.p, static_cast<size_t>(n_passes) * kFiltMaxPrograms * 4,
@@ -960,7 +907,7 @@ int filter_write(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t n_programs
   CU_TRY(c->filt_rows.reserve(static_cast<size_t>(std::max<int64_t>(total, 1))));
   if (with_ids) CU_TRY(c->filt_ids.reserve(static_cast<size_t>(std::max<int64_t>(total, 1))));
   int64_t base = 0;
-  for (int ps = 0; ps * kFiltMaxPrograms < n_programs; ++ps) {
+  for (int ps = 0; ps < filter_passes(n_programs); ++ps) {
     const FiltPass fp = filt_pass(c, ps, n_programs, n_rows);
     CU_TRY(launch_filter_write(fp.mask, fp.counts, fp.totals, fp.n_programs, n_rows, with_ids ? ix->d_ids : nullptr,
                                c->filt_rows.p + base, with_ids ? c->filt_ids.p + base : nullptr, s));
@@ -1022,9 +969,7 @@ int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_hos
 int index_device(const aur_index* ix) { return ix->device; }
 int index_bf16_queries(const aur_index* ix) { return ix->dtype == AUR_BF16 || ix->dtype == AUR_I8; }
 
-int filter_check(aur_index* ix, const FiltProgs& fp) {
-  return check_programs(ix, fp.prog, fp.prog_off, fp.n_programs, fp.bitmap, fp.bitmap_words);
-}
+AttrColumns& index_attrs(aur_index* ix) { return ix->attrs; }
 
 int filtered_legs(aur_index* const* shards, int n, const void* queries_host, int32_t nq, int32_t k, const FiltProgs& fp,
                   int64_t max_list_rows, const DenseLegsThen& then, float* scores_host, int64_t* ids_host) {
@@ -1141,8 +1086,7 @@ int aur_close(aur_index* ix) {
   cudaSetDevice(ix->device);
   cudaDeviceSynchronize();   // searches bound to caller streams may still be in flight
   cudaFree(ix->d_rows); cudaFree(ix->d_inv_norm); cudaFree(ix->d_ids); cudaFree(ix->d_user); cudaFree(ix->d_org);
-  for (int32_t* a : ix->d_attr) cudaFree(a);
-  ix->attr_stage.release();
+  ix->attrs.release();
   ix->i8_stage.release();
   for (auto& c : ix->ctxs) c->release();
   if (ix->stream) cudaStreamDestroy(ix->stream);
@@ -1241,18 +1185,13 @@ int aur_compact(aur_index* ix, int64_t* reclaimed) {
   // overwrites rows < i1 <= old(i1), i.e. rows whose content has already been gathered or moved.
   const int64_t chunk = 65536;
   DevBuf<int32_t> d_map; DevBuf<uint8_t> bounce; DevBuf<float> b_inv; DevBuf<int64_t> b_ids; DevBuf<int32_t> b_user, b_org, b_attr;
-  std::vector<int32_t*> attrs;
-  {
-    std::lock_guard<std::mutex> lk(ix->mu);
-    for (int32_t* a : ix->d_attr) if (a) attrs.push_back(a);
-  }
   cudaError_t e = d_map.reserve(static_cast<size_t>(chunk));
   if (e == cudaSuccess) e = bounce.reserve(static_cast<size_t>(chunk) * ix->dim * ix->elt);
   if (e == cudaSuccess) e = b_inv.reserve(chunk);
   if (e == cudaSuccess) e = b_ids.reserve(chunk);
   if (e == cudaSuccess) e = b_user.reserve(chunk);
   if (e == cudaSuccess) e = b_org.reserve(chunk);
-  if (e == cudaSuccess && !attrs.empty()) e = b_attr.reserve(chunk);
+  if (e == cudaSuccess && ix->attrs.any()) e = b_attr.reserve(chunk);
   auto drop = [&]() { d_map.release(); bounce.release(); b_inv.release(); b_ids.release(); b_user.release(); b_org.release(); b_attr.release(); };
   if (e != cudaSuccess) { drop(); return fail(AUR_ERR_NOMEM, "aur_compact: %s", cudaGetErrorString(e)); }
   cudaStream_t s = ix->ingest_stream;
@@ -1271,15 +1210,11 @@ int aur_compact(aur_index* ix, int64_t* reclaimed) {
     if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_ids + i0, b_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_user + i0, b_user.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_org + i0, b_org.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
-    for (int32_t* a : attrs) {
-      if (e == cudaSuccess) e = launch_gather_i32(a, d_map.p, m, b_attr.p, s);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(a + i0, b_attr.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
-    }
+    if (e == cudaSuccess) e = ix->attrs.gather(d_map.p, m, i0, b_attr.p, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);   // map_host is reused by the next chunk
   }
   // the freed rows are appended to again: their attributes start absent, as in a fresh column
-  for (int32_t* a : attrs)
-    if (e == cudaSuccess) e = cudaMemsetAsync(a + nlive, 0xFF, static_cast<size_t>(rows - nlive) * 4, s);
+  if (e == cudaSuccess) e = ix->attrs.clear(nlive, rows, s);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   drop();
   if (e != cudaSuccess) return fail(AUR_ERR_CUDA, "aur_compact: %s (the shard may be inconsistent: restore the last snapshot)", cudaGetErrorString(e));
@@ -1468,34 +1403,13 @@ int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_
 
 int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t* codes, int64_t n) {
   if (!ix || n < 0 || (n > 0 && (!ids || !codes))) return fail(AUR_ERR_INVALID, "null argument");
-  if (col < 2 || col >= kFiltCols) return fail(AUR_ERR_INVALID, "attribute columns are 2 .. %d", kFiltCols - 1);
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   std::lock_guard<std::mutex> wk(ix->mu_write);
   CU_TRY(cudaSetDevice(ix->device));
-  cudaStream_t s = ix->ingest_stream;
-  int32_t* a = nullptr;
-  {
-    std::lock_guard<std::mutex> lk(ix->mu);
-    a = ix->d_attr[col - 2];
-  }
-  if (!a) {   // first use: every row absent (-1), at the padded capacity like the tenant codes
-    cudaError_t e = cudaMalloc(&a, static_cast<size_t>(ix->cap_pad) * 4);
-    if (e != cudaSuccess) return fail(AUR_ERR_NOMEM, "attribute column: %s", cudaGetErrorString(e));
-    e = cudaMemsetAsync(a, 0xFF, static_cast<size_t>(ix->cap_pad) * 4, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { cudaFree(a); return fail(AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e)); }
-    std::lock_guard<std::mutex> lk(ix->mu);
-    ix->d_attr[col - 2] = a;
-  }
   std::vector<int32_t> pairs;
   pairs.reserve(2 * static_cast<size_t>(n));
   resolve_ids(ix, ids, n, INT64_MAX, [&](int64_t i, int32_t row) { pairs.push_back(row); pairs.push_back(codes[i]); });
-  if (pairs.empty()) return AUR_OK;
-  CU_TRY(ix->attr_stage.reserve(pairs.size()));
-  CU_TRY(cudaMemcpyAsync(ix->attr_stage.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s));
-  CU_TRY(launch_scatter_codes(ix->attr_stage.p, static_cast<int64_t>(pairs.size() / 2), a, s));
-  CU_TRY(cudaStreamSynchronize(s));
-  return AUR_OK;
+  return ix->attrs.write(col, pairs, ix->cap_pad, ix->ingest_stream);   // padded, like the tenant codes
 }
 
 int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* prog,
@@ -1504,12 +1418,10 @@ int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int
                         int64_t* matched_out, int64_t* snapshot_rows_out) {
   int rc = check_list_args(ix, queries_host, nq, k, scores_out, ids_out);
   if (rc != AUR_OK) return rc;
-  if ((rc = check_programs(ix, prog, prog_offsets, n_programs, bitmap, bitmap_words)) != AUR_OK) return rc;
-  if (!q_program) return fail(AUR_ERR_INVALID, "q_program is required");
-  for (int32_t q = 0; q < nq; ++q)
-    if (q_program[q] < 0 || q_program[q] >= n_programs) return fail(AUR_ERR_INVALID, "q_program[%d] = %d is not a program", q, q_program[q]);
-  if (max_list_rows < 0) return fail(AUR_ERR_INVALID, "max_list_rows < 0");
   const FiltProgs fp{prog, prog_offsets, n_programs, bitmap, bitmap_words, q_program};
+  if ((rc = filter_check_programs(fp)) != AUR_OK || (rc = ix->attrs.check(fp, "shard")) != AUR_OK ||
+      (rc = filter_check_queries(fp, nq, max_list_rows)) != AUR_OK)
+    return rc;
   return filtered_legs(&ix, 1, queries_host, nq, k, fp, max_list_rows, [&](const std::vector<DenseLeg>& legs) -> int {
     const DenseLeg& l = legs[0];
     const size_t nout = static_cast<size_t>(nq) * k;
@@ -1530,14 +1442,15 @@ int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const u
   if (!ix || !n_out || cap < 0 || (cap > 0 && !ids_out)) return fail(AUR_ERR_INVALID, "null argument");
   if (n_tokens < 0) return fail(AUR_ERR_INVALID, "n_tokens < 0");
   const int32_t off[2] = {0, n_tokens};
-  int rc = check_programs(ix, prog, off, 1, bitmap, bitmap_words);
-  if (rc != AUR_OK) return rc;
+  const FiltProgs fp{prog, off, 1, bitmap, bitmap_words, nullptr};
+  int rc = filter_check_programs(fp);
+  if (rc != AUR_OK || (rc = ix->attrs.check(fp, "shard")) != AUR_OK) return rc;
   HostCall call(ix);
   if ((rc = call.open()) != AUR_OK) return rc;
   SearchCtx* c = call.c;
   cudaStream_t s = call.s;
   std::vector<int64_t> tot;
-  if ((rc = filter_count(ix, c, s, FiltProgs{prog, off, 1, bitmap, bitmap_words, nullptr}, call.n_rows)) != AUR_OK) return rc;
+  if ((rc = filter_count(ix, c, s, fp, call.n_rows)) != AUR_OK) return rc;
   CU_TRY(cudaStreamSynchronize(s));
   filter_totals(c, 1, &tot);
   const int64_t n = tot[0], m = std::min(n, cap);

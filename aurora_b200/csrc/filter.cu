@@ -11,7 +11,12 @@
 //   filter_write_kernel  each program's matching rows in ascending row order (and optionally their ids) into one buffer:
 //                        the rows the host path stages after its sort and unique.
 // mask_match_kernel turns bit 0 of the mask into the masked inverse norms the tensor-core scan takes.
+// The host side is here too, one copy for the vector shard and the keyword store: program checks, attribute columns
+// (AttrColumns) and program uploads (filter_upload), so the two legs of a filtered hybrid query cannot disagree.
 #include <math.h>
+#include <string.h>
+
+#include "../../include/aurora_b200.h"
 #include "internal.h"
 
 namespace aur {
@@ -221,16 +226,127 @@ cudaError_t launch_mask_match(const float* inv, const uint32_t* mask, int64_t n,
   return cudaGetLastError();
 }
 
-cudaError_t launch_scatter_codes(const int32_t* pairs, int64_t n, int32_t* col, cudaStream_t s) {
-  if (n <= 0) return cudaSuccess;
-  scatter_codes_kernel<<<blocks_of(n, 256), 256, 0, s>>>(pairs, n, col);
-  return cudaGetLastError();
+// ---------------------------------------------------------------- host side: programs, attribute columns, uploads
+int filter_check_programs(const FiltProgs& fp) {
+  if (!fp.prog || !fp.prog_off) return report_error(AUR_ERR_INVALID, "null program");
+  if (fp.n_programs < 1 || fp.n_programs > kFiltCallPrograms) return report_error(AUR_ERR_INVALID, "1 <= n_programs <= %d", kFiltCallPrograms);
+  if (fp.bitmap_words < 0 || (fp.bitmap_words > 0 && !fp.bitmap)) return report_error(AUR_ERR_INVALID, "bitmap / bitmap_words");
+  if (fp.prog_off[0] != 0) return report_error(AUR_ERR_INVALID, "program offsets must start at 0");
+  for (int32_t q = 0; q < fp.n_programs; ++q) {
+    if (fp.prog_off[q + 1] < fp.prog_off[q]) return report_error(AUR_ERR_INVALID, "program offsets decrease at program %d", q);
+    int depth = 0, leaves = 0;
+    for (int32_t t = fp.prog_off[q]; t < fp.prog_off[q + 1]; ++t) {
+      const int32_t* tk = fp.prog + 4 * static_cast<int64_t>(t);
+      if (tk[0] == kFiltLeaf) {
+        if (++leaves > kFiltMaxLeaves) return report_error(AUR_ERR_INVALID, "program %d has more than %d leaves", q, kFiltMaxLeaves);
+        if (tk[1] < 0 || tk[1] >= kFiltCols) return report_error(AUR_ERR_INVALID, "program %d: column %d out of range", q, tk[1]);
+        if (tk[2] < 0 || tk[3] < 0 || static_cast<int64_t>(tk[2]) + tk[3] > fp.bitmap_words * 32)
+          return report_error(AUR_ERR_INVALID, "program %d: bitmap slice [%d, +%d) outside the bitmap", q, tk[2], tk[3]);
+        ++depth;
+      } else if (tk[0] == kFiltAnd || tk[0] == kFiltOr) {
+        if (depth < 2) return report_error(AUR_ERR_INVALID, "program %d: operator without two operands", q);
+        --depth;
+      } else {
+        return report_error(AUR_ERR_INVALID, "program %d: unknown token kind %d", q, tk[0]);
+      }
+    }
+    if (depth != 1) return report_error(AUR_ERR_INVALID, "program %d leaves %d values, not one", q, depth);
+  }
+  return AUR_OK;
 }
 
-cudaError_t launch_gather_i32(const int32_t* src, const int32_t* map, int64_t n, int32_t* out, cudaStream_t s) {
-  if (n <= 0) return cudaSuccess;
-  gather_i32_kernel<<<blocks_of(n, 256), 256, 0, s>>>(src, map, n, out);
-  return cudaGetLastError();
+int filter_check_queries(const FiltProgs& fp, int32_t nq, int64_t max_list_rows) {
+  if (!fp.q_program) return report_error(AUR_ERR_INVALID, "q_program is required");
+  for (int32_t q = 0; q < nq; ++q)
+    if (fp.q_program[q] < 0 || fp.q_program[q] >= fp.n_programs)
+      return report_error(AUR_ERR_INVALID, "q_program[%d] = %d is not a program", q, fp.q_program[q]);
+  if (max_list_rows < 0) return report_error(AUR_ERR_INVALID, "max_list_rows < 0");
+  return AUR_OK;
+}
+
+int AttrColumns::write(int32_t col, const std::vector<int32_t>& pairs, int64_t rows, cudaStream_t s) {
+  if (col < 2 || col >= kFiltCols) return report_error(AUR_ERR_INVALID, "attribute columns are 2 .. %d", kFiltCols - 1);
+  auto fail = [](cudaError_t e) { return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e)); };
+  int32_t* a = d_attr[col - 2];   // (writes are serialised: only this call stores a pointer)
+  if (!a) {
+    cudaError_t e = cudaMalloc(&a, static_cast<size_t>(rows) * 4);
+    if (e != cudaSuccess) return fail(e);
+    e = cudaMemsetAsync(a, 0xFF, static_cast<size_t>(rows) * 4, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) { cudaFree(a); return fail(e); }
+    std::lock_guard<std::mutex> lk(mu);
+    d_attr[col - 2] = a;
+  }
+  if (pairs.empty()) return AUR_OK;
+  cudaError_t e = stage.reserve(pairs.size());
+  if (e == cudaSuccess) e = cudaMemcpyAsync(stage.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) {
+    const int64_t n = static_cast<int64_t>(pairs.size() / 2);
+    scatter_codes_kernel<<<blocks_of(n, 256), 256, 0, s>>>(stage.p, n, a);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  return e == cudaSuccess ? AUR_OK : fail(e);
+}
+
+bool AttrColumns::any() { return std::any_of(std::begin(d_attr), std::end(d_attr), [](const int32_t* a) { return a != nullptr; }); }
+
+cudaError_t AttrColumns::gather(const int32_t* map, int64_t m, int64_t dst0, int32_t* bounce, cudaStream_t s) {
+  cudaError_t e = cudaSuccess;
+  for (int32_t* a : d_attr) {
+    if (!a || m <= 0 || e != cudaSuccess) continue;
+    gather_i32_kernel<<<blocks_of(m, 256), 256, 0, s>>>(a, map, m, bounce);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(a + dst0, bounce, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
+  }
+  return e;
+}
+
+cudaError_t AttrColumns::clear(int64_t r0, int64_t r1, cudaStream_t s) {
+  cudaError_t e = cudaSuccess;
+  for (int32_t* a : d_attr)
+    if (a && r1 > r0 && e == cudaSuccess) e = cudaMemsetAsync(a + r0, 0xFF, static_cast<size_t>(r1 - r0) * 4, s);
+  return e;
+}
+
+int AttrColumns::check(const FiltProgs& fp, const char* holder) {
+  std::lock_guard<std::mutex> lk(mu);
+  for (int32_t t = 0; t < fp.prog_off[fp.n_programs]; ++t) {
+    const int32_t* tk = fp.prog + 4 * static_cast<int64_t>(t);
+    if (tk[0] == kFiltLeaf && tk[1] >= 2 && !d_attr[tk[1] - 2])
+      return report_error(AUR_ERR_INVALID, "column %d was never set on the %s", tk[1], holder);
+  }
+  return AUR_OK;
+}
+
+void AttrColumns::fill(FiltParams* p) {
+  std::lock_guard<std::mutex> lk(mu);
+  for (int i = 0; i < kFiltAttrCols; ++i) p->cols[2 + i] = d_attr[i];
+}
+
+void AttrColumns::release() {
+  for (int32_t*& a : d_attr) { cudaFree(a); a = nullptr; }
+  stage.release();
+}
+
+cudaError_t filter_upload(const FiltProgs& fp, const int32_t* user, const int32_t* org, AttrColumns& attrs,
+                          DevBuf<int32_t>& stage, cudaStream_t s, FiltParams* p) {
+  const size_t n_tok = static_cast<size_t>(fp.prog_off[fp.n_programs]), n_off = static_cast<size_t>(fp.n_programs) + 1;
+  std::vector<int32_t> st(n_tok * 4 + n_off + static_cast<size_t>(fp.bitmap_words));
+  if (n_tok) memcpy(st.data(), fp.prog, n_tok * 16);
+  memcpy(st.data() + n_tok * 4, fp.prog_off, n_off * 4);
+  if (fp.bitmap_words) memcpy(st.data() + n_tok * 4 + n_off, fp.bitmap, static_cast<size_t>(fp.bitmap_words) * 4);
+  cudaError_t e = stage.reserve(st.size());
+  if (e == cudaSuccess) e = cudaMemcpyAsync(stage.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice, s);
+  if (e != cudaSuccess) return e;
+  *p = FiltParams{};
+  p->cols[0] = user; p->cols[1] = org;
+  attrs.fill(p);
+  p->tok = reinterpret_cast<const FiltToken*>(stage.p);
+  p->prog_off = stage.p + n_tok * 4;   // token indices stay absolute: a pass starts at its first offset
+  p->bitmap = reinterpret_cast<const uint32_t*>(p->prog_off + n_off);
+  p->n_programs = fp.n_programs;
+  return cudaSuccess;
 }
 
 }  // namespace aur

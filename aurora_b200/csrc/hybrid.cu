@@ -461,15 +461,11 @@ int hybrid_search(aur_index* const* shards, aur_kw* const* stores, int32_t n, co
                           index_device(shards[s]));
   }
   if (fp) {   // every shard and every store must hold every column the programs name
-    for (int s = 0; s < n; ++s) {
-      if ((rc = filter_check(shards[s], *fp)) != AUR_OK) return rc;
-      if ((rc = kw_check_columns(stores[s], *fp)) != AUR_OK) return rc;
-    }
-    if (!fp->q_program) return report_error(AUR_ERR_INVALID, "q_program is required");
-    for (int32_t q = 0; q < nq; ++q)
-      if (fp->q_program[q] < 0 || fp->q_program[q] >= fp->n_programs)
-        return report_error(AUR_ERR_INVALID, "q_program[%d] = %d is not a program", q, fp->q_program[q]);
-    if (max_list_rows < 0) return report_error(AUR_ERR_INVALID, "max_list_rows < 0");
+    if ((rc = filter_check_programs(*fp)) != AUR_OK) return rc;
+    for (int s = 0; s < n; ++s)
+      if ((rc = index_attrs(shards[s]).check(*fp, "shard")) != AUR_OK || (rc = kw_attrs(stores[s]).check(*fp, "keyword store")) != AUR_OK)
+        return rc;
+    if ((rc = filter_check_queries(*fp, nq, max_list_rows)) != AUR_OK) return rc;
   }
   std::vector<HybridCtx*> hs;
   std::vector<int64_t> rows(2 * static_cast<size_t>(n), 0);

@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <functional>
 #include <mutex>
 #include <vector>
@@ -228,6 +229,9 @@ struct FiltParams {
   int n_programs;
 };
 int filter_blocks(int64_t n_rows);
+// Passes of kFiltMaxPrograms programs a call of n_programs takes, and the programs of pass ps.
+inline int filter_passes(int32_t n_programs) { return (n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms; }
+inline int filter_pass_programs(int32_t n_programs, int ps) { return std::min(kFiltMaxPrograms, n_programs - ps * kFiltMaxPrograms); }
 // mask [n_rows] (bit q = program q), block_counts [n_programs][filter_blocks(n_rows)], totals [32] (zeroed here)
 cudaError_t launch_filter_count(const FiltParams& p, uint32_t* mask, uint32_t* block_counts, uint32_t* totals, cudaStream_t s);
 // The same pass over a keyword store's rows (liveness from p.live): mask [n_rows] only, no counts, nothing read back.
@@ -238,16 +242,16 @@ struct FiltProgs {
   const uint32_t* bitmap; int64_t bitmap_words;
   const int32_t* q_program;
 };
+// fp's structure (n_programs, offsets, tokens, depth, leaves, column range, bitmap slices), then a call's q_program
+// [nq] and max_list_rows.  Whether the columns are set is AttrColumns::check, per holder.
+int filter_check_programs(const FiltProgs& fp);
+int filter_check_queries(const FiltProgs& fp, int32_t nq, int64_t max_list_rows);
 // rows_out [sum of totals]: program q's matching rows, ascending, after those of programs < q; ids_out (nullable) their ids.
 // Scans block_counts in place.
 cudaError_t launch_filter_write(const uint32_t* mask, uint32_t* block_counts, const uint32_t* totals, int n_programs, int64_t n_rows,
                                 const int64_t* ids, int32_t* rows_out, int64_t* ids_out, cudaStream_t s);
 // out[i] = (mask[i] & 1) ? inv[i] : NaN
 cudaError_t launch_mask_match(const float* inv, const uint32_t* mask, int64_t n, float* out, cudaStream_t s);
-// col[pairs[2i]] = pairs[2i + 1]
-cudaError_t launch_scatter_codes(const int32_t* pairs, int64_t n, int32_t* col, cudaStream_t s);
-// out[i] = src[map[i]] (compaction of an attribute column)
-cudaError_t launch_gather_i32(const int32_t* src, const int32_t* map, int64_t n, int32_t* out, cudaStream_t s);
 
 // out[rows[i]] = inv[rows[i]] for the listed rows (out pre-filled with NaN): a resolved id subset as a row mask
 cudaError_t launch_scatter_inv_norm(const float* inv, const int32_t* rows, int64_t n, int64_t n_rows, float* out, cudaStream_t s);
@@ -327,6 +331,31 @@ struct DevBuf {   // grow-only device scratch
   void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
 };
 
+// ---------------------------------------------------------------- filter columns and uploads, host side (filter.cu)
+// The attribute columns of a vector shard or a keyword store (program columns 2..): `rows` int32 codes each, -1 =
+// absent.  The pointers only go from null to allocated until release().  write, any, gather and clear are the holder's
+// writes, serialised by its writers' lock; mu guards the pointers write stores against check and fill.
+class AttrColumns {
+ public:
+  // pairs (row, code) into column col (2 .. kFiltCols - 1), waited for; the first write allocates it, all -1.
+  int write(int32_t col, const std::vector<int32_t>& pairs, int64_t rows, cudaStream_t s);
+  bool any();
+  // Compaction, every set column: rows map[0 .. m) to rows [dst0, dst0 + m) through bounce [m]; rows [r0, r1) to -1.
+  cudaError_t gather(const int32_t* map, int64_t m, int64_t dst0, int32_t* bounce, cudaStream_t s);
+  cudaError_t clear(int64_t r0, int64_t r1, cudaStream_t s);
+  int check(const FiltProgs& fp, const char* holder);   // every column fp (structure checked) names is set
+  void fill(FiltParams* p);                             // p->cols[2 ..]
+  void release();
+ private:
+  std::mutex mu;
+  int32_t* d_attr[kFiltAttrCols] = {};
+  DevBuf<int32_t> stage;
+};
+// Checked programs into stage on s in one upload (pageable: staged on return), and *p reading them over the holder's
+// tenant codes and attribute columns.  *p spans every program: launch filter_pass(*p, ps), liveness and n_rows set.
+cudaError_t filter_upload(const FiltProgs& fp, const int32_t* user, const int32_t* org, AttrColumns& attrs,
+                          DevBuf<int32_t>& stage, cudaStream_t s, FiltParams* p);
+inline FiltParams filter_pass(FiltParams p, int ps) { p.n_programs = filter_pass_programs(p.n_programs, ps); p.prog_off += ps * kFiltMaxPrograms; return p; }
 // ---------------------------------------------------------------- the two legs of a hybrid query (hybrid.cu)
 // Dense leg: the search aur_search_ex runs for these host queries and per-query tenant codes (same scope handling, same
 // kernels, same answer), enqueued on stream s of `device` over the prefix published now, into the device arrays
@@ -351,11 +380,10 @@ using DenseLegsThen = std::function<int(const std::vector<DenseLeg>& legs)>;
 int filtered_legs(aur_index* const* shards, int n, const void* queries_host, int32_t nq, int32_t k, const FiltProgs& fp,
                   int64_t max_list_rows, const DenseLegsThen& then, float* scores_host = nullptr,
                   int64_t* ids_host = nullptr);
-// aur_search_filtered's program checks against one shard: structure, 1 <= n_programs <= 1024, columns set on it.
-int filter_check(aur_index* ix, const FiltProgs& fp);
+AttrColumns& index_attrs(aur_index* ix);
 // Keyword legs: aur_kw_search_multi's search over stores[0 .. n) (distinct, non-NULL, 1 <= n <= 64) taken as one
-// corpus, each store's part enqueued on its own context and stream; fp (nullable; programs checked by filter_check and
-// kw_check_columns) restricts query q to the live rows program fp->q_program[q] matches on each store, evaluated there
+// corpus, each store's part enqueued on its own context and stream; fp (nullable; programs checked, their columns set on
+// every store) restricts query q to the live rows program fp->q_program[q] matches on each store, evaluated there
 // (no allow-list, no read-back).  then(legs) runs with every
 // store's (device, stream, top-k lists, snapshot) -- device arrays [nq * k], valid once the stream reaches them,
 // sorted by (fp64 score desc, id asc) -- while every store's shared lock and every context are held.  Each store's
@@ -365,8 +393,8 @@ using KwLegsThen = std::function<int(const std::vector<KwLeg>& legs)>;
 int kw_legs(aur_kw* const* stores, int n, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k,
             const int32_t* q_user, const int32_t* q_org, const FiltProgs* fp, const KwLegsThen& then);
 int kw_check(const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k);   // aur_kw_search's query checks
-int kw_check_columns(aur_kw* kw, const FiltProgs& fp);   // every attribute column fp's leaves name was set on kw
 int kw_device(const aur_kw* kw);
+AttrColumns& kw_attrs(aur_kw* kw);
 // The store side of a text add (kw_text.cu): the rows of one batch as aur_kw_add publishes them.  Callers hold the
 // store's mu_write (kw_write_mutex) and have checked the arguments and the room (kw_check_room).  land(dst, stream)
 // enqueues the copy of the rows' total postings (term id, tf) to the store's device memory dst on the store's stream.

@@ -465,9 +465,7 @@ struct aur_kw {
   int64_t* d_off = nullptr; int32_t* d_len = nullptr; int64_t* d_ids = nullptr;
   int32_t* d_user = nullptr; int32_t* d_org = nullptr; uint8_t* d_live = nullptr;
   uint2* d_post = nullptr; int64_t post_cap = 0;
-  int32_t* d_attr[kFiltAttrCols] = {};   // attribute columns (program columns 2..), allocated on first aur_kw_set_attrs;
-                                         // the pointers are read and written under mu_stat
-  DevBuf<int32_t> attr_stage;            // aur_kw_set_attrs: (row, code) pairs (writers hold mu_write)
+  AttrColumns attrs;         // program columns 2.., capacity rows each (aur_kw_set_attrs, writers hold mu_write)
   // host mirrors (the writer's bookkeeping; searches read only the published statistics)
   std::vector<int64_t> h_off{0};
   std::vector<int32_t> h_len, h_user, h_org;
@@ -734,7 +732,7 @@ void kw_plan(const KwQuery& q, const std::vector<int32_t>& uniq, const std::vect
     b.b_qo = b.b_hv + 4 * static_cast<size_t>(hcap); b.b_sl = b.b_qo + 4 * qoff.size();
     b.b_qu = b.b_sl + 4 * std::max<size_t>(slot.size(), 1); b.b_qg = b.b_qu + 4 * static_cast<size_t>(nqb);
     b.b_qp = b.b_qg + 4 * static_cast<size_t>(nqb); b.b_pu = b.b_qp + 4 * static_cast<size_t>(nqb);
-    const int n_passes = q.fp ? (q.fp->n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms : 0;
+    const int n_passes = q.fp ? filter_passes(q.fp->n_programs) : 0;
     b.b_uk = q.fp ? b.b_pu + 4 * static_cast<size_t>(n_passes) : b.b_qp;
     b.tab.assign(b.b_uk + 4 * static_cast<size_t>(nu), 0);
     unsigned char* tab = b.tab.data();
@@ -837,31 +835,13 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
   int n_passes = 0;
   const bool scores = n_rows > 0 && N > 0 && std::any_of(blocks.begin(), blocks.end(), [](const KwBlock& b) { return b.nu > 0; });
   if (q.fp && scores) {
-    const FiltProgs& fp = *q.fp;
-    n_passes = (fp.n_programs + kFiltMaxPrograms - 1) / kFiltMaxPrograms;
-    const size_t n_tok = static_cast<size_t>(fp.prog_off[fp.n_programs]);
-    std::vector<int32_t> st(n_tok * 4 + static_cast<size_t>(fp.n_programs) + 1 + static_cast<size_t>(fp.bitmap_words));
-    if (n_tok) memcpy(st.data(), fp.prog, n_tok * 16);
-    memcpy(st.data() + n_tok * 4, fp.prog_off, (static_cast<size_t>(fp.n_programs) + 1) * 4);
-    if (fp.bitmap_words) memcpy(st.data() + n_tok * 4 + fp.n_programs + 1, fp.bitmap, static_cast<size_t>(fp.bitmap_words) * 4);
-    KW_TRY(c->fstage.reserve(st.size()));
+    n_passes = filter_passes(q.fp->n_programs);
     KW_TRY(c->fmask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(n_rows)));
-    KW_TRY(cudaMemcpyAsync(c->fstage.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice, s));   // pageable: staged on return
-    FiltParams fpp{};
-    fpp.cols[0] = kw->d_user; fpp.cols[1] = kw->d_org;
-    {
-      std::lock_guard<std::mutex> lk(kw->mu_stat);
-      for (int i = 0; i < kFiltAttrCols; ++i) fpp.cols[2 + i] = kw->d_attr[i];
-    }
-    const int32_t* d_off = c->fstage.p + n_tok * 4;   // token indices stay absolute: a pass starts at its first offset
-    fpp.tok = reinterpret_cast<const FiltToken*>(c->fstage.p);
-    fpp.bitmap = reinterpret_cast<const uint32_t*>(d_off + fp.n_programs + 1);
-    fpp.live = kw->d_live;
-    fpp.n_rows = n_rows;
+    FiltParams p;
+    KW_TRY(filter_upload(*q.fp, kw->d_user, kw->d_org, kw->attrs, c->fstage, s, &p));
+    p.live = kw->d_live; p.n_rows = n_rows;
     for (int ps = 0; ps < n_passes; ++ps) {
-      fpp.prog_off = d_off + ps * kFiltMaxPrograms;
-      fpp.n_programs = std::min(kFiltMaxPrograms, fp.n_programs - ps * kFiltMaxPrograms);
-      KW_TRY(launch_filter_mask(fpp, c->fmask.p + static_cast<size_t>(ps) * n_rows, s));
+      KW_TRY(launch_filter_mask(filter_pass(p, ps), c->fmask.p + static_cast<size_t>(ps) * n_rows, s));
       c->launches += 1;
     }
     d_fmask = c->fmask.p;
@@ -1135,17 +1115,8 @@ int kw_check(const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32
   return kw_check_query(KwQuery{q_terms, q_offsets, nq, k, nullptr, nullptr, nullptr, 0});
 }
 
-int kw_check_columns(aur_kw* kw, const FiltProgs& fp) {
-  std::lock_guard<std::mutex> st(kw->mu_stat);   // the attribute columns that exist
-  for (int32_t t = 0; t < fp.prog_off[fp.n_programs]; ++t) {
-    const int32_t* tk = fp.prog + 4 * static_cast<int64_t>(t);
-    if (tk[0] == kFiltLeaf && tk[1] >= 2 && !kw->d_attr[tk[1] - 2])
-      return report_error(AUR_ERR_INVALID, "column %d was never set on the keyword store", tk[1]);
-  }
-  return AUR_OK;
-}
-
 int kw_device(const aur_kw* kw) { return kw->device; }
+AttrColumns& kw_attrs(aur_kw* kw) { return kw->attrs; }
 }  // namespace aur
 
 
@@ -1199,8 +1170,7 @@ int aur_kw_close(aur_kw* kw) {
   for (auto& c : kw->ctxs) cudaStreamSynchronize(c->stream);
   cudaFree(kw->d_off); cudaFree(kw->d_len); cudaFree(kw->d_ids); cudaFree(kw->d_user); cudaFree(kw->d_org);
   cudaFree(kw->d_live); cudaFree(kw->d_post); cudaFree(kw->d_toff); cudaFree(kw->d_tpost);
-  for (int32_t* a : kw->d_attr) cudaFree(a);
-  kw->attr_stage.release();
+  kw->attrs.release();
   for (auto& c : kw->ctxs) c->release();
   if (kw->stream) cudaStreamDestroy(kw->stream);
   delete kw;
@@ -1400,14 +1370,9 @@ int aur_kw_compact(aur_kw* kw, int64_t* reclaimed) {
   }
   // attribute codes move with their rows (through a bounce buffer); the rows compaction frees start absent again
   int32_t* bounce = nullptr;
-  const bool any_attr = std::any_of(std::begin(kw->d_attr), std::end(kw->d_attr), [](const int32_t* a) { return a != nullptr; });
-  if (e == cudaSuccess && any_attr && nl) e = cudaMalloc(&bounce, static_cast<size_t>(nl) * 4);
-  for (int32_t* a : kw->d_attr) {
-    if (!a) continue;
-    if (e == cudaSuccess && nl) e = launch_gather_i32(a, d_map, nl, bounce, kw->stream);
-    if (e == cudaSuccess && nl) e = cudaMemcpyAsync(a, bounce, static_cast<size_t>(nl) * 4, cudaMemcpyDeviceToDevice, kw->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(a + nl, 0xFF, static_cast<size_t>(rows - nl) * 4, kw->stream);
-  }
+  if (e == cudaSuccess && kw->attrs.any() && nl) e = cudaMalloc(&bounce, static_cast<size_t>(nl) * 4);
+  if (e == cudaSuccess) e = kw->attrs.gather(d_map, nl, 0, bounce, kw->stream);
+  if (e == cudaSuccess) e = kw->attrs.clear(nl, rows, kw->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(kw->stream);
   cudaFree(d_map);
   cudaFree(bounce);
@@ -1456,36 +1421,16 @@ int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out) {
 
 int aur_kw_set_attrs(aur_kw* kw, int32_t col, const int64_t* ids, const int32_t* codes, int64_t n) {
   if (!kw || n < 0 || (n > 0 && (!ids || !codes))) return report_error(AUR_ERR_INVALID, "null argument");
-  if (col < 2 || col >= kFiltCols) return report_error(AUR_ERR_INVALID, "attribute columns are 2 .. %d", kFiltCols - 1);
   std::lock_guard<std::mutex> wk(kw->mu_write);
   std::shared_lock<std::shared_mutex> rl(kw->rw);
   KW_TRY(cudaSetDevice(kw->device));
-  cudaStream_t s = kw->stream;
-  int32_t* a = nullptr;
-  {
-    std::lock_guard<std::mutex> st(kw->mu_stat);
-    a = kw->d_attr[col - 2];
-  }
-  if (!a) {   // first use: every row absent (-1), at the store's capacity like its tenant codes
-    KW_TRY(cudaMalloc(&a, static_cast<size_t>(kw->capacity) * 4));
-    cudaError_t e = cudaMemsetAsync(a, 0xFF, static_cast<size_t>(kw->capacity) * 4, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { cudaFree(a); return report_error(AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e)); }
-    std::lock_guard<std::mutex> st(kw->mu_stat);
-    kw->d_attr[col - 2] = a;
-  }
   std::vector<int32_t> pairs;   // (row, code); id2row changes only under mu_write, which this call holds
   pairs.reserve(2 * static_cast<size_t>(n));
   for (int64_t i = 0; i < n; ++i) {
     auto it = kw->id2row.find(ids[i]);
     if (it != kw->id2row.end()) { pairs.push_back(static_cast<int32_t>(it->second)); pairs.push_back(codes[i]); }
   }
-  if (pairs.empty()) return AUR_OK;
-  KW_TRY(kw->attr_stage.reserve(pairs.size()));
-  KW_TRY(cudaMemcpyAsync(kw->attr_stage.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s));
-  KW_TRY(launch_scatter_codes(kw->attr_stage.p, static_cast<int64_t>(pairs.size() / 2), a, s));
-  KW_TRY(cudaStreamSynchronize(s));
-  return AUR_OK;
+  return kw->attrs.write(col, pairs, kw->capacity, kw->stream);   // the store's capacity, like its tenant codes
 }
 
 int aur_kw_search(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k, const int32_t* q_user,

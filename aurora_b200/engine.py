@@ -35,6 +35,18 @@ def _row_dtype(dtype: int):
     return {N.AUR_BF16: np.uint16, N.AUR_F32: np.float32, N.AUR_I8: np.int8}[dtype]
 
 
+def _program_args(programs, q_program, nq: int):
+    """The C arrays of a filtered call: ``pack_programs(programs)`` and q_program as int32 [nq] (None = every query on
+    program 0)."""
+    from .filters import pack_programs
+
+    tok, off, bm = pack_programs(programs)
+    ql = np.zeros(nq, np.int32) if q_program is None else np.ascontiguousarray(q_program, dtype=np.int32)
+    if ql.shape != (nq,):
+        raise ValueError("q_program must be [nq]")
+    return tok, off, bm, ql
+
+
 class Index:
     """One row-shard of the corpus, resident on one GPU.
 
@@ -227,14 +239,9 @@ class Index:
         (``filters.compile_program`` outputs, at most 32; ``q_program`` None = every query on program 0).  One program
         matching more than ``max_list_rows`` rows runs the masked full scan, anything else the list kernels.  Returns
         (ids [nq,k] int64, scores [nq,k] float32, matching rows per program int64, snapshot rows)."""
-        from .filters import pack_programs
-
         q = self._rows_buffer(queries)
         nq = q.shape[0]
-        tok, off, bm = pack_programs(programs)
-        ql = np.zeros(nq, np.int32) if q_program is None else np.ascontiguousarray(q_program, dtype=np.int32)
-        if ql.shape != (nq,):
-            raise ValueError("q_program must be [nq]")
+        tok, off, bm, ql = _program_args(programs, q_program, nq)
         scores = np.empty((nq, k), dtype=np.float32)
         ids = np.empty((nq, k), dtype=np.int64)
         matched = np.zeros(len(programs), dtype=np.int64)
@@ -665,14 +672,9 @@ def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_o
     ids = np.empty((nq, k_out), dtype=np.int64)
     cosine = np.empty((nq, k_out), dtype=np.float32)
     if programs is not None:
-        from .filters import pack_programs
-
         if q_user is not None or q_org is not None:
             raise ValueError("programs replace q_user / q_org: write the tenant scope into the programs")
-        tok, off, bm = pack_programs(programs)
-        ql = np.zeros(nq, np.int32) if q_program is None else np.ascontiguousarray(q_program, dtype=np.int32)
-        if ql.shape != (nq,):
-            raise ValueError("q_program must be [nq]")
+        tok, off, bm, ql = _program_args(programs, q_program, nq)
         shard_list = index.shards if multi else [index]
         store_list = kw_index.stores if multi else [kw_index]
         n = len(shard_list)
