@@ -11,6 +11,11 @@ AURORA_B200_CAPACITY (rows of HBM to reserve, default 1048576), AURORA_B200_DTYP
 default, or int8 for half the HBM), AURORA_B200_SNAPSHOT (directory: restored at
 start when present; see KnowledgeBase.save), AURORA_B200_MAX_TOKENS / AURORA_B200_MAX_SEQS (encoder workspace).
 There is no CPU fallback: without a CUDA device or with a variable missing this raises.
+
+With AURORA_B200_DEVICES (one owner process over several GPUs) every listed GPU holds an encoder replica as well as its
+shard (bf16 and int8 shards; f32 shards take host vectors and get no replicas), and ingest encodes each shard's share on its own GPU.  Each replica takes the weights plus its own workspace,
+sized by AURORA_B200_MAX_TOKENS / MAX_SEQS.  For bge-base at the defaults (32768 tokens, 2048 sequences), counted from
+aur_encoder_open's allocations, that is 218 MB of weights, 511 MB of activations and 9 MB of pooled outputs per GPU.
 """
 
 from __future__ import annotations
@@ -49,14 +54,18 @@ def configure_from_env() -> None:
     snap = os.environ.get("AURORA_B200_SNAPSHOT")
     wal = os.environ.get("AURORA_B200_WAL", "1") != "0"      # mutation log beside the snapshot (replayed after a crash)
 
-    # AURORA_B200_DEVICES = "all" or "0,1,2,...": this process owns one shard per listed GPU (engine.MultiIndex);
-    # the encoder stays on AURORA_B200_DEVICE
+    # AURORA_B200_DEVICES = "all" or "0,1,2,...": this process owns one shard per listed GPU (engine.MultiIndex) and
+    # one encoder on each of those GPUs (the weights are read once and copied device to device): every shard's share of
+    # an ingest is encoded on its own GPU.  Queries are encoded on AURORA_B200_DEVICE.
     devs = os.environ.get("AURORA_B200_DEVICES", "").strip()
     factory = loader = None
     if devs:
+        from . import _native as N
         from .engine import MultiIndex
 
-        devices = None if devs == "all" else [int(x) for x in devs.split(",")]
+        devices = list(range(N.load().aur_device_count())) if devs == "all" else [int(x) for x in devs.split(",")]
+        if dtype != "f32":              # f32 shards take host vectors (TextEncoder.can_append): replicas would sit idle
+            text_encoder.replicate(devices)
         factory = lambda dim, cap: MultiIndex(dim, cap, devices=devices, dtype=dtype)       # noqa: E731
         loader = lambda path, cap: MultiIndex.load(path, capacity=cap, devices=devices)     # noqa: E731
 

@@ -144,12 +144,8 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_qkv, const AttnParams p)
 
 cudaError_t attn_tc_launch(const void* tmap_qkv, const AttnParams& p, cudaStream_t s) {
   if (p.n_items <= 0) return cudaSuccess;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kSmemBytes));
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
+  cudaError_t e = raise_smem_limit(reinterpret_cast<const void*>(attn_tc_kernel), kSmemBytes);   // on every device
+  if (e != cudaSuccess) return e;
   return launch_pdl(attn_tc_kernel, dim3(static_cast<unsigned>(p.n_items * p.heads)), dim3(kThreads), kSmemBytes, s, 1,
                     *reinterpret_cast<const CUtensorMap*>(tmap_qkv), p);
 }

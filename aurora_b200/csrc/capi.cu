@@ -24,6 +24,7 @@
 #include <string.h>
 
 #include <atomic>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <shared_mutex>
@@ -61,6 +62,20 @@ EncodeTiledFn get_encode_fn() {
 }  // namespace
 
 namespace aur {
+cudaError_t raise_smem_limit(const void* kern, size_t smem) {
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, size_t> raised;   // (kernel, device) -> limit set so far
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  std::lock_guard<std::mutex> g(mu);
+  size_t& cur = raised[{kern, dev}];
+  if (cur >= smem) return cudaSuccess;
+  e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  if (e == cudaSuccess) cur = smem;
+  return e;
+}
+
 int report_error(int code, const char* fmt, ...) {
   char buf[512];
   va_list ap; va_start(ap, fmt); vsnprintf(buf, sizeof buf, fmt, ap); va_end(ap);

@@ -5,8 +5,11 @@
 //   ctx    [max_tokens_pad, H]    attention output
 //   inter  [max_tokens_pad, I]    FFN activation
 // and the TMA descriptors over them (activations as GEMM A operands, weights as B operands).
-// A forward is 2 + 7*L + 1 kernel launches on one stream; no CPU compute path exists.
+// A forward is 2 + 7*L + 1 kernel launches on one stream; no CPU compute path exists.  aur_encoder_replicate copies a
+// loaded encoder's parameters to a fresh encoder on any device; aur_encode_append_multi runs one encoder per shard of a
+// multi-GPU corpus, each on its own host thread, the pooled rows going straight into its shard.
 #include <algorithm>
+#include <functional>
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -17,6 +20,7 @@
 
 #include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "../../include/aurora_b200.h"
@@ -87,6 +91,21 @@ int dev_alloc(T** p, size_t n) {
   ENC_TRY(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
   ENC_TRY(cudaMemset(*p, 0, n * sizeof(T)));
   return AUR_OK;
+}
+
+// Every parameter buffer of e with its element count (the head-dim-32 layouts padded as stored), in one fixed order:
+// aur_encoder_open allocates them, aur_encoder_replicate copies them buffer for buffer.
+template <typename F>
+void for_each_param(aur_encoder* e, F&& f) {
+  const aur_encoder_config& c = e->cfg;
+  const size_t H = c.hidden, I = c.inter, HP = e->hp;
+  f(e->word, static_cast<size_t>(c.vocab) * H); f(e->pos, static_cast<size_t>(c.max_pos) * H);
+  f(e->type, static_cast<size_t>(c.type_vocab) * H); f(e->emb_g, H); f(e->emb_b, H);
+  for (Layer& l : e->layers) {
+    f(l.wqkv, 3 * HP * H); f(l.wo, H * HP); f(l.wi, I * H); f(l.wo2, H * I);
+    f(l.bqkv, 3 * HP); f(l.bo, H); f(l.bi, I); f(l.bo2, H);
+    f(l.ln1_g, H); f(l.ln1_b, H); f(l.ln2_g, H); f(l.ln2_b, H);
+  }
 }
 
 void free_all(aur_encoder* e) {
@@ -214,6 +233,50 @@ int stage_inputs(aur_encoder* e, const int32_t* tokens, const int32_t* cu, int n
   return AUR_OK;
 }
 
+bool same_config(const aur_encoder_config& a, const aur_encoder_config& b) {   // everything but the device
+  return a.hidden == b.hidden && a.layers == b.layers && a.heads == b.heads && a.inter == b.inter && a.vocab == b.vocab &&
+         a.max_pos == b.max_pos && a.type_vocab == b.type_vocab && a.pool == b.pool && a.normalize == b.normalize &&
+         a.max_tokens == b.max_tokens && a.max_seqs == b.max_seqs && memcmp(&a.ln_eps, &b.ln_eps, sizeof(float)) == 0 &&
+         a.reserved == b.reserved;
+}
+
+// One batch of aur_encode_append_multi: sequences seq[0 .. m) of the caller's packed input (already checked, within the
+// workspace) are staged, encoded, and their pooled bf16 rows appended to ix on the encoder's stream.
+int append_batch(aur_encoder* e, aur_index* ix, const int32_t* tokens, const int32_t* cu, const int32_t* seq, int m,
+                 const int64_t* ids, const int32_t* users, const int32_t* orgs) {
+  std::vector<int32_t> cu_b(static_cast<size_t>(m) + 1, 0), u_b, o_b;
+  std::vector<int64_t> id_b(static_cast<size_t>(m));
+  if (users) u_b.resize(static_cast<size_t>(m));
+  if (orgs) o_b.resize(static_cast<size_t>(m));
+  for (int i = 0; i < m; ++i) {
+    const int32_t s = seq[i];
+    cu_b[i + 1] = cu_b[i] + (cu[s + 1] - cu[s]);
+    id_b[i] = ids[s];
+    if (users) u_b[i] = users[s];
+    if (orgs) o_b[i] = orgs[s];
+  }
+  std::lock_guard<std::mutex> g(e->mu);
+  ENC_TRY(cudaSetDevice(e->cfg.device));
+  int n_items = 0;
+  for (int i = 0; i < m; ++i) {
+    const int32_t s = seq[i], len = cu[s + 1] - cu[s], at = cu_b[i];
+    memcpy(e->h_tok + at, tokens + cu[s], sizeof(int32_t) * len);
+    for (int t = 0; t < len; ++t) e->h_pos[at + t] = t;
+    for (int q0 = 0; q0 < len; q0 += 128) e->h_items[n_items++] = AttnItem{at, len, q0, 0};
+  }
+  int rc = forward_locked(e, cu_b.data(), m, n_items);
+  if (rc == AUR_OK)
+    rc = aur_add_dev(ix, e->d_pool_bf16, id_b.data(), users ? u_b.data() : nullptr, orgs ? o_b.data() : nullptr, m, e->stream);
+  // the pinned staging is reused by the next batch: the stream must be past its copies, whatever happened above
+  const cudaError_t ce = cudaStreamSynchronize(e->stream);
+  if (rc != AUR_OK) return rc;
+  if (ce != cudaSuccess) return report_error(AUR_ERR_CUDA, "encode_append_multi: %s", cudaGetErrorString(ce));
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]);
+  e->stats.total_ms = ms;
+  return AUR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -246,14 +309,7 @@ int aur_encoder_open(const aur_encoder_config* cfg, aur_encoder** out) {
   e->layers.resize(cfg->layers);
   int rc = AUR_OK;
   auto A = [&](auto** p, size_t n) { if (rc == AUR_OK) rc = dev_alloc(p, n); };
-  A(&e->word, static_cast<size_t>(cfg->vocab) * H); A(&e->pos, static_cast<size_t>(cfg->max_pos) * H);
-  A(&e->type, static_cast<size_t>(cfg->type_vocab) * H); A(&e->emb_g, H); A(&e->emb_b, H);
-  for (Layer& l : e->layers) {
-    A(&l.wqkv, static_cast<size_t>(3) * e->hp * H); A(&l.wo, static_cast<size_t>(H) * e->hp);
-    A(&l.wi, static_cast<size_t>(I) * H); A(&l.wo2, static_cast<size_t>(H) * I);
-    A(&l.bqkv, 3 * e->hp); A(&l.bo, H); A(&l.bi, I); A(&l.bo2, H);
-    A(&l.ln1_g, H); A(&l.ln1_b, H); A(&l.ln2_g, H); A(&l.ln2_b, H);
-  }
+  for_each_param(e, [&](auto*& p, size_t n) { A(&p, n); });
   const size_t R = e->rows_pad;
   A(&e->x, R * H); A(&e->y, R * H); A(&e->qkv, R * 3 * e->hp); A(&e->ctx, R * e->hp); A(&e->inter, R * I);
   A(&e->d_tok, cfg->max_tokens); A(&e->d_pos, cfg->max_tokens); A(&e->d_cu, cfg->max_seqs + 1);
@@ -381,6 +437,123 @@ int aur_encode_append(aur_encoder* e, aur_index* ix, const int32_t* tokens, cons
   float ms = 0.f;
   cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]);
   e->stats.total_ms = ms;
+  return AUR_OK;
+}
+
+int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out) {
+  if (!src || !out) return report_error(AUR_ERR_INVALID, "null argument");
+  *out = nullptr;
+  std::lock_guard<std::mutex> g(src->mu);   // no upload or close of src while its bits are read
+  if (!src->missing.empty())
+    return report_error(AUR_ERR_INVALID, "encoder parameters not loaded: %s (+%zu more)", src->missing[0].c_str(), src->missing.size() - 1);
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev)
+    return report_error(AUR_ERR_INVALID, "device %d of %d", device, ndev);
+  aur_encoder_config cfg = src->cfg;
+  cfg.device = device;
+  aur_encoder* r = nullptr;
+  int rc = aur_encoder_open(&cfg, &r);
+  if (rc != AUR_OK) return rc;
+  std::vector<const void*> from;
+  std::vector<size_t> bytes;
+  std::vector<void*> to;
+  for_each_param(src, [&](auto*& p, size_t n) { from.push_back(p); bytes.push_back(n * sizeof(*p)); });
+  for_each_param(r, [&](auto*& p, size_t) { to.push_back(p); });
+  cudaError_t ce = cudaSuccess;
+  for (size_t i = 0; i < to.size() && ce == cudaSuccess; ++i)   // staged by the driver when the devices are not peers
+    ce = cudaMemcpyPeerAsync(to[i], device, from[i], src->cfg.device, bytes[i], r->stream);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(r->stream);
+  if (ce != cudaSuccess) {
+    aur_encoder_close(r);
+    return report_error(AUR_ERR_CUDA, "encoder replica on device %d: %s", device, cudaGetErrorString(ce));
+  }
+  r->missing.clear();
+  *out = r;
+  return AUR_OK;
+}
+
+int aur_encode_append_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,
+                            const int32_t* cu, int32_t n_seq, const int64_t* ids, const int32_t* user_codes,
+                            const int32_t* org_codes, int32_t max_tokens_per_call, int32_t max_seqs_per_call) {
+  constexpr int kMaxShards = 64;
+  if (!encs || !shards) return report_error(AUR_ERR_INVALID, "null argument");
+  if (n < 1 || n > kMaxShards) return report_error(AUR_ERR_INVALID, "n must be in 1 .. %d", kMaxShards);
+  for (int32_t s = 0; s < n; ++s)
+    if (!shards[s] || !encs[s]) return report_error(AUR_ERR_INVALID, "shard or encoder %d is NULL", s);
+  std::vector<aur_index*> order(shards, shards + n);
+  std::sort(order.begin(), order.end(), std::less<aur_index*>());
+  if (std::adjacent_find(order.begin(), order.end()) != order.end()) return report_error(AUR_ERR_INVALID, "a shard is listed twice");
+  const aur_encoder_config& c = encs[0]->cfg;   // fixed at open
+  for (int32_t s = 0; s < n; ++s) {
+    aur_encoder* e = encs[s];
+    if (!same_config(e->cfg, c)) return report_error(AUR_ERR_INVALID, "encoder %d has another configuration than encoder 0", s);
+    {
+      std::lock_guard<std::mutex> g(e->mu);
+      if (!e->missing.empty())
+        return report_error(AUR_ERR_INVALID, "encoder %d parameters not loaded: %s (+%zu more)", s, e->missing[0].c_str(),
+                            e->missing.size() - 1);
+    }
+    if (e->cfg.device != index_device(shards[s]))
+      return report_error(AUR_ERR_INVALID, "encoder %d is on device %d, its shard on device %d", s, e->cfg.device, index_device(shards[s]));
+  }
+  std::vector<aur_stats> st(static_cast<size_t>(n));
+  for (int32_t s = 0; s < n; ++s) {
+    int rc = aur_get_stats(shards[s], &st[s]);
+    if (rc != AUR_OK) return rc;
+    if (st[s].dim != c.hidden || st[s].dtype == AUR_F32)   // (an int8 shard quantizes the bf16 rows as it adds them)
+      return report_error(AUR_ERR_INVALID, "shard %d is %d-d dtype %d; the encoder produces %d-d bf16", s, st[s].dim, st[s].dtype, c.hidden);
+  }
+  if (max_tokens_per_call < 0 || max_tokens_per_call > c.max_tokens || max_seqs_per_call < 0 || max_seqs_per_call > c.max_seqs)
+    return report_error(AUR_ERR_INVALID, "per-call limits must be 0 .. the workspace (%d tokens, %d sequences)", c.max_tokens, c.max_seqs);
+  const int tok_budget = max_tokens_per_call ? max_tokens_per_call : c.max_tokens;
+  const int seq_budget = max_seqs_per_call ? max_seqs_per_call : c.max_seqs;
+  if (n_seq < 0) return report_error(AUR_ERR_INVALID, "n_seq < 0");
+  if (n_seq == 0) return AUR_OK;
+  if (!tokens || !cu || !ids) return report_error(AUR_ERR_INVALID, "tokens, cu_seqlens and ids are required");
+  if (cu[0] != 0) return report_error(AUR_ERR_INVALID, "cu_seqlens[0] must be 0");
+  std::vector<std::vector<int32_t>> share(static_cast<size_t>(n));
+  for (int32_t i = 0; i < n_seq; ++i) {
+    const int len = cu[i + 1] - cu[i];
+    if (len < 1 || len > c.max_pos) return report_error(AUR_ERR_INVALID, "sequence %d has length %d (1..%d)", i, len, c.max_pos);
+    if (len > tok_budget) return report_error(AUR_ERR_NOMEM, "sequence %d has %d tokens > %d per call", i, len, tok_budget);
+    for (int t = 0; t < len; ++t) {
+      const int32_t id = tokens[cu[i] + t];
+      if (id < 0 || id >= c.vocab) return report_error(AUR_ERR_INVALID, "token id %d out of range at sequence %d", id, i);
+    }
+    if (ids[i] < 0) return report_error(AUR_ERR_INVALID, "ids must be >= 0");
+    share[static_cast<size_t>(ids[i] % n)].push_back(i);
+  }
+  for (int32_t s = 0; s < n; ++s)
+    if (st[s].rows + static_cast<int64_t>(share[s].size()) > st[s].capacity)
+      return report_error(AUR_ERR_NOMEM, "shard %d full: %lld + %zu > capacity %lld (aur_compact reclaims tombstones)", s,
+                          static_cast<long long>(st[s].rows), share[s].size(), static_cast<long long>(st[s].capacity));
+  // each shard's share, in input order, in greedy workspace batches; the shards run on their own host threads
+  std::vector<int> rcs(static_cast<size_t>(n), AUR_OK);
+  std::vector<std::string> errs(static_cast<size_t>(n));
+  auto run = [&](int32_t s) {
+    const std::vector<int32_t>& q = share[s];
+    for (size_t i = 0; i < q.size();) {
+      size_t j = i;
+      int64_t toks = 0;
+      while (j < q.size() && static_cast<int>(j - i) < seq_budget && toks + (cu[q[j] + 1] - cu[q[j]]) <= tok_budget)
+        toks += cu[q[j] + 1] - cu[q[j]], ++j;
+      const int rc = append_batch(encs[s], shards[s], tokens, cu, q.data() + i, static_cast<int>(j - i), ids, user_codes, org_codes);
+      if (rc != AUR_OK) {
+        rcs[s] = rc;
+        const char* msg = aur_last_error();
+        errs[s] = msg ? msg : "";
+        return;
+      }
+      i = j;
+    }
+  };
+  std::vector<std::thread> th;
+  for (int32_t s = 1; s < n; ++s)
+    if (!share[s].empty()) th.emplace_back(run, s);
+  run(0);
+  for (std::thread& t : th) t.join();
+  for (int32_t s = 0; s < n; ++s)
+    if (rcs[s] != AUR_OK) return report_error(rcs[s], "shard %d: %s", s, errs[s].c_str());
   return AUR_OK;
 }
 

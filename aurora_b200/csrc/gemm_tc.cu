@@ -169,13 +169,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 template <int BN, int EPI, int G>
 cudaError_t launch_one(int sm_count, const void* tmap_a, const void* tmap_b, const GemmParams& p, cudaStream_t s) {
   auto kern = gemm_tc_kernel<BN, EPI, G>;
-  static bool attr_set = false;   // per instantiation
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(GemmSmem<BN>::kTotal));
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
+  cudaError_t e = raise_smem_limit(reinterpret_cast<const void*>(kern), GemmSmem<BN>::kTotal);   // on every device
+  if (e != cudaSuccess) return e;
   const int tiles = p.m_tiles * p.n_tiles, groups = sm_count / G;
   return launch_pdl(kern, dim3(static_cast<unsigned>((tiles < groups ? tiles : groups) * G)), dim3(kGemmThreads),
                     GemmSmem<BN>::kTotal, s, G, *reinterpret_cast<const CUtensorMap*>(tmap_a),

@@ -412,6 +412,12 @@ void kw_after_append(aur_kw* kw, int rc);                         // the writer'
 std::mutex& kw_write_mutex(aur_kw* kw);
 int64_t kw_rows_appended(const aur_kw* kw);
 
+// Opt kernel `kern` in to at least `smem` bytes of dynamic shared memory on the current device.  The limit is one
+// setting per kernel and device, shared by every thread that launches it there: it is only ever raised, under a lock,
+// so a launch asking for less never lowers it under a concurrent launch that needs more, and a kernel first launched
+// on one device is still opted in on every other.  (capi.cu)
+cudaError_t raise_smem_limit(const void* kern, size_t smem);
+
 // Error reporting shared by the translation units behind the C ABI (thread-local message).
 int report_error(int code, const char* fmt, ...);
 // 2-D bf16 tensor map, 128-byte swizzle; returns 0 or a CUresult.

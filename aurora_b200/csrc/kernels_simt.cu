@@ -683,10 +683,10 @@ cudaError_t launch_finalize(const FinalizeArgs& a_in, cudaStream_t s) {
   a.sort_cap = P;
   const size_t smem = static_cast<size_t>(P) * 8 + static_cast<size_t>(a.dim) * 4;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(a.dtype == 0 ? (const void*)finalize_kernel<__nv_bfloat16>
-                                         : a.dtype == 2 ? (const void*)finalize_kernel<__nv_bfloat16, int8_t>
-                                                        : (const void*)finalize_kernel<float>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+    // raised only: concurrent searches on one device ask for different sizes (raise_smem_limit)
+    cudaError_t e = raise_smem_limit(a.dtype == 0 ? (const void*)finalize_kernel<__nv_bfloat16>
+                                     : a.dtype == 2 ? (const void*)finalize_kernel<__nv_bfloat16, int8_t>
+                                                    : (const void*)finalize_kernel<float>, smem);
     if (e != cudaSuccess) return e;
   }
   // programmatic dependent launch: blocks start (query -> shared memory, |q|^2) while the similarity kernel drains

@@ -945,7 +945,8 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
 template <int kCtaGroup, bool kMask, int kTileN, int kQReg = 0, bool kI8 = false>
 cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm, const TcParams& p, size_t smem) {
   auto kern = simtopk_tc_kernel<kCtaGroup, kMask, kTileN, kQReg, kI8>;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem));
+  // raised only: concurrent searches of the shards on one device ask for different sizes (raise_smem_limit)
+  cudaError_t e = raise_smem_limit(reinterpret_cast<const void*>(kern), smem);
   if (e != cudaSuccess) return e;
   return cudaLaunchKernelEx(&cfg, kern, tm, p);
 }

@@ -74,6 +74,15 @@ class Encoder:
                                ln_eps=cfg.ln_eps, reserved=0)
         N.check(self._lib.aur_encoder_open(C.byref(c), C.byref(self._h)))
 
+    def replicate(self, device: int) -> "Encoder":
+        """A second encoder on ``device`` (this one's too) with this one's parameters, copied device to device
+        (aur_encoder_replicate): its forward is this one's bit for bit, and it outlives this one."""
+        h = C.c_void_p()
+        N.check(self._lib.aur_encoder_replicate(self._h, int(device), C.byref(h)))
+        r = Encoder.__new__(Encoder)
+        r._lib, r.cfg, r.device, r.max_tokens, r.max_seqs, r._h = self._lib, self.cfg, int(device), self.max_tokens, self.max_seqs, h
+        return r
+
     def close(self) -> None:
         if getattr(self, "_h", None) is not None and self._h.value:
             self._lib.aur_encoder_close(self._h)
@@ -152,13 +161,40 @@ class Encoder:
         return out
 
 
+def encode_append_multi(encoders: Sequence[Encoder], shards, tokens: np.ndarray, cu_seqlens: np.ndarray, ids: np.ndarray,
+                        user_codes: Optional[np.ndarray] = None, org_codes: Optional[np.ndarray] = None,
+                        max_tokens_per_call: int = 0, max_seqs_per_call: int = 0) -> None:
+    """aur_encode_append_multi: packed sequences encoded and appended to ``shards`` (``engine.Index`` on their encoders'
+    devices) placed by ``id mod len(shards)``, sequence i by ``encoders[ids[i] % n]``; every shard's share at once,
+    in workspace batches (0 = the encoder's workspace)."""
+    n = len(shards)
+    if len(encoders) != n:
+        raise ValueError(f"{len(encoders)} encoders for {n} shards")
+    tokens = np.ascontiguousarray(tokens, dtype=np.int32)
+    cu = np.ascontiguousarray(cu_seqlens, dtype=np.int32)
+    if cu.ndim != 1 or cu.size < 1 or tokens.ndim != 1 or tokens.size != int(cu[-1]):
+        raise ValueError("tokens [total] and cu_seqlens [n_seq + 1] with cu[-1] == total are required")
+    ids = np.ascontiguousarray(ids, dtype=np.int64)
+    if ids.shape != (cu.size - 1,):
+        raise ValueError("ids must be [n_seq]")
+    u = None if user_codes is None else np.ascontiguousarray(user_codes, dtype=np.int32)
+    o = None if org_codes is None else np.ascontiguousarray(org_codes, dtype=np.int32)
+    encs = (C.c_void_p * n)(*[e._h.value for e in encoders])
+    hs = (C.c_void_p * n)(*[sh._h.value for sh in shards])
+    lib = N.load()
+    N.check(lib.aur_encode_append_multi(encs, hs, n, _ptr(tokens), _ptr(cu), cu.size - 1, _ptr(ids), _ptr(u), _ptr(o),
+                                        int(max_tokens_per_call), int(max_seqs_per_call)))
+
+
 class TextEncoder:
     """Adapter for aurora_b200.retriever.KnowledgeBase: ``dim`` + ``encode(texts)`` over a tokenizer and the CUDA
     ``Encoder``; ``encode_append`` is the fused ingest path (vectors never leave the device between the forward
-    pass and the shard append).
+    pass and the shard append).  ``replicate(devices)`` adds one encoder per further device, so that the fused path
+    also serves an ``engine.MultiIndex`` with every shard's share encoded on the shard's own GPU; queries
+    (``encode``) stay on the primary encoder.
 
-    ``tokenizer``: an ``aurora_b200.wordpiece.NativeTokenizer`` (C++, multi-threaded -- then whole batches go through
-    ONE C call, ``aur_encode_text_append``, with no Python per text) or any ``tokenize(text) -> list[int]`` callable.
+    ``tokenizer``: an ``aurora_b200.wordpiece.NativeTokenizer`` (C++, multi-threaded -- then a whole batch is tokenised
+    in ONE C call, with no Python per text) or any ``tokenize(text) -> list[int]`` callable.
 
     Texts longer than the position table (the reference's chunker can emit a 4 000-character chunk,
     document_processor.py:266-267) are not cut off: they are split into windows of ``max_pos`` tokens, each window is
@@ -170,6 +206,30 @@ class TextEncoder:
         self._native = hasattr(tokenizer, "encode_packed")
         self.dim = encoder.cfg.hidden
         self.max_len = int(max_len or encoder.cfg.max_pos)
+        self._encs: Dict[int, Encoder] = {encoder.device: encoder}    # device -> the encoder that appends there
+
+    def replicate(self, devices) -> "TextEncoder":
+        """Keep one encoder on each of ``devices``: the primary for its own device, a replica (``Encoder.replicate``,
+        the same parameters copied device to device) for every other.  Returns self."""
+        for d in devices:
+            if int(d) not in self._encs:
+                self._encs[int(d)] = self._enc.replicate(int(d))
+        return self
+
+    @staticmethod
+    def _shards(index) -> list:
+        from .engine import MultiIndex
+
+        return list(index.shards) if isinstance(index, MultiIndex) else [index]
+
+    def can_append(self, index) -> bool:
+        """Whether ``encode_append`` takes ``index``: an ``engine.Index``, or a ``MultiIndex`` of them, bf16 or int8,
+        ``dim`` wide, with an encoder on every shard's device."""
+        from .engine import Index
+
+        shards = self._shards(index)
+        return bool(shards) and all(isinstance(sh, Index) and sh.dtype != N.AUR_F32 and sh.dim == self.dim
+                                    and sh.device in self._encs for sh in shards)
 
     # ------------------------------------------------------------------ tokenisation
     def _tokenize(self, texts: Sequence[str], max_len: int):
@@ -245,32 +305,29 @@ class TextEncoder:
         return out
 
     def encode_append(self, index, texts: Sequence[str], ids: np.ndarray, user_codes=None, org_codes=None) -> None:
-        """Tokenise once (one multi-threaded C call with the native tokenizer), then encoder forward + shard append per
-        workspace-sized batch; nothing runs per text in Python."""
+        """Tokenise once (one multi-threaded C call with the native tokenizer), then ONE aur_encode_append_multi call
+        for every text that fits the position table: workspace batches, encoder forward and shard append inside the
+        library, each shard's share on its own device (``can_append`` says which indexes qualify); nothing runs per
+        text or per batch in Python.  Over-long texts are averaged over their windows on the host and added with
+        ``index.add``."""
+        if not self.can_append(index):
+            raise ValueError("encode_append needs bf16 or int8 engine.Index shards on devices this encoder has replicas on")
         ids = np.ascontiguousarray(ids, dtype=np.int64)
         tok, cu = self._tokenize(texts, self.max_len)
         lens = np.diff(cu)
         long_ones = self._over_long(texts, lens)
         u = None if user_codes is None else np.ascontiguousarray(user_codes, dtype=np.int32)
         o = None if org_codes is None else np.ascontiguousarray(org_codes, dtype=np.int32)
-        keep = np.ones(len(texts), dtype=bool)
-        keep[long_ones] = False
-        sel = np.nonzero(keep)[0]
-        i = 0
-        while i < len(sel):
-            j, toks = i, 0
-            while j < len(sel) and j - i < self._enc.max_seqs and toks + lens[sel[j]] <= self._enc.max_tokens:
-                toks += int(lens[sel[j]]); j += 1
-            if j == i:
-                raise ValueError(f"text {sel[i]} tokenizes to {lens[sel[i]]} tokens: more than max_tokens={self._enc.max_tokens}")
-            part = sel[i:j]
-            if len(part) == part[-1] - part[0] + 1:            # contiguous run: slice the packed buffer
-                t = tok[cu[part[0]]:cu[part[-1] + 1]]
-                c = (cu[part[0]:part[-1] + 2] - cu[part[0]]).astype(np.int32)
-            else:
-                t, c = pack_sequences([tok[cu[x]:cu[x + 1]] for x in part])
-            self._enc.encode_append(index, t, c, ids[part], None if u is None else u[part], None if o is None else o[part])
-            i = j
+        t, c, i_, u_, o_ = tok, cu, ids, u, o
+        if long_ones:                                                 # drop them from the packed buffer
+            keep = np.ones(len(texts), dtype=bool)
+            keep[long_ones] = False
+            t = tok[np.repeat(keep, lens)]
+            c = np.zeros(int(keep.sum()) + 1, dtype=np.int32)
+            np.cumsum(lens[keep], out=c[1:])
+            i_, u_, o_ = ids[keep], None if u is None else u[keep], None if o is None else o[keep]
+        shards = self._shards(index)
+        encode_append_multi([self._encs[sh.device] for sh in shards], shards, t, c, i_, u_, o_)
         if long_ones:                                                 # averaged windows: the vectors are formed on the host
             v = self._encode_long_many([texts[i] for i in long_ones])
             index.add(v, ids[long_ones], None if u is None else u[long_ones], None if o is None else o[long_ones])

@@ -268,7 +268,10 @@ class KnowledgeBase:
         if not objs:
             return 0
         texts = [t for _, _, t in objs]
-        fused = hasattr(self.encoder, "encode_append") and hasattr(self.index, "_h")   # CUDA encoder + CUDA shard
+        # fused when the encoder appends to this index on the device: a CUDA Index, or a MultiIndex with an encoder on
+        # every shard's GPU (TextEncoder.replicate); else encode, then index.add (CPU doubles, f32 shards)
+        can_append = getattr(self.encoder, "can_append", None)
+        fused = bool(can_append and can_append(self.index))
         vecs = None if fused else self.encoder.encode(texts)
         with self._lock:
             gen = self.mutations

@@ -542,6 +542,31 @@ int aur_encode(aur_encoder* enc, const int32_t* tokens, const int32_t* cu_seqlen
 int aur_encode_append(aur_encoder* enc, aur_index* ix, const int32_t* tokens,
                       const int32_t* cu_seqlens, int32_t n_seq, const int64_t* ids,
                       const int32_t* user_codes, const int32_t* org_codes);
+/* A new encoder on `device` (src's own device too) with src's configuration and src's parameters, copied device to device
+ * as stored (the head-dim-32 layouts included; cudaMemcpyPeerAsync, peer access neither required nor enabled), so its
+ * forward is src's bit for bit.  It has its own workspace, stream, tensor maps, lock and stats and outlives src.  src with
+ * a parameter still missing (named as aur_encode names it), device out of range or out NULL: AUR_ERR_INVALID before
+ * anything is allocated. */
+int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out);
+/* aur_encode_append over n (1 .. 64) shards taken as one corpus placed by id mod n (engine.MultiIndex): sequence i is
+ * encoded by encs[ids[i] mod n] and appended to shards[ids[i] mod n].  encs[s] must be on shards[s]'s device; entries of
+ * encs may repeat (shards on one device may share an encoder, which then serves them one batch at a time).  Each shard's
+ * share keeps input order and is cut greedily into batches of at most max_tokens_per_call tokens and max_seqs_per_call
+ * sequences (0: the encoder's max_tokens / max_seqs), appended in that order, so an id repeated in the call keeps its
+ * last occurrence as successive aur_encode_append calls would.  The pooled bf16 rows go into aur_add_dev on the
+ * encoder's stream and never leave the device.  Every shard's share runs on its own host thread, all at once; writers of
+ * one shard are serialised as aur_add_dev serialises them, and searches are never blocked.  Checked before any device
+ * work, leaving every shard and encoder untouched: NULL arguments, n out of range, a NULL or repeated shard, encoders
+ * whose configurations (all but the device) differ or with a parameter missing, an encoder on another device than its
+ * shard, an f32 shard or one whose dim is not the hidden size, per-call limits outside 0 .. the workspace, an id < 0, a
+ * sequence of length outside 1 .. max_pos, a token id outside the vocabulary (AUR_ERR_INVALID); a sequence longer than
+ * one call's token budget, a shard without room for its share (rows appended + share > capacity) (AUR_ERR_NOMEM).  A
+ * concurrent writer of the same shard may still use up its room: that shard's append then fails as aur_add_dev fails.
+ * A failure after device work has started (a CUDA error) may leave a prefix of some shards' shares appended, whole
+ * batches each; aur_last_error names the first failing shard.  aur_encode_append is this call with n = 1 on one batch. */
+int aur_encode_append_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,
+                            const int32_t* cu_seqlens, int32_t n_seq, const int64_t* ids, const int32_t* user_codes,
+                            const int32_t* org_codes, int32_t max_tokens_per_call, int32_t max_seqs_per_call);
 int aur_encoder_get_stats(aur_encoder* enc, aur_encoder_stats* out);
 
 /* ------------------------------------------------------------------ WordPiece tokenizer
