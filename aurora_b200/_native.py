@@ -35,8 +35,8 @@ EXPORTS = [
     "aur_kw_vocab_set_option", "aur_kw_add_text",
     "aur_hybrid_search", "aur_hybrid_search_multi", "aur_hybrid_search_filtered",
     "aur_encoder_open", "aur_encoder_close", "aur_encoder_load", "aur_encode", "aur_encode_append",
-    "aur_encoder_replicate", "aur_encode_append_multi", "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
-    "aur_tokenize", "aur_encode_text_append", "aur_debug_gemm", "aur_debug_attention", "aur_debug_encoder_hidden",
+    "aur_encoder_replicate", "aur_encode_append_multi", "aur_encode_texts", "aur_encode_append_texts_multi", "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
+    "aur_tokenize", "aur_tokenize_windows", "aur_encode_text_append", "aur_debug_gemm", "aur_debug_attention", "aur_debug_encoder_hidden",
 ]
 
 
@@ -173,12 +173,15 @@ def load():
         "aur_encode_append": (C.c_int, [vp, vp, vp, vp, i32, vp, vp, vp]),
         "aur_encoder_replicate": (C.c_int, [vp, i32, C.POINTER(vp)]),
         "aur_encode_append_multi": (C.c_int, [vp, vp, i32, vp, vp, i32, vp, vp, vp, i32, i32]),
+        "aur_encode_texts": (C.c_int, [vp, vp, vp, i32, vp, i32, vp, vp]),
+        "aur_encode_append_texts_multi": (C.c_int, [vp, vp, i32, vp, vp, i32, vp, i32, vp, vp, vp, i32, i32]),
         "aur_encoder_get_stats": (C.c_int, [vp, C.POINTER(AurEncoderStats)]),
         "aur_tokenizer_open": (C.c_int, [C.c_char_p, i32, C.POINTER(vp)]),
         "aur_tokenizer_open_mem": (C.c_int, [C.c_char_p, i64, i32, C.POINTER(vp)]),
         "aur_tokenizer_close": (C.c_int, [vp]),
         "aur_tokenizer_info": (C.c_int, [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]),
         "aur_tokenize": (C.c_int, [vp, C.c_char_p, vp, i32, i32, vp, i64, vp, i32]),
+        "aur_tokenize_windows": (C.c_int, [vp, C.c_char_p, vp, i32, i32, vp, i64, vp, i32, vp, vp, i32]),
         "aur_encode_text_append": (C.c_int, [vp, vp, vp, C.c_char_p, vp, i32, i32, i32, i32, vp, vp, vp, i32]),
         "aur_debug_gemm": (C.c_int, [i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, C.POINTER(C.c_float)]),
         "aur_debug_attention": (C.c_int, [i32, vp, vp, i32, i32, i32, vp, C.POINTER(C.c_float)]),

@@ -6,8 +6,12 @@
 //   inter  [max_tokens_pad, I]    FFN activation
 // and the TMA descriptors over them (activations as GEMM A operands, weights as B operands).
 // A forward is 2 + 7*L + 1 kernel launches on one stream; no CPU compute path exists.  aur_encoder_replicate copies a
-// loaded encoder's parameters to a fresh encoder on any device; aur_encode_append_multi runs one encoder per shard of a
-// multi-GPU corpus, each on its own host thread, the pooled rows going straight into its shard.
+// loaded encoder's parameters to a fresh encoder on any device; aur_encode_append_texts_multi runs one encoder per shard
+// of a multi-GPU corpus, each on its own host thread, the text vectors going straight into its shard.  A text longer than
+// the position table arrives as several windows (sequences); one more launch, window_fold_kernel, turns a batch's window
+// vectors into text vectors, with the running sum of a text still open at the batch's end kept in a carry row:
+//   fold   [max_seqs + 2, H] fp32  text vectors of the batch, then two carry rows (a batch may read one and write the other)
+// (6.3 MB at bge-base dims and the default 2048 sequences).  Batches without such a text launch no fold.
 #include <algorithm>
 #include <functional>
 #include <cuda.h>
@@ -70,6 +74,9 @@ struct aur_encoder {
   int max_items = 0;
   float* d_pool_f32 = nullptr;
   __nv_bfloat16* d_pool_bf16 = nullptr;
+  float* d_fold_f32 = nullptr;                        // [max_seqs + 2, H]: window_fold_kernel's text vectors + 2 carry rows
+  FoldItem* d_fold = nullptr;                         // [max_seqs]
+  FoldItem* h_fold = nullptr;                         // pinned
   float* d_stage = nullptr; size_t stage_elems = 0;   // fp32 staging for parameter upload
   int32_t *h_tok = nullptr, *h_pos = nullptr;          // pinned
   AttnItem* h_items = nullptr;
@@ -117,10 +124,11 @@ void free_all(aur_encoder* e) {
     f(l.ln1_g); f(l.ln1_b); f(l.ln2_g); f(l.ln2_b);
   }
   f(e->x); f(e->y); f(e->qkv); f(e->ctx); f(e->inter);
-  f(e->d_tok); f(e->d_pos); f(e->d_cu); f(e->d_items); f(e->d_pool_f32); f(e->d_pool_bf16); f(e->d_stage);
+  f(e->d_tok); f(e->d_pos); f(e->d_cu); f(e->d_items); f(e->d_pool_f32); f(e->d_pool_bf16); f(e->d_fold_f32); f(e->d_fold); f(e->d_stage);
   if (e->h_tok) cudaFreeHost(e->h_tok);
   if (e->h_pos) cudaFreeHost(e->h_pos);
   if (e->h_items) cudaFreeHost(e->h_items);
+  if (e->h_fold) cudaFreeHost(e->h_fold);
   for (auto& ev : e->ev) if (ev) cudaEventDestroy(ev);
   if (e->stream) cudaStreamDestroy(e->stream);
 }
@@ -240,40 +248,193 @@ bool same_config(const aur_encoder_config& a, const aur_encoder_config& b) {   /
          a.reserved == b.reserved;
 }
 
-// One batch of aur_encode_append_multi: sequences seq[0 .. m) of the caller's packed input (already checked, within the
-// workspace) are staged, encoded, and their pooled bf16 rows appended to ix on the encoder's stream.
-int append_batch(aur_encoder* e, aur_index* ix, const int32_t* tokens, const int32_t* cu, const int32_t* seq, int m,
-                 const int64_t* ids, const int32_t* users, const int32_t* orgs) {
-  std::vector<int32_t> cu_b(static_cast<size_t>(m) + 1, 0), u_b, o_b;
-  std::vector<int64_t> id_b(static_cast<size_t>(m));
-  if (users) u_b.resize(static_cast<size_t>(m));
-  if (orgs) o_b.resize(static_cast<size_t>(m));
-  for (int i = 0; i < m; ++i) {
-    const int32_t s = seq[i];
-    cu_b[i + 1] = cu_b[i] + (cu[s + 1] - cu[s]);
-    id_b[i] = ids[s];
-    if (users) u_b[i] = users[s];
-    if (orgs) o_b[i] = orgs[s];
+// The caller's packed windows: text j is sequences lo(j) .. hi(j) - 1 (one sequence per text without cu_texts).
+struct Texts {
+  const int32_t* tokens;
+  const int32_t* cu;
+  const int32_t* cu_texts;
+  int32_t lo(int32_t j) const { return cu_texts ? cu_texts[j] : j; }
+  int32_t hi(int32_t j) const { return cu_texts ? cu_texts[j + 1] : j + 1; }
+};
+
+// Checks of packed windows against the configuration c, before any device work: every window 1 .. max_pos long and
+// within one call's token budget, every token id in the vocabulary, cu_texts well formed and ending at n_seq.
+int check_texts(const aur_encoder_config& c, const Texts& in, int32_t n_seq, int32_t n_texts, int tok_budget) {
+  if (in.cu[0] != 0) return report_error(AUR_ERR_INVALID, "cu_seqlens[0] must be 0");
+  for (int32_t i = 0; i < n_seq; ++i) {
+    const int len = in.cu[i + 1] - in.cu[i];
+    if (len < 1 || len > c.max_pos) return report_error(AUR_ERR_INVALID, "sequence %d has length %d (1..%d)", i, len, c.max_pos);
+    if (len > tok_budget) return report_error(AUR_ERR_NOMEM, "sequence %d has %d tokens > %d per call", i, len, tok_budget);
+    for (int t = 0; t < len; ++t) {
+      const int32_t id = in.tokens[in.cu[i] + t];
+      if (id < 0 || id >= c.vocab) return report_error(AUR_ERR_INVALID, "token id %d out of range at sequence %d", id, i);
+    }
   }
-  std::lock_guard<std::mutex> g(e->mu);
-  ENC_TRY(cudaSetDevice(e->cfg.device));
-  int n_items = 0;
-  for (int i = 0; i < m; ++i) {
-    const int32_t s = seq[i], len = cu[s + 1] - cu[s], at = cu_b[i];
-    memcpy(e->h_tok + at, tokens + cu[s], sizeof(int32_t) * len);
-    for (int t = 0; t < len; ++t) e->h_pos[at + t] = t;
-    for (int q0 = 0; q0 < len; q0 += 128) e->h_items[n_items++] = AttnItem{at, len, q0, 0};
+  if (in.cu_texts) {
+    if (in.cu_texts[0] != 0) return report_error(AUR_ERR_INVALID, "cu_texts[0] must be 0");
+    for (int32_t j = 0; j < n_texts; ++j)
+      if (in.cu_texts[j + 1] <= in.cu_texts[j]) return report_error(AUR_ERR_INVALID, "text %d has no window (cu_texts must rise)", j);
+    if (in.cu_texts[n_texts] != n_seq)
+      return report_error(AUR_ERR_INVALID, "cu_texts[n_texts] = %d, n_seq = %d", in.cu_texts[n_texts], n_seq);
+  } else if (n_texts != n_seq) {
+    return report_error(AUR_ERR_INVALID, "%d texts of one window each, %d sequences", n_texts, n_seq);
   }
-  int rc = forward_locked(e, cu_b.data(), m, n_items);
-  if (rc == AUR_OK)
-    rc = aur_add_dev(ix, e->d_pool_bf16, id_b.data(), users ? u_b.data() : nullptr, orgs ? o_b.data() : nullptr, m, e->stream);
-  // the pinned staging is reused by the next batch: the stream must be past its copies, whatever happened above
-  const cudaError_t ce = cudaStreamSynchronize(e->stream);
+  return AUR_OK;
+}
+
+// Receives one batch's finished texts q[0 .. n): their bf16 rows are e->d_pool_bf16 [0, n), their fp32 rows f32 [0, n);
+// called on e's stream, under e's lock, before the batch's synchronise.
+using TextSink = std::function<int(aur_encoder* e, const int32_t* q, int n, const float* f32)>;
+
+// Texts q[0 .. nq) (already checked) through e, in order, in greedy batches of at most tok_budget tokens and seq_budget
+// windows; a text's windows may span batches.  A batch with a text of several windows (or one carried in or left open)
+// adds window_fold_kernel after the forward; the running sum of a text left open stays in e's carry row, and e stays
+// locked until that text is finished, so no other caller of e can overwrite it.
+int run_texts(aur_encoder* e, const Texts& in, const int32_t* q, int32_t nq, int tok_budget, int seq_budget, const TextSink& sink) {
+  const int H = e->cfg.hidden;
+  std::unique_lock<std::mutex> lk(e->mu, std::defer_lock);
+  std::vector<int32_t> cu_b, wins;
+  int32_t p = 0, w = nq > 0 ? in.lo(q[0]) : 0;   // next window: w, of text q[p]
+  int slot = 0;                                    // the carry row an open text's sum is read from next
+  while (p < nq) {
+    const int32_t p0 = p;
+    const bool carry_in = w != in.lo(q[p]);
+    wins.clear();
+    int64_t toks = 0;
+    while (p < nq && static_cast<int>(wins.size()) < seq_budget && toks + (in.cu[w + 1] - in.cu[w]) <= tok_budget) {
+      toks += in.cu[w + 1] - in.cu[w];
+      wins.push_back(w);
+      if (++w == in.hi(q[p]) && ++p < nq) w = in.lo(q[p]);
+    }
+    const int m = static_cast<int>(wins.size());
+    const bool open = p < nq && w != in.lo(q[p]);
+    const int n_closed = p - p0, n_fold = n_closed + (open ? 1 : 0);
+    if (!lk.owns_lock()) lk.lock();
+    ENC_TRY(cudaSetDevice(e->cfg.device));
+    cu_b.assign(static_cast<size_t>(m) + 1, 0);
+    int n_items = 0;
+    for (int i = 0; i < m; ++i) {
+      const int32_t len = in.cu[wins[i] + 1] - in.cu[wins[i]], at = cu_b[i];
+      memcpy(e->h_tok + at, in.tokens + in.cu[wins[i]], sizeof(int32_t) * len);
+      for (int t = 0; t < len; ++t) e->h_pos[at + t] = t;
+      for (int q0 = 0; q0 < len; q0 += 128) e->h_items[n_items++] = AttnItem{at, len, q0, 0};
+      cu_b[i + 1] = at + len;
+    }
+    bool fold = false;
+    for (int k = 0, row = 0; k < n_fold; ++k) {
+      const int32_t j = q[p0 + k], first = k == 0 ? wins[0] : in.lo(j), end = k == n_closed ? w : in.hi(j);
+      e->h_fold[k] = FoldItem{row, row + (end - first), in.hi(j) - in.lo(j),
+                              (k == 0 && carry_in ? kFoldCarryIn : 0) | (k == n_closed ? kFoldOpen : 0)};
+      row += end - first;
+      fold |= in.hi(j) - in.lo(j) > 1;
+    }
+    int rc = AUR_OK;
+    if (fold) ENC_TRY(cudaMemcpyAsync(e->d_fold, e->h_fold, sizeof(FoldItem) * n_fold, cudaMemcpyHostToDevice, e->stream));
+    rc = forward_locked(e, cu_b.data(), m, n_items);
+    if (rc == AUR_OK && fold) {
+      float* carry = e->d_fold_f32 + static_cast<size_t>(e->cfg.max_seqs) * H;
+      const cudaError_t ce = launch_window_fold(e->d_pool_f32, e->d_fold, n_fold, H, e->cfg.normalize, carry + slot * H,
+                                                carry + (1 - slot) * H, e->d_fold_f32, e->d_pool_bf16, e->stream);
+      if (open) slot = 1 - slot;
+      if (ce != cudaSuccess) rc = report_error(AUR_ERR_CUDA, "window_fold_kernel: %s", cudaGetErrorString(ce));
+      ++e->stats.launches;
+    }
+    if (rc == AUR_OK && n_closed > 0) rc = sink(e, q + p0, n_closed, fold ? e->d_fold_f32 : e->d_pool_f32);
+    // the pinned staging is reused by the next batch: the stream must be past its copies, whatever happened above
+    const cudaError_t ce = cudaStreamSynchronize(e->stream);
+    if (rc != AUR_OK) return rc;
+    if (ce != cudaSuccess) return report_error(AUR_ERR_CUDA, "encode: %s", cudaGetErrorString(ce));
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]);
+    e->stats.total_ms = ms;
+    if (!open) lk.unlock();
+  }
+  return AUR_OK;
+}
+
+// aur_encode_append_texts_multi, and aur_encode_append_multi with in.cu_texts = NULL (one window per text).
+int append_texts_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const Texts& in, int32_t n_seq,
+                       int32_t n_texts, const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes,
+                       int32_t max_tokens_per_call, int32_t max_seqs_per_call) {
+  constexpr int kMaxShards = 64;
+  if (!encs || !shards) return report_error(AUR_ERR_INVALID, "null argument");
+  if (n < 1 || n > kMaxShards) return report_error(AUR_ERR_INVALID, "n must be in 1 .. %d", kMaxShards);
+  for (int32_t s = 0; s < n; ++s)
+    if (!shards[s] || !encs[s]) return report_error(AUR_ERR_INVALID, "shard or encoder %d is NULL", s);
+  std::vector<aur_index*> order(shards, shards + n);
+  std::sort(order.begin(), order.end(), std::less<aur_index*>());
+  if (std::adjacent_find(order.begin(), order.end()) != order.end()) return report_error(AUR_ERR_INVALID, "a shard is listed twice");
+  const aur_encoder_config& c = encs[0]->cfg;   // fixed at open
+  for (int32_t s = 0; s < n; ++s) {
+    aur_encoder* e = encs[s];
+    if (!same_config(e->cfg, c)) return report_error(AUR_ERR_INVALID, "encoder %d has another configuration than encoder 0", s);
+    {
+      std::lock_guard<std::mutex> g(e->mu);
+      if (!e->missing.empty())
+        return report_error(AUR_ERR_INVALID, "encoder %d parameters not loaded: %s (+%zu more)", s, e->missing[0].c_str(),
+                            e->missing.size() - 1);
+    }
+    if (e->cfg.device != index_device(shards[s]))
+      return report_error(AUR_ERR_INVALID, "encoder %d is on device %d, its shard on device %d", s, e->cfg.device, index_device(shards[s]));
+  }
+  std::vector<aur_stats> st(static_cast<size_t>(n));
+  for (int32_t s = 0; s < n; ++s) {
+    int rc = aur_get_stats(shards[s], &st[s]);
+    if (rc != AUR_OK) return rc;
+    if (st[s].dim != c.hidden || st[s].dtype == AUR_F32)   // (an int8 shard quantizes the bf16 rows as it adds them)
+      return report_error(AUR_ERR_INVALID, "shard %d is %d-d dtype %d; the encoder produces %d-d bf16", s, st[s].dim, st[s].dtype, c.hidden);
+  }
+  if (max_tokens_per_call < 0 || max_tokens_per_call > c.max_tokens || max_seqs_per_call < 0 || max_seqs_per_call > c.max_seqs)
+    return report_error(AUR_ERR_INVALID, "per-call limits must be 0 .. the workspace (%d tokens, %d sequences)", c.max_tokens, c.max_seqs);
+  const int tok_budget = max_tokens_per_call ? max_tokens_per_call : c.max_tokens;
+  const int seq_budget = max_seqs_per_call ? max_seqs_per_call : c.max_seqs;
+  if (n_seq < 0 || n_texts < 0) return report_error(AUR_ERR_INVALID, "n_seq / n_texts < 0");
+  if (n_seq == 0 && n_texts == 0) return AUR_OK;
+  if (!in.tokens || !in.cu || !ids) return report_error(AUR_ERR_INVALID, "tokens, cu_seqlens and ids are required");
+  int rc = check_texts(c, in, n_seq, n_texts, tok_budget);
   if (rc != AUR_OK) return rc;
-  if (ce != cudaSuccess) return report_error(AUR_ERR_CUDA, "encode_append_multi: %s", cudaGetErrorString(ce));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]);
-  e->stats.total_ms = ms;
+  std::vector<std::vector<int32_t>> share(static_cast<size_t>(n));
+  for (int32_t j = 0; j < n_texts; ++j) {
+    if (ids[j] < 0) return report_error(AUR_ERR_INVALID, "ids must be >= 0");
+    share[static_cast<size_t>(ids[j] % n)].push_back(j);
+  }
+  for (int32_t s = 0; s < n; ++s)
+    if (st[s].rows + static_cast<int64_t>(share[s].size()) > st[s].capacity)
+      return report_error(AUR_ERR_NOMEM, "shard %d full: %lld + %zu > capacity %lld (aur_compact reclaims tombstones)", s,
+                          static_cast<long long>(st[s].rows), share[s].size(), static_cast<long long>(st[s].capacity));
+  // each shard's share, in input order, in greedy workspace batches; the shards run on their own host threads
+  std::vector<int> rcs(static_cast<size_t>(n), AUR_OK);
+  std::vector<std::string> errs(static_cast<size_t>(n));
+  auto run = [&](int32_t s) {
+    std::vector<int64_t> id_b;
+    std::vector<int32_t> u_b, o_b;
+    const int r = run_texts(encs[s], in, share[s].data(), static_cast<int32_t>(share[s].size()), tok_budget, seq_budget,
+                            [&](aur_encoder* e, const int32_t* q, int m, const float*) -> int {
+                              id_b.resize(static_cast<size_t>(m));
+                              if (user_codes) u_b.resize(static_cast<size_t>(m));
+                              if (org_codes) o_b.resize(static_cast<size_t>(m));
+                              for (int i = 0; i < m; ++i) {
+                                id_b[i] = ids[q[i]];
+                                if (user_codes) u_b[i] = user_codes[q[i]];
+                                if (org_codes) o_b[i] = org_codes[q[i]];
+                              }
+                              // the rows stay in HBM: the shard copies them device-to-device on the encoder's stream
+                              return aur_add_dev(shards[s], e->d_pool_bf16, id_b.data(), user_codes ? u_b.data() : nullptr,
+                                                 org_codes ? o_b.data() : nullptr, m, e->stream);
+                            });
+    if (r != AUR_OK) {
+      rcs[s] = r;
+      const char* msg = aur_last_error();
+      errs[s] = msg ? msg : "";
+    }
+  };
+  std::vector<std::thread> th;
+  for (int32_t s = 1; s < n; ++s)
+    if (!share[s].empty()) th.emplace_back(run, s);
+  run(0);
+  for (std::thread& t : th) t.join();
+  for (int32_t s = 0; s < n; ++s)
+    if (rcs[s] != AUR_OK) return report_error(rcs[s], "shard %d: %s", s, errs[s].c_str());
   return AUR_OK;
 }
 
@@ -316,11 +477,13 @@ int aur_encoder_open(const aur_encoder_config* cfg, aur_encoder** out) {
   e->max_items = cfg->max_seqs * 4;
   A(&e->d_items, e->max_items);
   A(&e->d_pool_f32, static_cast<size_t>(cfg->max_seqs) * H); A(&e->d_pool_bf16, static_cast<size_t>(cfg->max_seqs) * H);
+  A(&e->d_fold_f32, static_cast<size_t>(cfg->max_seqs + 2) * H); A(&e->d_fold, cfg->max_seqs);
   auto fail_open = [&](int code) { free_all(e); delete e; return code; };
   if (rc != AUR_OK) return fail_open(rc);
   if (cudaMallocHost(reinterpret_cast<void**>(&e->h_tok), sizeof(int32_t) * cfg->max_tokens) != cudaSuccess ||
       cudaMallocHost(reinterpret_cast<void**>(&e->h_pos), sizeof(int32_t) * cfg->max_tokens) != cudaSuccess ||
-      cudaMallocHost(reinterpret_cast<void**>(&e->h_items), sizeof(AttnItem) * e->max_items) != cudaSuccess)
+      cudaMallocHost(reinterpret_cast<void**>(&e->h_items), sizeof(AttnItem) * e->max_items) != cudaSuccess ||
+      cudaMallocHost(reinterpret_cast<void**>(&e->h_fold), sizeof(FoldItem) * cfg->max_seqs) != cudaSuccess)
     return fail_open(report_error(AUR_ERR_NOMEM, "pinned staging allocation failed"));
   if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess)
     return fail_open(report_error(AUR_ERR_CUDA, "cudaStreamCreate failed"));
@@ -472,89 +635,53 @@ int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out) {
   return AUR_OK;
 }
 
+int aur_encode_texts(aur_encoder* e, const int32_t* tokens, const int32_t* cu, int32_t n_seq, const int32_t* cu_texts,
+                     int32_t n_texts, float* out_f32, uint16_t* out_bf16) {
+  if (!e) return report_error(AUR_ERR_INVALID, "null encoder");
+  {
+    std::lock_guard<std::mutex> g(e->mu);
+    if (!e->missing.empty())
+      return report_error(AUR_ERR_INVALID, "encoder parameters not loaded: %s (+%zu more)", e->missing[0].c_str(), e->missing.size() - 1);
+  }
+  if (n_seq < 0 || n_texts < 0) return report_error(AUR_ERR_INVALID, "n_seq / n_texts < 0");
+  if (n_texts == 0 && n_seq == 0) return AUR_OK;
+  if (!tokens || !cu || !cu_texts) return report_error(AUR_ERR_INVALID, "tokens, cu_seqlens and cu_texts are required");
+  const Texts in{tokens, cu, cu_texts};
+  int rc = check_texts(e->cfg, in, n_seq, n_texts, e->cfg.max_tokens);
+  if (rc != AUR_OK) return rc;
+  const size_t H = e->cfg.hidden;
+  // outputs are written only on success: every batch lands in host staging first
+  std::vector<float> f32(out_f32 ? static_cast<size_t>(n_texts) * H : 0);
+  std::vector<uint16_t> bf16(out_bf16 ? static_cast<size_t>(n_texts) * H : 0);
+  std::vector<int32_t> q(static_cast<size_t>(n_texts));
+  for (int32_t j = 0; j < n_texts; ++j) q[j] = j;
+  rc = run_texts(e, in, q.data(), n_texts, e->cfg.max_tokens, e->cfg.max_seqs,
+                 [&](aur_encoder* enc, const int32_t* qs, int n, const float* rows) -> int {
+                   const size_t at = static_cast<size_t>(qs[0]) * H, len = static_cast<size_t>(n) * H;
+                   if (out_f32) ENC_TRY(cudaMemcpyAsync(f32.data() + at, rows, len * sizeof(float), cudaMemcpyDeviceToHost, enc->stream));
+                   if (out_bf16) ENC_TRY(cudaMemcpyAsync(bf16.data() + at, enc->d_pool_bf16, len * 2, cudaMemcpyDeviceToHost, enc->stream));
+                   return AUR_OK;
+                 });
+  if (rc != AUR_OK) return rc;
+  if (out_f32) memcpy(out_f32, f32.data(), f32.size() * sizeof(float));
+  if (out_bf16) memcpy(out_bf16, bf16.data(), bf16.size() * 2);
+  return AUR_OK;
+}
+
+int aur_encode_append_texts_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,
+                                  const int32_t* cu, int32_t n_seq, const int32_t* cu_texts, int32_t n_texts,
+                                  const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes,
+                                  int32_t max_tokens_per_call, int32_t max_seqs_per_call) {
+  if (!cu_texts && n_texts > 0) return report_error(AUR_ERR_INVALID, "cu_texts is required");
+  return append_texts_multi(encs, shards, n, Texts{tokens, cu, cu_texts}, n_seq, n_texts, ids, user_codes, org_codes,
+                            max_tokens_per_call, max_seqs_per_call);
+}
+
 int aur_encode_append_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,
                             const int32_t* cu, int32_t n_seq, const int64_t* ids, const int32_t* user_codes,
                             const int32_t* org_codes, int32_t max_tokens_per_call, int32_t max_seqs_per_call) {
-  constexpr int kMaxShards = 64;
-  if (!encs || !shards) return report_error(AUR_ERR_INVALID, "null argument");
-  if (n < 1 || n > kMaxShards) return report_error(AUR_ERR_INVALID, "n must be in 1 .. %d", kMaxShards);
-  for (int32_t s = 0; s < n; ++s)
-    if (!shards[s] || !encs[s]) return report_error(AUR_ERR_INVALID, "shard or encoder %d is NULL", s);
-  std::vector<aur_index*> order(shards, shards + n);
-  std::sort(order.begin(), order.end(), std::less<aur_index*>());
-  if (std::adjacent_find(order.begin(), order.end()) != order.end()) return report_error(AUR_ERR_INVALID, "a shard is listed twice");
-  const aur_encoder_config& c = encs[0]->cfg;   // fixed at open
-  for (int32_t s = 0; s < n; ++s) {
-    aur_encoder* e = encs[s];
-    if (!same_config(e->cfg, c)) return report_error(AUR_ERR_INVALID, "encoder %d has another configuration than encoder 0", s);
-    {
-      std::lock_guard<std::mutex> g(e->mu);
-      if (!e->missing.empty())
-        return report_error(AUR_ERR_INVALID, "encoder %d parameters not loaded: %s (+%zu more)", s, e->missing[0].c_str(),
-                            e->missing.size() - 1);
-    }
-    if (e->cfg.device != index_device(shards[s]))
-      return report_error(AUR_ERR_INVALID, "encoder %d is on device %d, its shard on device %d", s, e->cfg.device, index_device(shards[s]));
-  }
-  std::vector<aur_stats> st(static_cast<size_t>(n));
-  for (int32_t s = 0; s < n; ++s) {
-    int rc = aur_get_stats(shards[s], &st[s]);
-    if (rc != AUR_OK) return rc;
-    if (st[s].dim != c.hidden || st[s].dtype == AUR_F32)   // (an int8 shard quantizes the bf16 rows as it adds them)
-      return report_error(AUR_ERR_INVALID, "shard %d is %d-d dtype %d; the encoder produces %d-d bf16", s, st[s].dim, st[s].dtype, c.hidden);
-  }
-  if (max_tokens_per_call < 0 || max_tokens_per_call > c.max_tokens || max_seqs_per_call < 0 || max_seqs_per_call > c.max_seqs)
-    return report_error(AUR_ERR_INVALID, "per-call limits must be 0 .. the workspace (%d tokens, %d sequences)", c.max_tokens, c.max_seqs);
-  const int tok_budget = max_tokens_per_call ? max_tokens_per_call : c.max_tokens;
-  const int seq_budget = max_seqs_per_call ? max_seqs_per_call : c.max_seqs;
-  if (n_seq < 0) return report_error(AUR_ERR_INVALID, "n_seq < 0");
-  if (n_seq == 0) return AUR_OK;
-  if (!tokens || !cu || !ids) return report_error(AUR_ERR_INVALID, "tokens, cu_seqlens and ids are required");
-  if (cu[0] != 0) return report_error(AUR_ERR_INVALID, "cu_seqlens[0] must be 0");
-  std::vector<std::vector<int32_t>> share(static_cast<size_t>(n));
-  for (int32_t i = 0; i < n_seq; ++i) {
-    const int len = cu[i + 1] - cu[i];
-    if (len < 1 || len > c.max_pos) return report_error(AUR_ERR_INVALID, "sequence %d has length %d (1..%d)", i, len, c.max_pos);
-    if (len > tok_budget) return report_error(AUR_ERR_NOMEM, "sequence %d has %d tokens > %d per call", i, len, tok_budget);
-    for (int t = 0; t < len; ++t) {
-      const int32_t id = tokens[cu[i] + t];
-      if (id < 0 || id >= c.vocab) return report_error(AUR_ERR_INVALID, "token id %d out of range at sequence %d", id, i);
-    }
-    if (ids[i] < 0) return report_error(AUR_ERR_INVALID, "ids must be >= 0");
-    share[static_cast<size_t>(ids[i] % n)].push_back(i);
-  }
-  for (int32_t s = 0; s < n; ++s)
-    if (st[s].rows + static_cast<int64_t>(share[s].size()) > st[s].capacity)
-      return report_error(AUR_ERR_NOMEM, "shard %d full: %lld + %zu > capacity %lld (aur_compact reclaims tombstones)", s,
-                          static_cast<long long>(st[s].rows), share[s].size(), static_cast<long long>(st[s].capacity));
-  // each shard's share, in input order, in greedy workspace batches; the shards run on their own host threads
-  std::vector<int> rcs(static_cast<size_t>(n), AUR_OK);
-  std::vector<std::string> errs(static_cast<size_t>(n));
-  auto run = [&](int32_t s) {
-    const std::vector<int32_t>& q = share[s];
-    for (size_t i = 0; i < q.size();) {
-      size_t j = i;
-      int64_t toks = 0;
-      while (j < q.size() && static_cast<int>(j - i) < seq_budget && toks + (cu[q[j] + 1] - cu[q[j]]) <= tok_budget)
-        toks += cu[q[j] + 1] - cu[q[j]], ++j;
-      const int rc = append_batch(encs[s], shards[s], tokens, cu, q.data() + i, static_cast<int>(j - i), ids, user_codes, org_codes);
-      if (rc != AUR_OK) {
-        rcs[s] = rc;
-        const char* msg = aur_last_error();
-        errs[s] = msg ? msg : "";
-        return;
-      }
-      i = j;
-    }
-  };
-  std::vector<std::thread> th;
-  for (int32_t s = 1; s < n; ++s)
-    if (!share[s].empty()) th.emplace_back(run, s);
-  run(0);
-  for (std::thread& t : th) t.join();
-  for (int32_t s = 0; s < n; ++s)
-    if (rcs[s] != AUR_OK) return report_error(rcs[s], "shard %d: %s", s, errs[s].c_str());
-  return AUR_OK;
+  return append_texts_multi(encs, shards, n, Texts{tokens, cu, nullptr}, n_seq, n_seq, ids, user_codes, org_codes,
+                            max_tokens_per_call, max_seqs_per_call);
 }
 
 int aur_encoder_get_stats(aur_encoder* e, aur_encoder_stats* out) {

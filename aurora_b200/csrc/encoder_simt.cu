@@ -169,6 +169,49 @@ pool_kernel(const __nv_bfloat16* __restrict__ x, const int32_t* __restrict__ cu,
   }
 }
 
+// One vector per text from its windows' pooled fp32 vectors (aur_encode_texts in include/aurora_b200.h, restated by
+// oracle/window_mean.py).  One warp per text; lane c owns dims c, c + 32, ..  The window sum runs in window order with
+// one rounding per add; the fp64 sum of squares runs per lane in increasing dim, then over the 32 lane sums in lane
+// order (every lane adds the same shuffled values in the same order, so every lane holds the same q).  The _rn
+// intrinsics keep nvcc from contracting any of it.
+__global__ void __launch_bounds__(128)
+window_fold_kernel(const float* __restrict__ pool, const FoldItem* __restrict__ items, int n_items, int hidden,
+                   int normalize, const float* __restrict__ carry_in, float* __restrict__ carry_out, float* __restrict__ out_f32,
+                   __nv_bfloat16* __restrict__ out_bf16) {
+  ptx::grid_dep_launch();
+  ptx::grid_dep_wait();   // pool_kernel's rows
+  const int item = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (item >= n_items) return;
+  const FoldItem it = items[item];
+  const bool from_carry = it.flags & kFoldCarryIn;
+  const float winv = static_cast<float>(it.windows);
+  double q = 0.0;
+  for (int i = lane; i < hidden; i += 32) {
+    float s = from_carry ? carry_in[i] : pool[static_cast<size_t>(it.first) * hidden + i];
+    for (int r = it.first + (from_carry ? 0 : 1); r < it.end; ++r) s = __fadd_rn(s, pool[static_cast<size_t>(r) * hidden + i]);
+    if (it.flags & kFoldOpen) { carry_out[i] = s; continue; }
+    const float m = it.windows == 1 ? s : __fdiv_rn(s, winv);
+    q = __dadd_rn(q, __dmul_rn(static_cast<double>(m), static_cast<double>(m)));
+    out_f32[static_cast<size_t>(item) * hidden + i] = m;
+  }
+  if ((it.flags & kFoldOpen) || !normalize || it.windows == 1) {
+    if (!(it.flags & kFoldOpen))
+      for (int i = lane; i < hidden; i += 32)
+        out_bf16[static_cast<size_t>(item) * hidden + i] = __float2bfloat16_rn(out_f32[static_cast<size_t>(item) * hidden + i]);
+    return;
+  }
+  double tot = 0.0;
+#pragma unroll
+  for (int c = 0; c < 32; ++c) tot = __dadd_rn(tot, __shfl_sync(0xffffffffu, q, c));
+  const double root = tot > 0.0 ? __dsqrt_rn(tot) : 1.0;
+  for (int i = lane; i < hidden; i += 32) {
+    float* o = out_f32 + static_cast<size_t>(item) * hidden + i;
+    const float v = tot > 0.0 ? __double2float_rn(__ddiv_rn(static_cast<double>(*o), root)) : *o;
+    *o = v;
+    out_bf16[static_cast<size_t>(item) * hidden + i] = __float2bfloat16_rn(v);
+  }
+}
+
 __global__ void f32_to_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* __restrict__ out, int64_t n) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i < n) out[i] = __float2bfloat16_rn(in[i]);
@@ -195,6 +238,13 @@ cudaError_t launch_pool(const __nv_bfloat16* x, const int32_t* cu, int n_seq, in
   if (n_seq <= 0) return cudaSuccess;
   const int threads = ((hidden / 2 + 31) / 32) * 32;
   return launch_pdl(pool_kernel, dim3(n_seq), dim3(threads), 0, s, 1, x, cu, hidden, pool_mode, normalize, out_f32, out_bf16);
+}
+
+cudaError_t launch_window_fold(const float* pool_f32, const FoldItem* items, int n_items, int hidden, int normalize,
+                               const float* carry_in, float* carry_out, float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s) {
+  if (n_items <= 0) return cudaSuccess;
+  return launch_pdl(window_fold_kernel, dim3((n_items + 3) / 4), dim3(128), 0, s, 1, pool_f32, items, n_items, hidden,
+                    normalize, carry_in, carry_out, out_f32, out_bf16);
 }
 
 cudaError_t launch_f32_to_bf16(const float* in, __nv_bfloat16* out, int64_t n, cudaStream_t s) {

@@ -294,6 +294,15 @@ cudaError_t launch_layernorm(const __nv_bfloat16* in, const float* g, const floa
 cudaError_t launch_pool(const __nv_bfloat16* x, const int32_t* cu, int n_seq, int hidden, int pool_mode, int normalize,
                         float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s);
 cudaError_t launch_f32_to_bf16(const float* in, __nv_bfloat16* out, int64_t n, cudaStream_t s);
+// One text's share of a batch for window_fold_kernel: pooled rows [first, end) are its windows in this batch; windows is
+// its window count over all batches; kFoldCarryIn: the running sum of its earlier windows is in carry_in;
+// kFoldOpen: its windows continue in the next batch (the sum goes to carry_out, no output).  Item i writes row i.  One
+// batch may finish a carried text and leave another open, so carry_in and carry_out are two rows.
+struct FoldItem { int32_t first, end, windows, flags; };
+constexpr int32_t kFoldCarryIn = 1, kFoldOpen = 2;
+// pool_f32 [n, hidden] window vectors -> out_f32 / out_bf16 [item, hidden] text vectors; carry rows [hidden] fp32.
+cudaError_t launch_window_fold(const float* pool_f32, const FoldItem* items, int n_items, int hidden, int normalize,
+                               const float* carry_in, float* carry_out, float* out_f32, __nv_bfloat16* out_bf16, cudaStream_t s);
 
 // Launch with programmatic dependent launch enabled (and an optional cluster size): the kernel may
 // start its prologue while the previous kernel of the stream drains; it must call

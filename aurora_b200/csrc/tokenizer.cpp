@@ -200,11 +200,10 @@ struct aur_tokenizer {
     }
   }
 
-  // text -> [CLS] pieces [SEP], at most max_len ids.
-  void encode(const unsigned char* s, size_t n, int max_len, std::vector<int32_t>& out) const {
+  // text -> [CLS] pieces [SEP], at most body_max pieces.
+  void encode(const unsigned char* s, size_t n, size_t body_max, std::vector<int32_t>& out) const {
     out.clear();
     out.push_back(cls);
-    const size_t body_max = max_len > 2 ? static_cast<size_t>(max_len - 2) : 0;
     std::vector<uint32_t> word, offs;
     std::string buf;
     auto flush = [&]() {
@@ -243,6 +242,31 @@ struct aur_tokenizer {
     out.push_back(sep);
   }
 };
+
+// Every text through t->encode (at most body_max pieces each) into ids[i]: inline for n_threads == 1 or a handful of
+// texts, otherwise on the tokenizer's resident workers (all host cores up to 64, started on first use); when another
+// caller holds them, inline instead of waiting.
+static void tokenize_all(aur_tokenizer* t, const char* texts_utf8, const int64_t* offsets, int32_t n_texts, size_t body_max,
+                         std::vector<std::vector<int32_t>>& ids, int32_t n_threads) {
+  std::atomic<int32_t> next{0};
+  const std::function<void()> work = [&]() {
+    for (;;) {
+      const int32_t b = next.fetch_add(4);
+      if (b >= n_texts) break;
+      for (int32_t i = b; i < std::min(n_texts, b + 4); ++i)
+        t->encode(reinterpret_cast<const unsigned char*>(texts_utf8) + offsets[i], static_cast<size_t>(offsets[i + 1] - offsets[i]), body_max, ids[i]);
+    }
+  };
+  bool done = false;
+  if (n_threads != 1 && n_texts > 4) {
+    std::call_once(t->pool_once, [&] {
+      const int hw = static_cast<int>(std::thread::hardware_concurrency());
+      t->pool.start(std::max(1, std::min(hw > 0 ? hw : 8, 64) - 1));
+    });
+    done = t->pool.run(work);
+  }
+  if (!done) work();
+}
 
 extern "C" {
 
@@ -302,26 +326,7 @@ int aur_tokenize(aur_tokenizer* t, const char* texts_utf8, const int64_t* offset
     return aur::report_error(AUR_ERR_INVALID, "null argument");
   if (max_len < 2) return aur::report_error(AUR_ERR_INVALID, "max_len must be >= 2 ([CLS] and [SEP])");
   std::vector<std::vector<int32_t>> ids(static_cast<size_t>(n_texts));
-  std::atomic<int32_t> next{0};
-  const std::function<void()> work = [&]() {
-    for (;;) {
-      const int32_t b = next.fetch_add(4);
-      if (b >= n_texts) break;
-      for (int32_t i = b; i < std::min(n_texts, b + 4); ++i)
-        t->encode(reinterpret_cast<const unsigned char*>(texts_utf8) + offsets[i], static_cast<size_t>(offsets[i + 1] - offsets[i]), max_len, ids[i]);
-    }
-  };
-  // n_threads == 1 (or a handful of texts): inline.  Otherwise the tokenizer's resident workers (all host cores up to 64,
-  // started on first use) share the batch; when another caller holds them this call runs inline instead of waiting.
-  bool done = false;
-  if (n_threads != 1 && n_texts > 4) {
-    std::call_once(t->pool_once, [&] {
-      const int hw = static_cast<int>(std::thread::hardware_concurrency());
-      t->pool.start(std::max(1, std::min(hw > 0 ? hw : 8, 64) - 1));
-    });
-    done = t->pool.run(work);
-  }
-  if (!done) work();
+  tokenize_all(t, texts_utf8, offsets, n_texts, static_cast<size_t>(max_len - 2), ids, n_threads);
   int64_t total = 0;
   cu_seqlens_out[0] = 0;
   for (int32_t i = 0; i < n_texts; ++i) {
@@ -334,6 +339,50 @@ int aur_tokenize(aur_tokenizer* t, const char* texts_utf8, const int64_t* offset
     return aur::report_error(AUR_ERR_NOMEM, "tokens_out holds %lld ids, %lld needed (n_texts * max_len always suffices)", (long long)tokens_cap, (long long)total);
   for (int32_t i = 0; i < n_texts; ++i)
     if (!ids[i].empty()) memcpy(tokens_out + cu_seqlens_out[i], ids[i].data(), ids[i].size() * 4);
+  return AUR_OK;
+}
+
+int aur_tokenize_windows(aur_tokenizer* t, const char* texts_utf8, const int64_t* offsets, int32_t n_texts, int32_t max_len,
+                         int32_t* tokens_out, int64_t tokens_cap, int32_t* cu_seqlens_out, int32_t seqs_cap,
+                         int32_t* cu_texts_out, int64_t* totals_out, int32_t n_threads) {
+  if (!t || !offsets || !cu_texts_out || n_texts < 0 || (n_texts > 0 && !texts_utf8 && offsets[n_texts] > 0))
+    return aur::report_error(AUR_ERR_INVALID, "null argument");
+  if (max_len < 3) return aur::report_error(AUR_ERR_INVALID, "max_len must be >= 3 ([CLS], one piece, [SEP])");
+  if (tokens_cap < 0 || seqs_cap < 0) return aur::report_error(AUR_ERR_INVALID, "negative capacity");
+  std::vector<std::vector<int32_t>> ids(static_cast<size_t>(n_texts));
+  tokenize_all(t, texts_utf8, offsets, n_texts, SIZE_MAX, ids, n_threads);   // the whole text: [CLS] b [SEP]
+  const int64_t step = max_len - 2;
+  int64_t windows = 0, total = 0;
+  cu_texts_out[0] = 0;
+  for (int32_t i = 0; i < n_texts; ++i) {
+    const int64_t body = static_cast<int64_t>(ids[i].size()) - 2;
+    const int64_t w = body <= step ? 1 : (body + step - 1) / step;
+    windows += w;
+    total += body + 2 * w;
+    if (windows > 0x7FFFFFFFll || total > 0x7FFFFFFFll) return aur::report_error(AUR_ERR_INVALID, "more than 2^31 windows or tokens in one call");
+    cu_texts_out[i + 1] = static_cast<int32_t>(windows);
+  }
+  if (totals_out) { totals_out[0] = windows; totals_out[1] = total; }
+  if (!tokens_out && tokens_cap == 0 && !cu_seqlens_out && seqs_cap == 0) return AUR_OK;   // count mode
+  if (windows > seqs_cap || total > tokens_cap || !cu_seqlens_out || (total > 0 && !tokens_out))
+    return aur::report_error(AUR_ERR_NOMEM, "%lld windows of %lld tokens, the buffers hold %d and %lld", (long long)windows,
+                             (long long)total, seqs_cap, (long long)tokens_cap);
+  int64_t at = 0, k = 0;
+  cu_seqlens_out[0] = 0;
+  for (int32_t i = 0; i < n_texts; ++i) {
+    const std::vector<int32_t>& v = ids[i];
+    const int64_t body = static_cast<int64_t>(v.size()) - 2;
+    int64_t b = 0;
+    do {   // [CLS] b[b0 : b0 + step] [SEP]; a text that fits is one window, aur_tokenize's output
+      const int64_t len = std::min(step, body - b);
+      tokens_out[at] = v.front();
+      if (len > 0) memcpy(tokens_out + at + 1, v.data() + 1 + b, static_cast<size_t>(len) * 4);
+      tokens_out[at + 1 + len] = v.back();
+      at += len + 2;
+      cu_seqlens_out[++k] = static_cast<int32_t>(at);
+      b += step;
+    } while (b < body);
+  }
   return AUR_OK;
 }
 

@@ -124,6 +124,20 @@ class Encoder:
                                      _ptr(out) if bf16 else None))
         return out
 
+    def encode_texts(self, tokens: np.ndarray, cu_seqlens: np.ndarray, cu_texts: np.ndarray, bf16: bool = False) -> np.ndarray:
+        """aur_encode_texts: [n_texts, hidden] float32 (raw bf16 bits as uint16 when ``bf16``), text j the vector of windows
+        cu_texts[j] .. cu_texts[j + 1] - 1 (its one window's, or their mean, DESIGN.md section 4.5); any number of
+        windows, batched through the workspace inside the library."""
+        tokens = np.ascontiguousarray(tokens, dtype=np.int32)
+        cu = np.ascontiguousarray(cu_seqlens, dtype=np.int32)
+        ct = np.ascontiguousarray(cu_texts, dtype=np.int32)
+        if cu.ndim != 1 or cu.size < 1 or ct.ndim != 1 or ct.size < 1 or tokens.ndim != 1 or tokens.size != int(cu[-1]):
+            raise ValueError("tokens [total], cu_seqlens [n_seq + 1] with cu[-1] == total and cu_texts [n_texts + 1] are required")
+        out = np.empty((ct.size - 1, self.cfg.hidden), dtype=np.uint16 if bf16 else np.float32)
+        N.check(self._lib.aur_encode_texts(self._h, _ptr(tokens), _ptr(cu), cu.size - 1, _ptr(ct), ct.size - 1,
+                                           None if bf16 else _ptr(out), _ptr(out) if bf16 else None))
+        return out
+
     def encode(self, seqs: Sequence[Sequence[int]]) -> np.ndarray:
         """Token-id lists of any count: split into calls that fit the workspace."""
         out = np.empty((len(seqs), self.cfg.hidden), dtype=np.float32)
@@ -163,10 +177,12 @@ class Encoder:
 
 def encode_append_multi(encoders: Sequence[Encoder], shards, tokens: np.ndarray, cu_seqlens: np.ndarray, ids: np.ndarray,
                         user_codes: Optional[np.ndarray] = None, org_codes: Optional[np.ndarray] = None,
-                        max_tokens_per_call: int = 0, max_seqs_per_call: int = 0) -> None:
+                        max_tokens_per_call: int = 0, max_seqs_per_call: int = 0, cu_texts: Optional[np.ndarray] = None) -> None:
     """aur_encode_append_multi: packed sequences encoded and appended to ``shards`` (``engine.Index`` on their encoders'
     devices) placed by ``id mod len(shards)``, sequence i by ``encoders[ids[i] % n]``; every shard's share at once,
-    in workspace batches (0 = the encoder's workspace)."""
+    in workspace batches (0 = the encoder's workspace).  With ``cu_texts`` (aur_encode_append_texts_multi) the unit is
+    the text: text j is windows cu_texts[j] .. cu_texts[j + 1] - 1, stored as ``Encoder.encode_texts`` gives it, and
+    ids / user_codes / org_codes are per text."""
     n = len(shards)
     if len(encoders) != n:
         raise ValueError(f"{len(encoders)} encoders for {n} shards")
@@ -174,16 +190,22 @@ def encode_append_multi(encoders: Sequence[Encoder], shards, tokens: np.ndarray,
     cu = np.ascontiguousarray(cu_seqlens, dtype=np.int32)
     if cu.ndim != 1 or cu.size < 1 or tokens.ndim != 1 or tokens.size != int(cu[-1]):
         raise ValueError("tokens [total] and cu_seqlens [n_seq + 1] with cu[-1] == total are required")
+    ct = None if cu_texts is None else np.ascontiguousarray(cu_texts, dtype=np.int32)
+    n_units = cu.size - 1 if ct is None else ct.size - 1
     ids = np.ascontiguousarray(ids, dtype=np.int64)
-    if ids.shape != (cu.size - 1,):
-        raise ValueError("ids must be [n_seq]")
+    if ids.shape != (n_units,):
+        raise ValueError("ids must be [n_seq] ([n_texts] with cu_texts)")
     u = None if user_codes is None else np.ascontiguousarray(user_codes, dtype=np.int32)
     o = None if org_codes is None else np.ascontiguousarray(org_codes, dtype=np.int32)
     encs = (C.c_void_p * n)(*[e._h.value for e in encoders])
     hs = (C.c_void_p * n)(*[sh._h.value for sh in shards])
     lib = N.load()
-    N.check(lib.aur_encode_append_multi(encs, hs, n, _ptr(tokens), _ptr(cu), cu.size - 1, _ptr(ids), _ptr(u), _ptr(o),
-                                        int(max_tokens_per_call), int(max_seqs_per_call)))
+    if ct is None:
+        N.check(lib.aur_encode_append_multi(encs, hs, n, _ptr(tokens), _ptr(cu), cu.size - 1, _ptr(ids), _ptr(u), _ptr(o),
+                                            int(max_tokens_per_call), int(max_seqs_per_call)))
+    else:
+        N.check(lib.aur_encode_append_texts_multi(encs, hs, n, _ptr(tokens), _ptr(cu), cu.size - 1, _ptr(ct), n_units, _ptr(ids),
+                                                  _ptr(u), _ptr(o), int(max_tokens_per_call), int(max_seqs_per_call)))
 
 
 class TextEncoder:
@@ -199,7 +221,9 @@ class TextEncoder:
     Texts longer than the position table (the reference's chunker can emit a 4 000-character chunk,
     document_processor.py:266-267) are not cut off: they are split into windows of ``max_pos`` tokens, each window is
     encoded, and the text's vector is the L2-normalised mean of its windows -- the same idea as the t2v sidecar's
-    sentence batching + averaging (that container's exact splitting rule is not in the reference tree)."""
+    sentence batching + averaging (that container's exact splitting rule is not in the reference tree).  Windows,
+    forward, mean and append all stay in the library and on the device (``aur_tokenize_windows``, ``aur_encode_texts``,
+    ``aur_encode_append_texts_multi``; the arithmetic is in DESIGN.md section 4.5)."""
 
     def __init__(self, encoder: Encoder, tokenizer, max_len: Optional[int] = None):
         self._enc, self._tok = encoder, tokenizer
@@ -232,105 +256,46 @@ class TextEncoder:
                                     and sh.device in self._encs for sh in shards)
 
     # ------------------------------------------------------------------ tokenisation
-    def _tokenize(self, texts: Sequence[str], max_len: int):
+    def _tokenize_windows(self, texts: Sequence[str]):
+        """(tokens, cu_seqlens over windows, cu_texts): one C call with the native tokenizer, ``_windows`` per text
+        with a callable one."""
         if self._native:
-            return self._tok.encode_packed(list(texts), max_len)
-        seqs = []
-        for t in texts:
-            ids = list(self._tok(t))
-            seqs.append(ids if len(ids) <= max_len else ids[: max_len - 1] + ids[-1:])
-        return pack_sequences(seqs)
-
-    def _over_long(self, texts: Sequence[str], lens: np.ndarray) -> List[int]:
-        """Indices of the texts whose full tokenisation exceeds the position table.  Only texts that came back at
-        exactly ``max_len`` ids can have been truncated; those are re-measured without the limit -- with the native
-        tokenizer in ONE C call for all of them."""
-        cand = [int(i) for i in np.nonzero(np.asarray(lens) >= self.max_len)[0]]
-        if not cand:
-            return []
-        if self._native and hasattr(self._tok, "lengths"):
-            full = self._tok.lengths([texts[i] for i in cand])
-            return [i for i, n in zip(cand, full) if n > self.max_len]
-        return [i for i in cand if len(self._windows(texts[i])) > 1]
+            return self._tok.encode_windows(list(texts), self.max_len)
+        wins = [self._windows(t) for t in texts]
+        cu_texts = np.zeros(len(texts) + 1, dtype=np.int32)
+        cu_texts[1:] = np.cumsum([len(w) for w in wins])
+        tok, cu = pack_sequences([s for w in wins for s in w])
+        return tok, cu, cu_texts
 
     def _windows(self, text: str):
-        """Token windows of one over-long text: [CLS] body[i : i + max_len - 2] [SEP]."""
-        tok, cu = self._tokenize([text], 1 << 20) if self._native else pack_sequences([list(self._tok(text))])
+        """Token windows of one text: [CLS] body[i : i + max_len - 2] [SEP] for i = 0, max_len - 2, ... (one window
+        when the text fits).  The Python statement of aur_tokenize_windows' rule."""
+        if self._native:
+            tok, cu = self._tok.encode_packed([text], int(self._tok.lengths([text], max_len=0x7FFFFFFF)[0]))   # the whole text
+        else:
+            tok, cu = pack_sequences([list(self._tok(text))])
         ids = tok[cu[0]:cu[1]]
         cls, sep, body = ids[0], ids[-1], ids[1:-1]
         step = self.max_len - 2
         return [np.concatenate(([cls], body[i:i + step], [sep])).astype(np.int32) for i in range(0, max(len(body), 1), step)]
 
-    def _encode_packed_any(self, tok: np.ndarray, cu: np.ndarray) -> np.ndarray:
-        out = np.empty((len(cu) - 1, self.dim), dtype=np.float32)
-        i = 0
-        while i < len(cu) - 1:
-            j = i
-            while j < len(cu) - 1 and j - i < self._enc.max_seqs and cu[j + 1] - cu[i] <= self._enc.max_tokens:
-                j += 1
-            if j == i:
-                raise ValueError(f"text {i} tokenizes to {cu[i + 1] - cu[i]} tokens: more than max_tokens={self._enc.max_tokens}")
-            out[i:j] = self._enc.encode_packed(tok[cu[i]:cu[j]], (cu[i:j + 1] - cu[i]).astype(np.int32))
-            i = j
-        return out
-
-    def _encode_long(self, text: str) -> np.ndarray:
-        return self._encode_long_many([text])[0]
-
-    def _encode_long_many(self, texts: Sequence[str]) -> np.ndarray:
-        """Vectors of over-long texts: all their windows go through the encoder as ONE packed batch, then each text's
-        windows are averaged (and re-normalised when the encoder normalises)."""
-        wins, owner = [], []
-        for t, text in enumerate(texts):
-            w = self._windows(text)
-            wins += w
-            owner += [t] * len(w)
-        tok, cu = pack_sequences(wins)
-        vecs = self._encode_packed_any(tok, cu)
-        owner = np.asarray(owner)
-        out = np.empty((len(texts), self.dim), dtype=np.float32)
-        for t in range(len(texts)):
-            v = vecs[owner == t].mean(axis=0)
-            n = float(np.linalg.norm(v))
-            out[t] = v / n if (self._enc.cfg.normalize and n > 0) else v
-        return out
-
     # ------------------------------------------------------------------ API used by the retriever
     def encode(self, texts: Sequence[str]) -> np.ndarray:
-        tok, cu = self._tokenize(texts, self.max_len)
-        out = self._encode_packed_any(tok, cu)
-        long_ones = self._over_long(texts, np.diff(cu))               # truncated above: windows, averaged
-        if long_ones:
-            out[long_ones] = self._encode_long_many([texts[i] for i in long_ones])
-        return out
+        """[len(texts), dim] float32: one tokenisation and one aur_encode_texts call (windows, batches and the mean of
+        an over-long text's windows inside the library)."""
+        return self._enc.encode_texts(*self._tokenize_windows(texts))
 
     def encode_append(self, index, texts: Sequence[str], ids: np.ndarray, user_codes=None, org_codes=None) -> None:
-        """Tokenise once (one multi-threaded C call with the native tokenizer), then ONE aur_encode_append_multi call
-        for every text that fits the position table: workspace batches, encoder forward and shard append inside the
-        library, each shard's share on its own device (``can_append`` says which indexes qualify); nothing runs per
-        text or per batch in Python.  Over-long texts are averaged over their windows on the host and added with
-        ``index.add``."""
+        """Tokenise once (one multi-threaded C call with the native tokenizer), then ONE aur_encode_append_texts_multi
+        call: workspace batches, encoder forward, the mean of an over-long text's windows and the shard append inside
+        the library, each shard's share on its own device in input order (``can_append`` says which indexes qualify);
+        nothing runs per text or per batch in Python and no vector leaves the device."""
         if not self.can_append(index):
             raise ValueError("encode_append needs bf16 or int8 engine.Index shards on devices this encoder has replicas on")
-        ids = np.ascontiguousarray(ids, dtype=np.int64)
-        tok, cu = self._tokenize(texts, self.max_len)
-        lens = np.diff(cu)
-        long_ones = self._over_long(texts, lens)
-        u = None if user_codes is None else np.ascontiguousarray(user_codes, dtype=np.int32)
-        o = None if org_codes is None else np.ascontiguousarray(org_codes, dtype=np.int32)
-        t, c, i_, u_, o_ = tok, cu, ids, u, o
-        if long_ones:                                                 # drop them from the packed buffer
-            keep = np.ones(len(texts), dtype=bool)
-            keep[long_ones] = False
-            t = tok[np.repeat(keep, lens)]
-            c = np.zeros(int(keep.sum()) + 1, dtype=np.int32)
-            np.cumsum(lens[keep], out=c[1:])
-            i_, u_, o_ = ids[keep], None if u is None else u[keep], None if o is None else o[keep]
+        tok, cu, cu_texts = self._tokenize_windows(texts)
         shards = self._shards(index)
-        encode_append_multi([self._encs[sh.device] for sh in shards], shards, t, c, i_, u_, o_)
-        if long_ones:                                                 # averaged windows: the vectors are formed on the host
-            v = self._encode_long_many([texts[i] for i in long_ones])
-            index.add(v, ids[long_ones], None if u is None else u[long_ones], None if o is None else o[long_ones])
+        encode_append_multi([self._encs[sh.device] for sh in shards], shards, tok, cu, ids, user_codes, org_codes,
+                            cu_texts=cu_texts)
 
     def _append_texts_native(self, index, texts, ids, u, o) -> None:
         """The same ingest as ONE C call (aur_encode_text_append: tokenise + batches + append inside the library), for

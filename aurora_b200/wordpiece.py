@@ -177,6 +177,33 @@ class NativeTokenizer:
                                              cu.ctypes.data_as(C.c_void_p), int(threads)))
         return np.diff(cu)
 
+    def encode_windows(self, texts, max_len: int = 512, threads: int = 0):
+        """(tokens int32 [total], cu_seqlens int32 [windows + 1], cu_texts int32 [n + 1]): every text's whole
+        tokenisation [CLS] b [SEP] as windows for a position table of ``max_len`` (``aur_tokenize_windows``): one window,
+        ``encode_packed``'s, when it fits; otherwise [CLS] b[i : i + max_len - 2] [SEP] for i = 0, max_len - 2, ...
+        Text j is windows cu_texts[j] .. cu_texts[j + 1] - 1.  One C call (two if a text tokenises to more ids than it
+        has bytes, which the first call's buffers assume it does not)."""
+        import ctypes as C
+
+        import numpy as np
+
+        blob, offs = self._pack(texts)
+        n = len(offs) - 1
+        seqs = 2 * n + len(blob) // max(1, int(max_len) - 2)
+        toks = len(blob) + 2 * seqs
+        cu_texts = np.zeros(n + 1, dtype=np.int32)
+        totals = np.zeros(2, dtype=np.int64)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)      # noqa: E731
+        for _ in range(2):
+            tokens, cu = np.empty(max(1, toks), dtype=np.int32), np.zeros(seqs + 1, dtype=np.int32)
+            rc = self._lib.aur_tokenize_windows(self._h, blob, vp(offs), n, int(max_len), vp(tokens), tokens.size, vp(cu), seqs,
+                                                vp(cu_texts), vp(totals), int(threads))
+            if rc != self._N.AUR_ERR_NOMEM:
+                break
+            seqs, toks = int(totals[0]), int(totals[1])
+        self._N.check(rc)
+        return tokens[: int(totals[1])], cu[: int(totals[0]) + 1], cu_texts
+
     def encode_batch(self, texts, max_len: int = 512) -> List[List[int]]:
         tok, cu = self.encode_packed(texts, max_len)
         return [tok[cu[i]:cu[i + 1]].tolist() for i in range(len(cu) - 1)]

@@ -567,6 +567,29 @@ int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out);
 int aur_encode_append_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,
                             const int32_t* cu_seqlens, int32_t n_seq, const int64_t* ids, const int32_t* user_codes,
                             const int32_t* org_codes, int32_t max_tokens_per_call, int32_t max_seqs_per_call);
+/* Texts of any length in, one vector per text out.  A text is windows cu_texts[j] .. cu_texts[j+1]-1 of the packed
+ * sequences (aur_tokenize_windows' layout): cu_texts [n_texts + 1] starts at 0, rises by at least 1 per text and ends at
+ * n_seq.  The windows go through the workspace in greedy batches, in order; a text's windows may span batches, its fp32
+ * running sum then stays on the device from one batch to the next (the encoder is held for that long).  A text of one
+ * window gets aur_encode's vector for that sequence, bit for bit.  A text of w >= 2 windows with pooled vectors
+ * v_1 .. v_w (each normalised when the encoder normalises) gets, per component and never fused:
+ *   s = fl32(..fl32(v_1 + v_2) .. + v_w), m = fl32(s / w);
+ *   normalize: q = sum of the exact fp64 squares m_i^2, summed in fp64 as lane sums r_c = m_c^2 + m_{c+32}^2 + .. (in
+ *   increasing i) for c = 0 .. 31, then r_0 + r_1 + .. + r_31; out_i = fl32(m_i / sqrt(q)) in fp64 when q > 0, else m;
+ *   without normalize, out = m.  The bf16 row rounds out to nearest even (oracle/window_mean.py restates this).
+ * out_f32 / out_bf16 [n_texts, hidden] (either may be NULL) are written only on success.  Checked before any device
+ * work: the checks of aur_encode_append_multi that apply, and cu_texts (AUR_ERR_INVALID). */
+int aur_encode_texts(aur_encoder* enc, const int32_t* tokens, const int32_t* cu_seqlens, int32_t n_seq,
+                     const int32_t* cu_texts, int32_t n_texts, float* out_f32, uint16_t* out_bf16);
+/* aur_encode_append_multi with texts as the unit: text j (its windows, cu_texts as for aur_encode_texts) is encoded by
+ * encs[ids[j] mod n] into the vector aur_encode_texts gives it and appended, as bf16, to shards[ids[j] mod n]; each
+ * shard's rows are appended in input order; room is counted in texts; ids, user_codes and org_codes are [n_texts].  The
+ * checks, threads and failure behaviour are aur_encode_append_multi's, plus a malformed cu_texts (AUR_ERR_INVALID).
+ * aur_encode_append_multi is this call with one window per text. */
+int aur_encode_append_texts_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,
+                                  const int32_t* cu_seqlens, int32_t n_seq, const int32_t* cu_texts, int32_t n_texts,
+                                  const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes,
+                                  int32_t max_tokens_per_call, int32_t max_seqs_per_call);
 int aur_encoder_get_stats(aur_encoder* enc, aur_encoder_stats* out);
 
 /* ------------------------------------------------------------------ WordPiece tokenizer
@@ -584,6 +607,15 @@ int aur_tokenizer_info(aur_tokenizer* t, int32_t* vocab_size, int32_t* unk_id, i
  * tokens_cap = 0 asks for the lengths only (cu_seqlens_out is filled, no ids are written). */
 int aur_tokenize(aur_tokenizer* t, const char* texts_utf8, const int64_t* offsets, int32_t n_texts, int32_t max_len,
                  int32_t* tokens_out, int64_t tokens_cap, int32_t* cu_seqlens_out, int32_t n_threads);
+/* Every text as the windows of its whole tokenisation [CLS] b [SEP] for a position table of max_len (>= 3): one window,
+ * aur_tokenize's output, when 2 + |b| <= max_len; otherwise [CLS] b[i : i + max_len - 2] [SEP] for i = 0, max_len - 2,
+ * .. < |b|.  Packed: tokens_out (capacity tokens_cap ids), cu_seqlens_out [windows + 1] over windows (capacity seqs_cap
+ * windows) and cu_texts_out [n_texts + 1] (text j = windows cu_texts[j] .. cu_texts[j+1]-1).  totals_out [2] (may be
+ * NULL) receives the windows and tokens needed.  tokens_out = cu_seqlens_out = NULL with both capacities 0 is count mode
+ * (cu_texts_out and totals_out only); capacities too small: AUR_ERR_NOMEM, with cu_texts_out and totals_out written. */
+int aur_tokenize_windows(aur_tokenizer* t, const char* texts_utf8, const int64_t* offsets, int32_t n_texts, int32_t max_len,
+                         int32_t* tokens_out, int64_t tokens_cap, int32_t* cu_seqlens_out, int32_t seqs_cap,
+                         int32_t* cu_texts_out, int64_t* totals_out, int32_t n_threads);
 /* Text in, rows in the shard: tokenise, encoder forward, append -- insert_chunks (weaviate_client.py:136-212) without
  * Python on the path.  Batches are cut to max_tokens_per_call / max_seqs_per_call (the encoder's workspace). */
 int aur_encode_text_append(aur_encoder* enc, aur_tokenizer* tok, aur_index* ix, const char* texts_utf8,
