@@ -284,7 +284,7 @@ bool direct_outputs(float* scores_out, int64_t* ids_out, float** d_scores, int64
 
 // One call with host buffers: the index's shared lock, its device, an idle pool context locked for the call and given
 // back when the call ends, the context's own stream, and the prefix published when the call began (open()).  A search
-// call stages its queries and outputs with stage() and ends with finish().
+// call stages its queries and outputs with stage().
 struct HostCall {
   aur_index* ix;
   std::shared_lock<std::shared_mutex> rl;
@@ -313,7 +313,8 @@ struct HostCall {
     n_rows = ix->rows_pub.load(std::memory_order_acquire);
     return AUR_OK;
   }
-  // Uploads the queries to c->stage_q and picks the outputs (direct_outputs).
+  // Uploads the queries to c->stage_q and picks the outputs: the caller's host buffers when both are given, page-locked
+  // and mapped (direct_outputs), else the staging buffers.
   int stage(const void* queries_host, int32_t nq, int32_t k, float* scores_out, int64_t* ids_out) {
     const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->qelt;
     const size_t nout = static_cast<size_t>(nq) * k;
@@ -323,19 +324,7 @@ struct HostCall {
     CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
     d_scores = c->stage_scores.p;
     d_ids = c->stage_ids.p;
-    direct = direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
-    return AUR_OK;
-  }
-  // Ends a search whose enqueue returned rc.  The caller's buffers are written only when every kernel of the search was
-  // enqueued successfully; on any failure the stream drains and they are left untouched.
-  int finish(int rc, int32_t nq, int32_t k, float* scores_out, int64_t* ids_out) {
-    if (rc != AUR_OK) { cudaStreamSynchronize(s); return rc; }
-    if (!direct) {   // into the caller's pageable buffers
-      const size_t nout = static_cast<size_t>(nq) * k;
-      CU_TRY(cudaMemcpyAsync(scores_out, c->stage_scores.p, nout * 4, cudaMemcpyDeviceToHost, s));
-      CU_TRY(cudaMemcpyAsync(ids_out, c->stage_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
-    }
-    CU_TRY(cudaStreamSynchronize(s));
+    direct = scores_out && ids_out && direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
     return AUR_OK;
   }
 };
@@ -712,43 +701,6 @@ int stage_tenant_scope(SearchCtx* c, cudaStream_t s, int32_t nq, const int32_t* 
   return AUR_OK;
 }
 
-// Host-buffer search: H2D of the queries, kernels, D2H of the results on a pool context's own stream.
-int search_host(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user, const int32_t* q_org,
-                const int64_t* allow_ids, int64_t n_allow, float* scores_out, int64_t* ids_out, int64_t* snapshot_out) {
-  int rc = check_search_args(ix, queries_host, nq, k, scores_out, ids_out);
-  if (rc != AUR_OK) return rc;
-  const bool subset = allow_ids || n_allow > 0;
-  if (subset && (n_allow < 0 || (n_allow > 0 && !allow_ids))) return fail(AUR_ERR_INVALID, "allow_ids / n_allow");
-  if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
-  HostCall call(ix);
-  if ((rc = call.open()) != AUR_OK) return rc;
-  SearchCtx* c = call.c;
-  cudaStream_t s = call.s;
-  const int64_t n_rows = call.n_rows;
-  if ((rc = call.stage(queries_host, nq, k, scores_out, ids_out)) != AUR_OK) return rc;
-  Scope sc;
-  int32_t scope[2] = {0, -1};
-  std::vector<int32_t> rows_host;
-  if (subset) {
-    // resolved metadata pre-filter: ids -> rows of the published prefix (unknown / newer ids drop out)
-    rows_host.reserve(static_cast<size_t>(n_allow));
-    resolve_ids(ix, allow_ids, n_allow, n_rows, [&](int64_t, int32_t row) { rows_host.push_back(row); });
-    CU_TRY(c->allow_rows.reserve(rows_host.size() + 1));
-    if (!rows_host.empty())
-      CU_TRY(cudaMemcpyAsync(c->allow_rows.p, rows_host.data(), rows_host.size() * 4, cudaMemcpyHostToDevice, s));
-    sc.allow_rows = c->allow_rows.p;
-    sc.n_allow = static_cast<int64_t>(rows_host.size());
-  } else if (q_user && (rc = stage_tenant_scope(c, s, nq, q_user, q_org, scope, &sc)) != AUR_OK) {
-    return rc;
-  }
-  rc = stats_begin(c, s, nq, n_rows);
-  if (rc == AUR_OK) rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, call.d_scores, call.d_ids, nullptr, s);
-  if (rc == AUR_OK) rc = stats_end(ix, c, s);
-  if ((rc = call.finish(rc, nq, k, scores_out, ids_out)) != AUR_OK) return rc;
-  if (snapshot_out) *snapshot_out = n_rows;
-  return AUR_OK;
-}
-
 // Search with a pre-filter list per query (aur_search_lists).  The batch runs in blocks of kListQBlock queries (one
 // dense candidate buffer each, as on the generic path); a block's work items are (list, <= kListQMax of its queries
 // naming that list, kSimtSeg-row segment of the list), launched in batches whose score scratch stays within
@@ -953,49 +905,72 @@ int filtered_search(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t nq, int
   return run_list_search(ix, c, s, pl, nq, k, c->filt_rows.p, scores, ids);
 }
 
-}  // namespace
-
-namespace aur {
-int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
-              const int32_t* q_org, float* scores, int64_t* ids, int64_t* snapshot_rows) {
-  if (ix->dtype == AUR_F32) return fail(AUR_ERR_UNSUPPORTED, "hybrid search needs a bf16 or int8 index");
-  if (ix->device != device) return fail(AUR_ERR_INVALID, "the keyword store is on device %d, the index on device %d", device, ix->device);
-  int rc = check_batch(nq, k);
-  if (rc != AUR_OK) return rc;
-  std::shared_lock<std::shared_mutex> rl(ix->rw);   // (compaction waits for the device before it moves a row)
-  CU_TRY(cudaSetDevice(ix->device));
-  SearchCtx* c = nullptr;
-  if ((rc = acquire_ctx(ix, s, &c)) != AUR_OK) return rc;
-  std::lock_guard<std::mutex> cl(c->mu);
-  const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
-  const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->qelt;
-  CU_TRY(c->stage_q.reserve(qbytes));
-  CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
+// One shard's part of dense_legs: its call, its scope as the search reads it, and with programs every program's number
+// of matching rows.
+struct DensePart {
+  std::unique_ptr<HostCall> call;
   Scope sc;
-  int32_t scope[2] = {0, -1};
-  if (q_user && (rc = stage_tenant_scope(c, s, nq, q_user, q_org, scope, &sc)) != AUR_OK) return rc;
-  if ((rc = stats_begin(c, s, nq, n_rows)) != AUR_OK) return rc;
-  if ((rc = search_enqueue(ix, c, c->stage_q.p, nq, k, sc, n_rows, scores, ids, nullptr, s)) != AUR_OK) return rc;
-  if ((rc = stats_end(ix, c, s)) != AUR_OK) return rc;
-  *snapshot_rows = n_rows;
+  int32_t scope[2] = {0, -1};     // the batch's one tenant scope (sc.uniform)
+  std::vector<int32_t> allow;     // the allow-ids' rows
+  ListPlan pl;                    // the lists' rows and work items
+  std::vector<int64_t> tot;
+};
+
+// The host side of a staged call's scope: the tenant codes staged, the allow-ids resolved to rows of the published
+// prefix, or the lists resolved and planned.  Programs need nothing before their count pass.
+int prepare_scope(const DenseQuery& q, DensePart* pt) {
+  HostCall& call = *pt->call;
+  SearchCtx* c = call.c;
+  if (q.n_allow >= 0) {
+    // resolved metadata pre-filter: ids -> rows of the published prefix (unknown / newer ids drop out)
+    pt->allow.reserve(static_cast<size_t>(q.n_allow));
+    resolve_ids(call.ix, q.allow_ids, q.n_allow, call.n_rows, [&](int64_t, int32_t row) { pt->allow.push_back(row); });
+    CU_TRY(c->allow_rows.reserve(pt->allow.size() + 1));
+    if (!pt->allow.empty())
+      CU_TRY(cudaMemcpyAsync(c->allow_rows.p, pt->allow.data(), pt->allow.size() * 4, cudaMemcpyHostToDevice, call.s));
+    pt->sc.allow_rows = c->allow_rows.p;
+    pt->sc.n_allow = static_cast<int64_t>(pt->allow.size());
+    return AUR_OK;
+  }
+  if (q.q_list) {
+    // staging (int32): [every named list's rows of the published prefix, sorted, once each][the plan's blocks]
+    ListPlan& pl = pt->pl;
+    std::vector<char> named(static_cast<size_t>(q.n_lists), 0);
+    for (int32_t i = 0; i < q.nq; ++i) named[static_cast<size_t>(q.q_list[i])] = 1;
+    std::vector<int64_t> lrow0(static_cast<size_t>(q.n_lists), 0), llen(static_cast<size_t>(q.n_lists), 0);
+    for (int32_t l = 0; l < q.n_lists; ++l) {
+      const size_t r0 = pl.stage.size();
+      lrow0[static_cast<size_t>(l)] = static_cast<int64_t>(r0);
+      if (!named[static_cast<size_t>(l)]) continue;
+      resolve_ids(call.ix, q.list_ids + q.list_offsets[l], q.list_offsets[l + 1] - q.list_offsets[l], call.n_rows,
+                  [&](int64_t, int32_t row) { pl.stage.push_back(row); });
+      std::sort(pl.stage.begin() + r0, pl.stage.end());
+      pl.stage.erase(std::unique(pl.stage.begin() + r0, pl.stage.end()), pl.stage.end());
+      llen[static_cast<size_t>(l)] = static_cast<int64_t>(pl.stage.size() - r0);
+    }
+    return plan_list_search(q.nq, q.k, q.q_list, lrow0, llen, &pl);
+  }
+  if (q.q_user) return stage_tenant_scope(c, call.s, q.nq, q.q_user, q.q_org, pt->scope, &pt->sc);
   return AUR_OK;
 }
 
+}  // namespace
+
+namespace aur {
 int index_device(const aur_index* ix) { return ix->device; }
 int index_bf16_queries(const aur_index* ix) { return ix->dtype == AUR_BF16 || ix->dtype == AUR_I8; }
 
 AttrColumns& index_attrs(aur_index* ix) { return ix->attrs; }
 
-int filtered_legs(aur_index* const* shards, int n, const void* queries_host, int32_t nq, int32_t k, const FiltProgs& fp,
-                  int64_t max_list_rows, const DenseLegsThen& then, float* scores_host, int64_t* ids_host) {
-  struct Part { std::unique_ptr<HostCall> call; std::vector<int64_t> tot; };
-  std::vector<Part> parts(static_cast<size_t>(n));
+int dense_legs(aur_index* const* shards, int n, const DenseQuery& q, const DenseLegsThen& then, float* scores_host,
+               int64_t* ids_host) {
+  std::vector<DensePart> parts(static_cast<size_t>(n));
   // every stream drains before its context goes back to the pool (also on an error): declared after `parts`, so it
   // runs before their destructors
   struct Drain {
-    std::vector<Part>& v;
+    std::vector<DensePart>& v;
     ~Drain() {
-      for (Part& p : v)
+      for (DensePart& p : v)
         if (p.call && p.call->c) { cudaSetDevice(p.call->ix->device); cudaStreamSynchronize(p.call->s); }
     }
   } drain{parts};
@@ -1004,42 +979,59 @@ int filtered_legs(aur_index* const* shards, int n, const void* queries_host, int
   for (int s = 0; s < n; ++s) order[static_cast<size_t>(s)] = s;
   std::sort(order.begin(), order.end(), [&](int a, int b) { return std::less<aur_index*>()(shards[a], shards[b]); });
   for (int s : order) parts[static_cast<size_t>(s)].call.reset(new HostCall(shards[s]));
-  const size_t nout = static_cast<size_t>(nq) * k;
   int rc = AUR_OK;
-  // every shard's queries and count pass, then one wait for all the counts
-  for (Part& pt : parts) {
+  // every shard's queries, scope and (programs) count pass, then one wait for all the counts
+  for (DensePart& pt : parts) {
     HostCall& call = *pt.call;
     if ((rc = call.open()) != AUR_OK) return rc;
-    SearchCtx* c = call.c;
-    const size_t qbytes = static_cast<size_t>(nq) * call.ix->dim * call.ix->qelt;
-    CU_TRY(c->stage_q.reserve(qbytes));
-    CU_TRY(c->stage_scores.reserve(nout));
-    CU_TRY(c->stage_ids.reserve(nout));
-    CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, call.s));
-    call.d_scores = c->stage_scores.p;
-    call.d_ids = c->stage_ids.p;
-    if (n == 1 && scores_host && ids_host) call.direct = direct_outputs(scores_host, ids_host, &call.d_scores, &call.d_ids);
-    if ((rc = stats_begin(c, call.s, nq, call.n_rows)) != AUR_OK) return rc;
-    if ((rc = filter_count(call.ix, c, call.s, fp, call.n_rows)) != AUR_OK) return rc;
+    if ((rc = call.stage(q.queries, q.nq, q.k, n == 1 ? scores_host : nullptr, n == 1 ? ids_host : nullptr)) != AUR_OK) return rc;
+    if ((rc = prepare_scope(q, &pt)) != AUR_OK) return rc;
+    if ((rc = stats_begin(call.c, call.s, q.nq, call.n_rows)) != AUR_OK) return rc;
+    if (q.fp && (rc = filter_count(call.ix, call.c, call.s, *q.fp, call.n_rows)) != AUR_OK) return rc;
   }
-  for (Part& pt : parts) {
-    CU_TRY(cudaSetDevice(pt.call->ix->device));
-    CU_TRY(cudaStreamSynchronize(pt.call->s));
-    filter_totals(pt.call->c, fp.n_programs, &pt.tot);
-  }
+  if (q.fp)
+    for (DensePart& pt : parts) {
+      CU_TRY(cudaSetDevice(pt.call->ix->device));
+      CU_TRY(cudaStreamSynchronize(pt.call->s));
+      filter_totals(pt.call->c, q.fp->n_programs, &pt.tot);
+    }
   std::vector<DenseLeg> legs;
-  for (Part& pt : parts) {
+  for (DensePart& pt : parts) {
     HostCall& call = *pt.call;
-    SearchCtx* c = call.c;
     CU_TRY(cudaSetDevice(call.ix->device));
-    rc = filtered_search(call.ix, c, call.s, nq, k, fp, pt.tot, max_list_rows, call.n_rows, call.d_scores, call.d_ids);
-    if (rc == AUR_OK) rc = stats_end(call.ix, c, call.s);
+    if (q.fp)
+      rc = filtered_search(call.ix, call.c, call.s, q.nq, q.k, *q.fp, pt.tot, q.max_list_rows, call.n_rows, call.d_scores, call.d_ids);
+    else if (q.q_list)
+      rc = run_list_search(call.ix, call.c, call.s, pt.pl, q.nq, q.k, nullptr, call.d_scores, call.d_ids);
+    else
+      rc = search_enqueue(call.ix, call.c, call.c->stage_q.p, q.nq, q.k, pt.sc, call.n_rows, call.d_scores, call.d_ids, nullptr, call.s);
+    if (rc == AUR_OK) rc = stats_end(call.ix, call.c, call.s);
     if (rc != AUR_OK) return rc;
     legs.push_back(DenseLeg{call.ix->device, call.s, call.d_scores, call.d_ids, call.n_rows, &pt.tot, call.direct});
   }
   return then(legs);
 }
 }  // namespace aur
+
+namespace {
+// dense_legs over one shard, its lists copied into the caller's host buffers (directly written when they are
+// page-locked).  They are written only when every kernel of the search was enqueued; on any failure they stay untouched.
+int search_into_host(aur_index* ix, const DenseQuery& q, float* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out,
+                     int64_t* matched_out = nullptr) {
+  return dense_legs(&ix, 1, q, [&](const std::vector<DenseLeg>& legs) -> int {
+    const DenseLeg& l = legs[0];
+    if (!l.direct) {   // into the caller's pageable buffers
+      const size_t nout = static_cast<size_t>(q.nq) * q.k;
+      CU_TRY(cudaMemcpyAsync(scores_out, l.scores, nout * 4, cudaMemcpyDeviceToHost, l.stream));
+      CU_TRY(cudaMemcpyAsync(ids_out, l.ids, nout * 8, cudaMemcpyDeviceToHost, l.stream));
+    }
+    CU_TRY(cudaStreamSynchronize(l.stream));
+    if (matched_out) std::copy(l.matched->begin(), l.matched->end(), matched_out);
+    if (snapshot_rows_out) *snapshot_rows_out = l.snapshot_rows;
+    return AUR_OK;
+  }, scores_out, ids_out);
+}
+}  // namespace
 
 extern "C" {
 
@@ -1359,19 +1351,29 @@ int aur_search_dev(aur_index* ix, const void* queries_dev, int32_t nq, int32_t k
 
 int aur_search(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
                const int32_t* q_org, float* scores_out, int64_t* ids_out) {
-  return search_host(ix, queries_host, nq, k, q_user, q_org, nullptr, -1, scores_out, ids_out, nullptr);
+  return aur_search_ex(ix, queries_host, nq, k, q_user, q_org, scores_out, ids_out, nullptr);
 }
 
 int aur_search_ex(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
                   const int32_t* q_org, float* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out) {
-  return search_host(ix, queries_host, nq, k, q_user, q_org, nullptr, -1, scores_out, ids_out, snapshot_rows_out);
+  int rc = check_search_args(ix, queries_host, nq, k, scores_out, ids_out);
+  if (rc != AUR_OK) return rc;
+  if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
+  DenseQuery q{queries_host, nq, k};
+  q.q_user = q_user; q.q_org = q_org;
+  return search_into_host(ix, q, scores_out, ids_out, snapshot_rows_out);
 }
 
 int aur_search_subset(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int64_t* allow_ids,
                       int64_t n_allow, float* scores_out, int64_t* ids_out) {
   if (n_allow < 0) return fail(AUR_ERR_INVALID, "n_allow < 0");
-  static const int64_t none = 0;
-  return search_host(ix, queries_host, nq, k, nullptr, nullptr, allow_ids ? allow_ids : &none, n_allow, scores_out, ids_out, nullptr);
+  int rc = check_search_args(ix, queries_host, nq, k, scores_out, ids_out);
+  if (rc != AUR_OK) return rc;
+  if (n_allow > 0 && !allow_ids) return fail(AUR_ERR_INVALID, "allow_ids / n_allow");
+  if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
+  DenseQuery q{queries_host, nq, k};
+  q.allow_ids = allow_ids; q.n_allow = n_allow;
+  return search_into_host(ix, q, scores_out, ids_out, nullptr);
 }
 
 int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int64_t* list_ids,
@@ -1386,34 +1388,9 @@ int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_
   if (list_offsets[n_lists] > 0 && !list_ids) return fail(AUR_ERR_INVALID, "list_ids is required");
   for (int32_t q = 0; q < nq; ++q)
     if (q_list[q] < 0 || q_list[q] >= n_lists) return fail(AUR_ERR_INVALID, "q_list[%d] = %d is not a list", q, q_list[q]);
-
-  HostCall call(ix);
-  if ((rc = call.open()) != AUR_OK) return rc;
-  SearchCtx* c = call.c;
-  cudaStream_t s = call.s;
-  // staging (int32): [every named list's rows of the published prefix, sorted, once each][the plan's blocks]
-  std::vector<char> named(static_cast<size_t>(n_lists), 0);
-  for (int32_t q = 0; q < nq; ++q) named[static_cast<size_t>(q_list[q])] = 1;
-  ListPlan pl;
-  std::vector<int64_t> lrow0(static_cast<size_t>(n_lists), 0), llen(static_cast<size_t>(n_lists), 0);
-  for (int32_t l = 0; l < n_lists; ++l) {
-    const size_t r0 = pl.stage.size();
-    lrow0[static_cast<size_t>(l)] = static_cast<int64_t>(r0);
-    if (!named[static_cast<size_t>(l)]) continue;
-    resolve_ids(ix, list_ids + list_offsets[l], list_offsets[l + 1] - list_offsets[l], call.n_rows,
-                [&](int64_t, int32_t row) { pl.stage.push_back(row); });
-    std::sort(pl.stage.begin() + r0, pl.stage.end());
-    pl.stage.erase(std::unique(pl.stage.begin() + r0, pl.stage.end()), pl.stage.end());
-    llen[static_cast<size_t>(l)] = static_cast<int64_t>(pl.stage.size() - r0);
-  }
-  if ((rc = plan_list_search(nq, k, q_list, lrow0, llen, &pl)) != AUR_OK) return rc;
-  rc = stats_begin(c, s, nq, call.n_rows);
-  if (rc == AUR_OK) rc = call.stage(queries_host, nq, k, scores_out, ids_out);
-  if (rc == AUR_OK) rc = run_list_search(ix, c, s, pl, nq, k, nullptr, call.d_scores, call.d_ids);
-  if (rc == AUR_OK) rc = stats_end(ix, c, s);
-  if ((rc = call.finish(rc, nq, k, scores_out, ids_out)) != AUR_OK) return rc;
-  if (snapshot_rows_out) *snapshot_rows_out = call.n_rows;
-  return AUR_OK;
+  DenseQuery q{queries_host, nq, k};
+  q.list_ids = list_ids; q.list_offsets = list_offsets; q.n_lists = n_lists; q.q_list = q_list;
+  return search_into_host(ix, q, scores_out, ids_out, snapshot_rows_out);
 }
 
 int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t* codes, int64_t n) {
@@ -1437,19 +1414,9 @@ int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int
   if ((rc = filter_check_programs(fp)) != AUR_OK || (rc = ix->attrs.check(fp, "shard")) != AUR_OK ||
       (rc = filter_check_queries(fp, nq, max_list_rows)) != AUR_OK)
     return rc;
-  return filtered_legs(&ix, 1, queries_host, nq, k, fp, max_list_rows, [&](const std::vector<DenseLeg>& legs) -> int {
-    const DenseLeg& l = legs[0];
-    const size_t nout = static_cast<size_t>(nq) * k;
-    // (reached only when every kernel of the search was enqueued: on any failure the pageable outputs stay untouched)
-    if (!l.direct) {   // page-locked outputs were written by the re-rank kernel itself
-      CU_TRY(cudaMemcpyAsync(scores_out, l.scores, nout * 4, cudaMemcpyDeviceToHost, l.stream));
-      CU_TRY(cudaMemcpyAsync(ids_out, l.ids, nout * 8, cudaMemcpyDeviceToHost, l.stream));
-    }
-    CU_TRY(cudaStreamSynchronize(l.stream));
-    if (matched_out) for (int32_t q = 0; q < n_programs; ++q) matched_out[q] = (*l.matched)[static_cast<size_t>(q)];
-    if (snapshot_rows_out) *snapshot_rows_out = l.snapshot_rows;
-    return AUR_OK;
-  }, scores_out, ids_out);
+  DenseQuery q{queries_host, nq, k};
+  q.fp = &fp; q.max_list_rows = max_list_rows;
+  return search_into_host(ix, q, scores_out, ids_out, snapshot_rows_out, matched_out);
 }
 
 int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,

@@ -258,15 +258,13 @@ __global__ void __launch_bounds__(kFuseThreads) hybrid_merge_fuse_kernel(FusePar
   }
 }
 
-// Scratch of one shard's part of a hybrid call on one device: the stream its dense leg runs on and that leg's lists.
-// The context of shard 0 also hosts the join, the gathered lists of the other shards, the merge + fusion kernel and the
-// copy back.  Idle contexts are pooled for the life of the process.
+// Scratch of one shard's part of a hybrid call on one device: the events its legs' streams record for the join.  The
+// context of shard 0 also hosts the join on its stream, the gathered lists of the other shards, the merge + fusion
+// kernel and the copy back.  Idle contexts are pooled for the life of the process.
 struct HybridCtx {
   int device = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t kw_done = nullptr, dense_done = nullptr;
-  DevBuf<float> cos;
-  DevBuf<int64_t> ids;
   DevBuf<double> w;
   DevBuf<float> g_cos;              // gathered lists of shards 1 .. n-1: dense cosines and ids, keyword scores and ids
   DevBuf<int64_t> g_did, g_kid;
@@ -323,13 +321,10 @@ struct HybridArgs {
   int64_t max_list_rows;   // with fp: the dense legs' list-vs-scan bound, an even share per shard
 };
 
-// One shard's dense list [nq][fetch] on its device, valid once `stream` reaches it.
-struct DenseList { cudaStream_t stream; const float* cos; const int64_t* ids; };
-
-// The join on shard 0's device (every keyword leg, every dense leg not on its stream), the gather of the other shards'
-// lists, the merge + fusion and the copy into hs[0]->host.  Shard 0's buffers were prepared by run_on_devices.
+// The join on shard 0's device (every keyword leg, every dense leg), the gather of the other shards' lists, the merge +
+// fusion and the copy into hs[0]->host.  Shard 0's buffers were prepared by run_on_devices.
 int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const std::vector<KwLeg>& kl,
-                  const std::vector<DenseList>& dl) {
+                  const std::vector<DenseLeg>& dl) {
   const int n = a.n;
   const size_t nl = static_cast<size_t>(a.nq) * a.fetch, no = static_cast<size_t>(a.nq) * a.k_out;
   HybridCtx* h = hs[0];
@@ -337,7 +332,7 @@ int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const 
   for (int s = 0; s < n; ++s) {
     HybridCtx* o = hs[static_cast<size_t>(s)];
     HYB_TRY(cudaSetDevice(o->device));
-    if (dl[static_cast<size_t>(s)].stream != st) HYB_TRY(cudaEventRecord(o->dense_done, dl[static_cast<size_t>(s)].stream));
+    HYB_TRY(cudaEventRecord(o->dense_done, dl[static_cast<size_t>(s)].stream));
     HYB_TRY(cudaEventRecord(o->kw_done, kl[static_cast<size_t>(s)].stream));   // the store shares the shard's device
   }
   HYB_TRY(cudaSetDevice(h->device));
@@ -345,18 +340,18 @@ int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const 
   for (int s = 0; s < n; ++s) {
     const HybridCtx* o = hs[static_cast<size_t>(s)];
     const KwLeg& k = kl[static_cast<size_t>(s)];
-    const DenseList& d = dl[static_cast<size_t>(s)];
+    const DenseLeg& d = dl[static_cast<size_t>(s)];
     HYB_TRY(cudaStreamWaitEvent(st, o->kw_done, 0));
-    if (d.stream != st) HYB_TRY(cudaStreamWaitEvent(st, o->dense_done, 0));
+    HYB_TRY(cudaStreamWaitEvent(st, o->dense_done, 0));
     if (s == 0) continue;
     const size_t at = static_cast<size_t>(s - 1) * nl;
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_cos.p + at, h->device, d.cos, o->device, nl * 4, st));
+    HYB_TRY(cudaMemcpyPeerAsync(h->g_cos.p + at, h->device, d.scores, o->device, nl * 4, st));
     HYB_TRY(cudaMemcpyPeerAsync(h->g_did.p + at, h->device, d.ids, o->device, nl * 8, st));
     HYB_TRY(cudaMemcpyPeerAsync(h->g_ks.p + at, h->device, k.scores, k.device, nl * 8, st));
     HYB_TRY(cudaMemcpyPeerAsync(h->g_kid.p + at, h->device, k.ids, k.device, nl * 8, st));
   }
   FuseParams p;
-  p.dense = LegLists{dl[0].ids, dl[0].cos, h->g_did.p, h->g_cos.p, h->run_max.p};
+  p.dense = LegLists{dl[0].ids, dl[0].scores, h->g_did.p, h->g_cos.p, h->run_max.p};
   p.kw = LegLists{kl[0].ids, kl[0].scores, h->g_kid.p, h->g_ks.p, n > 1 ? h->run_max.p + static_cast<size_t>(n) * nl : nullptr};
   p.w = h->w.p;
   p.n = n; p.nq = a.nq; p.fetch = a.fetch; p.k_out = a.k_out; p.fusion = a.fusion;
@@ -373,8 +368,8 @@ int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const 
 }
 
 // Inside the keyword legs: shard 0's device takes the weights and the output space, every shard's dense leg is enqueued
-// (aur_search_ex's search on the shard's hybrid context, or with programs aur_search_filtered's on a pooled search
-// context: filtered_legs), then join_and_fuse.  hs[s] is on shard s's device; rows[s] receives shard s's snapshot.
+// (dense_legs: aur_search_ex's search, or with programs aur_search_filtered's), then join_and_fuse.  hs[s] is on shard
+// s's device; rows[s] receives shard s's snapshot.
 int run_on_devices(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const std::vector<KwLeg>& kl, int64_t* rows) {
   const int n = a.n;
   const size_t nl = static_cast<size_t>(a.nq) * a.fetch, no = static_cast<size_t>(a.nq) * a.k_out;
@@ -398,31 +393,19 @@ int run_on_devices(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const
     HYB_TRY(h->run_max.reserve(2 * static_cast<size_t>(n) * nl));
   }
   HYB_TRY(cudaMemcpyAsync(h->w.p, a.w.data(), a.w.size() * 8, cudaMemcpyHostToDevice, st));
-  // (pageable: staged before the call returns; behind the dense legs it would wait for their kernels)
-  if (a.fp) {
-    return filtered_legs(a.shards, n, a.queries_host, a.nq, a.fetch, *a.fp, a.max_list_rows / n,
-                         [&](const std::vector<DenseLeg>& legs) -> int {
-                           std::vector<DenseList> dl;
-                           for (int s = 0; s < n; ++s) {
-                             const DenseLeg& l = legs[static_cast<size_t>(s)];
-                             rows[s] = l.snapshot_rows;
-                             dl.push_back(DenseList{l.stream, l.scores, l.ids});
-                           }
-                           return join_and_fuse(a, hs, kl, dl);
-                         });
-  }
-  std::vector<DenseList> dl;
-  for (int s = 0; s < n; ++s) {
-    HybridCtx* o = hs[static_cast<size_t>(s)];
-    HYB_TRY(cudaSetDevice(o->device));
-    HYB_TRY(o->cos.reserve(nl));
-    HYB_TRY(o->ids.reserve(nl));
-    const int rc = dense_leg(a.shards[s], o->device, o->stream, a.queries_host, a.nq, a.fetch, a.q_user, a.q_org, o->cos.p,
-                             o->ids.p, &rows[s]);
-    if (rc != AUR_OK) return rc;
-    dl.push_back(DenseList{o->stream, o->cos.p, o->ids.p});
-  }
-  return join_and_fuse(a, hs, kl, dl);
+  // (pageable: staged before the call returns.  The dense legs run on their own streams, so the copy would not wait for
+  // their kernels after them either; it stays first, the order every hybrid measurement in DESIGN.md section 9 used)
+  DenseQuery q{a.queries_host, a.nq, a.fetch};
+  q.q_user = a.q_user; q.q_org = a.q_org;
+  q.fp = a.fp; q.max_list_rows = a.max_list_rows / n;
+  return dense_legs(a.shards, n, q, [&](const std::vector<DenseLeg>& legs) -> int {
+    for (int s = 0; s < n; ++s) rows[s] = legs[static_cast<size_t>(s)].snapshot_rows;
+    const int rc = join_and_fuse(a, hs, kl, legs);
+    // the join stream reads the dense lists in the legs' contexts: on an error it drains before dense_legs gives them
+    // back (on success join_and_fuse has drained it)
+    if (rc != AUR_OK) { cudaSetDevice(h->device); cudaStreamSynchronize(st); }
+    return rc;
+  });
 }
 
 template <typename T>

@@ -366,29 +366,32 @@ cudaError_t filter_upload(const FiltProgs& fp, const int32_t* user, const int32_
                           DevBuf<int32_t>& stage, cudaStream_t s, FiltParams* p);
 inline FiltParams filter_pass(FiltParams p, int ps) { p.n_programs = filter_pass_programs(p.n_programs, ps); p.prog_off += ps * kFiltMaxPrograms; return p; }
 // ---------------------------------------------------------------- the two legs of a hybrid query (hybrid.cu)
-// Dense leg: the search aur_search_ex runs for these host queries and per-query tenant codes (same scope handling, same
-// kernels, same answer), enqueued on stream s of `device` over the prefix published now, into the device arrays
-// scores / ids [nq * k].  Nothing waits; *snapshot_rows receives the prefix.  A bf16 or int8 index on `device` only
-// (else AUR_ERR_UNSUPPORTED / AUR_ERR_INVALID).  The leg's aur_stats.last_* are the index's last search.  (capi.cu)
-int dense_leg(aur_index* ix, int device, cudaStream_t s, const void* queries_host, int32_t nq, int32_t k, const int32_t* q_user,
-              const int32_t* q_org, float* scores, int64_t* ids, int64_t* snapshot_rows);
-int index_device(const aur_index* ix);
-int index_bf16_queries(const aur_index* ix);   // the index takes bf16 queries: bf16 or int8 rows
-// Filtered dense legs: aur_search_filtered's search of the host queries under the checked programs fp on every shard
-// of shards[0 .. n) (bf16, distinct), max_list_rows applied per shard, each shard's part on a pooled search context of
-// its device and that context's stream.  Every shard's count pass is enqueued before any is waited on; their read-back
-// is the only host sync.  Then every shard's search (list kernels or masked scan, as aur_search_filtered picks) is
-// enqueued and then(legs) runs with every shard's (device, stream, top-k lists [nq * k] in device memory, valid once the
-// stream reaches them, snapshot, matching rows per program) while the shards' shared locks and contexts are held; the
-// streams are idle again before this returns.  aur_stats.last_* of each shard describe its part.  scores_host /
-// ids_host (n = 1, nullable): the caller's host outputs; when both are page-locked and mapped, the search writes its
-// lists straight into them (DenseLeg.direct) instead of into device staging.  (capi.cu)
+// Dense legs: every host search of a vector shard (aur_search, aur_search_ex, aur_search_subset, aur_search_lists,
+// aur_search_filtered and the hybrid query's dense legs) over shards[0 .. n) (distinct, arguments checked), each shard's
+// part on a pooled search context of its device and that context's stream, over the prefix published when the part
+// began.  q holds the host queries and at most one scope: tenant codes (nullable), allow-ids or per-query lists (n = 1
+// only), or checked programs with max_list_rows applied per shard.  Every shard's shared lock is taken in address order;
+// with programs every shard's count pass is enqueued before any is waited on, and their read-back is the only host sync.
+// Then every shard's search is enqueued and then(legs) runs with every shard's (device, stream, top-k lists [nq * k] in
+// device memory, valid once the stream reaches them, snapshot, matching rows per program) while the shards' shared locks
+// and contexts are held; the streams are idle again before this returns.  aur_stats.last_* of each shard describe its
+// part.  scores_host / ids_host (n = 1, nullable): the caller's host outputs; when both are page-locked and mapped, the
+// search writes its lists straight into them (DenseLeg.direct) instead of into device staging.  (capi.cu)
+struct DenseQuery {
+  const void* queries; int32_t nq, k;
+  const int32_t* q_user = nullptr; const int32_t* q_org = nullptr;        // tenant codes [nq]
+  const int64_t* allow_ids = nullptr; int64_t n_allow = -1;               // allow-ids (n_allow >= 0)
+  const int64_t* list_ids = nullptr; const int64_t* list_offsets = nullptr; int32_t n_lists = 0;
+  const int32_t* q_list = nullptr;                                        // per-query lists (q_list non-NULL)
+  const FiltProgs* fp = nullptr; int64_t max_list_rows = 0;               // programs (fp non-NULL)
+};
 struct DenseLeg { int device; cudaStream_t stream; const float* scores; const int64_t* ids; int64_t snapshot_rows;
                   const std::vector<int64_t>* matched; bool direct; };
 using DenseLegsThen = std::function<int(const std::vector<DenseLeg>& legs)>;
-int filtered_legs(aur_index* const* shards, int n, const void* queries_host, int32_t nq, int32_t k, const FiltProgs& fp,
-                  int64_t max_list_rows, const DenseLegsThen& then, float* scores_host = nullptr,
-                  int64_t* ids_host = nullptr);
+int dense_legs(aur_index* const* shards, int n, const DenseQuery& q, const DenseLegsThen& then, float* scores_host = nullptr,
+               int64_t* ids_host = nullptr);
+int index_device(const aur_index* ix);
+int index_bf16_queries(const aur_index* ix);   // the index takes bf16 queries: bf16 or int8 rows
 AttrColumns& index_attrs(aur_index* ix);
 // Keyword legs: aur_kw_search_multi's search over stores[0 .. n) (distinct, non-NULL, 1 <= n <= 64) taken as one
 // corpus, each store's part enqueued on its own context and stream; fp (nullable; programs checked, their columns set on

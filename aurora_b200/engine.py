@@ -633,14 +633,15 @@ def _add_text(stores, vocab: KeywordVocab, ids, texts, user_codes, org_codes) ->
 def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_offsets,
                   w_dense, w_sparse=None, fusion: int = N.FUSION_RANKED, k_out: Optional[int] = None, q_user=None,
                   q_org=None, programs=None, q_program=None, max_list_rows: int = 0):
-    """Both legs of the hybrid query and their fusion in one device call (aur_hybrid_search): the dense leg's top-``fetch``
-    of ``queries`` over ``index`` and the keyword leg's top-``fetch`` of ``q_terms`` / ``q_offsets`` over ``kw_index``
-    (same tenant scope), fused per query with weights ``w_dense`` / ``w_sparse`` (default ``1 - w_dense``).  Returns
+    """Both legs of the hybrid query and their fusion in one device call (aur_hybrid_search_multi): the dense leg's
+    top-``fetch`` of ``queries`` over ``index`` and the keyword leg's top-``fetch`` of ``q_terms`` / ``q_offsets``
+    over ``kw_index`` (same tenant scope), fused per query with weights ``w_dense`` / ``w_sparse`` (default
+    ``1 - w_dense``).  Returns
     (ids [nq, k_out] int64, fused scores [nq, k_out] float64, dense cosines [nq, k_out] float32 (NaN: not in the dense
     list), (dense snapshot rows, keyword snapshot rows)); padding (-1, -inf, NaN).
 
     ``index`` / ``kw_index`` are an ``Index`` and a ``KeywordIndex``, or a ``MultiIndex`` of bf16 ``Index`` shards and a
-    ``MultiKeywordIndex`` on the same devices in the same order (aur_hybrid_search_multi): each leg is then the global
+    ``MultiKeywordIndex`` on the same devices in the same order (one pair per shard): each leg is then the global
     top-``fetch`` of ``MultiIndex.search`` / ``MultiKeywordIndex.search``, merged and fused on shard 0's GPU, and the
     snapshots are (one per shard, one per store).
 
@@ -671,36 +672,26 @@ def hybrid_search(index, kw_index, queries: np.ndarray, fetch: int, q_terms, q_o
     scores = np.empty((nq, k_out), dtype=np.float64)
     ids = np.empty((nq, k_out), dtype=np.int64)
     cosine = np.empty((nq, k_out), dtype=np.float32)
+    shard_list = index.shards if multi else [index]
+    store_list = kw_index.stores if multi else [kw_index]
+    n = len(shard_list)
+    shards = (C.c_void_p * n)(*[sh._h.value for sh in shard_list])
+    stores = (C.c_void_p * n)(*[st._h.value for st in store_list])
+    snaps = np.full(2 * n, -1, dtype=np.int64)
     if programs is not None:
         if q_user is not None or q_org is not None:
             raise ValueError("programs replace q_user / q_org: write the tenant scope into the programs")
         tok, off, bm, ql = _program_args(programs, q_program, nq)
-        shard_list = index.shards if multi else [index]
-        store_list = kw_index.stores if multi else [kw_index]
-        n = len(shard_list)
-        shards = (C.c_void_p * n)(*[sh._h.value for sh in shard_list])
-        stores = (C.c_void_p * n)(*[st._h.value for st in store_list])
-        snaps = np.full(2 * n, -1, dtype=np.int64)
         N.check(N.load().aur_hybrid_search_filtered(shards, stores, n, _ptr(q), nq, int(fetch), _ptr(qt), _ptr(q_off),
                                                     _ptr(tok), _ptr(off), len(programs), _ptr(bm), bm.shape[0], _ptr(ql),
                                                     int(max_list_rows), _ptr(wd), _ptr(ws), int(fusion), k_out,
                                                     _ptr(scores), _ptr(ids), _ptr(cosine), _ptr(snaps)))
-        if multi:
-            return ids, scores, cosine, (snaps[:n].tolist(), snaps[n:].tolist())
-        return ids, scores, cosine, (int(snaps[0]), int(snaps[1]))
-    if multi:
-        n = len(index.shards)
-        shards = (C.c_void_p * n)(*[sh._h.value for sh in index.shards])
-        stores = (C.c_void_p * n)(*[st._h.value for st in kw_index.stores])
-        snaps = np.full(2 * n, -1, dtype=np.int64)
+    else:
         N.check(N.load().aur_hybrid_search_multi(shards, stores, n, _ptr(q), nq, int(fetch), _ptr(qt), _ptr(q_off), _ptr(u),
                                                  _ptr(o), _ptr(wd), _ptr(ws), int(fusion), k_out, _ptr(scores), _ptr(ids),
                                                  _ptr(cosine), _ptr(snaps)))
+    if multi:
         return ids, scores, cosine, (snaps[:n].tolist(), snaps[n:].tolist())
-    snaps = (C.c_int64 * 2)(-1, -1)
-    N.check(index._lib.aur_hybrid_search(index._h, kw_index._h, _ptr(q), nq, int(fetch), _ptr(qt), _ptr(q_off), _ptr(u),
-                                         _ptr(o), _ptr(wd), _ptr(ws), int(fusion), k_out, _ptr(scores), _ptr(ids),
-                                         _ptr(cosine), snaps))
     return ids, scores, cosine, (int(snaps[0]), int(snaps[1]))
 
 

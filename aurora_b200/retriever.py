@@ -496,7 +496,7 @@ class KnowledgeBase:
                     ids, scores = self.index.search_lists(q, fetch, lists, np.array([slots[v] for v in vals], np.int32))
                 else:
                     # one launch for the whole group: up to 32 distinct tenant scopes per batch ride on the tensor-core
-                    # kernel as per-row bit masks (csrc/capi.cu search_host); the library falls back by itself beyond
+                    # kernel as per-row bit masks (csrc/capi.cu stage_tenant_scope); the library falls back by itself beyond
                     ids, scores = self.index.search(q, fetch, **self._scope_args(kind, vals))
                 for i, r_ids, r_scores in zip(g, ids, scores):
                     dense[i] = [(int(d), float(s)) for d, s in zip(r_ids, r_scores) if d >= 0]

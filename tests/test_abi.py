@@ -89,6 +89,13 @@ def test_invalid_arguments_are_rejected_without_touching_a_device(lib):
     assert lib.aur_open(C.byref(cfg), C.byref(h)) == N.AUR_ERR_INVALID
     assert b"dtype" in lib.aur_last_error()
     assert lib.aur_search(None, None, 1, 1, None, None, None, None) == N.AUR_ERR_INVALID
+    # a subset search's allow-list is checked before the handle is read (the handle here is a fake pointer)
+    q, sc, ids = np.zeros(64, np.uint16), np.empty(1, np.float32), np.empty(1, np.int64)
+    p = lambda a: a.ctypes.data_as(C.c_void_p)   # noqa: E731
+    assert lib.aur_search_subset(C.c_void_p(1), p(q), 1, 1, None, 3, p(sc), p(ids)) == N.AUR_ERR_INVALID
+    assert b"allow_ids / n_allow" in lib.aur_last_error()
+    assert lib.aur_search_subset(C.c_void_p(1), p(q), 1, 1, None, -1, p(sc), p(ids)) == N.AUR_ERR_INVALID
+    assert b"n_allow < 0" in lib.aur_last_error()
     assert lib.aur_close(None) == N.AUR_OK
 
 

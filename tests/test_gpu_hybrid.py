@@ -48,6 +48,35 @@ def assert_row(got, want, ctx):
     assert np.array_equal(gc[ok].view(np.int32), wc[ok].view(np.int32)), ctx
 
 
+def c_hybrid_search(ix, kw, qv, fetch, qt, qo, wd, ws=None, fusion=N.FUSION_RANKED, k_out=None, q_user=None, q_org=None):
+    """engine.hybrid_search's single-shard call made through aur_hybrid_search itself (engine.hybrid_search takes
+    aur_hybrid_search_multi with n = 1); the same arguments and return shape."""
+    import ctypes as C
+
+    p = lambda a: None if a is None else C.c_void_p(a.ctypes.data)   # noqa: E731
+    q = ix._rows_buffer(qv)
+    nq = q.shape[0]
+    k_out = 2 * int(fetch) if k_out is None else int(k_out)
+    wd = np.ascontiguousarray(np.broadcast_to(np.asarray(wd, dtype=np.float64), (nq,)))
+    ws = 1.0 - wd if ws is None else np.ascontiguousarray(np.broadcast_to(np.asarray(ws, dtype=np.float64), (nq,)))
+    qt = np.ascontiguousarray(qt, dtype=np.int32) if len(qt) else np.zeros(1, np.int32)
+    qo = np.ascontiguousarray(qo, dtype=np.int64)
+    u = None if q_user is None else np.ascontiguousarray(q_user, dtype=np.int32)
+    o = None if q_org is None else np.ascontiguousarray(q_org, dtype=np.int32)
+    scores, ids = np.empty((nq, k_out), np.float64), np.empty((nq, k_out), np.int64)
+    cosine, snaps = np.empty((nq, k_out), np.float32), np.full(2, -1, np.int64)
+    N.check(N.load().aur_hybrid_search(ix._h, kw._h, p(q), nq, int(fetch), p(qt), p(qo), p(u), p(o), p(wd), p(ws),
+                                       int(fusion), k_out, p(scores), p(ids), p(cosine), p(snaps)))
+    return ids, scores, cosine, (int(snaps[0]), int(snaps[1]))
+
+
+def assert_same(a, b):
+    """Two hybrid answers identical bit for bit, snapshots included."""
+    for x, y in zip(a[:3], b[:3]):
+        assert x.dtype == y.dtype and np.array_equal(x.view(np.uint8), y.view(np.uint8))
+    assert a[3] == b[3]
+
+
 def weights(nq, shift=0):
     wd = np.array([max(0.0, ALPHAS[(q + shift) % len(ALPHAS)]) for q in range(nq)])
     return wd, 1.0 - wd
@@ -80,6 +109,7 @@ class Corpus2:
         if wd is None:
             wd, ws = weights(nq)
         got = hybrid_search(self.ix, self.kw, qv, fetch, qt, qo, wd, ws, fusion, k_out, q_user, q_org)
+        assert_same(c_hybrid_search(self.ix, self.kw, qv, fetch, qt, qo, wd, ws, fusion, k_out, q_user, q_org), got)
         d_ids, d_sc, s_ids, s_sc = self.legs(qv, qt, qo, fetch, q_user, q_org)
         for q in range(nq):
             want = host_fuse(d_ids[q], d_sc[q], s_ids[q], s_sc[q], wd[q], ws[q], fusion, k_out)
@@ -181,9 +211,13 @@ def test_argument_errors(corpus):
     def code(**kw):
         args = dict(fetch=8, w=np.array([0.5, 0.5]), fusion=N.FUSION_RANKED, k_out=16, ix=corpus.ix, kw=corpus.kw)
         args.update(kw)
-        with pytest.raises(N.AuroraError) as e:
-            hybrid_search(args["ix"], args["kw"], qv, args["fetch"], qt, qo, args["w"], None, args["fusion"], args["k_out"])
-        return e.value.code
+        codes = []
+        for search in (hybrid_search, c_hybrid_search):   # aur_hybrid_search_multi with n = 1, aur_hybrid_search
+            with pytest.raises(N.AuroraError) as e:
+                search(args["ix"], args["kw"], qv, args["fetch"], qt, qo, args["w"], None, args["fusion"], args["k_out"])
+            codes.append(e.value.code)
+        assert codes[0] == codes[1], codes
+        return codes[0]
 
     assert code(fetch=129, k_out=1) == N.AUR_ERR_UNSUPPORTED
     assert code(fetch=0, k_out=1) == N.AUR_ERR_INVALID
@@ -248,7 +282,8 @@ def test_concurrent_writer_and_readers():
         i = 0
         while not done.is_set():
             fusion = FUSIONS[(i + r) % 2]
-            answers.append((fusion, hybrid_search(ix, kw, qv, fetch, qt, qo, 0.5, None, fusion, k_out)))
+            search = (hybrid_search, c_hybrid_search)[(i // 2 + r) % 2]   # both entry points under the writer
+            answers.append((fusion, search(ix, kw, qv, fetch, qt, qo, 0.5, None, fusion, k_out)))
             i += 1
 
     ths = [threading.Thread(target=writer)] + [threading.Thread(target=reader, args=(r,)) for r in range(3)]

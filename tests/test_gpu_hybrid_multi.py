@@ -15,7 +15,8 @@ from aurora_b200 import _native as N
 from aurora_b200 import bm25
 from aurora_b200.engine import Index, KeywordIndex, MultiIndex, MultiKeywordIndex, hybrid_search, to_bf16_bits
 from tests.keyword_mirror import Mirror, zipf_docs, zipf_queries
-from tests.test_gpu_hybrid import ALPHAS, FUSIONS, QUERIES, _fill, _scopes, _shape, assert_row, host_fuse, weights
+from tests.test_gpu_hybrid import (ALPHAS, FUSIONS, QUERIES, _fill, _scopes, _shape, assert_row, c_hybrid_search, host_fuse,
+                                   weights)
 from tests.test_gpu_keyword_multi import _rows, union_corpus
 
 pytestmark = pytest.mark.gpu
@@ -122,7 +123,7 @@ def test_bit_exact_against_the_host_merge_and_fusion(n, nq, fetch, scope, layout
 
 
 def test_one_shard_equals_aur_hybrid_search(layout):
-    """n = 1 is aur_hybrid_search on the same shard and store: identical arrays."""
+    """n = 1 is aur_hybrid_search on the same shard and store: identical arrays (b calls aur_hybrid_search itself)."""
     m = _multi(1, layout)
     ix, kw = m.mi.shards[0], m.mk.stores[0]
     qv, qt, qo, rng = _queries(300, seed=4)
@@ -131,7 +132,7 @@ def test_one_shard_equals_aur_hybrid_search(layout):
     for fusion in FUSIONS:
         for fetch, k_out in ((1, 2), (16, 9), (128, 256)):
             a = hybrid_search(m.mi, m.mk, qv, fetch, qt, qo, wd, ws, fusion, k_out, q_user, q_org)
-            b = hybrid_search(ix, kw, qv, fetch, qt, qo, wd, ws, fusion, k_out, q_user, q_org)
+            b = c_hybrid_search(ix, kw, qv, fetch, qt, qo, wd, ws, fusion, k_out, q_user, q_org)
             for x, y in zip(a[:3], b[:3]):
                 assert x.dtype == y.dtype and np.array_equal(x.view(np.uint8), y.view(np.uint8))
             assert a[3] == ([b[3][0]], [b[3][1]])

@@ -614,22 +614,47 @@ def test_multi_index_one_process_many_shards():
 
 
 def test_results_written_straight_into_pinned_host_buffers():
-    """aur_search with page-locked result buffers: the re-rank kernel writes through the UVA mapping (no device-to-host
-    copies); same answer as with pageable buffers, including a multi-pass batch (> 1024 queries) and the generic kernel."""
+    """aur_search, aur_search_ex, aur_search_subset and aur_search_lists with page-locked result buffers: the re-rank
+    kernel writes through the UVA mapping (no device-to-host copies); same answer as with pageable buffers, including a
+    multi-pass batch (> 1024 queries) and the generic kernel."""
     import ctypes as C
+    from aurora_b200.engine import lists_csr
     torch = pytest.importorskip("torch")
+
+    def vp(a):
+        return C.c_void_p(a.ctypes.data)
 
     n, d, k = 30000, 768, 24
     for nq, kernel in ((70, N.KERNEL_AUTO), (1300, N.KERNEL_AUTO), (9, N.KERNEL_SIMT)):
         C_, Q = _data(n, d, nq, seed=nq)
+        rng = np.random.default_rng(nq)
+        allow = np.ascontiguousarray(rng.choice(n, size=n // 3, replace=False).astype(np.int64))
+        lists = [rng.choice(n, size=m, replace=False) for m in (50, 3000, 9000)]
+        q_list = np.ascontiguousarray(rng.integers(0, len(lists), size=nq), dtype=np.int32)
+        flat, offsets = lists_csr(lists)
         with Index(d, n) as ix:
             ix.add(C_, np.arange(n, dtype=np.int64))
             ix.set_kernel(kernel)
             want_ids, want_sc = ix.search(Q, k)                       # numpy (pageable) buffers
+            want = {"search": (want_ids, want_sc), "search_ex": (want_ids, want_sc),
+                    "subset": ix.search_subset(Q, k, allow), "lists": ix.search_lists(Q, k, lists, q_list)}
             q = torch.from_numpy(to_bf16_bits(Q).view(np.int16)).pin_memory()
-            h_sc = torch.full((nq, k), float("nan"), dtype=torch.float32).pin_memory()
-            h_id = torch.full((nq, k), -7, dtype=torch.int64).pin_memory()
-            N.check(ix._lib.aur_search(ix._h, C.c_void_p(q.data_ptr()), nq, k, None, None, C.c_void_p(h_sc.data_ptr()),
-                                       C.c_void_p(h_id.data_ptr())))
-            assert np.array_equal(h_id.numpy(), want_ids) and np.array_equal(h_sc.numpy(), want_sc)
+            qp = C.c_void_p(q.data_ptr())
+            snap = C.c_int64(-1)
+            calls = {
+                "search": lambda s, i: ix._lib.aur_search(ix._h, qp, nq, k, None, None, s, i),
+                "search_ex": lambda s, i: ix._lib.aur_search_ex(ix._h, qp, nq, k, None, None, s, i, C.byref(snap)),
+                "subset": lambda s, i: ix._lib.aur_search_subset(ix._h, qp, nq, k, vp(allow), allow.shape[0], s, i),
+                "lists": lambda s, i: ix._lib.aur_search_lists(ix._h, qp, nq, k, vp(flat), vp(offsets), len(lists),
+                                                               vp(q_list), s, i, C.byref(snap)),
+            }
+            for name, call in calls.items():
+                h_sc = torch.full((nq, k), float("nan"), dtype=torch.float32).pin_memory()
+                h_id = torch.full((nq, k), -7, dtype=torch.int64).pin_memory()
+                snap.value = -1
+                N.check(call(C.c_void_p(h_sc.data_ptr()), C.c_void_p(h_id.data_ptr())))
+                w_ids, w_sc = want[name]
+                assert np.array_equal(h_id.numpy(), w_ids) and np.array_equal(h_sc.numpy(), w_sc), name
+                if name in ("search_ex", "lists"):
+                    assert snap.value == n, name
         _check(want_ids, want_sc, *O.cosine_topk(Q, C_, k))
