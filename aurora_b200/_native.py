@@ -28,7 +28,7 @@ EXPORTS = [
     "aur_set_option", "aur_sync", "aur_add", "aur_add_dev", "aur_export", "aur_read_rows", "aur_compact", "aur_remove", "aur_search", "aur_search_ex", "aur_search_subset", "aur_search_lists", "aur_set_attrs", "aur_search_filtered", "aur_filter_ids", "aur_search_dev",
     "aur_merge_topk_dev", "aur_merge_topk_packed_dev", "aur_merge_topk_host", "aur_merge_topk_host_f64", "aur_exchange_create", "aur_exchange_connect", "aur_exchange_close",
     "aur_exchange_status", "aur_search_exchange_dev", "aur_cosine_pairs", "aur_dev_malloc", "aur_dev_free", "aur_memcpy_h2d", "aur_memcpy_d2h",
-    "aur_debug_tc_scores",
+    "aur_debug_tc_scores", "aur_debug_simt_scores", "aur_debug_list_scores",
     "aur_kw_open", "aur_kw_close", "aur_kw_add", "aur_kw_remove", "aur_kw_compact", "aur_kw_get_stats", "aur_kw_set_attrs",
     "aur_kw_search", "aur_kw_search_multi", "aur_kw_reindex", "aur_kw_set_option", "aur_kw_get_index_stats",
     "aur_kw_read_rows", "aur_kw_vocab_open", "aur_kw_vocab_close", "aur_kw_vocab_size", "aur_kw_vocab_read",
@@ -142,7 +142,9 @@ def load():
         "aur_dev_free": (C.c_int, [i32, vp]),
         "aur_memcpy_h2d": (C.c_int, [i32, vp, vp, C.c_uint64]),
         "aur_memcpy_d2h": (C.c_int, [i32, vp, vp, C.c_uint64]),
-        "aur_debug_tc_scores": (C.c_int, [vp, vp, i32, i32, vp, C.POINTER(i32), vp]),
+        "aur_debug_tc_scores": (C.c_int, [vp, vp, i32, i32, vp, i64, C.POINTER(i32), C.POINTER(i32), vp]),
+        "aur_debug_simt_scores": (C.c_int, [vp, vp, i32, vp, vp, vp, i64, C.POINTER(i64)]),
+        "aur_debug_list_scores": (C.c_int, [vp, vp, i32, vp, vp, i32, vp, vp, i64, C.POINTER(i64)]),
         "aur_kw_open": (C.c_int, [i32, i64, i64, C.POINTER(vp)]),
         "aur_kw_close": (C.c_int, [vp]),
         "aur_kw_add": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, i64]),

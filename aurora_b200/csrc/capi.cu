@@ -342,10 +342,14 @@ void resolve_ids(aur_index* ix, const int64_t* ids, int64_t n, int64_t n_rows, F
 // Corpus rows per tile when the index leaves it to the launch.  A 128-row tile (wgmma m64n128) fetches each operand for
 // twice the work of a 64-row one, but its layout leaves fewer, larger ring stages: it runs with at least
 // kTcWideMinStages stages, so at dim 1024, at large k and for most tenant-scoped batches the 64-row kernel stays.  The
-// bring-up score dump (dbg) keeps the 64-row tile it documents.
+// score dump (dbg) keeps 64-row tiles unless the index's tc_tile option asks for 128.
 int tc_auto_tile(int ksel, int dim, size_t smem_optin, bool mask, bool dbg) {
   if (dbg) return kTcTileN;
   return tc_pick_stages(ksel, dim, smem_optin, kTcTileWide, mask) >= kTcWideMinStages ? kTcTileWide : kTcTileN;
+}
+// The tile width a launch runs: the index's tc_tile option, else tc_auto_tile.
+int tc_tile(const aur_index* ix, int ksel, bool mask, bool dbg) {
+  return ix->opt_tc_tile ? ix->opt_tc_tile : tc_auto_tile(ksel, ix->dim, ix->smem_optin, mask, dbg);
 }
 
 // Query super-blocks of a two-CTA launch (CTA pairs of 128 queries each that walk the same tiles side by side, sharing
@@ -375,8 +379,7 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   int grid = (cta_group == 2) ? (pairs / n_super) * n_super * 2 : (ix->sm_count & ~1);
   const int n_lists = (cta_group == 2) ? pairs / n_super : grid / n_qblocks;   // tile sets = candidate lists per query
   const bool mask = row_mask != nullptr;
-  int tile_n = ix->opt_tc_tile;
-  if (tile_n == 0) tile_n = tc_auto_tile(ksel, ix->dim, ix->smem_optin, mask, dbg != nullptr);
+  const int tile_n = tc_tile(ix, ksel, mask, dbg != nullptr);
   // The width is settled (from the all-in-shared-memory layout); a 128-row launch then moves its first query k-blocks
   // into registers and spends the shared memory they leave on ring stages.
   // The bring-up switch that issues no MMAs (dbg_flags & 2) keeps the whole block in shared memory: without MMAs
@@ -504,6 +507,17 @@ int candidate_tail(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* qb, 
   return AUR_OK;
 }
 
+constexpr int64_t kSimtChunk = 16 * kSimtSeg;   // rows the generic kernel scores per launch (32768)
+constexpr int kSimtQBlock = 1024;               // queries per generic-kernel launch
+
+// The generic kernel's tenant filter for the queries from q0 on: their own codes, unless the scope is a row subset or
+// already folded into the inverse norms (inv).
+FilterArgs simt_filter(const aur_index* ix, const Scope& sc, const float* inv, int q0) {
+  FilterArgs f{ix->d_user, ix->d_org, nullptr, nullptr};
+  if (sc.n_allow < 0 && sc.q_user && !inv) { f.q_user = sc.q_user + q0; f.q_org = sc.q_org ? sc.q_org + q0 : nullptr; }
+  return f;
+}
+
 // Enqueues one search over the published prefix `n_rows` on stream s using context c, inside the call's stats.
 int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k, const Scope& sc, int64_t n_rows,
                    float* scores, int64_t* ids, double* scores64, cudaStream_t s,
@@ -545,7 +559,7 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
 
   // queries per launch: the generic kernel takes 1024; the tensor-core kernel 128 per CTA pair and up to four pairs side by
   // side on the same corpus tiles (fewer when k + slack is too large for the threshold exchange of that geometry)
-  int qstep = 1024;
+  int qstep = kSimtQBlock;
   if (kernel == AUR_KERNEL_TC1) qstep = 2 * kTcQRows;
   else if (kernel == AUR_KERNEL_TC2) qstep = tc2_super_blocks(ix, ksel, 4) * 2 * kTcQRows;
   for (int q0 = 0; q0 < nq; q0 += qstep) {
@@ -560,13 +574,11 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
       } else {
         n_lists = static_cast<int>((n_rows + kSimtSeg - 1) / kSimtSeg);
         CU_TRY(c->cand_a.reserve(static_cast<size_t>(nqb) * n_lists * ksel));
-        const int64_t chunk = 16 * kSimtSeg;  // 32768 rows of scores at a time
-        CU_TRY(c->score_chunk.reserve(static_cast<size_t>(nqb) * chunk));
-        FilterArgs f{ix->d_user, ix->d_org, nullptr, nullptr};
-        if (!subset && sc.q_user && !inv) { f.q_user = sc.q_user + q0; f.q_org = sc.q_org ? sc.q_org + q0 : nullptr; }
+        CU_TRY(c->score_chunk.reserve(static_cast<size_t>(nqb) * kSimtChunk));
+        const FilterArgs f = simt_filter(ix, sc, inv, q0);
         if (!k_timed) CU_TRY(cudaEventRecord(c->ev_k0, s));
-        for (int64_t r0 = 0; r0 < n_rows; r0 += chunk) {
-          const int64_t nr = (n_rows - r0 < chunk) ? n_rows - r0 : chunk;
+        for (int64_t r0 = 0; r0 < n_rows; r0 += kSimtChunk) {
+          const int64_t nr = std::min(n_rows - r0, kSimtChunk);
           CU_TRY(launch_simt_scores(qb, ix->d_rows, ix->dtype, ix->dim, nqb, r0, nr, n_rows, inv ? inv : ix->d_inv_norm, f,
                                     c->score_chunk.p, s));
           CU_TRY(launch_simt_select(c->score_chunk.p, nqb, r0, nr, ksel, ix->d_ids, c->cand_a.p, n_lists,
@@ -715,6 +727,16 @@ int check_list_args(aur_index* ix, const void* q, int32_t nq, int32_t k, const v
   if (ix->dtype == AUR_F32) return fail(AUR_ERR_UNSUPPORTED, "list search needs a bf16 or int8 index");
   return AUR_OK;
 }
+int check_lists(int32_t nq, const int64_t* list_ids, const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list) {
+  if (!list_offsets || !q_list || n_lists < 1) return fail(AUR_ERR_INVALID, "list_offsets, q_list and n_lists >= 1 are required");
+  if (list_offsets[0] != 0) return fail(AUR_ERR_INVALID, "list_offsets[0] must be 0");
+  for (int32_t l = 0; l < n_lists; ++l)
+    if (list_offsets[l + 1] < list_offsets[l]) return fail(AUR_ERR_INVALID, "list_offsets decrease at list %d", l);
+  if (list_offsets[n_lists] > 0 && !list_ids) return fail(AUR_ERR_INVALID, "list_ids is required");
+  for (int32_t q = 0; q < nq; ++q)
+    if (q_list[q] < 0 || q_list[q] >= n_lists) return fail(AUR_ERR_INVALID, "q_list[%d] = %d is not a list", q, q_list[q]);
+  return AUR_OK;
+}
 
 // The host side of a list search, built from the lists' lengths alone: blocks of queries, each with its work items cut
 // into launches, and the int32 staging the device side uploads in one copy.
@@ -784,6 +806,25 @@ int plan_list_search(int32_t nq, int32_t k, const int32_t* q_list, const std::ve
   return AUR_OK;
 }
 
+// The list kernels' arguments for launch ln of block b, once the plan is in c->list_stage and the queries in c->stage_q.
+ListParams list_params(const aur_index* ix, const SearchCtx* c, const ListPlan::Block& b, const ListPlan::Launch& ln,
+                       const int32_t* list_rows, int ksel) {
+  ListParams p{};
+  p.q = reinterpret_cast<const __nv_bfloat16*>(c->stage_q.p + static_cast<size_t>(b.q0) * ix->dim * 2);
+  p.rows = ix->d_rows;
+  p.rows_i8 = ix->dtype == AUR_I8;
+  p.inv_norm = ix->d_inv_norm;
+  p.ids = ix->d_ids;
+  p.items = reinterpret_cast<const ListItem*>(c->list_stage.p + ln.items);
+  p.n_items = ln.n_items;
+  p.list_rows = list_rows ? list_rows : c->list_stage.p;
+  p.qidx = c->list_stage.p;
+  p.scores = c->list_scores.p;
+  p.cand = c->cand_a.p;
+  p.dim = ix->dim; p.ksel = ksel; p.n_lists = b.n_segs;
+  return p;
+}
+
 // The device side of a planned list search over the queries in c->stage_q: the plan is uploaded, every block's work
 // items launched, and its candidates folded and re-ranked exactly into d_scores / d_ids.  list_rows: the lists' rows on
 // the device (nullptr: at the front of the plan's staging).
@@ -802,20 +843,7 @@ int run_list_search(aur_index* ix, SearchCtx* c, cudaStream_t s, const ListPlan&
     CU_TRY(cudaMemsetAsync(c->cand_a.p, 0, static_cast<size_t>(b.nqb) * b.n_segs * ksel * 8, s));   // 0 = empty slot
     if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k0, s));
     for (const ListPlan::Launch& ln : b.launches) {
-      ListParams p{};
-      p.q = reinterpret_cast<const __nv_bfloat16*>(qb);
-      p.rows = ix->d_rows;
-      p.rows_i8 = ix->dtype == AUR_I8;
-      p.inv_norm = ix->d_inv_norm;
-      p.ids = ix->d_ids;
-      p.items = reinterpret_cast<const ListItem*>(c->list_stage.p + ln.items);
-      p.n_items = ln.n_items;
-      p.list_rows = list_rows ? list_rows : c->list_stage.p;
-      p.qidx = c->list_stage.p;
-      p.scores = c->list_scores.p;
-      p.cand = c->cand_a.p;
-      p.dim = ix->dim; p.ksel = ksel; p.n_lists = b.n_segs;
-      CU_TRY(launch_list_search(p, ln.max_nq, s));
+      CU_TRY(launch_list_search(list_params(ix, c, b, ln, list_rows, ksel), ln.max_nq, s));
       c->last_launches += 2;
     }
     if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k1, s));
@@ -1381,13 +1409,7 @@ int aur_search_lists(aur_index* ix, const void* queries_host, int32_t nq, int32_
                      int64_t* ids_out, int64_t* snapshot_rows_out) {
   int rc = check_list_args(ix, queries_host, nq, k, scores_out, ids_out);
   if (rc != AUR_OK) return rc;
-  if (!list_offsets || !q_list || n_lists < 1) return fail(AUR_ERR_INVALID, "list_offsets, q_list and n_lists >= 1 are required");
-  if (list_offsets[0] != 0) return fail(AUR_ERR_INVALID, "list_offsets[0] must be 0");
-  for (int32_t l = 0; l < n_lists; ++l)
-    if (list_offsets[l + 1] < list_offsets[l]) return fail(AUR_ERR_INVALID, "list_offsets decrease at list %d", l);
-  if (list_offsets[n_lists] > 0 && !list_ids) return fail(AUR_ERR_INVALID, "list_ids is required");
-  for (int32_t q = 0; q < nq; ++q)
-    if (q_list[q] < 0 || q_list[q] >= n_lists) return fail(AUR_ERR_INVALID, "q_list[%d] = %d is not a list", q, q_list[q]);
+  if ((rc = check_lists(nq, list_ids, list_offsets, n_lists, q_list)) != AUR_OK) return rc;
   DenseQuery q{queries_host, nq, k};
   q.list_ids = list_ids; q.list_offsets = list_offsets; q.n_lists = n_lists; q.q_list = q_list;
   return search_into_host(ix, q, scores_out, ids_out, snapshot_rows_out);
@@ -1654,24 +1676,108 @@ int aur_memcpy_d2h(int32_t device, void* dst_host, const void* src_dev, uint64_t
 }
 
 int aur_debug_tc_scores(aur_index* ix, const void* queries_dev, int32_t nq, int32_t cta_group, float* out_dev,
-                        int32_t* n_ctas_out, void* stream) {
+                        int64_t out_cap, int32_t* n_ctas_out, int32_t* tile_n_out, void* stream) {
   if (!ix || !queries_dev || !out_dev) return fail(AUR_ERR_INVALID, "null argument");
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   CU_TRY(cudaSetDevice(ix->device));
   if (!ix->tmap_ok) return fail(AUR_ERR_UNSUPPORTED, "index shape has no tensor-core path");
-  if (ix->dtype == AUR_I8) return fail(AUR_ERR_UNSUPPORTED, "the tensor-core score dump is for bf16 shards");
   if (nq <= 0 || nq > 2 * kTcQRows) return fail(AUR_ERR_INVALID, "1..%d queries", 2 * kTcQRows);
+  const int ksel = 32 + kSlack;
+  const int n_ctas = ix->sm_count & ~1;   // run_tc_block's grid for up to 2 * kTcQRows queries, either cta_group
+  const int tile_n = tc_tile(ix, ksel, false, true);
+  const int64_t need = static_cast<int64_t>(n_ctas) * kTcQRows * tile_n;
+  if (out_cap < need)
+    return fail(AUR_ERR_INVALID, "out_dev holds %lld floats; the dump needs %d CTAs x %d x %d = %lld", (long long)out_cap, n_ctas,
+                kTcQRows, tile_n, (long long)need);
   int n_lists = 0;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
   SearchCtx* c = nullptr;
   int rc = acquire_ctx(ix, s, &c);
   if (rc != AUR_OK) return rc;
   std::lock_guard<std::mutex> cl(c->mu);
-  rc = run_tc_block(ix, c, cta_group, queries_dev, nq, 32 + kSlack, ix->rows_pub.load(std::memory_order_acquire), out_dev,
+  rc = run_tc_block(ix, c, cta_group, queries_dev, nq, ksel, ix->rows_pub.load(std::memory_order_acquire), out_dev,
                     &n_lists, s);
   if (rc != AUR_OK) return rc;
   CU_TRY(cudaMemsetAsync(c->cand_count.p, 0, 8 * kTcQRows * 4, s));  // no finalize ran to reset them
-  if (n_ctas_out) *n_ctas_out = ix->sm_count & ~1;
+  if (n_ctas_out) *n_ctas_out = n_ctas;
+  if (tile_n_out) *tile_n_out = tile_n;
+  return AUR_OK;
+}
+
+int aur_debug_simt_scores(aur_index* ix, const void* queries_host, int32_t nq, const int32_t* q_user, const int32_t* q_org,
+                          float* out_host, int64_t out_cap, int64_t* n_rows_out) {
+  int rc = check_search_args(ix, queries_host, nq, 1, out_host, out_host);
+  if (rc != AUR_OK) return rc;
+  if (nq > kSimtQBlock) return fail(AUR_ERR_INVALID, "1..%d queries: one block of a search", kSimtQBlock);
+  HostCall call(ix);
+  if ((rc = call.open()) != AUR_OK) return rc;
+  const int64_t n = call.n_rows;
+  if (n_rows_out) *n_rows_out = n;
+  if (out_cap < nq * n) return fail(AUR_ERR_INVALID, "out holds %lld floats; the dump needs %d x %lld", (long long)out_cap, nq, (long long)n);
+  SearchCtx* c = call.c;
+  if ((rc = call.stage(queries_host, nq, 1, nullptr, nullptr)) != AUR_OK) return rc;
+  Scope sc;
+  int32_t scope[2];
+  if (q_user && (rc = stage_tenant_scope(c, call.s, nq, q_user, q_org, scope, &sc)) != AUR_OK) return rc;
+  CU_TRY(c->score_chunk.reserve(static_cast<size_t>(nq) * kSimtChunk));
+  std::vector<float> chunk;
+  for (int64_t r0 = 0; r0 < n; r0 += kSimtChunk) {   // the chunks and launches of search_enqueue's generic path
+    const int64_t nr = std::min(n - r0, kSimtChunk);
+    chunk.resize(static_cast<size_t>(nq) * nr);
+    CU_TRY(cudaMemsetAsync(c->score_chunk.p, 0xFF, chunk.size() * 4, call.s));   // NaN wherever the kernel writes nothing
+    CU_TRY(launch_simt_scores(c->stage_q.p, ix->d_rows, ix->dtype, ix->dim, nq, r0, nr, n, ix->d_inv_norm,
+                              simt_filter(ix, sc, nullptr, 0), c->score_chunk.p, call.s));
+    CU_TRY(cudaMemcpyAsync(chunk.data(), c->score_chunk.p, chunk.size() * 4, cudaMemcpyDeviceToHost, call.s));
+    CU_TRY(cudaStreamSynchronize(call.s));
+    for (int32_t q = 0; q < nq; ++q)
+      std::copy(chunk.begin() + q * nr, chunk.begin() + (q + 1) * nr, out_host + q * n + r0);
+  }
+  return AUR_OK;
+}
+
+int aur_debug_list_scores(aur_index* ix, const void* queries_host, int32_t nq, const int64_t* list_ids,
+                          const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list, float* out_host, int64_t out_cap,
+                          int64_t* n_rows_out) {
+  int rc = check_list_args(ix, queries_host, nq, 1, out_host, out_host);
+  if (rc != AUR_OK) return rc;
+  if ((rc = check_lists(nq, list_ids, list_offsets, n_lists, q_list)) != AUR_OK) return rc;
+  DenseQuery q{queries_host, nq, 1};
+  q.list_ids = list_ids; q.list_offsets = list_offsets; q.n_lists = n_lists; q.q_list = q_list;
+  DensePart pt;
+  pt.call.reset(new HostCall(ix));
+  HostCall& call = *pt.call;
+  if ((rc = call.open()) != AUR_OK) return rc;
+  const int64_t n = call.n_rows;
+  if (n_rows_out) *n_rows_out = n;
+  if (out_cap < nq * n) return fail(AUR_ERR_INVALID, "out holds %lld floats; the dump needs %d x %lld", (long long)out_cap, nq, (long long)n);
+  SearchCtx* c = call.c;
+  if ((rc = call.stage(queries_host, nq, 1, nullptr, nullptr)) != AUR_OK) return rc;
+  if ((rc = prepare_scope(q, &pt)) != AUR_OK) return rc;   // the lists resolved and planned as aur_search_lists does
+  const ListPlan& pl = pt.pl;
+  CU_TRY(c->list_stage.reserve(pl.stage.size()));
+  CU_TRY(c->list_scores.reserve(std::max<size_t>(pl.max_slots, 1) * kSimtSeg));
+  CU_TRY(c->cand_a.reserve(pl.max_cand));
+  CU_TRY(cudaMemcpyAsync(c->list_stage.p, pl.stage.data(), pl.stage.size() * 4, cudaMemcpyHostToDevice, call.s));
+  std::fill(out_host, out_host + nq * n, nanf(""));
+  std::vector<float> sc;
+  for (const ListPlan::Block& b : pl.blocks)
+    for (const ListPlan::Launch& ln : b.launches) {
+      // every work item's scores: query b.q0 + qidx[q0 + g] against row list_rows[row0 + j] (the plan's host copy)
+      const ListItem* items = reinterpret_cast<const ListItem*>(pl.stage.data() + ln.items);
+      sc.resize(static_cast<size_t>(items[ln.n_items - 1].out + items[ln.n_items - 1].nq) * kSimtSeg);
+      CU_TRY(cudaMemsetAsync(c->list_scores.p, 0xFF, sc.size() * 4, call.s));   // NaN wherever the kernel writes nothing
+      CU_TRY(launch_list_search(list_params(ix, c, b, ln, nullptr, 1 + kSlack), ln.max_nq, call.s));
+      CU_TRY(cudaMemcpyAsync(sc.data(), c->list_scores.p, sc.size() * 4, cudaMemcpyDeviceToHost, call.s));
+      CU_TRY(cudaStreamSynchronize(call.s));
+      for (int i = 0; i < ln.n_items; ++i) {
+        const ListItem& it = items[i];
+        for (int g = 0; g < it.nq; ++g) {
+          float* row = out_host + (b.q0 + pl.stage[static_cast<size_t>(it.q0 + g)]) * n;
+          const float* src = sc.data() + static_cast<size_t>(it.out + g) * kSimtSeg;
+          for (int j = 0; j < it.n_rows; ++j) row[pl.stage[static_cast<size_t>(it.row0 + j)]] = src[j];
+        }
+      }
+    }
   return AUR_OK;
 }
 

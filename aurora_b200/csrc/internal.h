@@ -83,7 +83,7 @@ struct TcParams {
   uint64_t* cand;          // [64 * n_qblocks, n_lists * ksel] candidate keys, compacted per
                             // query: only keys that pass the final threshold are appended
   uint32_t* cand_count;     // [64 * n_qblocks] appended keys per query (zero on entry)
-  float* dbg_scores;        // optional [grid, 64, 64]: first tile's scores of every CTA
+  float* dbg_scores;        // optional [grid, 64, tile_n]: the whole first tile's scores of every CTA
   uint64_t* pub;            // cross-CTA threshold exchange, entries (epoch << 32 | score bits):
                             // [n_qblocks, 64, n_lists (even)] each CTA's m-th best per query,
                             // then [n_qblocks, 64] the served thresholds

@@ -292,7 +292,11 @@ constexpr uint32_t kNaNBits = 0x7FC00000u;
 // and hands the epilogue fmaf(acc_hi, 256, acc_lo): |acc| <= 127 * 128 * 1024 < 2^24, so both convert exactly and the
 // combination rounds once.  That is q16 . c, the cosine times a positive per-query factor: every comparison the
 // epilogue, the threshold exchange and the candidate keys make is between scores of one query, so nothing else changes.
-template <int kCtaGroup, bool kMask, int kTileN, int kQReg, bool kI8 = false>
+//
+// kDump: the score dump of aur_debug_tc_scores (unmasked launches only).  Every CTA writes its first tile's scores, as
+// the epilogue sees them before any selection, to p.dbg_scores.  A separate instantiation, so the kernels searches run
+// carry none of its code.
+template <int kCtaGroup, bool kMask, int kTileN, int kQReg, bool kI8 = false, bool kDump = false>
 __global__ void __launch_bounds__(kThreads, 1)
 simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   static_assert(kTileN == kTcTileN || kTileN == kTcTileWide, "tile width");
@@ -824,13 +828,15 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
             }
             cmax[c] = m;
           }
-          if (p.dbg_scores != nullptr && it == 0 && h == 0 && !(p.dbg_flags & 64)) {
+          if constexpr (kDump) {   // the score dump: the whole first tile, [CTA][query][kTileN]
+            if (it == 0) {
 #pragma unroll
-            for (int c = 0; c < 4; ++c)
+              for (int c = 0; c < 4; ++c)
 #pragma unroll
-              for (int j = 0; j < 16; ++j)
-                p.dbg_scores[(static_cast<size_t>(blockIdx.x) * kTcQRows + r) * kTcTileN + c * 16 + j] =
-                    __uint_as_float(acc[c][j]);
+                for (int j = 0; j < 16; ++j)
+                  p.dbg_scores[(static_cast<size_t>(blockIdx.x) * kTcQRows + r) * kTileN + h * 64 + c * 16 + j] =
+                      __uint_as_float(acc[c][j]);
+            }
           }
 
           t_fast += TCLK() - t_fast0;
@@ -942,13 +948,21 @@ simtopk_tc_kernel(const __grid_constant__ CUtensorMap tmap, const TcParams p) {
   if constexpr (kCtaGroup == 2) cluster_sync_all();
 }
 
-template <int kCtaGroup, bool kMask, int kTileN, int kQReg = 0, bool kI8 = false>
+template <int kCtaGroup, bool kMask, int kTileN, int kQReg, bool kI8, bool kDump = false>
 cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm, const TcParams& p, size_t smem) {
-  auto kern = simtopk_tc_kernel<kCtaGroup, kMask, kTileN, kQReg, kI8>;
+  auto kern = simtopk_tc_kernel<kCtaGroup, kMask, kTileN, kQReg, kI8, kDump>;
   // raised only: concurrent searches of the shards on one device ask for different sizes (raise_smem_limit)
   cudaError_t e = raise_smem_limit(reinterpret_cast<const void*>(kern), smem);
   if (e != cudaSuccess) return e;
   return cudaLaunchKernelEx(&cfg, kern, tm, p);
+}
+
+// The masked, the dumping (a score buffer without the per-thread counters of dbg_flags 64) or the plain kernel.
+template <int kCtaGroup, int kTileN, int kQReg, bool kI8>
+cudaError_t launch_kind(const cudaLaunchConfig_t& cfg, const CUtensorMap& tm, const TcParams& p, size_t smem) {
+  if (p.row_mask != nullptr) return launch_variant<kCtaGroup, true, kTileN, kQReg, kI8>(cfg, tm, p, smem);
+  if (p.dbg_scores != nullptr && !(p.dbg_flags & 64)) return launch_variant<kCtaGroup, false, kTileN, kQReg, kI8, true>(cfg, tm, p, smem);
+  return launch_variant<kCtaGroup, false, kTileN, kQReg, kI8>(cfg, tm, p, smem);
 }
 
 }  // namespace
@@ -978,27 +992,19 @@ cudaError_t tc_launch(int cta_group, int tile_n, int qregs, bool i8, int grid, c
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   const CUtensorMap& tm = *reinterpret_cast<const CUtensorMap*>(tmap);
-  const bool mask = p.row_mask != nullptr;
   if (i8) {
     if (qregs != 0 || p.dim % kTcKBlockI8 != 0) return cudaErrorInvalidValue;
-    if (tile_n == kTcTileWide) {
-      if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileWide, 0, true>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileWide, 0, true>(cfg, tm, p, smem);
-      return mask ? launch_variant<1, true, kTcTileWide, 0, true>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileWide, 0, true>(cfg, tm, p, smem);
-    }
-    if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileN, 0, true>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileN, 0, true>(cfg, tm, p, smem);
-    return mask ? launch_variant<1, true, kTcTileN, 0, true>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileN, 0, true>(cfg, tm, p, smem);
+    if (tile_n == kTcTileWide)
+      return cta_group == 2 ? launch_kind<2, kTcTileWide, 0, true>(cfg, tm, p, smem) : launch_kind<1, kTcTileWide, 0, true>(cfg, tm, p, smem);
+    return cta_group == 2 ? launch_kind<2, kTcTileN, 0, true>(cfg, tm, p, smem) : launch_kind<1, kTcTileN, 0, true>(cfg, tm, p, smem);
   }
   if (qregs != 0) {   // smem was sized without these k-blocks' tiles: only the matching kernel may run
     if (qregs != kTcQRegs || tile_n != kTcTileWide || p.dim / kTcKBlock < qregs) return cudaErrorInvalidValue;
-    if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileWide, kTcQRegs>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileWide, kTcQRegs>(cfg, tm, p, smem);
-    return mask ? launch_variant<1, true, kTcTileWide, kTcQRegs>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileWide, kTcQRegs>(cfg, tm, p, smem);
+    return cta_group == 2 ? launch_kind<2, kTcTileWide, kTcQRegs, false>(cfg, tm, p, smem) : launch_kind<1, kTcTileWide, kTcQRegs, false>(cfg, tm, p, smem);
   }
-  if (tile_n == kTcTileWide) {
-    if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileWide>(cfg, tm, p, smem);
-    return mask ? launch_variant<1, true, kTcTileWide>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileWide>(cfg, tm, p, smem);
-  }
-  if (cta_group == 2) return mask ? launch_variant<2, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<2, false, kTcTileN>(cfg, tm, p, smem);
-  return mask ? launch_variant<1, true, kTcTileN>(cfg, tm, p, smem) : launch_variant<1, false, kTcTileN>(cfg, tm, p, smem);
+  if (tile_n == kTcTileWide)
+    return cta_group == 2 ? launch_kind<2, kTcTileWide, 0, false>(cfg, tm, p, smem) : launch_kind<1, kTcTileWide, 0, false>(cfg, tm, p, smem);
+  return cta_group == 2 ? launch_kind<2, kTcTileN, 0, false>(cfg, tm, p, smem) : launch_kind<1, kTcTileN, 0, false>(cfg, tm, p, smem);
 }
 
 }  // namespace aur

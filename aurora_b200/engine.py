@@ -273,11 +273,45 @@ class Index:
                                          C.c_void_p(q_org_ptr), C.c_void_p(scores_ptr), C.c_void_p(ids_ptr),
                                          C.c_void_p(scores64_ptr), C.c_void_p(stream)))
 
+    DEBUG_TC_CAP = 1024 * N.TC_QUERY_ROWS * 64   # floats of the buffer debug_tc_scores' callers allocate
+
     def debug_tc_scores(self, q_ptr: int, nq: int, cta_group: int, out_ptr: int, stream: int = 0) -> int:
-        n = C.c_int32(0)
-        N.check(self._lib.aur_debug_tc_scores(self._h, C.c_void_p(q_ptr), int(nq), int(cta_group),
-                                              C.c_void_p(out_ptr), C.byref(n), C.c_void_p(stream)))
-        return int(n.value)
+        """``debug_tc_tile`` into a buffer of DEBUG_TC_CAP floats (room for 1024 CTAs of 64-row tiles).  Returns
+        n_ctas."""
+        return self.debug_tc_tile(q_ptr, nq, cta_group, out_ptr, self.DEBUG_TC_CAP, stream)[0]
+
+    def debug_tc_tile(self, q_ptr: int, nq: int, cta_group: int, out_ptr: int, out_cap: int,
+                      stream: int = 0) -> Tuple[int, int]:
+        """The tensor-core kernel's first corpus tile of every CTA into the device buffer ``out_ptr`` (``out_cap``
+        floats) as [n_ctas, 64, tile_n].  Returns (n_ctas, tile_n)."""
+        n, tile = C.c_int32(0), C.c_int32(0)
+        N.check(self._lib.aur_debug_tc_scores(self._h, C.c_void_p(q_ptr), int(nq), int(cta_group), C.c_void_p(out_ptr),
+                                              int(out_cap), C.byref(n), C.byref(tile), C.c_void_p(stream)))
+        return int(n.value), int(tile.value)
+
+    def debug_simt_scores(self, queries: np.ndarray, q_user=None, q_org=None) -> np.ndarray:
+        """The generic kernel's first-pass scores [nq, rows] as a search launches it (-inf: invisible row)."""
+        q = self._rows_buffer(queries)
+        nq, rows = q.shape[0], self.stats()["rows"]
+        out = np.empty((nq, rows), dtype=np.float32)
+        u = None if q_user is None else np.ascontiguousarray(q_user, dtype=np.int32)
+        o = None if q_org is None else np.ascontiguousarray(q_org, dtype=np.int32)
+        n = C.c_int64(0)
+        N.check(self._lib.aur_debug_simt_scores(self._h, _ptr(q), nq, _ptr(u), _ptr(o), _ptr(out), out.size, C.byref(n)))
+        return out.reshape(-1)[:nq * n.value].reshape(nq, n.value)   # [nq, rows the call saw]
+
+    def debug_list_scores(self, queries: np.ndarray, lists, q_list) -> np.ndarray:
+        """The list kernel's first-pass scores [nq, rows] of ``search_lists(queries, ., lists, q_list)``: query q's
+        score against every row of its list, NaN elsewhere."""
+        q = self._rows_buffer(queries)
+        nq, rows = q.shape[0], self.stats()["rows"]
+        flat, offsets = lists_csr(lists)
+        ql = np.ascontiguousarray(q_list, dtype=np.int32)
+        out = np.empty((nq, rows), dtype=np.float32)
+        n = C.c_int64(0)
+        N.check(self._lib.aur_debug_list_scores(self._h, _ptr(q), nq, _ptr(flat), _ptr(offsets), len(offsets) - 1,
+                                                _ptr(ql), _ptr(out), out.size, C.byref(n)))
+        return out.reshape(-1)[:nq * n.value].reshape(nq, n.value)   # [nq, rows the call saw]
 
     # -------------------------------------------------------------- misc
     def set_kernel(self, kernel: int) -> None:

@@ -57,7 +57,7 @@ typedef enum aur_status {
  * as zeros and never returned by a search (as in a bf16 shard).  Cosine ignores the per-row scale, so scores are exact
  * cosines against the stored int8 rows.  aur_export / aur_read_rows return the int8 rows.  The tensor-core kernel
  * serves int8 shards with dim % 128 == 0 and dim <= 1024 (wgmma s8 over a two-byte query image); "tc_qregs" does not
- * apply to them, and aur_debug_tc_scores is unsupported. */
+ * apply to them. */
 typedef enum aur_dtype { AUR_BF16 = 0, AUR_F32 = 1, AUR_I8 = 2 } aur_dtype;
 
 /* Which similarity kernel serves a search (aur_set_option "kernel"). */
@@ -635,9 +635,23 @@ int aur_debug_attention(int32_t device, const uint16_t* qkv, const int32_t* cu_s
                         float* ms_out);
 /* Final hidden states [tokens, hidden] (bf16 bits) of the last aur_encode call. */
 int aur_debug_encoder_hidden(aur_encoder* enc, uint16_t* out, int64_t count);
-int aur_debug_tc_scores(aur_index* ix, const void* queries_dev, int32_t nq,
-                        int32_t cta_group, float* out_dev /* [n_ctas,64,64] */,
-                        int32_t* n_ctas_out, void* stream);
+/* The tensor-core similarity kernel's first pass, before any selection: nq <= 128 queries (device bf16) against the
+ * published rows, launched with the index's tc_tile / tc_qregs options (an unset tc_tile means 64-row tiles here).  Every
+ * CTA writes the whole first corpus tile of its tile set, unscaled by |q|: out_dev [n_ctas, 64 queries, tile_n rows].
+ * For int8 rows a score is q16 . c times the row's inverse norm, q16 the kernel's 16-bit query image.  out_cap: floats
+ * out_dev holds; too few for n_ctas * 64 * tile_n fails with AUR_ERR_INVALID before anything runs. */
+int aur_debug_tc_scores(aur_index* ix, const void* queries_dev, int32_t nq, int32_t cta_group, float* out_dev,
+                        int64_t out_cap, int32_t* n_ctas_out, int32_t* tile_n_out, void* stream);
+/* The generic kernel's first-pass scores of nq <= 1024 queries (host, as aur_search) over every published row, launched
+ * as aur_search launches it (q_user / q_org: tenant codes as aur_search, nullable): out_host [nq, n_rows] row-major,
+ * -inf where a row is invisible, NaN where the kernel wrote nothing.  *n_rows_out = the rows; out_cap as above. */
+int aur_debug_simt_scores(aur_index* ix, const void* queries_host, int32_t nq, const int32_t* q_user,
+                          const int32_t* q_org, float* out_host, int64_t out_cap, int64_t* n_rows_out);
+/* The list kernel's first-pass scores of aur_search_lists(ix, queries_host, nq, ., list_ids, list_offsets, n_lists,
+ * q_list, ...): out_host [nq, n_rows], the score of query q against every row of its list, NaN elsewhere. */
+int aur_debug_list_scores(aur_index* ix, const void* queries_host, int32_t nq, const int64_t* list_ids,
+                          const int64_t* list_offsets, int32_t n_lists, const int32_t* q_list, float* out_host,
+                          int64_t out_cap, int64_t* n_rows_out);
 
 #ifdef __cplusplus
 }

@@ -32,3 +32,17 @@ def int8_to_bf16_bits(q: np.ndarray) -> np.ndarray:
     """int8 values -> bf16 bit patterns (every int8 value is exact in bf16)."""
     f = np.ascontiguousarray(q, dtype=np.float32)
     return (f.view(np.uint32) >> np.uint32(16)).astype(np.uint16)
+
+
+def query_image(bits: np.ndarray):
+    """bf16 queries [nq, dim] (uint16 bits) -> (q16, hi, lo) int64 [nq, dim]: the tensor-core kernel's 16-bit query image
+    of an int8 shard (query_image_i8_kernel).  q16 = rint(q * 32512 / amax_q): the product is exact in fp64 and the
+    quotient one correctly rounded division, half to even; a zero query stays zero.  Split exactly as q16 = 256 hi + lo
+    with hi = (q16 + 128) >> 8, an arithmetic shift (floor), so hi in [-127, 127] and lo in [-128, 127], both int8."""
+    x = bf16_bits_to_f64(np.atleast_2d(bits))
+    amax = np.abs(x).max(axis=1, initial=0.0)
+    ok = (amax > 0.0) & np.isfinite(amax)
+    safe = np.where(ok, amax, 1.0)
+    q16 = np.where(ok[:, None], np.rint((x * 32512.0) / safe[:, None]), 0.0).astype(np.int64)
+    hi = (q16 + 128) >> 8
+    return q16, hi, q16 - 256 * hi

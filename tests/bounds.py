@@ -17,6 +17,7 @@ from __future__ import annotations
 import numpy as np
 
 from oracle import bert_encoder as B
+from oracle import quantize as QZ
 from oracle.cosine_topk import round_to_bf16
 
 U = 2.0 ** -24
@@ -65,6 +66,57 @@ def sim_reference(Q, C):
     ref = (Q @ C.T) * inv[None, :]
     bound = K * U * (np.abs(Q) @ np.abs(C).T) * inv[None, :] + (K / 2 + 4) * U * np.abs(ref)
     return ref, bound
+
+
+def sim_reference_f32(Q, C):
+    """sim_reference for fp32 queries and rows (the generic kernel over an f32 shard).  Returns (ref, bound).
+
+    A product of two fp32 values is no longer exact in fp32.  simt_scores_kernel folds each product into its running sum
+    with one fmaf, one rounding per step, which the K u (|q| . |c|) term already covers; an evaluation that rounds the
+    product on its own first adds at most u |q_k c_k| per term.  So bound = sim_reference's bound + u (|q| . |c|) / |c|.
+    The inverse norm's sum of squares rounds the same way, inside its (K / 2 + 4) u |ref| term."""
+    Q, C = _f64(Q), _f64(C)
+    ref, bound = sim_reference(Q, C)
+    cn = np.sqrt(np.einsum("ij,ij->i", C, C))
+    inv = np.divide(1.0, cn, out=np.zeros_like(cn), where=cn > 0)
+    return ref, bound + U * (np.abs(Q) @ np.abs(C).T) * inv[None, :]
+
+
+def int8_inv_norm(R):
+    """The fp32 inverse norm of int8 rows as the ingest kernel computes it, bit for bit: the sum of squares is an integer
+    below 2^24 (dim <= 1024), exact in fp32 in any order, and sqrtf and the division round once each; 0 for a zero row."""
+    ss = (np.asarray(R, np.int64) ** 2).sum(axis=1).astype(np.float32)
+    return np.divide(np.float32(1), np.sqrt(ss), out=np.zeros_like(ss), where=ss > 0)
+
+
+def int8_tc_reference(q_bits, R):
+    """The tensor-core kernel's int8 first pass, exactly (float32 [nq, n]).  q16 = 256 hi + lo is the query image
+    (oracle/quantize.py:query_image); acc_hi = hi . c and acc_lo = lo . c are exact int32 sums (|acc| < 2^24); the kernel
+    forms fmaf(acc_hi, 256, acc_lo) from their exact fp32 conversions, one rounding of 256 acc_hi + acc_lo, and scales it
+    by the row's fp32 inverse norm (int8_inv_norm) with one more rounding.  The dump must equal this bit for bit."""
+    _, hi, lo = QZ.query_image(q_bits)
+    R = np.asarray(R, np.int64)
+    acc = 256 * (hi @ R.T) + lo @ R.T
+    return acc.astype(np.float32) * int8_inv_norm(R)[None, :]
+
+
+def int8_cosine_reference(q_bits, R):
+    """What the int8 first pass approximates: (ref, bound, scale).  score * scale[:, None] (scale = amax_q / 32512, the
+    query image's step) against ref = q . c / |c| in fp64 over the stored int8 rows c.
+
+    The image rounds each query element to the nearest multiple of amax_q / 32512, so it moves q_k by at most
+    amax_q / 65024 (the per-dimension bound of the int8 design), and the score by at most amax_q / 65024 . |c| / |c|.  The
+    kernel's fp32 work is two roundings of the combination and the final product plus the inverse norm's (sqrtf and a
+    division of an exact sum): 4 u of (|q| + amax_q / 65024) . |c| / |c|."""
+    q = QZ.bf16_bits_to_f64(np.atleast_2d(q_bits))
+    R = _f64(R)
+    cn = np.sqrt(np.einsum("ij,ij->i", R, R))
+    inv = np.divide(1.0, cn, out=np.zeros_like(cn), where=cn > 0)
+    step = np.abs(q).max(axis=1, initial=0.0)[:, None] / 65024
+    ref = (q @ R.T) * inv[None, :]
+    absc = np.abs(R).T * inv[None, :]
+    bound = step * absc.sum(axis=0)[None, :] + 4 * U * ((np.abs(q) + step) @ absc)
+    return ref, bound, 2 * step[:, 0]
 
 
 # ------------------------------------------------------------------------------------------------------ GEMM
@@ -184,3 +236,10 @@ def tc_debug_tile(cta: int, nq: int):
     takes query block c % 2 (its rank in a pair, or every other single CTA) and tile set c // 2."""
     n_qblocks = 1 if nq <= 64 else 2
     return cta % n_qblocks, cta // n_qblocks
+
+
+def tc_debug_rows(cta: int, nq: int, tile_n: int):
+    """(query block, corpus rows) of CTA ``cta``'s [64 queries x tile_n rows] tile from Index.debug_tc_tile, tile_n = 64
+    or 128 as the call reports: tile set t starts at tile t whatever the width, rows t tile_n .. t tile_n + tile_n - 1."""
+    qb, tile = tc_debug_tile(cta, nq)
+    return qb, tile * tile_n + np.arange(tile_n)

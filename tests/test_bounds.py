@@ -299,3 +299,131 @@ def test_bf16_helpers_round_to_nearest_and_toward_zero():
     assert round_to_bf16(x).tolist() == [1.0 + 2 ** -7, -(1.0 + 2 ** -7)]
     assert _rtz_bf16(x).tolist() == [1.0, -1.0]
     assert f32_to_bf16_bits(np.array([1.0], F32))[0] == 0x3F80
+
+
+# --------------------------------------------------------------------------------- int8 first pass (tensor cores)
+def emulate_int8_first_pass(q_bits, R, mutant=None):
+    """simtopk_tc.cu's int8 first pass as the kernel computes it: the query image of query_image_i8_kernel (fp32 amax,
+    fp64 product and division, rint), int32 MMAs over hi and lo, fmaf(acc_hi, 256, acc_lo) in fp32, times the row's
+    fp32 inverse norm.  Mutants: drop_lo (acc_lo never added); logical_hi (hi taken from a logical shift of the 16-bit
+    image, i.e. read as the unsigned byte, so a negative q16 gets hi + 256)."""
+    q = bf16_bits_to_f32(q_bits).astype(np.float64)
+    amax = np.abs(q).max(axis=1, initial=0.0)
+    v = np.where(amax[:, None] > 0, np.rint(q * 32512.0 / np.where(amax > 0, amax, 1.0)[:, None]), 0).astype(np.int64)
+    hi = (v + 128) >> 8
+    lo = v - 256 * hi
+    if mutant == "logical_hi":
+        hi = ((v + 128) & 0xFFFF) >> 8
+    R = np.asarray(R, np.int64)
+    acc_hi, acc_lo = (hi @ R.T).astype(F32), (lo @ R.T).astype(F32)
+    if mutant == "drop_lo":
+        acc_lo = np.zeros_like(acc_lo)
+    s = (acc_hi.astype(np.float64) * 256 + acc_lo.astype(np.float64)).astype(F32)   # fmaf: one rounding
+    ss = (R * R).sum(axis=1).astype(F32)
+    inv = np.divide(F32(1), np.sqrt(ss), out=np.zeros_like(ss), where=ss > 0)
+    return s * inv[None, :]
+
+
+def _int8_case(dim):
+    from aurora_b200.engine import to_bf16_bits
+    from oracle.quantize import quantize_rows
+
+    rng = np.random.default_rng(dim)
+    Q = rng.standard_normal((6, dim))
+    Q[1] = 0.0
+    Q[2, 3] = 40.0
+    C = rng.standard_normal((90, dim))
+    C[4] = 0.0
+    R, _ = quantize_rows(to_bf16_bits(C.astype(F32)))
+    return to_bf16_bits(Q.astype(F32)), R
+
+
+@pytest.mark.parametrize("dim", [128, 384, 1024])
+def test_int8_emulation_matches_the_exact_reference_and_the_cosine_bound(dim):
+    q_bits, R = _int8_case(dim)
+    got = emulate_int8_first_pass(q_bits, R)
+    assert np.array_equal(got, BD.int8_tc_reference(q_bits, R))
+    ref, bound, scale = BD.int8_cosine_reference(q_bits, R)
+    assert BD.ratio(got * scale[:, None], ref, bound) <= 1.0
+
+
+@pytest.mark.parametrize("mutant", ["drop_lo", "logical_hi"])
+@pytest.mark.parametrize("dim", [128, 384, 1024])
+def test_int8_mutant_fails_the_exact_reference_and_the_cosine_bound(mutant, dim):
+    q_bits, R = _int8_case(dim)
+    got = emulate_int8_first_pass(q_bits, R, mutant)
+    assert not np.array_equal(got, BD.int8_tc_reference(q_bits, R))
+    ref, bound, scale = BD.int8_cosine_reference(q_bits, R)
+    assert BD.ratio(got * scale[:, None], ref, bound) > 1.0
+
+
+# ---------------------------------------------------------------------------------------------- list kernel
+def emulate_list_scores(Q, C, lists, q_list, mutant=None):
+    """list_scores_kernel as a dense [nq, n] matrix (NaN where a query's list does not reach): the queries of a list in
+    groups of up to 64 (stable order), each row scored over ceil(dim / 64) zero-filled 64-dim chunks accumulated in fp32
+    (a chunk's products summed exactly: a model of the MMA), times the row's fp32 inverse norm.  Mutants: drop_last_chunk
+    (dim // 64 chunks); shifted_partial_group (the queries of a group's last, partial 16-row block read the query one row
+    further on, zeros past the group); neighbour_norm (a row takes the inverse norm of the next row of its list)."""
+    Q, C = Q.astype(F32), C.astype(F32)
+    nq, dim = Q.shape
+    inv = np.sqrt((C * C).sum(axis=1, dtype=F32))
+    inv = np.divide(F32(1), inv, out=np.zeros_like(inv), where=inv > 0)
+    n_kc = dim // 64 if mutant == "drop_last_chunk" else -(-dim // 64)
+    out = np.full((nq, C.shape[0]), np.nan)
+    order = np.argsort(q_list, kind="stable")
+    for l, rows in enumerate(lists):
+        rows = np.unique(rows)
+        qs = order[q_list[order] == l]
+        for g0 in range(0, len(qs), 64):
+            grp = qs[g0:g0 + 64]
+            Qg = Q[grp].copy()
+            full = len(grp) // 16 * 16
+            if mutant == "shifted_partial_group" and full < len(grp):
+                Qg[full:] = np.concatenate([Q[grp[full + 1:]], np.zeros((1, dim), F32)])
+            acc = np.zeros((len(grp), len(rows)), F32)
+            for kc in range(n_kc):
+                k = slice(kc * 64, min(dim, kc * 64 + 64))
+                acc = acc + (Qg[:, k].astype(np.float64) @ C[rows, k].T.astype(np.float64)).astype(F32)
+            nv = inv[np.roll(rows, -1)] if mutant == "neighbour_norm" else inv[rows]
+            out[np.ix_(grp, rows)] = acc * nv[None, :]
+    return out
+
+
+def _list_case(dim):
+    rng = np.random.default_rng(dim)
+    C = round_to_bf16(rng.standard_normal((300, dim)).astype(F32))
+    lists = [rng.choice(300, size=s, replace=False) for s in (65, 130, 7)]
+    q_list = rng.permutation(np.repeat(np.arange(3), [17, 70, 1])).astype(np.int32)
+    Q = round_to_bf16(rng.standard_normal((len(q_list), dim)).astype(F32))
+    return Q, C, lists, q_list
+
+
+@pytest.mark.parametrize("dim", [72, 200, 1536])
+def test_list_emulation_within_bound(dim):
+    Q, C, lists, q_list = _list_case(dim)
+    got = emulate_list_scores(Q, C, lists, q_list)
+    ref, bound = BD.sim_reference(Q, C)
+    m = np.isfinite(got)
+    assert m.sum() == sum(len(lists[l]) for l in q_list)
+    assert BD.ratio(got[m], ref[m], bound[m]) <= 1.0
+
+
+@pytest.mark.parametrize("mutant", ["drop_last_chunk", "shifted_partial_group", "neighbour_norm"])
+@pytest.mark.parametrize("dim", [72, 200])
+def test_list_mutant_fails_bound(mutant, dim):
+    Q, C, lists, q_list = _list_case(dim)
+    got = emulate_list_scores(Q, C, lists, q_list, mutant)
+    ref, bound = BD.sim_reference(Q, C)
+    m = np.isfinite(got)
+    assert BD.ratio(got[m], ref[m], bound[m]) > 1.0
+
+
+def test_f32_reference_covers_rounded_products():
+    """sim_reference_f32 admits a dot product whose fp32 products each round before an fp32 sum."""
+    rng = np.random.default_rng(3)
+    Q = rng.standard_normal((8, 1025)).astype(F32)
+    C = rng.standard_normal((40, 1025)).astype(F32)
+    inv = F32(1) / np.sqrt((C * C).sum(axis=1, dtype=F32))
+    got = np.stack([np.stack([np.add.reduce(q * c, dtype=F32) for c in C]) for q in Q]) * inv[None, :]
+    ref, bound = BD.sim_reference_f32(Q, C)
+    assert BD.ratio(got, ref, bound) <= 1.0
