@@ -181,6 +181,7 @@ struct aur_index {
   size_t elt = 2;                        // bytes per stored row element (int8 rows: 1)
   size_t qelt = 2;                       // bytes per query / input row element (bf16 for bf16 and int8 rows, f32 for f32)
   DevBuf<uint8_t> i8_stage;              // int8 shards: host bf16 rows on their way to the quantizer (writers hold mu_write)
+  DevBuf<int32_t> tomb_rows;             // aur_remove: the rows it tombstones, one upload (writers hold mu_write)
   void* d_rows = nullptr;
   float* d_inv_norm = nullptr;
   int64_t* d_ids = nullptr;
@@ -1123,6 +1124,7 @@ int aur_close(aur_index* ix) {
   cudaFree(ix->d_rows); cudaFree(ix->d_inv_norm); cudaFree(ix->d_ids); cudaFree(ix->d_user); cudaFree(ix->d_org);
   ix->attrs.release();
   ix->i8_stage.release();
+  ix->tomb_rows.release();
   for (auto& c : ix->ctxs) c->release();
   if (ix->stream) cudaStreamDestroy(ix->stream);
   if (ix->ingest_stream) cudaStreamDestroy(ix->ingest_stream);
@@ -1340,21 +1342,28 @@ int aur_remove(aur_index* ix, const int64_t* ids, int64_t n, int64_t* removed) {
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   std::lock_guard<std::mutex> wk(ix->mu_write);
   CU_TRY(cudaSetDevice(ix->device));
-  const float nanv = nanf("");
-  std::vector<int64_t> dead;
+  if (removed) *removed = 0;
+  if (n <= 0) return AUR_OK;
+  CU_TRY(ix->tomb_rows.reserve(static_cast<size_t>(n)));   // before id2row changes: a failure here removes nothing
+  std::vector<int32_t> dead;
   {
     std::lock_guard<std::mutex> lk(ix->mu);
     for (int64_t i = 0; i < n; ++i) {
       auto it = ix->id2row.find(ids[i]);
       if (it == ix->id2row.end()) continue;
-      dead.push_back(it->second);
+      dead.push_back(static_cast<int32_t>(it->second));
       ix->id2row.erase(it);
       --ix->live;
     }
   }
-  for (int64_t row : dead) CU_TRY(cudaMemcpyAsync(ix->d_inv_norm + row, &nanv, 4, cudaMemcpyHostToDevice, ix->ingest_stream));
-  CU_TRY(cudaStreamSynchronize(ix->ingest_stream));
-  if (removed) *removed = static_cast<int64_t>(dead.size());
+  const int64_t m = static_cast<int64_t>(dead.size());
+  cudaStream_t s = ix->ingest_stream;
+  if (m) {
+    CU_TRY(cudaMemcpyAsync(ix->tomb_rows.p, dead.data(), static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, s));
+    CU_TRY(launch_tombstone_rows(ix->tomb_rows.p, m, ix->d_inv_norm, s));
+    CU_TRY(cudaStreamSynchronize(s));   // dead is pageable host memory and goes out of scope
+  }
+  if (removed) *removed = m;
   return AUR_OK;
 }
 
@@ -1463,6 +1472,62 @@ int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const u
   if (m) CU_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToHost, s));
   CU_TRY(cudaStreamSynchronize(s));
   if (m) memcpy(ids_out, got.data(), static_cast<size_t>(m) * 8);
+  *n_out = n;
+  return AUR_OK;
+}
+
+int aur_filter_count(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,
+                     int64_t* n_out) {
+  if (!ix || !n_out) return fail(AUR_ERR_INVALID, "null argument");
+  if (n_tokens < 0) return fail(AUR_ERR_INVALID, "n_tokens < 0");
+  const int32_t off[2] = {0, n_tokens};
+  const FiltProgs fp{prog, off, 1, bitmap, bitmap_words, nullptr};
+  int rc = filter_check_programs(fp);
+  if (rc != AUR_OK || (rc = ix->attrs.check(fp, "shard")) != AUR_OK) return rc;
+  HostCall call(ix);
+  if ((rc = call.open()) != AUR_OK) return rc;
+  if ((rc = filter_count(ix, call.c, call.s, fp, call.n_rows)) != AUR_OK) return rc;
+  CU_TRY(cudaStreamSynchronize(call.s));
+  std::vector<int64_t> tot;
+  filter_totals(call.c, 1, &tot);
+  *n_out = tot[0];
+  return AUR_OK;
+}
+
+int aur_remove_filtered(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,
+                        int64_t* ids_out, int64_t cap, int64_t* n_out) {
+  if (!ix || !n_out || cap < 0 || (cap > 0 && !ids_out)) return fail(AUR_ERR_INVALID, "null argument");
+  if (n_tokens < 0) return fail(AUR_ERR_INVALID, "n_tokens < 0");
+  const int32_t off[2] = {0, n_tokens};
+  const FiltProgs fp{prog, off, 1, bitmap, bitmap_words, nullptr};
+  int rc = filter_check_programs(fp);
+  if (rc != AUR_OK || (rc = ix->attrs.check(fp, "shard")) != AUR_OK) return rc;
+  HostCall call(ix);
+  // the writer lock, as aur_remove takes it: no append publishes rows and no other delete runs until the matching rows
+  // are tombstones and their ids have left id2row, so the rows counted are the rows removed
+  std::lock_guard<std::mutex> wk(ix->mu_write);
+  if ((rc = call.open()) != AUR_OK) return rc;
+  SearchCtx* c = call.c;
+  cudaStream_t s = call.s;
+  if ((rc = filter_count(ix, c, s, fp, call.n_rows)) != AUR_OK) return rc;
+  CU_TRY(cudaStreamSynchronize(s));
+  std::vector<int64_t> tot;
+  filter_totals(c, 1, &tot);
+  const int64_t n = tot[0];
+  if (n == 0 || n > cap) {   // nothing to remove, or no room for the ids: nothing removed, the caller retries
+    *n_out = n;
+    return AUR_OK;
+  }
+  if ((rc = filter_write(ix, c, s, 1, tot, call.n_rows, true)) != AUR_OK) return rc;
+  CU_TRY(launch_tombstone_rows(c->filt_rows.p, n, ix->d_inv_norm, s));
+  std::vector<int64_t> got(static_cast<size_t>(n));
+  CU_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost, s));
+  CU_TRY(cudaStreamSynchronize(s));
+  {
+    std::lock_guard<std::mutex> lk(ix->mu);
+    for (int64_t id : got) ix->live -= static_cast<int64_t>(ix->id2row.erase(id));
+  }
+  memcpy(ids_out, got.data(), static_cast<size_t>(n) * 8);
   *n_out = n;
   return AUR_OK;
 }

@@ -753,6 +753,18 @@ cudaError_t launch_scatter_inv_norm(const float* inv, const int32_t* rows, int64
   return cudaGetLastError();
 }
 
+// Deletes: the listed rows become tombstones (NaN inverse norm, or NaN scale on an int8 shard), one thread per row.
+__global__ void tombstone_rows_kernel(const int32_t* __restrict__ rows, int64_t n, float* __restrict__ inv) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n) inv[rows[i]] = __uint_as_float(0x7FC00000u);
+}
+
+cudaError_t launch_tombstone_rows(const int32_t* rows, int64_t n, float* inv, cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  tombstone_rows_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(rows, n, inv);
+  return cudaGetLastError();
+}
+
 // Compaction: gather the rows listed in map (and their side arrays) into bounce buffers.  One warp per row,
 // 16-byte pieces (row_bytes % 16 == 0 for bf16 dims % 8 == 0 and for f32 dims % 4 == 0; else byte loop).
 __global__ void gather_rows_kernel(const uint8_t* __restrict__ rows, const float* __restrict__ inv, const int64_t* __restrict__ ids,

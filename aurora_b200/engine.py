@@ -266,6 +266,31 @@ class Index:
                 return out[:n.value]
             cap = int(n.value)
 
+    def count_filtered(self, program) -> int:
+        """How many live rows one ``filters.compile_program`` program matches (counted on the device)."""
+        from .filters import pack_programs
+
+        tok, _, bm = pack_programs([program])
+        n = C.c_int64(0)
+        N.check(self._lib.aur_filter_count(self._h, _ptr(tok), tok.shape[0], _ptr(bm), bm.shape[0], C.byref(n)))
+        return int(n.value)
+
+    def remove_filtered(self, program) -> np.ndarray:
+        """Delete every live row one ``filters.compile_program`` program matches; returns their ids in row order.  The
+        rows are found and tombstoned on the device under the shard's writer lock."""
+        from .filters import pack_programs
+
+        tok, _, bm = pack_programs([program])
+        cap = 1 << 16
+        while True:                 # more matches than room removes nothing and reports the count: retry with room
+            out = np.empty(cap, dtype=np.int64)
+            n = C.c_int64(0)
+            N.check(self._lib.aur_remove_filtered(self._h, _ptr(tok), tok.shape[0], _ptr(bm), bm.shape[0], _ptr(out), cap,
+                                                  C.byref(n)))
+            if n.value <= cap:
+                return out[:n.value]
+            cap = int(n.value)
+
     def search_dev(self, q_ptr: int, nq: int, k: int, scores_ptr: int, ids_ptr: int, scores64_ptr: int = 0,
                    q_user_ptr: int = 0, q_org_ptr: int = 0, stream: int = 0) -> None:
         """Everything in HBM; asynchronous on ``stream`` (0 = the index's own stream)."""
@@ -452,6 +477,13 @@ class MultiIndex:
 
     def filter_ids(self, program) -> np.ndarray:
         return np.concatenate(self._each(lambda s, shard: shard.filter_ids(program)))
+
+    def count_filtered(self, program) -> int:
+        return int(sum(self._each(lambda s, shard: shard.count_filtered(program))))
+
+    def remove_filtered(self, program) -> np.ndarray:
+        """Index.remove_filtered on every shard at once; the removed ids shard after shard."""
+        return np.concatenate(self._each(lambda s, shard: shard.remove_filtered(program)))
 
     # -------------------------------------------------------------- maintenance
     def stats(self) -> dict:

@@ -158,7 +158,7 @@ def delete_incident_knowledge(user_id: str, incident_id: str) -> bool:
     """incident_feedback/weaviate_client.py:331-361.  True unless the backend failed."""
     try:
         f = Filter.by_property("user_id").equal(user_id) & Filter.by_property("incident_id").equal(incident_id)
-        n = _get_kb().delete_where(f.matches)
+        n = _get_kb().delete_where(f)
         logger.info(f"[AURORA LEARN B200] Deleted {n} knowledge entries for incident {_sanitize(incident_id)}")
         return True
     except Exception as e:
@@ -169,7 +169,7 @@ def delete_incident_knowledge(user_id: str, incident_id: str) -> bool:
 def delete_user_knowledge(user_id: str) -> int:
     """incident_feedback/weaviate_client.py:364-386.  Deleted count; -1 on error."""
     try:
-        n = _get_kb().delete_where(Filter.by_property("user_id").equal(user_id).matches)
+        n = _get_kb().delete_where(Filter.by_property("user_id").equal(user_id))
         logger.info(f"[AURORA LEARN B200] Deleted {n} knowledge entries for user {_sanitize(user_id)}")
         return n
     except Exception as e:

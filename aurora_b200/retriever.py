@@ -37,7 +37,7 @@ import numpy as np
 from . import bm25
 from ._native import AUR_BF16, AUR_I8, FUSION_RANKED, FUSION_RELATIVE_SCORE
 from .bm25 import BM25Index
-from .filters import AttrColumn, Filter, HybridFusion, compile_program  # noqa: F401  (Filter, HybridFusion: re-exported)
+from .filters import AttrColumn, Filter, HybridFusion, _Expr, compile_program  # noqa: F401  (Filter, HybridFusion: re-exported)
 
 logger = logging.getLogger(__name__)
 
@@ -666,34 +666,60 @@ class KnowledgeBase:
         return kb
 
     # ------------------------------------------------------------------ deletes / counts
+    def _delete_program(self, pred):
+        """``pred`` as a device program for ``remove_filtered`` / ``count_filtered``, or None when it is resolved by the
+        host scan: a plain predicate (not a ``Filter`` expression), an index without those calls (CPU doubles, a
+        ``MultiIndex`` of them), or whatever keeps ``_device_program`` on the host.  Caller holds the lock."""
+        shards = getattr(self.index, "shards", [self.index])
+        if not isinstance(pred, _Expr) or not all(hasattr(sh, "remove_filtered") for sh in [self.index, *shards]):
+            return None
+        return self._device_program(pred, False, None, None)
+
     def _matching_ids(self, pred) -> List[int]:
-        return [rid for rid, p in self._props.items() if pred(p)]
+        match = pred.matches if isinstance(pred, _Expr) else pred
+        return [rid for rid, p in self._props.items() if match(p)]
 
     def delete_where(self, pred) -> int:
+        """Delete the objects ``pred`` matches (a ``Filter`` expression or a predicate over the properties); returns how
+        many.  An expression that compiles to a device program is resolved on the GPU, so host work follows the matching
+        objects, not the store's size."""
         with self._lock:
-            return self._delete_ids(self._matching_ids(pred))
+            prog = self._delete_program(pred)
+            if prog is None:
+                return self._delete_ids(self._matching_ids(pred))
+            ids = [int(r) for r in self.index.remove_filtered(prog)]
+            if ids:
+                self._forget_ids(ids)
+            return len(ids)
 
     def _delete_ids(self, ids: List[int]) -> int:
         with self._lock:
             if ids:
-                gen = self.mutations
-                keys = [self._id2key.get(rid) for rid in ids]
                 self.index.remove(np.array(ids, dtype=np.int64))
-                if self._kw_device:
-                    self.sparse.remove_many(ids)
-                for rid in ids:
-                    p = self._props.pop(rid)
-                    self._unindex(rid, p)
-                    if not self._kw_device:
-                        self.sparse.remove(rid)
-                    self._key2id.pop(self._id2key.pop(rid, None), None)
-                self.mutations += len(ids)
-                self._log({"op": "del", "gen": gen, "keys": [k for k in keys if k]})
+                self._forget_ids(ids)
             return len(ids)
 
+    def _forget_ids(self, ids: List[int]) -> None:
+        """Everything but the vector shard's rows of deleted objects: the keyword store's, their properties and keys, the
+        mutation count and the log record.  Caller holds the lock."""
+        gen = self.mutations
+        keys = [self._id2key.get(rid) for rid in ids]
+        if self._kw_device:
+            self.sparse.remove_many(ids)
+        for rid in ids:
+            p = self._props.pop(rid)
+            self._unindex(rid, p)
+            if not self._kw_device:
+                self.sparse.remove(rid)
+            self._key2id.pop(self._id2key.pop(rid, None), None)
+        self.mutations += len(ids)
+        self._log({"op": "del", "gen": gen, "keys": [k for k in keys if k]})
+
     def count_where(self, pred) -> int:
+        """How many objects ``pred`` matches; counted on the GPU under the same rule as ``delete_where``."""
         with self._lock:
-            return len(self._matching_ids(pred))
+            prog = self._delete_program(pred)
+            return len(self._matching_ids(pred)) if prog is None else self.index.count_filtered(prog)
 
 
 # ---------------------------------------------------------------------- façade for _get_weaviate_client()
@@ -835,7 +861,8 @@ def search_knowledge_base_batch(requests: List[Tuple]) -> List[List[Dict[str, An
 def delete_document_chunks(user_id: str, document_id: str) -> int:
     """weaviate_client.py:288-319.  Deleted count; -1 on error."""
     try:
-        return _get_kb().delete_where(lambda p: p.get("user_id") == user_id and p.get("document_id") == document_id)
+        return _get_kb().delete_where(Filter.by_property("user_id").equal(user_id)
+                                      & Filter.by_property("document_id").equal(document_id))
     except Exception as e:
         logger.error(f"[KB B200] Error deleting chunks for doc {_sanitize(document_id)}: {_sanitize(e)}")
         return -1
@@ -844,7 +871,7 @@ def delete_document_chunks(user_id: str, document_id: str) -> int:
 def delete_user_chunks(user_id: str) -> int:
     """weaviate_client.py:322-344.  Deleted count; -1 on error."""
     try:
-        return _get_kb().delete_where(lambda p: p.get("user_id") == user_id)
+        return _get_kb().delete_where(Filter.by_property("user_id").equal(user_id))
     except Exception as e:
         logger.error(f"[KB B200] Error deleting chunks for user {_sanitize(user_id)}: {_sanitize(e)}")
         return -1
@@ -853,7 +880,8 @@ def delete_user_chunks(user_id: str) -> int:
 def get_document_chunk_count(user_id: str, document_id: str) -> int:
     """weaviate_client.py:347-371.  0 on error."""
     try:
-        return _get_kb().count_where(lambda p: p.get("user_id") == user_id and p.get("document_id") == document_id)
+        return _get_kb().count_where(Filter.by_property("user_id").equal(user_id)
+                                     & Filter.by_property("document_id").equal(document_id))
     except Exception as e:
         logger.error(f"[KB B200] Error getting chunk count: {e}")
         return 0
@@ -866,7 +894,7 @@ def delete_discovery_chunks(org_id: str, before: str = None) -> int:
         f = Filter.by_property("org_id").equal(org_id) & Filter.by_property("document_id").like("discovery:*")
         if before:
             f = f & Filter.by_property("created_at").less_than(before)
-        return _get_kb().delete_where(f.matches)
+        return _get_kb().delete_where(f)
     except Exception as e:
         logger.error(f"[KB B200] Error deleting discovery chunks: {e}")
         return 0

@@ -142,9 +142,8 @@ int aur_read_rows(aur_index* ix, int64_t row0, int64_t n, void* rows_out, int64_
  * (nullable) receives the number of rows freed. */
 int aur_compact(aur_index* ix, int64_t* reclaimed);
 
-/* Deletes.  Replaces collection.data.delete_many(where=...) (weaviate_client.py:309,
- * :336, :387): the Python layer resolves the filter to ids; rows become tombstones.
- * *removed receives how many ids were live. */
+/* Deletes by id: the rows of the live ids among ids[0, n) become tombstones (one upload of their rows, one kernel
+ * launch).  *removed receives how many ids were live.  aur_remove_filtered deletes by filter without naming ids. */
 int aur_remove(aur_index* ix, const int64_t* ids, int64_t n, int64_t* removed);
 
 /* Search.  Replaces the dense leg of collection.query.hybrid (weaviate_client.py:252-259)
@@ -221,6 +220,18 @@ int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int
  * *n_out receives how many there are (call again with a larger cap when it exceeds cap). */
 int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,
                    int64_t* ids_out, int64_t cap, int64_t* n_out);
+/* The number of live rows one program matches in the published prefix: the count pass of aur_filter_ids alone, no row
+ * or id leaves the device.  Replaces collection.aggregate.over_all(filters=...) (weaviate_client.py:366). */
+int aur_filter_count(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,
+                     int64_t* n_out);
+/* Deletes by filter.  Replaces collection.data.delete_many(where=...) (weaviate_client.py:309, :336, :387): every live
+ * row one program matches becomes a tombstone (one kernel launch over the matching rows), its id leaves the shard, and
+ * the removed ids go to ids_out in row order; *n_out receives how many.  Holds the writer lock throughout, as aur_remove
+ * does, so the rows removed are exactly the rows published when the call began that matched.  When there are more than
+ * cap, nothing is removed and *n_out receives how many there are: call again with a larger cap.  A malformed program or
+ * an attribute column never set is rejected (AUR_ERR_INVALID) with nothing removed and the outputs untouched. */
+int aur_remove_filtered(aur_index* ix, const int32_t* prog, int32_t n_tokens, const uint32_t* bitmap, int64_t bitmap_words,
+                        int64_t* ids_out, int64_t cap, int64_t* n_out);
 /* Device variant: everything in HBM; scores64_dev (nullable) additionally receives the
  * fp64 ranking keys needed for an exact cross-shard merge. */
 int aur_search_dev(aur_index* ix, const void* queries_dev, int32_t nq, int32_t k,
