@@ -217,27 +217,23 @@ int forward_locked(aur_encoder* e, const int32_t* cu_host, int n_seq, int n_item
   return AUR_OK;
 }
 
-int stage_inputs(aur_encoder* e, const int32_t* tokens, const int32_t* cu, int n_seq, int* n_items_out) {
-  const aur_encoder_config& c = e->cfg;
+int check_loaded(aur_encoder* e) {
+  std::lock_guard<std::mutex> g(e->mu);
   if (!e->missing.empty())
     return report_error(AUR_ERR_INVALID, "encoder parameters not loaded: %s (+%zu more)", e->missing[0].c_str(), e->missing.size() - 1);
+  return AUR_OK;
+}
+
+// aur_encode's and aur_encode_append's own checks, before any device work: the parameters loaded, and the sequences one
+// batch of the workspace (at most max_seqs sequences of at most max_tokens tokens in all).
+int check_one_batch(aur_encoder* e, const int32_t* tokens, const int32_t* cu, int32_t n_seq) {
+  const aur_encoder_config& c = e->cfg;
+  int rc = check_loaded(e);
+  if (rc != AUR_OK) return rc;
   if (!tokens || !cu || n_seq <= 0) return report_error(AUR_ERR_INVALID, "tokens / cu_seqlens / n_seq");
   if (n_seq > c.max_seqs) return report_error(AUR_ERR_NOMEM, "n_seq %d > max_seqs %d", n_seq, c.max_seqs);
   if (cu[0] != 0) return report_error(AUR_ERR_INVALID, "cu_seqlens[0] must be 0");
-  const int64_t T = cu[n_seq];
-  if (T > c.max_tokens) return report_error(AUR_ERR_NOMEM, "%lld tokens > max_tokens %d", static_cast<long long>(T), c.max_tokens);
-  int n_items = 0;
-  for (int i = 0; i < n_seq; ++i) {
-    const int len = cu[i + 1] - cu[i];
-    if (len < 1 || len > c.max_pos) return report_error(AUR_ERR_INVALID, "sequence %d has length %d (1..%d)", i, len, c.max_pos);
-    for (int t = 0; t < len; ++t) {
-      const int32_t id = tokens[cu[i] + t];
-      if (id < 0 || id >= c.vocab) return report_error(AUR_ERR_INVALID, "token id %d out of range at sequence %d", id, i);
-      e->h_tok[cu[i] + t] = id; e->h_pos[cu[i] + t] = t;
-    }
-    for (int q0 = 0; q0 < len; q0 += 128) e->h_items[n_items++] = AttnItem{cu[i], len, q0, 0};
-  }
-  *n_items_out = n_items;
+  if (cu[n_seq] > c.max_tokens) return report_error(AUR_ERR_NOMEM, "%d tokens > max_tokens %d", cu[n_seq], c.max_tokens);
   return AUR_OK;
 }
 
@@ -352,7 +348,38 @@ int run_texts(aur_encoder* e, const Texts& in, const int32_t* q, int32_t nq, int
   return AUR_OK;
 }
 
-// aur_encode_append_texts_multi, and aur_encode_append_multi with in.cu_texts = NULL (one window per text).
+// aur_encode_texts after its argument checks, and aur_encode with in.cu_texts = NULL (one window per text): every text
+// through e's whole workspace.  out_f32 / out_bf16 are written only on success.  One output of windows that fit one
+// batch (every aur_encode call that asks for one) is copied straight into the caller's buffer, behind the forward on
+// e's stream, which a failed forward never gets past.  Several batches, or both outputs (the first copy could land
+// before the second fails), are staged on the host and copied out once everything has succeeded.
+int encode_texts(aur_encoder* e, const Texts& in, int32_t n_seq, int32_t n_texts, float* out_f32, uint16_t* out_bf16) {
+  int rc = check_texts(e->cfg, in, n_seq, n_texts, e->cfg.max_tokens);
+  if (rc != AUR_OK) return rc;
+  const size_t H = e->cfg.hidden;
+  const bool one_batch = n_seq <= e->cfg.max_seqs && in.cu[n_seq] <= e->cfg.max_tokens;
+  const bool direct = one_batch && !(out_f32 && out_bf16);
+  std::vector<float> f32(out_f32 && !direct ? static_cast<size_t>(n_texts) * H : 0);
+  std::vector<uint16_t> bf16(out_bf16 && !direct ? static_cast<size_t>(n_texts) * H : 0);
+  float* const to_f32 = direct || !out_f32 ? out_f32 : f32.data();
+  uint16_t* const to_bf16 = direct || !out_bf16 ? out_bf16 : bf16.data();
+  std::vector<int32_t> q(static_cast<size_t>(n_texts));
+  for (int32_t j = 0; j < n_texts; ++j) q[j] = j;
+  rc = run_texts(e, in, q.data(), n_texts, e->cfg.max_tokens, e->cfg.max_seqs,
+                 [&](aur_encoder* enc, const int32_t* qs, int n, const float* rows) -> int {
+                   const size_t at = static_cast<size_t>(qs[0]) * H, len = static_cast<size_t>(n) * H;
+                   if (to_f32) ENC_TRY(cudaMemcpyAsync(to_f32 + at, rows, len * sizeof(float), cudaMemcpyDeviceToHost, enc->stream));
+                   if (to_bf16) ENC_TRY(cudaMemcpyAsync(to_bf16 + at, enc->d_pool_bf16, len * 2, cudaMemcpyDeviceToHost, enc->stream));
+                   return AUR_OK;
+                 });
+  if (rc != AUR_OK) return rc;
+  if (!f32.empty()) memcpy(out_f32, f32.data(), f32.size() * sizeof(float));
+  if (!bf16.empty()) memcpy(out_bf16, bf16.data(), bf16.size() * 2);
+  return AUR_OK;
+}
+
+// aur_encode_append_texts_multi, aur_encode_append_multi with in.cu_texts = NULL (one window per text), and
+// aur_encode_append, which is that with n = 1 after its one-batch checks.
 int append_texts_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const Texts& in, int32_t n_seq,
                        int32_t n_texts, const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes,
                        int32_t max_tokens_per_call, int32_t max_seqs_per_call) {
@@ -565,42 +592,17 @@ int aur_encoder_load(aur_encoder* e, const char* name, const float* data, int64_
 
 int aur_encode(aur_encoder* e, const int32_t* tokens, const int32_t* cu, int32_t n_seq, float* out_f32, uint16_t* out_bf16) {
   if (!e) return report_error(AUR_ERR_INVALID, "null encoder");
-  std::lock_guard<std::mutex> g(e->mu);
-  ENC_TRY(cudaSetDevice(e->cfg.device));
-  int n_items = 0, rc;
-  if ((rc = stage_inputs(e, tokens, cu, n_seq, &n_items))) return rc;
-  if ((rc = forward_locked(e, cu, n_seq, n_items))) return rc;
-  const size_t n = static_cast<size_t>(n_seq) * e->cfg.hidden;
-  // outputs are written only on success: copy into the caller's buffers after the forward is known good
-  ENC_TRY(cudaStreamSynchronize(e->stream));
-  if (out_f32) ENC_TRY(cudaMemcpy(out_f32, e->d_pool_f32, n * sizeof(float), cudaMemcpyDeviceToHost));
-  if (out_bf16) ENC_TRY(cudaMemcpy(out_bf16, e->d_pool_bf16, n * 2, cudaMemcpyDeviceToHost));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]);
-  e->stats.total_ms = ms;
-  return AUR_OK;
+  const int rc = check_one_batch(e, tokens, cu, n_seq);
+  if (rc != AUR_OK) return rc;
+  return encode_texts(e, Texts{tokens, cu, nullptr}, n_seq, n_seq, out_f32, out_bf16);
 }
 
 int aur_encode_append(aur_encoder* e, aur_index* ix, const int32_t* tokens, const int32_t* cu, int32_t n_seq,
                       const int64_t* ids, const int32_t* user_codes, const int32_t* org_codes) {
   if (!e || !ix || !ids) return report_error(AUR_ERR_INVALID, "null argument");
-  std::lock_guard<std::mutex> g(e->mu);
-  ENC_TRY(cudaSetDevice(e->cfg.device));
-  aur_stats st{};
-  int rc;
-  if ((rc = aur_get_stats(ix, &st))) return rc;
-  if (st.dim != e->cfg.hidden || st.dtype == AUR_F32)   // (an int8 index quantizes the bf16 rows as it adds them)
-    return report_error(AUR_ERR_INVALID, "index is %d-d dtype %d; the encoder produces %d-d bf16", st.dim, st.dtype, e->cfg.hidden);
-  int n_items = 0;
-  if ((rc = stage_inputs(e, tokens, cu, n_seq, &n_items))) return rc;
-  if ((rc = forward_locked(e, cu, n_seq, n_items))) return rc;
-  // the pooled rows stay in HBM: the shard copies them device-to-device on the encoder's stream
-  if ((rc = aur_add_dev(ix, e->d_pool_bf16, ids, user_codes, org_codes, n_seq, e->stream))) return rc;
-  ENC_TRY(cudaStreamSynchronize(e->stream));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]);
-  e->stats.total_ms = ms;
-  return AUR_OK;
+  const int rc = check_one_batch(e, tokens, cu, n_seq);
+  if (rc != AUR_OK) return rc;
+  return append_texts_multi(&e, &ix, 1, Texts{tokens, cu, nullptr}, n_seq, n_seq, ids, user_codes, org_codes, 0, 0);
 }
 
 int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out) {
@@ -638,34 +640,12 @@ int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out) {
 int aur_encode_texts(aur_encoder* e, const int32_t* tokens, const int32_t* cu, int32_t n_seq, const int32_t* cu_texts,
                      int32_t n_texts, float* out_f32, uint16_t* out_bf16) {
   if (!e) return report_error(AUR_ERR_INVALID, "null encoder");
-  {
-    std::lock_guard<std::mutex> g(e->mu);
-    if (!e->missing.empty())
-      return report_error(AUR_ERR_INVALID, "encoder parameters not loaded: %s (+%zu more)", e->missing[0].c_str(), e->missing.size() - 1);
-  }
+  const int rc = check_loaded(e);
+  if (rc != AUR_OK) return rc;
   if (n_seq < 0 || n_texts < 0) return report_error(AUR_ERR_INVALID, "n_seq / n_texts < 0");
   if (n_texts == 0 && n_seq == 0) return AUR_OK;
   if (!tokens || !cu || !cu_texts) return report_error(AUR_ERR_INVALID, "tokens, cu_seqlens and cu_texts are required");
-  const Texts in{tokens, cu, cu_texts};
-  int rc = check_texts(e->cfg, in, n_seq, n_texts, e->cfg.max_tokens);
-  if (rc != AUR_OK) return rc;
-  const size_t H = e->cfg.hidden;
-  // outputs are written only on success: every batch lands in host staging first
-  std::vector<float> f32(out_f32 ? static_cast<size_t>(n_texts) * H : 0);
-  std::vector<uint16_t> bf16(out_bf16 ? static_cast<size_t>(n_texts) * H : 0);
-  std::vector<int32_t> q(static_cast<size_t>(n_texts));
-  for (int32_t j = 0; j < n_texts; ++j) q[j] = j;
-  rc = run_texts(e, in, q.data(), n_texts, e->cfg.max_tokens, e->cfg.max_seqs,
-                 [&](aur_encoder* enc, const int32_t* qs, int n, const float* rows) -> int {
-                   const size_t at = static_cast<size_t>(qs[0]) * H, len = static_cast<size_t>(n) * H;
-                   if (out_f32) ENC_TRY(cudaMemcpyAsync(f32.data() + at, rows, len * sizeof(float), cudaMemcpyDeviceToHost, enc->stream));
-                   if (out_bf16) ENC_TRY(cudaMemcpyAsync(bf16.data() + at, enc->d_pool_bf16, len * 2, cudaMemcpyDeviceToHost, enc->stream));
-                   return AUR_OK;
-                 });
-  if (rc != AUR_OK) return rc;
-  if (out_f32) memcpy(out_f32, f32.data(), f32.size() * sizeof(float));
-  if (out_bf16) memcpy(out_bf16, bf16.data(), bf16.size() * 2);
-  return AUR_OK;
+  return encode_texts(e, Texts{tokens, cu, cu_texts}, n_seq, n_texts, out_f32, out_bf16);
 }
 
 int aur_encode_append_texts_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,

@@ -397,19 +397,8 @@ int aur_encode_text_append(aur_encoder* enc, aur_tokenizer* tok, aur_index* ix, 
   std::vector<int32_t> cu(static_cast<size_t>(n_texts) + 1);
   int rc = aur_tokenize(tok, texts_utf8, offsets, n_texts, max_len, tokens.data(), static_cast<int64_t>(tokens.size()), cu.data(), n_threads);
   if (rc != AUR_OK) return rc;
-  std::vector<int32_t> cu_b;
-  int32_t i = 0;
-  while (i < n_texts) {   // batches that fit the encoder's workspace
-    int32_t j = i;
-    while (j < n_texts && j - i < max_seqs_per_call && cu[j + 1] - cu[i] <= max_tokens_per_call) ++j;
-    cu_b.assign(static_cast<size_t>(j - i) + 1, 0);
-    for (int32_t s = i; s <= j; ++s) cu_b[static_cast<size_t>(s - i)] = cu[s] - cu[i];
-    rc = aur_encode_append(enc, ix, tokens.data() + cu[i], cu_b.data(), j - i, ids + i, user_codes ? user_codes + i : nullptr,
-                           org_codes ? org_codes + i : nullptr);
-    if (rc != AUR_OK) return rc;
-    i = j;
-  }
-  return AUR_OK;
+  return aur_encode_append_multi(&enc, &ix, 1, tokens.data(), cu.data(), n_texts, ids, user_codes, org_codes,
+                                 max_tokens_per_call, max_seqs_per_call);
 }
 
 }  // extern "C"

@@ -139,19 +139,13 @@ class Encoder:
         return out
 
     def encode(self, seqs: Sequence[Sequence[int]]) -> np.ndarray:
-        """Token-id lists of any count: split into calls that fit the workspace."""
-        out = np.empty((len(seqs), self.cfg.hidden), dtype=np.float32)
-        i = 0
-        while i < len(seqs):
-            j, toks = i, 0
-            while j < len(seqs) and j - i < self.max_seqs and toks + len(seqs[j]) <= self.max_tokens:
-                toks += len(seqs[j]); j += 1
-            if j == i:
-                raise ValueError(f"sequence {i} has {len(seqs[i])} tokens: more than max_tokens={self.max_tokens}")
-            tok, cu = pack_sequences(seqs[i:j])
-            out[i:j] = self.encode_packed(tok, cu)
-            i = j
-        return out
+        """Token-id lists of any count, [len(seqs), hidden] float32: one ``encode_texts`` call with one window per text,
+        cut into workspace batches inside the library."""
+        for i, s in enumerate(seqs):
+            if len(s) > self.max_tokens:
+                raise ValueError(f"sequence {i} has {len(s)} tokens: more than max_tokens={self.max_tokens}")
+        tok, cu = pack_sequences(seqs)
+        return self.encode_texts(tok, cu, np.arange(len(seqs) + 1, dtype=np.int32))
 
     def encode_append(self, index, tokens: np.ndarray, cu_seqlens: np.ndarray, ids: np.ndarray,
                       user_codes: Optional[np.ndarray] = None, org_codes: Optional[np.ndarray] = None) -> None:
@@ -296,13 +290,6 @@ class TextEncoder:
         shards = self._shards(index)
         encode_append_multi([self._encs[sh.device] for sh in shards], shards, tok, cu, ids, user_codes, org_codes,
                             cu_texts=cu_texts)
-
-    def _append_texts_native(self, index, texts, ids, u, o) -> None:
-        """The same ingest as ONE C call (aur_encode_text_append: tokenise + batches + append inside the library), for
-        callers that know their texts fit the position table (over-long texts would be truncated there)."""
-        blob, offs = self._tok._pack(list(texts))
-        N.check(self._enc._lib.aur_encode_text_append(self._enc._h, self._tok._h, index._h, blob, _ptr(offs), len(texts), self.max_len,
-                                                      self._enc.max_tokens, self._enc.max_seqs, _ptr(ids), _ptr(u), _ptr(o), 0))
 
 
 # ----------------------------------------------------------------------------- reference mirror

@@ -544,12 +544,20 @@ int aur_encoder_close(aur_encoder* enc);
  * l{l}.bo, l{l}.ln1_g, l{l}.ln1_b, l{l}.wi [I,H], l{l}.bi [I], l{l}.wo2 [H,I], l{l}.bo2,
  * l{l}.ln2_g, l{l}.ln2_b -- all [out_features, in_features] like torch.nn.Linear. */
 int aur_encoder_load(aur_encoder* enc, const char* name, const float* data, int64_t count);
-/* Host in / host out.  out_f32 [n_seq, hidden] and/or out_bf16 [n_seq, hidden] (either may be
- * NULL).  Fails with AUR_ERR_INVALID until every parameter has been loaded. */
+/* Host in / host out, one batch of the workspace: aur_encode_texts with one window per text, so out_f32 [n_seq, hidden]
+ * and/or out_bf16 [n_seq, hidden] (either may be NULL) hold each sequence's pooled vector and are written only on
+ * success.  Checked first, in this order, before any device work: a parameter not loaded yet, tokens or cu_seqlens NULL
+ * or n_seq <= 0 (AUR_ERR_INVALID); n_seq > max_seqs (AUR_ERR_NOMEM); cu_seqlens[0] != 0 (AUR_ERR_INVALID);
+ * cu_seqlens[n_seq] > max_tokens (AUR_ERR_NOMEM); then aur_encode_texts' checks of the sequences. */
 int aur_encode(aur_encoder* enc, const int32_t* tokens, const int32_t* cu_seqlens, int32_t n_seq,
                float* out_f32, uint16_t* out_bf16);
 /* Fused ingest: encode the chunks and append the pooled bf16 vectors to the shard without
- * leaving the device (insert_chunks, weaviate_client.py:136-212, minus the text handling). */
+ * leaving the device (insert_chunks, weaviate_client.py:136-212, minus the text handling).
+ * ids NULL (AUR_ERR_INVALID) and aur_encode's one-batch checks first, then aur_encode_append_multi with n = 1 on the
+ * caller's thread: every check of that call, a shard without room for the n_seq rows (AUR_ERR_NOMEM), an id < 0 or a
+ * shard on another device than the encoder (AUR_ERR_INVALID) among them, is made before any device work, so a rejected
+ * call leaves the shard and the encoder's stats untouched.  The one-batch checks come before the shard's: a call over
+ * max_seqs or max_tokens gets AUR_ERR_NOMEM even when its shard is f32 or of another dim. */
 int aur_encode_append(aur_encoder* enc, aur_index* ix, const int32_t* tokens,
                       const int32_t* cu_seqlens, int32_t n_seq, const int64_t* ids,
                       const int32_t* user_codes, const int32_t* org_codes);
@@ -574,7 +582,8 @@ int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out);
  * one call's token budget, a shard without room for its share (rows appended + share > capacity) (AUR_ERR_NOMEM).  A
  * concurrent writer of the same shard may still use up its room: that shard's append then fails as aur_add_dev fails.
  * A failure after device work has started (a CUDA error) may leave a prefix of some shards' shares appended, whole
- * batches each; aur_last_error names the first failing shard.  aur_encode_append is this call with n = 1 on one batch. */
+ * batches each; aur_last_error names the first failing shard.  aur_encode_append is this call with n = 1 after its
+ * one-batch checks, and aur_encode_text_append this call with n = 1 after tokenising. */
 int aur_encode_append_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,
                             const int32_t* cu_seqlens, int32_t n_seq, const int64_t* ids, const int32_t* user_codes,
                             const int32_t* org_codes, int32_t max_tokens_per_call, int32_t max_seqs_per_call);
@@ -582,8 +591,9 @@ int aur_encode_append_multi(aur_encoder* const* encs, aur_index* const* shards, 
  * sequences (aur_tokenize_windows' layout): cu_texts [n_texts + 1] starts at 0, rises by at least 1 per text and ends at
  * n_seq.  The windows go through the workspace in greedy batches, in order; a text's windows may span batches, its fp32
  * running sum then stays on the device from one batch to the next (the encoder is held for that long).  A text of one
- * window gets aur_encode's vector for that sequence, bit for bit.  A text of w >= 2 windows with pooled vectors
- * v_1 .. v_w (each normalised when the encoder normalises) gets, per component and never fused:
+ * window gets its window's pooled vector, bit for bit, whatever else its batch holds; aur_encode is this call with one
+ * window per text on one batch.  A text of w >= 2 windows with pooled vectors v_1 .. v_w (each normalised when the
+ * encoder normalises) gets, per component and never fused:
  *   s = fl32(..fl32(v_1 + v_2) .. + v_w), m = fl32(s / w);
  *   normalize: q = sum of the exact fp64 squares m_i^2, summed in fp64 as lane sums r_c = m_c^2 + m_{c+32}^2 + .. (in
  *   increasing i) for c = 0 .. 31, then r_0 + r_1 + .. + r_31; out_i = fl32(m_i / sqrt(q)) in fp64 when q > 0, else m;
@@ -628,7 +638,13 @@ int aur_tokenize_windows(aur_tokenizer* t, const char* texts_utf8, const int64_t
                          int32_t* tokens_out, int64_t tokens_cap, int32_t* cu_seqlens_out, int32_t seqs_cap,
                          int32_t* cu_texts_out, int64_t* totals_out, int32_t n_threads);
 /* Text in, rows in the shard: tokenise, encoder forward, append -- insert_chunks (weaviate_client.py:136-212) without
- * Python on the path.  Batches are cut to max_tokens_per_call / max_seqs_per_call (the encoder's workspace). */
+ * Python on the path.  Every text is tokenised by aur_tokenize, truncated to max_len ids (a longer text loses its tail:
+ * aur_tokenize_windows + aur_encode_append_texts_multi keep it), then the texts go, one sequence each, through
+ * aur_encode_append_multi(&enc, &ix, 1, ..., max_tokens_per_call, max_seqs_per_call): batches are cut to those limits,
+ * and every check of that call (a limit above the encoder's workspace, AUR_ERR_INVALID, among them) is made before any
+ * device work, so a rejected call appends nothing.  Checked first: NULL enc, tok, ix or ids (AUR_ERR_INVALID); then
+ * n_texts <= 0 returns AUR_OK with nothing done; then max_len outside 2 .. 512, max_tokens_per_call < max_len or
+ * max_seqs_per_call < 1 (AUR_ERR_INVALID). */
 int aur_encode_text_append(aur_encoder* enc, aur_tokenizer* tok, aur_index* ix, const char* texts_utf8,
                            const int64_t* offsets, int32_t n_texts, int32_t max_len, int32_t max_tokens_per_call,
                            int32_t max_seqs_per_call, const int64_t* ids, const int32_t* user_codes,
