@@ -122,9 +122,9 @@ int (&fail)(int, const char*, ...) = report_error;
 // pool and run on its own stream, so N threads can search at once.
 struct SearchCtx {
   std::mutex mu;                  // one enqueue at a time
-  cudaStream_t own_stream = nullptr;
+  Stream own_stream;
   cudaStream_t bound = nullptr;   // caller stream this context serves (nullptr = pool context)
-  cudaEvent_t ev_begin = nullptr, ev_k0 = nullptr, ev_k1 = nullptr, ev_fin = nullptr, ev_end = nullptr;
+  Event ev_begin, ev_k0, ev_k1, ev_fin, ev_end;
   bool have_timing = false;
   int last_kernel = 0, last_launches = 0, last_nq = 0;
   int last_tile_n = 0;             // corpus rows per tile of the last tensor-core launch (0: none)
@@ -152,21 +152,7 @@ struct SearchCtx {
   DevBuf<uint32_t> filt_counts;  // filtered search: [32] totals, then [n_programs][blocks] counts (scanned into offsets)
   DevBuf<int32_t> filt_rows;     // filtered search: every program's matching rows, ascending, program after program
   DevBuf<int64_t> filt_ids;      // aur_filter_ids: their ids
-  uint32_t* h_totals = nullptr;  // page-locked landing area of the count pass's totals (kFiltCallPrograms words)
-  void release() {
-    if (h_totals) cudaFreeHost(h_totals);
-    h_totals = nullptr;
-    cand_a.release(); cand_b.release(); pub.release(); cand_count.release(); d_epoch.release(); cand_read.release(); q_img.release(); score_chunk.release(); masked_inv.release();
-    allow_rows.release(); row_mask.release(); scope_tab.release(); q_scope.release(); stage_q.release(); stage_quser.release(); stage_qorg.release(); stage_scores.release();
-    stage_ids.release(); list_stage.release(); list_scores.release();
-    filt_stage.release(); filt_mask.release(); filt_counts.release(); filt_rows.release(); filt_ids.release();
-    if (ev_begin) cudaEventDestroy(ev_begin);
-    if (ev_k0) cudaEventDestroy(ev_k0);
-    if (ev_k1) cudaEventDestroy(ev_k1);
-    if (ev_fin) cudaEventDestroy(ev_fin);
-    if (ev_end) cudaEventDestroy(ev_end);
-    if (own_stream) cudaStreamDestroy(own_stream);
-  }
+  HostBuf<uint32_t> h_totals;    // page-locked landing area of the count pass's totals (kFiltCallPrograms words)
 };
 
 struct aur_index {
@@ -182,15 +168,14 @@ struct aur_index {
   size_t qelt = 2;                       // bytes per query / input row element (bf16 for bf16 and int8 rows, f32 for f32)
   DevBuf<uint8_t> i8_stage;              // int8 shards: host bf16 rows on their way to the quantizer (writers hold mu_write)
   DevBuf<int32_t> tomb_rows;             // aur_remove: the rows it tombstones, one upload (writers hold mu_write)
-  void* d_rows = nullptr;
-  float* d_inv_norm = nullptr;
-  int64_t* d_ids = nullptr;
-  int32_t* d_user = nullptr;
-  int32_t* d_org = nullptr;
+  DevBuf<uint8_t> d_rows;
+  DevBuf<float> d_inv_norm;
+  DevBuf<int64_t> d_ids;
+  DevBuf<int32_t> d_user, d_org;
   AttrColumns attrs;                     // program columns 2.., cap_pad rows each (aur_set_attrs, writers hold mu_write)
   std::unordered_map<int64_t, int64_t> id2row;
-  cudaStream_t stream = nullptr;         // the index's own stream: device-pointer calls with stream == NULL
-  cudaStream_t ingest_stream = nullptr;  // host appends / tombstones, lowest priority so queries overtake them
+  Stream stream;                         // the index's own stream: device-pointer calls with stream == NULL
+  Stream ingest_stream;                  // host appends / tombstones, lowest priority so queries overtake them
   CUtensorMap tmap[2][2];  // [64-row, 128-row tiles][cta_group 1, 2]: box rows tile / cta_group
   bool tmap_ok = false;
   int sm_count = 0;
@@ -219,8 +204,8 @@ int build_tmaps(aur_index* ix) {
       const int tile_n = w ? kTcTileWide : kTcTileN;
       const uint64_t cols = static_cast<uint64_t>(ix->dim), rows = static_cast<uint64_t>(ix->capacity);
       const uint32_t box_rows = static_cast<uint32_t>(tile_n / g);
-      const int r = i8 ? encode_tmap_2d_u8(&ix->tmap[w][g - 1], ix->d_rows, cols, rows, cols, kTcKBlockI8, box_rows)
-                       : encode_tmap_2d_bf16(&ix->tmap[w][g - 1], ix->d_rows, cols, rows, cols * 2, kTcKBlock, box_rows);
+      const int r = i8 ? encode_tmap_2d_u8(&ix->tmap[w][g - 1], ix->d_rows.p, cols, rows, cols, kTcKBlockI8, box_rows)
+                       : encode_tmap_2d_bf16(&ix->tmap[w][g - 1], ix->d_rows.p, cols, rows, cols * 2, kTcKBlock, box_rows);
       if (r < 0) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
       if (r != CUDA_SUCCESS) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", r);
     }
@@ -238,10 +223,10 @@ bool tc_shape_ok(const aur_index* ix, int k, bool filtered) {
 int ctx_init(SearchCtx* c) {
   int lo = 0, hi = 0;
   CU_TRY(cudaDeviceGetStreamPriorityRange(&lo, &hi));   // hi = numerically lowest = highest priority
-  CU_TRY(cudaStreamCreateWithPriority(&c->own_stream, cudaStreamNonBlocking, hi));
-  CU_TRY(cudaEventCreate(&c->ev_begin)); CU_TRY(cudaEventCreate(&c->ev_k0));
-  CU_TRY(cudaEventCreate(&c->ev_k1));    CU_TRY(cudaEventCreate(&c->ev_end));
-  CU_TRY(cudaEventCreate(&c->ev_fin));
+  CU_TRY(c->own_stream.create(cudaStreamNonBlocking, hi));
+  CU_TRY(c->ev_begin.create()); CU_TRY(c->ev_k0.create());
+  CU_TRY(c->ev_k1.create());    CU_TRY(c->ev_end.create());
+  CU_TRY(c->ev_fin.create());
   return AUR_OK;
 }
 
@@ -257,7 +242,7 @@ int acquire_ctx(aur_index* ix, cudaStream_t s, SearchCtx** out) {
   }
   std::unique_ptr<SearchCtx> c(new SearchCtx());
   int rc = ctx_init(c.get());
-  if (rc != AUR_OK) { c->release(); return rc; }
+  if (rc != AUR_OK) return rc;
   c->bound = s;
   *out = c.get();
   ix->ctxs.push_back(std::move(c));
@@ -416,9 +401,9 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   ++c->epoch;
   TcParams p;
   p.q = i8 ? reinterpret_cast<const __nv_bfloat16*>(c->q_img.p) : static_cast<const __nv_bfloat16*>(q_dev);
-  p.inv_norm = inv_norm ? inv_norm : ix->d_inv_norm;
+  p.inv_norm = inv_norm ? inv_norm : ix->d_inv_norm.p;
   p.row_mask = row_mask; p.q_scope = q_scope;
-  p.ids = ix->d_ids;
+  p.ids = ix->d_ids.p;
   p.cand = c->cand_a.p;
   p.cand_count = c->cand_count.p;
   p.dbg_scores = dbg;
@@ -488,7 +473,7 @@ int candidate_tail(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* qb, 
     DevBuf<uint64_t>& dst = in_a ? c->cand_b : c->cand_a;
     // rows of cand are indexed by the query position inside the block (TC pads to 128/256)
     CU_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
-    CU_TRY(launch_reduce_lists(cur, nqb, n_lists, ksel, group, ix->d_ids, dst.p, s));
+    CU_TRY(launch_reduce_lists(cur, nqb, n_lists, ksel, group, ix->d_ids.p, dst.p, s));
     c->last_launches += 1;
     cur = dst.p; n_lists = n_groups; in_a = !in_a;
   }
@@ -497,8 +482,8 @@ int candidate_tail(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* qb, 
   fa.counts = compact ? c->cand_count.p : nullptr;
   fa.epoch_bump = compact ? c->d_epoch.p : nullptr;
   fa.cand_read = c->cand_read.p + q0;
-  fa.q = qb; fa.rows = ix->d_rows; fa.dtype = ix->dtype; fa.dim = ix->dim; fa.nq = nqb; fa.k = k;
-  fa.ids = ix->d_ids;
+  fa.q = qb; fa.rows = ix->d_rows.p; fa.dtype = ix->dtype; fa.dim = ix->dim; fa.nq = nqb; fa.k = k;
+  fa.ids = ix->d_ids.p;
   fa.out_scores = scores ? scores + static_cast<size_t>(q0) * k : nullptr;
   fa.out_ids = ids ? ids + static_cast<size_t>(q0) * k : nullptr;
   fa.out_scores64 = scores64 ? scores64 + static_cast<size_t>(q0) * k : nullptr;
@@ -514,7 +499,7 @@ constexpr int kSimtQBlock = 1024;               // queries per generic-kernel la
 // The generic kernel's tenant filter for the queries from q0 on: their own codes, unless the scope is a row subset or
 // already folded into the inverse norms (inv).
 FilterArgs simt_filter(const aur_index* ix, const Scope& sc, const float* inv, int q0) {
-  FilterArgs f{ix->d_user, ix->d_org, nullptr, nullptr};
+  FilterArgs f{ix->d_user.p, ix->d_org.p, nullptr, nullptr};
   if (sc.n_allow < 0 && sc.q_user && !inv) { f.q_user = sc.q_user + q0; f.q_org = sc.q_org ? sc.q_org + q0 : nullptr; }
   return f;
 }
@@ -539,21 +524,21 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
   if (subset && n_rows > 0) {
     CU_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
     CU_TRY(launch_fill_f32(c->masked_inv.p, nanf(""), n_rows, s));
-    CU_TRY(launch_scatter_inv_norm(ix->d_inv_norm, sc.allow_rows, sc.n_allow, n_rows, c->masked_inv.p, s));
+    CU_TRY(launch_scatter_inv_norm(ix->d_inv_norm.p, sc.allow_rows, sc.n_allow, n_rows, c->masked_inv.p, s));
     c->last_launches += 2;
     inv = c->masked_inv.p;
   } else if (sc.match_mask && n_rows > 0) {
     CU_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
-    CU_TRY(launch_mask_match(ix->d_inv_norm, sc.match_mask, n_rows, c->masked_inv.p, s));
+    CU_TRY(launch_mask_match(ix->d_inv_norm.p, sc.match_mask, n_rows, c->masked_inv.p, s));
     ++c->last_launches;
     inv = c->masked_inv.p;
   } else if (kernel != AUR_KERNEL_SIMT && scoped_tc && n_rows > 0) {              // up to 32 scopes in the batch: row bit masks
     CU_TRY(c->row_mask.reserve(static_cast<size_t>(ix->capacity) + 64));
-    CU_TRY(launch_row_scope_mask(ix->d_user, ix->d_org, sc.scope_tab, sc.n_scopes, n_rows, c->row_mask.p, s));
+    CU_TRY(launch_row_scope_mask(ix->d_user.p, ix->d_org.p, sc.scope_tab, sc.n_scopes, n_rows, c->row_mask.p, s));
     ++c->last_launches;
   } else if (kernel != AUR_KERNEL_SIMT && sc.q_user != nullptr && sc.uniform != nullptr && n_rows > 0) {   // one scope for the whole batch
     CU_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
-    CU_TRY(launch_mask_inv_norm(ix->d_inv_norm, ix->d_user, ix->d_org, sc.uniform[0], sc.uniform[1], n_rows, c->masked_inv.p, s));
+    CU_TRY(launch_mask_inv_norm(ix->d_inv_norm.p, ix->d_user.p, ix->d_org.p, sc.uniform[0], sc.uniform[1], n_rows, c->masked_inv.p, s));
     ++c->last_launches;
     inv = c->masked_inv.p;
   }
@@ -580,9 +565,9 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
         if (!k_timed) CU_TRY(cudaEventRecord(c->ev_k0, s));
         for (int64_t r0 = 0; r0 < n_rows; r0 += kSimtChunk) {
           const int64_t nr = std::min(n_rows - r0, kSimtChunk);
-          CU_TRY(launch_simt_scores(qb, ix->d_rows, ix->dtype, ix->dim, nqb, r0, nr, n_rows, inv ? inv : ix->d_inv_norm, f,
+          CU_TRY(launch_simt_scores(qb, ix->d_rows.p, ix->dtype, ix->dim, nqb, r0, nr, n_rows, inv ? inv : ix->d_inv_norm.p, f,
                                     c->score_chunk.p, s));
-          CU_TRY(launch_simt_select(c->score_chunk.p, nqb, r0, nr, ksel, ix->d_ids, c->cand_a.p, n_lists,
+          CU_TRY(launch_simt_select(c->score_chunk.p, nqb, r0, nr, ksel, ix->d_ids.p, c->cand_a.p, n_lists,
                                     static_cast<int>(r0 / kSimtSeg), s));
           c->last_launches += 2;
         }
@@ -616,7 +601,7 @@ int add_common(aur_index* ix, const void* rows, bool rows_on_device, const int64
                 (long long)n, (long long)ix->capacity);
   for (int64_t i = 0; i < n; ++i)
     if (ids[i] < 0) return fail(AUR_ERR_INVALID, "ids must be >= 0");
-  uint8_t* dst = static_cast<uint8_t*>(ix->d_rows) + static_cast<size_t>(base) * ix->dim * ix->elt;
+  uint8_t* dst = static_cast<uint8_t*>(ix->d_rows.p) + static_cast<size_t>(base) * ix->dim * ix->elt;
   if (ix->dtype == AUR_I8) {
     // bf16 rows in, quantized on s before the publish below: a search never sees an unquantized row.  Host rows pass
     // through a bounded device staging buffer, a slice at a time (stream order keeps the slices apart).
@@ -631,20 +616,20 @@ int add_common(aur_index* ix, const void* rows, bool rows_on_device, const int64
         src = ix->i8_stage.p;
       }
       CU_TRY(launch_quantize_rows_i8(reinterpret_cast<const __nv_bfloat16*>(src), ix->dim, m,
-                                     reinterpret_cast<int8_t*>(dst) + static_cast<size_t>(r0) * ix->dim, ix->d_inv_norm + base + r0, s));
+                                     reinterpret_cast<int8_t*>(dst) + static_cast<size_t>(r0) * ix->dim, ix->d_inv_norm.p + base + r0, s));
     }
   } else {
     CU_TRY(cudaMemcpyAsync(dst, rows, static_cast<size_t>(n) * ix->dim * ix->elt,
                            rows_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
   }
-  CU_TRY(cudaMemcpyAsync(ix->d_ids + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
+  CU_TRY(cudaMemcpyAsync(ix->d_ids.p + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
   std::vector<int32_t> fill;
   if (!users) { fill.assign(static_cast<size_t>(n), 0); users = fill.data(); }
-  CU_TRY(cudaMemcpyAsync(ix->d_user + base, users, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  CU_TRY(cudaMemcpyAsync(ix->d_user.p + base, users, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
   std::vector<int32_t> fill2;
   if (!orgs) { fill2.assign(static_cast<size_t>(n), -1); orgs = fill2.data(); }
-  CU_TRY(cudaMemcpyAsync(ix->d_org + base, orgs, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  if (ix->dtype != AUR_I8) CU_TRY(launch_row_inv_norms(dst, ix->dtype, ix->dim, n, ix->d_inv_norm + base, s));
+  CU_TRY(cudaMemcpyAsync(ix->d_org.p + base, orgs, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  if (ix->dtype != AUR_I8) CU_TRY(launch_row_inv_norms(dst, ix->dtype, ix->dim, n, ix->d_inv_norm.p + base, s));
   // upsert: an id that already exists loses its old row (weaviate_client.py:172 uuid5 semantics).  The old rows
   // are tombstoned before the new ones are published: a racing search may briefly miss the object, never see it twice.
   std::vector<int64_t> dead;
@@ -657,7 +642,7 @@ int add_common(aur_index* ix, const void* rows, bool rows_on_device, const int64
     }
   }
   const float nanv = nanf("");
-  for (int64_t row : dead) CU_TRY(cudaMemcpyAsync(ix->d_inv_norm + row, &nanv, 4, cudaMemcpyHostToDevice, s));
+  for (int64_t row : dead) CU_TRY(cudaMemcpyAsync(ix->d_inv_norm.p + row, &nanv, 4, cudaMemcpyHostToDevice, s));
   CU_TRY(cudaStreamSynchronize(s));  // the data has landed (and the host staging vectors may go out of scope)
   ix->rows_pub.store(base + n, std::memory_order_release);
   return AUR_OK;
@@ -812,10 +797,10 @@ ListParams list_params(const aur_index* ix, const SearchCtx* c, const ListPlan::
                        const int32_t* list_rows, int ksel) {
   ListParams p{};
   p.q = reinterpret_cast<const __nv_bfloat16*>(c->stage_q.p + static_cast<size_t>(b.q0) * ix->dim * 2);
-  p.rows = ix->d_rows;
+  p.rows = ix->d_rows.p;
   p.rows_i8 = ix->dtype == AUR_I8;
-  p.inv_norm = ix->d_inv_norm;
-  p.ids = ix->d_ids;
+  p.inv_norm = ix->d_inv_norm.p;
+  p.ids = ix->d_ids.p;
   p.items = reinterpret_cast<const ListItem*>(c->list_stage.p + ln.items);
   p.n_items = ln.n_items;
   p.list_rows = list_rows ? list_rows : c->list_stage.p;
@@ -871,18 +856,18 @@ FiltPass filt_pass(SearchCtx* c, int ps, int n_programs, int64_t n_rows) {
 int filter_count(aur_index* ix, SearchCtx* c, cudaStream_t s, const FiltProgs& fp, int64_t n_rows) {
   const int n_passes = filter_passes(fp.n_programs);
   const size_t nb = static_cast<size_t>(std::max(filter_blocks(n_rows), 1));
-  if (!c->h_totals) CU_TRY(cudaHostAlloc(reinterpret_cast<void**>(&c->h_totals), kFiltCallPrograms * 4, cudaHostAllocPortable));
+  CU_TRY(c->h_totals.reserve(kFiltCallPrograms, cudaHostAllocPortable));
   CU_TRY(c->filt_mask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
   CU_TRY(c->filt_counts.reserve(static_cast<size_t>(n_passes) * kFiltMaxPrograms * (1 + nb)));
   FiltParams p;
-  CU_TRY(filter_upload(fp, ix->d_user, ix->d_org, ix->attrs, c->filt_stage, s, &p));
-  p.inv_norm = ix->d_inv_norm; p.n_rows = n_rows;
+  CU_TRY(filter_upload(fp, ix->d_user.p, ix->d_org.p, ix->attrs, c->filt_stage, s, &p));
+  p.inv_norm = ix->d_inv_norm.p; p.n_rows = n_rows;
   for (int ps = 0; ps < n_passes; ++ps) {
     const FiltPass pass = filt_pass(c, ps, fp.n_programs, n_rows);
     CU_TRY(launch_filter_count(filter_pass(p, ps), pass.mask, pass.counts, pass.totals, s));
     ++c->last_launches;
   }
-  CU_TRY(cudaMemcpyAsync(c->h_totals, c->filt_counts.p, static_cast<size_t>(n_passes) * kFiltMaxPrograms * 4,
+  CU_TRY(cudaMemcpyAsync(c->h_totals.p, c->filt_counts.p, static_cast<size_t>(n_passes) * kFiltMaxPrograms * 4,
                          cudaMemcpyDeviceToHost, s));
   return AUR_OK;
 }
@@ -890,7 +875,7 @@ int filter_count(aur_index* ix, SearchCtx* c, cudaStream_t s, const FiltProgs& f
 // After filter_count, with the stream idle: every program's number of matching rows (pass ps's totals are words
 // 32 ps .. 32 ps + 31: program order).
 void filter_totals(const SearchCtx* c, int32_t n_programs, std::vector<int64_t>* totals) {
-  totals->assign(c->h_totals, c->h_totals + n_programs);
+  totals->assign(c->h_totals.p, c->h_totals.p + n_programs);
 }
 
 // After filter_count: every program's matching rows, ascending, program after program, into c->filt_rows (and with
@@ -905,7 +890,7 @@ int filter_write(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t n_programs
   int64_t base = 0;
   for (int ps = 0; ps < filter_passes(n_programs); ++ps) {
     const FiltPass fp = filt_pass(c, ps, n_programs, n_rows);
-    CU_TRY(launch_filter_write(fp.mask, fp.counts, fp.totals, fp.n_programs, n_rows, with_ids ? ix->d_ids : nullptr,
+    CU_TRY(launch_filter_write(fp.mask, fp.counts, fp.totals, fp.n_programs, n_rows, with_ids ? ix->d_ids.p : nullptr,
                                c->filt_rows.p + base, with_ids ? c->filt_ids.p + base : nullptr, s));
     if (n_rows > 0) c->last_launches += 2;
     for (int q = 0; q < fp.n_programs; ++q) base += tot[static_cast<size_t>(ps * kFiltMaxPrograms + q)];
@@ -1089,31 +1074,30 @@ int aur_open(const aur_config* cfg, aur_index** out) {
   cudaDeviceProp prop;
   CU_TRY(cudaGetDeviceProperties(&prop, cfg->device));
   if (prop.major != 9) return fail(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
-  aur_index* ix = new aur_index();
+  std::unique_ptr<aur_index> ix(new aur_index());
   ix->device = cfg->device; ix->dim = cfg->dim; ix->dtype = cfg->dtype; ix->capacity = cfg->capacity;
   ix->elt = cfg->dtype == AUR_BF16 ? 2 : (cfg->dtype == AUR_I8 ? 1 : 4);
   ix->qelt = cfg->dtype == AUR_F32 ? 4 : 2;
   ix->sm_count = prop.multiProcessorCount;
   ix->smem_optin = prop.sharedMemPerBlockOptin;
-  auto bail = [&](int rc) { aur_close(ix); return rc; };
 #define OPEN_TRY(expr)                                                                                  \
-  do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return bail(fail(e_ == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, \
-                                                                 "%s: %s", #expr, cudaGetErrorString(e_))); } while (0)
+  do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return fail(e_ == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, \
+                                                              "%s: %s", #expr, cudaGetErrorString(e_)); } while (0)
   int prio_lo = 0, prio_hi = 0;
   OPEN_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-  OPEN_TRY(cudaStreamCreateWithPriority(&ix->stream, cudaStreamNonBlocking, prio_hi));
-  OPEN_TRY(cudaStreamCreateWithPriority(&ix->ingest_stream, cudaStreamNonBlocking, prio_lo));
+  OPEN_TRY(ix->stream.create(cudaStreamNonBlocking, prio_hi));
+  OPEN_TRY(ix->ingest_stream.create(cudaStreamNonBlocking, prio_lo));
   ix->cap_pad = (cfg->capacity + kTcTileN - 1) / kTcTileN * kTcTileN;
   const size_t cap_pad = static_cast<size_t>(ix->cap_pad);
-  OPEN_TRY(cudaMalloc(&ix->d_rows, cap_pad * ix->dim * ix->elt));
-  OPEN_TRY(cudaMalloc(&ix->d_inv_norm, cap_pad * 4));
-  OPEN_TRY(cudaMalloc(&ix->d_ids, cap_pad * 8));
-  OPEN_TRY(cudaMalloc(&ix->d_user, cap_pad * 4));
-  OPEN_TRY(cudaMalloc(&ix->d_org, cap_pad * 4));
+  OPEN_TRY(ix->d_rows.reserve(cap_pad * ix->dim * ix->elt));
+  OPEN_TRY(ix->d_inv_norm.reserve(cap_pad));
+  OPEN_TRY(ix->d_ids.reserve(cap_pad));
+  OPEN_TRY(ix->d_user.reserve(cap_pad));
+  OPEN_TRY(ix->d_org.reserve(cap_pad));
 #undef OPEN_TRY
-  int rc = build_tmaps(ix);
-  if (rc != AUR_OK) return bail(rc);
-  *out = ix;
+  int rc = build_tmaps(ix.get());
+  if (rc != AUR_OK) return rc;
+  *out = ix.release();
   return AUR_OK;
 }
 
@@ -1121,13 +1105,6 @@ int aur_close(aur_index* ix) {
   if (!ix) return AUR_OK;
   cudaSetDevice(ix->device);
   cudaDeviceSynchronize();   // searches bound to caller streams may still be in flight
-  cudaFree(ix->d_rows); cudaFree(ix->d_inv_norm); cudaFree(ix->d_ids); cudaFree(ix->d_user); cudaFree(ix->d_org);
-  ix->attrs.release();
-  ix->i8_stage.release();
-  ix->tomb_rows.release();
-  for (auto& c : ix->ctxs) c->release();
-  if (ix->stream) cudaStreamDestroy(ix->stream);
-  if (ix->ingest_stream) cudaStreamDestroy(ix->ingest_stream);
   delete ix;
   return AUR_OK;
 }
@@ -1173,11 +1150,11 @@ int aur_export(aur_index* ix, void* rows_out, int64_t* ids_out, int32_t* user_ou
   CU_TRY(cudaSetDevice(ix->device));
   CU_TRY(cudaDeviceSynchronize());
   std::vector<float> inv(static_cast<size_t>(n));
-  CU_TRY(cudaMemcpy(inv.data(), ix->d_inv_norm, sizeof(float) * n, cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(rows_out, ix->d_rows, static_cast<size_t>(n) * ix->dim * ix->elt, cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(ids_out, ix->d_ids, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
-  if (user_out) CU_TRY(cudaMemcpy(user_out, ix->d_user, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
-  if (org_out) CU_TRY(cudaMemcpy(org_out, ix->d_org, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemcpy(inv.data(), ix->d_inv_norm.p, sizeof(float) * n, cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemcpy(rows_out, ix->d_rows.p, static_cast<size_t>(n) * ix->dim * ix->elt, cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemcpy(ids_out, ix->d_ids.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
+  if (user_out) CU_TRY(cudaMemcpy(user_out, ix->d_user.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
+  if (org_out) CU_TRY(cudaMemcpy(org_out, ix->d_org.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
   // NaN = tombstone; an int8 row stored from a row with a NaN / inf (scale +inf, never returned) is live, reported as 2
   for (int64_t i = 0; i < n; ++i) {
     const float v = inv[static_cast<size_t>(i)];
@@ -1195,9 +1172,9 @@ int aur_read_rows(aur_index* ix, int64_t row0, int64_t n, void* rows_out, int64_
   if (n == 0) return AUR_OK;
   CU_TRY(cudaSetDevice(ix->device));
   const size_t rb = static_cast<size_t>(ix->dim) * ix->elt;
-  CU_TRY(cudaMemcpy(rows_out, static_cast<const uint8_t*>(ix->d_rows) + static_cast<size_t>(row0) * rb, static_cast<size_t>(n) * rb,
+  CU_TRY(cudaMemcpy(rows_out, static_cast<const uint8_t*>(ix->d_rows.p) + static_cast<size_t>(row0) * rb, static_cast<size_t>(n) * rb,
                     cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(ids_out, ix->d_ids + row0, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemcpy(ids_out, ix->d_ids.p + row0, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost));
   return AUR_OK;
 }
 
@@ -1222,38 +1199,40 @@ int aur_compact(aur_index* ix, int64_t* reclaimed) {
   // overwrites rows < i1 <= old(i1), i.e. rows whose content has already been gathered or moved.
   const int64_t chunk = 65536;
   DevBuf<int32_t> d_map; DevBuf<uint8_t> bounce; DevBuf<float> b_inv; DevBuf<int64_t> b_ids; DevBuf<int32_t> b_user, b_org, b_attr;
-  cudaError_t e = d_map.reserve(static_cast<size_t>(chunk));
-  if (e == cudaSuccess) e = bounce.reserve(static_cast<size_t>(chunk) * ix->dim * ix->elt);
-  if (e == cudaSuccess) e = b_inv.reserve(chunk);
-  if (e == cudaSuccess) e = b_ids.reserve(chunk);
-  if (e == cudaSuccess) e = b_user.reserve(chunk);
-  if (e == cudaSuccess) e = b_org.reserve(chunk);
-  if (e == cudaSuccess && ix->attrs.any()) e = b_attr.reserve(chunk);
-  auto drop = [&]() { d_map.release(); bounce.release(); b_inv.release(); b_ids.release(); b_user.release(); b_org.release(); b_attr.release(); };
-  if (e != cudaSuccess) { drop(); return fail(AUR_ERR_NOMEM, "aur_compact: %s", cudaGetErrorString(e)); }
+  cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(d_map.reserve(static_cast<size_t>(chunk)));
+    AUR_CU_RET(bounce.reserve(static_cast<size_t>(chunk) * ix->dim * ix->elt));
+    AUR_CU_RET(b_inv.reserve(chunk));
+    AUR_CU_RET(b_ids.reserve(chunk));
+    AUR_CU_RET(b_user.reserve(chunk));
+    AUR_CU_RET(b_org.reserve(chunk));
+    return ix->attrs.any() ? b_attr.reserve(chunk) : cudaSuccess;
+  }();
+  if (e != cudaSuccess) return fail(AUR_ERR_NOMEM, "aur_compact: %s", cudaGetErrorString(e));
   cudaStream_t s = ix->ingest_stream;
   std::vector<int32_t> map_host(static_cast<size_t>(chunk));
   int64_t first_moved = 0;
   while (first_moved < nlive && order[static_cast<size_t>(first_moved)].first == first_moved) ++first_moved;   // untouched prefix
-  for (int64_t i0 = first_moved; i0 < nlive && e == cudaSuccess; i0 += chunk) {
-    const int64_t m = (nlive - i0 < chunk) ? nlive - i0 : chunk;
-    for (int64_t j = 0; j < m; ++j) map_host[static_cast<size_t>(j)] = static_cast<int32_t>(order[static_cast<size_t>(i0 + j)].first);
-    e = cudaMemcpyAsync(d_map.p, map_host.data(), static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, s);
-    if (e == cudaSuccess) e = launch_gather_rows(ix->d_rows, ix->d_inv_norm, ix->d_ids, ix->d_user, ix->d_org, d_map.p, m,
-                                                 static_cast<int>(ix->dim * ix->elt), bounce.p, b_inv.p, b_ids.p, b_user.p, b_org.p, s);
+  e = [&]() -> cudaError_t {
     const size_t rb = static_cast<size_t>(ix->dim) * ix->elt;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(static_cast<uint8_t*>(ix->d_rows) + static_cast<size_t>(i0) * rb, bounce.p, static_cast<size_t>(m) * rb, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_inv_norm + i0, b_inv.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_ids + i0, b_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_user + i0, b_user.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ix->d_org + i0, b_org.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = ix->attrs.gather(d_map.p, m, i0, b_attr.p, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);   // map_host is reused by the next chunk
-  }
-  // the freed rows are appended to again: their attributes start absent, as in a fresh column
-  if (e == cudaSuccess) e = ix->attrs.clear(nlive, rows, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  drop();
+    for (int64_t i0 = first_moved; i0 < nlive; i0 += chunk) {
+      const int64_t m = (nlive - i0 < chunk) ? nlive - i0 : chunk;
+      for (int64_t j = 0; j < m; ++j) map_host[static_cast<size_t>(j)] = static_cast<int32_t>(order[static_cast<size_t>(i0 + j)].first);
+      AUR_CU_RET(cudaMemcpyAsync(d_map.p, map_host.data(), static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, s));
+      AUR_CU_RET(launch_gather_rows(ix->d_rows.p, ix->d_inv_norm.p, ix->d_ids.p, ix->d_user.p, ix->d_org.p, d_map.p, m,
+                                    static_cast<int>(ix->dim * ix->elt), bounce.p, b_inv.p, b_ids.p, b_user.p, b_org.p, s));
+      AUR_CU_RET(cudaMemcpyAsync(ix->d_rows.p + static_cast<size_t>(i0) * rb, bounce.p, static_cast<size_t>(m) * rb, cudaMemcpyDeviceToDevice, s));
+      AUR_CU_RET(cudaMemcpyAsync(ix->d_inv_norm.p + i0, b_inv.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s));
+      AUR_CU_RET(cudaMemcpyAsync(ix->d_ids.p + i0, b_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToDevice, s));
+      AUR_CU_RET(cudaMemcpyAsync(ix->d_user.p + i0, b_user.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s));
+      AUR_CU_RET(cudaMemcpyAsync(ix->d_org.p + i0, b_org.p, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s));
+      AUR_CU_RET(ix->attrs.gather(d_map.p, m, i0, b_attr.p, s));
+      AUR_CU_RET(cudaStreamSynchronize(s));   // map_host is reused by the next chunk
+    }
+    // the freed rows are appended to again: their attributes start absent, as in a fresh column
+    AUR_CU_RET(ix->attrs.clear(nlive, rows, s));
+    return cudaStreamSynchronize(s);
+  }();
   if (e != cudaSuccess) return fail(AUR_ERR_CUDA, "aur_compact: %s (the shard may be inconsistent: restore the last snapshot)", cudaGetErrorString(e));
   {
     std::lock_guard<std::mutex> lk(ix->mu);
@@ -1360,7 +1339,7 @@ int aur_remove(aur_index* ix, const int64_t* ids, int64_t n, int64_t* removed) {
   cudaStream_t s = ix->ingest_stream;
   if (m) {
     CU_TRY(cudaMemcpyAsync(ix->tomb_rows.p, dead.data(), static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, s));
-    CU_TRY(launch_tombstone_rows(ix->tomb_rows.p, m, ix->d_inv_norm, s));
+    CU_TRY(launch_tombstone_rows(ix->tomb_rows.p, m, ix->d_inv_norm.p, s));
     CU_TRY(cudaStreamSynchronize(s));   // dead is pageable host memory and goes out of scope
   }
   if (removed) *removed = m;
@@ -1519,7 +1498,7 @@ int aur_remove_filtered(aur_index* ix, const int32_t* prog, int32_t n_tokens, co
     return AUR_OK;
   }
   if ((rc = filter_write(ix, c, s, 1, tot, call.n_rows, true)) != AUR_OK) return rc;
-  CU_TRY(launch_tombstone_rows(c->filt_rows.p, n, ix->d_inv_norm, s));
+  CU_TRY(launch_tombstone_rows(c->filt_rows.p, n, ix->d_inv_norm.p, s));
   std::vector<int64_t> got(static_cast<size_t>(n));
   CU_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost, s));
   CU_TRY(cudaStreamSynchronize(s));
@@ -1541,10 +1520,10 @@ int aur_remove_filtered(aur_index* ix, const int32_t* prog, int32_t n_tokens, co
 struct aur_exchange {
   int device = 0, rank = 0, world = 1, nq_max = 0, k_max = 0;
   size_t entries = 0, slot_stride = 0, parity_stride = 0, bytes = 0;   // slot_stride / parity_stride in 8-byte words
-  uint64_t* local = nullptr;           // this rank's buffer (cudaMalloc, exported through cudaIpc)
+  DevBuf<uint64_t> local;              // this rank's buffer (exported through cudaIpc)
   uint64_t* peer[8] = {};              // every rank's buffer as mapped here (peer[rank] == local)
-  uint64_t* d_seq = nullptr;           // exchanges completed
-  uint32_t* d_done = nullptr;          // merge kernel's block counter, then the status word
+  DevBuf<uint64_t> d_seq;              // exchanges completed
+  DevBuf<uint32_t> d_done;             // merge kernel's block counter, then the status word
   bool connected = false;
 };
 
@@ -1582,29 +1561,28 @@ int aur_exchange_create(int32_t device, int32_t rank, int32_t world, int32_t nq_
   if (aur_device_count() == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device");
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
   CU_TRY(cudaSetDevice(device));
-  aur_exchange* ex = new aur_exchange();
+  std::unique_ptr<aur_exchange> ex(new aur_exchange());
   ex->device = device; ex->rank = rank; ex->world = world; ex->nq_max = nq_max; ex->k_max = k_max;
   ex->entries = static_cast<size_t>(nq_max) * k_max;
   ex->slot_stride = 4 * ex->entries;                       // an entry = 4 tagged words (score lo / hi, id lo / hi)
   ex->parity_stride = static_cast<size_t>(world) * ex->slot_stride;
   ex->bytes = 2 * ex->parity_stride * 8 + 256;
-  cudaError_t e = cudaMalloc(&ex->local, ex->bytes);
-  if (e == cudaSuccess) e = cudaMemset(ex->local, 0, ex->bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&ex->d_seq, 8);
-  if (e == cudaSuccess) e = cudaMemset(ex->d_seq, 0, 8);
-  if (e == cudaSuccess) e = cudaMalloc(&ex->d_done, 16);      // [0] merge block counter, [1] status, [2] finalize block counter
-  if (e == cudaSuccess) e = cudaMemset(ex->d_done, 0, 16);
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
   cudaIpcMemHandle_t h;
-  if (e == cudaSuccess && world > 1) e = cudaIpcGetMemHandle(&h, ex->local);
-  if (e != cudaSuccess) {
-    cudaFree(ex->local); cudaFree(ex->d_seq); cudaFree(ex->d_done); delete ex;
-    return fail(AUR_ERR_CUDA, "aur_exchange_create: %s", cudaGetErrorString(e));
-  }
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(ex->local.reserve(ex->bytes / 8));
+    AUR_CU_RET(cudaMemset(ex->local.p, 0, ex->bytes));
+    AUR_CU_RET(ex->d_seq.reserve(1));
+    AUR_CU_RET(cudaMemset(ex->d_seq.p, 0, 8));
+    AUR_CU_RET(ex->d_done.reserve(4));      // [0] merge block counter, [1] status, [2] finalize block counter
+    AUR_CU_RET(cudaMemset(ex->d_done.p, 0, 16));
+    AUR_CU_RET(cudaDeviceSynchronize());
+    return world > 1 ? cudaIpcGetMemHandle(&h, ex->local.p) : cudaSuccess;
+  }();
+  if (e != cudaSuccess) return fail(AUR_ERR_CUDA, "aur_exchange_create: %s", cudaGetErrorString(e));
   if (world > 1) memcpy(handle_out, &h, 64); else memset(handle_out, 0, 64);
-  ex->peer[rank] = ex->local;
+  ex->peer[rank] = ex->local.p;
   ex->connected = world == 1;
-  *out = ex;
+  *out = ex.release();
   return AUR_OK;
 }
 
@@ -1630,7 +1608,6 @@ int aur_exchange_close(aur_exchange* ex) {
   cudaDeviceSynchronize();
   for (int r = 0; r < ex->world; ++r)
     if (r != ex->rank && ex->peer[r]) cudaIpcCloseMemHandle(ex->peer[r]);
-  cudaFree(ex->local); cudaFree(ex->d_seq); cudaFree(ex->d_done);
   delete ex;
   return AUR_OK;
 }
@@ -1639,8 +1616,8 @@ int aur_exchange_status(aur_exchange* ex, int64_t* exchanges_done, int32_t* stat
   if (!ex) return fail(AUR_ERR_INVALID, "null argument");
   CU_TRY(cudaSetDevice(ex->device));
   uint64_t seq = 0; uint32_t st[2] = {0, 0};
-  CU_TRY(cudaMemcpy(&seq, ex->d_seq, 8, cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(st, ex->d_done, 8, cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemcpy(&seq, ex->d_seq.p, 8, cudaMemcpyDeviceToHost));
+  CU_TRY(cudaMemcpy(st, ex->d_done.p, 8, cudaMemcpyDeviceToHost));
   if (exchanges_done) *exchanges_done = static_cast<int64_t>(seq);
   if (status) *status = static_cast<int32_t>(st[1]);
   return AUR_OK;
@@ -1664,7 +1641,7 @@ int aur_search_exchange_dev(aur_index* ix, aur_exchange* ex, const void* queries
   FinalizeArgs::ExchangeOut eo{};
   eo.n_peers = ex->world;
   for (int r = 0; r < ex->world; ++r) eo.slot[r] = ex->peer[r] + static_cast<size_t>(ex->rank) * ex->slot_stride;
-  eo.seq = ex->d_seq;
+  eo.seq = ex->d_seq.p;
   eo.parity_stride = ex->parity_stride;
   const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
   Scope sc;
@@ -1672,8 +1649,8 @@ int aur_search_exchange_dev(aur_index* ix, aur_exchange* ex, const void* queries
   if ((rc = search_enqueue(ix, c, queries_dev, nq, k, sc, n_rows, nullptr, nullptr, nullptr, s, &eo)) != AUR_OK) return rc;
   if ((rc = stats_end(ix, c, s)) != AUR_OK) return rc;
   ExchangeParams p{};
-  p.slots = ex->local;
-  p.seq = ex->d_seq; p.done = ex->d_done; p.status = ex->d_done + 1;
+  p.slots = ex->local.p;
+  p.seq = ex->d_seq.p; p.done = ex->d_done.p; p.status = ex->d_done.p + 1;
   p.world = ex->world; p.rank = ex->rank; p.nq = nq; p.k = k;
   p.parity_stride = ex->parity_stride; p.slot_stride = ex->slot_stride;
   p.out_scores = scores_dev; p.out_ids = ids_dev;
@@ -1691,17 +1668,18 @@ int aur_cosine_pairs(int32_t device, const float* a_host, const float* b_host, i
   if (aur_device_count() == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device: aurora_b200 has no CPU fallback");
   CU_TRY(cudaSetDevice(device));
   if (dim == 0) { for (int64_t i = 0; i < n; ++i) out_host[i] = 0.0; return AUR_OK; }
-  float *da = nullptr, *db = nullptr; double* dout = nullptr;
-  const size_t bytes = static_cast<size_t>(n) * dim * 4;
-  cudaError_t e = cudaMalloc(&da, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&db, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&dout, static_cast<size_t>(n) * 8);
-  if (e == cudaSuccess) e = cudaMemcpy(da, a_host, bytes, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(db, b_host, bytes, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = launch_cosine_pairs(da, db, n, dim, clamp, dout, nullptr);
+  DevBuf<float> da, db; DevBuf<double> dout;
+  const size_t elems = static_cast<size_t>(n) * dim, bytes = elems * 4;
   std::vector<double> tmp(static_cast<size_t>(n));
-  if (e == cudaSuccess) e = cudaMemcpy(tmp.data(), dout, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost);
-  cudaFree(da); cudaFree(db); cudaFree(dout);
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(da.reserve(elems));
+    AUR_CU_RET(db.reserve(elems));
+    AUR_CU_RET(dout.reserve(static_cast<size_t>(n)));
+    AUR_CU_RET(cudaMemcpy(da.p, a_host, bytes, cudaMemcpyHostToDevice));
+    AUR_CU_RET(cudaMemcpy(db.p, b_host, bytes, cudaMemcpyHostToDevice));
+    AUR_CU_RET(launch_cosine_pairs(da.p, db.p, n, dim, clamp, dout.p, nullptr));
+    return cudaMemcpy(tmp.data(), dout.p, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost);
+  }();
   if (e != cudaSuccess) return fail(AUR_ERR_CUDA, "cosine_pairs: %s", cudaGetErrorString(e));
   memcpy(out_host, tmp.data(), static_cast<size_t>(n) * 8);
   return AUR_OK;
@@ -1790,7 +1768,7 @@ int aur_debug_simt_scores(aur_index* ix, const void* queries_host, int32_t nq, c
     const int64_t nr = std::min(n - r0, kSimtChunk);
     chunk.resize(static_cast<size_t>(nq) * nr);
     CU_TRY(cudaMemsetAsync(c->score_chunk.p, 0xFF, chunk.size() * 4, call.s));   // NaN wherever the kernel writes nothing
-    CU_TRY(launch_simt_scores(c->stage_q.p, ix->d_rows, ix->dtype, ix->dim, nq, r0, nr, n, ix->d_inv_norm,
+    CU_TRY(launch_simt_scores(c->stage_q.p, ix->d_rows.p, ix->dtype, ix->dim, nq, r0, nr, n, ix->d_inv_norm.p,
                               simt_filter(ix, sc, nullptr, 0), c->score_chunk.p, call.s));
     CU_TRY(cudaMemcpyAsync(chunk.data(), c->score_chunk.p, chunk.size() * 4, cudaMemcpyDeviceToHost, call.s));
     CU_TRY(cudaStreamSynchronize(call.s));

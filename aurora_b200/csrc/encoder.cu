@@ -22,6 +22,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -42,9 +43,9 @@ using namespace aur;
 namespace {
 
 struct Layer {
-  __nv_bfloat16 *wqkv = nullptr, *wo = nullptr, *wi = nullptr, *wo2 = nullptr;
-  float *bqkv = nullptr, *bo = nullptr, *bi = nullptr, *bo2 = nullptr;
-  float *ln1_g = nullptr, *ln1_b = nullptr, *ln2_g = nullptr, *ln2_b = nullptr;
+  DevBuf<__nv_bfloat16> wqkv, wo, wi, wo2;
+  DevBuf<float> bqkv, bo, bi, bo2;
+  DevBuf<float> ln1_g, ln1_b, ln2_g, ln2_b;
   CUtensorMap tm_wqkv, tm_wo, tm_wi, tm_wo2;
 };
 
@@ -61,25 +62,25 @@ struct aur_encoder {
   int dh = 64;                 // real head dim (64, or 32 zero-padded to 64 inside the qkv / ctx layout)
   int hp = 0;                  // heads * 64: width of each of q, k, v in the qkv buffer and of ctx
   int sm_count = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  __nv_bfloat16 *word = nullptr, *pos = nullptr, *type = nullptr;
-  float *emb_g = nullptr, *emb_b = nullptr;
+  Stream stream;
+  Event ev[4];
+  DevBuf<__nv_bfloat16> word, pos, type;
+  DevBuf<float> emb_g, emb_b;
   std::vector<Layer> layers;
   std::vector<std::string> missing;   // parameter names not loaded yet
-  __nv_bfloat16 *x = nullptr, *y = nullptr, *qkv = nullptr, *ctx = nullptr, *inter = nullptr;
+  DevBuf<__nv_bfloat16> x, y, qkv, ctx, inter;
   CUtensorMap tm_x, tm_ctx, tm_inter, tm_qkv;       // loads: box {64, 128}
-  int32_t *d_tok = nullptr, *d_pos = nullptr, *d_cu = nullptr;
-  AttnItem* d_items = nullptr;
+  DevBuf<int32_t> d_tok, d_pos, d_cu;
+  DevBuf<AttnItem> d_items;
   int max_items = 0;
-  float* d_pool_f32 = nullptr;
-  __nv_bfloat16* d_pool_bf16 = nullptr;
-  float* d_fold_f32 = nullptr;                        // [max_seqs + 2, H]: window_fold_kernel's text vectors + 2 carry rows
-  FoldItem* d_fold = nullptr;                         // [max_seqs]
-  FoldItem* h_fold = nullptr;                         // pinned
-  float* d_stage = nullptr; size_t stage_elems = 0;   // fp32 staging for parameter upload
-  int32_t *h_tok = nullptr, *h_pos = nullptr;          // pinned
-  AttnItem* h_items = nullptr;
+  DevBuf<float> d_pool_f32;
+  DevBuf<__nv_bfloat16> d_pool_bf16;
+  DevBuf<float> d_fold_f32;                           // [max_seqs + 2, H]: window_fold_kernel's text vectors + 2 carry rows
+  DevBuf<FoldItem> d_fold;                            // [max_seqs]
+  HostBuf<FoldItem> h_fold;
+  DevBuf<float> d_stage;                              // fp32 staging for parameter upload
+  HostBuf<int32_t> h_tok, h_pos;
+  HostBuf<AttnItem> h_items;
   aur_encoder_stats stats{};
   int64_t last_tokens = 0;
 };
@@ -94,13 +95,13 @@ int make_tmap(CUtensorMap* tm, const void* base, int cols, int rows, int box_row
 }
 
 template <typename T>
-int dev_alloc(T** p, size_t n) {
-  ENC_TRY(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
-  ENC_TRY(cudaMemset(*p, 0, n * sizeof(T)));
+int dev_alloc(DevBuf<T>& b, size_t n) {
+  ENC_TRY(b.reserve(n));
+  ENC_TRY(cudaMemset(b.p, 0, n * sizeof(T)));
   return AUR_OK;
 }
 
-// Every parameter buffer of e with its element count (the head-dim-32 layouts padded as stored), in one fixed order:
+// Every parameter buffer of e (its owner) with its element count (the head-dim-32 layouts padded as stored), in one fixed order:
 // aur_encoder_open allocates them, aur_encoder_replicate copies them buffer for buffer.
 template <typename F>
 void for_each_param(aur_encoder* e, F&& f) {
@@ -115,24 +116,6 @@ void for_each_param(aur_encoder* e, F&& f) {
   }
 }
 
-void free_all(aur_encoder* e) {
-  cudaSetDevice(e->cfg.device);
-  auto f = [](auto*& p) { if (p) cudaFree(p); p = nullptr; };
-  f(e->word); f(e->pos); f(e->type); f(e->emb_g); f(e->emb_b);
-  for (Layer& l : e->layers) {
-    f(l.wqkv); f(l.wo); f(l.wi); f(l.wo2); f(l.bqkv); f(l.bo); f(l.bi); f(l.bo2);
-    f(l.ln1_g); f(l.ln1_b); f(l.ln2_g); f(l.ln2_b);
-  }
-  f(e->x); f(e->y); f(e->qkv); f(e->ctx); f(e->inter);
-  f(e->d_tok); f(e->d_pos); f(e->d_cu); f(e->d_items); f(e->d_pool_f32); f(e->d_pool_bf16); f(e->d_fold_f32); f(e->d_fold); f(e->d_stage);
-  if (e->h_tok) cudaFreeHost(e->h_tok);
-  if (e->h_pos) cudaFreeHost(e->h_pos);
-  if (e->h_items) cudaFreeHost(e->h_items);
-  if (e->h_fold) cudaFreeHost(e->h_fold);
-  for (auto& ev : e->ev) if (ev) cudaEventDestroy(ev);
-  if (e->stream) cudaStreamDestroy(e->stream);
-}
-
 // pad: 0 none; 1 rows are [3][heads][dh] -> [3][heads][64] (wqkv / bqkv); 2 columns are [heads][dh] -> [heads][64] (wo)
 struct ParamSlot { void* dst; int64_t count; bool bf16; int pad; };
 
@@ -140,28 +123,28 @@ struct ParamSlot { void* dst; int64_t count; bool bf16; int pad; };
 bool find_param(aur_encoder* e, const std::string& name, ParamSlot* out) {
   const aur_encoder_config& c = e->cfg;
   const int64_t H = c.hidden, I = c.inter;
-  if (name == "word_emb") { *out = {e->word, static_cast<int64_t>(c.vocab) * H, true, 0}; return true; }
-  if (name == "pos_emb") { *out = {e->pos, static_cast<int64_t>(c.max_pos) * H, true, 0}; return true; }
-  if (name == "type_emb") { *out = {e->type, static_cast<int64_t>(c.type_vocab) * H, true, 0}; return true; }
-  if (name == "emb_ln_g") { *out = {e->emb_g, H, false, 0}; return true; }
-  if (name == "emb_ln_b") { *out = {e->emb_b, H, false, 0}; return true; }
+  if (name == "word_emb") { *out = {e->word.p, static_cast<int64_t>(c.vocab) * H, true, 0}; return true; }
+  if (name == "pos_emb") { *out = {e->pos.p, static_cast<int64_t>(c.max_pos) * H, true, 0}; return true; }
+  if (name == "type_emb") { *out = {e->type.p, static_cast<int64_t>(c.type_vocab) * H, true, 0}; return true; }
+  if (name == "emb_ln_g") { *out = {e->emb_g.p, H, false, 0}; return true; }
+  if (name == "emb_ln_b") { *out = {e->emb_b.p, H, false, 0}; return true; }
   int l = -1; char leaf[32] = {0};
   if (sscanf(name.c_str(), "l%d.%31s", &l, leaf) != 2 || l < 0 || l >= c.layers) return false;
   Layer& L = e->layers[l];
   const std::string f = leaf;
   const int padded = e->dh != 64;
-  if (f == "wqkv") { *out = {L.wqkv, 3 * H * H, true, padded ? 1 : 0}; return true; }
-  if (f == "wo") { *out = {L.wo, H * H, true, padded ? 2 : 0}; return true; }
-  if (f == "wi") { *out = {L.wi, I * H, true, 0}; return true; }
-  if (f == "wo2") { *out = {L.wo2, H * I, true, 0}; return true; }
-  if (f == "bqkv") { *out = {L.bqkv, 3 * H, false, padded ? 1 : 0}; return true; }
-  if (f == "bo") { *out = {L.bo, H, false, 0}; return true; }
-  if (f == "bi") { *out = {L.bi, I, false, 0}; return true; }
-  if (f == "bo2") { *out = {L.bo2, H, false, 0}; return true; }
-  if (f == "ln1_g") { *out = {L.ln1_g, H, false, 0}; return true; }
-  if (f == "ln1_b") { *out = {L.ln1_b, H, false, 0}; return true; }
-  if (f == "ln2_g") { *out = {L.ln2_g, H, false, 0}; return true; }
-  if (f == "ln2_b") { *out = {L.ln2_b, H, false, 0}; return true; }
+  if (f == "wqkv") { *out = {L.wqkv.p, 3 * H * H, true, padded ? 1 : 0}; return true; }
+  if (f == "wo") { *out = {L.wo.p, H * H, true, padded ? 2 : 0}; return true; }
+  if (f == "wi") { *out = {L.wi.p, I * H, true, 0}; return true; }
+  if (f == "wo2") { *out = {L.wo2.p, H * I, true, 0}; return true; }
+  if (f == "bqkv") { *out = {L.bqkv.p, 3 * H, false, padded ? 1 : 0}; return true; }
+  if (f == "bo") { *out = {L.bo.p, H, false, 0}; return true; }
+  if (f == "bi") { *out = {L.bi.p, I, false, 0}; return true; }
+  if (f == "bo2") { *out = {L.bo2.p, H, false, 0}; return true; }
+  if (f == "ln1_g") { *out = {L.ln1_g.p, H, false, 0}; return true; }
+  if (f == "ln1_b") { *out = {L.ln1_b.p, H, false, 0}; return true; }
+  if (f == "ln2_g") { *out = {L.ln2_g.p, H, false, 0}; return true; }
+  if (f == "ln2_b") { *out = {L.ln2_b.p, H, false, 0}; return true; }
   return false;
 }
 
@@ -181,31 +164,31 @@ int forward_locked(aur_encoder* e, const int32_t* cu_host, int n_seq, int n_item
   const int T = cu_host[n_seq], H = c.hidden, I = c.inter;
   const int t_pad = round_up(T, 256);
   cudaStream_t s = e->stream;
-  ENC_TRY(cudaMemcpyAsync(e->d_tok, e->h_tok, sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
-  ENC_TRY(cudaMemcpyAsync(e->d_pos, e->h_pos, sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
-  ENC_TRY(cudaMemcpyAsync(e->d_cu, cu_host, sizeof(int32_t) * (n_seq + 1), cudaMemcpyHostToDevice, s));
-  ENC_TRY(cudaMemcpyAsync(e->d_items, e->h_items, sizeof(AttnItem) * n_items, cudaMemcpyHostToDevice, s));
+  ENC_TRY(cudaMemcpyAsync(e->d_tok.p, e->h_tok.p, sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
+  ENC_TRY(cudaMemcpyAsync(e->d_pos.p, e->h_pos.p, sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
+  ENC_TRY(cudaMemcpyAsync(e->d_cu.p, cu_host, sizeof(int32_t) * (n_seq + 1), cudaMemcpyHostToDevice, s));
+  ENC_TRY(cudaMemcpyAsync(e->d_items.p, e->h_items.p, sizeof(AttnItem) * n_items, cudaMemcpyHostToDevice, s));
   ENC_TRY(cudaEventRecord(e->ev[0], s));
   int launches = 0;
-  ENC_TRY(launch_embed_ln(e->d_tok, e->d_pos, T, t_pad, e->word, e->pos, e->type, e->emb_g, e->emb_b, c.ln_eps, H, e->x, s));
+  ENC_TRY(launch_embed_ln(e->d_tok.p, e->d_pos.p, T, t_pad, e->word.p, e->pos.p, e->type.p, e->emb_g.p, e->emb_b.p, c.ln_eps, H, e->x.p, s));
   ++launches;
   AttnParams ap{};
   const int HP = e->hp;
-  ap.items = e->d_items; ap.n_items = n_items; ap.heads = c.heads; ap.hidden = HP; ap.ctx = e->ctx; ap.ld_ctx = HP;
+  ap.items = e->d_items.p; ap.n_items = n_items; ap.heads = c.heads; ap.hidden = HP; ap.ctx = e->ctx.p; ap.ld_ctx = HP;
   ap.scale_log2e = 1.4426950408889634f / sqrtf(static_cast<float>(e->dh));
   for (int l = 0; l < c.layers; ++l) {
     Layer& L = e->layers[l];
     int rc;
-    if ((rc = gemm(e, &e->tm_x, &L.tm_wqkv, e->qkv, T, 3 * HP, H, kEpiBias, L.bqkv, nullptr, 0))) return rc;
+    if ((rc = gemm(e, &e->tm_x, &L.tm_wqkv, e->qkv.p, T, 3 * HP, H, kEpiBias, L.bqkv.p, nullptr, 0))) return rc;
     ENC_TRY(attn_tc_launch(&e->tm_qkv, ap, s));
-    if ((rc = gemm(e, &e->tm_ctx, &L.tm_wo, e->y, T, H, HP, kEpiBiasResid, L.bo, e->x, H))) return rc;
-    ENC_TRY(launch_layernorm(e->y, L.ln1_g, L.ln1_b, c.ln_eps, T, H, e->x, s));
-    if ((rc = gemm(e, &e->tm_x, &L.tm_wi, e->inter, T, I, H, kEpiBiasGelu, L.bi, nullptr, 0))) return rc;
-    if ((rc = gemm(e, &e->tm_inter, &L.tm_wo2, e->y, T, H, I, kEpiBiasResid, L.bo2, e->x, H))) return rc;
-    ENC_TRY(launch_layernorm(e->y, L.ln2_g, L.ln2_b, c.ln_eps, T, H, e->x, s));
+    if ((rc = gemm(e, &e->tm_ctx, &L.tm_wo, e->y.p, T, H, HP, kEpiBiasResid, L.bo.p, e->x.p, H))) return rc;
+    ENC_TRY(launch_layernorm(e->y.p, L.ln1_g.p, L.ln1_b.p, c.ln_eps, T, H, e->x.p, s));
+    if ((rc = gemm(e, &e->tm_x, &L.tm_wi, e->inter.p, T, I, H, kEpiBiasGelu, L.bi.p, nullptr, 0))) return rc;
+    if ((rc = gemm(e, &e->tm_inter, &L.tm_wo2, e->y.p, T, H, I, kEpiBiasResid, L.bo2.p, e->x.p, H))) return rc;
+    ENC_TRY(launch_layernorm(e->y.p, L.ln2_g.p, L.ln2_b.p, c.ln_eps, T, H, e->x.p, s));
     launches += 7;
   }
-  ENC_TRY(launch_pool(e->x, e->d_cu, n_seq, H, c.pool, c.normalize, e->d_pool_f32, e->d_pool_bf16, s));
+  ENC_TRY(launch_pool(e->x.p, e->d_cu.p, n_seq, H, c.pool, c.normalize, e->d_pool_f32.p, e->d_pool_bf16.p, s));
   ++launches;
   ENC_TRY(cudaEventRecord(e->ev[1], s));
   e->stats.tokens = T; e->stats.seqs = n_seq; e->stats.launches = launches;
@@ -278,7 +261,7 @@ int check_texts(const aur_encoder_config& c, const Texts& in, int32_t n_seq, int
   return AUR_OK;
 }
 
-// Receives one batch's finished texts q[0 .. n): their bf16 rows are e->d_pool_bf16 [0, n), their fp32 rows f32 [0, n);
+// Receives one batch's finished texts q[0 .. n): their bf16 rows are e->d_pool_bf16.p [0, n), their fp32 rows f32 [0, n);
 // called on e's stream, under e's lock, before the batch's synchronise.
 using TextSink = std::function<int(aur_encoder* e, const int32_t* q, int n, const float* f32)>;
 
@@ -311,31 +294,31 @@ int run_texts(aur_encoder* e, const Texts& in, const int32_t* q, int32_t nq, int
     int n_items = 0;
     for (int i = 0; i < m; ++i) {
       const int32_t len = in.cu[wins[i] + 1] - in.cu[wins[i]], at = cu_b[i];
-      memcpy(e->h_tok + at, in.tokens + in.cu[wins[i]], sizeof(int32_t) * len);
-      for (int t = 0; t < len; ++t) e->h_pos[at + t] = t;
-      for (int q0 = 0; q0 < len; q0 += 128) e->h_items[n_items++] = AttnItem{at, len, q0, 0};
+      memcpy(e->h_tok.p + at, in.tokens + in.cu[wins[i]], sizeof(int32_t) * len);
+      for (int t = 0; t < len; ++t) e->h_pos.p[at + t] = t;
+      for (int q0 = 0; q0 < len; q0 += 128) e->h_items.p[n_items++] = AttnItem{at, len, q0, 0};
       cu_b[i + 1] = at + len;
     }
     bool fold = false;
     for (int k = 0, row = 0; k < n_fold; ++k) {
       const int32_t j = q[p0 + k], first = k == 0 ? wins[0] : in.lo(j), end = k == n_closed ? w : in.hi(j);
-      e->h_fold[k] = FoldItem{row, row + (end - first), in.hi(j) - in.lo(j),
+      e->h_fold.p[k] = FoldItem{row, row + (end - first), in.hi(j) - in.lo(j),
                               (k == 0 && carry_in ? kFoldCarryIn : 0) | (k == n_closed ? kFoldOpen : 0)};
       row += end - first;
       fold |= in.hi(j) - in.lo(j) > 1;
     }
     int rc = AUR_OK;
-    if (fold) ENC_TRY(cudaMemcpyAsync(e->d_fold, e->h_fold, sizeof(FoldItem) * n_fold, cudaMemcpyHostToDevice, e->stream));
+    if (fold) ENC_TRY(cudaMemcpyAsync(e->d_fold.p, e->h_fold.p, sizeof(FoldItem) * n_fold, cudaMemcpyHostToDevice, e->stream));
     rc = forward_locked(e, cu_b.data(), m, n_items);
     if (rc == AUR_OK && fold) {
-      float* carry = e->d_fold_f32 + static_cast<size_t>(e->cfg.max_seqs) * H;
-      const cudaError_t ce = launch_window_fold(e->d_pool_f32, e->d_fold, n_fold, H, e->cfg.normalize, carry + slot * H,
-                                                carry + (1 - slot) * H, e->d_fold_f32, e->d_pool_bf16, e->stream);
+      float* carry = e->d_fold_f32.p + static_cast<size_t>(e->cfg.max_seqs) * H;
+      const cudaError_t ce = launch_window_fold(e->d_pool_f32.p, e->d_fold.p, n_fold, H, e->cfg.normalize, carry + slot * H,
+                                                carry + (1 - slot) * H, e->d_fold_f32.p, e->d_pool_bf16.p, e->stream);
       if (open) slot = 1 - slot;
       if (ce != cudaSuccess) rc = report_error(AUR_ERR_CUDA, "window_fold_kernel: %s", cudaGetErrorString(ce));
       ++e->stats.launches;
     }
-    if (rc == AUR_OK && n_closed > 0) rc = sink(e, q + p0, n_closed, fold ? e->d_fold_f32 : e->d_pool_f32);
+    if (rc == AUR_OK && n_closed > 0) rc = sink(e, q + p0, n_closed, fold ? e->d_fold_f32.p : e->d_pool_f32.p);
     // the pinned staging is reused by the next batch: the stream must be past its copies, whatever happened above
     const cudaError_t ce = cudaStreamSynchronize(e->stream);
     if (rc != AUR_OK) return rc;
@@ -369,7 +352,7 @@ int encode_texts(aur_encoder* e, const Texts& in, int32_t n_seq, int32_t n_texts
                  [&](aur_encoder* enc, const int32_t* qs, int n, const float* rows) -> int {
                    const size_t at = static_cast<size_t>(qs[0]) * H, len = static_cast<size_t>(n) * H;
                    if (to_f32) ENC_TRY(cudaMemcpyAsync(to_f32 + at, rows, len * sizeof(float), cudaMemcpyDeviceToHost, enc->stream));
-                   if (to_bf16) ENC_TRY(cudaMemcpyAsync(to_bf16 + at, enc->d_pool_bf16, len * 2, cudaMemcpyDeviceToHost, enc->stream));
+                   if (to_bf16) ENC_TRY(cudaMemcpyAsync(to_bf16 + at, enc->d_pool_bf16.p, len * 2, cudaMemcpyDeviceToHost, enc->stream));
                    return AUR_OK;
                  });
   if (rc != AUR_OK) return rc;
@@ -446,7 +429,7 @@ int append_texts_multi(aur_encoder* const* encs, aur_index* const* shards, int32
                                 if (org_codes) o_b[i] = org_codes[q[i]];
                               }
                               // the rows stay in HBM: the shard copies them device-to-device on the encoder's stream
-                              return aur_add_dev(shards[s], e->d_pool_bf16, id_b.data(), user_codes ? u_b.data() : nullptr,
+                              return aur_add_dev(shards[s], e->d_pool_bf16.p, id_b.data(), user_codes ? u_b.data() : nullptr,
                                                  org_codes ? o_b.data() : nullptr, m, e->stream);
                             });
     if (r != AUR_OK) {
@@ -486,7 +469,7 @@ int aur_encoder_open(const aur_encoder_config* cfg, aur_encoder** out) {
   cudaDeviceProp prop;
   ENC_TRY(cudaGetDeviceProperties(&prop, cfg->device));
   if (prop.major != 9) return report_error(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
-  aur_encoder* e = new aur_encoder();
+  std::unique_ptr<aur_encoder> e(new aur_encoder());
   e->cfg = *cfg;
   e->sm_count = prop.multiProcessorCount;
   e->rows_pad = round_up(cfg->max_tokens, 256) + 512;   // + one full key window past the last sequence
@@ -496,50 +479,48 @@ int aur_encoder_open(const aur_encoder_config* cfg, aur_encoder** out) {
   e->bn = (H % 256 == 0 && I % 256 == 0 && e->hp % 256 == 0) ? 256 : 128;
   e->layers.resize(cfg->layers);
   int rc = AUR_OK;
-  auto A = [&](auto** p, size_t n) { if (rc == AUR_OK) rc = dev_alloc(p, n); };
-  for_each_param(e, [&](auto*& p, size_t n) { A(&p, n); });
+  auto A = [&](auto& b, size_t n) { if (rc == AUR_OK) rc = dev_alloc(b, n); };
+  for_each_param(e.get(), A);
   const size_t R = e->rows_pad;
-  A(&e->x, R * H); A(&e->y, R * H); A(&e->qkv, R * 3 * e->hp); A(&e->ctx, R * e->hp); A(&e->inter, R * I);
-  A(&e->d_tok, cfg->max_tokens); A(&e->d_pos, cfg->max_tokens); A(&e->d_cu, cfg->max_seqs + 1);
+  A(e->x, R * H); A(e->y, R * H); A(e->qkv, R * 3 * e->hp); A(e->ctx, R * e->hp); A(e->inter, R * I);
+  A(e->d_tok, cfg->max_tokens); A(e->d_pos, cfg->max_tokens); A(e->d_cu, cfg->max_seqs + 1);
   e->max_items = cfg->max_seqs * 4;
-  A(&e->d_items, e->max_items);
-  A(&e->d_pool_f32, static_cast<size_t>(cfg->max_seqs) * H); A(&e->d_pool_bf16, static_cast<size_t>(cfg->max_seqs) * H);
-  A(&e->d_fold_f32, static_cast<size_t>(cfg->max_seqs + 2) * H); A(&e->d_fold, cfg->max_seqs);
-  auto fail_open = [&](int code) { free_all(e); delete e; return code; };
-  if (rc != AUR_OK) return fail_open(rc);
-  if (cudaMallocHost(reinterpret_cast<void**>(&e->h_tok), sizeof(int32_t) * cfg->max_tokens) != cudaSuccess ||
-      cudaMallocHost(reinterpret_cast<void**>(&e->h_pos), sizeof(int32_t) * cfg->max_tokens) != cudaSuccess ||
-      cudaMallocHost(reinterpret_cast<void**>(&e->h_items), sizeof(AttnItem) * e->max_items) != cudaSuccess ||
-      cudaMallocHost(reinterpret_cast<void**>(&e->h_fold), sizeof(FoldItem) * cfg->max_seqs) != cudaSuccess)
-    return fail_open(report_error(AUR_ERR_NOMEM, "pinned staging allocation failed"));
-  if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess)
-    return fail_open(report_error(AUR_ERR_CUDA, "cudaStreamCreate failed"));
-  for (auto& ev : e->ev)
-    if (cudaEventCreate(&ev) != cudaSuccess) return fail_open(report_error(AUR_ERR_CUDA, "cudaEventCreate failed"));
+  A(e->d_items, e->max_items);
+  A(e->d_pool_f32, static_cast<size_t>(cfg->max_seqs) * H); A(e->d_pool_bf16, static_cast<size_t>(cfg->max_seqs) * H);
+  A(e->d_fold_f32, static_cast<size_t>(cfg->max_seqs + 2) * H); A(e->d_fold, cfg->max_seqs);
+  if (rc != AUR_OK) return rc;
+  if (e->h_tok.reserve(cfg->max_tokens, cudaHostAllocDefault) != cudaSuccess ||
+      e->h_pos.reserve(cfg->max_tokens, cudaHostAllocDefault) != cudaSuccess ||
+      e->h_items.reserve(e->max_items, cudaHostAllocDefault) != cudaSuccess ||
+      e->h_fold.reserve(cfg->max_seqs, cudaHostAllocDefault) != cudaSuccess)
+    return report_error(AUR_ERR_NOMEM, "pinned staging allocation failed");
+  if (e->stream.create(cudaStreamNonBlocking) != cudaSuccess) return report_error(AUR_ERR_CUDA, "cudaStreamCreate failed");
+  for (Event& ev : e->ev)
+    if (ev.create() != cudaSuccess) return report_error(AUR_ERR_CUDA, "cudaEventCreate failed");
   // tensor maps: activations are A operands (box 128 rows), weights B operands (box bn rows)
   const int Ri = static_cast<int>(R);
   const int HP = e->hp;
-  if ((rc = make_tmap(&e->tm_x, e->x, H, Ri, 128)) || (rc = make_tmap(&e->tm_ctx, e->ctx, HP, Ri, 128)) ||
-      (rc = make_tmap(&e->tm_inter, e->inter, I, Ri, 128)) || (rc = make_tmap(&e->tm_qkv, e->qkv, 3 * HP, Ri, 128)))
-    return fail_open(rc);
+  if ((rc = make_tmap(&e->tm_x, e->x.p, H, Ri, 128)) || (rc = make_tmap(&e->tm_ctx, e->ctx.p, HP, Ri, 128)) ||
+      (rc = make_tmap(&e->tm_inter, e->inter.p, I, Ri, 128)) || (rc = make_tmap(&e->tm_qkv, e->qkv.p, 3 * HP, Ri, 128)))
+    return rc;
   for (Layer& l : e->layers) {
-    if ((rc = make_tmap(&l.tm_wqkv, l.wqkv, H, 3 * HP, e->bn / e->cta_group)) ||
-        (rc = make_tmap(&l.tm_wo, l.wo, HP, H, e->bn / e->cta_group)) ||
-        (rc = make_tmap(&l.tm_wi, l.wi, H, I, e->bn / e->cta_group)) ||
-        (rc = make_tmap(&l.tm_wo2, l.wo2, I, H, e->bn / e->cta_group)))
-      return fail_open(rc);
+    if ((rc = make_tmap(&l.tm_wqkv, l.wqkv.p, H, 3 * HP, e->bn / e->cta_group)) ||
+        (rc = make_tmap(&l.tm_wo, l.wo.p, HP, H, e->bn / e->cta_group)) ||
+        (rc = make_tmap(&l.tm_wi, l.wi.p, H, I, e->bn / e->cta_group)) ||
+        (rc = make_tmap(&l.tm_wo2, l.wo2.p, I, H, e->bn / e->cta_group)))
+      return rc;
   }
   e->missing = {"word_emb", "pos_emb", "type_emb", "emb_ln_g", "emb_ln_b"};
   for (int l = 0; l < cfg->layers; ++l)
     for (const char* leaf : {"wqkv", "bqkv", "wo", "bo", "ln1_g", "ln1_b", "wi", "bi", "wo2", "bo2", "ln2_g", "ln2_b"})
       e->missing.push_back("l" + std::to_string(l) + "." + leaf);
-  *out = e;
+  *out = e.release();
   return AUR_OK;
 }
 
 int aur_encoder_close(aur_encoder* e) {
   if (!e) return AUR_OK;
-  { std::lock_guard<std::mutex> g(e->mu); cudaSetDevice(e->cfg.device); cudaStreamSynchronize(e->stream); free_all(e); }
+  { std::lock_guard<std::mutex> g(e->mu); cudaSetDevice(e->cfg.device); cudaStreamSynchronize(e->stream); }
   delete e;
   return AUR_OK;
 }
@@ -573,14 +554,9 @@ int aur_encoder_load(aur_encoder* e, const char* name, const float* data, int64_
     n_up = static_cast<int64_t>(padded.size());
   }
   if (slot.bf16) {
-    if (e->stage_elems < static_cast<size_t>(n_up)) {
-      if (e->d_stage) cudaFree(e->d_stage);
-      e->d_stage = nullptr; e->stage_elems = 0;
-      ENC_TRY(cudaMalloc(reinterpret_cast<void**>(&e->d_stage), sizeof(float) * n_up));
-      e->stage_elems = n_up;
-    }
-    ENC_TRY(cudaMemcpyAsync(e->d_stage, data, sizeof(float) * n_up, cudaMemcpyHostToDevice, e->stream));
-    ENC_TRY(launch_f32_to_bf16(e->d_stage, static_cast<__nv_bfloat16*>(slot.dst), n_up, e->stream));
+    ENC_TRY(e->d_stage.reserve(static_cast<size_t>(n_up)));
+    ENC_TRY(cudaMemcpyAsync(e->d_stage.p, data, sizeof(float) * n_up, cudaMemcpyHostToDevice, e->stream));
+    ENC_TRY(launch_f32_to_bf16(e->d_stage.p, static_cast<__nv_bfloat16*>(slot.dst), n_up, e->stream));
   } else {
     ENC_TRY(cudaMemcpyAsync(slot.dst, data, sizeof(float) * n_up, cudaMemcpyHostToDevice, e->stream));
   }
@@ -622,12 +598,13 @@ int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out) {
   std::vector<const void*> from;
   std::vector<size_t> bytes;
   std::vector<void*> to;
-  for_each_param(src, [&](auto*& p, size_t n) { from.push_back(p); bytes.push_back(n * sizeof(*p)); });
-  for_each_param(r, [&](auto*& p, size_t) { to.push_back(p); });
-  cudaError_t ce = cudaSuccess;
-  for (size_t i = 0; i < to.size() && ce == cudaSuccess; ++i)   // staged by the driver when the devices are not peers
-    ce = cudaMemcpyPeerAsync(to[i], device, from[i], src->cfg.device, bytes[i], r->stream);
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(r->stream);
+  for_each_param(src, [&](auto& b, size_t n) { from.push_back(b.p); bytes.push_back(n * sizeof(*b.p)); });
+  for_each_param(r, [&](auto& b, size_t) { to.push_back(b.p); });
+  const cudaError_t ce = [&]() -> cudaError_t {
+    for (size_t i = 0; i < to.size(); ++i)   // staged by the driver when the devices are not peers
+      AUR_CU_RET(cudaMemcpyPeerAsync(to[i], device, from[i], src->cfg.device, bytes[i], r->stream));
+    return cudaStreamSynchronize(r->stream);
+  }();
   if (ce != cudaSuccess) {
     aur_encoder_close(r);
     return report_error(AUR_ERR_CUDA, "encoder replica on device %d: %s", device, cudaGetErrorString(ce));
@@ -677,7 +654,7 @@ int aur_debug_encoder_hidden(aur_encoder* e, uint16_t* out, int64_t count) {
   ENC_TRY(cudaSetDevice(e->cfg.device));
   if (count != e->last_tokens * e->cfg.hidden) return report_error(AUR_ERR_INVALID, "count must be tokens * hidden of the last call");
   ENC_TRY(cudaStreamSynchronize(e->stream));
-  ENC_TRY(cudaMemcpy(out, e->x, count * 2, cudaMemcpyDeviceToHost));
+  ENC_TRY(cudaMemcpy(out, e->x.p, count * 2, cudaMemcpyDeviceToHost));
   return AUR_OK;
 }
 
@@ -690,25 +667,23 @@ int aur_debug_gemm(int32_t device, const uint16_t* a, const uint16_t* w, const f
   cudaDeviceProp prop;
   ENC_TRY(cudaGetDeviceProperties(&prop, device));
   const int m_pad = round_up(m, 128 * cta_group), bn = n % 256 == 0 ? 256 : 128;
-  __nv_bfloat16 *da = nullptr, *dw = nullptr, *dr = nullptr, *dout = nullptr; float* db = nullptr;
+  DevBuf<__nv_bfloat16> da, dw, dr, dout; DevBuf<float> db;   // freed on return (cudaFree waits for the device)
   int rc = AUR_OK;
-  auto A = [&](auto** p, size_t cnt) { if (rc == AUR_OK) rc = dev_alloc(p, cnt); };
-  A(&da, static_cast<size_t>(m_pad) * k); A(&dw, static_cast<size_t>(n) * k); A(&dr, static_cast<size_t>(m_pad) * n);
-  A(&dout, static_cast<size_t>(m_pad) * n); A(&db, n);
-  auto cleanup = [&](int code) { cudaDeviceSynchronize(); cudaFree(da); cudaFree(dw); cudaFree(dr); cudaFree(dout); cudaFree(db); return code; };
-  if (rc) return cleanup(rc);
-  cudaMemcpy(da, a, static_cast<size_t>(m) * k * 2, cudaMemcpyHostToDevice);
-  cudaMemcpy(dw, w, static_cast<size_t>(n) * k * 2, cudaMemcpyHostToDevice);
-  cudaMemcpy(db, bias, sizeof(float) * n, cudaMemcpyHostToDevice);
-  if (resid) cudaMemcpy(dr, resid, static_cast<size_t>(m) * n * 2, cudaMemcpyHostToDevice);
+  auto A = [&](auto& b, size_t cnt) { if (rc == AUR_OK) rc = dev_alloc(b, cnt); };
+  A(da, static_cast<size_t>(m_pad) * k); A(dw, static_cast<size_t>(n) * k); A(dr, static_cast<size_t>(m_pad) * n);
+  A(dout, static_cast<size_t>(m_pad) * n); A(db, n);
+  if (rc) return rc;
+  cudaMemcpy(da.p, a, static_cast<size_t>(m) * k * 2, cudaMemcpyHostToDevice);
+  cudaMemcpy(dw.p, w, static_cast<size_t>(n) * k * 2, cudaMemcpyHostToDevice);
+  cudaMemcpy(db.p, bias, sizeof(float) * n, cudaMemcpyHostToDevice);
+  if (resid) cudaMemcpy(dr.p, resid, static_cast<size_t>(m) * n * 2, cudaMemcpyHostToDevice);
   CUtensorMap tm_a, tm_w;
-  if ((rc = make_tmap(&tm_a, da, k, m_pad, 128)) || (rc = make_tmap(&tm_w, dw, k, n, bn / cta_group)))
-    return cleanup(rc);
+  if ((rc = make_tmap(&tm_a, da.p, k, m_pad, 128)) || (rc = make_tmap(&tm_w, dw.p, k, n, bn / cta_group))) return rc;
   GemmParams p{};
-  p.bias = db; p.resid = dr; p.ldr = n; p.out = dout; p.ldo = n;
+  p.bias = db.p; p.resid = dr.p; p.ldr = n; p.out = dout.p; p.ldo = n;
   p.m_tiles = m_pad / (128 * cta_group); p.n_tiles = n / bn; p.k_blocks = k / 64;
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
+  Event e0, e1;
+  e0.create(); e1.create();
   cudaError_t ce = cudaSuccess;
   for (int rep = 0; rep < 3 && ce == cudaSuccess; ++rep) {   // last repetition is the timed one
     cudaEventRecord(e0, nullptr);
@@ -718,12 +693,11 @@ int aur_debug_gemm(int32_t device, const uint16_t* a, const uint16_t* w, const f
   if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
   float ms = 0.f;
   if (ce == cudaSuccess) cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  if (ce != cudaSuccess) return cleanup(report_error(AUR_ERR_CUDA, "gemm: %s", cudaGetErrorString(ce)));
-  ce = cudaMemcpy(out, dout, static_cast<size_t>(m) * n * 2, cudaMemcpyDeviceToHost);
-  if (ce != cudaSuccess) return cleanup(report_error(AUR_ERR_CUDA, "gemm d2h: %s", cudaGetErrorString(ce)));
+  if (ce != cudaSuccess) return report_error(AUR_ERR_CUDA, "gemm: %s", cudaGetErrorString(ce));
+  ce = cudaMemcpy(out, dout.p, static_cast<size_t>(m) * n * 2, cudaMemcpyDeviceToHost);
+  if (ce != cudaSuccess) return report_error(AUR_ERR_CUDA, "gemm d2h: %s", cudaGetErrorString(ce));
   if (ms_out) *ms_out = ms;
-  return cleanup(AUR_OK);
+  return AUR_OK;
 }
 
 int aur_debug_attention(int32_t device, const uint16_t* qkv, const int32_t* cu, int32_t n_seq, int32_t heads,
@@ -740,21 +714,20 @@ int aur_debug_attention(int32_t device, const uint16_t* qkv, const int32_t* cu, 
     if (len < 1 || len > 512) return report_error(AUR_ERR_INVALID, "sequence length %d", len);
     for (int q0 = 0; q0 < len; q0 += 128) items.push_back(AttnItem{cu[i], len, q0, 0});
   }
-  __nv_bfloat16 *dq = nullptr, *dc = nullptr; AttnItem* di = nullptr;
+  DevBuf<__nv_bfloat16> dq, dc; DevBuf<AttnItem> di;   // freed on return (cudaFree waits for the device)
   int rc = AUR_OK;
-  auto A = [&](auto** p, size_t cnt) { if (rc == AUR_OK) rc = dev_alloc(p, cnt); };
-  A(&dq, static_cast<size_t>(rows) * 3 * hidden); A(&dc, static_cast<size_t>(rows) * hidden); A(&di, items.size());
-  auto cleanup = [&](int code) { cudaDeviceSynchronize(); cudaFree(dq); cudaFree(dc); cudaFree(di); return code; };
-  if (rc) return cleanup(rc);
-  cudaMemcpy(dq, qkv, static_cast<size_t>(T) * 3 * hidden * 2, cudaMemcpyHostToDevice);
-  cudaMemcpy(di, items.data(), sizeof(AttnItem) * items.size(), cudaMemcpyHostToDevice);
+  auto A = [&](auto& b, size_t cnt) { if (rc == AUR_OK) rc = dev_alloc(b, cnt); };
+  A(dq, static_cast<size_t>(rows) * 3 * hidden); A(dc, static_cast<size_t>(rows) * hidden); A(di, items.size());
+  if (rc) return rc;
+  cudaMemcpy(dq.p, qkv, static_cast<size_t>(T) * 3 * hidden * 2, cudaMemcpyHostToDevice);
+  cudaMemcpy(di.p, items.data(), sizeof(AttnItem) * items.size(), cudaMemcpyHostToDevice);
   CUtensorMap tm;
-  if ((rc = make_tmap(&tm, dq, 3 * hidden, rows, 128))) return cleanup(rc);
+  if ((rc = make_tmap(&tm, dq.p, 3 * hidden, rows, 128))) return rc;
   AttnParams ap{};
-  ap.items = di; ap.n_items = static_cast<int>(items.size()); ap.heads = heads; ap.hidden = hidden; ap.ctx = dc; ap.ld_ctx = hidden;
+  ap.items = di.p; ap.n_items = static_cast<int>(items.size()); ap.heads = heads; ap.hidden = hidden; ap.ctx = dc.p; ap.ld_ctx = hidden;
   ap.scale_log2e = 1.4426950408889634f / 8.0f;
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
+  Event e0, e1;
+  e0.create(); e1.create();
   cudaError_t ce = cudaSuccess;
   for (int rep = 0; rep < 3 && ce == cudaSuccess; ++rep) {
     cudaEventRecord(e0, nullptr);
@@ -764,12 +737,11 @@ int aur_debug_attention(int32_t device, const uint16_t* qkv, const int32_t* cu, 
   if (ce == cudaSuccess) ce = cudaDeviceSynchronize();
   float ms = 0.f;
   if (ce == cudaSuccess) cudaEventElapsedTime(&ms, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  if (ce != cudaSuccess) return cleanup(report_error(AUR_ERR_CUDA, "attention: %s", cudaGetErrorString(ce)));
-  ce = cudaMemcpy(ctx, dc, static_cast<size_t>(T) * hidden * 2, cudaMemcpyDeviceToHost);
-  if (ce != cudaSuccess) return cleanup(report_error(AUR_ERR_CUDA, "attention d2h: %s", cudaGetErrorString(ce)));
+  if (ce != cudaSuccess) return report_error(AUR_ERR_CUDA, "attention: %s", cudaGetErrorString(ce));
+  ce = cudaMemcpy(ctx, dc.p, static_cast<size_t>(T) * hidden * 2, cudaMemcpyDeviceToHost);
+  if (ce != cudaSuccess) return report_error(AUR_ERR_CUDA, "attention d2h: %s", cudaGetErrorString(ce));
   if (ms_out) *ms_out = ms;
-  return cleanup(AUR_OK);
+  return AUR_OK;
 }
 
 }  // extern "C"

@@ -266,54 +266,50 @@ int filter_check_queries(const FiltProgs& fp, int32_t nq, int64_t max_list_rows)
 
 int AttrColumns::write(int32_t col, const std::vector<int32_t>& pairs, int64_t rows, cudaStream_t s) {
   if (col < 2 || col >= kFiltCols) return report_error(AUR_ERR_INVALID, "attribute columns are 2 .. %d", kFiltCols - 1);
-  auto fail = [](cudaError_t e) { return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e)); };
-  int32_t* a = d_attr[col - 2];   // (writes are serialised: only this call stores a pointer)
-  if (!a) {
-    cudaError_t e = cudaMalloc(&a, static_cast<size_t>(rows) * 4);
-    if (e != cudaSuccess) return fail(e);
-    e = cudaMemsetAsync(a, 0xFF, static_cast<size_t>(rows) * 4, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { cudaFree(a); return fail(e); }
-    std::lock_guard<std::mutex> lk(mu);
-    d_attr[col - 2] = a;
-  }
-  if (pairs.empty()) return AUR_OK;
-  cudaError_t e = stage.reserve(pairs.size());
-  if (e == cudaSuccess) e = cudaMemcpyAsync(stage.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) {
+  const cudaError_t e = [&]() -> cudaError_t {
+    if (!d_attr[col - 2].p) {   // (writes are serialised: only this call stores a column)
+      DevBuf<int32_t> a;
+      AUR_CU_RET(a.reserve(static_cast<size_t>(rows)));
+      AUR_CU_RET(cudaMemsetAsync(a.p, 0xFF, static_cast<size_t>(rows) * 4, s));
+      AUR_CU_RET(cudaStreamSynchronize(s));
+      std::lock_guard<std::mutex> lk(mu);
+      d_attr[col - 2] = std::move(a);
+    }
+    if (pairs.empty()) return cudaSuccess;
+    AUR_CU_RET(stage.reserve(pairs.size()));
+    AUR_CU_RET(cudaMemcpyAsync(stage.p, pairs.data(), pairs.size() * 4, cudaMemcpyHostToDevice, s));
     const int64_t n = static_cast<int64_t>(pairs.size() / 2);
-    scatter_codes_kernel<<<blocks_of(n, 256), 256, 0, s>>>(stage.p, n, a);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  return e == cudaSuccess ? AUR_OK : fail(e);
+    scatter_codes_kernel<<<blocks_of(n, 256), 256, 0, s>>>(stage.p, n, d_attr[col - 2].p);
+    AUR_CU_RET(cudaGetLastError());
+    return cudaStreamSynchronize(s);
+  }();
+  if (e == cudaSuccess) return AUR_OK;
+  return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e));
 }
 
-bool AttrColumns::any() { return std::any_of(std::begin(d_attr), std::end(d_attr), [](const int32_t* a) { return a != nullptr; }); }
+bool AttrColumns::any() { return std::any_of(std::begin(d_attr), std::end(d_attr), [](const DevBuf<int32_t>& a) { return a.p != nullptr; }); }
 
 cudaError_t AttrColumns::gather(const int32_t* map, int64_t m, int64_t dst0, int32_t* bounce, cudaStream_t s) {
-  cudaError_t e = cudaSuccess;
-  for (int32_t* a : d_attr) {
-    if (!a || m <= 0 || e != cudaSuccess) continue;
-    gather_i32_kernel<<<blocks_of(m, 256), 256, 0, s>>>(a, map, m, bounce);
-    e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(a + dst0, bounce, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s);
+  for (const DevBuf<int32_t>& a : d_attr) {
+    if (!a.p || m <= 0) continue;
+    gather_i32_kernel<<<blocks_of(m, 256), 256, 0, s>>>(a.p, map, m, bounce);
+    AUR_CU_RET(cudaGetLastError());
+    AUR_CU_RET(cudaMemcpyAsync(a.p + dst0, bounce, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToDevice, s));
   }
-  return e;
+  return cudaSuccess;
 }
 
 cudaError_t AttrColumns::clear(int64_t r0, int64_t r1, cudaStream_t s) {
-  cudaError_t e = cudaSuccess;
-  for (int32_t* a : d_attr)
-    if (a && r1 > r0 && e == cudaSuccess) e = cudaMemsetAsync(a + r0, 0xFF, static_cast<size_t>(r1 - r0) * 4, s);
-  return e;
+  for (const DevBuf<int32_t>& a : d_attr)
+    if (a.p && r1 > r0) AUR_CU_RET(cudaMemsetAsync(a.p + r0, 0xFF, static_cast<size_t>(r1 - r0) * 4, s));
+  return cudaSuccess;
 }
 
 int AttrColumns::check(const FiltProgs& fp, const char* holder) {
   std::lock_guard<std::mutex> lk(mu);
   for (int32_t t = 0; t < fp.prog_off[fp.n_programs]; ++t) {
     const int32_t* tk = fp.prog + 4 * static_cast<int64_t>(t);
-    if (tk[0] == kFiltLeaf && tk[1] >= 2 && !d_attr[tk[1] - 2])
+    if (tk[0] == kFiltLeaf && tk[1] >= 2 && !d_attr[tk[1] - 2].p)
       return report_error(AUR_ERR_INVALID, "column %d was never set on the %s", tk[1], holder);
   }
   return AUR_OK;
@@ -321,12 +317,7 @@ int AttrColumns::check(const FiltProgs& fp, const char* holder) {
 
 void AttrColumns::fill(FiltParams* p) {
   std::lock_guard<std::mutex> lk(mu);
-  for (int i = 0; i < kFiltAttrCols; ++i) p->cols[2 + i] = d_attr[i];
-}
-
-void AttrColumns::release() {
-  for (int32_t*& a : d_attr) { cudaFree(a); a = nullptr; }
-  stage.release();
+  for (int i = 0; i < kFiltAttrCols; ++i) p->cols[2 + i] = d_attr[i].p;
 }
 
 cudaError_t filter_upload(const FiltProgs& fp, const int32_t* user, const int32_t* org, AttrColumns& attrs,
@@ -336,9 +327,8 @@ cudaError_t filter_upload(const FiltProgs& fp, const int32_t* user, const int32_
   if (n_tok) memcpy(st.data(), fp.prog, n_tok * 16);
   memcpy(st.data() + n_tok * 4, fp.prog_off, n_off * 4);
   if (fp.bitmap_words) memcpy(st.data() + n_tok * 4 + n_off, fp.bitmap, static_cast<size_t>(fp.bitmap_words) * 4);
-  cudaError_t e = stage.reserve(st.size());
-  if (e == cudaSuccess) e = cudaMemcpyAsync(stage.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice, s);
-  if (e != cudaSuccess) return e;
+  AUR_CU_RET(stage.reserve(st.size()));
+  AUR_CU_RET(cudaMemcpyAsync(stage.p, st.data(), st.size() * 4, cudaMemcpyHostToDevice, s));
   *p = FiltParams{};
   p->cols[0] = user; p->cols[1] = org;
   attrs.fill(p);

@@ -260,19 +260,19 @@ __global__ void __launch_bounds__(kFuseThreads) hybrid_merge_fuse_kernel(FusePar
 
 // Scratch of one shard's part of a hybrid call on one device: the events its legs' streams record for the join.  The
 // context of shard 0 also hosts the join on its stream, the gathered lists of the other shards, the merge + fusion
-// kernel and the copy back.  Idle contexts are pooled for the life of the process.
+// kernel and the copy back.  Idle contexts are pooled for the life of the process and never destroyed: the pool is
+// static, and the statically linked CUDA runtime may already be torn down when static destructors run.
 struct HybridCtx {
   int device = 0;
-  cudaStream_t stream = nullptr;
-  cudaEvent_t kw_done = nullptr, dense_done = nullptr;
+  Stream stream;
+  Event kw_done, dense_done;
   DevBuf<double> w;
   DevBuf<float> g_cos;              // gathered lists of shards 1 .. n-1: dense cosines and ids, keyword scores and ids
   DevBuf<int64_t> g_did, g_kid;
   DevBuf<double> g_ks;
   DevBuf<int64_t> run_max;          // the merge's scratch, both legs
   DevBuf<unsigned char> out;        // fused [nq][k_out] scores | ids | cosines, copied back in one piece
-  unsigned char* host = nullptr;    // page-locked landing area of that copy
-  size_t host_n = 0;
+  HostBuf<unsigned char> host;      // page-locked landing area of that copy
 };
 
 std::mutex g_pool_mu;
@@ -291,16 +291,14 @@ int hyb_acquire(int device, HybridCtx** out) {
   std::unique_ptr<HybridCtx> h(new HybridCtx());
   h->device = device;
   int lo = 0, hi = 0;   // hi = numerically lowest = highest priority, as the search contexts' streams
-  cudaError_t e = cudaSetDevice(device);
-  if (e == cudaSuccess) e = cudaDeviceGetStreamPriorityRange(&lo, &hi);
-  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&h->stream, cudaStreamNonBlocking, hi);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->kw_done, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->dense_done, cudaEventDisableTiming);
-  if (e != cudaSuccess) {
-    if (h->kw_done) cudaEventDestroy(h->kw_done);
-    if (h->stream) cudaStreamDestroy(h->stream);
-    return report_error(AUR_ERR_CUDA, "hybrid search context: %s", cudaGetErrorString(e));
-  }
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(cudaSetDevice(device));
+    AUR_CU_RET(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+    AUR_CU_RET(h->stream.create(cudaStreamNonBlocking, hi));
+    AUR_CU_RET(h->kw_done.create(cudaEventDisableTiming));
+    return h->dense_done.create(cudaEventDisableTiming);
+  }();
+  if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "hybrid search context: %s", cudaGetErrorString(e));
   *out = h.release();
   return AUR_OK;
 }
@@ -362,7 +360,7 @@ int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const 
   p.o_c = reinterpret_cast<float*>(h->out.p + no * 16);
   hybrid_merge_fuse_kernel<<<static_cast<unsigned>(a.nq), kFuseThreads, 0, st>>>(p);
   HYB_TRY(cudaGetLastError());
-  HYB_TRY(cudaMemcpyAsync(h->host, h->out.p, no * kOutBytes, cudaMemcpyDeviceToHost, st));
+  HYB_TRY(cudaMemcpyAsync(h->host.p, h->out.p, no * kOutBytes, cudaMemcpyDeviceToHost, st));
   HYB_TRY(cudaStreamSynchronize(st));
   return AUR_OK;
 }
@@ -378,12 +376,7 @@ int run_on_devices(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const
   HYB_TRY(cudaSetDevice(h->device));
   HYB_TRY(h->w.reserve(a.w.size()));
   HYB_TRY(h->out.reserve(no * kOutBytes));
-  if (h->host_n < no * kOutBytes) {
-    if (h->host) cudaFreeHost(h->host);
-    h->host = nullptr; h->host_n = 0;
-    HYB_TRY(cudaHostAlloc(reinterpret_cast<void**>(&h->host), no * kOutBytes, cudaHostAllocDefault));
-    h->host_n = no * kOutBytes;
-  }
+  HYB_TRY(h->host.reserve(no * kOutBytes, cudaHostAllocDefault));
   if (n > 1) {
     const size_t ng = static_cast<size_t>(n - 1) * nl;
     HYB_TRY(h->g_cos.reserve(ng));
@@ -465,9 +458,9 @@ int hybrid_search(aur_index* const* shards, aur_kw* const* stores, int32_t n, co
   });
   if (rc == AUR_OK) {
     const size_t no = static_cast<size_t>(nq) * k_out;
-    memcpy(scores_out, hs[0]->host, no * 8);
-    memcpy(ids_out, hs[0]->host + no * 8, no * 8);
-    memcpy(cosine_out, hs[0]->host + no * 16, no * 4);
+    memcpy(scores_out, hs[0]->host.p, no * 8);
+    memcpy(ids_out, hs[0]->host.p + no * 8, no * 8);
+    memcpy(cosine_out, hs[0]->host.p + no * 16, no * 4);
     if (snapshot_rows_out) memcpy(snapshot_rows_out, rows.data(), rows.size() * 8);
   }
   for (HybridCtx* h : hs) hyb_release(h);

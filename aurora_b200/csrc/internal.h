@@ -328,24 +328,98 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
+// ---------------------------------------------------------------- owners of CUDA resources
+// Move-only; the destructor frees.  An owner is destroyed with its own device current (every close sets it first).
+// None has static storage: cudart is linked statically, so a destructor run at process exit may find it torn down.
 template <typename T>
 struct DevBuf {   // grow-only device scratch
   T* p = nullptr; size_t n = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) { release(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+    return *this;
+  }
+  ~DevBuf() { release(); }
   cudaError_t reserve(size_t want) {
     if (want <= n) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr; n = 0;
+    release();
     cudaError_t e = cudaMalloc(&p, want * sizeof(T));
-    if (e == cudaSuccess) n = want;
+    if (e == cudaSuccess) n = want; else { p = nullptr; cudaGetLastError(); }   // not left behind for a later launch check
+    return e;
+  }
+  // Grows to max(need, 2 n) elements keeping the first `used`, copied on s and waited for.
+  cudaError_t grow_keep(size_t need, size_t used, cudaStream_t s) {
+    if (need <= n) return cudaSuccess;
+    DevBuf<T> nb;
+    cudaError_t e = nb.reserve(std::max(need, 2 * n));
+    if (e == cudaSuccess && used) e = cudaMemcpyAsync(nb.p, p, used * sizeof(T), cudaMemcpyDeviceToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e == cudaSuccess) *this = std::move(nb);
     return e;
   }
   void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
 };
+template <typename T>
+struct HostBuf {  // grow-only page-locked host buffer; flags: cudaHostAlloc's, per call site
+  T* p = nullptr; size_t n = 0;
+  HostBuf() = default;
+  HostBuf(const HostBuf&) = delete;
+  HostBuf& operator=(const HostBuf&) = delete;
+  HostBuf(HostBuf&& o) noexcept : p(o.p), n(o.n) { o.p = nullptr; o.n = 0; }
+  HostBuf& operator=(HostBuf&& o) noexcept {
+    if (this != &o) { release(); p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+    return *this;
+  }
+  ~HostBuf() { release(); }
+  cudaError_t reserve(size_t want, unsigned flags) {
+    if (want <= n) return cudaSuccess;
+    release();
+    cudaError_t e = cudaHostAlloc(reinterpret_cast<void**>(&p), want * sizeof(T), flags);
+    if (e == cudaSuccess) n = want; else { p = nullptr; cudaGetLastError(); }
+    return e;
+  }
+  void release() { if (p) cudaFreeHost(p); p = nullptr; n = 0; }
+};
+struct Stream {
+  cudaStream_t s = nullptr;
+  Stream() = default;
+  Stream(const Stream&) = delete;
+  Stream& operator=(const Stream&) = delete;
+  Stream(Stream&& o) noexcept : s(o.s) { o.s = nullptr; }
+  Stream& operator=(Stream&& o) noexcept { std::swap(s, o.s); return *this; }
+  ~Stream() { if (s) cudaStreamDestroy(s); }
+  cudaError_t create(unsigned flags, int priority = 0) {
+    const cudaError_t e = cudaStreamCreateWithPriority(&s, flags, priority);
+    if (e != cudaSuccess) { s = nullptr; cudaGetLastError(); }
+    return e;
+  }
+  operator cudaStream_t() const { return s; }
+};
+struct Event {
+  cudaEvent_t ev = nullptr;
+  Event() = default;
+  Event(const Event&) = delete;
+  Event& operator=(const Event&) = delete;
+  Event(Event&& o) noexcept : ev(o.ev) { o.ev = nullptr; }
+  Event& operator=(Event&& o) noexcept { std::swap(ev, o.ev); return *this; }
+  ~Event() { if (ev) cudaEventDestroy(ev); }
+  cudaError_t create(unsigned flags = cudaEventDefault) {
+    const cudaError_t e = cudaEventCreateWithFlags(&ev, flags);
+    if (e != cudaSuccess) { ev = nullptr; cudaGetLastError(); }
+    return e;
+  }
+  operator cudaEvent_t() const { return ev; }
+};
+// Returns expr's cudaError_t from the enclosing function unless it is cudaSuccess.
+#define AUR_CU_RET(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return e_; } while (0)
 
 // ---------------------------------------------------------------- filter columns and uploads, host side (filter.cu)
 // The attribute columns of a vector shard or a keyword store (program columns 2..): `rows` int32 codes each, -1 =
-// absent.  The pointers only go from null to allocated until release().  write, any, gather and clear are the holder's
-// writes, serialised by its writers' lock; mu guards the pointers write stores against check and fill.
+// absent.  A column only goes from unallocated to allocated.  write, any, gather and clear are the holder's writes,
+// serialised by its writers' lock; mu guards the columns write stores against check and fill.
 class AttrColumns {
  public:
   // pairs (row, code) into column col (2 .. kFiltCols - 1), waited for; the first write allocates it, all -1.
@@ -356,10 +430,9 @@ class AttrColumns {
   cudaError_t clear(int64_t r0, int64_t r1, cudaStream_t s);
   int check(const FiltProgs& fp, const char* holder);   // every column fp (structure checked) names is set
   void fill(FiltParams* p);                             // p->cols[2 ..]
-  void release();
  private:
   std::mutex mu;
-  int32_t* d_attr[kFiltAttrCols] = {};
+  DevBuf<int32_t> d_attr[kFiltAttrCols];
   DevBuf<int32_t> stage;
 };
 // Checked programs into stage on s in one upload (pageable: staged on return), and *p reading them over the holder's

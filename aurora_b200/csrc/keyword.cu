@@ -419,8 +419,8 @@ __global__ void kw_gather_postings(const uint2* post, const int64_t* old_off, co
 
 // Scratch of one in-flight search (a pool, so several host threads can search at once).
 struct KwCtx {
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  Stream stream;
+  Event ev0, ev1;
   DevBuf<unsigned char> tab;     // launch term table
   DevBuf<Cand> buf, lists_a, lists_b;
   DevBuf<double> cval, out_s;
@@ -435,13 +435,6 @@ struct KwCtx {
                                               // launches whose contribution table spilled to global memory
   int path = 0;                  // of the last search: AUR_KW_PATH_* bits
   int64_t postings = 0;          // of the last search: postings it read
-  void release() {
-    tab.release(); buf.release(); lists_a.release(); lists_b.release(); cval.release(); out_s.release(); out_ids.release();
-    allow.release(); allow_rows.release(); fstage.release(); fmask.release(); acc.release();
-    if (ev0) cudaEventDestroy(ev0);
-    if (ev1) cudaEventDestroy(ev1);
-    if (stream) cudaStreamDestroy(stream);
-  }
 };
 
 // flags[rows[i]] = v for the listed rows (allow-list rows of a search; tombstones)
@@ -460,11 +453,11 @@ struct aur_kw {
   int device = 0, sm_count = 0;
   size_t smem_optin = 0;
   int64_t capacity = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   // device
-  int64_t* d_off = nullptr; int32_t* d_len = nullptr; int64_t* d_ids = nullptr;
-  int32_t* d_user = nullptr; int32_t* d_org = nullptr; uint8_t* d_live = nullptr;
-  uint2* d_post = nullptr; int64_t post_cap = 0;
+  DevBuf<int64_t> d_off; DevBuf<int32_t> d_len; DevBuf<int64_t> d_ids;
+  DevBuf<int32_t> d_user, d_org; DevBuf<uint8_t> d_live;
+  DevBuf<uint2> d_post;      // d_post.n: the postings capacity
   AttrColumns attrs;         // program columns 2.., capacity rows each (aur_kw_set_attrs, writers hold mu_write)
   // host mirrors (the writer's bookkeeping; searches read only the published statistics)
   std::vector<int64_t> h_off{0};
@@ -477,7 +470,7 @@ struct aur_kw {
   std::vector<int64_t> df;
   // term-major index of rows [0, ix_rows) (ix_post postings), published under mu_stat and replaced only under the
   // exclusive lock: d_toff [ix_terms + 1], d_tpost [ix_post]; h_toff mirrors d_toff
-  int64_t* d_toff = nullptr; uint2* d_tpost = nullptr;
+  DevBuf<int64_t> d_toff; DevBuf<uint2> d_tpost;
   int64_t ix_rows = 0, ix_post = 0, ix_terms = 0, ix_builds = 0;
   std::vector<int64_t> h_toff;
   float ix_build_ms = 0.f;
@@ -498,10 +491,12 @@ int kw_ctx_acquire(aur_kw* kw, KwCtx** out) {
     if (!kw->idle.empty()) { *out = kw->idle.back(); kw->idle.pop_back(); return AUR_OK; }
   }
   std::unique_ptr<KwCtx> c(new KwCtx());
-  cudaError_t e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreate(&c->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&c->ev1);
-  if (e != cudaSuccess) { c->release(); return report_error(AUR_ERR_CUDA, "search context: %s", cudaGetErrorString(e)); }
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(c->stream.create(cudaStreamNonBlocking));
+    AUR_CU_RET(c->ev0.create());
+    return c->ev1.create();
+  }();
+  if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "search context: %s", cudaGetErrorString(e));
   std::lock_guard<std::mutex> lk(kw->mu_pool);
   *out = c.get();
   kw->ctxs.push_back(std::move(c));
@@ -527,21 +522,19 @@ int tombstone_rows(aur_kw* kw, const std::vector<int64_t>& rows) {
   std::vector<uint2> terms(static_cast<size_t>(noff[m]));
   DevBuf<int32_t> d_map; DevBuf<int64_t> d_noff; DevBuf<uint2> d_terms;
   cudaStream_t s = kw->stream;
-  cudaError_t e = d_map.reserve(m);
-  if (e == cudaSuccess) e = d_noff.reserve(m + 1);
-  if (e == cudaSuccess) e = d_terms.reserve(std::max<size_t>(terms.size(), 1));
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_map.p, map.data(), m * 4, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(d_noff.p, noff.data(), (m + 1) * 8, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) {
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(d_map.reserve(m));
+    AUR_CU_RET(d_noff.reserve(m + 1));
+    AUR_CU_RET(d_terms.reserve(std::max<size_t>(terms.size(), 1)));
+    AUR_CU_RET(cudaMemcpyAsync(d_map.p, map.data(), m * 4, cudaMemcpyHostToDevice, s));
+    AUR_CU_RET(cudaMemcpyAsync(d_noff.p, noff.data(), (m + 1) * 8, cudaMemcpyHostToDevice, s));
     kw_gather_postings<<<static_cast<unsigned>((static_cast<int64_t>(m) * 32 + 255) / 256), 256, 0, s>>>(
-        kw->d_post, kw->d_off, d_map.p, d_noff.p, static_cast<int64_t>(m), d_terms.p);
-    kw_scatter_flag<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(d_map.p, static_cast<int64_t>(m), kw->d_live, 0);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess && !terms.empty())
-    e = cudaMemcpyAsync(terms.data(), d_terms.p, terms.size() * 8, cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  d_map.release(); d_noff.release(); d_terms.release();
+        kw->d_post.p, kw->d_off.p, d_map.p, d_noff.p, static_cast<int64_t>(m), d_terms.p);
+    kw_scatter_flag<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(d_map.p, static_cast<int64_t>(m), kw->d_live.p, 0);
+    AUR_CU_RET(cudaGetLastError());
+    if (!terms.empty()) AUR_CU_RET(cudaMemcpyAsync(terms.data(), d_terms.p, terms.size() * 8, cudaMemcpyDeviceToHost, s));
+    return cudaStreamSynchronize(s);
+  }();
   if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "tombstone: %s", cudaGetErrorString(e));
   for (const uint2& p : terms) --kw->df[p.x];
   for (int64_t r : rows) {
@@ -552,29 +545,13 @@ int tombstone_rows(aur_kw* kw, const std::vector<int64_t>& rows) {
   return AUR_OK;
 }
 
-int grow_postings(aur_kw* kw, int64_t need) {
-  if (need <= kw->post_cap) return AUR_OK;
-  int64_t cap = std::max<int64_t>(need, kw->post_cap * 2);
-  uint2* p = nullptr;
-  KW_TRY(cudaMalloc(&p, static_cast<size_t>(cap) * 8));
-  const int64_t used = kw->h_off.back();
-  cudaError_t e = used ? cudaMemcpy(p, kw->d_post, static_cast<size_t>(used) * 8, cudaMemcpyDeviceToDevice) : cudaSuccess;
-  if (e != cudaSuccess) { cudaFree(p); return report_error(AUR_ERR_CUDA, "posting growth: %s", cudaGetErrorString(e)); }
-  cudaFree(kw->d_post);
-  kw->d_post = p; kw->post_cap = cap;
-  return AUR_OK;
-}
-
 // Drop the term-major index (rows are about to move).  Caller holds the exclusive lock.
 void drop_index(aur_kw* kw) {
-  int64_t* toff = nullptr; uint2* tpost = nullptr;
-  {
-    std::lock_guard<std::mutex> st(kw->mu_stat);
-    std::swap(toff, kw->d_toff); std::swap(tpost, kw->d_tpost);
-    kw->ix_rows = kw->ix_post = kw->ix_terms = 0;
-    kw->h_toff.clear();
-  }
-  cudaFree(toff); cudaFree(tpost);
+  DevBuf<int64_t> toff; DevBuf<uint2> tpost;   // the index, freed on return outside mu_stat
+  std::lock_guard<std::mutex> st(kw->mu_stat);
+  std::swap(toff, kw->d_toff); std::swap(tpost, kw->d_tpost);
+  kw->ix_rows = kw->ix_post = kw->ix_terms = 0;
+  kw->h_toff.clear();
 }
 
 // Build the term-major index of every appended row into fresh buffers on the store's stream and publish it.  The
@@ -586,26 +563,24 @@ int build_index(aur_kw* kw) {
   const int64_t T = static_cast<int64_t>(kw->df.size());   // every term id seen so far (writers resize df)
   KW_TRY(cudaSetDevice(kw->device));
   cudaStream_t s = kw->stream;
-  int64_t* toff = nullptr; uint2* tpost = nullptr;
-  DevBuf<unsigned> cnt; DevBuf<unsigned long long> cur;
+  DevBuf<int64_t> toff; DevBuf<uint2> tpost;
   std::vector<int64_t> h_toff(static_cast<size_t>(T) + 1);
   const unsigned row_blocks = static_cast<unsigned>((R * 32 + 255) / 256);
-  cudaError_t e = cudaMalloc(&toff, (static_cast<size_t>(T) + 1) * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&tpost, static_cast<size_t>(std::max<int64_t>(P, 1)) * 8);
-  if (e == cudaSuccess) e = cnt.reserve(static_cast<size_t>(std::max<int64_t>(T, 1)));
-  if (e == cudaSuccess) e = cur.reserve(static_cast<size_t>(std::max<int64_t>(T, 1)));
-  if (e == cudaSuccess) e = cudaMemsetAsync(cnt.p, 0, static_cast<size_t>(T) * 4, s);
-  if (e == cudaSuccess) {
-    if (R) kw_ix_count<<<row_blocks, 256, 0, s>>>(kw->d_off, kw->d_post, R, cnt.p);
-    kw_ix_scan<<<1, 1024, 0, s>>>(cnt.p, T, toff, cur.p);
-    if (R) kw_ix_scatter<<<row_blocks, 256, 0, s>>>(kw->d_off, kw->d_post, R, cur.p, tpost);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(h_toff.data(), toff, h_toff.size() * 8, cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  cnt.release(); cur.release();
+  const cudaError_t e = [&]() -> cudaError_t {
+    DevBuf<unsigned> cnt; DevBuf<unsigned long long> cur;
+    AUR_CU_RET(toff.reserve(static_cast<size_t>(T) + 1));
+    AUR_CU_RET(tpost.reserve(static_cast<size_t>(std::max<int64_t>(P, 1))));
+    AUR_CU_RET(cnt.reserve(static_cast<size_t>(std::max<int64_t>(T, 1))));
+    AUR_CU_RET(cur.reserve(static_cast<size_t>(std::max<int64_t>(T, 1))));
+    AUR_CU_RET(cudaMemsetAsync(cnt.p, 0, static_cast<size_t>(T) * 4, s));
+    if (R) kw_ix_count<<<row_blocks, 256, 0, s>>>(kw->d_off.p, kw->d_post.p, R, cnt.p);
+    kw_ix_scan<<<1, 1024, 0, s>>>(cnt.p, T, toff.p, cur.p);
+    if (R) kw_ix_scatter<<<row_blocks, 256, 0, s>>>(kw->d_off.p, kw->d_post.p, R, cur.p, tpost.p);
+    AUR_CU_RET(cudaGetLastError());
+    AUR_CU_RET(cudaMemcpyAsync(h_toff.data(), toff.p, h_toff.size() * 8, cudaMemcpyDeviceToHost, s));
+    return cudaStreamSynchronize(s);
+  }();
   if (e != cudaSuccess) {
-    cudaFree(toff); cudaFree(tpost);
     return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "keyword index build: %s",
                         cudaGetErrorString(e));
   }
@@ -619,8 +594,7 @@ int build_index(aur_kw* kw) {
     ++kw->ix_builds;
     kw->ix_build_ms = ms;
   }
-  cudaFree(toff); cudaFree(tpost);   // the previous index: no search holds it any more
-  return AUR_OK;
+  return AUR_OK;   // toff / tpost now hold the previous index, freed here: no search holds it any more
 }
 
 // The writer's rule: rebuild once the unindexed tail holds more than 1 / kIxTailFrac of the indexed postings (any
@@ -670,7 +644,7 @@ void kw_snapshot(aur_kw* kw, const std::vector<int32_t>& uniq, KwSnap* s) {
   s->udf.assign(uniq.size(), 0);
   for (size_t i = 0; i < uniq.size(); ++i)
     s->udf[i] = (uniq[i] >= 0 && uniq[i] < static_cast<int32_t>(kw->df.size())) ? kw->df[static_cast<size_t>(uniq[i])] : 0;
-  s->toff = kw->d_toff; s->tpost = kw->d_tpost;
+  s->toff = kw->d_toff.p; s->tpost = kw->d_tpost.p;
   s->ix_rows = kw->ix_rows; s->ix_post = kw->ix_post; s->ix_terms = kw->ix_terms;
   s->ulen.assign(uniq.size(), 0);
   for (size_t i = 0; i < uniq.size(); ++i)
@@ -838,8 +812,8 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
     n_passes = filter_passes(q.fp->n_programs);
     KW_TRY(c->fmask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(n_rows)));
     FiltParams p;
-    KW_TRY(filter_upload(*q.fp, kw->d_user, kw->d_org, kw->attrs, c->fstage, s, &p));
-    p.live = kw->d_live; p.n_rows = n_rows;
+    KW_TRY(filter_upload(*q.fp, kw->d_user.p, kw->d_org.p, kw->attrs, c->fstage, s, &p));
+    p.live = kw->d_live.p; p.n_rows = n_rows;
     for (int ps = 0; ps < n_passes; ++ps) {
       KW_TRY(launch_filter_mask(filter_pass(p, ps), c->fmask.p + static_cast<size_t>(ps) * n_rows, s));
       c->launches += 1;
@@ -875,8 +849,8 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
     KW_TRY(c->buf.reserve(static_cast<size_t>(std::max(gi, gt)) * nqb * kKwBufCap));
     KW_TRY(c->lists_a.reserve(static_cast<size_t>(nqb) * n_lists * ksel));
     KwParams p{};
-    p.off = kw->d_off; p.post = kw->d_post; p.len = kw->d_len; p.ids = kw->d_ids; p.user = kw->d_user; p.org = kw->d_org;
-    p.live = kw->d_live; p.allow = d_allow; p.n_rows = n_rows;
+    p.off = kw->d_off.p; p.post = kw->d_post.p; p.len = kw->d_len.p; p.ids = kw->d_ids.p; p.user = kw->d_user.p; p.org = kw->d_org.p;
+    p.live = kw->d_live.p; p.allow = d_allow; p.n_rows = n_rows;
     p.idf = reinterpret_cast<const double*>(c->tab.p); p.n_uniq = nu;
     p.hkey = reinterpret_cast<const int32_t*>(c->tab.p + b.b_hk); p.hval = reinterpret_cast<const int32_t*>(c->tab.p + b.b_hv);
     p.hmask = b.hcap - 1;
@@ -899,7 +873,7 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
         const int ng = std::min(ix.group, nqb - g0);
         int J = 0;
         for (int i = g0; i < g0 + ng; ++i) J = std::max(J, b.qoff[static_cast<size_t>(i) + 1] - b.qoff[static_cast<size_t>(i)]);
-        KwIxTerm t{sn.tpost, sn.toff, sn.ix_terms, kw->d_len, reinterpret_cast<const int32_t*>(c->tab.p + b.b_uk), p.idf,
+        KwIxTerm t{sn.tpost, sn.toff, sn.ix_terms, kw->d_len.p, reinterpret_cast<const int32_t*>(c->tab.p + b.b_uk), p.idf,
                    p.q_off + g0, p.slot_u, c->acc.p, R, avgdl, 0};
         for (int j = 0; j < J; ++j) {
           int64_t longest = 0;   // the longest list this launch reads
@@ -1138,27 +1112,23 @@ int aur_kw_open(int32_t device, int64_t doc_capacity, int64_t postings_capacity,
   std::unique_ptr<aur_kw> kw(new aur_kw());
   kw->device = device; kw->capacity = doc_capacity;
   kw->sm_count = prop.multiProcessorCount; kw->smem_optin = prop.sharedMemPerBlockOptin;
-  auto bail = [&](cudaError_t e) {
-    aur_kw_close(kw.release());
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(kw->stream.create(cudaStreamNonBlocking));
+    const size_t cap = static_cast<size_t>(doc_capacity);
+    AUR_CU_RET(kw->d_off.reserve(cap + 1));
+    AUR_CU_RET(kw->d_len.reserve(cap));
+    AUR_CU_RET(kw->d_ids.reserve(cap));
+    AUR_CU_RET(kw->d_user.reserve(cap));
+    AUR_CU_RET(kw->d_org.reserve(cap));
+    AUR_CU_RET(kw->d_live.reserve(cap));
+    AUR_CU_RET(kw->d_post.reserve(static_cast<size_t>(postings_capacity ? postings_capacity : (int64_t(1) << 20))));
+    AUR_CU_RET(cudaMemset(kw->d_off.p, 0, 8));
+    // once, at the device's limit: the attribute belongs to the kernel, not to a search, and searches run concurrently
+    AUR_CU_RET(cudaFuncSetAttribute(kw_score_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kw->smem_optin)));
+    return cudaFuncSetAttribute(kw_score_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kw->smem_optin));
+  }();
+  if (e != cudaSuccess)
     return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "aur_kw_open: %s", cudaGetErrorString(e));
-  };
-  cudaError_t e = cudaStreamCreateWithFlags(&kw->stream, cudaStreamNonBlocking);
-  const size_t cap = static_cast<size_t>(doc_capacity);
-  if (e == cudaSuccess) e = cudaMalloc(&kw->d_off, (cap + 1) * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&kw->d_len, cap * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&kw->d_ids, cap * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&kw->d_user, cap * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&kw->d_org, cap * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&kw->d_live, cap);
-  kw->post_cap = postings_capacity ? postings_capacity : (int64_t(1) << 20);
-  if (e == cudaSuccess) e = cudaMalloc(&kw->d_post, static_cast<size_t>(kw->post_cap) * 8);
-  if (e == cudaSuccess) e = cudaMemset(kw->d_off, 0, 8);
-  // once, at the device's limit: the attribute belongs to the kernel, not to a search, and searches run concurrently
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(kw_score_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kw->smem_optin));
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(kw_score_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kw->smem_optin));
-  if (e != cudaSuccess) return bail(e);
   *out = kw.release();
   return AUR_OK;
 }
@@ -1168,11 +1138,6 @@ int aur_kw_close(aur_kw* kw) {
   cudaSetDevice(kw->device);
   if (kw->stream) cudaStreamSynchronize(kw->stream);   // this store's work only: other users of the GPU are not waited on
   for (auto& c : kw->ctxs) cudaStreamSynchronize(c->stream);
-  cudaFree(kw->d_off); cudaFree(kw->d_len); cudaFree(kw->d_ids); cudaFree(kw->d_user); cudaFree(kw->d_org);
-  cudaFree(kw->d_live); cudaFree(kw->d_post); cudaFree(kw->d_toff); cudaFree(kw->d_tpost);
-  kw->attrs.release();
-  for (auto& c : kw->ctxs) c->release();
-  if (kw->stream) cudaStreamDestroy(kw->stream);
   delete kw;
   return AUR_OK;
 }
@@ -1242,13 +1207,14 @@ int kw_append_rows(aur_kw* kw, const KwRows& r, const KwLand& land) {
   const int64_t post0 = kw->h_off.back();
   bool replaces = false;
   for (int64_t i = 0; i < n && !replaces; ++i) replaces = kw->id2row.count(ids[i]) != 0;
-  const bool exclusive = replaces || post0 + total > kw->post_cap;
+  const bool exclusive = replaces || post0 + total > static_cast<int64_t>(kw->d_post.n);
   std::shared_lock<std::shared_mutex> rl(kw->rw, std::defer_lock);
   std::unique_lock<std::shared_mutex> xl(kw->rw, std::defer_lock);
   if (exclusive) xl.lock(); else rl.lock();
   KW_TRY(cudaSetDevice(kw->device));
-  int rc = grow_postings(kw, post0 + total);
-  if (rc != AUR_OK) return rc;
+  const cudaError_t ge = kw->d_post.grow_keep(static_cast<size_t>(post0 + total), static_cast<size_t>(post0), kw->stream);
+  if (ge != cudaSuccess)
+    return report_error(ge == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "posting growth: %s", cudaGetErrorString(ge));
   std::vector<int64_t> off(static_cast<size_t>(n));
   std::vector<int32_t> user(static_cast<size_t>(n)), org(static_cast<size_t>(n));
   std::vector<uint8_t> live(static_cast<size_t>(n), 1);
@@ -1262,13 +1228,13 @@ int kw_append_rows(aur_kw* kw, const KwRows& r, const KwLand& land) {
   for (int64_t i = 0; i < n; ++i) last[ids[i]] = i;
   for (int64_t i = 0; i < n; ++i) if (last[ids[i]] != i) live[static_cast<size_t>(i)] = 0;
   cudaStream_t s = kw->stream;
-  KW_TRY(land(kw->d_post + post0, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_off + base + 1, off.data(), static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_len + base, r.len, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_ids + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_user + base, user.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_org + base, org.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_live + base, live.data(), static_cast<size_t>(n), cudaMemcpyHostToDevice, s));
+  KW_TRY(land(kw->d_post.p + post0, s));
+  KW_TRY(cudaMemcpyAsync(kw->d_off.p + base + 1, off.data(), static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
+  KW_TRY(cudaMemcpyAsync(kw->d_len.p + base, r.len, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  KW_TRY(cudaMemcpyAsync(kw->d_ids.p + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
+  KW_TRY(cudaMemcpyAsync(kw->d_user.p + base, user.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  KW_TRY(cudaMemcpyAsync(kw->d_org.p + base, org.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  KW_TRY(cudaMemcpyAsync(kw->d_live.p + base, live.data(), static_cast<size_t>(n), cudaMemcpyHostToDevice, s));
   KW_TRY(cudaStreamSynchronize(s));
   for (int64_t i = 0; i < n; ++i) {
     kw->h_off.push_back(off[static_cast<size_t>(i)]);
@@ -1287,7 +1253,8 @@ int kw_append_rows(aur_kw* kw, const KwRows& r, const KwLand& land) {
       auto it = kw->id2row.find(ids[i]);
       if (it != kw->id2row.end()) old.push_back(it->second);
     }
-    if ((rc = tombstone_rows(kw, old)) != AUR_OK) return rc;
+    const int rc = tombstone_rows(kw, old);
+    if (rc != AUR_OK) return rc;
   }
   for (int64_t i = 0; i < n; ++i) {
     if (!live[static_cast<size_t>(i)]) continue;
@@ -1355,38 +1322,38 @@ int aur_kw_compact(aur_kw* kw, int64_t* reclaimed) {
     ids[static_cast<size_t>(j)] = kw->h_ids[r]; len[static_cast<size_t>(j)] = kw->h_len[r];
     user[static_cast<size_t>(j)] = kw->h_user[r]; org[static_cast<size_t>(j)] = kw->h_org[r];
   }
-  uint2* np_ = nullptr;
-  int32_t* d_map = nullptr;
-  int64_t* d_noff = nullptr;
-  cudaError_t e = cudaMalloc(&np_, static_cast<size_t>(kw->post_cap) * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&d_map, std::max<size_t>(1, map.size()) * 4);
-  if (e == cudaSuccess) e = cudaMalloc(&d_noff, off.size() * 8);
-  if (e == cudaSuccess && nl) e = cudaMemcpy(d_map, map.data(), map.size() * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(d_noff, off.data(), off.size() * 8, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && nl) {
-    const int64_t threads = nl * 32;
-    kw_gather_postings<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, kw->stream>>>(kw->d_post, kw->d_off, d_map, d_noff, nl, np_);
-    e = cudaGetLastError();
-  }
-  // attribute codes move with their rows (through a bounce buffer); the rows compaction frees start absent again
-  int32_t* bounce = nullptr;
-  if (e == cudaSuccess && kw->attrs.any() && nl) e = cudaMalloc(&bounce, static_cast<size_t>(nl) * 4);
-  if (e == cudaSuccess) e = kw->attrs.gather(d_map, nl, 0, bounce, kw->stream);
-  if (e == cudaSuccess) e = kw->attrs.clear(nl, rows, kw->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(kw->stream);
-  cudaFree(d_map);
-  cudaFree(bounce);
-  if (e != cudaSuccess) { cudaFree(np_); cudaFree(d_noff); return report_error(AUR_ERR_CUDA, "aur_kw_compact: %s", cudaGetErrorString(e)); }
-  cudaFree(kw->d_post);
-  kw->d_post = np_;
+  DevBuf<uint2> np;
+  cudaStream_t st = kw->stream;
+  cudaError_t e = [&]() -> cudaError_t {
+    DevBuf<int32_t> d_map, bounce; DevBuf<int64_t> d_noff;
+    AUR_CU_RET(np.reserve(kw->d_post.n));
+    AUR_CU_RET(d_map.reserve(std::max<size_t>(1, map.size())));
+    AUR_CU_RET(d_noff.reserve(off.size()));
+    if (nl) AUR_CU_RET(cudaMemcpy(d_map.p, map.data(), map.size() * 4, cudaMemcpyHostToDevice));
+    AUR_CU_RET(cudaMemcpy(d_noff.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
+    if (nl) {
+      const int64_t threads = nl * 32;
+      kw_gather_postings<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, st>>>(kw->d_post.p, kw->d_off.p, d_map.p, d_noff.p, nl, np.p);
+      AUR_CU_RET(cudaGetLastError());
+    }
+    // attribute codes move with their rows (through a bounce buffer); the rows compaction frees start absent again
+    if (kw->attrs.any() && nl) AUR_CU_RET(bounce.reserve(static_cast<size_t>(nl)));
+    AUR_CU_RET(kw->attrs.gather(d_map.p, nl, 0, bounce.p, st));
+    AUR_CU_RET(kw->attrs.clear(nl, rows, st));
+    return cudaStreamSynchronize(st);
+  }();
+  if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "aur_kw_compact: %s", cudaGetErrorString(e));
+  kw->d_post = std::move(np);
   std::vector<uint8_t> live(static_cast<size_t>(nl), 1);
-  e = cudaMemcpy(kw->d_off, off.data(), off.size() * 8, cudaMemcpyHostToDevice);
-  cudaFree(d_noff);
-  if (e == cudaSuccess && nl) e = cudaMemcpy(kw->d_len, len.data(), static_cast<size_t>(nl) * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && nl) e = cudaMemcpy(kw->d_ids, ids.data(), static_cast<size_t>(nl) * 8, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && nl) e = cudaMemcpy(kw->d_user, user.data(), static_cast<size_t>(nl) * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && nl) e = cudaMemcpy(kw->d_org, org.data(), static_cast<size_t>(nl) * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && nl) e = cudaMemcpy(kw->d_live, live.data(), static_cast<size_t>(nl), cudaMemcpyHostToDevice);
+  e = [&]() -> cudaError_t {
+    AUR_CU_RET(cudaMemcpy(kw->d_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice));
+    if (!nl) return cudaSuccess;
+    AUR_CU_RET(cudaMemcpy(kw->d_len.p, len.data(), static_cast<size_t>(nl) * 4, cudaMemcpyHostToDevice));
+    AUR_CU_RET(cudaMemcpy(kw->d_ids.p, ids.data(), static_cast<size_t>(nl) * 8, cudaMemcpyHostToDevice));
+    AUR_CU_RET(cudaMemcpy(kw->d_user.p, user.data(), static_cast<size_t>(nl) * 4, cudaMemcpyHostToDevice));
+    AUR_CU_RET(cudaMemcpy(kw->d_org.p, org.data(), static_cast<size_t>(nl) * 4, cudaMemcpyHostToDevice));
+    return cudaMemcpy(kw->d_live.p, live.data(), static_cast<size_t>(nl), cudaMemcpyHostToDevice);
+  }();
   if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "aur_kw_compact: %s (the store may be inconsistent: rebuild it)", cudaGetErrorString(e));
   kw->h_off = off; kw->h_len = len; kw->h_ids = ids; kw->h_user = user; kw->h_org = org; kw->h_live = live;
   kw->id2row.clear();
@@ -1410,7 +1377,7 @@ int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out) {
     out->postings_used = kw->post_pub;
   }
   std::lock_guard<std::mutex> lk(kw->mu_pool);
-  out->postings_allocated = kw->post_cap;
+  out->postings_allocated = static_cast<int64_t>(kw->d_post.n);
   out->capacity = kw->capacity;
   out->last_launches = kw->last_launches;
   out->last_ms = kw->last_ms;
@@ -1488,7 +1455,7 @@ int aur_kw_read_rows(aur_kw* kw, int64_t row0, int64_t n, int64_t* ids_out, int6
   if (!term_ids_out || !tfs_out || cap < total || total == 0) return AUR_OK;   // count mode
   KW_TRY(cudaSetDevice(kw->device));
   std::vector<uint2> post(static_cast<size_t>(total));
-  KW_TRY(cudaMemcpyAsync(post.data(), kw->d_post + p0, static_cast<size_t>(total) * 8, cudaMemcpyDeviceToHost, kw->stream));
+  KW_TRY(cudaMemcpyAsync(post.data(), kw->d_post.p + p0, static_cast<size_t>(total) * 8, cudaMemcpyDeviceToHost, kw->stream));
   KW_TRY(cudaStreamSynchronize(kw->stream));
   for (int64_t j = 0; j < total; ++j) {
     term_ids_out[j] = static_cast<int32_t>(post[static_cast<size_t>(j)].x);
@@ -1520,7 +1487,7 @@ int aur_kw_get_index_stats(aur_kw* kw, aur_kw_index_stats* out) {
     std::lock_guard<std::mutex> st(kw->mu_stat);
     out->indexed_rows = kw->ix_rows;
     out->index_postings = kw->ix_post;
-    out->index_bytes = kw->d_toff ? kw->ix_post * 8 + (kw->ix_terms + 1) * 8 : 0;
+    out->index_bytes = kw->d_toff.p ? kw->ix_post * 8 + (kw->ix_terms + 1) * 8 : 0;
     out->builds = kw->ix_builds;
     out->last_build_ms = kw->ix_build_ms;
   }

@@ -237,69 +237,43 @@ __global__ void tx_gather(const uint2* post, const int64_t* src_off, const int32
 struct aur_kw_vocab {
   std::mutex mu;                   // one text add (or read) at a time
   int device = 0;
-  cudaStream_t stream = nullptr;
+  Stream stream;
   int hash_bits = 64;
   int64_t words = 0, bytes = 0;    // V and the pool bytes in use
-  uint64_t* hkey = nullptr; int32_t* hid = nullptr; int64_t tcap = 0;   // table (power of two)
-  uint8_t* pool = nullptr; int64_t pool_cap = 0;
-  int64_t* woff = nullptr; int64_t woff_cap = 0;                       // [words + 1]
+  DevBuf<uint64_t> hkey; DevBuf<int32_t> hid;                         // table (power of two entries)
+  DevBuf<uint8_t> pool;
+  DevBuf<int64_t> woff;                                                // [words + 1]
   // one slice's scratch (grow-only)
-  uint8_t* h_stage = nullptr; size_t stage_cap = 0;                    // page-locked text staging
+  HostBuf<uint8_t> h_stage;                                            // page-locked text staging
   DevBuf<uint8_t> text, norm, cub_tmp;
   DevBuf<int64_t> doff, totals, goff_src, goff_dst;
   DevBuf<int32_t> is_w, is_s, cpos, widx, wstart, wdoc, found, bslot, occ, first, is_first, rank, nlen, noff;
   DevBuf<int32_t> cnt, n_runs, tid, dcnt, dlen, gmap;
   DevBuf<uint64_t> wh, key, key_sorted, ukey;
   DevBuf<uint2> post, spost;
-  void release() {
-    for (auto* b : {&text, &norm, &cub_tmp}) b->release();
-    for (auto* b : {&doff, &totals, &goff_src, &goff_dst}) b->release();
-    for (auto* b : {&is_w, &is_s, &cpos, &widx, &wstart, &wdoc, &found, &bslot, &occ, &first, &is_first, &rank, &nlen, &noff,
-                    &cnt, &n_runs, &tid, &dcnt, &dlen, &gmap}) b->release();
-    for (auto* b : {&wh, &key, &key_sorted, &ukey}) b->release();
-    post.release(); spost.release();
-    cudaFree(hkey); cudaFree(hid); cudaFree(pool); cudaFree(woff);
-    if (h_stage) cudaFreeHost(h_stage);
-    if (stream) cudaStreamDestroy(stream);
-  }
 };
 
 namespace {
 
 int ensure_table(aur_kw_vocab* v, int64_t need_words) {
-  if (v->tcap && 2 * need_words <= v->tcap) return AUR_OK;
-  int64_t cap = std::max<int64_t>(v->tcap, 1024);
+  const int64_t tcap = static_cast<int64_t>(v->hkey.n);
+  if (tcap && 2 * need_words <= tcap) return AUR_OK;
+  int64_t cap = std::max<int64_t>(tcap, 1024);
   while (2 * need_words > cap) cap *= 2;
-  uint64_t* hk = nullptr; int32_t* hi = nullptr;
-  cudaError_t e = cudaMalloc(&hk, static_cast<size_t>(cap) * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&hi, static_cast<size_t>(cap) * 4);
-  if (e == cudaSuccess) e = cudaMemsetAsync(hi, 0xFF, static_cast<size_t>(cap) * 4, v->stream);
-  if (e == cudaSuccess && v->tcap) {
-    tx_rehash<<<blocks(v->tcap), kT, 0, v->stream>>>(v->hkey, v->hid, v->tcap, hk, hi, static_cast<uint64_t>(cap - 1));
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(v->stream);
-  if (e != cudaSuccess) {
-    cudaFree(hk); cudaFree(hi);
+  DevBuf<uint64_t> hk; DevBuf<int32_t> hi;
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(hk.reserve(static_cast<size_t>(cap)));
+    AUR_CU_RET(hi.reserve(static_cast<size_t>(cap)));
+    AUR_CU_RET(cudaMemsetAsync(hi.p, 0xFF, static_cast<size_t>(cap) * 4, v->stream));
+    if (tcap) {
+      tx_rehash<<<blocks(tcap), kT, 0, v->stream>>>(v->hkey.p, v->hid.p, tcap, hk.p, hi.p, static_cast<uint64_t>(cap - 1));
+      AUR_CU_RET(cudaGetLastError());
+    }
+    return cudaStreamSynchronize(v->stream);
+  }();
+  if (e != cudaSuccess)
     return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "vocabulary table: %s", cudaGetErrorString(e));
-  }
-  cudaFree(v->hkey); cudaFree(v->hid);
-  v->hkey = hk; v->hid = hi; v->tcap = cap;
-  return AUR_OK;
-}
-
-// Grow-only device array with its contents kept (used bytes).
-template <typename T>
-int grow_keep(T** p, int64_t* cap, int64_t need, int64_t used, cudaStream_t s) {
-  if (need <= *cap) return AUR_OK;
-  const int64_t c = std::max<int64_t>(need, 2 * *cap);
-  T* q = nullptr;
-  TX_TRY(cudaMalloc(&q, static_cast<size_t>(c) * sizeof(T)));
-  cudaError_t e = used ? cudaMemcpyAsync(q, *p, static_cast<size_t>(used) * sizeof(T), cudaMemcpyDeviceToDevice, s) : cudaSuccess;
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e != cudaSuccess) { cudaFree(q); return report_error(AUR_ERR_CUDA, "vocabulary growth: %s", cudaGetErrorString(e)); }
-  cudaFree(*p);
-  *p = q; *cap = c;
+  v->hkey = std::move(hk); v->hid = std::move(hi);
   return AUR_OK;
 }
 
@@ -317,19 +291,15 @@ struct SliceRows {
 int analyse(aur_kw_vocab* v, const char* text, const int64_t* off, int32_t n, SliceRows* out) {
   cudaStream_t s = v->stream;
   const int64_t nb = off[n];
-  if (v->stage_cap < static_cast<size_t>(nb)) {
-    if (v->h_stage) cudaFreeHost(v->h_stage);
-    v->h_stage = nullptr; v->stage_cap = 0;
-    TX_TRY(cudaHostAlloc(&v->h_stage, static_cast<size_t>(std::max<int64_t>(nb, 1 << 20)), cudaHostAllocDefault));
-    v->stage_cap = static_cast<size_t>(std::max<int64_t>(nb, 1 << 20));
-  }
+  if (v->h_stage.n < static_cast<size_t>(nb))
+    TX_TRY(v->h_stage.reserve(static_cast<size_t>(std::max<int64_t>(nb, 1 << 20)), cudaHostAllocDefault));
   // 1. text in (the staging buffer is reused only after this slice's work has completed)
-  if (nb) memcpy(v->h_stage, text, static_cast<size_t>(nb));
+  if (nb) memcpy(v->h_stage.p, text, static_cast<size_t>(nb));
   const size_t B = static_cast<size_t>(std::max<int64_t>(nb, 1));
   TX_TRY(v->text.reserve(B)); TX_TRY(v->doff.reserve(static_cast<size_t>(n) + 1));
   TX_TRY(v->is_w.reserve(B)); TX_TRY(v->is_s.reserve(B)); TX_TRY(v->cpos.reserve(B)); TX_TRY(v->widx.reserve(B));
   TX_TRY(v->totals.reserve(2));
-  if (nb) TX_TRY(cudaMemcpyAsync(v->text.p, v->h_stage, static_cast<size_t>(nb), cudaMemcpyHostToDevice, s));
+  if (nb) TX_TRY(cudaMemcpyAsync(v->text.p, v->h_stage.p, static_cast<size_t>(nb), cudaMemcpyHostToDevice, s));
   TX_TRY(cudaMemcpyAsync(v->doff.p, off, (static_cast<size_t>(n) + 1) * 8, cudaMemcpyHostToDevice, s));
   // 2. classify, scans: normalised bytes and word starts
   int32_t nw = 0, nl = 0;
@@ -370,7 +340,7 @@ int analyse(aur_kw_vocab* v, const char* text, const int64_t* off, int32_t n, Sl
   TX_TRY(v->wh.reserve(W)); TX_TRY(v->found.reserve(W)); TX_TRY(v->bslot.reserve(W));
   const uint64_t hmask = v->hash_bits >= 64 ? ~0ull : ((1ull << v->hash_bits) - 1);
   tx_hash<<<blocks(nw), kT, 0, s>>>(w, hmask, v->wh.p);
-  tx_lookup<<<blocks(nw), kT, 0, s>>>(w, v->wh.p, VocabDev{v->hkey, v->hid, static_cast<uint64_t>(v->tcap - 1), v->pool, v->woff},
+  tx_lookup<<<blocks(nw), kT, 0, s>>>(w, v->wh.p, VocabDev{v->hkey.p, v->hid.p, static_cast<uint64_t>(v->hkey.n - 1), v->pool.p, v->woff.p},
                                       v->found.p);
   TX_TRY(cudaGetLastError());
   // 5. new words: group, rank by first occurrence
@@ -410,13 +380,17 @@ int analyse(aur_kw_vocab* v, const char* text, const int64_t* off, int32_t n, Sl
   TX_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, tb_rle, v->key_sorted.p, v->ukey.p, v->cnt.p, v->n_runs.p, nw, s));
   TX_TRY(v->cub_tmp.reserve(std::max<size_t>(std::max(tb_sort, tb_rle), 1)));
   // growth, then insertion
-  int rc = ensure_table(v, V + n_new);
-  if (rc == AUR_OK) rc = grow_keep(&v->pool, &v->pool_cap, v->bytes + new_bytes, v->bytes, s);
-  if (rc == AUR_OK) rc = grow_keep(&v->woff, &v->woff_cap, V + n_new + 1, V + 1, s);
+  const int rc = ensure_table(v, V + n_new);
   if (rc != AUR_OK) return rc;
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(v->pool.grow_keep(static_cast<size_t>(v->bytes + new_bytes), static_cast<size_t>(v->bytes), s));
+    return v->woff.grow_keep(static_cast<size_t>(V + n_new + 1), static_cast<size_t>(V + 1), s);
+  }();
+  if (e != cudaSuccess)
+    return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "vocabulary growth: %s", cudaGetErrorString(e));
   if (n_new) {
-    tx_insert<<<blocks(nw), kT, 0, s>>>(w, v->wh.p, v->is_first.p, v->rank.p, v->noff.p, V, v->bytes, v->hkey, v->hid,
-                                        static_cast<uint64_t>(v->tcap - 1), v->pool, v->woff);
+    tx_insert<<<blocks(nw), kT, 0, s>>>(w, v->wh.p, v->is_first.p, v->rank.p, v->noff.p, V, v->bytes, v->hkey.p, v->hid.p,
+                                        static_cast<uint64_t>(v->hkey.n - 1), v->pool.p, v->woff.p);
     TX_TRY(cudaGetLastError());
     v->words = V + n_new;
     v->bytes += new_bytes;
@@ -526,23 +500,17 @@ int aur_kw_vocab_open(int32_t device, aur_kw_vocab** out) {
   if (prop.major != 9) return report_error(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
   std::unique_ptr<aur_kw_vocab> v(new aur_kw_vocab());
   v->device = device;
-  cudaError_t e = cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) {
-    v->woff_cap = 1024;
-    e = cudaMalloc(&v->woff, static_cast<size_t>(v->woff_cap) * 8);
-  }
-  if (e == cudaSuccess) e = cudaMemsetAsync(v->woff, 0, 8, v->stream);
-  if (e == cudaSuccess) {
-    v->pool_cap = 1 << 16;
-    e = cudaMalloc(&v->pool, static_cast<size_t>(v->pool_cap));
-  }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(v->stream);
-  if (e != cudaSuccess) {
-    v->release();
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(v->stream.create(cudaStreamNonBlocking));
+    AUR_CU_RET(v->woff.reserve(1024));
+    AUR_CU_RET(cudaMemsetAsync(v->woff.p, 0, 8, v->stream));
+    AUR_CU_RET(v->pool.reserve(1 << 16));
+    return cudaStreamSynchronize(v->stream);
+  }();
+  if (e != cudaSuccess)
     return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "aur_kw_vocab_open: %s", cudaGetErrorString(e));
-  }
   const int rc = ensure_table(v.get(), 0);
-  if (rc != AUR_OK) { v->release(); return rc; }
+  if (rc != AUR_OK) return rc;
   *out = v.release();
   return AUR_OK;
 }
@@ -551,7 +519,6 @@ int aur_kw_vocab_close(aur_kw_vocab* v) {
   if (!v) return AUR_OK;
   cudaSetDevice(v->device);
   if (v->stream) cudaStreamSynchronize(v->stream);
-  v->release();
   delete v;
   return AUR_OK;
 }
@@ -572,13 +539,13 @@ int aur_kw_vocab_read(aur_kw_vocab* v, int64_t id0, int64_t n, char* bytes_out, 
                         (long long)v->words);
   std::vector<int64_t> wo(static_cast<size_t>(n) + 1);
   TX_TRY(cudaSetDevice(v->device));
-  TX_TRY(cudaMemcpyAsync(wo.data(), v->woff + id0, wo.size() * 8, cudaMemcpyDeviceToHost, v->stream));
+  TX_TRY(cudaMemcpyAsync(wo.data(), v->woff.p + id0, wo.size() * 8, cudaMemcpyDeviceToHost, v->stream));
   TX_TRY(cudaStreamSynchronize(v->stream));
   const int64_t nbytes = wo.back() - wo[0];
   if (bytes_out && bytes_cap < nbytes)
     return report_error(AUR_ERR_INVALID, "bytes_cap %lld < %lld bytes", (long long)bytes_cap, (long long)nbytes);
   if (bytes_out && nbytes) {
-    TX_TRY(cudaMemcpyAsync(bytes_out, v->pool + wo[0], static_cast<size_t>(nbytes), cudaMemcpyDeviceToHost, v->stream));
+    TX_TRY(cudaMemcpyAsync(bytes_out, v->pool.p + wo[0], static_cast<size_t>(nbytes), cudaMemcpyDeviceToHost, v->stream));
     TX_TRY(cudaStreamSynchronize(v->stream));
   }
   for (int64_t i = 0; i <= n; ++i) offsets_out[i] = wo[static_cast<size_t>(i)] - wo[0];

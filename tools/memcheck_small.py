@@ -1,6 +1,7 @@
 """Small end-to-end run for `compute-sanitizer --tool memcheck` (seconds under the tool):
 tensor-core + generic search with partial query blocks, deletes, repeated launches; a tiny encoder forward
-with fused ingest.  Exits non-zero on a parity mismatch."""
+with fused ingest; text added to, searched in and closed with a keyword store and its vocabulary.  Exits non-zero on a
+parity mismatch."""
 import os
 import sys
 
@@ -9,7 +10,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from aurora_b200 import _native as N
 from aurora_b200.encoder import Encoder, EncoderConfig
-from aurora_b200.engine import Index
+from aurora_b200.engine import Index, KeywordIndex, KeywordVocab
 from oracle import bert_encoder as B
 from oracle import cosine_topk as O
 
@@ -62,3 +63,10 @@ with Encoder(cfg, max_tokens=2048, max_seqs=8) as enc, Index(128, 32) as ix:
     assert ix.stats()["live"] == 5
 print("encoder ok (attention v2)")
 
+
+vocab, store = KeywordVocab(0), KeywordIndex(64)
+store.add_text(vocab, np.arange(3, dtype=np.int64), ["alpha beta", "gamma alpha delta", "beta beta epsilon"])
+ids, _, snap = store.search(np.array([1, 2], np.int32), np.array([0, 1, 2], np.int64), 2)   # beta; gamma
+assert snap == 3 and ids[0].tolist() == [2, 0] and ids[1].tolist() == [1, -1], ids
+store.close(); vocab.close()
+print("keyword ok")
