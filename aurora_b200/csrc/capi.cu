@@ -109,21 +109,14 @@ int encode_tmap_2d_u8(void* tmap, const void* base, uint64_t cols, uint64_t rows
 
 namespace {
 int (&fail)(int, const char*, ...) = report_error;
-#define CU_TRY(expr)                                                                               \
-  do {                                                                                             \
-    cudaError_t e_ = (expr);                                                                       \
-    if (e_ != cudaSuccess) return fail(AUR_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e_), \
-                                       __FILE__, __LINE__);                                        \
-  } while (0)
 }  // namespace
 
 // Scratch and bookkeeping of ONE in-flight search.  Device-pointer searches are bound to the caller's stream
-// (same stream -> same context -> stream order protects the scratch); host-buffer searches take a context from a
-// pool and run on its own stream, so N threads can search at once.
+// (same stream -> same context -> stream order protects the scratch); host-buffer searches lease a context from the
+// index's pool and run on its own stream, so N threads can search at once.
 struct SearchCtx {
   std::mutex mu;                  // one enqueue at a time
-  Stream own_stream;
-  cudaStream_t bound = nullptr;   // caller stream this context serves (nullptr = pool context)
+  Stream stream;
   Event ev_begin, ev_k0, ev_k1, ev_fin, ev_end;
   bool have_timing = false;
   int last_kernel = 0, last_launches = 0, last_nq = 0;
@@ -153,11 +146,21 @@ struct SearchCtx {
   DevBuf<int32_t> filt_rows;     // filtered search: every program's matching rows, ascending, program after program
   DevBuf<int64_t> filt_ids;      // aur_filter_ids: their ids
   HostBuf<uint32_t> h_totals;    // page-locked landing area of the count pass's totals (kFiltCallPrograms words)
+
+  int init(int /* device: current */) {
+    int lo = 0, hi = 0;
+    AUR_TRY(cudaDeviceGetStreamPriorityRange(&lo, &hi));   // hi = numerically lowest = highest priority
+    AUR_TRY(stream.create(cudaStreamNonBlocking, hi));
+    AUR_TRY(ev_begin.create()); AUR_TRY(ev_k0.create());
+    AUR_TRY(ev_k1.create());    AUR_TRY(ev_end.create());
+    AUR_TRY(ev_fin.create());
+    return AUR_OK;
+  }
 };
 
 struct aur_index {
   std::shared_mutex rw;          // shared: searches and appends; exclusive: compaction, export, close
-  std::mutex mu;                 // host metadata: id2row, live, options, the context pool
+  std::mutex mu;                 // host metadata: id2row, live, options, the bound contexts
   std::mutex mu_write;           // one writer at a time (append / remove)
   int device = 0, dim = 0, dtype = 0;
   int64_t capacity = 0, live = 0;
@@ -186,8 +189,8 @@ struct aur_index {
   int opt_tc_stages = 0;         // cap on the TMA ring's depth: 0 = the deepest that fits
   int opt_tc_qregs = -1;         // query k-blocks in the MMA warpgroup's registers: -1 = auto, 0 = none, kTcQRegs
   std::atomic<uint32_t> opt_dbg_epoch{0};   // bring-up: start value of the contexts' launch counters (0 = 1)
-  std::vector<std::unique_ptr<SearchCtx>> ctxs;
-  std::vector<SearchCtx*> free_ctxs;   // idle pool contexts
+  CtxPool<SearchCtx> ctxs;             // host-buffer calls (HostCall)
+  std::unordered_map<cudaStream_t, std::unique_ptr<SearchCtx>> bound;   // device-pointer calls, by caller stream
   SearchCtx* last_ctx = nullptr;       // context of the most recently enqueued search (aur_get_stats)
 };
 
@@ -220,37 +223,19 @@ bool tc_shape_ok(const aur_index* ix, int k, bool filtered) {
   return tc_pick_stages(k + kSlack, ix->dim, ix->smem_optin, kTcTileN, true) >= 2;
 }
 
-int ctx_init(SearchCtx* c) {
-  int lo = 0, hi = 0;
-  CU_TRY(cudaDeviceGetStreamPriorityRange(&lo, &hi));   // hi = numerically lowest = highest priority
-  CU_TRY(c->own_stream.create(cudaStreamNonBlocking, hi));
-  CU_TRY(c->ev_begin.create()); CU_TRY(c->ev_k0.create());
-  CU_TRY(c->ev_k1.create());    CU_TRY(c->ev_end.create());
-  CU_TRY(c->ev_fin.create());
-  return AUR_OK;
-}
-
-// Context for a search on the caller's stream `s` (bound) or, with s == nullptr, an idle pool context.
-int acquire_ctx(aur_index* ix, cudaStream_t s, SearchCtx** out) {
+// The context of the device-pointer searches on the caller's stream s, made on first use.  It is never pooled and never
+// drained: those calls are asynchronous, and stream order protects its scratch.
+int bound_ctx(aur_index* ix, cudaStream_t s, SearchCtx** out) {
   std::lock_guard<std::mutex> lk(ix->mu);
-  if (s) {
-    for (auto& c : ix->ctxs)
-      if (c->bound == s) { *out = c.get(); return AUR_OK; }
-  } else if (!ix->free_ctxs.empty()) {
-    *out = ix->free_ctxs.back(); ix->free_ctxs.pop_back();
-    return AUR_OK;
+  auto it = ix->bound.find(s);
+  if (it == ix->bound.end()) {
+    std::unique_ptr<SearchCtx> c(new SearchCtx());
+    const int rc = c->init(ix->device);
+    if (rc != AUR_OK) return rc;
+    it = ix->bound.emplace(s, std::move(c)).first;
   }
-  std::unique_ptr<SearchCtx> c(new SearchCtx());
-  int rc = ctx_init(c.get());
-  if (rc != AUR_OK) return rc;
-  c->bound = s;
-  *out = c.get();
-  ix->ctxs.push_back(std::move(c));
+  *out = it->second.get();
   return AUR_OK;
-}
-void release_ctx(aur_index* ix, SearchCtx* c) {
-  std::lock_guard<std::mutex> lk(ix->mu);
-  if (!c->bound) ix->free_ctxs.push_back(c);
 }
 
 // Pinned caller buffers are mapped into the device's address space (UVA): the re-rank kernel then writes its nq x k
@@ -268,13 +253,14 @@ bool direct_outputs(float* scores_out, int64_t* ids_out, float** d_scores, int64
   return false;
 }
 
-// One call with host buffers: the index's shared lock, its device, an idle pool context locked for the call and given
-// back when the call ends, the context's own stream, and the prefix published when the call began (open()).  A search
-// call stages its queries and outputs with stage().
+// One call with host buffers: the index's shared lock, its device, a context leased from the index's pool and locked
+// for the call, the context's own stream, and the prefix published when the call began (open()).  The lease comes after
+// the shared lock, so the stream is idle before the lock is released.  A search call stages its queries and outputs
+// with stage().
 struct HostCall {
   aur_index* ix;
   std::shared_lock<std::shared_mutex> rl;
-  SearchCtx* c = nullptr;
+  CtxLease<SearchCtx> c;
   std::unique_lock<std::mutex> cl;
   cudaStream_t s = nullptr;
   int64_t n_rows = 0;
@@ -285,17 +271,12 @@ struct HostCall {
   explicit HostCall(aur_index* index) : ix(index), rl(index->rw) {}
   HostCall(const HostCall&) = delete;
   HostCall& operator=(const HostCall&) = delete;
-  ~HostCall() {
-    if (!c) return;
-    cl.unlock();
-    release_ctx(ix, c);
-  }
   int open() {
-    CU_TRY(cudaSetDevice(ix->device));
-    const int rc = acquire_ctx(ix, nullptr, &c);
+    AUR_TRY(cudaSetDevice(ix->device));
+    const int rc = ix->ctxs.lease(&c);
     if (rc != AUR_OK) return rc;
     cl = std::unique_lock<std::mutex>(c->mu);
-    s = c->own_stream;
+    s = c->stream;
     n_rows = ix->rows_pub.load(std::memory_order_acquire);
     return AUR_OK;
   }
@@ -304,10 +285,10 @@ struct HostCall {
   int stage(const void* queries_host, int32_t nq, int32_t k, float* scores_out, int64_t* ids_out) {
     const size_t qbytes = static_cast<size_t>(nq) * ix->dim * ix->qelt;
     const size_t nout = static_cast<size_t>(nq) * k;
-    CU_TRY(c->stage_q.reserve(qbytes));
-    CU_TRY(c->stage_scores.reserve(nout));
-    CU_TRY(c->stage_ids.reserve(nout));
-    CU_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
+    AUR_TRY(c->stage_q.reserve(qbytes));
+    AUR_TRY(c->stage_scores.reserve(nout));
+    AUR_TRY(c->stage_ids.reserve(nout));
+    AUR_TRY(cudaMemcpyAsync(c->stage_q.p, queries_host, qbytes, cudaMemcpyHostToDevice, s));
     d_scores = c->stage_scores.p;
     d_ids = c->stage_ids.p;
     direct = scores_out && ids_out && direct_outputs(scores_out, ids_out, &d_scores, &d_ids);
@@ -378,24 +359,24 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   if (ix->opt_tc_stages >= 2 && ix->opt_tc_stages < stages) stages = ix->opt_tc_stages;
   const size_t smem = tc_smem_bytes(stages, ksel, ix->dim, tile_n, mask, qregs);
   const size_t ncand = static_cast<size_t>(n_qblocks) * kTcQRows * n_lists * ksel;
-  CU_TRY(c->cand_a.reserve(ncand));
+  AUR_TRY(c->cand_a.reserve(ncand));
   const size_t npub = static_cast<size_t>(n_qblocks) * kTcQRows * (((n_lists + 1) & ~1) + 1);
   if (npub > c->pub.n) {
-    CU_TRY(c->pub.reserve(npub));
-    CU_TRY(cudaMemsetAsync(c->pub.p, 0, npub * 8, s));  // epoch 0 is never used by a launch
+    AUR_TRY(c->pub.reserve(npub));
+    AUR_TRY(cudaMemsetAsync(c->pub.p, 0, npub * 8, s));  // epoch 0 is never used by a launch
   }
   if (c->cand_count.n < 8 * kTcQRows) {
-    CU_TRY(c->cand_count.reserve(8 * kTcQRows));
-    CU_TRY(cudaMemsetAsync(c->cand_count.p, 0, 8 * kTcQRows * 4, s));
+    AUR_TRY(c->cand_count.reserve(8 * kTcQRows));
+    AUR_TRY(cudaMemsetAsync(c->cand_count.p, 0, 8 * kTcQRows * 4, s));
   }
   if (c->d_epoch.n == 0) {
     const uint32_t e0 = ix->opt_dbg_epoch.load() ? ix->opt_dbg_epoch.load() : 1u;
-    CU_TRY(c->d_epoch.reserve(1));
-    CU_TRY(cudaMemcpyAsync(c->d_epoch.p, &e0, 4, cudaMemcpyHostToDevice, s));   // pageable source: staged before return
+    AUR_TRY(c->d_epoch.reserve(1));
+    AUR_TRY(cudaMemcpyAsync(c->d_epoch.p, &e0, 4, cudaMemcpyHostToDevice, s));   // pageable source: staged before return
   }
   if (i8) {
-    CU_TRY(c->q_img.reserve(static_cast<size_t>(nqb) * ix->dim * 2));
-    CU_TRY(launch_query_image_i8(static_cast<const __nv_bfloat16*>(q_dev), ix->dim, nqb, c->q_img.p, s));
+    AUR_TRY(c->q_img.reserve(static_cast<size_t>(nqb) * ix->dim * 2));
+    AUR_TRY(launch_query_image_i8(static_cast<const __nv_bfloat16*>(q_dev), ix->dim, nqb, c->q_img.p, s));
     c->last_launches += 1;
   }
   ++c->epoch;
@@ -417,7 +398,7 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   p.num_stages = stages;
   p.dbg_flags = ix->opt_dbg_flags;
   p.n_tiles = static_cast<int>((n_rows + tile_n - 1) / tile_n);
-  CU_TRY(tc_launch(cta_group, tile_n, qregs, i8, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
+  AUR_TRY(tc_launch(cta_group, tile_n, qregs, i8, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
   c->last_tile_n = tile_n;
   *n_lists_out = n_lists;
   return AUR_OK;
@@ -447,12 +428,12 @@ int stats_begin(SearchCtx* c, cudaStream_t s, int nq, int64_t n_rows) {
   c->last_tile_n = 0;
   c->last_nq = nq;
   c->snapshot_rows = n_rows;
-  CU_TRY(cudaEventRecord(c->ev_begin, s));
+  AUR_TRY(cudaEventRecord(c->ev_begin, s));
   return AUR_OK;
 }
 int stats_end(aur_index* ix, SearchCtx* c, cudaStream_t s) {
-  CU_TRY(cudaEventRecord(c->ev_fin, s));
-  CU_TRY(cudaEventRecord(c->ev_end, s));
+  AUR_TRY(cudaEventRecord(c->ev_fin, s));
+  AUR_TRY(cudaEventRecord(c->ev_end, s));
   c->have_timing = true;
   std::lock_guard<std::mutex> lk(ix->mu);
   ix->last_ctx = c;
@@ -472,8 +453,8 @@ int candidate_tail(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* qb, 
     const int n_groups = (n_lists + group - 1) / group;
     DevBuf<uint64_t>& dst = in_a ? c->cand_b : c->cand_a;
     // rows of cand are indexed by the query position inside the block (TC pads to 128/256)
-    CU_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
-    CU_TRY(launch_reduce_lists(cur, nqb, n_lists, ksel, group, ix->d_ids.p, dst.p, s));
+    AUR_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
+    AUR_TRY(launch_reduce_lists(cur, nqb, n_lists, ksel, group, ix->d_ids.p, dst.p, s));
     c->last_launches += 1;
     cur = dst.p; n_lists = n_groups; in_a = !in_a;
   }
@@ -488,7 +469,7 @@ int candidate_tail(aur_index* ix, SearchCtx* c, cudaStream_t s, const void* qb, 
   fa.out_ids = ids ? ids + static_cast<size_t>(q0) * k : nullptr;
   fa.out_scores64 = scores64 ? scores64 + static_cast<size_t>(q0) * k : nullptr;
   if (ex) { fa.ex = *ex; fa.ex.q0 = q0; }
-  CU_TRY(launch_finalize(fa, s));
+  AUR_TRY(launch_finalize(fa, s));
   c->last_launches += 1;
   return AUR_OK;
 }
@@ -518,27 +499,27 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
     return fail(AUR_ERR_UNSUPPORTED, "tensor-core path needs bf16 rows with dim %% 64 == 0 or int8 rows with dim %% 128 == 0, dim <= %d, "
                 "no per-query tenant filter, and k small enough for its shared-memory lists at this dim", kTcMaxDim);
   c->last_kernel = kernel;
-  CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
+  AUR_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
   bool k_timed = false;
   const float* inv = nullptr;   // masked inverse norms (nullptr = the shard's own)
   if (subset && n_rows > 0) {
-    CU_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
-    CU_TRY(launch_fill_f32(c->masked_inv.p, nanf(""), n_rows, s));
-    CU_TRY(launch_scatter_inv_norm(ix->d_inv_norm.p, sc.allow_rows, sc.n_allow, n_rows, c->masked_inv.p, s));
+    AUR_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
+    AUR_TRY(launch_fill_f32(c->masked_inv.p, nanf(""), n_rows, s));
+    AUR_TRY(launch_scatter_inv_norm(ix->d_inv_norm.p, sc.allow_rows, sc.n_allow, n_rows, c->masked_inv.p, s));
     c->last_launches += 2;
     inv = c->masked_inv.p;
   } else if (sc.match_mask && n_rows > 0) {
-    CU_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
-    CU_TRY(launch_mask_match(ix->d_inv_norm.p, sc.match_mask, n_rows, c->masked_inv.p, s));
+    AUR_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
+    AUR_TRY(launch_mask_match(ix->d_inv_norm.p, sc.match_mask, n_rows, c->masked_inv.p, s));
     ++c->last_launches;
     inv = c->masked_inv.p;
   } else if (kernel != AUR_KERNEL_SIMT && scoped_tc && n_rows > 0) {              // up to 32 scopes in the batch: row bit masks
-    CU_TRY(c->row_mask.reserve(static_cast<size_t>(ix->capacity) + 64));
-    CU_TRY(launch_row_scope_mask(ix->d_user.p, ix->d_org.p, sc.scope_tab, sc.n_scopes, n_rows, c->row_mask.p, s));
+    AUR_TRY(c->row_mask.reserve(static_cast<size_t>(ix->capacity) + 64));
+    AUR_TRY(launch_row_scope_mask(ix->d_user.p, ix->d_org.p, sc.scope_tab, sc.n_scopes, n_rows, c->row_mask.p, s));
     ++c->last_launches;
   } else if (kernel != AUR_KERNEL_SIMT && sc.q_user != nullptr && sc.uniform != nullptr && n_rows > 0) {   // one scope for the whole batch
-    CU_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
-    CU_TRY(launch_mask_inv_norm(ix->d_inv_norm.p, ix->d_user.p, ix->d_org.p, sc.uniform[0], sc.uniform[1], n_rows, c->masked_inv.p, s));
+    AUR_TRY(c->masked_inv.reserve(static_cast<size_t>(ix->capacity) + 64));
+    AUR_TRY(launch_mask_inv_norm(ix->d_inv_norm.p, ix->d_user.p, ix->d_org.p, sc.uniform[0], sc.uniform[1], n_rows, c->masked_inv.p, s));
     ++c->last_launches;
     inv = c->masked_inv.p;
   }
@@ -555,37 +536,37 @@ int search_enqueue(aur_index* ix, SearchCtx* c, const void* q_dev, int nq, int k
     if (kernel == AUR_KERNEL_SIMT) {
       if (n_rows == 0) {
         n_lists = 1;
-        CU_TRY(c->cand_a.reserve(static_cast<size_t>(nqb) * ksel));
-        CU_TRY(cudaMemsetAsync(c->cand_a.p, 0, static_cast<size_t>(nqb) * ksel * 8, s));
+        AUR_TRY(c->cand_a.reserve(static_cast<size_t>(nqb) * ksel));
+        AUR_TRY(cudaMemsetAsync(c->cand_a.p, 0, static_cast<size_t>(nqb) * ksel * 8, s));
       } else {
         n_lists = static_cast<int>((n_rows + kSimtSeg - 1) / kSimtSeg);
-        CU_TRY(c->cand_a.reserve(static_cast<size_t>(nqb) * n_lists * ksel));
-        CU_TRY(c->score_chunk.reserve(static_cast<size_t>(nqb) * kSimtChunk));
+        AUR_TRY(c->cand_a.reserve(static_cast<size_t>(nqb) * n_lists * ksel));
+        AUR_TRY(c->score_chunk.reserve(static_cast<size_t>(nqb) * kSimtChunk));
         const FilterArgs f = simt_filter(ix, sc, inv, q0);
-        if (!k_timed) CU_TRY(cudaEventRecord(c->ev_k0, s));
+        if (!k_timed) AUR_TRY(cudaEventRecord(c->ev_k0, s));
         for (int64_t r0 = 0; r0 < n_rows; r0 += kSimtChunk) {
           const int64_t nr = std::min(n_rows - r0, kSimtChunk);
-          CU_TRY(launch_simt_scores(qb, ix->d_rows.p, ix->dtype, ix->dim, nqb, r0, nr, n_rows, inv ? inv : ix->d_inv_norm.p, f,
-                                    c->score_chunk.p, s));
-          CU_TRY(launch_simt_select(c->score_chunk.p, nqb, r0, nr, ksel, ix->d_ids.p, c->cand_a.p, n_lists,
-                                    static_cast<int>(r0 / kSimtSeg), s));
+          AUR_TRY(launch_simt_scores(qb, ix->d_rows.p, ix->dtype, ix->dim, nqb, r0, nr, n_rows, inv ? inv : ix->d_inv_norm.p, f,
+                                     c->score_chunk.p, s));
+          AUR_TRY(launch_simt_select(c->score_chunk.p, nqb, r0, nr, ksel, ix->d_ids.p, c->cand_a.p, n_lists,
+                                     static_cast<int>(r0 / kSimtSeg), s));
           c->last_launches += 2;
         }
-        if (!k_timed) { CU_TRY(cudaEventRecord(c->ev_k1, s)); k_timed = true; }
+        if (!k_timed) { AUR_TRY(cudaEventRecord(c->ev_k1, s)); k_timed = true; }
       }
     } else {
-      if (!k_timed) CU_TRY(cudaEventRecord(c->ev_k0, s));
+      if (!k_timed) AUR_TRY(cudaEventRecord(c->ev_k0, s));
       const bool use_mask = scoped_tc && n_rows > 0;
       int rc = run_tc_block(ix, c, kernel == AUR_KERNEL_TC1 ? 1 : 2, qb, nqb, ksel, n_rows, nullptr, &n_lists, s, inv,
                             use_mask ? c->row_mask.p : nullptr, use_mask ? sc.q_scope + q0 : nullptr);
       if (rc != AUR_OK) return rc;
-      if (!k_timed) { CU_TRY(cudaEventRecord(c->ev_k1, s)); k_timed = true; }
+      if (!k_timed) { AUR_TRY(cudaEventRecord(c->ev_k1, s)); k_timed = true; }
       c->last_launches += 1;
     }
     const int rc = candidate_tail(ix, c, s, qb, q0, nqb, k, n_lists, kernel != AUR_KERNEL_SIMT, scores, ids, scores64, ex);
     if (rc != AUR_OK) return rc;
   }
-  if (!k_timed) { CU_TRY(cudaEventRecord(c->ev_k0, s)); CU_TRY(cudaEventRecord(c->ev_k1, s)); }
+  if (!k_timed) { AUR_TRY(cudaEventRecord(c->ev_k0, s)); AUR_TRY(cudaEventRecord(c->ev_k1, s)); }
   return AUR_OK;
 }
 
@@ -607,29 +588,29 @@ int add_common(aur_index* ix, const void* rows, bool rows_on_device, const int64
     // through a bounded device staging buffer, a slice at a time (stream order keeps the slices apart).
     const int64_t slice = rows_on_device ? n : std::min<int64_t>(n, 65536);
     const size_t in_row = static_cast<size_t>(ix->dim) * 2;
-    if (!rows_on_device) CU_TRY(ix->i8_stage.reserve(static_cast<size_t>(slice) * in_row));
+    if (!rows_on_device) AUR_TRY(ix->i8_stage.reserve(static_cast<size_t>(slice) * in_row));
     for (int64_t r0 = 0; r0 < n; r0 += slice) {
       const int64_t m = std::min(slice, n - r0);
       const uint8_t* src = static_cast<const uint8_t*>(rows) + static_cast<size_t>(r0) * in_row;
       if (!rows_on_device) {
-        CU_TRY(cudaMemcpyAsync(ix->i8_stage.p, src, static_cast<size_t>(m) * in_row, cudaMemcpyHostToDevice, s));
+        AUR_TRY(cudaMemcpyAsync(ix->i8_stage.p, src, static_cast<size_t>(m) * in_row, cudaMemcpyHostToDevice, s));
         src = ix->i8_stage.p;
       }
-      CU_TRY(launch_quantize_rows_i8(reinterpret_cast<const __nv_bfloat16*>(src), ix->dim, m,
-                                     reinterpret_cast<int8_t*>(dst) + static_cast<size_t>(r0) * ix->dim, ix->d_inv_norm.p + base + r0, s));
+      AUR_TRY(launch_quantize_rows_i8(reinterpret_cast<const __nv_bfloat16*>(src), ix->dim, m,
+                                      reinterpret_cast<int8_t*>(dst) + static_cast<size_t>(r0) * ix->dim, ix->d_inv_norm.p + base + r0, s));
     }
   } else {
-    CU_TRY(cudaMemcpyAsync(dst, rows, static_cast<size_t>(n) * ix->dim * ix->elt,
-                           rows_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
+    AUR_TRY(cudaMemcpyAsync(dst, rows, static_cast<size_t>(n) * ix->dim * ix->elt,
+                            rows_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, s));
   }
-  CU_TRY(cudaMemcpyAsync(ix->d_ids.p + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(ix->d_ids.p + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
   std::vector<int32_t> fill;
   if (!users) { fill.assign(static_cast<size_t>(n), 0); users = fill.data(); }
-  CU_TRY(cudaMemcpyAsync(ix->d_user.p + base, users, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(ix->d_user.p + base, users, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
   std::vector<int32_t> fill2;
   if (!orgs) { fill2.assign(static_cast<size_t>(n), -1); orgs = fill2.data(); }
-  CU_TRY(cudaMemcpyAsync(ix->d_org.p + base, orgs, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  if (ix->dtype != AUR_I8) CU_TRY(launch_row_inv_norms(dst, ix->dtype, ix->dim, n, ix->d_inv_norm.p + base, s));
+  AUR_TRY(cudaMemcpyAsync(ix->d_org.p + base, orgs, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  if (ix->dtype != AUR_I8) AUR_TRY(launch_row_inv_norms(dst, ix->dtype, ix->dim, n, ix->d_inv_norm.p + base, s));
   // upsert: an id that already exists loses its old row (weaviate_client.py:172 uuid5 semantics).  The old rows
   // are tombstoned before the new ones are published: a racing search may briefly miss the object, never see it twice.
   std::vector<int64_t> dead;
@@ -642,8 +623,8 @@ int add_common(aur_index* ix, const void* rows, bool rows_on_device, const int64
     }
   }
   const float nanv = nanf("");
-  for (int64_t row : dead) CU_TRY(cudaMemcpyAsync(ix->d_inv_norm.p + row, &nanv, 4, cudaMemcpyHostToDevice, s));
-  CU_TRY(cudaStreamSynchronize(s));  // the data has landed (and the host staging vectors may go out of scope)
+  for (int64_t row : dead) AUR_TRY(cudaMemcpyAsync(ix->d_inv_norm.p + row, &nanv, 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaStreamSynchronize(s));  // the data has landed (and the host staging vectors may go out of scope)
   ix->rows_pub.store(base + n, std::memory_order_release);
   return AUR_OK;
 }
@@ -668,12 +649,12 @@ int check_batch(int32_t nq, int32_t k) {
 // gives every corpus row a bit mask (one pre-pass) on the same kernel; more scopes -> the generic kernel.
 int stage_tenant_scope(SearchCtx* c, cudaStream_t s, int32_t nq, const int32_t* q_user, const int32_t* q_org, int32_t* scope,
                        Scope* sc) {
-  CU_TRY(c->stage_quser.reserve(nq));
-  CU_TRY(cudaMemcpyAsync(c->stage_quser.p, q_user, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(c->stage_quser.reserve(nq));
+  AUR_TRY(cudaMemcpyAsync(c->stage_quser.p, q_user, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
   sc->q_user = c->stage_quser.p;
   if (q_org) {
-    CU_TRY(c->stage_qorg.reserve(nq));
-    CU_TRY(cudaMemcpyAsync(c->stage_qorg.p, q_org, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
+    AUR_TRY(c->stage_qorg.reserve(nq));
+    AUR_TRY(cudaMemcpyAsync(c->stage_qorg.p, q_org, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
     sc->q_org = c->stage_qorg.p;
   }
   bool uniform = true;
@@ -691,10 +672,10 @@ int stage_tenant_scope(SearchCtx* c, cudaStream_t s, int32_t nq, const int32_t* 
     }
     qs[static_cast<size_t>(i)] = found;
   }
-  CU_TRY(c->scope_tab.reserve(64)); CU_TRY(c->q_scope.reserve(static_cast<size_t>(nq)));
-  CU_TRY(cudaMemcpyAsync(c->scope_tab.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, s));
-  CU_TRY(cudaMemcpyAsync(c->q_scope.p, qs.data(), static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
-  CU_TRY(cudaStreamSynchronize(s));          // tab / qs are host temporaries
+  AUR_TRY(c->scope_tab.reserve(64)); AUR_TRY(c->q_scope.reserve(static_cast<size_t>(nq)));
+  AUR_TRY(cudaMemcpyAsync(c->scope_tab.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(c->q_scope.p, qs.data(), static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaStreamSynchronize(s));          // tab / qs are host temporaries
   sc->scope_tab = c->scope_tab.p; sc->q_scope = c->q_scope.p; sc->n_scopes = static_cast<int>(tab.size() / 2);
   return AUR_OK;
 }
@@ -817,22 +798,22 @@ ListParams list_params(const aur_index* ix, const SearchCtx* c, const ListPlan::
 int run_list_search(aur_index* ix, SearchCtx* c, cudaStream_t s, const ListPlan& pl, int32_t nq, int32_t k,
                     const int32_t* list_rows, float* d_scores, int64_t* d_ids) {
   const int ksel = k + kSlack;
-  CU_TRY(c->list_stage.reserve(pl.stage.size()));
-  CU_TRY(c->list_scores.reserve(std::max<size_t>(pl.max_slots, 1) * kSimtSeg));
-  CU_TRY(c->cand_a.reserve(pl.max_cand));
-  CU_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
+  AUR_TRY(c->list_stage.reserve(pl.stage.size()));
+  AUR_TRY(c->list_scores.reserve(std::max<size_t>(pl.max_slots, 1) * kSimtSeg));
+  AUR_TRY(c->cand_a.reserve(pl.max_cand));
+  AUR_TRY(c->cand_read.reserve(static_cast<size_t>(nq)));
   c->last_kernel = AUR_KERNEL_LIST;
-  CU_TRY(cudaMemcpyAsync(c->list_stage.p, pl.stage.data(), pl.stage.size() * 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(c->list_stage.p, pl.stage.data(), pl.stage.size() * 4, cudaMemcpyHostToDevice, s));
   for (size_t bi = 0; bi < pl.blocks.size(); ++bi) {
     const ListPlan::Block& b = pl.blocks[bi];
     const uint8_t* qb = c->stage_q.p + static_cast<size_t>(b.q0) * ix->dim * 2;
-    CU_TRY(cudaMemsetAsync(c->cand_a.p, 0, static_cast<size_t>(b.nqb) * b.n_segs * ksel * 8, s));   // 0 = empty slot
-    if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k0, s));
+    AUR_TRY(cudaMemsetAsync(c->cand_a.p, 0, static_cast<size_t>(b.nqb) * b.n_segs * ksel * 8, s));   // 0 = empty slot
+    if (bi == 0) AUR_TRY(cudaEventRecord(c->ev_k0, s));
     for (const ListPlan::Launch& ln : b.launches) {
-      CU_TRY(launch_list_search(list_params(ix, c, b, ln, list_rows, ksel), ln.max_nq, s));
+      AUR_TRY(launch_list_search(list_params(ix, c, b, ln, list_rows, ksel), ln.max_nq, s));
       c->last_launches += 2;
     }
-    if (bi == 0) CU_TRY(cudaEventRecord(c->ev_k1, s));
+    if (bi == 0) AUR_TRY(cudaEventRecord(c->ev_k1, s));
     const int rc = candidate_tail(ix, c, s, qb, b.q0, b.nqb, k, b.n_segs, false, d_scores, d_ids, nullptr, nullptr);
     if (rc != AUR_OK) return rc;
   }
@@ -856,19 +837,19 @@ FiltPass filt_pass(SearchCtx* c, int ps, int n_programs, int64_t n_rows) {
 int filter_count(aur_index* ix, SearchCtx* c, cudaStream_t s, const FiltProgs& fp, int64_t n_rows) {
   const int n_passes = filter_passes(fp.n_programs);
   const size_t nb = static_cast<size_t>(std::max(filter_blocks(n_rows), 1));
-  CU_TRY(c->h_totals.reserve(kFiltCallPrograms, cudaHostAllocPortable));
-  CU_TRY(c->filt_mask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
-  CU_TRY(c->filt_counts.reserve(static_cast<size_t>(n_passes) * kFiltMaxPrograms * (1 + nb)));
+  AUR_TRY(c->h_totals.reserve(kFiltCallPrograms, cudaHostAllocPortable));
+  AUR_TRY(c->filt_mask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
+  AUR_TRY(c->filt_counts.reserve(static_cast<size_t>(n_passes) * kFiltMaxPrograms * (1 + nb)));
   FiltParams p;
-  CU_TRY(filter_upload(fp, ix->d_user.p, ix->d_org.p, ix->attrs, c->filt_stage, s, &p));
+  AUR_TRY(filter_upload(fp, ix->d_user.p, ix->d_org.p, ix->attrs, c->filt_stage, s, &p));
   p.inv_norm = ix->d_inv_norm.p; p.n_rows = n_rows;
   for (int ps = 0; ps < n_passes; ++ps) {
     const FiltPass pass = filt_pass(c, ps, fp.n_programs, n_rows);
-    CU_TRY(launch_filter_count(filter_pass(p, ps), pass.mask, pass.counts, pass.totals, s));
+    AUR_TRY(launch_filter_count(filter_pass(p, ps), pass.mask, pass.counts, pass.totals, s));
     ++c->last_launches;
   }
-  CU_TRY(cudaMemcpyAsync(c->h_totals.p, c->filt_counts.p, static_cast<size_t>(n_passes) * kFiltMaxPrograms * 4,
-                         cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaMemcpyAsync(c->h_totals.p, c->filt_counts.p, static_cast<size_t>(n_passes) * kFiltMaxPrograms * 4,
+                          cudaMemcpyDeviceToHost, s));
   return AUR_OK;
 }
 
@@ -885,13 +866,13 @@ int filter_write(aur_index* ix, SearchCtx* c, cudaStream_t s, int32_t n_programs
   int64_t total = 0;
   for (int64_t t : tot) total += t;
   if (total > INT32_MAX) return fail(AUR_ERR_UNSUPPORTED, "the programs of this call match too many rows for one call: split it");
-  CU_TRY(c->filt_rows.reserve(static_cast<size_t>(std::max<int64_t>(total, 1))));
-  if (with_ids) CU_TRY(c->filt_ids.reserve(static_cast<size_t>(std::max<int64_t>(total, 1))));
+  AUR_TRY(c->filt_rows.reserve(static_cast<size_t>(std::max<int64_t>(total, 1))));
+  if (with_ids) AUR_TRY(c->filt_ids.reserve(static_cast<size_t>(std::max<int64_t>(total, 1))));
   int64_t base = 0;
   for (int ps = 0; ps < filter_passes(n_programs); ++ps) {
     const FiltPass fp = filt_pass(c, ps, n_programs, n_rows);
-    CU_TRY(launch_filter_write(fp.mask, fp.counts, fp.totals, fp.n_programs, n_rows, with_ids ? ix->d_ids.p : nullptr,
-                               c->filt_rows.p + base, with_ids ? c->filt_ids.p + base : nullptr, s));
+    AUR_TRY(launch_filter_write(fp.mask, fp.counts, fp.totals, fp.n_programs, n_rows, with_ids ? ix->d_ids.p : nullptr,
+                                c->filt_rows.p + base, with_ids ? c->filt_ids.p + base : nullptr, s));
     if (n_rows > 0) c->last_launches += 2;
     for (int q = 0; q < fp.n_programs; ++q) base += tot[static_cast<size_t>(ps * kFiltMaxPrograms + q)];
   }
@@ -939,9 +920,9 @@ int prepare_scope(const DenseQuery& q, DensePart* pt) {
     // resolved metadata pre-filter: ids -> rows of the published prefix (unknown / newer ids drop out)
     pt->allow.reserve(static_cast<size_t>(q.n_allow));
     resolve_ids(call.ix, q.allow_ids, q.n_allow, call.n_rows, [&](int64_t, int32_t row) { pt->allow.push_back(row); });
-    CU_TRY(c->allow_rows.reserve(pt->allow.size() + 1));
+    AUR_TRY(c->allow_rows.reserve(pt->allow.size() + 1));
     if (!pt->allow.empty())
-      CU_TRY(cudaMemcpyAsync(c->allow_rows.p, pt->allow.data(), pt->allow.size() * 4, cudaMemcpyHostToDevice, call.s));
+      AUR_TRY(cudaMemcpyAsync(c->allow_rows.p, pt->allow.data(), pt->allow.size() * 4, cudaMemcpyHostToDevice, call.s));
     pt->sc.allow_rows = c->allow_rows.p;
     pt->sc.n_allow = static_cast<int64_t>(pt->allow.size());
     return AUR_OK;
@@ -979,15 +960,6 @@ AttrColumns& index_attrs(aur_index* ix) { return ix->attrs; }
 int dense_legs(aur_index* const* shards, int n, const DenseQuery& q, const DenseLegsThen& then, float* scores_host,
                int64_t* ids_host) {
   std::vector<DensePart> parts(static_cast<size_t>(n));
-  // every stream drains before its context goes back to the pool (also on an error): declared after `parts`, so it
-  // runs before their destructors
-  struct Drain {
-    std::vector<DensePart>& v;
-    ~Drain() {
-      for (DensePart& p : v)
-        if (p.call && p.call->c) { cudaSetDevice(p.call->ix->device); cudaStreamSynchronize(p.call->s); }
-    }
-  } drain{parts};
   // shared locks in one order (by address), as the keyword legs take theirs
   std::vector<int> order(static_cast<size_t>(n));
   for (int s = 0; s < n; ++s) order[static_cast<size_t>(s)] = s;
@@ -1005,14 +977,14 @@ int dense_legs(aur_index* const* shards, int n, const DenseQuery& q, const Dense
   }
   if (q.fp)
     for (DensePart& pt : parts) {
-      CU_TRY(cudaSetDevice(pt.call->ix->device));
-      CU_TRY(cudaStreamSynchronize(pt.call->s));
+      AUR_TRY(cudaSetDevice(pt.call->ix->device));
+      AUR_TRY(cudaStreamSynchronize(pt.call->s));
       filter_totals(pt.call->c, q.fp->n_programs, &pt.tot);
     }
   std::vector<DenseLeg> legs;
   for (DensePart& pt : parts) {
     HostCall& call = *pt.call;
-    CU_TRY(cudaSetDevice(call.ix->device));
+    AUR_TRY(cudaSetDevice(call.ix->device));
     if (q.fp)
       rc = filtered_search(call.ix, call.c, call.s, q.nq, q.k, *q.fp, pt.tot, q.max_list_rows, call.n_rows, call.d_scores, call.d_ids);
     else if (q.q_list)
@@ -1036,10 +1008,10 @@ int search_into_host(aur_index* ix, const DenseQuery& q, float* scores_out, int6
     const DenseLeg& l = legs[0];
     if (!l.direct) {   // into the caller's pageable buffers
       const size_t nout = static_cast<size_t>(q.nq) * q.k;
-      CU_TRY(cudaMemcpyAsync(scores_out, l.scores, nout * 4, cudaMemcpyDeviceToHost, l.stream));
-      CU_TRY(cudaMemcpyAsync(ids_out, l.ids, nout * 8, cudaMemcpyDeviceToHost, l.stream));
+      AUR_TRY(cudaMemcpyAsync(scores_out, l.scores, nout * 4, cudaMemcpyDeviceToHost, l.stream));
+      AUR_TRY(cudaMemcpyAsync(ids_out, l.ids, nout * 8, cudaMemcpyDeviceToHost, l.stream));
     }
-    CU_TRY(cudaStreamSynchronize(l.stream));
+    AUR_TRY(cudaStreamSynchronize(l.stream));
     if (matched_out) std::copy(l.matched->begin(), l.matched->end(), matched_out);
     if (snapshot_rows_out) *snapshot_rows_out = l.snapshot_rows;
     return AUR_OK;
@@ -1070,9 +1042,9 @@ int aur_open(const aur_config* cfg, aur_index** out) {
   int ndev = aur_device_count();
   if (ndev == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device: aurora_b200 has no CPU fallback");
   if (cfg->device < 0 || cfg->device >= ndev) return fail(AUR_ERR_INVALID, "device %d out of range", cfg->device);
-  CU_TRY(cudaSetDevice(cfg->device));
+  AUR_TRY(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
-  CU_TRY(cudaGetDeviceProperties(&prop, cfg->device));
+  AUR_TRY(cudaGetDeviceProperties(&prop, cfg->device));
   if (prop.major != 9) return fail(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
   std::unique_ptr<aur_index> ix(new aur_index());
   ix->device = cfg->device; ix->dim = cfg->dim; ix->dtype = cfg->dtype; ix->capacity = cfg->capacity;
@@ -1080,21 +1052,18 @@ int aur_open(const aur_config* cfg, aur_index** out) {
   ix->qelt = cfg->dtype == AUR_F32 ? 4 : 2;
   ix->sm_count = prop.multiProcessorCount;
   ix->smem_optin = prop.sharedMemPerBlockOptin;
-#define OPEN_TRY(expr)                                                                                  \
-  do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return fail(e_ == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, \
-                                                              "%s: %s", #expr, cudaGetErrorString(e_)); } while (0)
+  ix->ctxs.device = cfg->device;
   int prio_lo = 0, prio_hi = 0;
-  OPEN_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-  OPEN_TRY(ix->stream.create(cudaStreamNonBlocking, prio_hi));
-  OPEN_TRY(ix->ingest_stream.create(cudaStreamNonBlocking, prio_lo));
+  AUR_TRY(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
+  AUR_TRY(ix->stream.create(cudaStreamNonBlocking, prio_hi));
+  AUR_TRY(ix->ingest_stream.create(cudaStreamNonBlocking, prio_lo));
   ix->cap_pad = (cfg->capacity + kTcTileN - 1) / kTcTileN * kTcTileN;
   const size_t cap_pad = static_cast<size_t>(ix->cap_pad);
-  OPEN_TRY(ix->d_rows.reserve(cap_pad * ix->dim * ix->elt));
-  OPEN_TRY(ix->d_inv_norm.reserve(cap_pad));
-  OPEN_TRY(ix->d_ids.reserve(cap_pad));
-  OPEN_TRY(ix->d_user.reserve(cap_pad));
-  OPEN_TRY(ix->d_org.reserve(cap_pad));
-#undef OPEN_TRY
+  AUR_TRY(ix->d_rows.reserve(cap_pad * ix->dim * ix->elt));
+  AUR_TRY(ix->d_inv_norm.reserve(cap_pad));
+  AUR_TRY(ix->d_ids.reserve(cap_pad));
+  AUR_TRY(ix->d_user.reserve(cap_pad));
+  AUR_TRY(ix->d_org.reserve(cap_pad));
   int rc = build_tmaps(ix.get());
   if (rc != AUR_OK) return rc;
   *out = ix.release();
@@ -1123,14 +1092,14 @@ int aur_get_stats(aur_index* ix, aur_stats* out) {
     std::lock_guard<std::mutex> cl(c->mu);
     out->last_kernel = c->last_kernel; out->last_launches = c->last_launches; out->last_tile_n = c->last_tile_n;
     if (c->have_timing) {
-      CU_TRY(cudaSetDevice(ix->device));
-      CU_TRY(cudaEventSynchronize(c->ev_end));
-      CU_TRY(cudaEventElapsedTime(&out->last_kernel_ms, c->ev_k0, c->ev_k1));
-      CU_TRY(cudaEventElapsedTime(&out->last_total_ms, c->ev_begin, c->ev_end));
-      CU_TRY(cudaEventElapsedTime(&out->last_finalize_ms, c->ev_k1, c->ev_fin));
-      CU_TRY(cudaEventElapsedTime(&out->last_merge_ms, c->ev_fin, c->ev_end));
+      AUR_TRY(cudaSetDevice(ix->device));
+      AUR_TRY(cudaEventSynchronize(c->ev_end));
+      AUR_TRY(cudaEventElapsedTime(&out->last_kernel_ms, c->ev_k0, c->ev_k1));
+      AUR_TRY(cudaEventElapsedTime(&out->last_total_ms, c->ev_begin, c->ev_end));
+      AUR_TRY(cudaEventElapsedTime(&out->last_finalize_ms, c->ev_k1, c->ev_fin));
+      AUR_TRY(cudaEventElapsedTime(&out->last_merge_ms, c->ev_fin, c->ev_end));
       std::vector<uint32_t> n(std::min(static_cast<size_t>(c->last_nq), c->cand_read.n));
-      CU_TRY(cudaMemcpy(n.data(), c->cand_read.p, n.size() * 4, cudaMemcpyDeviceToHost));
+      AUR_TRY(cudaMemcpy(n.data(), c->cand_read.p, n.size() * 4, cudaMemcpyDeviceToHost));
       for (uint32_t v : n) {
         out->last_candidates += v;
         out->last_candidates_max = std::max(out->last_candidates_max, static_cast<int32_t>(v));
@@ -1147,14 +1116,14 @@ int aur_export(aur_index* ix, void* rows_out, int64_t* ids_out, int32_t* user_ou
   const int64_t rows = ix->rows_pub.load(std::memory_order_acquire);
   if (n != rows) return fail(AUR_ERR_INVALID, "n must equal aur_stats.rows (%lld)", (long long)rows);
   if (n == 0) return AUR_OK;
-  CU_TRY(cudaSetDevice(ix->device));
-  CU_TRY(cudaDeviceSynchronize());
+  AUR_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaDeviceSynchronize());
   std::vector<float> inv(static_cast<size_t>(n));
-  CU_TRY(cudaMemcpy(inv.data(), ix->d_inv_norm.p, sizeof(float) * n, cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(rows_out, ix->d_rows.p, static_cast<size_t>(n) * ix->dim * ix->elt, cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(ids_out, ix->d_ids.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
-  if (user_out) CU_TRY(cudaMemcpy(user_out, ix->d_user.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
-  if (org_out) CU_TRY(cudaMemcpy(org_out, ix->d_org.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaMemcpy(inv.data(), ix->d_inv_norm.p, sizeof(float) * n, cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaMemcpy(rows_out, ix->d_rows.p, static_cast<size_t>(n) * ix->dim * ix->elt, cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaMemcpy(ids_out, ix->d_ids.p, sizeof(int64_t) * n, cudaMemcpyDeviceToHost));
+  if (user_out) AUR_TRY(cudaMemcpy(user_out, ix->d_user.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
+  if (org_out) AUR_TRY(cudaMemcpy(org_out, ix->d_org.p, sizeof(int32_t) * n, cudaMemcpyDeviceToHost));
   // NaN = tombstone; an int8 row stored from a row with a NaN / inf (scale +inf, never returned) is live, reported as 2
   for (int64_t i = 0; i < n; ++i) {
     const float v = inv[static_cast<size_t>(i)];
@@ -1170,11 +1139,11 @@ int aur_read_rows(aur_index* ix, int64_t row0, int64_t n, void* rows_out, int64_
   if (row0 < 0 || n < 0 || row0 + n > rows) return fail(AUR_ERR_INVALID, "rows [%lld, %lld) are not inside the published prefix of %lld",
                                                         (long long)row0, (long long)(row0 + n), (long long)rows);
   if (n == 0) return AUR_OK;
-  CU_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaSetDevice(ix->device));
   const size_t rb = static_cast<size_t>(ix->dim) * ix->elt;
-  CU_TRY(cudaMemcpy(rows_out, static_cast<const uint8_t*>(ix->d_rows.p) + static_cast<size_t>(row0) * rb, static_cast<size_t>(n) * rb,
-                    cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(ids_out, ix->d_ids.p + row0, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaMemcpy(rows_out, static_cast<const uint8_t*>(ix->d_rows.p) + static_cast<size_t>(row0) * rb, static_cast<size_t>(n) * rb,
+                     cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaMemcpy(ids_out, ix->d_ids.p + row0, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost));
   return AUR_OK;
 }
 
@@ -1183,8 +1152,8 @@ int aur_compact(aur_index* ix, int64_t* reclaimed) {
   if (reclaimed) *reclaimed = 0;
   std::unique_lock<std::shared_mutex> wl(ix->rw);   // no search or append is being enqueued ...
   std::lock_guard<std::mutex> wk(ix->mu_write);
-  CU_TRY(cudaSetDevice(ix->device));
-  CU_TRY(cudaDeviceSynchronize());                  // ... and none is still running
+  AUR_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaDeviceSynchronize());                  // ... and none is still running
   const int64_t rows = ix->rows_pub.load(std::memory_order_acquire);
   std::vector<std::pair<int64_t, int64_t>> order;   // (old row, id) of the live rows, in row order
   {
@@ -1252,15 +1221,16 @@ int aur_set_option(aur_index* ix, const char* key, int64_t value) {
     {
       std::lock_guard<std::mutex> lk(ix->mu);
       ix->opt_dbg_epoch.store(static_cast<uint32_t>(value));   // contexts that start their counter later
-      for (auto& c : ix->ctxs) cs.push_back(c.get());
+      cs = ix->ctxs.contexts();
+      for (auto& b : ix->bound) cs.push_back(b.second.get());
     }
-    CU_TRY(cudaSetDevice(ix->device));
+    AUR_TRY(cudaSetDevice(ix->device));
     const uint32_t e = static_cast<uint32_t>(value);
     for (SearchCtx* c : cs) {
       std::lock_guard<std::mutex> cl(c->mu);
       if (c->d_epoch.n == 0) continue;
-      CU_TRY(cudaDeviceSynchronize());   // searches already enqueued on the context finish with their own counter
-      CU_TRY(cudaMemcpy(c->d_epoch.p, &e, 4, cudaMemcpyHostToDevice));
+      AUR_TRY(cudaDeviceSynchronize());   // searches already enqueued on the context finish with their own counter
+      AUR_TRY(cudaMemcpy(c->d_epoch.p, &e, 4, cudaMemcpyHostToDevice));
     }
     return AUR_OK;
   }
@@ -1292,8 +1262,8 @@ int aur_set_option(aur_index* ix, const char* key, int64_t value) {
 
 int aur_sync(aur_index* ix) {
   if (!ix) return fail(AUR_ERR_INVALID, "null argument");
-  CU_TRY(cudaSetDevice(ix->device));
-  CU_TRY(cudaStreamSynchronize(ix->stream));
+  AUR_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaStreamSynchronize(ix->stream));
   return AUR_OK;
 }
 
@@ -1302,7 +1272,7 @@ int aur_add(aur_index* ix, const void* rows_host, const int64_t* ids, const int3
   if (!ix) return fail(AUR_ERR_INVALID, "null index");
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   std::lock_guard<std::mutex> wk(ix->mu_write);
-  CU_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaSetDevice(ix->device));
   return add_common(ix, rows_host, false, ids, user_codes, org_codes, n, ix->ingest_stream);
 }
 
@@ -1311,7 +1281,7 @@ int aur_add_dev(aur_index* ix, const void* rows_dev, const int64_t* ids_host, co
   if (!ix) return fail(AUR_ERR_INVALID, "null index");
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   std::lock_guard<std::mutex> wk(ix->mu_write);
-  CU_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaSetDevice(ix->device));
   return add_common(ix, rows_dev, true, ids_host, user_codes_host, org_codes_host, n,
                     stream ? static_cast<cudaStream_t>(stream) : ix->ingest_stream);
 }
@@ -1320,10 +1290,10 @@ int aur_remove(aur_index* ix, const int64_t* ids, int64_t n, int64_t* removed) {
   if (!ix || (n > 0 && !ids)) return fail(AUR_ERR_INVALID, "null argument");
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   std::lock_guard<std::mutex> wk(ix->mu_write);
-  CU_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaSetDevice(ix->device));
   if (removed) *removed = 0;
   if (n <= 0) return AUR_OK;
-  CU_TRY(ix->tomb_rows.reserve(static_cast<size_t>(n)));   // before id2row changes: a failure here removes nothing
+  AUR_TRY(ix->tomb_rows.reserve(static_cast<size_t>(n)));   // before id2row changes: a failure here removes nothing
   std::vector<int32_t> dead;
   {
     std::lock_guard<std::mutex> lk(ix->mu);
@@ -1338,9 +1308,9 @@ int aur_remove(aur_index* ix, const int64_t* ids, int64_t n, int64_t* removed) {
   const int64_t m = static_cast<int64_t>(dead.size());
   cudaStream_t s = ix->ingest_stream;
   if (m) {
-    CU_TRY(cudaMemcpyAsync(ix->tomb_rows.p, dead.data(), static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, s));
-    CU_TRY(launch_tombstone_rows(ix->tomb_rows.p, m, ix->d_inv_norm.p, s));
-    CU_TRY(cudaStreamSynchronize(s));   // dead is pageable host memory and goes out of scope
+    AUR_TRY(cudaMemcpyAsync(ix->tomb_rows.p, dead.data(), static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, s));
+    AUR_TRY(launch_tombstone_rows(ix->tomb_rows.p, m, ix->d_inv_norm.p, s));
+    AUR_TRY(cudaStreamSynchronize(s));   // dead is pageable host memory and goes out of scope
   }
   if (removed) *removed = m;
   return AUR_OK;
@@ -1352,10 +1322,10 @@ int aur_search_dev(aur_index* ix, const void* queries_dev, int32_t nq, int32_t k
   if (rc != AUR_OK) return rc;
   if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
   std::shared_lock<std::shared_mutex> rl(ix->rw);
-  CU_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaSetDevice(ix->device));
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
   SearchCtx* c = nullptr;
-  if ((rc = acquire_ctx(ix, s, &c)) != AUR_OK) return rc;
+  if ((rc = bound_ctx(ix, s, &c)) != AUR_OK) return rc;
   std::lock_guard<std::mutex> cl(c->mu);
   const int64_t n_rows = ix->rows_pub.load(std::memory_order_acquire);
   Scope sc;
@@ -1407,7 +1377,7 @@ int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t*
   if (!ix || n < 0 || (n > 0 && (!ids || !codes))) return fail(AUR_ERR_INVALID, "null argument");
   std::shared_lock<std::shared_mutex> rl(ix->rw);
   std::lock_guard<std::mutex> wk(ix->mu_write);
-  CU_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaSetDevice(ix->device));
   std::vector<int32_t> pairs;
   pairs.reserve(2 * static_cast<size_t>(n));
   resolve_ids(ix, ids, n, INT64_MAX, [&](int64_t i, int32_t row) { pairs.push_back(row); pairs.push_back(codes[i]); });
@@ -1443,13 +1413,13 @@ int aur_filter_ids(aur_index* ix, const int32_t* prog, int32_t n_tokens, const u
   cudaStream_t s = call.s;
   std::vector<int64_t> tot;
   if ((rc = filter_count(ix, c, s, fp, call.n_rows)) != AUR_OK) return rc;
-  CU_TRY(cudaStreamSynchronize(s));
+  AUR_TRY(cudaStreamSynchronize(s));
   filter_totals(c, 1, &tot);
   const int64_t n = tot[0], m = std::min(n, cap);
   if ((rc = filter_write(ix, c, s, 1, tot, call.n_rows, true)) != AUR_OK) return rc;
   std::vector<int64_t> got(static_cast<size_t>(m));
-  if (m) CU_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToHost, s));
-  CU_TRY(cudaStreamSynchronize(s));
+  if (m) AUR_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaStreamSynchronize(s));
   if (m) memcpy(ids_out, got.data(), static_cast<size_t>(m) * 8);
   *n_out = n;
   return AUR_OK;
@@ -1466,7 +1436,7 @@ int aur_filter_count(aur_index* ix, const int32_t* prog, int32_t n_tokens, const
   HostCall call(ix);
   if ((rc = call.open()) != AUR_OK) return rc;
   if ((rc = filter_count(ix, call.c, call.s, fp, call.n_rows)) != AUR_OK) return rc;
-  CU_TRY(cudaStreamSynchronize(call.s));
+  AUR_TRY(cudaStreamSynchronize(call.s));
   std::vector<int64_t> tot;
   filter_totals(call.c, 1, &tot);
   *n_out = tot[0];
@@ -1489,7 +1459,7 @@ int aur_remove_filtered(aur_index* ix, const int32_t* prog, int32_t n_tokens, co
   SearchCtx* c = call.c;
   cudaStream_t s = call.s;
   if ((rc = filter_count(ix, c, s, fp, call.n_rows)) != AUR_OK) return rc;
-  CU_TRY(cudaStreamSynchronize(s));
+  AUR_TRY(cudaStreamSynchronize(s));
   std::vector<int64_t> tot;
   filter_totals(c, 1, &tot);
   const int64_t n = tot[0];
@@ -1498,10 +1468,10 @@ int aur_remove_filtered(aur_index* ix, const int32_t* prog, int32_t n_tokens, co
     return AUR_OK;
   }
   if ((rc = filter_write(ix, c, s, 1, tot, call.n_rows, true)) != AUR_OK) return rc;
-  CU_TRY(launch_tombstone_rows(c->filt_rows.p, n, ix->d_inv_norm.p, s));
+  AUR_TRY(launch_tombstone_rows(c->filt_rows.p, n, ix->d_inv_norm.p, s));
   std::vector<int64_t> got(static_cast<size_t>(n));
-  CU_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost, s));
-  CU_TRY(cudaStreamSynchronize(s));
+  AUR_TRY(cudaMemcpyAsync(got.data(), c->filt_ids.p, static_cast<size_t>(n) * 8, cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaStreamSynchronize(s));
   {
     std::lock_guard<std::mutex> lk(ix->mu);
     for (int64_t id : got) ix->live -= static_cast<int64_t>(ix->id2row.erase(id));
@@ -1532,9 +1502,9 @@ int aur_merge_topk_dev(int32_t device, const double* in_scores64, const int64_t*
   if (!in_scores64 || !in_ids || !out_scores || !out_ids) return fail(AUR_ERR_INVALID, "null argument");
   if (n_shards <= 0 || nq <= 0 || k <= 0 || k > kMaxK || n_shards * k > 2048) return fail(AUR_ERR_INVALID, "bad merge shape");
   if (aur_device_count() == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device");
-  CU_TRY(cudaSetDevice(device));
-  CU_TRY(launch_merge_topk(in_scores64, in_ids, static_cast<size_t>(nq) * k, n_shards, nq, k, out_scores, out_ids,
-                           out_scores64, static_cast<cudaStream_t>(stream)));
+  AUR_TRY(cudaSetDevice(device));
+  AUR_TRY(launch_merge_topk(in_scores64, in_ids, static_cast<size_t>(nq) * k, n_shards, nq, k, out_scores, out_ids,
+                            out_scores64, static_cast<cudaStream_t>(stream)));
   return AUR_OK;
 }
 
@@ -1543,12 +1513,12 @@ int aur_merge_topk_packed_dev(int32_t device, const void* packed, int32_t n_shar
   if (!packed || !out_scores || !out_ids) return fail(AUR_ERR_INVALID, "null argument");
   if (n_shards <= 0 || nq <= 0 || k <= 0 || k > kMaxK || n_shards * k > 2048) return fail(AUR_ERR_INVALID, "bad merge shape");
   if (aur_device_count() == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device");
-  CU_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaSetDevice(device));
   const size_t plane = static_cast<size_t>(nq) * k;
   const double* s64 = static_cast<const double*>(packed);
   const int64_t* ids = static_cast<const int64_t*>(packed) + plane;
-  CU_TRY(launch_merge_topk(s64, ids, 2 * plane, n_shards, nq, k, out_scores, out_ids, out_scores64,
-                           static_cast<cudaStream_t>(stream)));
+  AUR_TRY(launch_merge_topk(s64, ids, 2 * plane, n_shards, nq, k, out_scores, out_ids, out_scores64,
+                            static_cast<cudaStream_t>(stream)));
   return AUR_OK;
 }
 
@@ -1560,7 +1530,7 @@ int aur_exchange_create(int32_t device, int32_t rank, int32_t world, int32_t nq_
   if (nq_max <= 0 || k_max <= 0 || k_max > kMaxK || world * k_max > 2048) return fail(AUR_ERR_INVALID, "bad nq_max / k_max");
   if (aur_device_count() == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device");
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
-  CU_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaSetDevice(device));
   std::unique_ptr<aur_exchange> ex(new aur_exchange());
   ex->device = device; ex->rank = rank; ex->world = world; ex->nq_max = nq_max; ex->k_max = k_max;
   ex->entries = static_cast<size_t>(nq_max) * k_max;
@@ -1588,7 +1558,7 @@ int aur_exchange_create(int32_t device, int32_t rank, int32_t world, int32_t nq_
 
 int aur_exchange_connect(aur_exchange* ex, const uint8_t* all_handles /* [world][64], rank order */) {
   if (!ex || !all_handles) return fail(AUR_ERR_INVALID, "null argument");
-  CU_TRY(cudaSetDevice(ex->device));
+  AUR_TRY(cudaSetDevice(ex->device));
   for (int r = 0; r < ex->world; ++r) {
     if (r == ex->rank || ex->peer[r]) continue;
     cudaIpcMemHandle_t h;
@@ -1614,10 +1584,10 @@ int aur_exchange_close(aur_exchange* ex) {
 
 int aur_exchange_status(aur_exchange* ex, int64_t* exchanges_done, int32_t* status) {
   if (!ex) return fail(AUR_ERR_INVALID, "null argument");
-  CU_TRY(cudaSetDevice(ex->device));
+  AUR_TRY(cudaSetDevice(ex->device));
   uint64_t seq = 0; uint32_t st[2] = {0, 0};
-  CU_TRY(cudaMemcpy(&seq, ex->d_seq.p, 8, cudaMemcpyDeviceToHost));
-  CU_TRY(cudaMemcpy(st, ex->d_done.p, 8, cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaMemcpy(&seq, ex->d_seq.p, 8, cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaMemcpy(st, ex->d_done.p, 8, cudaMemcpyDeviceToHost));
   if (exchanges_done) *exchanges_done = static_cast<int64_t>(seq);
   if (status) *status = static_cast<int32_t>(st[1]);
   return AUR_OK;
@@ -1633,10 +1603,10 @@ int aur_search_exchange_dev(aur_index* ix, aur_exchange* ex, const void* queries
     return fail(AUR_ERR_INVALID, "batch %d x top-%d exceeds the exchange's %d x %d", nq, k, ex->nq_max, ex->k_max);
   if ((rc = check_batch(nq, k)) != AUR_OK) return rc;
   std::shared_lock<std::shared_mutex> rl(ix->rw);
-  CU_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaSetDevice(ix->device));
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
   SearchCtx* c = nullptr;
-  if ((rc = acquire_ctx(ix, s, &c)) != AUR_OK) return rc;
+  if ((rc = bound_ctx(ix, s, &c)) != AUR_OK) return rc;
   std::lock_guard<std::mutex> cl(c->mu);
   FinalizeArgs::ExchangeOut eo{};
   eo.n_peers = ex->world;
@@ -1654,9 +1624,9 @@ int aur_search_exchange_dev(aur_index* ix, aur_exchange* ex, const void* queries
   p.world = ex->world; p.rank = ex->rank; p.nq = nq; p.k = k;
   p.parity_stride = ex->parity_stride; p.slot_stride = ex->slot_stride;
   p.out_scores = scores_dev; p.out_ids = ids_dev;
-  CU_TRY(launch_exchange_merge(p, s));
+  AUR_TRY(launch_exchange_merge(p, s));
   c->last_launches += 1;
-  CU_TRY(cudaEventRecord(c->ev_end, s));
+  AUR_TRY(cudaEventRecord(c->ev_end, s));
   return AUR_OK;
 }
 
@@ -1666,7 +1636,7 @@ int aur_cosine_pairs(int32_t device, const float* a_host, const float* b_host, i
   if (n == 0) return AUR_OK;
   if (!a_host || !b_host || !out_host) return fail(AUR_ERR_INVALID, "null argument");
   if (aur_device_count() == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device: aurora_b200 has no CPU fallback");
-  CU_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaSetDevice(device));
   if (dim == 0) { for (int64_t i = 0; i < n; ++i) out_host[i] = 0.0; return AUR_OK; }
   DevBuf<float> da, db; DevBuf<double> dout;
   const size_t elems = static_cast<size_t>(n) * dim, bytes = elems * 4;
@@ -1689,7 +1659,7 @@ int aur_dev_malloc(int32_t device, uint64_t bytes, void** out) {
   if (!out) return fail(AUR_ERR_INVALID, "null argument");
   *out = nullptr;
   if (aur_device_count() == 0) return fail(AUR_ERR_NO_DEVICE, "no CUDA device");
-  CU_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaSetDevice(device));
   void* p = nullptr;
   cudaError_t e = cudaMalloc(&p, bytes ? bytes : 1);
   if (e != cudaSuccess) return fail(AUR_ERR_NOMEM, "cudaMalloc(%llu): %s", (unsigned long long)bytes, cudaGetErrorString(e));
@@ -1698,23 +1668,23 @@ int aur_dev_malloc(int32_t device, uint64_t bytes, void** out) {
 }
 int aur_dev_free(int32_t device, void* p) {
   if (!p) return AUR_OK;
-  CU_TRY(cudaSetDevice(device));
-  CU_TRY(cudaFree(p));
+  AUR_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaFree(p));
   return AUR_OK;
 }
 int aur_memcpy_h2d(int32_t device, void* dst_dev, const void* src_host, uint64_t bytes) {
   if (bytes == 0) return AUR_OK;
   if (!dst_dev || !src_host) return fail(AUR_ERR_INVALID, "null argument");
-  CU_TRY(cudaSetDevice(device));
-  CU_TRY(cudaMemcpy(dst_dev, src_host, bytes, cudaMemcpyHostToDevice));
+  AUR_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaMemcpy(dst_dev, src_host, bytes, cudaMemcpyHostToDevice));
   return AUR_OK;
 }
 int aur_memcpy_d2h(int32_t device, void* dst_host, const void* src_dev, uint64_t bytes) {
   if (bytes == 0) return AUR_OK;
   if (!dst_host || !src_dev) return fail(AUR_ERR_INVALID, "null argument");
-  CU_TRY(cudaSetDevice(device));
-  CU_TRY(cudaDeviceSynchronize());
-  CU_TRY(cudaMemcpy(dst_host, src_dev, bytes, cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaDeviceSynchronize());
+  AUR_TRY(cudaMemcpy(dst_host, src_dev, bytes, cudaMemcpyDeviceToHost));
   return AUR_OK;
 }
 
@@ -1722,7 +1692,7 @@ int aur_debug_tc_scores(aur_index* ix, const void* queries_dev, int32_t nq, int3
                         int64_t out_cap, int32_t* n_ctas_out, int32_t* tile_n_out, void* stream) {
   if (!ix || !queries_dev || !out_dev) return fail(AUR_ERR_INVALID, "null argument");
   std::shared_lock<std::shared_mutex> rl(ix->rw);
-  CU_TRY(cudaSetDevice(ix->device));
+  AUR_TRY(cudaSetDevice(ix->device));
   if (!ix->tmap_ok) return fail(AUR_ERR_UNSUPPORTED, "index shape has no tensor-core path");
   if (nq <= 0 || nq > 2 * kTcQRows) return fail(AUR_ERR_INVALID, "1..%d queries", 2 * kTcQRows);
   const int ksel = 32 + kSlack;
@@ -1735,13 +1705,13 @@ int aur_debug_tc_scores(aur_index* ix, const void* queries_dev, int32_t nq, int3
   int n_lists = 0;
   cudaStream_t s = stream ? static_cast<cudaStream_t>(stream) : ix->stream;
   SearchCtx* c = nullptr;
-  int rc = acquire_ctx(ix, s, &c);
+  int rc = bound_ctx(ix, s, &c);
   if (rc != AUR_OK) return rc;
   std::lock_guard<std::mutex> cl(c->mu);
   rc = run_tc_block(ix, c, cta_group, queries_dev, nq, ksel, ix->rows_pub.load(std::memory_order_acquire), out_dev,
                     &n_lists, s);
   if (rc != AUR_OK) return rc;
-  CU_TRY(cudaMemsetAsync(c->cand_count.p, 0, 8 * kTcQRows * 4, s));  // no finalize ran to reset them
+  AUR_TRY(cudaMemsetAsync(c->cand_count.p, 0, 8 * kTcQRows * 4, s));  // no finalize ran to reset them
   if (n_ctas_out) *n_ctas_out = n_ctas;
   if (tile_n_out) *tile_n_out = tile_n;
   return AUR_OK;
@@ -1762,16 +1732,16 @@ int aur_debug_simt_scores(aur_index* ix, const void* queries_host, int32_t nq, c
   Scope sc;
   int32_t scope[2];
   if (q_user && (rc = stage_tenant_scope(c, call.s, nq, q_user, q_org, scope, &sc)) != AUR_OK) return rc;
-  CU_TRY(c->score_chunk.reserve(static_cast<size_t>(nq) * kSimtChunk));
+  AUR_TRY(c->score_chunk.reserve(static_cast<size_t>(nq) * kSimtChunk));
   std::vector<float> chunk;
   for (int64_t r0 = 0; r0 < n; r0 += kSimtChunk) {   // the chunks and launches of search_enqueue's generic path
     const int64_t nr = std::min(n - r0, kSimtChunk);
     chunk.resize(static_cast<size_t>(nq) * nr);
-    CU_TRY(cudaMemsetAsync(c->score_chunk.p, 0xFF, chunk.size() * 4, call.s));   // NaN wherever the kernel writes nothing
-    CU_TRY(launch_simt_scores(c->stage_q.p, ix->d_rows.p, ix->dtype, ix->dim, nq, r0, nr, n, ix->d_inv_norm.p,
-                              simt_filter(ix, sc, nullptr, 0), c->score_chunk.p, call.s));
-    CU_TRY(cudaMemcpyAsync(chunk.data(), c->score_chunk.p, chunk.size() * 4, cudaMemcpyDeviceToHost, call.s));
-    CU_TRY(cudaStreamSynchronize(call.s));
+    AUR_TRY(cudaMemsetAsync(c->score_chunk.p, 0xFF, chunk.size() * 4, call.s));   // NaN wherever the kernel writes nothing
+    AUR_TRY(launch_simt_scores(c->stage_q.p, ix->d_rows.p, ix->dtype, ix->dim, nq, r0, nr, n, ix->d_inv_norm.p,
+                               simt_filter(ix, sc, nullptr, 0), c->score_chunk.p, call.s));
+    AUR_TRY(cudaMemcpyAsync(chunk.data(), c->score_chunk.p, chunk.size() * 4, cudaMemcpyDeviceToHost, call.s));
+    AUR_TRY(cudaStreamSynchronize(call.s));
     for (int32_t q = 0; q < nq; ++q)
       std::copy(chunk.begin() + q * nr, chunk.begin() + (q + 1) * nr, out_host + q * n + r0);
   }
@@ -1797,10 +1767,10 @@ int aur_debug_list_scores(aur_index* ix, const void* queries_host, int32_t nq, c
   if ((rc = call.stage(queries_host, nq, 1, nullptr, nullptr)) != AUR_OK) return rc;
   if ((rc = prepare_scope(q, &pt)) != AUR_OK) return rc;   // the lists resolved and planned as aur_search_lists does
   const ListPlan& pl = pt.pl;
-  CU_TRY(c->list_stage.reserve(pl.stage.size()));
-  CU_TRY(c->list_scores.reserve(std::max<size_t>(pl.max_slots, 1) * kSimtSeg));
-  CU_TRY(c->cand_a.reserve(pl.max_cand));
-  CU_TRY(cudaMemcpyAsync(c->list_stage.p, pl.stage.data(), pl.stage.size() * 4, cudaMemcpyHostToDevice, call.s));
+  AUR_TRY(c->list_stage.reserve(pl.stage.size()));
+  AUR_TRY(c->list_scores.reserve(std::max<size_t>(pl.max_slots, 1) * kSimtSeg));
+  AUR_TRY(c->cand_a.reserve(pl.max_cand));
+  AUR_TRY(cudaMemcpyAsync(c->list_stage.p, pl.stage.data(), pl.stage.size() * 4, cudaMemcpyHostToDevice, call.s));
   std::fill(out_host, out_host + nq * n, nanf(""));
   std::vector<float> sc;
   for (const ListPlan::Block& b : pl.blocks)
@@ -1808,10 +1778,10 @@ int aur_debug_list_scores(aur_index* ix, const void* queries_host, int32_t nq, c
       // every work item's scores: query b.q0 + qidx[q0 + g] against row list_rows[row0 + j] (the plan's host copy)
       const ListItem* items = reinterpret_cast<const ListItem*>(pl.stage.data() + ln.items);
       sc.resize(static_cast<size_t>(items[ln.n_items - 1].out + items[ln.n_items - 1].nq) * kSimtSeg);
-      CU_TRY(cudaMemsetAsync(c->list_scores.p, 0xFF, sc.size() * 4, call.s));   // NaN wherever the kernel writes nothing
-      CU_TRY(launch_list_search(list_params(ix, c, b, ln, nullptr, 1 + kSlack), ln.max_nq, call.s));
-      CU_TRY(cudaMemcpyAsync(sc.data(), c->list_scores.p, sc.size() * 4, cudaMemcpyDeviceToHost, call.s));
-      CU_TRY(cudaStreamSynchronize(call.s));
+      AUR_TRY(cudaMemsetAsync(c->list_scores.p, 0xFF, sc.size() * 4, call.s));   // NaN wherever the kernel writes nothing
+      AUR_TRY(launch_list_search(list_params(ix, c, b, ln, nullptr, 1 + kSlack), ln.max_nq, call.s));
+      AUR_TRY(cudaMemcpyAsync(sc.data(), c->list_scores.p, sc.size() * 4, cudaMemcpyDeviceToHost, call.s));
+      AUR_TRY(cudaStreamSynchronize(call.s));
       for (int i = 0; i < ln.n_items; ++i) {
         const ListItem& it = items[i];
         for (int g = 0; g < it.nq; ++g) {

@@ -33,13 +33,6 @@
 
 using namespace aur;
 
-#define ENC_TRY(expr)                                                                                  \
-  do {                                                                                                 \
-    cudaError_t e_ = (expr);                                                                           \
-    if (e_ != cudaSuccess)                                                                             \
-      return report_error(AUR_ERR_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(e_), __FILE__, __LINE__); \
-  } while (0)
-
 namespace {
 
 struct Layer {
@@ -96,8 +89,8 @@ int make_tmap(CUtensorMap* tm, const void* base, int cols, int rows, int box_row
 
 template <typename T>
 int dev_alloc(DevBuf<T>& b, size_t n) {
-  ENC_TRY(b.reserve(n));
-  ENC_TRY(cudaMemset(b.p, 0, n * sizeof(T)));
+  AUR_TRY(b.reserve(n));
+  AUR_TRY(cudaMemset(b.p, 0, n * sizeof(T)));
   return AUR_OK;
 }
 
@@ -154,7 +147,7 @@ int gemm(aur_encoder* e, const CUtensorMap* tm_a, const CUtensorMap* tm_w, __nv_
   p.bias = bias; p.resid = resid; p.ldr = ldr; p.out = out; p.ldo = n;
   const int tile_m = 128 * e->cta_group;
   p.m_tiles = (m_rows + tile_m - 1) / tile_m; p.n_tiles = n / e->bn; p.k_blocks = k / 64;
-  ENC_TRY(gemm_tc_launch(e->cta_group, e->bn, epi, e->sm_count, tm_a, tm_w, p, e->stream));
+  AUR_TRY(gemm_tc_launch(e->cta_group, e->bn, epi, e->sm_count, tm_a, tm_w, p, e->stream));
   return AUR_OK;
 }
 
@@ -164,13 +157,13 @@ int forward_locked(aur_encoder* e, const int32_t* cu_host, int n_seq, int n_item
   const int T = cu_host[n_seq], H = c.hidden, I = c.inter;
   const int t_pad = round_up(T, 256);
   cudaStream_t s = e->stream;
-  ENC_TRY(cudaMemcpyAsync(e->d_tok.p, e->h_tok.p, sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
-  ENC_TRY(cudaMemcpyAsync(e->d_pos.p, e->h_pos.p, sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
-  ENC_TRY(cudaMemcpyAsync(e->d_cu.p, cu_host, sizeof(int32_t) * (n_seq + 1), cudaMemcpyHostToDevice, s));
-  ENC_TRY(cudaMemcpyAsync(e->d_items.p, e->h_items.p, sizeof(AttnItem) * n_items, cudaMemcpyHostToDevice, s));
-  ENC_TRY(cudaEventRecord(e->ev[0], s));
+  AUR_TRY(cudaMemcpyAsync(e->d_tok.p, e->h_tok.p, sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(e->d_pos.p, e->h_pos.p, sizeof(int32_t) * T, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(e->d_cu.p, cu_host, sizeof(int32_t) * (n_seq + 1), cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(e->d_items.p, e->h_items.p, sizeof(AttnItem) * n_items, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaEventRecord(e->ev[0], s));
   int launches = 0;
-  ENC_TRY(launch_embed_ln(e->d_tok.p, e->d_pos.p, T, t_pad, e->word.p, e->pos.p, e->type.p, e->emb_g.p, e->emb_b.p, c.ln_eps, H, e->x.p, s));
+  AUR_TRY(launch_embed_ln(e->d_tok.p, e->d_pos.p, T, t_pad, e->word.p, e->pos.p, e->type.p, e->emb_g.p, e->emb_b.p, c.ln_eps, H, e->x.p, s));
   ++launches;
   AttnParams ap{};
   const int HP = e->hp;
@@ -180,17 +173,17 @@ int forward_locked(aur_encoder* e, const int32_t* cu_host, int n_seq, int n_item
     Layer& L = e->layers[l];
     int rc;
     if ((rc = gemm(e, &e->tm_x, &L.tm_wqkv, e->qkv.p, T, 3 * HP, H, kEpiBias, L.bqkv.p, nullptr, 0))) return rc;
-    ENC_TRY(attn_tc_launch(&e->tm_qkv, ap, s));
+    AUR_TRY(attn_tc_launch(&e->tm_qkv, ap, s));
     if ((rc = gemm(e, &e->tm_ctx, &L.tm_wo, e->y.p, T, H, HP, kEpiBiasResid, L.bo.p, e->x.p, H))) return rc;
-    ENC_TRY(launch_layernorm(e->y.p, L.ln1_g.p, L.ln1_b.p, c.ln_eps, T, H, e->x.p, s));
+    AUR_TRY(launch_layernorm(e->y.p, L.ln1_g.p, L.ln1_b.p, c.ln_eps, T, H, e->x.p, s));
     if ((rc = gemm(e, &e->tm_x, &L.tm_wi, e->inter.p, T, I, H, kEpiBiasGelu, L.bi.p, nullptr, 0))) return rc;
     if ((rc = gemm(e, &e->tm_inter, &L.tm_wo2, e->y.p, T, H, I, kEpiBiasResid, L.bo2.p, e->x.p, H))) return rc;
-    ENC_TRY(launch_layernorm(e->y.p, L.ln2_g.p, L.ln2_b.p, c.ln_eps, T, H, e->x.p, s));
+    AUR_TRY(launch_layernorm(e->y.p, L.ln2_g.p, L.ln2_b.p, c.ln_eps, T, H, e->x.p, s));
     launches += 7;
   }
-  ENC_TRY(launch_pool(e->x.p, e->d_cu.p, n_seq, H, c.pool, c.normalize, e->d_pool_f32.p, e->d_pool_bf16.p, s));
+  AUR_TRY(launch_pool(e->x.p, e->d_cu.p, n_seq, H, c.pool, c.normalize, e->d_pool_f32.p, e->d_pool_bf16.p, s));
   ++launches;
-  ENC_TRY(cudaEventRecord(e->ev[1], s));
+  AUR_TRY(cudaEventRecord(e->ev[1], s));
   e->stats.tokens = T; e->stats.seqs = n_seq; e->stats.launches = launches;
   double af = 0.0;
   for (int i = 0; i < n_seq; ++i) { const double len = cu_host[i + 1] - cu_host[i]; af += 4.0 * len * len * H; }
@@ -289,7 +282,7 @@ int run_texts(aur_encoder* e, const Texts& in, const int32_t* q, int32_t nq, int
     const bool open = p < nq && w != in.lo(q[p]);
     const int n_closed = p - p0, n_fold = n_closed + (open ? 1 : 0);
     if (!lk.owns_lock()) lk.lock();
-    ENC_TRY(cudaSetDevice(e->cfg.device));
+    AUR_TRY(cudaSetDevice(e->cfg.device));
     cu_b.assign(static_cast<size_t>(m) + 1, 0);
     int n_items = 0;
     for (int i = 0; i < m; ++i) {
@@ -308,7 +301,7 @@ int run_texts(aur_encoder* e, const Texts& in, const int32_t* q, int32_t nq, int
       fold |= in.hi(j) - in.lo(j) > 1;
     }
     int rc = AUR_OK;
-    if (fold) ENC_TRY(cudaMemcpyAsync(e->d_fold.p, e->h_fold.p, sizeof(FoldItem) * n_fold, cudaMemcpyHostToDevice, e->stream));
+    if (fold) AUR_TRY(cudaMemcpyAsync(e->d_fold.p, e->h_fold.p, sizeof(FoldItem) * n_fold, cudaMemcpyHostToDevice, e->stream));
     rc = forward_locked(e, cu_b.data(), m, n_items);
     if (rc == AUR_OK && fold) {
       float* carry = e->d_fold_f32.p + static_cast<size_t>(e->cfg.max_seqs) * H;
@@ -351,8 +344,8 @@ int encode_texts(aur_encoder* e, const Texts& in, int32_t n_seq, int32_t n_texts
   rc = run_texts(e, in, q.data(), n_texts, e->cfg.max_tokens, e->cfg.max_seqs,
                  [&](aur_encoder* enc, const int32_t* qs, int n, const float* rows) -> int {
                    const size_t at = static_cast<size_t>(qs[0]) * H, len = static_cast<size_t>(n) * H;
-                   if (to_f32) ENC_TRY(cudaMemcpyAsync(to_f32 + at, rows, len * sizeof(float), cudaMemcpyDeviceToHost, enc->stream));
-                   if (to_bf16) ENC_TRY(cudaMemcpyAsync(to_bf16 + at, enc->d_pool_bf16.p, len * 2, cudaMemcpyDeviceToHost, enc->stream));
+                   if (to_f32) AUR_TRY(cudaMemcpyAsync(to_f32 + at, rows, len * sizeof(float), cudaMemcpyDeviceToHost, enc->stream));
+                   if (to_bf16) AUR_TRY(cudaMemcpyAsync(to_bf16 + at, enc->d_pool_bf16.p, len * 2, cudaMemcpyDeviceToHost, enc->stream));
                    return AUR_OK;
                  });
   if (rc != AUR_OK) return rc;
@@ -465,9 +458,9 @@ int aur_encoder_open(const aur_encoder_config* cfg, aur_encoder** out) {
   if (cfg->max_pos < 1 || cfg->max_pos > 512) return report_error(AUR_ERR_UNSUPPORTED, "max_pos must be 1..512");
   if (cfg->layers < 1 || cfg->vocab < 1 || cfg->type_vocab < 1 || cfg->max_tokens < 1 || cfg->max_seqs < 1)
     return report_error(AUR_ERR_INVALID, "layers / vocab / type_vocab / max_tokens / max_seqs must be positive");
-  ENC_TRY(cudaSetDevice(cfg->device));
+  AUR_TRY(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
-  ENC_TRY(cudaGetDeviceProperties(&prop, cfg->device));
+  AUR_TRY(cudaGetDeviceProperties(&prop, cfg->device));
   if (prop.major != 9) return report_error(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
   std::unique_ptr<aur_encoder> e(new aur_encoder());
   e->cfg = *cfg;
@@ -528,7 +521,7 @@ int aur_encoder_close(aur_encoder* e) {
 int aur_encoder_load(aur_encoder* e, const char* name, const float* data, int64_t count) {
   if (!e || !name || !data) return report_error(AUR_ERR_INVALID, "null argument");
   std::lock_guard<std::mutex> g(e->mu);
-  ENC_TRY(cudaSetDevice(e->cfg.device));
+  AUR_TRY(cudaSetDevice(e->cfg.device));
   ParamSlot slot{};
   if (!find_param(e, name, &slot)) return report_error(AUR_ERR_INVALID, "unknown parameter '%s'", name);
   if (slot.count != count) return report_error(AUR_ERR_INVALID, "parameter '%s' has %lld elements, expected %lld", name,
@@ -554,13 +547,13 @@ int aur_encoder_load(aur_encoder* e, const char* name, const float* data, int64_
     n_up = static_cast<int64_t>(padded.size());
   }
   if (slot.bf16) {
-    ENC_TRY(e->d_stage.reserve(static_cast<size_t>(n_up)));
-    ENC_TRY(cudaMemcpyAsync(e->d_stage.p, data, sizeof(float) * n_up, cudaMemcpyHostToDevice, e->stream));
-    ENC_TRY(launch_f32_to_bf16(e->d_stage.p, static_cast<__nv_bfloat16*>(slot.dst), n_up, e->stream));
+    AUR_TRY(e->d_stage.reserve(static_cast<size_t>(n_up)));
+    AUR_TRY(cudaMemcpyAsync(e->d_stage.p, data, sizeof(float) * n_up, cudaMemcpyHostToDevice, e->stream));
+    AUR_TRY(launch_f32_to_bf16(e->d_stage.p, static_cast<__nv_bfloat16*>(slot.dst), n_up, e->stream));
   } else {
-    ENC_TRY(cudaMemcpyAsync(slot.dst, data, sizeof(float) * n_up, cudaMemcpyHostToDevice, e->stream));
+    AUR_TRY(cudaMemcpyAsync(slot.dst, data, sizeof(float) * n_up, cudaMemcpyHostToDevice, e->stream));
   }
-  ENC_TRY(cudaStreamSynchronize(e->stream));
+  AUR_TRY(cudaStreamSynchronize(e->stream));
   for (size_t i = 0; i < e->missing.size(); ++i)
     if (e->missing[i] == name) { e->missing.erase(e->missing.begin() + i); break; }
   return AUR_OK;
@@ -651,10 +644,10 @@ int aur_encoder_get_stats(aur_encoder* e, aur_encoder_stats* out) {
 int aur_debug_encoder_hidden(aur_encoder* e, uint16_t* out, int64_t count) {
   if (!e || !out) return report_error(AUR_ERR_INVALID, "null argument");
   std::lock_guard<std::mutex> g(e->mu);
-  ENC_TRY(cudaSetDevice(e->cfg.device));
+  AUR_TRY(cudaSetDevice(e->cfg.device));
   if (count != e->last_tokens * e->cfg.hidden) return report_error(AUR_ERR_INVALID, "count must be tokens * hidden of the last call");
-  ENC_TRY(cudaStreamSynchronize(e->stream));
-  ENC_TRY(cudaMemcpy(out, e->x.p, count * 2, cudaMemcpyDeviceToHost));
+  AUR_TRY(cudaStreamSynchronize(e->stream));
+  AUR_TRY(cudaMemcpy(out, e->x.p, count * 2, cudaMemcpyDeviceToHost));
   return AUR_OK;
 }
 
@@ -663,9 +656,9 @@ int aur_debug_gemm(int32_t device, const uint16_t* a, const uint16_t* w, const f
   if (!a || !w || !bias || !out || m <= 0) return report_error(AUR_ERR_INVALID, "null argument");
   if (n % 128 || k % 64 || epi < 0 || epi > 2 || (epi == kEpiBiasResid && !resid) || (cta_group != 1 && cta_group != 2))
     return report_error(AUR_ERR_UNSUPPORTED, "n %% 128, k %% 64, epi 0..2, cta_group 1..2");
-  ENC_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaSetDevice(device));
   cudaDeviceProp prop;
-  ENC_TRY(cudaGetDeviceProperties(&prop, device));
+  AUR_TRY(cudaGetDeviceProperties(&prop, device));
   const int m_pad = round_up(m, 128 * cta_group), bn = n % 256 == 0 ? 256 : 128;
   DevBuf<__nv_bfloat16> da, dw, dr, dout; DevBuf<float> db;   // freed on return (cudaFree waits for the device)
   int rc = AUR_OK;
@@ -704,9 +697,9 @@ int aur_debug_attention(int32_t device, const uint16_t* qkv, const int32_t* cu, 
                         int32_t hidden, uint16_t* ctx, float* ms_out) {
   if (!qkv || !cu || !ctx || n_seq <= 0) return report_error(AUR_ERR_INVALID, "null argument");
   if (heads <= 0 || hidden != heads * 64) return report_error(AUR_ERR_UNSUPPORTED, "head dim must be 64");
-  ENC_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaSetDevice(device));
   cudaDeviceProp prop;
-  ENC_TRY(cudaGetDeviceProperties(&prop, device));
+  AUR_TRY(cudaGetDeviceProperties(&prop, device));
   const int T = cu[n_seq], rows = round_up(T, 128) + 512;
   std::vector<AttnItem> items;
   for (int i = 0; i < n_seq; ++i) {

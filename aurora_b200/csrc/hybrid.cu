@@ -23,6 +23,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <vector>
@@ -33,14 +34,6 @@
 using namespace aur;
 
 namespace {
-
-#define HYB_TRY(expr)                                                                                            \
-  do {                                                                                                           \
-    cudaError_t e_ = (expr);                                                                                     \
-    if (e_ != cudaSuccess)                                                                                       \
-      return report_error(e_ == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "%s: %s (%s:%d)", #expr, \
-                          cudaGetErrorString(e_), __FILE__, __LINE__);                                           \
-  } while (0)
 
 constexpr int kFuseThreads = kMaxK;        // thread t holds entry t of each merged leg (fetch <= kMaxK)
 constexpr int kFuseWarps = kFuseThreads / 32;
@@ -260,8 +253,8 @@ __global__ void __launch_bounds__(kFuseThreads) hybrid_merge_fuse_kernel(FusePar
 
 // Scratch of one shard's part of a hybrid call on one device: the events its legs' streams record for the join.  The
 // context of shard 0 also hosts the join on its stream, the gathered lists of the other shards, the merge + fusion
-// kernel and the copy back.  Idle contexts are pooled for the life of the process and never destroyed: the pool is
-// static, and the statically linked CUDA runtime may already be torn down when static destructors run.
+// kernel and the copy back.  Every device's pool lives for the life of the process and is never destroyed: the
+// statically linked CUDA runtime may already be torn down when static destructors run.
 struct HybridCtx {
   int device = 0;
   Stream stream;
@@ -273,39 +266,29 @@ struct HybridCtx {
   DevBuf<int64_t> run_max;          // the merge's scratch, both legs
   DevBuf<unsigned char> out;        // fused [nq][k_out] scores | ids | cosines, copied back in one piece
   HostBuf<unsigned char> host;      // page-locked landing area of that copy
+
+  int init(int dev) {
+    device = dev;
+    int lo = 0, hi = 0;   // hi = numerically lowest = highest priority, as the search contexts' streams
+    const cudaError_t e = [&]() -> cudaError_t {
+      AUR_CU_RET(cudaSetDevice(device));
+      AUR_CU_RET(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+      AUR_CU_RET(stream.create(cudaStreamNonBlocking, hi));
+      AUR_CU_RET(kw_done.create(cudaEventDisableTiming));
+      return dense_done.create(cudaEventDisableTiming);
+    }();
+    if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "hybrid search context: %s", cudaGetErrorString(e));
+    return AUR_OK;
+  }
 };
 
-std::mutex g_pool_mu;
-std::vector<HybridCtx*> g_idle;
-
-int hyb_acquire(int device, HybridCtx** out) {
-  {
-    std::lock_guard<std::mutex> lk(g_pool_mu);
-    for (size_t i = 0; i < g_idle.size(); ++i)
-      if (g_idle[i]->device == device) {
-        *out = g_idle[i];
-        g_idle.erase(g_idle.begin() + static_cast<std::ptrdiff_t>(i));
-        return AUR_OK;
-      }
-  }
-  std::unique_ptr<HybridCtx> h(new HybridCtx());
-  h->device = device;
-  int lo = 0, hi = 0;   // hi = numerically lowest = highest priority, as the search contexts' streams
-  const cudaError_t e = [&]() -> cudaError_t {
-    AUR_CU_RET(cudaSetDevice(device));
-    AUR_CU_RET(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    AUR_CU_RET(h->stream.create(cudaStreamNonBlocking, hi));
-    AUR_CU_RET(h->kw_done.create(cudaEventDisableTiming));
-    return h->dense_done.create(cudaEventDisableTiming);
-  }();
-  if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "hybrid search context: %s", cudaGetErrorString(e));
-  *out = h.release();
-  return AUR_OK;
-}
-
-void hyb_release(HybridCtx* h) {
-  std::lock_guard<std::mutex> lk(g_pool_mu);
-  g_idle.push_back(h);
+CtxPool<HybridCtx>& hyb_pool(int device) {
+  static std::mutex mu;
+  static auto* pools = new std::map<int, CtxPool<HybridCtx>>();   // never destroyed (see HybridCtx)
+  std::lock_guard<std::mutex> lk(mu);
+  auto made = pools->try_emplace(device);
+  if (made.second) made.first->second.device = device;
+  return made.first->second;
 }
 
 // The arguments of one call, checked.
@@ -321,7 +304,7 @@ struct HybridArgs {
 
 // The join on shard 0's device (every keyword leg, every dense leg), the gather of the other shards' lists, the merge +
 // fusion and the copy into hs[0]->host.  Shard 0's buffers were prepared by run_on_devices.
-int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const std::vector<KwLeg>& kl,
+int join_and_fuse(const HybridArgs& a, const std::vector<CtxLease<HybridCtx>>& hs, const std::vector<KwLeg>& kl,
                   const std::vector<DenseLeg>& dl) {
   const int n = a.n;
   const size_t nl = static_cast<size_t>(a.nq) * a.fetch, no = static_cast<size_t>(a.nq) * a.k_out;
@@ -329,24 +312,24 @@ int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const 
   cudaStream_t st = h->stream;
   for (int s = 0; s < n; ++s) {
     HybridCtx* o = hs[static_cast<size_t>(s)];
-    HYB_TRY(cudaSetDevice(o->device));
-    HYB_TRY(cudaEventRecord(o->dense_done, dl[static_cast<size_t>(s)].stream));
-    HYB_TRY(cudaEventRecord(o->kw_done, kl[static_cast<size_t>(s)].stream));   // the store shares the shard's device
+    AUR_TRY(cudaSetDevice(o->device));
+    AUR_TRY(cudaEventRecord(o->dense_done, dl[static_cast<size_t>(s)].stream));
+    AUR_TRY(cudaEventRecord(o->kw_done, kl[static_cast<size_t>(s)].stream));   // the store shares the shard's device
   }
-  HYB_TRY(cudaSetDevice(h->device));
+  AUR_TRY(cudaSetDevice(h->device));
   // their lists come over by peer copies (also between shards of one device, so that every shard count runs the same code)
   for (int s = 0; s < n; ++s) {
     const HybridCtx* o = hs[static_cast<size_t>(s)];
     const KwLeg& k = kl[static_cast<size_t>(s)];
     const DenseLeg& d = dl[static_cast<size_t>(s)];
-    HYB_TRY(cudaStreamWaitEvent(st, o->kw_done, 0));
-    HYB_TRY(cudaStreamWaitEvent(st, o->dense_done, 0));
+    AUR_TRY(cudaStreamWaitEvent(st, o->kw_done, 0));
+    AUR_TRY(cudaStreamWaitEvent(st, o->dense_done, 0));
     if (s == 0) continue;
     const size_t at = static_cast<size_t>(s - 1) * nl;
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_cos.p + at, h->device, d.scores, o->device, nl * 4, st));
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_did.p + at, h->device, d.ids, o->device, nl * 8, st));
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_ks.p + at, h->device, k.scores, k.device, nl * 8, st));
-    HYB_TRY(cudaMemcpyPeerAsync(h->g_kid.p + at, h->device, k.ids, k.device, nl * 8, st));
+    AUR_TRY(cudaMemcpyPeerAsync(h->g_cos.p + at, h->device, d.scores, o->device, nl * 4, st));
+    AUR_TRY(cudaMemcpyPeerAsync(h->g_did.p + at, h->device, d.ids, o->device, nl * 8, st));
+    AUR_TRY(cudaMemcpyPeerAsync(h->g_ks.p + at, h->device, k.scores, k.device, nl * 8, st));
+    AUR_TRY(cudaMemcpyPeerAsync(h->g_kid.p + at, h->device, k.ids, k.device, nl * 8, st));
   }
   FuseParams p;
   p.dense = LegLists{dl[0].ids, dl[0].scores, h->g_did.p, h->g_cos.p, h->run_max.p};
@@ -359,33 +342,33 @@ int join_and_fuse(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const 
   p.o_i = reinterpret_cast<int64_t*>(h->out.p + no * 8);
   p.o_c = reinterpret_cast<float*>(h->out.p + no * 16);
   hybrid_merge_fuse_kernel<<<static_cast<unsigned>(a.nq), kFuseThreads, 0, st>>>(p);
-  HYB_TRY(cudaGetLastError());
-  HYB_TRY(cudaMemcpyAsync(h->host.p, h->out.p, no * kOutBytes, cudaMemcpyDeviceToHost, st));
-  HYB_TRY(cudaStreamSynchronize(st));
+  AUR_TRY(cudaGetLastError());
+  AUR_TRY(cudaMemcpyAsync(h->host.p, h->out.p, no * kOutBytes, cudaMemcpyDeviceToHost, st));
+  AUR_TRY(cudaStreamSynchronize(st));
   return AUR_OK;
 }
 
 // Inside the keyword legs: shard 0's device takes the weights and the output space, every shard's dense leg is enqueued
 // (dense_legs: aur_search_ex's search, or with programs aur_search_filtered's), then join_and_fuse.  hs[s] is on shard
 // s's device; rows[s] receives shard s's snapshot.
-int run_on_devices(const HybridArgs& a, const std::vector<HybridCtx*>& hs, const std::vector<KwLeg>& kl, int64_t* rows) {
+int run_on_devices(const HybridArgs& a, const std::vector<CtxLease<HybridCtx>>& hs, const std::vector<KwLeg>& kl, int64_t* rows) {
   const int n = a.n;
   const size_t nl = static_cast<size_t>(a.nq) * a.fetch, no = static_cast<size_t>(a.nq) * a.k_out;
   HybridCtx* h = hs[0];
   cudaStream_t st = h->stream;
-  HYB_TRY(cudaSetDevice(h->device));
-  HYB_TRY(h->w.reserve(a.w.size()));
-  HYB_TRY(h->out.reserve(no * kOutBytes));
-  HYB_TRY(h->host.reserve(no * kOutBytes, cudaHostAllocDefault));
+  AUR_TRY(cudaSetDevice(h->device));
+  AUR_TRY(h->w.reserve(a.w.size()));
+  AUR_TRY(h->out.reserve(no * kOutBytes));
+  AUR_TRY(h->host.reserve(no * kOutBytes, cudaHostAllocDefault));
   if (n > 1) {
     const size_t ng = static_cast<size_t>(n - 1) * nl;
-    HYB_TRY(h->g_cos.reserve(ng));
-    HYB_TRY(h->g_did.reserve(ng));
-    HYB_TRY(h->g_ks.reserve(ng));
-    HYB_TRY(h->g_kid.reserve(ng));
-    HYB_TRY(h->run_max.reserve(2 * static_cast<size_t>(n) * nl));
+    AUR_TRY(h->g_cos.reserve(ng));
+    AUR_TRY(h->g_did.reserve(ng));
+    AUR_TRY(h->g_ks.reserve(ng));
+    AUR_TRY(h->g_kid.reserve(ng));
+    AUR_TRY(h->run_max.reserve(2 * static_cast<size_t>(n) * nl));
   }
-  HYB_TRY(cudaMemcpyAsync(h->w.p, a.w.data(), a.w.size() * 8, cudaMemcpyHostToDevice, st));
+  AUR_TRY(cudaMemcpyAsync(h->w.p, a.w.data(), a.w.size() * 8, cudaMemcpyHostToDevice, st));
   // (pageable: staged before the call returns.  The dense legs run on their own streams, so the copy would not wait for
   // their kernels after them either; it stays first, the order every hybrid measurement in DESIGN.md section 9 used)
   DenseQuery q{a.queries_host, a.nq, a.fetch};
@@ -443,18 +426,15 @@ int hybrid_search(aur_index* const* shards, aur_kw* const* stores, int32_t n, co
         return rc;
     if ((rc = filter_check_queries(*fp, nq, max_list_rows)) != AUR_OK) return rc;
   }
-  std::vector<HybridCtx*> hs;
+  std::vector<CtxLease<HybridCtx>> hs(static_cast<size_t>(n));   // outlives kw_legs: the copy out reads hs[0]
   std::vector<int64_t> rows(2 * static_cast<size_t>(n), 0);
   rc = kw_legs(stores, n, q_terms, q_offsets, nq, fetch, q_user, q_org, fp, [&](const std::vector<KwLeg>& kl) {
     int r = AUR_OK;
     for (int s = 0; s < n && r == AUR_OK; ++s) {
-      HybridCtx* h = nullptr;
-      if ((r = hyb_acquire(kl[static_cast<size_t>(s)].device, &h)) == AUR_OK) hs.push_back(h);
+      r = hyb_pool(kl[static_cast<size_t>(s)].device).lease(&hs[static_cast<size_t>(s)]);
       rows[static_cast<size_t>(n + s)] = kl[static_cast<size_t>(s)].snapshot_rows;
     }
-    if (r == AUR_OK) r = run_on_devices(a, hs, kl, rows.data());
-    for (HybridCtx* h : hs) { cudaSetDevice(h->device); cudaStreamSynchronize(h->stream); }   // nothing stays in flight
-    return r;
+    return r == AUR_OK ? run_on_devices(a, hs, kl, rows.data()) : r;
   });
   if (rc == AUR_OK) {
     const size_t no = static_cast<size_t>(nq) * k_out;
@@ -463,7 +443,6 @@ int hybrid_search(aur_index* const* shards, aur_kw* const* stores, int32_t n, co
     memcpy(cosine_out, hs[0]->host.p + no * 16, no * 4);
     if (snapshot_rows_out) memcpy(snapshot_rows_out, rows.data(), rows.size() * 8);
   }
-  for (HybridCtx* h : hs) hyb_release(h);
   return rc;
 }
 

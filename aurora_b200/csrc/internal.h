@@ -7,8 +7,11 @@
 
 #include <algorithm>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <vector>
+
+#include "../../include/aurora_b200.h"
 
 struct aur_index;
 struct aur_kw;
@@ -415,6 +418,78 @@ struct Event {
 };
 // Returns expr's cudaError_t from the enclosing function unless it is cudaSuccess.
 #define AUR_CU_RET(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return e_; } while (0)
+// Returns from the enclosing C-ABI function unless expr is cudaSuccess: AUR_ERR_NOMEM for a failed allocation, else
+// AUR_ERR_CUDA, with the expression, the error and where it failed as the message.
+#define AUR_TRY(expr)                                                                                                    \
+  do {                                                                                                                   \
+    cudaError_t e_ = (expr);                                                                                             \
+    if (e_ != cudaSuccess)                                                                                               \
+      return ::aur::report_error(e_ == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "%s: %s (%s:%d)", #expr, \
+                                 cudaGetErrorString(e_), __FILE__, __LINE__);                                            \
+  } while (0)
+
+// Per-call contexts (stream, events, grow-only scratch) of one device, pooled so that calls on several host threads
+// each run on their own.  lease() hands out an idle context, or builds one with T::init(device) (which reports its own
+// error) when none is idle.  Every context lives as long as the pool; T has a `stream`.
+template <typename T> class CtxPool;
+// One context taken from a pool for one call.  Its destructor makes the pool's device current, waits for the context's
+// stream and only then gives the context back, so a context is never reused while work that reads its scratch is still
+// in flight, on success or on an error.  A lease declared after the lock the call holds (a shard's or store's shared
+// lock) is destroyed before that lock: the stream is idle before the lock is released.
+template <typename T>
+class CtxLease {
+ public:
+  CtxLease() = default;
+  CtxLease(const CtxLease&) = delete;
+  CtxLease& operator=(const CtxLease&) = delete;
+  ~CtxLease() {
+    if (!c_) return;
+    cudaSetDevice(pool_->device);
+    cudaStreamSynchronize(c_->stream);
+    pool_->give_back(c_);
+  }
+  T* operator->() const { return c_; }
+  operator T*() const { return c_; }
+ private:
+  friend class CtxPool<T>;
+  CtxPool<T>* pool_ = nullptr;
+  T* c_ = nullptr;
+};
+template <typename T>
+class CtxPool {
+ public:
+  int device = 0;   // set before the first lease
+  // An idle context or a new one into *out (empty); AUR_OK or T::init's error.
+  int lease(CtxLease<T>* out) {
+    out->pool_ = this;
+    {
+      std::lock_guard<std::mutex> lk(mu_);
+      if (!idle_.empty()) { out->c_ = idle_.back(); idle_.pop_back(); return AUR_OK; }
+    }
+    std::unique_ptr<T> c(new T());
+    const int rc = c->init(device);
+    if (rc != AUR_OK) return rc;
+    std::lock_guard<std::mutex> lk(mu_);
+    out->c_ = c.get();
+    all_.push_back(std::move(c));
+    return AUR_OK;
+  }
+  std::vector<T*> contexts() {   // every context made so far, leased or idle
+    std::lock_guard<std::mutex> lk(mu_);
+    std::vector<T*> v;
+    for (auto& c : all_) v.push_back(c.get());
+    return v;
+  }
+ private:
+  friend class CtxLease<T>;
+  void give_back(T* c) {
+    std::lock_guard<std::mutex> lk(mu_);
+    idle_.push_back(c);
+  }
+  std::mutex mu_;
+  std::vector<std::unique_ptr<T>> all_;
+  std::vector<T*> idle_;
+};
 
 // ---------------------------------------------------------------- filter columns and uploads, host side (filter.cu)
 // The attribute columns of a vector shard or a keyword store (program columns 2..): `rows` int32 codes each, -1 =
@@ -443,15 +518,16 @@ inline FiltParams filter_pass(FiltParams p, int ps) { p.n_programs = filter_pass
 // ---------------------------------------------------------------- the two legs of a hybrid query (hybrid.cu)
 // Dense legs: every host search of a vector shard (aur_search, aur_search_ex, aur_search_subset, aur_search_lists,
 // aur_search_filtered and the hybrid query's dense legs) over shards[0 .. n) (distinct, arguments checked), each shard's
-// part on a pooled search context of its device and that context's stream, over the prefix published when the part
-// began.  q holds the host queries and at most one scope: tenant codes (nullable), allow-ids or per-query lists (n = 1
-// only), or checked programs with max_list_rows applied per shard.  Every shard's shared lock is taken in address order;
-// with programs every shard's count pass is enqueued before any is waited on, and their read-back is the only host sync.
-// Then every shard's search is enqueued and then(legs) runs with every shard's (device, stream, top-k lists [nq * k] in
-// device memory, valid once the stream reaches them, snapshot, matching rows per program) while the shards' shared locks
-// and contexts are held; the streams are idle again before this returns.  aur_stats.last_* of each shard describe its
-// part.  scores_host / ids_host (n = 1, nullable): the caller's host outputs; when both are page-locked and mapped, the
-// search writes its lists straight into them (DenseLeg.direct) instead of into device staging.  (capi.cu)
+// part on a search context leased from its shard's pool and that context's stream, over the prefix published when the
+// part began.  q holds the host queries and at most one scope: tenant codes (nullable), allow-ids or per-query lists
+// (n = 1 only), or checked programs with max_list_rows applied per shard.  Every shard's shared lock is taken in address
+// order; with programs every shard's count pass is enqueued before any is waited on, and their read-back is the only
+// host sync.  Then every shard's search is enqueued and then(legs) runs with every shard's (device, stream, top-k lists
+// [nq * k] in device memory, valid once the stream reaches them, snapshot, matching rows per program) while the shards'
+// shared locks and leases are held; each lease (CtxLease) drains its stream before its shard's lock is released, also
+// on an error, so the streams are idle again before this returns.  aur_stats.last_* of each shard describe its part.
+// scores_host / ids_host (n = 1, nullable): the caller's host outputs; when both are page-locked and mapped, the search
+// writes its lists straight into them (DenseLeg.direct) instead of into device staging.  (capi.cu)
 struct DenseQuery {
   const void* queries; int32_t nq, k;
   const int32_t* q_user = nullptr; const int32_t* q_org = nullptr;        // tenant codes [nq]

@@ -71,14 +71,6 @@ constexpr int kIxSelBlocksPerSm = 4;                       // selection grid ove
 // accumulator entry scanned, per launch
 constexpr double kFwdNsPerPosting = 0.02, kIxNsPerPosting = 0.05, kIxNsPerAcc = 0.005, kIxNsPerLaunch = 3000.0;
 
-#define KW_TRY(expr)                                                                                             \
-  do {                                                                                                           \
-    cudaError_t e_ = (expr);                                                                                     \
-    if (e_ != cudaSuccess)                                                                                       \
-      return report_error(e_ == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "%s: %s (%s:%d)", #expr, \
-                          cudaGetErrorString(e_), __FILE__, __LINE__);                                           \
-  } while (0)
-
 struct Cand { double s; int64_t id; };   // (score, id); worse = lower score, then higher id
 
 __device__ __forceinline__ bool better(const Cand& a, const Cand& b) {
@@ -435,6 +427,16 @@ struct KwCtx {
                                               // launches whose contribution table spilled to global memory
   int path = 0;                  // of the last search: AUR_KW_PATH_* bits
   int64_t postings = 0;          // of the last search: postings it read
+
+  int init(int /* device: current */) {
+    const cudaError_t e = [&]() -> cudaError_t {
+      AUR_CU_RET(stream.create(cudaStreamNonBlocking));
+      AUR_CU_RET(ev0.create());
+      return ev1.create();
+    }();
+    if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "search context: %s", cudaGetErrorString(e));
+    return AUR_OK;
+  }
 };
 
 // flags[rows[i]] = v for the listed rows (allow-list rows of a search; tombstones)
@@ -449,7 +451,7 @@ struct aur_kw {
   std::shared_mutex rw;      // shared: searches and pure appends; exclusive: tombstones, posting growth, compaction
   std::mutex mu_write;       // one writer at a time (taken before rw)
   std::mutex mu_stat;        // the published prefix and its statistics, read and written together
-  std::mutex mu_pool;
+  std::mutex mu_last;        // the last search's statistics (last_*)
   int device = 0, sm_count = 0;
   size_t smem_optin = 0;
   int64_t capacity = 0;
@@ -475,37 +477,13 @@ struct aur_kw {
   std::vector<int64_t> h_toff;
   float ix_build_ms = 0.f;
   std::atomic<int> kw_path{0};   // aur_kw_set_option "kw_path": 0 auto, 1 forward, 2 index
-  // search pool + last search's stats
-  std::vector<std::unique_ptr<KwCtx>> ctxs;
-  std::vector<KwCtx*> idle;
+  CtxPool<KwCtx> ctxs;           // search contexts
   int last_launches = 0, last_terms = 0, last_spilled = 0, last_path = 0;
   int64_t last_postings = 0;
   float last_ms = 0.f;
 };
 
 namespace {
-
-int kw_ctx_acquire(aur_kw* kw, KwCtx** out) {
-  {
-    std::lock_guard<std::mutex> lk(kw->mu_pool);
-    if (!kw->idle.empty()) { *out = kw->idle.back(); kw->idle.pop_back(); return AUR_OK; }
-  }
-  std::unique_ptr<KwCtx> c(new KwCtx());
-  const cudaError_t e = [&]() -> cudaError_t {
-    AUR_CU_RET(c->stream.create(cudaStreamNonBlocking));
-    AUR_CU_RET(c->ev0.create());
-    return c->ev1.create();
-  }();
-  if (e != cudaSuccess) return report_error(AUR_ERR_CUDA, "search context: %s", cudaGetErrorString(e));
-  std::lock_guard<std::mutex> lk(kw->mu_pool);
-  *out = c.get();
-  kw->ctxs.push_back(std::move(c));
-  return AUR_OK;
-}
-void kw_ctx_release(aur_kw* kw, KwCtx* c) {
-  std::lock_guard<std::mutex> lk(kw->mu_pool);
-  kw->idle.push_back(c);
-}
 
 // Tombstone distinct published rows in one pass: their postings are gathered on the device and read back with one copy
 // (their terms leave df), one kernel clears their live flags.  Caller holds the exclusive lock and mu_stat.
@@ -561,7 +539,7 @@ int build_index(aur_kw* kw) {
   const auto t0 = std::chrono::steady_clock::now();
   const int64_t R = static_cast<int64_t>(kw->h_len.size()), P = kw->h_off.back();
   const int64_t T = static_cast<int64_t>(kw->df.size());   // every term id seen so far (writers resize df)
-  KW_TRY(cudaSetDevice(kw->device));
+  AUR_TRY(cudaSetDevice(kw->device));
   cudaStream_t s = kw->stream;
   DevBuf<int64_t> toff; DevBuf<uint2> tpost;
   std::vector<int64_t> h_toff(static_cast<size_t>(T) + 1);
@@ -777,12 +755,12 @@ KwIxPlan kw_ix_plan(const aur_kw* kw, const KwSnap& sn, const KwBlock& b) {
 // of the store's prefix sn.n_rows (index and / or forward scan) and the folds into c's [nq][k] output.  Nothing waits.
 int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>& blocks, const KwSnap& sn, int64_t N,
               double avgdl) {
-  KW_TRY(cudaSetDevice(kw->device));
+  AUR_TRY(cudaSetDevice(kw->device));
   cudaStream_t s = c->stream;
   const int k = q.k;
   const int64_t n_rows = sn.n_rows;
   c->launches = 0; c->terms = 0; c->spilled = 0; c->path = 0; c->postings = 0;
-  KW_TRY(cudaEventRecord(c->ev0, s));
+  AUR_TRY(cudaEventRecord(c->ev0, s));
   const uint8_t* d_allow = nullptr;
   if (q.allow) {
     std::vector<int32_t> rows;
@@ -793,13 +771,13 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
         if (it != kw->id2row.end() && it->second < n_rows) rows.push_back(static_cast<int32_t>(it->second));
       }
     }
-    KW_TRY(c->allow.reserve(static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
-    KW_TRY(c->allow_rows.reserve(std::max<size_t>(rows.size(), 1)));
-    KW_TRY(cudaMemsetAsync(c->allow.p, 0, static_cast<size_t>(std::max<int64_t>(n_rows, 1)), s));
+    AUR_TRY(c->allow.reserve(static_cast<size_t>(std::max<int64_t>(n_rows, 1))));
+    AUR_TRY(c->allow_rows.reserve(std::max<size_t>(rows.size(), 1)));
+    AUR_TRY(cudaMemsetAsync(c->allow.p, 0, static_cast<size_t>(std::max<int64_t>(n_rows, 1)), s));
     if (!rows.empty()) {
-      KW_TRY(cudaMemcpyAsync(c->allow_rows.p, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
+      AUR_TRY(cudaMemcpyAsync(c->allow_rows.p, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
       kw_scatter_flag<<<static_cast<unsigned>((rows.size() + 255) / 256), 256, 0, s>>>(c->allow_rows.p, static_cast<int64_t>(rows.size()), c->allow.p, 1);
-      KW_TRY(cudaGetLastError());
+      AUR_TRY(cudaGetLastError());
       c->launches += 1;
     }
     d_allow = c->allow.p;
@@ -810,19 +788,19 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
   const bool scores = n_rows > 0 && N > 0 && std::any_of(blocks.begin(), blocks.end(), [](const KwBlock& b) { return b.nu > 0; });
   if (q.fp && scores) {
     n_passes = filter_passes(q.fp->n_programs);
-    KW_TRY(c->fmask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(n_rows)));
+    AUR_TRY(c->fmask.reserve(static_cast<size_t>(n_passes) * static_cast<size_t>(n_rows)));
     FiltParams p;
-    KW_TRY(filter_upload(*q.fp, kw->d_user.p, kw->d_org.p, kw->attrs, c->fstage, s, &p));
+    AUR_TRY(filter_upload(*q.fp, kw->d_user.p, kw->d_org.p, kw->attrs, c->fstage, s, &p));
     p.live = kw->d_live.p; p.n_rows = n_rows;
     for (int ps = 0; ps < n_passes; ++ps) {
-      KW_TRY(launch_filter_mask(filter_pass(p, ps), c->fmask.p + static_cast<size_t>(ps) * n_rows, s));
+      AUR_TRY(launch_filter_mask(filter_pass(p, ps), c->fmask.p + static_cast<size_t>(ps) * n_rows, s));
       c->launches += 1;
     }
     d_fmask = c->fmask.p;
   }
   const size_t nout = static_cast<size_t>(q.nq) * k;
-  KW_TRY(c->out_s.reserve(nout));
-  KW_TRY(c->out_ids.reserve(nout));
+  AUR_TRY(c->out_s.reserve(nout));
+  AUR_TRY(c->out_ids.reserve(nout));
   for (const KwBlock& b : blocks) {
     const int nqb = b.nqb, nu = b.nu;
     double* o_s = c->out_s.p + static_cast<size_t>(b.q0) * k;
@@ -830,12 +808,12 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
     if (nu == 0 || n_rows == 0 || N == 0) {   // nothing can match: padding only
       std::vector<double> ps(static_cast<size_t>(nqb) * k, -INFINITY);
       std::vector<int64_t> pi(static_cast<size_t>(nqb) * k, -1);
-      KW_TRY(cudaMemcpyAsync(o_s, ps.data(), ps.size() * 8, cudaMemcpyHostToDevice, s));
-      KW_TRY(cudaMemcpyAsync(o_i, pi.data(), pi.size() * 8, cudaMemcpyHostToDevice, s));
+      AUR_TRY(cudaMemcpyAsync(o_s, ps.data(), ps.size() * 8, cudaMemcpyHostToDevice, s));
+      AUR_TRY(cudaMemcpyAsync(o_i, pi.data(), pi.size() * 8, cudaMemcpyHostToDevice, s));
       continue;
     }
-    KW_TRY(c->tab.reserve(b.tab.size()));
-    KW_TRY(cudaMemcpyAsync(c->tab.p, b.tab.data(), b.tab.size(), cudaMemcpyHostToDevice, s));   // pageable: staged before return
+    AUR_TRY(c->tab.reserve(b.tab.size()));
+    AUR_TRY(cudaMemcpyAsync(c->tab.p, b.tab.data(), b.tab.size(), cudaMemcpyHostToDevice, s));   // pageable: staged before return
     const int ksel = k;
     c->terms = std::max(c->terms, nu);
     // rows [0, R) from the term-major index when the path rule picks it, rows [R, n_rows) by the forward scan; the
@@ -846,8 +824,8 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
     const int gi = R > 0 ? kw_grid(R, kIxSelBlocksPerSm * static_cast<int64_t>(kw->sm_count), &rpb_i) : 0;
     const int gt = tail > 0 ? kw_grid(tail, 2 * static_cast<int64_t>(kw->sm_count), &rpb_t) : 0;
     int n_lists = gi + gt;   // folded below
-    KW_TRY(c->buf.reserve(static_cast<size_t>(std::max(gi, gt)) * nqb * kKwBufCap));
-    KW_TRY(c->lists_a.reserve(static_cast<size_t>(nqb) * n_lists * ksel));
+    AUR_TRY(c->buf.reserve(static_cast<size_t>(std::max(gi, gt)) * nqb * kKwBufCap));
+    AUR_TRY(c->lists_a.reserve(static_cast<size_t>(nqb) * n_lists * ksel));
     KwParams p{};
     p.off = kw->d_off.p; p.post = kw->d_post.p; p.len = kw->d_len.p; p.ids = kw->d_ids.p; p.user = kw->d_user.p; p.org = kw->d_org.p;
     p.live = kw->d_live.p; p.allow = d_allow; p.n_rows = n_rows;
@@ -866,8 +844,8 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
     }
     if (R > 0) {
       const size_t acc_n = static_cast<size_t>(ix.group) * static_cast<size_t>(R);
-      if (c->acc.n < acc_n) { KW_TRY(c->acc.reserve(acc_n)); c->acc_clean = false; }
-      if (!c->acc_clean) KW_TRY(cudaMemsetAsync(c->acc.p, 0, c->acc.n * 8, s));
+      if (c->acc.n < acc_n) { AUR_TRY(c->acc.reserve(acc_n)); c->acc_clean = false; }
+      if (!c->acc_clean) AUR_TRY(cudaMemsetAsync(c->acc.p, 0, c->acc.n * 8, s));
       c->acc_clean = false;   // until every group's selection has been enqueued
       for (int g0 = 0; g0 < nqb; g0 += ix.group) {
         const int ng = std::min(ix.group, nqb - g0);
@@ -886,7 +864,7 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
           t.j = j;
           const unsigned gx = static_cast<unsigned>(std::min<int64_t>((longest + 1023) / 1024, 65535));
           kw_ix_term_kernel<<<dim3(gx, static_cast<unsigned>(ng)), 256, 0, s>>>(t);
-          KW_TRY(cudaGetLastError());
+          AUR_TRY(cudaGetLastError());
           c->launches += 1;
         }
         KwParams ps = p;
@@ -897,7 +875,7 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
         const size_t smem = static_cast<size_t>(ng) * sizeof(Cand) + kKwWarps * kKwBufCap * sizeof(Cand) + 4 * static_cast<size_t>(ng);
         if (d_fmask) kw_ix_select_kernel<true><<<gi, kKwThreads, smem, s>>>(ps, c->acc.p, R, n_lists);
         else kw_ix_select_kernel<false><<<gi, kKwThreads, smem, s>>>(ps, c->acc.p, R, n_lists);
-        KW_TRY(cudaGetLastError());
+        AUR_TRY(cudaGetLastError());
         c->launches += 1;
       }
       c->acc_clean = true;
@@ -913,8 +891,8 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
       const bool in_smem = smem + cval_smem <= kw->smem_optin;
       if (!in_smem) ++c->spilled;
       if (in_smem) smem += cval_smem;
-      else KW_TRY(c->cval.reserve(static_cast<size_t>(g) * kKwWarps * nu));
-      if (gi) KW_TRY(c->lists_b.reserve(static_cast<size_t>(nqb) * g * ksel));
+      else AUR_TRY(c->cval.reserve(static_cast<size_t>(g) * kKwWarps * nu));
+      if (gi) AUR_TRY(c->lists_b.reserve(static_cast<size_t>(nqb) * g * ksel));
       KwParams pf = p;
       pf.off += R; pf.len += R; pf.ids += R; pf.user += R; pf.org += R; pf.live += R;
       if (pf.allow) pf.allow += R;
@@ -924,12 +902,12 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
       pf.lists = gi ? c->lists_b.p : c->lists_a.p;
       if (d_fmask) kw_score_kernel<true><<<g, kKwThreads, smem, s>>>(pf, in_smem ? 1 : 0);
       else kw_score_kernel<false><<<g, kKwThreads, smem, s>>>(pf, in_smem ? 1 : 0);
-      KW_TRY(cudaGetLastError());
+      AUR_TRY(cudaGetLastError());
       c->launches += 1;
       if (gi) {   // into lists gi .. n_lists - 1 of every query
         const size_t w = static_cast<size_t>(g) * ksel * sizeof(Cand);
-        KW_TRY(cudaMemcpy2DAsync(c->lists_a.p + static_cast<size_t>(gi) * ksel, static_cast<size_t>(n_lists) * ksel * sizeof(Cand),
-                                 c->lists_b.p, w, w, static_cast<size_t>(nqb), cudaMemcpyDeviceToDevice, s));
+        AUR_TRY(cudaMemcpy2DAsync(c->lists_a.p + static_cast<size_t>(gi) * ksel, static_cast<size_t>(n_lists) * ksel * sizeof(Cand),
+                                  c->lists_b.p, w, w, static_cast<size_t>(nqb), cudaMemcpyDeviceToDevice, s));
       }
       c->path |= AUR_KW_PATH_FORWARD;
       c->postings += sn.post - (R > 0 ? sn.ix_post : 0);
@@ -946,27 +924,27 @@ int kw_launch(aur_kw* kw, KwCtx* c, const KwQuery& q, const std::vector<KwBlock>
       const size_t fsmem = static_cast<size_t>(sort_n) * sizeof(Cand);
       if (n_groups == 1) {
         kw_fold_kernel<<<dim3(1, nqb), 256, fsmem, s>>>(cur, n_lists, ksel, group, sort_n, nullptr, o_s, o_i, k);
-        KW_TRY(cudaGetLastError());
+        AUR_TRY(cudaGetLastError());
         c->launches += 1;
         break;
       }
       DevBuf<Cand>& dst = in_a ? c->lists_b : c->lists_a;
-      KW_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
+      AUR_TRY(dst.reserve(static_cast<size_t>(nqb) * n_groups * ksel));
       kw_fold_kernel<<<dim3(n_groups, nqb), 256, fsmem, s>>>(cur, n_lists, ksel, group, sort_n, dst.p, nullptr, nullptr, k);
-      KW_TRY(cudaGetLastError());
+      AUR_TRY(cudaGetLastError());
       c->launches += 1;
       cur = dst.p; n_lists = n_groups; in_a = !in_a;
     }
   }
-  KW_TRY(cudaEventRecord(c->ev1, s));
+  AUR_TRY(cudaEventRecord(c->ev1, s));
   return AUR_OK;
 }
 
 // Publish the last_* statistics of a search whose part on c's stream has completed.
 int kw_publish(aur_kw* kw, KwCtx* c) {
   float ms = 0.f;
-  KW_TRY(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-  std::lock_guard<std::mutex> lk(kw->mu_pool);
+  AUR_TRY(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
+  std::lock_guard<std::mutex> lk(kw->mu_last);
   kw->last_launches = c->launches; kw->last_ms = ms;
   kw->last_terms = c->terms; kw->last_spilled = c->spilled;
   kw->last_path = c->path; kw->last_postings = c->postings;
@@ -975,12 +953,12 @@ int kw_publish(aur_kw* kw, KwCtx* c) {
 
 // Wait for one store's part, copy its [nq][k] lists to the host and publish its last_* statistics.
 int kw_collect(aur_kw* kw, KwCtx* c, const KwQuery& q, double* scores_out, int64_t* ids_out) {
-  KW_TRY(cudaSetDevice(kw->device));
+  AUR_TRY(cudaSetDevice(kw->device));
   cudaStream_t s = c->stream;
   const size_t nout = static_cast<size_t>(q.nq) * q.k;
-  KW_TRY(cudaMemcpyAsync(scores_out, c->out_s.p, nout * 8, cudaMemcpyDeviceToHost, s));
-  KW_TRY(cudaMemcpyAsync(ids_out, c->out_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
-  KW_TRY(cudaStreamSynchronize(s));
+  AUR_TRY(cudaMemcpyAsync(scores_out, c->out_s.p, nout * 8, cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaMemcpyAsync(ids_out, c->out_ids.p, nout * 8, cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaStreamSynchronize(s));
   return kw_publish(kw, c);
 }
 
@@ -1012,8 +990,8 @@ void kw_prepare(aur_kw* const* stores, int n, const KwQuery& q, KwPlan* pl) {
 
 // Search stores[0 .. n) (distinct, arguments checked) as one corpus and hand the enqueued parts to
 // after(ctxs, snaps): ctxs[s] = store s's context, whose stream computes its top-k lists into out_s / out_ids, scored
-// with the idf and avgdl of the union of the snapshots snaps.  Every store's shared lock is held, and every context
-// stays out of its pool, until after() has returned and the context's stream is idle (also on an error).
+// with the idf and avgdl of the union of the snapshots snaps.  Every store's shared lock and every context's lease are
+// held until after() has returned; each lease drains its stream before the locks are released (also on an error).
 template <typename After>
 int kw_run(aur_kw* const* stores, int n, const KwQuery& q, After&& after) {
   // shared locks for the whole search, in one order (by address) so that searches over overlapping store sets cannot
@@ -1025,22 +1003,15 @@ int kw_run(aur_kw* const* stores, int n, const KwQuery& q, After&& after) {
   for (aur_kw* kw : order) locks.emplace_back(kw->rw);
   KwPlan pl;
   kw_prepare(stores, n, q, &pl);
-  // every store's work enqueued before any is waited on; the contexts go back to their pools only once their streams
-  // are idle (also on an error), before the locks are released
-  struct Ctxs {
-    std::vector<std::pair<aur_kw*, KwCtx*>> v;
-    ~Ctxs() {
-      for (auto& e : v) { cudaSetDevice(e.first->device); cudaStreamSynchronize(e.second->stream); kw_ctx_release(e.first, e.second); }
-    }
-  } ctxs;
+  // every store's work enqueued before any is waited on; the leases come after the locks
+  std::vector<CtxLease<KwCtx>> leases(static_cast<size_t>(n));
   std::vector<KwCtx*> cs;
   for (int s = 0; s < n; ++s) {
     aur_kw* kw = stores[s];
-    KW_TRY(cudaSetDevice(kw->device));
-    KwCtx* c = nullptr;
-    int rc = kw_ctx_acquire(kw, &c);
+    AUR_TRY(cudaSetDevice(kw->device));
+    int rc = kw->ctxs.lease(&leases[static_cast<size_t>(s)]);
     if (rc != AUR_OK) return rc;
-    ctxs.v.emplace_back(kw, c);
+    KwCtx* c = leases[static_cast<size_t>(s)];
     cs.push_back(c);
     const KwSnap& sn = pl.snaps[static_cast<size_t>(s)];
     if ((rc = kw_launch(kw, c, q, pl.blocks, sn, pl.N, pl.avgdl)) != AUR_OK) return rc;
@@ -1077,8 +1048,8 @@ int kw_legs(aur_kw* const* stores, int n, const int32_t* q_terms, const int64_t*
     int rc = then(legs);
     if (rc != AUR_OK) return rc;
     for (int s = 0; s < n; ++s) {
-      KW_TRY(cudaSetDevice(stores[s]->device));
-      KW_TRY(cudaStreamSynchronize(cs[static_cast<size_t>(s)]->stream));
+      AUR_TRY(cudaSetDevice(stores[s]->device));
+      AUR_TRY(cudaStreamSynchronize(cs[static_cast<size_t>(s)]->stream));
       if ((rc = kw_publish(stores[s], cs[static_cast<size_t>(s)])) != AUR_OK) return rc;
     }
     return AUR_OK;
@@ -1105,12 +1076,13 @@ int aur_kw_open(int32_t device, int64_t doc_capacity, int64_t postings_capacity,
   if (cudaGetDeviceCount(&ndev) != cudaSuccess) { cudaGetLastError(); ndev = 0; }
   if (ndev == 0) return report_error(AUR_ERR_NO_DEVICE, "no CUDA device: aurora_b200 has no CPU fallback");
   if (device < 0 || device >= ndev) return report_error(AUR_ERR_INVALID, "device %d out of range", device);
-  KW_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaSetDevice(device));
   cudaDeviceProp prop;
-  KW_TRY(cudaGetDeviceProperties(&prop, device));
+  AUR_TRY(cudaGetDeviceProperties(&prop, device));
   if (prop.major != 9) return report_error(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
   std::unique_ptr<aur_kw> kw(new aur_kw());
   kw->device = device; kw->capacity = doc_capacity;
+  kw->ctxs.device = device;
   kw->sm_count = prop.multiProcessorCount; kw->smem_optin = prop.sharedMemPerBlockOptin;
   const cudaError_t e = [&]() -> cudaError_t {
     AUR_CU_RET(kw->stream.create(cudaStreamNonBlocking));
@@ -1137,8 +1109,7 @@ int aur_kw_close(aur_kw* kw) {
   if (!kw) return AUR_OK;
   cudaSetDevice(kw->device);
   if (kw->stream) cudaStreamSynchronize(kw->stream);   // this store's work only: other users of the GPU are not waited on
-  for (auto& c : kw->ctxs) cudaStreamSynchronize(c->stream);
-  delete kw;
+  delete kw;                                           // (its search contexts are idle: each lease drained its stream)
   return AUR_OK;
 }
 
@@ -1211,7 +1182,7 @@ int kw_append_rows(aur_kw* kw, const KwRows& r, const KwLand& land) {
   std::shared_lock<std::shared_mutex> rl(kw->rw, std::defer_lock);
   std::unique_lock<std::shared_mutex> xl(kw->rw, std::defer_lock);
   if (exclusive) xl.lock(); else rl.lock();
-  KW_TRY(cudaSetDevice(kw->device));
+  AUR_TRY(cudaSetDevice(kw->device));
   const cudaError_t ge = kw->d_post.grow_keep(static_cast<size_t>(post0 + total), static_cast<size_t>(post0), kw->stream);
   if (ge != cudaSuccess)
     return report_error(ge == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "posting growth: %s", cudaGetErrorString(ge));
@@ -1228,14 +1199,14 @@ int kw_append_rows(aur_kw* kw, const KwRows& r, const KwLand& land) {
   for (int64_t i = 0; i < n; ++i) last[ids[i]] = i;
   for (int64_t i = 0; i < n; ++i) if (last[ids[i]] != i) live[static_cast<size_t>(i)] = 0;
   cudaStream_t s = kw->stream;
-  KW_TRY(land(kw->d_post.p + post0, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_off.p + base + 1, off.data(), static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_len.p + base, r.len, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_ids.p + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_user.p + base, user.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_org.p + base, org.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaMemcpyAsync(kw->d_live.p + base, live.data(), static_cast<size_t>(n), cudaMemcpyHostToDevice, s));
-  KW_TRY(cudaStreamSynchronize(s));
+  AUR_TRY(land(kw->d_post.p + post0, s));
+  AUR_TRY(cudaMemcpyAsync(kw->d_off.p + base + 1, off.data(), static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(kw->d_len.p + base, r.len, static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(kw->d_ids.p + base, ids, static_cast<size_t>(n) * 8, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(kw->d_user.p + base, user.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(kw->d_org.p + base, org.data(), static_cast<size_t>(n) * 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(kw->d_live.p + base, live.data(), static_cast<size_t>(n), cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaStreamSynchronize(s));
   for (int64_t i = 0; i < n; ++i) {
     kw->h_off.push_back(off[static_cast<size_t>(i)]);
     kw->h_len.push_back(r.len[i]);
@@ -1284,7 +1255,7 @@ int aur_kw_remove(aur_kw* kw, const int64_t* ids, int64_t n, int64_t* removed) {
   if (!kw || (n > 0 && !ids) || n < 0) return report_error(AUR_ERR_INVALID, "null argument or n < 0");
   std::lock_guard<std::mutex> wk(kw->mu_write);
   std::unique_lock<std::shared_mutex> xl(kw->rw);
-  KW_TRY(cudaSetDevice(kw->device));
+  AUR_TRY(cudaSetDevice(kw->device));
   std::lock_guard<std::mutex> st(kw->mu_stat);
   std::vector<int64_t> dead;
   for (int64_t i = 0; i < n; ++i) {
@@ -1304,8 +1275,8 @@ int aur_kw_compact(aur_kw* kw, int64_t* reclaimed) {
   if (reclaimed) *reclaimed = 0;
   std::lock_guard<std::mutex> wk(kw->mu_write);
   std::unique_lock<std::shared_mutex> xl(kw->rw);
-  KW_TRY(cudaSetDevice(kw->device));
-  KW_TRY(cudaStreamSynchronize(kw->stream));        // searches are host-synchronous: the exclusive lock already drained them
+  AUR_TRY(cudaSetDevice(kw->device));
+  AUR_TRY(cudaStreamSynchronize(kw->stream));        // searches are host-synchronous: the exclusive lock already drained them
   const int64_t rows = static_cast<int64_t>(kw->h_len.size());
   std::vector<int32_t> map;
   for (int64_t r = 0; r < rows; ++r) if (kw->h_live[static_cast<size_t>(r)]) map.push_back(static_cast<int32_t>(r));
@@ -1376,7 +1347,7 @@ int aur_kw_get_stats(aur_kw* kw, aur_kw_stats* out) {
     out->docs = kw->rows_pub; out->live = kw->n_live; out->total_len = kw->total_len;
     out->postings_used = kw->post_pub;
   }
-  std::lock_guard<std::mutex> lk(kw->mu_pool);
+  std::lock_guard<std::mutex> lk(kw->mu_last);
   out->postings_allocated = static_cast<int64_t>(kw->d_post.n);
   out->capacity = kw->capacity;
   out->last_launches = kw->last_launches;
@@ -1390,7 +1361,7 @@ int aur_kw_set_attrs(aur_kw* kw, int32_t col, const int64_t* ids, const int32_t*
   if (!kw || n < 0 || (n > 0 && (!ids || !codes))) return report_error(AUR_ERR_INVALID, "null argument");
   std::lock_guard<std::mutex> wk(kw->mu_write);
   std::shared_lock<std::shared_mutex> rl(kw->rw);
-  KW_TRY(cudaSetDevice(kw->device));
+  AUR_TRY(cudaSetDevice(kw->device));
   std::vector<int32_t> pairs;   // (row, code); id2row changes only under mu_write, which this call holds
   pairs.reserve(2 * static_cast<size_t>(n));
   for (int64_t i = 0; i < n; ++i) {
@@ -1453,10 +1424,10 @@ int aur_kw_read_rows(aur_kw* kw, int64_t row0, int64_t n, int64_t* ids_out, int6
   if (ids_out) std::copy(kw->h_ids.begin() + row0, kw->h_ids.begin() + row0 + n, ids_out);
   *postings_out = total;
   if (!term_ids_out || !tfs_out || cap < total || total == 0) return AUR_OK;   // count mode
-  KW_TRY(cudaSetDevice(kw->device));
+  AUR_TRY(cudaSetDevice(kw->device));
   std::vector<uint2> post(static_cast<size_t>(total));
-  KW_TRY(cudaMemcpyAsync(post.data(), kw->d_post.p + p0, static_cast<size_t>(total) * 8, cudaMemcpyDeviceToHost, kw->stream));
-  KW_TRY(cudaStreamSynchronize(kw->stream));
+  AUR_TRY(cudaMemcpyAsync(post.data(), kw->d_post.p + p0, static_cast<size_t>(total) * 8, cudaMemcpyDeviceToHost, kw->stream));
+  AUR_TRY(cudaStreamSynchronize(kw->stream));
   for (int64_t j = 0; j < total; ++j) {
     term_ids_out[j] = static_cast<int32_t>(post[static_cast<size_t>(j)].x);
     tfs_out[j] = static_cast<int32_t>(post[static_cast<size_t>(j)].y);
@@ -1491,7 +1462,7 @@ int aur_kw_get_index_stats(aur_kw* kw, aur_kw_index_stats* out) {
     out->builds = kw->ix_builds;
     out->last_build_ms = kw->ix_build_ms;
   }
-  std::lock_guard<std::mutex> lk(kw->mu_pool);
+  std::lock_guard<std::mutex> lk(kw->mu_last);
   out->last_path = kw->last_path;
   out->last_postings = kw->last_postings;
   return AUR_OK;

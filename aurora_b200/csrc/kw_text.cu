@@ -38,14 +38,6 @@ constexpr int64_t kMaxDocBytes = 0x7FFFFFFFll;        // byte positions of a sli
 constexpr int kMaxStores = 64;
 constexpr int kT = 256;
 
-#define TX_TRY(expr)                                                                                             \
-  do {                                                                                                           \
-    cudaError_t e_ = (expr);                                                                                     \
-    if (e_ != cudaSuccess)                                                                                       \
-      return report_error(e_ == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "%s: %s (%s:%d)", #expr, \
-                          cudaGetErrorString(e_), __FILE__, __LINE__);                                           \
-  } while (0)
-
 unsigned blocks(int64_t n) { return static_cast<unsigned>(std::max<int64_t>(1, (n + kT - 1) / kT)); }
 
 // ------------------------------------------------------------------------------------------------------- kernels
@@ -292,33 +284,33 @@ int analyse(aur_kw_vocab* v, const char* text, const int64_t* off, int32_t n, Sl
   cudaStream_t s = v->stream;
   const int64_t nb = off[n];
   if (v->h_stage.n < static_cast<size_t>(nb))
-    TX_TRY(v->h_stage.reserve(static_cast<size_t>(std::max<int64_t>(nb, 1 << 20)), cudaHostAllocDefault));
+    AUR_TRY(v->h_stage.reserve(static_cast<size_t>(std::max<int64_t>(nb, 1 << 20)), cudaHostAllocDefault));
   // 1. text in (the staging buffer is reused only after this slice's work has completed)
   if (nb) memcpy(v->h_stage.p, text, static_cast<size_t>(nb));
   const size_t B = static_cast<size_t>(std::max<int64_t>(nb, 1));
-  TX_TRY(v->text.reserve(B)); TX_TRY(v->doff.reserve(static_cast<size_t>(n) + 1));
-  TX_TRY(v->is_w.reserve(B)); TX_TRY(v->is_s.reserve(B)); TX_TRY(v->cpos.reserve(B)); TX_TRY(v->widx.reserve(B));
-  TX_TRY(v->totals.reserve(2));
-  if (nb) TX_TRY(cudaMemcpyAsync(v->text.p, v->h_stage.p, static_cast<size_t>(nb), cudaMemcpyHostToDevice, s));
-  TX_TRY(cudaMemcpyAsync(v->doff.p, off, (static_cast<size_t>(n) + 1) * 8, cudaMemcpyHostToDevice, s));
+  AUR_TRY(v->text.reserve(B)); AUR_TRY(v->doff.reserve(static_cast<size_t>(n) + 1));
+  AUR_TRY(v->is_w.reserve(B)); AUR_TRY(v->is_s.reserve(B)); AUR_TRY(v->cpos.reserve(B)); AUR_TRY(v->widx.reserve(B));
+  AUR_TRY(v->totals.reserve(2));
+  if (nb) AUR_TRY(cudaMemcpyAsync(v->text.p, v->h_stage.p, static_cast<size_t>(nb), cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaMemcpyAsync(v->doff.p, off, (static_cast<size_t>(n) + 1) * 8, cudaMemcpyHostToDevice, s));
   // 2. classify, scans: normalised bytes and word starts
   int32_t nw = 0, nl = 0;
   if (nb) {
     tx_classify<<<blocks(nb), kT, 0, s>>>(v->text.p, nb, v->doff.p, n, v->is_w.p, v->is_s.p);
-    TX_TRY(cudaGetLastError());
+    AUR_TRY(cudaGetLastError());
     size_t tb = 0, tb2 = 0;
-    TX_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, v->is_w.p, v->cpos.p, static_cast<int>(nb), s));
-    TX_TRY(v->cub_tmp.reserve(std::max<size_t>(tb, 1)));
-    TX_TRY(cub::DeviceScan::ExclusiveSum(v->cub_tmp.p, tb, v->is_w.p, v->cpos.p, static_cast<int>(nb), s));
-    TX_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb2, v->is_s.p, v->widx.p, static_cast<int>(nb), s));
-    TX_TRY(v->cub_tmp.reserve(std::max<size_t>(tb2, 1)));
-    TX_TRY(cub::DeviceScan::ExclusiveSum(v->cub_tmp.p, tb2, v->is_s.p, v->widx.p, static_cast<int>(nb), s));
+    AUR_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, v->is_w.p, v->cpos.p, static_cast<int>(nb), s));
+    AUR_TRY(v->cub_tmp.reserve(std::max<size_t>(tb, 1)));
+    AUR_TRY(cub::DeviceScan::ExclusiveSum(v->cub_tmp.p, tb, v->is_w.p, v->cpos.p, static_cast<int>(nb), s));
+    AUR_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb2, v->is_s.p, v->widx.p, static_cast<int>(nb), s));
+    AUR_TRY(v->cub_tmp.reserve(std::max<size_t>(tb2, 1)));
+    AUR_TRY(cub::DeviceScan::ExclusiveSum(v->cub_tmp.p, tb2, v->is_s.p, v->widx.p, static_cast<int>(nb), s));
     int32_t tail[4];
-    TX_TRY(cudaMemcpyAsync(tail, v->cpos.p + nb - 1, 4, cudaMemcpyDeviceToHost, s));
-    TX_TRY(cudaMemcpyAsync(tail + 1, v->is_w.p + nb - 1, 4, cudaMemcpyDeviceToHost, s));
-    TX_TRY(cudaMemcpyAsync(tail + 2, v->widx.p + nb - 1, 4, cudaMemcpyDeviceToHost, s));
-    TX_TRY(cudaMemcpyAsync(tail + 3, v->is_s.p + nb - 1, 4, cudaMemcpyDeviceToHost, s));
-    TX_TRY(cudaStreamSynchronize(s));
+    AUR_TRY(cudaMemcpyAsync(tail, v->cpos.p + nb - 1, 4, cudaMemcpyDeviceToHost, s));
+    AUR_TRY(cudaMemcpyAsync(tail + 1, v->is_w.p + nb - 1, 4, cudaMemcpyDeviceToHost, s));
+    AUR_TRY(cudaMemcpyAsync(tail + 2, v->widx.p + nb - 1, 4, cudaMemcpyDeviceToHost, s));
+    AUR_TRY(cudaMemcpyAsync(tail + 3, v->is_s.p + nb - 1, 4, cudaMemcpyDeviceToHost, s));
+    AUR_TRY(cudaStreamSynchronize(s));
     nl = tail[0] + tail[1];
     nw = tail[2] + tail[3];
   }
@@ -330,55 +322,55 @@ int analyse(aur_kw_vocab* v, const char* text, const int64_t* off, int32_t n, Sl
   out->max_term = -1;
   if (nw == 0) return AUR_OK;
   const size_t W = static_cast<size_t>(nw);
-  TX_TRY(v->norm.reserve(static_cast<size_t>(nl))); TX_TRY(v->wstart.reserve(W + 1)); TX_TRY(v->wdoc.reserve(W));
+  AUR_TRY(v->norm.reserve(static_cast<size_t>(nl))); AUR_TRY(v->wstart.reserve(W + 1)); AUR_TRY(v->wdoc.reserve(W));
   tx_compact<<<blocks(nb), kT, 0, s>>>(v->text.p, nb, v->doff.p, n, v->is_w.p, v->is_s.p, v->cpos.p, v->widx.p, v->norm.p,
                                       v->wstart.p, v->wdoc.p);
-  TX_TRY(cudaGetLastError());
-  TX_TRY(cudaMemcpyAsync(v->wstart.p + nw, &nl, 4, cudaMemcpyHostToDevice, s));
+  AUR_TRY(cudaGetLastError());
+  AUR_TRY(cudaMemcpyAsync(v->wstart.p + nw, &nl, 4, cudaMemcpyHostToDevice, s));
   const Words w{v->norm.p, v->wstart.p, nw};
   // 3. hash, 4. lookup
-  TX_TRY(v->wh.reserve(W)); TX_TRY(v->found.reserve(W)); TX_TRY(v->bslot.reserve(W));
+  AUR_TRY(v->wh.reserve(W)); AUR_TRY(v->found.reserve(W)); AUR_TRY(v->bslot.reserve(W));
   const uint64_t hmask = v->hash_bits >= 64 ? ~0ull : ((1ull << v->hash_bits) - 1);
   tx_hash<<<blocks(nw), kT, 0, s>>>(w, hmask, v->wh.p);
   tx_lookup<<<blocks(nw), kT, 0, s>>>(w, v->wh.p, VocabDev{v->hkey.p, v->hid.p, static_cast<uint64_t>(v->hkey.n - 1), v->pool.p, v->woff.p},
                                       v->found.p);
-  TX_TRY(cudaGetLastError());
+  AUR_TRY(cudaGetLastError());
   // 5. new words: group, rank by first occurrence
   int64_t bcap = 1024;
   while (bcap < 2 * static_cast<int64_t>(nw)) bcap *= 2;
-  TX_TRY(v->occ.reserve(static_cast<size_t>(bcap))); TX_TRY(v->first.reserve(static_cast<size_t>(bcap)));
-  TX_TRY(v->is_first.reserve(W)); TX_TRY(v->rank.reserve(W)); TX_TRY(v->nlen.reserve(W)); TX_TRY(v->noff.reserve(W));
-  TX_TRY(cudaMemsetAsync(v->occ.p, 0xFF, static_cast<size_t>(bcap) * 4, s));
-  TX_TRY(cudaMemsetAsync(v->first.p, 0x7F, static_cast<size_t>(bcap) * 4, s));
+  AUR_TRY(v->occ.reserve(static_cast<size_t>(bcap))); AUR_TRY(v->first.reserve(static_cast<size_t>(bcap)));
+  AUR_TRY(v->is_first.reserve(W)); AUR_TRY(v->rank.reserve(W)); AUR_TRY(v->nlen.reserve(W)); AUR_TRY(v->noff.reserve(W));
+  AUR_TRY(cudaMemsetAsync(v->occ.p, 0xFF, static_cast<size_t>(bcap) * 4, s));
+  AUR_TRY(cudaMemsetAsync(v->first.p, 0x7F, static_cast<size_t>(bcap) * 4, s));
   tx_group<<<blocks(nw), kT, 0, s>>>(w, v->wh.p, v->found.p, v->occ.p, v->first.p, static_cast<uint64_t>(bcap - 1), v->bslot.p);
   tx_mark<<<blocks(nw), kT, 0, s>>>(w, v->bslot.p, v->first.p, v->is_first.p, v->nlen.p);
-  TX_TRY(cudaGetLastError());
+  AUR_TRY(cudaGetLastError());
   {
     size_t tb = 0;
-    TX_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, v->is_first.p, v->rank.p, nw, s));
-    TX_TRY(v->cub_tmp.reserve(std::max<size_t>(tb, 1)));
-    TX_TRY(cub::DeviceScan::ExclusiveSum(v->cub_tmp.p, tb, v->is_first.p, v->rank.p, nw, s));
-    TX_TRY(cub::DeviceScan::ExclusiveSum(v->cub_tmp.p, tb, v->nlen.p, v->noff.p, nw, s));
+    AUR_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, v->is_first.p, v->rank.p, nw, s));
+    AUR_TRY(v->cub_tmp.reserve(std::max<size_t>(tb, 1)));
+    AUR_TRY(cub::DeviceScan::ExclusiveSum(v->cub_tmp.p, tb, v->is_first.p, v->rank.p, nw, s));
+    AUR_TRY(cub::DeviceScan::ExclusiveSum(v->cub_tmp.p, tb, v->nlen.p, v->noff.p, nw, s));
   }
   tx_totals<<<1, 1, 0, s>>>(v->is_first.p, v->rank.p, v->nlen.p, v->noff.p, nw, v->totals.p);
   int64_t tot[2];
-  TX_TRY(cudaMemcpyAsync(tot, v->totals.p, 16, cudaMemcpyDeviceToHost, s));
-  TX_TRY(cudaStreamSynchronize(s));
+  AUR_TRY(cudaMemcpyAsync(tot, v->totals.p, 16, cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaStreamSynchronize(s));
   const int64_t n_new = tot[0], new_bytes = tot[1], V = v->words;
   if (V + n_new > kMaxWords)
     return report_error(AUR_ERR_INVALID, "the vocabulary would hold %lld words (at most 2^28)", (long long)(V + n_new));
   // Everything the rest of the slice allocates is reserved before the vocabulary changes, and the new words are
   // committed (V, bytes) as soon as their insertion is enqueued: a failure after that point leaves them fully in the
   // vocabulary (ids V .. V + n_new - 1, as the table and pool hold them), never in the table without being counted.
-  TX_TRY(v->key.reserve(W)); TX_TRY(v->key_sorted.reserve(W)); TX_TRY(v->ukey.reserve(W)); TX_TRY(v->cnt.reserve(W));
-  TX_TRY(v->n_runs.reserve(1)); TX_TRY(v->post.reserve(W)); TX_TRY(v->tid.reserve(W));
-  TX_TRY(v->dcnt.reserve(static_cast<size_t>(n))); TX_TRY(v->dlen.reserve(static_cast<size_t>(n)));
+  AUR_TRY(v->key.reserve(W)); AUR_TRY(v->key_sorted.reserve(W)); AUR_TRY(v->ukey.reserve(W)); AUR_TRY(v->cnt.reserve(W));
+  AUR_TRY(v->n_runs.reserve(1)); AUR_TRY(v->post.reserve(W)); AUR_TRY(v->tid.reserve(W));
+  AUR_TRY(v->dcnt.reserve(static_cast<size_t>(n))); AUR_TRY(v->dlen.reserve(static_cast<size_t>(n)));
   int end_bit = 28;
   while (end_bit < 64 && (int64_t(1) << (end_bit - 28)) < n) ++end_bit;
   size_t tb_sort = 0, tb_rle = 0;
-  TX_TRY(cub::DeviceRadixSort::SortKeys(nullptr, tb_sort, v->key.p, v->key_sorted.p, nw, 0, end_bit, s));
-  TX_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, tb_rle, v->key_sorted.p, v->ukey.p, v->cnt.p, v->n_runs.p, nw, s));
-  TX_TRY(v->cub_tmp.reserve(std::max<size_t>(std::max(tb_sort, tb_rle), 1)));
+  AUR_TRY(cub::DeviceRadixSort::SortKeys(nullptr, tb_sort, v->key.p, v->key_sorted.p, nw, 0, end_bit, s));
+  AUR_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, tb_rle, v->key_sorted.p, v->ukey.p, v->cnt.p, v->n_runs.p, nw, s));
+  AUR_TRY(v->cub_tmp.reserve(std::max<size_t>(std::max(tb_sort, tb_rle), 1)));
   // growth, then insertion
   const int rc = ensure_table(v, V + n_new);
   if (rc != AUR_OK) return rc;
@@ -391,29 +383,29 @@ int analyse(aur_kw_vocab* v, const char* text, const int64_t* off, int32_t n, Sl
   if (n_new) {
     tx_insert<<<blocks(nw), kT, 0, s>>>(w, v->wh.p, v->is_first.p, v->rank.p, v->noff.p, V, v->bytes, v->hkey.p, v->hid.p,
                                         static_cast<uint64_t>(v->hkey.n - 1), v->pool.p, v->woff.p);
-    TX_TRY(cudaGetLastError());
+    AUR_TRY(cudaGetLastError());
     v->words = V + n_new;
     v->bytes += new_bytes;
   }
   // 6. rows: sort (document, term id), run lengths as tf
   tx_keys<<<blocks(nw), kT, 0, s>>>(v->wdoc.p, v->found.p, v->bslot.p, v->first.p, v->rank.p, V, nw, v->key.p);
-  TX_TRY(cudaGetLastError());
-  TX_TRY(cub::DeviceRadixSort::SortKeys(v->cub_tmp.p, tb_sort, v->key.p, v->key_sorted.p, nw, 0, end_bit, s));
-  TX_TRY(cub::DeviceRunLengthEncode::Encode(v->cub_tmp.p, tb_rle, v->key_sorted.p, v->ukey.p, v->cnt.p, v->n_runs.p, nw, s));
-  TX_TRY(cudaMemsetAsync(v->dcnt.p, 0, static_cast<size_t>(n) * 4, s));
-  TX_TRY(cudaMemsetAsync(v->dlen.p, 0, static_cast<size_t>(n) * 4, s));
+  AUR_TRY(cudaGetLastError());
+  AUR_TRY(cub::DeviceRadixSort::SortKeys(v->cub_tmp.p, tb_sort, v->key.p, v->key_sorted.p, nw, 0, end_bit, s));
+  AUR_TRY(cub::DeviceRunLengthEncode::Encode(v->cub_tmp.p, tb_rle, v->key_sorted.p, v->ukey.p, v->cnt.p, v->n_runs.p, nw, s));
+  AUR_TRY(cudaMemsetAsync(v->dcnt.p, 0, static_cast<size_t>(n) * 4, s));
+  AUR_TRY(cudaMemsetAsync(v->dlen.p, 0, static_cast<size_t>(n) * 4, s));
   tx_postings<<<blocks(nw), kT, 0, s>>>(v->ukey.p, v->cnt.p, v->n_runs.p, v->post.p, v->tid.p, v->dcnt.p, v->dlen.p);
-  TX_TRY(cudaGetLastError());
+  AUR_TRY(cudaGetLastError());
   // the host's share: per document (postings, length), then every posting's term id
-  TX_TRY(cudaMemcpyAsync(out->dcnt.data(), v->dcnt.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, s));
-  TX_TRY(cudaMemcpyAsync(out->dlen.data(), v->dlen.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, s));
-  TX_TRY(cudaStreamSynchronize(s));
+  AUR_TRY(cudaMemcpyAsync(out->dcnt.data(), v->dcnt.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaMemcpyAsync(out->dlen.data(), v->dlen.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaStreamSynchronize(s));
   for (int32_t i = 0; i < n; ++i) out->off[static_cast<size_t>(i) + 1] = out->off[static_cast<size_t>(i)] + out->dcnt[static_cast<size_t>(i)];
   out->total = out->off.back();
   out->tid.resize(static_cast<size_t>(out->total));
   if (out->total) {
-    TX_TRY(cudaMemcpyAsync(out->tid.data(), v->tid.p, static_cast<size_t>(out->total) * 4, cudaMemcpyDeviceToHost, s));
-    TX_TRY(cudaStreamSynchronize(s));
+    AUR_TRY(cudaMemcpyAsync(out->tid.data(), v->tid.p, static_cast<size_t>(out->total) * 4, cudaMemcpyDeviceToHost, s));
+    AUR_TRY(cudaStreamSynchronize(s));
   }
   out->max_term = *std::max_element(out->tid.begin(), out->tid.end());   // nw > 0: at least one posting
   return AUR_OK;
@@ -441,14 +433,14 @@ int publish(aur_kw_vocab* v, aur_kw* const* stores, int ns, const int64_t* ids, 
     }
     sbase[static_cast<size_t>(ns)] = at;
     const int64_t m = static_cast<int64_t>(map.size());
-    TX_TRY(v->gmap.reserve(static_cast<size_t>(m))); TX_TRY(v->goff_dst.reserve(static_cast<size_t>(m)));
-    TX_TRY(v->goff_src.reserve(static_cast<size_t>(n) + 1)); TX_TRY(v->spost.reserve(static_cast<size_t>(r.total)));
-    TX_TRY(cudaMemcpyAsync(v->gmap.p, map.data(), static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, v->stream));
-    TX_TRY(cudaMemcpyAsync(v->goff_dst.p, doff.data(), static_cast<size_t>(m) * 8, cudaMemcpyHostToDevice, v->stream));
-    TX_TRY(cudaMemcpyAsync(v->goff_src.p, r.off.data(), (static_cast<size_t>(n) + 1) * 8, cudaMemcpyHostToDevice, v->stream));
+    AUR_TRY(v->gmap.reserve(static_cast<size_t>(m))); AUR_TRY(v->goff_dst.reserve(static_cast<size_t>(m)));
+    AUR_TRY(v->goff_src.reserve(static_cast<size_t>(n) + 1)); AUR_TRY(v->spost.reserve(static_cast<size_t>(r.total)));
+    AUR_TRY(cudaMemcpyAsync(v->gmap.p, map.data(), static_cast<size_t>(m) * 4, cudaMemcpyHostToDevice, v->stream));
+    AUR_TRY(cudaMemcpyAsync(v->goff_dst.p, doff.data(), static_cast<size_t>(m) * 8, cudaMemcpyHostToDevice, v->stream));
+    AUR_TRY(cudaMemcpyAsync(v->goff_src.p, r.off.data(), (static_cast<size_t>(n) + 1) * 8, cudaMemcpyHostToDevice, v->stream));
     tx_gather<<<blocks(m * 32), kT, 0, v->stream>>>(v->post.p, v->goff_src.p, v->gmap.p, v->goff_dst.p, m, v->spost.p);
-    TX_TRY(cudaGetLastError());
-    TX_TRY(cudaStreamSynchronize(v->stream));
+    AUR_TRY(cudaGetLastError());
+    AUR_TRY(cudaStreamSynchronize(v->stream));
     src = v->spost.p;
   }
   int rc = AUR_OK;
@@ -494,9 +486,9 @@ int aur_kw_vocab_open(int32_t device, aur_kw_vocab** out) {
   if (cudaGetDeviceCount(&ndev) != cudaSuccess) { cudaGetLastError(); ndev = 0; }
   if (ndev == 0) return report_error(AUR_ERR_NO_DEVICE, "no CUDA device: aurora_b200 has no CPU fallback");
   if (device < 0 || device >= ndev) return report_error(AUR_ERR_INVALID, "device %d out of range", device);
-  TX_TRY(cudaSetDevice(device));
+  AUR_TRY(cudaSetDevice(device));
   cudaDeviceProp prop;
-  TX_TRY(cudaGetDeviceProperties(&prop, device));
+  AUR_TRY(cudaGetDeviceProperties(&prop, device));
   if (prop.major != 9) return report_error(AUR_ERR_UNSUPPORTED, "sm_%d%d device: this library is built for sm_90a only", prop.major, prop.minor);
   std::unique_ptr<aur_kw_vocab> v(new aur_kw_vocab());
   v->device = device;
@@ -538,15 +530,15 @@ int aur_kw_vocab_read(aur_kw_vocab* v, int64_t id0, int64_t n, char* bytes_out, 
     return report_error(AUR_ERR_INVALID, "words [%lld, %lld) outside the vocabulary's %lld", (long long)id0, (long long)(id0 + n),
                         (long long)v->words);
   std::vector<int64_t> wo(static_cast<size_t>(n) + 1);
-  TX_TRY(cudaSetDevice(v->device));
-  TX_TRY(cudaMemcpyAsync(wo.data(), v->woff.p + id0, wo.size() * 8, cudaMemcpyDeviceToHost, v->stream));
-  TX_TRY(cudaStreamSynchronize(v->stream));
+  AUR_TRY(cudaSetDevice(v->device));
+  AUR_TRY(cudaMemcpyAsync(wo.data(), v->woff.p + id0, wo.size() * 8, cudaMemcpyDeviceToHost, v->stream));
+  AUR_TRY(cudaStreamSynchronize(v->stream));
   const int64_t nbytes = wo.back() - wo[0];
   if (bytes_out && bytes_cap < nbytes)
     return report_error(AUR_ERR_INVALID, "bytes_cap %lld < %lld bytes", (long long)bytes_cap, (long long)nbytes);
   if (bytes_out && nbytes) {
-    TX_TRY(cudaMemcpyAsync(bytes_out, v->pool.p + wo[0], static_cast<size_t>(nbytes), cudaMemcpyDeviceToHost, v->stream));
-    TX_TRY(cudaStreamSynchronize(v->stream));
+    AUR_TRY(cudaMemcpyAsync(bytes_out, v->pool.p + wo[0], static_cast<size_t>(nbytes), cudaMemcpyDeviceToHost, v->stream));
+    AUR_TRY(cudaStreamSynchronize(v->stream));
   }
   for (int64_t i = 0; i <= n; ++i) offsets_out[i] = wo[static_cast<size_t>(i)] - wo[0];
   return AUR_OK;
@@ -594,7 +586,7 @@ int aur_kw_add_text(aur_kw* const* stores, int32_t n_stores, aur_kw_vocab* v, co
     if (rc != AUR_OK) return rc;
   }
   std::lock_guard<std::mutex> vl(v->mu);
-  TX_TRY(cudaSetDevice(v->device));
+  AUR_TRY(cudaSetDevice(v->device));
   int rc = AUR_OK;
   SliceRows rows;
   std::vector<int64_t> soff;
@@ -604,7 +596,7 @@ int aur_kw_add_text(aur_kw* const* stores, int32_t n_stores, aur_kw_vocab* v, co
     const int32_t m = static_cast<int32_t>(d1 - d0);
     soff.resize(static_cast<size_t>(m) + 1);
     for (int32_t i = 0; i <= m; ++i) soff[static_cast<size_t>(i)] = text_offsets[d0 + i] - text_offsets[d0];
-    TX_TRY(cudaSetDevice(v->device));
+    AUR_TRY(cudaSetDevice(v->device));
     rc = analyse(v, soff[m] ? texts_utf8 + text_offsets[d0] : nullptr, soff.data(), m, &rows);
     if (rc == AUR_OK)
       rc = publish(v, stores, n_stores, ids + d0, user_codes ? user_codes + d0 : nullptr, org_codes ? org_codes + d0 : nullptr,

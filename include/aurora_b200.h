@@ -12,6 +12,8 @@
  * Conventions
  *   - every function returns AUR_OK (0) or a negative aur_status; on failure no output
  *     buffer has been written and aur_last_error() (thread-local) describes why;
+ *   - a device or page-locked allocation that fails is AUR_ERR_NOMEM, any other CUDA failure
+ *     AUR_ERR_CUDA;
  *   - "host" entry points take host pointers and include the H2D / D2H copies;
  *     "_dev" entry points take device pointers on the index's device and a cudaStream_t
  *     passed as void* (NULL = the index's own stream; pass cudaStreamLegacy, (void*)1, for
@@ -162,7 +164,10 @@ int aur_search(aur_index* ix, const void* queries_host, int32_t nq, int32_t k,
 /* Same call, additionally reporting the snapshot it answered from: *snapshot_rows_out = number of
  * appended rows (tombstones included) that were visible to this search.  With a writer appending
  * concurrently (the reference: Celery ingest workers next to gunicorn search threads,
- * docker-compose.yaml:191,283-285) the answer is the top-k of exactly that prefix. */
+ * docker-compose.yaml:191,283-285) the answer is the top-k of exactly that prefix.
+ * A search whose context cannot grow its scratch fails with AUR_ERR_NOMEM, as does every other call on a shard that
+ * runs out of device memory (aur_search_dev, aur_remove, the filter calls and the debug dumps included); earlier
+ * releases reported these allocation failures as AUR_ERR_CUDA. */
 int aur_search_ex(aur_index* ix, const void* queries_host, int32_t nq, int32_t k,
                   const int32_t* q_user, const int32_t* q_org,
                   float* scores_out, int64_t* ids_out, int64_t* snapshot_rows_out);
@@ -536,6 +541,8 @@ typedef struct aur_encoder_stats {
   double  attn_flops;        /* 4 * len^2 * hidden per sequence and layer                  */
 } aur_encoder_stats;
 
+/* Out of device memory (aur_encoder_open, aur_encoder_load, aur_encoder_replicate): AUR_ERR_NOMEM; earlier releases
+ * reported it as AUR_ERR_CUDA. */
 int aur_encoder_open(const aur_encoder_config* cfg, aur_encoder** out);
 int aur_encoder_close(aur_encoder* enc);
 /* Upload one parameter tensor (host fp32; matrices are stored as bf16 on the device).  Names:
