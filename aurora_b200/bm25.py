@@ -219,6 +219,10 @@ class DeviceBM25:
     def __len__(self) -> int:
         return len(self._docs)
 
+    def reserve(self, capacity: int) -> None:
+        """The store's ``reserve``: room for at least ``capacity`` documents."""
+        self.store.reserve(capacity)
+
     def add(self, doc_id: int, text: str, user_code: int = 0, org_code: int = -1) -> None:
         self.add_many([doc_id], [text], [user_code], [org_code])
 

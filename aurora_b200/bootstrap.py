@@ -7,7 +7,7 @@ behind the reference's module API.  Used as the daemon's boot hook:
 
 Variables: AURORA_B200_MODEL (bge-base | bge-large | minilm-l6, default bge-base), AURORA_B200_ENCODER_WEIGHTS
 (HuggingFace BertModel safetensors), AURORA_B200_VOCAB (WordPiece vocab.txt), AURORA_B200_DEVICE (0),
-AURORA_B200_CAPACITY (rows of HBM to reserve, default 1048576), AURORA_B200_DTYPE (row format of the shards: bf16, the
+AURORA_B200_CAPACITY (rows to map in HBM at start, default 1048576; the shards grow as chunks arrive), AURORA_B200_DTYPE (row format of the shards: bf16, the
 default, or int8 for half the HBM), AURORA_B200_SNAPSHOT (directory: restored at
 start when present; see KnowledgeBase.save), AURORA_B200_MAX_TOKENS / AURORA_B200_MAX_SEQS (encoder workspace).
 There is no CPU fallback: without a CUDA device or with a variable missing this raises.

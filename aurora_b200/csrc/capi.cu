@@ -4,6 +4,7 @@
 //   inv_norm  [capacity] f32   1/|row|; 0 for zero rows; NaN marks a tombstone
 //   ids       [capacity] i64   caller ids;  user / org [capacity] i32 tenant codes
 //   attr      up to 16 x [capacity] i32 attribute codes for device-evaluated filters (allocated on first aur_set_attrs)
+// each on a growable virtual-memory mapping (VmmBuf): aur_reserve maps more rows at its end and nothing moves;
 // plus grow-only scratch for candidate lists.  No CPU compute path exists here: without
 // a CUDA device every entry point fails with AUR_ERR_NO_DEVICE.
 //
@@ -29,6 +30,7 @@
 #include <mutex>
 #include <shared_mutex>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <algorithm>
 #include <vector>
@@ -59,9 +61,119 @@ EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
+// The driver's virtual memory management entry points (VmmRange), obtained as cuTensorMapEncodeTiled is.
+struct VmmFns {
+  decltype(&cuMemAddressReserve) reserve = nullptr;
+  decltype(&cuMemAddressFree) free = nullptr;
+  decltype(&cuMemCreate) create = nullptr;
+  decltype(&cuMemRelease) release = nullptr;
+  decltype(&cuMemMap) map = nullptr;
+  decltype(&cuMemUnmap) unmap = nullptr;
+  decltype(&cuMemSetAccess) set_access = nullptr;
+  decltype(&cuMemGetAllocationGranularity) granularity = nullptr;
+  bool ok = false;
+};
+const VmmFns& vmm_fns() {
+  static VmmFns f;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    auto get = [](const char* name, auto* fn) {
+      void* p = nullptr;
+      cudaDriverEntryPointQueryResult qres;
+      if (cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &qres) != cudaSuccess || qres != cudaDriverEntryPointSuccess) {
+        cudaGetLastError();
+        return false;
+      }
+      *fn = reinterpret_cast<std::remove_pointer_t<decltype(fn)>>(p);
+      return true;
+    };
+    f.ok = get("cuMemAddressReserve", &f.reserve) && get("cuMemAddressFree", &f.free) && get("cuMemCreate", &f.create) &&
+           get("cuMemRelease", &f.release) && get("cuMemMap", &f.map) && get("cuMemUnmap", &f.unmap) &&
+           get("cuMemSetAccess", &f.set_access) && get("cuMemGetAllocationGranularity", &f.granularity);
+  });
+  return f;
+}
+cudaError_t vmm_err(CUresult r) {
+  if (r == CUDA_SUCCESS) return cudaSuccess;
+  return r == CUDA_ERROR_OUT_OF_MEMORY ? cudaErrorMemoryAllocation : cudaErrorUnknown;
+}
+CUmemAllocationProp vmm_prop(int device) {
+  CUmemAllocationProp prop{};
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = device;
+  return prop;
+}
+
 }  // namespace
 
 namespace aur {
+cudaError_t vmm_max_rows(size_t row_bytes, size_t* out) {
+  size_t free_b = 0, total_b = 0;
+  AUR_CU_RET(cudaMemGetInfo(&free_b, &total_b));
+  *out = std::min(static_cast<size_t>(kMaxRows), total_b / std::max<size_t>(row_bytes, 1));
+  return cudaSuccess;
+}
+
+cudaError_t VmmRange::open(int device, size_t max_bytes, size_t bytes) {
+  release();
+  const VmmFns& f = vmm_fns();
+  if (!f.ok) return cudaErrorNotSupported;
+  const CUmemAllocationProp prop = vmm_prop(device);
+  size_t g = 0;
+  AUR_CU_RET(vmm_err(f.granularity(&g, &prop, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED)));
+  const size_t want = std::max(max_bytes, bytes);
+  const size_t reserved = (want + g - 1) / g * g;
+  CUdeviceptr b = 0;
+  AUR_CU_RET(vmm_err(f.reserve(&b, reserved, g, 0, 0)));
+  base_ = b; reserved_ = reserved; mapped_ = 0; gran_ = g; device_ = device;
+  const cudaError_t e = grow(bytes);
+  if (e != cudaSuccess) release();
+  return e;
+}
+
+cudaError_t VmmRange::grow(size_t bytes) {
+  bytes = (bytes + gran_ - 1) / gran_ * gran_;
+  if (bytes <= mapped_) return cudaSuccess;
+  if (bytes > reserved_) return cudaErrorMemoryAllocation;   // more than the device could ever hold
+  const VmmFns& f = vmm_fns();
+  const CUmemAllocationProp prop = vmm_prop(device_);
+  const size_t add = bytes - mapped_;
+  const CUdeviceptr at = base_ + mapped_;
+  CUmemGenericAllocationHandle h = 0;
+  AUR_CU_RET(vmm_err(f.create(&h, add, &prop, 0)));
+  CUresult r = f.map(at, add, 0, h, 0);
+  if (r == CUDA_SUCCESS) {
+    CUmemAccessDesc acc{};
+    acc.location = prop.location;
+    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+    r = f.set_access(at, add, &acc, 1);
+    if (r != CUDA_SUCCESS) f.unmap(at, add);
+  }
+  if (r != CUDA_SUCCESS) { f.release(h); return vmm_err(r); }
+  chunks_.push_back(Chunk{h, mapped_, add});
+  mapped_ = bytes;
+  return cudaSuccess;
+}
+
+void VmmRange::shrink_to(size_t bytes) {
+  const VmmFns& f = vmm_fns();
+  while (!chunks_.empty() && chunks_.back().offset >= bytes) {
+    const Chunk c = chunks_.back();
+    f.unmap(base_ + c.offset, c.bytes);
+    f.release(c.handle);
+    chunks_.pop_back();
+    mapped_ = c.offset;
+  }
+}
+
+void VmmRange::release() {
+  if (!base_) return;
+  shrink_to(0);
+  vmm_fns().free(base_, reserved_);
+  base_ = 0; reserved_ = mapped_ = 0;
+}
+
 cudaError_t raise_smem_limit(const void* kern, size_t smem) {
   static std::mutex mu;
   static std::map<std::pair<const void*, int>, size_t> raised;   // (kernel, device) -> limit set so far
@@ -163,18 +275,24 @@ struct aur_index {
   std::mutex mu;                 // host metadata: id2row, live, options, the bound contexts
   std::mutex mu_write;           // one writer at a time (append / remove)
   int device = 0, dim = 0, dtype = 0;
-  int64_t capacity = 0, live = 0;
-  int64_t cap_pad = 0;                // capacity rounded up to a whole tile (TMA boxes never straddle an allocation):
-                                      // the length of every per-row array
+  int64_t live = 0;
+  // capacity, cap_pad and tmap change only in aur_reserve, published together under tmap_mu; a search copies its
+  // tensor map under it (tc_tmap) when it launches.  A lock of its own: an append holds mu over its id bookkeeping,
+  // and a launch does not wait for that.
+  std::mutex tmap_mu;
+  std::atomic<int64_t> capacity{0};
+  std::atomic<int64_t> cap_pad{0};    // capacity rounded up to a whole tile (TMA boxes never straddle an allocation):
+                                      // the rows mapped in every per-row array
   std::atomic<int64_t> rows_pub{0};   // rows visible to searches (published after the data landed)
   size_t elt = 2;                        // bytes per stored row element (int8 rows: 1)
   size_t qelt = 2;                       // bytes per query / input row element (bf16 for bf16 and int8 rows, f32 for f32)
   DevBuf<uint8_t> i8_stage;              // int8 shards: host bf16 rows on their way to the quantizer (writers hold mu_write)
   DevBuf<int32_t> tomb_rows;             // aur_remove: the rows it tombstones, one upload (writers hold mu_write)
-  DevBuf<uint8_t> d_rows;
-  DevBuf<float> d_inv_norm;
-  DevBuf<int64_t> d_ids;
-  DevBuf<int32_t> d_user, d_org;
+  // per-row arrays on growable mappings (aur_reserve): their addresses never change
+  VmmBuf<uint8_t> d_rows;
+  VmmBuf<float> d_inv_norm;
+  VmmBuf<int64_t> d_ids;
+  VmmBuf<int32_t> d_user, d_org;
   AttrColumns attrs;                     // program columns 2.., cap_pad rows each (aur_set_attrs, writers hold mu_write)
   std::unordered_map<int64_t, int64_t> id2row;
   Stream stream;                         // the index's own stream: device-pointer calls with stream == NULL
@@ -196,24 +314,34 @@ struct aur_index {
 
 namespace {
 
-int build_tmaps(aur_index* ix) {
-  ix->tmap_ok = false;
-  const bool i8 = ix->dtype == AUR_I8;
+bool tc_layout(const aur_index* ix) {
   // int8 rows: 128 of them per 128-byte k-block, so the path needs dim % 128 == 0
-  if (ix->dtype == AUR_F32 || ix->dim % (i8 ? kTcKBlockI8 : kTcKBlock) != 0 || ix->dim > kTcMaxDim) return AUR_OK;  // SIMT only
+  return ix->dtype != AUR_F32 && ix->dim % (ix->dtype == AUR_I8 ? kTcKBlockI8 : kTcKBlock) == 0 && ix->dim <= kTcMaxDim;
+}
+
+// The tensor maps of the rows over `capacity` rows into out (nothing for a shape without the tensor-core path).
+int encode_tmaps(const aur_index* ix, int64_t capacity, CUtensorMap (&out)[2][2]) {
+  if (!tc_layout(ix)) return AUR_OK;   // SIMT only
+  const bool i8 = ix->dtype == AUR_I8;
   // rows past the capacity (a tile's tail, a whole half of the last tile of a pair) arrive as zeros
   for (int w = 0; w < 2; ++w)
     for (int g = 1; g <= 2; ++g) {
       const int tile_n = w ? kTcTileWide : kTcTileN;
-      const uint64_t cols = static_cast<uint64_t>(ix->dim), rows = static_cast<uint64_t>(ix->capacity);
+      const uint64_t cols = static_cast<uint64_t>(ix->dim), rows = static_cast<uint64_t>(capacity);
       const uint32_t box_rows = static_cast<uint32_t>(tile_n / g);
-      const int r = i8 ? encode_tmap_2d_u8(&ix->tmap[w][g - 1], ix->d_rows.p, cols, rows, cols, kTcKBlockI8, box_rows)
-                       : encode_tmap_2d_bf16(&ix->tmap[w][g - 1], ix->d_rows.p, cols, rows, cols * 2, kTcKBlock, box_rows);
+      const int r = i8 ? encode_tmap_2d_u8(&out[w][g - 1], ix->d_rows.p, cols, rows, cols, kTcKBlockI8, box_rows)
+                       : encode_tmap_2d_bf16(&out[w][g - 1], ix->d_rows.p, cols, rows, cols * 2, kTcKBlock, box_rows);
       if (r < 0) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled entry point not found");
       if (r != CUDA_SUCCESS) return fail(AUR_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", r);
     }
-  ix->tmap_ok = true;
   return AUR_OK;
+}
+
+// A copy of one tensor map as last published: a launch passes it by value (__grid_constant__), so a launch enqueued
+// before a growth keeps the map of the capacity it was enqueued under.
+CUtensorMap tc_tmap(aur_index* ix, int wide, int cta_group) {
+  std::lock_guard<std::mutex> lk(ix->tmap_mu);
+  return ix->tmap[wide][cta_group - 1];
 }
 
 bool tc_shape_ok(const aur_index* ix, int k, bool filtered) {
@@ -398,7 +526,8 @@ int run_tc_block(aur_index* ix, SearchCtx* c, int cta_group, const void* q_dev, 
   p.num_stages = stages;
   p.dbg_flags = ix->opt_dbg_flags;
   p.n_tiles = static_cast<int>((n_rows + tile_n - 1) / tile_n);
-  AUR_TRY(tc_launch(cta_group, tile_n, qregs, i8, grid, &ix->tmap[tile_n == kTcTileWide][cta_group - 1], p, smem, s));
+  const CUtensorMap tm = tc_tmap(ix, tile_n == kTcTileWide, cta_group);
+  AUR_TRY(tc_launch(cta_group, tile_n, qregs, i8, grid, &tm, p, smem, s));
   c->last_tile_n = tile_n;
   *n_lists_out = n_lists;
   return AUR_OK;
@@ -1059,14 +1188,60 @@ int aur_open(const aur_config* cfg, aur_index** out) {
   AUR_TRY(ix->ingest_stream.create(cudaStreamNonBlocking, prio_lo));
   ix->cap_pad = (cfg->capacity + kTcTileN - 1) / kTcTileN * kTcTileN;
   const size_t cap_pad = static_cast<size_t>(ix->cap_pad);
-  AUR_TRY(ix->d_rows.reserve(cap_pad * ix->dim * ix->elt));
-  AUR_TRY(ix->d_inv_norm.reserve(cap_pad));
-  AUR_TRY(ix->d_ids.reserve(cap_pad));
-  AUR_TRY(ix->d_user.reserve(cap_pad));
-  AUR_TRY(ix->d_org.reserve(cap_pad));
-  int rc = build_tmaps(ix.get());
+  AUR_TRY(ix->d_rows.open(ix->device, static_cast<size_t>(ix->dim) * ix->elt, cap_pad));
+  AUR_TRY(ix->d_inv_norm.open(ix->device, 1, cap_pad));
+  AUR_TRY(ix->d_ids.open(ix->device, 1, cap_pad));
+  AUR_TRY(ix->d_user.open(ix->device, 1, cap_pad));
+  AUR_TRY(ix->d_org.open(ix->device, 1, cap_pad));
+  int rc = encode_tmaps(ix.get(), cfg->capacity, ix->tmap);
   if (rc != AUR_OK) return rc;
+  ix->tmap_ok = tc_layout(ix.get());
   *out = ix.release();
+  return AUR_OK;
+}
+
+int aur_reserve(aur_index* ix, int64_t capacity) {
+  if (!ix) return fail(AUR_ERR_INVALID, "null index");
+  if (capacity > kMaxRows) return fail(AUR_ERR_INVALID, "capacity exceeds int32 row indexing");
+  std::shared_lock<std::shared_mutex> rl(ix->rw);   // a writer: searches and their enqueue go on
+  std::lock_guard<std::mutex> wk(ix->mu_write);
+  const int64_t old_cap = ix->capacity.load(), old_pad = ix->cap_pad.load();
+  if (capacity <= old_cap) return AUR_OK;
+  AUR_TRY(cudaSetDevice(ix->device));
+  const int64_t pad = (capacity + kTcTileN - 1) / kTcTileN * kTcTileN;
+  const size_t rows = static_cast<size_t>(pad);
+  // the maps need only the rows' address, which never changes: encoded before anything grows
+  CUtensorMap tm[2][2];
+  int rc = encode_tmaps(ix, capacity, tm);
+  if (rc != AUR_OK) return rc;
+  // every array maps its new rows at its end, or none keeps them: the shard stays as it was on a failure
+  const size_t b_rows = ix->d_rows.r.mapped(), b_inv = ix->d_inv_norm.r.mapped(), b_ids = ix->d_ids.r.mapped(),
+               b_user = ix->d_user.r.mapped(), b_org = ix->d_org.r.mapped();
+  cudaStream_t s = ix->ingest_stream;
+  cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(ix->d_rows.grow(rows * ix->dim * ix->elt));
+    AUR_CU_RET(ix->d_inv_norm.grow(rows));
+    AUR_CU_RET(ix->d_ids.grow(rows));
+    AUR_CU_RET(ix->d_user.grow(rows));
+    AUR_CU_RET(ix->d_org.grow(rows));
+    // the new rows start absent in the tenant columns, as in the attribute columns
+    AUR_CU_RET(cudaMemsetAsync(ix->d_user.p + old_pad, 0xFF, static_cast<size_t>(pad - old_pad) * 4, s));
+    AUR_CU_RET(cudaMemsetAsync(ix->d_org.p + old_pad, 0xFF, static_cast<size_t>(pad - old_pad) * 4, s));
+    AUR_CU_RET(cudaStreamSynchronize(s));
+    return ix->attrs.grow(old_pad, pad, s);   // (rolls its own columns back on a failure)
+  }();
+  if (e != cudaSuccess) {
+    cudaStreamSynchronize(s);   // a tail memset may still be pending: nothing is unmapped under it
+    cudaGetLastError();
+    ix->d_rows.shrink_to_bytes(b_rows); ix->d_inv_norm.shrink_to_bytes(b_inv); ix->d_ids.shrink_to_bytes(b_ids);
+    ix->d_user.shrink_to_bytes(b_user); ix->d_org.shrink_to_bytes(b_org);
+    return fail(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "aur_reserve(%lld): %s (the shard keeps %lld rows)",
+                (long long)capacity, cudaGetErrorString(e), (long long)old_cap);
+  }
+  std::lock_guard<std::mutex> lk(ix->tmap_mu);
+  if (ix->tmap_ok) memcpy(ix->tmap, tm, sizeof tm);
+  ix->cap_pad.store(pad);
+  ix->capacity.store(capacity);
   return AUR_OK;
 }
 
@@ -1381,7 +1556,7 @@ int aur_set_attrs(aur_index* ix, int32_t col, const int64_t* ids, const int32_t*
   std::vector<int32_t> pairs;
   pairs.reserve(2 * static_cast<size_t>(n));
   resolve_ids(ix, ids, n, INT64_MAX, [&](int64_t i, int32_t row) { pairs.push_back(row); pairs.push_back(codes[i]); });
-  return ix->attrs.write(col, pairs, ix->cap_pad, ix->ingest_stream);   // padded, like the tenant codes
+  return ix->attrs.write(col, pairs, ix->cap_pad.load(), ix->ingest_stream);   // padded, like the tenant codes
 }
 
 int aur_search_filtered(aur_index* ix, const void* queries_host, int32_t nq, int32_t k, const int32_t* prog,

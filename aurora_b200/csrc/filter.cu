@@ -268,8 +268,10 @@ int AttrColumns::write(int32_t col, const std::vector<int32_t>& pairs, int64_t r
   if (col < 2 || col >= kFiltCols) return report_error(AUR_ERR_INVALID, "attribute columns are 2 .. %d", kFiltCols - 1);
   const cudaError_t e = [&]() -> cudaError_t {
     if (!d_attr[col - 2].p) {   // (writes are serialised: only this call stores a column)
-      DevBuf<int32_t> a;
-      AUR_CU_RET(a.reserve(static_cast<size_t>(rows)));
+      int dev = 0;
+      AUR_CU_RET(cudaGetDevice(&dev));
+      VmmBuf<int32_t> a;
+      AUR_CU_RET(a.open(dev, 1, static_cast<size_t>(rows)));
       AUR_CU_RET(cudaMemsetAsync(a.p, 0xFF, static_cast<size_t>(rows) * 4, s));
       AUR_CU_RET(cudaStreamSynchronize(s));
       std::lock_guard<std::mutex> lk(mu);
@@ -287,10 +289,29 @@ int AttrColumns::write(int32_t col, const std::vector<int32_t>& pairs, int64_t r
   return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "attribute column: %s", cudaGetErrorString(e));
 }
 
-bool AttrColumns::any() { return std::any_of(std::begin(d_attr), std::end(d_attr), [](const DevBuf<int32_t>& a) { return a.p != nullptr; }); }
+bool AttrColumns::any() { return std::any_of(std::begin(d_attr), std::end(d_attr), [](const VmmBuf<int32_t>& a) { return a.p != nullptr; }); }
+
+cudaError_t AttrColumns::grow(int64_t old_rows, int64_t rows, cudaStream_t s) {
+  size_t before[kFiltAttrCols] = {};
+  for (int i = 0; i < kFiltAttrCols; ++i) before[i] = d_attr[i].r.mapped();
+  const cudaError_t e = [&]() -> cudaError_t {
+    for (VmmBuf<int32_t>& a : d_attr) {
+      if (!a.p || rows <= old_rows) continue;
+      AUR_CU_RET(a.grow(static_cast<size_t>(rows)));
+      AUR_CU_RET(cudaMemsetAsync(a.p + old_rows, 0xFF, static_cast<size_t>(rows - old_rows) * 4, s));
+    }
+    return cudaStreamSynchronize(s);
+  }();
+  if (e != cudaSuccess) {
+    cudaStreamSynchronize(s);   // a tail memset may still be pending: nothing is unmapped under it
+    cudaGetLastError();
+    for (int i = 0; i < kFiltAttrCols; ++i) d_attr[i].shrink_to_bytes(before[i]);
+  }
+  return e;
+}
 
 cudaError_t AttrColumns::gather(const int32_t* map, int64_t m, int64_t dst0, int32_t* bounce, cudaStream_t s) {
-  for (const DevBuf<int32_t>& a : d_attr) {
+  for (const VmmBuf<int32_t>& a : d_attr) {
     if (!a.p || m <= 0) continue;
     gather_i32_kernel<<<blocks_of(m, 256), 256, 0, s>>>(a.p, map, m, bounce);
     AUR_CU_RET(cudaGetLastError());
@@ -300,7 +321,7 @@ cudaError_t AttrColumns::gather(const int32_t* map, int64_t m, int64_t dst0, int
 }
 
 cudaError_t AttrColumns::clear(int64_t r0, int64_t r1, cudaStream_t s) {
-  for (const DevBuf<int32_t>& a : d_attr)
+  for (const VmmBuf<int32_t>& a : d_attr)
     if (a.p && r1 > r0) AUR_CU_RET(cudaMemsetAsync(a.p + r0, 0xFF, static_cast<size_t>(r1 - r0) * 4, s));
   return cudaSuccess;
 }

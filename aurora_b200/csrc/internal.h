@@ -365,6 +365,72 @@ struct DevBuf {   // grow-only device scratch
   }
   void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
 };
+// A device array that grows without moving (CUDA virtual memory management): open() reserves an address range for the
+// most bytes it may ever hold and maps physical memory over its first `bytes`; grow() maps more at the end.  Every
+// growth is one physical allocation, so shrink_to() a size the range had before unmaps exactly the later ones.  Only
+// the owning device has access; the range is never exported or peer-mapped.  Failures come back as cudaError_t
+// (cudaErrorMemoryAllocation when the device or the reserved range has no room) and leave the range as it was.
+class VmmRange {
+ public:
+  VmmRange() = default;
+  VmmRange(const VmmRange&) = delete;
+  VmmRange& operator=(const VmmRange&) = delete;
+  VmmRange(VmmRange&& o) noexcept { *this = std::move(o); }
+  VmmRange& operator=(VmmRange&& o) noexcept {
+    if (this != &o) {
+      release();
+      base_ = o.base_; reserved_ = o.reserved_; mapped_ = o.mapped_; gran_ = o.gran_; device_ = o.device_;
+      chunks_ = std::move(o.chunks_);
+      o.base_ = 0; o.reserved_ = o.mapped_ = 0; o.chunks_.clear();
+    }
+    return *this;
+  }
+  ~VmmRange() { release(); }
+  cudaError_t open(int device, size_t max_bytes, size_t bytes);
+  cudaError_t grow(size_t bytes);        // to at least `bytes` mapped
+  void shrink_to(size_t bytes);          // back to a mapped size the range had before
+  void* base() const { return reinterpret_cast<void*>(base_); }
+  size_t mapped() const { return mapped_; }
+ private:
+  void release();
+  unsigned long long base_ = 0;
+  size_t reserved_ = 0, mapped_ = 0, gran_ = 0;
+  int device_ = 0;
+  struct Chunk { unsigned long long handle; size_t offset, bytes; };
+  std::vector<Chunk> chunks_;            // in address order
+};
+constexpr int64_t kMaxRows = 0x7FFFFFC0ll;   // rows of a shard or keyword store: every row index fits an int32
+// The most rows of row_bytes each that the current device's memory could hold, at most kMaxRows: the address room of a
+// per-row array, so that it can grow as far as the device lets it without moving.
+cudaError_t vmm_max_rows(size_t row_bytes, size_t* out);
+// A per-row array on a VmmRange: n elements mapped at p, which never changes once open() succeeded.
+template <typename T>
+struct VmmBuf {
+  T* p = nullptr; size_t n = 0;
+  VmmRange r;
+  VmmBuf() = default;
+  VmmBuf(VmmBuf&& o) noexcept : p(o.p), n(o.n), r(std::move(o.r)) { o.p = nullptr; o.n = 0; }
+  VmmBuf& operator=(VmmBuf&& o) noexcept {
+    if (this != &o) { r = std::move(o.r); p = o.p; n = o.n; o.p = nullptr; o.n = 0; }
+    return *this;
+  }
+  // row_elems elements a row; address room for vmm_max_rows of them, `rows` mapped.  The device is current.
+  cudaError_t open(int device, size_t row_elems, size_t rows) {
+    const size_t rb = row_elems * sizeof(T);
+    size_t max_rows = 0;
+    cudaError_t e = vmm_max_rows(rb, &max_rows);
+    if (e == cudaSuccess) e = r.open(device, std::max(max_rows, rows) * rb, rows * rb);
+    if (e == cudaSuccess) { p = static_cast<T*>(r.base()); n = r.mapped() / sizeof(T); }
+    return e;
+  }
+  cudaError_t grow(size_t want) {   // to at least `want` elements
+    const cudaError_t e = r.grow(want * sizeof(T));
+    n = r.mapped() / sizeof(T);
+    return e;
+  }
+  void shrink_to_bytes(size_t bytes) { r.shrink_to(bytes); n = r.mapped() / sizeof(T); }
+};
+
 template <typename T>
 struct HostBuf {  // grow-only page-locked host buffer; flags: cudaHostAlloc's, per call site
   T* p = nullptr; size_t n = 0;
@@ -493,13 +559,16 @@ class CtxPool {
 
 // ---------------------------------------------------------------- filter columns and uploads, host side (filter.cu)
 // The attribute columns of a vector shard or a keyword store (program columns 2..): `rows` int32 codes each, -1 =
-// absent.  A column only goes from unallocated to allocated.  write, any, gather and clear are the holder's writes,
-// serialised by its writers' lock; mu guards the columns write stores against check and fill.
+// absent.  A column only goes from unallocated to allocated, and grows in place (VmmBuf): its address never changes.
+// write, any, grow, gather and clear are the holder's writes, serialised by its writers' lock; mu guards the columns
+// write stores against check and fill.
 class AttrColumns {
  public:
   // pairs (row, code) into column col (2 .. kFiltCols - 1), waited for; the first write allocates it, all -1.
   int write(int32_t col, const std::vector<int32_t>& pairs, int64_t rows, cudaStream_t s);
   bool any();
+  // Every set column from old_rows to rows, the new rows -1, waited for; on a failure every column is as it was.
+  cudaError_t grow(int64_t old_rows, int64_t rows, cudaStream_t s);
   // Compaction, every set column: rows map[0 .. m) to rows [dst0, dst0 + m) through bounce [m]; rows [r0, r1) to -1.
   cudaError_t gather(const int32_t* map, int64_t m, int64_t dst0, int32_t* bounce, cudaStream_t s);
   cudaError_t clear(int64_t r0, int64_t r1, cudaStream_t s);
@@ -507,7 +576,7 @@ class AttrColumns {
   void fill(FiltParams* p);                             // p->cols[2 ..]
  private:
   std::mutex mu;
-  DevBuf<int32_t> d_attr[kFiltAttrCols];
+  VmmBuf<int32_t> d_attr[kFiltAttrCols];
   DevBuf<int32_t> stage;
 };
 // Checked programs into stage on s in one upload (pageable: staged on return), and *p reading them over the holder's

@@ -454,7 +454,7 @@ struct aur_kw {
   std::mutex mu_last;        // the last search's statistics (last_*)
   int device = 0, sm_count = 0;
   size_t smem_optin = 0;
-  int64_t capacity = 0;
+  std::atomic<int64_t> capacity{0};   // document rows; grows under mu_write and the exclusive lock (aur_kw_reserve)
   Stream stream;
   // device
   DevBuf<int64_t> d_off; DevBuf<int32_t> d_len; DevBuf<int64_t> d_ids;
@@ -1165,7 +1165,7 @@ int kw_check_room(aur_kw* kw, int64_t n) {
   const int64_t base = static_cast<int64_t>(kw->h_len.size());
   if (base + n > kw->capacity)
     return report_error(AUR_ERR_NOMEM, "keyword store full: %lld + %lld > capacity %lld (aur_kw_compact reclaims tombstones)",
-                        (long long)base, (long long)n, (long long)kw->capacity);
+                        (long long)base, (long long)n, (long long)kw->capacity.load());
   return AUR_OK;
 }
 
@@ -1368,7 +1368,36 @@ int aur_kw_set_attrs(aur_kw* kw, int32_t col, const int64_t* ids, const int32_t*
     auto it = kw->id2row.find(ids[i]);
     if (it != kw->id2row.end()) { pairs.push_back(static_cast<int32_t>(it->second)); pairs.push_back(codes[i]); }
   }
-  return kw->attrs.write(col, pairs, kw->capacity, kw->stream);   // the store's capacity, like its tenant codes
+  return kw->attrs.write(col, pairs, kw->capacity.load(), kw->stream);   // the store's capacity, like its tenant codes
+}
+
+int aur_kw_reserve(aur_kw* kw, int64_t doc_capacity) {
+  if (!kw) return report_error(AUR_ERR_INVALID, "null store");
+  if (doc_capacity > kKwMaxRows) return report_error(AUR_ERR_INVALID, "doc_capacity exceeds 2^31 - 64");
+  std::lock_guard<std::mutex> wk(kw->mu_write);
+  const int64_t old_cap = kw->capacity.load();
+  if (doc_capacity <= old_cap) return AUR_OK;
+  // the per-document arrays move: every keyword search is a host call under the shared lock, so none holds them now
+  std::unique_lock<std::shared_mutex> xl(kw->rw);
+  AUR_TRY(cudaSetDevice(kw->device));
+  const size_t cap = static_cast<size_t>(doc_capacity), used = kw->h_len.size();
+  cudaStream_t st = kw->stream;
+  const cudaError_t e = [&]() -> cudaError_t {
+    AUR_CU_RET(kw->d_off.grow_keep(cap + 1, used + 1, st));
+    AUR_CU_RET(kw->d_len.grow_keep(cap, used, st));
+    AUR_CU_RET(kw->d_ids.grow_keep(cap, used, st));
+    AUR_CU_RET(kw->d_user.grow_keep(cap, used, st));
+    AUR_CU_RET(kw->d_org.grow_keep(cap, used, st));
+    AUR_CU_RET(kw->d_live.grow_keep(cap, used, st));
+    return kw->attrs.grow(old_cap, doc_capacity, st);
+  }();
+  if (e != cudaSuccess)   // arrays that did grow keep their rows and the old capacity still holds
+    return report_error(e == cudaErrorMemoryAllocation ? AUR_ERR_NOMEM : AUR_ERR_CUDA, "aur_kw_reserve(%lld): %s (the store keeps %lld rows)",
+                        (long long)doc_capacity, cudaGetErrorString(e), (long long)old_cap);
+  kw->h_off.reserve(cap + 1); kw->h_len.reserve(cap); kw->h_ids.reserve(cap);
+  kw->h_user.reserve(cap); kw->h_org.reserve(cap); kw->h_live.reserve(cap);
+  kw->capacity.store(doc_capacity);
+  return AUR_OK;
 }
 
 int aur_kw_search(aur_kw* kw, const int32_t* q_terms, const int64_t* q_offsets, int32_t nq, int32_t k, const int32_t* q_user,

@@ -151,6 +151,7 @@ class Index:
         dtype = _DTYPE_NAMES[int(z["dtype"])]
         ix = cls(int(z["dim"]), int(capacity or z["capacity"]), dtype=dtype, device=device)
         if len(z["ids"]):
+            grow_for(ix, z["ids"])
             ix.add(_snapshot_rows(z), z["ids"], z["user"], z["org"])
         return ix
 
@@ -190,6 +191,12 @@ class Index:
         freed = C.c_int64(0)
         N.check(self._lib.aur_compact(self._h, C.byref(freed)))
         return int(freed.value)
+
+    def reserve(self, capacity: int) -> None:
+        """Grow the shard to at least ``capacity`` rows in place, while it serves (aur_reserve): rows and device pointers
+        stay where they are.  A smaller value does nothing."""
+        N.check(self._lib.aur_reserve(self._h, int(capacity)))
+        self.capacity = max(self.capacity, int(capacity))
 
     def search_subset(self, queries: np.ndarray, k: int, allow_ids: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
         """Search restricted to the rows whose ids are listed (a resolved metadata pre-filter): the other rows'
@@ -377,6 +384,30 @@ def shard_capacity(capacity: int, n: int) -> int:
     return per + max(64, per // 8)
 
 
+GROW_STEP = 1 << 16   # rows: growth maps or copies only what it adds, so there is nothing to amortise with larger steps
+
+
+def grow_for(holder, ids) -> None:
+    """Make room for one appended row per id in ``holder``: an ``Index`` or ``KeywordIndex``, or the shards / stores
+    of a ``MultiIndex`` / ``MultiKeywordIndex``, each receiving the ids placed on it by ``id mod n``.  A part whose rows
+    appended so far plus its share exceed its capacity grows to that need rounded up to ``GROW_STEP``.  Parts without
+    ``reserve`` (the CPU doubles) are left alone: their add raises when they are full."""
+    parts = getattr(holder, "shards", None) or getattr(holder, "stores", None) or [holder]
+    ids = np.asarray(ids, dtype=np.int64).reshape(-1)
+    share = np.bincount(np.mod(ids, len(parts)), minlength=len(parts)) if len(ids) else np.zeros(len(parts), np.int64)
+    grew = False
+    for part, m in zip(parts, share):
+        if not m or not hasattr(part, "reserve"):
+            continue
+        st = part.stats()
+        need = int(st["rows"] if "rows" in st else st["docs"]) + int(m)
+        if need > part.capacity:
+            part.reserve(-(-need // GROW_STEP) * GROW_STEP)
+            grew = True
+    if grew and len(parts) > 1:
+        holder.capacity = max(holder.capacity, sum(int(p.capacity) for p in parts))
+
+
 class MultiIndex:
     """One process, one shard per GPU of the host (the daemon's deployment on an 8-GPU box): the corpus is row-sharded
     by ``id mod n`` -- an upsert or a delete always lands on the shard that holds the old row -- every search runs on
@@ -497,6 +528,12 @@ class MultiIndex:
     def compact(self) -> int:
         return int(sum(self._each(lambda s, shard: shard.compact())))
 
+    def reserve(self, capacity: int) -> None:
+        """Grow to a total of at least ``capacity`` rows: every shard to its ``shard_capacity`` share, in place."""
+        per = shard_capacity(capacity, len(self.shards))
+        self._each(lambda s, shard: shard.reserve(per))
+        self.capacity = max(self.capacity, int(capacity))
+
     def sync(self) -> None:
         self._each(lambda s, shard: shard.sync())
 
@@ -515,6 +552,7 @@ class MultiIndex:
         dtype = _DTYPE_NAMES[int(z["dtype"])]
         mi = cls(int(z["dim"]), int(capacity or z["capacity"]), devices=devices, dtype=dtype, shard_factory=shard_factory)
         if len(z["ids"]):
+            grow_for(mi, z["ids"])
             mi.add(_snapshot_rows(z), z["ids"], z["user"], z["org"])
         return mi
 
@@ -576,6 +614,11 @@ class KeywordIndex:
         freed = C.c_int64(0)
         N.check(self._lib.aur_kw_compact(self._h, C.byref(freed)))
         return int(freed.value)
+
+    def reserve(self, capacity: int) -> None:
+        """Grow the store to at least ``capacity`` documents (aur_kw_reserve); waits for searches in flight."""
+        N.check(self._lib.aur_kw_reserve(self._h, int(capacity)))
+        self.capacity = max(self.capacity, int(capacity))
 
     def stats(self) -> dict:
         st = N.AurKwStats()
@@ -861,6 +904,12 @@ class MultiKeywordIndex:
 
     def compact(self) -> int:
         return int(sum(self._each(lambda s, store: store.compact())))
+
+    def reserve(self, capacity: int) -> None:
+        """Grow to a total of at least ``capacity`` documents: every store to its ``shard_capacity`` share."""
+        per = shard_capacity(capacity, len(self.stores))
+        self._each(lambda s, store: store.reserve(per))
+        self.capacity = max(self.capacity, int(capacity))
 
     def stats(self) -> dict:
         """KeywordIndex.stats summed over the stores (the last search: launches and spills summed, terms and device time

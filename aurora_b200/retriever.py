@@ -284,6 +284,7 @@ class KnowledgeBase:
                 ids[i] = self._key2id[key]
             ucode = np.full(len(objs), self._code(self._user_code, user_id, True), dtype=np.int32)
             ocode = np.full(len(objs), self._code(self._org_code, org_id, True), dtype=np.int32)
+            self._make_room(ids)
             if fused:
                 self.encoder.encode_append(self.index, texts, ids, ucode, ocode)
             else:
@@ -306,6 +307,16 @@ class KnowledgeBase:
             self.mutations += len(objs)
             self._log({"op": "put", "gen": gen, "user": user_id, "org": org_id, "objs": [list(o) for o in objs]})
         return len(objs)
+
+    def _make_room(self, ids: np.ndarray) -> None:
+        """Grow every vector shard and keyword store that lacks room for these ids' rows before anything is appended,
+        so the store keeps accepting chunks past the capacity it opened with (``engine.grow_for``)."""
+        from .engine import grow_for
+
+        grow_for(self.index, ids)
+        store = getattr(self.sparse, "store", None) if self._kw_device else None
+        if store is not None:
+            grow_for(store, ids)
 
     def _tenant_scope(self, user_id: Optional[str], org_id: Optional[str]):
         """(set, ascending int64 array) of the ids a tenant sees (its user's rows OR its org's), kept until the next
@@ -660,6 +671,9 @@ class KnowledgeBase:
                 kb.sparse.add(rid, text_of(p))
         if kb._kw_device and kb._props:     # one device append for the whole store
             rids = list(kb._props)
+            from .engine import grow_for
+
+            grow_for(kb.sparse.store, rids)   # (the index loader made room for the vectors it added)
             kb.sparse.add_many(rids, [text_of(kb._props[r]) for r in rids],
                                np.array([kb._code(kb._user_code, kb._props[r].get("user_id"), False) for r in rids], np.int32),
                                np.array([kb._code(kb._org_code, kb._props[r].get("org_id"), False) for r in rids], np.int32))
@@ -764,8 +778,8 @@ _state_lock = threading.Lock()
 
 def configure(encoder=None, capacity: Optional[int] = None, device: Optional[int] = None, index_factory=None,
               factory: Optional[Callable[[], KnowledgeBase]] = None, dtype: Optional[str] = None) -> None:
-    """Install the backend.  Environment: AURORA_B200_CAPACITY, AURORA_B200_DEVICE, AURORA_B200_DTYPE (the shard's row
-    format: bf16, the default, or int8)."""
+    """Install the backend.  Environment: AURORA_B200_CAPACITY (the initial capacity: the shards grow as chunks arrive),
+    AURORA_B200_DEVICE, AURORA_B200_DTYPE (the shard's row format: bf16, the default, or int8)."""
     global _kb, _kb_factory
     with _state_lock:
         _kb = None

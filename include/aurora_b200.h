@@ -78,7 +78,7 @@ typedef struct aur_config {
   int32_t dim;        /* vector dimension                                           */
   int32_t dtype;      /* aur_dtype                                                  */
   int32_t reserved;
-  int64_t capacity;   /* rows of HBM to reserve for this shard (grow = reopen)      */
+  int64_t capacity;   /* rows to map in HBM when the shard opens; aur_reserve grows it */
 } aur_config;
 
 typedef struct aur_stats {
@@ -143,6 +143,17 @@ int aur_read_rows(aur_index* ix, int64_t row0, int64_t n, void* rows_out, int64_
  * aur_stats.rows drops to aur_stats.live.  Exclusive: waits for in-flight searches.  *reclaimed
  * (nullable) receives the number of rows freed. */
 int aur_compact(aur_index* ix, int64_t* reclaimed);
+
+/* Grows the shard to at least `capacity` rows, in place.  Existing rows, ids, tenant codes, attribute codes and
+ * tombstones stay where they are.  No device pointer of the shard changes, and neither a search in flight nor a
+ * captured CUDA graph is affected.  New rows start absent in every attribute column.
+ *   capacity <= current: AUR_OK, nothing done.
+ *   > 0x7FFFFFC0 (the int32 row limit aur_open enforces), or null: AUR_ERR_INVALID.
+ *   Out of device memory: AUR_ERR_NOMEM, and the shard is unchanged and still serving.
+ * Every per-row array of a shard lives on a CUDA virtual-memory mapping whose address range, reserved at aur_open,
+ * could hold as many rows as the device's memory; growth maps more physical memory at its end.  Serialised with the
+ * writers; searches go on meanwhile.  aur_stats.capacity reports the new value.  aur_add still fails when full. */
+int aur_reserve(aur_index* ix, int64_t capacity);
 
 /* Deletes by id: the rows of the live ids among ids[0, n) become tombstones (one upload of their rows, one kernel
  * launch).  *removed receives how many ids were live.  aur_remove_filtered deletes by filter without naming ids. */
@@ -319,7 +330,7 @@ typedef struct aur_kw aur_kw;
 typedef struct aur_kw_stats {
   int64_t docs;               /* rows ever appended (including tombstones)          */
   int64_t live;               /* documents visible to search (N)                    */
-  int64_t capacity;           /* document rows reserved at open                     */
+  int64_t capacity;           /* document rows reserved (at open, then aur_kw_reserve) */
   int64_t postings_used;      /* postings of the appended rows                      */
   int64_t postings_allocated; /* posting slots in HBM (grows on demand)             */
   int64_t total_len;          /* tokens over the live documents                     */
@@ -330,10 +341,14 @@ typedef struct aur_kw_stats {
                                  memory and lived in global memory instead          */
 } aur_kw_stats;
 
-/* Lifecycle; the keyword half of _ensure_collection (weaviate_client.py:35-133).  postings_capacity 0 = 2^20 to start
- * with.  Without a device: AUR_ERR_NO_DEVICE. */
+/* Lifecycle; the keyword half of _ensure_collection (weaviate_client.py:35-133).  doc_capacity: document rows to start
+ * with (aur_kw_reserve grows them); postings_capacity 0 = 2^20 to start with.  Without a device: AUR_ERR_NO_DEVICE. */
 int aur_kw_open(int32_t device, int64_t doc_capacity, int64_t postings_capacity, aur_kw** out);
 int aur_kw_close(aur_kw* kw);
+/* aur_reserve's contract, for documents: grows the store to at least doc_capacity documents.  Its per-document arrays
+ * are copied into larger ones under the exclusive lock, as posting growth is, so it waits for searches in flight; rows,
+ * postings, the term-major index and the BM25 statistics are unchanged.  aur_kw_add still fails when full. */
+int aur_kw_reserve(aur_kw* kw, int64_t doc_capacity);
 /* Upsert n documents (the text side of add_object, weaviate_client.py:167-186): document i has postings
  * [offsets[i], offsets[i + 1]) of term_ids / tfs, term ids strictly increasing (0 .. 2^28 - 1), tf >= 1; an existing id
  * loses its old row (weaviate_client.py:172).  user_codes / org_codes as for aur_add (NULL: user 0, org -1). */
@@ -586,7 +601,7 @@ int aur_encoder_replicate(aur_encoder* src, int32_t device, aur_encoder** out);
  * whose configurations (all but the device) differ or with a parameter missing, an encoder on another device than its
  * shard, an f32 shard or one whose dim is not the hidden size, per-call limits outside 0 .. the workspace, an id < 0, a
  * sequence of length outside 1 .. max_pos, a token id outside the vocabulary (AUR_ERR_INVALID); a sequence longer than
- * one call's token budget, a shard without room for its share (rows appended + share > capacity) (AUR_ERR_NOMEM).  A
+ * one call's token budget, a shard without room for its share (rows appended + share > the capacity at the call) (AUR_ERR_NOMEM).  A
  * concurrent writer of the same shard may still use up its room: that shard's append then fails as aur_add_dev fails.
  * A failure after device work has started (a CUDA error) may leave a prefix of some shards' shares appended, whole
  * batches each; aur_last_error names the first failing shard.  aur_encode_append is this call with n = 1 after its
