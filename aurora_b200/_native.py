@@ -35,7 +35,7 @@ EXPORTS = [
     "aur_kw_vocab_set_option", "aur_kw_add_text",
     "aur_hybrid_search", "aur_hybrid_search_multi", "aur_hybrid_search_filtered",
     "aur_encoder_open", "aur_encoder_close", "aur_encoder_load", "aur_encode", "aur_encode_append",
-    "aur_encoder_replicate", "aur_encode_append_multi", "aur_encode_texts", "aur_encode_append_texts_multi", "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
+    "aur_encoder_replicate", "aur_encode_append_multi", "aur_encode_texts", "aur_encode_pair_cosines", "aur_encode_append_texts_multi", "aur_encoder_get_stats", "aur_tokenizer_open", "aur_tokenizer_open_mem", "aur_tokenizer_close", "aur_tokenizer_info",
     "aur_tokenize", "aur_tokenize_windows", "aur_encode_text_append", "aur_debug_gemm", "aur_debug_attention", "aur_debug_encoder_hidden",
 ]
 
@@ -180,6 +180,7 @@ def load():
         "aur_encoder_replicate": (C.c_int, [vp, i32, C.POINTER(vp)]),
         "aur_encode_append_multi": (C.c_int, [vp, vp, i32, vp, vp, i32, vp, vp, vp, i32, i32]),
         "aur_encode_texts": (C.c_int, [vp, vp, vp, i32, vp, i32, vp, vp]),
+        "aur_encode_pair_cosines": (C.c_int, [vp, vp, vp, i32, vp, i32, vp, vp, i64, i32, vp, vp]),
         "aur_encode_append_texts_multi": (C.c_int, [vp, vp, i32, vp, vp, i32, vp, i32, vp, vp, vp, i32, i32]),
         "aur_encoder_get_stats": (C.c_int, [vp, C.POINTER(AurEncoderStats)]),
         "aur_tokenizer_open": (C.c_int, [C.c_char_p, i32, C.POINTER(vp)]),

@@ -34,7 +34,7 @@ def _model_config(name: str):
 
 def configure_from_env() -> None:
     from . import retriever
-    from .encoder import Encoder, TextEncoder, from_hf_bert, read_safetensors
+    from .encoder import EmbeddingClient, Encoder, TextEncoder, configure_embedding_client, from_hf_bert, read_safetensors
     from .wordpiece import NativeTokenizer
 
     missing = [v for v in ("AURORA_B200_ENCODER_WEIGHTS", "AURORA_B200_VOCAB") if not os.environ.get(v)]
@@ -51,6 +51,8 @@ def configure_from_env() -> None:
     if tok.vocab_size != cfg.vocab:
         raise RuntimeError(f"vocabulary has {tok.vocab_size} entries, the model expects {cfg.vocab}")
     text_encoder = TextEncoder(enc, tok, max_len=cfg.max_pos)
+    # the correlation path's embedding client (daemon ops embed / embed_batch / similarity_scores) on the same encoder
+    configure_embedding_client(lambda: EmbeddingClient(enc, lambda text: tok.encode(text, cfg.max_pos)))
     snap = os.environ.get("AURORA_B200_SNAPSHOT")
     wal = os.environ.get("AURORA_B200_WAL", "1") != "0"      # mutation log beside the snapshot (replayed after a crash)
 

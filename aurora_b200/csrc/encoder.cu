@@ -354,6 +354,54 @@ int encode_texts(aur_encoder* e, const Texts& in, int32_t n_seq, int32_t n_texts
   return AUR_OK;
 }
 
+// aur_encode_pair_cosines after aur_encode_texts' own checks, with n_texts > 0: every text through e's whole workspace
+// as encode_texts runs it, each batch's fp32 text rows copied device to device into this call's vecs [n_texts, hidden]
+// (per call: run_texts drops e's lock between batches, so nothing of e's may hold them across batches).  The sink of the
+// batch that finishes the last text uploads the pairs, launches cosine_gather_kernel and copies the cosines (and the
+// vectors) back, all on e's stream before that batch's synchronise.  Outputs are staged and written only on success.
+int pair_cosines(aur_encoder* e, const Texts& in, int32_t n_seq, int32_t n_texts, const int32_t* pair_a,
+                 const int32_t* pair_b, int64_t n_pairs, int32_t clamp, double* cos_out, float* vec_out) {
+  int rc = check_texts(e->cfg, in, n_seq, n_texts, e->cfg.max_tokens);
+  if (rc != AUR_OK) return rc;
+  for (int64_t p = 0; p < n_pairs; ++p)
+    if (pair_a[p] < 0 || pair_a[p] >= n_texts || pair_b[p] < 0 || pair_b[p] >= n_texts)
+      return report_error(AUR_ERR_INVALID, "pair %lld is (%d, %d): indices must be in 0 .. %d", static_cast<long long>(p),
+                          pair_a[p], pair_b[p], n_texts - 1);
+  if (n_pairs == 0 && !vec_out) return AUR_OK;
+  const size_t H = e->cfg.hidden, np = static_cast<size_t>(n_pairs);
+  AUR_TRY(cudaSetDevice(e->cfg.device));
+  DevBuf<float> d_vec;
+  DevBuf<int32_t> d_pairs;   // pair_a, then pair_b
+  DevBuf<double> d_cos;
+  AUR_TRY(d_vec.reserve(static_cast<size_t>(n_texts) * H));
+  AUR_TRY(d_pairs.reserve(2 * np));
+  AUR_TRY(d_cos.reserve(np));
+  std::vector<double> cos_h(np);
+  std::vector<float> vec_h(vec_out ? static_cast<size_t>(n_texts) * H : 0);
+  std::vector<int32_t> q(static_cast<size_t>(n_texts));
+  for (int32_t j = 0; j < n_texts; ++j) q[j] = j;
+  rc = run_texts(e, in, q.data(), n_texts, e->cfg.max_tokens, e->cfg.max_seqs,
+                 [&](aur_encoder* enc, const int32_t* qs, int n, const float* rows) -> int {
+                   cudaStream_t s = enc->stream;
+                   AUR_TRY(cudaMemcpyAsync(d_vec.p + static_cast<size_t>(qs[0]) * H, rows, static_cast<size_t>(n) * H * sizeof(float),
+                                           cudaMemcpyDeviceToDevice, s));
+                   if (qs[n - 1] != n_texts - 1) return AUR_OK;   // texts finish in order: the last one is the call's end
+                   if (np > 0) {
+                     AUR_TRY(cudaMemcpyAsync(d_pairs.p, pair_a, np * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+                     AUR_TRY(cudaMemcpyAsync(d_pairs.p + np, pair_b, np * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+                     AUR_TRY(launch_cosine_gather(d_vec.p, d_pairs.p, d_pairs.p + np, n_pairs, static_cast<int>(H), clamp, d_cos.p, s));
+                     ++enc->stats.launches;
+                     AUR_TRY(cudaMemcpyAsync(cos_h.data(), d_cos.p, np * sizeof(double), cudaMemcpyDeviceToHost, s));
+                   }
+                   if (vec_out) AUR_TRY(cudaMemcpyAsync(vec_h.data(), d_vec.p, vec_h.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
+                   return AUR_OK;
+                 });
+  if (rc != AUR_OK) return rc;
+  if (np > 0) memcpy(cos_out, cos_h.data(), np * sizeof(double));
+  if (vec_out) memcpy(vec_out, vec_h.data(), vec_h.size() * sizeof(float));
+  return AUR_OK;
+}
+
 // aur_encode_append_texts_multi, aur_encode_append_multi with in.cu_texts = NULL (one window per text), and
 // aur_encode_append, which is that with n = 1 after its one-batch checks.
 int append_texts_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const Texts& in, int32_t n_seq,
@@ -616,6 +664,24 @@ int aur_encode_texts(aur_encoder* e, const int32_t* tokens, const int32_t* cu, i
   if (n_texts == 0 && n_seq == 0) return AUR_OK;
   if (!tokens || !cu || !cu_texts) return report_error(AUR_ERR_INVALID, "tokens, cu_seqlens and cu_texts are required");
   return encode_texts(e, Texts{tokens, cu, cu_texts}, n_seq, n_texts, out_f32, out_bf16);
+}
+
+int aur_encode_pair_cosines(aur_encoder* e, const int32_t* tokens, const int32_t* cu, int32_t n_seq, const int32_t* cu_texts,
+                            int32_t n_texts, const int32_t* pair_a, const int32_t* pair_b, int64_t n_pairs, int32_t clamp,
+                            double* cos_out, float* vec_out) {
+  if (!e) return report_error(AUR_ERR_INVALID, "null encoder");
+  const int rc = check_loaded(e);
+  if (rc != AUR_OK) return rc;
+  if (n_seq < 0 || n_texts < 0) return report_error(AUR_ERR_INVALID, "n_seq / n_texts < 0");
+  if (n_pairs < 0) return report_error(AUR_ERR_INVALID, "n_pairs < 0");
+  if (n_pairs > 0 && (!pair_a || !pair_b || !cos_out)) return report_error(AUR_ERR_INVALID, "pair_a, pair_b and cos_out are required");
+  if (clamp != 0 && clamp != 1) return report_error(AUR_ERR_INVALID, "clamp must be 0 or 1");
+  if (n_texts == 0 && n_seq == 0) {
+    if (n_pairs > 0) return report_error(AUR_ERR_INVALID, "%lld pairs over no texts", static_cast<long long>(n_pairs));
+    return AUR_OK;
+  }
+  if (!tokens || !cu || !cu_texts) return report_error(AUR_ERR_INVALID, "tokens, cu_seqlens and cu_texts are required");
+  return pair_cosines(e, Texts{tokens, cu, cu_texts}, n_seq, n_texts, pair_a, pair_b, n_pairs, clamp, cos_out, vec_out);
 }
 
 int aur_encode_append_texts_multi(aur_encoder* const* encs, aur_index* const* shards, int32_t n, const int32_t* tokens,

@@ -182,6 +182,9 @@ cudaError_t launch_merge_topk(const double* in_s, const int64_t* in_ids, size_t 
                               float* out_s, int64_t* out_ids, double* out_s64, cudaStream_t s);
 cudaError_t launch_cosine_pairs(const float* a, const float* b, int64_t n, int dim, int clamp, double* out,
                                 cudaStream_t s);
+// out[p] = the cosine launch_cosine_pairs gives rows pa[p] and pb[p] of vecs [*, dim], bit for bit.
+cudaError_t launch_cosine_gather(const float* vecs, const int32_t* pa, const int32_t* pb, int64_t n, int dim, int clamp,
+                                 double* out, cudaStream_t s);
 cudaError_t launch_fill_f32(float* p, float v, int64_t n, cudaStream_t s);
 // out[i] = OR over the batch's distinct tenant scopes s < n_scopes of (visible(row i, scope s) << s); scopes = {user, org} pairs
 cudaError_t launch_row_scope_mask(const int32_t* row_user, const int32_t* row_org, const int32_t* scopes, int n_scopes, int64_t n,

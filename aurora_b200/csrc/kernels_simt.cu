@@ -583,13 +583,11 @@ exchange_merge_kernel(ExchangeParams p) {
   }
 }
 
-// Pairwise cosine, fp64 accumulate, optional [0,1] clamp (similarity.py:84-98).
-__global__ void cosine_pairs_kernel(const float* __restrict__ a, const float* __restrict__ b, int64_t n, int dim,
-                                    int clamp, double* __restrict__ out) {
-  const int64_t pair = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (pair >= n) return;
-  const float* x = a + pair * dim; const float* y = b + pair * dim;
+// Cosine of x and y [dim] by one warp, fp64 accumulate, optional [0,1] clamp (similarity.py:84-98); lane 0 writes
+// out[pair].  The one statement of this arithmetic: cosine_pairs_kernel and cosine_gather_kernel agree bit for bit
+// through it.
+__device__ __forceinline__ void cosine_pair_warp(const float* __restrict__ x, const float* __restrict__ y, int dim,
+                                                 int clamp, int lane, double* __restrict__ out, int64_t pair) {
   double dot = 0.0, xx = 0.0, yy = 0.0;
   for (int i = lane; i < dim; i += 32) {
     const double u = x[i], v = y[i];
@@ -602,6 +600,26 @@ __global__ void cosine_pairs_kernel(const float* __restrict__ a, const float* __
     if (clamp) c = fmax(0.0, fmin(1.0, c));
     out[pair] = c;
   }
+}
+
+// Pairwise cosine of row i of a with row i of b.
+__global__ void cosine_pairs_kernel(const float* __restrict__ a, const float* __restrict__ b, int64_t n, int dim,
+                                    int clamp, double* __restrict__ out) {
+  const int64_t pair = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (pair >= n) return;
+  cosine_pair_warp(a + pair * dim, b + pair * dim, dim, clamp, lane, out, pair);
+}
+
+// Pair p = rows pa[p] and pb[p] of vecs [*, dim], one warp each (aur_encode_pair_cosines).
+__global__ void cosine_gather_kernel(const float* __restrict__ vecs, const int32_t* __restrict__ pa,
+                                     const int32_t* __restrict__ pb, int64_t n, int dim, int clamp,
+                                     double* __restrict__ out) {
+  const int64_t pair = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (pair >= n) return;
+  cosine_pair_warp(vecs + static_cast<int64_t>(pa[pair]) * dim, vecs + static_cast<int64_t>(pb[pair]) * dim, dim, clamp,
+                   lane, out, pair);
 }
 
 __global__ void fill_f32_kernel(float* p, float v, int64_t n) {
@@ -716,6 +734,15 @@ cudaError_t launch_cosine_pairs(const float* a, const float* b, int64_t n, int d
   const int threads = 256;
   const int64_t blocks = (n * 32 + threads - 1) / threads;
   cosine_pairs_kernel<<<static_cast<unsigned>(blocks), threads, 0, s>>>(a, b, n, dim, clamp, out);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_cosine_gather(const float* vecs, const int32_t* pa, const int32_t* pb, int64_t n, int dim, int clamp,
+                                 double* out, cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  const int threads = 256;
+  const int64_t blocks = (n * 32 + threads - 1) / threads;
+  cosine_gather_kernel<<<static_cast<unsigned>(blocks), threads, 0, s>>>(vecs, pa, pb, n, dim, clamp, out);
   return cudaGetLastError();
 }
 

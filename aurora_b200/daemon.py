@@ -23,6 +23,12 @@ empty kernels), so concurrent ``search_knowledge_base`` calls are gathered for a
 their query texts go through ONE encoder batch, and the dense leg runs as one kernel launch per distinct tenant scope
 in the window (the scope folds into the row scale, see csrc/capi.cu); each caller gets its own result back.
 
+Alert correlation.  ``embed`` / ``embed_batch`` answer with the daemon's encoder (``encoder.get_embedding_client()``), so a
+Celery child's embedding client can be this ``Client`` instead of an encoder and a CUDA context of its own;
+``similarity_scores`` is ``correlation.SimilarityStrategy.score_alerts`` over the socket, concurrent calls gathered in
+the same window into one ``similarities`` call.  An unreachable daemon gives ``embed`` None and Jaccard title scores,
+the reference's behaviour when its t2v sidecar is down.
+
 Durability.  The daemon owns the only copy of the vectors: it snapshots the knowledge base (KnowledgeBase.save:
 atomic rename of shard + metadata) after ``save_every`` mutations or ``save_seconds`` seconds with unsaved
 mutations, on SIGTERM / shutdown, and on the ``save`` call; it compacts tombstones when more than a quarter of the
@@ -82,8 +88,9 @@ class _Pending:
         self.args, self.event, self.result, self.error = args, threading.Event(), None, None
 
 
-class SearchCoalescer:
-    """Gathers concurrent search_knowledge_base calls into one encoder batch (+ one dense launch per tenant scope)."""
+class _Coalescer:
+    """Gathers the requests that arrive within ``window_us`` of the first into one batch, served by ``_serve`` on one
+    thread; each caller gets its own result back (or the batch's exception)."""
 
     def __init__(self, module, window_us: int = 200, max_batch: int = 256):
         self.module, self.window, self.max_batch = module, window_us * 1e-6, max_batch
@@ -94,10 +101,8 @@ class SearchCoalescer:
         self._t = threading.Thread(target=self._run, name="aurora-b200-coalescer", daemon=True)
         self._t.start()
 
-    def submit(self, user_id, query, limit=5, alpha=0.5, min_score=0.0, org_id=None):
-        if not isinstance(query, str) or not query.strip():
-            return []
-        p = _Pending((user_id, query, limit, alpha, min_score, org_id))
+    def _submit(self, args):
+        p = _Pending(args)
         with self._cv:
             self._q.append(p)
             self._cv.notify()
@@ -129,19 +134,50 @@ class SearchCoalescer:
             self.batches += 1
             self.requests += len(batch)
             try:
-                batched = getattr(self.module, "search_knowledge_base_batch", None)
-                if batched is not None and len(batch) > 1:
-                    results = batched([p.args for p in batch])
-                else:
-                    results = [self.module.search_knowledge_base(*p.args[:2], limit=p.args[2], alpha=p.args[3], min_score=p.args[4],
-                                                                 org_id=p.args[5]) for p in batch]
-                for p, r in zip(batch, results):
+                for p, r in zip(batch, self._serve(batch)):
                     p.result = r
-            except Exception as e:          # search swallows errors itself (-> []); this is a programming error
+            except Exception as e:          # the served calls swallow errors themselves; this is a programming error
                 for p in batch:
                     p.error = e
             for p in batch:
                 p.event.set()
+
+    def _serve(self, batch: List[_Pending]) -> list:
+        raise NotImplementedError
+
+
+class SearchCoalescer(_Coalescer):
+    """Gathers concurrent search_knowledge_base calls into one encoder batch (+ one dense launch per tenant scope)."""
+
+    def submit(self, user_id, query, limit=5, alpha=0.5, min_score=0.0, org_id=None):
+        if not isinstance(query, str) or not query.strip():
+            return []
+        return self._submit((user_id, query, limit, alpha, min_score, org_id))
+
+    def _serve(self, batch):
+        batched = getattr(self.module, "search_knowledge_base_batch", None)
+        if batched is not None and len(batch) > 1:
+            return batched([p.args for p in batch])
+        return [self.module.search_knowledge_base(*p.args[:2], limit=p.args[2], alpha=p.args[3], min_score=p.args[4],
+                                                  org_id=p.args[5]) for p in batch]
+
+
+class SimilarityCoalescer(_Coalescer):
+    """Gathers concurrent similarity_scores calls (an alert storm reaches the daemon from several Celery children at
+    once) into one SimilarityStrategy.score_alerts call: one EmbeddingClient.similarities call, one device call."""
+
+    def submit(self, items):
+        return self._submit(list(items))
+
+    def _serve(self, batch):
+        from .correlation import SimilarityStrategy
+
+        scores = SimilarityStrategy().score_alerts([it for p in batch for it in p.args])
+        out, at = [], 0
+        for p in batch:
+            out.append(scores[at:at + len(p.args)])
+            at += len(p.args)
+        return out
 
 
 # ----------------------------------------------------------------------------- snapshot policy
@@ -240,6 +276,12 @@ class _Handler(socketserver.BaseRequestHandler):
                     res = getattr(module, fn)(*args, **kwargs)
                 elif fn in ("hybrid", "near_text"):      # the private facade of rca_prompt_builder.py:276-298, over the wire
                     res = _facade_query(module, fn, kwargs)
+                elif fn in ("embed", "embed_batch"):    # the daemon's own encoder: Celery children load none
+                    from .encoder import get_embedding_client
+
+                    res = getattr(get_embedding_client(), fn)(*args, **kwargs)
+                elif fn == "similarity_scores":
+                    res = srv.similarity.submit(*args, **kwargs) if srv.similarity is not None else _score_alerts(*args, **kwargs)
                 elif fn in LEARN_API:
                     if srv.learn_module is None:
                         raise RuntimeError("Aurora Learn is not configured in this daemon")
@@ -249,6 +291,12 @@ class _Handler(socketserver.BaseRequestHandler):
                 _send(self.request, {"ok": True, "result": res})
             except Exception as e:           # insert_chunks re-raises by design: report it to the caller
                 _send(self.request, {"ok": False, "error": f"{type(e).__name__}: {e}"})
+
+
+def _score_alerts(items):
+    from .correlation import SimilarityStrategy
+
+    return SimilarityStrategy().score_alerts(items)
 
 
 def _facade_query(module, fn: str, kw: Dict[str, Any]):
@@ -277,8 +325,9 @@ class _Server(socketserver.ThreadingMixIn, socketserver.UnixStreamServer):
             os.umask(old)
 
     def close_all(self, final_save: bool = True):
-        if self.coalescer is not None:
-            self.coalescer.close()
+        for c in (self.coalescer, self.similarity):
+            if c is not None:
+                c.close()
         self.snapshots.close(final_save)
 
 
@@ -293,6 +342,7 @@ def serve(socket_path: str, module=None, background: bool = False, learn_module=
     srv.module = module                     # type: ignore[attr-defined]
     srv.learn_module = learn_module
     srv.coalescer = SearchCoalescer(module, coalesce_us) if coalesce_us > 0 else None
+    srv.similarity = SimilarityCoalescer(module, coalesce_us) if coalesce_us > 0 else None
     srv.snapshots = SnapshotPolicy(module, snapshot_dir, save_every, save_seconds)
     if background:
         t = threading.Thread(target=srv.serve_forever, name="aurora-b200-daemon", daemon=True)
@@ -422,6 +472,37 @@ class Client:
         if not self.health().get("ready"):
             raise DaemonUnavailable(self._path)
         return SimpleNamespace(is_ready=lambda: True, close=lambda: None), SimpleNamespace(name="KnowledgeBaseChunk", query=_RemoteQuery(self))
+
+    # ---- alert correlation (services/correlation): the daemon's encoder behind get_embedding_client() of a Celery child
+    def embed(self, text: str):
+        """EmbeddingClient.embed in the daemon; None for blank text and when the daemon is unreachable (the reference's
+        answer when the t2v sidecar is down, embedding_client.py:66-70), so the strategy falls back to Jaccard."""
+        if not text or not text.strip():
+            return None
+        try:
+            return self._call("embed", text)
+        except Exception as e:
+            logger.warning(f"[KB B200 client] embed failed: {e}")
+            return None
+
+    def embed_batch(self, texts):
+        try:
+            return self._call("embed_batch", list(texts))
+        except Exception as e:
+            logger.warning(f"[KB B200 client] embed_batch failed: {e}")
+            return [None] * len(texts)
+
+    def similarity_scores(self, items):
+        """SimilarityStrategy.score_alerts run in the daemon: items [(alert_title, alert_service, [(incident_title,
+        incident_services), ...]), ...] -> one score list per alert; concurrent calls share one device call there.
+        Unreachable daemon: every title scored by Jaccard, as ``score`` does when ``embed`` gives None."""
+        try:
+            return self._call("similarity_scores", list(items))
+        except Exception as e:
+            from .correlation import SimilarityStrategy
+
+            logger.warning(f"[KB B200 client] similarity_scores failed, titles by Jaccard: {e}")
+            return SimilarityStrategy().weigh(items, lambda pairs: [None] * len(pairs))
 
     # ---- Aurora Learn (routes/incident_feedback/weaviate_client.py:165-386), same conventions
     def store_good_rca(self, user_id, incident_id, feedback_id, alert_title, alert_service, source_type, severity, aurora_summary,

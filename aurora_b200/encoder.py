@@ -15,7 +15,7 @@ import ctypes as C
 import logging
 from dataclasses import dataclass
 from functools import lru_cache
-from typing import Callable, Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -137,6 +137,27 @@ class Encoder:
         N.check(self._lib.aur_encode_texts(self._h, _ptr(tokens), _ptr(cu), cu.size - 1, _ptr(ct), ct.size - 1,
                                            None if bf16 else _ptr(out), _ptr(out) if bf16 else None))
         return out
+
+    def pair_cosines(self, tokens: np.ndarray, cu_seqlens: np.ndarray, cu_texts: np.ndarray, pair_a, pair_b,
+                     clamp: bool = True, vectors: bool = False):
+        """aur_encode_pair_cosines: [n_pairs] float64 cosines of texts pair_a[p] and pair_b[p] (texts packed as for
+        ``encode_texts``), equal bit for bit to ``engine.cosine_pairs`` over ``encode_texts``' vectors with the same
+        ``clamp``; one call, the vectors never leave the device.  ``vectors``: also return those vectors,
+        (cosines, [n_texts, hidden] float32)."""
+        tokens = np.ascontiguousarray(tokens, dtype=np.int32)
+        cu = np.ascontiguousarray(cu_seqlens, dtype=np.int32)
+        ct = np.ascontiguousarray(cu_texts, dtype=np.int32)
+        if cu.ndim != 1 or cu.size < 1 or ct.ndim != 1 or ct.size < 1 or tokens.ndim != 1 or tokens.size != int(cu[-1]):
+            raise ValueError("tokens [total], cu_seqlens [n_seq + 1] with cu[-1] == total and cu_texts [n_texts + 1] are required")
+        pa = np.ascontiguousarray(pair_a, dtype=np.int32)
+        pb = np.ascontiguousarray(pair_b, dtype=np.int32)
+        if pa.ndim != 1 or pa.shape != pb.shape:
+            raise ValueError("pair_a and pair_b must be 1-d and of one length")
+        cos = np.empty(pa.size, dtype=np.float64)
+        vec = np.empty((ct.size - 1, self.cfg.hidden), dtype=np.float32) if vectors else None
+        N.check(self._lib.aur_encode_pair_cosines(self._h, _ptr(tokens), _ptr(cu), cu.size - 1, _ptr(ct), ct.size - 1, _ptr(pa),
+                                                  _ptr(pb), pa.size, int(bool(clamp)), _ptr(cos), _ptr(vec)))
+        return (cos, vec) if vectors else cos
 
     def encode(self, seqs: Sequence[Sequence[int]]) -> np.ndarray:
         """Token-id lists of any count, [len(seqs), hidden] float32: one ``encode_texts`` call with one window per text,
@@ -323,7 +344,49 @@ class EmbeddingClient:
             logger.warning("[EmbeddingClient] embed_batch failed: %s", e)
         return out
 
-    def close(self) -> None:                                    # embedding_client.py:76-78
+    def similarities(self, pairs: Sequence[Tuple[str, str]]) -> List[Optional[float]]:
+        """Clamped cosine of each pair's two texts, from the vectors ``embed`` would return for them, in ONE
+        ``Encoder.pair_cosines`` call instead of two ``embed`` calls and a Python cosine per pair: every distinct text
+        is tokenised and encoded once.  A pair holding a text ``embed`` answers None for (blank, a tokenizer error, a
+        sequence of 0 or more than max_pos tokens, a token id outside the vocabulary) is None, and the other pairs are
+        unaffected; a failed device call makes every pair None, as the serial path is when every ``embed`` fails."""
+        cfg = self._enc.cfg
+        limit = min(cfg.max_pos, self._enc.max_tokens)
+        seq: Dict[str, Optional[np.ndarray]] = {}          # text -> its one sequence, None when embed would give None
+        for pair in pairs:
+            for t in pair:
+                if t in seq:
+                    continue
+                seq[t] = None
+                if not t or not t.strip():
+                    continue
+                try:
+                    ids = np.asarray(self._tok(t), dtype=np.int64)
+                except Exception as e:                          # embed: any failure -> None
+                    logger.warning("[EmbeddingClient] tokenize failed: %s", e)
+                    continue
+                if ids.ndim == 1 and 1 <= ids.size <= limit and ids.min() >= 0 and ids.max() < cfg.vocab:
+                    seq[t] = ids.astype(np.int32)
+        out: List[Optional[float]] = [None] * len(pairs)
+        live = [p for p, (a, b) in enumerate(pairs) if seq[a] is not None and seq[b] is not None]
+        if not live:
+            return out
+        row: Dict[str, int] = {}
+        for p in live:
+            for t in pairs[p]:
+                row.setdefault(t, len(row))
+        try:
+            tok, cu = pack_sequences([seq[t] for t in row])
+            cos = self._enc.pair_cosines(tok, cu, np.arange(len(row) + 1, dtype=np.int32), [row[pairs[p][0]] for p in live],
+                                         [row[pairs[p][1]] for p in live], clamp=True)
+        except Exception as e:
+            logger.warning("[EmbeddingClient] similarities failed: %s", e)
+            return out
+        for p, c in zip(live, cos.tolist()):
+            out[p] = c
+        return out
+
+    def close(self) -> None:                                   # embedding_client.py:76-78
         self._enc.close()
 
 

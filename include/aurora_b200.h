@@ -624,6 +624,19 @@ int aur_encode_append_multi(aur_encoder* const* encs, aur_index* const* shards, 
  * work: the checks of aur_encode_append_multi that apply, and cu_texts (AUR_ERR_INVALID). */
 int aur_encode_texts(aur_encoder* enc, const int32_t* tokens, const int32_t* cu_seqlens, int32_t n_seq,
                      const int32_t* cu_texts, int32_t n_texts, float* out_f32, uint16_t* out_bf16);
+/* Texts in (aur_encode_texts' packed windows), cosines of text pairs out: pair p is (pair_a[p], pair_b[p]), indices
+ * into the n_texts texts.  cos_out [n_pairs] fp64; vec_out [n_texts, hidden] fp32 (nullable).  vec_out is
+ * aur_encode_texts' out_f32 for the same inputs, bit for bit, and cos_out[p] is what aur_cosine_pairs returns for rows
+ * pair_a[p] and pair_b[p] of it with the same clamp, bit for bit (0.0 for a zero norm; clamp = 1 applies the [0, 1]
+ * clamp of similarity.py:98).  The texts go through the workspace as aur_encode_texts runs them; their vectors stay on
+ * the device until one gather launch has scored every pair, and one copy brings the cosines back (and one the vectors).
+ * Outputs are written only on success.  Checked before any device work, leaving the outputs and the encoder's stats
+ * untouched: every check of aur_encode_texts, n_pairs < 0, pair_a, pair_b or cos_out NULL while n_pairs > 0, a pair
+ * index outside 0 .. n_texts - 1, clamp not 0 or 1 (AUR_ERR_INVALID).  A failed allocation of the call's device
+ * buffers (the text vectors, the pairs, the cosines) is AUR_ERR_NOMEM. */
+int aur_encode_pair_cosines(aur_encoder* enc, const int32_t* tokens, const int32_t* cu_seqlens, int32_t n_seq,
+                            const int32_t* cu_texts, int32_t n_texts, const int32_t* pair_a, const int32_t* pair_b,
+                            int64_t n_pairs, int32_t clamp, double* cos_out, float* vec_out);
 /* aur_encode_append_multi with texts as the unit: text j (its windows, cu_texts as for aur_encode_texts) is encoded by
  * encs[ids[j] mod n] into the vector aur_encode_texts gives it and appended, as bf16, to shards[ids[j] mod n]; each
  * shard's rows are appended in input order; room is counted in texts; ids, user_codes and org_codes are [n_texts].  The
