@@ -25,7 +25,7 @@ TC_QUERY_ROWS = 64   # queries per CTA of the tensor-core kernel (kTcQRows, csrc
 # every symbol include/aurora_b200.h declares (tests check the .so exports all of them)
 EXPORTS = [
     "aur_abi_version", "aur_last_error", "aur_device_count", "aur_open", "aur_close", "aur_get_stats",
-    "aur_set_option", "aur_sync", "aur_add", "aur_add_dev", "aur_export", "aur_read_rows", "aur_compact", "aur_reserve", "aur_remove", "aur_search", "aur_search_ex", "aur_search_subset", "aur_search_lists", "aur_set_attrs", "aur_search_filtered", "aur_filter_ids", "aur_filter_count", "aur_remove_filtered", "aur_search_dev",
+    "aur_set_option", "aur_sync", "aur_add", "aur_add_dev", "aur_export", "aur_read_rows", "aur_live_bits", "aur_export_rows", "aur_compact", "aur_reserve", "aur_remove", "aur_search", "aur_search_ex", "aur_search_subset", "aur_search_lists", "aur_set_attrs", "aur_search_filtered", "aur_filter_ids", "aur_filter_count", "aur_remove_filtered", "aur_search_dev",
     "aur_merge_topk_dev", "aur_merge_topk_packed_dev", "aur_merge_topk_host", "aur_merge_topk_host_f64", "aur_exchange_create", "aur_exchange_connect", "aur_exchange_close",
     "aur_exchange_status", "aur_search_exchange_dev", "aur_cosine_pairs", "aur_dev_malloc", "aur_dev_free", "aur_memcpy_h2d", "aur_memcpy_d2h",
     "aur_debug_tc_scores", "aur_debug_simt_scores", "aur_debug_list_scores",
@@ -121,6 +121,8 @@ def load():
         "aur_compact": (C.c_int, [vp, C.POINTER(i64)]),
         "aur_reserve": (C.c_int, [vp, i64]),
         "aur_read_rows": (C.c_int, [vp, i64, i64, vp, vp]),
+        "aur_live_bits": (C.c_int, [vp, vp, vp, i64, C.POINTER(i64), C.POINTER(i64)]),
+        "aur_export_rows": (C.c_int, [vp, i64, i64, vp, vp, vp, vp]),
         "aur_search_ex": (C.c_int, [vp, vp, i32, i32, vp, vp, vp, vp, C.POINTER(i64)]),
         "aur_search_subset": (C.c_int, [vp, vp, i32, i32, vp, i64, vp, vp]),
         "aur_search_lists": (C.c_int, [vp, vp, i32, i32, vp, vp, i32, vp, vp, vp, C.POINTER(i64)]),

@@ -294,6 +294,12 @@ struct aur_index {
   VmmBuf<int64_t> d_ids;
   VmmBuf<int32_t> d_user, d_org;
   AttrColumns attrs;                     // program columns 2.., cap_pad rows each (aur_set_attrs, writers hold mu_write)
+  int64_t compactions = 0;               // aur_compact calls over the shard's life (bumped under the exclusive lock)
+  DevBuf<uint32_t> live_bits;            // aur_live_bits: live and nonfinite words (writers hold mu_write)
+  HostBuf<uint32_t> live_bits_host;      // (their page-locked landing area)
+  std::mutex mu_export;                  // aur_export_rows' staging: one copy-out at a time
+  HostBuf<uint8_t> export_stage;         // two halves, each filled by the ingest stream while the host drains the other
+  Event export_ev[2];
   std::unordered_map<int64_t, int64_t> id2row;
   Stream stream;                         // the index's own stream: device-pointer calls with stream == NULL
   Stream ingest_stream;                  // host appends / tombstones, lowest priority so queries overtake them
@@ -1322,11 +1328,87 @@ int aur_read_rows(aur_index* ix, int64_t row0, int64_t n, void* rows_out, int64_
   return AUR_OK;
 }
 
+int aur_live_bits(aur_index* ix, uint32_t* live_out, uint32_t* nonfinite_out, int64_t words, int64_t* rows_out,
+                  int64_t* compactions_out) {
+  if (!ix || !live_out || !rows_out) return fail(AUR_ERR_INVALID, "null argument");
+  if (ix->dtype == AUR_I8 && !nonfinite_out) return fail(AUR_ERR_INVALID, "an int8 shard needs nonfinite_out");
+  // the writers' lock orders this after every append and remove that has returned; searches go on
+  std::shared_lock<std::shared_mutex> rl(ix->rw);
+  std::lock_guard<std::mutex> wk(ix->mu_write);
+  const int64_t rows = ix->rows_pub.load(std::memory_order_acquire);
+  const int64_t need = (rows + 31) / 32;
+  if (words < need) return fail(AUR_ERR_INVALID, "%lld rows need %lld words, got %lld", (long long)rows, (long long)need, (long long)words);
+  *rows_out = rows;
+  if (compactions_out) *compactions_out = ix->compactions;
+  if (rows == 0) return AUR_OK;
+  AUR_TRY(cudaSetDevice(ix->device));
+  const size_t w = static_cast<size_t>(need);
+  AUR_TRY(ix->live_bits.reserve(2 * w));
+  AUR_TRY(ix->live_bits_host.reserve(2 * w, cudaHostAllocDefault));
+  cudaStream_t s = ix->ingest_stream;
+  AUR_TRY(launch_live_bits(ix->d_inv_norm.p, rows, ix->dtype == AUR_I8, ix->live_bits.p, ix->live_bits.p + w, s));
+  AUR_TRY(cudaMemcpyAsync(ix->live_bits_host.p, ix->live_bits.p, 2 * w * 4, cudaMemcpyDeviceToHost, s));
+  AUR_TRY(cudaStreamSynchronize(s));
+  memcpy(live_out, ix->live_bits_host.p, w * 4);
+  if (nonfinite_out) memcpy(nonfinite_out, ix->live_bits_host.p + w, w * 4);
+  return AUR_OK;
+}
+
+int aur_export_rows(aur_index* ix, int64_t row0, int64_t n, void* rows_out, int64_t* ids_out, int32_t* user_out,
+                    int32_t* org_out) {
+  if (!ix || (n > 0 && (!rows_out || !ids_out))) return fail(AUR_ERR_INVALID, "null argument");
+  std::shared_lock<std::shared_mutex> rl(ix->rw);   // published rows never change under it: appends and searches go on
+  const int64_t rows = ix->rows_pub.load(std::memory_order_acquire);
+  if (row0 < 0 || n < 0 || row0 + n > rows) return fail(AUR_ERR_INVALID, "rows [%lld, %lld) are not inside the published prefix of %lld",
+                                                        (long long)row0, (long long)(row0 + n), (long long)rows);
+  if (n == 0) return AUR_OK;
+  AUR_TRY(cudaSetDevice(ix->device));
+  std::lock_guard<std::mutex> ek(ix->mu_export);
+  const size_t rb = static_cast<size_t>(ix->dim) * ix->elt, per = rb + 16;   // a row, its id and its two tenant codes
+  const int64_t chunk = std::max<int64_t>(1, static_cast<int64_t>((size_t(4) << 20) / per));   // rows per half: ~4 MB
+  AUR_TRY(ix->export_stage.reserve(2 * static_cast<size_t>(chunk) * per, cudaHostAllocDefault));
+  for (Event& ev : ix->export_ev)
+    if (!ev.ev) AUR_TRY(ev.create(cudaEventDisableTiming));
+  cudaStream_t s = ix->ingest_stream;
+  const uint8_t* d_rows = static_cast<const uint8_t*>(ix->d_rows.p);
+  auto half = [&](int64_t c) { return ix->export_stage.p + static_cast<size_t>(c & 1) * static_cast<size_t>(chunk) * per; };
+  auto enqueue = [&](int64_t c) -> cudaError_t {   // chunk c's rows, ids, user and org codes into its half
+    const int64_t r = row0 + c * chunk, m = std::min(chunk, row0 + n - r);
+    uint8_t* h = half(c);
+    AUR_CU_RET(cudaMemcpyAsync(h, d_rows + static_cast<size_t>(r) * rb, static_cast<size_t>(m) * rb, cudaMemcpyDeviceToHost, s));
+    h += static_cast<size_t>(m) * rb;
+    AUR_CU_RET(cudaMemcpyAsync(h, ix->d_ids.p + r, static_cast<size_t>(m) * 8, cudaMemcpyDeviceToHost, s));
+    AUR_CU_RET(cudaMemcpyAsync(h + m * 8, ix->d_user.p + r, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToHost, s));
+    AUR_CU_RET(cudaMemcpyAsync(h + m * 12, ix->d_org.p + r, static_cast<size_t>(m) * 4, cudaMemcpyDeviceToHost, s));
+    return cudaEventRecord(ix->export_ev[c & 1], s);
+  };
+  const int64_t n_chunks = (n + chunk - 1) / chunk;
+  cudaError_t e = enqueue(0);
+  for (int64_t c = 0; e == cudaSuccess && c < n_chunks; ++c) {
+    if (c + 1 < n_chunks) e = enqueue(c + 1);   // the other half: its last contents were drained in the previous pass
+    if (e == cudaSuccess) e = cudaEventSynchronize(ix->export_ev[c & 1]);
+    if (e != cudaSuccess) break;
+    const int64_t m = std::min(chunk, n - c * chunk), o = c * chunk;
+    const uint8_t* h = half(c);
+    memcpy(static_cast<uint8_t*>(rows_out) + static_cast<size_t>(o) * rb, h, static_cast<size_t>(m) * rb);
+    h += static_cast<size_t>(m) * rb;
+    memcpy(ids_out + o, h, static_cast<size_t>(m) * 8);
+    if (user_out) memcpy(user_out + o, h + m * 8, static_cast<size_t>(m) * 4);
+    if (org_out) memcpy(org_out + o, h + m * 12, static_cast<size_t>(m) * 4);
+  }
+  if (e != cudaSuccess) {
+    cudaStreamSynchronize(s);   // no copy may still land in the staging after the lock is released
+    return fail(AUR_ERR_CUDA, "aur_export_rows: %s", cudaGetErrorString(e));
+  }
+  return AUR_OK;
+}
+
 int aur_compact(aur_index* ix, int64_t* reclaimed) {
   if (!ix) return fail(AUR_ERR_INVALID, "null index");
   if (reclaimed) *reclaimed = 0;
   std::unique_lock<std::shared_mutex> wl(ix->rw);   // no search or append is being enqueued ...
   std::lock_guard<std::mutex> wk(ix->mu_write);
+  ++ix->compactions;                                 // counted before anything can fail: a failed one may have moved rows
   AUR_TRY(cudaSetDevice(ix->device));
   AUR_TRY(cudaDeviceSynchronize());                  // ... and none is still running
   const int64_t rows = ix->rows_pub.load(std::memory_order_acquire);

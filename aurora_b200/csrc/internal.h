@@ -263,6 +263,9 @@ cudaError_t launch_mask_match(const float* inv, const uint32_t* mask, int64_t n,
 cudaError_t launch_scatter_inv_norm(const float* inv, const int32_t* rows, int64_t n, int64_t n_rows, float* out, cudaStream_t s);
 // deletes: inv[rows[i]] = NaN (the tombstone) for the listed rows, one launch
 cudaError_t launch_tombstone_rows(const int32_t* rows, int64_t n, float* inv, cudaStream_t s);
+// checkpoints: bit r % 32 of word r / 32 of live = row r's inverse norm is not NaN, of nonfinite (i8 only) = it is
+// infinite, for rows [0, n); one warp per word, every word of ceil(n / 32) written
+cudaError_t launch_live_bits(const float* inv, int64_t n, int i8, uint32_t* live, uint32_t* nonfinite, cudaStream_t s);
 // compaction: rows map[0..n) (and their side arrays) -> bounce buffers
 cudaError_t launch_gather_rows(const void* rows, const float* inv, const int64_t* ids, const int32_t* user, const int32_t* org,
                                const int32_t* map, int64_t n, int row_bytes, void* o_rows, float* o_inv, int64_t* o_ids,

@@ -792,6 +792,27 @@ cudaError_t launch_tombstone_rows(const int32_t* rows, int64_t n, float* inv, cu
   return cudaGetLastError();
 }
 
+// Checkpoints: liveness of rows [0, n) packed 32 to a word, one warp per word.  A row is live when its inverse norm is
+// not NaN; on an int8 shard an infinite one (a row stored from a NaN or inf) is also set in nonfinite, as aur_export
+// reports it live = 2.  Lanes past n vote 0, so the last word's tail bits are clear.
+__global__ void live_bits_kernel(const float* __restrict__ inv, int64_t n, int i8, uint32_t* __restrict__ live,
+                                 uint32_t* __restrict__ nonfinite) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const float v = i < n ? __ldg(inv + i) : __uint_as_float(0x7FC00000u);
+  const uint32_t l = __ballot_sync(0xFFFFFFFFu, v == v);
+  const uint32_t f = __ballot_sync(0xFFFFFFFFu, i8 && isinf(v));
+  if ((threadIdx.x & 31) == 0 && i < n) {
+    live[i >> 5] = l;
+    nonfinite[i >> 5] = f;
+  }
+}
+
+cudaError_t launch_live_bits(const float* inv, int64_t n, int i8, uint32_t* live, uint32_t* nonfinite, cudaStream_t s) {
+  if (n <= 0) return cudaSuccess;
+  live_bits_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(inv, n, i8, live, nonfinite);
+  return cudaGetLastError();
+}
+
 // Compaction: gather the rows listed in map (and their side arrays) into bounce buffers.  One warp per row,
 // 16-byte pieces (row_bytes % 16 == 0 for bf16 dims % 8 == 0 and for f32 dims % 4 == 0; else byte loop).
 __global__ void gather_rows_kernel(const uint8_t* __restrict__ rows, const float* __restrict__ inv, const int64_t* __restrict__ ids,

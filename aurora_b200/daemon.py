@@ -29,10 +29,12 @@ Celery child's embedding client can be this ``Client`` instead of an encoder and
 the same window into one ``similarities`` call.  An unreachable daemon gives ``embed`` None and Jaccard title scores,
 the reference's behaviour when its t2v sidecar is down.
 
-Durability.  The daemon owns the only copy of the vectors: it snapshots the knowledge base (KnowledgeBase.save:
-atomic rename of shard + metadata) after ``save_every`` mutations or ``save_seconds`` seconds with unsaved
-mutations, on SIGTERM / shutdown, and on the ``save`` call; it compacts tombstones when more than a quarter of the
-shard is dead.  Between snapshots every acknowledged insert / delete is in the mutation log beside the snapshot
+Durability.  The daemon owns the only copy of the vectors: it snapshots the knowledge base (KnowledgeBase.checkpoint:
+the rows and metadata changed since the last snapshot, written while searches and ingest go on, made durable by an
+atomic rename of the manifest) after ``save_every`` mutations or ``save_seconds`` seconds with unsaved mutations, on
+SIGTERM / shutdown, and on the ``save`` call, whose result reports the snapshot's kind (base or delta), its bytes and
+the milliseconds it held the knowledge base's lock; it compacts tombstones when more than a quarter of the shard is
+dead (the next snapshot is then a base).  Between snapshots every acknowledged insert / delete is in the mutation log beside the snapshot
 (KnowledgeBase.attach_wal, fsync'd before the reply; bootstrap.configure_from_env attaches it): a restart loads the
 last snapshot and replays the log.  The socket is created with mode 0600: any local process that can open it can read every tenant.
 """
@@ -182,7 +184,7 @@ class SimilarityCoalescer(_Coalescer):
 
 # ----------------------------------------------------------------------------- snapshot policy
 class SnapshotPolicy:
-    """Saves the knowledge base after N mutations / T seconds with unsaved mutations, and on demand."""
+    """Checkpoints the knowledge base after N mutations / T seconds with unsaved mutations, and on demand."""
 
     def __init__(self, module, directory: Optional[str], save_every: int = 2000, save_seconds: float = 60.0):
         self.module, self.dir, self.every, self.seconds = module, directory, save_every, save_seconds
@@ -225,9 +227,15 @@ class SnapshotPolicy:
                         kb.sparse.compact()
             except Exception:
                 pass
-            kb.save(self.dir)
+            res = {"saved": True, "directory": self.dir}
+            if hasattr(kb, "checkpoint"):   # incremental, and searches and ingest go on while it is written
+                ck = kb.checkpoint(self.dir)
+                res.update(kind=ck["kind"], bytes=ck["bytes"], locked_ms=ck["locked_ms"])
+            else:
+                kb.save(self.dir)
             self.saves += 1
-            return {"saved": True, "directory": self.dir, "seconds": round(time.perf_counter() - t0, 3), "compacted_rows": dead}
+            res.update(seconds=round(time.perf_counter() - t0, 3), compacted_rows=dead)
+            return res
 
     def _run(self) -> None:
         last = time.perf_counter()

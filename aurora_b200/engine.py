@@ -186,6 +186,32 @@ class Index:
         N.check(self._lib.aur_read_rows(self._h, int(row0), int(n), _ptr(rows), _ptr(ids)))
         return rows, ids
 
+    def capture(self):
+        """What an incremental snapshot needs of the shard now (aur_live_bits), ordered after every add and remove that
+        has returned, while searches go on: (rows, live bits, nonfinite bits, compactions).  The bits are uint32 words
+        [ceil(rows / 32)], bit r % 32 of word r // 32 for row r; nonfinite marks the rows ``export_raw`` reports as 2.
+        Rows [0, rows) keep their numbers until ``compactions`` moves."""
+        words = (self.stats()["rows"] + 31) // 32 + 64        # room for rows appended before the call takes the lock
+        while True:
+            live, nonfinite = np.zeros(words, np.uint32), np.zeros(words, np.uint32)
+            rows, compactions = C.c_int64(0), C.c_int64(0)
+            rc = self._lib.aur_live_bits(self._h, _ptr(live), _ptr(nonfinite), words, C.byref(rows), C.byref(compactions))
+            if rc == N.AUR_ERR_INVALID and (self.stats()["rows"] + 31) // 32 > words:
+                words = (self.stats()["rows"] + 31) // 32 + 4096    # more rows arrived: retry with room for them
+                continue
+            N.check(rc)
+            w = (int(rows.value) + 31) // 32
+            return int(rows.value), live[:w], nonfinite[:w], int(compactions.value)
+
+    def export_rows(self, row0: int, n: int):
+        """(rows [n, dim] as ``export`` gives them, ids, user codes, org codes) of appended rows row0 .. row0 + n
+        (aur_export_rows: searches and appends go on meanwhile)."""
+        rows = np.empty((int(n), self.dim), dtype=_row_dtype(self.dtype))
+        ids = np.empty(int(n), dtype=np.int64)
+        user, org = np.empty(int(n), dtype=np.int32), np.empty(int(n), dtype=np.int32)
+        N.check(self._lib.aur_export_rows(self._h, int(row0), int(n), _ptr(rows), _ptr(ids), _ptr(user), _ptr(org)))
+        return rows, ids, user, org
+
     def compact(self) -> int:
         """Reclaim tombstoned rows (exclusive; waits for searches in flight).  Returns the rows freed."""
         freed = C.c_int64(0)
@@ -527,6 +553,14 @@ class MultiIndex:
 
     def compact(self) -> int:
         return int(sum(self._each(lambda s, shard: shard.compact())))
+
+    def capture(self) -> list:
+        """Index.capture of every shard at once, in shard order."""
+        return self._each(lambda s, shard: shard.capture())
+
+    def export_rows(self, ranges) -> list:
+        """Index.export_rows of every shard at once: ``ranges`` holds one (row0, n) per shard; results in shard order."""
+        return self._each(lambda s, shard: shard.export_rows(*ranges[s]))
 
     def reserve(self, capacity: int) -> None:
         """Grow to a total of at least ``capacity`` rows: every shard to its ``shard_capacity`` share, in place."""

@@ -134,6 +134,13 @@ class KnowledgeBase:
         self._attr_cols: Dict[str, AttrColumn] = {}
         self._attr_free = list(_ATTR_COLS)
         self._attr_host: set = set()    # properties with a value that has no code (unhashable): their filters stay on the host
+        # incremental checkpoints: what the last one left on disk (None: the next one writes a base) and, once a
+        # checkpoint has captured, the objects upserted / deleted since its capture (id -> key)
+        self._ckpt: Optional[Dict[str, Any]] = None
+        self._ckpt_lock = threading.Lock()   # one checkpoint at a time
+        self._tracking = False
+        self._dirty_put: Dict[int, str] = {}
+        self._dirty_del: Dict[int, Optional[str]] = {}
 
     def _keyword_store(self, capacity: int):
         """``DeviceBM25`` on the vector index's GPU when that index is an ``engine.Index``; over a ``MultiIndex`` of them,
@@ -191,7 +198,8 @@ class KnowledgeBase:
         loses nothing a caller was told had been stored -- Weaviate keeps its own WAL on the data volume
         (docker-compose.yaml:477-478).  Records already in the file that are newer than this store's state (a restart
         after a crash: ``load`` restored the last snapshot) are replayed first: inserts re-encode their text -- the encoder
-        is deterministic -- deletes name the object keys.  ``save`` truncates the log.  Returns the replayed count."""
+        is deterministic -- deletes name the object keys.  ``save`` truncates the log; ``checkpoint`` keeps only the records
+        written after its capture.  Returns the replayed count."""
         import json
 
         with self._lock:
@@ -295,6 +303,8 @@ class KnowledgeBase:
                 if old is not None:
                     self._unindex(rid, old)
                 self._props[rid] = props
+                if self._tracking:
+                    self._dirty_put[rid] = self._id2key.get(rid)
                 self._by_user.setdefault(props.get("user_id"), set()).add(rid)
                 if props.get("org_id"):
                     self._by_org.setdefault(props["org_id"], set()).add(rid)
@@ -627,6 +637,8 @@ class KnowledgeBase:
                     except OSError:
                         pass
             self.saved_mutations = gen
+            if self._ckpt is not None and self._ckpt["dir"] == os.path.abspath(directory):
+                self._ckpt_reset()                  # the directory no longer holds the checkpoint's base
             if self._wal is not None:               # everything logged so far is inside the snapshot: start a fresh log.
                 self._wal.close()                   # (a crash before this point leaves old records; replay skips them by gen)
                 tmp_wal = self._wal_path + ".tmp"
@@ -634,12 +646,165 @@ class KnowledgeBase:
                 os.replace(tmp_wal, self._wal_path)
                 self._wal = open(self._wal_path, "a", encoding="utf-8")
 
+    def _ckpt_reset(self) -> None:
+        """The next checkpoint writes a base; nothing is tracked until it captures.  Caller holds the lock or owns the
+        store alone."""
+        self._ckpt, self._tracking = None, False
+        self._dirty_put, self._dirty_del = {}, {}
+
+    def checkpoint(self, directory: str, on_stage: Optional[Callable[[str], None]] = None) -> Dict[str, Any]:
+        """Durable snapshot like ``save``, but incremental and without pausing the store (DESIGN.md section 8,
+        "Snapshots").  Under the lock only the change is captured: every shard's row count, live bitmap and compaction
+        count (``Index.capture``), the objects upserted and deleted since the last checkpoint, and the mutation log's
+        length.  Outside it the rows appended since the last checkpoint are read (``Index.export_rows``) and written with
+        the bitmaps as one delta file per shard plus the metadata delta, then the manifest ``meta.json`` is renamed into
+        place; searches, inserts and deletes go on meanwhile.  Last, under the lock again, the log keeps only the records
+        written after the capture.
+
+        A base (every live row and the whole property table) is written instead when there is none yet in this
+        directory from this store, a shard was compacted since the last capture, the rows appended since the base exceed
+        a quarter of its rows, or more than 16 deltas would be on disk.  ``on_stage(name)`` is called after the capture
+        ("captured"), once the segment files are durable ("segment"), once the manifest is ("manifest") and before the log
+        is trimmed ("trim").  Returns {"kind": "base" | "delta", "generation", "bytes", "locked_ms", "seconds"}."""
+        os.makedirs(directory, exist_ok=True)
+        directory = os.path.abspath(directory)
+        with self._ckpt_lock:
+            for _ in range(4):     # a compaction that lands between capture and copy discards the segment: retry as a base
+                res = self._checkpoint_once(directory, on_stage or (lambda stage: None))
+                if res is not None:
+                    return res
+            raise RuntimeError("checkpoint: every attempt raced a compaction")
+
+    def _checkpoint_once(self, directory: str, on_stage) -> Optional[Dict[str, Any]]:
+        import json
+        import time
+
+        from . import checkpoint as K
+
+        t0 = time.perf_counter()
+        with self._lock:
+            t_lock = time.perf_counter()
+            st = self._ckpt
+            if st is None or st["dir"] != directory or st["shards"].index is not self.index:
+                st = None
+            shards = st["shards"] if st else K.Shards(self.index)
+            caps = shards.capture()
+            gen = int(self.mutations)
+            base = (st is None or any(c[3] != k for c, k in zip(caps, st["compactions"]))
+                    or sum(c[0] - m for c, m in zip(caps, st["base_marks"])) > K.MAX_DELTA_FRACTION * st["base_entries"]
+                    or len(st["meta"]["deltas"]) + 1 > K.MAX_DELTAS)
+            if base:
+                objs = (dict(self._props), dict(self._id2key))          # shallow: property dicts are replaced, never edited
+            else:
+                objs = ([(rid, key, self._props[rid]) for rid, key in self._dirty_put.items()], list(self._dirty_del.items()))
+            self._tracking = True
+            self._dirty_put, self._dirty_del = {}, {}
+            codes = (dict(self._user_code), dict(self._org_code), int(self._next_id))
+            wal_off = None
+            if self._wal is not None:
+                self._wal.flush()
+                wal_off = os.fstat(self._wal.fileno()).st_size
+            locked_ms = (time.perf_counter() - t_lock) * 1e3
+        try:
+            on_stage("captured")
+            ranges = [(0, c[0]) if base else (m, c[0] - m) for c, m in zip(caps, [0] * len(caps) if base else st["marks"])]
+            data = shards.export_rows(ranges)
+            if any(a[3] != c[3] for a, c in zip(shards.capture(), caps)):
+                self._ckpt = None           # renumbered while the rows were read: what was read is discarded
+                return None
+            tag = K.new_tag(gen)
+            written = 0
+            # only the rows live at capture: a row dead then never comes back, so nothing later needs it
+            keep = [K.bits_at(c[1], np.arange(r0, r0 + n)) for c, (r0, n) in zip(caps, ranges)]
+            if base:
+                props, id2key = objs
+                part = np.concatenate([np.full(int(k.sum()), s, np.int32) for s, k in enumerate(keep)])
+                row = np.concatenate([np.arange(r0, r0 + n, dtype=np.int64)[k] for (r0, n), k in zip(ranges, keep)])
+                ids = np.concatenate([d[1][k] for d, k in zip(data, keep)])
+                nonfinite = np.concatenate([K.bits_at(c[2], np.arange(r0, r0 + n))[k]
+                                            for c, (r0, n), k in zip(caps, ranges, keep)])
+                shard_name = f"shard.{gen}.npz"
+                written += K.write_npz(os.path.join(directory, shard_name),
+                                       rows=np.concatenate([d[0][k] for d, k in zip(data, keep)]), ids=ids,
+                                       user=np.concatenate([d[2][k] for d, k in zip(data, keep)]),
+                                       org=np.concatenate([d[3][k] for d, k in zip(data, keep)]), nonfinite=nonfinite,
+                                       dim=self.dim, dtype=getattr(self.index, "dtype", AUR_BF16),
+                                       capacity=int(getattr(self.index, "capacity", len(ids))))
+                seg = {"tag": tag, "rows": f"base.{tag}.npz", "meta": f"base.{tag}.jsonl", "entries": int(len(ids))}
+                written += K.write_npz(os.path.join(directory, seg["rows"]), ids=ids, part=part, row=row)
+                written += K.write_jsonl(os.path.join(directory, seg["meta"]),
+                                         ([rid, id2key.get(rid), p] for rid, p in props.items()))
+                meta_base, deltas = seg, []
+            else:
+                puts, dels = objs
+                seg = {"tag": tag, "generation": gen, "shards": [f"delta.{tag}.{s}.npz" for s in range(len(caps))],
+                       "meta": f"delta.{tag}.jsonl"}
+                for s, (c, (r0, n), d, k) in enumerate(zip(caps, ranges, data, keep)):
+                    written += K.write_npz(os.path.join(directory, seg["shards"][s]), rows=d[0][k], ids=d[1][k],
+                                           user=d[2][k], org=d[3][k],
+                                           nonfinite=K.bits_at(c[2], np.arange(r0, r0 + n))[k],
+                                           row=np.arange(r0, r0 + n, dtype=np.int64)[k], live=c[1], nonfinite_bits=c[2],
+                                           rows_total=c[0])
+                written += K.write_jsonl(os.path.join(directory, seg["meta"]),
+                                         [["put", rid, key, p] for rid, key, p in puts] + [["del", rid, key] for rid, key in dels])
+                shard_name, meta_base, deltas = st["meta"]["shard"], st["meta"]["base"], st["meta"]["deltas"] + [seg]
+            K.fsync_dir(directory)
+            on_stage("segment")
+            user_code, org_code, next_id = codes
+            meta = {"shard": shard_name, "version": 2, "generation": gen, "dim": self.dim, "next_id": next_id,
+                    "user_code": user_code, "org_code": org_code, "parts": len(caps), "base": meta_base, "deltas": deltas}
+            path = os.path.join(directory, "meta.json")
+            written += K.write_file(path, lambda f: f.write(json.dumps(meta).encode("utf-8")))
+            K.fsync_dir(directory)
+            self.saved_mutations = max(self.saved_mutations, gen)
+            on_stage("manifest")
+            K.remove_unreferenced(directory, meta)
+            self._ckpt = {"dir": directory, "shards": shards, "meta": meta, "marks": [c[0] for c in caps],
+                          "compactions": [c[3] for c in caps],
+                          "base_marks": [c[0] for c in caps] if base else st["base_marks"],
+                          "base_entries": meta_base["entries"]}
+            on_stage("trim")
+            with self._lock:
+                t_trim = time.perf_counter()
+                self._trim_wal(wal_off)
+                locked_ms += (time.perf_counter() - t_trim) * 1e3
+        except BaseException:
+            with self._lock:
+                self._ckpt_reset()          # the next checkpoint starts over from a base
+            raise
+        return {"kind": "base" if base else "delta", "generation": gen, "bytes": int(written),
+                "locked_ms": round(locked_ms, 3), "seconds": round(time.perf_counter() - t0, 3)}
+
+    def _trim_wal(self, offset: Optional[int]) -> None:
+        """Keep only the log's bytes from ``offset`` on (the records written after a checkpoint's capture), under the
+        same file name.  Caller holds the lock."""
+        from .checkpoint import fsync_dir
+
+        if self._wal is None or offset is None:
+            return
+        self._wal.flush()
+        with open(self._wal_path, "rb") as f:
+            f.seek(offset)
+            tail = f.read()
+        tmp = self._wal_path + ".tmp"
+        with open(tmp, "wb") as f:
+            f.write(tail)
+            f.flush()
+            os.fsync(f.fileno())
+        self._wal.close()
+        os.replace(tmp, self._wal_path)
+        fsync_dir(os.path.dirname(os.path.abspath(self._wal_path)))
+        self._wal = open(self._wal_path, "a", encoding="utf-8")
+
     @classmethod
     def load(cls, directory: str, encoder, capacity: int = 1 << 20, device: int = 0, index_loader=None,
              text_of: Optional[Callable[[Dict[str, Any]], str]] = None) -> "KnowledgeBase":
-        """Rebuild from ``save``: vectors go back into HBM as they were stored (no re-encoding), the
-        keyword index is rebuilt from the chunk texts."""
+        """Rebuild from ``save`` or ``checkpoint``: vectors go back into HBM as they were stored (no re-encoding), the
+        keyword index is rebuilt from the chunk texts.  A checkpoint's base goes through ``index_loader``, its deltas
+        through the loaded index's own ``remove`` and ``add``; the store's next checkpoint writes a new base."""
         import json
+
+        from . import checkpoint as K
 
         if text_of is None:
             def text_of(p):
@@ -655,14 +820,19 @@ class KnowledgeBase:
             def index_loader(path, cap):
                 return Index.load(path, capacity=cap, device=device)
         loaded = index_loader(os.path.join(directory, meta.get("shard", "shard.npz")), int(capacity))
+        if "base" in meta:
+            K.apply_deltas(loaded, directory, meta)
+            props, key2id = K.read_objects(directory, meta)
+        else:
+            props, key2id = {int(k): v for k, v in meta["props"].items()}, meta["key2id"]
         kb = cls(encoder, capacity=capacity, device=device, index_factory=lambda dim, cap: loaded)
         kb._next_id = int(meta["next_id"])
         kb.mutations = kb.saved_mutations = int(meta.get("generation", 0))     # the log's records are ordered by it
         kb._user_code = {k: int(v) for k, v in meta["user_code"].items()}
         kb._org_code = {k: int(v) for k, v in meta["org_code"].items()}
-        kb._key2id = {k: int(v) for k, v in meta["key2id"].items()}
+        kb._key2id = {k: int(v) for k, v in key2id.items()}
         kb._id2key = {v: k for k, v in kb._key2id.items()}
-        kb._props = {int(k): v for k, v in meta["props"].items()}
+        kb._props = props
         for rid, p in kb._props.items():
             kb._by_user.setdefault(p.get("user_id"), set()).add(rid)
             if p.get("org_id"):
@@ -720,8 +890,11 @@ class KnowledgeBase:
         keys = [self._id2key.get(rid) for rid in ids]
         if self._kw_device:
             self.sparse.remove_many(ids)
-        for rid in ids:
+        for rid, key in zip(ids, keys):
             p = self._props.pop(rid)
+            if self._tracking:
+                self._dirty_put.pop(rid, None)
+                self._dirty_del[rid] = key
             self._unindex(rid, p)
             if not self._kw_device:
                 self.sparse.remove(rid)

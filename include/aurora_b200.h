@@ -138,6 +138,27 @@ int aur_export(aur_index* ix, void* rows_out, int64_t* ids_out, int32_t* user_ou
  * a partial aur_export, e.g. to snapshot only what was appended since the last snapshot. */
 int aur_read_rows(aur_index* ix, int64_t row0, int64_t n, void* rows_out, int64_t* ids_out);
 
+/* Incremental snapshots.  Published rows never change, a delete only tombstones a row, and growth moves nothing, so a
+ * snapshot needs only the rows appended since the last one plus one liveness bit per row; aur_compact is the only call
+ * that renumbers rows.
+ *
+ * aur_live_bits: under the shard's shared lock and its writers' lock (ordered after every aur_add / aur_remove that has
+ * returned; searches go on), *rows_out = aur_stats.rows and one kernel on the low-priority ingest stream packs rows
+ * [0, rows) into words: bit r % 32 of live_out[r / 32] = row r is live (its inverse norm is not NaN), of
+ * nonfinite_out[r / 32] = aur_export would report it live = 2 (AUR_I8 only; zero words for bf16 and f32, where
+ * nonfinite_out may be NULL).  Bits past rows are 0.  One copy back and a wait for that stream; no device-wide sync.
+ * *compactions_out (nullable) = aur_compact calls over the shard's life: rows kept their numbers between two captures
+ * with the same count.  words < ceil(rows / 32): AUR_ERR_INVALID before anything is launched.
+ *
+ * aur_export_rows: rows [row0, row0 + n) of the published prefix (tombstones included) with their ids and tenant codes
+ * (user_out / org_out nullable), as aur_export gives them, but under the shared lock only: searches and appends go on.
+ * The copy runs on the ingest stream through page-locked staging in bounded chunks.  A range outside the published
+ * prefix: AUR_ERR_INVALID, as in aur_read_rows. */
+int aur_live_bits(aur_index* ix, uint32_t* live_out, uint32_t* nonfinite_out, int64_t words, int64_t* rows_out,
+                  int64_t* compactions_out);
+int aur_export_rows(aur_index* ix, int64_t row0, int64_t n, void* rows_out, int64_t* ids_out, int32_t* user_out,
+                    int32_t* org_out);
+
 /* Reclaims the tombstones left by upserts and deletes (the reference's prediscovery job deletes and
  * re-inserts its chunks periodically, weaviate_client.py:374-394): live rows move down in append order,
  * aur_stats.rows drops to aur_stats.live.  Exclusive: waits for in-flight searches.  *reclaimed
